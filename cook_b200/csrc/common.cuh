@@ -159,10 +159,11 @@ __device__ __forceinline__ bool grid_exact(const GridFlag* f, long long n, doubl
   const double m = __longlong_as_double((long long)f->max_bits);
   return grid_value_ok(start) && ((double)(n + 1) * fmax(m, 1.0) + start) < 8796093022208.0;   // 2^43
 }
-__device__ __forceinline__ double warp_incl_scan(double x, const int lane) {
+template <class T>
+__device__ __forceinline__ T warp_incl_scan(T x, const int lane) {
 #pragma unroll
   for (int o = 1; o < 32; o <<= 1) {
-    const double y = __shfl_up_sync(0xffffffffu, x, o);
+    const T y = __shfl_up_sync(0xffffffffu, x, o);
     if (lane >= o) x = x + y;
   }
   return x;

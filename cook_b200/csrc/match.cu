@@ -32,7 +32,7 @@
 #include <mutex>
 #include <numeric>
 
-#include "common.cuh"
+#include "fold.cuh"
 #include "sort.cuh"
 
 namespace {
@@ -1881,20 +1881,6 @@ struct LessUserPos {
   }
 };
 
-__global__ void iota_k(int32_t* p, int n) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) p[i] = i;
-}
-
-__global__ void cons_seg_kernel(const int32_t* pos_by_user, const int32_t* ranked,
-                                const int32_t* user, int n, int32_t* seg_start, int32_t* seg_end) {
-  int p = blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= n) return;
-  int u = user[ranked[pos_by_user[p]]];
-  if (p == 0 || user[ranked[pos_by_user[p - 1]]] != u) seg_start[u] = p;
-  if (p == n - 1 || user[ranked[pos_by_user[p + 1]]] != u) seg_end[u] = p + 1;
-}
-
 // tools.clj:903-915 + :940-959: warp per user, lane-serial left fold over the
 // user's queued jobs in queue order, starting from the user's running usage.
 __global__ void __launch_bounds__(128) cons_user_kernel(ConsArgs a, const int32_t* pos_by_user,
@@ -1905,10 +1891,11 @@ __global__ void __launch_bounds__(128) cons_user_kernel(ConsArgs a, const int32_
   if (u >= a.n_users) return;
   const int s = seg_start[u], e = seg_end[u];
   if (e <= s) return;
-  double an = a.u_count ? a.u_count[u] : 0.0, ac = a.u_cpus ? a.u_cpus[u] : 0.0;
-  double am = a.u_mem ? a.u_mem[u] : 0.0, ag = a.u_gpus ? a.u_gpus[u] : 0.0;
+  double acc[4] = {a.u_count ? a.u_count[u] : 0.0, a.u_cpus ? a.u_cpus[u] : 0.0, a.u_mem ? a.u_mem[u] : 0.0,
+                    a.u_gpus ? a.u_gpus[u] : 0.0};
   const double qn = a.q_count[u], qc = a.q_cpus[u], qm = a.q_mem[u], qg = a.q_gpus[u];
   const int tokens = a.tokens ? a.tokens[u] : 0x7fffffff;
+  __shared__ double stage[4][4][32];
   // No quota on any resource (quota.clj default = Double/MAX_VALUE) and no rate limit in
   // force: every finite running sum passes, so the order-dependent fold is not needed.
   const double dmax = 1.7976931348623157e308;
@@ -1919,114 +1906,81 @@ __global__ void __launch_bounds__(128) cons_user_kernel(ConsArgs a, const int32_
   int seen = 0;
   // every partial sum exact (addends and start values on the 2^-10 grid, total below 2^43): a
   // parallel scan yields the left fold's bits; otherwise the lane-serial chain keeps the association
-  const bool exact = grid_exact(gf, e - s, fmax(fmax(an, ac), fmax(am, ag))) && grid_value_ok(an) && grid_value_ok(ac) &&
-                     grid_value_ok(am) && grid_value_ok(ag);
+  const bool exact = grid_exact(gf, e - s, fmax(fmax(acc[0], acc[1]), fmax(acc[2], acc[3]))) && grid_value_ok(acc[0]) &&
+                     grid_value_ok(acc[1]) && grid_value_ok(acc[2]) && grid_value_ok(acc[3]);
   for (int base0 = s; base0 < e; base0 += 128) {   // four chunks of gathers in flight
-   double xc4[4], xm4[4], xg4[4];
-   int pos4[4];
+    double x4[4][4];   // count, cpus, mem, gpus
+    int pos4[4];
 #pragma unroll
-   for (int q = 0; q < 4; q++) {
-     const int p = base0 + 32 * q + lane;
-     xc4[q] = xm4[q] = xg4[q] = 0.0; pos4[q] = -1;
-     if (p < e) {
-       pos4[q] = pos_by_user[p];
-       const int j = a.ranked[pos4[q]];
-       xc4[q] = a.jb.cpus[j]; xm4[q] = a.jb.mem[j]; xg4[q] = a.jb.gpus ? a.jb.gpus[j] : 0.0;
-     }
-   }
-#pragma unroll
-   for (int q = 0; q < 4; q++) {
-    const int base = base0 + 32 * q;
-    if (base >= e) break;
-    const int p = base + lane;
-    const double xc = xc4[q], xm = xm4[q], xg = xg4[q];
-    const int pos = pos4[q];
-    double mc = 0, mm = 0, mg = 0, mn = 0;
-    int cntn = min(32, e - base);
-    if (exact) {
-      mn = an + (double)(lane + 1);
-      mc = ac + warp_incl_scan(xc, lane); mm = am + warp_incl_scan(xm, lane); mg = ag + warp_incl_scan(xg, lane);
-      an = an + (double)cntn;
-      ac = __shfl_sync(0xffffffffu, mc, cntn - 1); am = __shfl_sync(0xffffffffu, mm, cntn - 1);
-      ag = __shfl_sync(0xffffffffu, mg, cntn - 1);
-    } else
-    for (int l = 0; l < cntn; l++) {
-      an = an + 1.0;
-      ac = ac + __shfl_sync(0xffffffffu, xc, l);
-      am = am + __shfl_sync(0xffffffffu, xm, l);
-      ag = ag + __shfl_sync(0xffffffffu, xg, l);
-      if (lane == l) { mn = an; mc = ac; mm = am; mg = ag; }
+    for (int q = 0; q < 4; q++) {
+      const int p = base0 + 32 * q + lane;
+      x4[q][0] = x4[q][1] = x4[q][2] = x4[q][3] = 0.0; pos4[q] = -1;
+      if (p < e) {
+        pos4[q] = pos_by_user[p];
+        const int j = a.ranked[pos4[q]];
+        x4[q][0] = 1.0; x4[q][1] = a.jb.cpus[j]; x4[q][2] = a.jb.mem[j]; x4[q][3] = a.jb.gpus ? a.jb.gpus[j] : 0.0;
+      }
     }
-    bool ok = (p < e) && (mn <= qn && mc <= qc && mm <= qm && mg <= qg);
-    unsigned ob = __ballot_sync(0xffffffffu, ok);
-    int kth = seen + __popc(ob & (0xffffffffu >> (31 - lane)));  // k-th surviving job of the user
-    bool limited = kth > tokens;
-    if (ok && limited && a.enforce_rate_limit) ok = false;
-    if (p < e) keep[pos] = ok ? 1 : 0;
-    seen += __popc(ob);
-   }
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+      const int base = base0 + 32 * q;
+      if (base >= e) break;
+      const int p = base + lane;
+      warp_fold_prefix(x4[q], acc, min(32, e - base), exact, stage[threadIdx.x >> 5]);
+      bool ok = (p < e) && (x4[q][0] <= qn && x4[q][1] <= qc && x4[q][2] <= qm && x4[q][3] <= qg);
+      unsigned ob = __ballot_sync(0xffffffffu, ok);
+      int kth = seen + __popc(ob & (0xffffffffu >> (31 - lane)));  // k-th surviving job of the user
+      bool limited = kth > tokens;
+      if (ok && limited && a.enforce_rate_limit) ok = false;
+      if (p < e) keep[pos4[q]] = ok ? 1 : 0;
+      seen += __popc(ob);
+    }
   }
 }
 
-// Queue-order pass (single warp): pool quota over survivors (tools.clj:917-933),
-// allowed + launch-plugin masks (scheduler.clj:749-750), take N (:751);
-// gathers the per-k hot columns.
-__global__ void cons_queue_kernel(ConsArgs a, const uint8_t* keep, int32_t* cons, double* kc,
-                                  double* km, double* kg, int32_t* kports, uint8_t* kflags,
-                                  int32_t* out_n) {
-  const int lane = threadIdx.x;
-  double pn = 0, pc = 0, pm = 0, pg = 0;
-  if (a.pool_q.enabled) {  // (reduce (partial merge-with +) (vals user->usage)), tools.clj:969
-    for (int base = 0; base < a.n_users; base += 32) {
-      int u = base + lane;
-      double xn = (u < a.n_users && a.u_count) ? a.u_count[u] : 0.0;
-      double xc = (u < a.n_users && a.u_cpus) ? a.u_cpus[u] : 0.0;
-      double xm = (u < a.n_users && a.u_mem) ? a.u_mem[u] : 0.0;
-      double xg = (u < a.n_users && a.u_gpus) ? a.u_gpus[u] : 0.0;
-      int cntn = min(32, a.n_users - base);
-      for (int l = 0; l < cntn; l++) {
-        pn = pn + __shfl_sync(0xffffffffu, xn, l);
-        pc = pc + __shfl_sync(0xffffffffu, xc, l);
-        pm = pm + __shfl_sync(0xffffffffu, xm, l);
-        pg = pg + __shfl_sync(0xffffffffu, xg, l);
-      }
-    }
+// The considerable set and its per-k hot columns, slot by slot.
+struct ConsOut {
+  int32_t* cons; double *kc, *km, *kg; int32_t* kports; uint8_t* kflags;
+  __device__ void put(const JobDev& jb, int j, int slot) const {
+    cons[slot] = j;
+    kc[slot] = jb.cpus[j];
+    km[slot] = jb.mem[j];
+    kg[slot] = jb.gpus ? jb.gpus[j] : 0.0;
+    kports[slot] = jb.ports ? jb.ports[j] : 0;
+    uint8_t fl = 0;
+    if (jb.group_off && jb.group_off[j + 1] > jb.group_off[j]) fl |= 1;
+    kflags[slot] = fl;
   }
+};
+
+// Queue-order pass (single warp): pool quota over survivors (tools.clj:917-933),
+// allowed + launch-plugin masks (scheduler.clj:749-750), take N (:751).
+__global__ void cons_queue_kernel(ConsArgs a, const uint8_t* keep, ConsOut out, int32_t* out_n) {
+  const int lane = threadIdx.x;
+  __shared__ double stage[4][32];
+  double pool[4] = {0.0, 0.0, 0.0, 0.0};   // count, cpus, mem, gpus
+  if (a.pool_q.enabled)  // (reduce (partial merge-with +) (vals user->usage)), tools.clj:969
+    warp_fold_sum<4, 1>(pool, a.n_users, false, [&](int u, double (&x)[4]) {
+      x[0] = a.u_count ? a.u_count[u] : 0.0; x[1] = a.u_cpus ? a.u_cpus[u] : 0.0;
+      x[2] = a.u_mem ? a.u_mem[u] : 0.0; x[3] = a.u_gpus ? a.u_gpus[u] : 0.0;
+      return true;
+    }, stage);
   int n_out = 0;
   for (int base = 0; base < a.n_ranked && n_out < a.num_considerable; base += 32) {
     int i = base + lane;
     bool k = i < a.n_ranked && keep[i];
     int j = i < a.n_ranked ? a.ranked[i] : 0;
-    double xc = 0, xm = 0, xg = 0;
-    if (k) { xc = a.jb.cpus[j]; xm = a.jb.mem[j]; xg = a.jb.gpus ? a.jb.gpus[j] : 0.0; }
     if (a.pool_q.enabled) {
-      unsigned mask = __ballot_sync(0xffffffffu, k);
-      double mc = 0, mm = 0, mg = 0, mn = 0;
-      while (mask) {
-        int l = __ffs(mask) - 1;
-        mask &= mask - 1;
-        pn = pn + 1.0;
-        pc = pc + __shfl_sync(0xffffffffu, xc, l);
-        pm = pm + __shfl_sync(0xffffffffu, xm, l);
-        pg = pg + __shfl_sync(0xffffffffu, xg, l);
-        if (lane == l) { mn = pn; mc = pc; mm = pm; mg = pg; }
-      }
-      if (k) k = mn <= a.pool_q.count && mc <= a.pool_q.cpus && mm <= a.pool_q.mem && mg <= a.pool_q.gpus;
+      double x[4] = {0.0, 0.0, 0.0, 0.0}, mine[4] = {0.0, 0.0, 0.0, 0.0};
+      if (k) { x[0] = 1.0; x[1] = a.jb.cpus[j]; x[2] = a.jb.mem[j]; x[3] = a.jb.gpus ? a.jb.gpus[j] : 0.0; }
+      warp_chain(x, pool, mine, __ballot_sync(0xffffffffu, k), stage);
+      if (k) k = mine[0] <= a.pool_q.count && mine[1] <= a.pool_q.cpus && mine[2] <= a.pool_q.mem && mine[3] <= a.pool_q.gpus;
     }
     if (k && a.jb.allowed && !a.jb.allowed[j]) k = false;
     if (k && a.jb.plugin && !a.jb.plugin[j]) k = false;
     unsigned kb = __ballot_sync(0xffffffffu, k);
     int slot = n_out + __popc(kb & ((1u << lane) - 1u));
-    if (k && slot < a.num_considerable) {
-      cons[slot] = j;
-      kc[slot] = a.jb.cpus[j];
-      km[slot] = a.jb.mem[j];
-      kg[slot] = a.jb.gpus ? a.jb.gpus[j] : 0.0;
-      kports[slot] = a.jb.ports ? a.jb.ports[j] : 0;
-      uint8_t fl = 0;
-      if (a.jb.group_off && a.jb.group_off[j + 1] > a.jb.group_off[j]) fl |= 1;
-      kflags[slot] = fl;
-    }
+    if (k && slot < a.num_considerable) out.put(a.jb, j, slot);
     n_out += __popc(kb);
   }
   if (lane == 0) *out_n = min(n_out, a.num_considerable);
@@ -2034,97 +1988,18 @@ __global__ void cons_queue_kernel(ConsArgs a, const uint8_t* keep, int32_t* cons
 
 // Parallel form of the queue-order pass for the common case of NO global pool
 // quota (tools.clj:923 `(if (nil? quota) queue ...)`): the filters are then
-// element-wise and "take N" is a stable compaction => three-kernel scan.
-constexpr int SCAN_TB = 256;
-constexpr int SCAN_ITEMS = 4;  // elements per thread
-
-__device__ __forceinline__ bool cons_flag(const ConsArgs& a, const uint8_t* keep, int i) {
-  if (i >= a.n_ranked || !keep[i]) return false;
-  const int j = a.ranked[i];
-  if (a.jb.allowed && !a.jb.allowed[j]) return false;
-  if (a.jb.plugin && !a.jb.plugin[j]) return false;
-  return true;
-}
-
-__global__ void __launch_bounds__(SCAN_TB) cons_count_kernel(ConsArgs a, const uint8_t* keep,
-                                                             int32_t* block_sums) {
-  __shared__ int warp_sums[SCAN_TB / 32];
-  const int base = (blockIdx.x * SCAN_TB + threadIdx.x) * SCAN_ITEMS;
-  int c = 0;
-#pragma unroll
-  for (int q = 0; q < SCAN_ITEMS; q++) c += cons_flag(a, keep, base + q) ? 1 : 0;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-  if ((threadIdx.x & 31) == 0) warp_sums[threadIdx.x >> 5] = c;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    int t = 0;
-    for (int w = 0; w < SCAN_TB / 32; w++) t += warp_sums[w];
-    block_sums[blockIdx.x] = t;
+// element-wise and "take N" is a stable compaction.
+struct ConsSurvivors {
+  ConsArgs a; const uint8_t* kept; ConsOut out;
+  __device__ bool keep(int i) const {
+    if (!kept[i]) return false;
+    const int j = a.ranked[i];
+    if (a.jb.allowed && !a.jb.allowed[j]) return false;
+    if (a.jb.plugin && !a.jb.plugin[j]) return false;
+    return true;
   }
-}
-
-__global__ void cons_scan_blocks_kernel(int32_t* block_sums, int nblocks, int32_t* out_n, int cap) {
-  // single warp, sequential over chunks of 32 block sums (nblocks <= ~10k)
-  const int lane = threadIdx.x;
-  int carry = 0;
-  for (int base = 0; base < nblocks; base += 32) {
-    int i = base + lane;
-    int v = i < nblocks ? block_sums[i] : 0;
-    int incl = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int n = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += n;
-    }
-    if (i < nblocks) block_sums[i] = carry + incl - v;  // exclusive
-    carry += __shfl_sync(0xffffffffu, incl, 31);
-  }
-  if (lane == 0) *out_n = min(carry, cap);
-}
-
-__global__ void __launch_bounds__(SCAN_TB) cons_scatter_kernel(ConsArgs a, const uint8_t* keep,
-                                                               const int32_t* block_off, int32_t* cons,
-                                                               double* kc, double* km, double* kg,
-                                                               int32_t* kports, uint8_t* kflags) {
-  __shared__ int warp_off[SCAN_TB / 32];
-  const int base = (blockIdx.x * SCAN_TB + threadIdx.x) * SCAN_ITEMS;
-  bool f[SCAN_ITEMS];
-  int c = 0;
-#pragma unroll
-  for (int q = 0; q < SCAN_ITEMS; q++) { f[q] = cons_flag(a, keep, base + q); c += f[q] ? 1 : 0; }
-  int incl = c;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    int n = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += n;
-  }
-  if (lane == 31) warp_off[warp] = incl;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    int t = 0;
-    for (int w = 0; w < SCAN_TB / 32; w++) { int x = warp_off[w]; warp_off[w] = t; t += x; }
-  }
-  __syncthreads();
-  int slot = block_off[blockIdx.x] + warp_off[warp] + incl - c;
-#pragma unroll
-  for (int q = 0; q < SCAN_ITEMS; q++) {
-    if (!f[q]) continue;
-    if (slot < a.num_considerable) {
-      const int j = a.ranked[base + q];
-      cons[slot] = j;
-      kc[slot] = a.jb.cpus[j];
-      km[slot] = a.jb.mem[j];
-      kg[slot] = a.jb.gpus ? a.jb.gpus[j] : 0.0;
-      kports[slot] = a.jb.ports ? a.jb.ports[j] : 0;
-      uint8_t fl = 0;
-      if (a.jb.group_off && a.jb.group_off[j + 1] > a.jb.group_off[j]) fl |= 1;
-      kflags[slot] = fl;
-    }
-    slot++;
-  }
-}
+  __device__ void emit(int i, int slot) const { out.put(a.jb, a.ranked[i], slot); }
+};
 
 // ------------------------------------------------------------------ setup
 __global__ void gather_offers_kernel(const int32_t* perm, int O, const double* c, const double* m,
@@ -2423,43 +2298,15 @@ __global__ void __launch_bounds__(128) usage_delta_kernel(ConsArgs a, const int3
   const int lane = threadIdx.x & 31;
   if (u >= a.n_users) return;
   const int s = seg_start[u], e = seg_end[u];
-  double dn = 0.0, dc = 0.0, dm = 0.0, dg = 0.0;
-  const bool exact = grid_exact(gf, e - s);
-  for (int base = s; base < e; base += 128) {   // four chunks of gathers in flight
-    double xn4[4], xc4[4], xm4[4], xg4[4];
-#pragma unroll
-    for (int q = 0; q < 4; q++) {
-      const int p = base + 32 * q + lane;
-      xn4[q] = xc4[q] = xm4[q] = xg4[q] = 0.0;
-      if (p < e) {
-        const int j = a.ranked[pos_by_user[p]];
-        if (placed_job[j]) { xn4[q] = 1.0; xc4[q] = a.jb.cpus[j]; xm4[q] = a.jb.mem[j]; xg4[q] = a.jb.gpus ? a.jb.gpus[j] : 0.0; }
-      }
-    }
-#pragma unroll
-    for (int q = 0; q < 4; q++) {
-      if (base + 32 * q >= e) break;
-      const double xn = xn4[q], xc = xc4[q], xm = xm4[q], xg = xg4[q];
-      if (exact) {   // association-free sums
-        double rn = xn, rc = xc, rm = xm, rg = xg;
-        for (int o = 16; o > 0; o >>= 1) {
-          rn += __shfl_xor_sync(0xffffffffu, rn, o); rc += __shfl_xor_sync(0xffffffffu, rc, o);
-          rm += __shfl_xor_sync(0xffffffffu, rm, o); rg += __shfl_xor_sync(0xffffffffu, rg, o);
-        }
-        dn += rn; dc += rc; dm += rm; dg += rg;
-      } else {
-        const unsigned any = __ballot_sync(0xffffffffu, xn != 0.0);
-        for (unsigned m = any; m; m &= m - 1) {   // only the placed ones add (x + 0.0 == x anyway)
-          const int l = __ffs(m) - 1;
-          dn = dn + __shfl_sync(0xffffffffu, xn, l);
-          dc = dc + __shfl_sync(0xffffffffu, xc, l);
-          dm = dm + __shfl_sync(0xffffffffu, xm, l);
-          dg = dg + __shfl_sync(0xffffffffu, xg, l);
-        }
-      }
-    }
-  }
-  if (lane == 0) { delta[4 * u] = dn; delta[4 * u + 1] = dc; delta[4 * u + 2] = dm; delta[4 * u + 3] = dg; }
+  __shared__ double stage[4][4][32];
+  double d[4] = {0.0, 0.0, 0.0, 0.0};
+  warp_fold_sum<4, 4>(d, e - s, grid_exact(gf, e - s), [&](int k, double (&x)[4]) {
+    const int j = a.ranked[pos_by_user[s + k]];
+    if (!placed_job[j]) return false;   // only the placed ones add (x + 0.0 == x anyway)
+    x[0] = 1.0; x[1] = a.jb.cpus[j]; x[2] = a.jb.mem[j]; x[3] = a.jb.gpus ? a.jb.gpus[j] : 0.0;
+    return true;
+  }, stage[threadIdx.x >> 5]);
+  if (lane == 0) { delta[4 * u] = d[0]; delta[4 * u + 1] = d[1]; delta[4 * u + 2] = d[2]; delta[4 * u + 3] = d[3]; }
 }
 
 __global__ void count_flags_kernel(const int32_t* flags, int n, int32_t* out) {
@@ -2825,29 +2672,23 @@ static int32_t run_plan(cook_pool* pool, MatchPlan* mp, int32_t* out_considerabl
       launches++;
     }
   }
-  iota_k<<<(n_ranked + TB - 1) / TB, TB, 0, st>>>(mp->d_pos, n_ranked);
   CK(pool, csort::sort_indices(mp->d_pos, mp->d_tmp, n_ranked, LessUserPos{ca.ranked, ca.jb.user}, st));
-  launches += 2;
+  launches++;
   for (long long w = csort::TILE; w < n_ranked; w <<= 1) launches++;
-  cons_seg_kernel<<<(n_ranked + TB - 1) / TB, TB, 0, st>>>(mp->d_pos, ca.ranked, ca.jb.user, n_ranked,
-                                                           mp->d_seg_s, mp->d_seg_e);
+  seg_bounds_kernel<<<(n_ranked + TB - 1) / TB, TB, 0, st>>>(SortedKey{mp->d_pos, ca.ranked, ca.jb.user}, n_ranked,
+                                                             mp->d_seg_s, mp->d_seg_e, nullptr);
   CK(pool, cudaMemsetAsync(mp->d_gf, 0, sizeof(GridFlag), st));
   grid_check_kernel<<<(mp->J + TB - 1) / TB, TB, 0, st>>>(ca.jb.cpus, ca.jb.mem, ca.jb.gpus, mp->J, mp->d_gf);
   cons_user_kernel<<<(U + 3) / 4, 128, 0, st>>>(ca, mp->d_pos, mp->d_seg_s, mp->d_seg_e, mp->d_keep, mp->d_gf);
   launches++;
+  const ConsOut cons_out{mp->d_cons, mp->d_kc, mp->d_km, mp->d_kg, mp->d_kports, mp->d_kflags};
   if (ca.pool_q.enabled) {
     // global pool quota: an order-dependent f64 left fold over the survivors
     // (filter-sequential) => exact single-warp pass
-    cons_queue_kernel<<<1, 32, 0, st>>>(ca, mp->d_keep, mp->d_cons, mp->d_kc, mp->d_km, mp->d_kg,
-                                        mp->d_kports, mp->d_kflags, mp->d_counters);
+    cons_queue_kernel<<<1, 32, 0, st>>>(ca, mp->d_keep, cons_out, mp->d_counters);
     launches += 3;
   } else {
-    const int per_block = SCAN_TB * SCAN_ITEMS;
-    const int nsb = (n_ranked + per_block - 1) / per_block;
-    cons_count_kernel<<<nsb, SCAN_TB, 0, st>>>(ca, mp->d_keep, mp->d_tmp);
-    cons_scan_blocks_kernel<<<1, 32, 0, st>>>(mp->d_tmp, nsb, mp->d_counters, ca.num_considerable);
-    cons_scatter_kernel<<<nsb, SCAN_TB, 0, st>>>(ca, mp->d_keep, mp->d_tmp, mp->d_cons, mp->d_kc, mp->d_km,
-                                                 mp->d_kg, mp->d_kports, mp->d_kflags);
+    compact(ConsSurvivors{ca, mp->d_keep, cons_out}, n_ranked, nullptr, mp->d_tmp, mp->d_counters, ca.num_considerable, st);
     launches += 5;
   }
   CK(pool, cudaGetLastError());

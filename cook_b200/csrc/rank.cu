@@ -6,7 +6,7 @@
 // (scheduler.clj:2134-2157) and filter-offensive-jobs (:2198-2229).
 //
 // Pipeline (all on the pool's stream, no host round trips):
-//   K1 iota + comparator sort by (user name rank, -priority, start, task id,
+//   K1 comparator sort by (user name rank, -priority, start, task id,
 //      job id)                      -> per-user segments in tools.clj:614-641 order
 //   K2 segment bounds
 //   K3 warp-per-user fold           -> cumulative usage in the reference's
@@ -15,7 +15,7 @@
 //   K4 comparator sort of positions by (dru, k-way-merge tie rule)
 //   K5 single-warp queue filter     -> pending only, pool quota, group quota,
 //      offensive filter, stable compaction.
-#include "common.cuh"
+#include "fold.cuh"
 #include "sort.cuh"
 
 namespace {
@@ -29,26 +29,6 @@ struct TaskCols {
   const double* cpus;
   const double* mem;
   const double* gpus;
-};
-
-// tools.clj:614-641 compare of feature vectors, prefixed by the user's name
-// rank so that one global sort yields all per-user lists, users in name order.
-struct LessUserTask {
-  TaskCols t;
-  const int32_t* name_rank;
-  __device__ bool operator()(int32_t a, int32_t b) const {
-    int ua = name_rank[t.user[a]], ub = name_rank[t.user[b]];
-    if (ua != ub) return ua < ub;
-    int pa = -t.prio[a], pb = -t.prio[b];
-    if (pa != pb) return pa < pb;
-    long long sa = t.start[a], sb = t.start[b];
-    if (sa != sb) return sa < sb;
-    long long ta = t.tid[a], tb = t.tid[b];
-    if (ta != tb) return ta < tb;
-    long long ja = t.jid[a], jb = t.jid[b];
-    if (ja != jb) return ja < jb;
-    return a < b;
-  }
 };
 
 // Global emission order of dru/sorted-merge (dru.clj:82-104).  X, Y are
@@ -90,34 +70,19 @@ __global__ void scatter_dru_kernel(const int32_t* __restrict__ idx, const double
   if (p < n) dru_task[idx[p]] = dru_at[p];
 }
 
-__global__ void iota_kernel(int32_t* p, int n) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) p[i] = i;
-}
-
-__global__ void seg_bounds_kernel(const int32_t* __restrict__ idx, const int32_t* __restrict__ user,
-                                  int n, int32_t* seg_start, int32_t* seg_end,
-                                  int32_t* user_at) {
-  int p = blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= n) return;
-  int u = user[idx[p]];
-  user_at[p] = u;
-  if (p == 0 || user[idx[p - 1]] != u) seg_start[u] = p;
-  if (p == n - 1 || user[idx[p + 1]] != u) seg_end[u] = p + 1;
-}
-
 struct UserCols {
   const double *div_mem, *div_cpus, *div_gpus;
   const double *q_count, *q_cpus, *q_mem, *q_gpus;
 };
 
-// K3: one warp per user.  Lane-serial fold keeps the reference's left-fold
-// association: acc = ((acc + x0) + x1) + ... exactly as `reductions` does.
+// K3: one warp per user, the running sums in the reference's left-fold order
+// (fold.cuh): acc = ((acc + x0) + x1) + ... exactly as `reductions` does.
 __global__ void __launch_bounds__(128) user_fold_kernel(
     const int32_t* __restrict__ idx, TaskCols t, UserCols uc, const int32_t* __restrict__ seg_start,
     const int32_t* __restrict__ seg_end, int n_users, int dru_mode, int max_over_quota,
     double* __restrict__ dru_at, int32_t* n_kept_total, const GridFlag* gf, int n_scan) {
   if (n_scan > 0 && grid_exact(gf, n_scan)) return;   // the order-wide scans below did it
+  __shared__ double stage[4][3][32];
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (warp >= n_users) return;
@@ -126,225 +91,97 @@ __global__ void __launch_bounds__(128) user_fold_kernel(
   if (e <= s) return;
   const double md = uc.div_mem[u], cd = uc.div_cpus[u], gd = uc.div_gpus[u];
   const double qn = uc.q_count[u], qc = uc.q_cpus[u], qm = uc.q_mem[u], qg = uc.q_gpus[u];
-  // The three cumulative sums are independent serial chains: lanes 0..2 run one each over
-  // the batch staged in shared memory (carried in `acc`), then every lane reads its prefix.
-  __shared__ double fold_s[4][3][32];
-  double (*fs)[32] = fold_s[threadIdx.x >> 5];
-  double acc = 0.0;
-  double am = 0.0, ac = 0.0, ag = 0.0;   // carries of the scan path
-  const bool exact = grid_exact(gf, e - s);   // every partial sum is exact: a parallel scan gives the left fold's bits
+  const bool exact = grid_exact(gf, e - s);
+  double acc[3] = {0.0, 0.0, 0.0};   // mem, cpus, gpus
   int over = 0;
   bool cut = false;
   int kept = 0;
   const double NaN = __longlong_as_double(0x7ff8000000000000LL);
-  auto chunk = [&](const int base, const double xm, const double xc, const double xg) {
-    const int p = base + lane;
-    double mym, myc, myg;
-    if (exact) {
-      mym = am + warp_incl_scan(xm, lane); myc = ac + warp_incl_scan(xc, lane); myg = ag + warp_incl_scan(xg, lane);
-      am = __shfl_sync(0xffffffffu, mym, 31); ac = __shfl_sync(0xffffffffu, myc, 31); ag = __shfl_sync(0xffffffffu, myg, 31);
-    } else {
-      fs[0][lane] = xm; fs[1][lane] = xc; fs[2][lane] = xg;
-      __syncwarp();
-      int cntn = min(32, e - base);
-      if (lane < 3) {
-        double* row = fs[lane];
-#pragma unroll 8
-        for (int l = 0; l < cntn; l++) { acc = acc + row[l]; row[l] = acc; }
-      }
-      __syncwarp();
-      mym = fs[0][lane]; myc = fs[1][lane]; myg = fs[2][lane];
-      __syncwarp();
-    }
-    // scheduler.clj:2057-2071: keep while #violating prefixes <= limit
-    bool viol = false;
-    if (p < e) {
-      double cnt = (double)(p - s + 1);
-      viol = !(cnt <= qn && myc <= qc && mym <= qm && myg <= qg);
-    }
-    unsigned vb = __ballot_sync(0xffffffffu, viol);
-    int over_incl = over + __popc(vb & (0xffffffffu >> (31 - lane)));
-    bool keep = (p < e) && !cut && (over_incl <= max_over_quota);
-    double d = NaN;
-    if (keep) {
-      if (dru_mode == 0) {
-        double a = mym / md, b = myc / cd;
-        d = a > b ? a : b;
-      } else {
-        d = myg / gd;
-      }
-    }
-    if (p < e) dru_at[p] = d;
-    unsigned kb = __ballot_sync(0xffffffffu, keep);
-    kept += __popc(kb);
-    over += __popc(vb);
-    if (over > max_over_quota) cut = true;  // later batches are all beyond the cut
-  };
-  if (exact) {
+  for (int base0 = s; base0 < e; base0 += 128) {
     // the gathers (idx -> amounts) are what a long segment waits for: four chunks in flight
-    for (int base = s; base < e; base += 128) {
-      double xm4[4], xc4[4], xg4[4];
+    double x4[4][3];
 #pragma unroll
-      for (int q = 0; q < 4; q++) {
-        const int p = base + 32 * q + lane;
-        xm4[q] = xc4[q] = xg4[q] = 0.0;
-        if (p < e) { const int ti = idx[p]; xm4[q] = t.mem[ti]; xc4[q] = t.cpus[ti]; xg4[q] = t.gpus[ti]; }
-      }
-#pragma unroll
-      for (int q = 0; q < 4; q++)
-        if (base + 32 * q < e) chunk(base + 32 * q, xm4[q], xc4[q], xg4[q]);
+    for (int q = 0; q < 4; q++) {
+      const int p = base0 + 32 * q + lane;
+      x4[q][0] = x4[q][1] = x4[q][2] = 0.0;
+      if (p < e) { const int ti = idx[p]; x4[q][0] = t.mem[ti]; x4[q][1] = t.cpus[ti]; x4[q][2] = t.gpus[ti]; }
     }
-  } else {
-    for (int base = s; base < e; base += 32) {
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+      const int base = base0 + 32 * q;
+      if (base >= e) break;
       const int p = base + lane;
-      double xm = 0.0, xc = 0.0, xg = 0.0;
-      if (p < e) { const int ti = idx[p]; xm = t.mem[ti]; xc = t.cpus[ti]; xg = t.gpus[ti]; }
-      chunk(base, xm, xc, xg);
+      warp_fold_prefix(x4[q], acc, min(32, e - base), exact, stage[threadIdx.x >> 5]);
+      const double mym = x4[q][0], myc = x4[q][1], myg = x4[q][2];
+      // scheduler.clj:2057-2071: keep while #violating prefixes <= limit
+      bool viol = false;
+      if (p < e) {
+        double cnt = (double)(p - s + 1);
+        viol = !(cnt <= qn && myc <= qc && mym <= qm && myg <= qg);
+      }
+      unsigned vb = __ballot_sync(0xffffffffu, viol);
+      int over_incl = over + __popc(vb & (0xffffffffu >> (31 - lane)));
+      bool keep = (p < e) && !cut && (over_incl <= max_over_quota);
+      double d = NaN;
+      if (keep) {
+        if (dru_mode == 0) {
+          double a = mym / md, b = myc / cd;
+          d = a > b ? a : b;
+        } else {
+          d = myg / gd;
+        }
+      }
+      if (p < e) dru_at[p] = d;
+      unsigned kb = __ballot_sync(0xffffffffu, keep);
+      kept += __popc(kb);
+      over += __popc(vb);
+      if (over > max_over_quota) cut = true;  // later batches are all beyond the cut
     }
   }
   if (lane == 0 && kept) atomicAdd(n_kept_total, kept);
 }
 
-// K3 for exact-grid amounts (common.cuh: any association gives the left fold's bits): the per-user
-// running sums are ONE inclusive scan over the whole sorted order minus the scan just before the
-// user's first slot, the over-quota count is a second scan over the violation flags.  No user, however
-// long its list, sits on one warp.  Five launches: amount tiles, their totals, violation tiles, their
-// totals, the finish (keep / dru / kept count).
-constexpr int OS_TB = 256, OS_IPT = 8, OS_TILE = OS_TB * OS_IPT;
-
-struct OrderScan {
-  const int32_t* idx; TaskCols t; UserCols uc;
-  const int32_t* user_at; const int32_t* seg_start;
+// K3 for exact-grid amounts (fold.cuh: any association gives the left fold's bits): the per-user
+// running sums are the order-wide scan of the amounts, the over-quota count is a second one over the
+// violation flags.  No user, however long its list, sits on one warp.  Five launches: the two scans,
+// the finish (keep / dru / kept count).
+struct RankScan {
+  const int32_t* user_at; const int32_t* seg_start; UserCols uc;
+  OrderScan<double, 3> amt;   // mem, cpus, gpus
+  OrderScan<int, 1> viol;     // violating prefixes
   int n, dru_mode, max_over_quota;
-  const GridFlag* gf;
-  double *pm, *pc, *pg;      // [n] tile-local inclusive sums
-  double *bm, *bc, *bg;      // [tiles] totals, then exclusive offsets
-  int32_t* pv; int32_t* bv;  // the same for the violation flags
   double* dru_at; int32_t* n_kept_total;
+  // scheduler.clj:2057-2071: a prefix violates when (count, cpus, mem, gpus) is not within the quota
+  __device__ void operator()(int p, int (&v)[1]) const {
+    const int u = user_at[p], s = seg_start[u];
+    const double cnt = (double)(p - s + 1);
+    v[0] = !(cnt <= uc.q_count[u] && amt.segment_sum(1, p, s) <= uc.q_cpus[u] && amt.segment_sum(0, p, s) <= uc.q_mem[u] &&
+             amt.segment_sum(2, p, s) <= uc.q_gpus[u]) ? 1 : 0;
+  }
 };
 
-__device__ __forceinline__ void os_user_sums(const OrderScan& a, int p, int s, double& m, double& c, double& g) {
-  const int tp = p / OS_TILE;
-  m = a.pm[p] + a.bm[tp]; c = a.pc[p] + a.bc[tp]; g = a.pg[p] + a.bg[tp];
-  if (s > 0) {
-    const int ts = (s - 1) / OS_TILE;
-    m = m - (a.pm[s - 1] + a.bm[ts]); c = c - (a.pc[s - 1] + a.bc[ts]); g = g - (a.pg[s - 1] + a.bg[ts]);
+struct LoadAmounts {
+  const int32_t* idx; TaskCols t;
+  __device__ void operator()(int p, double (&x)[3]) const {
+    const int ti = idx[p];
+    x[0] = t.mem[ti]; x[1] = t.cpus[ti]; x[2] = t.gpus[ti];
   }
-}
+};
 
-__global__ void __launch_bounds__(OS_TB) os_amount_tiles(OrderScan a) {
-  if (!grid_exact(a.gf, a.n)) return;
-  __shared__ double s_m[OS_TB / 32], s_c[OS_TB / 32], s_g[OS_TB / 32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int p0 = blockIdx.x * OS_TILE + threadIdx.x * OS_IPT;
-  double xm[OS_IPT], xc[OS_IPT], xg[OS_IPT];
-#pragma unroll
-  for (int k = 0; k < OS_IPT; k++) {
-    const int p = p0 + k;
-    xm[k] = xc[k] = xg[k] = 0.0;
-    if (p < a.n) { const int ti = a.idx[p]; xm[k] = a.t.mem[ti]; xc[k] = a.t.cpus[ti]; xg[k] = a.t.gpus[ti]; }
-  }
-#pragma unroll
-  for (int k = 1; k < OS_IPT; k++) { xm[k] = xm[k - 1] + xm[k]; xc[k] = xc[k - 1] + xc[k]; xg[k] = xg[k - 1] + xg[k]; }
-  const double im = warp_incl_scan(xm[OS_IPT - 1], lane), ic = warp_incl_scan(xc[OS_IPT - 1], lane),
-               ig = warp_incl_scan(xg[OS_IPT - 1], lane);
-  if (lane == 31) { s_m[warp] = im; s_c[warp] = ic; s_g[warp] = ig; }
-  __syncthreads();
-  double om = im - xm[OS_IPT - 1], oc = ic - xc[OS_IPT - 1], og = ig - xg[OS_IPT - 1];
-  for (int w = 0; w < warp; w++) { om = om + s_m[w]; oc = oc + s_c[w]; og = og + s_g[w]; }
-#pragma unroll
-  for (int k = 0; k < OS_IPT; k++) {
-    const int p = p0 + k;
-    if (p < a.n) { a.pm[p] = om + xm[k]; a.pc[p] = oc + xc[k]; a.pg[p] = og + xg[k]; }
-  }
-  if (threadIdx.x == OS_TB - 1) {
-    a.bm[blockIdx.x] = om + xm[OS_IPT - 1]; a.bc[blockIdx.x] = oc + xc[OS_IPT - 1]; a.bg[blockIdx.x] = og + xg[OS_IPT - 1];
-  }
-}
-
-__global__ void os_amount_totals(OrderScan a, int nb) {   // one warp: totals -> exclusive offsets
-  if (!grid_exact(a.gf, a.n)) return;
-  const int lane = threadIdx.x;
-  double am = 0.0, ac = 0.0, ag = 0.0;
-  for (int base = 0; base < nb; base += 32) {
-    const int b = base + lane;
-    const double xm = b < nb ? a.bm[b] : 0.0, xc = b < nb ? a.bc[b] : 0.0, xg = b < nb ? a.bg[b] : 0.0;
-    const double im = am + warp_incl_scan(xm, lane), ic = ac + warp_incl_scan(xc, lane), ig = ag + warp_incl_scan(xg, lane);
-    if (b < nb) { a.bm[b] = im - xm; a.bc[b] = ic - xc; a.bg[b] = ig - xg; }
-    am = __shfl_sync(0xffffffffu, im, 31); ac = __shfl_sync(0xffffffffu, ic, 31); ag = __shfl_sync(0xffffffffu, ig, 31);
-  }
-}
-
-// scheduler.clj:2057-2071: a prefix violates when (count, cpus, mem, gpus) is not within the quota
-__global__ void __launch_bounds__(OS_TB) os_violation_tiles(OrderScan a) {
-  if (!grid_exact(a.gf, a.n)) return;
-  __shared__ int s_v[OS_TB / 32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int p0 = blockIdx.x * OS_TILE + threadIdx.x * OS_IPT;
-  int v[OS_IPT];
-#pragma unroll
-  for (int k = 0; k < OS_IPT; k++) {
-    const int p = p0 + k;
-    v[k] = 0;
-    if (p < a.n) {
-      const int u = a.user_at[p], s = a.seg_start[u];
-      double m, c, g;
-      os_user_sums(a, p, s, m, c, g);
-      const double cnt = (double)(p - s + 1);
-      v[k] = !(cnt <= a.uc.q_count[u] && c <= a.uc.q_cpus[u] && m <= a.uc.q_mem[u] && g <= a.uc.q_gpus[u]) ? 1 : 0;
-    }
-  }
-#pragma unroll
-  for (int k = 1; k < OS_IPT; k++) v[k] += v[k - 1];
-  int iv = v[OS_IPT - 1];
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, iv, o); if (lane >= o) iv += y; }
-  if (lane == 31) s_v[warp] = iv;
-  __syncthreads();
-  int ov = iv - v[OS_IPT - 1];
-  for (int w = 0; w < warp; w++) ov += s_v[w];
-#pragma unroll
-  for (int k = 0; k < OS_IPT; k++) {
-    const int p = p0 + k;
-    if (p < a.n) a.pv[p] = ov + v[k];
-  }
-  if (threadIdx.x == OS_TB - 1) a.bv[blockIdx.x] = ov + v[OS_IPT - 1];
-}
-
-__global__ void os_violation_totals(OrderScan a, int nb) {
-  if (!grid_exact(a.gf, a.n)) return;
-  const int lane = threadIdx.x;
-  int acc = 0;
-  for (int base = 0; base < nb; base += 32) {
-    const int b = base + lane;
-    const int x = b < nb ? a.bv[b] : 0;
-    int iv = x;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int y = __shfl_up_sync(0xffffffffu, iv, o); if (lane >= o) iv += y; }
-    iv += acc;
-    if (b < nb) a.bv[b] = iv - x;
-    acc = __shfl_sync(0xffffffffu, iv, 31);
-  }
-}
-
-__global__ void __launch_bounds__(OS_TB) os_finish(OrderScan a) {
-  if (!grid_exact(a.gf, a.n)) return;
+__global__ void __launch_bounds__(OS_TB) os_finish(RankScan a, const GridFlag* gf) {
+  if (!grid_exact(gf, a.n)) return;
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   bool keep = false;
   if (p < a.n) {
     const int u = a.user_at[p], s = a.seg_start[u];
-    int over = a.pv[p] + a.bv[p / OS_TILE];
-    if (s > 0) over -= a.pv[s - 1] + a.bv[(s - 1) / OS_TILE];
-    keep = over <= a.max_over_quota;
+    keep = a.viol.segment_sum(0, p, s) <= a.max_over_quota;
     double d = __longlong_as_double(0x7ff8000000000000LL);
     if (keep) {
-      double m, c, g;
-      os_user_sums(a, p, s, m, c, g);
       if (a.dru_mode == 0) {
-        const double x = m / a.uc.div_mem[u], y = c / a.uc.div_cpus[u];
+        const double x = a.amt.segment_sum(0, p, s) / a.uc.div_mem[u], y = a.amt.segment_sum(1, p, s) / a.uc.div_cpus[u];
         d = x > y ? x : y;
       } else {
-        d = g / a.uc.div_gpus[u];
+        d = a.amt.segment_sum(2, p, s) / a.uc.div_gpus[u];
       }
     }
     a.dru_at[p] = d;
@@ -370,36 +207,21 @@ struct QueueFilterArgs {
   int32_t* ti_at;
   uint8_t* flag;              // pending job still in the queue after the filters so far
   double *xc, *xm, *xg;       // its request (0 for running tasks)
-  int32_t* blk_cnt;           // per block of QF_TB entries: survivors, then exclusive offsets
+  int32_t* blk_cnt;           // per block of CP_BLOCK entries: survivors, then exclusive offsets
 };
 
 constexpr int QF_TB = 256;
 
-// Σ running usage of the pool (scheduler.clj:2118-2123) in input order.
+// Σ running usage of the pool (scheduler.clj:2118-2123) in input order, on one warp.
 __global__ void pool_usage_kernel(const double* cpus, const double* mem, const double* gpus, int R,
                                   double* out4, const GridFlag* gf) {
-  // single warp, lane-serial fold => left-fold association (any association when the sums are exact)
-  const int lane = threadIdx.x;
-  double ac = 0.0, am = 0.0, ag = 0.0;
-  if (grid_exact(gf, R)) {
-    for (int i = lane; i < R; i += 32) { ac += cpus[i]; am += mem[i]; ag += gpus[i]; }
-    for (int o = 16; o > 0; o >>= 1) {
-      ac += __shfl_xor_sync(0xffffffffu, ac, o); am += __shfl_xor_sync(0xffffffffu, am, o); ag += __shfl_xor_sync(0xffffffffu, ag, o);
-    }
-    if (lane == 0) { out4[0] = (double)R; out4[1] = ac; out4[2] = am; out4[3] = ag; }
-    return;
-  }
-  for (int base = 0; base < R; base += 32) {
-    int i = base + lane;
-    double xc = i < R ? cpus[i] : 0.0, xm = i < R ? mem[i] : 0.0, xg = i < R ? gpus[i] : 0.0;
-    int cntn = min(32, R - base);
-    for (int l = 0; l < cntn; l++) {
-      ac = ac + __shfl_sync(0xffffffffu, xc, l);
-      am = am + __shfl_sync(0xffffffffu, xm, l);
-      ag = ag + __shfl_sync(0xffffffffu, xg, l);
-    }
-  }
-  if (lane == 0) { out4[0] = (double)R; out4[1] = ac; out4[2] = am; out4[3] = ag; }
+  __shared__ double stage[3][32];
+  double acc[3] = {0.0, 0.0, 0.0};
+  warp_fold_sum<3, 4>(acc, R, grid_exact(gf, R), [&](int i, double (&x)[3]) {
+    x[0] = cpus[i]; x[1] = mem[i]; x[2] = gpus[i];
+    return true;
+  }, stage);
+  if (threadIdx.x == 0) { out4[0] = (double)R; out4[1] = acc[0]; out4[2] = acc[1]; out4[3] = acc[2]; }
 }
 
 // K5 step 1: the merged order as task indices, with each pending job's request
@@ -480,66 +302,14 @@ __global__ void __launch_bounds__(QF_CH) qf_quota_kernel(QueueFilterArgs a, cook
 }
 
 // K5 step 3: offensive-job filter (scheduler.clj:2198-2229) and order-preserving
-// compaction of the survivors: per-block counts, one scan, scatter.
-__global__ void __launch_bounds__(QF_TB) qf_count_kernel(QueueFilterArgs a) {
-  const int i = blockIdx.x * QF_TB + threadIdx.x, n = *a.n_kept;
-  bool keep = false;
-  if (i < n) {
-    keep = a.flag[i];
-    if (keep && a.filter_offensive && (a.xm[i] > a.off_mem || a.xc[i] > a.off_cpus)) {
-      keep = false;
-      a.flag[i] = 0;
-    }
+// compaction of the survivors.
+struct QueueSurvivors {
+  QueueFilterArgs a;
+  __device__ bool keep(int i) const {
+    return a.flag[i] && !(a.filter_offensive && (a.xm[i] > a.off_mem || a.xc[i] > a.off_cpus));
   }
-  const int c = __syncthreads_count(keep);
-  if (threadIdx.x == 0) a.blk_cnt[blockIdx.x] = c;
-}
-
-__global__ void __launch_bounds__(1024) qf_scan_kernel(QueueFilterArgs a, int nblk_max) {
-  __shared__ int wsum[32];
-  __shared__ int carry_s;
-  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  const int nblk = (*a.n_kept + QF_TB - 1) / QF_TB;
-  if (tid == 0) carry_s = 0;
-  __syncthreads();
-  for (int base = 0; base < nblk && base < nblk_max; base += 1024) {
-    const int b = base + tid;
-    const int v = b < nblk ? a.blk_cnt[b] : 0;
-    int x = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { int y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-    if (lane == 31) wsum[w] = x;
-    __syncthreads();
-    if (w == 0) {
-      int t = wsum[lane];
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { int y = __shfl_up_sync(0xffffffffu, t, o); if (lane >= o) t += y; }
-      wsum[lane] = t;
-    }
-    __syncthreads();
-    const int carry = carry_s;
-    const int incl = x + (w ? wsum[w - 1] : 0);
-    if (b < nblk) a.blk_cnt[b] = carry + incl - v;
-    __syncthreads();
-    if (tid == 1023) carry_s = carry + incl;
-    __syncthreads();
-  }
-  if (tid == 0) *a.out_n = carry_s;
-}
-
-__global__ void __launch_bounds__(QF_TB) qf_scatter_kernel(QueueFilterArgs a) {
-  __shared__ int wcnt[QF_TB / 32];
-  const int i = blockIdx.x * QF_TB + threadIdx.x, n = *a.n_kept;
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  const bool keep = i < n && a.flag[i];
-  const unsigned kb = __ballot_sync(0xffffffffu, keep);
-  if (lane == 0) wcnt[w] = __popc(kb);
-  __syncthreads();
-  if (blockIdx.x * QF_TB >= n) return;
-  int off = a.blk_cnt[blockIdx.x];
-  for (int k = 0; k < w; k++) off += wcnt[k];
-  if (keep) a.out_ranked[off + __popc(kb & ((1u << lane) - 1u))] = a.ti_at[i] - a.R;
-}
+  __device__ void emit(int i, int slot) const { a.out_ranked[slot] = a.ti_at[i] - a.R; }
+};
 
 template <class T>
 cudaError_t upload2(Arena& ar, cudaStream_t st, const T* a, int na, const T* b, int nb, T** out) {
@@ -588,7 +358,7 @@ extern "C" int32_t cook_rank(cook_pool* pool, const cook_tasks_soa* running,
   sz.add<double>(N + 1);                                 // dru by task (output)
   for (int k = 0; k < 3; k++) sz.add<double>(N + 1);     // queue-order requests
   sz.add<int32_t>(N + 1); sz.add<uint8_t>(N + 1);        // queue-order task index, flags
-  sz.add<int32_t>(N / QF_TB + 2); sz.add<GridFlag>(1);
+  sz.add<int32_t>(N / CP_BLOCK + 2); sz.add<GridFlag>(1);
   for (int k = 0; k < 3; k++) sz.add<double>(N + 1);     // order-wide scans: tile-local sums
   sz.add<double>(3 * (N / OS_TILE + 2)); sz.add<int32_t>(N + 1); sz.add<int32_t>(N / OS_TILE + 2);
   CK(pool, ar.reserve(sz.off + 4096));
@@ -647,27 +417,24 @@ extern "C" int32_t cook_rank(cook_pool* pool, const cook_tasks_soa* running,
   CK(pool, cudaEventRecord(pool->ev[9], st));
   const int TB = 256, nb = (N + TB - 1) / TB;
   grid_check_kernel<<<nb, TB, 0, st>>>(d_cpus, d_mem, d_gpus, N, d_gf);
-  iota_kernel<<<nb, TB, 0, st>>>(d_idx, N);
-  CK(pool, csort::sort_indices(d_idx, d_tmp, N, LessUserTask{t, d_name_rank}, st));
-  seg_bounds_kernel<<<nb, TB, 0, st>>>(d_idx, d_user, N, d_seg_start, d_seg_end, d_user_at);
+  CK(pool, csort::sort_indices(d_idx, d_tmp, N, LessUserTask{d_user, d_prio, d_start, d_tid, d_jid, d_name_rank}, st));
+  seg_bounds_kernel<<<nb, TB, 0, st>>>(SortedKey{d_idx, nullptr, d_user}, N, d_seg_start, d_seg_end, d_user_at);
   {
-    OrderScan os;
-    os.idx = d_idx; os.t = t; os.uc = uc; os.user_at = d_user_at; os.seg_start = d_seg_start;
-    os.n = N; os.dru_mode = pool->dru_mode; os.max_over_quota = params->max_over_quota_jobs; os.gf = d_gf;
-    os.pm = d_os_pm; os.pc = d_os_pc; os.pg = d_os_pg; os.bm = d_os_b; os.bc = d_os_b + os_nb + 1; os.bg = d_os_b + 2 * (os_nb + 1);
-    os.pv = d_os_pv; os.bv = d_os_bv; os.dru_at = d_dru_at; os.n_kept_total = d_counters;
-    os_amount_tiles<<<os_nb, OS_TB, 0, st>>>(os);
-    os_amount_totals<<<1, 32, 0, st>>>(os, os_nb);
-    os_violation_tiles<<<os_nb, OS_TB, 0, st>>>(os);
-    os_violation_totals<<<1, 32, 0, st>>>(os, os_nb);
-    os_finish<<<(N + OS_TB - 1) / OS_TB, OS_TB, 0, st>>>(os);
+    RankScan os;
+    os.user_at = d_user_at; os.seg_start = d_seg_start; os.uc = uc;
+    os.amt = OrderScan<double, 3>{{d_os_pm, d_os_pc, d_os_pg}, {d_os_b, d_os_b + os_nb + 1, d_os_b + 2 * (os_nb + 1)}};
+    os.viol = OrderScan<int, 1>{{d_os_pv}, {d_os_bv}};
+    os.n = N; os.dru_mode = pool->dru_mode; os.max_over_quota = params->max_over_quota_jobs;
+    os.dru_at = d_dru_at; os.n_kept_total = d_counters;
+    order_scan(os.amt, LoadAmounts{d_idx, t}, N, d_gf, st);
+    order_scan(os.viol, os, N, d_gf, st);
+    os_finish<<<(N + OS_TB - 1) / OS_TB, OS_TB, 0, st>>>(os, d_gf);
     int warps_per_block = 4;
     int blocks = (U + warps_per_block - 1) / warps_per_block;
     user_fold_kernel<<<blocks, warps_per_block * 32, 0, st>>>(
         d_idx, t, uc, d_seg_start, d_seg_end, U, pool->dru_mode, params->max_over_quota_jobs,
         d_dru_at, d_counters, d_gf, N);
   }
-  iota_kernel<<<nb, TB, 0, st>>>(d_pos, N);
   CK(pool, csort::sort_indices(d_pos, d_tmp, N,
                                LessMerge{d_dru_at, d_user_at, d_seg_start, d_name_rank}, st));
   QueueFilterArgs qa;
@@ -679,21 +446,25 @@ extern "C" int32_t cook_rank(cook_pool* pool, const cook_tasks_soa* running,
   qa.ti_at = ar.take<int32_t>(N + 1); qa.flag = ar.take<uint8_t>(N + 1);
   qa.xc = ar.take<double>(N + 1); qa.xm = ar.take<double>(N + 1); qa.xg = ar.take<double>(N + 1);
   const int qnb = (N + QF_TB - 1) / QF_TB;
-  qa.blk_cnt = ar.take<int32_t>(qnb + 1);
+  qa.blk_cnt = ar.take<int32_t>(N / CP_BLOCK + 2);
   if (!qa.blk_cnt) return set_err(pool, COOK_E_OOM, "cook_rank: arena exhausted");
   qf_gather_kernel<<<qnb, QF_TB, 0, st>>>(qa);
+  int nl = 0;   // launches besides the 14 every call makes
   if (pool_quota && pool_quota->enabled) {
+    nl += 2;
     pool_usage_kernel<<<1, 32, 0, st>>>(d_cpus, d_mem, d_gpus, R, d_pool_usage, d_gf);
     qf_quota_kernel<<<1, QF_CH, 0, st>>>(qa, *pool_quota, d_pool_usage, d_gf);
   }
   if (group_quota && group_usage && group_quota->enabled) {
     CK(pool, cudaMemcpyAsync(d_pool_usage + 4, group_usage, sizeof(double) * 4, cudaMemcpyHostToDevice, st));
+    nl++;
     qf_quota_kernel<<<1, QF_CH, 0, st>>>(qa, *group_quota, d_pool_usage + 4, d_gf);
   }
-  qf_count_kernel<<<qnb, QF_TB, 0, st>>>(qa);
-  qf_scan_kernel<<<1, 1024, 0, st>>>(qa, qnb);
-  qf_scatter_kernel<<<qnb, QF_TB, 0, st>>>(qa);
-  if (out_dru) scatter_dru_kernel<<<nb, TB, 0, st>>>(d_idx, d_dru_at, N, d_dru_task);
+  compact(QueueSurvivors{qa}, N, qa.n_kept, qa.blk_cnt, qa.out_n, N, st);
+  if (out_dru) {
+    scatter_dru_kernel<<<nb, TB, 0, st>>>(d_idx, d_dru_at, N, d_dru_task);
+    nl++;
+  }
   CK(pool, cudaGetLastError());
   CK(pool, cudaEventRecord(pool->ev[10], st));
   int32_t h_counters[2] = {0, 0};
@@ -716,9 +487,10 @@ extern "C" int32_t cook_rank(cook_pool* pool, const cook_tasks_soa* running,
     ps.ms_d2h = ev_ms(pool->ev[10], pool->ev[11]);
     ps.h2d_bytes = (int64_t)N * 56 + (int64_t)U * (4 + 7 * 8);   // task columns (56 B per task) + user tables
     ps.d2h_bytes = (int64_t)n_out * 4 + (out_order ? (int64_t)n_kept * 4 : 0) + (out_dru ? (int64_t)N * 8 : 0) + 8;
-    int nl = 0;
     for (long long w = csort::TILE; w < N; w <<= 1) nl += 2;   // the two sorts' merge passes
-    ps.n_launches = nl + 12;
+    // grid check, 2 tile sorts, segment bounds, 2 order-wide scans (2 each), finish, per-user fold,
+    // gather, compaction (3)
+    ps.n_launches = nl + 14;
   }
   *out_n = n_out;
   if (out_order_n) *out_order_n = n_kept;

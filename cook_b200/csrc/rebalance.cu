@@ -28,7 +28,7 @@
 
 #include <algorithm>
 
-#include "common.cuh"
+#include "fold.cuh"
 #include "sort.cuh"
 
 namespace {
@@ -40,21 +40,6 @@ struct RTasks {  // capacity R + max_preemption; synthetic tasks appended
   double* cm; double* cc;  // cumulative mem / cpus of the user up to and including this slot
 };
 
-struct LessUser {  // keys only: dead tasks keep their place
-  RTasks t;
-  const int32_t* name_rank;
-  __device__ bool operator()(int32_t a, int32_t b) const {
-    int ua = name_rank[t.user[a]], ub = name_rank[t.user[b]];
-    if (ua != ub) return ua < ub;
-    int pa = -t.prio[a], pb = -t.prio[b];
-    if (pa != pb) return pa < pb;
-    if (t.start[a] != t.start[b]) return t.start[a] < t.start[b];
-    if (t.tid[a] != t.tid[b]) return t.tid[a] < t.tid[b];
-    if (t.jid[a] != t.jid[b]) return t.jid[a] < t.jid[b];
-    return a < b;
-  }
-};
-
 struct LessHost {
   RTasks t;
   __device__ bool operator()(int32_t a, int32_t b) const {
@@ -63,19 +48,6 @@ struct LessHost {
     return a < b;
   }
 };
-
-__global__ void iota_r(int32_t* p, int n) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) p[i] = i;
-}
-
-__global__ void user_seg_kernel(const int32_t* ord, RTasks t, int n, int32_t* seg_start, int32_t* seg_end) {
-  int p = blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= n) return;
-  int u = t.user[ord[p]];
-  if (p == 0 || t.user[ord[p - 1]] != u) seg_start[u] = p;
-  if (p == n - 1 || t.user[ord[p + 1]] != u) seg_end[u] = p + 1;
-}
 
 // Users to re-fold after a decision, written by the kernel's next-state step.
 struct Refold {
@@ -93,116 +65,52 @@ struct Refold {
   double base_m, base_c;
 };
 
-// dru.clj:50-66: lane-serial left fold (exact association) of the users in `rf`
-// (or of every user when rf == nullptr), restarted at the first slot that changed.
+// dru.clj:50-66: one warp per user, the running sums in the reference's left-fold order (fold.cuh).
 __global__ void __launch_bounds__(128) user_dru_kernel(const int32_t* ord, RTasks t, const double* div_mem,
                                                        const double* div_cpus, const int32_t* seg_start,
-                                                       const int32_t* seg_end, int n_users, const Refold* rf,
-                                                       const GridFlag* gf, int n_scan) {
+                                                       const int32_t* seg_end, int n_users, const GridFlag* gf,
+                                                       int n_scan) {
   if (n_scan > 0 && grid_exact(gf, n_scan)) return;   // the order-wide scan below does it
-  const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int u = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
-  const bool all = rf == nullptr || rf->all;
-  if (w >= (all ? n_users : rf->n)) return;
-  const int u = all ? w : rf->user[w];
+  if (u >= n_users) return;
   const int s = seg_start[u], e = seg_end[u];
   if (e <= s) return;
-  int f = s;
-  if (!all) {
-    f = rf->from[w];
-    if (f == 0x7fffffff) f = rf->q_ins;           // only the insertion touches this user
-    else if (f >= rf->q_ins) f++;                 // slots at and after the insertion moved by one
-    if (u == rf->pu) f = min(f, rf->q_ins);
-    f = min(max(f, s), e);
-  }
+  __shared__ double stage[4][2][32];
   const double md = div_mem[u], cd = div_cpus[u];
-  double am = 0.0, ac = 0.0;
-  if (f > s) { int j = ord[f - 1]; am = t.cm[j]; ac = t.cc[j]; }
+  double acc[2] = {0.0, 0.0};   // mem, cpus
   const bool exact = grid_exact(gf, e - s);
-  for (int base = f; base < e; base += 32) {
+  for (int base = s; base < e; base += 32) {
     int p = base + lane;
     int i = p < e ? ord[p] : -1;
     const bool live = i >= 0 && t.alive[i];
-    double xm = live ? t.mem[i] : 0.0, xc = live ? t.cpus[i] : 0.0;
-    double mym = 0.0, myc = 0.0;
-    int cntn = min(32, e - base);
-    if (exact) {   // association-free sums: parallel scan
-      mym = am + warp_incl_scan(xm, lane); myc = ac + warp_incl_scan(xc, lane);
-      am = __shfl_sync(0xffffffffu, mym, 31); ac = __shfl_sync(0xffffffffu, myc, 31);
-    } else
-    for (int l = 0; l < cntn; l++) {
-      am = am + __shfl_sync(0xffffffffu, xm, l);
-      ac = ac + __shfl_sync(0xffffffffu, xc, l);
-      if (lane == l) { mym = am; myc = ac; }
-    }
+    double x[2] = {live ? t.mem[i] : 0.0, live ? t.cpus[i] : 0.0};
+    warp_fold_prefix(x, acc, min(32, e - base), exact, stage[threadIdx.x >> 5]);
     if (i >= 0) {
-      t.cm[i] = mym; t.cc[i] = myc;
-      double a = mym / md, b = myc / cd;
+      t.cm[i] = x[0]; t.cc[i] = x[1];
+      double a = x[0] / md, b = x[1] / cd;
       t.dru[i] = a > b ? a : b;
       t.pos[i] = p - s;
     }
   }
 }
 
-// The same fold for exact-grid amounts (any association gives the same bits, common.cuh): ONE
-// inclusive scan over the whole user order, a task's running sums are the scan at its slot minus the
-// scan just before its user's first slot.  A user with tens of thousands of tasks no longer sits on
-// one warp.  Three launches: tile scans, the tile totals, the per-task finish.
-constexpr int SCAN_TB = 256, SCAN_IPT = 8, SCAN_TILE = SCAN_TB * SCAN_IPT;
-
-__global__ void __launch_bounds__(SCAN_TB) order_scan_tiles(const int32_t* ord, RTasks t, int n, const GridFlag* gf,
-                                                            double* pm, double* pc, double* bt_m, double* bt_c) {
-  if (!grid_exact(gf, n)) return;
-  __shared__ double s_m[SCAN_TB / 32], s_c[SCAN_TB / 32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int p0 = blockIdx.x * SCAN_TILE + threadIdx.x * SCAN_IPT;
-  double xm[SCAN_IPT], xc[SCAN_IPT];
-#pragma unroll
-  for (int k = 0; k < SCAN_IPT; k++) {
-    const int p = p0 + k;
-    const int i = p < n ? ord[p] : -1;
-    const bool live = i >= 0 && t.alive[i];
-    xm[k] = live ? t.mem[i] : 0.0; xc[k] = live ? t.cpus[i] : 0.0;
+// The same fold for exact-grid amounts: the order-wide scan (fold.cuh) of the live amounts.
+struct LoadAlive {
+  const int32_t* ord; RTasks t;
+  __device__ void operator()(int p, double (&x)[2]) const {
+    const int i = ord[p];
+    if (t.alive[i]) { x[0] = t.mem[i]; x[1] = t.cpus[i]; }
   }
-#pragma unroll
-  for (int k = 1; k < SCAN_IPT; k++) { xm[k] = xm[k - 1] + xm[k]; xc[k] = xc[k - 1] + xc[k]; }
-  const double im = warp_incl_scan(xm[SCAN_IPT - 1], lane), ic = warp_incl_scan(xc[SCAN_IPT - 1], lane);
-  if (lane == 31) { s_m[warp] = im; s_c[warp] = ic; }
-  __syncthreads();
-  double om = im - xm[SCAN_IPT - 1], oc = ic - xc[SCAN_IPT - 1];   // exact: both on the grid
-  for (int w = 0; w < warp; w++) { om = om + s_m[w]; oc = oc + s_c[w]; }
-#pragma unroll
-  for (int k = 0; k < SCAN_IPT; k++) {
-    const int p = p0 + k;
-    if (p < n) { pm[p] = om + xm[k]; pc[p] = oc + xc[k]; }
-  }
-  if (threadIdx.x == SCAN_TB - 1) { bt_m[blockIdx.x] = om + xm[SCAN_IPT - 1]; bt_c[blockIdx.x] = oc + xc[SCAN_IPT - 1]; }
-}
+};
 
-// tile totals -> exclusive offsets, in place (one warp)
-__global__ void order_scan_totals(double* bt_m, double* bt_c, int nb, int n, const GridFlag* gf) {
-  if (!grid_exact(gf, n)) return;
-  const int lane = threadIdx.x;
-  double am = 0.0, ac = 0.0;
-  for (int base = 0; base < nb; base += 32) {
-    const int b = base + lane;
-    const double xm = b < nb ? bt_m[b] : 0.0, xc = b < nb ? bt_c[b] : 0.0;
-    const double im = am + warp_incl_scan(xm, lane), ic = ac + warp_incl_scan(xc, lane);
-    if (b < nb) { bt_m[b] = im - xm; bt_c[b] = ic - xc; }
-    am = __shfl_sync(0xffffffffu, im, 31); ac = __shfl_sync(0xffffffffu, ic, 31);
-  }
-}
-
-__global__ void order_dru_finish(const int32_t* ord, RTasks t, int n, const GridFlag* gf, const double* pm, const double* pc,
-                                 const double* bt_m, const double* bt_c, const int32_t* seg_start,
-                                 const double* div_mem, const double* div_cpus) {
+__global__ void order_dru_finish(const int32_t* ord, RTasks t, int n, const GridFlag* gf, OrderScan<double, 2> os,
+                                 const int32_t* seg_start, const double* div_mem, const double* div_cpus) {
   if (!grid_exact(gf, n)) return;
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= n) return;
   const int i = ord[p], u = t.user[i], s = seg_start[u];
-  const double gm = pm[p] + bt_m[p / SCAN_TILE], gc = pc[p] + bt_c[p / SCAN_TILE];
-  const double hm = s > 0 ? pm[s - 1] + bt_m[(s - 1) / SCAN_TILE] : 0.0, hcv = s > 0 ? pc[s - 1] + bt_c[(s - 1) / SCAN_TILE] : 0.0;
-  const double cm = gm - hm, cc = gc - hcv;
+  const double cm = os.segment_sum(0, p, s), cc = os.segment_sum(1, p, s);
   t.cm[i] = cm; t.cc[i] = cc;
   const double a = cm / div_mem[u], b = cc / div_cpus[u];
   t.dru[i] = a > b ? a : b;
@@ -250,15 +158,6 @@ __device__ __forceinline__ double csr_get(const int32_t* off, const int32_t* key
 __global__ void host_has_task_kernel(RTasks t, int n, uint8_t* has_task) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n && t.alive[i]) has_task[t.host[i]] = 1;
-}
-
-// host segments of the tasks grouped by host
-__global__ void host_seg_kernel(const int32_t* hord, RTasks t, int n, int32_t* hs, int32_t* he) {
-  int p = blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= n) return;
-  int h = t.host[hord[p]];
-  if (p == 0 || t.host[hord[p - 1]] != h) hs[h] = p;
-  if (p == n - 1 || t.host[hord[p + 1]] != h) he[h] = p + 1;
 }
 
 struct HostBest {  // best sufficient prefix of one host
@@ -556,7 +455,7 @@ __device__ __forceinline__ bool task_le_pending(const RTasks& t, int i, int ppri
 
 // P1 for one warp: job-below-quota (:210-220) and pending dru (:182-208) of pending job p.
 __device__ void pending_scalars(const RebArgs& a, const int32_t* ord, const int32_t* us, const int32_t* ue, int p,
-                                PendScalars* out) {
+                                PendScalars* out, double (*stage)[32]) {
   const int lane = threadIdx.x & 31;
   const RTasks& t = a.t;
   const PendCols& pc = a.pc;
@@ -594,31 +493,14 @@ __device__ void pending_scalars(const RebArgs& a, const int32_t* ord, const int3
   const double dmax = 1.7976931348623157e308;
   int below = 1;
   if (!(qn >= dmax && qc >= dmax && qm >= dmax && qg >= dmax)) {
-    double an = 1.0, ac = pcpu, am = pm, ag = pg;  // (conj running-jobs p): p first
+    double acc[4] = {1.0, pcpu, pm, pg};  // (conj running-jobs p): p first
     const bool exact = grid_exact(a.gf, e - s + 1) && grid_value_ok(pcpu) && grid_value_ok(pm) && grid_value_ok(pg);
-    for (int base = s; base < e; base += 32) {
-      const int q = base + lane;
-      int i = q < e ? ord[q] : -1;
-      if (i >= 0 && !t.alive[i]) i = -1;   // preempted earlier in this cycle: adds 0.0
-      const double xc = i >= 0 ? t.cpus[i] : 0.0, xm = i >= 0 ? t.mem[i] : 0.0, xg = i >= 0 ? t.gpus[i] : 0.0;
-      const double xn = i >= 0 ? 1.0 : 0.0;
-      const int cntn = min(32, e - base);
-      if (exact) {   // association-free sums: warp reduction
-        double rn = xn, rc = xc, rm = xm, rg = xg;
-        for (int o = 16; o > 0; o >>= 1) {
-          rn += __shfl_xor_sync(0xffffffffu, rn, o); rc += __shfl_xor_sync(0xffffffffu, rc, o);
-          rm += __shfl_xor_sync(0xffffffffu, rm, o); rg += __shfl_xor_sync(0xffffffffu, rg, o);
-        }
-        an += rn; ac += rc; am += rm; ag += rg;
-      } else
-      for (int l = 0; l < cntn; l++) {
-        an = an + __shfl_sync(0xffffffffu, xn, l);
-        ac = ac + __shfl_sync(0xffffffffu, xc, l);
-        am = am + __shfl_sync(0xffffffffu, xm, l);
-        ag = ag + __shfl_sync(0xffffffffu, xg, l);
-      }
-    }
-    below = (an <= qn && ac <= qc && am <= qm && ag <= qg) ? 1 : 0;
+    warp_fold_sum<4, 1>(acc, e - s, exact, [&](int k, double (&x)[4]) {
+      const int i = ord[s + k];
+      if (t.alive[i]) { x[0] = 1.0; x[1] = t.cpus[i]; x[2] = t.mem[i]; x[3] = t.gpus[i]; }   // preempted earlier in this cycle: adds 0.0
+      return true;
+    }, stage);
+    below = (acc[0] <= qn && acc[1] <= qc && acc[2] <= qm && acc[3] <= qg) ? 1 : 0;
   }
   if (lane == 0) {
     out->below_quota = below;
@@ -811,6 +693,7 @@ __global__ void __launch_bounds__(REB_TB) rebalance_kernel(RebArgs a) {
   __shared__ int s_ru[64], s_rfrom[64];
   __shared__ double s_dru[REB_TB / 32];
   __shared__ int s_rank[REB_TB / 32], s_host[REB_TB / 32];
+  __shared__ double s_stage[REB_TB / 32][4][32];   // each warp's staging area of the serial folds
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int nw = blockDim.x >> 5;
   const int gw = blockIdx.x * nw + warp, n_gw = gridDim.x * nw;
@@ -831,7 +714,7 @@ __global__ void __launch_bounds__(REB_TB) rebalance_kernel(RebArgs a) {
     const int32_t* ue = a.ue[cur];
     // ---- A: scalars of the job, then this CTA's hosts
     if (warp == 0) {
-      pending_scalars(a, ord, us, ue, p, &s_ps);
+      pending_scalars(a, ord, us, ue, p, &s_ps, s_stage[warp]);
     }
     if (warp == nw - 1) group_prepare(a, p, a.cnt[3], &s_gp);
     __syncthreads();
@@ -979,7 +862,7 @@ __global__ void __launch_bounds__(REB_TB) rebalance_kernel(RebArgs a) {
         // where the new task goes in the user order: after every task that is not greater
         // (32-ary search: the predicate "new task < ord[q]" is monotone in q)
         { const long long t1 = clock64(); tb[2] += t1 - tq; tq = t1; }
-        LessUser less{t, a.user_rank};
+        const LessUserTask less{t.user, t.prio, t.start, t.tid, t.jid, a.user_rank};
         const int ps = us[pu], pe = ue[pu];
         int lo = pe > ps ? ps : 0, hi = pe > ps ? pe : n;   // a user with tasks: inside its own segment
         while (lo < hi) {
@@ -1016,12 +899,10 @@ __global__ void __launch_bounds__(REB_TB) rebalance_kernel(RebArgs a) {
       int32_t* nus = a.us[cur ^ 1];
       int32_t* nue = a.ue[cur ^ 1];
       auto new_at = [&](int j) { return j < q ? ord[j] : (j == q ? ni : ord[j - 1]); };
+      auto user_at = [&](int j) { return t.user[new_at(j)]; };
       for (int j = gt; j <= n; j += n_gt) {
-        const int i = new_at(j);
-        nord[j] = i;
-        const int u = t.user[i];
-        if (j == 0 || t.user[new_at(j - 1)] != u) nus[u] = j;
-        if (j == n || t.user[new_at(j + 1)] != u) nue[u] = j + 1;
+        nord[j] = new_at(j);
+        mark_segment(j, n + 1, user_at, nus, nue);
       }
       const bool all = rf.all != 0;
       const int n_fold = all ? a.U : rf.n;
@@ -1078,27 +959,18 @@ __global__ void __launch_bounds__(REB_TB) rebalance_kernel(RebArgs a) {
           f = min(max(f, s), e);
         }
         const double md = a.div_mem[u], cd = a.div_cpus[u];
-        double am = 0.0, ac = 0.0;
-        if (f > s) { const int j = new_at(f - 1); am = t.cm[j]; ac = t.cc[j]; }
+        double acc[2] = {0.0, 0.0};   // mem, cpus
+        if (f > s) { const int j = new_at(f - 1); acc[0] = t.cm[j]; acc[1] = t.cc[j]; }
         const bool exact = grid_exact(a.gf, e - s);
         if (exact && !all) continue;   // done element-wise above
         for (int base = f; base < e; base += 32) {
           const int pp = base + lane;
           const int i = pp < e ? new_at(pp) : -1;
           const bool live = i >= 0 && t.alive[i];
-          const double xm = live ? t.mem[i] : 0.0, xc = live ? t.cpus[i] : 0.0;
-          double mym = 0.0, myc = 0.0;
-          const int cntn = min(32, e - base);
-          if (exact) {   // association-free sums: parallel scan
-            mym = am + warp_incl_scan(xm, lane); myc = ac + warp_incl_scan(xc, lane);
-            am = __shfl_sync(0xffffffffu, mym, 31); ac = __shfl_sync(0xffffffffu, myc, 31);
-          } else
-          for (int l = 0; l < cntn; l++) {
-            am = am + __shfl_sync(0xffffffffu, xm, l);
-            ac = ac + __shfl_sync(0xffffffffu, xc, l);
-            if (lane == l) { mym = am; myc = ac; }
-          }
+          double v[2] = {live ? t.mem[i] : 0.0, live ? t.cpus[i] : 0.0};
+          warp_fold_prefix(v, acc, min(32, e - base), exact, s_stage[warp]);
           if (i >= 0) {
+            const double mym = v[0], myc = v[1];
             t.cm[i] = mym; t.cc[i] = myc;
             const double x = mym / md, y = myc / cd;
             const double dr = x > y ? x : y;
@@ -1174,7 +1046,7 @@ static int32_t rebalance_run(cook_pool* pool, const cook_running_soa* running,
   for (int k = 0; k < 2; k++) sz.add<int32_t>(U + 1);            // second segment buffers
   sz.add<CtaBest>(4 * pool->sm_count + 8); sz.add<GridFlag>(1); sz.add<int32_t>(H + 1);
   sz.add<TaskHot>(CAP); sz.add<int32_t>(CAP); sz.add<int32_t>(H + 1); sz.add<int32_t>(CAP); sz.add<WalkBar>(1);
-  sz.add<double>(CAP); sz.add<double>(CAP); sz.add<double>(CAP / SCAN_TILE + 2); sz.add<double>(CAP / SCAN_TILE + 2);
+  sz.add<double>(CAP); sz.add<double>(CAP); sz.add<double>(CAP / OS_TILE + 2); sz.add<double>(CAP / OS_TILE + 2);
   if (tr && tr->n_forced > 0) { sz.add<cook_decision>(tr->n_forced + 1); sz.add<int32_t>(CAP + MP); }
   CK(pool, ar.reserve(sz.off + (1 << 16)));
   ar.reset();
@@ -1297,7 +1169,7 @@ static int32_t rebalance_run(cook_pool* pool, const cook_running_soa* running,
   int32_t* d_synn = ar.take<int32_t>(CAP);
   WalkBar* d_bar = ar.take<WalkBar>(1);
   double* d_pm = ar.take<double>(CAP); double* d_pc = ar.take<double>(CAP);
-  double* d_btm = ar.take<double>(CAP / SCAN_TILE + 2); double* d_btc = ar.take<double>(CAP / SCAN_TILE + 2);
+  double* d_btm = ar.take<double>(CAP / OS_TILE + 2); double* d_btc = ar.take<double>(CAP / OS_TILE + 2);
   if (ar.failed) return set_err(pool, COOK_E_OOM, "cook_rebalance: arena exhausted");
   CK(pool, cudaMemsetAsync(d_gf, 0, sizeof(GridFlag), st));
   CK(pool, cudaMemsetAsync(d_syn, 0, sizeof(int32_t) * (H + 1), st));
@@ -1321,23 +1193,20 @@ static int32_t rebalance_run(cook_pool* pool, const cook_running_soa* running,
   CK(pool, cudaMemsetAsync(d_has_task, 0, H + 1, st));
   int launches = 0;
   if (R > 0) {
-    iota_r<<<(R + TB - 1) / TB, TB, 0, st>>>(d_ord, R);
-    CK(pool, csort::sort_indices(d_ord, d_tmp, R, LessUser{t, d_urank}, st));
-    user_seg_kernel<<<(R + TB - 1) / TB, TB, 0, st>>>(d_ord, t, R, d_us, d_ue);
+    CK(pool, csort::sort_indices(d_ord, d_tmp, R, LessUserTask{t.user, t.prio, t.start, t.tid, t.jid, d_urank}, st));
+    seg_bounds_kernel<<<(R + TB - 1) / TB, TB, 0, st>>>(SortedKey{d_ord, nullptr, t.user}, R, d_us, d_ue, nullptr);
     {
-      const int nb = (R + SCAN_TILE - 1) / SCAN_TILE;
-      order_scan_tiles<<<nb, SCAN_TB, 0, st>>>(d_ord, t, R, d_gf, d_pm, d_pc, d_btm, d_btc);
-      order_scan_totals<<<1, 32, 0, st>>>(d_btm, d_btc, nb, R, d_gf);
-      order_dru_finish<<<(R + TB - 1) / TB, TB, 0, st>>>(d_ord, t, R, d_gf, d_pm, d_pc, d_btm, d_btc, d_us, d_divm, d_divc);
+      const OrderScan<double, 2> os{{d_pm, d_pc}, {d_btm, d_btc}};
+      order_scan(os, LoadAlive{d_ord, t}, R, d_gf, st);
+      order_dru_finish<<<(R + TB - 1) / TB, TB, 0, st>>>(d_ord, t, R, d_gf, os, d_us, d_divm, d_divc);
       launches += 3;
     }
-    user_dru_kernel<<<(U + 3) / 4, 128, 0, st>>>(d_ord, t, d_divm, d_divc, d_us, d_ue, U, nullptr, d_gf, R);
-    iota_r<<<(R + TB - 1) / TB, TB, 0, st>>>(d_hord, R);
+    user_dru_kernel<<<(U + 3) / 4, 128, 0, st>>>(d_ord, t, d_divm, d_divc, d_us, d_ue, U, d_gf, R);
     CK(pool, csort::sort_indices(d_hord, d_tmp, R, LessHost{t}, st));
-    host_seg_kernel<<<(R + TB - 1) / TB, TB, 0, st>>>(d_hord, t, R, d_hs, d_he);
+    seg_bounds_kernel<<<(R + TB - 1) / TB, TB, 0, st>>>(SortedKey{d_hord, nullptr, t.host}, R, d_hs, d_he, nullptr);
     host_has_task_kernel<<<(R + TB - 1) / TB, TB, 0, st>>>(t, R, d_has_task);
     hot_build_kernel<<<(R + TB - 1) / TB, TB, 0, st>>>(d_hord, t, d_urank, R, d_hot, d_hq);
-    launches += 9;
+    launches += 7;
     for (long long w = csort::TILE; w < R; w <<= 1) launches += 2;
   }
   // ---- the walk over the pending jobs: one cooperative launch, no host round trip inside

@@ -28,7 +28,7 @@ __global__ void __launch_bounds__(TILE_THREADS) tile_sort_kernel(int32_t* __rest
   const int base = blockIdx.x * TILE;
   for (int i = threadIdx.x; i < TILE; i += TILE_THREADS) {
     int g = base + i;
-    s[i] = g < n ? idx[g] : -1;  // -1 = +inf padding
+    s[i] = g < n ? g : -1;  // the identity; -1 = +inf padding
   }
   __syncthreads();
   auto lt = [&](int32_t a, int32_t b) {
@@ -90,11 +90,10 @@ __global__ void merge_pass_kernel(const int32_t* __restrict__ src, int32_t* __re
   }
 }
 
-// Sorts idx[0..n) in place; tmp must hold n int32.  Returns pointer semantics:
-// result is always left in idx.
+// Sorts the indices 0..n-1 into idx[0..n); tmp must hold n int32.
 template <class Less>
 inline cudaError_t sort_indices(int32_t* idx, int32_t* tmp, int n, Less less, cudaStream_t st) {
-  if (n <= 1) return cudaSuccess;
+  if (n <= 0) return cudaSuccess;
   int tiles = (n + TILE - 1) / TILE;
   tile_sort_kernel<Less><<<tiles, TILE_THREADS, 0, st>>>(idx, n, less);
   int32_t* src = idx;
