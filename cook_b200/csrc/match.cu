@@ -32,6 +32,7 @@
 #include <mutex>
 #include <numeric>
 
+#include "constraints.cuh"
 #include "fold.cuh"
 #include "sort.cuh"
 
@@ -247,10 +248,12 @@ __device__ __forceinline__ JobRegs load_job(const MatchArgs& a, int k) {
   return r;
 }
 
-// Static + count-dependent hard constraints of one (job, VM) pair, in Cook's
-// evaluation order (see oracle eval_pair; constraints.clj).  Group constraints
-// are handled by group_pass().  `an` = tasks assigned to the VM this cycle.
-__device__ bool constraints_pass(const MatchArgs& a, const JobRegs& r, int v, int an) {
+// Static + count-dependent hard constraints of one (job, VM) pair in Cook's evaluation order (see
+// oracle eval_pair; constraints.clj): -1, or the index of the first failing check (0 checkpoint
+// locality, 1 estimated completion, 2 user-defined attribute equals, 3 disk, 4 gpu host, 5 novel host,
+// 6 max tasks per host, 7 reservation).  Group constraints are first_failing_group's.
+// `an` = tasks assigned to the VM this cycle.
+__device__ int first_failing_constraint(const MatchArgs& a, const JobRegs& r, int v, int an) {
   const JobDev& jb = a.jb;
   const OfferDev& of = a.of;
   const int j = r.j;
@@ -263,18 +266,18 @@ __device__ bool constraints_pass(const MatchArgs& a, const JobRegs& r, int v, in
   const int disk_lo = c2.z, disk_n = c2.w;
   const int gpu_n = flags >> 8;
   if (jb.ckpt_location && jb.ckpt_location[j] >= 0) {
-    if (location != jb.ckpt_location[j]) return false;
+    if (location != jb.ckpt_location[j]) return 0;
   }
   if (jb.est_end_ms && jb.est_end_ms[j] >= 0 && host_start >= 0) {
     long long death = 1000LL * host_start + 60000LL * a.host_lifetime_mins;
-    if (!(jb.est_end_ms[j] < death)) return false;
+    if (!(jb.est_end_ms[j] < death)) return 1;
   }
   if (jb.attr_off) {
     for (int k = jb.attr_off[j]; k < jb.attr_off[j + 1]; k++) {
       int col = jb.attr_col[k], val = jb.attr_val[k];
-      if (col < 0 || col >= of.n_attr_cols) return false;
+      if (col < 0 || col >= of.n_attr_cols) return 2;
       int hv = of.attr_v[(size_t)col * of.O + v];
-      if (val <= 0 || hv != val) return false;
+      if (val <= 0 || hv != val) return 2;
     }
   }
   const bool k8s = flags & VC_K8S;
@@ -283,7 +286,7 @@ __device__ bool constraints_pass(const MatchArgs& a, const JobRegs& r, int v, in
     double space = 0.0;
     for (int i = 0; i < disk_n; i++)
       if (of.disk_type[disk_lo + i] == want) { space = of.disk_space[disk_lo + i]; break; }
-    if (!(space >= jb.disk_request[j])) return false;
+    if (!(space >= jb.disk_request[j])) return 3;
   }
   if (k8s) {
     if (r.g > 0.0) {
@@ -292,77 +295,64 @@ __device__ bool constraints_pass(const MatchArgs& a, const JobRegs& r, int v, in
       for (int i = 0; i < gpu_n; i++)
         if (of.gpu_model[gpu_lo + i] == want) { have = of.gpu_count[gpu_lo + i]; break; }
       int on_vm = run_count + an;
-      if (!(have == r.g && on_vm == 0)) return false;
+      if (!(have == r.g && on_vm == 0)) return 4;
     } else {
-      if (gpu_n != 0) return false;
+      if (gpu_n != 0) return 4;
     }
   } else if (!(r.g == 0.0)) {
-    return false;
+    return 4;
   }
   if (jb.novel_off) {
     for (int k = jb.novel_off[j]; k < jb.novel_off[j + 1]; k++)
-      if (jb.novel_host[k] == hostname) return false;
+      if (jb.novel_host[k] == hostname) return 5;
   }
   if (max_tasks >= 0) {
     int total = num_tasks + an;
-    if (!(total < max_tasks)) return false;
+    if (!(total < max_tasks)) return 6;
   }
   if (flags & VC_RESERVED) {
     int mine = jb.reserved_host ? jb.reserved_host[j] : -1;
-    if (mine != hostname) return false;
+    if (mine != hostname) return 7;
   }
-  return true;
+  return -1;
 }
 
 __device__ __forceinline__ int vm_attr(const OfferDev& of, int col, int v) {
   return (col >= 0 && col < of.n_attr_cols) ? of.attr_v[(size_t)col * of.O + v] : 0;
 }
 
-// Group constraints (constraints.clj:586-678) against the CURRENT group state
-// (running cotasks known to Fenzo + cotasks placed earlier in this cycle).
-__device__ bool group_pass(const MatchArgs& a, const JobRegs& r, int v) {
+// Group constraints of job j on VM v (constraints.clj:586-678): -1, or the index of the first failing
+// one.  A group's known members are its running cotasks, then the first n_placed(g) entries of the
+// group's placed list.  The resolver appends to that list in queue order, so the members placed by the
+// jobs before turn k are a prefix of it.
+template <class Placed>
+__device__ __forceinline__ int first_failing_group(const MatchArgs& a, int j, int v, Placed n_placed) {
   const JobDev& jb = a.jb;
   const GroupDev& gr = a.gr;
   const OfferDev& of = a.of;
-  for (int k = jb.group_off[r.j]; k < jb.group_off[r.j + 1]; k++) {
+  for (int k = jb.group_off[j]; k < jb.group_off[j + 1]; k++) {
     const int g = jb.group_idx[k];
     const int kind = gr.kind[g];
-    const int c0 = gr.cot_off[g], c1 = gr.cot_off[g + 1];
-    const int p0 = gr.gp_off[g], pn = __ldcg(gr.gp_n + g);
-    if (kind == COOK_GROUP_UNIQUE) {
+    const int c0 = gr.cot_off[g], nc = gr.cot_off[g + 1] - c0;
+    const int p0 = gr.gp_off[g], n = nc + n_placed(g);
+    auto placed = [&](int i) { return __ldcg(gr.gp_vm + p0 + i - nc); };
+    int f;
+    if (kind == COOK_GROUP_UNIQUE) {   // cotasks by hostname, this cycle's members by VM
       const int h = of.vc[v].hostname_id;
-      for (int c = c0; c < c1; c++)
-        if (gr.cot_host[c] == h) return false;
-      for (int p = 0; p < pn; p++)
-        if (__ldcg(gr.gp_vm + p0 + p) == v) return false;
+      f = group_fail(kind, n, h, 0, [&](int i) { return i < nc ? gr.cot_host[c0 + i] : (placed(i) == v ? h : ~h); });
     } else {
       const int col = gr.attr_col[g];
-      const int target = vm_attr(of, col, v);
-      const int n = (c1 - c0) + pn;
-      if (n == 0) continue;
-      auto val_at = [&](int i) { return i < c1 - c0 ? gr.cot_attr[c0 + i] : vm_attr(of, col, __ldcg(gr.gp_vm + p0 + i - (c1 - c0))); };
-      int tf = 0;
-      for (int i = 0; i < n; i++) tf += (val_at(i) == target);
-      if (kind == COOK_GROUP_ATTR_EQUALS) {
-        if (tf == 0) return false;
-      } else {  // balanced
-        if (tf == 0) continue;  // (nil? target-freq) => passes
-        int mn = 0x7fffffff, mx = 0, distinct = 0;
-        for (int i = 0; i < n; i++) {
-          int vi = val_at(i), f = 0;
-          bool first = true;
-          for (int q = 0; q < n; q++) {
-            int vq = val_at(q);
-            if (vq == vi) { f++; if (q < i) first = false; }
-          }
-          if (first) { distinct++; mn = min(mn, f); mx = max(mx, f); }
-        }
-        if (gr.minimum[g] > distinct) mn = 0;
-        if (!(mn == mx || tf < mx)) return false;
-      }
+      f = group_fail(kind, n, vm_attr(of, col, v), gr.minimum[g],
+                     [&](int i) { return i < nc ? gr.cot_attr[c0 + i] : vm_attr(of, col, placed(i)); });
     }
+    if (f >= 0) return f;
   }
-  return true;
+  return -1;
+}
+
+// against the live group state: every member placed so far
+__device__ bool group_pass(const MatchArgs& a, const JobRegs& r, int v) {
+  return first_failing_group(a, r.j, v, [&](int g) { return __ldcg(a.gr.gp_n + g); }) < 0;
 }
 
 // x / den with y = RN(1 / den) (or 0 => plain division): three dependent f64 ops
@@ -398,7 +388,7 @@ __device__ __forceinline__ double eval_vm(const MatchArgs& a, const JobRegs& r, 
       const int tot = a.of.vc[v].ports_total;
       if (r.ports > tot - st.pu) return 0.0;
     }
-    if (!constraints_pass(a, r, v, st.an)) return 0.0;
+    if (first_failing_constraint(a, r, v, st.an) >= 0) return 0.0;
     if (with_groups && !group_pass(a, r, v)) return 0.0;
   }
   return fit_fitness(r.c, r.m, st);
@@ -2159,96 +2149,17 @@ __global__ void __launch_bounds__(256) explain_kernel(MatchArgs a, const int32_t
     if (no_m) atomicAdd(&s_cnt[COOK_FAILC_MEM], 1);
     if (no_p) atomicAdd(&s_cnt[COOK_FAILC_N + 1], 1);
     if (no_c || no_m || no_p) continue;        // Fenzo evaluates constraints only when the resources fit
-    int first = -1;
-    if (has_cons) {
-      const JobDev& jb = a.jb;
-      const OfferDev& of = a.of;
-      const VmCons vc = of.vc[v];
-      const int gpu_n = vc.flags >> 8;
-      const bool k8s = vc.flags & VC_K8S;
-      if (jb.ckpt_location && jb.ckpt_location[j] >= 0 && vc.location != jb.ckpt_location[j]) first = 0;
-      if (first < 0 && jb.est_end_ms && jb.est_end_ms[j] >= 0 && vc.host_start >= 0) {
-        const long long death = 1000LL * vc.host_start + 60000LL * a.host_lifetime_mins;
-        if (!(jb.est_end_ms[j] < death)) first = 1;
-      }
-      if (first < 0 && jb.attr_off)
-        for (int q = jb.attr_off[j]; q < jb.attr_off[j + 1]; q++) {
-          const int col = jb.attr_col[q], val = jb.attr_val[q];
-          if (col < 0 || col >= of.n_attr_cols || val <= 0 || of.attr_v[(size_t)col * of.O + v] != val) { first = 2; break; }
+    int first = has_cons ? first_failing_constraint(a, r, v, an) : -1;
+    if (first < 0 && grp)   // the members Fenzo knew at the job's turn: those placed by the jobs before k
+      first = first_failing_group(a, j, v, [&](int g) {
+        int n = 0;
+        for (int k2 = 0; k2 < k; k2++) {
+          if (!(a.kflags[k2] & 1) || a.assign[k2] < 0) continue;
+          const int j2 = a.cons[k2];
+          for (int e = a.jb.group_off[j2]; e < a.jb.group_off[j2 + 1]; e++) n += a.jb.group_idx[e] == g;
         }
-      if (first < 0 && jb.disk_request && jb.disk_request[j] >= 0.0 && k8s) {
-        const int want = jb.disk_type ? jb.disk_type[j] : -1;
-        double space = 0.0;
-        for (int i = 0; i < vc.disk_n; i++)
-          if (of.disk_type[vc.disk_lo + i] == want) { space = of.disk_space[vc.disk_lo + i]; break; }
-        if (!(space >= jb.disk_request[j])) first = 3;
-      }
-      if (first < 0) {
-        bool ok = true;
-        if (k8s) {
-          if (r.g > 0.0) {
-            const int want = jb.gpu_model ? jb.gpu_model[j] : -1;
-            double have = 0.0;
-            for (int i = 0; i < gpu_n; i++)
-              if (of.gpu_model[vc.gpu_lo + i] == want) { have = of.gpu_count[vc.gpu_lo + i]; break; }
-            ok = have == r.g && vc.run_count + an == 0;
-          } else ok = gpu_n == 0;
-        } else ok = r.g == 0.0;
-        if (!ok) first = 4;
-      }
-      if (first < 0 && jb.novel_off)
-        for (int q = jb.novel_off[j]; q < jb.novel_off[j + 1]; q++)
-          if (jb.novel_host[q] == vc.hostname_id) { first = 5; break; }
-      if (first < 0 && vc.max_tasks >= 0 && !(vc.num_tasks + an < vc.max_tasks)) first = 6;
-      if (first < 0 && (vc.flags & VC_RESERVED)) {
-        const int mine = jb.reserved_host ? jb.reserved_host[j] : -1;
-        if (mine != vc.hostname_id) first = 7;
-      }
-      if (first < 0 && grp) {
-        // group constraints against the cotasks Fenzo knew at the job's turn: running cotasks + members
-        // placed EARLIER in this cycle (rebuilt from the assignments of the jobs before k)
-        for (int q = jb.group_off[j]; q < jb.group_off[j + 1] && first < 0; q++) {
-          const int g = jb.group_idx[q];
-          const int kind = a.gr.kind[g];
-          const int c0 = a.gr.cot_off[g], c1 = a.gr.cot_off[g + 1];
-          const int col = a.gr.attr_col[g];
-          int tf = 0, n = 0, mn = 0x7fffffff, mx = 0, distinct = 0;
-          const int target = vm_attr(of, col, v);
-          auto member_vm = [&](int k2) -> int {   // VM of an earlier job of group g, or -1
-            if (!(a.kflags[k2] & 1) || a.assign[k2] < 0) return -1;
-            const int j2 = a.cons[k2];
-            for (int e = jb.group_off[j2]; e < jb.group_off[j2 + 1]; e++) if (jb.group_idx[e] == g) return a.assign[k2];
-            return -1;
-          };
-          if (kind == COOK_GROUP_UNIQUE) {
-            bool clash = false;
-            for (int c = c0; c < c1; c++) clash |= a.gr.cot_host[c] == vc.hostname_id;
-            for (int k2 = 0; k2 < k && !clash; k2++) clash = member_vm(k2) == v;
-            if (clash) first = 8;
-          } else {
-            // value frequencies over (running cotasks ++ earlier members): O(n^2) over a handful of values
-            int vals[64];   // members of one group known to Fenzo at the turn (cook_groups are small)
-            int nv = 0;
-            for (int c = c0; c < c1 && nv < 64; c++) vals[nv++] = a.gr.cot_attr[c];
-            for (int k2 = 0; k2 < k && nv < 64; k2++) { const int mv = member_vm(k2); if (mv >= 0) vals[nv++] = vm_attr(of, col, mv); }
-            n = nv;
-            for (int i = 0; i < n; i++) tf += vals[i] == target;
-            if (n > 0) {
-              if (kind == COOK_GROUP_ATTR_EQUALS) { if (tf == 0) first = 10; }
-              else if (tf != 0) {
-                for (int i = 0; i < n; i++) {
-                  int f = 0; bool fst = true;
-                  for (int e = 0; e < n; e++) if (vals[e] == vals[i]) { f++; if (e < i) fst = false; }
-                  if (fst) { distinct++; mn = min(mn, f); mx = max(mx, f); }
-                }
-                if (a.gr.minimum[g] > distinct) mn = 0;
-                if (!(mn == mx || tf < mx)) first = 9;
-              }
-            }
-          }
-        }
-      }
-    }
+        return n;
+      });
     if (first >= 0) atomicAdd(&s_cnt[COOK_FAILC_FIRST_CONSTRAINT + first], 1);
     else atomicAdd(&s_cnt[COOK_FAILC_N], 1);
   }

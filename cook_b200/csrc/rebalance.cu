@@ -28,6 +28,7 @@
 
 #include <algorithm>
 
+#include "constraints.cuh"
 #include "fold.cuh"
 #include "sort.cuh"
 
@@ -596,10 +597,7 @@ __device__ bool host_groups_ok(const RebArgs& a, const GroupPre& G, int h, int n
       const unsigned m = __ballot_sync(0xffffffffu, e > 0);
       const int tf = m ? __shfl_sync(0xffffffffu, e, __ffs(m) - 1) : 0;
       if (kind == COOK_GROUP_ATTR_EQUALS) { if (tf == 0) return false; }
-      else if (tf != 0) {
-        const int mn = G.minimum[g] > nv ? 0 : G.mn[g], mx = G.mx[g];
-        if (!(mn == mx || tf < mx)) return false;
-      }
+      else if (tf != 0 && !balanced_ok(tf, G.mn[g], G.mx[g], nv, G.minimum[g])) return false;
     }
   }
   return true;
@@ -648,37 +646,23 @@ __device__ bool host_ok(const RebArgs& a, int p, int h, int np, const GroupPre& 
     if (loc != pc.ckpt_location[p]) pass = false;
   }
   if (pass && !G.slow) return host_groups_ok(a, G, h, np, have);
-  if (pass && pc.group_off && gc.n > 0) {
-    for (int k = pc.group_off[p]; k < pc.group_off[p + 1] && pass; k++) {
+  if (pass && pc.group_off && gc.n > 0) {   // over [hosts preempted so far ; cotasks]
+    for (int k = pc.group_off[p]; k < pc.group_off[p + 1]; k++) {
       const int gi = pc.group_idx[k];
       const int kind = gc.kind[gi];
-      const int col = gc.attr_col ? gc.attr_col[gi] : -1;
-      const int c0 = gc.cot_off[gi], c1 = gc.cot_off[gi + 1];
-      auto hattr = [&](int hh) { return (col >= 0 && col < hc.n_attr_cols) ? hc.attr[(size_t)col * hc.H + hh] : 0; };
+      const int c0 = gc.cot_off[gi], nc = gc.cot_off[gi + 1] - c0;
+      int f;
       if (kind == COOK_GROUP_UNIQUE) {
-        if (!have) { pass = false; break; }
-        const int hn = hc.hostname_id[h];
-        for (int q = 0; q < np; q++) if (hc.hostname_id[a.preempted_hosts[q]] == hn) pass = false;
-        for (int c = c0; c < c1; c++) if (gc.cot_host[c] == hn) pass = false;
+        if (!have) return false;
+        f = group_fail(kind, np + nc, hc.hostname_id[h], 0,
+                       [&](int i) { return i < np ? hc.hostname_id[a.preempted_hosts[i]] : gc.cot_host[c0 + i - np]; });
       } else {
-        const int n = np + (c1 - c0);
-        if (n == 0) continue;
-        auto val_at = [&](int i) { return i < np ? hattr(a.preempted_hosts[i]) : gc.cot_attr[c0 + i - np]; };
-        const int target = have ? hattr(h) : 0;
-        int tf = 0;
-        for (int i = 0; i < n; i++) tf += (val_at(i) == target);
-        if (kind == COOK_GROUP_ATTR_EQUALS) { if (tf == 0) pass = false; }
-        else if (tf != 0) {
-          int mn = 0x7fffffff, mx = 0, distinct = 0;
-          for (int i = 0; i < n; i++) {
-            int vi = val_at(i), f = 0; bool first = true;
-            for (int q = 0; q < n; q++) { int vq = val_at(q); if (vq == vi) { f++; if (q < i) first = false; } }
-            if (first) { distinct++; mn = min(mn, f); mx = max(mx, f); }
-          }
-          if (gc.minimum[gi] > distinct) mn = 0;
-          if (!(mn == mx || tf < mx)) pass = false;
-        }
+        const int col = gc.attr_col ? gc.attr_col[gi] : -1;
+        auto hattr = [&](int hh) { return (col >= 0 && col < hc.n_attr_cols) ? hc.attr[(size_t)col * hc.H + hh] : 0; };
+        f = group_fail(kind, np + nc, have ? hattr(h) : 0, gc.minimum[gi],
+                       [&](int i) { return i < np ? hattr(a.preempted_hosts[i]) : gc.cot_attr[c0 + i - np]; });
       }
+      if (f >= 0) return false;
     }
   }
   return pass;
