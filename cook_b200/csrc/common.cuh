@@ -15,11 +15,10 @@ struct cook_ctx {
   std::vector<int> devices;
 };
 
-// Grow-only device arena: one cudaMalloc per high-water mark, carved per call.
+// Grow-only device arena: one cudaMalloc per high-water mark, carved per call by carve() below.
 struct Arena {
   char* base = nullptr;
-  size_t cap = 0, off = 0;
-  bool failed = false;  // sticky: some take() since the last reset() did not fit
+  size_t cap = 0;
   cudaError_t reserve(size_t bytes) {
     if (bytes <= cap) return cudaSuccess;
     if (base) cudaFree(base);
@@ -30,28 +29,89 @@ struct Arena {
     if (e == cudaSuccess) cap = want;
     return e;
   }
-  void reset() { off = 0; failed = false; }
-  template <class T>
-  T* take(size_t n) {
-    size_t bytes = (n * sizeof(T) + 255) & ~size_t(255);
-    if (off + bytes > cap) { failed = true; return nullptr; }
-    T* p = reinterpret_cast<T*>(base + off);
-    off += bytes;
-    return p;
-  }
   void release() {
     if (base) cudaFree(base);
     base = nullptr;
-    cap = off = 0;
+    cap = 0;
   }
 };
 
-// Sizing pass helper: mirrors Arena::take without memory.
-struct Sizer {
-  size_t off = 0;
+// One pass over a call's device buffers (see carve()).  While measuring (base == nullptr) every take
+// returns nullptr and only advances the offset; while carving it returns the arena's memory and the
+// uploads are queued on the stream.
+struct Carve {
+  char* base = nullptr;
+  size_t cap = 0, off = 0;
+  cudaStream_t st = nullptr;
+  int64_t h2d = 0;                   // bytes uploaded
+  cudaError_t err = cudaSuccess;     // sticky: the first take that did not fit or the first failed copy
   template <class T>
-  void add(size_t n) { off += (n * sizeof(T) + 255) & ~size_t(255); }
+  T* take(size_t n) {
+    const size_t bytes = (n * sizeof(T) + 255) & ~size_t(255);
+    T* p = nullptr;
+    if (base && off + bytes <= cap) p = reinterpret_cast<T*>(base + off);
+    else if (base && err == cudaSuccess) err = cudaErrorMemoryAllocation;
+    off += bytes;
+    return p;
+  }
+  template <class T>
+  void copy(T* dev, const T* host, size_t n) {
+    if (!dev || n == 0 || err != cudaSuccess) return;
+    err = host ? cudaMemcpyAsync(dev, host, n * sizeof(T), cudaMemcpyHostToDevice, st) : cudaErrorInvalidValue;
+    h2d += (int64_t)(n * sizeof(T));
+  }
+  // a host column: null stays null (no take), an empty one gets one element
+  template <class T>
+  T* up(const T* host, size_t n) {
+    if (!host) return nullptr;
+    T* d = take<T>(n ? n : 1);
+    copy(d, host, n);
+    return d;
+  }
+  // a[0, na) followed by b[0, nb), and one spare element
+  template <class T>
+  T* cat(const T* a, size_t na, const T* b, size_t nb) {
+    T* d = take<T>(na + nb + 1);
+    copy(d, a, na);
+    if (d) copy(d + na, b, nb);
+    return d;
+  }
+  // cap_n elements that start with host[0, n).  `zero`: all cap_n are zeroed first, and a null host
+  // leaves them so.
+  template <class T>
+  T* part(const T* host, size_t n, size_t cap_n, bool zero = false) {
+    T* d = take<T>(cap_n);
+    if (zero && d && err == cudaSuccess) err = cudaMemsetAsync(d, 0, cap_n * sizeof(T), st);
+    if (host || !zero) copy(d, host, n);
+    return d;
+  }
 };
+
+// Carves one call's buffers from `a`.  body(Carve&) lists them once and runs twice: measuring, with no
+// CUDA call, then (after the arena is grown to the measured size) carving.  Both runs make the same takes
+// in the same order, so the arena is sized by the list it is carved by; the body therefore branches on
+// host data only.  `start` (if any) is recorded on st once the arena is large enough, before the first
+// upload.  Adds the uploaded bytes to *h2d.
+template <class Body>
+inline cudaError_t carve(Arena& a, cudaStream_t st, cudaEvent_t start, int64_t* h2d, const Body& body) {
+  Carve m;
+  body(m);
+  cudaError_t e = a.reserve(m.off);
+  if (e == cudaSuccess && start) e = cudaEventRecord(start, st);
+  if (e != cudaSuccess) return e;
+  Carve c;
+  c.base = a.base; c.cap = a.cap; c.st = st;
+  body(c);
+  *h2d += c.h2d;
+  return c.err;
+}
+
+// A device-to-host copy on st whose bytes count towards *d2h.
+template <class T>
+inline cudaError_t download(T* host, const T* dev, size_t n, cudaStream_t st, int64_t* d2h) {
+  *d2h += (int64_t)(n * sizeof(T));
+  return cudaMemcpyAsync(host, dev, n * sizeof(T), cudaMemcpyDeviceToHost, st);
+}
 
 struct cook_pool {
   cook_ctx* ctx = nullptr;
@@ -65,8 +125,6 @@ struct cook_pool {
   double* xchg = nullptr;                // exchange buffers: [n_pad] local + [world * n_pad] gathered
   size_t xchg_cap = 0;
   Arena arena;
-  void* pinned = nullptr;  // small pinned scratch for result scalars
-  size_t pinned_cap = 0;
   void* match_plan = nullptr;            // MatchPlan (match.cu), resident inputs
   void (*match_plan_free)(void*) = nullptr;
   char err[512] = {0};
@@ -90,20 +148,6 @@ inline int32_t set_err(cook_pool* p, int32_t code, const char* fmt, ...) {
                      "%s:%d %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(_e)); \
   } while (0)
 
-// Upload a host column (may be NULL => returns nullptr without copying).
-template <class T>
-inline cudaError_t upload(Arena& a, cudaStream_t s, const T* host, size_t n, T** out) {
-  *out = nullptr;
-  if (!host || n == 0) {
-    if (host) *out = a.take<T>(1);
-    return cudaSuccess;
-  }
-  T* d = a.take<T>(n);
-  if (!d) return cudaErrorMemoryAllocation;
-  *out = d;
-  return cudaMemcpyAsync(d, host, n * sizeof(T), cudaMemcpyHostToDevice, s);
-}
-
 // Host-side range check of an index column: a bad index from the shim must come back as
 // COOK_E_BADARG, not as an illegal-address fault that poisons the CUDA context of every pool.
 inline bool idx_in_range(const int32_t* col, size_t n, int32_t lo, int32_t hi_excl) {
@@ -117,6 +161,13 @@ inline float ev_ms(cudaEvent_t a, cudaEvent_t b) {
   float ms = 0.f;
   cudaEventElapsedTime(&ms, a, b);
   return ms;
+}
+
+// The statistics of the last call of `phase`: its upload, device and download stages lie between the
+// events up .. dev .. d2h .. end (a null `up`: no upload stage).
+inline void record_phase(cook_pool* p, int phase, cudaEvent_t up, cudaEvent_t dev, cudaEvent_t d2h, cudaEvent_t end,
+                         int64_t h2d_bytes, int64_t d2h_bytes, int32_t launches) {
+  p->phase[phase] = {up ? ev_ms(up, dev) : 0.0, ev_ms(dev, d2h), ev_ms(d2h, end), h2d_bytes, d2h_bytes, launches, 0};
 }
 
 // ---------------------------------------------------------------------------------------------

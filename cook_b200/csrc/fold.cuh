@@ -150,7 +150,7 @@ __global__ void seg_bounds_kernel(SortedKey key, int n, int32_t* seg_start, int3
 // ---- order-wide scan, exact grid only: a running sum over one segment of a sorted order is ONE
 // inclusive scan over the whole order minus the scan just before the segment's first position, so no
 // segment, however long, sits on one warp.  Two launches: tile scans, then one warp turns the tile
-// totals into exclusive offsets.  Both do nothing unless grid_exact(gf, n).
+// totals into exclusive offsets.  Both do nothing unless grid_exact(gf, n); *launches (if given) counts them.
 constexpr int OS_TB = 256, OS_IPT = 8, OS_TILE = OS_TB * OS_IPT;
 
 template <class T, int K>
@@ -225,16 +225,19 @@ __global__ void order_scan_totals(OrderScan<T, K> os, int nb, int n, const GridF
 }
 
 template <class T, int K, class Load>
-inline void order_scan(const OrderScan<T, K>& os, const Load& load, int n, const GridFlag* gf, cudaStream_t st) {
+inline void order_scan(const OrderScan<T, K>& os, const Load& load, int n, const GridFlag* gf, cudaStream_t st,
+                       int* launches = nullptr) {
   const int nb = (n + OS_TILE - 1) / OS_TILE;
   order_scan_tiles<<<nb, OS_TB, 0, st>>>(os, load, n, gf);
   order_scan_totals<<<1, 32, 0, st>>>(os, nb, n, gf);
+  if (launches) *launches += 2;
 }
 
 // ---- stable stream compaction: the items i < n with f.keep(i) go, in order, to slots 0, 1, ... through
 // f.emit(i, slot) for the slots below cap, and *out_n = min(count, cap).  n is *n_dev when that is given
 // (a count only the device knows), at most n_max, which sizes the grid and blk[n_max / CP_BLOCK + 1].
-// Three launches: per-block counts, one warp turns them into exclusive offsets, scatter.
+// Three launches, counted in *launches if given: per-block counts, one warp turns them into exclusive offsets,
+// scatter.
 constexpr int CP_TB = 256, CP_ITEMS = 4, CP_BLOCK = CP_TB * CP_ITEMS;
 
 __device__ __forceinline__ int compact_n(const int32_t* n_dev, int n_max) { return n_dev ? min(*n_dev, n_max) : n_max; }
@@ -300,11 +303,13 @@ __global__ void __launch_bounds__(CP_TB) compact_scatter_kernel(F f, const int32
 }
 
 template <class F>
-inline void compact(const F& f, int n_max, const int32_t* n_dev, int32_t* blk, int32_t* out_n, int cap, cudaStream_t st) {
+inline void compact(const F& f, int n_max, const int32_t* n_dev, int32_t* blk, int32_t* out_n, int cap, cudaStream_t st,
+                    int* launches = nullptr) {
   const int nb = (n_max + CP_BLOCK - 1) / CP_BLOCK;
   compact_count_kernel<<<nb, CP_TB, 0, st>>>(f, n_dev, n_max, blk);
   compact_scan_kernel<<<1, 32, 0, st>>>(blk, n_dev, n_max, out_n, cap);
   compact_scatter_kernel<<<nb, CP_TB, 0, st>>>(f, n_dev, n_max, blk, cap);
+  if (launches) *launches += 3;
 }
 
 }  // namespace

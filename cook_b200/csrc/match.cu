@@ -2274,12 +2274,6 @@ static void plan_free(void* p) {
   if (mp) { mp->arena.release(); delete mp; }
 }
 
-#define UP(dst, src, n)                                                   \
-  do {                                                                    \
-    CK(pool, upload(ar, st, (src), (size_t)(n), &(dst)));                 \
-    if (src) mp->h2d_bytes += (int64_t)sizeof(*(src)) * (int64_t)(n);     \
-  } while (0)
-
 static int32_t build_plan(cook_pool* pool, MatchPlan* mp, const int32_t* ranked_idx,
                           int32_t n_ranked, const cook_jobs_soa* jobs,
                           const cook_offers_soa* offers, const cook_groups* groups,
@@ -2289,7 +2283,6 @@ static int32_t build_plan(cook_pool* pool, MatchPlan* mp, const int32_t* ranked_
   Arena& ar = mp->arena;
   const int J = jobs->n, O = offers->n, U = users->n_users, NC = params->num_considerable;
   mp->valid = false;
-  mp->h2d_bytes = 0;
   // host-side prep: offers sorted by hostname rank (tie-break order)
   std::vector<int32_t> perm(O, -1);
   bool dense = true;  // name_rank is normally a permutation of 0..O-1: invert it directly
@@ -2338,186 +2331,147 @@ static int32_t build_plan(cook_pool* pool, MatchPlan* mp, const int32_t* ranked_
   if (const char* eb = getenv("COOK_MATCH_TARGET")) { int v = atoi(eb); if (v >= 1) btarget = v; }
   bmax = std::max(bmax, std::max(B, bmin));
   const size_t max_blocks = (size_t)NC / std::min(B, bmin) + 8;
-  Sizer sz;
-  sz.add<int32_t>(n_ranked);
-  for (int k = 0; k < 3; k++) sz.add<double>(J + 1);
-  sz.add<int32_t>(J + 1); sz.add<int32_t>(J + 1);
-  sz.add<uint8_t>(J + 1); sz.add<uint8_t>(J + 1); sz.add<uint8_t>(J + 1); sz.add<GridFlag>(1);
-  size_t csr_j = (jobs->novel_off ? jobs->novel_off[J] : 0) + 2 * (size_t)(jobs->attr_off ? jobs->attr_off[J] : 0) + n_memb;
-  sz.add<int32_t>(4 * (size_t)(J + 2) + csr_j + 64);
-  sz.add<double>(J + 1); sz.add<int32_t>(3 * (size_t)(J + 1)); sz.add<int64_t>(J + 1);
-  sz.add<int32_t>(O + 1);
-  for (int k = 0; k < 8; k++) sz.add<double>(O + 1);
-  sz.add<int32_t>(12 * (size_t)(O + 2));
-  size_t csr_o = (offers->port_off ? 2 * (size_t)offers->port_off[O] : 0) +
-                 (offers->gpu_off ? (size_t)offers->gpu_off[O] : 0) +
-                 (offers->disk_off ? (size_t)offers->disk_off[O] : 0);
-  sz.add<int32_t>(csr_o + 64); sz.add<double>(csr_o + 64);
-  sz.add<int64_t>(O + 1); sz.add<uint8_t>(2 * (size_t)(O + 1));
-  sz.add<int32_t>((size_t)offers->n_attr_cols * O + 1);
-  if (G) {
-    sz.add<int32_t>(6 * (size_t)(G + 2));
-    sz.add<int32_t>(2 * (size_t)(groups->cot_off ? groups->cot_off[G] : 0) + 64);
-    sz.add<int32_t>(n_memb + 64);
-  }
-  for (int k = 0; k < 9; k++) sz.add<double>(U);
-  sz.add<int32_t>(U);
-  for (int k = 0; k < 4; k++) sz.add<double>(O + 1);
-  for (int k = 0; k < 4; k++) sz.add<int32_t>(O + 1);
-  for (int k = 0; k < 6; k++) sz.add<int32_t>(n_ranked + 1);
-  sz.add<uint8_t>(n_ranked + 1);
-  sz.add<int32_t>(NC + 1); sz.add<double>(NC + 1); sz.add<double>(NC + 1); sz.add<uint8_t>(NC + 1);
-  sz.add<unsigned char>((size_t)2 * bmax * ROW_BYTES); sz.add<double>(NC + bmax + 1); sz.add<int32_t>(NC + bmax + 1);
-  sz.add<unsigned>((size_t)2 * bmax * ((O + 31) / 32) + 4);
-  sz.add<int32_t>(2 * bmax + 16); sz.add<unsigned>(max_blocks + 8); sz.add<int32_t>(max_blocks + 8);
-  sz.add<int32_t>(NC + 1); sz.add<int32_t>(NC + 1); sz.add<uint8_t>(NC + 1);
-  sz.add<int32_t>(NC + 1); sz.add<int32_t>((size_t)NC * std::max(max_ports, 1) + 1);
-  sz.add<int32_t>(O + 1);
-  sz.add<unsigned long long>(32); sz.add<int32_t>(16);
-  sz.add<VmStatic>(O + 1); sz.add<VmDyn>(O + 1); sz.add<VmDyn>(O + 1); sz.add<int>(O + 1);
-  sz.add<VmCnt>(O + 1); sz.add<VmCnt>(O + 1);
-  sz.add<VmCons>(O + 1); sz.add<int32_t>((size_t)offers->n_attr_cols * O + 1);
-  sz.add<double>(NC + 1); sz.add<double>(NC + 1); sz.add<double>(NC / 256 + 2); sz.add<double>(NC / 256 + 2);
-  sz.add<LogEnt>(LOGN); sz.add<int4>(LOGN); sz.add<unsigned long long>(4); sz.add<int32_t>(max_blocks + 8);
-  sz.add<SpecOut>(GRING); sz.add<unsigned>(GRING); sz.add<int>((size_t)(MAX_SPEC_CTAS + 1) * (O + 1));
-  CK(pool, ar.reserve(sz.off + (1 << 18)));
-  ar.reset();
-
   ConsArgs& ca = mp->ca;
-  memset(&ca, 0, sizeof(ca));
-  int32_t* d_ranked; UP(d_ranked, ranked_idx, n_ranked);
+  MatchArgs& ma = mp->ma;
   JobDev jb;
-  memset(&jb, 0, sizeof(jb));
-  { int32_t* p; UP(p, jobs->user, J); jb.user = p; }
-  { double* p; UP(p, jobs->cpus, J); jb.cpus = p; UP(p, jobs->mem, J); jb.mem = p;
-    UP(p, jobs->gpus, J); jb.gpus = p; }
-  { int32_t* p; UP(p, jobs->ports, J); jb.ports = p; }
-  { uint8_t* p; UP(p, jobs->allowed, J); jb.allowed = p; UP(p, jobs->plugin_accept, J); jb.plugin = p; }
-  if (jobs->novel_off) { int32_t* p; UP(p, jobs->novel_off, J + 1); jb.novel_off = p;
-    UP(p, jobs->novel_host, std::max(1, jobs->novel_off[J])); jb.novel_host = p; }
-  { int32_t* p; UP(p, jobs->gpu_model, J); jb.gpu_model = p; }
-  { double* p; UP(p, jobs->disk_request, J); jb.disk_request = p; }
-  { int32_t* p; UP(p, jobs->disk_type, J); jb.disk_type = p; }
-  if (jobs->attr_off) { int32_t* p; UP(p, jobs->attr_off, J + 1); jb.attr_off = p;
-    int na = std::max(1, jobs->attr_off[J]);
-    UP(p, jobs->attr_col, na); jb.attr_col = p; UP(p, jobs->attr_val, na); jb.attr_val = p; }
-  { int64_t* p; UP(p, jobs->est_end_ms, J); jb.est_end_ms = p; }
-  { int32_t* p; UP(p, jobs->ckpt_location, J); jb.ckpt_location = p;
-    UP(p, jobs->reserved_host, J); jb.reserved_host = p; }
-  if (jobs->group_off && G) { int32_t* p; UP(p, jobs->group_off, J + 1); jb.group_off = p;
-    UP(p, jobs->group_idx, std::max<size_t>(1, n_memb)); jb.group_idx = p; }
-
   OfferDev of;
-  memset(&of, 0, sizeof(of));
-  of.O = O;
-  { const int32_t* hp = perm.data(); UP(mp->d_perm, hp, O); of.perm = mp->d_perm; }
-  UP(mp->d_oc, offers->cpus, O); UP(mp->d_om, offers->mem, O);
-  UP(mp->d_orc, offers->run_cpus, O); UP(mp->d_orm, offers->run_mem, O);
-  mp->d_vs = ar.take<VmStatic>(O + 1);
-  of.vs = mp->d_vs;
-  { int32_t* p; UP(p, offers->hostname_id, O); of.hostname_id = p;
-    UP(p, offers->run_count, O); of.run_count = p; }
-  mp->d_ports_total = nullptr;
-  if (offers->port_off) { int32_t* p; UP(p, offers->port_off, O + 1); of.port_off = p;
-    int np = std::max(1, offers->port_off[O]);
-    UP(p, offers->port_begin, np); of.port_begin = p; UP(p, offers->port_end, np); of.port_end = p;
-    mp->d_ports_total = ar.take<int32_t>(O + 1); of.ports_total = mp->d_ports_total; }
-  { uint8_t* p; UP(p, offers->is_k8s, O); of.is_k8s = p; UP(p, offers->reserved, O); of.reserved = p; }
-  { int32_t* p; UP(p, offers->location, O); of.location = p; }
-  if (offers->gpu_off) { int32_t* p; UP(p, offers->gpu_off, O + 1); of.gpu_off = p;
-    int ng = std::max(1, offers->gpu_off[O]); UP(p, offers->gpu_model, ng); of.gpu_model = p;
-    double* q; UP(q, offers->gpu_count, ng); of.gpu_count = q; }
-  if (offers->disk_off) { int32_t* p; UP(p, offers->disk_off, O + 1); of.disk_off = p;
-    int nd = std::max(1, offers->disk_off[O]); UP(p, offers->disk_type, nd); of.disk_type = p;
-    double* q; UP(q, offers->disk_space, nd); of.disk_space = q; }
-  { int32_t* p; UP(p, offers->max_tasks, O); of.max_tasks = p; UP(p, offers->num_tasks, O); of.num_tasks = p; }
-  { int64_t* p; UP(p, offers->host_start_time, O); of.host_start = p; }
-  of.n_attr_cols = offers->attr ? offers->n_attr_cols : 0;
-  if (of.n_attr_cols > 0) { int32_t* p; UP(p, offers->attr, (size_t)of.n_attr_cols * O); of.attr = p; }
-  mp->d_vc = ar.take<VmCons>(O + 1);
-  mp->d_attr_v = ar.take<int32_t>((size_t)of.n_attr_cols * O + 1);
-  of.vc = mp->d_vc; of.attr_v = mp->d_attr_v;
-  if ((jb.novel_off || of.reserved || (G && jb.group_off)) && !of.hostname_id)
-    return set_err(pool, COOK_E_BADARG, "cook_match: hostname_id column required by constraints");
-
   GroupDev gr;
+  memset(&ca, 0, sizeof(ca));
+  memset(&ma, 0, sizeof(ma));
+  memset(&jb, 0, sizeof(jb));
+  memset(&of, 0, sizeof(of));
   memset(&gr, 0, sizeof(gr));
-  if (G && jb.group_off) {
-    gr.n_groups = G;
-    int32_t* p;
-    UP(p, groups->kind, G); gr.kind = p;
-    UP(p, groups->attr_col, G); gr.attr_col = p;
-    UP(p, groups->minimum, G); gr.minimum = p;
-    UP(p, groups->cot_off, G + 1); gr.cot_off = p;
-    int nc = std::max(1, groups->cot_off ? groups->cot_off[G] : 0);
-    UP(p, groups->cot_hostname_id, nc); gr.cot_host = p;
-    UP(p, groups->cot_attr_val, nc); gr.cot_attr = p;
-    { const int32_t* hp = gp_off.data(); UP(p, hp, G + 1); gr.gp_off = p; }
-    gr.gp_n = ar.take<int32_t>(G + 1);
-    gr.gp_vm = ar.take<int32_t>(n_memb + 1);
-    if (!gr.cot_off || !gr.kind) return set_err(pool, COOK_E_BADARG, "cook_match: incomplete cook_groups");
-  }
-  ca.ranked = d_ranked; ca.n_ranked = n_ranked; ca.jb = jb; ca.n_users = U;
-  { double* p;
-    UP(p, users->quota_count, U); ca.q_count = p; UP(p, users->quota_cpus, U); ca.q_cpus = p;
-    UP(p, users->quota_mem, U); ca.q_mem = p; UP(p, users->quota_gpus, U); ca.q_gpus = p;
-    UP(p, users->usage_count, U); ca.u_count = p; UP(p, users->usage_cpus, U); ca.u_cpus = p;
-    UP(p, users->usage_mem, U); ca.u_mem = p; UP(p, users->usage_gpus, U); ca.u_gpus = p; }
-  { int32_t* p; UP(p, users->tokens, U); ca.tokens = p; }
+  of.O = O;
+  of.n_attr_cols = offers->attr ? offers->n_attr_cols : 0;
+  mp->h2d_bytes = 0;
+  const cudaError_t carved = carve(ar, st, nullptr, &mp->h2d_bytes, [&](Carve& c) {
+    ca.ranked = c.up(ranked_idx, n_ranked);
+    jb.user = c.up(jobs->user, J);
+    jb.cpus = c.up(jobs->cpus, J); jb.mem = c.up(jobs->mem, J); jb.gpus = c.up(jobs->gpus, J);
+    jb.ports = c.up(jobs->ports, J);
+    jb.allowed = c.up(jobs->allowed, J); jb.plugin = c.up(jobs->plugin_accept, J);
+    if (jobs->novel_off) {
+      jb.novel_off = c.up(jobs->novel_off, J + 1);
+      jb.novel_host = c.up(jobs->novel_host, std::max(1, jobs->novel_off[J]));
+    }
+    jb.gpu_model = c.up(jobs->gpu_model, J);
+    jb.disk_request = c.up(jobs->disk_request, J);
+    jb.disk_type = c.up(jobs->disk_type, J);
+    if (jobs->attr_off) {
+      const int na = std::max(1, jobs->attr_off[J]);
+      jb.attr_off = c.up(jobs->attr_off, J + 1);
+      jb.attr_col = c.up(jobs->attr_col, na); jb.attr_val = c.up(jobs->attr_val, na);
+    }
+    jb.est_end_ms = c.up(jobs->est_end_ms, J);
+    jb.ckpt_location = c.up(jobs->ckpt_location, J); jb.reserved_host = c.up(jobs->reserved_host, J);
+    if (jobs->group_off && G) {
+      jb.group_off = c.up(jobs->group_off, J + 1);
+      jb.group_idx = c.up(jobs->group_idx, std::max<size_t>(1, n_memb));
+    }
+
+    mp->d_perm = c.up(perm.data(), O); of.perm = mp->d_perm;
+    mp->d_oc = c.up(offers->cpus, O); mp->d_om = c.up(offers->mem, O);
+    mp->d_orc = c.up(offers->run_cpus, O); mp->d_orm = c.up(offers->run_mem, O);
+    mp->d_vs = c.take<VmStatic>(O + 1); of.vs = mp->d_vs;
+    of.hostname_id = c.up(offers->hostname_id, O); of.run_count = c.up(offers->run_count, O);
+    mp->d_ports_total = nullptr;
+    if (offers->port_off) {
+      const int np = std::max(1, offers->port_off[O]);
+      of.port_off = c.up(offers->port_off, O + 1);
+      of.port_begin = c.up(offers->port_begin, np); of.port_end = c.up(offers->port_end, np);
+      mp->d_ports_total = c.take<int32_t>(O + 1); of.ports_total = mp->d_ports_total;
+    }
+    of.is_k8s = c.up(offers->is_k8s, O); of.reserved = c.up(offers->reserved, O);
+    of.location = c.up(offers->location, O);
+    if (offers->gpu_off) {
+      const int ng = std::max(1, offers->gpu_off[O]);
+      of.gpu_off = c.up(offers->gpu_off, O + 1);
+      of.gpu_model = c.up(offers->gpu_model, ng); of.gpu_count = c.up(offers->gpu_count, ng);
+    }
+    if (offers->disk_off) {
+      const int nd = std::max(1, offers->disk_off[O]);
+      of.disk_off = c.up(offers->disk_off, O + 1);
+      of.disk_type = c.up(offers->disk_type, nd); of.disk_space = c.up(offers->disk_space, nd);
+    }
+    of.max_tasks = c.up(offers->max_tasks, O); of.num_tasks = c.up(offers->num_tasks, O);
+    of.host_start = c.up(offers->host_start_time, O);
+    if (of.n_attr_cols > 0) of.attr = c.up(offers->attr, (size_t)of.n_attr_cols * O);
+    mp->d_vc = c.take<VmCons>(O + 1);
+    mp->d_attr_v = c.take<int32_t>((size_t)of.n_attr_cols * O + 1);
+    of.vc = mp->d_vc; of.attr_v = mp->d_attr_v;
+
+    if (G && jobs->group_off) {
+      gr.n_groups = G;
+      gr.kind = c.up(groups->kind, G);
+      gr.attr_col = c.up(groups->attr_col, G);
+      gr.minimum = c.up(groups->minimum, G);
+      gr.cot_off = c.up(groups->cot_off, G + 1);
+      const int nc = std::max(1, groups->cot_off[G]);
+      gr.cot_host = c.up(groups->cot_hostname_id, nc);
+      gr.cot_attr = c.up(groups->cot_attr_val, nc);
+      gr.gp_off = c.up(gp_off.data(), G + 1);
+      gr.gp_n = c.take<int32_t>(G + 1);
+      gr.gp_vm = c.take<int32_t>(n_memb + 1);
+    }
+    ca.q_count = c.up(users->quota_count, U); ca.q_cpus = c.up(users->quota_cpus, U);
+    ca.q_mem = c.up(users->quota_mem, U); ca.q_gpus = c.up(users->quota_gpus, U);
+    ca.u_count = c.up(users->usage_count, U); ca.u_cpus = c.up(users->usage_cpus, U);
+    ca.u_mem = c.up(users->usage_mem, U); ca.u_gpus = c.up(users->usage_gpus, U);
+    ca.tokens = c.up(users->tokens, U);
+
+    for (int b = 0; b < 2; b++) {
+      ma.dyn.d[b] = c.take<VmDyn>(O + 1);
+      ma.dyn.n[b] = c.take<VmCnt>(O + 1);
+    }
+    mp->d_pos = c.take<int32_t>(n_ranked + 1);
+    mp->d_tmp = c.take<int32_t>(n_ranked + 1);
+    mp->d_seg_s = c.take<int32_t>(U + 1);
+    mp->d_seg_e = c.take<int32_t>(U + 1);
+    mp->d_keep = c.take<uint8_t>(n_ranked + 1);
+    mp->d_placed = c.take<uint8_t>(J + 1);
+    mp->d_gf = c.take<GridFlag>(1);
+    mp->d_cons = c.take<int32_t>(NC + 1);
+    mp->d_kc = c.take<double>(NC + 1);
+    mp->d_km = c.take<double>(NC + 1);
+    mp->d_kflags = c.take<uint8_t>(NC + 1);
+    ma.rows = c.take<unsigned char>((size_t)2 * bmax * ROW_BYTES);
+    ma.sbits = c.take<unsigned>((size_t)2 * bmax * ((O + 31) / 32) + 4);
+    mp->d_kg = c.take<double>(NC + bmax + 1);
+    mp->d_kports = c.take<int32_t>(NC + bmax + 1);
+    ma.feas = c.take<int32_t>(2 * bmax + 16);
+    mp->d_smin_c = c.take<double>(NC + 1);
+    mp->d_smin_m = c.take<double>(NC + 1);
+    mp->d_smin_bc = c.take<double>(NC / 256 + 2);
+    mp->d_smin_bm = c.take<double>(NC / 256 + 2);
+    ma.rows_ready = c.take<unsigned>(max_blocks + 8);
+    ma.bk0 = c.take<int32_t>(max_blocks + 8);
+    ma.assign = c.take<int32_t>(NC + 1);
+    ma.ports_start = c.take<int32_t>(NC + 1);
+    ma.fail = c.take<uint8_t>(NC + 1);
+    mp->d_out_assign = c.take<int32_t>(NC + 1);
+    mp->d_out_ports = c.take<int32_t>((size_t)NC * std::max(max_ports, 1) + 1);
+    mp->d_used = c.take<int32_t>(O + 1);
+    mp->d_stats = c.take<unsigned long long>(32);
+    mp->d_counters = c.take<int32_t>(16);
+    mp->d_latest = c.take<int>((size_t)(MAX_SPEC_CTAS + 1) * (O + 1));
+    ma.glog = c.take<LogEnt>(LOGN);
+    ma.glogx = c.take<int4>(LOGN);
+    mp->d_gchain = c.take<unsigned long long>(4);
+    ma.lo_g = c.take<int32_t>(max_blocks + 8);
+    ma.gres = c.take<SpecOut>(GRING);
+    ma.gres_seq = c.take<unsigned>(GRING);
+  });
+  CK(pool, carved);
+  ca.n_ranked = n_ranked; ca.jb = jb; ca.n_users = U;
   ca.enforce_rate_limit = params->enforce_rate_limit;
   cook_pool_quota qoff{0, 0, 0, 0, 0};
   ca.pool_q = pool_quota ? *pool_quota : qoff;
   ca.num_considerable = NC;
-
-  MatchArgs& ma = mp->ma;
-  memset(&ma, 0, sizeof(ma));
-  for (int b = 0; b < 2; b++) {
-    ma.dyn.d[b] = ar.take<VmDyn>(O + 1);
-    ma.dyn.n[b] = ar.take<VmCnt>(O + 1);
-  }
-  mp->d_pos = ar.take<int32_t>(n_ranked + 1);
-  mp->d_tmp = ar.take<int32_t>(n_ranked + 1);
-  mp->d_seg_s = ar.take<int32_t>(U + 1);
-  mp->d_seg_e = ar.take<int32_t>(U + 1);
-  mp->d_keep = ar.take<uint8_t>(n_ranked + 1);
-  mp->d_placed = ar.take<uint8_t>(J + 1);
-  mp->d_gf = ar.take<GridFlag>(1);
-  mp->d_cons = ar.take<int32_t>(NC + 1);
-  mp->d_kc = ar.take<double>(NC + 1);
-  mp->d_km = ar.take<double>(NC + 1);
-  mp->d_kflags = ar.take<uint8_t>(NC + 1);
-  ma.rows = ar.take<unsigned char>((size_t)2 * bmax * ROW_BYTES);
-  ma.sbits = ar.take<unsigned>((size_t)2 * bmax * ((O + 31) / 32) + 4);
-  mp->d_kg = ar.take<double>(NC + bmax + 1);
-  mp->d_kports = ar.take<int32_t>(NC + bmax + 1);
   ma.kg = mp->d_kg; ma.kports = mp->d_kports;
-  ma.feas = ar.take<int32_t>(2 * bmax + 16);
-  mp->d_smin_c = ar.take<double>(NC + 1);
-  mp->d_smin_m = ar.take<double>(NC + 1);
-  mp->d_smin_bc = ar.take<double>(NC / 256 + 2);
-  mp->d_smin_bm = ar.take<double>(NC / 256 + 2);
   ma.smin_c = mp->d_smin_c; ma.smin_m = mp->d_smin_m;
-  ma.rows_ready = ar.take<unsigned>(max_blocks + 8);
-  ma.bk0 = ar.take<int32_t>(max_blocks + 8);
   mp->max_blocks = max_blocks;
-  ma.assign = ar.take<int32_t>(NC + 1);
-  ma.ports_start = ar.take<int32_t>(NC + 1);
-  ma.fail = ar.take<uint8_t>(NC + 1);
-  mp->d_out_assign = ar.take<int32_t>(NC + 1);
-  mp->d_out_ports = ar.take<int32_t>((size_t)NC * std::max(max_ports, 1) + 1);
-  mp->d_used = ar.take<int32_t>(O + 1);
-  mp->d_stats = ar.take<unsigned long long>(32);
-  mp->d_counters = ar.take<int32_t>(16);
-  mp->d_latest = ar.take<int>((size_t)(MAX_SPEC_CTAS + 1) * (O + 1));
-  ma.glog = ar.take<LogEnt>(LOGN);
-  ma.glogx = ar.take<int4>(LOGN);
-  mp->d_gchain = ar.take<unsigned long long>(4);
   ma.gchain = mp->d_gchain;
-  ma.lo_g = ar.take<int32_t>(max_blocks + 8);
   mp->lo_g_n = max_blocks + 8;
-  ma.gres = ar.take<SpecOut>(GRING);
-  ma.gres_seq = ar.take<unsigned>(GRING);
-  if (ar.failed) return set_err(pool, COOK_E_OOM, "cook_match: arena exhausted");
   ma.jb = jb; ma.of = of; ma.gr = gr;
   ma.cons = mp->d_cons; ma.kc = mp->d_kc; ma.km = mp->d_km; ma.kflags = mp->d_kflags;
   ma.B = B; ma.bmin = bmin; ma.bmax = bmax; ma.btarget = btarget;
@@ -2583,13 +2537,13 @@ static int32_t run_plan(cook_pool* pool, MatchPlan* mp, int32_t* out_considerabl
       launches++;
     }
   }
-  CK(pool, csort::sort_indices(mp->d_pos, mp->d_tmp, n_ranked, LessUserPos{ca.ranked, ca.jb.user}, st));
-  launches++;
-  for (long long w = csort::TILE; w < n_ranked; w <<= 1) launches++;
+  CK(pool, csort::sort_indices(mp->d_pos, mp->d_tmp, n_ranked, LessUserPos{ca.ranked, ca.jb.user}, st, &launches));
   seg_bounds_kernel<<<(n_ranked + TB - 1) / TB, TB, 0, st>>>(SortedKey{mp->d_pos, ca.ranked, ca.jb.user}, n_ranked,
                                                              mp->d_seg_s, mp->d_seg_e, nullptr);
+  launches++;
   CK(pool, cudaMemsetAsync(mp->d_gf, 0, sizeof(GridFlag), st));
   grid_check_kernel<<<(mp->J + TB - 1) / TB, TB, 0, st>>>(ca.jb.cpus, ca.jb.mem, ca.jb.gpus, mp->J, mp->d_gf);
+  launches++;
   cons_user_kernel<<<(U + 3) / 4, 128, 0, st>>>(ca, mp->d_pos, mp->d_seg_s, mp->d_seg_e, mp->d_keep, mp->d_gf);
   launches++;
   const ConsOut cons_out{mp->d_cons, mp->d_kc, mp->d_km, mp->d_kg, mp->d_kports, mp->d_kflags};
@@ -2597,14 +2551,15 @@ static int32_t run_plan(cook_pool* pool, MatchPlan* mp, int32_t* out_considerabl
     // global pool quota: an order-dependent f64 left fold over the survivors
     // (filter-sequential) => exact single-warp pass
     cons_queue_kernel<<<1, 32, 0, st>>>(ca, mp->d_keep, cons_out, mp->d_counters);
-    launches += 3;
+    launches++;
   } else {
-    compact(ConsSurvivors{ca, mp->d_keep, cons_out}, n_ranked, nullptr, mp->d_tmp, mp->d_counters, ca.num_considerable, st);
-    launches += 5;
+    compact(ConsSurvivors{ca, mp->d_keep, cons_out}, n_ranked, nullptr, mp->d_tmp, mp->d_counters, ca.num_considerable, st,
+            &launches);
   }
   CK(pool, cudaGetLastError());
   int32_t n_cons = 0;
-  CK(pool, cudaMemcpyAsync(&n_cons, mp->d_counters, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  int64_t d2h = 0;
+  CK(pool, download(&n_cons, mp->d_counters, 1, st, &d2h));
   CK(pool, cudaEventRecord(pool->ev[2], st));
   CK(pool, cudaStreamSynchronize(st));
 
@@ -2697,15 +2652,12 @@ static int32_t run_plan(cook_pool* pool, MatchPlan* mp, int32_t* out_considerabl
   }
   CK(pool, cudaEventRecord(pool->ev[3], st));
   if (n_cons > 0) {
-    CK(pool, cudaMemcpyAsync(out_considerable, mp->d_cons, sizeof(int32_t) * n_cons, cudaMemcpyDeviceToHost, st));
-    CK(pool, cudaMemcpyAsync(out_assign, mp->d_out_assign, sizeof(int32_t) * n_cons, cudaMemcpyDeviceToHost, st));
-    if (out_ports && max_ports > 0)
-      CK(pool, cudaMemcpyAsync(out_ports, mp->d_out_ports, sizeof(int32_t) * (size_t)n_cons * max_ports,
-                               cudaMemcpyDeviceToHost, st));
-    if (out_fail_reason)
-      CK(pool, cudaMemcpyAsync(out_fail_reason, ma.fail, n_cons, cudaMemcpyDeviceToHost, st));
-    CK(pool, cudaMemcpyAsync(hstats, mp->d_stats, sizeof(hstats), cudaMemcpyDeviceToHost, st));
-    CK(pool, cudaMemcpyAsync(&n_used, mp->d_counters + 1, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CK(pool, download(out_considerable, mp->d_cons, n_cons, st, &d2h));
+    CK(pool, download(out_assign, mp->d_out_assign, n_cons, st, &d2h));
+    if (out_ports && max_ports > 0) CK(pool, download(out_ports, mp->d_out_ports, (size_t)n_cons * max_ports, st, &d2h));
+    if (out_fail_reason) CK(pool, download(out_fail_reason, ma.fail, n_cons, st, &d2h));
+    CK(pool, download(hstats, mp->d_stats, 32, st, &d2h));
+    CK(pool, download(&n_used, mp->d_counters + 1, 1, st, &d2h));
   }
   CK(pool, cudaEventRecord(pool->ev[4], st));
   CK(pool, cudaStreamSynchronize(st));
@@ -2717,16 +2669,10 @@ static int32_t run_plan(cook_pool* pool, MatchPlan* mp, int32_t* out_considerabl
     for (int i = 0; i < 27; i++) fprintf(stderr, "[cook_prof] %-14s %llu\n", nm[i], hstats[i]);
   }
   mp->last_n_cons = n_cons;
-  {
-    cook_phase_stats& ps = pool->phase[COOK_PHASE_MATCH];
-    ps.ms_h2d = uploaded ? ev_ms(pool->ev[0], pool->ev[1]) : 0.0;
-    ps.ms_device = ev_ms(pool->ev[1], pool->ev[3]);
-    ps.ms_d2h = ev_ms(pool->ev[3], pool->ev[4]);
-    ps.h2d_bytes = uploaded ? mp->h2d_bytes : 0;
-    ps.d2h_bytes = (int64_t)n_cons * (8 + (out_fail_reason ? 1 : 0) + (out_ports ? 4 * (int64_t)max_ports : 0)) + 44;
-    ps.n_launches = launches;
-  }
+  record_phase(pool, COOK_PHASE_MATCH, uploaded ? pool->ev[0] : nullptr, pool->ev[1], pool->ev[3], pool->ev[4],
+               uploaded ? mp->h2d_bytes : 0, d2h, launches);
   if (out_stats) {
+    const cook_phase_stats& ps = pool->phase[COOK_PHASE_MATCH];
     out_stats->n_considerable = n_cons;
     out_stats->n_matched = (int)hstats[3];
     out_stats->head_matched = (n_cons > 0 && out_assign[0] >= 0) ? 1 : 0;
@@ -2735,15 +2681,14 @@ static int32_t run_plan(cook_pool* pool, MatchPlan* mp, int32_t* out_considerabl
     out_stats->n_fast = (int64_t)(hstats[0] + hstats[6]);
     out_stats->n_chunk_rescan = (int64_t)(hstats[1] + hstats[4]);
     out_stats->n_full_rescan = (int64_t)hstats[2];
-    out_stats->ms_h2d = uploaded ? ev_ms(pool->ev[0], pool->ev[1]) : 0.0;
+    out_stats->ms_h2d = ps.ms_h2d;
     out_stats->ms_considerable = ev_ms(pool->ev[1], pool->ev[2]);
     out_stats->ms_match = ev_ms(pool->ev[2], pool->ev[3]);
     out_stats->ms_match_kernel = ev_ms(pool->ev[5], pool->ev[6]);
-    out_stats->ms_d2h = ev_ms(pool->ev[3], pool->ev[4]);
-    out_stats->n_launches = launches;
-    out_stats->h2d_bytes = uploaded ? mp->h2d_bytes : 0;
-    out_stats->d2h_bytes = (int64_t)n_cons * (8 + (out_fail_reason ? 1 : 0) +
-                                               (out_ports ? 4 * (int64_t)max_ports : 0)) + 44;
+    out_stats->ms_d2h = ps.ms_d2h;
+    out_stats->n_launches = ps.n_launches;
+    out_stats->h2d_bytes = ps.h2d_bytes;
+    out_stats->d2h_bytes = ps.d2h_bytes;
   }
   return COOK_OK;
 }
@@ -2778,6 +2723,10 @@ extern "C" int32_t cook_match(cook_pool* pool, const int32_t* ranked_idx, int32_
     if (!offers->name_rank && O > 0) return set_err(pool, COOK_E_BADARG, "cook_match: offers.name_rank required");
     if (groups && !idx_in_range(groups->attr_col, groups->n_groups, -1, std::max(1, offers->n_attr_cols)))
       return set_err(pool, COOK_E_BADARG, "cook_match: groups.attr_col out of range");
+    const bool grouped = groups && groups->n_groups && jobs->group_off;
+    if ((jobs->novel_off || offers->reserved || grouped) && !offers->hostname_id)
+      return set_err(pool, COOK_E_BADARG, "cook_match: hostname_id column required by constraints");
+    if (grouped && (!groups->cot_off || !groups->kind)) return set_err(pool, COOK_E_BADARG, "cook_match: incomplete cook_groups");
   }
   CK(pool, cudaSetDevice(pool->device));
   if (!pool->match_plan) {
@@ -2854,16 +2803,11 @@ static int32_t exchange_run(cook_pool* const* pools, int32_t n_pools, void* comm
     if (world != 1) return set_err(pool, COOK_E_BADARG, "cook_exchange_usage: world > 1 needs a communicator");
   }
   CK(pool, cudaEventRecord(pool->ev[17], st));
-  CK(pool, cudaMemcpyAsync(out_all, d_all, sizeof(double) * (size_t)world * per_rank, cudaMemcpyDeviceToHost, st));
+  int64_t d2h = 0;
+  CK(pool, download(out_all, d_all, (size_t)world * per_rank, st, &d2h));
   CK(pool, cudaEventRecord(pool->ev[18], st));
   CK(pool, cudaStreamSynchronize(st));
-  cook_phase_stats& ps = pool->phase[COOK_PHASE_EXCHANGE];
-  ps.ms_h2d = 0.0;
-  ps.ms_device = ev_ms(pool->ev[16], pool->ev[17]);
-  ps.ms_d2h = ev_ms(pool->ev[17], pool->ev[18]);
-  ps.h2d_bytes = 0;
-  ps.d2h_bytes = (int64_t)sizeof(double) * world * (int64_t)per_rank;
-  ps.n_launches = launches;
+  record_phase(pool, COOK_PHASE_EXCHANGE, nullptr, pool->ev[16], pool->ev[17], pool->ev[18], 0, d2h, launches);
   return COOK_OK;
 }
 

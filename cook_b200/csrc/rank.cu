@@ -311,18 +311,6 @@ struct QueueSurvivors {
   __device__ void emit(int i, int slot) const { a.out_ranked[slot] = a.ti_at[i] - a.R; }
 };
 
-template <class T>
-cudaError_t upload2(Arena& ar, cudaStream_t st, const T* a, int na, const T* b, int nb, T** out) {
-  T* d = ar.take<T>((size_t)na + nb + 1);
-  if (!d) return cudaErrorMemoryAllocation;
-  *out = d;
-  cudaError_t e = cudaSuccess;
-  if (na) e = cudaMemcpyAsync(d, a, sizeof(T) * na, cudaMemcpyHostToDevice, st);
-  if (e != cudaSuccess) return e;
-  if (nb) e = cudaMemcpyAsync(d + na, b, sizeof(T) * nb, cudaMemcpyHostToDevice, st);
-  return e;
-}
-
 }  // namespace
 
 extern "C" int32_t cook_rank(cook_pool* pool, const cook_tasks_soa* running,
@@ -343,82 +331,63 @@ extern "C" int32_t cook_rank(cook_pool* pool, const cook_tasks_soa* running,
   if (N == 0) return COOK_OK;
   CK(pool, cudaSetDevice(pool->device));
   cudaStream_t st = pool->stream;
-  Arena& ar = pool->arena;
-  Sizer sz;
-  for (int k = 0; k < 2; k++) sz.add<int32_t>(N + 1);
-  for (int k = 0; k < 3; k++) sz.add<int64_t>(N + 1);
-  for (int k = 0; k < 3; k++) sz.add<double>(N + 1);
-  sz.add<int32_t>(U);
-  for (int k = 0; k < 7; k++) sz.add<double>(U);
-  for (int k = 0; k < 6; k++) sz.add<int32_t>(N + 1);  // idx,tmp,user_at,pos,out_order,out_ranked
-  sz.add<double>(N + 1);                                 // dru_at
-  for (int k = 0; k < 2; k++) sz.add<int32_t>(U);        // seg bounds
-  sz.add<double>(8);
-  sz.add<int32_t>(8);
-  sz.add<double>(N + 1);                                 // dru by task (output)
-  for (int k = 0; k < 3; k++) sz.add<double>(N + 1);     // queue-order requests
-  sz.add<int32_t>(N + 1); sz.add<uint8_t>(N + 1);        // queue-order task index, flags
-  sz.add<int32_t>(N / CP_BLOCK + 2); sz.add<GridFlag>(1);
-  for (int k = 0; k < 3; k++) sz.add<double>(N + 1);     // order-wide scans: tile-local sums
-  sz.add<double>(3 * (N / OS_TILE + 2)); sz.add<int32_t>(N + 1); sz.add<int32_t>(N / OS_TILE + 2);
-  CK(pool, ar.reserve(sz.off + 4096));
-  ar.reset();
-
-  CK(pool, cudaEventRecord(pool->ev[8], st));
   TaskCols t;
-  int32_t *d_user, *d_prio; int64_t *d_start, *d_tid, *d_jid; double *d_cpus, *d_mem, *d_gpus;
-  CK(pool, upload2(ar, st, running->user, R, pending->user, J, &d_user));
-  CK(pool, upload2(ar, st, running->priority, R, pending->priority, J, &d_prio));
-  CK(pool, upload2(ar, st, running->start_time, R, pending->start_time, J, &d_start));
-  CK(pool, upload2(ar, st, running->task_id, R, pending->task_id, J, &d_tid));
-  CK(pool, upload2(ar, st, running->job_id, R, pending->job_id, J, &d_jid));
-  CK(pool, upload2(ar, st, running->cpus, R, pending->cpus, J, &d_cpus));
-  CK(pool, upload2(ar, st, running->mem, R, pending->mem, J, &d_mem));
-  CK(pool, upload2(ar, st, running->gpus, R, pending->gpus, J, &d_gpus));
-  t = TaskCols{d_user, d_prio, d_start, d_tid, d_jid, d_cpus, d_mem, d_gpus};
-  int32_t* d_name_rank;
   UserCols uc;
-  double *dm, *dc, *dg, *qn, *qc, *qm, *qg;
-  CK(pool, upload(ar, st, users->name_rank, U, &d_name_rank));
-  CK(pool, upload(ar, st, users->div_mem, U, &dm));
-  CK(pool, upload(ar, st, users->div_cpus, U, &dc));
-  CK(pool, upload(ar, st, users->div_gpus, U, &dg));
-  CK(pool, upload(ar, st, users->quota_count, U, &qn));
-  CK(pool, upload(ar, st, users->quota_cpus, U, &qc));
-  CK(pool, upload(ar, st, users->quota_mem, U, &qm));
-  CK(pool, upload(ar, st, users->quota_gpus, U, &qg));
-  uc = UserCols{dm, dc, dg, qn, qc, qm, qg};
-
-  int32_t* d_idx = ar.take<int32_t>(N + 1);
-  int32_t* d_tmp = ar.take<int32_t>(N + 1);
-  int32_t* d_user_at = ar.take<int32_t>(N + 1);
-  int32_t* d_pos = ar.take<int32_t>(N + 1);
-  int32_t* d_out_order = ar.take<int32_t>(N + 1);
-  int32_t* d_out_ranked = ar.take<int32_t>(N + 1);
-  double* d_dru_at = ar.take<double>(N + 1);
-  int32_t* d_seg_start = ar.take<int32_t>(U);
-  int32_t* d_seg_end = ar.take<int32_t>(U);
-  double* d_pool_usage = ar.take<double>(8);
-  int32_t* d_counters = ar.take<int32_t>(8);  // [0]=n_kept [1]=n_out
-  double* d_dru_task = ar.take<double>(N + 1);
-  if (!d_dru_task) return set_err(pool, COOK_E_OOM, "cook_rank: arena exhausted");
-
-  GridFlag* d_gf = ar.take<GridFlag>(1);
+  const int32_t* d_name_rank;
+  int32_t *d_idx, *d_tmp, *d_user_at, *d_pos, *d_out_order, *d_out_ranked, *d_seg_start, *d_seg_end, *d_counters;
+  int32_t *d_os_pv, *d_os_bv;
+  double *d_dru_at, *d_pool_usage, *d_dru_task, *d_os_pm, *d_os_pc, *d_os_pg, *d_os_b;
+  GridFlag* d_gf;
+  QueueFilterArgs qa;
   const int os_nb = (N + OS_TILE - 1) / OS_TILE;
-  double* d_os_pm = ar.take<double>(N + 1); double* d_os_pc = ar.take<double>(N + 1); double* d_os_pg = ar.take<double>(N + 1);
-  double* d_os_b = ar.take<double>(3 * (os_nb + 1));
-  int32_t* d_os_pv = ar.take<int32_t>(N + 1); int32_t* d_os_bv = ar.take<int32_t>(os_nb + 1);
-  if (ar.failed) return set_err(pool, COOK_E_OOM, "cook_rank: arena exhausted");
+  int64_t h2d = 0, d2h = 0;
+  const cudaError_t carved = carve(pool->arena, st, pool->ev[8], &h2d, [&](Carve& c) {
+    t.user = c.cat(running->user, R, pending->user, J);
+    t.prio = c.cat(running->priority, R, pending->priority, J);
+    t.start = c.cat(running->start_time, R, pending->start_time, J);
+    t.tid = c.cat(running->task_id, R, pending->task_id, J);
+    t.jid = c.cat(running->job_id, R, pending->job_id, J);
+    t.cpus = c.cat(running->cpus, R, pending->cpus, J);
+    t.mem = c.cat(running->mem, R, pending->mem, J);
+    t.gpus = c.cat(running->gpus, R, pending->gpus, J);
+    d_name_rank = c.up(users->name_rank, U);
+    uc.div_mem = c.up(users->div_mem, U); uc.div_cpus = c.up(users->div_cpus, U); uc.div_gpus = c.up(users->div_gpus, U);
+    uc.q_count = c.up(users->quota_count, U); uc.q_cpus = c.up(users->quota_cpus, U);
+    uc.q_mem = c.up(users->quota_mem, U); uc.q_gpus = c.up(users->quota_gpus, U);
+    d_idx = c.take<int32_t>(N + 1);
+    d_tmp = c.take<int32_t>(N + 1);
+    d_user_at = c.take<int32_t>(N + 1);
+    d_pos = c.take<int32_t>(N + 1);
+    d_out_order = c.take<int32_t>(N + 1);
+    d_out_ranked = c.take<int32_t>(N + 1);
+    d_dru_at = c.take<double>(N + 1);
+    d_seg_start = c.take<int32_t>(U);
+    d_seg_end = c.take<int32_t>(U);
+    d_pool_usage = c.take<double>(8);
+    d_counters = c.take<int32_t>(8);  // [0]=n_kept [1]=n_out
+    d_dru_task = c.take<double>(N + 1);
+    d_gf = c.take<GridFlag>(1);
+    d_os_pm = c.take<double>(N + 1); d_os_pc = c.take<double>(N + 1); d_os_pg = c.take<double>(N + 1);
+    d_os_b = c.take<double>(3 * (os_nb + 1));
+    d_os_pv = c.take<int32_t>(N + 1); d_os_bv = c.take<int32_t>(os_nb + 1);
+    qa.ti_at = c.take<int32_t>(N + 1); qa.flag = c.take<uint8_t>(N + 1);
+    qa.xc = c.take<double>(N + 1); qa.xm = c.take<double>(N + 1); qa.xg = c.take<double>(N + 1);
+    qa.blk_cnt = c.take<int32_t>(N / CP_BLOCK + 2);
+  });
+  CK(pool, carved);
   CK(pool, cudaMemsetAsync(d_gf, 0, sizeof(GridFlag), st));
   CK(pool, cudaMemsetAsync(d_seg_start, 0, sizeof(int32_t) * U, st));
   CK(pool, cudaMemsetAsync(d_seg_end, 0, sizeof(int32_t) * U, st));
   CK(pool, cudaMemsetAsync(d_counters, 0, sizeof(int32_t) * 8, st));
 
   CK(pool, cudaEventRecord(pool->ev[9], st));
+  int nl = 0;
   const int TB = 256, nb = (N + TB - 1) / TB;
-  grid_check_kernel<<<nb, TB, 0, st>>>(d_cpus, d_mem, d_gpus, N, d_gf);
-  CK(pool, csort::sort_indices(d_idx, d_tmp, N, LessUserTask{d_user, d_prio, d_start, d_tid, d_jid, d_name_rank}, st));
-  seg_bounds_kernel<<<nb, TB, 0, st>>>(SortedKey{d_idx, nullptr, d_user}, N, d_seg_start, d_seg_end, d_user_at);
+  grid_check_kernel<<<nb, TB, 0, st>>>(t.cpus, t.mem, t.gpus, N, d_gf);
+  nl++;
+  CK(pool, csort::sort_indices(d_idx, d_tmp, N, LessUserTask{t.user, t.prio, t.start, t.tid, t.jid, d_name_rank}, st, &nl));
+  seg_bounds_kernel<<<nb, TB, 0, st>>>(SortedKey{d_idx, nullptr, t.user}, N, d_seg_start, d_seg_end, d_user_at);
+  nl++;
   {
     RankScan os;
     os.user_at = d_user_at; os.seg_start = d_seg_start; os.uc = uc;
@@ -426,41 +395,37 @@ extern "C" int32_t cook_rank(cook_pool* pool, const cook_tasks_soa* running,
     os.viol = OrderScan<int, 1>{{d_os_pv}, {d_os_bv}};
     os.n = N; os.dru_mode = pool->dru_mode; os.max_over_quota = params->max_over_quota_jobs;
     os.dru_at = d_dru_at; os.n_kept_total = d_counters;
-    order_scan(os.amt, LoadAmounts{d_idx, t}, N, d_gf, st);
-    order_scan(os.viol, os, N, d_gf, st);
+    order_scan(os.amt, LoadAmounts{d_idx, t}, N, d_gf, st, &nl);
+    order_scan(os.viol, os, N, d_gf, st, &nl);
     os_finish<<<(N + OS_TB - 1) / OS_TB, OS_TB, 0, st>>>(os, d_gf);
     int warps_per_block = 4;
     int blocks = (U + warps_per_block - 1) / warps_per_block;
     user_fold_kernel<<<blocks, warps_per_block * 32, 0, st>>>(
         d_idx, t, uc, d_seg_start, d_seg_end, U, pool->dru_mode, params->max_over_quota_jobs,
         d_dru_at, d_counters, d_gf, N);
+    nl += 2;
   }
   CK(pool, csort::sort_indices(d_pos, d_tmp, N,
-                               LessMerge{d_dru_at, d_user_at, d_seg_start, d_name_rank}, st));
-  QueueFilterArgs qa;
+                               LessMerge{d_dru_at, d_user_at, d_seg_start, d_name_rank}, st, &nl));
   qa.pos_sorted = d_pos; qa.idx = d_idx; qa.n_kept = d_counters; qa.R = R;
-  qa.cpus = d_cpus; qa.mem = d_mem; qa.gpus = d_gpus;
+  qa.cpus = t.cpus; qa.mem = t.mem; qa.gpus = t.gpus;
   qa.filter_offensive = params->filter_offensive;
   qa.off_mem = params->offensive_max_mem_mb; qa.off_cpus = params->offensive_max_cpus;
   qa.out_order = d_out_order; qa.out_ranked = d_out_ranked; qa.out_n = d_counters + 1;
-  qa.ti_at = ar.take<int32_t>(N + 1); qa.flag = ar.take<uint8_t>(N + 1);
-  qa.xc = ar.take<double>(N + 1); qa.xm = ar.take<double>(N + 1); qa.xg = ar.take<double>(N + 1);
   const int qnb = (N + QF_TB - 1) / QF_TB;
-  qa.blk_cnt = ar.take<int32_t>(N / CP_BLOCK + 2);
-  if (!qa.blk_cnt) return set_err(pool, COOK_E_OOM, "cook_rank: arena exhausted");
   qf_gather_kernel<<<qnb, QF_TB, 0, st>>>(qa);
-  int nl = 0;   // launches besides the 14 every call makes
+  nl++;
   if (pool_quota && pool_quota->enabled) {
-    nl += 2;
-    pool_usage_kernel<<<1, 32, 0, st>>>(d_cpus, d_mem, d_gpus, R, d_pool_usage, d_gf);
+    pool_usage_kernel<<<1, 32, 0, st>>>(t.cpus, t.mem, t.gpus, R, d_pool_usage, d_gf);
     qf_quota_kernel<<<1, QF_CH, 0, st>>>(qa, *pool_quota, d_pool_usage, d_gf);
+    nl += 2;
   }
   if (group_quota && group_usage && group_quota->enabled) {
     CK(pool, cudaMemcpyAsync(d_pool_usage + 4, group_usage, sizeof(double) * 4, cudaMemcpyHostToDevice, st));
-    nl++;
     qf_quota_kernel<<<1, QF_CH, 0, st>>>(qa, *group_quota, d_pool_usage + 4, d_gf);
+    nl++;
   }
-  compact(QueueSurvivors{qa}, N, qa.n_kept, qa.blk_cnt, qa.out_n, N, st);
+  compact(QueueSurvivors{qa}, N, qa.n_kept, qa.blk_cnt, qa.out_n, N, st, &nl);
   if (out_dru) {
     scatter_dru_kernel<<<nb, TB, 0, st>>>(d_idx, d_dru_at, N, d_dru_task);
     nl++;
@@ -468,30 +433,15 @@ extern "C" int32_t cook_rank(cook_pool* pool, const cook_tasks_soa* running,
   CK(pool, cudaGetLastError());
   CK(pool, cudaEventRecord(pool->ev[10], st));
   int32_t h_counters[2] = {0, 0};
-  CK(pool, cudaMemcpyAsync(h_counters, d_counters, sizeof(int32_t) * 2, cudaMemcpyDeviceToHost, st));
+  CK(pool, download(h_counters, d_counters, 2, st, &d2h));
   CK(pool, cudaStreamSynchronize(st));
   const int32_t n_kept = h_counters[0], n_out = h_counters[1];
-  if (n_out > 0)
-    CK(pool, cudaMemcpyAsync(out_ranked_idx, d_out_ranked, sizeof(int32_t) * n_out,
-                             cudaMemcpyDeviceToHost, st));
-  if (out_order && n_kept > 0)
-    CK(pool, cudaMemcpyAsync(out_order, d_out_order, sizeof(int32_t) * n_kept,
-                             cudaMemcpyDeviceToHost, st));
-  if (out_dru) CK(pool, cudaMemcpyAsync(out_dru, d_dru_task, sizeof(double) * N, cudaMemcpyDeviceToHost, st));
+  if (n_out > 0) CK(pool, download(out_ranked_idx, d_out_ranked, n_out, st, &d2h));
+  if (out_order && n_kept > 0) CK(pool, download(out_order, d_out_order, n_kept, st, &d2h));
+  if (out_dru) CK(pool, download(out_dru, d_dru_task, N, st, &d2h));
   CK(pool, cudaEventRecord(pool->ev[11], st));
   CK(pool, cudaStreamSynchronize(st));
-  {
-    cook_phase_stats& ps = pool->phase[COOK_PHASE_RANK];
-    ps.ms_h2d = ev_ms(pool->ev[8], pool->ev[9]);
-    ps.ms_device = ev_ms(pool->ev[9], pool->ev[10]);
-    ps.ms_d2h = ev_ms(pool->ev[10], pool->ev[11]);
-    ps.h2d_bytes = (int64_t)N * 56 + (int64_t)U * (4 + 7 * 8);   // task columns (56 B per task) + user tables
-    ps.d2h_bytes = (int64_t)n_out * 4 + (out_order ? (int64_t)n_kept * 4 : 0) + (out_dru ? (int64_t)N * 8 : 0) + 8;
-    for (long long w = csort::TILE; w < N; w <<= 1) nl += 2;   // the two sorts' merge passes
-    // grid check, 2 tile sorts, segment bounds, 2 order-wide scans (2 each), finish, per-user fold,
-    // gather, compaction (3)
-    ps.n_launches = nl + 14;
-  }
+  record_phase(pool, COOK_PHASE_RANK, pool->ev[8], pool->ev[9], pool->ev[10], pool->ev[11], h2d, d2h, nl);
   *out_n = n_out;
   if (out_order_n) *out_order_n = n_kept;
   return COOK_OK;

@@ -978,8 +978,6 @@ __global__ void __launch_bounds__(REB_TB) rebalance_kernel(RebArgs a) {
 
 }  // namespace
 
-#define RUP(dst, src, n) CK(pool, upload(ar, st, (src), (size_t)(n), &(dst)))
-
 static int32_t rebalance_run(cook_pool* pool, const cook_running_soa* running,
                              const cook_jobs_soa* pending, const int64_t* pending_job_id,
                              const int32_t* pending_priority, const cook_host_table* hosts,
@@ -1002,165 +1000,142 @@ static int32_t rebalance_run(cook_pool* pool, const cook_running_soa* running,
   if (!idx_in_range(running->host, R, 0, H)) return set_err(pool, COOK_E_BADARG, "cook_rebalance: running.host out of range");
   if (groups && pending->group_off && !idx_in_range(pending->group_idx, pending->group_off[P], 0, groups->n_groups))
     return set_err(pool, COOK_E_BADARG, "cook_rebalance: group index out of range");
+  const int G = groups ? groups->n_groups : 0;
+  if (G && pending->group_off && (!groups->cot_off || !groups->kind))
+    return set_err(pool, COOK_E_BADARG, "cook_rebalance: incomplete cook_groups");
+  const int CAP = R + MP + 1;
+  const int NF = tr ? tr->n_forced : 0;
+  int nfv = 0;   // forced victims
+  for (int q = 0; q < NF; q++) {
+    const cook_decision& f = tr->forced[q];
+    if (f.pending_idx < 0 || f.pending_idx >= P || f.host < 0 || f.host >= H || f.victim_count < 0 || f.victim_begin < 0)
+      return set_err(pool, COOK_E_BADARG, "cook_rebalance_trace: bad forced decision");
+    nfv = std::max(nfv, f.victim_begin + f.victim_count);
+  }
+  if (nfv > CAP + MP) return set_err(pool, COOK_E_BADARG, "cook_rebalance_trace: too many forced victims");
   CK(pool, cudaSetDevice(pool->device));
   cudaStream_t st = pool->stream;
-  Arena& ar = pool->arena;
-  const int CAP = R + MP + 1;
-  const int G = groups ? groups->n_groups : 0;
-  Sizer sz;
-  for (int k = 0; k < 6; k++) sz.add<int64_t>(CAP);  // generous: covers int32/int64/double columns
-  for (int k = 0; k < 10; k++) sz.add<double>(CAP);
-  for (int k = 0; k < 8; k++) sz.add<int32_t>(CAP);
-  sz.add<Refold>(2);
-  for (int k = 0; k < 12; k++) sz.add<double>(std::max(U, H) + 1);
-  for (int k = 0; k < 16; k++) sz.add<int32_t>(std::max(U, H) + 2);
-  size_t csr_h = (hosts->gpu_off ? hosts->gpu_off[H] : 0) + (hosts->disk_off ? hosts->disk_off[H] : 0);
-  sz.add<double>(csr_h + 64); sz.add<int32_t>(csr_h + 64);
-  sz.add<int32_t>((size_t)hosts->n_attr_cols * H + 1);
-  sz.add<int64_t>(H + 1);
-  for (int k = 0; k < 8; k++) sz.add<double>(P + 1);
-  for (int k = 0; k < 12; k++) sz.add<int32_t>(P + 2);
-  size_t csr_p = (pending->novel_off ? pending->novel_off[P] : 0) + 2 * (size_t)(pending->attr_off ? pending->attr_off[P] : 0) +
-                 (pending->group_off ? pending->group_off[P] : 0);
-  sz.add<int32_t>(csr_p + 64); sz.add<int64_t>(P + 1);
-  if (G) { sz.add<int32_t>(6 * (size_t)(G + 2)); sz.add<int32_t>(2 * (size_t)(groups->cot_off ? groups->cot_off[G] : 0) + 64); }
-  sz.add<HostBest>(H + 1); sz.add<cook_decision>(MP + 1); sz.add<int32_t>(CAP + MP);
-  sz.add<PendScalars>(P + 4); sz.add<int32_t>(64);
-  sz.add<int32_t>(CAP); sz.add<int32_t>(CAP + MP); sz.add<int32_t>(CAP + MP);   // second order buffer, preempted hosts (+ their hostname ids)
-  for (int k = 0; k < 2; k++) sz.add<int32_t>(U + 1);            // second segment buffers
-  sz.add<CtaBest>(4 * pool->sm_count + 8); sz.add<GridFlag>(1); sz.add<int32_t>(H + 1);
-  sz.add<TaskHot>(CAP); sz.add<int32_t>(CAP); sz.add<int32_t>(H + 1); sz.add<int32_t>(CAP); sz.add<WalkBar>(1);
-  sz.add<double>(CAP); sz.add<double>(CAP); sz.add<double>(CAP / OS_TILE + 2); sz.add<double>(CAP / OS_TILE + 2);
-  if (tr && tr->n_forced > 0) { sz.add<cook_decision>(tr->n_forced + 1); sz.add<int32_t>(CAP + MP); }
-  CK(pool, ar.reserve(sz.off + (1 << 16)));
-  ar.reset();
-
-  CK(pool, cudaEventRecord(pool->ev[12], st));
-  RTasks t;
-  t.user = ar.take<int32_t>(CAP); t.prio = ar.take<int32_t>(CAP); t.start = ar.take<int64_t>(CAP);
-  t.tid = ar.take<int64_t>(CAP); t.jid = ar.take<int64_t>(CAP); t.cpus = ar.take<double>(CAP);
-  t.mem = ar.take<double>(CAP); t.gpus = ar.take<double>(CAP); t.host = ar.take<int32_t>(CAP);
-  t.alive = ar.take<uint8_t>(CAP); t.dru = ar.take<double>(CAP); t.pos = ar.take<int32_t>(CAP);
-  t.cm = ar.take<double>(CAP); t.cc = ar.take<double>(CAP);
-  if (!t.cc) return set_err(pool, COOK_E_OOM, "cook_rebalance: arena exhausted");
   const cook_tasks_soa& rt = running->t;
-#define CPY(dst, src, T) if (R) CK(pool, cudaMemcpyAsync(dst, src, sizeof(T) * R, cudaMemcpyHostToDevice, st))
-  CPY(t.user, rt.user, int32_t); CPY(t.prio, rt.priority, int32_t); CPY(t.start, rt.start_time, int64_t);
-  CPY(t.tid, rt.task_id, int64_t); CPY(t.jid, rt.job_id, int64_t); CPY(t.cpus, rt.cpus, double);
-  CPY(t.mem, rt.mem, double); CPY(t.host, running->host, int32_t);
-  if (rt.gpus) { CPY(t.gpus, rt.gpus, double); } else CK(pool, cudaMemsetAsync(t.gpus, 0, sizeof(double) * CAP, st));
-#undef CPY
+  RTasks t;
+  HostCols hc;
+  PendCols pc;
+  GroupCols gc;
+  memset(&hc, 0, sizeof(hc));
+  memset(&pc, 0, sizeof(pc));
+  memset(&gc, 0, sizeof(gc));
+  hc.H = H;
+  hc.n_attr_cols = hosts->attr ? hosts->n_attr_cols : 0;
+  int32_t *d_urank, *d_ord, *d_ord2, *d_hord, *d_tmp, *d_us, *d_ue, *d_us2, *d_ue2, *d_hs, *d_he, *d_vict, *d_pre, *d_prehn;
+  int32_t *d_cnt, *d_fvict = nullptr, *d_syn, *d_hq, *d_synh, *d_synn;
+  double *d_divm, *d_divc, *d_qn, *d_qc, *d_qm, *d_qg, *d_pm, *d_pc, *d_btm, *d_btc;
+  uint8_t* d_has_task;
+  HostBest* d_best;
+  CtaBest* d_cta;
+  cook_decision *d_dec, *d_forced = nullptr;
+  PendScalars* d_ps;
+  Refold* d_rf;
+  GridFlag* d_gf;
+  TaskHot* d_hot;
+  WalkBar* d_bar;
+  int64_t h2d = 0, d2h = 0;
+  const cudaError_t carved = carve(pool->arena, st, pool->ev[12], &h2d, [&](Carve& c) {
+    t.user = c.part(rt.user, R, CAP); t.prio = c.part(rt.priority, R, CAP); t.start = c.part(rt.start_time, R, CAP);
+    t.tid = c.part(rt.task_id, R, CAP); t.jid = c.part(rt.job_id, R, CAP); t.cpus = c.part(rt.cpus, R, CAP);
+    t.mem = c.part(rt.mem, R, CAP); t.gpus = rt.gpus ? c.part(rt.gpus, R, CAP) : c.take<double>(CAP);
+    t.host = c.part(running->host, R, CAP);
+    t.alive = c.take<uint8_t>(CAP); t.dru = c.take<double>(CAP); t.pos = c.take<int32_t>(CAP);
+    t.cm = c.take<double>(CAP); t.cc = c.take<double>(CAP);
+
+    d_urank = c.up(users->name_rank, U); d_divm = c.up(users->div_mem, U); d_divc = c.up(users->div_cpus, U);
+    d_qn = c.up(users->quota_count, U); d_qc = c.up(users->quota_cpus, U); d_qm = c.up(users->quota_mem, U);
+    d_qg = c.up(users->quota_gpus, U);
+
+    hc.hostname_id = c.up(hosts->hostname_id, H); hc.name_rank = c.up(hosts->name_rank, H);
+    hc.has_spare = c.part(hosts->has_spare, H, H + 1, true); hc.spare_cpus = c.part(hosts->spare_cpus, H, H + 1, true);
+    hc.spare_mem = c.part(hosts->spare_mem, H, H + 1, true); hc.spare_gpus = c.part(hosts->spare_gpus, H, H + 1, true);
+    hc.is_k8s = c.up(hosts->is_k8s, H);
+    hc.location = c.up(hosts->location, H);
+    if (hosts->gpu_off) {
+      const int n = std::max(1, hosts->gpu_off[H]);
+      hc.gpu_off = c.up(hosts->gpu_off, H + 1); hc.gpu_model = c.up(hosts->gpu_model, n); hc.gpu_count = c.up(hosts->gpu_count, n);
+    }
+    if (hosts->disk_off) {
+      const int n = std::max(1, hosts->disk_off[H]);
+      hc.disk_off = c.up(hosts->disk_off, H + 1); hc.disk_type = c.up(hosts->disk_type, n); hc.disk_space = c.up(hosts->disk_space, n);
+    }
+    hc.host_start = c.up(hosts->host_start_time, H);
+    if (hc.n_attr_cols > 0) hc.attr = c.up(hosts->attr, (size_t)hc.n_attr_cols * H);
+
+    pc.user = c.up(pending->user, P); pc.prio = c.up(pending_priority, P);
+    pc.cpus = c.up(pending->cpus, P); pc.mem = c.up(pending->mem, P); pc.gpus = c.up(pending->gpus, P);
+    pc.jid = c.up(pending_job_id, P); pc.est_end_ms = c.up(pending->est_end_ms, P);
+    if (pending->novel_off) {
+      pc.novel_off = c.up(pending->novel_off, P + 1);
+      pc.novel_host = c.up(pending->novel_host, std::max(1, pending->novel_off[P]));
+    }
+    pc.gpu_model = c.up(pending->gpu_model, P); pc.disk_type = c.up(pending->disk_type, P);
+    pc.ckpt_location = c.up(pending->ckpt_location, P);
+    pc.disk_request = c.up(pending->disk_request, P);
+    if (pending->attr_off) {
+      const int n = std::max(1, pending->attr_off[P]);
+      pc.attr_off = c.up(pending->attr_off, P + 1); pc.attr_col = c.up(pending->attr_col, n); pc.attr_val = c.up(pending->attr_val, n);
+    }
+    if (G && pending->group_off) {
+      pc.group_off = c.up(pending->group_off, P + 1);
+      pc.group_idx = c.up(pending->group_idx, std::max(1, pending->group_off[P]));
+      gc.n = G;
+      gc.kind = c.up(groups->kind, G); gc.attr_col = c.up(groups->attr_col, G);
+      gc.minimum = c.up(groups->minimum, G); gc.cot_off = c.up(groups->cot_off, G + 1);
+      const int n = std::max(1, groups->cot_off[G]);
+      gc.cot_host = c.up(groups->cot_hostname_id, n); gc.cot_attr = c.up(groups->cot_attr_val, n);
+    }
+
+    d_ord = c.take<int32_t>(CAP); d_ord2 = c.take<int32_t>(CAP);
+    d_hord = c.take<int32_t>(CAP);
+    d_tmp = c.take<int32_t>(CAP);
+    d_us = c.take<int32_t>(U + 1); d_ue = c.take<int32_t>(U + 1);
+    d_us2 = c.take<int32_t>(U + 1); d_ue2 = c.take<int32_t>(U + 1);
+    d_hs = c.take<int32_t>(H + 1); d_he = c.take<int32_t>(H + 1);
+    d_has_task = c.take<uint8_t>(H + 1);
+    d_best = c.take<HostBest>(H + 1);
+    d_cta = c.take<CtaBest>(4 * pool->sm_count + 8);
+    d_dec = c.take<cook_decision>(MP + 1);
+    d_vict = c.take<int32_t>(CAP + MP);
+    d_pre = c.take<int32_t>(CAP + MP);
+    d_prehn = c.take<int32_t>(CAP + MP);
+    d_ps = c.take<PendScalars>(P + 4);
+    d_rf = c.take<Refold>(1);
+    d_cnt = c.take<int32_t>(64);  // [0] n_tasks [1] n_dec [2] n_vict [3] n_preempted [4] changed
+    if (NF > 0) {
+      d_forced = c.part(tr->forced, NF, NF + 1);
+      d_fvict = c.part(tr->forced_victims, nfv, CAP + MP);
+    }
+    d_gf = c.take<GridFlag>(1);
+    d_syn = c.take<int32_t>(H + 1);
+    d_hot = c.take<TaskHot>(CAP);
+    d_hq = c.take<int32_t>(CAP);
+    d_synh = c.take<int32_t>(H + 1);
+    d_synn = c.take<int32_t>(CAP);
+    d_bar = c.take<WalkBar>(1);
+    d_pm = c.take<double>(CAP); d_pc = c.take<double>(CAP);
+    d_btm = c.take<double>(CAP / OS_TILE + 2); d_btc = c.take<double>(CAP / OS_TILE + 2);
+  });
+  CK(pool, carved);
+  if (!rt.gpus) CK(pool, cudaMemsetAsync(t.gpus, 0, sizeof(double) * CAP, st));
   CK(pool, cudaMemsetAsync(t.alive, 0, CAP, st));
   if (R) CK(pool, cudaMemsetAsync(t.alive, 1, R, st));
   CK(pool, cudaMemsetAsync(t.dru, 0, sizeof(double) * CAP, st));
-
-  int32_t* d_urank; double *d_divm, *d_divc, *d_qn, *d_qc, *d_qm, *d_qg;
-  RUP(d_urank, users->name_rank, U); RUP(d_divm, users->div_mem, U); RUP(d_divc, users->div_cpus, U);
-  RUP(d_qn, users->quota_count, U); RUP(d_qc, users->quota_cpus, U); RUP(d_qm, users->quota_mem, U);
-  RUP(d_qg, users->quota_gpus, U);
-
-  HostCols hc;
-  memset(&hc, 0, sizeof(hc));
-  hc.H = H;
-  { int32_t* p; RUP(p, hosts->hostname_id, H); hc.hostname_id = p; RUP(p, hosts->name_rank, H); hc.name_rank = p; }
-  hc.has_spare = ar.take<uint8_t>(H + 1); hc.spare_cpus = ar.take<double>(H + 1);
-  hc.spare_mem = ar.take<double>(H + 1); hc.spare_gpus = ar.take<double>(H + 1);
-  CK(pool, cudaMemsetAsync(hc.has_spare, 0, H + 1, st));
-  CK(pool, cudaMemsetAsync(hc.spare_cpus, 0, sizeof(double) * (H + 1), st));
-  CK(pool, cudaMemsetAsync(hc.spare_mem, 0, sizeof(double) * (H + 1), st));
-  CK(pool, cudaMemsetAsync(hc.spare_gpus, 0, sizeof(double) * (H + 1), st));
-  if (hosts->has_spare) CK(pool, cudaMemcpyAsync(hc.has_spare, hosts->has_spare, H, cudaMemcpyHostToDevice, st));
-  if (hosts->spare_cpus) CK(pool, cudaMemcpyAsync(hc.spare_cpus, hosts->spare_cpus, sizeof(double) * H, cudaMemcpyHostToDevice, st));
-  if (hosts->spare_mem) CK(pool, cudaMemcpyAsync(hc.spare_mem, hosts->spare_mem, sizeof(double) * H, cudaMemcpyHostToDevice, st));
-  if (hosts->spare_gpus) CK(pool, cudaMemcpyAsync(hc.spare_gpus, hosts->spare_gpus, sizeof(double) * H, cudaMemcpyHostToDevice, st));
-  { uint8_t* p; RUP(p, hosts->is_k8s, H); hc.is_k8s = p; }
-  { int32_t* p; RUP(p, hosts->location, H); hc.location = p; }
-  if (hosts->gpu_off) { int32_t* p; RUP(p, hosts->gpu_off, H + 1); hc.gpu_off = p;
-    int n = std::max(1, hosts->gpu_off[H]); RUP(p, hosts->gpu_model, n); hc.gpu_model = p;
-    double* q; RUP(q, hosts->gpu_count, n); hc.gpu_count = q; }
-  if (hosts->disk_off) { int32_t* p; RUP(p, hosts->disk_off, H + 1); hc.disk_off = p;
-    int n = std::max(1, hosts->disk_off[H]); RUP(p, hosts->disk_type, n); hc.disk_type = p;
-    double* q; RUP(q, hosts->disk_space, n); hc.disk_space = q; }
-  { int64_t* p; RUP(p, hosts->host_start_time, H); hc.host_start = p; }
-  hc.n_attr_cols = hosts->attr ? hosts->n_attr_cols : 0;
-  if (hc.n_attr_cols > 0) { int32_t* p; RUP(p, hosts->attr, (size_t)hc.n_attr_cols * H); hc.attr = p; }
-
-  PendCols pc;
-  memset(&pc, 0, sizeof(pc));
-  { int32_t* p; RUP(p, pending->user, P); pc.user = p; RUP(p, pending_priority, P); pc.prio = p; }
-  { double* p; RUP(p, pending->cpus, P); pc.cpus = p; RUP(p, pending->mem, P); pc.mem = p; RUP(p, pending->gpus, P); pc.gpus = p; }
-  { int64_t* p; RUP(p, pending_job_id, P); pc.jid = p; RUP(p, pending->est_end_ms, P); pc.est_end_ms = p; }
-  if (pending->novel_off) { int32_t* p; RUP(p, pending->novel_off, P + 1); pc.novel_off = p;
-    RUP(p, pending->novel_host, std::max(1, pending->novel_off[P])); pc.novel_host = p; }
-  { int32_t* p; RUP(p, pending->gpu_model, P); pc.gpu_model = p; RUP(p, pending->disk_type, P); pc.disk_type = p;
-    RUP(p, pending->ckpt_location, P); pc.ckpt_location = p; }
-  { double* p; RUP(p, pending->disk_request, P); pc.disk_request = p; }
-  if (pending->attr_off) { int32_t* p; RUP(p, pending->attr_off, P + 1); pc.attr_off = p;
-    int n = std::max(1, pending->attr_off[P]); RUP(p, pending->attr_col, n); pc.attr_col = p;
-    RUP(p, pending->attr_val, n); pc.attr_val = p; }
-  GroupCols gc;
-  memset(&gc, 0, sizeof(gc));
-  if (G && pending->group_off) {
-    int32_t* p; RUP(p, pending->group_off, P + 1); pc.group_off = p;
-    RUP(p, pending->group_idx, std::max(1, pending->group_off[P])); pc.group_idx = p;
-    gc.n = G;
-    RUP(p, groups->kind, G); gc.kind = p; RUP(p, groups->attr_col, G); gc.attr_col = p;
-    RUP(p, groups->minimum, G); gc.minimum = p; RUP(p, groups->cot_off, G + 1); gc.cot_off = p;
-    int n = std::max(1, groups->cot_off ? groups->cot_off[G] : 0);
-    RUP(p, groups->cot_hostname_id, n); gc.cot_host = p; RUP(p, groups->cot_attr_val, n); gc.cot_attr = p;
-    if (!gc.cot_off || !gc.kind) return set_err(pool, COOK_E_BADARG, "cook_rebalance: incomplete cook_groups");
-  }
-
-  int32_t* d_ord = ar.take<int32_t>(CAP); int32_t* d_ord2 = ar.take<int32_t>(CAP);
-  int32_t* d_hord = ar.take<int32_t>(CAP);
-  int32_t* d_tmp = ar.take<int32_t>(CAP);
-  int32_t* d_us = ar.take<int32_t>(U + 1); int32_t* d_ue = ar.take<int32_t>(U + 1);
-  int32_t* d_us2 = ar.take<int32_t>(U + 1); int32_t* d_ue2 = ar.take<int32_t>(U + 1);
-  int32_t* d_hs = ar.take<int32_t>(H + 1); int32_t* d_he = ar.take<int32_t>(H + 1);
-  uint8_t* d_has_task = ar.take<uint8_t>(H + 1);
-  HostBest* d_best = ar.take<HostBest>(H + 1);
-  CtaBest* d_cta = ar.take<CtaBest>(4 * pool->sm_count + 8);
-  cook_decision* d_dec = ar.take<cook_decision>(MP + 1);
-  int32_t* d_vict = ar.take<int32_t>(CAP + MP);
-  int32_t* d_pre = ar.take<int32_t>(CAP + MP);
-  int32_t* d_prehn = ar.take<int32_t>(CAP + MP);
-  PendScalars* d_ps = ar.take<PendScalars>(P + 4);
-  Refold* d_rf = ar.take<Refold>(1);
-  int32_t* d_cnt = ar.take<int32_t>(64);  // [0] n_tasks [1] n_dec [2] n_vict [3] n_preempted [4] changed
-  cook_decision* d_forced = nullptr;
-  int32_t* d_fvict = nullptr;
-  const int NF = tr ? tr->n_forced : 0;
-  if (NF > 0) {
-    int nfv = 0;
-    for (int q = 0; q < NF; q++) {
-      const cook_decision& f = tr->forced[q];
-      if (f.pending_idx < 0 || f.pending_idx >= P || f.host < 0 || f.host >= H || f.victim_count < 0 || f.victim_begin < 0)
-        return set_err(pool, COOK_E_BADARG, "cook_rebalance_trace: bad forced decision");
-      nfv = std::max(nfv, f.victim_begin + f.victim_count);
-    }
-    if (nfv > CAP + MP) return set_err(pool, COOK_E_BADARG, "cook_rebalance_trace: too many forced victims");
-    d_forced = ar.take<cook_decision>(NF + 1);
-    d_fvict = ar.take<int32_t>(CAP + MP);
-    if (d_forced) CK(pool, cudaMemcpyAsync(d_forced, tr->forced, sizeof(cook_decision) * NF, cudaMemcpyHostToDevice, st));
-    if (d_fvict && nfv > 0) CK(pool, cudaMemcpyAsync(d_fvict, tr->forced_victims, sizeof(int32_t) * nfv, cudaMemcpyHostToDevice, st));
-  }
-  if (ar.failed) return set_err(pool, COOK_E_OOM, "cook_rebalance: arena exhausted");
-  GridFlag* d_gf = ar.take<GridFlag>(1);
-  int32_t* d_syn = ar.take<int32_t>(H + 1);
-  TaskHot* d_hot = ar.take<TaskHot>(CAP);
-  int32_t* d_hq = ar.take<int32_t>(CAP);
-  int32_t* d_synh = ar.take<int32_t>(H + 1);
-  int32_t* d_synn = ar.take<int32_t>(CAP);
-  WalkBar* d_bar = ar.take<WalkBar>(1);
-  double* d_pm = ar.take<double>(CAP); double* d_pc = ar.take<double>(CAP);
-  double* d_btm = ar.take<double>(CAP / OS_TILE + 2); double* d_btc = ar.take<double>(CAP / OS_TILE + 2);
-  if (ar.failed) return set_err(pool, COOK_E_OOM, "cook_rebalance: arena exhausted");
   CK(pool, cudaMemsetAsync(d_gf, 0, sizeof(GridFlag), st));
   CK(pool, cudaMemsetAsync(d_syn, 0, sizeof(int32_t) * (H + 1), st));
   CK(pool, cudaMemsetAsync(d_synh, 0xff, sizeof(int32_t) * (H + 1), st));
   CK(pool, cudaMemsetAsync(d_bar, 0, sizeof(WalkBar), st));
-  if (R > 0) grid_check_kernel<<<(R + 255) / 256, 256, 0, st>>>(t.cpus, t.mem, t.gpus, R, d_gf);
+  int launches = 0;
+  if (R > 0) {
+    grid_check_kernel<<<(R + 255) / 256, 256, 0, st>>>(t.cpus, t.mem, t.gpus, R, d_gf);
+    launches++;
+  }
   grid_check_kernel<<<(P + 255) / 256, 256, 0, st>>>(pc.cpus, pc.mem, pc.gpus, P, d_gf);
+  launches++;
   int32_t h_cnt[16] = {R, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
   CK(pool, cudaMemcpyAsync(d_cnt, h_cnt, sizeof(h_cnt), cudaMemcpyHostToDevice, st));
   CK(pool, cudaMemsetAsync(d_ps, 0xff, sizeof(PendScalars) * (P + 4), st));   // below_quota -1, dru NaN: not reached
@@ -1175,23 +1150,23 @@ static int32_t rebalance_run(cook_pool* pool, const cook_running_soa* running,
   CK(pool, cudaMemsetAsync(d_hs, 0, sizeof(int32_t) * (H + 1), st));
   CK(pool, cudaMemsetAsync(d_he, 0, sizeof(int32_t) * (H + 1), st));
   CK(pool, cudaMemsetAsync(d_has_task, 0, H + 1, st));
-  int launches = 0;
   if (R > 0) {
-    CK(pool, csort::sort_indices(d_ord, d_tmp, R, LessUserTask{t.user, t.prio, t.start, t.tid, t.jid, d_urank}, st));
+    CK(pool, csort::sort_indices(d_ord, d_tmp, R, LessUserTask{t.user, t.prio, t.start, t.tid, t.jid, d_urank}, st, &launches));
     seg_bounds_kernel<<<(R + TB - 1) / TB, TB, 0, st>>>(SortedKey{d_ord, nullptr, t.user}, R, d_us, d_ue, nullptr);
+    launches++;
     {
       const OrderScan<double, 2> os{{d_pm, d_pc}, {d_btm, d_btc}};
-      order_scan(os, LoadAlive{d_ord, t}, R, d_gf, st);
+      order_scan(os, LoadAlive{d_ord, t}, R, d_gf, st, &launches);
       order_dru_finish<<<(R + TB - 1) / TB, TB, 0, st>>>(d_ord, t, R, d_gf, os, d_us, d_divm, d_divc);
-      launches += 3;
+      launches++;
     }
     user_dru_kernel<<<(U + 3) / 4, 128, 0, st>>>(d_ord, t, d_divm, d_divc, d_us, d_ue, U, d_gf, R);
-    CK(pool, csort::sort_indices(d_hord, d_tmp, R, LessHost{t}, st));
+    launches++;
+    CK(pool, csort::sort_indices(d_hord, d_tmp, R, LessHost{t}, st, &launches));
     seg_bounds_kernel<<<(R + TB - 1) / TB, TB, 0, st>>>(SortedKey{d_hord, nullptr, t.host}, R, d_hs, d_he, nullptr);
     host_has_task_kernel<<<(R + TB - 1) / TB, TB, 0, st>>>(t, R, d_has_task);
     hot_build_kernel<<<(R + TB - 1) / TB, TB, 0, st>>>(d_hord, t, d_urank, R, d_hot, d_hq);
-    launches += 7;
-    for (long long w = csort::TILE; w < R; w <<= 1) launches += 2;
+    launches += 3;
   }
   // ---- the walk over the pending jobs: one cooperative launch, no host round trip inside
   RebArgs ra;
@@ -1220,7 +1195,7 @@ static int32_t rebalance_run(cook_pool* pool, const cook_running_soa* running,
     launches++;
   }
   CK(pool, cudaEventRecord(pool->ev[14], st));
-  CK(pool, cudaMemcpyAsync(h_cnt, d_cnt, sizeof(int32_t) * 5, cudaMemcpyDeviceToHost, st));
+  CK(pool, download(h_cnt, d_cnt, 5, st, &d2h));
   CK(pool, cudaStreamSynchronize(st));
   if (getenv("COOK_PROF")) {
     int32_t hp[10];
@@ -1233,26 +1208,25 @@ static int32_t rebalance_run(cook_pool* pool, const cook_running_soa* running,
   }
   const int n_dec = h_cnt[1], n_tasks = h_cnt[0];
   if (n_dec > 0) {
-    CK(pool, cudaMemcpyAsync(out_decisions, d_dec, sizeof(cook_decision) * n_dec, cudaMemcpyDeviceToHost, st));
-    if (h_cnt[2] > 0)
-      CK(pool, cudaMemcpyAsync(out_victims, d_vict, sizeof(int32_t) * h_cnt[2], cudaMemcpyDeviceToHost, st));
+    CK(pool, download(out_decisions, d_dec, n_dec, st, &d2h));
+    if (h_cnt[2] > 0) CK(pool, download(out_victims, d_vict, h_cnt[2], st, &d2h));
   }
   if (tr) {   // the state the reference's own tests read (K18 pending dru, K21 next-state, job-below-quota)
     std::vector<PendScalars> hps(P);
     std::vector<double> hdru(n_tasks);
     std::vector<uint8_t> halive(n_tasks);
     std::vector<int32_t> hpos(n_tasks), huser(n_tasks);
-    CK(pool, cudaMemcpyAsync(hps.data(), d_ps, sizeof(PendScalars) * P, cudaMemcpyDeviceToHost, st));
+    CK(pool, download(hps.data(), d_ps, P, st, &d2h));
     if (n_tasks > 0) {
-      CK(pool, cudaMemcpyAsync(hdru.data(), t.dru, sizeof(double) * n_tasks, cudaMemcpyDeviceToHost, st));
-      CK(pool, cudaMemcpyAsync(halive.data(), t.alive, n_tasks, cudaMemcpyDeviceToHost, st));
-      CK(pool, cudaMemcpyAsync(hpos.data(), t.pos, sizeof(int32_t) * n_tasks, cudaMemcpyDeviceToHost, st));
-      CK(pool, cudaMemcpyAsync(huser.data(), t.user, sizeof(int32_t) * n_tasks, cudaMemcpyDeviceToHost, st));
+      CK(pool, download(hdru.data(), t.dru, n_tasks, st, &d2h));
+      CK(pool, download(halive.data(), t.alive, n_tasks, st, &d2h));
+      CK(pool, download(hpos.data(), t.pos, n_tasks, st, &d2h));
+      CK(pool, download(huser.data(), t.user, n_tasks, st, &d2h));
     }
-    if (tr->has_spare) CK(pool, cudaMemcpyAsync(tr->has_spare, hc.has_spare, H, cudaMemcpyDeviceToHost, st));
-    if (tr->spare_mem) CK(pool, cudaMemcpyAsync(tr->spare_mem, hc.spare_mem, sizeof(double) * H, cudaMemcpyDeviceToHost, st));
-    if (tr->spare_cpus) CK(pool, cudaMemcpyAsync(tr->spare_cpus, hc.spare_cpus, sizeof(double) * H, cudaMemcpyDeviceToHost, st));
-    if (tr->spare_gpus) CK(pool, cudaMemcpyAsync(tr->spare_gpus, hc.spare_gpus, sizeof(double) * H, cudaMemcpyDeviceToHost, st));
+    if (tr->has_spare) CK(pool, download(tr->has_spare, hc.has_spare, H, st, &d2h));
+    if (tr->spare_mem) CK(pool, download(tr->spare_mem, hc.spare_mem, H, st, &d2h));
+    if (tr->spare_cpus) CK(pool, download(tr->spare_cpus, hc.spare_cpus, H, st, &d2h));
+    if (tr->spare_gpus) CK(pool, download(tr->spare_gpus, hc.spare_gpus, H, st, &d2h));
     CK(pool, cudaStreamSynchronize(st));
     for (int p = 0; p < P; p++) {
       if (hps[p].below_quota < 0) continue;   // the walk did not reach this job
@@ -1276,15 +1250,7 @@ static int32_t rebalance_run(cook_pool* pool, const cook_running_soa* running,
   }
   CK(pool, cudaEventRecord(pool->ev[15], st));
   CK(pool, cudaStreamSynchronize(st));
-  {
-    cook_phase_stats& ps = pool->phase[COOK_PHASE_REBALANCE];
-    ps.ms_h2d = ev_ms(pool->ev[12], pool->ev[13]);
-    ps.ms_device = ev_ms(pool->ev[13], pool->ev[14]);
-    ps.ms_d2h = ev_ms(pool->ev[14], pool->ev[15]);
-    ps.h2d_bytes = (int64_t)R * 60 + (int64_t)P * 48 + (int64_t)H * 48 + (int64_t)U * 60;
-    ps.d2h_bytes = (int64_t)n_dec * (int64_t)sizeof(cook_decision) + (int64_t)h_cnt[2] * 4 + 20;
-    ps.n_launches = launches;
-  }
+  record_phase(pool, COOK_PHASE_REBALANCE, pool->ev[12], pool->ev[13], pool->ev[14], pool->ev[15], h2d, d2h, launches);
   *out_n = n_dec;
   return COOK_OK;
 }

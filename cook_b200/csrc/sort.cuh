@@ -90,18 +90,20 @@ __global__ void merge_pass_kernel(const int32_t* __restrict__ src, int32_t* __re
   }
 }
 
-// Sorts the indices 0..n-1 into idx[0..n); tmp must hold n int32.
+// Sorts the indices 0..n-1 into idx[0..n); tmp must hold n int32.  Adds its kernel launches to *launches.
 template <class Less>
-inline cudaError_t sort_indices(int32_t* idx, int32_t* tmp, int n, Less less, cudaStream_t st) {
+inline cudaError_t sort_indices(int32_t* idx, int32_t* tmp, int n, Less less, cudaStream_t st, int* launches) {
   if (n <= 0) return cudaSuccess;
   int tiles = (n + TILE - 1) / TILE;
   tile_sort_kernel<Less><<<tiles, TILE_THREADS, 0, st>>>(idx, n, less);
+  ++*launches;
   int32_t* src = idx;
   int32_t* dst = tmp;
   for (long long width = TILE; width < n; width <<= 1) {
     long long threads = ((long long)n + ITEMS - 1) / ITEMS;
     int blocks = (int)((threads + 255) / 256);
     merge_pass_kernel<Less><<<blocks, 256, 0, st>>>(src, dst, n, (int)width, less);
+    ++*launches;
     int32_t* t = src; src = dst; dst = t;
   }
   if (src != idx)
