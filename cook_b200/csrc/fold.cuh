@@ -3,7 +3,8 @@
 // Every running sum is the reference's left fold (common.cuh, "Exact-grid fast path"): a parallel
 // scan when grid_exact says every partial sum is exact, else the lane-serial chain below, which keeps
 // the association.  Around them: segment bounds of a sorted order, the order-wide tile scan that
-// replaces per-segment folds on the grid, and stable stream compaction.
+// replaces per-segment folds on the grid, and stable stream compaction.  Beside the per-user task order
+// (LessUserTask): the order of dru/sorted-merge over those lists (LessMerge).
 #pragma once
 #include "common.cuh"
 
@@ -138,6 +139,65 @@ struct LessUserTask {
     return a < b;
   }
 };
+
+// Global emission order of dru/sorted-merge (dru.clj:82-104).  X, Y are
+// positions in the user-sorted array.  The merge emits, at every step, the head
+// with the smallest (dru, -arrival, name) where arrival = step at which the
+// user's previous task was emitted (0 for a user's first task): the popped
+// user's remainder is consed to the FRONT before a STABLE re-sort (:93-94).
+// Hence for equal dru:  X before Y  <=>  prev(X) was emitted AFTER prev(Y),
+// which recurses on the previous tasks with the roles swapped.
+// That rule holds only for two tasks that are heads at the same time.  A user's
+// run of equal consecutive scores (GPU mode: every task with gpus = 0; a user
+// with a zero share: +inf on every task) is emitted contiguously: once its first
+// task is popped, the user's next head has the newest arrival and the smallest
+// score present.  So between users, a task stands for the first task of its run,
+// and two run starts of equal score are heads together.
+struct LessMerge {
+  const double* dru;   // by sorted position; NaN = cut by limit-over-quota
+  const int64_t* tie;  // by kept sorted position: merge_tie_word, all a tie needs in one load
+  __device__ bool operator()(int32_t x, int32_t y) const {
+    double dx = dru[x], dy = dru[y];
+    bool kx = dx == dx, ky = dy == dy;
+    if (kx != ky) return kx;  // truncated tasks sort last
+    if (!kx) return x < y;
+    while (true) {
+      if (dx != dy) return dx < dy;
+      const int64_t tx = tie[x], ty = tie[y];
+      if ((tx >> 32) == (ty >> 32)) return x < y;  // same user: queue order
+      const int32_t rx = (int32_t)(uint32_t)tx, ry = (int32_t)(uint32_t)ty;
+      if (rx < 0 && ry < 0) return rx > ry;  // both runs start their lists: name order
+      if (rx < 0) return false;  // X has arrival 0 => Y first
+      if (ry < 0) return true;
+      // before(X,Y) = before(prev(Y), prev(X)) of the run starts: swap roles and step back
+      x = ry - 1; y = rx - 1;
+      dx = dru[x]; dy = dru[y];
+    }
+  }
+};
+
+// LessMerge::tie of kept position p (score d) of user u, whose list starts at s: the user in the high 32
+// bits; in the low 32 bits the first position of p's run of equal scores, or -1 - (the user's name rank)
+// when that run starts the list (arrival 0).  score(m) is the score of position m of the same list.  A
+// user's kept scores never decrease (non-negative left-fold sums over a positive divisor, maxed), so the
+// run start is the first position of [s, p] with score d: usually p itself, else a binary search.  Written
+// where the scores are made (rank.cu: os_finish / user_fold), so it costs no launch of its own.
+template <class Score>
+__device__ __forceinline__ int64_t merge_tie_word(int p, int s, int u, int32_t name_rank_u, double d,
+                                                  const Score& score) {
+  int lo = p;
+  if (p > s && score(p - 1) == d) {
+    lo = s;
+    int hi = p - 1;
+    while (lo < hi) {
+      const int m = (lo + hi) >> 1;
+      if (score(m) < d) lo = m + 1;
+      else hi = m;
+    }
+  }
+  const int32_t code = lo > s ? lo : -1 - name_rank_u;
+  return (int64_t)((uint64_t)(uint32_t)u << 32 | (uint32_t)code);
+}
 
 // key_at (may be null): the segment of every position
 __global__ void seg_bounds_kernel(SortedKey key, int n, int32_t* seg_start, int32_t* seg_end, int32_t* key_at) {

@@ -12,7 +12,8 @@
 //   K3 warp-per-user fold           -> cumulative usage in the reference's
 //      left-fold order (lane-serial shuffle chain keeps f64 association),
 //      over-quota truncation, DRU = max(mem/div, cpus/div) (IEEE div.rn.f64)
-//   K4 comparator sort of positions by (dru, k-way-merge tie rule)
+//   K4 comparator sort of positions by (dru, k-way-merge tie rule); K3 wrote
+//      each kept task's run of equal scores for it (merge_tie_word)
 //   K5 single-warp queue filter     -> pending only, pool quota, group quota,
 //      offensive filter, stable compaction.
 #include "fold.cuh"
@@ -31,39 +32,6 @@ struct TaskCols {
   const double* gpus;
 };
 
-// Global emission order of dru/sorted-merge (dru.clj:82-104).  X, Y are
-// positions in the user-sorted array.  The merge emits, at every step, the head
-// with the smallest (dru, -arrival, name) where arrival = step at which the
-// user's previous task was emitted (0 for a user's first task): the popped
-// user's remainder is consed to the FRONT before a STABLE re-sort (:93-94).
-// Hence for equal dru:  X before Y  <=>  prev(X) was emitted AFTER prev(Y),
-// which recurses on the previous tasks with the roles swapped.
-struct LessMerge {
-  const double* dru;        // by sorted position; NaN = cut by limit-over-quota
-  const int32_t* user_at;   // user of sorted position
-  const int32_t* seg_start; // per user
-  const int32_t* name_rank;
-  __device__ bool operator()(int32_t x, int32_t y) const {
-    double dx = dru[x], dy = dru[y];
-    bool kx = dx == dx, ky = dy == dy;
-    if (kx != ky) return kx;  // truncated tasks sort last
-    if (!kx) return x < y;
-    while (true) {
-      if (dx != dy) return dx < dy;
-      int ux = user_at[x], uy = user_at[y];
-      if (ux == uy) return x < y;  // same user: queue order
-      bool hx = x > seg_start[ux], hy = y > seg_start[uy];
-      if (!hx && !hy) return name_rank[ux] < name_rank[uy];
-      if (!hx) return false;  // X has arrival 0 => Y first
-      if (!hy) return true;
-      // before(X,Y) = before(prev(Y), prev(X)): swap roles and step back
-      int nx = y - 1, ny = x - 1;
-      x = nx; y = ny;
-      dx = dru[x]; dy = dru[y];
-    }
-  }
-};
-
 __global__ void scatter_dru_kernel(const int32_t* __restrict__ idx, const double* __restrict__ dru_at,
                                    int n, double* __restrict__ dru_task) {
   int p = blockIdx.x * blockDim.x + threadIdx.x;
@@ -79,8 +47,9 @@ struct UserCols {
 // (fold.cuh): acc = ((acc + x0) + x1) + ... exactly as `reductions` does.
 __global__ void __launch_bounds__(128) user_fold_kernel(
     const int32_t* __restrict__ idx, TaskCols t, UserCols uc, const int32_t* __restrict__ seg_start,
-    const int32_t* __restrict__ seg_end, int n_users, int dru_mode, int max_over_quota,
-    double* __restrict__ dru_at, int32_t* n_kept_total, const GridFlag* gf, int n_scan) {
+    const int32_t* __restrict__ seg_end, const int32_t* __restrict__ name_rank, int n_users, int dru_mode,
+    int max_over_quota, double* __restrict__ dru_at, int64_t* __restrict__ tie, int32_t* n_kept_total,
+    const GridFlag* gf, int n_scan) {
   if (n_scan > 0 && grid_exact(gf, n_scan)) return;   // the order-wide scans below did it
   __shared__ double stage[4][3][32];
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -138,6 +107,11 @@ __global__ void __launch_bounds__(128) user_fold_kernel(
       if (over > max_over_quota) cut = true;  // later batches are all beyond the cut
     }
   }
+  // the merge comparator's word of every kept task, from the scores this warp just wrote
+  __syncwarp();
+  const int32_t nr = name_rank[u];
+  for (int p = s + lane; p < s + kept; p += 32)
+    tie[p] = merge_tie_word(p, s, u, nr, dru_at[p], [&](int m) { return dru_at[m]; });
   if (lane == 0 && kept) atomicAdd(n_kept_total, kept);
 }
 
@@ -146,11 +120,19 @@ __global__ void __launch_bounds__(128) user_fold_kernel(
 // violation flags.  No user, however long its list, sits on one warp.  Five launches: the two scans,
 // the finish (keep / dru / kept count).
 struct RankScan {
-  const int32_t* user_at; const int32_t* seg_start; UserCols uc;
+  const int32_t* user_at; const int32_t* seg_start; const int32_t* name_rank; UserCols uc;
   OrderScan<double, 3> amt;   // mem, cpus, gpus
   OrderScan<int, 1> viol;     // violating prefixes
   int n, dru_mode, max_over_quota;
-  double* dru_at; int32_t* n_kept_total;
+  double* dru_at; int64_t* tie; int32_t* n_kept_total;
+  // the score of kept position p of user u, whose list starts at s
+  __device__ double score(int p, int s, int u) const {
+    if (dru_mode == 0) {
+      const double x = amt.segment_sum(0, p, s) / uc.div_mem[u], y = amt.segment_sum(1, p, s) / uc.div_cpus[u];
+      return x > y ? x : y;
+    }
+    return amt.segment_sum(2, p, s) / uc.div_gpus[u];
+  }
   // scheduler.clj:2057-2071: a prefix violates when (count, cpus, mem, gpus) is not within the quota
   __device__ void operator()(int p, int (&v)[1]) const {
     const int u = user_at[p], s = seg_start[u];
@@ -177,12 +159,10 @@ __global__ void __launch_bounds__(OS_TB) os_finish(RankScan a, const GridFlag* g
     keep = a.viol.segment_sum(0, p, s) <= a.max_over_quota;
     double d = __longlong_as_double(0x7ff8000000000000LL);
     if (keep) {
-      if (a.dru_mode == 0) {
-        const double x = a.amt.segment_sum(0, p, s) / a.uc.div_mem[u], y = a.amt.segment_sum(1, p, s) / a.uc.div_cpus[u];
-        d = x > y ? x : y;
-      } else {
-        d = a.amt.segment_sum(2, p, s) / a.uc.div_gpus[u];
-      }
+      d = a.score(p, s, u);
+      // the merge comparator's word: the scores before p are recomputed (same bits), not read back, since
+      // other blocks write them.  A kept task's predecessors are kept.
+      a.tie[p] = merge_tie_word(p, s, u, a.name_rank[u], d, [&](int m) { return a.score(m, s, u); });
     }
     a.dru_at[p] = d;
   }
@@ -335,6 +315,7 @@ extern "C" int32_t cook_rank(cook_pool* pool, const cook_tasks_soa* running,
   UserCols uc;
   const int32_t* d_name_rank;
   int32_t *d_idx, *d_tmp, *d_user_at, *d_pos, *d_out_order, *d_out_ranked, *d_seg_start, *d_seg_end, *d_counters;
+  int64_t* d_tie;
   int32_t *d_os_pv, *d_os_bv;
   double *d_dru_at, *d_pool_usage, *d_dru_task, *d_os_pm, *d_os_pc, *d_os_pg, *d_os_b;
   GridFlag* d_gf;
@@ -361,6 +342,7 @@ extern "C" int32_t cook_rank(cook_pool* pool, const cook_tasks_soa* running,
     d_out_order = c.take<int32_t>(N + 1);
     d_out_ranked = c.take<int32_t>(N + 1);
     d_dru_at = c.take<double>(N + 1);
+    d_tie = c.take<int64_t>(N + 1);
     d_seg_start = c.take<int32_t>(U);
     d_seg_end = c.take<int32_t>(U);
     d_pool_usage = c.take<double>(8);
@@ -390,23 +372,22 @@ extern "C" int32_t cook_rank(cook_pool* pool, const cook_tasks_soa* running,
   nl++;
   {
     RankScan os;
-    os.user_at = d_user_at; os.seg_start = d_seg_start; os.uc = uc;
+    os.user_at = d_user_at; os.seg_start = d_seg_start; os.name_rank = d_name_rank; os.uc = uc;
     os.amt = OrderScan<double, 3>{{d_os_pm, d_os_pc, d_os_pg}, {d_os_b, d_os_b + os_nb + 1, d_os_b + 2 * (os_nb + 1)}};
     os.viol = OrderScan<int, 1>{{d_os_pv}, {d_os_bv}};
     os.n = N; os.dru_mode = pool->dru_mode; os.max_over_quota = params->max_over_quota_jobs;
-    os.dru_at = d_dru_at; os.n_kept_total = d_counters;
+    os.dru_at = d_dru_at; os.tie = d_tie; os.n_kept_total = d_counters;
     order_scan(os.amt, LoadAmounts{d_idx, t}, N, d_gf, st, &nl);
     order_scan(os.viol, os, N, d_gf, st, &nl);
     os_finish<<<(N + OS_TB - 1) / OS_TB, OS_TB, 0, st>>>(os, d_gf);
     int warps_per_block = 4;
     int blocks = (U + warps_per_block - 1) / warps_per_block;
     user_fold_kernel<<<blocks, warps_per_block * 32, 0, st>>>(
-        d_idx, t, uc, d_seg_start, d_seg_end, U, pool->dru_mode, params->max_over_quota_jobs,
-        d_dru_at, d_counters, d_gf, N);
+        d_idx, t, uc, d_seg_start, d_seg_end, d_name_rank, U, pool->dru_mode, params->max_over_quota_jobs,
+        d_dru_at, d_tie, d_counters, d_gf, N);
     nl += 2;
   }
-  CK(pool, csort::sort_indices(d_pos, d_tmp, N,
-                               LessMerge{d_dru_at, d_user_at, d_seg_start, d_name_rank}, st, &nl));
+  CK(pool, csort::sort_indices(d_pos, d_tmp, N, LessMerge{d_dru_at, d_tie}, st, &nl));
   qa.pos_sorted = d_pos; qa.idx = d_idx; qa.n_kept = d_counters; qa.R = R;
   qa.cpus = t.cpus; qa.mem = t.mem; qa.gpus = t.gpus;
   qa.filter_offensive = params->filter_offensive;
@@ -425,7 +406,8 @@ extern "C" int32_t cook_rank(cook_pool* pool, const cook_tasks_soa* running,
     qf_quota_kernel<<<1, QF_CH, 0, st>>>(qa, *group_quota, d_pool_usage + 4, d_gf);
     nl++;
   }
-  compact(QueueSurvivors{qa}, N, qa.n_kept, qa.blk_cnt, qa.out_n, N, st, &nl);
+  // at most J survivors: the caller's out_ranked_idx holds J, so no order can make the download overrun it
+  compact(QueueSurvivors{qa}, N, qa.n_kept, qa.blk_cnt, qa.out_n, J, st, &nl);
   if (out_dru) {
     scatter_dru_kernel<<<nb, TB, 0, st>>>(d_idx, d_dru_at, N, d_dru_task);
     nl++;

@@ -1,10 +1,13 @@
-// fold_probe.cu — test-only harness: drives each primitive of cook_b200/csrc/fold.cuh with host inputs.
+// fold_probe.cu — test-only harness: drives each primitive of cook_b200/csrc/fold.cuh, the comparator
+// sort of sort.cuh and the merge comparator LessMerge with host inputs.
 //
 // Built by __graft_entry__.build() into tests/libfoldprobe.so with the product's nvcc flags and loaded by
-// tests/test_fold_primitives.py.  Every entry point copies its host inputs to the device, runs the
-// primitive exactly as the product kernels do, copies the outputs back and returns a cudaError_t
-// (0 = success).  Device buffers are sized from the host arguments, so no call reads or writes past them.
+// tests/test_fold_primitives.py and tests/test_merge_primitives.py.  Every entry point copies its host
+// inputs to the device, runs the primitive exactly as the product kernels do, copies the outputs back and
+// returns a cudaError_t (0 = success).  Device buffers are sized from the host arguments, so no call
+// reads or writes past them.
 #include "../cook_b200/csrc/fold.cuh"
+#include "../cook_b200/csrc/sort.cuh"
 
 namespace {
 
@@ -164,6 +167,30 @@ struct KeepEmit {
   __device__ void emit(int i, int slot) const { out[slot] = i; }
 };
 
+// ---- csort::sort_indices: by key alone (ties left to the sort), or by (key, index)
+struct LessKey {
+  const double* key; int by_index;
+  __device__ bool operator()(int32_t a, int32_t b) const {
+    if (key[a] != key[b]) return key[a] < key[b];
+    return by_index && a < b;
+  }
+};
+
+// ---- LessMerge's tie words, from the scores as the product's fold leaves them (NaN = cut)
+__global__ void tie_kernel(const double* dru, const int* user_at, const int* seg_start, const int* name_rank, int n,
+                           int64_t* tie) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n || dru[p] != dru[p]) return;
+  const int u = user_at[p];
+  tie[p] = merge_tie_word(p, seg_start[u], u, name_rank[u], dru[p], [&](int m) { return dru[m]; });
+}
+
+// ---- LessMerge as a relation: out[i * n + j] = less(i, j)
+__global__ void less_matrix_kernel(LessMerge less, int n, uint8_t* out) {
+  const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < (long long)n * n) out[k] = less((int)(k / n), (int)(k % n)) ? 1 : 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -306,6 +333,52 @@ int fp_compact(const uint8_t* keep, int n_max, int n_dev, int cap, int* out, int
   compact(KeepEmit{d_keep, d_out}, n_max, d_n, d_blk, d_outn, cap, 0);
   b.download(out, d_out, out_len);
   b.download(out_n, d_outn, 1);
+  return b.finish();
+}
+
+int fp_sort_tile() { return csort::TILE; }
+
+// csort::sort_indices of 0 .. n-1 under LessKey{key, by_index}; out: [n]; *launches: the launches it counted
+int fp_sort_indices(const double* key, int n, int by_index, int* out, int* launches) {
+  if (n < 0) return (int)cudaErrorInvalidValue;
+  Bufs b;
+  const double* d_key = b.upload(key, n);
+  int32_t* d_idx = b.alloc<int32_t>(n);
+  int32_t* d_tmp = b.alloc<int32_t>(n);
+  if (b.err != cudaSuccess) return b.err;
+  *launches = 0;
+  b.err = csort::sort_indices(d_idx, d_tmp, n, LessKey{d_key, by_index}, 0, launches);
+  b.download(out, d_idx, n);
+  return b.finish();
+}
+
+// LessMerge over n sorted positions: dru, user_at: [n]; seg_start, name_rank: [n_users].  less: [n][n] gets
+// less(i, j) when non-null; order: [n] gets csort::sort_indices under it when non-null
+int fp_less_merge(const double* dru, const int* user_at, const int* seg_start, const int* name_rank, int n,
+                  int n_users, uint8_t* less, int* order) {
+  if (n < 1 || n_users < 1) return (int)cudaErrorInvalidValue;
+  Bufs b;
+  const double* d_dru = b.upload(dru, n);
+  const int* d_user = b.upload(user_at, n);
+  const int* d_seg = b.upload(seg_start, n_users);
+  const int* d_rank = b.upload(name_rank, n_users);
+  int64_t* d_tie = b.alloc<int64_t>(n);
+  uint8_t* d_less = less ? b.alloc<uint8_t>((size_t)n * n) : nullptr;
+  int32_t* d_idx = order ? b.alloc<int32_t>(n) : nullptr;
+  int32_t* d_tmp = order ? b.alloc<int32_t>(n) : nullptr;
+  if (b.err != cudaSuccess) return b.err;
+  tie_kernel<<<(n + 255) / 256, 256>>>(d_dru, d_user, d_seg, d_rank, n, d_tie);
+  const LessMerge lm{d_dru, d_tie};
+  if (less) {
+    const long long nn = (long long)n * n;
+    less_matrix_kernel<<<(unsigned)((nn + 255) / 256), 256>>>(lm, n, d_less);
+    b.download(less, d_less, (size_t)n * n);
+  }
+  if (order) {
+    int launches = 0;
+    b.err = csort::sort_indices(d_idx, d_tmp, n, lm, 0, &launches);
+    b.download(order, d_idx, n);
+  }
   return b.finish();
 }
 
