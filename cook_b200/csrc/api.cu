@@ -67,6 +67,7 @@ int32_t cook_pool_close(cook_pool* p) {
   p->arena.release();
   if (p->xchg) cudaFree(p->xchg);
   if (p->match_plan && p->match_plan_free) p->match_plan_free(p->match_plan);
+  if (p->state && p->state_free) p->state_free(p->state);
   for (auto& e : p->ev)
     if (e) cudaEventDestroy(e);
   if (p->stream) cudaStreamDestroy(p->stream);
@@ -82,7 +83,7 @@ int32_t cook_last_error(cook_pool* p, char* buf, int32_t len) {
 }
 
 int32_t cook_last_stats(cook_pool* p, int32_t phase, cook_phase_stats* out) {
-  if (!p || !out || phase < 0 || phase > 3) return COOK_E_BADARG;
+  if (!p || !out || phase < 0 || phase > COOK_PHASE_STATE) return COOK_E_BADARG;
   *out = p->phase[phase];
   return COOK_OK;
 }

@@ -120,15 +120,60 @@ struct cook_pool {
   int device = 0;
   int sm_count = 0;
   cudaStream_t stream = nullptr;
-  cudaEvent_t ev[20] = {};
-  cook_phase_stats phase[4] = {};        // last rank / match / rebalance / exchange call
+  cudaEvent_t ev[24] = {};
+  cook_phase_stats phase[5] = {};        // last rank / match / rebalance / exchange / state-apply call
   double* xchg = nullptr;                // exchange buffers: [n_pad] local + [world * n_pad] gathered
   size_t xchg_cap = 0;
   Arena arena;
   void* match_plan = nullptr;            // MatchPlan (match.cu), resident inputs
   void (*match_plan_free)(void*) = nullptr;
+  void* state = nullptr;                 // PoolState (state.cu), the resident job and task tables
+  void (*state_free)(void*) = nullptr;
   char err[512] = {0};
 };
+
+// ---- device sources of rank and match (state.cu feeds them from its resident tables)
+// Dense task columns on the device, running tasks [0, R) then pending jobs [R, R + J).
+struct DevTasks {
+  int R, J;
+  const int32_t* user; const int32_t* prio; const int64_t* start; const int64_t* tid; const int64_t* jid;
+  const double* cpus; const double* mem; const double* gpus;
+};
+// The job columns of a match that the plan carves and the caller then writes on the device (row d of
+// the queue is job d, ranked[d] = d).  Null: the column is absent.
+struct DevJobCols {
+  int32_t* ranked; int32_t* user; double* cpus; double* mem; double* gpus; int64_t* job_id;
+  int32_t* ports; uint8_t* allowed; uint8_t* plugin;
+  int32_t* novel_off; int32_t* novel_host; int32_t* gpu_model; double* disk_request; int32_t* disk_type;
+  int32_t* attr_off; int32_t* attr_col; int32_t* attr_val; int64_t* est_end_ms; int32_t* ckpt_location;
+  int32_t* reserved_host; int32_t* group_off; int32_t* group_idx;
+};
+// What such a match holds, known on the host without looking at the rows: which columns carry a
+// non-absent value somewhere, and upper bounds of the list lengths (0: the list is absent).
+struct DevJobSpec {
+  bool ports, allowed, plugin, gpu_model, disk, est_end, ckpt, reserved, any_gpus;
+  int64_t n_novel, n_attr, n_group;
+  const int32_t* gp_off;   // host [n_groups + 1]: per-group member capacity offsets
+  DevJobCols out;          // set by the plan
+};
+
+#include <functional>
+// rank.cu: cook_rank over host columns (dev == nullptr) or dense device columns.  With dev,
+// out_ranked_idx may be null (not downloaded) and on_queue, if given, is called with the device queue
+// (pending indices) and its device length before the result download, on the pool's stream.
+int32_t rank_impl(cook_pool* pool, const cook_tasks_soa* running, const cook_tasks_soa* pending, const DevTasks* dev,
+                  const cook_user_table* users, const cook_pool_quota* pool_quota, const cook_pool_quota* group_quota,
+                  const double* group_usage, const cook_rank_params* params, int32_t* out_ranked_idx, int32_t* out_n,
+                  double* out_dru, int32_t* out_order, int32_t* out_order_n,
+                  const std::function<int32_t(const int32_t* d_ranked, const int32_t* d_n, int* launches)>* on_queue);
+// match.cu: cook_match over n_ranked jobs whose columns `fill` writes on the device once the plan has
+// carved them (dj->out); out_job_id receives the job id of every considerable job.
+int32_t match_device_jobs(cook_pool* pool, int32_t n_ranked, DevJobSpec* dj,
+                          const std::function<int32_t(const DevJobCols&, int* launches)>& fill,
+                          const cook_offers_soa* offers, const cook_groups* groups, const cook_user_table* users,
+                          const cook_pool_quota* pool_quota, const cook_match_params* params, int64_t* out_job_id,
+                          int32_t* out_assign, int32_t* out_ports, int32_t max_ports, uint8_t* out_fail_reason,
+                          cook_match_stats* out_stats);
 
 inline int32_t set_err(cook_pool* p, int32_t code, const char* fmt, ...) {
   if (p) {

@@ -2220,6 +2220,11 @@ __global__ void __launch_bounds__(128) usage_delta_kernel(ConsArgs a, const int3
   if (lane == 0) { delta[4 * u] = d[0]; delta[4 * u + 1] = d[1]; delta[4 * u + 2] = d[2]; delta[4 * u + 3] = d[3]; }
 }
 
+__global__ void cons_job_id_kernel(const int32_t* cons, const int64_t* job_id, int n, int64_t* out) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < n) out[k] = job_id[cons[k]];
+}
+
 __global__ void count_flags_kernel(const int32_t* flags, int n, int32_t* out) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   int v = (i < n && flags[i]) ? 1 : 0;
@@ -2267,6 +2272,8 @@ struct MatchPlan {
   double *d_smin_c = nullptr, *d_smin_m = nullptr, *d_smin_bc = nullptr, *d_smin_bm = nullptr;
   size_t max_blocks = 0;
   int32_t bk_init[3] = {0, 0, 0};
+  int64_t* d_job_id = nullptr;    // device-source plans: job id per row, and per considerable job
+  int64_t* d_cons_jid = nullptr;
 };
 
 static void plan_free(void* p) {
@@ -2274,13 +2281,30 @@ static void plan_free(void* p) {
   if (mp) { mp->arena.release(); delete mp; }
 }
 
+// A job column of the plan: uploaded from the host, or (dj) carved for the caller to write when present.
+template <class T>
+static T* job_col(Carve& c, const T* host, size_t n, const DevJobSpec* dj, bool present, T** dev_out) {
+  if (!dj) return c.up(host, n);
+  T* d = present ? c.take<T>(n ? n : 1) : nullptr;
+  *dev_out = d;
+  return d;
+}
+
+// dj: the job columns come from the device (match_device_jobs); `jobs` is then unused and the ranked
+// queue is 0 .. n_ranked-1 over n_ranked jobs.
 static int32_t build_plan(cook_pool* pool, MatchPlan* mp, const int32_t* ranked_idx,
-                          int32_t n_ranked, const cook_jobs_soa* jobs,
+                          int32_t n_ranked, const cook_jobs_soa* jobs_in,
                           const cook_offers_soa* offers, const cook_groups* groups,
                           const cook_user_table* users, const cook_pool_quota* pool_quota,
-                          const cook_match_params* params, int32_t max_ports) {
+                          const cook_match_params* params, int32_t max_ports, DevJobSpec* dj = nullptr) {
   cudaStream_t st = pool->stream;
   Arena& ar = mp->arena;
+  cook_jobs_soa none;
+  memset(&none, 0, sizeof(none));
+  none.n = n_ranked;
+  const cook_jobs_soa* jobs = dj ? &none : jobs_in;
+  DevJobCols dc;
+  memset(&dc, 0, sizeof(dc));
   const int J = jobs->n, O = offers->n, U = users->n_users, NC = params->num_considerable;
   mp->valid = false;
   // host-side prep: offers sorted by hostname rank (tie-break order)
@@ -2299,7 +2323,10 @@ static int32_t build_plan(cook_pool* pool, MatchPlan* mp, const int32_t* ranked_
   const int G = groups ? groups->n_groups : 0;
   std::vector<int32_t> gp_off(G + 1, 0);
   size_t n_memb = 0;
-  if (G && jobs->group_off) {
+  if (G && dj && dj->n_group) {
+    gp_off.assign(dj->gp_off, dj->gp_off + G + 1);
+    n_memb = gp_off[G];
+  } else if (G && jobs->group_off) {
     n_memb = jobs->group_off[J];
     for (size_t i = 0; i < n_memb; i++) {
       int g = jobs->group_idx[i];
@@ -2314,6 +2341,9 @@ static int32_t build_plan(cook_pool* pool, MatchPlan* mp, const int32_t* ranked_
                     jobs->est_end_ms || jobs->ckpt_location || jobs->reserved_host ||
                     (jobs->group_off && G) || offers->is_k8s || offers->max_tasks ||
                     offers->reserved || offers->gpu_off;
+  if (dj)   // the state counts its non-absent values per column as rows come and go
+    constr_eff = constr_eff || dj->n_novel || dj->gpu_model || dj->disk || dj->n_attr || dj->est_end || dj->ckpt ||
+                 dj->reserved || (dj->n_group && G) || dj->any_gpus || dj->ports;
   if (!constr_eff && jobs->gpus)
     for (int j = 0; j < J && !constr_eff; j++) constr_eff = jobs->gpus[j] != 0.0;
   if (!constr_eff && jobs->ports)
@@ -2345,29 +2375,39 @@ static int32_t build_plan(cook_pool* pool, MatchPlan* mp, const int32_t* ranked_
   of.n_attr_cols = offers->attr ? offers->n_attr_cols : 0;
   mp->h2d_bytes = 0;
   const cudaError_t carved = carve(ar, st, nullptr, &mp->h2d_bytes, [&](Carve& c) {
-    ca.ranked = c.up(ranked_idx, n_ranked);
-    jb.user = c.up(jobs->user, J);
-    jb.cpus = c.up(jobs->cpus, J); jb.mem = c.up(jobs->mem, J); jb.gpus = c.up(jobs->gpus, J);
-    jb.ports = c.up(jobs->ports, J);
-    jb.allowed = c.up(jobs->allowed, J); jb.plugin = c.up(jobs->plugin_accept, J);
-    if (jobs->novel_off) {
-      jb.novel_off = c.up(jobs->novel_off, J + 1);
-      jb.novel_host = c.up(jobs->novel_host, std::max(1, jobs->novel_off[J]));
+    ca.ranked = job_col(c, ranked_idx, n_ranked, dj, true, &dc.ranked);
+    jb.user = job_col(c, jobs->user, J, dj, true, &dc.user);
+    jb.cpus = job_col(c, jobs->cpus, J, dj, true, &dc.cpus);
+    jb.mem = job_col(c, jobs->mem, J, dj, true, &dc.mem);
+    jb.gpus = job_col(c, jobs->gpus, J, dj, true, &dc.gpus);
+    jb.ports = job_col(c, jobs->ports, J, dj, dj && dj->ports, &dc.ports);
+    jb.allowed = job_col(c, jobs->allowed, J, dj, dj && dj->allowed, &dc.allowed);
+    jb.plugin = job_col(c, jobs->plugin_accept, J, dj, dj && dj->plugin, &dc.plugin);
+    if (jobs->novel_off || (dj && dj->n_novel)) {
+      jb.novel_off = job_col(c, jobs->novel_off, J + 1, dj, true, &dc.novel_off);
+      jb.novel_host = job_col(c, jobs->novel_host, std::max<size_t>(1, dj ? dj->n_novel : jobs->novel_off[J]), dj, true,
+                              &dc.novel_host);
     }
-    jb.gpu_model = c.up(jobs->gpu_model, J);
-    jb.disk_request = c.up(jobs->disk_request, J);
-    jb.disk_type = c.up(jobs->disk_type, J);
-    if (jobs->attr_off) {
-      const int na = std::max(1, jobs->attr_off[J]);
-      jb.attr_off = c.up(jobs->attr_off, J + 1);
-      jb.attr_col = c.up(jobs->attr_col, na); jb.attr_val = c.up(jobs->attr_val, na);
+    jb.gpu_model = job_col(c, jobs->gpu_model, J, dj, dj && dj->gpu_model, &dc.gpu_model);
+    jb.disk_request = job_col(c, jobs->disk_request, J, dj, dj && dj->disk, &dc.disk_request);
+    jb.disk_type = job_col(c, jobs->disk_type, J, dj, dj && dj->disk, &dc.disk_type);
+    if (jobs->attr_off || (dj && dj->n_attr)) {
+      const size_t na = std::max<size_t>(1, dj ? dj->n_attr : jobs->attr_off[J]);
+      jb.attr_off = job_col(c, jobs->attr_off, J + 1, dj, true, &dc.attr_off);
+      jb.attr_col = job_col(c, jobs->attr_col, na, dj, true, &dc.attr_col);
+      jb.attr_val = job_col(c, jobs->attr_val, na, dj, true, &dc.attr_val);
     }
-    jb.est_end_ms = c.up(jobs->est_end_ms, J);
-    jb.ckpt_location = c.up(jobs->ckpt_location, J); jb.reserved_host = c.up(jobs->reserved_host, J);
-    if (jobs->group_off && G) {
-      jb.group_off = c.up(jobs->group_off, J + 1);
-      jb.group_idx = c.up(jobs->group_idx, std::max<size_t>(1, n_memb));
+    jb.est_end_ms = job_col(c, jobs->est_end_ms, J, dj, dj && dj->est_end, &dc.est_end_ms);
+    jb.ckpt_location = job_col(c, jobs->ckpt_location, J, dj, dj && dj->ckpt, &dc.ckpt_location);
+    jb.reserved_host = job_col(c, jobs->reserved_host, J, dj, dj && dj->reserved, &dc.reserved_host);
+    if ((jobs->group_off || (dj && dj->n_group)) && G) {
+      jb.group_off = job_col(c, jobs->group_off, J + 1, dj, true, &dc.group_off);
+      jb.group_idx = job_col(c, jobs->group_idx, std::max<size_t>(1, n_memb), dj, true, &dc.group_idx);
     }
+    // the job ids of the rows, for the result (device source only)
+    mp->d_job_id = dj ? c.take<int64_t>(J + 1) : nullptr;
+    dc.job_id = mp->d_job_id;
+    mp->d_cons_jid = dj ? c.take<int64_t>(NC + 1) : nullptr;
 
     mp->d_perm = c.up(perm.data(), O); of.perm = mp->d_perm;
     mp->d_oc = c.up(offers->cpus, O); mp->d_om = c.up(offers->mem, O);
@@ -2400,7 +2440,7 @@ static int32_t build_plan(cook_pool* pool, MatchPlan* mp, const int32_t* ranked_
     mp->d_attr_v = c.take<int32_t>((size_t)of.n_attr_cols * O + 1);
     of.vc = mp->d_vc; of.attr_v = mp->d_attr_v;
 
-    if (G && jobs->group_off) {
+    if (G && (jobs->group_off || (dj && dj->n_group))) {
       gr.n_groups = G;
       gr.kind = c.up(groups->kind, G);
       gr.attr_col = c.up(groups->attr_col, G);
@@ -2488,13 +2528,15 @@ static int32_t build_plan(cook_pool* pool, MatchPlan* mp, const int32_t* ranked_
   if (const char* el = getenv("COOK_LOOKAHEAD")) { int v = atoi(el); if (v >= 2 && v <= RING - 1) ma.lookahead = v; }
   mp->J = J; mp->O = O; mp->U = U; mp->n_ranked = n_ranked; mp->NC = NC; mp->max_ports = max_ports;
   mp->G = G; mp->B = B; mp->constr = constr_eff; mp->n_memb = n_memb;
+  if (dj) dj->out = dc;
   mp->valid = true;
   return COOK_OK;
 }
 
+// out_job_id (device-source plans, instead of out_considerable): the job id of every considerable job
 static int32_t run_plan(cook_pool* pool, MatchPlan* mp, int32_t* out_considerable,
                         int32_t* out_assign, int32_t* out_ports, uint8_t* out_fail_reason,
-                        cook_match_stats* out_stats, bool uploaded, int max_ctas) {
+                        cook_match_stats* out_stats, bool uploaded, int max_ctas, int64_t* out_job_id = nullptr) {
   cudaStream_t st = pool->stream;
   const int O = mp->O, U = mp->U, n_ranked = mp->n_ranked, max_ports = mp->max_ports;
   MatchArgs& ma = mp->ma;
@@ -2648,11 +2690,16 @@ static int32_t run_plan(cook_pool* pool, MatchPlan* mp, int32_t* out_considerabl
                                                            max_ports, mp->d_used);
     count_flags_kernel<<<(O + TB) / TB, TB, 0, st>>>(mp->d_used, O, mp->d_counters + 1);
     launches += 2;
+    if (out_job_id && mp->d_cons_jid) {
+      cons_job_id_kernel<<<(n_cons + TB - 1) / TB, TB, 0, st>>>(mp->d_cons, mp->d_job_id, n_cons, mp->d_cons_jid);
+      launches++;
+    }
     CK(pool, cudaGetLastError());
   }
   CK(pool, cudaEventRecord(pool->ev[3], st));
   if (n_cons > 0) {
-    CK(pool, download(out_considerable, mp->d_cons, n_cons, st, &d2h));
+    if (out_considerable) CK(pool, download(out_considerable, mp->d_cons, n_cons, st, &d2h));
+    if (out_job_id && mp->d_cons_jid) CK(pool, download(out_job_id, mp->d_cons_jid, n_cons, st, &d2h));
     CK(pool, download(out_assign, mp->d_out_assign, n_cons, st, &d2h));
     if (out_ports && max_ports > 0) CK(pool, download(out_ports, mp->d_out_ports, (size_t)n_cons * max_ports, st, &d2h));
     if (out_fail_reason) CK(pool, download(out_fail_reason, ma.fail, n_cons, st, &d2h));
@@ -2747,6 +2794,41 @@ extern "C" int32_t cook_match(cook_pool* pool, const int32_t* ranked_idx, int32_
   }
   return run_plan(pool, mp, out_considerable, out_assign, out_ports, out_fail_reason, out_stats, !reuse,
                   params->max_ctas);
+}
+
+// cook_match over jobs whose columns live on the device (state.cu): the same checks of the offer and
+// group tables, the same plan with the job columns carved for `fill`, the same run.
+int32_t match_device_jobs(cook_pool* pool, int32_t n_ranked, DevJobSpec* dj,
+                          const std::function<int32_t(const DevJobCols&, int*)>& fill,
+                          const cook_offers_soa* offers, const cook_groups* groups, const cook_user_table* users,
+                          const cook_pool_quota* pool_quota, const cook_match_params* params, int64_t* out_job_id,
+                          int32_t* out_assign, int32_t* out_ports, int32_t max_ports, uint8_t* out_fail_reason,
+                          cook_match_stats* out_stats) {
+  const int O = offers->n, NC = params->num_considerable;
+  if (out_stats) memset(out_stats, 0, sizeof(*out_stats));
+  if (n_ranked == 0 || NC == 0) return COOK_OK;
+  if (!offers->name_rank && O > 0) return set_err(pool, COOK_E_BADARG, "cook_state_match: offers.name_rank required");
+  if (groups && !idx_in_range(groups->attr_col, groups->n_groups, -1, std::max(1, offers->n_attr_cols)))
+    return set_err(pool, COOK_E_BADARG, "cook_state_match: groups.attr_col out of range");
+  const bool grouped = groups && groups->n_groups && dj->n_group;
+  if ((dj->n_novel || offers->reserved || grouped) && !offers->hostname_id)
+    return set_err(pool, COOK_E_BADARG, "cook_state_match: hostname_id column required by constraints");
+  if (grouped && (!groups->cot_off || !groups->kind)) return set_err(pool, COOK_E_BADARG, "cook_state_match: incomplete cook_groups");
+  CK(pool, cudaSetDevice(pool->device));
+  if (!pool->match_plan) {
+    pool->match_plan = new MatchPlan();
+    pool->match_plan_free = plan_free;
+  }
+  MatchPlan* mp = static_cast<MatchPlan*>(pool->match_plan);
+  CK(pool, cudaEventRecord(pool->ev[0], pool->stream));
+  int32_t rc = build_plan(pool, mp, nullptr, n_ranked, nullptr, offers, groups, users, pool_quota, params, max_ports, dj);
+  int fill_launches = 0;
+  if (rc == COOK_OK) rc = fill(dj->out, &fill_launches);
+  if (rc != COOK_OK) { mp->valid = false; return rc; }
+  rc = run_plan(pool, mp, nullptr, out_assign, out_ports, out_fail_reason, out_stats, true, params->max_ctas, out_job_id);
+  pool->phase[COOK_PHASE_MATCH].n_launches += fill_launches;
+  if (out_stats) out_stats->n_launches += fill_launches;
+  return rc;
 }
 
 

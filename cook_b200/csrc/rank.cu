@@ -300,11 +300,21 @@ extern "C" int32_t cook_rank(cook_pool* pool, const cook_tasks_soa* running,
                              int32_t* out_ranked_idx, int32_t* out_n, double* out_dru,
                              int32_t* out_order, int32_t* out_order_n) {
   if (!pool) return COOK_E_BADARG;
-  if (!running || !pending || !users || !params || !out_ranked_idx || !out_n)
-    return set_err(pool, COOK_E_BADARG, "cook_rank: null argument");
-  const int R = running->n, J = pending->n, N = R + J, U = users->n_users;
+  if (!running || !pending || !out_ranked_idx) return set_err(pool, COOK_E_BADARG, "cook_rank: null argument");
+  return rank_impl(pool, running, pending, nullptr, users, pool_quota, group_quota, group_usage, params, out_ranked_idx,
+                   out_n, out_dru, out_order, out_order_n, nullptr);
+}
+
+int32_t rank_impl(cook_pool* pool, const cook_tasks_soa* running, const cook_tasks_soa* pending, const DevTasks* dev,
+                  const cook_user_table* users, const cook_pool_quota* pool_quota, const cook_pool_quota* group_quota,
+                  const double* group_usage, const cook_rank_params* params, int32_t* out_ranked_idx, int32_t* out_n,
+                  double* out_dru, int32_t* out_order, int32_t* out_order_n,
+                  const std::function<int32_t(const int32_t*, const int32_t*, int*)>* on_queue) {
+  if (!users || !params || !out_n) return set_err(pool, COOK_E_BADARG, "cook_rank: null argument");
+  const int R = dev ? dev->R : running->n, J = dev ? dev->J : pending->n, N = R + J, U = users->n_users;
   if (R < 0 || J < 0 || U <= 0) return set_err(pool, COOK_E_BADARG, "cook_rank: bad sizes");
-  if (!idx_in_range(running->user, R, 0, U) || !idx_in_range(pending->user, J, 0, U))
+  // device rows had their user codes checked when they entered (state.cu)
+  if (!dev && (!idx_in_range(running->user, R, 0, U) || !idx_in_range(pending->user, J, 0, U)))
     return set_err(pool, COOK_E_BADARG, "cook_rank: task user index out of range");
   *out_n = 0;
   if (out_order_n) *out_order_n = 0;
@@ -323,14 +333,18 @@ extern "C" int32_t cook_rank(cook_pool* pool, const cook_tasks_soa* running,
   const int os_nb = (N + OS_TILE - 1) / OS_TILE;
   int64_t h2d = 0, d2h = 0;
   const cudaError_t carved = carve(pool->arena, st, pool->ev[8], &h2d, [&](Carve& c) {
-    t.user = c.cat(running->user, R, pending->user, J);
-    t.prio = c.cat(running->priority, R, pending->priority, J);
-    t.start = c.cat(running->start_time, R, pending->start_time, J);
-    t.tid = c.cat(running->task_id, R, pending->task_id, J);
-    t.jid = c.cat(running->job_id, R, pending->job_id, J);
-    t.cpus = c.cat(running->cpus, R, pending->cpus, J);
-    t.mem = c.cat(running->mem, R, pending->mem, J);
-    t.gpus = c.cat(running->gpus, R, pending->gpus, J);
+    if (dev) {
+      t = TaskCols{dev->user, dev->prio, dev->start, dev->tid, dev->jid, dev->cpus, dev->mem, dev->gpus};
+    } else {
+      t.user = c.cat(running->user, R, pending->user, J);
+      t.prio = c.cat(running->priority, R, pending->priority, J);
+      t.start = c.cat(running->start_time, R, pending->start_time, J);
+      t.tid = c.cat(running->task_id, R, pending->task_id, J);
+      t.jid = c.cat(running->job_id, R, pending->job_id, J);
+      t.cpus = c.cat(running->cpus, R, pending->cpus, J);
+      t.mem = c.cat(running->mem, R, pending->mem, J);
+      t.gpus = c.cat(running->gpus, R, pending->gpus, J);
+    }
     d_name_rank = c.up(users->name_rank, U);
     uc.div_mem = c.up(users->div_mem, U); uc.div_cpus = c.up(users->div_cpus, U); uc.div_gpus = c.up(users->div_gpus, U);
     uc.q_count = c.up(users->quota_count, U); uc.q_cpus = c.up(users->quota_cpus, U);
@@ -413,12 +427,16 @@ extern "C" int32_t cook_rank(cook_pool* pool, const cook_tasks_soa* running,
     nl++;
   }
   CK(pool, cudaGetLastError());
+  if (on_queue) {
+    const int32_t rc = (*on_queue)(d_out_ranked, qa.out_n, &nl);
+    if (rc != COOK_OK) return rc;
+  }
   CK(pool, cudaEventRecord(pool->ev[10], st));
   int32_t h_counters[2] = {0, 0};
   CK(pool, download(h_counters, d_counters, 2, st, &d2h));
   CK(pool, cudaStreamSynchronize(st));
   const int32_t n_kept = h_counters[0], n_out = h_counters[1];
-  if (n_out > 0) CK(pool, download(out_ranked_idx, d_out_ranked, n_out, st, &d2h));
+  if (n_out > 0 && out_ranked_idx) CK(pool, download(out_ranked_idx, d_out_ranked, n_out, st, &d2h));
   if (out_order && n_kept > 0) CK(pool, download(out_order, d_out_order, n_kept, st, &d2h));
   if (out_dru) CK(pool, download(out_dru, d_dru_task, N, st, &d2h));
   CK(pool, cudaEventRecord(pool->ev[11], st));

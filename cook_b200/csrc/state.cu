@@ -1,0 +1,761 @@
+// state.cu — the resident pool state (SURVEY §8f-1, device half): a pool's pending jobs and running
+// tasks kept on the device between cycles, changed by deltas, ranked and matched in place.
+//
+// Host, O(delta) per batch: the id -> slot maps and free lists, per-slot facts (user code, list lengths,
+// which columns hold a non-absent value, the group and attribute-column codes) and the counts and code
+// maxima derived from them.  Device: one SoA table per kind whose capacity doubles with device-to-device
+// copies, a live flag and a generation stamp per slot, and one append-only arena per CSR list with a
+// per-slot (off, len), compacted once its dead entries outnumber the live ones.
+// Rank and match gather dense columns from the tables with fold.cuh's compaction and order-wide scan and
+// then run cook_rank's and cook_match's own code on them (rank_impl, match_device_jobs).  The ranked
+// queue stays on the device as (slot, generation) pairs; a match keeps the entries whose slot still holds
+// that generation, so a job removed or replaced since the rank leaves the queue.
+#include <algorithm>
+#include <map>
+#include <unordered_map>
+#include <unordered_set>
+
+#include "fold.cuh"
+
+namespace {
+
+// ---- device tables: column k of a table is cols[k] (sz bytes per slot)
+enum PCol {
+  P_USER, P_PRIO, P_JID, P_CPUS, P_MEM, P_GPUS, P_PORTS, P_ALLOWED, P_PLUGIN, P_GPU_MODEL, P_DISK_REQ, P_DISK_TYPE,
+  P_EST, P_CKPT, P_RESERVED, P_NDATA,   // the columns a delta row carries
+  P_LIVE = P_NDATA, P_GEN, P_NOFF, P_NLEN, P_AOFF, P_ALEN, P_GOFF, P_GLEN, P_NCOL
+};
+constexpr int P_SZ[P_NCOL] = {4, 4, 8, 8, 8, 8, 4, 1, 1, 4, 8, 4, 8, 4, 4, 1, 4, 4, 4, 4, 4, 4, 4};
+enum RCol { R_USER, R_PRIO, R_START, R_TID, R_JID, R_CPUS, R_MEM, R_GPUS, R_NDATA, R_LIVE = R_NDATA, R_GEN, R_NCOL };
+constexpr int R_SZ[R_NCOL] = {4, 4, 8, 8, 8, 8, 8, 8, 1, 4};
+
+enum { L_NOVEL = 0, L_ATTR = 1, L_GROUP = 2 };
+
+// ---- scatter: row i of a batch to slot[i].  Upserts write the columns (a null source writes the
+// column's absent value) and the rows' list ranges; removals clear the live flag.  Both bump the
+// generation, which is what retires a queue entry.
+constexpr int MAXC = 16;
+struct ScatterCol { char* dst; const char* src; long long dflt; int sz; };
+struct ScatterArgs {
+  ScatterCol c[MAXC];
+  int nc, n, upsert;
+  const int32_t* slot;
+  uint8_t* live;
+  uint32_t* gen;
+  int32_t* loff[3];        // per-slot list range; null: the table has no lists
+  int32_t* llen[3];
+  const int32_t* doff[3];  // the batch's CSR offsets (null: empty lists)
+  int32_t tail[3];         // where the batch's lists were appended
+};
+
+__global__ void scatter_kernel(ScatterArgs a) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= a.n) return;
+  const int s = a.slot[i];
+#pragma unroll
+  for (int k = 0; k < MAXC; k++) {
+    if (k >= a.nc) break;
+    const ScatterCol& c = a.c[k];
+    if (c.sz == 1) reinterpret_cast<uint8_t*>(c.dst)[s] = c.src ? reinterpret_cast<const uint8_t*>(c.src)[i] : (uint8_t)c.dflt;
+    else if (c.sz == 4) reinterpret_cast<int32_t*>(c.dst)[s] = c.src ? reinterpret_cast<const int32_t*>(c.src)[i] : (int32_t)c.dflt;
+    else reinterpret_cast<long long*>(c.dst)[s] = c.src ? reinterpret_cast<const long long*>(c.src)[i] : c.dflt;
+  }
+  a.live[s] = a.upsert ? 1 : 0;
+  a.gen[s] += 1u;
+#pragma unroll
+  for (int l = 0; l < 3; l++)
+    if (a.loff[l]) {
+      const bool has = a.upsert && a.doff[l];
+      const int o = has ? a.doff[l][i] : 0;
+      a.loff[l][s] = a.tail[l] + o;
+      a.llen[l][s] = has ? a.doff[l][i + 1] - o : 0;
+    }
+}
+
+// ---- list lengths for the order-wide scan (integer sums: any association is exact)
+struct SlotLen {   // arena compaction: slot p, dead slots hold nothing
+  const uint8_t* live; const int32_t* len;
+  __device__ void operator()(int p, int (&x)[1]) const { x[0] = live[p] ? len[p] : 0; }
+};
+struct RowLen {    // the match's row p is slot m_slot[p]
+  const int32_t* m_slot; const int32_t* len;
+  __device__ void operator()(int p, int (&x)[1]) const { x[0] = len[m_slot[p]]; }
+};
+
+// warp per live slot: its list moves to the exclusive scan of the live lengths in the new arena
+__global__ void list_compact_kernel(OrderScan<int, 1> os, const uint8_t* live, int32_t* off, const int32_t* len, int n,
+                                    const int32_t* src0, const int32_t* src1, int32_t* dst0, int32_t* dst1) {
+  const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (w >= n || !live[w]) return;
+  const int l = len[w], start = os.at(0, w) - l, o = off[w];
+  for (int i = lane; i < l; i += 32) {
+    dst0[start + i] = src0[o + i];
+    if (dst1) dst1[start + i] = src1[o + i];
+  }
+  __syncwarp();
+  if (lane == 0) off[w] = start;
+}
+
+// warp per match row: the row's list into the dense CSR (doff[n + 1], values) cook_match reads
+__global__ void csr_gather_kernel(OrderScan<int, 1> os, const int32_t* m_slot, int n, const int32_t* off,
+                                  const int32_t* len, const int32_t* src0, const int32_t* src1, int32_t* doff,
+                                  int32_t* dst0, int32_t* dst1) {
+  const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (w >= n) return;
+  const int s = m_slot[w], l = len[s], end = os.at(0, w), start = end - l, o = off[s];
+  for (int i = lane; i < l; i += 32) {
+    dst0[start + i] = src0[o + i];
+    if (dst1) dst1[start + i] = src1[o + i];
+  }
+  if (lane == 0) {
+    doff[w + 1] = end;
+    if (w == 0) doff[0] = 0;
+  }
+}
+
+// ---- rank: live rows -> dense task columns (running first), compacted in slot order
+struct DenseTasks {
+  int32_t* user; int32_t* prio; int64_t* start; int64_t* tid; int64_t* jid; double* cpus; double* mem; double* gpus;
+  int32_t* pslot;   // dense pending index -> slot
+};
+struct RunningRows {
+  void* const* col; DenseTasks o;
+  __device__ bool keep(int i) const { return static_cast<const uint8_t*>(col[R_LIVE])[i]; }
+  __device__ void emit(int i, int d) const {
+    o.user[d] = static_cast<const int32_t*>(col[R_USER])[i];
+    o.prio[d] = static_cast<const int32_t*>(col[R_PRIO])[i];
+    o.start[d] = static_cast<const int64_t*>(col[R_START])[i];
+    o.tid[d] = static_cast<const int64_t*>(col[R_TID])[i];
+    o.jid[d] = static_cast<const int64_t*>(col[R_JID])[i];
+    o.cpus[d] = static_cast<const double*>(col[R_CPUS])[i];
+    o.mem[d] = static_cast<const double*>(col[R_MEM])[i];
+    o.gpus[d] = static_cast<const double*>(col[R_GPUS])[i];
+  }
+};
+struct PendingRows {
+  void* const* col; DenseTasks o; int R;
+  __device__ bool keep(int i) const { return static_cast<const uint8_t*>(col[P_LIVE])[i]; }
+  __device__ void emit(int i, int d) const {
+    o.pslot[d] = i;
+    d += R;
+    o.user[d] = static_cast<const int32_t*>(col[P_USER])[i];
+    o.prio[d] = static_cast<const int32_t*>(col[P_PRIO])[i];
+    o.start[d] = INT64_MAX;   // a pending job's synthetic task (tools.clj:582-588)
+    o.tid[d] = -1;
+    o.jid[d] = static_cast<const int64_t*>(col[P_JID])[i];
+    o.cpus[d] = static_cast<const double*>(col[P_CPUS])[i];
+    o.mem[d] = static_cast<const double*>(col[P_MEM])[i];
+    o.gpus[d] = static_cast<const double*>(col[P_GPUS])[i];
+  }
+};
+
+// the ranked queue (dense pending indices) as (slot, generation) pairs, and its job ids
+__global__ void queue_kernel(const int32_t* ranked, const int32_t* n, const int32_t* pslot, const uint32_t* gen,
+                             const int64_t* jid, int32_t* q_slot, uint32_t* q_gen, int64_t* q_jid) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= *n) return;
+  const int s = pslot[ranked[k]];
+  q_slot[k] = s; q_gen[k] = gen[s]; q_jid[k] = jid[s];
+}
+
+// ---- match: the queue entries whose slot still holds their generation, in queue order
+struct QueueLive {
+  const int32_t* q_slot; const uint32_t* q_gen; const uint8_t* live; const uint32_t* gen; int32_t* m_slot;
+  __device__ bool keep(int k) const { const int s = q_slot[k]; return live[s] && gen[s] == q_gen[k]; }
+  __device__ void emit(int k, int d) const { m_slot[d] = q_slot[k]; }
+};
+
+// row d of the match is slot m_slot[d]: its columns into the plan's (ranked[d] = d)
+__global__ void fill_rows_kernel(DevJobCols o, void* const* col, const int32_t* m_slot, int n) {
+  const int d = blockIdx.x * blockDim.x + threadIdx.x;
+  if (d >= n) return;
+  const int s = m_slot[d];
+  o.ranked[d] = d;
+  o.user[d] = static_cast<const int32_t*>(col[P_USER])[s];
+  o.cpus[d] = static_cast<const double*>(col[P_CPUS])[s];
+  o.mem[d] = static_cast<const double*>(col[P_MEM])[s];
+  o.gpus[d] = static_cast<const double*>(col[P_GPUS])[s];
+  o.job_id[d] = static_cast<const int64_t*>(col[P_JID])[s];
+  if (o.ports) o.ports[d] = static_cast<const int32_t*>(col[P_PORTS])[s];
+  if (o.allowed) o.allowed[d] = static_cast<const uint8_t*>(col[P_ALLOWED])[s];
+  if (o.plugin) o.plugin[d] = static_cast<const uint8_t*>(col[P_PLUGIN])[s];
+  if (o.gpu_model) o.gpu_model[d] = static_cast<const int32_t*>(col[P_GPU_MODEL])[s];
+  if (o.disk_request) {
+    o.disk_request[d] = static_cast<const double*>(col[P_DISK_REQ])[s];
+    o.disk_type[d] = static_cast<const int32_t*>(col[P_DISK_TYPE])[s];
+  }
+  if (o.est_end_ms) o.est_end_ms[d] = static_cast<const int64_t*>(col[P_EST])[s];
+  if (o.ckpt_location) o.ckpt_location[d] = static_cast<const int32_t*>(col[P_CKPT])[s];
+  if (o.reserved_host) o.reserved_host[d] = static_cast<const int32_t*>(col[P_RESERVED])[s];
+}
+
+// ---- host side
+// the non-absent values of a pending row, counted per column (the match's constraint switch)
+enum { F_GPUS, F_PORTS, F_NOT_ALLOWED, F_NOT_PLUGIN, F_GPU_MODEL, F_DISK, F_EST, F_CKPT, F_RESERVED, F_N };
+
+struct PendingInfo {
+  int32_t user = 0;
+  int32_t len[3] = {0, 0, 0};
+  uint16_t flags = 0;
+  std::vector<int32_t> groups, attr_cols;
+};
+
+template <class T>
+cudaError_t ensure(T*& p, size_t& cap, size_t n) {   // scratch: contents are not kept
+  if (n <= cap && p) return cudaSuccess;
+  if (p) cudaFree(p);
+  p = nullptr;
+  const size_t want = std::max(n, 2 * cap) + 1;
+  cap = 0;
+  cudaError_t e = cudaMalloc(&p, want * sizeof(T));
+  if (e == cudaSuccess) cap = want;
+  return e;
+}
+
+struct Table {
+  int ncol = 0;
+  const int* sz = nullptr;
+  void* col[P_NCOL] = {};
+  void** d_col = nullptr;        // the column pointers on the device (for the gather kernels)
+  int32_t cap = 0, hw = 0;       // slots allocated, slots ever used
+  std::unordered_map<int64_t, int32_t> slot_of;
+  std::vector<int32_t> free;
+
+  // capacity >= n: new columns, zeroed, the old contents copied (device to device)
+  cudaError_t grow(int32_t n, cudaStream_t st) {
+    if (n <= cap) return cudaSuccess;
+    const int32_t ncap = std::max<int32_t>(n, std::max<int32_t>(2 * cap, 1024));
+    void* nc[P_NCOL] = {};
+    for (int k = 0; k < ncol; k++) {
+      cudaError_t e = cudaMalloc(&nc[k], (size_t)ncap * sz[k]);
+      if (e == cudaSuccess) e = cudaMemsetAsync(nc[k], 0, (size_t)ncap * sz[k], st);
+      if (e == cudaSuccess && col[k]) e = cudaMemcpyAsync(nc[k], col[k], (size_t)cap * sz[k], cudaMemcpyDeviceToDevice, st);
+      if (e != cudaSuccess) {
+        for (int j = 0; j <= k; j++) if (nc[j]) cudaFree(nc[j]);
+        return e;
+      }
+    }
+    if (!d_col) {
+      cudaError_t e = cudaMalloc(&d_col, sizeof(void*) * P_NCOL);
+      if (e != cudaSuccess) return e;
+    }
+    cudaError_t e = cudaMemcpyAsync(d_col, nc, sizeof(void*) * P_NCOL, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return e;
+    for (int k = 0; k < ncol; k++) {
+      if (col[k]) cudaFree(col[k]);
+      col[k] = nc[k];
+    }
+    cap = ncap;
+    return cudaSuccess;
+  }
+  int32_t take_slot() {
+    if (!free.empty()) { const int32_t s = free.back(); free.pop_back(); return s; }
+    return hw++;
+  }
+  void release() {
+    for (int k = 0; k < ncol; k++) if (col[k]) cudaFree(col[k]);
+    if (d_col) cudaFree(d_col);
+  }
+};
+
+struct ListArena {
+  int k = 1;                      // value arrays: 2 for (attribute column, value)
+  int32_t* v[2] = {};
+  int32_t* alt[2] = {};           // compaction target, same capacity
+  int64_t cap = 0, tail = 0, live = 0;
+  cudaError_t grow(int64_t n, cudaStream_t st) {
+    if (n <= cap) return cudaSuccess;
+    const int64_t ncap = std::max<int64_t>(n, std::max<int64_t>(2 * cap, 4096));
+    for (int i = 0; i < k; i++) {
+      int32_t* p = nullptr;
+      cudaError_t e = cudaMalloc(&p, sizeof(int32_t) * ncap);
+      if (e == cudaSuccess && tail) e = cudaMemcpyAsync(p, v[i], sizeof(int32_t) * tail, cudaMemcpyDeviceToDevice, st);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+      if (e != cudaSuccess) { if (p) cudaFree(p); return e; }
+      if (v[i]) cudaFree(v[i]);
+      v[i] = p;
+      if (alt[i]) cudaFree(alt[i]);
+      alt[i] = nullptr;
+    }
+    cap = ncap;
+    return cudaSuccess;
+  }
+  void release() {
+    for (int i = 0; i < 2; i++) { if (v[i]) cudaFree(v[i]); if (alt[i]) cudaFree(alt[i]); }
+  }
+};
+
+void count_add(std::map<int32_t, int64_t>& m, int32_t code, int64_t d) {
+  auto it = m.emplace(code, 0).first;
+  if ((it->second += d) == 0) m.erase(it);
+}
+int32_t count_max(const std::map<int32_t, int64_t>& m) { return m.empty() ? -1 : m.rbegin()->first; }
+
+struct PoolState {
+  Table pend, run;
+  std::vector<PendingInfo> pinfo;    // by pending slot
+  std::vector<int32_t> ruser;        // by running slot
+  ListArena lists[3];
+  std::map<int32_t, int64_t> users_p, users_r, attr_cols, groups;   // code -> live uses
+  int64_t nflag[F_N] = {};
+  Arena stage;                        // one batch's uploads
+  // scratch
+  int32_t* blk = nullptr; size_t blk_cap = 0;
+  int32_t* counters = nullptr;        // [0] running rows, [1] pending rows, [2] live queue entries
+  GridFlag* gf0 = nullptr;            // stays zero: integer scans are always exact
+  int32_t* scan_part = nullptr; size_t scan_part_cap = 0;
+  int32_t* scan_tile = nullptr; size_t scan_tile_cap = 0;
+  // rank: dense columns, and the resident queue
+  DenseTasks dense = {};
+  size_t dense_cap = 0;
+  int32_t* q_slot = nullptr; uint32_t* q_gen = nullptr; int64_t* q_jid = nullptr; size_t q_cap = 0;
+  int32_t n_q = 0;
+  bool ranked = false;
+  int32_t* m_slot = nullptr; size_t m_cap = 0;
+
+  PoolState() {
+    pend.ncol = P_NCOL; pend.sz = P_SZ;
+    run.ncol = R_NCOL; run.sz = R_SZ;
+    lists[L_ATTR].k = 2;
+  }
+  void release() {
+    pend.release(); run.release();
+    for (auto& l : lists) l.release();
+    stage.release();
+    for (void* p : {(void*)blk, (void*)counters, (void*)gf0, (void*)scan_part, (void*)scan_tile, (void*)dense.user,
+                    (void*)dense.prio, (void*)dense.start, (void*)dense.tid, (void*)dense.jid, (void*)dense.cpus,
+                    (void*)dense.mem, (void*)dense.gpus, (void*)dense.pslot, (void*)q_slot, (void*)q_gen, (void*)q_jid,
+                    (void*)m_slot})
+      if (p) cudaFree(p);
+  }
+  void add_pending(int32_t slot, const PendingInfo& pi, int64_t sign) {
+    count_add(users_p, pi.user, sign);
+    for (int32_t g : pi.groups) count_add(groups, g, sign);
+    for (int32_t c : pi.attr_cols) count_add(attr_cols, c, sign);
+    for (int l = 0; l < 3; l++) lists[l].live += sign * pi.len[l];
+    for (int f = 0; f < F_N; f++) if ((pi.flags >> f) & 1) nflag[f] += sign;
+    (void)slot;
+  }
+};
+
+void state_free(void* p) {
+  PoolState* s = static_cast<PoolState*>(p);
+  if (s) { s->release(); delete s; }
+}
+
+PoolState* state_of(cook_pool* pool, bool create) {
+  if (!pool->state && create) {
+    PoolState* s = new PoolState();
+    if (cudaMalloc(&s->counters, sizeof(int32_t) * 8) != cudaSuccess ||
+        cudaMalloc(&s->gf0, sizeof(GridFlag)) != cudaSuccess || cudaMemset(s->gf0, 0, sizeof(GridFlag)) != cudaSuccess) {
+      state_free(s);
+      return nullptr;
+    }
+    pool->state = s;
+    pool->state_free = state_free;
+  }
+  return static_cast<PoolState*>(pool->state);
+}
+
+bool csr_ok(const int32_t* off, int n, const int32_t* v0, const int32_t* v1, bool two) {
+  if (!off) return true;
+  if (off[0] != 0) return false;
+  for (int i = 0; i < n; i++) if (off[i + 1] < off[i]) return false;
+  return off[n] == 0 || (v0 && (!two || v1));
+}
+
+long long bits_of(double x) { long long b; memcpy(&b, &x, 8); return b; }
+
+// compaction of every list arena whose dead entries outnumber its live ones
+int32_t compact_lists(cook_pool* pool, PoolState* S, cudaStream_t st, int* nl) {
+  const int n = S->pend.hw;
+  const int loff[3] = {P_NOFF, P_AOFF, P_GOFF}, llen[3] = {P_NLEN, P_ALEN, P_GLEN};
+  for (int l = 0; l < 3; l++) {
+    ListArena& A = S->lists[l];
+    if (A.tail - A.live <= A.live) continue;
+    if (A.live > 0 && n > 0) {
+      for (int i = 0; i < A.k; i++)
+        if (!A.alt[i]) CK(pool, cudaMalloc(&A.alt[i], sizeof(int32_t) * std::max<int64_t>(A.cap, 1)));
+      const int nb = (n + OS_TILE - 1) / OS_TILE;
+      CK(pool, ensure(S->scan_part, S->scan_part_cap, (size_t)n));
+      CK(pool, ensure(S->scan_tile, S->scan_tile_cap, (size_t)nb + 1));
+      const OrderScan<int, 1> os{{S->scan_part}, {S->scan_tile}};
+      const uint8_t* live = static_cast<const uint8_t*>(S->pend.col[P_LIVE]);
+      int32_t* off = static_cast<int32_t*>(S->pend.col[loff[l]]);
+      const int32_t* len = static_cast<const int32_t*>(S->pend.col[llen[l]]);
+      order_scan(os, SlotLen{live, len}, n, S->gf0, st, nl);
+      list_compact_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, live, off, len, n, A.v[0], A.v[1], A.alt[0],
+                                                       A.k > 1 ? A.alt[1] : nullptr);
+      (*nl)++;
+      CK(pool, cudaGetLastError());
+      for (int i = 0; i < A.k; i++) std::swap(A.v[i], A.alt[i]);
+    }
+    A.tail = A.live;
+  }
+  return COOK_OK;
+}
+
+int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
+  const cook_jobs_soa& P = d->pending;
+  const cook_tasks_soa& T = d->running;
+  const int np = P.n, nr = T.n, npr = d->n_pending_rm, nrr = d->n_running_rm;
+  if (np < 0 || nr < 0 || npr < 0 || nrr < 0) return set_err(pool, COOK_E_BADARG, "cook_state_apply: bad sizes");
+  if (np && (!P.user || !P.cpus || !P.mem || !d->pending_priority || !d->pending_job_id))
+    return set_err(pool, COOK_E_BADARG, "cook_state_apply: pending upserts need user, cpus, mem, priority and job id");
+  if (nr && (!T.user || !T.priority || !T.start_time || !T.task_id || !T.job_id || !T.cpus || !T.mem))
+    return set_err(pool, COOK_E_BADARG, "cook_state_apply: running upserts need every column but gpus");
+  if ((npr && !d->pending_rm_job_id) || (nrr && !d->running_rm_task_id))
+    return set_err(pool, COOK_E_BADARG, "cook_state_apply: null removal ids");
+  if (!csr_ok(P.novel_off, np, P.novel_host, nullptr, false) || !csr_ok(P.attr_off, np, P.attr_col, P.attr_val, true) ||
+      !csr_ok(P.group_off, np, P.group_idx, nullptr, false))
+    return set_err(pool, COOK_E_BADARG, "cook_state_apply: malformed CSR offsets");
+  // codes are checked where they enter
+  if (!idx_in_range(P.user, np, 0, INT32_MAX) || !idx_in_range(T.user, nr, 0, INT32_MAX))
+    return set_err(pool, COOK_E_BADARG, "cook_state_apply: negative user code");
+  if ((P.attr_off && !idx_in_range(P.attr_col, P.attr_off[np], 0, INT32_MAX)) ||
+      (P.group_off && !idx_in_range(P.group_idx, P.group_off[np], 0, INT32_MAX)) ||
+      (P.novel_off && !idx_in_range(P.novel_host, P.novel_off[np], 0, INT32_MAX)) ||
+      !idx_in_range(P.reserved_host, np, -1, INT32_MAX))
+    return set_err(pool, COOK_E_BADARG, "cook_state_apply: bad attribute column, group or hostname code");
+  const bool rs = d->reset != 0;
+  {
+    std::unordered_set<int64_t> seen;
+    seen.reserve((size_t)np + npr);
+    for (int i = 0; i < np; i++)
+      if (!seen.insert(d->pending_job_id[i]).second) return set_err(pool, COOK_E_BADARG, "cook_state_apply: job id twice in one batch");
+    for (int i = 0; i < npr; i++) {
+      const int64_t id = d->pending_rm_job_id[i];
+      if (!seen.insert(id).second) return set_err(pool, COOK_E_BADARG, "cook_state_apply: job id twice in one batch");
+      if (rs || !S->pend.slot_of.count(id)) return set_err(pool, COOK_E_BADARG, "cook_state_apply: removal of an unknown job id");
+    }
+    seen.clear();
+    for (int i = 0; i < nr; i++)
+      if (!seen.insert(T.task_id[i]).second) return set_err(pool, COOK_E_BADARG, "cook_state_apply: task id twice in one batch");
+    for (int i = 0; i < nrr; i++) {
+      const int64_t id = d->running_rm_task_id[i];
+      if (!seen.insert(id).second) return set_err(pool, COOK_E_BADARG, "cook_state_apply: task id twice in one batch");
+      if (rs || !S->run.slot_of.count(id)) return set_err(pool, COOK_E_BADARG, "cook_state_apply: removal of an unknown task id");
+    }
+  }
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  // ---- the batch is valid: the host side first (slots, counts), all O(delta)
+  if (rs) {
+    for (Table* t : {&S->pend, &S->run}) {
+      if (t->hw) {
+        const int lc = t == &S->pend ? (int)P_LIVE : (int)R_LIVE;
+        CK(pool, cudaMemsetAsync(t->col[lc], 0, (size_t)t->hw, st));
+      }
+      t->slot_of.clear(); t->free.clear(); t->hw = 0;
+    }
+    S->users_p.clear(); S->users_r.clear(); S->attr_cols.clear(); S->groups.clear();
+    for (auto& f : S->nflag) f = 0;
+    for (auto& l : S->lists) l.tail = l.live = 0;
+  }
+  std::vector<int32_t> prm_slot(npr), pup_slot(np), rrm_slot(nrr), rup_slot(nr);
+  for (int i = 0; i < npr; i++) {
+    auto it = S->pend.slot_of.find(d->pending_rm_job_id[i]);
+    const int32_t s = it->second;
+    S->pend.slot_of.erase(it);
+    S->add_pending(s, S->pinfo[s], -1);
+    S->pend.free.push_back(s);
+    prm_slot[i] = s;
+  }
+  for (int i = 0; i < nrr; i++) {
+    auto it = S->run.slot_of.find(d->running_rm_task_id[i]);
+    const int32_t s = it->second;
+    S->run.slot_of.erase(it);
+    count_add(S->users_r, S->ruser[s], -1);
+    S->run.free.push_back(s);
+    rrm_slot[i] = s;
+  }
+  for (int i = 0; i < np; i++) {
+    auto it = S->pend.slot_of.find(d->pending_job_id[i]);
+    int32_t s;
+    if (it != S->pend.slot_of.end()) { s = it->second; S->add_pending(s, S->pinfo[s], -1); }
+    else { s = S->pend.take_slot(); S->pend.slot_of.emplace(d->pending_job_id[i], s); }
+    if ((size_t)s >= S->pinfo.size()) S->pinfo.resize(std::max<size_t>(s + 1, 2 * S->pinfo.size()));
+    PendingInfo& pi = S->pinfo[s];
+    pi.user = P.user[i];
+    pi.len[L_NOVEL] = P.novel_off ? P.novel_off[i + 1] - P.novel_off[i] : 0;
+    pi.len[L_ATTR] = P.attr_off ? P.attr_off[i + 1] - P.attr_off[i] : 0;
+    pi.len[L_GROUP] = P.group_off ? P.group_off[i + 1] - P.group_off[i] : 0;
+    pi.attr_cols.assign(P.attr_off ? P.attr_col + P.attr_off[i] : nullptr, P.attr_off ? P.attr_col + P.attr_off[i + 1] : nullptr);
+    pi.groups.assign(P.group_off ? P.group_idx + P.group_off[i] : nullptr, P.group_off ? P.group_idx + P.group_off[i + 1] : nullptr);
+    const bool f[F_N] = {P.gpus && P.gpus[i] != 0.0, P.ports && P.ports[i] != 0, P.allowed && !P.allowed[i],
+                         P.plugin_accept && !P.plugin_accept[i], P.gpu_model && P.gpu_model[i] != -1,
+                         P.disk_request && P.disk_request[i] >= 0.0, P.est_end_ms && P.est_end_ms[i] != -1,
+                         P.ckpt_location && P.ckpt_location[i] != -1, P.reserved_host && P.reserved_host[i] != -1};
+    pi.flags = 0;
+    for (int k = 0; k < F_N; k++) if (f[k]) pi.flags |= (uint16_t)(1u << k);
+    S->add_pending(s, pi, +1);
+    pup_slot[i] = s;
+  }
+  for (int i = 0; i < nr; i++) {
+    auto it = S->run.slot_of.find(T.task_id[i]);
+    int32_t s;
+    if (it != S->run.slot_of.end()) { s = it->second; count_add(S->users_r, S->ruser[s], -1); }
+    else { s = S->run.take_slot(); S->run.slot_of.emplace(T.task_id[i], s); }
+    if ((size_t)s >= S->ruser.size()) S->ruser.resize(std::max<size_t>(s + 1, 2 * S->ruser.size()));
+    S->ruser[s] = T.user[i];
+    count_add(S->users_r, T.user[i], +1);
+    rup_slot[i] = s;
+  }
+  // ---- device: capacity, the upload, then the scatters (removals before upserts: a slot a removal
+  // frees may be taken by an upsert of the same batch)
+  CK(pool, S->pend.grow(S->pend.hw, st));
+  CK(pool, S->run.grow(S->run.hw, st));
+  const int32_t* lists_off[3] = {P.novel_off, P.attr_off, P.group_off};
+  const int32_t* lists_v[3][2] = {{P.novel_host, nullptr}, {P.attr_col, P.attr_val}, {P.group_idx, nullptr}};
+  int32_t tail0[3];
+  for (int l = 0; l < 3; l++) {
+    tail0[l] = (int32_t)S->lists[l].tail;
+    const int64_t add = lists_off[l] ? lists_off[l][np] : 0;
+    CK(pool, S->lists[l].grow(S->lists[l].tail + add, st));
+    S->lists[l].tail += add;
+  }
+  ScatterArgs pu, pr, ru, rr;
+  memset(&pu, 0, sizeof(pu)); memset(&pr, 0, sizeof(pr)); memset(&ru, 0, sizeof(ru)); memset(&rr, 0, sizeof(rr));
+  int64_t h2d = 0;
+  const cudaError_t carved = carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
+    if (np) {
+      const void* src[P_NDATA] = {P.user, d->pending_priority, d->pending_job_id, P.cpus, P.mem, P.gpus, P.ports,
+                                  P.allowed, P.plugin_accept, P.gpu_model, P.disk_request, P.disk_type, P.est_end_ms,
+                                  P.ckpt_location, P.reserved_host};
+      const long long dflt[P_NDATA] = {0, 0, 0, 0, 0, 0, 0, 1, 1, -1, bits_of(-1.0), -1, -1, -1, -1};
+      for (int k = 0; k < P_NDATA; k++) {
+        const char* up = nullptr;
+        if (P_SZ[k] == 1) up = reinterpret_cast<const char*>(c.up(static_cast<const uint8_t*>(src[k]), np));
+        else if (P_SZ[k] == 4) up = reinterpret_cast<const char*>(c.up(static_cast<const int32_t*>(src[k]), np));
+        else up = reinterpret_cast<const char*>(c.up(static_cast<const int64_t*>(src[k]), np));
+        pu.c[k] = ScatterCol{static_cast<char*>(S->pend.col[k]), up, dflt[k], P_SZ[k]};
+      }
+      pu.nc = P_NDATA;
+      pu.slot = c.up(pup_slot.data(), np);
+      for (int l = 0; l < 3; l++) {
+        pu.doff[l] = c.up(lists_off[l], np + 1);
+        const int64_t nv = lists_off[l] ? lists_off[l][np] : 0;
+        for (int i = 0; i < S->lists[l].k; i++)
+          if (c.base && nv) c.copy(S->lists[l].v[i] + tail0[l], lists_v[l][i], nv);
+      }
+    }
+    if (npr) pr.slot = c.up(prm_slot.data(), npr);
+    if (nr) {
+      const void* src[R_NDATA] = {T.user, T.priority, T.start_time, T.task_id, T.job_id, T.cpus, T.mem, T.gpus};
+      for (int k = 0; k < R_NDATA; k++) {
+        const char* up = R_SZ[k] == 4 ? reinterpret_cast<const char*>(c.up(static_cast<const int32_t*>(src[k]), nr))
+                                      : reinterpret_cast<const char*>(c.up(static_cast<const int64_t*>(src[k]), nr));
+        ru.c[k] = ScatterCol{static_cast<char*>(S->run.col[k]), up, 0, R_SZ[k]};
+      }
+      ru.nc = R_NDATA;
+      ru.slot = c.up(rup_slot.data(), nr);
+    }
+    if (nrr) rr.slot = c.up(rrm_slot.data(), nrr);
+  });
+  CK(pool, carved);
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  int nl = 0;
+  auto launch = [&](ScatterArgs& a, Table& t, int n, int upsert, int live_col, bool lists) {
+    if (!n) return;
+    a.n = n; a.upsert = upsert;
+    a.live = static_cast<uint8_t*>(t.col[live_col]);
+    a.gen = static_cast<uint32_t*>(t.col[live_col + 1]);
+    if (lists) {
+      const int loff[3] = {P_NOFF, P_AOFF, P_GOFF};
+      for (int l = 0; l < 3; l++) {
+        a.loff[l] = static_cast<int32_t*>(t.col[loff[l]]);
+        a.llen[l] = static_cast<int32_t*>(t.col[loff[l] + 1]);
+        a.tail[l] = tail0[l];
+      }
+    }
+    scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(a);
+    nl++;
+  };
+  launch(pr, S->pend, npr, 0, P_LIVE, true);
+  launch(rr, S->run, nrr, 0, R_LIVE, false);
+  launch(pu, S->pend, np, 1, P_LIVE, true);
+  launch(ru, S->run, nr, 1, R_LIVE, false);
+  CK(pool, cudaGetLastError());
+  int32_t rc = compact_lists(pool, S, st, &nl);
+  if (rc != COOK_OK) return rc;
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  CK(pool, cudaStreamSynchronize(st));
+  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
+  return COOK_OK;
+}
+
+}  // namespace
+
+extern "C" int32_t cook_state_apply(cook_pool* pool, const cook_state_delta* delta) {
+  if (!pool) return COOK_E_BADARG;
+  if (!delta) return set_err(pool, COOK_E_BADARG, "cook_state_apply: null argument");
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_apply: out of device memory");
+  return apply(pool, S, delta);
+}
+
+extern "C" int32_t cook_state_rank(cook_pool* pool, const cook_user_table* users, const cook_pool_quota* pool_quota,
+                                   const cook_pool_quota* group_quota, const double* group_usage,
+                                   const cook_rank_params* params, int64_t* out_ranked_job_id, int32_t* out_n) {
+  if (!pool) return COOK_E_BADARG;
+  if (!users || !params || !out_n) return set_err(pool, COOK_E_BADARG, "cook_state_rank: null argument");
+  *out_n = 0;
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_rank: out of device memory");
+  const int U = users->n_users;
+  if (U <= 0) return set_err(pool, COOK_E_BADARG, "cook_state_rank: bad sizes");
+  if (std::max(count_max(S->users_p), count_max(S->users_r)) >= U)
+    return set_err(pool, COOK_E_BADARG, "cook_state_rank: a resident row's user code is >= n_users");
+  cudaStream_t st = pool->stream;
+  const int R = (int)S->run.slot_of.size(), J = (int)S->pend.slot_of.size();
+  const size_t N = (size_t)R + J;
+  S->ranked = false;
+  CK(pool, cudaEventRecord(pool->ev[7], st));
+  int nl = 0;
+  if (N > 0) {
+    if (N > S->dense_cap) {
+      size_t c = 0;
+      DenseTasks& o = S->dense;
+      for (void** p : {(void**)&o.user, (void**)&o.prio, (void**)&o.start, (void**)&o.tid, (void**)&o.jid, (void**)&o.cpus,
+                       (void**)&o.mem, (void**)&o.gpus, (void**)&o.pslot}) {
+        if (*p) cudaFree(*p);
+        *p = nullptr;
+      }
+      c = std::max(N, 2 * S->dense_cap);
+      CK(pool, cudaMalloc(&o.user, c * 4)); CK(pool, cudaMalloc(&o.prio, c * 4));
+      CK(pool, cudaMalloc(&o.start, c * 8)); CK(pool, cudaMalloc(&o.tid, c * 8)); CK(pool, cudaMalloc(&o.jid, c * 8));
+      CK(pool, cudaMalloc(&o.cpus, c * 8)); CK(pool, cudaMalloc(&o.mem, c * 8)); CK(pool, cudaMalloc(&o.gpus, c * 8));
+      CK(pool, cudaMalloc(&o.pslot, c * 4));
+      S->dense_cap = c;
+    }
+    CK(pool, ensure(S->blk, S->blk_cap, (size_t)std::max(S->pend.hw, S->run.hw) / CP_BLOCK + 2));
+    if (R) compact(RunningRows{S->run.d_col, S->dense}, S->run.hw, nullptr, S->blk, S->counters, R, st, &nl);
+    if (J) compact(PendingRows{S->pend.d_col, S->dense, R}, S->pend.hw, nullptr, S->blk, S->counters + 1, J, st, &nl);
+    CK(pool, cudaGetLastError());
+    CK(pool, cudaEventRecord(pool->ev[23], st));
+    if ((size_t)J + 1 > S->q_cap) {
+      if (S->q_slot) cudaFree(S->q_slot);
+      if (S->q_gen) cudaFree(S->q_gen);
+      if (S->q_jid) cudaFree(S->q_jid);
+      S->q_slot = nullptr; S->q_gen = nullptr; S->q_jid = nullptr; S->q_cap = 0;
+      const size_t c = std::max<size_t>(J + 1, 2 * S->q_cap);
+      CK(pool, cudaMalloc(&S->q_slot, c * 4)); CK(pool, cudaMalloc(&S->q_gen, c * 4)); CK(pool, cudaMalloc(&S->q_jid, c * 8));
+      S->q_cap = c;
+    }
+  }
+  const DenseTasks& o = S->dense;
+  const DevTasks dt{R, J, o.user, o.prio, o.start, o.tid, o.jid, o.cpus, o.mem, o.gpus};
+  const uint32_t* gen = static_cast<const uint32_t*>(S->pend.col[P_GEN]);
+  const int64_t* jid = static_cast<const int64_t*>(S->pend.col[P_JID]);
+  const std::function<int32_t(const int32_t*, const int32_t*, int*)> on_queue =
+      [&](const int32_t* d_ranked, const int32_t* d_n, int* launches) -> int32_t {
+    if (J == 0) return COOK_OK;   // running tasks only: the queue is empty
+    queue_kernel<<<(J + 255) / 256, 256, 0, st>>>(d_ranked, d_n, o.pslot, gen, jid, S->q_slot, S->q_gen, S->q_jid);
+    (*launches)++;
+    CK(pool, cudaGetLastError());
+    return COOK_OK;
+  };
+  int32_t n = 0;
+  const int32_t rc = rank_impl(pool, nullptr, nullptr, &dt, users, pool_quota, group_quota, group_usage, params, nullptr,
+                               &n, nullptr, nullptr, nullptr, &on_queue);
+  if (rc != COOK_OK) return rc;
+  cook_phase_stats& ps = pool->phase[COOK_PHASE_RANK];
+  if (N > 0) ps.ms_device += ev_ms(pool->ev[7], pool->ev[23]);   // the gathering of the live rows
+  ps.n_launches += nl;
+  if (out_ranked_job_id && n > 0) {
+    int64_t d2h = 0;
+    CK(pool, download(out_ranked_job_id, S->q_jid, n, st, &d2h));
+    CK(pool, cudaStreamSynchronize(st));
+    ps.d2h_bytes += d2h;
+  }
+  S->n_q = n;
+  S->ranked = true;
+  *out_n = n;
+  return COOK_OK;
+}
+
+extern "C" int32_t cook_state_match(cook_pool* pool, const cook_offers_soa* offers, const cook_groups* groups,
+                                    const cook_user_table* users, const cook_pool_quota* pool_quota,
+                                    const cook_match_params* params, int64_t* out_considerable_job_id,
+                                    int32_t* out_assign, int32_t* out_ports, int32_t max_ports,
+                                    uint8_t* out_fail_reason, cook_match_stats* out_stats) {
+  if (!pool) return COOK_E_BADARG;
+  if (!offers || !users || !params || !out_considerable_job_id || !out_assign)
+    return set_err(pool, COOK_E_BADARG, "cook_state_match: null argument");
+  if (params->reuse_resident)
+    return set_err(pool, COOK_E_BADARG, "cook_state_match: reuse_resident does not apply: the queue's rows are resident");
+  if (params->good_enough_fitness < 1.0)
+    return set_err(pool, COOK_E_BADARG, "cook_state_match: good_enough_fitness < 1.0 is not supported (see cook_match)");
+  if (params->fitness_kind != 0) return set_err(pool, COOK_E_UNSUPPORTED_CONSTRAINT, "cook_state_match: only cpuMemBinPacker");
+  const int O = offers->n, U = users->n_users, NC = params->num_considerable;
+  if (O < 0 || U <= 0 || NC < 0 || max_ports < 0) return set_err(pool, COOK_E_BADARG, "cook_state_match: bad sizes");
+  PoolState* S = static_cast<PoolState*>(pool->state);
+  if (!S || !S->ranked) return set_err(pool, COOK_E_BADARG, "cook_state_match: no cook_state_rank on this handle yet");
+  if (count_max(S->users_p) >= U) return set_err(pool, COOK_E_BADARG, "cook_state_match: a pending row's user code is >= n_users");
+  if (count_max(S->attr_cols) >= std::max(1, offers->n_attr_cols))
+    return set_err(pool, COOK_E_BADARG, "cook_state_match: a pending row's attribute column is >= n_attr_cols");
+  const int G = groups ? groups->n_groups : 0;
+  if (G > 0 && count_max(S->groups) >= G)
+    return set_err(pool, COOK_E_BADARG, "cook_state_match: a pending row's group code is >= n_groups");
+  if (out_stats) memset(out_stats, 0, sizeof(*out_stats));
+  if (S->n_q == 0 || NC == 0) return COOK_OK;
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  // ---- the queue minus what left it since the rank
+  int nl = 0;
+  CK(pool, ensure(S->m_slot, S->m_cap, (size_t)S->n_q));
+  CK(pool, ensure(S->blk, S->blk_cap, (size_t)S->n_q / CP_BLOCK + 2));
+  const QueueLive ql{S->q_slot, S->q_gen, static_cast<const uint8_t*>(S->pend.col[P_LIVE]),
+                     static_cast<const uint32_t*>(S->pend.col[P_GEN]), S->m_slot};
+  compact(ql, S->n_q, nullptr, S->blk, S->counters + 2, S->n_q, st, &nl);
+  CK(pool, cudaGetLastError());
+  int32_t n = 0;
+  int64_t d2h = 0;
+  CK(pool, download(&n, S->counters + 2, 1, st, &d2h));
+  CK(pool, cudaStreamSynchronize(st));
+  if (n == 0) return COOK_OK;
+  // ---- what the rows hold, from the host-side counts
+  std::vector<int32_t> gp_off(G + 1, 0);
+  for (const auto& kv : S->groups) if (kv.first < G) gp_off[kv.first + 1] = (int32_t)kv.second;
+  for (int g = 0; g < G; g++) gp_off[g + 1] += gp_off[g];
+  DevJobSpec dj;
+  memset(&dj, 0, sizeof(dj));
+  dj.ports = S->nflag[F_PORTS] > 0; dj.allowed = S->nflag[F_NOT_ALLOWED] > 0; dj.plugin = S->nflag[F_NOT_PLUGIN] > 0;
+  dj.gpu_model = S->nflag[F_GPU_MODEL] > 0; dj.disk = S->nflag[F_DISK] > 0; dj.est_end = S->nflag[F_EST] > 0;
+  dj.ckpt = S->nflag[F_CKPT] > 0; dj.reserved = S->nflag[F_RESERVED] > 0; dj.any_gpus = S->nflag[F_GPUS] > 0;
+  dj.n_novel = S->lists[L_NOVEL].live; dj.n_attr = S->lists[L_ATTR].live; dj.n_group = S->lists[L_GROUP].live;
+  dj.gp_off = gp_off.data();
+  const auto fill = [&](const DevJobCols& o, int* launches) -> int32_t {
+    fill_rows_kernel<<<(n + 255) / 256, 256, 0, st>>>(o, S->pend.d_col, S->m_slot, n);
+    (*launches)++;
+    const int nb = (n + OS_TILE - 1) / OS_TILE;
+    CK(pool, ensure(S->scan_part, S->scan_part_cap, (size_t)n));
+    CK(pool, ensure(S->scan_tile, S->scan_tile_cap, (size_t)nb + 1));
+    const OrderScan<int, 1> os{{S->scan_part}, {S->scan_tile}};
+    const int loff[3] = {P_NOFF, P_AOFF, P_GOFF};
+    int32_t* doff[3] = {o.novel_off, o.attr_off, o.group_off};
+    int32_t* dst[3][2] = {{o.novel_host, nullptr}, {o.attr_col, o.attr_val}, {o.group_idx, nullptr}};
+    for (int l = 0; l < 3; l++) {
+      if (!doff[l]) continue;
+      const int32_t* off = static_cast<const int32_t*>(S->pend.col[loff[l]]);
+      const int32_t* len = static_cast<const int32_t*>(S->pend.col[loff[l] + 1]);
+      order_scan(os, RowLen{S->m_slot, len}, n, S->gf0, st, launches);
+      csr_gather_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, S->m_slot, n, off, len, S->lists[l].v[0], S->lists[l].v[1],
+                                                     doff[l], dst[l][0], dst[l][1]);
+      (*launches)++;
+    }
+    CK(pool, cudaGetLastError());
+    return COOK_OK;
+  };
+  const int32_t rc = match_device_jobs(pool, n, &dj, fill, offers, groups, users, pool_quota, params, out_considerable_job_id,
+                                       out_assign, out_ports, max_ports, out_fail_reason, out_stats);
+  if (rc != COOK_OK) return rc;
+  cook_phase_stats& ps = pool->phase[COOK_PHASE_MATCH];
+  ps.n_launches += nl;
+  ps.d2h_bytes += d2h;
+  if (out_stats) { out_stats->n_launches += nl; out_stats->d2h_bytes += d2h; }
+  return COOK_OK;
+}

@@ -61,7 +61,7 @@ def load_library(path=None):
                  "cook_last_error", "cook_rank", "cook_match", "cook_rebalance",
                  "cook_allgather_usage", "cook_last_stats", "cook_comm_unique_id", "cook_comm_init",
                  "cook_comm_destroy", "cook_exchange_usage", "cook_exchange_usage_batch", "cook_rebalance_trace",
-                 "cook_match_failures"):
+                 "cook_match_failures", "cook_state_apply", "cook_state_rank", "cook_state_match"):
         getattr(lib, name).restype = C.c_int32
     return lib
 
@@ -149,6 +149,56 @@ class GpuEngine:
         if rc != 0:
             self._err(rc)
         return [{"n_vms": o.n_vms, "n_passed": o.n_passed, "n_ports": o.n_ports, "counts": list(o.counts)} for o in out[:len(k)]]
+
+    # -- resident pool state (§8f-1) ----------------------------------------
+    def state_apply(self, delta):
+        """cook_state_apply: one batch of changes (abi.make_delta), all or nothing."""
+        rc = self.lib.cook_state_apply(self.pool, C.byref(delta))
+        if rc != 0:
+            self._err(rc)
+        # the live pending ids, O(delta): they size state_rank's output
+        live = getattr(self, "_state_pending_ids", set())
+        if delta.reset:
+            live = set()
+        rm = delta.col("pending_rm_job_id")
+        live.difference_update(rm.tolist() if rm is not None else [])
+        up = delta.col("pending_job_id")
+        live.update(up.tolist() if up is not None else [])
+        self._state_pending_ids = live
+
+    def state_rank(self, users, pool_quota=None, group_quota=None, group_usage=None, params=None):
+        """cook_state_rank: the live rows ranked; the queue stays on the device.  Returns its job ids."""
+        pool_quota = pool_quota or abi.make_pool_quota(None)
+        group_quota = group_quota or abi.make_pool_quota(None)
+        params = params or abi.RankParams(100, 0, 0.0, 0.0)
+        gu = np.ascontiguousarray(group_usage if group_usage is not None else np.zeros(4), np.float64)
+        out = np.zeros(max(len(getattr(self, "_state_pending_ids", ())), 1), np.int64)
+        n = C.c_int32(0)
+        rc = self.lib.cook_state_rank(self.pool, C.byref(users), C.byref(pool_quota), C.byref(group_quota),
+                                      abi.ptr(gu, abi.P_F64), C.byref(params), abi.ptr(out, abi.P_I64), C.byref(n))
+        if rc != 0:
+            self._err(rc)
+        return out[:n.value].copy()
+
+    def state_match(self, offers, users, params, groups=None, pool_quota=None, max_ports=0):
+        """cook_state_match: the resident queue (minus what left it since the rank) matched against
+        `offers`.  'considerable' holds job ids."""
+        pool_quota = pool_quota or abi.make_pool_quota(None)
+        k = max(params.num_considerable, 1)
+        cons = np.full(k, -1, np.int64)
+        _, assign, ports, fail, stats = _CallShapes.match_buffers(params, max_ports)
+        rc = self.lib.cook_state_match(self.pool, C.byref(offers),
+                                       C.byref(groups) if groups is not None else None,
+                                       C.byref(users), C.byref(pool_quota), C.byref(params),
+                                       abi.ptr(cons, abi.P_I64), abi.ptr(assign, abi.P_I32),
+                                       abi.ptr(ports, abi.P_I32) if max_ports > 0 else None,
+                                       int(max_ports), abi.ptr(fail, abi.P_U8), C.byref(stats))
+        if rc != 0:
+            self._err(rc)
+        n = stats.n_considerable
+        return {"considerable": cons[:n].copy(), "assign": assign[:n].copy(),
+                "ports": ports[:n * max(max_ports, 1)].reshape(n, max(max_ports, 1)).copy(),
+                "fail": fail[:n].copy(), "stats": stats.as_dict()}
 
     # -- B1-B6 -------------------------------------------------------------
     def rebalance(self, running, pending, pending_job_id, pending_priority, hosts, users, params,

@@ -412,10 +412,77 @@ int32_t cook_rebalance_trace(cook_pool* pool, const cook_running_soa* running,
                              const cook_rebalance_params* params, cook_decision* out_decisions,
                              int32_t* out_victims, int32_t* out_n, const cook_reb_trace* trace);
 
+/* ------------------------------------------------------ resident pool state */
+/* §8f-1, device half: the pool's pending jobs and running tasks stay on the device between cycles and
+ * change by deltas, as Cook's own state changes by transactions (monitor-tx-report-queue,
+ * scheduler.clj:378-448).  rank-jobs (:2262-2284) ranks them in place and the match cycles between two
+ * ranks take from that queue, which loses only what the caller's launch deltas remove
+ * (remove-matched-jobs-from-pending-jobs :790-795).  Nothing that scales with the pool is uploaded or
+ * scanned on the host per cycle.
+ *
+ * One batch of changes, applied all or nothing:
+ *   reset               drop every row first (new leadership)
+ *   pending             upserts keyed by pending_job_id: the columns of cook_jobs_soa, CSR lists over
+ *                       the delta rows, plus pending_priority.  A pending row ranks with start_time =
+ *                       INT64_MAX and task_id = -1.  Required: user, cpus, mem, pending_priority,
+ *                       pending_job_id; a NULL column takes its "absent" value (gpus 0, ports 0, allowed
+ *                       and plugin_accept 1, gpu_model / disk_type / ckpt_location / reserved_host -1,
+ *                       disk_request -1, est_end_ms -1, empty lists).  An upsert of a known id replaces
+ *                       the row.
+ *   pending_rm_job_id   removals
+ *   running             running-task upserts keyed by task_id (all cook_tasks_soa columns but gpus)
+ *   running_rm_task_id  removals
+ * A launch is one batch: remove pending job j, upsert its running task.
+ * COOK_E_BADARG, state unchanged: an unknown id in a removal, an id twice in one table of the batch, a
+ * malformed CSR offset column, a negative user / attr_col / group / novel hostname code, a
+ * reserved_host below -1.
+ * Codes are checked here, when they enter; their maxima are kept on the host, and rank / match reject a
+ * user, offer or group table too small for them.  Group codes and attribute value codes must therefore
+ * come from stable, append-only dictionaries (INTEGRATION.md §3b).
+ * Uploads exactly: every non-NULL column of the delta (n rows; CSR offsets n+1, lists their length)
+ * plus one int32 slot per upserted or removed row.  Statistics: cook_last_stats(COOK_PHASE_STATE).   */
+typedef struct {
+  int32_t reset;
+  cook_jobs_soa pending;
+  const int32_t* pending_priority;
+  const int64_t* pending_job_id;
+  int32_t n_pending_rm;
+  const int64_t* pending_rm_job_id;
+  cook_tasks_soa running;
+  int32_t n_running_rm;
+  const int64_t* running_rm_task_id;
+} cook_state_delta;
+int32_t cook_state_apply(cook_pool* pool, const cook_state_delta* delta);
+
+/* cook_rank over the live rows (running = live running tasks, pending = live pending jobs).  The ranked
+ * queue stays on the device as the handle's resident queue; out_ranked_job_id[<= #pending] (may be
+ * NULL) receives it as job ids, *out_n its length.  Rank is a total order on (user, -priority, start,
+ * task id, job id) over unique ids, so the result does not depend on where rows are stored.  Uploads
+ * only the user table's rank columns; cook_last_stats(COOK_PHASE_RANK) as after cook_rank.          */
+int32_t cook_state_rank(cook_pool* pool, const cook_user_table* users, const cook_pool_quota* pool_quota,
+                        const cook_pool_quota* group_quota, const double* group_usage,
+                        const cook_rank_params* params, int64_t* out_ranked_job_id, int32_t* out_n);
+
+/* cook_match with ranked_idx = the resident queue minus every job removed or replaced since that
+ * cook_state_rank, reading the rows' current columns (a changed reserved_host or allowed counts).
+ * Outputs as cook_match, with the job id of the k-th considerable job in out_considerable_job_id[k];
+ * afterwards cook_match_failures and cook_exchange_usage(_batch) work on this round, their k being
+ * positions in out_considerable_job_id.  Uploads only the offers, the users' match columns and the
+ * groups.  COOK_E_BADARG before any cook_state_rank and with params->reuse_resident set;
+ * COOK_E_TOO_LARGE exactly as cook_match.  stats->ms_h2d covers the upload and the gathering of the
+ * queue's rows into the matcher's columns.                                                        */
+int32_t cook_state_match(cook_pool* pool, const cook_offers_soa* offers, const cook_groups* groups,
+                         const cook_user_table* users, const cook_pool_quota* pool_quota,
+                         const cook_match_params* params, int64_t* out_considerable_job_id,
+                         int32_t* out_assign, int32_t* out_ports, int32_t max_ports,
+                         uint8_t* out_fail_reason, cook_match_stats* out_stats);
+
 /* ------------------------------------------------------------ phase timing */
 /* Device-side timing of the last call of each kind on this handle (CUDA events on the
- * pool's stream): what bench.py's `phases` block and roofline lines are computed from. */
-enum { COOK_PHASE_RANK = 0, COOK_PHASE_MATCH = 1, COOK_PHASE_REBALANCE = 2, COOK_PHASE_EXCHANGE = 3 };
+ * pool's stream): what bench.py's `phases` block and roofline lines are computed from.
+ * COOK_PHASE_STATE: the last cook_state_apply (upload, then the scatter / compaction kernels). */
+enum { COOK_PHASE_RANK = 0, COOK_PHASE_MATCH = 1, COOK_PHASE_REBALANCE = 2, COOK_PHASE_EXCHANGE = 3,
+       COOK_PHASE_STATE = 4 };
 typedef struct {
   double ms_h2d;      /* upload stage                                              */
   double ms_device;   /* kernels (for the exchange: delta kernels + the collective) */

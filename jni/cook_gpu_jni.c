@@ -154,6 +154,53 @@ JFN(jint, matchFailures)(JNIEnv* env, jclass k, jlong pool, jobject k_idx, jint 
   return cook_match_failures((cook_pool*)(intptr_t)pool, one(env, k_idx), n, (cook_failure_counts*)one(env, out_counts));
 }
 
+/* ---- resident pool state (§8f-1) --------------------------------------------------------------- */
+/* one batch from the tx-report tap: `pending` holds the jobs_from columns of the upserted rows */
+JFN(jint, stateApply)(JNIEnv* env, jclass k, jlong pool, jint reset, jint n_pending, jobjectArray pending,
+                      jobject pending_priority, jobject pending_job_id, jint n_pending_rm, jobject pending_rm_job_id,
+                      jint n_running, jobjectArray running, jint n_running_rm, jobject running_rm_task_id) {
+  cook_state_delta d;
+  memset(&d, 0, sizeof(d));
+  d.reset = reset;
+  if (pending) jobs_from(env, n_pending, pending, &d.pending);
+  d.pending_priority = one(env, pending_priority); d.pending_job_id = one(env, pending_job_id);
+  d.n_pending_rm = n_pending_rm; d.pending_rm_job_id = one(env, pending_rm_job_id);
+  if (running) tasks_from(env, n_running, running, &d.running);
+  d.n_running_rm = n_running_rm; d.running_rm_task_id = one(env, running_rm_task_id);
+  return cook_state_apply((cook_pool*)(intptr_t)pool, &d);
+}
+JFN(jint, stateRank)(JNIEnv* env, jclass k, jlong pool, jint n_users, jobjectArray users, jdoubleArray pool_quota,
+                     jdoubleArray group_quota, jobject group_usage, jint max_over_quota_jobs, jint filter_offensive,
+                     jdouble off_mem_mb, jdouble off_cpus, jobject out_ranked_job_id, jintArray out_n) {
+  cook_user_table u; cook_pool_quota pq, gq; cook_rank_params prm;
+  memset(&u, 0, sizeof(u));
+  users_from(env, n_users, users, &u); quota_from(env, pool_quota, &pq); quota_from(env, group_quota, &gq);
+  prm.max_over_quota_jobs = max_over_quota_jobs; prm.filter_offensive = filter_offensive;
+  prm.offensive_max_mem_mb = off_mem_mb; prm.offensive_max_cpus = off_cpus;
+  int32_t n = 0;
+  jint rc = cook_state_rank((cook_pool*)(intptr_t)pool, &u, &pq, &gq, one(env, group_usage), &prm,
+                            one(env, out_ranked_job_id), &n);
+  (*env)->SetIntArrayRegion(env, out_n, 0, 1, (jint*)&n);
+  return rc;
+}
+JFN(jint, stateMatch)(JNIEnv* env, jclass k, jlong pool, jint n_offers, jint n_attr_cols, jobjectArray offers,
+                      jint n_groups, jobjectArray groups, jint n_users, jobjectArray users, jdoubleArray pool_quota,
+                      jintArray iparams /* as match */, jdouble good_enough_fitness, jobject out_considerable_job_id,
+                      jobject out_assign, jobject out_ports, jint max_ports, jobject out_fail, jobject out_stats) {
+  cook_offers_soa o; cook_groups g; cook_user_table u; cook_pool_quota pq; cook_match_params prm;
+  memset(&o, 0, sizeof(o)); memset(&g, 0, sizeof(g)); memset(&u, 0, sizeof(u));
+  offers_from(env, n_offers, n_attr_cols, offers, &o);
+  int have_g = groups_from(env, n_groups, groups, &g);
+  users_from(env, n_users, users, &u); quota_from(env, pool_quota, &pq);
+  jint ip[6]; (*env)->GetIntArrayRegion(env, iparams, 0, 6, ip);
+  memset(&prm, 0, sizeof(prm));
+  prm.num_considerable = ip[0]; prm.enforce_rate_limit = ip[1]; prm.host_lifetime_mins = ip[2]; prm.fitness_kind = ip[3];
+  prm.good_enough_fitness = good_enough_fitness; prm.reuse_resident = ip[4]; prm.max_ctas = ip[5];
+  return cook_state_match((cook_pool*)(intptr_t)pool, &o, have_g ? &g : NULL, &u, &pq, &prm,
+                          one(env, out_considerable_job_id), one(env, out_assign), one(env, out_ports), max_ports,
+                          one(env, out_fail), (cook_match_stats*)one(env, out_stats));
+}
+
 /* ---- B1-B6 ------------------------------------------------------------------------------------ */
 JFN(jint, rebalance)(JNIEnv* env, jclass k, jlong pool, jint n_running, jobjectArray running, jobject running_host,
                      jint n_pending, jobjectArray pending, jobject pending_job_id, jobject pending_priority, jint n_hosts,

@@ -1,0 +1,181 @@
+"""Steady-state cycles on the resident pool state (cook_state_*) against cook_rank + cook_match on host tables.
+
+Each cycle applies one realistic batch to the resident handle: the jobs the previous match placed are launched
+(pending -> running), a few percent of the running tasks finish, as many new jobs are submitted, and a few
+priorities change.  Then both arms rank and match the same rows: the resident arm from the device tables, the
+host arm from dense host tables built from the same state.  Per cycle and arm it prints the device time per
+phase (CUDA events), the host wall time of the library calls, the bytes uploaded, and whether the outputs are
+identical.  The host arm's wall time excludes building its tables in Python.
+
+  python tools/prof_state.py --pool c2 --cycles 8
+  python tools/prof_state.py --pool c5 --c5-pool 5 --cycles 5      # the config-#5 pool of ~640 k jobs
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from cook_b200 import abi, traces  # noqa: E402
+from cook_b200.engine import GpuEngine  # noqa: E402
+
+COLS = ("user", "cpus", "mem", "gpus", "ports", "allowed", "plugin_accept", "gpu_model", "disk_request", "disk_type",
+        "est_end_ms", "ckpt_location", "reserved_host")
+LISTS = (("novel_off", ("novel_host",)), ("attr_off", ("attr_col", "attr_val")), ("group_off", ("group_idx",)))
+
+
+def csr_take(off, vals, rows):
+    lens = (off[1:] - off[:-1])[rows]
+    noff = np.zeros(len(rows) + 1, np.int32)
+    np.cumsum(lens, out=noff[1:])
+    idx = np.repeat(off[:-1][rows] - noff[:-1], lens) + np.arange(noff[-1])
+    return noff, [v[idx] if noff[-1] else np.zeros(1, v.dtype) for v in vals]
+
+
+class Jobs:
+    """Every job of the run (live or not) as columns; rows are positions."""
+
+    def __init__(self, jobs, prio, jid):
+        self.c = {n: jobs.col(n) for n in COLS if jobs.col(n) is not None}
+        self.l = {o: (jobs.col(o), [jobs.col(v) for v in vs]) for o, vs in LISTS if jobs.col(o) is not None}
+        self.prio, self.jid = prio.copy(), jid.copy()
+
+    def soa(self, rows):
+        kw = {n: c[rows] for n, c in self.c.items()}
+        for o, vs in LISTS:
+            if o not in self.l:
+                continue
+            off, vals = csr_take(self.l[o][0], self.l[o][1], rows)
+            kw[o] = off
+            kw.update(dict(zip(vs, vals)))
+        return abi.JobsSoA(n=len(rows), **kw)
+
+
+def card():
+    try:
+        out = subprocess.check_output(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], text=True)
+        return out.strip().splitlines()[0]
+    except Exception as e:   # noqa: BLE001
+        return f"unknown ({e})"
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--pool", choices=("c2", "c5"), default="c2")
+    ap.add_argument("--c5-pool", type=int, default=5)
+    ap.add_argument("--cycles", type=int, default=6)
+    ap.add_argument("--seed", type=int, default=7)
+    a = ap.parse_args()
+    t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
+    jobs, pc, rc = t["jobs"], t["cols"]["pending"], t["cols"]["running"]
+    J = jobs.n
+    print(json.dumps({"card": card(), "pool": a.pool, "jobs": J, "offers": t["offers"].n, "running": len(rc["task_id"])}),
+          flush=True)
+    rng = np.random.default_rng(a.seed)
+    J0 = int(J * 0.8)                       # the rest are submitted during the run
+    store = Jobs(jobs, pc["priority"], pc["job_id"])
+    alive = np.zeros(J, bool)
+    alive[:J0] = True
+    nxt = J0
+    run = {k: np.asarray(v).copy() for k, v in rc.items()}
+    next_tid = int(run["task_id"].max()) + 10 if len(run["task_id"]) else 10
+    users, offers, groups = t["users"], t["offers"], t.get("groups")
+    params = traces.match_params(J, host_lifetime_mins=t.get("host_lifetime_mins", 0))
+    max_ports = int(jobs.col("ports").max()) if jobs.col("ports") is not None else 0
+    res, host = GpuEngine(pool_name="resident"), GpuEngine(pool_name="host")
+    pos_of = {int(j): i for i, j in enumerate(store.jid)}
+    next_jid = int(store.jid.max()) + 10
+
+    def pend_delta(rows):
+        return dict(pending=store.soa(rows), pending_priority=store.prio[rows], pending_job_id=store.jid[rows])
+
+    res.state_apply(abi.make_delta(reset=True, running=abi.make_tasks(**run), **pend_delta(np.flatnonzero(alive))))
+    placed = np.zeros(0, np.int64)
+    for cycle in range(a.cycles):
+        # ---- the batch
+        launch_rows = np.array([pos_of[int(j)] for j in placed], np.int64)
+        n_fin = int(len(run["task_id"]) * 0.03)
+        fin = rng.choice(len(run["task_id"]), n_fin, replace=False) if n_fin else np.zeros(0, np.int64)
+        fin_ids = run["task_id"][fin]
+        keep = np.ones(len(run["task_id"]), bool)
+        keep[fin] = False
+        sc = store.c
+        lt = {"user": sc["user"][launch_rows], "priority": store.prio[launch_rows],
+              "start_time": np.full(len(launch_rows), 1_700_000_000_000 + cycle, np.int64),
+              "task_id": next_tid + 2 * np.arange(len(launch_rows), dtype=np.int64), "job_id": store.jid[launch_rows].copy(),
+              "cpus": sc["cpus"][launch_rows], "mem": sc["mem"][launch_rows], "gpus": sc["gpus"][launch_rows]}
+        next_tid += 2 * len(launch_rows) + 2
+        launched_ids = store.jid[launch_rows].copy()
+        # as many submissions as launches + finishes: a launched job's row comes back under a new job id (same
+        # shape), the finishes are made up from the rows not yet submitted
+        store.jid[launch_rows] = next_jid + 2 * np.arange(len(launch_rows), dtype=np.int64)
+        next_jid += 2 * len(launch_rows) + 2
+        pos_of.update({int(j): int(i) for j, i in zip(store.jid[launch_rows], launch_rows)})
+        n_new = min(n_fin, J - nxt)
+        sub = np.concatenate([launch_rows, np.arange(nxt, nxt + n_new)]).astype(np.int64)
+        nxt += n_new
+        n_sub = len(sub)
+        alive[sub] = True
+        live = np.flatnonzero(alive & ~np.isin(np.arange(J), sub))
+        chg = rng.choice(live, min(len(live), max(1, len(live) // 1000)), replace=False)
+        store.prio[chg] = rng.choice(np.array([10, 50, 90], np.int32), len(chg))
+        up = np.concatenate([sub, chg])
+        d = abi.make_delta(running=abi.make_tasks(**lt) if len(launch_rows) else None, pending_rm=launched_ids,
+                           running_rm=fin_ids, **pend_delta(up))
+        run = {k: np.concatenate([v[keep], lt[k]]) for k, v in run.items()}
+        w0 = time.perf_counter()
+        res.state_apply(d)
+        w_apply = time.perf_counter() - w0
+        st_apply = res.last_stats(abi.PHASE_STATE)
+        # ---- resident arm
+        w0 = time.perf_counter()
+        q = res.state_rank(users)
+        w_rank = time.perf_counter() - w0
+        rs_rank = res.last_stats(abi.PHASE_RANK)
+        w0 = time.perf_counter()
+        mr = res.state_match(offers, users, params, groups=groups, max_ports=max_ports)
+        w_match = time.perf_counter() - w0
+        # ---- host arm on the same rows
+        rows = np.flatnonzero(alive)
+        hj = store.soa(rows)
+        hp = abi.make_tasks(user=sc["user"][rows], priority=store.prio[rows], start_time=np.full(len(rows), abi.INT64_MAX),
+                            task_id=np.full(len(rows), -1, np.int64), job_id=store.jid[rows], cpus=sc["cpus"][rows],
+                            mem=sc["mem"][rows], gpus=sc["gpus"][rows])
+        hr = abi.make_tasks(**run)
+        w0 = time.perf_counter()
+        r = host.rank(hr, hp, users)
+        hw_rank = time.perf_counter() - w0
+        hs_rank = host.last_stats(abi.PHASE_RANK)
+        w0 = time.perf_counter()
+        mh = host.match(r["ranked"], hj, offers, users, params, groups=groups, max_ports=max_ports)
+        hw_match = time.perf_counter() - w0
+        same = (np.array_equal(q, store.jid[rows][r["ranked"]]) and
+                np.array_equal(mr["considerable"], store.jid[rows][mh["considerable"]]) and
+                all(np.array_equal(mr[k], mh[k]) for k in ("assign", "ports", "fail")))
+        placed = mr["considerable"][mr["assign"] >= 0]
+
+        def ms(s):
+            return {k: round(s[k], 3) for k in ("ms_h2d", "ms_device", "ms_d2h")} if "ms_device" in s else \
+                {k: round(s[k], 3) for k in ("ms_h2d", "ms_considerable", "ms_match", "ms_d2h")}
+
+        print(json.dumps({
+            "cycle": cycle, "pending": int(alive.sum()), "running": len(run["task_id"]),
+            "batch": {"launched": len(launch_rows), "finished": n_fin, "submitted": n_sub, "reprioritised": len(chg)},
+            "resident": {"apply": {**ms(st_apply), "wall_ms": round(1e3 * w_apply, 3), "h2d_bytes": st_apply["h2d_bytes"]},
+                         "rank": {**ms(rs_rank), "wall_ms": round(1e3 * w_rank, 3), "h2d_bytes": rs_rank["h2d_bytes"]},
+                         "match": {**ms(mr["stats"]), "wall_ms": round(1e3 * w_match, 3),
+                                   "h2d_bytes": mr["stats"]["h2d_bytes"]}},
+            "host": {"rank": {**ms(hs_rank), "wall_ms": round(1e3 * hw_rank, 3), "h2d_bytes": hs_rank["h2d_bytes"]},
+                     "match": {**ms(mh["stats"]), "wall_ms": round(1e3 * hw_match, 3),
+                               "h2d_bytes": mh["stats"]["h2d_bytes"]}},
+            "identical": bool(same), "n_matched": int(mr["stats"]["n_matched"])}), flush=True)
+    res.close()
+    host.close()
+
+
+if __name__ == "__main__":
+    main()
