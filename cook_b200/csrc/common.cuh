@@ -91,7 +91,7 @@ struct Carve {
 // CUDA call, then (after the arena is grown to the measured size) carving.  Both runs make the same takes
 // in the same order, so the arena is sized by the list it is carved by; the body therefore branches on
 // host data only.  `start` (if any) is recorded on st once the arena is large enough, before the first
-// upload.  Adds the uploaded bytes to *h2d.
+// upload.  Adds the uploaded bytes to *h2d (if given).
 template <class Body>
 inline cudaError_t carve(Arena& a, cudaStream_t st, cudaEvent_t start, int64_t* h2d, const Body& body) {
   Carve m;
@@ -102,7 +102,7 @@ inline cudaError_t carve(Arena& a, cudaStream_t st, cudaEvent_t start, int64_t* 
   Carve c;
   c.base = a.base; c.cap = a.cap; c.st = st;
   body(c);
-  *h2d += c.h2d;
+  if (h2d) *h2d += c.h2d;
   return c.err;
 }
 
@@ -132,48 +132,88 @@ struct cook_pool {
   char err[512] = {0};
 };
 
-// ---- device sources of rank and match (state.cu feeds them from its resident tables)
-// Dense task columns on the device, running tasks [0, R) then pending jobs [R, R + J).
-struct DevTasks {
-  int R, J;
-  const int32_t* user; const int32_t* prio; const int64_t* start; const int64_t* tid; const int64_t* jid;
-  const double* cpus; const double* mem; const double* gpus;
-};
-// The job columns of a match that the plan carves and the caller then writes on the device (row d of
-// the queue is job d, ranked[d] = d).  Null: the column is absent.
-struct DevJobCols {
-  int32_t* ranked; int32_t* user; double* cpus; double* mem; double* gpus; int64_t* job_id;
-  int32_t* ports; uint8_t* allowed; uint8_t* plugin;
-  int32_t* novel_off; int32_t* novel_host; int32_t* gpu_model; double* disk_request; int32_t* disk_type;
-  int32_t* attr_off; int32_t* attr_col; int32_t* attr_val; int64_t* est_end_ms; int32_t* ckpt_location;
-  int32_t* reserved_host; int32_t* group_off; int32_t* group_idx;
-};
-// What such a match holds, known on the host without looking at the rows: which columns carry a
-// non-absent value somewhere, and upper bounds of the list lengths (0: the list is absent).
-struct DevJobSpec {
-  bool ports, allowed, plugin, gpu_model, disk, est_end, ckpt, reserved, any_gpus;
-  int64_t n_novel, n_attr, n_group;
-  const int32_t* gp_off;   // host [n_groups + 1]: per-group member capacity offsets
-  DevJobCols out;          // set by the plan
+// ---- the inputs of rank and match on the device, uploaded from host tables or gathered from the resident
+// state (state.cu)
+// Rank's task columns: running tasks [0, R) then pending jobs [R, R + J).
+struct TaskCols {
+  const int32_t* user;
+  const int32_t* prio;
+  const int64_t* start;
+  const int64_t* tid;
+  const int64_t* jid;
+  const double* cpus;
+  const double* mem;
+  const double* gpus;
 };
 
-#include <functional>
-// rank.cu: cook_rank over host columns (dev == nullptr) or dense device columns.  With dev,
-// out_ranked_idx may be null (not downloaded) and on_queue, if given, is called with the device queue
-// (pending indices) and its device length before the result download, on the pool's stream.
-int32_t rank_impl(cook_pool* pool, const cook_tasks_soa* running, const cook_tasks_soa* pending, const DevTasks* dev,
-                  const cook_user_table* users, const cook_pool_quota* pool_quota, const cook_pool_quota* group_quota,
-                  const double* group_usage, const cook_rank_params* params, int32_t* out_ranked_idx, int32_t* out_n,
-                  double* out_dru, int32_t* out_order, int32_t* out_order_n,
-                  const std::function<int32_t(const int32_t* d_ranked, const int32_t* d_n, int* launches)>* on_queue);
-// match.cu: cook_match over n_ranked jobs whose columns `fill` writes on the device once the plan has
-// carved them (dj->out); out_job_id receives the job id of every considerable job.
-int32_t match_device_jobs(cook_pool* pool, int32_t n_ranked, DevJobSpec* dj,
-                          const std::function<int32_t(const DevJobCols&, int* launches)>& fill,
-                          const cook_offers_soa* offers, const cook_groups* groups, const cook_user_table* users,
-                          const cook_pool_quota* pool_quota, const cook_match_params* params, int64_t* out_job_id,
-                          int32_t* out_assign, int32_t* out_ports, int32_t max_ports, uint8_t* out_fail_reason,
-                          cook_match_stats* out_stats);
+// The match's job columns in job index space (null: absent).
+struct JobDev {
+  const int32_t* user;
+  const double* cpus;
+  const double* mem;
+  const double* gpus;
+  const int32_t* ports;
+  const uint8_t* allowed;
+  const uint8_t* plugin;
+  const int32_t* novel_off; const int32_t* novel_host;
+  const int32_t* gpu_model;
+  const double* disk_request; const int32_t* disk_type;
+  const int32_t* attr_off; const int32_t* attr_col; const int32_t* attr_val;
+  const int64_t* est_end_ms;
+  const int32_t* ckpt_location;
+  const int32_t* reserved_host;
+  const int32_t* group_off; const int32_t* group_idx;
+};
+
+// Rank and match only read their device columns, so they hold them as const.  The gathers of the resident
+// state are what fills columns carved for them, and write through this.
+template <class T>
+__host__ __device__ inline T* writable(const T* p) { return const_cast<T*>(p); }
+
+// rank.cu: cook_rank over R running tasks and J pending jobs, from the host tables `running` and `pending`
+// or from task columns already on the device (`dev`).  out_ranked_idx may be null (not downloaded).
+// *queue (if given) receives the ranked pending indices on the device and their device count; they live in
+// the pool's arena until it is carved again.
+struct RankQueue {
+  const int32_t* ranked;
+  const int32_t* n;
+};
+int32_t rank_impl(cook_pool* pool, int R, int J, const cook_tasks_soa* running, const cook_tasks_soa* pending,
+                  const TaskCols* dev, const cook_user_table* users, const cook_pool_quota* pool_quota,
+                  const cook_pool_quota* group_quota, const double* group_usage, const cook_rank_params* params,
+                  int32_t* out_ranked_idx, int32_t* out_n, double* out_dru, int32_t* out_order, int32_t* out_order_n,
+                  RankQueue* queue);
+
+// match.cu: what a match's plan needs to know about its jobs before it carves their columns.
+struct JobShape {
+  int J = 0;                      // job rows
+  JobDev cols = {};               // the columns to carve (null: absent): host columns to upload when
+                                  // `upload`, else the resident columns the caller gathers them from
+  bool upload = false;
+  int64_t n_novel = 0, n_attr = 0, n_group = 0;   // entries of each CSR list
+  std::vector<int32_t> gp_off;    // [n_groups + 1] per-group member capacity offsets (empty: no groups)
+  bool any_gpus_ports = false;    // some job asks for gpus or ports
+  bool job_ids = false;           // carve a job id per row, and report the considerable jobs by job id
+};
+// The carved rows of a plan whose columns the caller writes: row d is ranked[d] = d.
+struct MatchRows {
+  JobDev jb;
+  int32_t* ranked;
+  int64_t* job_id;
+};
+// The checks of a match's offers, groups, users, params and sizes, with `who` in the messages.  The offer
+// and group tables are checked when `tables`; `novel` and `grouped`: some job has novel-host or group lists.
+int32_t check_match_inputs(cook_pool* pool, const char* who, const cook_offers_soa* offers, const cook_groups* groups,
+                           const cook_user_table* users, const cook_match_params* params, int32_t max_ports,
+                           bool tables, bool novel, bool grouped);
+// The pool's match plan is built for n_ranked rows of the jobs `sh` describes (ranked_idx: uploaded, null:
+// the caller writes *rows before the run), then run.  A failed build leaves no valid plan.
+int32_t match_build(cook_pool* pool, const int32_t* ranked_idx, int32_t n_ranked, const JobShape& sh,
+                    const cook_offers_soa* offers, const cook_groups* groups, const cook_user_table* users,
+                    const cook_pool_quota* pool_quota, const cook_match_params* params, int32_t max_ports,
+                    MatchRows* rows);
+int32_t match_run(cook_pool* pool, int32_t* out_considerable, int64_t* out_job_id, int32_t* out_assign,
+                  int32_t* out_ports, uint8_t* out_fail_reason, cook_match_stats* out_stats, bool uploaded, int max_ctas);
 
 inline int32_t set_err(cook_pool* p, int32_t code, const char* fmt, ...) {
   if (p) {

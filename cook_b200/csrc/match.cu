@@ -72,24 +72,6 @@ struct VmState {  // everything one fit evaluation needs about a VM
   int ptot;   // ports offered
 };
 
-struct JobDev {   // columns in ORIGINAL job index space (may be null)
-  const int32_t* user;
-  const double* cpus;
-  const double* mem;
-  const double* gpus;
-  const int32_t* ports;
-  const uint8_t* allowed;
-  const uint8_t* plugin;
-  const int32_t* novel_off; const int32_t* novel_host;
-  const int32_t* gpu_model;
-  const double* disk_request; const int32_t* disk_type;
-  const int32_t* attr_off; const int32_t* attr_col; const int32_t* attr_val;
-  const int64_t* est_end_ms;
-  const int32_t* ckpt_location;
-  const int32_t* reserved_host;
-  const int32_t* group_off; const int32_t* group_idx;
-};
-
 struct OfferDev {
   int O;
   // hot columns, gathered into rank-sorted index space v
@@ -2281,31 +2263,33 @@ static void plan_free(void* p) {
   if (mp) { mp->arena.release(); delete mp; }
 }
 
-// A job column of the plan: uploaded from the host, or (dj) carved for the caller to write when present.
+// The pool's plan, made on first use.
+static MatchPlan* plan_of(cook_pool* pool) {
+  if (!pool->match_plan) {
+    pool->match_plan = new MatchPlan();
+    pool->match_plan_free = plan_free;
+  }
+  return static_cast<MatchPlan*>(pool->match_plan);
+}
+
+// A job column of the plan: carved when the shape has it, and filled from the host when the shape uploads.
 template <class T>
-static T* job_col(Carve& c, const T* host, size_t n, const DevJobSpec* dj, bool present, T** dev_out) {
-  if (!dj) return c.up(host, n);
-  T* d = present ? c.take<T>(n ? n : 1) : nullptr;
-  *dev_out = d;
+static T* job_col(Carve& c, const JobShape& sh, const T* col, size_t n) {
+  if (!col) return nullptr;
+  T* d = c.take<T>(n ? n : 1);
+  if (sh.upload) c.copy(d, col, n);
   return d;
 }
 
-// dj: the job columns come from the device (match_device_jobs); `jobs` is then unused and the ranked
-// queue is 0 .. n_ranked-1 over n_ranked jobs.
-static int32_t build_plan(cook_pool* pool, MatchPlan* mp, const int32_t* ranked_idx,
-                          int32_t n_ranked, const cook_jobs_soa* jobs_in,
-                          const cook_offers_soa* offers, const cook_groups* groups,
-                          const cook_user_table* users, const cook_pool_quota* pool_quota,
-                          const cook_match_params* params, int32_t max_ports, DevJobSpec* dj = nullptr) {
+int32_t match_build(cook_pool* pool, const int32_t* ranked_idx, int32_t n_ranked, const JobShape& sh,
+                    const cook_offers_soa* offers, const cook_groups* groups, const cook_user_table* users,
+                    const cook_pool_quota* pool_quota, const cook_match_params* params, int32_t max_ports,
+                    MatchRows* rows) {
   cudaStream_t st = pool->stream;
+  MatchPlan* mp = plan_of(pool);
   Arena& ar = mp->arena;
-  cook_jobs_soa none;
-  memset(&none, 0, sizeof(none));
-  none.n = n_ranked;
-  const cook_jobs_soa* jobs = dj ? &none : jobs_in;
-  DevJobCols dc;
-  memset(&dc, 0, sizeof(dc));
-  const int J = jobs->n, O = offers->n, U = users->n_users, NC = params->num_considerable;
+  const JobDev& jc = sh.cols;
+  const int J = sh.J, O = offers->n, U = users->n_users, NC = params->num_considerable;
   mp->valid = false;
   // host-side prep: offers sorted by hostname rank (tie-break order)
   std::vector<int32_t> perm(O, -1);
@@ -2321,33 +2305,13 @@ static int32_t build_plan(cook_pool* pool, MatchPlan* mp, const int32_t* ranked_
   }
   // per-group capacity of the placed list = #member jobs
   const int G = groups ? groups->n_groups : 0;
-  std::vector<int32_t> gp_off(G + 1, 0);
-  size_t n_memb = 0;
-  if (G && dj && dj->n_group) {
-    gp_off.assign(dj->gp_off, dj->gp_off + G + 1);
-    n_memb = gp_off[G];
-  } else if (G && jobs->group_off) {
-    n_memb = jobs->group_off[J];
-    for (size_t i = 0; i < n_memb; i++) {
-      int g = jobs->group_idx[i];
-      if (g < 0 || g >= G) return set_err(pool, COOK_E_BADARG, "cook_match: bad group index");
-      gp_off[g + 1]++;
-    }
-    for (int g = 0; g < G; g++) gp_off[g + 1] += gp_off[g];
-  }
+  const bool grouped = jc.group_off && G;
+  const size_t n_memb = grouped ? sh.gp_off[G] : 0;
   // The cpu+mem-only kernel is used when no constraint column can affect a
   // placement (all-zero ports/gpus columns count as absent).
-  bool constr_eff = jobs->novel_off || jobs->gpu_model || jobs->disk_request || jobs->attr_off ||
-                    jobs->est_end_ms || jobs->ckpt_location || jobs->reserved_host ||
-                    (jobs->group_off && G) || offers->is_k8s || offers->max_tasks ||
-                    offers->reserved || offers->gpu_off;
-  if (dj)   // the state counts its non-absent values per column as rows come and go
-    constr_eff = constr_eff || dj->n_novel || dj->gpu_model || dj->disk || dj->n_attr || dj->est_end || dj->ckpt ||
-                 dj->reserved || (dj->n_group && G) || dj->any_gpus || dj->ports;
-  if (!constr_eff && jobs->gpus)
-    for (int j = 0; j < J && !constr_eff; j++) constr_eff = jobs->gpus[j] != 0.0;
-  if (!constr_eff && jobs->ports)
-    for (int j = 0; j < J && !constr_eff; j++) constr_eff = jobs->ports[j] != 0;
+  const bool constr_eff = jc.novel_off || jc.gpu_model || jc.disk_request || jc.attr_off || jc.est_end_ms ||
+                          jc.ckpt_location || jc.reserved_host || grouped || offers->is_k8s || offers->max_tasks ||
+                          offers->reserved || offers->gpu_off || sh.any_gpus_ports;
 
   // blocks: B jobs at the start, then sized by the resolver to ~btarget placements per block
   int B = 64, bmin = 64, bmax = MAXB, btarget = 32;
@@ -2366,6 +2330,7 @@ static int32_t build_plan(cook_pool* pool, MatchPlan* mp, const int32_t* ranked_
   JobDev jb;
   OfferDev of;
   GroupDev gr;
+  int32_t* ranked = nullptr;
   memset(&ca, 0, sizeof(ca));
   memset(&ma, 0, sizeof(ma));
   memset(&jb, 0, sizeof(jb));
@@ -2375,39 +2340,37 @@ static int32_t build_plan(cook_pool* pool, MatchPlan* mp, const int32_t* ranked_
   of.n_attr_cols = offers->attr ? offers->n_attr_cols : 0;
   mp->h2d_bytes = 0;
   const cudaError_t carved = carve(ar, st, nullptr, &mp->h2d_bytes, [&](Carve& c) {
-    ca.ranked = job_col(c, ranked_idx, n_ranked, dj, true, &dc.ranked);
-    jb.user = job_col(c, jobs->user, J, dj, true, &dc.user);
-    jb.cpus = job_col(c, jobs->cpus, J, dj, true, &dc.cpus);
-    jb.mem = job_col(c, jobs->mem, J, dj, true, &dc.mem);
-    jb.gpus = job_col(c, jobs->gpus, J, dj, true, &dc.gpus);
-    jb.ports = job_col(c, jobs->ports, J, dj, dj && dj->ports, &dc.ports);
-    jb.allowed = job_col(c, jobs->allowed, J, dj, dj && dj->allowed, &dc.allowed);
-    jb.plugin = job_col(c, jobs->plugin_accept, J, dj, dj && dj->plugin, &dc.plugin);
-    if (jobs->novel_off || (dj && dj->n_novel)) {
-      jb.novel_off = job_col(c, jobs->novel_off, J + 1, dj, true, &dc.novel_off);
-      jb.novel_host = job_col(c, jobs->novel_host, std::max<size_t>(1, dj ? dj->n_novel : jobs->novel_off[J]), dj, true,
-                              &dc.novel_host);
+    ranked = c.take<int32_t>(n_ranked ? n_ranked : 1);
+    if (ranked_idx) c.copy(ranked, ranked_idx, n_ranked);
+    jb.user = job_col(c, sh, jc.user, J);
+    jb.cpus = job_col(c, sh, jc.cpus, J);
+    jb.mem = job_col(c, sh, jc.mem, J);
+    jb.gpus = job_col(c, sh, jc.gpus, J);
+    jb.ports = job_col(c, sh, jc.ports, J);
+    jb.allowed = job_col(c, sh, jc.allowed, J);
+    jb.plugin = job_col(c, sh, jc.plugin, J);
+    if (jc.novel_off) {
+      jb.novel_off = job_col(c, sh, jc.novel_off, J + 1);
+      jb.novel_host = job_col(c, sh, jc.novel_host, std::max<size_t>(1, sh.n_novel));
     }
-    jb.gpu_model = job_col(c, jobs->gpu_model, J, dj, dj && dj->gpu_model, &dc.gpu_model);
-    jb.disk_request = job_col(c, jobs->disk_request, J, dj, dj && dj->disk, &dc.disk_request);
-    jb.disk_type = job_col(c, jobs->disk_type, J, dj, dj && dj->disk, &dc.disk_type);
-    if (jobs->attr_off || (dj && dj->n_attr)) {
-      const size_t na = std::max<size_t>(1, dj ? dj->n_attr : jobs->attr_off[J]);
-      jb.attr_off = job_col(c, jobs->attr_off, J + 1, dj, true, &dc.attr_off);
-      jb.attr_col = job_col(c, jobs->attr_col, na, dj, true, &dc.attr_col);
-      jb.attr_val = job_col(c, jobs->attr_val, na, dj, true, &dc.attr_val);
+    jb.gpu_model = job_col(c, sh, jc.gpu_model, J);
+    jb.disk_request = job_col(c, sh, jc.disk_request, J);
+    jb.disk_type = job_col(c, sh, jc.disk_type, J);
+    if (jc.attr_off) {
+      const size_t na = std::max<size_t>(1, sh.n_attr);
+      jb.attr_off = job_col(c, sh, jc.attr_off, J + 1);
+      jb.attr_col = job_col(c, sh, jc.attr_col, na);
+      jb.attr_val = job_col(c, sh, jc.attr_val, na);
     }
-    jb.est_end_ms = job_col(c, jobs->est_end_ms, J, dj, dj && dj->est_end, &dc.est_end_ms);
-    jb.ckpt_location = job_col(c, jobs->ckpt_location, J, dj, dj && dj->ckpt, &dc.ckpt_location);
-    jb.reserved_host = job_col(c, jobs->reserved_host, J, dj, dj && dj->reserved, &dc.reserved_host);
-    if ((jobs->group_off || (dj && dj->n_group)) && G) {
-      jb.group_off = job_col(c, jobs->group_off, J + 1, dj, true, &dc.group_off);
-      jb.group_idx = job_col(c, jobs->group_idx, std::max<size_t>(1, n_memb), dj, true, &dc.group_idx);
+    jb.est_end_ms = job_col(c, sh, jc.est_end_ms, J);
+    jb.ckpt_location = job_col(c, sh, jc.ckpt_location, J);
+    jb.reserved_host = job_col(c, sh, jc.reserved_host, J);
+    if (grouped) {
+      jb.group_off = job_col(c, sh, jc.group_off, J + 1);
+      jb.group_idx = job_col(c, sh, jc.group_idx, std::max<size_t>(1, n_memb));
     }
-    // the job ids of the rows, for the result (device source only)
-    mp->d_job_id = dj ? c.take<int64_t>(J + 1) : nullptr;
-    dc.job_id = mp->d_job_id;
-    mp->d_cons_jid = dj ? c.take<int64_t>(NC + 1) : nullptr;
+    mp->d_job_id = sh.job_ids ? c.take<int64_t>(J + 1) : nullptr;
+    mp->d_cons_jid = sh.job_ids ? c.take<int64_t>(NC + 1) : nullptr;
 
     mp->d_perm = c.up(perm.data(), O); of.perm = mp->d_perm;
     mp->d_oc = c.up(offers->cpus, O); mp->d_om = c.up(offers->mem, O);
@@ -2440,7 +2403,7 @@ static int32_t build_plan(cook_pool* pool, MatchPlan* mp, const int32_t* ranked_
     mp->d_attr_v = c.take<int32_t>((size_t)of.n_attr_cols * O + 1);
     of.vc = mp->d_vc; of.attr_v = mp->d_attr_v;
 
-    if (G && (jobs->group_off || (dj && dj->n_group))) {
+    if (grouped) {
       gr.n_groups = G;
       gr.kind = c.up(groups->kind, G);
       gr.attr_col = c.up(groups->attr_col, G);
@@ -2449,7 +2412,7 @@ static int32_t build_plan(cook_pool* pool, MatchPlan* mp, const int32_t* ranked_
       const int nc = std::max(1, groups->cot_off[G]);
       gr.cot_host = c.up(groups->cot_hostname_id, nc);
       gr.cot_attr = c.up(groups->cot_attr_val, nc);
-      gr.gp_off = c.up(gp_off.data(), G + 1);
+      gr.gp_off = c.up(sh.gp_off.data(), G + 1);
       gr.gp_n = c.take<int32_t>(G + 1);
       gr.gp_vm = c.take<int32_t>(n_memb + 1);
     }
@@ -2502,7 +2465,7 @@ static int32_t build_plan(cook_pool* pool, MatchPlan* mp, const int32_t* ranked_
     ma.gres_seq = c.take<unsigned>(GRING);
   });
   CK(pool, carved);
-  ca.n_ranked = n_ranked; ca.jb = jb; ca.n_users = U;
+  ca.ranked = ranked; ca.n_ranked = n_ranked; ca.jb = jb; ca.n_users = U;
   ca.enforce_rate_limit = params->enforce_rate_limit;
   cook_pool_quota qoff{0, 0, 0, 0, 0};
   ca.pool_q = pool_quota ? *pool_quota : qoff;
@@ -2528,15 +2491,15 @@ static int32_t build_plan(cook_pool* pool, MatchPlan* mp, const int32_t* ranked_
   if (const char* el = getenv("COOK_LOOKAHEAD")) { int v = atoi(el); if (v >= 2 && v <= RING - 1) ma.lookahead = v; }
   mp->J = J; mp->O = O; mp->U = U; mp->n_ranked = n_ranked; mp->NC = NC; mp->max_ports = max_ports;
   mp->G = G; mp->B = B; mp->constr = constr_eff; mp->n_memb = n_memb;
-  if (dj) dj->out = dc;
-  mp->valid = true;
+  if (rows) *rows = MatchRows{jb, ranked, mp->d_job_id};
   return COOK_OK;
 }
 
-// out_job_id (device-source plans, instead of out_considerable): the job id of every considerable job
-static int32_t run_plan(cook_pool* pool, MatchPlan* mp, int32_t* out_considerable,
-                        int32_t* out_assign, int32_t* out_ports, uint8_t* out_fail_reason,
-                        cook_match_stats* out_stats, bool uploaded, int max_ctas, int64_t* out_job_id = nullptr) {
+// out_job_id (plans with job ids): the job id of every considerable job
+int32_t match_run(cook_pool* pool, int32_t* out_considerable, int64_t* out_job_id, int32_t* out_assign,
+                  int32_t* out_ports, uint8_t* out_fail_reason, cook_match_stats* out_stats, bool uploaded, int max_ctas) {
+  MatchPlan* mp = plan_of(pool);
+  mp->valid = true;   // the plan's inputs are complete: a caller that writes its rows did so before the run
   cudaStream_t st = pool->stream;
   const int O = mp->O, U = mp->U, n_ranked = mp->n_ranked, max_ports = mp->max_ports;
   MatchArgs& ma = mp->ma;
@@ -2740,6 +2703,56 @@ static int32_t run_plan(cook_pool* pool, MatchPlan* mp, int32_t* out_considerabl
   return COOK_OK;
 }
 
+int32_t check_match_inputs(cook_pool* pool, const char* who, const cook_offers_soa* offers, const cook_groups* groups,
+                           const cook_user_table* users, const cook_match_params* params, int32_t max_ports,
+                           bool tables, bool novel, bool grouped) {
+  if (params->good_enough_fitness < 1.0)
+    return set_err(pool, COOK_E_BADARG,
+                   "%s: good_enough_fitness < 1.0 is Fenzo's racy early-exit mode; "
+                   "only the deterministic mode (>= 1.0) is supported", who);
+  if (params->fitness_kind != 0) return set_err(pool, COOK_E_UNSUPPORTED_CONSTRAINT, "%s: only cpuMemBinPacker", who);
+  const int O = offers->n;
+  if (O < 0 || users->n_users <= 0 || params->num_considerable < 0 || max_ports < 0)
+    return set_err(pool, COOK_E_BADARG, "%s: bad sizes", who);
+  if (!tables) return COOK_OK;
+  if (!offers->name_rank && O > 0) return set_err(pool, COOK_E_BADARG, "%s: offers.name_rank required", who);
+  if (groups && !idx_in_range(groups->attr_col, groups->n_groups, -1, std::max(1, offers->n_attr_cols)))
+    return set_err(pool, COOK_E_BADARG, "%s: groups.attr_col out of range", who);
+  grouped = grouped && groups && groups->n_groups;
+  if ((novel || offers->reserved || grouped) && !offers->hostname_id)
+    return set_err(pool, COOK_E_BADARG, "%s: hostname_id column required by constraints", who);
+  if (grouped && (!groups->cot_off || !groups->kind)) return set_err(pool, COOK_E_BADARG, "%s: incomplete cook_groups", who);
+  return COOK_OK;
+}
+
+// The shape of host-table jobs: their columns as given, uploaded; the group members counted per group.
+static int32_t host_shape(cook_pool* pool, const cook_jobs_soa* jobs, int G, JobShape* sh) {
+  const int J = jobs->n;
+  sh->J = J;
+  sh->cols = JobDev{jobs->user, jobs->cpus, jobs->mem, jobs->gpus, jobs->ports, jobs->allowed, jobs->plugin_accept,
+                    jobs->novel_off, jobs->novel_host, jobs->gpu_model, jobs->disk_request, jobs->disk_type,
+                    jobs->attr_off, jobs->attr_col, jobs->attr_val, jobs->est_end_ms, jobs->ckpt_location,
+                    jobs->reserved_host, jobs->group_off, jobs->group_idx};
+  sh->upload = true;
+  sh->n_novel = jobs->novel_off ? jobs->novel_off[J] : 0;
+  sh->n_attr = jobs->attr_off ? jobs->attr_off[J] : 0;
+  sh->n_group = jobs->group_off ? jobs->group_off[J] : 0;
+  if (G && jobs->group_off) {
+    sh->gp_off.assign(G + 1, 0);
+    for (int64_t i = 0; i < sh->n_group; i++) {
+      const int g = jobs->group_idx[i];
+      if (g < 0 || g >= G) return set_err(pool, COOK_E_BADARG, "cook_match: bad group index");
+      sh->gp_off[g + 1]++;
+    }
+    for (int g = 0; g < G; g++) sh->gp_off[g + 1] += sh->gp_off[g];
+  }
+  if (jobs->gpus)
+    for (int j = 0; j < J && !sh->any_gpus_ports; j++) sh->any_gpus_ports = jobs->gpus[j] != 0.0;
+  if (jobs->ports)
+    for (int j = 0; j < J && !sh->any_gpus_ports; j++) sh->any_gpus_ports = jobs->ports[j] != 0;
+  return COOK_OK;
+}
+
 extern "C" int32_t cook_match(cook_pool* pool, const int32_t* ranked_idx, int32_t n_ranked,
                               const cook_jobs_soa* jobs, const cook_offers_soa* offers,
                               const cook_groups* groups, const cook_user_table* users,
@@ -2750,16 +2763,12 @@ extern "C" int32_t cook_match(cook_pool* pool, const int32_t* ranked_idx, int32_
   if (!pool) return COOK_E_BADARG;
   if (!ranked_idx || !jobs || !offers || !users || !params || !out_considerable || !out_assign)
     return set_err(pool, COOK_E_BADARG, "cook_match: null argument");
-  if (params->good_enough_fitness < 1.0)
-    return set_err(pool, COOK_E_BADARG,
-                   "cook_match: good_enough_fitness < 1.0 is Fenzo's racy early-exit mode; "
-                   "only the deterministic mode (>= 1.0) is supported");
-  if (params->fitness_kind != 0)
-    return set_err(pool, COOK_E_UNSUPPORTED_CONSTRAINT, "cook_match: only cpuMemBinPacker");
   const int J = jobs->n, O = offers->n, U = users->n_users;
   const int NC = params->num_considerable;
-  if (J < 0 || O < 0 || U <= 0 || n_ranked < 0 || NC < 0 || max_ports < 0)
-    return set_err(pool, COOK_E_BADARG, "cook_match: bad sizes");
+  int32_t rc = check_match_inputs(pool, "cook_match", offers, groups, users, params, max_ports,
+                                  !params->reuse_resident && n_ranked > 0 && NC > 0, jobs->novel_off, jobs->group_off);
+  if (rc != COOK_OK) return rc;
+  if (J < 0 || n_ranked < 0) return set_err(pool, COOK_E_BADARG, "cook_match: bad sizes");
   if (out_stats) memset(out_stats, 0, sizeof(*out_stats));
   if (n_ranked == 0 || NC == 0) return COOK_OK;
   if (!params->reuse_resident) {   // index columns are dereferenced on the device: check them here
@@ -2767,20 +2776,9 @@ extern "C" int32_t cook_match(cook_pool* pool, const int32_t* ranked_idx, int32_
     if (!idx_in_range(jobs->user, J, 0, U)) return set_err(pool, COOK_E_BADARG, "cook_match: jobs.user out of range");
     if (jobs->attr_off && !idx_in_range(jobs->attr_col, jobs->attr_off[J], 0, std::max(1, offers->n_attr_cols)))
       return set_err(pool, COOK_E_BADARG, "cook_match: jobs.attr_col out of range");
-    if (!offers->name_rank && O > 0) return set_err(pool, COOK_E_BADARG, "cook_match: offers.name_rank required");
-    if (groups && !idx_in_range(groups->attr_col, groups->n_groups, -1, std::max(1, offers->n_attr_cols)))
-      return set_err(pool, COOK_E_BADARG, "cook_match: groups.attr_col out of range");
-    const bool grouped = groups && groups->n_groups && jobs->group_off;
-    if ((jobs->novel_off || offers->reserved || grouped) && !offers->hostname_id)
-      return set_err(pool, COOK_E_BADARG, "cook_match: hostname_id column required by constraints");
-    if (grouped && (!groups->cot_off || !groups->kind)) return set_err(pool, COOK_E_BADARG, "cook_match: incomplete cook_groups");
   }
   CK(pool, cudaSetDevice(pool->device));
-  if (!pool->match_plan) {
-    pool->match_plan = new MatchPlan();
-    pool->match_plan_free = plan_free;
-  }
-  MatchPlan* mp = static_cast<MatchPlan*>(pool->match_plan);
+  MatchPlan* mp = plan_of(pool);
   const bool reuse = params->reuse_resident && mp->valid && mp->J == J && mp->O == O && mp->U == U &&
                      mp->n_ranked == n_ranked && mp->NC == NC && mp->max_ports == max_ports;
   if (params->reuse_resident && !reuse)
@@ -2788,49 +2786,16 @@ extern "C" int32_t cook_match(cook_pool* pool, const int32_t* ranked_idx, int32_
                    "cook_match: reuse_resident set but no matching resident inputs on this handle");
   CK(pool, cudaEventRecord(pool->ev[0], pool->stream));
   if (!reuse) {
-    int32_t rc = build_plan(pool, mp, ranked_idx, n_ranked, jobs, offers, groups, users, pool_quota,
-                            params, max_ports);
-    if (rc != COOK_OK) { mp->valid = false; return rc; }
+    mp->valid = false;
+    JobShape sh;
+    rc = host_shape(pool, jobs, groups ? groups->n_groups : 0, &sh);
+    if (rc == COOK_OK)
+      rc = match_build(pool, ranked_idx, n_ranked, sh, offers, groups, users, pool_quota, params, max_ports, nullptr);
+    if (rc != COOK_OK) return rc;
   }
-  return run_plan(pool, mp, out_considerable, out_assign, out_ports, out_fail_reason, out_stats, !reuse,
-                  params->max_ctas);
+  return match_run(pool, out_considerable, nullptr, out_assign, out_ports, out_fail_reason, out_stats, !reuse,
+                   params->max_ctas);
 }
-
-// cook_match over jobs whose columns live on the device (state.cu): the same checks of the offer and
-// group tables, the same plan with the job columns carved for `fill`, the same run.
-int32_t match_device_jobs(cook_pool* pool, int32_t n_ranked, DevJobSpec* dj,
-                          const std::function<int32_t(const DevJobCols&, int*)>& fill,
-                          const cook_offers_soa* offers, const cook_groups* groups, const cook_user_table* users,
-                          const cook_pool_quota* pool_quota, const cook_match_params* params, int64_t* out_job_id,
-                          int32_t* out_assign, int32_t* out_ports, int32_t max_ports, uint8_t* out_fail_reason,
-                          cook_match_stats* out_stats) {
-  const int O = offers->n, NC = params->num_considerable;
-  if (out_stats) memset(out_stats, 0, sizeof(*out_stats));
-  if (n_ranked == 0 || NC == 0) return COOK_OK;
-  if (!offers->name_rank && O > 0) return set_err(pool, COOK_E_BADARG, "cook_state_match: offers.name_rank required");
-  if (groups && !idx_in_range(groups->attr_col, groups->n_groups, -1, std::max(1, offers->n_attr_cols)))
-    return set_err(pool, COOK_E_BADARG, "cook_state_match: groups.attr_col out of range");
-  const bool grouped = groups && groups->n_groups && dj->n_group;
-  if ((dj->n_novel || offers->reserved || grouped) && !offers->hostname_id)
-    return set_err(pool, COOK_E_BADARG, "cook_state_match: hostname_id column required by constraints");
-  if (grouped && (!groups->cot_off || !groups->kind)) return set_err(pool, COOK_E_BADARG, "cook_state_match: incomplete cook_groups");
-  CK(pool, cudaSetDevice(pool->device));
-  if (!pool->match_plan) {
-    pool->match_plan = new MatchPlan();
-    pool->match_plan_free = plan_free;
-  }
-  MatchPlan* mp = static_cast<MatchPlan*>(pool->match_plan);
-  CK(pool, cudaEventRecord(pool->ev[0], pool->stream));
-  int32_t rc = build_plan(pool, mp, nullptr, n_ranked, nullptr, offers, groups, users, pool_quota, params, max_ports, dj);
-  int fill_launches = 0;
-  if (rc == COOK_OK) rc = fill(dj->out, &fill_launches);
-  if (rc != COOK_OK) { mp->valid = false; return rc; }
-  rc = run_plan(pool, mp, nullptr, out_assign, out_ports, out_fail_reason, out_stats, true, params->max_ctas, out_job_id);
-  pool->phase[COOK_PHASE_MATCH].n_launches += fill_launches;
-  if (out_stats) out_stats->n_launches += fill_launches;
-  return rc;
-}
-
 
 // §8e: usage delta of this handle's last match round (device) -> one all-gather -> host.
 // the per-user usage delta of `src`'s last match round into d_local[n_pad] (zeroed by the caller), on stream st

@@ -21,17 +21,6 @@
 
 namespace {
 
-struct TaskCols {
-  const int32_t* user;
-  const int32_t* prio;
-  const int64_t* start;
-  const int64_t* tid;
-  const int64_t* jid;
-  const double* cpus;
-  const double* mem;
-  const double* gpus;
-};
-
 __global__ void scatter_dru_kernel(const int32_t* __restrict__ idx, const double* __restrict__ dru_at,
                                    int n, double* __restrict__ dru_task) {
   int p = blockIdx.x * blockDim.x + threadIdx.x;
@@ -301,17 +290,17 @@ extern "C" int32_t cook_rank(cook_pool* pool, const cook_tasks_soa* running,
                              int32_t* out_order, int32_t* out_order_n) {
   if (!pool) return COOK_E_BADARG;
   if (!running || !pending || !out_ranked_idx) return set_err(pool, COOK_E_BADARG, "cook_rank: null argument");
-  return rank_impl(pool, running, pending, nullptr, users, pool_quota, group_quota, group_usage, params, out_ranked_idx,
-                   out_n, out_dru, out_order, out_order_n, nullptr);
+  return rank_impl(pool, running->n, pending->n, running, pending, nullptr, users, pool_quota, group_quota, group_usage,
+                   params, out_ranked_idx, out_n, out_dru, out_order, out_order_n, nullptr);
 }
 
-int32_t rank_impl(cook_pool* pool, const cook_tasks_soa* running, const cook_tasks_soa* pending, const DevTasks* dev,
-                  const cook_user_table* users, const cook_pool_quota* pool_quota, const cook_pool_quota* group_quota,
-                  const double* group_usage, const cook_rank_params* params, int32_t* out_ranked_idx, int32_t* out_n,
-                  double* out_dru, int32_t* out_order, int32_t* out_order_n,
-                  const std::function<int32_t(const int32_t*, const int32_t*, int*)>* on_queue) {
+int32_t rank_impl(cook_pool* pool, int R, int J, const cook_tasks_soa* running, const cook_tasks_soa* pending,
+                  const TaskCols* dev, const cook_user_table* users, const cook_pool_quota* pool_quota,
+                  const cook_pool_quota* group_quota, const double* group_usage, const cook_rank_params* params,
+                  int32_t* out_ranked_idx, int32_t* out_n, double* out_dru, int32_t* out_order, int32_t* out_order_n,
+                  RankQueue* queue) {
   if (!users || !params || !out_n) return set_err(pool, COOK_E_BADARG, "cook_rank: null argument");
-  const int R = dev ? dev->R : running->n, J = dev ? dev->J : pending->n, N = R + J, U = users->n_users;
+  const int N = R + J, U = users->n_users;
   if (R < 0 || J < 0 || U <= 0) return set_err(pool, COOK_E_BADARG, "cook_rank: bad sizes");
   // device rows had their user codes checked when they entered (state.cu)
   if (!dev && (!idx_in_range(running->user, R, 0, U) || !idx_in_range(pending->user, J, 0, U)))
@@ -334,7 +323,7 @@ int32_t rank_impl(cook_pool* pool, const cook_tasks_soa* running, const cook_tas
   int64_t h2d = 0, d2h = 0;
   const cudaError_t carved = carve(pool->arena, st, pool->ev[8], &h2d, [&](Carve& c) {
     if (dev) {
-      t = TaskCols{dev->user, dev->prio, dev->start, dev->tid, dev->jid, dev->cpus, dev->mem, dev->gpus};
+      t = *dev;
     } else {
       t.user = c.cat(running->user, R, pending->user, J);
       t.prio = c.cat(running->priority, R, pending->priority, J);
@@ -427,10 +416,7 @@ int32_t rank_impl(cook_pool* pool, const cook_tasks_soa* running, const cook_tas
     nl++;
   }
   CK(pool, cudaGetLastError());
-  if (on_queue) {
-    const int32_t rc = (*on_queue)(d_out_ranked, qa.out_n, &nl);
-    if (rc != COOK_OK) return rc;
-  }
+  if (queue) *queue = RankQueue{d_out_ranked, qa.out_n};
   CK(pool, cudaEventRecord(pool->ev[10], st));
   int32_t h_counters[2] = {0, 0};
   CK(pool, download(h_counters, d_counters, 2, st, &d2h));

@@ -7,9 +7,10 @@
 // copies, a live flag and a generation stamp per slot, and one append-only arena per CSR list with a
 // per-slot (off, len), compacted once its dead entries outnumber the live ones.
 // Rank and match gather dense columns from the tables with fold.cuh's compaction and order-wide scan and
-// then run cook_rank's and cook_match's own code on them (rank_impl, match_device_jobs).  The ranked
-// queue stays on the device as (slot, generation) pairs; a match keeps the entries whose slot still holds
-// that generation, so a job removed or replaced since the rank leaves the queue.
+// run cook_rank's and cook_match's own code on them: rank_impl over the gathered task columns, and the
+// match plan's build, the gathers into the job columns it carved, then its run.  The ranked queue stays
+// on the device as (slot, generation) pairs; a match keeps the entries whose slot still holds that
+// generation, so a job removed or replaced since the rank leaves the queue.
 #include <algorithm>
 #include <map>
 #include <unordered_map>
@@ -114,38 +115,36 @@ __global__ void csr_gather_kernel(OrderScan<int, 1> os, const int32_t* m_slot, i
 }
 
 // ---- rank: live rows -> dense task columns (running first), compacted in slot order
-struct DenseTasks {
-  int32_t* user; int32_t* prio; int64_t* start; int64_t* tid; int64_t* jid; double* cpus; double* mem; double* gpus;
-  int32_t* pslot;   // dense pending index -> slot
-};
 struct RunningRows {
-  void* const* col; DenseTasks o;
+  void* const* col; TaskCols o;
   __device__ bool keep(int i) const { return static_cast<const uint8_t*>(col[R_LIVE])[i]; }
   __device__ void emit(int i, int d) const {
-    o.user[d] = static_cast<const int32_t*>(col[R_USER])[i];
-    o.prio[d] = static_cast<const int32_t*>(col[R_PRIO])[i];
-    o.start[d] = static_cast<const int64_t*>(col[R_START])[i];
-    o.tid[d] = static_cast<const int64_t*>(col[R_TID])[i];
-    o.jid[d] = static_cast<const int64_t*>(col[R_JID])[i];
-    o.cpus[d] = static_cast<const double*>(col[R_CPUS])[i];
-    o.mem[d] = static_cast<const double*>(col[R_MEM])[i];
-    o.gpus[d] = static_cast<const double*>(col[R_GPUS])[i];
+    writable(o.user)[d] = static_cast<const int32_t*>(col[R_USER])[i];
+    writable(o.prio)[d] = static_cast<const int32_t*>(col[R_PRIO])[i];
+    writable(o.start)[d] = static_cast<const int64_t*>(col[R_START])[i];
+    writable(o.tid)[d] = static_cast<const int64_t*>(col[R_TID])[i];
+    writable(o.jid)[d] = static_cast<const int64_t*>(col[R_JID])[i];
+    writable(o.cpus)[d] = static_cast<const double*>(col[R_CPUS])[i];
+    writable(o.mem)[d] = static_cast<const double*>(col[R_MEM])[i];
+    writable(o.gpus)[d] = static_cast<const double*>(col[R_GPUS])[i];
   }
 };
 struct PendingRows {
-  void* const* col; DenseTasks o; int R;
+  void* const* col; TaskCols o;
+  int32_t* pslot;   // dense pending index -> slot
+  int R;
   __device__ bool keep(int i) const { return static_cast<const uint8_t*>(col[P_LIVE])[i]; }
   __device__ void emit(int i, int d) const {
-    o.pslot[d] = i;
+    pslot[d] = i;
     d += R;
-    o.user[d] = static_cast<const int32_t*>(col[P_USER])[i];
-    o.prio[d] = static_cast<const int32_t*>(col[P_PRIO])[i];
-    o.start[d] = INT64_MAX;   // a pending job's synthetic task (tools.clj:582-588)
-    o.tid[d] = -1;
-    o.jid[d] = static_cast<const int64_t*>(col[P_JID])[i];
-    o.cpus[d] = static_cast<const double*>(col[P_CPUS])[i];
-    o.mem[d] = static_cast<const double*>(col[P_MEM])[i];
-    o.gpus[d] = static_cast<const double*>(col[P_GPUS])[i];
+    writable(o.user)[d] = static_cast<const int32_t*>(col[P_USER])[i];
+    writable(o.prio)[d] = static_cast<const int32_t*>(col[P_PRIO])[i];
+    writable(o.start)[d] = INT64_MAX;   // a pending job's synthetic task (tools.clj:582-588)
+    writable(o.tid)[d] = -1;
+    writable(o.jid)[d] = static_cast<const int64_t*>(col[P_JID])[i];
+    writable(o.cpus)[d] = static_cast<const double*>(col[P_CPUS])[i];
+    writable(o.mem)[d] = static_cast<const double*>(col[P_MEM])[i];
+    writable(o.gpus)[d] = static_cast<const double*>(col[P_GPUS])[i];
   }
 };
 
@@ -165,28 +164,29 @@ struct QueueLive {
   __device__ void emit(int k, int d) const { m_slot[d] = q_slot[k]; }
 };
 
-// row d of the match is slot m_slot[d]: its columns into the plan's (ranked[d] = d)
-__global__ void fill_rows_kernel(DevJobCols o, void* const* col, const int32_t* m_slot, int n) {
+// row d of the match is slot m_slot[d]: its columns into the plan's
+__global__ void fill_rows_kernel(MatchRows r, void* const* col, const int32_t* m_slot, int n) {
   const int d = blockIdx.x * blockDim.x + threadIdx.x;
   if (d >= n) return;
   const int s = m_slot[d];
-  o.ranked[d] = d;
-  o.user[d] = static_cast<const int32_t*>(col[P_USER])[s];
-  o.cpus[d] = static_cast<const double*>(col[P_CPUS])[s];
-  o.mem[d] = static_cast<const double*>(col[P_MEM])[s];
-  o.gpus[d] = static_cast<const double*>(col[P_GPUS])[s];
-  o.job_id[d] = static_cast<const int64_t*>(col[P_JID])[s];
-  if (o.ports) o.ports[d] = static_cast<const int32_t*>(col[P_PORTS])[s];
-  if (o.allowed) o.allowed[d] = static_cast<const uint8_t*>(col[P_ALLOWED])[s];
-  if (o.plugin) o.plugin[d] = static_cast<const uint8_t*>(col[P_PLUGIN])[s];
-  if (o.gpu_model) o.gpu_model[d] = static_cast<const int32_t*>(col[P_GPU_MODEL])[s];
+  const JobDev& o = r.jb;
+  r.ranked[d] = d;
+  writable(o.user)[d] = static_cast<const int32_t*>(col[P_USER])[s];
+  writable(o.cpus)[d] = static_cast<const double*>(col[P_CPUS])[s];
+  writable(o.mem)[d] = static_cast<const double*>(col[P_MEM])[s];
+  writable(o.gpus)[d] = static_cast<const double*>(col[P_GPUS])[s];
+  r.job_id[d] = static_cast<const int64_t*>(col[P_JID])[s];
+  if (o.ports) writable(o.ports)[d] = static_cast<const int32_t*>(col[P_PORTS])[s];
+  if (o.allowed) writable(o.allowed)[d] = static_cast<const uint8_t*>(col[P_ALLOWED])[s];
+  if (o.plugin) writable(o.plugin)[d] = static_cast<const uint8_t*>(col[P_PLUGIN])[s];
+  if (o.gpu_model) writable(o.gpu_model)[d] = static_cast<const int32_t*>(col[P_GPU_MODEL])[s];
   if (o.disk_request) {
-    o.disk_request[d] = static_cast<const double*>(col[P_DISK_REQ])[s];
-    o.disk_type[d] = static_cast<const int32_t*>(col[P_DISK_TYPE])[s];
+    writable(o.disk_request)[d] = static_cast<const double*>(col[P_DISK_REQ])[s];
+    writable(o.disk_type)[d] = static_cast<const int32_t*>(col[P_DISK_TYPE])[s];
   }
-  if (o.est_end_ms) o.est_end_ms[d] = static_cast<const int64_t*>(col[P_EST])[s];
-  if (o.ckpt_location) o.ckpt_location[d] = static_cast<const int32_t*>(col[P_CKPT])[s];
-  if (o.reserved_host) o.reserved_host[d] = static_cast<const int32_t*>(col[P_RESERVED])[s];
+  if (o.est_end_ms) writable(o.est_end_ms)[d] = static_cast<const int64_t*>(col[P_EST])[s];
+  if (o.ckpt_location) writable(o.ckpt_location)[d] = static_cast<const int32_t*>(col[P_CKPT])[s];
+  if (o.reserved_host) writable(o.reserved_host)[d] = static_cast<const int32_t*>(col[P_RESERVED])[s];
 }
 
 // ---- host side
@@ -200,18 +200,6 @@ struct PendingInfo {
   std::vector<int32_t> groups, attr_cols;
 };
 
-template <class T>
-cudaError_t ensure(T*& p, size_t& cap, size_t n) {   // scratch: contents are not kept
-  if (n <= cap && p) return cudaSuccess;
-  if (p) cudaFree(p);
-  p = nullptr;
-  const size_t want = std::max(n, 2 * cap) + 1;
-  cap = 0;
-  cudaError_t e = cudaMalloc(&p, want * sizeof(T));
-  if (e == cudaSuccess) cap = want;
-  return e;
-}
-
 struct Table {
   int ncol = 0;
   const int* sz = nullptr;
@@ -221,6 +209,8 @@ struct Table {
   std::unordered_map<int64_t, int32_t> slot_of;
   std::vector<int32_t> free;
 
+  template <class T>
+  const T* at(int k) const { return static_cast<const T*>(col[k]); }
   // capacity >= n: new columns, zeroed, the old contents copied (device to device)
   cudaError_t grow(int32_t n, cudaStream_t st) {
     if (n <= cap) return cudaSuccess;
@@ -300,19 +290,13 @@ struct PoolState {
   std::map<int32_t, int64_t> users_p, users_r, attr_cols, groups;   // code -> live uses
   int64_t nflag[F_N] = {};
   Arena stage;                        // one batch's uploads
-  // scratch
-  int32_t* blk = nullptr; size_t blk_cap = 0;
+  Arena scratch;                      // one call's device buffers
+  Arena queue;                        // the ranked queue, carved by rank only: it lives until the match
   int32_t* counters = nullptr;        // [0] running rows, [1] pending rows, [2] live queue entries
   GridFlag* gf0 = nullptr;            // stays zero: integer scans are always exact
-  int32_t* scan_part = nullptr; size_t scan_part_cap = 0;
-  int32_t* scan_tile = nullptr; size_t scan_tile_cap = 0;
-  // rank: dense columns, and the resident queue
-  DenseTasks dense = {};
-  size_t dense_cap = 0;
-  int32_t* q_slot = nullptr; uint32_t* q_gen = nullptr; int64_t* q_jid = nullptr; size_t q_cap = 0;
+  const int32_t* q_slot = nullptr; const uint32_t* q_gen = nullptr; const int64_t* q_jid = nullptr;
   int32_t n_q = 0;
   bool ranked = false;
-  int32_t* m_slot = nullptr; size_t m_cap = 0;
 
   PoolState() {
     pend.ncol = P_NCOL; pend.sz = P_SZ;
@@ -322,12 +306,9 @@ struct PoolState {
   void release() {
     pend.release(); run.release();
     for (auto& l : lists) l.release();
-    stage.release();
-    for (void* p : {(void*)blk, (void*)counters, (void*)gf0, (void*)scan_part, (void*)scan_tile, (void*)dense.user,
-                    (void*)dense.prio, (void*)dense.start, (void*)dense.tid, (void*)dense.jid, (void*)dense.cpus,
-                    (void*)dense.mem, (void*)dense.gpus, (void*)dense.pslot, (void*)q_slot, (void*)q_gen, (void*)q_jid,
-                    (void*)m_slot})
-      if (p) cudaFree(p);
+    stage.release(); scratch.release(); queue.release();
+    if (counters) cudaFree(counters);
+    if (gf0) cudaFree(gf0);
   }
   void add_pending(int32_t slot, const PendingInfo& pi, int64_t sign) {
     count_add(users_p, pi.user, sign);
@@ -377,10 +358,11 @@ int32_t compact_lists(cook_pool* pool, PoolState* S, cudaStream_t st, int* nl) {
     if (A.live > 0 && n > 0) {
       for (int i = 0; i < A.k; i++)
         if (!A.alt[i]) CK(pool, cudaMalloc(&A.alt[i], sizeof(int32_t) * std::max<int64_t>(A.cap, 1)));
-      const int nb = (n + OS_TILE - 1) / OS_TILE;
-      CK(pool, ensure(S->scan_part, S->scan_part_cap, (size_t)n));
-      CK(pool, ensure(S->scan_tile, S->scan_tile_cap, (size_t)nb + 1));
-      const OrderScan<int, 1> os{{S->scan_part}, {S->scan_tile}};
+      OrderScan<int, 1> os;
+      CK(pool, carve(S->scratch, st, nullptr, nullptr, [&](Carve& c) {
+        os.part[0] = c.take<int32_t>(n);
+        os.tile[0] = c.take<int32_t>((n + OS_TILE - 1) / OS_TILE + 1);
+      }));
       const uint8_t* live = static_cast<const uint8_t*>(S->pend.col[P_LIVE]);
       int32_t* off = static_cast<int32_t*>(S->pend.col[loff[l]]);
       const int32_t* len = static_cast<const int32_t*>(S->pend.col[llen[l]]);
@@ -615,62 +597,50 @@ extern "C" int32_t cook_state_rank(cook_pool* pool, const cook_user_table* users
   S->ranked = false;
   CK(pool, cudaEventRecord(pool->ev[7], st));
   int nl = 0;
+  TaskCols dt = {};
+  int32_t* pslot = nullptr;
   if (N > 0) {
-    if (N > S->dense_cap) {
-      size_t c = 0;
-      DenseTasks& o = S->dense;
-      for (void** p : {(void**)&o.user, (void**)&o.prio, (void**)&o.start, (void**)&o.tid, (void**)&o.jid, (void**)&o.cpus,
-                       (void**)&o.mem, (void**)&o.gpus, (void**)&o.pslot}) {
-        if (*p) cudaFree(*p);
-        *p = nullptr;
-      }
-      c = std::max(N, 2 * S->dense_cap);
-      CK(pool, cudaMalloc(&o.user, c * 4)); CK(pool, cudaMalloc(&o.prio, c * 4));
-      CK(pool, cudaMalloc(&o.start, c * 8)); CK(pool, cudaMalloc(&o.tid, c * 8)); CK(pool, cudaMalloc(&o.jid, c * 8));
-      CK(pool, cudaMalloc(&o.cpus, c * 8)); CK(pool, cudaMalloc(&o.mem, c * 8)); CK(pool, cudaMalloc(&o.gpus, c * 8));
-      CK(pool, cudaMalloc(&o.pslot, c * 4));
-      S->dense_cap = c;
-    }
-    CK(pool, ensure(S->blk, S->blk_cap, (size_t)std::max(S->pend.hw, S->run.hw) / CP_BLOCK + 2));
-    if (R) compact(RunningRows{S->run.d_col, S->dense}, S->run.hw, nullptr, S->blk, S->counters, R, st, &nl);
-    if (J) compact(PendingRows{S->pend.d_col, S->dense, R}, S->pend.hw, nullptr, S->blk, S->counters + 1, J, st, &nl);
+    int32_t* blk = nullptr;
+    CK(pool, carve(S->scratch, st, nullptr, nullptr, [&](Carve& c) {
+      dt.user = c.take<int32_t>(N); dt.prio = c.take<int32_t>(N);
+      dt.start = c.take<int64_t>(N); dt.tid = c.take<int64_t>(N); dt.jid = c.take<int64_t>(N);
+      dt.cpus = c.take<double>(N); dt.mem = c.take<double>(N); dt.gpus = c.take<double>(N);
+      pslot = c.take<int32_t>(J);
+      blk = c.take<int32_t>((size_t)std::max(S->pend.hw, S->run.hw) / CP_BLOCK + 2);
+    }));
+    if (R) compact(RunningRows{S->run.d_col, dt}, S->run.hw, nullptr, blk, S->counters, R, st, &nl);
+    if (J) compact(PendingRows{S->pend.d_col, dt, pslot, R}, S->pend.hw, nullptr, blk, S->counters + 1, J, st, &nl);
     CK(pool, cudaGetLastError());
     CK(pool, cudaEventRecord(pool->ev[23], st));
-    if ((size_t)J + 1 > S->q_cap) {
-      if (S->q_slot) cudaFree(S->q_slot);
-      if (S->q_gen) cudaFree(S->q_gen);
-      if (S->q_jid) cudaFree(S->q_jid);
-      S->q_slot = nullptr; S->q_gen = nullptr; S->q_jid = nullptr; S->q_cap = 0;
-      const size_t c = std::max<size_t>(J + 1, 2 * S->q_cap);
-      CK(pool, cudaMalloc(&S->q_slot, c * 4)); CK(pool, cudaMalloc(&S->q_gen, c * 4)); CK(pool, cudaMalloc(&S->q_jid, c * 8));
-      S->q_cap = c;
-    }
   }
-  const DenseTasks& o = S->dense;
-  const DevTasks dt{R, J, o.user, o.prio, o.start, o.tid, o.jid, o.cpus, o.mem, o.gpus};
-  const uint32_t* gen = static_cast<const uint32_t*>(S->pend.col[P_GEN]);
-  const int64_t* jid = static_cast<const int64_t*>(S->pend.col[P_JID]);
-  const std::function<int32_t(const int32_t*, const int32_t*, int*)> on_queue =
-      [&](const int32_t* d_ranked, const int32_t* d_n, int* launches) -> int32_t {
-    if (J == 0) return COOK_OK;   // running tasks only: the queue is empty
-    queue_kernel<<<(J + 255) / 256, 256, 0, st>>>(d_ranked, d_n, o.pslot, gen, jid, S->q_slot, S->q_gen, S->q_jid);
-    (*launches)++;
-    CK(pool, cudaGetLastError());
-    return COOK_OK;
-  };
   int32_t n = 0;
-  const int32_t rc = rank_impl(pool, nullptr, nullptr, &dt, users, pool_quota, group_quota, group_usage, params, nullptr,
-                               &n, nullptr, nullptr, nullptr, &on_queue);
+  RankQueue rq = {};
+  const int32_t rc = rank_impl(pool, R, J, nullptr, nullptr, &dt, users, pool_quota, group_quota, group_usage, params,
+                               nullptr, &n, nullptr, nullptr, nullptr, &rq);
   if (rc != COOK_OK) return rc;
   cook_phase_stats& ps = pool->phase[COOK_PHASE_RANK];
   if (N > 0) ps.ms_device += ev_ms(pool->ev[7], pool->ev[23]);   // the gathering of the live rows
-  ps.n_launches += nl;
-  if (out_ranked_job_id && n > 0) {
-    int64_t d2h = 0;
-    CK(pool, download(out_ranked_job_id, S->q_jid, n, st, &d2h));
+  if (J > 0) {   // the ranked list as (slot, generation) pairs, while it is still in the pool's arena
+    int32_t* q_slot = nullptr; uint32_t* q_gen = nullptr; int64_t* q_jid = nullptr;
+    CK(pool, carve(S->queue, st, nullptr, nullptr, [&](Carve& c) {
+      q_slot = c.take<int32_t>(J + 1); q_gen = c.take<uint32_t>(J + 1); q_jid = c.take<int64_t>(J + 1);
+    }));
+    S->q_slot = q_slot; S->q_gen = q_gen; S->q_jid = q_jid;
+    CK(pool, cudaEventRecord(pool->ev[7], st));
+    queue_kernel<<<(J + 255) / 256, 256, 0, st>>>(rq.ranked, rq.n, pslot, S->pend.at<uint32_t>(P_GEN),
+                                                  S->pend.at<int64_t>(P_JID), q_slot, q_gen, q_jid);
+    nl++;
+    CK(pool, cudaGetLastError());
+    CK(pool, cudaEventRecord(pool->ev[23], st));
+    if (out_ranked_job_id && n > 0) {
+      int64_t d2h = 0;
+      CK(pool, download(out_ranked_job_id, S->q_jid, n, st, &d2h));
+      ps.d2h_bytes += d2h;
+    }
     CK(pool, cudaStreamSynchronize(st));
-    ps.d2h_bytes += d2h;
+    ps.ms_device += ev_ms(pool->ev[7], pool->ev[23]);
   }
+  ps.n_launches += nl;
   S->n_q = n;
   S->ranked = true;
   *out_n = n;
@@ -687,13 +657,37 @@ extern "C" int32_t cook_state_match(cook_pool* pool, const cook_offers_soa* offe
     return set_err(pool, COOK_E_BADARG, "cook_state_match: null argument");
   if (params->reuse_resident)
     return set_err(pool, COOK_E_BADARG, "cook_state_match: reuse_resident does not apply: the queue's rows are resident");
-  if (params->good_enough_fitness < 1.0)
-    return set_err(pool, COOK_E_BADARG, "cook_state_match: good_enough_fitness < 1.0 is not supported (see cook_match)");
-  if (params->fitness_kind != 0) return set_err(pool, COOK_E_UNSUPPORTED_CONSTRAINT, "cook_state_match: only cpuMemBinPacker");
-  const int O = offers->n, U = users->n_users, NC = params->num_considerable;
-  if (O < 0 || U <= 0 || NC < 0 || max_ports < 0) return set_err(pool, COOK_E_BADARG, "cook_state_match: bad sizes");
   PoolState* S = static_cast<PoolState*>(pool->state);
+  const int NC = params->num_considerable;
+  cudaStream_t st = pool->stream;
+  // ---- the queue minus what left it since the rank.  This comes first: as in cook_match, the offer and
+  // group tables are checked only when some row is left to match.
+  int nl = 0;
+  int32_t n = 0;
+  int64_t d2h = 0;
+  int32_t* m_slot = nullptr;
+  OrderScan<int, 1> os;
+  if (S && S->ranked && S->n_q > 0 && NC > 0) {
+    CK(pool, cudaSetDevice(pool->device));
+    const int nq = S->n_q;
+    int32_t* blk = nullptr;
+    CK(pool, carve(S->scratch, st, nullptr, nullptr, [&](Carve& c) {
+      m_slot = c.take<int32_t>(nq);
+      blk = c.take<int32_t>((size_t)nq / CP_BLOCK + 2);
+      os.part[0] = c.take<int32_t>(nq);
+      os.tile[0] = c.take<int32_t>((nq + OS_TILE - 1) / OS_TILE + 1);
+    }));
+    const QueueLive ql{S->q_slot, S->q_gen, S->pend.at<uint8_t>(P_LIVE), S->pend.at<uint32_t>(P_GEN), m_slot};
+    compact(ql, nq, nullptr, blk, S->counters + 2, nq, st, &nl);
+    CK(pool, cudaGetLastError());
+    CK(pool, download(&n, S->counters + 2, 1, st, &d2h));
+    CK(pool, cudaStreamSynchronize(st));
+  }
+  int32_t rc = check_match_inputs(pool, "cook_state_match", offers, groups, users, params, max_ports, n > 0,
+                                  S && S->lists[L_NOVEL].live > 0, S && S->lists[L_GROUP].live > 0);
+  if (rc != COOK_OK) return rc;
   if (!S || !S->ranked) return set_err(pool, COOK_E_BADARG, "cook_state_match: no cook_state_rank on this handle yet");
+  const int U = users->n_users;
   if (count_max(S->users_p) >= U) return set_err(pool, COOK_E_BADARG, "cook_state_match: a pending row's user code is >= n_users");
   if (count_max(S->attr_cols) >= std::max(1, offers->n_attr_cols))
     return set_err(pool, COOK_E_BADARG, "cook_state_match: a pending row's attribute column is >= n_attr_cols");
@@ -701,57 +695,56 @@ extern "C" int32_t cook_state_match(cook_pool* pool, const cook_offers_soa* offe
   if (G > 0 && count_max(S->groups) >= G)
     return set_err(pool, COOK_E_BADARG, "cook_state_match: a pending row's group code is >= n_groups");
   if (out_stats) memset(out_stats, 0, sizeof(*out_stats));
-  if (S->n_q == 0 || NC == 0) return COOK_OK;
-  CK(pool, cudaSetDevice(pool->device));
-  cudaStream_t st = pool->stream;
-  // ---- the queue minus what left it since the rank
-  int nl = 0;
-  CK(pool, ensure(S->m_slot, S->m_cap, (size_t)S->n_q));
-  CK(pool, ensure(S->blk, S->blk_cap, (size_t)S->n_q / CP_BLOCK + 2));
-  const QueueLive ql{S->q_slot, S->q_gen, static_cast<const uint8_t*>(S->pend.col[P_LIVE]),
-                     static_cast<const uint32_t*>(S->pend.col[P_GEN]), S->m_slot};
-  compact(ql, S->n_q, nullptr, S->blk, S->counters + 2, S->n_q, st, &nl);
-  CK(pool, cudaGetLastError());
-  int32_t n = 0;
-  int64_t d2h = 0;
-  CK(pool, download(&n, S->counters + 2, 1, st, &d2h));
-  CK(pool, cudaStreamSynchronize(st));
   if (n == 0) return COOK_OK;
-  // ---- what the rows hold, from the host-side counts
-  std::vector<int32_t> gp_off(G + 1, 0);
-  for (const auto& kv : S->groups) if (kv.first < G) gp_off[kv.first + 1] = (int32_t)kv.second;
-  for (int g = 0; g < G; g++) gp_off[g + 1] += gp_off[g];
-  DevJobSpec dj;
-  memset(&dj, 0, sizeof(dj));
-  dj.ports = S->nflag[F_PORTS] > 0; dj.allowed = S->nflag[F_NOT_ALLOWED] > 0; dj.plugin = S->nflag[F_NOT_PLUGIN] > 0;
-  dj.gpu_model = S->nflag[F_GPU_MODEL] > 0; dj.disk = S->nflag[F_DISK] > 0; dj.est_end = S->nflag[F_EST] > 0;
-  dj.ckpt = S->nflag[F_CKPT] > 0; dj.reserved = S->nflag[F_RESERVED] > 0; dj.any_gpus = S->nflag[F_GPUS] > 0;
-  dj.n_novel = S->lists[L_NOVEL].live; dj.n_attr = S->lists[L_ATTR].live; dj.n_group = S->lists[L_GROUP].live;
-  dj.gp_off = gp_off.data();
-  const auto fill = [&](const DevJobCols& o, int* launches) -> int32_t {
-    fill_rows_kernel<<<(n + 255) / 256, 256, 0, st>>>(o, S->pend.d_col, S->m_slot, n);
-    (*launches)++;
-    const int nb = (n + OS_TILE - 1) / OS_TILE;
-    CK(pool, ensure(S->scan_part, S->scan_part_cap, (size_t)n));
-    CK(pool, ensure(S->scan_tile, S->scan_tile_cap, (size_t)nb + 1));
-    const OrderScan<int, 1> os{{S->scan_part}, {S->scan_tile}};
-    const int loff[3] = {P_NOFF, P_AOFF, P_GOFF};
-    int32_t* doff[3] = {o.novel_off, o.attr_off, o.group_off};
-    int32_t* dst[3][2] = {{o.novel_host, nullptr}, {o.attr_col, o.attr_val}, {o.group_idx, nullptr}};
-    for (int l = 0; l < 3; l++) {
-      if (!doff[l]) continue;
-      const int32_t* off = static_cast<const int32_t*>(S->pend.col[loff[l]]);
-      const int32_t* len = static_cast<const int32_t*>(S->pend.col[loff[l] + 1]);
-      order_scan(os, RowLen{S->m_slot, len}, n, S->gf0, st, launches);
-      csr_gather_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, S->m_slot, n, off, len, S->lists[l].v[0], S->lists[l].v[1],
-                                                     doff[l], dst[l][0], dst[l][1]);
-      (*launches)++;
-    }
-    CK(pool, cudaGetLastError());
-    return COOK_OK;
-  };
-  const int32_t rc = match_device_jobs(pool, n, &dj, fill, offers, groups, users, pool_quota, params, out_considerable_job_id,
-                                       out_assign, out_ports, max_ports, out_fail_reason, out_stats);
+  // ---- what the rows hold, from the host-side counts: the resident columns of the kinds some live row
+  // holds a non-absent value of
+  JobShape sh;
+  sh.J = n;
+  sh.job_ids = true;
+  const Table& P = S->pend;
+  const ListArena* L = S->lists;
+  const auto has = [&](int f) { return S->nflag[f] > 0; };
+  JobDev& c = sh.cols;
+  c.user = P.at<int32_t>(P_USER); c.cpus = P.at<double>(P_CPUS); c.mem = P.at<double>(P_MEM);
+  c.gpus = P.at<double>(P_GPUS);
+  if (has(F_PORTS)) c.ports = P.at<int32_t>(P_PORTS);
+  if (has(F_NOT_ALLOWED)) c.allowed = P.at<uint8_t>(P_ALLOWED);
+  if (has(F_NOT_PLUGIN)) c.plugin = P.at<uint8_t>(P_PLUGIN);
+  if (L[L_NOVEL].live) { c.novel_off = P.at<int32_t>(P_NOFF); c.novel_host = L[L_NOVEL].v[0]; }
+  if (has(F_GPU_MODEL)) c.gpu_model = P.at<int32_t>(P_GPU_MODEL);
+  if (has(F_DISK)) { c.disk_request = P.at<double>(P_DISK_REQ); c.disk_type = P.at<int32_t>(P_DISK_TYPE); }
+  if (L[L_ATTR].live) { c.attr_off = P.at<int32_t>(P_AOFF); c.attr_col = L[L_ATTR].v[0]; c.attr_val = L[L_ATTR].v[1]; }
+  if (has(F_EST)) c.est_end_ms = P.at<int64_t>(P_EST);
+  if (has(F_CKPT)) c.ckpt_location = P.at<int32_t>(P_CKPT);
+  if (has(F_RESERVED)) c.reserved_host = P.at<int32_t>(P_RESERVED);
+  if (L[L_GROUP].live) { c.group_off = P.at<int32_t>(P_GOFF); c.group_idx = L[L_GROUP].v[0]; }
+  sh.n_novel = L[L_NOVEL].live; sh.n_attr = L[L_ATTR].live; sh.n_group = L[L_GROUP].live;
+  sh.gp_off.assign(G + 1, 0);
+  for (const auto& kv : S->groups) if (kv.first < G) sh.gp_off[kv.first + 1] = (int32_t)kv.second;
+  for (int g = 0; g < G; g++) sh.gp_off[g + 1] += sh.gp_off[g];
+  sh.any_gpus_ports = has(F_GPUS) || has(F_PORTS);
+  // ---- the plan, the gathers into the job columns it carved, the run
+  CK(pool, cudaEventRecord(pool->ev[0], st));
+  MatchRows rows;
+  rc = match_build(pool, nullptr, n, sh, offers, groups, users, pool_quota, params, max_ports, &rows);
+  if (rc != COOK_OK) return rc;
+  fill_rows_kernel<<<(n + 255) / 256, 256, 0, st>>>(rows, S->pend.d_col, m_slot, n);
+  nl++;
+  const JobDev& o = rows.jb;
+  const int32_t* doff[3] = {o.novel_off, o.attr_off, o.group_off};
+  const int32_t* dst[3][2] = {{o.novel_host, nullptr}, {o.attr_col, o.attr_val}, {o.group_idx, nullptr}};
+  const int loff[3] = {P_NOFF, P_AOFF, P_GOFF};
+  for (int l = 0; l < 3; l++) {
+    if (!doff[l]) continue;
+    const int32_t* len = P.at<int32_t>(loff[l] + 1);
+    order_scan(os, RowLen{m_slot, len}, n, S->gf0, st, &nl);
+    csr_gather_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, m_slot, n, P.at<int32_t>(loff[l]), len, L[l].v[0], L[l].v[1],
+                                                   writable(doff[l]), writable(dst[l][0]), writable(dst[l][1]));
+    nl++;
+  }
+  CK(pool, cudaGetLastError());
+  rc = match_run(pool, nullptr, out_considerable_job_id, out_assign, out_ports, out_fail_reason, out_stats, true,
+                 params->max_ctas);
   if (rc != COOK_OK) return rc;
   cook_phase_stats& ps = pool->phase[COOK_PHASE_MATCH];
   ps.n_launches += nl;
