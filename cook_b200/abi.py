@@ -146,12 +146,14 @@ class StateDelta(_SoA):
     """cook_state_delta: one batch of changes to a handle's resident pool state."""
     _fields_ = [("reset", C.c_int32), ("pending", JobsSoA), ("pending_priority", P_I32),
                 ("pending_job_id", P_I64), ("n_pending_rm", C.c_int32), ("pending_rm_job_id", P_I64),
-                ("running", TasksSoA), ("n_running_rm", C.c_int32), ("running_rm_task_id", P_I64)]
+                ("running", TasksSoA), ("n_running_rm", C.c_int32), ("running_rm_task_id", P_I64),
+                ("running_hostname_id", P_I32)]
 
 
 def make_delta(reset=False, pending=None, pending_priority=None, pending_job_id=None, pending_rm=(),
-               running=None, running_rm=()):
-    """A StateDelta; `pending` is a JobsSoA of the upserted rows, `running` a TasksSoA."""
+               running=None, running_rm=(), running_hostname_id=None):
+    """A StateDelta; `pending` is a JobsSoA of the upserted rows, `running` a TasksSoA, `running_hostname_id`
+    the hostname code of each running row (None: host unknown)."""
     pending = pending if pending is not None else JobsSoA(n=0)
     running = running if running is not None else TasksSoA(n=0)
     prm = np.asarray(pending_rm, np.int64)
@@ -159,7 +161,8 @@ def make_delta(reset=False, pending=None, pending_priority=None, pending_job_id=
     return StateDelta(reset=int(bool(reset)), pending=pending, pending_priority=pending_priority,
                       pending_job_id=pending_job_id, n_pending_rm=len(prm),
                       pending_rm_job_id=prm if len(prm) else None, running=running,
-                      n_running_rm=len(rrm), running_rm_task_id=rrm if len(rrm) else None)
+                      n_running_rm=len(rrm), running_rm_task_id=rrm if len(rrm) else None,
+                      running_hostname_id=running_hostname_id)
 
 
 class RunningSoA(_SoA):

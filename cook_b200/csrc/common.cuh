@@ -6,6 +6,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -214,6 +215,38 @@ int32_t match_build(cook_pool* pool, const int32_t* ranked_idx, int32_t n_ranked
                     MatchRows* rows);
 int32_t match_run(cook_pool* pool, int32_t* out_considerable, int64_t* out_job_id, int32_t* out_assign,
                   int32_t* out_ports, uint8_t* out_fail_reason, cook_match_stats* out_stats, bool uploaded, int max_ctas);
+
+// rebalance.cu: what a rebalance needs to know about its rows before it carves their columns.
+struct RebShape {
+  int R = 0, P = 0;                               // running tasks, pending jobs
+  // host tables to upload (cook_rebalance); a null `running`: the caller writes the carved rows (RebRows)
+  const cook_running_soa* running = nullptr;
+  const cook_jobs_soa* pending = nullptr;
+  const int64_t* job_id = nullptr;
+  const int32_t* priority = nullptr;
+  int64_t n_novel = 0, n_attr = 0, n_group = 0;   // caller-written rows: entries each list may hold (0: no list)
+};
+// The carved rows a caller writes before the run: running task r < R (host: index into the host table) and
+// pending job p < P, with the pending lists the shape asked for.
+struct RebRows {
+  TaskCols t;
+  const int32_t* host;
+  JobDev jb;
+  const int64_t* jid;
+  const int32_t* prio;
+  const int32_t* hostname_id;   // the host table's codes, uploaded [hosts->n]
+};
+struct RebPlan;
+struct RebPlanFree { void operator()(RebPlan* p) const; };
+using RebPlanPtr = std::unique_ptr<RebPlan, RebPlanFree>;
+// The build carves (and uploads the host table, the users' rebalance columns and the groups); the run is
+// cook_rebalance's own, with each victim reported as its task id (a synthetic victim, the task of the job
+// decision e placed, as -1 - e) and each decision's job id.  The caller checks the inputs.
+int32_t rebalance_build(cook_pool* pool, const RebShape& sh, const cook_host_table* hosts, const cook_groups* groups,
+                        const cook_user_table* users, const cook_rebalance_params* prm, RebPlanPtr* plan,
+                        RebRows* rows);
+int32_t rebalance_run(cook_pool* pool, RebPlan& plan, cook_decision* out_decisions, int64_t* out_victim_tid,
+                      int64_t* out_decision_jid, int32_t* out_n);
 
 inline int32_t set_err(cook_pool* p, int32_t code, const char* fmt, ...) {
   if (p) {

@@ -27,6 +27,7 @@
 #include <cooperative_groups.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "constraints.cuh"
 #include "fold.cuh"
@@ -976,55 +977,32 @@ __global__ void __launch_bounds__(REB_TB) rebalance_kernel(RebArgs a) {
   if (blockIdx.x == 0 && tid == 0) { a.cnt[8] = (int)(tA >> 10); a.cnt[9] = (int)(tB >> 10); a.cnt[10] = (int)(tC >> 10); a.cnt[11] = (int)(tS >> 10); a.cnt[12] = (int)(tA0 >> 10); for (int k = 0; k < 5; k++) a.cnt[13 + k] = (int)(tb[k] >> 10); }
 }
 
+// caller-written rows: each victim as its task id (a synthetic one as -1 - the decision that placed it: the
+// walk appends decision e's task at index R + e), each decision's job id
+__global__ void victim_ids_kernel(const int32_t* cnt, const int32_t* victims, const int64_t* tid, int R,
+                                  const cook_decision* dec, const int64_t* jid, int64_t* out_tid, int64_t* out_jid) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < cnt[2]) {
+    const int i = victims[k];
+    out_tid[k] = i < R ? tid[i] : -1 - (int64_t)(i - R);
+  }
+  if (k < cnt[1]) out_jid[k] = jid[dec[k].pending_idx];
+}
+
 }  // namespace
 
-static int32_t rebalance_run(cook_pool* pool, const cook_running_soa* running,
-                             const cook_jobs_soa* pending, const int64_t* pending_job_id,
-                             const int32_t* pending_priority, const cook_host_table* hosts,
-                             const cook_groups* groups, const cook_user_table* users,
-                             const cook_rebalance_params* prm, cook_decision* out_decisions,
-                             int32_t* out_victims, int32_t* out_n, const cook_reb_trace* tr) {
-  if (!pool) return COOK_E_BADARG;
-  if (!running || !pending || !pending_job_id || !pending_priority || !hosts || !users || !prm ||
-      !out_decisions || !out_victims || !out_n)
-    return set_err(pool, COOK_E_BADARG, "cook_rebalance: null argument");
-  if (pool->dru_mode != 0)
-    return set_err(pool, COOK_E_UNSUPPORTED_CONSTRAINT,
-                   "cook_rebalance: GPU DRU mode has no reference behaviour (rebalancer.clj:339-349 throws)");
-  const int R = running->t.n, P = pending->n, H = hosts->n, U = users->n_users;
-  const int MP = prm->max_preemption;
-  *out_n = 0;
-  if (P <= 0 || MP <= 0 || H <= 0) return COOK_OK;
-  if (!idx_in_range(running->t.user, R, 0, U) || !idx_in_range(pending->user, P, 0, U))
-    return set_err(pool, COOK_E_BADARG, "cook_rebalance: user index out of range");
-  if (!idx_in_range(running->host, R, 0, H)) return set_err(pool, COOK_E_BADARG, "cook_rebalance: running.host out of range");
-  if (groups && pending->group_off && !idx_in_range(pending->group_idx, pending->group_off[P], 0, groups->n_groups))
-    return set_err(pool, COOK_E_BADARG, "cook_rebalance: group index out of range");
-  const int G = groups ? groups->n_groups : 0;
-  if (G && pending->group_off && (!groups->cot_off || !groups->kind))
-    return set_err(pool, COOK_E_BADARG, "cook_rebalance: incomplete cook_groups");
-  const int CAP = R + MP + 1;
-  const int NF = tr ? tr->n_forced : 0;
-  int nfv = 0;   // forced victims
-  for (int q = 0; q < NF; q++) {
-    const cook_decision& f = tr->forced[q];
-    if (f.pending_idx < 0 || f.pending_idx >= P || f.host < 0 || f.host >= H || f.victim_count < 0 || f.victim_begin < 0)
-      return set_err(pool, COOK_E_BADARG, "cook_rebalance_trace: bad forced decision");
-    nfv = std::max(nfv, f.victim_begin + f.victim_count);
-  }
-  if (nfv > CAP + MP) return set_err(pool, COOK_E_BADARG, "cook_rebalance_trace: too many forced victims");
-  CK(pool, cudaSetDevice(pool->device));
-  cudaStream_t st = pool->stream;
-  const cook_tasks_soa& rt = running->t;
-  RTasks t;
-  HostCols hc;
-  PendCols pc;
-  GroupCols gc;
-  memset(&hc, 0, sizeof(hc));
-  memset(&pc, 0, sizeof(pc));
-  memset(&gc, 0, sizeof(gc));
-  hc.H = H;
-  hc.n_attr_cols = hosts->attr ? hosts->n_attr_cols : 0;
+// One rebalance's device buffers (carved by rebalance_build from the pool's arena) and what its run needs.
+struct RebPlan {
+  int R = 0, P = 0, H = 0, U = 0, MP = 0, CAP = 0, NF = 0;
+  bool zero_gpus = false;   // no gpus column uploaded: the task gpus are zeros
+  bool ids = false;         // caller-written rows: report task ids and job ids
+  const cook_reb_trace* tr = nullptr;
+  const cook_user_table* users = nullptr;
+  cook_rebalance_params prm = {};
+  RTasks t = {};
+  HostCols hc = {};
+  PendCols pc = {};
+  GroupCols gc = {};
   int32_t *d_urank, *d_ord, *d_ord2, *d_hord, *d_tmp, *d_us, *d_ue, *d_us2, *d_ue2, *d_hs, *d_he, *d_vict, *d_pre, *d_prehn;
   int32_t *d_cnt, *d_fvict = nullptr, *d_syn, *d_hq, *d_synh, *d_synn;
   double *d_divm, *d_divc, *d_qn, *d_qc, *d_qm, *d_qg, *d_pm, *d_pc, *d_btm, *d_btc;
@@ -1037,18 +1015,62 @@ static int32_t rebalance_run(cook_pool* pool, const cook_running_soa* running,
   GridFlag* d_gf;
   TaskHot* d_hot;
   WalkBar* d_bar;
-  int64_t h2d = 0, d2h = 0;
-  const cudaError_t carved = carve(pool->arena, st, pool->ev[12], &h2d, [&](Carve& c) {
-    t.user = c.part(rt.user, R, CAP); t.prio = c.part(rt.priority, R, CAP); t.start = c.part(rt.start_time, R, CAP);
-    t.tid = c.part(rt.task_id, R, CAP); t.jid = c.part(rt.job_id, R, CAP); t.cpus = c.part(rt.cpus, R, CAP);
-    t.mem = c.part(rt.mem, R, CAP); t.gpus = rt.gpus ? c.part(rt.gpus, R, CAP) : c.take<double>(CAP);
-    t.host = c.part(running->host, R, CAP);
+  int64_t *d_vtid = nullptr, *d_djid = nullptr;
+  int64_t h2d = 0;
+};
+
+void RebPlanFree::operator()(RebPlan* p) const { delete p; }
+
+// The build: the call's buffers, carved from one description of its rows.  Host tables (sh.running) are
+// uploaded in the same pass; otherwise the running and pending columns are carved for the caller to write.
+// The host table, the users' rebalance columns and the groups are uploaded either way.
+static int32_t build(cook_pool* pool, const RebShape& sh, const cook_host_table* hosts, const cook_groups* groups,
+                     const cook_user_table* users, const cook_rebalance_params* prm, const cook_reb_trace* tr,
+                     RebPlan& q) {
+  static const cook_running_soa no_running = {};
+  static const cook_jobs_soa no_pending = {};
+  const bool up = sh.running != nullptr;
+  const cook_tasks_soa& rt = (up ? sh.running : &no_running)->t;
+  const cook_running_soa& running = up ? *sh.running : no_running;
+  const cook_jobs_soa& pending = up ? *sh.pending : no_pending;
+  const int R = sh.R, P = sh.P, H = hosts->n, U = users->n_users, MP = prm->max_preemption;
+  const int G = groups ? groups->n_groups : 0;
+  const int CAP = R + MP + 1;
+  const int NF = tr ? tr->n_forced : 0;
+  int nfv = 0;   // forced victims (checked by the caller)
+  for (int k = 0; k < NF; k++) nfv = std::max(nfv, tr->forced[k].victim_begin + tr->forced[k].victim_count);
+  q.R = R; q.P = P; q.H = H; q.U = U; q.MP = MP; q.CAP = CAP; q.NF = NF;
+  q.zero_gpus = up && !rt.gpus; q.ids = !up; q.tr = tr; q.users = users; q.prm = *prm;
+  RTasks& t = q.t;
+  HostCols& hc = q.hc;
+  PendCols& pc = q.pc;
+  GroupCols& gc = q.gc;
+  hc.H = H;
+  hc.n_attr_cols = hosts->attr ? hosts->n_attr_cols : 0;
+  const bool novel = up ? pending.novel_off != nullptr : sh.n_novel > 0;
+  const bool attr = up ? pending.attr_off != nullptr : sh.n_attr > 0;
+  const bool grouped = G && (up ? pending.group_off != nullptr : sh.n_group > 0);
+  CK(pool, cudaSetDevice(pool->device));
+  const cudaError_t carved = carve(pool->arena, pool->stream, pool->ev[12], &q.h2d, [&](Carve& c) {
+    // a running column: the host's R rows in CAP, or CAP for the caller; a pending column likewise
+    const auto run_col = [&](auto* host) {
+      using T = std::remove_const_t<std::remove_pointer_t<decltype(host)>>;
+      return up ? c.part(host, (size_t)R, (size_t)CAP) : c.take<T>(CAP);
+    };
+    const auto pend_col = [&](auto* host, size_t n) {
+      using T = std::remove_const_t<std::remove_pointer_t<decltype(host)>>;
+      return up ? c.up(host, n) : c.take<T>(n);
+    };
+    t.user = run_col(rt.user); t.prio = run_col(rt.priority); t.start = run_col(rt.start_time);
+    t.tid = run_col(rt.task_id); t.jid = run_col(rt.job_id); t.cpus = run_col(rt.cpus);
+    t.mem = run_col(rt.mem); t.gpus = rt.gpus ? run_col(rt.gpus) : c.take<double>(CAP);
+    t.host = run_col(running.host);
     t.alive = c.take<uint8_t>(CAP); t.dru = c.take<double>(CAP); t.pos = c.take<int32_t>(CAP);
     t.cm = c.take<double>(CAP); t.cc = c.take<double>(CAP);
 
-    d_urank = c.up(users->name_rank, U); d_divm = c.up(users->div_mem, U); d_divc = c.up(users->div_cpus, U);
-    d_qn = c.up(users->quota_count, U); d_qc = c.up(users->quota_cpus, U); d_qm = c.up(users->quota_mem, U);
-    d_qg = c.up(users->quota_gpus, U);
+    q.d_urank = c.up(users->name_rank, U); q.d_divm = c.up(users->div_mem, U); q.d_divc = c.up(users->div_cpus, U);
+    q.d_qn = c.up(users->quota_count, U); q.d_qc = c.up(users->quota_cpus, U); q.d_qm = c.up(users->quota_mem, U);
+    q.d_qg = c.up(users->quota_gpus, U);
 
     hc.hostname_id = c.up(hosts->hostname_id, H); hc.name_rank = c.up(hosts->name_rank, H);
     hc.has_spare = c.part(hosts->has_spare, H, H + 1, true); hc.spare_cpus = c.part(hosts->spare_cpus, H, H + 1, true);
@@ -1066,23 +1088,23 @@ static int32_t rebalance_run(cook_pool* pool, const cook_running_soa* running,
     hc.host_start = c.up(hosts->host_start_time, H);
     if (hc.n_attr_cols > 0) hc.attr = c.up(hosts->attr, (size_t)hc.n_attr_cols * H);
 
-    pc.user = c.up(pending->user, P); pc.prio = c.up(pending_priority, P);
-    pc.cpus = c.up(pending->cpus, P); pc.mem = c.up(pending->mem, P); pc.gpus = c.up(pending->gpus, P);
-    pc.jid = c.up(pending_job_id, P); pc.est_end_ms = c.up(pending->est_end_ms, P);
-    if (pending->novel_off) {
-      pc.novel_off = c.up(pending->novel_off, P + 1);
-      pc.novel_host = c.up(pending->novel_host, std::max(1, pending->novel_off[P]));
+    pc.user = pend_col(pending.user, P); pc.prio = pend_col(sh.priority, P);
+    pc.cpus = pend_col(pending.cpus, P); pc.mem = pend_col(pending.mem, P); pc.gpus = pend_col(pending.gpus, P);
+    pc.jid = pend_col(sh.job_id, P); pc.est_end_ms = pend_col(pending.est_end_ms, P);
+    if (novel) {
+      pc.novel_off = pend_col(pending.novel_off, P + 1);
+      pc.novel_host = pend_col(pending.novel_host, std::max<int64_t>(1, up ? pending.novel_off[P] : sh.n_novel));
     }
-    pc.gpu_model = c.up(pending->gpu_model, P); pc.disk_type = c.up(pending->disk_type, P);
-    pc.ckpt_location = c.up(pending->ckpt_location, P);
-    pc.disk_request = c.up(pending->disk_request, P);
-    if (pending->attr_off) {
-      const int n = std::max(1, pending->attr_off[P]);
-      pc.attr_off = c.up(pending->attr_off, P + 1); pc.attr_col = c.up(pending->attr_col, n); pc.attr_val = c.up(pending->attr_val, n);
+    pc.gpu_model = pend_col(pending.gpu_model, P); pc.disk_type = pend_col(pending.disk_type, P);
+    pc.ckpt_location = pend_col(pending.ckpt_location, P);
+    pc.disk_request = pend_col(pending.disk_request, P);
+    if (attr) {
+      const int64_t n = std::max<int64_t>(1, up ? pending.attr_off[P] : sh.n_attr);
+      pc.attr_off = pend_col(pending.attr_off, P + 1); pc.attr_col = pend_col(pending.attr_col, n); pc.attr_val = pend_col(pending.attr_val, n);
     }
-    if (G && pending->group_off) {
-      pc.group_off = c.up(pending->group_off, P + 1);
-      pc.group_idx = c.up(pending->group_idx, std::max(1, pending->group_off[P]));
+    if (grouped) {
+      pc.group_off = pend_col(pending.group_off, P + 1);
+      pc.group_idx = pend_col(pending.group_idx, std::max<int64_t>(1, up ? pending.group_off[P] : sh.n_group));
       gc.n = G;
       gc.kind = c.up(groups->kind, G); gc.attr_col = c.up(groups->attr_col, G);
       gc.minimum = c.up(groups->minimum, G); gc.cot_off = c.up(groups->cot_off, G + 1);
@@ -1090,97 +1112,113 @@ static int32_t rebalance_run(cook_pool* pool, const cook_running_soa* running,
       gc.cot_host = c.up(groups->cot_hostname_id, n); gc.cot_attr = c.up(groups->cot_attr_val, n);
     }
 
-    d_ord = c.take<int32_t>(CAP); d_ord2 = c.take<int32_t>(CAP);
-    d_hord = c.take<int32_t>(CAP);
-    d_tmp = c.take<int32_t>(CAP);
-    d_us = c.take<int32_t>(U + 1); d_ue = c.take<int32_t>(U + 1);
-    d_us2 = c.take<int32_t>(U + 1); d_ue2 = c.take<int32_t>(U + 1);
-    d_hs = c.take<int32_t>(H + 1); d_he = c.take<int32_t>(H + 1);
-    d_has_task = c.take<uint8_t>(H + 1);
-    d_best = c.take<HostBest>(H + 1);
-    d_cta = c.take<CtaBest>(4 * pool->sm_count + 8);
-    d_dec = c.take<cook_decision>(MP + 1);
-    d_vict = c.take<int32_t>(CAP + MP);
-    d_pre = c.take<int32_t>(CAP + MP);
-    d_prehn = c.take<int32_t>(CAP + MP);
-    d_ps = c.take<PendScalars>(P + 4);
-    d_rf = c.take<Refold>(1);
-    d_cnt = c.take<int32_t>(64);  // [0] n_tasks [1] n_dec [2] n_vict [3] n_preempted [4] changed
+    q.d_ord = c.take<int32_t>(CAP); q.d_ord2 = c.take<int32_t>(CAP);
+    q.d_hord = c.take<int32_t>(CAP);
+    q.d_tmp = c.take<int32_t>(CAP);
+    q.d_us = c.take<int32_t>(U + 1); q.d_ue = c.take<int32_t>(U + 1);
+    q.d_us2 = c.take<int32_t>(U + 1); q.d_ue2 = c.take<int32_t>(U + 1);
+    q.d_hs = c.take<int32_t>(H + 1); q.d_he = c.take<int32_t>(H + 1);
+    q.d_has_task = c.take<uint8_t>(H + 1);
+    q.d_best = c.take<HostBest>(H + 1);
+    q.d_cta = c.take<CtaBest>(4 * pool->sm_count + 8);
+    q.d_dec = c.take<cook_decision>(MP + 1);
+    q.d_vict = c.take<int32_t>(CAP + MP);
+    q.d_pre = c.take<int32_t>(CAP + MP);
+    q.d_prehn = c.take<int32_t>(CAP + MP);
+    q.d_ps = c.take<PendScalars>(P + 4);
+    q.d_rf = c.take<Refold>(1);
+    q.d_cnt = c.take<int32_t>(64);  // [0] n_tasks [1] n_dec [2] n_vict [3] n_preempted [4] changed
     if (NF > 0) {
-      d_forced = c.part(tr->forced, NF, NF + 1);
-      d_fvict = c.part(tr->forced_victims, nfv, CAP + MP);
+      q.d_forced = c.part(tr->forced, NF, NF + 1);
+      q.d_fvict = c.part(tr->forced_victims, nfv, CAP + MP);
     }
-    d_gf = c.take<GridFlag>(1);
-    d_syn = c.take<int32_t>(H + 1);
-    d_hot = c.take<TaskHot>(CAP);
-    d_hq = c.take<int32_t>(CAP);
-    d_synh = c.take<int32_t>(H + 1);
-    d_synn = c.take<int32_t>(CAP);
-    d_bar = c.take<WalkBar>(1);
-    d_pm = c.take<double>(CAP); d_pc = c.take<double>(CAP);
-    d_btm = c.take<double>(CAP / OS_TILE + 2); d_btc = c.take<double>(CAP / OS_TILE + 2);
+    q.d_gf = c.take<GridFlag>(1);
+    q.d_syn = c.take<int32_t>(H + 1);
+    q.d_hot = c.take<TaskHot>(CAP);
+    q.d_hq = c.take<int32_t>(CAP);
+    q.d_synh = c.take<int32_t>(H + 1);
+    q.d_synn = c.take<int32_t>(CAP);
+    q.d_bar = c.take<WalkBar>(1);
+    q.d_pm = c.take<double>(CAP); q.d_pc = c.take<double>(CAP);
+    q.d_btm = c.take<double>(CAP / OS_TILE + 2); q.d_btc = c.take<double>(CAP / OS_TILE + 2);
+    if (q.ids) { q.d_vtid = c.take<int64_t>(CAP + MP); q.d_djid = c.take<int64_t>(MP + 1); }
   });
   CK(pool, carved);
-  if (!rt.gpus) CK(pool, cudaMemsetAsync(t.gpus, 0, sizeof(double) * CAP, st));
+  return COOK_OK;
+}
+
+// The run: the grid checks, init-state (sorts, initial fold, host grouping), the walk, the download.
+static int32_t run(cook_pool* pool, RebPlan& q, cook_decision* out_decisions, int32_t* out_victims,
+                   int64_t* out_victim_tid, int64_t* out_decision_jid, int32_t* out_n) {
+  cudaStream_t st = pool->stream;
+  const int R = q.R, P = q.P, H = q.H, U = q.U, MP = q.MP, CAP = q.CAP, NF = q.NF;
+  const cook_reb_trace* tr = q.tr;
+  const cook_rebalance_params* prm = &q.prm;
+  const cook_user_table* users = q.users;
+  RTasks& t = q.t;
+  HostCols& hc = q.hc;
+  int64_t d2h = 0;
+  if (q.zero_gpus) CK(pool, cudaMemsetAsync(t.gpus, 0, sizeof(double) * CAP, st));
   CK(pool, cudaMemsetAsync(t.alive, 0, CAP, st));
   if (R) CK(pool, cudaMemsetAsync(t.alive, 1, R, st));
   CK(pool, cudaMemsetAsync(t.dru, 0, sizeof(double) * CAP, st));
-  CK(pool, cudaMemsetAsync(d_gf, 0, sizeof(GridFlag), st));
-  CK(pool, cudaMemsetAsync(d_syn, 0, sizeof(int32_t) * (H + 1), st));
-  CK(pool, cudaMemsetAsync(d_synh, 0xff, sizeof(int32_t) * (H + 1), st));
-  CK(pool, cudaMemsetAsync(d_bar, 0, sizeof(WalkBar), st));
+  CK(pool, cudaMemsetAsync(q.d_gf, 0, sizeof(GridFlag), st));
+  CK(pool, cudaMemsetAsync(q.d_syn, 0, sizeof(int32_t) * (H + 1), st));
+  CK(pool, cudaMemsetAsync(q.d_synh, 0xff, sizeof(int32_t) * (H + 1), st));
+  CK(pool, cudaMemsetAsync(q.d_bar, 0, sizeof(WalkBar), st));
   int launches = 0;
   if (R > 0) {
-    grid_check_kernel<<<(R + 255) / 256, 256, 0, st>>>(t.cpus, t.mem, t.gpus, R, d_gf);
+    grid_check_kernel<<<(R + 255) / 256, 256, 0, st>>>(t.cpus, t.mem, t.gpus, R, q.d_gf);
     launches++;
   }
-  grid_check_kernel<<<(P + 255) / 256, 256, 0, st>>>(pc.cpus, pc.mem, pc.gpus, P, d_gf);
+  grid_check_kernel<<<(P + 255) / 256, 256, 0, st>>>(q.pc.cpus, q.pc.mem, q.pc.gpus, P, q.d_gf);
   launches++;
   int32_t h_cnt[16] = {R, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
-  CK(pool, cudaMemcpyAsync(d_cnt, h_cnt, sizeof(h_cnt), cudaMemcpyHostToDevice, st));
-  CK(pool, cudaMemsetAsync(d_ps, 0xff, sizeof(PendScalars) * (P + 4), st));   // below_quota -1, dru NaN: not reached
+  CK(pool, cudaMemcpyAsync(q.d_cnt, h_cnt, sizeof(h_cnt), cudaMemcpyHostToDevice, st));
+  CK(pool, cudaMemsetAsync(q.d_ps, 0xff, sizeof(PendScalars) * (P + 4), st));   // below_quota -1, dru NaN: not reached
 
   CK(pool, cudaEventRecord(pool->ev[13], st));
   const int TB = 256;
   // ---- init-state: user order + DRU of every user, tasks grouped by host
-  CK(pool, cudaMemsetAsync(d_us, 0, sizeof(int32_t) * (U + 1), st));
-  CK(pool, cudaMemsetAsync(d_ue, 0, sizeof(int32_t) * (U + 1), st));
-  CK(pool, cudaMemsetAsync(d_us2, 0, sizeof(int32_t) * (U + 1), st));
-  CK(pool, cudaMemsetAsync(d_ue2, 0, sizeof(int32_t) * (U + 1), st));
-  CK(pool, cudaMemsetAsync(d_hs, 0, sizeof(int32_t) * (H + 1), st));
-  CK(pool, cudaMemsetAsync(d_he, 0, sizeof(int32_t) * (H + 1), st));
-  CK(pool, cudaMemsetAsync(d_has_task, 0, H + 1, st));
+  CK(pool, cudaMemsetAsync(q.d_us, 0, sizeof(int32_t) * (U + 1), st));
+  CK(pool, cudaMemsetAsync(q.d_ue, 0, sizeof(int32_t) * (U + 1), st));
+  CK(pool, cudaMemsetAsync(q.d_us2, 0, sizeof(int32_t) * (U + 1), st));
+  CK(pool, cudaMemsetAsync(q.d_ue2, 0, sizeof(int32_t) * (U + 1), st));
+  CK(pool, cudaMemsetAsync(q.d_hs, 0, sizeof(int32_t) * (H + 1), st));
+  CK(pool, cudaMemsetAsync(q.d_he, 0, sizeof(int32_t) * (H + 1), st));
+  CK(pool, cudaMemsetAsync(q.d_has_task, 0, H + 1, st));
   if (R > 0) {
-    CK(pool, csort::sort_indices(d_ord, d_tmp, R, LessUserTask{t.user, t.prio, t.start, t.tid, t.jid, d_urank}, st, &launches));
-    seg_bounds_kernel<<<(R + TB - 1) / TB, TB, 0, st>>>(SortedKey{d_ord, nullptr, t.user}, R, d_us, d_ue, nullptr);
+    CK(pool, csort::sort_indices(q.d_ord, q.d_tmp, R, LessUserTask{t.user, t.prio, t.start, t.tid, t.jid, q.d_urank}, st, &launches));
+    seg_bounds_kernel<<<(R + TB - 1) / TB, TB, 0, st>>>(SortedKey{q.d_ord, nullptr, t.user}, R, q.d_us, q.d_ue, nullptr);
     launches++;
     {
-      const OrderScan<double, 2> os{{d_pm, d_pc}, {d_btm, d_btc}};
-      order_scan(os, LoadAlive{d_ord, t}, R, d_gf, st, &launches);
-      order_dru_finish<<<(R + TB - 1) / TB, TB, 0, st>>>(d_ord, t, R, d_gf, os, d_us, d_divm, d_divc);
+      const OrderScan<double, 2> os{{q.d_pm, q.d_pc}, {q.d_btm, q.d_btc}};
+      order_scan(os, LoadAlive{q.d_ord, t}, R, q.d_gf, st, &launches);
+      order_dru_finish<<<(R + TB - 1) / TB, TB, 0, st>>>(q.d_ord, t, R, q.d_gf, os, q.d_us, q.d_divm, q.d_divc);
       launches++;
     }
-    user_dru_kernel<<<(U + 3) / 4, 128, 0, st>>>(d_ord, t, d_divm, d_divc, d_us, d_ue, U, d_gf, R);
+    user_dru_kernel<<<(U + 3) / 4, 128, 0, st>>>(q.d_ord, t, q.d_divm, q.d_divc, q.d_us, q.d_ue, U, q.d_gf, R);
     launches++;
-    CK(pool, csort::sort_indices(d_hord, d_tmp, R, LessHost{t}, st, &launches));
-    seg_bounds_kernel<<<(R + TB - 1) / TB, TB, 0, st>>>(SortedKey{d_hord, nullptr, t.host}, R, d_hs, d_he, nullptr);
-    host_has_task_kernel<<<(R + TB - 1) / TB, TB, 0, st>>>(t, R, d_has_task);
-    hot_build_kernel<<<(R + TB - 1) / TB, TB, 0, st>>>(d_hord, t, d_urank, R, d_hot, d_hq);
+    CK(pool, csort::sort_indices(q.d_hord, q.d_tmp, R, LessHost{t}, st, &launches));
+    seg_bounds_kernel<<<(R + TB - 1) / TB, TB, 0, st>>>(SortedKey{q.d_hord, nullptr, t.host}, R, q.d_hs, q.d_he, nullptr);
+    host_has_task_kernel<<<(R + TB - 1) / TB, TB, 0, st>>>(t, R, q.d_has_task);
+    hot_build_kernel<<<(R + TB - 1) / TB, TB, 0, st>>>(q.d_hord, t, q.d_urank, R, q.d_hot, q.d_hq);
     launches += 3;
   }
   // ---- the walk over the pending jobs: one cooperative launch, no host round trip inside
   RebArgs ra;
   ra.t = t; ra.R = R;
-  ra.ord[0] = d_ord; ra.ord[1] = d_ord2; ra.us[0] = d_us; ra.us[1] = d_us2; ra.ue[0] = d_ue; ra.ue[1] = d_ue2;
-  ra.hord = d_hord; ra.hs = d_hs; ra.he = d_he;
-  ra.hc = hc; ra.pc = pc; ra.gc = gc; ra.P = P; ra.U = U; ra.MP = MP;
-  ra.user_rank = d_urank; ra.div_mem = d_divm; ra.div_cpus = d_divc;
-  ra.q_count = d_qn; ra.q_cpus = d_qc; ra.q_mem = d_qm; ra.q_gpus = d_qg;
-  ra.has_task = d_has_task; ra.preempted_hosts = d_pre; ra.preempted_hn = d_prehn;
+  ra.ord[0] = q.d_ord; ra.ord[1] = q.d_ord2; ra.us[0] = q.d_us; ra.us[1] = q.d_us2; ra.ue[0] = q.d_ue; ra.ue[1] = q.d_ue2;
+  ra.hord = q.d_hord; ra.hs = q.d_hs; ra.he = q.d_he;
+  ra.hc = hc; ra.pc = q.pc; ra.gc = q.gc; ra.P = P; ra.U = U; ra.MP = MP;
+  ra.user_rank = q.d_urank; ra.div_mem = q.d_divm; ra.div_cpus = q.d_divc;
+  ra.q_count = q.d_qn; ra.q_cpus = q.d_qc; ra.q_mem = q.d_qm; ra.q_gpus = q.d_qg;
+  ra.has_task = q.d_has_task; ra.preempted_hosts = q.d_pre; ra.preempted_hn = q.d_prehn;
   ra.min_diff = prm->min_dru_diff; ra.safe = prm->safe_dru_threshold; ra.host_lifetime_mins = prm->host_lifetime_mins;
-  ra.best = d_best; ra.cta_best = d_cta; ra.dec = d_dec; ra.victims = d_vict; ra.cnt = d_cnt; ra.rf = d_rf;
-  ra.ps_all = d_ps; ra.gf = d_gf; ra.syn_cnt = d_syn; ra.hot = d_hot; ra.hq = d_hq; ra.syn_head = d_synh; ra.syn_next = d_synn; ra.bar = d_bar;
-  ra.n_forced = NF; ra.forced = d_forced; ra.forced_victims = d_fvict; ra.forced_only = tr ? tr->forced_only : 0;
+  ra.best = q.d_best; ra.cta_best = q.d_cta; ra.dec = q.d_dec; ra.victims = q.d_vict; ra.cnt = q.d_cnt; ra.rf = q.d_rf;
+  ra.ps_all = q.d_ps; ra.gf = q.d_gf; ra.syn_cnt = q.d_syn; ra.hot = q.d_hot; ra.hq = q.d_hq; ra.syn_head = q.d_synh;
+  ra.syn_next = q.d_synn; ra.bar = q.d_bar;
+  ra.n_forced = NF; ra.forced = q.d_forced; ra.forced_victims = q.d_fvict; ra.forced_only = tr ? tr->forced_only : 0;
   {
     int occ = 0;
     CK(pool, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, rebalance_kernel, REB_TB, 0));
@@ -1194,12 +1232,18 @@ static int32_t rebalance_run(cook_pool* pool, const cook_running_soa* running,
     CK(pool, cudaLaunchCooperativeKernel((void*)rebalance_kernel, dim3(grid), dim3(REB_TB), kargs, 0, st));
     launches++;
   }
+  if (q.ids) {
+    victim_ids_kernel<<<(CAP + MP + 255) / 256, 256, 0, st>>>(q.d_cnt, q.d_vict, t.tid, R, q.d_dec, q.pc.jid, q.d_vtid,
+                                                             q.d_djid);
+    launches++;
+    CK(pool, cudaGetLastError());
+  }
   CK(pool, cudaEventRecord(pool->ev[14], st));
-  CK(pool, download(h_cnt, d_cnt, 5, st, &d2h));
+  CK(pool, download(h_cnt, q.d_cnt, 5, st, &d2h));
   CK(pool, cudaStreamSynchronize(st));
   if (getenv("COOK_PROF")) {
     int32_t hp[10];
-    CK(pool, cudaMemcpy(hp, d_cnt + 8, sizeof(hp), cudaMemcpyDeviceToHost));
+    CK(pool, cudaMemcpy(hp, q.d_cnt + 8, sizeof(hp), cudaMemcpyDeviceToHost));
     float pre = 0.f, walk = 0.f;
     if (R > 0 && P > 0) { cudaEventElapsedTime(&pre, pool->ev[13], pool->ev[19]); cudaEventElapsedTime(&walk, pool->ev[19], pool->ev[14]); }
     fprintf(stderr, "[cook_prof] rebalance kcycles (CTA 0): hosts %d (scalars+groups %d)  next-state %d  refold %d  grid-sync %d | setup %.3f ms walk %.3f ms\n",
@@ -1208,15 +1252,20 @@ static int32_t rebalance_run(cook_pool* pool, const cook_running_soa* running,
   }
   const int n_dec = h_cnt[1], n_tasks = h_cnt[0];
   if (n_dec > 0) {
-    CK(pool, download(out_decisions, d_dec, n_dec, st, &d2h));
-    if (h_cnt[2] > 0) CK(pool, download(out_victims, d_vict, h_cnt[2], st, &d2h));
+    CK(pool, download(out_decisions, q.d_dec, n_dec, st, &d2h));
+    if (q.ids) {
+      CK(pool, download(out_decision_jid, q.d_djid, n_dec, st, &d2h));
+      if (h_cnt[2] > 0) CK(pool, download(out_victim_tid, q.d_vtid, h_cnt[2], st, &d2h));
+    } else if (h_cnt[2] > 0) {
+      CK(pool, download(out_victims, q.d_vict, h_cnt[2], st, &d2h));
+    }
   }
   if (tr) {   // the state the reference's own tests read (K18 pending dru, K21 next-state, job-below-quota)
     std::vector<PendScalars> hps(P);
     std::vector<double> hdru(n_tasks);
     std::vector<uint8_t> halive(n_tasks);
     std::vector<int32_t> hpos(n_tasks), huser(n_tasks);
-    CK(pool, download(hps.data(), d_ps, P, st, &d2h));
+    CK(pool, download(hps.data(), q.d_ps, P, st, &d2h));
     if (n_tasks > 0) {
       CK(pool, download(hdru.data(), t.dru, n_tasks, st, &d2h));
       CK(pool, download(halive.data(), t.alive, n_tasks, st, &d2h));
@@ -1250,9 +1299,82 @@ static int32_t rebalance_run(cook_pool* pool, const cook_running_soa* running,
   }
   CK(pool, cudaEventRecord(pool->ev[15], st));
   CK(pool, cudaStreamSynchronize(st));
-  record_phase(pool, COOK_PHASE_REBALANCE, pool->ev[12], pool->ev[13], pool->ev[14], pool->ev[15], h2d, d2h, launches);
+  record_phase(pool, COOK_PHASE_REBALANCE, pool->ev[12], pool->ev[13], pool->ev[14], pool->ev[15], q.h2d, d2h, launches);
   *out_n = n_dec;
   return COOK_OK;
+}
+
+int32_t rebalance_build(cook_pool* pool, const RebShape& sh, const cook_host_table* hosts, const cook_groups* groups,
+                        const cook_user_table* users, const cook_rebalance_params* prm, RebPlanPtr* plan,
+                        RebRows* rows) {
+  plan->reset(new RebPlan());
+  RebPlan& q = **plan;
+  const int32_t rc = build(pool, sh, hosts, groups, users, prm, nullptr, q);
+  if (rc != COOK_OK) return rc;
+  const PendCols& pc = q.pc;
+  rows->t = TaskCols{q.t.user, q.t.prio, q.t.start, q.t.tid, q.t.jid, q.t.cpus, q.t.mem, q.t.gpus};
+  rows->host = q.t.host;
+  rows->jb = JobDev{};
+  JobDev& jb = rows->jb;
+  jb.user = pc.user; jb.cpus = pc.cpus; jb.mem = pc.mem; jb.gpus = pc.gpus;
+  jb.novel_off = pc.novel_off; jb.novel_host = pc.novel_host; jb.gpu_model = pc.gpu_model;
+  jb.disk_request = pc.disk_request; jb.disk_type = pc.disk_type;
+  jb.attr_off = pc.attr_off; jb.attr_col = pc.attr_col; jb.attr_val = pc.attr_val;
+  jb.est_end_ms = pc.est_end_ms; jb.ckpt_location = pc.ckpt_location;
+  jb.group_off = pc.group_off; jb.group_idx = pc.group_idx;
+  rows->jid = pc.jid; rows->prio = pc.prio;
+  rows->hostname_id = q.hc.hostname_id;
+  return COOK_OK;
+}
+
+int32_t rebalance_run(cook_pool* pool, RebPlan& plan, cook_decision* out_decisions, int64_t* out_victim_tid,
+                      int64_t* out_decision_jid, int32_t* out_n) {
+  return run(pool, plan, out_decisions, nullptr, out_victim_tid, out_decision_jid, out_n);
+}
+
+// cook_rebalance(_trace) on host tables: the checks, then build and run
+static int32_t rebalance_host(cook_pool* pool, const cook_running_soa* running,
+                              const cook_jobs_soa* pending, const int64_t* pending_job_id,
+                              const int32_t* pending_priority, const cook_host_table* hosts,
+                              const cook_groups* groups, const cook_user_table* users,
+                              const cook_rebalance_params* prm, cook_decision* out_decisions,
+                              int32_t* out_victims, int32_t* out_n, const cook_reb_trace* tr) {
+  if (!pool) return COOK_E_BADARG;
+  if (!running || !pending || !pending_job_id || !pending_priority || !hosts || !users || !prm ||
+      !out_decisions || !out_victims || !out_n)
+    return set_err(pool, COOK_E_BADARG, "cook_rebalance: null argument");
+  if (pool->dru_mode != 0)
+    return set_err(pool, COOK_E_UNSUPPORTED_CONSTRAINT,
+                   "cook_rebalance: GPU DRU mode has no reference behaviour (rebalancer.clj:339-349 throws)");
+  const int R = running->t.n, P = pending->n, H = hosts->n, U = users->n_users;
+  const int MP = prm->max_preemption;
+  *out_n = 0;
+  if (P <= 0 || MP <= 0 || H <= 0) return COOK_OK;
+  if (!idx_in_range(running->t.user, R, 0, U) || !idx_in_range(pending->user, P, 0, U))
+    return set_err(pool, COOK_E_BADARG, "cook_rebalance: user index out of range");
+  if (!idx_in_range(running->host, R, 0, H)) return set_err(pool, COOK_E_BADARG, "cook_rebalance: running.host out of range");
+  if (groups && pending->group_off && !idx_in_range(pending->group_idx, pending->group_off[P], 0, groups->n_groups))
+    return set_err(pool, COOK_E_BADARG, "cook_rebalance: group index out of range");
+  const int G = groups ? groups->n_groups : 0;
+  if (G && pending->group_off && (!groups->cot_off || !groups->kind))
+    return set_err(pool, COOK_E_BADARG, "cook_rebalance: incomplete cook_groups");
+  const int CAP = R + MP + 1;
+  const int NF = tr ? tr->n_forced : 0;
+  int nfv = 0;   // forced victims
+  for (int q = 0; q < NF; q++) {
+    const cook_decision& f = tr->forced[q];
+    if (f.pending_idx < 0 || f.pending_idx >= P || f.host < 0 || f.host >= H || f.victim_count < 0 || f.victim_begin < 0)
+      return set_err(pool, COOK_E_BADARG, "cook_rebalance_trace: bad forced decision");
+    nfv = std::max(nfv, f.victim_begin + f.victim_count);
+  }
+  if (nfv > CAP + MP) return set_err(pool, COOK_E_BADARG, "cook_rebalance_trace: too many forced victims");
+  RebShape sh;
+  sh.R = R; sh.P = P;
+  sh.running = running; sh.pending = pending; sh.job_id = pending_job_id; sh.priority = pending_priority;
+  RebPlan q;
+  const int32_t rc = build(pool, sh, hosts, groups, users, prm, tr, q);
+  if (rc != COOK_OK) return rc;
+  return run(pool, q, out_decisions, out_victims, nullptr, nullptr, out_n);
 }
 
 extern "C" int32_t cook_rebalance(cook_pool* pool, const cook_running_soa* running,
@@ -1261,8 +1383,8 @@ extern "C" int32_t cook_rebalance(cook_pool* pool, const cook_running_soa* runni
                                   const cook_groups* groups, const cook_user_table* users,
                                   const cook_rebalance_params* prm, cook_decision* out_decisions,
                                   int32_t* out_victims, int32_t* out_n) {
-  return rebalance_run(pool, running, pending, pending_job_id, pending_priority, hosts, groups, users, prm,
-                       out_decisions, out_victims, out_n, nullptr);
+  return rebalance_host(pool, running, pending, pending_job_id, pending_priority, hosts, groups, users, prm,
+                        out_decisions, out_victims, out_n, nullptr);
 }
 
 extern "C" int32_t cook_rebalance_trace(cook_pool* pool, const cook_running_soa* running,
@@ -1272,6 +1394,6 @@ extern "C" int32_t cook_rebalance_trace(cook_pool* pool, const cook_running_soa*
                                         const cook_rebalance_params* prm, cook_decision* out_decisions,
                                         int32_t* out_victims, int32_t* out_n, const cook_reb_trace* tr) {
   if (!tr) return set_err(pool, COOK_E_BADARG, "cook_rebalance_trace: null trace");
-  return rebalance_run(pool, running, pending, pending_job_id, pending_priority, hosts, groups, users, prm,
-                       out_decisions, out_victims, out_n, tr);
+  return rebalance_host(pool, running, pending, pending_job_id, pending_priority, hosts, groups, users, prm,
+                        out_decisions, out_victims, out_n, tr);
 }

@@ -10,7 +10,9 @@
 // run cook_rank's and cook_match's own code on them: rank_impl over the gathered task columns, and the
 // match plan's build, the gathers into the job columns it carved, then its run.  The ranked queue stays
 // on the device as (slot, generation) pairs; a match keeps the entries whose slot still holds that
-// generation, so a job removed or replaced since the rank leaves the queue.
+// generation, so a job removed or replaced since the rank leaves the queue.  A rebalance takes the first
+// allowed jobs of that queue and every live running task on its host, gathered into the columns the
+// rebalancer's build carved, and runs cook_rebalance's walk on them.
 #include <algorithm>
 #include <map>
 #include <unordered_map>
@@ -27,8 +29,9 @@ enum PCol {
   P_LIVE = P_NDATA, P_GEN, P_NOFF, P_NLEN, P_AOFF, P_ALEN, P_GOFF, P_GLEN, P_NCOL
 };
 constexpr int P_SZ[P_NCOL] = {4, 4, 8, 8, 8, 8, 4, 1, 1, 4, 8, 4, 8, 4, 4, 1, 4, 4, 4, 4, 4, 4, 4};
-enum RCol { R_USER, R_PRIO, R_START, R_TID, R_JID, R_CPUS, R_MEM, R_GPUS, R_NDATA, R_LIVE = R_NDATA, R_GEN, R_NCOL };
-constexpr int R_SZ[R_NCOL] = {4, 4, 8, 8, 8, 8, 8, 8, 1, 4};
+enum RCol { R_USER, R_PRIO, R_START, R_TID, R_JID, R_CPUS, R_MEM, R_GPUS, R_HOST, R_NDATA, R_LIVE = R_NDATA, R_GEN,
+            R_NCOL };
+constexpr int R_SZ[R_NCOL] = {4, 4, 8, 8, 8, 8, 8, 8, 4, 1, 4};
 
 enum { L_NOVEL = 0, L_ATTR = 1, L_GROUP = 2 };
 
@@ -189,6 +192,44 @@ __global__ void fill_rows_kernel(MatchRows r, void* const* col, const int32_t* m
   if (o.reserved_host) writable(o.reserved_host)[d] = static_cast<const int32_t*>(col[P_RESERVED])[s];
 }
 
+// ---- rebalance: the live running rows, host = the index of the row's hostname code in the host table
+__global__ void host_map_kernel(const int32_t* hostname_id, int H, int32_t* host_of) {
+  const int h = blockIdx.x * blockDim.x + threadIdx.x;
+  if (h < H) host_of[hostname_id[h]] = h;
+}
+struct RebRunningRows {
+  RunningRows r; int32_t* host; const int32_t* host_of;
+  __device__ bool keep(int i) const { return r.keep(i); }
+  __device__ void emit(int i, int d) const {
+    r.emit(i, d);
+    host[d] = host_of[static_cast<const int32_t*>(r.col[R_HOST])[i]];
+  }
+};
+// jobs-to-make-room-for: the live queue entries whose job is allowed to start
+struct QueueAllowed {
+  QueueLive q; const uint8_t* allowed;
+  __device__ bool keep(int k) const { return q.keep(k) && allowed[q.q_slot[k]]; }
+  __device__ void emit(int k, int d) const { q.emit(k, d); }
+};
+// pending job d of the rebalance is slot m_slot[d]: its columns into the build's
+__global__ void reb_pending_kernel(RebRows r, void* const* col, const int32_t* m_slot, int n) {
+  const int d = blockIdx.x * blockDim.x + threadIdx.x;
+  if (d >= n) return;
+  const int s = m_slot[d];
+  const JobDev& o = r.jb;
+  writable(o.user)[d] = static_cast<const int32_t*>(col[P_USER])[s];
+  writable(o.cpus)[d] = static_cast<const double*>(col[P_CPUS])[s];
+  writable(o.mem)[d] = static_cast<const double*>(col[P_MEM])[s];
+  writable(o.gpus)[d] = static_cast<const double*>(col[P_GPUS])[s];
+  writable(r.jid)[d] = static_cast<const int64_t*>(col[P_JID])[s];
+  writable(r.prio)[d] = static_cast<const int32_t*>(col[P_PRIO])[s];
+  writable(o.gpu_model)[d] = static_cast<const int32_t*>(col[P_GPU_MODEL])[s];
+  writable(o.disk_request)[d] = static_cast<const double*>(col[P_DISK_REQ])[s];
+  writable(o.disk_type)[d] = static_cast<const int32_t*>(col[P_DISK_TYPE])[s];
+  writable(o.est_end_ms)[d] = static_cast<const int64_t*>(col[P_EST])[s];
+  writable(o.ckpt_location)[d] = static_cast<const int32_t*>(col[P_CKPT])[s];
+}
+
 // ---- host side
 // the non-absent values of a pending row, counted per column (the match's constraint switch)
 enum { F_GPUS, F_PORTS, F_NOT_ALLOWED, F_NOT_PLUGIN, F_GPU_MODEL, F_DISK, F_EST, F_CKPT, F_RESERVED, F_N };
@@ -285,9 +326,10 @@ int32_t count_max(const std::map<int32_t, int64_t>& m) { return m.empty() ? -1 :
 struct PoolState {
   Table pend, run;
   std::vector<PendingInfo> pinfo;    // by pending slot
-  std::vector<int32_t> ruser;        // by running slot
+  std::vector<int32_t> ruser, rhost; // by running slot
   ListArena lists[3];
   std::map<int32_t, int64_t> users_p, users_r, attr_cols, groups;   // code -> live uses
+  std::map<int32_t, int64_t> hosts_r;                               // running rows' hostname codes (-1 too)
   int64_t nflag[F_N] = {};
   Arena stage;                        // one batch's uploads
   Arena scratch;                      // one call's device buffers
@@ -348,6 +390,23 @@ bool csr_ok(const int32_t* off, int n, const int32_t* v0, const int32_t* v1, boo
 
 long long bits_of(double x) { long long b; memcpy(&b, &x, 8); return b; }
 
+// the CSR lists of rows m_slot[0, n) into the dense lists of `o` that are carved (non-null)
+void gather_lists(const PoolState* S, const JobDev& o, const int32_t* m_slot, int n, const OrderScan<int, 1>& os,
+                  cudaStream_t st, int* nl) {
+  const int32_t* doff[3] = {o.novel_off, o.attr_off, o.group_off};
+  const int32_t* dst[3][2] = {{o.novel_host, nullptr}, {o.attr_col, o.attr_val}, {o.group_idx, nullptr}};
+  const int loff[3] = {P_NOFF, P_AOFF, P_GOFF};
+  for (int l = 0; l < 3; l++) {
+    if (!doff[l]) continue;
+    const int32_t* len = S->pend.at<int32_t>(loff[l] + 1);
+    order_scan(os, RowLen{m_slot, len}, n, S->gf0, st, nl);
+    csr_gather_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, m_slot, n, S->pend.at<int32_t>(loff[l]), len, S->lists[l].v[0],
+                                                   S->lists[l].v[1], writable(doff[l]), writable(dst[l][0]),
+                                                   writable(dst[l][1]));
+    (*nl)++;
+  }
+}
+
 // compaction of every list arena whose dead entries outnumber its live ones
 int32_t compact_lists(cook_pool* pool, PoolState* S, cudaStream_t st, int* nl) {
   const int n = S->pend.hw;
@@ -398,7 +457,7 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
   if ((P.attr_off && !idx_in_range(P.attr_col, P.attr_off[np], 0, INT32_MAX)) ||
       (P.group_off && !idx_in_range(P.group_idx, P.group_off[np], 0, INT32_MAX)) ||
       (P.novel_off && !idx_in_range(P.novel_host, P.novel_off[np], 0, INT32_MAX)) ||
-      !idx_in_range(P.reserved_host, np, -1, INT32_MAX))
+      !idx_in_range(P.reserved_host, np, -1, INT32_MAX) || !idx_in_range(d->running_hostname_id, nr, -1, INT32_MAX))
     return set_err(pool, COOK_E_BADARG, "cook_state_apply: bad attribute column, group or hostname code");
   const bool rs = d->reset != 0;
   {
@@ -431,7 +490,7 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
       }
       t->slot_of.clear(); t->free.clear(); t->hw = 0;
     }
-    S->users_p.clear(); S->users_r.clear(); S->attr_cols.clear(); S->groups.clear();
+    S->users_p.clear(); S->users_r.clear(); S->attr_cols.clear(); S->groups.clear(); S->hosts_r.clear();
     for (auto& f : S->nflag) f = 0;
     for (auto& l : S->lists) l.tail = l.live = 0;
   }
@@ -449,6 +508,7 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
     const int32_t s = it->second;
     S->run.slot_of.erase(it);
     count_add(S->users_r, S->ruser[s], -1);
+    count_add(S->hosts_r, S->rhost[s], -1);
     S->run.free.push_back(s);
     rrm_slot[i] = s;
   }
@@ -477,11 +537,22 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
   for (int i = 0; i < nr; i++) {
     auto it = S->run.slot_of.find(T.task_id[i]);
     int32_t s;
-    if (it != S->run.slot_of.end()) { s = it->second; count_add(S->users_r, S->ruser[s], -1); }
-    else { s = S->run.take_slot(); S->run.slot_of.emplace(T.task_id[i], s); }
-    if ((size_t)s >= S->ruser.size()) S->ruser.resize(std::max<size_t>(s + 1, 2 * S->ruser.size()));
+    if (it != S->run.slot_of.end()) {
+      s = it->second;
+      count_add(S->users_r, S->ruser[s], -1);
+      count_add(S->hosts_r, S->rhost[s], -1);
+    } else {
+      s = S->run.take_slot();
+      S->run.slot_of.emplace(T.task_id[i], s);
+    }
+    if ((size_t)s >= S->ruser.size()) {
+      S->ruser.resize(std::max<size_t>(s + 1, 2 * S->ruser.size()));
+      S->rhost.resize(S->ruser.size());
+    }
     S->ruser[s] = T.user[i];
+    S->rhost[s] = d->running_hostname_id ? d->running_hostname_id[i] : -1;
     count_add(S->users_r, T.user[i], +1);
+    count_add(S->hosts_r, S->rhost[s], +1);
     rup_slot[i] = s;
   }
   // ---- device: capacity, the upload, then the scatters (removals before upserts: a slot a removal
@@ -524,11 +595,13 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
     }
     if (npr) pr.slot = c.up(prm_slot.data(), npr);
     if (nr) {
-      const void* src[R_NDATA] = {T.user, T.priority, T.start_time, T.task_id, T.job_id, T.cpus, T.mem, T.gpus};
+      const void* src[R_NDATA] = {T.user, T.priority, T.start_time, T.task_id, T.job_id, T.cpus, T.mem, T.gpus,
+                                  d->running_hostname_id};
+      const long long dflt[R_NDATA] = {0, 0, 0, 0, 0, 0, 0, 0, -1};
       for (int k = 0; k < R_NDATA; k++) {
         const char* up = R_SZ[k] == 4 ? reinterpret_cast<const char*>(c.up(static_cast<const int32_t*>(src[k]), nr))
                                       : reinterpret_cast<const char*>(c.up(static_cast<const int64_t*>(src[k]), nr));
-        ru.c[k] = ScatterCol{static_cast<char*>(S->run.col[k]), up, 0, R_SZ[k]};
+        ru.c[k] = ScatterCol{static_cast<char*>(S->run.col[k]), up, dflt[k], R_SZ[k]};
       }
       ru.nc = R_NDATA;
       ru.slot = c.up(rup_slot.data(), nr);
@@ -730,18 +803,7 @@ extern "C" int32_t cook_state_match(cook_pool* pool, const cook_offers_soa* offe
   if (rc != COOK_OK) return rc;
   fill_rows_kernel<<<(n + 255) / 256, 256, 0, st>>>(rows, S->pend.d_col, m_slot, n);
   nl++;
-  const JobDev& o = rows.jb;
-  const int32_t* doff[3] = {o.novel_off, o.attr_off, o.group_off};
-  const int32_t* dst[3][2] = {{o.novel_host, nullptr}, {o.attr_col, o.attr_val}, {o.group_idx, nullptr}};
-  const int loff[3] = {P_NOFF, P_AOFF, P_GOFF};
-  for (int l = 0; l < 3; l++) {
-    if (!doff[l]) continue;
-    const int32_t* len = P.at<int32_t>(loff[l] + 1);
-    order_scan(os, RowLen{m_slot, len}, n, S->gf0, st, &nl);
-    csr_gather_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, m_slot, n, P.at<int32_t>(loff[l]), len, L[l].v[0], L[l].v[1],
-                                                   writable(doff[l]), writable(dst[l][0]), writable(dst[l][1]));
-    nl++;
-  }
+  gather_lists(S, rows.jb, m_slot, n, os, st, &nl);
   CK(pool, cudaGetLastError());
   rc = match_run(pool, nullptr, out_considerable_job_id, out_assign, out_ports, out_fail_reason, out_stats, true,
                  params->max_ctas);
@@ -750,5 +812,101 @@ extern "C" int32_t cook_state_match(cook_pool* pool, const cook_offers_soa* offe
   ps.n_launches += nl;
   ps.d2h_bytes += d2h;
   if (out_stats) { out_stats->n_launches += nl; out_stats->d2h_bytes += d2h; }
+  return COOK_OK;
+}
+
+extern "C" int32_t cook_state_rebalance(cook_pool* pool, const cook_host_table* hosts, const cook_groups* groups,
+                                        const cook_user_table* users, const cook_rebalance_params* params,
+                                        cook_decision* out_decisions, int64_t* out_decision_job_id,
+                                        int64_t* out_victim_task_id, int32_t victim_cap, int32_t* out_n) {
+  if (!pool) return COOK_E_BADARG;
+  if (!hosts || !users || !params || !out_decisions || !out_decision_job_id || !out_victim_task_id || !out_n)
+    return set_err(pool, COOK_E_BADARG, "cook_state_rebalance: null argument");
+  if (pool->dru_mode != 0)
+    return set_err(pool, COOK_E_UNSUPPORTED_CONSTRAINT,
+                   "cook_state_rebalance: GPU DRU mode has no reference behaviour (rebalancer.clj:339-349 throws)");
+  PoolState* S = static_cast<PoolState*>(pool->state);
+  if (!S || !S->ranked) return set_err(pool, COOK_E_BADARG, "cook_state_rebalance: no cook_state_rank on this handle yet");
+  *out_n = 0;
+  const int H = hosts->n, MP = params->max_preemption;
+  if (MP <= 0 || H <= 0) return COOK_OK;
+  // ---- every check before any device work, from the host-side counts
+  const int R = (int)S->run.slot_of.size();
+  if ((int64_t)victim_cap < (int64_t)R + MP)
+    return set_err(pool, COOK_E_BADARG, "cook_state_rebalance: victim_cap < live running rows + max_preemption");
+  if (!hosts->hostname_id) return set_err(pool, COOK_E_BADARG, "cook_state_rebalance: null hosts->hostname_id");
+  std::unordered_set<int32_t> codes;
+  codes.reserve((size_t)H);
+  int32_t max_code = 0;
+  for (int h = 0; h < H; h++) {
+    const int32_t c = hosts->hostname_id[h];
+    if (c < 0 || !codes.insert(c).second)
+      return set_err(pool, COOK_E_BADARG, "cook_state_rebalance: a hostname_id is negative or twice in the host table");
+    max_code = std::max(max_code, c);
+  }
+  for (const auto& kv : S->hosts_r)
+    if (!codes.count(kv.first))
+      return set_err(pool, COOK_E_BADARG, "cook_state_rebalance: a running row's host is unknown or not in the host table");
+  if (std::max(count_max(S->users_p), count_max(S->users_r)) >= users->n_users)
+    return set_err(pool, COOK_E_BADARG, "cook_state_rebalance: a resident row's user code is >= n_users");
+  const int G = groups ? groups->n_groups : 0;
+  if (groups && count_max(S->groups) >= G)
+    return set_err(pool, COOK_E_BADARG, "cook_state_rebalance: a pending row's group code is >= n_groups");
+  if (G && S->lists[L_GROUP].live && (!groups->cot_off || !groups->kind))
+    return set_err(pool, COOK_E_BADARG, "cook_state_rebalance: incomplete cook_groups");
+  if (count_max(S->attr_cols) >= std::max(1, hosts->n_attr_cols))
+    return set_err(pool, COOK_E_BADARG, "cook_state_rebalance: a pending row's attribute column is >= n_attr_cols");
+  const int nq = S->n_q;
+  if (nq == 0) return COOK_OK;
+  // ---- jobs-to-make-room-for: the first allowed jobs of the live queue, their count downloaded
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  const int PM = std::min(MP, nq);
+  int nl = 0;
+  int64_t d2h = 0;
+  int32_t *m_slot = nullptr, *blk = nullptr, *host_of = nullptr;
+  OrderScan<int, 1> os;
+  CK(pool, carve(S->scratch, st, nullptr, nullptr, [&](Carve& c) {
+    m_slot = c.take<int32_t>(PM);
+    blk = c.take<int32_t>((size_t)std::max(nq, S->run.hw) / CP_BLOCK + 2);
+    host_of = c.take<int32_t>((size_t)max_code + 1);
+    os.part[0] = c.take<int32_t>(PM);
+    os.tile[0] = c.take<int32_t>((PM + OS_TILE - 1) / OS_TILE + 1);
+  }));
+  CK(pool, cudaEventRecord(pool->ev[20], st));
+  const QueueLive ql{S->q_slot, S->q_gen, S->pend.at<uint8_t>(P_LIVE), S->pend.at<uint32_t>(P_GEN), m_slot};
+  compact(QueueAllowed{ql, S->pend.at<uint8_t>(P_ALLOWED)}, nq, nullptr, blk, S->counters + 2, PM, st, &nl);
+  CK(pool, cudaGetLastError());
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  int32_t P = 0;
+  CK(pool, download(&P, S->counters + 2, 1, st, &d2h));
+  CK(pool, cudaStreamSynchronize(st));
+  if (P == 0) return COOK_OK;
+  // ---- the build, the gathers into the rows it carved, the run
+  RebShape sh;
+  sh.R = R; sh.P = P;
+  sh.n_novel = S->lists[L_NOVEL].live; sh.n_attr = S->lists[L_ATTR].live; sh.n_group = S->lists[L_GROUP].live;
+  RebPlanPtr plan;
+  RebRows rows;
+  int32_t rc = rebalance_build(pool, sh, hosts, groups, users, params, &plan, &rows);
+  if (rc != COOK_OK) return rc;
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  if (R > 0) {
+    host_map_kernel<<<(H + 255) / 256, 256, 0, st>>>(rows.hostname_id, H, host_of);
+    nl++;
+    compact(RebRunningRows{RunningRows{S->run.d_col, rows.t}, writable(rows.host), host_of}, S->run.hw, nullptr, blk,
+            S->counters, R, st, &nl);
+  }
+  reb_pending_kernel<<<(P + 255) / 256, 256, 0, st>>>(rows, S->pend.d_col, m_slot, P);
+  nl++;
+  gather_lists(S, rows.jb, m_slot, P, os, st, &nl);
+  CK(pool, cudaGetLastError());
+  CK(pool, cudaEventRecord(pool->ev[23], st));
+  rc = rebalance_run(pool, *plan, out_decisions, out_victim_task_id, out_decision_job_id, out_n);
+  if (rc != COOK_OK) return rc;
+  cook_phase_stats& ps = pool->phase[COOK_PHASE_REBALANCE];
+  ps.ms_device += ev_ms(pool->ev[20], pool->ev[21]) + ev_ms(pool->ev[22], pool->ev[23]);   // the gathers
+  ps.n_launches += nl;
+  ps.d2h_bytes += d2h;
   return COOK_OK;
 }

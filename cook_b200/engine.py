@@ -61,7 +61,8 @@ def load_library(path=None):
                  "cook_last_error", "cook_rank", "cook_match", "cook_rebalance",
                  "cook_allgather_usage", "cook_last_stats", "cook_comm_unique_id", "cook_comm_init",
                  "cook_comm_destroy", "cook_exchange_usage", "cook_exchange_usage_batch", "cook_rebalance_trace",
-                 "cook_match_failures", "cook_state_apply", "cook_state_rank", "cook_state_match"):
+                 "cook_match_failures", "cook_state_apply", "cook_state_rank", "cook_state_match",
+                 "cook_state_rebalance"):
         getattr(lib, name).restype = C.c_int32
     return lib
 
@@ -165,6 +166,15 @@ class GpuEngine:
         up = delta.col("pending_job_id")
         live.update(up.tolist() if up is not None else [])
         self._state_pending_ids = live
+        # the live running ids likewise: they size state_rebalance's victims
+        run = getattr(self, "_state_running_ids", set())
+        if delta.reset:
+            run = set()
+        rm = delta.col("running_rm_task_id")
+        run.difference_update(rm.tolist() if rm is not None else [])
+        tid = delta.col("running").col("task_id") if delta.running.n else None
+        run.update(tid.tolist() if tid is not None else [])
+        self._state_running_ids = run
 
     def state_rank(self, users, pool_quota=None, group_quota=None, group_usage=None, params=None):
         """cook_state_rank: the live rows ranked; the queue stays on the device.  Returns its job ids."""
@@ -199,6 +209,26 @@ class GpuEngine:
         return {"considerable": cons[:n].copy(), "assign": assign[:n].copy(),
                 "ports": ports[:n * max(max_ports, 1)].reshape(n, max(max_ports, 1)).copy(),
                 "fail": fail[:n].copy(), "stats": stats.as_dict()}
+
+    def state_rebalance(self, hosts, users, params, groups=None):
+        """cook_state_rebalance: the rebalancer over the live running tasks and the first allowed jobs of the
+        resident queue.  As rebalance(), plus each decision's 'job_id'; 'victims' are task ids (the task
+        of the job an earlier decision e placed: -1 - e)."""
+        mp = max(params.max_preemption, 1)
+        dec = (abi.Decision * mp)()
+        jid = np.full(mp, -1, np.int64)
+        cap = len(getattr(self, "_state_running_ids", ())) + mp
+        vict = np.full(cap, -1, np.int64)
+        n = C.c_int32(0)
+        rc = self.lib.cook_state_rebalance(self.pool, C.byref(hosts), C.byref(groups) if groups is not None else None,
+                                           C.byref(users), C.byref(params), dec, abi.ptr(jid, abi.P_I64),
+                                           abi.ptr(vict, abi.P_I64), int(cap), C.byref(n))
+        if rc != 0:
+            self._err(rc)
+        out = decisions_to_list(dec, vict, n.value)
+        for d, j in zip(out, jid[:n.value].tolist()):
+            d["job_id"] = j
+        return out
 
     # -- B1-B6 -------------------------------------------------------------
     def rebalance(self, running, pending, pending_job_id, pending_priority, hosts, users, params,

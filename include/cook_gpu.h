@@ -432,10 +432,13 @@ int32_t cook_rebalance_trace(cook_pool* pool, const cook_running_soa* running,
  *   pending_rm_job_id   removals
  *   running             running-task upserts keyed by task_id (all cook_tasks_soa columns but gpus)
  *   running_rm_task_id  removals
+ *   running_hostname_id the host of each running upsert: a code of the global hostname dictionary (the
+ *                       code space of cook_offers_soa.hostname_id and cook_host_table.hostname_id).  NULL
+ *                       stores -1, "host unknown"; only cook_state_rebalance reads it.
  * A launch is one batch: remove pending job j, upsert its running task.
  * COOK_E_BADARG, state unchanged: an unknown id in a removal, an id twice in one table of the batch, a
  * malformed CSR offset column, a negative user / attr_col / group / novel hostname code, a
- * reserved_host below -1.
+ * reserved_host or running_hostname_id below -1.
  * Codes are checked here, when they enter; their maxima are kept on the host, and rank / match reject a
  * user, offer or group table too small for them.  Group codes and attribute value codes must therefore
  * come from stable, append-only dictionaries (INTEGRATION.md §3b).
@@ -451,6 +454,7 @@ typedef struct {
   cook_tasks_soa running;
   int32_t n_running_rm;
   const int64_t* running_rm_task_id;
+  const int32_t* running_hostname_id;
 } cook_state_delta;
 int32_t cook_state_apply(cook_pool* pool, const cook_state_delta* delta);
 
@@ -476,6 +480,28 @@ int32_t cook_state_match(cook_pool* pool, const cook_offers_soa* offers, const c
                          const cook_match_params* params, int64_t* out_considerable_job_id,
                          int32_t* out_assign, int32_t* out_ports, int32_t max_ports,
                          uint8_t* out_fail_reason, cook_match_stats* out_stats);
+
+/* cook_rebalance over the resident rows, as rebalancer.clj reads them: init-state (:222-266) takes every
+ * live running task on its host, and jobs-to-make-room-for (:588-590) the first max_preemption jobs of the
+ * last cook_state_rank's queue that are still live, still hold their generation (not removed or replaced
+ * since the rank) and are allowed to start, in queue order.  A running row's host is the index in `hosts`
+ * whose hostname_id equals the row's running_hostname_id.
+ * Outputs as cook_rebalance, except: pending_idx is the job's position among the jobs the walk took and
+ * out_decision_job_id[d] its job id; victims are task ids in out_victim_task_id (a synthetic victim, the
+ * task of the job an earlier decision e of the same walk placed, as -1 - e).  Capacity:
+ * out_decisions[max_preemption], out_decision_job_id[max_preemption], out_victim_task_id[victim_cap].
+ * Changes nothing resident: the caller applies the decisions through deltas, as transact-preemption! does.
+ * COOK_E_BADARG, before any device work and with the handle unchanged: no cook_state_rank yet, a null
+ * required argument, victim_cap < live running rows + max_preemption, a live running row whose hostname is
+ * -1 or a code no entry of `hosts` carries, a hostname_id twice (or negative) in `hosts`, a resident user
+ * code >= n_users, a pending group code >= n_groups, a pending attribute column >= max(1, n_attr_cols).
+ * COOK_E_UNSUPPORTED_CONSTRAINT in GPU DRU mode.  COOK_OK with *out_n = 0 where cook_rebalance returns
+ * early: max_preemption <= 0, hosts->n == 0, no job taken.  Uploads only the host table, the users'
+ * rebalance columns and the groups; cook_last_stats(COOK_PHASE_REBALANCE), ms_device including the gathers. */
+int32_t cook_state_rebalance(cook_pool* pool, const cook_host_table* hosts, const cook_groups* groups,
+                             const cook_user_table* users, const cook_rebalance_params* params,
+                             cook_decision* out_decisions, int64_t* out_decision_job_id,
+                             int64_t* out_victim_task_id, int32_t victim_cap, int32_t* out_n);
 
 /* ------------------------------------------------------------ phase timing */
 /* Device-side timing of the last call of each kind on this handle (CUDA events on the

@@ -158,7 +158,8 @@ JFN(jint, matchFailures)(JNIEnv* env, jclass k, jlong pool, jobject k_idx, jint 
 /* one batch from the tx-report tap: `pending` holds the jobs_from columns of the upserted rows */
 JFN(jint, stateApply)(JNIEnv* env, jclass k, jlong pool, jint reset, jint n_pending, jobjectArray pending,
                       jobject pending_priority, jobject pending_job_id, jint n_pending_rm, jobject pending_rm_job_id,
-                      jint n_running, jobjectArray running, jint n_running_rm, jobject running_rm_task_id) {
+                      jint n_running, jobjectArray running, jint n_running_rm, jobject running_rm_task_id,
+                      jobject running_hostname_id) {
   cook_state_delta d;
   memset(&d, 0, sizeof(d));
   d.reset = reset;
@@ -167,6 +168,7 @@ JFN(jint, stateApply)(JNIEnv* env, jclass k, jlong pool, jint reset, jint n_pend
   d.n_pending_rm = n_pending_rm; d.pending_rm_job_id = one(env, pending_rm_job_id);
   if (running) tasks_from(env, n_running, running, &d.running);
   d.n_running_rm = n_running_rm; d.running_rm_task_id = one(env, running_rm_task_id);
+  d.running_hostname_id = one(env, running_hostname_id);
   return cook_state_apply((cook_pool*)(intptr_t)pool, &d);
 }
 JFN(jint, stateRank)(JNIEnv* env, jclass k, jlong pool, jint n_users, jobjectArray users, jdoubleArray pool_quota,
@@ -199,6 +201,26 @@ JFN(jint, stateMatch)(JNIEnv* env, jclass k, jlong pool, jint n_offers, jint n_a
   return cook_state_match((cook_pool*)(intptr_t)pool, &o, have_g ? &g : NULL, &u, &pq, &prm,
                           one(env, out_considerable_job_id), one(env, out_assign), one(env, out_ports), max_ports,
                           one(env, out_fail), (cook_match_stats*)one(env, out_stats));
+}
+
+/* the rebalancer over the resident rows; out_victim_task_id holds victim_cap task ids */
+JFN(jint, stateRebalance)(JNIEnv* env, jclass k, jlong pool, jint n_hosts, jint n_attr_cols, jobjectArray hosts,
+                          jint n_groups, jobjectArray groups, jint n_users, jobjectArray users, jint max_preemption,
+                          jdouble min_dru_diff, jdouble safe_dru_threshold, jint host_lifetime_mins,
+                          jobject out_decisions, jobject out_decision_job_id, jobject out_victim_task_id,
+                          jint victim_cap, jintArray out_n) {
+  cook_host_table h; cook_groups g; cook_user_table u; cook_rebalance_params prm;
+  memset(&h, 0, sizeof(h)); memset(&g, 0, sizeof(g)); memset(&u, 0, sizeof(u));
+  hosts_from(env, n_hosts, n_attr_cols, hosts, &h);
+  int have_g = groups_from(env, n_groups, groups, &g); users_from(env, n_users, users, &u);
+  prm.max_preemption = max_preemption; prm.min_dru_diff = min_dru_diff; prm.safe_dru_threshold = safe_dru_threshold;
+  prm.host_lifetime_mins = host_lifetime_mins;
+  int32_t n = 0;
+  jint rc = cook_state_rebalance((cook_pool*)(intptr_t)pool, &h, have_g ? &g : NULL, &u, &prm,
+                                 (cook_decision*)one(env, out_decisions), one(env, out_decision_job_id),
+                                 one(env, out_victim_task_id), victim_cap, &n);
+  (*env)->SetIntArrayRegion(env, out_n, 0, 1, (jint*)&n);
+  return rc;
 }
 
 /* ---- B1-B6 ------------------------------------------------------------------------------------ */

@@ -9,6 +9,12 @@ identical.  The host arm's wall time excludes building its tables in Python.
 
   python tools/prof_state.py --pool c2 --cycles 8
   python tools/prof_state.py --pool c5 --c5-pool 5 --cycles 5      # the config-#5 pool of ~640 k jobs
+
+--rebalance instead loads a config-#4 pool's rebalancer input (running tasks on their hosts, pending jobs) into a
+resident handle, ranks it, and per cycle runs cook_state_rebalance against cook_rebalance on host tables holding
+the same rows (the queue's first max_preemption jobs): device time, wall time, bytes uploaded, identical outputs.
+
+  python tools/prof_state.py --rebalance --c4-pool 0 --cycles 5
 """
 import argparse
 import json
@@ -63,13 +69,56 @@ def card():
         return f"unknown ({e})"
 
 
+def rebalance(a):
+    r = traces.gen_config_pool("c4", a.c4_pool)["rebalance"]
+    rt, hosts, users, groups, prm = r["running"].col("t"), r["hosts"], r["users"], r["groups"], r["params"]
+    code = hosts.col("hostname_id")[r["running"].col("host")]
+    store = Jobs(r["pending"], r["pending_priority"], r["pending_job_id"])
+    print(json.dumps({"card": card(), "pool": f"c4/{a.c4_pool}", "running": rt.n, "pending": r["pending"].n,
+                      "hosts": hosts.n, "max_preemption": prm.max_preemption}), flush=True)
+    res, host = GpuEngine(pool_name="resident"), GpuEngine(pool_name="host")
+    rows = np.arange(r["pending"].n)
+    res.state_apply(abi.make_delta(reset=True, running=rt, running_hostname_id=code, pending=store.soa(rows),
+                                   pending_priority=store.prio, pending_job_id=store.jid))
+    q = res.state_rank(users)
+    pos = {int(j): i for i, j in enumerate(store.jid)}
+    take = np.array([pos[int(j)] for j in q[:prm.max_preemption]], np.int64)
+    hj, tid = store.soa(take), rt.col("task_id")
+    for cycle in range(a.cycles):
+        w0 = time.perf_counter()
+        got = res.state_rebalance(hosts, users, prm, groups=groups)
+        w_res = time.perf_counter() - w0
+        st_res = res.last_stats(abi.PHASE_REBALANCE)
+        w0 = time.perf_counter()
+        want = host.rebalance(r["running"], hj, store.jid[take], store.prio[take], hosts, users, prm, groups=groups)
+        w_host = time.perf_counter() - w0
+        st_host = host.last_stats(abi.PHASE_REBALANCE)
+        same = len(got) == len(want) and all(
+            (g["pending_idx"], g["host"], g["dru"], g["mem"], g["cpus"], g["gpus"]) ==
+            (w["pending_idx"], w["host"], w["dru"], w["mem"], w["cpus"], w["gpus"]) and
+            g["victims"] == [int(tid[v]) if v < rt.n else -1 - (v - rt.n) for v in w["victims"]] for g, w in zip(got, want))
+
+        def arm(s, wall):
+            return {**{k: round(s[k], 3) for k in ("ms_h2d", "ms_device", "ms_d2h")}, "wall_ms": round(1e3 * wall, 3),
+                    "h2d_bytes": s["h2d_bytes"], "n_launches": s["n_launches"]}
+
+        print(json.dumps({"cycle": cycle, "decisions": len(got), "resident": arm(st_res, w_res),
+                          "host": arm(st_host, w_host), "identical": bool(same)}), flush=True)
+    res.close()
+    host.close()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--pool", choices=("c2", "c5"), default="c2")
     ap.add_argument("--c5-pool", type=int, default=5)
+    ap.add_argument("--rebalance", action="store_true")
+    ap.add_argument("--c4-pool", type=int, default=0)
     ap.add_argument("--cycles", type=int, default=6)
     ap.add_argument("--seed", type=int, default=7)
     a = ap.parse_args()
+    if a.rebalance:
+        return rebalance(a)
     t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
     jobs, pc, rc = t["jobs"], t["cols"]["pending"], t["cols"]["running"]
     J = jobs.n
