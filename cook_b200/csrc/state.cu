@@ -13,6 +13,9 @@
 // generation, so a job removed or replaced since the rank leaves the queue.  A rebalance takes the first
 // allowed jobs of that queue and every live running task on its host, gathered into the columns the
 // rebalancer's build carved, and runs cook_rebalance's walk on them.
+// By job id, without re-sending rows: a launch moves pending rows to the running table on the device and
+// leaves the state a delta would; a patch writes the match-time columns (allowed, plugin_accept,
+// reserved_host) in place and keeps the generation, so the job keeps its queue entry.
 #include <algorithm>
 #include <map>
 #include <unordered_map>
@@ -37,14 +40,15 @@ enum { L_NOVEL = 0, L_ATTR = 1, L_GROUP = 2 };
 
 // ---- scatter: row i of a batch to slot[i].  Upserts write the columns (a null source writes the
 // column's absent value) and the rows' list ranges; removals clear the live flag.  Both bump the
-// generation, which is what retires a queue entry.
+// generation, which is what retires a queue entry.  A patch (live null) writes its columns only: the
+// slot keeps its live flag and generation, so its queue entry stays.
 constexpr int MAXC = 16;
 struct ScatterCol { char* dst; const char* src; long long dflt; int sz; };
 struct ScatterArgs {
   ScatterCol c[MAXC];
   int nc, n, upsert;
   const int32_t* slot;
-  uint8_t* live;
+  uint8_t* live;           // null: a patch
   uint32_t* gen;
   int32_t* loff[3];        // per-slot list range; null: the table has no lists
   int32_t* llen[3];
@@ -64,6 +68,7 @@ __global__ void scatter_kernel(ScatterArgs a) {
     else if (c.sz == 4) reinterpret_cast<int32_t*>(c.dst)[s] = c.src ? reinterpret_cast<const int32_t*>(c.src)[i] : (int32_t)c.dflt;
     else reinterpret_cast<long long*>(c.dst)[s] = c.src ? reinterpret_cast<const long long*>(c.src)[i] : c.dflt;
   }
+  if (!a.live) return;
   a.live[s] = a.upsert ? 1 : 0;
   a.gen[s] += 1u;
 #pragma unroll
@@ -74,6 +79,27 @@ __global__ void scatter_kernel(ScatterArgs a) {
       a.loff[l][s] = a.tail[l] + o;
       a.llen[l][s] = has ? a.doff[l][i + 1] - o : 0;
     }
+}
+
+// ---- launch: pending slot pslot[i] becomes running slot rslot[i].  What the task shares with its job moves
+// from the pending table; task id, start time and host (null: -1) come from the call.  The pending slot is
+// retired afterwards by a removal scatter.
+__global__ void launch_kernel(const int32_t* pslot, const int32_t* rslot, const int64_t* tid, const int64_t* start,
+                              const int32_t* host, void* const* pc, void* const* rc, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int s = pslot[i], r = rslot[i];
+  static_cast<int32_t*>(rc[R_USER])[r] = static_cast<const int32_t*>(pc[P_USER])[s];
+  static_cast<int32_t*>(rc[R_PRIO])[r] = static_cast<const int32_t*>(pc[P_PRIO])[s];
+  static_cast<int64_t*>(rc[R_JID])[r] = static_cast<const int64_t*>(pc[P_JID])[s];
+  static_cast<double*>(rc[R_CPUS])[r] = static_cast<const double*>(pc[P_CPUS])[s];
+  static_cast<double*>(rc[R_MEM])[r] = static_cast<const double*>(pc[P_MEM])[s];
+  static_cast<double*>(rc[R_GPUS])[r] = static_cast<const double*>(pc[P_GPUS])[s];
+  static_cast<int64_t*>(rc[R_START])[r] = start[i];
+  static_cast<int64_t*>(rc[R_TID])[r] = tid[i];
+  static_cast<int32_t*>(rc[R_HOST])[r] = host ? host[i] : -1;
+  static_cast<uint8_t*>(rc[R_LIVE])[r] = 1;
+  static_cast<uint32_t*>(rc[R_GEN])[r] += 1u;
 }
 
 // ---- list lengths for the order-wide scan (integer sums: any association is exact)
@@ -331,6 +357,7 @@ struct PoolState {
   std::map<int32_t, int64_t> users_p, users_r, attr_cols, groups;   // code -> live uses
   std::map<int32_t, int64_t> hosts_r;                               // running rows' hostname codes (-1 too)
   int64_t nflag[F_N] = {};
+  std::unordered_set<int32_t> reserved;   // the live pending slots whose reserved_host is not -1
   Arena stage;                        // one batch's uploads
   Arena scratch;                      // one call's device buffers
   Arena queue;                        // the ranked queue, carved by rank only: it lives until the match
@@ -358,7 +385,21 @@ struct PoolState {
     for (int32_t c : pi.attr_cols) count_add(attr_cols, c, sign);
     for (int l = 0; l < 3; l++) lists[l].live += sign * pi.len[l];
     for (int f = 0; f < F_N; f++) if ((pi.flags >> f) & 1) nflag[f] += sign;
-    (void)slot;
+    if ((pi.flags >> F_RESERVED) & 1) {
+      if (sign > 0) reserved.insert(slot);
+      else reserved.erase(slot);
+    }
+  }
+  // a live pending slot's flag f after a patch of its column
+  void set_flag(int32_t slot, int f, bool on) {
+    PendingInfo& pi = pinfo[slot];
+    if ((bool)((pi.flags >> f) & 1) == on) return;
+    pi.flags ^= (uint16_t)(1u << f);
+    nflag[f] += on ? 1 : -1;
+    if (f == F_RESERVED) {
+      if (on) reserved.insert(slot);
+      else reserved.erase(slot);
+    }
   }
 };
 
@@ -437,6 +478,27 @@ int32_t compact_lists(cook_pool* pool, PoolState* S, cudaStream_t st, int* nl) {
   return COOK_OK;
 }
 
+// one scatter_kernel launch of a batch's n rows into table t.  live_col < 0: a patch (live flag and generation
+// untouched); `tail` (the pending table's upserts and removals): where the batch's lists were appended.
+void scatter(ScatterArgs& a, Table& t, int n, int upsert, int live_col, const int32_t* tail, cudaStream_t st, int* nl) {
+  if (!n) return;
+  a.n = n; a.upsert = upsert;
+  if (live_col >= 0) {
+    a.live = static_cast<uint8_t*>(t.col[live_col]);
+    a.gen = static_cast<uint32_t*>(t.col[live_col + 1]);
+  }
+  if (tail) {
+    const int loff[3] = {P_NOFF, P_AOFF, P_GOFF};
+    for (int l = 0; l < 3; l++) {
+      a.loff[l] = static_cast<int32_t*>(t.col[loff[l]]);
+      a.llen[l] = static_cast<int32_t*>(t.col[loff[l] + 1]);
+      a.tail[l] = tail[l];
+    }
+  }
+  scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(a);
+  (*nl)++;
+}
+
 int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
   const cook_jobs_soa& P = d->pending;
   const cook_tasks_soa& T = d->running;
@@ -491,6 +553,7 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
       t->slot_of.clear(); t->free.clear(); t->hw = 0;
     }
     S->users_p.clear(); S->users_r.clear(); S->attr_cols.clear(); S->groups.clear(); S->hosts_r.clear();
+    S->reserved.clear();
     for (auto& f : S->nflag) f = 0;
     for (auto& l : S->lists) l.tail = l.live = 0;
   }
@@ -611,29 +674,156 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
   CK(pool, carved);
   CK(pool, cudaEventRecord(pool->ev[21], st));
   int nl = 0;
-  auto launch = [&](ScatterArgs& a, Table& t, int n, int upsert, int live_col, bool lists) {
-    if (!n) return;
-    a.n = n; a.upsert = upsert;
-    a.live = static_cast<uint8_t*>(t.col[live_col]);
-    a.gen = static_cast<uint32_t*>(t.col[live_col + 1]);
-    if (lists) {
-      const int loff[3] = {P_NOFF, P_AOFF, P_GOFF};
-      for (int l = 0; l < 3; l++) {
-        a.loff[l] = static_cast<int32_t*>(t.col[loff[l]]);
-        a.llen[l] = static_cast<int32_t*>(t.col[loff[l] + 1]);
-        a.tail[l] = tail0[l];
-      }
-    }
-    scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(a);
-    nl++;
-  };
-  launch(pr, S->pend, npr, 0, P_LIVE, true);
-  launch(rr, S->run, nrr, 0, R_LIVE, false);
-  launch(pu, S->pend, np, 1, P_LIVE, true);
-  launch(ru, S->run, nr, 1, R_LIVE, false);
+  scatter(pr, S->pend, npr, 0, P_LIVE, tail0, st, &nl);
+  scatter(rr, S->run, nrr, 0, R_LIVE, nullptr, st, &nl);
+  scatter(pu, S->pend, np, 1, P_LIVE, tail0, st, &nl);
+  scatter(ru, S->run, nr, 1, R_LIVE, nullptr, st, &nl);
   CK(pool, cudaGetLastError());
   int32_t rc = compact_lists(pool, S, st, &nl);
   if (rc != COOK_OK) return rc;
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  CK(pool, cudaStreamSynchronize(st));
+  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
+  return COOK_OK;
+}
+
+// the slots of n distinct live pending job ids, or why not
+const char* pending_slots(const PoolState* S, int n, const int64_t* job_id, std::vector<int32_t>* slot) {
+  std::unordered_set<int64_t> seen;
+  seen.reserve((size_t)n);
+  slot->resize(n);
+  for (int i = 0; i < n; i++) {
+    if (!seen.insert(job_id[i]).second) return "job id twice";
+    auto it = S->pend.slot_of.find(job_id[i]);
+    if (it == S->pend.slot_of.end()) return "unknown job id";
+    (*slot)[i] = it->second;
+  }
+  return nullptr;
+}
+
+// pending_rm = job_id plus the running upserts built from the rows, without their columns crossing the bus
+int32_t launch(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, const int64_t* task_id,
+               const int64_t* start_time, const int32_t* hostname_id) {
+  if (n < 0) return set_err(pool, COOK_E_BADARG, "cook_state_launch: n < 0");
+  if (n && (!job_id || !task_id || !start_time))
+    return set_err(pool, COOK_E_BADARG, "cook_state_launch: null job_id, task_id or start_time");
+  if (!idx_in_range(hostname_id, n, -1, INT32_MAX))
+    return set_err(pool, COOK_E_BADARG, "cook_state_launch: a hostname code below -1");
+  std::vector<int32_t> pslot, rslot(n);
+  if (const char* why = pending_slots(S, n, job_id, &pslot)) return set_err(pool, COOK_E_BADARG, "cook_state_launch: %s", why);
+  {
+    std::unordered_set<int64_t> seen;
+    seen.reserve((size_t)n);
+    for (int i = 0; i < n; i++) {
+      if (!seen.insert(task_id[i]).second) return set_err(pool, COOK_E_BADARG, "cook_state_launch: task id twice");
+      if (S->run.slot_of.count(task_id[i])) return set_err(pool, COOK_E_BADARG, "cook_state_launch: task id already running");
+    }
+  }
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  // ---- host side, in cook_state_apply's order: the removals free their slots, then the tasks take theirs
+  for (int i = 0; i < n; i++) {
+    const int32_t s = pslot[i];
+    S->pend.slot_of.erase(job_id[i]);
+    S->add_pending(s, S->pinfo[s], -1);
+    S->pend.free.push_back(s);
+  }
+  for (int i = 0; i < n; i++) {
+    const int32_t r = S->run.take_slot();
+    S->run.slot_of.emplace(task_id[i], r);
+    if ((size_t)r >= S->ruser.size()) {
+      S->ruser.resize(std::max<size_t>(r + 1, 2 * S->ruser.size()));
+      S->rhost.resize(S->ruser.size());
+    }
+    S->ruser[r] = S->pinfo[pslot[i]].user;
+    S->rhost[r] = hostname_id ? hostname_id[i] : -1;
+    count_add(S->users_r, S->ruser[r], +1);
+    count_add(S->hosts_r, S->rhost[r], +1);
+    rslot[i] = r;
+  }
+  // ---- device: capacity, the upload, the move, the pending slots' removal, then the arena rule
+  CK(pool, S->run.grow(S->run.hw, st));
+  const int32_t *d_pslot = nullptr, *d_rslot = nullptr, *d_host = nullptr;
+  const int64_t *d_tid = nullptr, *d_start = nullptr;
+  int64_t h2d = 0;
+  CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
+    if (!n) return;
+    d_pslot = c.up(pslot.data(), n); d_rslot = c.up(rslot.data(), n);
+    d_tid = c.up(task_id, n); d_start = c.up(start_time, n);
+    d_host = c.up(hostname_id, n);
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  int nl = 0;
+  if (n) {
+    launch_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_pslot, d_rslot, d_tid, d_start, d_host, S->pend.d_col,
+                                                   S->run.d_col, n);
+    nl++;
+    ScatterArgs rm;
+    memset(&rm, 0, sizeof(rm));
+    rm.slot = d_pslot;
+    int32_t tail[3];
+    for (int l = 0; l < 3; l++) tail[l] = (int32_t)S->lists[l].tail;
+    scatter(rm, S->pend, n, 0, P_LIVE, tail, st, &nl);
+  }
+  CK(pool, cudaGetLastError());
+  int32_t rc = compact_lists(pool, S, st, &nl);
+  if (rc != COOK_OK) return rc;
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  CK(pool, cudaStreamSynchronize(st));
+  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
+  return COOK_OK;
+}
+
+// the given match-time columns of live pending rows, in place; clear: every reservation is dropped first
+int32_t patch(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, const uint8_t* allowed,
+              const uint8_t* plugin_accept, const int32_t* reserved_host, bool clear) {
+  if (n < 0) return set_err(pool, COOK_E_BADARG, "cook_state_patch: n < 0");
+  if (n && !job_id) return set_err(pool, COOK_E_BADARG, "cook_state_patch: null job_id");
+  if (!idx_in_range(reserved_host, n, -1, INT32_MAX))
+    return set_err(pool, COOK_E_BADARG, "cook_state_patch: a reserved_host below -1");
+  std::vector<int32_t> slot;
+  if (const char* why = pending_slots(S, n, job_id, &slot)) return set_err(pool, COOK_E_BADARG, "cook_state_patch: %s", why);
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  // ---- host side: the per-slot flags and their counts, O(n + reservations cleared)
+  std::vector<int32_t> cleared;
+  if (clear) {
+    cleared.assign(S->reserved.begin(), S->reserved.end());
+    for (int32_t s : cleared) S->set_flag(s, F_RESERVED, false);
+  }
+  for (int i = 0; i < n; i++) {
+    const int32_t s = slot[i];
+    if (allowed) S->set_flag(s, F_NOT_ALLOWED, !allowed[i]);
+    if (plugin_accept) S->set_flag(s, F_NOT_PLUGIN, !plugin_accept[i]);
+    if (reserved_host) S->set_flag(s, F_RESERVED, reserved_host[i] != -1);
+  }
+  // ---- device: the cleared slots get -1, then the batch's columns
+  const int nc = (int)cleared.size();
+  const bool cols = n && (allowed || plugin_accept || reserved_host);
+  ScatterArgs cl, pa;
+  memset(&cl, 0, sizeof(cl)); memset(&pa, 0, sizeof(pa));
+  int64_t h2d = 0;
+  CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
+    if (nc) {
+      cl.c[0] = ScatterCol{static_cast<char*>(S->pend.col[P_RESERVED]), nullptr, -1, P_SZ[P_RESERVED]};
+      cl.nc = 1;
+      cl.slot = c.up(cleared.data(), nc);
+    }
+    if (cols) {
+      pa.slot = c.up(slot.data(), n);
+      if (allowed) pa.c[pa.nc++] = ScatterCol{static_cast<char*>(S->pend.col[P_ALLOWED]),
+                                              reinterpret_cast<const char*>(c.up(allowed, n)), 1, 1};
+      if (plugin_accept) pa.c[pa.nc++] = ScatterCol{static_cast<char*>(S->pend.col[P_PLUGIN]),
+                                                    reinterpret_cast<const char*>(c.up(plugin_accept, n)), 1, 1};
+      if (reserved_host) pa.c[pa.nc++] = ScatterCol{static_cast<char*>(S->pend.col[P_RESERVED]),
+                                                    reinterpret_cast<const char*>(c.up(reserved_host, n)), -1, 4};
+    }
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  int nl = 0;
+  scatter(cl, S->pend, nc, 0, -1, nullptr, st, &nl);
+  scatter(pa, S->pend, cols ? n : 0, 0, -1, nullptr, st, &nl);
+  CK(pool, cudaGetLastError());
   CK(pool, cudaEventRecord(pool->ev[22], st));
   CK(pool, cudaStreamSynchronize(st));
   record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
@@ -649,6 +839,25 @@ extern "C" int32_t cook_state_apply(cook_pool* pool, const cook_state_delta* del
   PoolState* S = state_of(pool, true);
   if (!S) return set_err(pool, COOK_E_OOM, "cook_state_apply: out of device memory");
   return apply(pool, S, delta);
+}
+
+extern "C" int32_t cook_state_launch(cook_pool* pool, int32_t n, const int64_t* job_id, const int64_t* task_id,
+                                     const int64_t* start_time, const int32_t* hostname_id) {
+  if (!pool) return COOK_E_BADARG;
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_launch: out of device memory");
+  return launch(pool, S, n, job_id, task_id, start_time, hostname_id);
+}
+
+extern "C" int32_t cook_state_patch(cook_pool* pool, int32_t n, const int64_t* job_id, const uint8_t* allowed,
+                                    const uint8_t* plugin_accept, const int32_t* reserved_host,
+                                    int32_t clear_reservations) {
+  if (!pool) return COOK_E_BADARG;
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_patch: out of device memory");
+  return patch(pool, S, n, job_id, allowed, plugin_accept, reserved_host, clear_reservations != 0);
 }
 
 extern "C" int32_t cook_state_rank(cook_pool* pool, const cook_user_table* users, const cook_pool_quota* pool_quota,

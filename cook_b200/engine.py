@@ -62,7 +62,7 @@ def load_library(path=None):
                  "cook_allgather_usage", "cook_last_stats", "cook_comm_unique_id", "cook_comm_init",
                  "cook_comm_destroy", "cook_exchange_usage", "cook_exchange_usage_batch", "cook_rebalance_trace",
                  "cook_match_failures", "cook_state_apply", "cook_state_rank", "cook_state_match",
-                 "cook_state_rebalance"):
+                 "cook_state_rebalance", "cook_state_launch", "cook_state_patch"):
         getattr(lib, name).restype = C.c_int32
     return lib
 
@@ -175,6 +175,42 @@ class GpuEngine:
         tid = delta.col("running").col("task_id") if delta.running.n else None
         run.update(tid.tolist() if tid is not None else [])
         self._state_running_ids = run
+
+    def state_launch(self, job_id, task_id, start_time, hostname_id=None):
+        """cook_state_launch: live pending job job_id[i] becomes running task task_id[i] (started at
+        start_time[i] on hostname code hostname_id[i]; None: host unknown), its columns copied on the device."""
+        jid = np.ascontiguousarray(job_id, np.int64)
+        tid = np.ascontiguousarray(task_id, np.int64)
+        st = np.ascontiguousarray(start_time, np.int64)
+        hn = np.ascontiguousarray(hostname_id, np.int32) if hostname_id is not None else None
+        if not (len(tid) == len(st) == len(jid) and (hn is None or len(hn) == len(jid))):
+            raise ValueError("state_launch: job_id, task_id, start_time and hostname_id differ in length")
+        rc = self.lib.cook_state_launch(self.pool, len(jid), abi.ptr(jid, abi.P_I64), abi.ptr(tid, abi.P_I64),
+                                        abi.ptr(st, abi.P_I64), abi.ptr(hn, abi.P_I32) if hn is not None else None)
+        if rc != 0:
+            self._err(rc)
+        live = getattr(self, "_state_pending_ids", set())
+        live.difference_update(jid.tolist())
+        self._state_pending_ids = live
+        run = getattr(self, "_state_running_ids", set())
+        run.update(tid.tolist())
+        self._state_running_ids = run
+
+    def state_patch(self, job_id, allowed=None, plugin_accept=None, reserved_host=None, clear_reservations=False):
+        """cook_state_patch: the given match-time columns of live pending jobs, in place (None: unchanged).
+        The jobs keep their place in the queue.  clear_reservations: every reservation is dropped first."""
+        jid = np.ascontiguousarray(job_id, np.int64)
+        cols = [np.ascontiguousarray(c, dt) if c is not None else None
+                for c, dt in ((allowed, np.uint8), (plugin_accept, np.uint8), (reserved_host, np.int32))]
+        if any(c is not None and len(c) != len(jid) for c in cols):
+            raise ValueError("state_patch: a column's length differs from job_id's")
+        al, pa, rh = cols
+        rc = self.lib.cook_state_patch(self.pool, len(jid), abi.ptr(jid, abi.P_I64),
+                                       abi.ptr(al, abi.P_U8) if al is not None else None,
+                                       abi.ptr(pa, abi.P_U8) if pa is not None else None,
+                                       abi.ptr(rh, abi.P_I32) if rh is not None else None, int(bool(clear_reservations)))
+        if rc != 0:
+            self._err(rc)
 
     def state_rank(self, users, pool_quota=None, group_quota=None, group_usage=None, params=None):
         """cook_state_rank: the live rows ranked; the queue stays on the device.  Returns its job ids."""

@@ -435,7 +435,9 @@ int32_t cook_rebalance_trace(cook_pool* pool, const cook_running_soa* running,
  *   running_hostname_id the host of each running upsert: a code of the global hostname dictionary (the
  *                       code space of cook_offers_soa.hostname_id and cook_host_table.hostname_id).  NULL
  *                       stores -1, "host unknown"; only cook_state_rebalance reads it.
- * A launch is one batch: remove pending job j, upsert its running task.
+ * A launch can be one batch (remove pending job j, upsert its running task); cook_state_launch does the
+ * same from job ids without re-sending the rows.  An upsert of a pending row gives it a new generation,
+ * so it leaves the last rank's queue; cook_state_patch changes the match-time columns without that.
  * COOK_E_BADARG, state unchanged: an unknown id in a removal, an id twice in one table of the batch, a
  * malformed CSR offset column, a negative user / attr_col / group / novel hostname code, a
  * reserved_host or running_hostname_id below -1.
@@ -458,6 +460,34 @@ typedef struct {
 } cook_state_delta;
 int32_t cook_state_apply(cook_pool* pool, const cook_state_delta* delta);
 
+/* Launches by job id: live pending job job_id[i] becomes running task task_id[i], started at start_time[i] on
+ * hostname_id[i] (a code of the global hostname dictionary; a NULL column stores -1, "host unknown").  User,
+ * priority, job id, cpus, mem and gpus are copied on the device from the pending row.  Leaves exactly the
+ * state cook_state_apply leaves after the batch pending_rm_job_id = job_id plus the running upserts built
+ * from those rows with running_hostname_id = hostname_id: the job leaves the last rank's queue, its list
+ * entries, counts and reservation leave with the row, and the list arenas compact by the same rule.
+ * COOK_E_BADARG, before any change: n < 0; a NULL job_id, task_id or start_time while n > 0; a job id that
+ * is not live or appears twice; a task id that appears twice or is already live; a hostname code below -1.
+ * Uploads exactly n * (4 + 4 + 8 + 8) bytes (pending slot, running slot, task id, start time), plus 4 * n
+ * when hostname_id is not NULL.  Statistics: cook_last_stats(COOK_PHASE_STATE).                        */
+int32_t cook_state_launch(cook_pool* pool, int32_t n, const int64_t* job_id, const int64_t* task_id,
+                          const int64_t* start_time, const int32_t* hostname_id);
+
+/* The columns Cook reads from live state at match time, written in place on live pending rows:
+ * allowed (job-allowed-to-start?), plugin_accept (the launch-filter plugin) and reserved_host (the
+ * rebalancer's reservation map); a NULL column is left unchanged.  Unlike an upsert, a patch keeps the
+ * row's live flag and generation: the job keeps its place in the last rank's queue, and the next
+ * cook_state_match and cook_state_rebalance read the new values.  clear_reservations != 0 first sets
+ * reserved_host = -1 on every live row that holds one, then writes the batch: reserve-hosts! replacing the
+ * whole map.  Priority is not patchable: the order changes only at the next rank (an upsert, as before).
+ * COOK_E_BADARG, before any change: n < 0; a NULL job_id while n > 0; a job id that is not live or appears
+ * twice; a reserved_host below -1.
+ * Uploads exactly: when n > 0 and some column is given, n * (4 + [allowed] 1 + [plugin_accept] 1 +
+ * [reserved_host] 4) bytes (a slot per row plus each non-NULL column); when clearing, 4 bytes per live row
+ * that held a reservation.  Statistics: cook_last_stats(COOK_PHASE_STATE).                              */
+int32_t cook_state_patch(cook_pool* pool, int32_t n, const int64_t* job_id, const uint8_t* allowed,
+                         const uint8_t* plugin_accept, const int32_t* reserved_host, int32_t clear_reservations);
+
 /* cook_rank over the live rows (running = live running tasks, pending = live pending jobs).  The ranked
  * queue stays on the device as the handle's resident queue; out_ranked_job_id[<= #pending] (may be
  * NULL) receives it as job ids, *out_n its length.  Rank is a total order on (user, -priority, start,
@@ -468,7 +498,7 @@ int32_t cook_state_rank(cook_pool* pool, const cook_user_table* users, const coo
                         const cook_rank_params* params, int64_t* out_ranked_job_id, int32_t* out_n);
 
 /* cook_match with ranked_idx = the resident queue minus every job removed or replaced since that
- * cook_state_rank, reading the rows' current columns (a changed reserved_host or allowed counts).
+ * cook_state_rank, reading the rows' current columns (what cook_state_patch wrote since the rank counts).
  * Outputs as cook_match, with the job id of the k-th considerable job in out_considerable_job_id[k];
  * afterwards cook_match_failures and cook_exchange_usage(_batch) work on this round, their k being
  * positions in out_considerable_job_id.  Uploads only the offers, the users' match columns and the
@@ -506,7 +536,8 @@ int32_t cook_state_rebalance(cook_pool* pool, const cook_host_table* hosts, cons
 /* ------------------------------------------------------------ phase timing */
 /* Device-side timing of the last call of each kind on this handle (CUDA events on the
  * pool's stream): what bench.py's `phases` block and roofline lines are computed from.
- * COOK_PHASE_STATE: the last cook_state_apply (upload, then the scatter / compaction kernels). */
+ * COOK_PHASE_STATE: the last cook_state_apply, cook_state_launch or cook_state_patch (upload, then the
+ * scatter / move / compaction kernels). */
 enum { COOK_PHASE_RANK = 0, COOK_PHASE_MATCH = 1, COOK_PHASE_REBALANCE = 2, COOK_PHASE_EXCHANGE = 3,
        COOK_PHASE_STATE = 4 };
 typedef struct {

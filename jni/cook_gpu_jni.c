@@ -171,6 +171,19 @@ JFN(jint, stateApply)(JNIEnv* env, jclass k, jlong pool, jint reset, jint n_pend
   d.running_hostname_id = one(env, running_hostname_id);
   return cook_state_apply((cook_pool*)(intptr_t)pool, &d);
 }
+/* launches by job id: the task columns the device already holds are not sent (hostname_id may be null) */
+JFN(jint, stateLaunch)(JNIEnv* env, jclass k, jlong pool, jint n, jobject job_id, jobject task_id, jobject start_time,
+                       jobject hostname_id) {
+  return cook_state_launch((cook_pool*)(intptr_t)pool, n, one(env, job_id), one(env, task_id), one(env, start_time),
+                           one(env, hostname_id));
+}
+/* match-time columns of pending jobs in place (a null column is unchanged); clear_reservations != 0 first
+ * drops every reservation (reserve-hosts!) */
+JFN(jint, statePatch)(JNIEnv* env, jclass k, jlong pool, jint n, jobject job_id, jobject allowed, jobject plugin_accept,
+                      jobject reserved_host, jint clear_reservations) {
+  return cook_state_patch((cook_pool*)(intptr_t)pool, n, one(env, job_id), one(env, allowed), one(env, plugin_accept),
+                          one(env, reserved_host), clear_reservations);
+}
 JFN(jint, stateRank)(JNIEnv* env, jclass k, jlong pool, jint n_users, jobjectArray users, jdoubleArray pool_quota,
                      jdoubleArray group_quota, jobject group_usage, jint max_over_quota_jobs, jint filter_offensive,
                      jdouble off_mem_mb, jdouble off_cpus, jobject out_ranked_job_id, jintArray out_n) {

@@ -15,6 +15,15 @@ resident handle, ranks it, and per cycle runs cook_state_rebalance against cook_
 the same rows (the queue's first max_preemption jobs): device time, wall time, bytes uploaded, identical outputs.
 
   python tools/prof_state.py --rebalance --c4-pool 0 --cycles 5
+
+--launch runs the same cycles on two resident handles instead of the host arm.  Each cycle's launches go to one
+handle through cook_state_launch (job ids, task ids, start times, the hosts the match chose) and to its twin through
+the equivalent cook_state_apply batch (the jobs' removal plus their task rows); the rest of the batch goes to both
+as one delta.  Per cycle and arm it prints the launch call's bytes uploaded, device time and host wall time around
+the (synchronising) binding call, and whether the following rank and match outputs of the two handles are identical.
+
+  python tools/prof_state.py --launch --pool c2 --cycles 6
+  python tools/prof_state.py --launch --pool c5 --c5-pool 5 --cycles 4
 """
 import argparse
 import json
@@ -108,11 +117,44 @@ def rebalance(a):
     host.close()
 
 
+def launch_cycle(cycle, res, twin, job_id, lt, hosts, rest, match_args):
+    """One cycle of --launch: the launches by id on `res` and as a delta on `twin`, the rest of the batch on both,
+    then rank and match on both.  Returns the jobs the match placed and their hosts' codes."""
+    users, offers, params, groups, max_ports = match_args
+    n = len(job_id)
+    d = abi.make_delta(running=abi.make_tasks(**lt) if n else None, pending_rm=job_id,
+                       running_hostname_id=hosts if n else None)
+    w0 = time.perf_counter()
+    res.state_launch(job_id, lt["task_id"], lt["start_time"], hosts)
+    w_launch = time.perf_counter() - w0
+    st_launch = res.last_stats(abi.PHASE_STATE)
+    w0 = time.perf_counter()
+    twin.state_apply(d)
+    w_delta = time.perf_counter() - w0
+    st_delta = twin.last_stats(abi.PHASE_STATE)
+    for e in (res, twin):
+        e.state_apply(rest)
+    q, q2 = res.state_rank(users), twin.state_rank(users)
+    m1 = res.state_match(offers, users, params, groups=groups, max_ports=max_ports)
+    m2 = twin.state_match(offers, users, params, groups=groups, max_ports=max_ports)
+    same = np.array_equal(q, q2) and all(np.array_equal(m1[k], m2[k]) for k in ("considerable", "assign", "ports", "fail"))
+
+    def arm(s, wall):
+        return {"h2d_bytes": s["h2d_bytes"], "ms_h2d": round(s["ms_h2d"], 3), "ms_device": round(s["ms_device"], 3),
+                "wall_ms": round(1e3 * wall, 3), "n_launches": s["n_launches"]}
+
+    print(json.dumps({"cycle": cycle, "launched": n, "launch": arm(st_launch, w_launch), "delta": arm(st_delta, w_delta),
+                      "identical": bool(same), "n_matched": int(m1["stats"]["n_matched"])}), flush=True)
+    ok = m1["assign"] >= 0
+    return m1["considerable"][ok], offers.col("hostname_id")[m1["assign"][ok]].astype(np.int32)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--pool", choices=("c2", "c5"), default="c2")
     ap.add_argument("--c5-pool", type=int, default=5)
     ap.add_argument("--rebalance", action="store_true")
+    ap.add_argument("--launch", action="store_true")
     ap.add_argument("--c4-pool", type=int, default=0)
     ap.add_argument("--cycles", type=int, default=6)
     ap.add_argument("--seed", type=int, default=7)
@@ -135,15 +177,19 @@ def main():
     users, offers, groups = t["users"], t["offers"], t.get("groups")
     params = traces.match_params(J, host_lifetime_mins=t.get("host_lifetime_mins", 0))
     max_ports = int(jobs.col("ports").max()) if jobs.col("ports") is not None else 0
-    res, host = GpuEngine(pool_name="resident"), GpuEngine(pool_name="host")
+    # --launch: `host` is the twin resident handle that receives launches as deltas
+    res, host = GpuEngine(pool_name="resident"), GpuEngine(pool_name="twin" if a.launch else "host")
     pos_of = {int(j): i for i, j in enumerate(store.jid)}
     next_jid = int(store.jid.max()) + 10
 
     def pend_delta(rows):
         return dict(pending=store.soa(rows), pending_priority=store.prio[rows], pending_job_id=store.jid[rows])
 
-    res.state_apply(abi.make_delta(reset=True, running=abi.make_tasks(**run), **pend_delta(np.flatnonzero(alive))))
+    init =abi.make_delta(reset=True, running=abi.make_tasks(**run), **pend_delta(np.flatnonzero(alive)))
+    for e in (res, host) if a.launch else (res,):
+        e.state_apply(init)
     placed = np.zeros(0, np.int64)
+    placed_host = np.zeros(0, np.int32)
     for cycle in range(a.cycles):
         # ---- the batch
         launch_rows = np.array([pos_of[int(j)] for j in placed], np.int64)
@@ -173,9 +219,14 @@ def main():
         chg = rng.choice(live, min(len(live), max(1, len(live) // 1000)), replace=False)
         store.prio[chg] = rng.choice(np.array([10, 50, 90], np.int32), len(chg))
         up = np.concatenate([sub, chg])
+        run = {k: np.concatenate([v[keep], lt[k]]) for k, v in run.items()}
+        if a.launch:
+            placed, placed_host = launch_cycle(cycle, res, host, launched_ids, lt, placed_host,
+                                               abi.make_delta(running_rm=fin_ids, **pend_delta(up)),
+                                               (users, offers, params, groups, max_ports))
+            continue
         d = abi.make_delta(running=abi.make_tasks(**lt) if len(launch_rows) else None, pending_rm=launched_ids,
                            running_rm=fin_ids, **pend_delta(up))
-        run = {k: np.concatenate([v[keep], lt[k]]) for k, v in run.items()}
         w0 = time.perf_counter()
         res.state_apply(d)
         w_apply = time.perf_counter() - w0
