@@ -139,7 +139,7 @@ class PhaseStats(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved0"}
 
 
-PHASE_RANK, PHASE_MATCH, PHASE_REBALANCE, PHASE_EXCHANGE, PHASE_STATE = 0, 1, 2, 3, 4
+PHASE_RANK, PHASE_MATCH, PHASE_REBALANCE, PHASE_EXCHANGE, PHASE_STATE, PHASE_USAGE = 0, 1, 2, 3, 4, 5
 
 
 class StateDelta(_SoA):

@@ -16,12 +16,15 @@
 // By job id, without re-sending rows: a launch moves pending rows to the running table on the device and
 // leaves the state a delta would; a patch writes the match-time columns (allowed, plugin_accept,
 // reserved_host) in place and keeps the generation, so the job keeps its queue entry.
+// Running usage per user, of the pool and per listed host: the live running rows compacted, sorted by (key, task
+// id) and folded per segment, each sum a left fold in ascending task id (DESIGN.md §2).
 #include <algorithm>
 #include <map>
 #include <unordered_map>
 #include <unordered_set>
 
 #include "fold.cuh"
+#include "sort.cuh"
 
 namespace {
 
@@ -254,6 +257,90 @@ __global__ void reb_pending_kernel(RebRows r, void* const* col, const int32_t* m
   writable(o.disk_type)[d] = static_cast<const int32_t*>(col[P_DISK_TYPE])[s];
   writable(o.est_end_ms)[d] = static_cast<const int64_t*>(col[P_EST])[s];
   writable(o.ckpt_location)[d] = static_cast<const int32_t*>(col[P_CKPT])[s];
+}
+
+// ---- running usage: the live running rows, dense in slot order; host = the index of the row's hostname
+// code in the caller's list, or H when the row's host is -1 or not listed (a segment no output reads)
+struct UsageRows {
+  void* const* col;
+  int32_t* user; int64_t* tid; int32_t* host; double* amt[3];   // host null: no host list
+  const int32_t* host_of; int32_t n_codes, H;
+  __device__ bool keep(int i) const { return static_cast<const uint8_t*>(col[R_LIVE])[i]; }
+  __device__ void emit(int i, int d) const {
+    user[d] = static_cast<const int32_t*>(col[R_USER])[i];
+    tid[d] = static_cast<const int64_t*>(col[R_TID])[i];
+    amt[0][d] = static_cast<const double*>(col[R_CPUS])[i];
+    amt[1][d] = static_cast<const double*>(col[R_MEM])[i];
+    amt[2][d] = static_cast<const double*>(col[R_GPUS])[i];
+    if (host) {
+      const int32_t code = static_cast<const int32_t*>(col[R_HOST])[i];
+      const int32_t h = code >= 0 && code < n_codes ? host_of[code] : -1;
+      host[d] = h < 0 ? H : h;
+    }
+  }
+};
+// (key, task id); key null: task id alone.  Task ids are unique among live rows, so the order is total.
+struct LessKeyTid {
+  const int32_t* key; const int64_t* tid;
+  __device__ bool operator()(int32_t a, int32_t b) const {
+    if (key && key[a] != key[b]) return key[a] < key[b];
+    return tid[a] < tid[b];
+  }
+};
+struct LoadSorted {   // the order-wide scan's addends: cpus, mem, gpus of the row at position p
+  const int32_t* ord; const double* amt[3];
+  __device__ void operator()(int p, double (&x)[3]) const {
+    const int i = ord[p];
+    x[0] = amt[0][i]; x[1] = amt[1][i]; x[2] = amt[2][i];
+  }
+};
+// The segments of one kind: segment g is positions [start[g], end[g]) of `ord` (start null: [0, R)).
+// `scan`: os holds the order-wide scan of ord, read when the whole order is on the grid.
+struct UsageSegs {
+  const int32_t* ord; const int32_t* start; const int32_t* end;
+  OrderScan<double, 3> os; int scan, n;
+};
+enum { US_USER, US_HOST, US_POOL, US_N };
+struct UsageArgs {
+  UsageSegs seg[US_N];
+  const double* amt[3];
+  const GridFlag* gf; int R;
+  double* user_out; int U;                                 // [4][U]: count, cpus, mem, gpus
+  double* host_cpus; double* host_mem; int32_t* host_count; // [H]
+  double* pool_out;                                        // [4]
+};
+
+// Warp per segment (users, then hosts, then the pool): the left fold of cpus, mem and gpus in the segment's
+// order (ascending task id within it).  The whole order on the grid: the two ends of the order-wide scan;
+// else warp_fold_sum, association-free when the segment alone is on the grid, else the serial chain.
+__global__ void __launch_bounds__(128) usage_fold_kernel(UsageArgs a) {
+  __shared__ double stage[4][3][32];
+  int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, kind = 0;
+  while (kind < US_N && g >= a.seg[kind].n) g -= a.seg[kind++].n;
+  if (kind == US_N) return;
+  const UsageSegs& q = a.seg[kind];
+  const int s = q.start ? q.start[g] : 0, e = q.start ? q.end[g] : a.R;
+  double acc[3] = {0.0, 0.0, 0.0};
+  if (q.scan && grid_exact(a.gf, a.R)) {
+    if (e > s)
+#pragma unroll
+      for (int k = 0; k < 3; k++) acc[k] = q.os.segment_sum(k, e - 1, s);
+  } else {
+    warp_fold_sum<3, 4>(acc, e - s, grid_exact(a.gf, e - s), [&](int k, double (&x)[3]) {
+      const int i = q.ord[s + k];
+      x[0] = a.amt[0][i]; x[1] = a.amt[1][i]; x[2] = a.amt[2][i];
+      return true;
+    }, stage[threadIdx.x >> 5]);
+  }
+  if (threadIdx.x & 31) return;
+  if (kind == US_USER) {
+    a.user_out[g] = (double)(e - s);
+    a.user_out[a.U + g] = acc[0]; a.user_out[2 * a.U + g] = acc[1]; a.user_out[3 * a.U + g] = acc[2];
+  } else if (kind == US_HOST) {
+    a.host_count[g] = e - s; a.host_cpus[g] = acc[0]; a.host_mem[g] = acc[1];
+  } else {
+    a.pool_out[0] = (double)(e - s); a.pool_out[1] = acc[0]; a.pool_out[2] = acc[1]; a.pool_out[3] = acc[2];
+  }
 }
 
 // ---- host side
@@ -830,6 +917,124 @@ int32_t patch(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, const
   return COOK_OK;
 }
 
+// the running usage per user, of the pool and per listed host, each a left fold in ascending task id
+int32_t usage(cook_pool* pool, PoolState* S, int U, double* out_user, double* out_pool, int H, const int32_t* hostname_id,
+              double* out_run_cpus, double* out_run_mem, int32_t* out_run_count) {
+  // ---- every check before any device work: the rows' codes from the host-side counts, the list itself
+  if (out_user && count_max(S->users_r) >= U)
+    return set_err(pool, COOK_E_BADARG, "cook_state_usage: a live running row's user code is >= n_users");
+  if (H < 0) return set_err(pool, COOK_E_BADARG, "cook_state_usage: n_hosts < 0");
+  if (H > 0 && !hostname_id) return set_err(pool, COOK_E_BADARG, "cook_state_usage: null hostname_id");
+  int32_t n_codes = 0;
+  {
+    std::unordered_set<int32_t> codes;
+    codes.reserve((size_t)H);
+    for (int h = 0; h < H; h++) {
+      const int32_t c = hostname_id[h];
+      if (c < 0 || !codes.insert(c).second)
+        return set_err(pool, COOK_E_BADARG, "cook_state_usage: a hostname_id is negative or twice in the list");
+      n_codes = std::max(n_codes, c + 1);
+    }
+  }
+  const int R = (int)S->run.slot_of.size();
+  const bool users = out_user && U > 0, hosts = H > 0 && (out_run_cpus || out_run_mem || out_run_count);
+  if (R == 0) {   // nothing live: every sum is the empty fold
+    if (users) memset(out_user, 0, sizeof(double) * 4 * (size_t)U);
+    if (out_pool) memset(out_pool, 0, sizeof(double) * 4);
+    if (out_run_cpus) memset(out_run_cpus, 0, sizeof(double) * (size_t)H);
+    if (out_run_mem) memset(out_run_mem, 0, sizeof(double) * (size_t)H);
+    if (out_run_count) memset(out_run_count, 0, sizeof(int32_t) * (size_t)H);
+    pool->phase[COOK_PHASE_USAGE] = cook_phase_stats{};
+    return COOK_OK;
+  }
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  UsageRows rows = {};
+  rows.col = S->run.d_col; rows.n_codes = n_codes; rows.H = H;
+  UsageArgs a = {};
+  int32_t *blk = nullptr, *tmp = nullptr, *d_codes = nullptr, *host_of = nullptr;
+  GridFlag* gf = nullptr;
+  int64_t h2d = 0, d2h = 0;
+  CK(pool, carve(S->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+    rows.user = c.take<int32_t>(R); rows.tid = c.take<int64_t>(R);
+    for (int k = 0; k < 3; k++) rows.amt[k] = c.take<double>(R);
+    blk = c.take<int32_t>((size_t)S->run.hw / CP_BLOCK + 2);
+    tmp = c.take<int32_t>(R);
+    gf = c.take<GridFlag>(1);
+    const auto segs = [&](UsageSegs& q, int n_seg, bool bounds) {
+      q.n = n_seg;
+      q.ord = c.take<int32_t>(R);
+      if (!bounds) return;
+      q.start = c.take<int32_t>(n_seg + 1); q.end = c.take<int32_t>(n_seg + 1);
+      q.scan = 1;
+      for (int k = 0; k < 3; k++) {
+        q.os.part[k] = c.take<double>(R);
+        q.os.tile[k] = c.take<double>(R / OS_TILE + 2);
+      }
+    };
+    if (users) { segs(a.seg[US_USER], U, true); a.user_out = c.take<double>(4 * (size_t)U); }
+    if (hosts) {
+      rows.host = c.take<int32_t>(R);
+      host_of = c.take<int32_t>(n_codes);
+      segs(a.seg[US_HOST], H, true);
+      a.host_cpus = c.take<double>(H); a.host_mem = c.take<double>(H); a.host_count = c.take<int32_t>(H);
+    }
+    if (out_pool) { segs(a.seg[US_POOL], 1, false); a.pool_out = c.take<double>(4); }
+    if (H > 0) d_codes = c.up(hostname_id, H);
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  // ---- the code -> index map, the live rows, the grid check
+  int nl = 0;
+  CK(pool, cudaMemsetAsync(gf, 0, sizeof(GridFlag), st));
+  if (hosts) {
+    CK(pool, cudaMemsetAsync(host_of, 0xff, sizeof(int32_t) * (size_t)n_codes, st));
+    host_map_kernel<<<(H + 255) / 256, 256, 0, st>>>(d_codes, H, host_of);
+    nl++;
+    rows.host_of = host_of;
+  }
+  compact(rows, S->run.hw, nullptr, blk, S->counters, R, st, &nl);
+  grid_check_kernel<<<(R + 255) / 256, 256, 0, st>>>(rows.amt[0], rows.amt[1], rows.amt[2], R, gf);
+  nl++;
+  // ---- the orders, their segments and (on the grid) their order-wide scans
+  const int32_t* key[US_N] = {rows.user, rows.host, nullptr};
+  for (int k = 0; k < US_N; k++) {
+    UsageSegs& q = a.seg[k];
+    if (!q.n) continue;
+    CK(pool, csort::sort_indices(writable(q.ord), tmp, R, LessKeyTid{key[k], rows.tid}, st, &nl));
+    if (!q.start) continue;
+    // +1: the hosts' segment H holds the rows no listed host carries
+    CK(pool, cudaMemsetAsync(writable(q.start), 0, sizeof(int32_t) * (q.n + 1), st));
+    CK(pool, cudaMemsetAsync(writable(q.end), 0, sizeof(int32_t) * (q.n + 1), st));
+    seg_bounds_kernel<<<(R + 255) / 256, 256, 0, st>>>(SortedKey{q.ord, nullptr, key[k]}, R, writable(q.start),
+                                                       writable(q.end), nullptr);
+    nl++;
+    order_scan(q.os, LoadSorted{q.ord, {rows.amt[0], rows.amt[1], rows.amt[2]}}, R, gf, st, &nl);
+  }
+  // the pool's total from an order-wide scan when there is one (the sum is the same over any order there)
+  if (a.seg[US_POOL].n) {
+    for (int k : {US_USER, US_HOST})
+      if (a.seg[k].scan && !a.seg[US_POOL].scan) { a.seg[US_POOL].os = a.seg[k].os; a.seg[US_POOL].scan = 1; }
+  }
+  for (int k = 0; k < 3; k++) a.amt[k] = rows.amt[k];
+  a.gf = gf; a.R = R; a.U = U;
+  const int nseg = a.seg[US_USER].n + a.seg[US_HOST].n + a.seg[US_POOL].n;
+  usage_fold_kernel<<<(nseg + 3) / 4, 128, 0, st>>>(a);
+  nl++;
+  CK(pool, cudaGetLastError());
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  if (users) CK(pool, download(out_user, a.user_out, 4 * (size_t)U, st, &d2h));
+  if (out_pool) CK(pool, download(out_pool, a.pool_out, 4, st, &d2h));
+  if (hosts) {
+    if (out_run_cpus) CK(pool, download(out_run_cpus, a.host_cpus, H, st, &d2h));
+    if (out_run_mem) CK(pool, download(out_run_mem, a.host_mem, H, st, &d2h));
+    if (out_run_count) CK(pool, download(out_run_count, a.host_count, H, st, &d2h));
+  }
+  CK(pool, cudaEventRecord(pool->ev[23], st));
+  CK(pool, cudaStreamSynchronize(st));
+  record_phase(pool, COOK_PHASE_USAGE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[23], h2d, d2h, nl);
+  return COOK_OK;
+}
+
 }  // namespace
 
 extern "C" int32_t cook_state_apply(cook_pool* pool, const cook_state_delta* delta) {
@@ -858,6 +1063,17 @@ extern "C" int32_t cook_state_patch(cook_pool* pool, int32_t n, const int64_t* j
   PoolState* S = state_of(pool, true);
   if (!S) return set_err(pool, COOK_E_OOM, "cook_state_patch: out of device memory");
   return patch(pool, S, n, job_id, allowed, plugin_accept, reserved_host, clear_reservations != 0);
+}
+
+extern "C" int32_t cook_state_usage(cook_pool* pool, int32_t n_users, double* out_user_usage, double* out_pool_usage,
+                                    int32_t n_hosts, const int32_t* hostname_id, double* out_run_cpus,
+                                    double* out_run_mem, int32_t* out_run_count) {
+  if (!pool) return COOK_E_BADARG;
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_usage: out of device memory");
+  return usage(pool, S, n_users, out_user_usage, out_pool_usage, n_hosts, hostname_id, out_run_cpus, out_run_mem,
+               out_run_count);
 }
 
 extern "C" int32_t cook_state_rank(cook_pool* pool, const cook_user_table* users, const cook_pool_quota* pool_quota,

@@ -62,7 +62,7 @@ def load_library(path=None):
                  "cook_allgather_usage", "cook_last_stats", "cook_comm_unique_id", "cook_comm_init",
                  "cook_comm_destroy", "cook_exchange_usage", "cook_exchange_usage_batch", "cook_rebalance_trace",
                  "cook_match_failures", "cook_state_apply", "cook_state_rank", "cook_state_match",
-                 "cook_state_rebalance", "cook_state_launch", "cook_state_patch"):
+                 "cook_state_rebalance", "cook_state_launch", "cook_state_patch", "cook_state_usage"):
         getattr(lib, name).restype = C.c_int32
     return lib
 
@@ -211,6 +211,25 @@ class GpuEngine:
                                        abi.ptr(rh, abi.P_I32) if rh is not None else None, int(bool(clear_reservations)))
         if rc != 0:
             self._err(rc)
+
+    def state_usage(self, n_users, hostname_id=None):
+        """cook_state_usage: the running usage of the live running rows, each sum a left fold in ascending task
+        id.  Returns 'user' as {count, cpus, mem, gpus} arrays of n_users (abi.make_users' `usage`), 'pool' as
+        [count, cpus, mem, gpus] (one term of state_rank's group_usage) and, for the hosts of hostname_id,
+        'run_cpus', 'run_mem' and 'run_count' arrays (an offer table's run_* columns)."""
+        hn = np.ascontiguousarray(hostname_id if hostname_id is not None else np.zeros(0), np.int32)
+        H = len(hn)
+        user = np.zeros(4 * max(int(n_users), 1), np.float64)
+        pool = np.zeros(4, np.float64)
+        rc_, rm, rn = np.zeros(max(H, 1), np.float64), np.zeros(max(H, 1), np.float64), np.zeros(max(H, 1), np.int32)
+        rc = self.lib.cook_state_usage(self.pool, int(n_users), abi.ptr(user, abi.P_F64), abi.ptr(pool, abi.P_F64), H,
+                                       abi.ptr(hn, abi.P_I32) if H else None, abi.ptr(rc_, abi.P_F64),
+                                       abi.ptr(rm, abi.P_F64), abi.ptr(rn, abi.P_I32))
+        if rc != 0:
+            self._err(rc)
+        U = int(n_users)
+        return {"user": {k: user[i * U:(i + 1) * U].copy() for i, k in enumerate(("count", "cpus", "mem", "gpus"))},
+                "pool": pool, "run_cpus": rc_[:H].copy(), "run_mem": rm[:H].copy(), "run_count": rn[:H].copy()}
 
     def state_rank(self, users, pool_quota=None, group_quota=None, group_usage=None, params=None):
         """cook_state_rank: the live rows ranked; the queue stays on the device.  Returns its job ids."""

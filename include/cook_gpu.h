@@ -533,13 +533,36 @@ int32_t cook_state_rebalance(cook_pool* pool, const cook_host_table* hosts, cons
                              cook_decision* out_decisions, int64_t* out_decision_job_id,
                              int64_t* out_victim_task_id, int32_t victim_cap, int32_t* out_n);
 
+/* Running usage read from the live running rows (generate-user-usage-map scheduler.clj:711-727,
+ * task-ents->usage :2118-2123, Fenzo's tracker state per host :877-881).  Every output may be NULL.
+ *   out_user_usage[4][n_users]  rows count, cpus, mem, gpus: pass out, out+n_users, ... straight
+ *                               into cook_user_table.usage_*; users without a live row get 0
+ *   out_pool_usage[4]           count, cpus, mem, gpus over every live running row: one pool's entry
+ *                               of aggregate-quota-groups, i.e. one term of cook_state_rank's group_usage
+ *   hostname_id[n_hosts]        codes of the global hostname dictionary, e.g. offers->hostname_id
+ *   out_run_cpus/_mem/_count[n_hosts]  sums over the live running rows whose running_hostname_id is
+ *                               hostname_id[h]: cook_offers_soa.run_* for that offer table.  A row whose
+ *                               host is -1 or not listed counts for its user and the pool only; a listed
+ *                               host without rows gets 0.
+ * Fold order: each sum is a left fold in ascending task id (DESIGN.md §2); count is the number of rows
+ * as a double, and a row without gpus adds 0.0.  The result does not depend on where rows are stored.
+ * Changes nothing resident; needs no cook_state_rank.  COOK_E_BADARG before any device work: n_users
+ * <= a live running row's user code (when out_user_usage is given), n_hosts < 0, a NULL hostname_id
+ * with n_hosts > 0, or a hostname_id that is negative or appears twice.  Uploads exactly 4 * n_hosts
+ * bytes (nothing when no running row is live: every output is then 0 without device work).
+ * Statistics: cook_last_stats(COOK_PHASE_USAGE).                                                     */
+int32_t cook_state_usage(cook_pool* pool, int32_t n_users, double* out_user_usage, double* out_pool_usage,
+                         int32_t n_hosts, const int32_t* hostname_id, double* out_run_cpus,
+                         double* out_run_mem, int32_t* out_run_count);
+
 /* ------------------------------------------------------------ phase timing */
 /* Device-side timing of the last call of each kind on this handle (CUDA events on the
  * pool's stream): what bench.py's `phases` block and roofline lines are computed from.
  * COOK_PHASE_STATE: the last cook_state_apply, cook_state_launch or cook_state_patch (upload, then the
- * scatter / move / compaction kernels). */
+ * scatter / move / compaction kernels).  COOK_PHASE_USAGE: the last cook_state_usage (upload of the
+ * hostname list, the compaction, sorts and folds, the download of the sums). */
 enum { COOK_PHASE_RANK = 0, COOK_PHASE_MATCH = 1, COOK_PHASE_REBALANCE = 2, COOK_PHASE_EXCHANGE = 3,
-       COOK_PHASE_STATE = 4 };
+       COOK_PHASE_STATE = 4, COOK_PHASE_USAGE = 5 };
 typedef struct {
   double ms_h2d;      /* upload stage                                              */
   double ms_device;   /* kernels (for the exchange: delta kernels + the collective) */

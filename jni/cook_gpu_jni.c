@@ -184,6 +184,15 @@ JFN(jint, statePatch)(JNIEnv* env, jclass k, jlong pool, jint n, jobject job_id,
   return cook_state_patch((cook_pool*)(intptr_t)pool, n, one(env, job_id), one(env, allowed), one(env, plugin_accept),
                           one(env, reserved_host), clear_reservations);
 }
+/* the running usage of the live running rows: per user ([4][n_users] doubles), of the pool (4 doubles) and per
+ * host of hostname_id (run_cpus, run_mem, run_count); every output may be null */
+JFN(jint, stateUsage)(JNIEnv* env, jclass k, jlong pool, jint n_users, jobject out_user_usage, jobject out_pool_usage,
+                      jint n_hosts, jobject hostname_id, jobject out_run_cpus, jobject out_run_mem,
+                      jobject out_run_count) {
+  return cook_state_usage((cook_pool*)(intptr_t)pool, n_users, one(env, out_user_usage), one(env, out_pool_usage),
+                          n_hosts, one(env, hostname_id), one(env, out_run_cpus), one(env, out_run_mem),
+                          one(env, out_run_count));
+}
 JFN(jint, stateRank)(JNIEnv* env, jclass k, jlong pool, jint n_users, jobjectArray users, jdoubleArray pool_quota,
                      jdoubleArray group_quota, jobject group_usage, jint max_over_quota_jobs, jint filter_offensive,
                      jdouble off_mem_mb, jdouble off_cpus, jobject out_ranked_job_id, jintArray out_n) {

@@ -24,6 +24,14 @@ the (synchronising) binding call, and whether the following rank and match outpu
 
   python tools/prof_state.py --launch --pool c2 --cycles 6
   python tools/prof_state.py --launch --pool c5 --c5-pool 5 --cycles 4
+
+--usage loads the pool's running tasks, each on a random host of the offer table (1 % with host unknown), into a
+resident handle and per cycle runs cook_state_usage for every user and every offer's host, on the grid and off it
+(cpus + 0.1, mem / 3).  It prints the call's device time, wall time and bytes, the wall time of the same left folds
+on the host (what a shim runs without the call), and whether the two agree to the bit.
+
+  python tools/prof_state.py --usage --pool c2 --cycles 5
+  python tools/prof_state.py --usage --pool c5 --c5-pool 5 --cycles 5
 """
 import argparse
 import json
@@ -117,6 +125,67 @@ def rebalance(a):
     host.close()
 
 
+def host_fold(run, host, U, codes):
+    """What a shim computes without cook_state_usage: the same sums on the host, in ascending task id.  np.add.at
+    and np.cumsum add in index order, so every sum is the left fold."""
+    o = np.argsort(run["task_id"], kind="stable")
+    u, hc = run["user"][o], host[o]
+    amt = [run[k][o] for k in ("cpus", "mem", "gpus")]
+    user = np.zeros((4, U))
+    np.add.at(user[0], u, 1.0)
+    for k in range(3):
+        np.add.at(user[k + 1], u, amt[k])
+    pool = np.array([float(len(o))] + [np.cumsum(x)[-1] if len(x) else 0.0 for x in amt])
+    idx = np.full(max(int(codes.max()), int(hc.max())) + 1, -1, np.int64)
+    idx[codes] = np.arange(len(codes))
+    hi = np.where(hc >= 0, idx[np.maximum(hc, 0)], -1)
+    sel = hi >= 0
+    H = len(codes)
+    rc, rm, rn = np.zeros(H), np.zeros(H), np.zeros(H, np.int32)
+    np.add.at(rc, hi[sel], amt[0][sel])
+    np.add.at(rm, hi[sel], amt[1][sel])
+    np.add.at(rn, hi[sel], 1)
+    return user, pool, rc, rm, rn
+
+
+def usage(a):
+    t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
+    rc0, codes, U = t["cols"]["running"], t["offers"].col("hostname_id").astype(np.int32), t["users"].n_users
+    rng = np.random.default_rng(a.seed)
+    n = len(rc0["task_id"])
+    host = codes[rng.integers(0, len(codes), n)].astype(np.int32)
+    host[rng.random(n) < 0.01] = -1
+    print(json.dumps({"card": card(), "pool": a.pool if a.pool == "c2" else f"c5/{a.c5_pool}", "running": n,
+                      "hosts": len(codes), "users": U}), flush=True)
+    for regime in ("grid", "off"):
+        run = {k: np.asarray(v).copy() for k, v in rc0.items()}
+        if regime == "off":   # every partial sum rounds: the folds take the serial chain
+            run["cpus"] = run["cpus"] + 0.1
+            run["mem"] = run["mem"] / 3.0
+        e = GpuEngine(pool_name="usage")
+        e.state_apply(abi.make_delta(reset=True, running=abi.make_tasks(**run), running_hostname_id=host))
+        for cycle in range(a.cycles):
+            w0 = time.perf_counter()
+            got = e.state_usage(U, codes)
+            w_dev = time.perf_counter() - w0
+            st = e.last_stats(abi.PHASE_USAGE)
+            w0 = time.perf_counter()
+            user, pool, hc, hm, hn = host_fold(run, host, U, codes)
+            w_host = time.perf_counter() - w0
+            same = (all(np.array_equal(got["user"][k].view(np.uint64), user[i].view(np.uint64))
+                        for i, k in enumerate(("count", "cpus", "mem", "gpus"))) and
+                    np.array_equal(got["pool"].view(np.uint64), pool.view(np.uint64)) and
+                    np.array_equal(got["run_cpus"].view(np.uint64), hc.view(np.uint64)) and
+                    np.array_equal(got["run_mem"].view(np.uint64), hm.view(np.uint64)) and
+                    np.array_equal(got["run_count"], hn))
+            print(json.dumps({"regime": regime, "cycle": cycle,
+                              "state_usage": {**{k: round(st[k], 3) for k in ("ms_h2d", "ms_device", "ms_d2h")},
+                                              "wall_ms": round(1e3 * w_dev, 3), "h2d_bytes": st["h2d_bytes"],
+                                              "d2h_bytes": st["d2h_bytes"], "n_launches": st["n_launches"]},
+                              "host_fold_wall_ms": round(1e3 * w_host, 3), "identical": bool(same)}), flush=True)
+        e.close()
+
+
 def launch_cycle(cycle, res, twin, job_id, lt, hosts, rest, match_args):
     """One cycle of --launch: the launches by id on `res` and as a delta on `twin`, the rest of the batch on both,
     then rank and match on both.  Returns the jobs the match placed and their hosts' codes."""
@@ -158,9 +227,12 @@ def main():
     ap.add_argument("--c4-pool", type=int, default=0)
     ap.add_argument("--cycles", type=int, default=6)
     ap.add_argument("--seed", type=int, default=7)
+    ap.add_argument("--usage", action="store_true")
     a = ap.parse_args()
     if a.rebalance:
         return rebalance(a)
+    if a.usage:
+        return usage(a)
     t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
     jobs, pc, rc = t["jobs"], t["cols"]["pending"], t["cols"]["running"]
     J = jobs.n
