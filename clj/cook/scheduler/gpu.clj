@@ -155,6 +155,14 @@
                       :launched-job-uuids #{})))
     decisions))
 
+(defn cotasks!
+  "Each group's running cotasks from the resident running rows (cook_state_cotasks), for the groups columns of
+   the next state match or rebalance: `args` are Native/stateCotasks' arguments after the handle, with
+   out-cot-hostname-id nil to ask for the size first.  Replaces the host index running task -> job -> groups
+   -> host that get-cotasks-from-tracker-state (constraints.clj:539-552) would otherwise need."
+  [handle args]
+  (check! handle (apply #(Native/stateCotasks handle %&) args) "cook_state_cotasks"))
+
 (defn exchange-usage!
   "§8e: after a pool's match round; `comm` from Native/commInit (rank 0's Native/commUniqueId bytes travel
    over Cook's own control plane).  Returns the [world n-pad] table as a DoubleBuffer."

@@ -139,7 +139,7 @@ class PhaseStats(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_ if n != "reserved0"}
 
 
-PHASE_RANK, PHASE_MATCH, PHASE_REBALANCE, PHASE_EXCHANGE, PHASE_STATE, PHASE_USAGE = 0, 1, 2, 3, 4, 5
+PHASE_RANK, PHASE_MATCH, PHASE_REBALANCE, PHASE_EXCHANGE, PHASE_STATE, PHASE_USAGE, PHASE_COTASKS = 0, 1, 2, 3, 4, 5, 6
 
 
 class StateDelta(_SoA):
@@ -147,13 +147,15 @@ class StateDelta(_SoA):
     _fields_ = [("reset", C.c_int32), ("pending", JobsSoA), ("pending_priority", P_I32),
                 ("pending_job_id", P_I64), ("n_pending_rm", C.c_int32), ("pending_rm_job_id", P_I64),
                 ("running", TasksSoA), ("n_running_rm", C.c_int32), ("running_rm_task_id", P_I64),
-                ("running_hostname_id", P_I32)]
+                ("running_hostname_id", P_I32), ("running_group_off", P_I32), ("running_group_idx", P_I32)]
 
 
 def make_delta(reset=False, pending=None, pending_priority=None, pending_job_id=None, pending_rm=(),
-               running=None, running_rm=(), running_hostname_id=None):
+               running=None, running_rm=(), running_hostname_id=None, running_group_off=None,
+               running_group_idx=None):
     """A StateDelta; `pending` is a JobsSoA of the upserted rows, `running` a TasksSoA, `running_hostname_id`
-    the hostname code of each running row (None: host unknown)."""
+    the hostname code of each running row (None: host unknown), `running_group_off` / `running_group_idx` the
+    CSR of each running row's group list (csr(); None: empty lists)."""
     pending = pending if pending is not None else JobsSoA(n=0)
     running = running if running is not None else TasksSoA(n=0)
     prm = np.asarray(pending_rm, np.int64)
@@ -162,7 +164,8 @@ def make_delta(reset=False, pending=None, pending_priority=None, pending_job_id=
                       pending_job_id=pending_job_id, n_pending_rm=len(prm),
                       pending_rm_job_id=prm if len(prm) else None, running=running,
                       n_running_rm=len(rrm), running_rm_task_id=rrm if len(rrm) else None,
-                      running_hostname_id=running_hostname_id)
+                      running_hostname_id=running_hostname_id, running_group_off=running_group_off,
+                      running_group_idx=running_group_idx)
 
 
 class RunningSoA(_SoA):

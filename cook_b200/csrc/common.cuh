@@ -122,7 +122,7 @@ struct cook_pool {
   int sm_count = 0;
   cudaStream_t stream = nullptr;
   cudaEvent_t ev[24] = {};
-  cook_phase_stats phase[6] = {};        // last rank / match / rebalance / exchange / state-apply / usage call
+  cook_phase_stats phase[7] = {};        // last rank / match / rebalance / exchange / state-apply / usage / cotasks call
   double* xchg = nullptr;                // exchange buffers: [n_pad] local + [world * n_pad] gathered
   size_t xchg_cap = 0;
   Arena arena;

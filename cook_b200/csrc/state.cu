@@ -18,6 +18,9 @@
 // reserved_host) in place and keeps the generation, so the job keeps its queue entry.
 // Running usage per user, of the pool and per listed host: the live running rows compacted, sorted by (key, task
 // id) and folded per segment, each sum a left fold in ascending task id (DESIGN.md §2).
+// Running rows carry their job's group list (a fourth arena, filled by running upserts and moved on the device
+// by a launch).  A group's cotasks: the live running rows with a known host expanded into one entry per group,
+// sorted by (group, task id).
 #include <algorithm>
 #include <map>
 #include <unordered_map>
@@ -36,10 +39,11 @@ enum PCol {
 };
 constexpr int P_SZ[P_NCOL] = {4, 4, 8, 8, 8, 8, 4, 1, 1, 4, 8, 4, 8, 4, 4, 1, 4, 4, 4, 4, 4, 4, 4};
 enum RCol { R_USER, R_PRIO, R_START, R_TID, R_JID, R_CPUS, R_MEM, R_GPUS, R_HOST, R_NDATA, R_LIVE = R_NDATA, R_GEN,
-            R_NCOL };
-constexpr int R_SZ[R_NCOL] = {4, 4, 8, 8, 8, 8, 8, 8, 4, 1, 4};
+            R_GOFF, R_GLEN, R_NCOL };
+constexpr int R_SZ[R_NCOL] = {4, 4, 8, 8, 8, 8, 8, 8, 4, 1, 4, 4, 4};
 
-enum { L_NOVEL = 0, L_ATTR = 1, L_GROUP = 2 };
+// the pending rows' three lists, then the running rows' group list
+enum { L_NOVEL = 0, L_ATTR = 1, L_GROUP = 2, L_RGROUP = 3, L_N };
 
 // ---- scatter: row i of a batch to slot[i].  Upserts write the columns (a null source writes the
 // column's absent value) and the rows' list ranges; removals clear the live flag.  Both bump the
@@ -85,10 +89,11 @@ __global__ void scatter_kernel(ScatterArgs a) {
 }
 
 // ---- launch: pending slot pslot[i] becomes running slot rslot[i].  What the task shares with its job moves
-// from the pending table; task id, start time and host (null: -1) come from the call.  The pending slot is
-// retired afterwards by a removal scatter.
+// from the pending table; task id, start time and host (null: -1) come from the call.  The group list starts
+// empty at the running arena's tail `rtail`; launch_lists_kernel moves the job's list there when some launched
+// job has one.  The pending slot is retired afterwards by a removal scatter.
 __global__ void launch_kernel(const int32_t* pslot, const int32_t* rslot, const int64_t* tid, const int64_t* start,
-                              const int32_t* host, void* const* pc, void* const* rc, int n) {
+                              const int32_t* host, void* const* pc, void* const* rc, int n, int32_t rtail) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int s = pslot[i], r = rslot[i];
@@ -103,6 +108,8 @@ __global__ void launch_kernel(const int32_t* pslot, const int32_t* rslot, const 
   static_cast<int32_t*>(rc[R_HOST])[r] = host ? host[i] : -1;
   static_cast<uint8_t*>(rc[R_LIVE])[r] = 1;
   static_cast<uint32_t*>(rc[R_GEN])[r] += 1u;
+  static_cast<int32_t*>(rc[R_GOFF])[r] = rtail;
+  static_cast<int32_t*>(rc[R_GLEN])[r] = 0;
 }
 
 // ---- list lengths for the order-wide scan (integer sums: any association is exact)
@@ -127,6 +134,21 @@ __global__ void list_compact_kernel(OrderScan<int, 1> os, const uint8_t* live, i
   }
   __syncwarp();
   if (lane == 0) off[w] = start;
+}
+
+// warp per launched row: pending slot pslot[w]'s group list moves to the running arena at rtail + the exclusive scan
+// of the launched rows' lengths, where the equivalent delta's CSR puts it, and becomes running slot rslot[w]'s list
+__global__ void launch_lists_kernel(OrderScan<int, 1> os, const int32_t* pslot, const int32_t* rslot, int n,
+                                    const int32_t* poff, const int32_t* plen, const int32_t* src, int32_t* roff,
+                                    int32_t* rlen, int32_t* dst, int32_t rtail) {
+  const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (w >= n) return;
+  const int s = pslot[w], l = plen[s], start = rtail + os.at(0, w) - l, o = poff[s];
+  for (int i = lane; i < l; i += 32) dst[start + i] = src[o + i];
+  if (lane == 0) {
+    roff[rslot[w]] = start;
+    rlen[rslot[w]] = l;
+  }
 }
 
 // warp per match row: the row's list into the dense CSR (doff[n + 1], values) cook_match reads
@@ -343,6 +365,58 @@ __global__ void __launch_bounds__(128) usage_fold_kernel(UsageArgs a) {
   }
 }
 
+// ---- cotasks: the live running slots whose host is known and whose group list is not empty, in slot order
+struct CotaskRows {
+  const uint8_t* live; const int32_t* host; const int32_t* len; int32_t* slot;
+  __device__ bool keep(int i) const { return live[i] && host[i] != -1 && len[i] > 0; }
+  __device__ void emit(int i, int d) const { slot[d] = i; }
+};
+struct CotaskArgs {
+  OrderScan<int, 1> os;     // inclusive scan of the compacted rows' list lengths
+  const int32_t* slot; int K;
+  const int32_t* goff; const int32_t* glen; const int32_t* arena; const int32_t* host; const int64_t* tid;
+  const int32_t* host_of; int32_t n_codes;   // hostname code -> index of the listed host, or -1; null: none listed
+  const int32_t* gcol;      // [n_groups] the group's column among the uploaded ones, or -1
+  const int32_t* attr; int H;   // the uploaded columns, [columns][H]
+  int32_t* e_grp; int64_t* e_tid; int32_t* e_host; int32_t* e_attr;
+};
+// thread per compacted row: one entry per group of its list, placed where the scan puts the row
+__global__ void cotask_expand_kernel(CotaskArgs a) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= a.K) return;
+  const int s = a.slot[k], l = a.glen[s], start = a.os.at(0, k) - l, o = a.goff[s];
+  const int32_t code = a.host[s];
+  const int32_t h = a.host_of && code < a.n_codes ? a.host_of[code] : -1;
+  const int64_t t = a.tid[s];
+  for (int i = 0; i < l; i++) {
+    const int32_t g = a.arena[o + i], c = a.gcol[g];
+    a.e_grp[start + i] = g;
+    a.e_tid[start + i] = t;
+    a.e_host[start + i] = code;
+    a.e_attr[start + i] = c >= 0 && h >= 0 ? a.attr[(size_t)c * a.H + h] : 0;
+  }
+}
+// Position p < N of the (group, task id) order into the value columns; p <= G: the first position of group p,
+// i.e. the entries of smaller groups (a binary search), so a group without entries gets an empty range.
+__global__ void cotask_out_kernel(const int32_t* ord, const int32_t* e_grp, const int32_t* e_host,
+                                  const int32_t* e_attr, int N, int G, int32_t* off, int32_t* o_host, int32_t* o_attr) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p < N) {
+    const int i = ord[p];
+    o_host[p] = e_host[i];
+    o_attr[p] = e_attr[i];
+  }
+  if (p <= G) {
+    int lo = 0, hi = N;
+    while (lo < hi) {
+      const int m = (lo + hi) >> 1;
+      if (e_grp[ord[m]] < p) lo = m + 1;
+      else hi = m;
+    }
+    off[p] = lo;
+  }
+}
+
 // ---- host side
 // the non-absent values of a pending row, counted per column (the match's constraint switch)
 enum { F_GPUS, F_PORTS, F_NOT_ALLOWED, F_NOT_PLUGIN, F_GPU_MODEL, F_DISK, F_EST, F_CKPT, F_RESERVED, F_N };
@@ -360,6 +434,7 @@ struct Table {
   void* col[P_NCOL] = {};
   void** d_col = nullptr;        // the column pointers on the device (for the gather kernels)
   int32_t cap = 0, hw = 0;       // slots allocated, slots ever used
+  int nlist = 0, lcol[3] = {};   // the per-slot (off, len) column pairs of the table's lists: off at lcol[l]
   std::unordered_map<int64_t, int32_t> slot_of;
   std::vector<int32_t> free;
 
@@ -440,9 +515,12 @@ struct PoolState {
   Table pend, run;
   std::vector<PendingInfo> pinfo;    // by pending slot
   std::vector<int32_t> ruser, rhost; // by running slot
-  ListArena lists[3];
+  std::vector<std::vector<int32_t>> rgroups;   // by running slot: its group list
+  ListArena lists[L_N];
   std::map<int32_t, int64_t> users_p, users_r, attr_cols, groups;   // code -> live uses
   std::map<int32_t, int64_t> hosts_r;                               // running rows' hostname codes (-1 too)
+  std::map<int32_t, int64_t> groups_r;                              // running rows' group codes
+  int64_t cot_rows = 0, cot_n = 0;   // live running rows with a known host and a group list, and their entries
   int64_t nflag[F_N] = {};
   std::unordered_set<int32_t> reserved;   // the live pending slots whose reserved_host is not -1
   Arena stage;                        // one batch's uploads
@@ -457,6 +535,8 @@ struct PoolState {
   PoolState() {
     pend.ncol = P_NCOL; pend.sz = P_SZ;
     run.ncol = R_NCOL; run.sz = R_SZ;
+    pend.nlist = 3; pend.lcol[L_NOVEL] = P_NOFF; pend.lcol[L_ATTR] = P_AOFF; pend.lcol[L_GROUP] = P_GOFF;
+    run.nlist = 1; run.lcol[0] = R_GOFF;
     lists[L_ATTR].k = 2;
   }
   void release() {
@@ -476,6 +556,23 @@ struct PoolState {
       if (sign > 0) reserved.insert(slot);
       else reserved.erase(slot);
     }
+  }
+  // running slot `slot`'s row (ruser, rhost, rgroups) enters (+1) or leaves (-1) the counts
+  void add_running(int32_t slot, int64_t sign) {
+    count_add(users_r, ruser[slot], sign);
+    count_add(hosts_r, rhost[slot], sign);
+    const std::vector<int32_t>& g = rgroups[slot];
+    for (int32_t c : g) count_add(groups_r, c, sign);
+    lists[L_RGROUP].live += sign * (int64_t)g.size();
+    if (rhost[slot] != -1 && !g.empty()) {
+      cot_rows += sign;
+      cot_n += sign * (int64_t)g.size();
+    }
+  }
+  void running_room(int32_t slot) {
+    if ((size_t)slot < ruser.size()) return;
+    const size_t n = std::max<size_t>(slot + 1, 2 * ruser.size());
+    ruser.resize(n); rhost.resize(n); rgroups.resize(n);
   }
   // a live pending slot's flag f after a patch of its column
   void set_flag(int32_t slot, int f, bool on) {
@@ -537,11 +634,12 @@ void gather_lists(const PoolState* S, const JobDev& o, const int32_t* m_slot, in
 
 // compaction of every list arena whose dead entries outnumber its live ones
 int32_t compact_lists(cook_pool* pool, PoolState* S, cudaStream_t st, int* nl) {
-  const int n = S->pend.hw;
-  const int loff[3] = {P_NOFF, P_AOFF, P_GOFF}, llen[3] = {P_NLEN, P_ALEN, P_GLEN};
-  for (int l = 0; l < 3; l++) {
+  for (int l = 0; l < L_N; l++) {
     ListArena& A = S->lists[l];
     if (A.tail - A.live <= A.live) continue;
+    const bool run = l == L_RGROUP;
+    const Table& t = run ? S->run : S->pend;
+    const int n = t.hw, oc = t.lcol[run ? 0 : l];
     if (A.live > 0 && n > 0) {
       for (int i = 0; i < A.k; i++)
         if (!A.alt[i]) CK(pool, cudaMalloc(&A.alt[i], sizeof(int32_t) * std::max<int64_t>(A.cap, 1)));
@@ -550,9 +648,9 @@ int32_t compact_lists(cook_pool* pool, PoolState* S, cudaStream_t st, int* nl) {
         os.part[0] = c.take<int32_t>(n);
         os.tile[0] = c.take<int32_t>((n + OS_TILE - 1) / OS_TILE + 1);
       }));
-      const uint8_t* live = static_cast<const uint8_t*>(S->pend.col[P_LIVE]);
-      int32_t* off = static_cast<int32_t*>(S->pend.col[loff[l]]);
-      const int32_t* len = static_cast<const int32_t*>(S->pend.col[llen[l]]);
+      const uint8_t* live = static_cast<const uint8_t*>(t.col[run ? (int)R_LIVE : (int)P_LIVE]);
+      int32_t* off = static_cast<int32_t*>(t.col[oc]);
+      const int32_t* len = static_cast<const int32_t*>(t.col[oc + 1]);
       order_scan(os, SlotLen{live, len}, n, S->gf0, st, nl);
       list_compact_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, live, off, len, n, A.v[0], A.v[1], A.alt[0],
                                                        A.k > 1 ? A.alt[1] : nullptr);
@@ -566,7 +664,7 @@ int32_t compact_lists(cook_pool* pool, PoolState* S, cudaStream_t st, int* nl) {
 }
 
 // one scatter_kernel launch of a batch's n rows into table t.  live_col < 0: a patch (live flag and generation
-// untouched); `tail` (the pending table's upserts and removals): where the batch's lists were appended.
+// untouched); `tail` (upserts and removals): where the batch's lists were appended, one per list of the table.
 void scatter(ScatterArgs& a, Table& t, int n, int upsert, int live_col, const int32_t* tail, cudaStream_t st, int* nl) {
   if (!n) return;
   a.n = n; a.upsert = upsert;
@@ -575,10 +673,9 @@ void scatter(ScatterArgs& a, Table& t, int n, int upsert, int live_col, const in
     a.gen = static_cast<uint32_t*>(t.col[live_col + 1]);
   }
   if (tail) {
-    const int loff[3] = {P_NOFF, P_AOFF, P_GOFF};
-    for (int l = 0; l < 3; l++) {
-      a.loff[l] = static_cast<int32_t*>(t.col[loff[l]]);
-      a.llen[l] = static_cast<int32_t*>(t.col[loff[l] + 1]);
+    for (int l = 0; l < t.nlist; l++) {
+      a.loff[l] = static_cast<int32_t*>(t.col[t.lcol[l]]);
+      a.llen[l] = static_cast<int32_t*>(t.col[t.lcol[l] + 1]);
       a.tail[l] = tail[l];
     }
   }
@@ -598,13 +695,15 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
   if ((npr && !d->pending_rm_job_id) || (nrr && !d->running_rm_task_id))
     return set_err(pool, COOK_E_BADARG, "cook_state_apply: null removal ids");
   if (!csr_ok(P.novel_off, np, P.novel_host, nullptr, false) || !csr_ok(P.attr_off, np, P.attr_col, P.attr_val, true) ||
-      !csr_ok(P.group_off, np, P.group_idx, nullptr, false))
+      !csr_ok(P.group_off, np, P.group_idx, nullptr, false) ||
+      !csr_ok(d->running_group_off, nr, d->running_group_idx, nullptr, false))
     return set_err(pool, COOK_E_BADARG, "cook_state_apply: malformed CSR offsets");
   // codes are checked where they enter
   if (!idx_in_range(P.user, np, 0, INT32_MAX) || !idx_in_range(T.user, nr, 0, INT32_MAX))
     return set_err(pool, COOK_E_BADARG, "cook_state_apply: negative user code");
   if ((P.attr_off && !idx_in_range(P.attr_col, P.attr_off[np], 0, INT32_MAX)) ||
       (P.group_off && !idx_in_range(P.group_idx, P.group_off[np], 0, INT32_MAX)) ||
+      (d->running_group_off && !idx_in_range(d->running_group_idx, d->running_group_off[nr], 0, INT32_MAX)) ||
       (P.novel_off && !idx_in_range(P.novel_host, P.novel_off[np], 0, INT32_MAX)) ||
       !idx_in_range(P.reserved_host, np, -1, INT32_MAX) || !idx_in_range(d->running_hostname_id, nr, -1, INT32_MAX))
     return set_err(pool, COOK_E_BADARG, "cook_state_apply: bad attribute column, group or hostname code");
@@ -640,6 +739,8 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
       t->slot_of.clear(); t->free.clear(); t->hw = 0;
     }
     S->users_p.clear(); S->users_r.clear(); S->attr_cols.clear(); S->groups.clear(); S->hosts_r.clear();
+    S->groups_r.clear();
+    S->cot_rows = S->cot_n = 0;
     S->reserved.clear();
     for (auto& f : S->nflag) f = 0;
     for (auto& l : S->lists) l.tail = l.live = 0;
@@ -657,8 +758,7 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
     auto it = S->run.slot_of.find(d->running_rm_task_id[i]);
     const int32_t s = it->second;
     S->run.slot_of.erase(it);
-    count_add(S->users_r, S->ruser[s], -1);
-    count_add(S->hosts_r, S->rhost[s], -1);
+    S->add_running(s, -1);
     S->run.free.push_back(s);
     rrm_slot[i] = s;
   }
@@ -684,25 +784,22 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
     S->add_pending(s, pi, +1);
     pup_slot[i] = s;
   }
+  const int32_t* rgo = d->running_group_off;
   for (int i = 0; i < nr; i++) {
     auto it = S->run.slot_of.find(T.task_id[i]);
     int32_t s;
     if (it != S->run.slot_of.end()) {
       s = it->second;
-      count_add(S->users_r, S->ruser[s], -1);
-      count_add(S->hosts_r, S->rhost[s], -1);
+      S->add_running(s, -1);
     } else {
       s = S->run.take_slot();
       S->run.slot_of.emplace(T.task_id[i], s);
     }
-    if ((size_t)s >= S->ruser.size()) {
-      S->ruser.resize(std::max<size_t>(s + 1, 2 * S->ruser.size()));
-      S->rhost.resize(S->ruser.size());
-    }
+    S->running_room(s);
     S->ruser[s] = T.user[i];
     S->rhost[s] = d->running_hostname_id ? d->running_hostname_id[i] : -1;
-    count_add(S->users_r, T.user[i], +1);
-    count_add(S->hosts_r, S->rhost[s], +1);
+    S->rgroups[s].assign(rgo ? d->running_group_idx + rgo[i] : nullptr, rgo ? d->running_group_idx + rgo[i + 1] : nullptr);
+    S->add_running(s, +1);
     rup_slot[i] = s;
   }
   // ---- device: capacity, the upload, then the scatters (removals before upserts: a slot a removal
@@ -718,6 +815,11 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
     CK(pool, S->lists[l].grow(S->lists[l].tail + add, st));
     S->lists[l].tail += add;
   }
+  ListArena& RG = S->lists[L_RGROUP];
+  const int32_t rtail0 = (int32_t)RG.tail;
+  const int64_t radd = rgo ? rgo[nr] : 0;
+  CK(pool, RG.grow(RG.tail + radd, st));
+  RG.tail += radd;
   ScatterArgs pu, pr, ru, rr;
   memset(&pu, 0, sizeof(pu)); memset(&pr, 0, sizeof(pr)); memset(&ru, 0, sizeof(ru)); memset(&rr, 0, sizeof(rr));
   int64_t h2d = 0;
@@ -755,6 +857,8 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
       }
       ru.nc = R_NDATA;
       ru.slot = c.up(rup_slot.data(), nr);
+      ru.doff[0] = c.up(rgo, nr + 1);
+      if (c.base && radd) c.copy(RG.v[0] + rtail0, d->running_group_idx, radd);
     }
     if (nrr) rr.slot = c.up(rrm_slot.data(), nrr);
   });
@@ -762,9 +866,9 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
   CK(pool, cudaEventRecord(pool->ev[21], st));
   int nl = 0;
   scatter(pr, S->pend, npr, 0, P_LIVE, tail0, st, &nl);
-  scatter(rr, S->run, nrr, 0, R_LIVE, nullptr, st, &nl);
+  scatter(rr, S->run, nrr, 0, R_LIVE, &rtail0, st, &nl);
   scatter(pu, S->pend, np, 1, P_LIVE, tail0, st, &nl);
-  scatter(ru, S->run, nr, 1, R_LIVE, nullptr, st, &nl);
+  scatter(ru, S->run, nr, 1, R_LIVE, &rtail0, st, &nl);
   CK(pool, cudaGetLastError());
   int32_t rc = compact_lists(pool, S, st, &nl);
   if (rc != COOK_OK) return rc;
@@ -815,36 +919,53 @@ int32_t launch(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, cons
     S->add_pending(s, S->pinfo[s], -1);
     S->pend.free.push_back(s);
   }
+  int64_t ng = 0;   // group list entries that move with the jobs
   for (int i = 0; i < n; i++) {
     const int32_t r = S->run.take_slot();
     S->run.slot_of.emplace(task_id[i], r);
-    if ((size_t)r >= S->ruser.size()) {
-      S->ruser.resize(std::max<size_t>(r + 1, 2 * S->ruser.size()));
-      S->rhost.resize(S->ruser.size());
-    }
+    S->running_room(r);
     S->ruser[r] = S->pinfo[pslot[i]].user;
     S->rhost[r] = hostname_id ? hostname_id[i] : -1;
-    count_add(S->users_r, S->ruser[r], +1);
-    count_add(S->hosts_r, S->rhost[r], +1);
+    S->rgroups[r] = S->pinfo[pslot[i]].groups;
+    S->add_running(r, +1);
+    ng += (int64_t)S->rgroups[r].size();
     rslot[i] = r;
   }
-  // ---- device: capacity, the upload, the move, the pending slots' removal, then the arena rule
+  // ---- device: capacity, the upload, the move (rows, then group lists), the pending slots' removal, then the
+  // arena rule
   CK(pool, S->run.grow(S->run.hw, st));
+  ListArena& RG = S->lists[L_RGROUP];
+  const int32_t rtail0 = (int32_t)RG.tail;
+  CK(pool, RG.grow(RG.tail + ng, st));
+  RG.tail += ng;
   const int32_t *d_pslot = nullptr, *d_rslot = nullptr, *d_host = nullptr;
   const int64_t *d_tid = nullptr, *d_start = nullptr;
+  OrderScan<int, 1> os;
   int64_t h2d = 0;
   CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
     if (!n) return;
     d_pslot = c.up(pslot.data(), n); d_rslot = c.up(rslot.data(), n);
     d_tid = c.up(task_id, n); d_start = c.up(start_time, n);
     d_host = c.up(hostname_id, n);
+    if (ng) {   // device-only buffers: nothing uploaded
+      os.part[0] = c.take<int32_t>(n);
+      os.tile[0] = c.take<int32_t>((n + OS_TILE - 1) / OS_TILE + 1);
+    }
   }));
   CK(pool, cudaEventRecord(pool->ev[21], st));
   int nl = 0;
   if (n) {
     launch_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_pslot, d_rslot, d_tid, d_start, d_host, S->pend.d_col,
-                                                   S->run.d_col, n);
+                                                   S->run.d_col, n, rtail0);
     nl++;
+    if (ng) {
+      const int32_t* plen = S->pend.at<int32_t>(P_GLEN);
+      order_scan(os, RowLen{d_pslot, plen}, n, S->gf0, st, &nl);
+      launch_lists_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, d_pslot, d_rslot, n, S->pend.at<int32_t>(P_GOFF), plen,
+                                                       S->lists[L_GROUP].v[0], static_cast<int32_t*>(S->run.col[R_GOFF]),
+                                                       static_cast<int32_t*>(S->run.col[R_GLEN]), RG.v[0], rtail0);
+      nl++;
+    }
     ScatterArgs rm;
     memset(&rm, 0, sizeof(rm));
     rm.slot = d_pslot;
@@ -1035,6 +1156,113 @@ int32_t usage(cook_pool* pool, PoolState* S, int U, double* out_user, double* ou
   return COOK_OK;
 }
 
+// each group's running cotasks (cook_groups.cot_*): the live running rows with a known host, by (group, task id)
+int32_t cotasks(cook_pool* pool, PoolState* S, int G, const int32_t* attr_col, const cook_host_table* hosts, int cap,
+                int32_t* out_off, int32_t* out_host, int32_t* out_attr, int32_t* out_n) {
+  // ---- every check before any device work or output: the rows' codes and the size from the host-side counts
+  const bool query = !out_host;
+  if (!out_n || (!query && (!out_off || !out_attr)))
+    return set_err(pool, COOK_E_BADARG, "cook_state_cotasks: null output");
+  if (G < 0) return set_err(pool, COOK_E_BADARG, "cook_state_cotasks: n_groups < 0");
+  if (S && count_max(S->groups_r) >= G)
+    return set_err(pool, COOK_E_BADARG, "cook_state_cotasks: a live running row's group code is >= n_groups");
+  const int H = hosts ? hosts->n : 0;
+  if (H < 0) return set_err(pool, COOK_E_BADARG, "cook_state_cotasks: hosts->n < 0");
+  if (H > 0 && !hosts->hostname_id) return set_err(pool, COOK_E_BADARG, "cook_state_cotasks: null hosts->hostname_id");
+  int32_t n_codes = 0;
+  {
+    std::unordered_set<int32_t> codes;
+    codes.reserve((size_t)H);
+    for (int h = 0; h < H; h++) {
+      const int32_t c = hosts->hostname_id[h];
+      if (c < 0 || !codes.insert(c).second)
+        return set_err(pool, COOK_E_BADARG, "cook_state_cotasks: a hostname_id is negative or twice in `hosts`");
+      n_codes = std::max(n_codes, c + 1);
+    }
+  }
+  // the distinct attribute columns the groups name, in first-named order; gcol[g]: the group's among them
+  std::vector<int32_t> gcol(G, -1), cols;
+  if (hosts && attr_col) {
+    std::vector<int32_t> at(std::max(hosts->n_attr_cols, 0), -1);
+    for (int g = 0; g < G; g++) {
+      const int32_t c = attr_col[g];
+      if (c < -1 || c >= hosts->n_attr_cols)
+        return set_err(pool, COOK_E_BADARG, "cook_state_cotasks: attr_col outside [-1, hosts->n_attr_cols)");
+      if (c < 0 || H == 0) continue;
+      if (at[c] < 0) { at[c] = (int32_t)cols.size(); cols.push_back(c); }
+      gcol[g] = at[c];
+    }
+    if (!cols.empty() && !hosts->attr) return set_err(pool, COOK_E_BADARG, "cook_state_cotasks: null hosts->attr");
+  }
+  const int64_t N = S ? S->cot_n : 0;
+  if (N > INT32_MAX) return set_err(pool, COOK_E_TOO_LARGE, "cook_state_cotasks: more than 2^31 - 1 entries");
+  if (!query && cap < N) return set_err(pool, COOK_E_BADARG, "cook_state_cotasks: cap < the required size");
+  *out_n = (int32_t)N;
+  if (query || N == 0) {   // no device work
+    if (!query) memset(out_off, 0, sizeof(int32_t) * ((size_t)G + 1));
+    pool->phase[COOK_PHASE_COTASKS] = cook_phase_stats{};
+    return COOK_OK;
+  }
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  const int K = (int)S->cot_rows, D = (int)cols.size();
+  CotaskArgs a = {};
+  a.K = K; a.H = H; a.n_codes = n_codes;
+  a.goff = S->run.at<int32_t>(R_GOFF); a.glen = S->run.at<int32_t>(R_GLEN); a.arena = S->lists[L_RGROUP].v[0];
+  a.host = S->run.at<int32_t>(R_HOST); a.tid = S->run.at<int64_t>(R_TID);
+  int32_t *blk = nullptr, *ord = nullptr, *tmp = nullptr, *d_off = nullptr, *d_host = nullptr, *d_attr = nullptr;
+  int32_t *slot = nullptr, *host_of = nullptr, *attr = nullptr;
+  const int32_t* d_codes = nullptr;
+  int64_t h2d = 0, d2h = 0;
+  CK(pool, carve(S->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+    slot = c.take<int32_t>(K);
+    blk = c.take<int32_t>((size_t)S->run.hw / CP_BLOCK + 2);
+    a.os.part[0] = c.take<int32_t>(K);
+    a.os.tile[0] = c.take<int32_t>((K + OS_TILE - 1) / OS_TILE + 1);
+    a.e_grp = c.take<int32_t>(N); a.e_tid = c.take<int64_t>(N); a.e_host = c.take<int32_t>(N);
+    a.e_attr = c.take<int32_t>(N);
+    ord = c.take<int32_t>(N); tmp = c.take<int32_t>(N);
+    d_off = c.take<int32_t>((size_t)G + 1); d_host = c.take<int32_t>(N); d_attr = c.take<int32_t>(N);
+    if (H > 0) {
+      d_codes = c.up(hosts->hostname_id, H);
+      host_of = c.take<int32_t>(n_codes);
+    }
+    if (D) {
+      attr = c.take<int32_t>((size_t)D * H);
+      if (attr)
+        for (int j = 0; j < D; j++) c.copy(attr + (size_t)j * H, hosts->attr + (size_t)cols[j] * H, H);
+    }
+    a.gcol = c.up(gcol.data(), G);
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  a.slot = slot; a.host_of = host_of; a.attr = attr;
+  // ---- the code -> index map, the rows, their entries, the (group, task id) order, the outputs
+  int nl = 0;
+  if (H > 0) {
+    CK(pool, cudaMemsetAsync(host_of, 0xff, sizeof(int32_t) * (size_t)n_codes, st));
+    host_map_kernel<<<(H + 255) / 256, 256, 0, st>>>(d_codes, H, host_of);
+    nl++;
+  }
+  compact(CotaskRows{S->run.at<uint8_t>(R_LIVE), a.host, a.glen, slot}, S->run.hw, nullptr, blk, S->counters + 3, K,
+          st, &nl);
+  order_scan(a.os, RowLen{slot, a.glen}, K, S->gf0, st, &nl);
+  cotask_expand_kernel<<<(K + 255) / 256, 256, 0, st>>>(a);
+  nl++;
+  CK(pool, csort::sort_indices(ord, tmp, (int)N, LessKeyTid{a.e_grp, a.e_tid}, st, &nl));
+  const int np = std::max((int)N, G + 1);
+  cotask_out_kernel<<<(np + 255) / 256, 256, 0, st>>>(ord, a.e_grp, a.e_host, a.e_attr, (int)N, G, d_off, d_host, d_attr);
+  nl++;
+  CK(pool, cudaGetLastError());
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  CK(pool, download(out_off, d_off, (size_t)G + 1, st, &d2h));
+  CK(pool, download(out_host, d_host, (size_t)N, st, &d2h));
+  CK(pool, download(out_attr, d_attr, (size_t)N, st, &d2h));
+  CK(pool, cudaEventRecord(pool->ev[23], st));
+  CK(pool, cudaStreamSynchronize(st));
+  record_phase(pool, COOK_PHASE_COTASKS, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[23], h2d, d2h, nl);
+  return COOK_OK;
+}
+
 }  // namespace
 
 extern "C" int32_t cook_state_apply(cook_pool* pool, const cook_state_delta* delta) {
@@ -1074,6 +1302,14 @@ extern "C" int32_t cook_state_usage(cook_pool* pool, int32_t n_users, double* ou
   if (!S) return set_err(pool, COOK_E_OOM, "cook_state_usage: out of device memory");
   return usage(pool, S, n_users, out_user_usage, out_pool_usage, n_hosts, hostname_id, out_run_cpus, out_run_mem,
                out_run_count);
+}
+
+extern "C" int32_t cook_state_cotasks(cook_pool* pool, int32_t n_groups, const int32_t* attr_col,
+                                      const cook_host_table* hosts, int32_t cap, int32_t* out_cot_off,
+                                      int32_t* out_cot_hostname_id, int32_t* out_cot_attr_val, int32_t* out_n) {
+  if (!pool) return COOK_E_BADARG;
+  return cotasks(pool, static_cast<PoolState*>(pool->state), n_groups, attr_col, hosts, cap, out_cot_off,
+                 out_cot_hostname_id, out_cot_attr_val, out_n);
 }
 
 extern "C" int32_t cook_state_rank(cook_pool* pool, const cook_user_table* users, const cook_pool_quota* pool_quota,

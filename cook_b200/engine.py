@@ -62,7 +62,8 @@ def load_library(path=None):
                  "cook_allgather_usage", "cook_last_stats", "cook_comm_unique_id", "cook_comm_init",
                  "cook_comm_destroy", "cook_exchange_usage", "cook_exchange_usage_batch", "cook_rebalance_trace",
                  "cook_match_failures", "cook_state_apply", "cook_state_rank", "cook_state_match",
-                 "cook_state_rebalance", "cook_state_launch", "cook_state_patch", "cook_state_usage"):
+                 "cook_state_rebalance", "cook_state_launch", "cook_state_patch", "cook_state_usage",
+                 "cook_state_cotasks"):
         getattr(lib, name).restype = C.c_int32
     return lib
 
@@ -230,6 +231,32 @@ class GpuEngine:
         U = int(n_users)
         return {"user": {k: user[i * U:(i + 1) * U].copy() for i, k in enumerate(("count", "cpus", "mem", "gpus"))},
                 "pool": pool, "run_cpus": rc_[:H].copy(), "run_mem": rm[:H].copy(), "run_count": rn[:H].copy()}
+
+    def state_cotasks(self, n_groups, attr_col=None, hosts=None):
+        """cook_state_cotasks: each group's running cotasks from the live running rows with a known host, by (group,
+        task id).  Returns (cot_off, cot_hostname_id, cot_attr_val), the cot_* fields of abi.Groups; the attribute
+        value is hosts' (an abi.OffersSoA or abi.HostTable) in the group's attr_col, 0 where there is none."""
+        ac = np.ascontiguousarray(attr_col, np.int32) if attr_col is not None else None
+        if ac is not None and len(ac) != n_groups:
+            raise ValueError("state_cotasks: attr_col needs one column per group")
+        hp = None
+        if hosts is not None:   # the fields cook_state_cotasks reads, from an offer table or a host table
+            hp = abi.HostTable(n=hosts.n, hostname_id=hosts.col("hostname_id"), n_attr_cols=hosts.n_attr_cols,
+                               attr=hosts.col("attr"))
+        args = (self.pool, int(n_groups), abi.ptr(ac, abi.P_I32) if ac is not None else None,
+                C.byref(hp) if hp is not None else None)
+        n = C.c_int32(0)
+        rc = self.lib.cook_state_cotasks(*args, 0, None, None, None, C.byref(n))
+        if rc != 0:
+            self._err(rc)
+        cap = n.value
+        off = np.zeros(int(n_groups) + 1, np.int32)
+        host, val = np.zeros(max(cap, 1), np.int32), np.zeros(max(cap, 1), np.int32)
+        rc = self.lib.cook_state_cotasks(*args, cap, abi.ptr(off, abi.P_I32), abi.ptr(host, abi.P_I32),
+                                         abi.ptr(val, abi.P_I32), C.byref(n))
+        if rc != 0:
+            self._err(rc)
+        return off, host[:n.value], val[:n.value]
 
     def state_rank(self, users, pool_quota=None, group_quota=None, group_usage=None, params=None):
         """cook_state_rank: the live rows ranked; the queue stays on the device.  Returns its job ids."""

@@ -434,13 +434,19 @@ int32_t cook_rebalance_trace(cook_pool* pool, const cook_running_soa* running,
  *   running_rm_task_id  removals
  *   running_hostname_id the host of each running upsert: a code of the global hostname dictionary (the
  *                       code space of cook_offers_soa.hostname_id and cook_host_table.hostname_id).  NULL
- *                       stores -1, "host unknown"; only cook_state_rebalance reads it.
- * A launch can be one batch (remove pending job j, upsert its running task); cook_state_launch does the
- * same from job ids without re-sending the rows.  An upsert of a pending row gives it a new generation,
- * so it leaves the last rank's queue; cook_state_patch changes the match-time columns without that.
+ *                       stores -1, "host unknown"; cook_state_rebalance, cook_state_usage and
+ *                       cook_state_cotasks read it.
+ *   running_group_off   the group list of each running upsert, its job's groups (:group/_job): CSR
+ *   running_group_idx   offsets [running.n + 1] over the upserts and group codes.  NULL stores empty lists.
+ *                       Only cook_state_cotasks reads them.
+ * An upsert of a known id replaces the row with its lists; a removal or reset drops them.
+ * A launch can be one batch (remove pending job j, upsert its running task with j's group list);
+ * cook_state_launch does the same from job ids without re-sending the rows.  An upsert of a pending row gives
+ * it a new generation, so it leaves the last rank's queue; cook_state_patch changes the match-time columns
+ * without that.
  * COOK_E_BADARG, state unchanged: an unknown id in a removal, an id twice in one table of the batch, a
- * malformed CSR offset column, a negative user / attr_col / group / novel hostname code, a
- * reserved_host or running_hostname_id below -1.
+ * malformed CSR offset column, a negative user / attr_col / group (pending or running) / novel hostname
+ * code, a reserved_host or running_hostname_id below -1.
  * Codes are checked here, when they enter; their maxima are kept on the host, and rank / match reject a
  * user, offer or group table too small for them.  Group codes and attribute value codes must therefore
  * come from stable, append-only dictionaries (INTEGRATION.md §3b).
@@ -457,6 +463,8 @@ typedef struct {
   int32_t n_running_rm;
   const int64_t* running_rm_task_id;
   const int32_t* running_hostname_id;
+  const int32_t* running_group_off;
+  const int32_t* running_group_idx;
 } cook_state_delta;
 int32_t cook_state_apply(cook_pool* pool, const cook_state_delta* delta);
 
@@ -464,8 +472,10 @@ int32_t cook_state_apply(cook_pool* pool, const cook_state_delta* delta);
  * hostname_id[i] (a code of the global hostname dictionary; a NULL column stores -1, "host unknown").  User,
  * priority, job id, cpus, mem and gpus are copied on the device from the pending row.  Leaves exactly the
  * state cook_state_apply leaves after the batch pending_rm_job_id = job_id plus the running upserts built
- * from those rows with running_hostname_id = hostname_id: the job leaves the last rank's queue, its list
- * entries, counts and reservation leave with the row, and the list arenas compact by the same rule.
+ * from those rows with running_hostname_id = hostname_id and, as running_group_off / running_group_idx, the
+ * pending rows' group lists: the job leaves the last rank's queue, its counts and reservation leave with the
+ * row, its group list moves to the task (copied on the device, in launch order) while its other list
+ * entries leave, and the list arenas compact by the same rule.
  * COOK_E_BADARG, before any change: n < 0; a NULL job_id, task_id or start_time while n > 0; a job id that
  * is not live or appears twice; a task id that appears twice or is already live; a hostname code below -1.
  * Uploads exactly n * (4 + 4 + 8 + 8) bytes (pending slot, running slot, task id, start time), plus 4 * n
@@ -555,14 +565,47 @@ int32_t cook_state_usage(cook_pool* pool, int32_t n_users, double* out_user_usag
                          int32_t n_hosts, const int32_t* hostname_id, double* out_run_cpus,
                          double* out_run_mem, int32_t* out_run_count);
 
+/* Each group's running cotasks, read from the live running rows: the lists cook_groups.cot_* takes, for
+ * cook_state_match and cook_state_rebalance.  A group's cotasks are the running instances of its jobs
+ * (group->running-task-set, group.clj:47-57) that Fenzo's tracker knows, i.e. that are assigned to a host
+ * (get-cotasks-from-tracker-state, constraints.clj:539-552).
+ *   Entries     one per (live running row, group in its running_group_idx list) whose running_hostname_id is
+ *               not -1.
+ *   Order       grouped by group code; within a group, ascending task id (DESIGN.md §2).
+ *               out_cot_off[n_groups + 1] is the CSR over groups; a group without entries has an empty range.
+ *   Values      out_cot_hostname_id[k]: the row's running_hostname_id.  out_cot_attr_val[k]:
+ *               hosts->attr[attr_col[g]][h], h the index in `hosts` whose hostname_id is the row's host; 0 (nil)
+ *               when that host is not listed, when hosts is NULL, or when attr_col is NULL or attr_col[g] == -1.
+ *               An unlisted host keeps its entry and hostname code, so unique groups still see it.  Only n,
+ *               hostname_id, n_attr_cols and attr of `hosts` are read: for a match, point them at the offer
+ *               table's columns; for a rebalance, pass the host table given to cook_state_rebalance.
+ * Size query: with out_cot_hostname_id NULL only *out_n is written, the required capacity (known on the host,
+ * no device work).  Otherwise *out_n receives the number of entries and the capacity of the two value outputs is
+ * cap.
+ * COOK_E_BADARG, before any device work and with nothing written: a NULL out_n, or (not a size query) a NULL
+ * out_cot_off or out_cot_attr_val; n_groups < 0 or <= a live running row's group code; cap < the required size
+ * (not a size query); attr_col[g] outside [-1, hosts->n_attr_cols) (read only when hosts is given); hosts->n < 0,
+ * a NULL hostname_id with hosts->n > 0, a hostname_id that is negative or appears twice; a NULL hosts->attr when
+ * some group names a column and hosts->n > 0.
+ * No state, or no live running row with a known host and a group: every offset is 0, *out_n = 0, no device work.
+ * Transfers exactly: up 4 * hosts->n (the hostname codes) + 4 * hosts->n per distinct column the groups name
+ * + 4 * n_groups; down 4 * (n_groups + 1) + 8 * *out_n.  Nothing proportional to the running table moves, and
+ * nothing when there is no device work.  Changes nothing resident; needs no cook_state_rank.
+ * Statistics: cook_last_stats(COOK_PHASE_COTASKS).                                                          */
+int32_t cook_state_cotasks(cook_pool* pool, int32_t n_groups, const int32_t* attr_col, const cook_host_table* hosts,
+                           int32_t cap, int32_t* out_cot_off, int32_t* out_cot_hostname_id, int32_t* out_cot_attr_val,
+                           int32_t* out_n);
+
 /* ------------------------------------------------------------ phase timing */
 /* Device-side timing of the last call of each kind on this handle (CUDA events on the
  * pool's stream): what bench.py's `phases` block and roofline lines are computed from.
  * COOK_PHASE_STATE: the last cook_state_apply, cook_state_launch or cook_state_patch (upload, then the
  * scatter / move / compaction kernels).  COOK_PHASE_USAGE: the last cook_state_usage (upload of the
- * hostname list, the compaction, sorts and folds, the download of the sums). */
+ * hostname list, the compaction, sorts and folds, the download of the sums).  COOK_PHASE_COTASKS: the last
+ * cook_state_cotasks (upload of the host codes, attribute columns and group map, the compaction, expansion and
+ * sort, the download of the lists; all zero after a call without device work). */
 enum { COOK_PHASE_RANK = 0, COOK_PHASE_MATCH = 1, COOK_PHASE_REBALANCE = 2, COOK_PHASE_EXCHANGE = 3,
-       COOK_PHASE_STATE = 4, COOK_PHASE_USAGE = 5 };
+       COOK_PHASE_STATE = 4, COOK_PHASE_USAGE = 5, COOK_PHASE_COTASKS = 6 };
 typedef struct {
   double ms_h2d;      /* upload stage                                              */
   double ms_device;   /* kernels (for the exchange: delta kernels + the collective) */

@@ -159,7 +159,7 @@ JFN(jint, matchFailures)(JNIEnv* env, jclass k, jlong pool, jobject k_idx, jint 
 JFN(jint, stateApply)(JNIEnv* env, jclass k, jlong pool, jint reset, jint n_pending, jobjectArray pending,
                       jobject pending_priority, jobject pending_job_id, jint n_pending_rm, jobject pending_rm_job_id,
                       jint n_running, jobjectArray running, jint n_running_rm, jobject running_rm_task_id,
-                      jobject running_hostname_id) {
+                      jobject running_hostname_id, jobject running_group_off, jobject running_group_idx) {
   cook_state_delta d;
   memset(&d, 0, sizeof(d));
   d.reset = reset;
@@ -169,6 +169,7 @@ JFN(jint, stateApply)(JNIEnv* env, jclass k, jlong pool, jint reset, jint n_pend
   if (running) tasks_from(env, n_running, running, &d.running);
   d.n_running_rm = n_running_rm; d.running_rm_task_id = one(env, running_rm_task_id);
   d.running_hostname_id = one(env, running_hostname_id);
+  d.running_group_off = one(env, running_group_off); d.running_group_idx = one(env, running_group_idx);
   return cook_state_apply((cook_pool*)(intptr_t)pool, &d);
 }
 /* launches by job id: the task columns the device already holds are not sent (hostname_id may be null) */
@@ -192,6 +193,20 @@ JFN(jint, stateUsage)(JNIEnv* env, jclass k, jlong pool, jint n_users, jobject o
   return cook_state_usage((cook_pool*)(intptr_t)pool, n_users, one(env, out_user_usage), one(env, out_pool_usage),
                           n_hosts, one(env, hostname_id), one(env, out_run_cpus), one(env, out_run_mem),
                           one(env, out_run_count));
+}
+/* each group's running cotasks (the cot_* columns of `groups` for stateMatch / stateRebalance); `hosts` holds the
+ * hosts_from columns (only hostname_id and attr are read) or is null; out_cot_hostname_id null: a size query */
+JFN(jint, stateCotasks)(JNIEnv* env, jclass k, jlong pool, jint n_groups, jobject attr_col, jint n_hosts,
+                        jint n_attr_cols, jobjectArray hosts, jint cap, jobject out_cot_off, jobject out_cot_hostname_id,
+                        jobject out_cot_attr_val, jintArray out_n) {
+  cook_host_table h;
+  memset(&h, 0, sizeof(h));
+  if (hosts) hosts_from(env, n_hosts, n_attr_cols, hosts, &h);
+  int32_t n = 0;
+  jint rc = cook_state_cotasks((cook_pool*)(intptr_t)pool, n_groups, one(env, attr_col), hosts ? &h : NULL, cap,
+                               one(env, out_cot_off), one(env, out_cot_hostname_id), one(env, out_cot_attr_val), &n);
+  if (rc == COOK_OK) (*env)->SetIntArrayRegion(env, out_n, 0, 1, (jint*)&n);
+  return rc;
 }
 JFN(jint, stateRank)(JNIEnv* env, jclass k, jlong pool, jint n_users, jobjectArray users, jdoubleArray pool_quota,
                      jdoubleArray group_quota, jobject group_usage, jint max_over_quota_jobs, jint filter_offensive,

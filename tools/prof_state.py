@@ -32,6 +32,14 @@ on the host (what a shim runs without the call), and whether the two agree to th
 
   python tools/prof_state.py --usage --pool c2 --cycles 5
   python tools/prof_state.py --usage --pool c5 --c5-pool 5 --cycles 5
+
+--cotasks loads a config-#3-shaped pool (its pending jobs, and its running tasks on random hosts of the offer table,
+one in five in a group, 1 % with host unknown) and per cycle launches group members, finishes 3 % of the running
+tasks and submits new group members.  It then runs cook_state_cotasks against the same lists built by numpy from a
+host mirror of the running tasks (task -> host, groups), printing the call's device time, wall time and bytes, the
+wall time of the host build, and whether the two are identical.
+
+  python tools/prof_state.py --cotasks --cycles 6
 """
 import argparse
 import json
@@ -186,6 +194,107 @@ def usage(a):
         e.close()
 
 
+def host_cotasks(tid, host, gidx, goff, G, acol, codes, attr):
+    """What a shim computes without cook_state_cotasks, from its mirror of the running tasks: one entry per (task
+    with a host, group), by (group, task id), with the host's attribute in the group's column (0: unlisted)."""
+    lens = np.diff(goff)
+    keep = np.repeat(host != -1, lens)
+    g = gidx[keep]
+    t = np.repeat(tid, lens)[keep]
+    h = np.repeat(host, lens)[keep]
+    o = np.lexsort((t, g))
+    g, h = g[o], h[o]
+    idx = np.full(max(int(codes.max()), int(h.max()) if len(h) else 0) + 1, -1, np.int64)
+    idx[codes] = np.arange(len(codes))
+    hi = idx[h]
+    c = acol[g]
+    val = np.where((hi >= 0) & (c >= 0), attr[np.maximum(c, 0), np.maximum(hi, 0)], 0).astype(np.int32)
+    off = np.searchsorted(g, np.arange(G + 1)).astype(np.int32)
+    return off, h.astype(np.int32), val
+
+
+def cotasks_prof(a):
+    t = traces.gen_config_pool("c3", a.c3_pool) if a.c3_pool >= 0 else traces.gen_c3_pool(a.seed)
+    jobs, pc, rc = t["jobs"], t["cols"]["pending"], t["cols"]["running"]
+    offers, groups = t["offers"], t["groups"]
+    G, acol = groups.n_groups, groups.col("attr_col")
+    codes = offers.col("hostname_id").astype(np.int32)
+    attr = offers.col("attr").reshape(offers.n_attr_cols, offers.n)
+    rng = np.random.default_rng(a.seed)
+    J, R = jobs.n, len(rc["task_id"])
+    goff_j, gidx_j = jobs.col("group_off"), jobs.col("group_idx")
+    jgroups = [gidx_j[goff_j[i]:goff_j[i + 1]] for i in range(J)]
+    members = [i for i in range(J) if len(jgroups[i])]
+    # the host mirror: task id -> (host, groups)
+    run = {int(rc["task_id"][i]): (int(codes[rng.integers(len(codes))]) if rng.random() > 0.01 else -1,
+                                   [int(rng.integers(G))] if rng.random() < 0.2 else []) for i in range(R)}
+    print(json.dumps({"card": card(), "pool": f"c3/{a.c3_pool}" if a.c3_pool >= 0 else "c3-shaped", "jobs": J,
+                      "running": R, "groups": G, "offers": offers.n}), flush=True)
+    e = GpuEngine(pool_name="cotasks")
+
+    def run_delta(items, rm=()):
+        tids = np.array([k for k, _ in items], np.int64)
+        n = len(items)
+        off, idx = abi.csr([v[1] for _, v in items])
+        return abi.make_delta(running=abi.make_tasks(user=np.zeros(n, np.int32), priority=np.full(n, 50, np.int32),
+                                                     start_time=np.full(n, 1_700_000_000_000, np.int64), task_id=tids,
+                                                     job_id=tids + 1, cpus=np.ones(n), mem=np.ones(n)) if n else None,
+                              running_hostname_id=np.array([v[0] for _, v in items], np.int32) if n else None,
+                              running_group_off=off if n else None, running_group_idx=idx if n else None,
+                              running_rm=rm)
+
+    e.state_apply(run_delta(list(run.items())))
+    # pending group members, launched a batch per cycle on the device
+    jid0 = 10 ** 12
+    pend = {jid0 + i: list(map(int, jgroups[m])) for i, m in enumerate(members)}
+    off, idx = abi.csr(list(pend.values()))
+    n = len(pend)
+    e.state_apply(abi.make_delta(pending=abi.JobsSoA(n=n, user=np.zeros(n, np.int32), cpus=np.ones(n), mem=np.ones(n),
+                                                     group_off=off, group_idx=idx),
+                                 pending_priority=np.full(n, 50, np.int32), pending_job_id=np.array(list(pend), np.int64)))
+    next_tid = max(run) + 10
+    for cycle in range(a.cycles):
+        # ---- the churn: launch group members, finish 3 %, submit as many new members
+        nl = min(len(pend), max(1, len(members) // 8))
+        lj = [int(j) for j in rng.choice(sorted(pend), nl, replace=False)]
+        lt = [next_tid + 2 * i for i in range(nl)]
+        next_tid += 2 * nl + 2
+        lh = codes[rng.integers(0, len(codes), nl)].astype(np.int32)
+        e.state_launch(lj, lt, np.full(nl, 1_700_000_000_000, np.int64), lh)
+        for j, t_, h in zip(lj, lt, lh):
+            run[t_] = (int(h), pend.pop(j))
+        fin = [int(x) for x in rng.choice(sorted(run), int(len(run) * 0.03), replace=False)]
+        for x in fin:
+            del run[x]
+        new = {jid0 + 10 ** 6 * (cycle + 1) + i: [int(rng.integers(G))] for i in range(nl)}
+        off, idx = abi.csr(list(new.values()))
+        e.state_apply(abi.make_delta(pending=abi.JobsSoA(n=nl, user=np.zeros(nl, np.int32), cpus=np.ones(nl),
+                                                         mem=np.ones(nl), group_off=off, group_idx=idx),
+                                     pending_priority=np.full(nl, 50, np.int32),
+                                     pending_job_id=np.array(list(new), np.int64), running_rm=fin))
+        pend.update(new)
+        # ---- the lists, on the device and from the host mirror
+        w0 = time.perf_counter()
+        got = e.state_cotasks(G, acol, offers)
+        w_dev = time.perf_counter() - w0
+        st = e.last_stats(abi.PHASE_COTASKS)
+        w0 = time.perf_counter()
+        tid = np.fromiter(run.keys(), np.int64, len(run))
+        host = np.fromiter((v[0] for v in run.values()), np.int32, len(run))
+        goff = np.zeros(len(run) + 1, np.int64)
+        np.cumsum([len(v[1]) for v in run.values()], out=goff[1:])
+        gidx = np.fromiter((g for v in run.values() for g in v[1]), np.int32, int(goff[-1]))
+        want = host_cotasks(tid, host, gidx, goff, G, acol, codes, attr)
+        w_host = time.perf_counter() - w0
+        same = all(np.array_equal(x, y) for x, y in zip(got, want))
+        print(json.dumps({"cycle": cycle, "running": len(run), "entries": len(got[1]),
+                          "state_cotasks": {**{k: round(st[k], 3) for k in ("ms_h2d", "ms_device", "ms_d2h")},
+                                            "wall_ms": round(1e3 * w_dev, 3), "h2d_bytes": st["h2d_bytes"],
+                                            "d2h_bytes": st["d2h_bytes"], "n_launches": st["n_launches"]},
+                          "host_build_wall_ms": round(1e3 * w_host, 3), "identical": bool(same)}), flush=True)
+    e.close()
+
+
 def launch_cycle(cycle, res, twin, job_id, lt, hosts, rest, match_args):
     """One cycle of --launch: the launches by id on `res` and as a delta on `twin`, the rest of the batch on both,
     then rank and match on both.  Returns the jobs the match placed and their hosts' codes."""
@@ -228,11 +337,15 @@ def main():
     ap.add_argument("--cycles", type=int, default=6)
     ap.add_argument("--seed", type=int, default=7)
     ap.add_argument("--usage", action="store_true")
+    ap.add_argument("--cotasks", action="store_true")
+    ap.add_argument("--c3-pool", type=int, default=-1, help="--cotasks: a config-#3 pool (-1: the smaller c3-shaped pool)")
     a = ap.parse_args()
     if a.rebalance:
         return rebalance(a)
     if a.usage:
         return usage(a)
+    if a.cotasks:
+        return cotasks_prof(a)
     t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
     jobs, pc, rc = t["jobs"], t["cols"]["pending"], t["cols"]["running"]
     J = jobs.n
