@@ -163,6 +163,20 @@
   [handle args]
   (check! handle (apply #(Native/stateCotasks handle %&) args) "cook_state_cotasks"))
 
+(defn match-derived!
+  "The resident match cycle in one call (cook_state_match_derived): the users' usage, the offers' run columns and
+   the groups' cotask lists are read from the resident running rows on the device, so `args` (Native/stateMatch's
+   arguments after the handle) may leave those columns nil.  Replaces cotasks! and the usage fold before a state
+   match."
+  [handle args]
+  (check! handle (apply #(Native/stateMatchDerived handle %&) args) "cook_state_match_derived"))
+
+(defn rebalance-derived!
+  "cook_state_rebalance_derived: the rebalancer over the resident rows with the groups' cotask lists derived on the
+   device over the host table in `args` (Native/stateRebalance's arguments after the handle)."
+  [handle args]
+  (check! handle (apply #(Native/stateRebalanceDerived handle %&) args) "cook_state_rebalance_derived"))
+
 (defn exchange-usage!
   "§8e: after a pool's match round; `comm` from Native/commInit (rank 0's Native/commUniqueId bytes travel
    over Cook's own control plane).  Returns the [world n-pad] table as a DoubleBuffer."

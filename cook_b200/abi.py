@@ -218,6 +218,18 @@ def ptr(arr, ctype):
     return arr.ctypes.data_as(ctype)
 
 
+_STATE_MATCH = [C.c_void_p, C.POINTER(OffersSoA), C.POINTER(Groups), C.POINTER(UserTable), C.POINTER(PoolQuota),
+                C.POINTER(MatchParams), P_I64, P_I32, P_I32, C.c_int32, P_U8, C.POINTER(MatchStats)]
+_STATE_REBALANCE = [C.c_void_p, C.POINTER(HostTable), C.POINTER(Groups), C.POINTER(UserTable),
+                    C.POINTER(RebalanceParams), C.POINTER(Decision), P_I64, P_I64, C.c_int32, C.POINTER(C.c_int32)]
+# ctypes argument types of the entry points that declare them (engine.load_library sets them); the derived calls
+# take exactly cook_state_match's and cook_state_rebalance's arguments
+ARGTYPES = {
+    "cook_state_match_derived": _STATE_MATCH,
+    "cook_state_rebalance_derived": _STATE_REBALANCE,
+}
+
+
 # ------------------------------------------------------------------ builders
 def make_tasks(user, priority, start_time, task_id, job_id, cpus, mem, gpus=None):
     n = len(user)

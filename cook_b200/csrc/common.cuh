@@ -185,6 +185,15 @@ int32_t rank_impl(cook_pool* pool, int R, int J, const cook_tasks_soa* running, 
                   int32_t* out_ranked_idx, int32_t* out_n, double* out_dru, int32_t* out_order, int32_t* out_order_n,
                   RankQueue* queue);
 
+// The running-side inputs of a match or rebalance that the resident state derives on the device after the build:
+// carved, not uploaded.  usage: the users' usage_* as one [4][n_users] block (count, cpus, mem, gpus); run: the
+// offers' run_cpus, run_mem and run_count; cot: the groups' cot_* lists, sized for n_cot entries (carved where
+// the plan reads the lists).
+struct Derived {
+  bool usage = false, run = false, cot = false;
+  int64_t n_cot = 0;
+};
+
 // match.cu: what a match's plan needs to know about its jobs before it carves their columns.
 struct JobShape {
   int J = 0;                      // job rows
@@ -195,18 +204,28 @@ struct JobShape {
   std::vector<int32_t> gp_off;    // [n_groups + 1] per-group member capacity offsets (empty: no groups)
   bool any_gpus_ports = false;    // some job asks for gpus or ports
   bool job_ids = false;           // carve a job id per row, and report the considerable jobs by job id
+  Derived dev;                    // the users', offers' and groups' columns the caller fills on the device
 };
 // The carved rows of a plan whose columns the caller writes: row d is ranked[d] = d.
+// The columns of shape.dev, null where not carved: usage [4][n_users]; run_* [offers->n] by input index;
+// cot_off [n_groups + 1], cot_host / cot_attr [max(1, n_cot)].  What a derivation reads from the plan's uploads:
+// the offers' hostname codes, their [n_attr_cols][offers->n] attribute matrix and the groups' attr_col (each
+// null when not uploaded).
 struct MatchRows {
   JobDev jb;
   int32_t* ranked;
   int64_t* job_id;
+  double* usage;
+  double* run_cpus; double* run_mem; int32_t* run_count;
+  int32_t* cot_off; int32_t* cot_host; int32_t* cot_attr;
+  const int32_t* hostname_id; const int32_t* attr; const int32_t* gcol;
 };
 // The checks of a match's offers, groups, users, params and sizes, with `who` in the messages.  The offer
 // and group tables are checked when `tables`; `novel` and `grouped`: some job has novel-host or group lists.
+// `cot_derived`: the groups' cot_* lists are derived on the device, so they are not required.
 int32_t check_match_inputs(cook_pool* pool, const char* who, const cook_offers_soa* offers, const cook_groups* groups,
                            const cook_user_table* users, const cook_match_params* params, int32_t max_ports,
-                           bool tables, bool novel, bool grouped);
+                           bool tables, bool novel, bool grouped, bool cot_derived = false);
 // The pool's match plan is built for n_ranked rows of the jobs `sh` describes (ranked_idx: uploaded, null:
 // the caller writes *rows before the run), then run.  A failed build leaves no valid plan.
 int32_t match_build(cook_pool* pool, const int32_t* ranked_idx, int32_t n_ranked, const JobShape& sh,
@@ -225,6 +244,7 @@ struct RebShape {
   const int64_t* job_id = nullptr;
   const int32_t* priority = nullptr;
   int64_t n_novel = 0, n_attr = 0, n_group = 0;   // caller-written rows: entries each list may hold (0: no list)
+  Derived dev;                                    // caller-written rows: only .cot applies
 };
 // The carved rows a caller writes before the run: running task r < R (host: index into the host table) and
 // pending job p < P, with the pending lists the shape asked for.
@@ -235,6 +255,9 @@ struct RebRows {
   const int64_t* jid;
   const int32_t* prio;
   const int32_t* hostname_id;   // the host table's codes, uploaded [hosts->n]
+  const int32_t* attr;          // its [n_attr_cols][hosts->n] attribute matrix (null: none uploaded)
+  const int32_t* gcol;          // the groups' attr_col, uploaded (null: none)
+  int32_t* cot_off; int32_t* cot_host; int32_t* cot_attr;   // sh.dev.cot and the walk reads the lists, else null
 };
 struct RebPlan;
 struct RebPlanFree { void operator()(RebPlan* p) const; };

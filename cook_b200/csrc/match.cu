@@ -2331,6 +2331,7 @@ int32_t match_build(cook_pool* pool, const int32_t* ranked_idx, int32_t n_ranked
   OfferDev of;
   GroupDev gr;
   int32_t* ranked = nullptr;
+  double* usage = nullptr;
   memset(&ca, 0, sizeof(ca));
   memset(&ma, 0, sizeof(ma));
   memset(&jb, 0, sizeof(jb));
@@ -2374,9 +2375,14 @@ int32_t match_build(cook_pool* pool, const int32_t* ranked_idx, int32_t n_ranked
 
     mp->d_perm = c.up(perm.data(), O); of.perm = mp->d_perm;
     mp->d_oc = c.up(offers->cpus, O); mp->d_om = c.up(offers->mem, O);
-    mp->d_orc = c.up(offers->run_cpus, O); mp->d_orm = c.up(offers->run_mem, O);
+    if (sh.dev.run) {
+      mp->d_orc = c.take<double>(O ? O : 1); mp->d_orm = c.take<double>(O ? O : 1);
+    } else {
+      mp->d_orc = c.up(offers->run_cpus, O); mp->d_orm = c.up(offers->run_mem, O);
+    }
     mp->d_vs = c.take<VmStatic>(O + 1); of.vs = mp->d_vs;
-    of.hostname_id = c.up(offers->hostname_id, O); of.run_count = c.up(offers->run_count, O);
+    of.hostname_id = c.up(offers->hostname_id, O);
+    of.run_count = sh.dev.run ? c.take<int32_t>(O ? O : 1) : c.up(offers->run_count, O);
     mp->d_ports_total = nullptr;
     if (offers->port_off) {
       const int np = std::max(1, offers->port_off[O]);
@@ -2408,18 +2414,30 @@ int32_t match_build(cook_pool* pool, const int32_t* ranked_idx, int32_t n_ranked
       gr.kind = c.up(groups->kind, G);
       gr.attr_col = c.up(groups->attr_col, G);
       gr.minimum = c.up(groups->minimum, G);
-      gr.cot_off = c.up(groups->cot_off, G + 1);
-      const int nc = std::max(1, groups->cot_off[G]);
-      gr.cot_host = c.up(groups->cot_hostname_id, nc);
-      gr.cot_attr = c.up(groups->cot_attr_val, nc);
+      if (sh.dev.cot) {
+        const size_t nc = std::max<int64_t>(1, sh.dev.n_cot);
+        gr.cot_off = c.take<int32_t>(G + 1);
+        gr.cot_host = c.take<int32_t>(nc); gr.cot_attr = c.take<int32_t>(nc);
+      } else {
+        gr.cot_off = c.up(groups->cot_off, G + 1);
+        const int nc = std::max(1, groups->cot_off[G]);
+        gr.cot_host = c.up(groups->cot_hostname_id, nc);
+        gr.cot_attr = c.up(groups->cot_attr_val, nc);
+      }
       gr.gp_off = c.up(sh.gp_off.data(), G + 1);
       gr.gp_n = c.take<int32_t>(G + 1);
       gr.gp_vm = c.take<int32_t>(n_memb + 1);
     }
     ca.q_count = c.up(users->quota_count, U); ca.q_cpus = c.up(users->quota_cpus, U);
     ca.q_mem = c.up(users->quota_mem, U); ca.q_gpus = c.up(users->quota_gpus, U);
-    ca.u_count = c.up(users->usage_count, U); ca.u_cpus = c.up(users->usage_cpus, U);
-    ca.u_mem = c.up(users->usage_mem, U); ca.u_gpus = c.up(users->usage_gpus, U);
+    if (sh.dev.usage) {
+      usage = c.take<double>(4 * (size_t)U);
+      ca.u_count = usage; ca.u_cpus = usage ? usage + U : nullptr;
+      ca.u_mem = usage ? usage + 2 * U : nullptr; ca.u_gpus = usage ? usage + 3 * U : nullptr;
+    } else {
+      ca.u_count = c.up(users->usage_count, U); ca.u_cpus = c.up(users->usage_cpus, U);
+      ca.u_mem = c.up(users->usage_mem, U); ca.u_gpus = c.up(users->usage_gpus, U);
+    }
     ca.tokens = c.up(users->tokens, U);
 
     for (int b = 0; b < 2; b++) {
@@ -2491,7 +2509,13 @@ int32_t match_build(cook_pool* pool, const int32_t* ranked_idx, int32_t n_ranked
   if (const char* el = getenv("COOK_LOOKAHEAD")) { int v = atoi(el); if (v >= 2 && v <= RING - 1) ma.lookahead = v; }
   mp->J = J; mp->O = O; mp->U = U; mp->n_ranked = n_ranked; mp->NC = NC; mp->max_ports = max_ports;
   mp->G = G; mp->B = B; mp->constr = constr_eff; mp->n_memb = n_memb;
-  if (rows) *rows = MatchRows{jb, ranked, mp->d_job_id};
+  if (rows) {
+    const bool run = sh.dev.run, cot = sh.dev.cot && grouped;
+    *rows = MatchRows{jb, ranked, mp->d_job_id, usage, run ? mp->d_orc : nullptr, run ? mp->d_orm : nullptr,
+                      run ? writable(of.run_count) : nullptr, cot ? writable(gr.cot_off) : nullptr,
+                      cot ? writable(gr.cot_host) : nullptr, cot ? writable(gr.cot_attr) : nullptr, of.hostname_id,
+                      of.attr, gr.attr_col};
+  }
   return COOK_OK;
 }
 
@@ -2705,7 +2729,7 @@ int32_t match_run(cook_pool* pool, int32_t* out_considerable, int64_t* out_job_i
 
 int32_t check_match_inputs(cook_pool* pool, const char* who, const cook_offers_soa* offers, const cook_groups* groups,
                            const cook_user_table* users, const cook_match_params* params, int32_t max_ports,
-                           bool tables, bool novel, bool grouped) {
+                           bool tables, bool novel, bool grouped, bool cot_derived) {
   if (params->good_enough_fitness < 1.0)
     return set_err(pool, COOK_E_BADARG,
                    "%s: good_enough_fitness < 1.0 is Fenzo's racy early-exit mode; "
@@ -2721,7 +2745,7 @@ int32_t check_match_inputs(cook_pool* pool, const char* who, const cook_offers_s
   grouped = grouped && groups && groups->n_groups;
   if ((novel || offers->reserved || grouped) && !offers->hostname_id)
     return set_err(pool, COOK_E_BADARG, "%s: hostname_id column required by constraints", who);
-  if (grouped && (!groups->cot_off || !groups->kind)) return set_err(pool, COOK_E_BADARG, "%s: incomplete cook_groups", who);
+  if (grouped && ((!cot_derived && !groups->cot_off) || !groups->kind)) return set_err(pool, COOK_E_BADARG, "%s: incomplete cook_groups", who);
   return COOK_OK;
 }
 

@@ -1107,9 +1107,15 @@ static int32_t build(cook_pool* pool, const RebShape& sh, const cook_host_table*
       pc.group_idx = pend_col(pending.group_idx, std::max<int64_t>(1, up ? pending.group_off[P] : sh.n_group));
       gc.n = G;
       gc.kind = c.up(groups->kind, G); gc.attr_col = c.up(groups->attr_col, G);
-      gc.minimum = c.up(groups->minimum, G); gc.cot_off = c.up(groups->cot_off, G + 1);
-      const int n = std::max(1, groups->cot_off[G]);
-      gc.cot_host = c.up(groups->cot_hostname_id, n); gc.cot_attr = c.up(groups->cot_attr_val, n);
+      gc.minimum = c.up(groups->minimum, G);
+      if (sh.dev.cot) {   // derived by the caller on the device
+        const size_t n = std::max<int64_t>(1, sh.dev.n_cot);
+        gc.cot_off = c.take<int32_t>(G + 1); gc.cot_host = c.take<int32_t>(n); gc.cot_attr = c.take<int32_t>(n);
+      } else {
+        gc.cot_off = c.up(groups->cot_off, G + 1);
+        const int n = std::max(1, groups->cot_off[G]);
+        gc.cot_host = c.up(groups->cot_hostname_id, n); gc.cot_attr = c.up(groups->cot_attr_val, n);
+      }
     }
 
     q.d_ord = c.take<int32_t>(CAP); q.d_ord2 = c.take<int32_t>(CAP);
@@ -1324,6 +1330,12 @@ int32_t rebalance_build(cook_pool* pool, const RebShape& sh, const cook_host_tab
   jb.group_off = pc.group_off; jb.group_idx = pc.group_idx;
   rows->jid = pc.jid; rows->prio = pc.prio;
   rows->hostname_id = q.hc.hostname_id;
+  rows->attr = q.hc.attr;
+  rows->gcol = q.gc.attr_col;
+  const bool cot = sh.dev.cot && q.gc.cot_off;
+  rows->cot_off = cot ? writable(q.gc.cot_off) : nullptr;
+  rows->cot_host = cot ? writable(q.gc.cot_host) : nullptr;
+  rows->cot_attr = cot ? writable(q.gc.cot_attr) : nullptr;
   return COOK_OK;
 }
 

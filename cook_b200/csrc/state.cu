@@ -525,6 +525,7 @@ struct PoolState {
   std::unordered_set<int32_t> reserved;   // the live pending slots whose reserved_host is not -1
   Arena stage;                        // one batch's uploads
   Arena scratch;                      // one call's device buffers
+  Arena derive;                       // a derived match's or rebalance's running-side scratch (scratch is live then)
   Arena queue;                        // the ranked queue, carved by rank only: it lives until the match
   int32_t* counters = nullptr;        // [0] running rows, [1] pending rows, [2] live queue entries
   GridFlag* gf0 = nullptr;            // stays zero: integer scans are always exact
@@ -542,7 +543,7 @@ struct PoolState {
   void release() {
     pend.release(); run.release();
     for (auto& l : lists) l.release();
-    stage.release(); scratch.release(); queue.release();
+    stage.release(); scratch.release(); derive.release(); queue.release();
     if (counters) cudaFree(counters);
     if (gf0) cudaFree(gf0);
   }
@@ -614,6 +615,18 @@ bool csr_ok(const int32_t* off, int n, const int32_t* v0, const int32_t* v1, boo
 }
 
 long long bits_of(double x) { long long b; memcpy(&b, &x, 8); return b; }
+
+// hostname codes that are non-negative and distinct; *n_codes: one past the largest
+bool host_codes(const int32_t* code, int H, int32_t* n_codes) {
+  std::unordered_set<int32_t> seen;
+  seen.reserve((size_t)H);
+  *n_codes = 0;
+  for (int h = 0; h < H; h++) {
+    if (code[h] < 0 || !seen.insert(code[h]).second) return false;
+    *n_codes = std::max(*n_codes, code[h] + 1);
+  }
+  return true;
+}
 
 // the CSR lists of rows m_slot[0, n) into the dense lists of `o` that are carved (non-null)
 void gather_lists(const PoolState* S, const JobDev& o, const int32_t* m_slot, int n, const OrderScan<int, 1>& os,
@@ -1038,48 +1051,35 @@ int32_t patch(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, const
   return COOK_OK;
 }
 
-// the running usage per user, of the pool and per listed host, each a left fold in ascending task id
-int32_t usage(cook_pool* pool, PoolState* S, int U, double* out_user, double* out_pool, int H, const int32_t* hostname_id,
-              double* out_run_cpus, double* out_run_mem, int32_t* out_run_count) {
-  // ---- every check before any device work: the rows' codes from the host-side counts, the list itself
-  if (out_user && count_max(S->users_r) >= U)
-    return set_err(pool, COOK_E_BADARG, "cook_state_usage: a live running row's user code is >= n_users");
-  if (H < 0) return set_err(pool, COOK_E_BADARG, "cook_state_usage: n_hosts < 0");
-  if (H > 0 && !hostname_id) return set_err(pool, COOK_E_BADARG, "cook_state_usage: null hostname_id");
-  int32_t n_codes = 0;
-  {
-    std::unordered_set<int32_t> codes;
-    codes.reserve((size_t)H);
-    for (int h = 0; h < H; h++) {
-      const int32_t c = hostname_id[h];
-      if (c < 0 || !codes.insert(c).second)
-        return set_err(pool, COOK_E_BADARG, "cook_state_usage: a hostname_id is negative or twice in the list");
-      n_codes = std::max(n_codes, c + 1);
-    }
-  }
-  const int R = (int)S->run.slot_of.size();
-  const bool users = out_user && U > 0, hosts = H > 0 && (out_run_cpus || out_run_mem || out_run_count);
-  if (R == 0) {   // nothing live: every sum is the empty fold
-    if (users) memset(out_user, 0, sizeof(double) * 4 * (size_t)U);
-    if (out_pool) memset(out_pool, 0, sizeof(double) * 4);
-    if (out_run_cpus) memset(out_run_cpus, 0, sizeof(double) * (size_t)H);
-    if (out_run_mem) memset(out_run_mem, 0, sizeof(double) * (size_t)H);
-    if (out_run_count) memset(out_run_count, 0, sizeof(int32_t) * (size_t)H);
-    pool->phase[COOK_PHASE_USAGE] = cook_phase_stats{};
-    return COOK_OK;
-  }
-  CK(pool, cudaSetDevice(pool->device));
-  cudaStream_t st = pool->stream;
+// ---- the two running-side pipelines.  Each lists its scratch on a carve (take), writes into device
+// destinations its caller sets (a standalone call's download buffers, or the columns a match or rebalance
+// plan carved) and launches its kernels on the stream (run).  cook_state_usage and cook_state_cotasks are
+// these plus their uploads and downloads; a derived match or rebalance runs the same kernels into its plan.
+
+// hostname code -> index h of the code in d_codes[0, H), -1 for a code not listed (n_codes: one past the largest)
+cudaError_t map_hosts(int32_t* host_of, int32_t n_codes, const int32_t* d_codes, int H, cudaStream_t st, int* nl) {
+  const cudaError_t e = cudaMemsetAsync(host_of, 0xff, sizeof(int32_t) * (size_t)n_codes, st);
+  if (e != cudaSuccess) return e;
+  host_map_kernel<<<(H + 255) / 256, 256, 0, st>>>(d_codes, H, host_of);
+  (*nl)++;
+  return cudaGetLastError();
+}
+
+// The running usage of R live rows, each sum a left fold in ascending task id: per user (U > 0), per listed host
+// (H > 0) and of the pool.  The caller sets rows.host_of / rows.n_codes (H > 0) and the destinations
+// a.user_out [4][U], a.host_cpus / host_mem / host_count [H] and a.pool_out [4] of the sums it asked for.
+struct UsageFold {
+  int R = 0, U = 0, H = 0;
+  bool pool = false;
   UsageRows rows = {};
-  rows.col = S->run.d_col; rows.n_codes = n_codes; rows.H = H;
   UsageArgs a = {};
-  int32_t *blk = nullptr, *tmp = nullptr, *d_codes = nullptr, *host_of = nullptr;
+  int32_t *blk = nullptr, *tmp = nullptr;
   GridFlag* gf = nullptr;
-  int64_t h2d = 0, d2h = 0;
-  CK(pool, carve(S->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+
+  void take(Carve& c, int hw) {
     rows.user = c.take<int32_t>(R); rows.tid = c.take<int64_t>(R);
     for (int k = 0; k < 3; k++) rows.amt[k] = c.take<double>(R);
-    blk = c.take<int32_t>((size_t)S->run.hw / CP_BLOCK + 2);
+    blk = c.take<int32_t>((size_t)hw / CP_BLOCK + 2);
     tmp = c.take<int32_t>(R);
     gf = c.take<GridFlag>(1);
     const auto segs = [&](UsageSegs& q, int n_seg, bool bounds) {
@@ -1093,55 +1093,135 @@ int32_t usage(cook_pool* pool, PoolState* S, int U, double* out_user, double* ou
         q.os.tile[k] = c.take<double>(R / OS_TILE + 2);
       }
     };
-    if (users) { segs(a.seg[US_USER], U, true); a.user_out = c.take<double>(4 * (size_t)U); }
-    if (hosts) {
+    if (U > 0) segs(a.seg[US_USER], U, true);
+    if (H > 0) {
       rows.host = c.take<int32_t>(R);
-      host_of = c.take<int32_t>(n_codes);
       segs(a.seg[US_HOST], H, true);
+    }
+    if (pool) segs(a.seg[US_POOL], 1, false);
+  }
+
+  // the live rows, the grid check, the orders with their segments and (on the grid) order-wide scans, the folds
+  cudaError_t run(const PoolState* S, cudaStream_t st, int* nl) {
+    rows.col = S->run.d_col; rows.H = H;
+    cudaError_t e = cudaMemsetAsync(gf, 0, sizeof(GridFlag), st);
+    if (e != cudaSuccess) return e;
+    compact(rows, S->run.hw, nullptr, blk, S->counters, R, st, nl);
+    grid_check_kernel<<<(R + 255) / 256, 256, 0, st>>>(rows.amt[0], rows.amt[1], rows.amt[2], R, gf);
+    (*nl)++;
+    const int32_t* key[US_N] = {rows.user, rows.host, nullptr};
+    for (int k = 0; k < US_N; k++) {
+      UsageSegs& q = a.seg[k];
+      if (!q.n) continue;
+      if ((e = csort::sort_indices(writable(q.ord), tmp, R, LessKeyTid{key[k], rows.tid}, st, nl)) != cudaSuccess) return e;
+      if (!q.start) continue;
+      // +1: the hosts' segment H holds the rows no listed host carries
+      if ((e = cudaMemsetAsync(writable(q.start), 0, sizeof(int32_t) * (q.n + 1), st)) != cudaSuccess) return e;
+      if ((e = cudaMemsetAsync(writable(q.end), 0, sizeof(int32_t) * (q.n + 1), st)) != cudaSuccess) return e;
+      seg_bounds_kernel<<<(R + 255) / 256, 256, 0, st>>>(SortedKey{q.ord, nullptr, key[k]}, R, writable(q.start),
+                                                         writable(q.end), nullptr);
+      (*nl)++;
+      order_scan(q.os, LoadSorted{q.ord, {rows.amt[0], rows.amt[1], rows.amt[2]}}, R, gf, st, nl);
+    }
+    // the pool's total from an order-wide scan when there is one (the sum is the same over any order there)
+    if (a.seg[US_POOL].n) {
+      for (int k : {US_USER, US_HOST})
+        if (a.seg[k].scan && !a.seg[US_POOL].scan) { a.seg[US_POOL].os = a.seg[k].os; a.seg[US_POOL].scan = 1; }
+    }
+    for (int k = 0; k < 3; k++) a.amt[k] = rows.amt[k];
+    a.gf = gf; a.R = R; a.U = U;
+    const int nseg = a.seg[US_USER].n + a.seg[US_HOST].n + a.seg[US_POOL].n;
+    usage_fold_kernel<<<(nseg + 3) / 4, 128, 0, st>>>(a);
+    (*nl)++;
+    return cudaGetLastError();
+  }
+};
+
+// Each group's running cotasks: the K live running rows with a known host and a group list, expanded into their N
+// entries and ordered by (group, task id).  The caller sets a.host_of / a.n_codes (null: no host listed), a.gcol
+// [G] (a group's column of a.attr, or -1), a.attr [columns][a.H] and the destinations off [G + 1], o_host and
+// o_attr [N].
+struct CotaskList {
+  int K = 0, N = 0, G = 0;
+  CotaskArgs a = {};
+  int32_t *blk = nullptr, *ord = nullptr, *tmp = nullptr;
+  int32_t *off = nullptr, *o_host = nullptr, *o_attr = nullptr;
+
+  void take(Carve& c, int hw) {
+    a.slot = c.take<int32_t>(K);
+    blk = c.take<int32_t>((size_t)hw / CP_BLOCK + 2);
+    a.os.part[0] = c.take<int32_t>(K);
+    a.os.tile[0] = c.take<int32_t>((K + OS_TILE - 1) / OS_TILE + 1);
+    a.e_grp = c.take<int32_t>(N); a.e_tid = c.take<int64_t>(N); a.e_host = c.take<int32_t>(N);
+    a.e_attr = c.take<int32_t>(N);
+    ord = c.take<int32_t>(N); tmp = c.take<int32_t>(N);
+  }
+
+  // the rows, their entries, the (group, task id) order, the outputs
+  cudaError_t run(const PoolState* S, cudaStream_t st, int* nl) {
+    a.K = K;
+    a.goff = S->run.at<int32_t>(R_GOFF); a.glen = S->run.at<int32_t>(R_GLEN); a.arena = S->lists[L_RGROUP].v[0];
+    a.host = S->run.at<int32_t>(R_HOST); a.tid = S->run.at<int64_t>(R_TID);
+    compact(CotaskRows{S->run.at<uint8_t>(R_LIVE), a.host, a.glen, writable(a.slot)}, S->run.hw, nullptr, blk,
+            S->counters + 3, K, st, nl);
+    order_scan(a.os, RowLen{a.slot, a.glen}, K, S->gf0, st, nl);
+    cotask_expand_kernel<<<(K + 255) / 256, 256, 0, st>>>(a);
+    (*nl)++;
+    const cudaError_t e = csort::sort_indices(ord, tmp, N, LessKeyTid{a.e_grp, a.e_tid}, st, nl);
+    if (e != cudaSuccess) return e;
+    const int np = std::max(N, G + 1);
+    cotask_out_kernel<<<(np + 255) / 256, 256, 0, st>>>(ord, a.e_grp, a.e_host, a.e_attr, N, G, off, o_host, o_attr);
+    (*nl)++;
+    return cudaGetLastError();
+  }
+};
+
+// the running usage per user, of the pool and per listed host, each a left fold in ascending task id
+int32_t usage(cook_pool* pool, PoolState* S, int U, double* out_user, double* out_pool, int H, const int32_t* hostname_id,
+              double* out_run_cpus, double* out_run_mem, int32_t* out_run_count) {
+  // ---- every check before any device work: the rows' codes from the host-side counts, the list itself
+  if (out_user && count_max(S->users_r) >= U)
+    return set_err(pool, COOK_E_BADARG, "cook_state_usage: a live running row's user code is >= n_users");
+  if (H < 0) return set_err(pool, COOK_E_BADARG, "cook_state_usage: n_hosts < 0");
+  if (H > 0 && !hostname_id) return set_err(pool, COOK_E_BADARG, "cook_state_usage: null hostname_id");
+  int32_t n_codes = 0;
+  if (!host_codes(hostname_id, H, &n_codes))
+    return set_err(pool, COOK_E_BADARG, "cook_state_usage: a hostname_id is negative or twice in the list");
+  const int R = (int)S->run.slot_of.size();
+  const bool users = out_user && U > 0, hosts = H > 0 && (out_run_cpus || out_run_mem || out_run_count);
+  if (R == 0) {   // nothing live: every sum is the empty fold
+    if (users) memset(out_user, 0, sizeof(double) * 4 * (size_t)U);
+    if (out_pool) memset(out_pool, 0, sizeof(double) * 4);
+    if (out_run_cpus) memset(out_run_cpus, 0, sizeof(double) * (size_t)H);
+    if (out_run_mem) memset(out_run_mem, 0, sizeof(double) * (size_t)H);
+    if (out_run_count) memset(out_run_count, 0, sizeof(int32_t) * (size_t)H);
+    pool->phase[COOK_PHASE_USAGE] = cook_phase_stats{};
+    return COOK_OK;
+  }
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  UsageFold f;
+  f.R = R; f.U = users ? U : 0; f.H = hosts ? H : 0; f.pool = out_pool != nullptr;
+  UsageArgs& a = f.a;
+  int32_t *d_codes = nullptr, *host_of = nullptr;
+  int64_t h2d = 0, d2h = 0;
+  CK(pool, carve(S->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+    f.take(c, S->run.hw);
+    if (users) a.user_out = c.take<double>(4 * (size_t)U);
+    if (hosts) {
+      host_of = c.take<int32_t>(n_codes);
       a.host_cpus = c.take<double>(H); a.host_mem = c.take<double>(H); a.host_count = c.take<int32_t>(H);
     }
-    if (out_pool) { segs(a.seg[US_POOL], 1, false); a.pool_out = c.take<double>(4); }
+    if (out_pool) a.pool_out = c.take<double>(4);
     if (H > 0) d_codes = c.up(hostname_id, H);
   }));
   CK(pool, cudaEventRecord(pool->ev[21], st));
-  // ---- the code -> index map, the live rows, the grid check
   int nl = 0;
-  CK(pool, cudaMemsetAsync(gf, 0, sizeof(GridFlag), st));
   if (hosts) {
-    CK(pool, cudaMemsetAsync(host_of, 0xff, sizeof(int32_t) * (size_t)n_codes, st));
-    host_map_kernel<<<(H + 255) / 256, 256, 0, st>>>(d_codes, H, host_of);
-    nl++;
-    rows.host_of = host_of;
+    CK(pool, map_hosts(host_of, n_codes, d_codes, H, st, &nl));
+    f.rows.host_of = host_of; f.rows.n_codes = n_codes;
   }
-  compact(rows, S->run.hw, nullptr, blk, S->counters, R, st, &nl);
-  grid_check_kernel<<<(R + 255) / 256, 256, 0, st>>>(rows.amt[0], rows.amt[1], rows.amt[2], R, gf);
-  nl++;
-  // ---- the orders, their segments and (on the grid) their order-wide scans
-  const int32_t* key[US_N] = {rows.user, rows.host, nullptr};
-  for (int k = 0; k < US_N; k++) {
-    UsageSegs& q = a.seg[k];
-    if (!q.n) continue;
-    CK(pool, csort::sort_indices(writable(q.ord), tmp, R, LessKeyTid{key[k], rows.tid}, st, &nl));
-    if (!q.start) continue;
-    // +1: the hosts' segment H holds the rows no listed host carries
-    CK(pool, cudaMemsetAsync(writable(q.start), 0, sizeof(int32_t) * (q.n + 1), st));
-    CK(pool, cudaMemsetAsync(writable(q.end), 0, sizeof(int32_t) * (q.n + 1), st));
-    seg_bounds_kernel<<<(R + 255) / 256, 256, 0, st>>>(SortedKey{q.ord, nullptr, key[k]}, R, writable(q.start),
-                                                       writable(q.end), nullptr);
-    nl++;
-    order_scan(q.os, LoadSorted{q.ord, {rows.amt[0], rows.amt[1], rows.amt[2]}}, R, gf, st, &nl);
-  }
-  // the pool's total from an order-wide scan when there is one (the sum is the same over any order there)
-  if (a.seg[US_POOL].n) {
-    for (int k : {US_USER, US_HOST})
-      if (a.seg[k].scan && !a.seg[US_POOL].scan) { a.seg[US_POOL].os = a.seg[k].os; a.seg[US_POOL].scan = 1; }
-  }
-  for (int k = 0; k < 3; k++) a.amt[k] = rows.amt[k];
-  a.gf = gf; a.R = R; a.U = U;
-  const int nseg = a.seg[US_USER].n + a.seg[US_HOST].n + a.seg[US_POOL].n;
-  usage_fold_kernel<<<(nseg + 3) / 4, 128, 0, st>>>(a);
-  nl++;
-  CK(pool, cudaGetLastError());
+  CK(pool, f.run(S, st, &nl));
   CK(pool, cudaEventRecord(pool->ev[22], st));
   if (users) CK(pool, download(out_user, a.user_out, 4 * (size_t)U, st, &d2h));
   if (out_pool) CK(pool, download(out_pool, a.pool_out, 4, st, &d2h));
@@ -1170,16 +1250,8 @@ int32_t cotasks(cook_pool* pool, PoolState* S, int G, const int32_t* attr_col, c
   if (H < 0) return set_err(pool, COOK_E_BADARG, "cook_state_cotasks: hosts->n < 0");
   if (H > 0 && !hosts->hostname_id) return set_err(pool, COOK_E_BADARG, "cook_state_cotasks: null hosts->hostname_id");
   int32_t n_codes = 0;
-  {
-    std::unordered_set<int32_t> codes;
-    codes.reserve((size_t)H);
-    for (int h = 0; h < H; h++) {
-      const int32_t c = hosts->hostname_id[h];
-      if (c < 0 || !codes.insert(c).second)
-        return set_err(pool, COOK_E_BADARG, "cook_state_cotasks: a hostname_id is negative or twice in `hosts`");
-      n_codes = std::max(n_codes, c + 1);
-    }
-  }
+  if (!host_codes(H > 0 ? hosts->hostname_id : nullptr, H, &n_codes))
+    return set_err(pool, COOK_E_BADARG, "cook_state_cotasks: a hostname_id is negative or twice in `hosts`");
   // the distinct attribute columns the groups name, in first-named order; gcol[g]: the group's among them
   std::vector<int32_t> gcol(G, -1), cols;
   if (hosts && attr_col) {
@@ -1205,24 +1277,16 @@ int32_t cotasks(cook_pool* pool, PoolState* S, int G, const int32_t* attr_col, c
   }
   CK(pool, cudaSetDevice(pool->device));
   cudaStream_t st = pool->stream;
-  const int K = (int)S->cot_rows, D = (int)cols.size();
-  CotaskArgs a = {};
-  a.K = K; a.H = H; a.n_codes = n_codes;
-  a.goff = S->run.at<int32_t>(R_GOFF); a.glen = S->run.at<int32_t>(R_GLEN); a.arena = S->lists[L_RGROUP].v[0];
-  a.host = S->run.at<int32_t>(R_HOST); a.tid = S->run.at<int64_t>(R_TID);
-  int32_t *blk = nullptr, *ord = nullptr, *tmp = nullptr, *d_off = nullptr, *d_host = nullptr, *d_attr = nullptr;
-  int32_t *slot = nullptr, *host_of = nullptr, *attr = nullptr;
+  const int D = (int)cols.size();
+  CotaskList l;
+  l.K = (int)S->cot_rows; l.N = (int)N; l.G = G;
+  l.a.H = H; l.a.n_codes = n_codes;
+  int32_t *host_of = nullptr, *attr = nullptr;
   const int32_t* d_codes = nullptr;
   int64_t h2d = 0, d2h = 0;
   CK(pool, carve(S->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
-    slot = c.take<int32_t>(K);
-    blk = c.take<int32_t>((size_t)S->run.hw / CP_BLOCK + 2);
-    a.os.part[0] = c.take<int32_t>(K);
-    a.os.tile[0] = c.take<int32_t>((K + OS_TILE - 1) / OS_TILE + 1);
-    a.e_grp = c.take<int32_t>(N); a.e_tid = c.take<int64_t>(N); a.e_host = c.take<int32_t>(N);
-    a.e_attr = c.take<int32_t>(N);
-    ord = c.take<int32_t>(N); tmp = c.take<int32_t>(N);
-    d_off = c.take<int32_t>((size_t)G + 1); d_host = c.take<int32_t>(N); d_attr = c.take<int32_t>(N);
+    l.take(c, S->run.hw);
+    l.off = c.take<int32_t>((size_t)G + 1); l.o_host = c.take<int32_t>(N); l.o_attr = c.take<int32_t>(N);
     if (H > 0) {
       d_codes = c.up(hosts->hostname_id, H);
       host_of = c.take<int32_t>(n_codes);
@@ -1232,34 +1296,107 @@ int32_t cotasks(cook_pool* pool, PoolState* S, int G, const int32_t* attr_col, c
       if (attr)
         for (int j = 0; j < D; j++) c.copy(attr + (size_t)j * H, hosts->attr + (size_t)cols[j] * H, H);
     }
-    a.gcol = c.up(gcol.data(), G);
+    l.a.gcol = c.up(gcol.data(), G);
   }));
   CK(pool, cudaEventRecord(pool->ev[21], st));
-  a.slot = slot; a.host_of = host_of; a.attr = attr;
-  // ---- the code -> index map, the rows, their entries, the (group, task id) order, the outputs
+  l.a.host_of = host_of; l.a.attr = attr;
   int nl = 0;
-  if (H > 0) {
-    CK(pool, cudaMemsetAsync(host_of, 0xff, sizeof(int32_t) * (size_t)n_codes, st));
-    host_map_kernel<<<(H + 255) / 256, 256, 0, st>>>(d_codes, H, host_of);
-    nl++;
-  }
-  compact(CotaskRows{S->run.at<uint8_t>(R_LIVE), a.host, a.glen, slot}, S->run.hw, nullptr, blk, S->counters + 3, K,
-          st, &nl);
-  order_scan(a.os, RowLen{slot, a.glen}, K, S->gf0, st, &nl);
-  cotask_expand_kernel<<<(K + 255) / 256, 256, 0, st>>>(a);
-  nl++;
-  CK(pool, csort::sort_indices(ord, tmp, (int)N, LessKeyTid{a.e_grp, a.e_tid}, st, &nl));
-  const int np = std::max((int)N, G + 1);
-  cotask_out_kernel<<<(np + 255) / 256, 256, 0, st>>>(ord, a.e_grp, a.e_host, a.e_attr, (int)N, G, d_off, d_host, d_attr);
-  nl++;
-  CK(pool, cudaGetLastError());
+  if (H > 0) CK(pool, map_hosts(host_of, n_codes, d_codes, H, st, &nl));
+  CK(pool, l.run(S, st, &nl));
   CK(pool, cudaEventRecord(pool->ev[22], st));
-  CK(pool, download(out_off, d_off, (size_t)G + 1, st, &d2h));
-  CK(pool, download(out_host, d_host, (size_t)N, st, &d2h));
-  CK(pool, download(out_attr, d_attr, (size_t)N, st, &d2h));
+  CK(pool, download(out_off, l.off, (size_t)G + 1, st, &d2h));
+  CK(pool, download(out_host, l.o_host, (size_t)N, st, &d2h));
+  CK(pool, download(out_attr, l.o_attr, (size_t)N, st, &d2h));
   CK(pool, cudaEventRecord(pool->ev[23], st));
   CK(pool, cudaStreamSynchronize(st));
   record_phase(pool, COOK_PHASE_COTASKS, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[23], h2d, d2h, nl);
+  return COOK_OK;
+}
+
+// ---- a derived match or rebalance: the running-side columns its plan carved, filled on the device.  The scratch
+// comes from the state's `derive` arena: `scratch` still holds the queue rows and maps the call carved before
+// its build.
+
+// A group's column of the plan's attribute matrix: the plan's copy of groups->attr_col, or (none given) a column
+// of -1 in `derive_gcol`, which the caller carved.
+cudaError_t group_cols(const int32_t* plan_gcol, int32_t* derive_gcol, int G, cudaStream_t st, const int32_t** gcol) {
+  *gcol = plan_gcol;
+  if (plan_gcol) return cudaSuccess;
+  *gcol = derive_gcol;
+  return cudaMemsetAsync(derive_gcol, 0xff, sizeof(int32_t) * (size_t)G, st);
+}
+
+// The users' usage [4][U], the offers' run_* [O] at their input index (n_codes: one past the largest offer
+// hostname code) and, when the plan reads the lists (rows.cot_off), the groups' cot_* lists.  No live running
+// row: zeros, without a kernel.
+int32_t derive_match(cook_pool* pool, PoolState* S, const MatchRows& rows, int U, int O, int32_t n_codes, int G,
+                     const int32_t* attr_col, int* nl) {
+  cudaStream_t st = pool->stream;
+  const int R = (int)S->run.slot_of.size();
+  const bool lists = rows.cot_off != nullptr, entries = lists && S->cot_n > 0;
+  if (R == 0 || !entries) {
+    if (lists) CK(pool, cudaMemsetAsync(rows.cot_off, 0, sizeof(int32_t) * ((size_t)G + 1), st));
+  }
+  if (R == 0) {
+    CK(pool, cudaMemsetAsync(rows.usage, 0, sizeof(double) * 4 * (size_t)U, st));
+    if (O > 0) {
+      CK(pool, cudaMemsetAsync(rows.run_cpus, 0, sizeof(double) * (size_t)O, st));
+      CK(pool, cudaMemsetAsync(rows.run_mem, 0, sizeof(double) * (size_t)O, st));
+      CK(pool, cudaMemsetAsync(rows.run_count, 0, sizeof(int32_t) * (size_t)O, st));
+    }
+    return COOK_OK;
+  }
+  UsageFold f;
+  f.R = R; f.U = U; f.H = O;
+  CotaskList l;
+  l.K = (int)S->cot_rows; l.N = (int)S->cot_n; l.G = G;
+  int32_t *host_of = nullptr, *gcol = nullptr;
+  CK(pool, carve(S->derive, st, nullptr, nullptr, [&](Carve& c) {
+    f.take(c, S->run.hw);
+    if (O > 0) host_of = c.take<int32_t>(n_codes);
+    if (entries) {
+      l.take(c, S->run.hw);
+      if (!attr_col) gcol = c.take<int32_t>(G);
+    }
+  }));
+  if (O > 0) {
+    CK(pool, map_hosts(host_of, n_codes, rows.hostname_id, O, st, nl));
+    f.rows.host_of = host_of; f.rows.n_codes = n_codes;
+  }
+  f.a.user_out = rows.usage;
+  f.a.host_cpus = rows.run_cpus; f.a.host_mem = rows.run_mem; f.a.host_count = rows.run_count;
+  CK(pool, f.run(S, st, nl));
+  if (!entries) return COOK_OK;
+  l.a.host_of = O > 0 ? host_of : nullptr; l.a.n_codes = n_codes;
+  l.a.attr = rows.attr; l.a.H = O;
+  CK(pool, group_cols(rows.gcol, gcol, G, st, &l.a.gcol));
+  l.off = rows.cot_off; l.o_host = rows.cot_host; l.o_attr = rows.cot_attr;
+  CK(pool, l.run(S, st, nl));
+  return COOK_OK;
+}
+
+// The groups' cot_* lists of a rebalance (rows.cot_off: the plan reads them) over its host table, through the
+// host_of map the rebalance built from it (n_codes: one past the largest code of the table).
+int32_t derive_rebalance(cook_pool* pool, PoolState* S, const RebRows& rows, const int32_t* host_of, int32_t n_codes,
+                         int H, int G, const int32_t* attr_col, int* nl) {
+  cudaStream_t st = pool->stream;
+  if (!rows.cot_off) return COOK_OK;
+  if (S->cot_n == 0) {
+    CK(pool, cudaMemsetAsync(rows.cot_off, 0, sizeof(int32_t) * ((size_t)G + 1), st));
+    return COOK_OK;
+  }
+  CotaskList l;
+  l.K = (int)S->cot_rows; l.N = (int)S->cot_n; l.G = G;
+  int32_t* gcol = nullptr;
+  CK(pool, carve(S->derive, st, nullptr, nullptr, [&](Carve& c) {
+    l.take(c, S->run.hw);
+    if (!attr_col) gcol = c.take<int32_t>(G);
+  }));
+  l.a.host_of = host_of; l.a.n_codes = n_codes;
+  l.a.attr = rows.attr; l.a.H = H;
+  CK(pool, group_cols(rows.gcol, gcol, G, st, &l.a.gcol));
+  l.off = rows.cot_off; l.o_host = rows.cot_host; l.o_attr = rows.cot_attr;
+  CK(pool, l.run(S, st, nl));
   return COOK_OK;
 }
 
@@ -1381,16 +1518,19 @@ extern "C" int32_t cook_state_rank(cook_pool* pool, const cook_user_table* users
   return COOK_OK;
 }
 
-extern "C" int32_t cook_state_match(cook_pool* pool, const cook_offers_soa* offers, const cook_groups* groups,
-                                    const cook_user_table* users, const cook_pool_quota* pool_quota,
-                                    const cook_match_params* params, int64_t* out_considerable_job_id,
-                                    int32_t* out_assign, int32_t* out_ports, int32_t max_ports,
-                                    uint8_t* out_fail_reason, cook_match_stats* out_stats) {
+namespace {
+
+// cook_state_match, and with `derived` cook_state_match_derived: the users' usage, the offers' run_* and the
+// groups' cot_* lists come from the live running rows, filled on the device into the columns the plan carved
+int32_t state_match(cook_pool* pool, const char* who, bool derived, const cook_offers_soa* offers,
+                    const cook_groups* groups, const cook_user_table* users, const cook_pool_quota* pool_quota,
+                    const cook_match_params* params, int64_t* out_considerable_job_id, int32_t* out_assign,
+                    int32_t* out_ports, int32_t max_ports, uint8_t* out_fail_reason, cook_match_stats* out_stats) {
   if (!pool) return COOK_E_BADARG;
   if (!offers || !users || !params || !out_considerable_job_id || !out_assign)
-    return set_err(pool, COOK_E_BADARG, "cook_state_match: null argument");
+    return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
   if (params->reuse_resident)
-    return set_err(pool, COOK_E_BADARG, "cook_state_match: reuse_resident does not apply: the queue's rows are resident");
+    return set_err(pool, COOK_E_BADARG, "%s: reuse_resident does not apply: the queue's rows are resident", who);
   PoolState* S = static_cast<PoolState*>(pool->state);
   const int NC = params->num_considerable;
   cudaStream_t st = pool->stream;
@@ -1417,17 +1557,42 @@ extern "C" int32_t cook_state_match(cook_pool* pool, const cook_offers_soa* offe
     CK(pool, download(&n, S->counters + 2, 1, st, &d2h));
     CK(pool, cudaStreamSynchronize(st));
   }
-  int32_t rc = check_match_inputs(pool, "cook_state_match", offers, groups, users, params, max_ports, n > 0,
-                                  S && S->lists[L_NOVEL].live > 0, S && S->lists[L_GROUP].live > 0);
+  int32_t rc = check_match_inputs(pool, who, offers, groups, users, params, max_ports, n > 0,
+                                  S && S->lists[L_NOVEL].live > 0, S && S->lists[L_GROUP].live > 0, derived);
   if (rc != COOK_OK) return rc;
-  if (!S || !S->ranked) return set_err(pool, COOK_E_BADARG, "cook_state_match: no cook_state_rank on this handle yet");
+  if (!S || !S->ranked) return set_err(pool, COOK_E_BADARG, "%s: no cook_state_rank on this handle yet", who);
   const int U = users->n_users;
-  if (count_max(S->users_p) >= U) return set_err(pool, COOK_E_BADARG, "cook_state_match: a pending row's user code is >= n_users");
+  if (count_max(S->users_p) >= U) return set_err(pool, COOK_E_BADARG, "%s: a pending row's user code is >= n_users", who);
   if (count_max(S->attr_cols) >= std::max(1, offers->n_attr_cols))
-    return set_err(pool, COOK_E_BADARG, "cook_state_match: a pending row's attribute column is >= n_attr_cols");
+    return set_err(pool, COOK_E_BADARG, "%s: a pending row's attribute column is >= n_attr_cols", who);
   const int G = groups ? groups->n_groups : 0;
   if (G > 0 && count_max(S->groups) >= G)
-    return set_err(pool, COOK_E_BADARG, "cook_state_match: a pending row's group code is >= n_groups");
+    return set_err(pool, COOK_E_BADARG, "%s: a pending row's group code is >= n_groups", who);
+  // ---- what the derivation reads, checked from the host-side counts and the offer and group tables
+  const int O = offers->n;
+  int32_t n_codes = 0;
+  if (derived) {
+    if (count_max(S->users_r) >= U)
+      return set_err(pool, COOK_E_BADARG, "%s: a live running row's user code is >= n_users", who);
+    if (n > 0) {
+      if (O > 0 && !offers->hostname_id) return set_err(pool, COOK_E_BADARG, "%s: null offers->hostname_id", who);
+      if (!host_codes(offers->hostname_id, O, &n_codes))
+        return set_err(pool, COOK_E_BADARG, "%s: an offers->hostname_id is negative or twice in the table", who);
+      if (G > 0) {
+        if (count_max(S->groups_r) >= G)
+          return set_err(pool, COOK_E_BADARG, "%s: a live running row's group code is >= n_groups", who);
+        bool named = false;
+        for (int g = 0; groups->attr_col && g < G; g++) {
+          const int32_t c = groups->attr_col[g];
+          if (c < -1 || c >= offers->n_attr_cols)
+            return set_err(pool, COOK_E_BADARG, "%s: groups->attr_col outside [-1, offers->n_attr_cols)", who);
+          named = named || c >= 0;
+        }
+        if (named && O > 0 && !offers->attr) return set_err(pool, COOK_E_BADARG, "%s: null offers->attr", who);
+        if (S->cot_n > INT32_MAX) return set_err(pool, COOK_E_TOO_LARGE, "%s: more than 2^31 - 1 cotask entries", who);
+      }
+    }
+  }
   if (out_stats) memset(out_stats, 0, sizeof(*out_stats));
   if (n == 0) return COOK_OK;
   // ---- what the rows hold, from the host-side counts: the resident columns of the kinds some live row
@@ -1457,7 +1622,9 @@ extern "C" int32_t cook_state_match(cook_pool* pool, const cook_offers_soa* offe
   for (const auto& kv : S->groups) if (kv.first < G) sh.gp_off[kv.first + 1] = (int32_t)kv.second;
   for (int g = 0; g < G; g++) sh.gp_off[g + 1] += sh.gp_off[g];
   sh.any_gpus_ports = has(F_GPUS) || has(F_PORTS);
-  // ---- the plan, the gathers into the job columns it carved, the run
+  sh.dev.usage = sh.dev.run = sh.dev.cot = derived;
+  sh.dev.n_cot = S->cot_n;
+  // ---- the plan, the gathers into the job columns it carved, the derived columns, the run
   CK(pool, cudaEventRecord(pool->ev[0], st));
   MatchRows rows;
   rc = match_build(pool, nullptr, n, sh, offers, groups, users, pool_quota, params, max_ports, &rows);
@@ -1466,6 +1633,10 @@ extern "C" int32_t cook_state_match(cook_pool* pool, const cook_offers_soa* offe
   nl++;
   gather_lists(S, rows.jb, m_slot, n, os, st, &nl);
   CK(pool, cudaGetLastError());
+  if (derived) {
+    rc = derive_match(pool, S, rows, U, O, n_codes, G, groups ? groups->attr_col : nullptr, &nl);
+    if (rc != COOK_OK) return rc;
+  }
   rc = match_run(pool, nullptr, out_considerable_job_id, out_assign, out_ports, out_fail_reason, out_stats, true,
                  params->max_ctas);
   if (rc != COOK_OK) return rc;
@@ -1476,47 +1647,62 @@ extern "C" int32_t cook_state_match(cook_pool* pool, const cook_offers_soa* offe
   return COOK_OK;
 }
 
-extern "C" int32_t cook_state_rebalance(cook_pool* pool, const cook_host_table* hosts, const cook_groups* groups,
-                                        const cook_user_table* users, const cook_rebalance_params* params,
-                                        cook_decision* out_decisions, int64_t* out_decision_job_id,
-                                        int64_t* out_victim_task_id, int32_t victim_cap, int32_t* out_n) {
+// cook_state_rebalance, and with `derived` cook_state_rebalance_derived: the groups' cot_* lists come from the live
+// running rows over `hosts`, filled on the device into the lists the build carved
+int32_t state_rebalance(cook_pool* pool, const char* who, bool derived, const cook_host_table* hosts,
+                        const cook_groups* groups, const cook_user_table* users, const cook_rebalance_params* params,
+                        cook_decision* out_decisions, int64_t* out_decision_job_id, int64_t* out_victim_task_id,
+                        int32_t victim_cap, int32_t* out_n) {
   if (!pool) return COOK_E_BADARG;
   if (!hosts || !users || !params || !out_decisions || !out_decision_job_id || !out_victim_task_id || !out_n)
-    return set_err(pool, COOK_E_BADARG, "cook_state_rebalance: null argument");
+    return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
   if (pool->dru_mode != 0)
     return set_err(pool, COOK_E_UNSUPPORTED_CONSTRAINT,
-                   "cook_state_rebalance: GPU DRU mode has no reference behaviour (rebalancer.clj:339-349 throws)");
+                   "%s: GPU DRU mode has no reference behaviour (rebalancer.clj:339-349 throws)", who);
   PoolState* S = static_cast<PoolState*>(pool->state);
-  if (!S || !S->ranked) return set_err(pool, COOK_E_BADARG, "cook_state_rebalance: no cook_state_rank on this handle yet");
+  if (!S || !S->ranked) return set_err(pool, COOK_E_BADARG, "%s: no cook_state_rank on this handle yet", who);
   *out_n = 0;
   const int H = hosts->n, MP = params->max_preemption;
   if (MP <= 0 || H <= 0) return COOK_OK;
   // ---- every check before any device work, from the host-side counts
   const int R = (int)S->run.slot_of.size();
   if ((int64_t)victim_cap < (int64_t)R + MP)
-    return set_err(pool, COOK_E_BADARG, "cook_state_rebalance: victim_cap < live running rows + max_preemption");
-  if (!hosts->hostname_id) return set_err(pool, COOK_E_BADARG, "cook_state_rebalance: null hosts->hostname_id");
+    return set_err(pool, COOK_E_BADARG, "%s: victim_cap < live running rows + max_preemption", who);
+  if (!hosts->hostname_id) return set_err(pool, COOK_E_BADARG, "%s: null hosts->hostname_id", who);
   std::unordered_set<int32_t> codes;
   codes.reserve((size_t)H);
   int32_t max_code = 0;
   for (int h = 0; h < H; h++) {
     const int32_t c = hosts->hostname_id[h];
     if (c < 0 || !codes.insert(c).second)
-      return set_err(pool, COOK_E_BADARG, "cook_state_rebalance: a hostname_id is negative or twice in the host table");
+      return set_err(pool, COOK_E_BADARG, "%s: a hostname_id is negative or twice in the host table", who);
     max_code = std::max(max_code, c);
   }
   for (const auto& kv : S->hosts_r)
     if (!codes.count(kv.first))
-      return set_err(pool, COOK_E_BADARG, "cook_state_rebalance: a running row's host is unknown or not in the host table");
+      return set_err(pool, COOK_E_BADARG, "%s: a running row's host is unknown or not in the host table", who);
   if (std::max(count_max(S->users_p), count_max(S->users_r)) >= users->n_users)
-    return set_err(pool, COOK_E_BADARG, "cook_state_rebalance: a resident row's user code is >= n_users");
+    return set_err(pool, COOK_E_BADARG, "%s: a resident row's user code is >= n_users", who);
   const int G = groups ? groups->n_groups : 0;
   if (groups && count_max(S->groups) >= G)
-    return set_err(pool, COOK_E_BADARG, "cook_state_rebalance: a pending row's group code is >= n_groups");
-  if (G && S->lists[L_GROUP].live && (!groups->cot_off || !groups->kind))
-    return set_err(pool, COOK_E_BADARG, "cook_state_rebalance: incomplete cook_groups");
+    return set_err(pool, COOK_E_BADARG, "%s: a pending row's group code is >= n_groups", who);
+  if (G && S->lists[L_GROUP].live && ((!derived && !groups->cot_off) || !groups->kind))
+    return set_err(pool, COOK_E_BADARG, "%s: incomplete cook_groups", who);
   if (count_max(S->attr_cols) >= std::max(1, hosts->n_attr_cols))
-    return set_err(pool, COOK_E_BADARG, "cook_state_rebalance: a pending row's attribute column is >= n_attr_cols");
+    return set_err(pool, COOK_E_BADARG, "%s: a pending row's attribute column is >= n_attr_cols", who);
+  if (derived && G > 0) {   // what the derivation of the lists reads
+    if (count_max(S->groups_r) >= G)
+      return set_err(pool, COOK_E_BADARG, "%s: a live running row's group code is >= n_groups", who);
+    bool named = false;
+    for (int g = 0; groups->attr_col && g < G; g++) {
+      const int32_t c = groups->attr_col[g];
+      if (c < -1 || c >= hosts->n_attr_cols)
+        return set_err(pool, COOK_E_BADARG, "%s: groups->attr_col outside [-1, hosts->n_attr_cols)", who);
+      named = named || c >= 0;
+    }
+    if (named && !hosts->attr) return set_err(pool, COOK_E_BADARG, "%s: null hosts->attr", who);
+    if (S->cot_n > INT32_MAX) return set_err(pool, COOK_E_TOO_LARGE, "%s: more than 2^31 - 1 cotask entries", who);
+  }
   const int nq = S->n_q;
   if (nq == 0) return COOK_OK;
   // ---- jobs-to-make-room-for: the first allowed jobs of the live queue, their count downloaded
@@ -1547,6 +1733,8 @@ extern "C" int32_t cook_state_rebalance(cook_pool* pool, const cook_host_table* 
   RebShape sh;
   sh.R = R; sh.P = P;
   sh.n_novel = S->lists[L_NOVEL].live; sh.n_attr = S->lists[L_ATTR].live; sh.n_group = S->lists[L_GROUP].live;
+  sh.dev.cot = derived;
+  sh.dev.n_cot = S->cot_n;
   RebPlanPtr plan;
   RebRows rows;
   int32_t rc = rebalance_build(pool, sh, hosts, groups, users, params, &plan, &rows);
@@ -1562,6 +1750,10 @@ extern "C" int32_t cook_state_rebalance(cook_pool* pool, const cook_host_table* 
   nl++;
   gather_lists(S, rows.jb, m_slot, P, os, st, &nl);
   CK(pool, cudaGetLastError());
+  if (derived) {
+    rc = derive_rebalance(pool, S, rows, host_of, max_code + 1, H, G, groups ? groups->attr_col : nullptr, &nl);
+    if (rc != COOK_OK) return rc;
+  }
   CK(pool, cudaEventRecord(pool->ev[23], st));
   rc = rebalance_run(pool, *plan, out_decisions, out_victim_task_id, out_decision_job_id, out_n);
   if (rc != COOK_OK) return rc;
@@ -1570,4 +1762,40 @@ extern "C" int32_t cook_state_rebalance(cook_pool* pool, const cook_host_table* 
   ps.n_launches += nl;
   ps.d2h_bytes += d2h;
   return COOK_OK;
+}
+
+}  // namespace
+
+extern "C" int32_t cook_state_match(cook_pool* pool, const cook_offers_soa* offers, const cook_groups* groups,
+                                    const cook_user_table* users, const cook_pool_quota* pool_quota,
+                                    const cook_match_params* params, int64_t* out_considerable_job_id,
+                                    int32_t* out_assign, int32_t* out_ports, int32_t max_ports,
+                                    uint8_t* out_fail_reason, cook_match_stats* out_stats) {
+  return state_match(pool, "cook_state_match", false, offers, groups, users, pool_quota, params,
+                     out_considerable_job_id, out_assign, out_ports, max_ports, out_fail_reason, out_stats);
+}
+
+extern "C" int32_t cook_state_match_derived(cook_pool* pool, const cook_offers_soa* offers, const cook_groups* groups,
+                                            const cook_user_table* users, const cook_pool_quota* pool_quota,
+                                            const cook_match_params* params, int64_t* out_considerable_job_id,
+                                            int32_t* out_assign, int32_t* out_ports, int32_t max_ports,
+                                            uint8_t* out_fail_reason, cook_match_stats* out_stats) {
+  return state_match(pool, "cook_state_match_derived", true, offers, groups, users, pool_quota, params,
+                     out_considerable_job_id, out_assign, out_ports, max_ports, out_fail_reason, out_stats);
+}
+
+extern "C" int32_t cook_state_rebalance(cook_pool* pool, const cook_host_table* hosts, const cook_groups* groups,
+                                        const cook_user_table* users, const cook_rebalance_params* params,
+                                        cook_decision* out_decisions, int64_t* out_decision_job_id,
+                                        int64_t* out_victim_task_id, int32_t victim_cap, int32_t* out_n) {
+  return state_rebalance(pool, "cook_state_rebalance", false, hosts, groups, users, params, out_decisions,
+                         out_decision_job_id, out_victim_task_id, victim_cap, out_n);
+}
+
+extern "C" int32_t cook_state_rebalance_derived(cook_pool* pool, const cook_host_table* hosts, const cook_groups* groups,
+                                                const cook_user_table* users, const cook_rebalance_params* params,
+                                                cook_decision* out_decisions, int64_t* out_decision_job_id,
+                                                int64_t* out_victim_task_id, int32_t victim_cap, int32_t* out_n) {
+  return state_rebalance(pool, "cook_state_rebalance_derived", true, hosts, groups, users, params, out_decisions,
+                         out_decision_job_id, out_victim_task_id, victim_cap, out_n);
 }

@@ -63,8 +63,10 @@ def load_library(path=None):
                  "cook_comm_destroy", "cook_exchange_usage", "cook_exchange_usage_batch", "cook_rebalance_trace",
                  "cook_match_failures", "cook_state_apply", "cook_state_rank", "cook_state_match",
                  "cook_state_rebalance", "cook_state_launch", "cook_state_patch", "cook_state_usage",
-                 "cook_state_cotasks"):
+                 "cook_state_cotasks", "cook_state_match_derived", "cook_state_rebalance_derived"):
         getattr(lib, name).restype = C.c_int32
+    for name, argtypes in abi.ARGTYPES.items():
+        getattr(lib, name).argtypes = argtypes
     return lib
 
 
@@ -272,14 +274,17 @@ class GpuEngine:
             self._err(rc)
         return out[:n.value].copy()
 
-    def state_match(self, offers, users, params, groups=None, pool_quota=None, max_ports=0):
+    def state_match(self, offers, users, params, groups=None, pool_quota=None, max_ports=0, derived=False):
         """cook_state_match: the resident queue (minus what left it since the rank) matched against
-        `offers`.  'considerable' holds job ids."""
+        `offers`.  'considerable' holds job ids.  derived: cook_state_match_derived, the users' usage_*, the
+        offers' run_* and the groups' cot_* read from the resident running rows on the device (those fields of
+        `users`, `offers` and `groups` are ignored)."""
         pool_quota = pool_quota or abi.make_pool_quota(None)
         k = max(params.num_considerable, 1)
         cons = np.full(k, -1, np.int64)
         _, assign, ports, fail, stats = _CallShapes.match_buffers(params, max_ports)
-        rc = self.lib.cook_state_match(self.pool, C.byref(offers),
+        fn = self.lib.cook_state_match_derived if derived else self.lib.cook_state_match
+        rc = fn(self.pool, C.byref(offers),
                                        C.byref(groups) if groups is not None else None,
                                        C.byref(users), C.byref(pool_quota), C.byref(params),
                                        abi.ptr(cons, abi.P_I64), abi.ptr(assign, abi.P_I32),
@@ -292,19 +297,20 @@ class GpuEngine:
                 "ports": ports[:n * max(max_ports, 1)].reshape(n, max(max_ports, 1)).copy(),
                 "fail": fail[:n].copy(), "stats": stats.as_dict()}
 
-    def state_rebalance(self, hosts, users, params, groups=None):
+    def state_rebalance(self, hosts, users, params, groups=None, derived=False):
         """cook_state_rebalance: the rebalancer over the live running tasks and the first allowed jobs of the
         resident queue.  As rebalance(), plus each decision's 'job_id'; 'victims' are task ids (the task
-        of the job an earlier decision e placed: -1 - e)."""
+        of the job an earlier decision e placed: -1 - e).  derived: cook_state_rebalance_derived, the groups'
+        cot_* read from the resident running rows over `hosts` on the device (those fields are ignored)."""
         mp = max(params.max_preemption, 1)
         dec = (abi.Decision * mp)()
         jid = np.full(mp, -1, np.int64)
         cap = len(getattr(self, "_state_running_ids", ())) + mp
         vict = np.full(cap, -1, np.int64)
         n = C.c_int32(0)
-        rc = self.lib.cook_state_rebalance(self.pool, C.byref(hosts), C.byref(groups) if groups is not None else None,
-                                           C.byref(users), C.byref(params), dec, abi.ptr(jid, abi.P_I64),
-                                           abi.ptr(vict, abi.P_I64), int(cap), C.byref(n))
+        fn = self.lib.cook_state_rebalance_derived if derived else self.lib.cook_state_rebalance
+        rc = fn(self.pool, C.byref(hosts), C.byref(groups) if groups is not None else None, C.byref(users),
+                C.byref(params), dec, abi.ptr(jid, abi.P_I64), abi.ptr(vict, abi.P_I64), int(cap), C.byref(n))
         if rc != 0:
             self._err(rc)
         out = decisions_to_list(dec, vict, n.value)

@@ -596,6 +596,45 @@ int32_t cook_state_cotasks(cook_pool* pool, int32_t n_groups, const int32_t* att
                            int32_t cap, int32_t* out_cot_off, int32_t* out_cot_hostname_id, int32_t* out_cot_attr_val,
                            int32_t* out_n);
 
+/* cook_state_match with its running-side inputs read from the live running rows as they are at the call, on the
+ * device, without a round trip: the resident match cycle in one call.  These fields are not read (may be NULL):
+ *   users->usage_count/_cpus/_mem/_gpus   = what cook_state_usage(n_users, ...) returns now
+ *   offers->run_cpus/_mem/_count          = what cook_state_usage(..., offers->n, offers->hostname_id, ...) returns
+ *   groups->cot_off/_hostname_id/_attr_val (when groups has groups) = what cook_state_cotasks(groups->n_groups,
+ *                                           groups->attr_col, <the offers' n, hostname_id, n_attr_cols, attr>, ...)
+ *                                           returns now
+ * Every other input is read as cook_state_match reads it, and the outputs are bit-identical to cook_state_match fed
+ * by those calls (same kernels, same fold orders), fail reasons and ports included; cook_match_failures and
+ * cook_exchange_usage(_batch) work on the round as after cook_state_match.  Edges: no live running row gives zero
+ * sums and empty lists without a derivation kernel; no live queue row returns as cook_state_match does.
+ * COOK_E_BADARG, before the build, with nothing written and the handle unchanged: every case cook_state_match
+ * rejects except NULL cot_* lists; a live running row's user code >= n_users; and, when a queue row is left to
+ * match, a NULL offers->hostname_id with offers->n > 0, an offers->hostname_id that is negative or appears twice,
+ * and (groups with groups) a live running row's group code >= n_groups, an attr_col outside [-1, n_attr_cols) or
+ * a NULL offers->attr while some group names a column and offers->n > 0.
+ * Transfers exactly: up = the equivalent cook_state_match's upload minus 32 * n_users (usage), minus 20 *
+ * offers->n (run columns), minus 4 * (n_groups + 1) + 8 * max(1, entries) (the lists, when a pending row has a
+ * group list); nothing is added.  Down = cook_state_match's.  The derivation counts into COOK_PHASE_MATCH and
+ * stats->ms_h2d with the queue gathers; COOK_PHASE_USAGE and COOK_PHASE_COTASKS are left as they were.        */
+int32_t cook_state_match_derived(cook_pool* pool, const cook_offers_soa* offers, const cook_groups* groups,
+                                 const cook_user_table* users, const cook_pool_quota* pool_quota,
+                                 const cook_match_params* params, int64_t* out_considerable_job_id,
+                                 int32_t* out_assign, int32_t* out_ports, int32_t max_ports,
+                                 uint8_t* out_fail_reason, cook_match_stats* out_stats);
+
+/* cook_state_rebalance with groups->cot_off/_hostname_id/_attr_val (not read, may be NULL) derived on the device
+ * from the live running rows over `hosts`: what cook_state_cotasks(groups->n_groups, groups->attr_col, hosts, ...)
+ * returns now.  Outputs bit-identical to cook_state_rebalance fed by that call.  COOK_E_BADARG, before any device
+ * work with nothing written: every case cook_state_rebalance rejects except NULL cot_* lists; and (groups with
+ * groups) a live running row's group code >= n_groups, an attr_col outside [-1, hosts->n_attr_cols) or a NULL
+ * hosts->attr while some group names a column.  COOK_E_UNSUPPORTED_CONSTRAINT in GPU DRU mode.  Upload =
+ * cook_state_rebalance's minus 4 * (n_groups + 1) + 8 * max(1, entries) when a pending row has a group list; the
+ * derivation counts into COOK_PHASE_REBALANCE with the gathers.                                                */
+int32_t cook_state_rebalance_derived(cook_pool* pool, const cook_host_table* hosts, const cook_groups* groups,
+                                     const cook_user_table* users, const cook_rebalance_params* params,
+                                     cook_decision* out_decisions, int64_t* out_decision_job_id,
+                                     int64_t* out_victim_task_id, int32_t victim_cap, int32_t* out_n);
+
 /* ------------------------------------------------------------ phase timing */
 /* Device-side timing of the last call of each kind on this handle (CUDA events on the
  * pool's stream): what bench.py's `phases` block and roofline lines are computed from.

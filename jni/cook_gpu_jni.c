@@ -222,10 +222,13 @@ JFN(jint, stateRank)(JNIEnv* env, jclass k, jlong pool, jint n_users, jobjectArr
   (*env)->SetIntArrayRegion(env, out_n, 0, 1, (jint*)&n);
   return rc;
 }
-JFN(jint, stateMatch)(JNIEnv* env, jclass k, jlong pool, jint n_offers, jint n_attr_cols, jobjectArray offers,
-                      jint n_groups, jobjectArray groups, jint n_users, jobjectArray users, jdoubleArray pool_quota,
-                      jintArray iparams /* as match */, jdouble good_enough_fitness, jobject out_considerable_job_id,
-                      jobject out_assign, jobject out_ports, jint max_ports, jobject out_fail, jobject out_stats) {
+typedef int32_t (*state_match_fn)(cook_pool*, const cook_offers_soa*, const cook_groups*, const cook_user_table*,
+                                  const cook_pool_quota*, const cook_match_params*, int64_t*, int32_t*, int32_t*, int32_t,
+                                  uint8_t*, cook_match_stats*);
+static jint state_match(state_match_fn fn, JNIEnv* env, jlong pool, jint n_offers, jint n_attr_cols, jobjectArray offers,
+                        jint n_groups, jobjectArray groups, jint n_users, jobjectArray users, jdoubleArray pool_quota,
+                        jintArray iparams, jdouble good_enough_fitness, jobject out_considerable_job_id,
+                        jobject out_assign, jobject out_ports, jint max_ports, jobject out_fail, jobject out_stats) {
   cook_offers_soa o; cook_groups g; cook_user_table u; cook_pool_quota pq; cook_match_params prm;
   memset(&o, 0, sizeof(o)); memset(&g, 0, sizeof(g)); memset(&u, 0, sizeof(u));
   offers_from(env, n_offers, n_attr_cols, offers, &o);
@@ -235,17 +238,36 @@ JFN(jint, stateMatch)(JNIEnv* env, jclass k, jlong pool, jint n_offers, jint n_a
   memset(&prm, 0, sizeof(prm));
   prm.num_considerable = ip[0]; prm.enforce_rate_limit = ip[1]; prm.host_lifetime_mins = ip[2]; prm.fitness_kind = ip[3];
   prm.good_enough_fitness = good_enough_fitness; prm.reuse_resident = ip[4]; prm.max_ctas = ip[5];
-  return cook_state_match((cook_pool*)(intptr_t)pool, &o, have_g ? &g : NULL, &u, &pq, &prm,
-                          one(env, out_considerable_job_id), one(env, out_assign), one(env, out_ports), max_ports,
-                          one(env, out_fail), (cook_match_stats*)one(env, out_stats));
+  return fn((cook_pool*)(intptr_t)pool, &o, have_g ? &g : NULL, &u, &pq, &prm, one(env, out_considerable_job_id),
+            one(env, out_assign), one(env, out_ports), max_ports, one(env, out_fail), (cook_match_stats*)one(env, out_stats));
+}
+JFN(jint, stateMatch)(JNIEnv* env, jclass k, jlong pool, jint n_offers, jint n_attr_cols, jobjectArray offers,
+                      jint n_groups, jobjectArray groups, jint n_users, jobjectArray users, jdoubleArray pool_quota,
+                      jintArray iparams /* as match */, jdouble good_enough_fitness, jobject out_considerable_job_id,
+                      jobject out_assign, jobject out_ports, jint max_ports, jobject out_fail, jobject out_stats) {
+  return state_match(cook_state_match, env, pool, n_offers, n_attr_cols, offers, n_groups, groups, n_users, users,
+                     pool_quota, iparams, good_enough_fitness, out_considerable_job_id, out_assign, out_ports, max_ports,
+                     out_fail, out_stats);
+}
+/* stateMatch with the users' usage, the offers' run columns and the groups' cot lists derived on the device from
+ * the resident running rows: those columns of `users`, `offers` and `groups` are not read and may be null */
+JFN(jint, stateMatchDerived)(JNIEnv* env, jclass k, jlong pool, jint n_offers, jint n_attr_cols, jobjectArray offers,
+                             jint n_groups, jobjectArray groups, jint n_users, jobjectArray users, jdoubleArray pool_quota,
+                             jintArray iparams, jdouble good_enough_fitness, jobject out_considerable_job_id,
+                             jobject out_assign, jobject out_ports, jint max_ports, jobject out_fail, jobject out_stats) {
+  return state_match(cook_state_match_derived, env, pool, n_offers, n_attr_cols, offers, n_groups, groups, n_users,
+                     users, pool_quota, iparams, good_enough_fitness, out_considerable_job_id, out_assign, out_ports,
+                     max_ports, out_fail, out_stats);
 }
 
 /* the rebalancer over the resident rows; out_victim_task_id holds victim_cap task ids */
-JFN(jint, stateRebalance)(JNIEnv* env, jclass k, jlong pool, jint n_hosts, jint n_attr_cols, jobjectArray hosts,
-                          jint n_groups, jobjectArray groups, jint n_users, jobjectArray users, jint max_preemption,
-                          jdouble min_dru_diff, jdouble safe_dru_threshold, jint host_lifetime_mins,
-                          jobject out_decisions, jobject out_decision_job_id, jobject out_victim_task_id,
-                          jint victim_cap, jintArray out_n) {
+typedef int32_t (*state_rebalance_fn)(cook_pool*, const cook_host_table*, const cook_groups*, const cook_user_table*,
+                                      const cook_rebalance_params*, cook_decision*, int64_t*, int64_t*, int32_t, int32_t*);
+static jint state_rebalance(state_rebalance_fn fn, JNIEnv* env, jlong pool, jint n_hosts, jint n_attr_cols,
+                            jobjectArray hosts, jint n_groups, jobjectArray groups, jint n_users, jobjectArray users,
+                            jint max_preemption, jdouble min_dru_diff, jdouble safe_dru_threshold, jint host_lifetime_mins,
+                            jobject out_decisions, jobject out_decision_job_id, jobject out_victim_task_id,
+                            jint victim_cap, jintArray out_n) {
   cook_host_table h; cook_groups g; cook_user_table u; cook_rebalance_params prm;
   memset(&h, 0, sizeof(h)); memset(&g, 0, sizeof(g)); memset(&u, 0, sizeof(u));
   hosts_from(env, n_hosts, n_attr_cols, hosts, &h);
@@ -253,11 +275,29 @@ JFN(jint, stateRebalance)(JNIEnv* env, jclass k, jlong pool, jint n_hosts, jint 
   prm.max_preemption = max_preemption; prm.min_dru_diff = min_dru_diff; prm.safe_dru_threshold = safe_dru_threshold;
   prm.host_lifetime_mins = host_lifetime_mins;
   int32_t n = 0;
-  jint rc = cook_state_rebalance((cook_pool*)(intptr_t)pool, &h, have_g ? &g : NULL, &u, &prm,
-                                 (cook_decision*)one(env, out_decisions), one(env, out_decision_job_id),
-                                 one(env, out_victim_task_id), victim_cap, &n);
+  jint rc = fn((cook_pool*)(intptr_t)pool, &h, have_g ? &g : NULL, &u, &prm, (cook_decision*)one(env, out_decisions),
+               one(env, out_decision_job_id), one(env, out_victim_task_id), victim_cap, &n);
   (*env)->SetIntArrayRegion(env, out_n, 0, 1, (jint*)&n);
   return rc;
+}
+JFN(jint, stateRebalance)(JNIEnv* env, jclass k, jlong pool, jint n_hosts, jint n_attr_cols, jobjectArray hosts,
+                          jint n_groups, jobjectArray groups, jint n_users, jobjectArray users, jint max_preemption,
+                          jdouble min_dru_diff, jdouble safe_dru_threshold, jint host_lifetime_mins,
+                          jobject out_decisions, jobject out_decision_job_id, jobject out_victim_task_id,
+                          jint victim_cap, jintArray out_n) {
+  return state_rebalance(cook_state_rebalance, env, pool, n_hosts, n_attr_cols, hosts, n_groups, groups, n_users, users,
+                         max_preemption, min_dru_diff, safe_dru_threshold, host_lifetime_mins, out_decisions,
+                         out_decision_job_id, out_victim_task_id, victim_cap, out_n);
+}
+/* stateRebalance with the groups' cot lists derived on the device over `hosts` (those columns are not read) */
+JFN(jint, stateRebalanceDerived)(JNIEnv* env, jclass k, jlong pool, jint n_hosts, jint n_attr_cols, jobjectArray hosts,
+                                 jint n_groups, jobjectArray groups, jint n_users, jobjectArray users, jint max_preemption,
+                                 jdouble min_dru_diff, jdouble safe_dru_threshold, jint host_lifetime_mins,
+                                 jobject out_decisions, jobject out_decision_job_id, jobject out_victim_task_id,
+                                 jint victim_cap, jintArray out_n) {
+  return state_rebalance(cook_state_rebalance_derived, env, pool, n_hosts, n_attr_cols, hosts, n_groups, groups, n_users,
+                         users, max_preemption, min_dru_diff, safe_dru_threshold, host_lifetime_mins, out_decisions,
+                         out_decision_job_id, out_victim_task_id, victim_cap, out_n);
 }
 
 /* ---- B1-B6 ------------------------------------------------------------------------------------ */

@@ -40,6 +40,17 @@ host mirror of the running tasks (task -> host, groups), printing the call's dev
 wall time of the host build, and whether the two are identical.
 
   python tools/prof_state.py --cotasks --cycles 6
+
+--derived loads the pool's pending jobs and its running tasks (on random hosts of the offer table, 1 % with host
+unknown; with the pool's groups, one task in five in a group) and per cycle ranks, then matches twice on the same
+handle: the three-call sequence (cook_state_usage and cook_state_cotasks downloaded, then cook_state_match fed with
+them) and one cook_state_match_derived.  Per arm it prints the bytes up and down, the host wall time of the library
+calls (building the fed tables in Python excluded), the device time of the calls' events, and whether the outputs are
+identical.  The placed jobs are then launched on their hosts and 3 % of the running tasks finish.
+
+  python tools/prof_state.py --derived --pool c2 --cycles 6
+  python tools/prof_state.py --derived --pool c5 --c5-pool 5 --cycles 4
+  python tools/prof_state.py --derived --c3-pool 0 --cycles 4      # a config-#3 pool with groups
 """
 import argparse
 import json
@@ -295,6 +306,100 @@ def cotasks_prof(a):
     e.close()
 
 
+def _with(s, **over):
+    """A copy of the SoA struct `s` with fields replaced (None: NULL)."""
+    kw = {n: s.col(n) if t in (abi.P_I32, abi.P_I64, abi.P_F64, abi.P_U8) else getattr(s, n) for n, t in s._fields_}
+    kw.update(over)
+    return type(s)(**kw)
+
+
+def derived_prof(a):
+    if a.c3_pool >= 0:
+        t, name = traces.gen_config_pool("c3", a.c3_pool), f"c3/{a.c3_pool}"
+    elif a.pool == "c2":
+        t, name = traces.gen_c2(), "c2"
+    else:
+        t, name = traces.gen_config_pool("c5", a.c5_pool), f"c5/{a.c5_pool}"
+    jobs, pc, rc = t["jobs"], t["cols"]["pending"], t["cols"]["running"]
+    users, offers, groups = t["users"], t["offers"], t.get("groups")
+    G = groups.n_groups if groups is not None else 0
+    codes = offers.col("hostname_id").astype(np.int32)
+    U, R = users.n_users, len(rc["task_id"])
+    rng = np.random.default_rng(a.seed)
+    host = codes[rng.integers(0, len(codes), R)].astype(np.int32)
+    host[rng.random(R) < 0.01] = -1
+    rgroups = [[int(rng.integers(G))] if G and rng.random() < 0.2 else [] for _ in range(R)]
+    print(json.dumps({"card": card(), "pool": name, "jobs": jobs.n, "running": R, "offers": offers.n, "users": U,
+                      "groups": G}), flush=True)
+    store = Jobs(jobs, pc["priority"], pc["job_id"])
+    e = GpuEngine(pool_name="derived")
+    off, idx = abi.csr(rgroups)
+    e.state_apply(abi.make_delta(reset=True, running=abi.make_tasks(**rc), running_hostname_id=host,
+                                 running_group_off=off, running_group_idx=idx, **dict(
+                                     pending=store.soa(np.arange(jobs.n)), pending_priority=store.prio,
+                                     pending_job_id=store.jid)))
+    params = traces.match_params(jobs.n, host_lifetime_mins=t.get("host_lifetime_mins", 0))
+    max_ports = int(jobs.col("ports").max()) if jobs.col("ports") is not None else 0
+    d_users = _with(users, usage_count=None, usage_cpus=None, usage_mem=None, usage_gpus=None)
+    d_offers = _with(offers, run_cpus=None, run_mem=None, run_count=None)
+    d_groups = _with(groups, cot_off=None, cot_hostname_id=None, cot_attr_val=None) if G else groups
+    live = set(int(x) for x in rc["task_id"])
+    next_tid = int(max(live)) + 10 if live else 10
+
+    def dev_ms(s):
+        return sum(s[k] for k in ("ms_h2d", "ms_device", "ms_d2h") if k in s) + \
+            sum(s[k] for k in ("ms_considerable", "ms_match") if k in s)
+
+    for cycle in range(a.cycles):
+        e.state_rank(users)
+        # ---- the three-call sequence
+        w0 = time.perf_counter()
+        us = e.state_usage(U, codes)
+        wall = time.perf_counter() - w0
+        st = [e.last_stats(abi.PHASE_USAGE)]
+        f_users = _with(users, usage_count=us["user"]["count"], usage_cpus=us["user"]["cpus"],
+                        usage_mem=us["user"]["mem"], usage_gpus=us["user"]["gpus"])
+        f_offers = _with(offers, run_cpus=us["run_cpus"], run_mem=us["run_mem"], run_count=us["run_count"])
+        f_groups = groups
+        if G:
+            w0 = time.perf_counter()
+            cot = e.state_cotasks(G, groups.col("attr_col"), offers)
+            wall += time.perf_counter() - w0
+            st.append(e.last_stats(abi.PHASE_COTASKS))
+            f_groups = _with(groups, cot_off=cot[0], cot_hostname_id=cot[1] if len(cot[1]) else np.zeros(1, np.int32),
+                             cot_attr_val=cot[2] if len(cot[2]) else np.zeros(1, np.int32))
+        w0 = time.perf_counter()
+        ms = e.state_match(f_offers, f_users, params, groups=f_groups, max_ports=max_ports)
+        wall += time.perf_counter() - w0
+        st.append(ms["stats"])
+        seq = {"h2d_bytes": sum(x["h2d_bytes"] for x in st), "d2h_bytes": sum(x["d2h_bytes"] for x in st),
+               "wall_ms": round(1e3 * wall, 3), "device_ms": round(sum(dev_ms(x) for x in st), 3),
+               "calls": len(st)}
+        # ---- the derived call
+        w0 = time.perf_counter()
+        md = e.state_match(d_offers, d_users, params, groups=d_groups, max_ports=max_ports, derived=True)
+        wall = time.perf_counter() - w0
+        sd = md["stats"]
+        der = {"h2d_bytes": sd["h2d_bytes"], "d2h_bytes": sd["d2h_bytes"], "wall_ms": round(1e3 * wall, 3),
+               "device_ms": round(dev_ms(sd), 3), "ms_h2d": round(sd["ms_h2d"], 3),
+               "ms_match_kernel": round(sd["ms_match_kernel"], 3), "calls": 1}
+        same = all(np.array_equal(ms[k], md[k]) for k in ("considerable", "assign", "ports", "fail"))
+        print(json.dumps({"cycle": cycle, "running": len(live), "entries": int(f_groups.col("cot_off")[-1]) if G else 0,
+                          "considerable": len(md["considerable"]), "sequenced": seq, "derived": der,
+                          "identical": bool(same)}), flush=True)
+        # ---- launches on the chosen hosts, 3 % of the running tasks finish
+        ok = md["assign"] >= 0
+        jl = md["considerable"][ok]
+        tl = next_tid + 2 * np.arange(len(jl), dtype=np.int64)
+        next_tid += 2 * len(jl) + 2
+        e.state_launch(jl, tl, np.full(len(jl), 1_700_000_000_000 + cycle, np.int64), codes[md["assign"][ok]])
+        live.update(int(x) for x in tl)
+        fin = [int(x) for x in rng.choice(sorted(live), int(len(live) * 0.03), replace=False)]
+        live.difference_update(fin)
+        e.state_apply(abi.make_delta(running_rm=fin))
+    e.close()
+
+
 def launch_cycle(cycle, res, twin, job_id, lt, hosts, rest, match_args):
     """One cycle of --launch: the launches by id on `res` and as a delta on `twin`, the rest of the batch on both,
     then rank and match on both.  Returns the jobs the match placed and their hosts' codes."""
@@ -338,7 +443,10 @@ def main():
     ap.add_argument("--seed", type=int, default=7)
     ap.add_argument("--usage", action="store_true")
     ap.add_argument("--cotasks", action="store_true")
-    ap.add_argument("--c3-pool", type=int, default=-1, help="--cotasks: a config-#3 pool (-1: the smaller c3-shaped pool)")
+    ap.add_argument("--c3-pool", type=int, default=-1,
+                    help="--cotasks: a config-#3 pool (-1: the smaller c3-shaped pool); --derived: a config-#3 pool "
+                         "instead of --pool")
+    ap.add_argument("--derived", action="store_true")
     a = ap.parse_args()
     if a.rebalance:
         return rebalance(a)
@@ -346,6 +454,8 @@ def main():
         return usage(a)
     if a.cotasks:
         return cotasks_prof(a)
+    if a.derived:
+        return derived_prof(a)
     t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
     jobs, pc, rc = t["jobs"], t["cols"]["pending"], t["cols"]["running"]
     J = jobs.n
