@@ -5,6 +5,9 @@
 ;;   :1339-1535 handle-resource-offers!      -> (handle-resource-offers! ...)       [cook_match]
 ;;   rebalancer.clj:434-467 rebalance        -> (rebalance! ...)                    [cook_rebalance]
 ;;   :2125-2157 quota-group usage            -> (exchange-usage! ...)               [cook_exchange_usage]
+;;   :2262-2284 rank-jobs, resident pool     -> (rank-resident! ...)                [cook_state_rank_offensive]
+;;   :1749-1800 Kubernetes-scheduler pool    -> (kubernetes-considerable! ...)      [cook_state_considerable]
+;;   :1283-1335 autoscaling helper           -> (autoscalable-jobs! ...)            [cook_state_considerable]
 ;; selected per pool with {:scheduler-config {:scheduler "gpu"}} next to "fenzo" / "kubernetes"
 ;; (config.clj:110-122, make-pool-handler :2425-2466).  Everything numeric happens in libcookgpu;
 ;; this namespace marshals columns and keeps the state Fenzo kept (cook_b200/cycle.py is the same
@@ -12,7 +15,8 @@
 ;;
 ;; NOT COMPILED in this repository's image (no JVM): reviewed against scheduler.clj and abi.py.
 (ns cook.scheduler.gpu
-  (:require [clojure.tools.logging :as log]
+  (:require [clojure.core.async :as async]
+            [clojure.tools.logging :as log]
             [cook.config :as config]
             [cook.scheduler.constraints :as constraints]
             [cook.tools :as tools])
@@ -170,6 +174,41 @@
    match."
   [handle args]
   (check! handle (apply #(Native/stateMatchDerived handle %&) args) "cook_state_match_derived"))
+
+(defn rank-resident!
+  "Ranks the resident pool (cook_state_rank_offensive) and pushes the jobs the rank dropped as offensive to
+   offensive-jobs-ch, as filter-offensive-jobs (scheduler.clj:2198-2229) does: the stifler marks them completed.
+   `args` are Native/stateRankOffensive's arguments after the handle; `job-id->job` resolves a job id, `out-off` /
+   `out-n-off` are its offensive-job-id buffer and count array.  Returns the queue's length."
+  [handle args ^ByteBuffer out-off ^ints out-n-off job-id->job offensive-jobs-ch]
+  (check! handle (apply #(Native/stateRankOffensive handle %&) args) "cook_state_rank_offensive")
+  (let [n (aget out-n-off 0)
+        lb (.asLongBuffer out-off)
+        jobs (mapv #(job-id->job (.get lb (int %))) (range n))]
+    (when (seq jobs) (async/>!! offensive-jobs-ch jobs))
+    n))
+
+(defn kubernetes-considerable!
+  "handle-kubernetes-scheduler-pool (scheduler.clj:1749-1800) on a resident pool: pending-jobs->considerable-jobs in
+   one call (cook_state_considerable with the allowed / plugin masks read, the usage derived from the resident running
+   rows, consume on: the jobs leave the queue until the next rank, as remove-matched-jobs-from-pending-jobs does).
+   `args` are Native/stateConsiderable's arguments after the handle and before iparams.  Returns the job ids; the
+   caller launches them."
+  [handle num-considerable enforce-rate-limit? args ^ByteBuffer out ^ints out-n]
+  (check! handle (apply #(Native/stateConsiderable handle %&)
+                        (concat args [(int-array [num-considerable (if enforce-rate-limit? 1 0) 0 1 1]) out out-n]))
+          "cook_state_considerable")
+  (let [lb (.asLongBuffer out)] (mapv #(.get lb (int %)) (range (aget out-n 0)))))
+
+(defn autoscalable-jobs!
+  "handle-resource-offers-autoscaling-helper (scheduler.clj:1283-1335) after a resident match and its launches:
+   filter-pending-jobs-for-quota over what is left of the queue (quota_only), with the usage the match read
+   (COOK_USAGE_LAST_MATCH).  `n` is the scaled maximum; the recent-synthetic-pod skip stays with the caller."
+  [handle n enforce-rate-limit? args ^ByteBuffer out ^ints out-n]
+  (check! handle (apply #(Native/stateConsiderable handle %&)
+                        (concat args [(int-array [n (if enforce-rate-limit? 1 0) 1 2 0]) out out-n]))
+          "cook_state_considerable")
+  (let [lb (.asLongBuffer out)] (mapv #(.get lb (int %)) (range (aget out-n 0)))))
 
 (defn rebalance-derived!
   "cook_state_rebalance_derived: the rebalancer over the resident rows with the groups' cotask lists derived on the

@@ -140,6 +140,15 @@ class PhaseStats(C.Structure):
 
 
 PHASE_RANK, PHASE_MATCH, PHASE_REBALANCE, PHASE_EXCHANGE, PHASE_STATE, PHASE_USAGE, PHASE_COTASKS = 0, 1, 2, 3, 4, 5, 6
+PHASE_CONSIDERABLE = 7
+
+USAGE_GIVEN, USAGE_DERIVED, USAGE_LAST_MATCH = 0, 1, 2
+
+
+class ConsiderableParams(C.Structure):
+    """cook_considerable_params: M0 over the resident queue (cook_state_considerable)."""
+    _fields_ = [("num_considerable", C.c_int32), ("enforce_rate_limit", C.c_int32), ("quota_only", C.c_int32),
+                ("usage_source", C.c_int32), ("consume", C.c_int32)]
 
 
 class StateDelta(_SoA):
@@ -227,6 +236,10 @@ _STATE_REBALANCE = [C.c_void_p, C.POINTER(HostTable), C.POINTER(Groups), C.POINT
 ARGTYPES = {
     "cook_state_match_derived": _STATE_MATCH,
     "cook_state_rebalance_derived": _STATE_REBALANCE,
+    "cook_state_considerable": [C.c_void_p, C.POINTER(UserTable), C.POINTER(PoolQuota), C.POINTER(ConsiderableParams),
+                                P_I64, P_I32],
+    "cook_state_rank_offensive": [C.c_void_p, C.POINTER(UserTable), C.POINTER(PoolQuota), C.POINTER(PoolQuota), P_F64,
+                                  C.POINTER(RankParams), P_I64, P_I32, P_I64, C.c_int32, P_I32],
 }
 
 

@@ -83,7 +83,7 @@ int32_t cook_last_error(cook_pool* p, char* buf, int32_t len) {
 }
 
 int32_t cook_last_stats(cook_pool* p, int32_t phase, cook_phase_stats* out) {
-  if (!p || !out || phase < 0 || phase > COOK_PHASE_COTASKS) return COOK_E_BADARG;
+  if (!p || !out || phase < 0 || phase > COOK_PHASE_CONSIDERABLE) return COOK_E_BADARG;
   *out = p->phase[phase];
   return COOK_OK;
 }

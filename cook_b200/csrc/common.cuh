@@ -122,7 +122,8 @@ struct cook_pool {
   int sm_count = 0;
   cudaStream_t stream = nullptr;
   cudaEvent_t ev[24] = {};
-  cook_phase_stats phase[7] = {};        // last rank / match / rebalance / exchange / state-apply / usage / cotasks call
+  cook_phase_stats phase[8] = {};        // last rank / match / rebalance / exchange / state-apply / usage / cotasks /
+                                         // considerable call
   double* xchg = nullptr;                // exchange buffers: [n_pad] local + [world * n_pad] gathered
   size_t xchg_cap = 0;
   Arena arena;
@@ -179,11 +180,19 @@ struct RankQueue {
   const int32_t* ranked;
   const int32_t* n;
 };
+// `offensive` (if given): the pending jobs that survive the quota filters and are offensive, in rank order, as job
+// ids jid[pslot[pending index]] into the host's out[<= J], their number in *out_n (downloaded with the counts).
+struct RankOffensive {
+  const int32_t* pslot;
+  const int64_t* jid;
+  int64_t* out;
+  int32_t* out_n;
+};
 int32_t rank_impl(cook_pool* pool, int R, int J, const cook_tasks_soa* running, const cook_tasks_soa* pending,
                   const TaskCols* dev, const cook_user_table* users, const cook_pool_quota* pool_quota,
                   const cook_pool_quota* group_quota, const double* group_usage, const cook_rank_params* params,
                   int32_t* out_ranked_idx, int32_t* out_n, double* out_dru, int32_t* out_order, int32_t* out_order_n,
-                  RankQueue* queue);
+                  RankQueue* queue, const RankOffensive* offensive = nullptr);
 
 // The running-side inputs of a match or rebalance that the resident state derives on the device after the build:
 // carved, not uploaded.  usage: the users' usage_* as one [4][n_users] block (count, cpus, mem, gpus); run: the
@@ -234,6 +243,36 @@ int32_t match_build(cook_pool* pool, const int32_t* ranked_idx, int32_t n_ranked
                     MatchRows* rows);
 int32_t match_run(cook_pool* pool, int32_t* out_considerable, int64_t* out_job_id, int32_t* out_assign,
                   int32_t* out_ports, uint8_t* out_fail_reason, cook_match_stats* out_stats, bool uploaded, int max_ctas);
+
+// match.cu: M0 (pending-jobs->considerable-jobs, filter-pending-jobs-for-quota) over n job rows already on the
+// device, by cook_match's own launches: the per-user folds in the order `ranked` gives, the pool-quota fold over
+// users 0 .. n_users - 1, the masks (null: not read), take num_considerable.  Quotas [4] and usage [4] are count,
+// cpus, mem, gpus columns of n_users (a null usage column reads 0); tokens may be null.  Scratch: pos, tmp [n + 1],
+// seg_s, seg_e [n_users + 1], keep [n + 1], gf.  out_row[k] receives the row of the k-th considerable job, *out_n
+// (device) their number.
+struct GridFlag;
+struct ConsRows {
+  int n = 0, n_users = 0;
+  const int32_t* ranked = nullptr;
+  const int32_t* user = nullptr;
+  const double *cpus = nullptr, *mem = nullptr, *gpus = nullptr;
+  const uint8_t *allowed = nullptr, *plugin = nullptr;
+  const double* quota[4] = {};
+  const double* usage[4] = {};
+  const int32_t* tokens = nullptr;
+  int enforce_rate_limit = 0;
+  cook_pool_quota pool_q = {0, 0, 0, 0, 0};
+  int num_considerable = 0;
+  int32_t *pos = nullptr, *tmp = nullptr, *seg_s = nullptr, *seg_e = nullptr;
+  uint8_t* keep = nullptr;
+  GridFlag* gf = nullptr;
+  int32_t* out_row = nullptr;
+  int32_t* out_n = nullptr;
+};
+cudaError_t considerable_rows(const ConsRows& r, cudaStream_t st, int* launches);
+// The [4][n_users] usage columns the last match on this handle read, from its plan; false when no plan is valid or
+// it was built for another n_users.
+bool match_last_usage(cook_pool* pool, int n_users, const double* (&usage)[4]);
 
 // rebalance.cu: what a rebalance needs to know about its rows before it carves their columns.
 struct RebShape {

@@ -1927,7 +1927,9 @@ struct ConsOut {
 
 // Queue-order pass (single warp): pool quota over survivors (tools.clj:917-933),
 // allowed + launch-plugin masks (scheduler.clj:749-750), take N (:751).
-__global__ void cons_queue_kernel(ConsArgs a, const uint8_t* keep, ConsOut out, int32_t* out_n) {
+// Out::put(jb, j, slot) receives the slot-th considerable job j.
+template <class Out>
+__global__ void cons_queue_kernel(ConsArgs a, const uint8_t* keep, Out out, int32_t* out_n) {
   const int lane = threadIdx.x;
   __shared__ double stage[4][32];
   double pool[4] = {0.0, 0.0, 0.0, 0.0};   // count, cpus, mem, gpus
@@ -1961,8 +1963,9 @@ __global__ void cons_queue_kernel(ConsArgs a, const uint8_t* keep, ConsOut out, 
 // Parallel form of the queue-order pass for the common case of NO global pool
 // quota (tools.clj:923 `(if (nil? quota) queue ...)`): the filters are then
 // element-wise and "take N" is a stable compaction.
+template <class Out>
 struct ConsSurvivors {
-  ConsArgs a; const uint8_t* kept; ConsOut out;
+  ConsArgs a; const uint8_t* kept; Out out;
   __device__ bool keep(int i) const {
     if (!kept[i]) return false;
     const int j = a.ranked[i];
@@ -1972,6 +1975,40 @@ struct ConsSurvivors {
   }
   __device__ void emit(int i, int slot) const { out.put(a.jb, a.ranked[i], slot); }
 };
+
+// The considerable set as job indices alone (the resident state's considerable call).
+struct ConsIdx {
+  int32_t* cons;
+  __device__ void put(const JobDev&, int j, int slot) const { cons[slot] = j; }
+};
+
+// M0 over the rows a.ranked names, after the caller zeroed seg_s / seg_e [n_users + 1]: the per-user order, its
+// segments, the grid check of the J job rows, the per-user folds, then the queue-order pass (pool quota: one warp;
+// else the stable compaction).  *count receives the number of considerable jobs.  Shared by cook_match and
+// cook_state_considerable, so both run the same launches on the same columns.
+template <class Out>
+cudaError_t cons_pass(const ConsArgs& ca, int J, int32_t* pos, int32_t* tmp, int32_t* seg_s, int32_t* seg_e,
+                      uint8_t* keep, GridFlag* gf, const Out& out, int32_t* count, cudaStream_t st, int* launches) {
+  const int TB = 256, n = ca.n_ranked, U = ca.n_users;
+  cudaError_t e = csort::sort_indices(pos, tmp, n, LessUserPos{ca.ranked, ca.jb.user}, st, launches);
+  if (e != cudaSuccess) return e;
+  seg_bounds_kernel<<<(n + TB - 1) / TB, TB, 0, st>>>(SortedKey{pos, ca.ranked, ca.jb.user}, n, seg_s, seg_e, nullptr);
+  (*launches)++;
+  if ((e = cudaMemsetAsync(gf, 0, sizeof(GridFlag), st)) != cudaSuccess) return e;
+  grid_check_kernel<<<(J + TB - 1) / TB, TB, 0, st>>>(ca.jb.cpus, ca.jb.mem, ca.jb.gpus, J, gf);
+  (*launches)++;
+  cons_user_kernel<<<(U + 3) / 4, 128, 0, st>>>(ca, pos, seg_s, seg_e, keep, gf);
+  (*launches)++;
+  if (ca.pool_q.enabled) {
+    // global pool quota: an order-dependent f64 left fold over the survivors
+    // (filter-sequential) => exact single-warp pass
+    cons_queue_kernel<<<1, 32, 0, st>>>(ca, keep, out, count);
+    (*launches)++;
+  } else {
+    compact(ConsSurvivors<Out>{ca, keep, out}, n, nullptr, tmp, count, ca.num_considerable, st, launches);
+  }
+  return cudaGetLastError();
+}
 
 // ------------------------------------------------------------------ setup
 __global__ void gather_offers_kernel(const int32_t* perm, int O, const double* c, const double* m,
@@ -2525,7 +2562,7 @@ int32_t match_run(cook_pool* pool, int32_t* out_considerable, int64_t* out_job_i
   MatchPlan* mp = plan_of(pool);
   mp->valid = true;   // the plan's inputs are complete: a caller that writes its rows did so before the run
   cudaStream_t st = pool->stream;
-  const int O = mp->O, U = mp->U, n_ranked = mp->n_ranked, max_ports = mp->max_ports;
+  const int O = mp->O, U = mp->U, max_ports = mp->max_ports;
   MatchArgs& ma = mp->ma;
   ConsArgs& ca = mp->ca;
   int launches = 0;
@@ -2566,26 +2603,9 @@ int32_t match_run(cook_pool* pool, int32_t* out_considerable, int64_t* out_job_i
       launches++;
     }
   }
-  CK(pool, csort::sort_indices(mp->d_pos, mp->d_tmp, n_ranked, LessUserPos{ca.ranked, ca.jb.user}, st, &launches));
-  seg_bounds_kernel<<<(n_ranked + TB - 1) / TB, TB, 0, st>>>(SortedKey{mp->d_pos, ca.ranked, ca.jb.user}, n_ranked,
-                                                             mp->d_seg_s, mp->d_seg_e, nullptr);
-  launches++;
-  CK(pool, cudaMemsetAsync(mp->d_gf, 0, sizeof(GridFlag), st));
-  grid_check_kernel<<<(mp->J + TB - 1) / TB, TB, 0, st>>>(ca.jb.cpus, ca.jb.mem, ca.jb.gpus, mp->J, mp->d_gf);
-  launches++;
-  cons_user_kernel<<<(U + 3) / 4, 128, 0, st>>>(ca, mp->d_pos, mp->d_seg_s, mp->d_seg_e, mp->d_keep, mp->d_gf);
-  launches++;
   const ConsOut cons_out{mp->d_cons, mp->d_kc, mp->d_km, mp->d_kg, mp->d_kports, mp->d_kflags};
-  if (ca.pool_q.enabled) {
-    // global pool quota: an order-dependent f64 left fold over the survivors
-    // (filter-sequential) => exact single-warp pass
-    cons_queue_kernel<<<1, 32, 0, st>>>(ca, mp->d_keep, cons_out, mp->d_counters);
-    launches++;
-  } else {
-    compact(ConsSurvivors{ca, mp->d_keep, cons_out}, n_ranked, nullptr, mp->d_tmp, mp->d_counters, ca.num_considerable, st,
-            &launches);
-  }
-  CK(pool, cudaGetLastError());
+  CK(pool, cons_pass(ca, mp->J, mp->d_pos, mp->d_tmp, mp->d_seg_s, mp->d_seg_e, mp->d_keep, mp->d_gf, cons_out,
+                     mp->d_counters, st, &launches));
   int32_t n_cons = 0;
   int64_t d2h = 0;
   CK(pool, download(&n_cons, mp->d_counters, 1, st, &d2h));
@@ -2725,6 +2745,33 @@ int32_t match_run(cook_pool* pool, int32_t* out_considerable, int64_t* out_job_i
     out_stats->d2h_bytes = ps.d2h_bytes;
   }
   return COOK_OK;
+}
+
+cudaError_t considerable_rows(const ConsRows& r, cudaStream_t st, int* launches) {
+  ConsArgs ca;
+  memset(&ca, 0, sizeof(ca));
+  ca.ranked = r.ranked; ca.n_ranked = r.n;
+  ca.jb.user = r.user; ca.jb.cpus = r.cpus; ca.jb.mem = r.mem; ca.jb.gpus = r.gpus;
+  ca.jb.allowed = r.allowed; ca.jb.plugin = r.plugin;
+  ca.n_users = r.n_users;
+  ca.q_count = r.quota[0]; ca.q_cpus = r.quota[1]; ca.q_mem = r.quota[2]; ca.q_gpus = r.quota[3];
+  ca.u_count = r.usage[0]; ca.u_cpus = r.usage[1]; ca.u_mem = r.usage[2]; ca.u_gpus = r.usage[3];
+  ca.tokens = r.tokens;
+  ca.enforce_rate_limit = r.enforce_rate_limit;
+  ca.pool_q = r.pool_q;
+  ca.num_considerable = r.num_considerable;
+  const size_t segs = sizeof(int32_t) * ((size_t)r.n_users + 1);
+  cudaError_t e = cudaMemsetAsync(r.seg_s, 0, segs, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(r.seg_e, 0, segs, st);
+  if (e != cudaSuccess) return e;
+  return cons_pass(ca, r.n, r.pos, r.tmp, r.seg_s, r.seg_e, r.keep, r.gf, ConsIdx{r.out_row}, r.out_n, st, launches);
+}
+
+bool match_last_usage(cook_pool* pool, int n_users, const double* (&usage)[4]) {
+  const MatchPlan* mp = static_cast<const MatchPlan*>(pool->match_plan);
+  if (!mp || !mp->valid || mp->U != n_users) return false;
+  usage[0] = mp->ca.u_count; usage[1] = mp->ca.u_cpus; usage[2] = mp->ca.u_mem; usage[3] = mp->ca.u_gpus;
+  return true;
 }
 
 int32_t check_match_inputs(cook_pool* pool, const char* who, const cook_offers_soa* offers, const cook_groups* groups,

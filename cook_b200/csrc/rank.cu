@@ -280,6 +280,14 @@ struct QueueSurvivors {
   __device__ void emit(int i, int slot) const { a.out_ranked[slot] = a.ti_at[i] - a.R; }
 };
 
+// The jobs filter-offensive-jobs puts on its channel: past the quota filters and offensive, in rank order, as job
+// ids (dense pending index -> slot -> job id).
+struct QueueOffensive {
+  QueueFilterArgs a; const int32_t* pslot; const int64_t* jid; int64_t* out;
+  __device__ bool keep(int i) const { return a.flag[i] && (a.xm[i] > a.off_mem || a.xc[i] > a.off_cpus); }
+  __device__ void emit(int i, int slot) const { out[slot] = jid[pslot[a.ti_at[i] - a.R]]; }
+};
+
 }  // namespace
 
 extern "C" int32_t cook_rank(cook_pool* pool, const cook_tasks_soa* running,
@@ -298,7 +306,7 @@ int32_t rank_impl(cook_pool* pool, int R, int J, const cook_tasks_soa* running, 
                   const TaskCols* dev, const cook_user_table* users, const cook_pool_quota* pool_quota,
                   const cook_pool_quota* group_quota, const double* group_usage, const cook_rank_params* params,
                   int32_t* out_ranked_idx, int32_t* out_n, double* out_dru, int32_t* out_order, int32_t* out_order_n,
-                  RankQueue* queue) {
+                  RankQueue* queue, const RankOffensive* offensive) {
   if (!users || !params || !out_n) return set_err(pool, COOK_E_BADARG, "cook_rank: null argument");
   const int N = R + J, U = users->n_users;
   if (R < 0 || J < 0 || U <= 0) return set_err(pool, COOK_E_BADARG, "cook_rank: bad sizes");
@@ -307,6 +315,7 @@ int32_t rank_impl(cook_pool* pool, int R, int J, const cook_tasks_soa* running, 
     return set_err(pool, COOK_E_BADARG, "cook_rank: task user index out of range");
   *out_n = 0;
   if (out_order_n) *out_order_n = 0;
+  if (offensive) *offensive->out_n = 0;
   if (N == 0) return COOK_OK;
   CK(pool, cudaSetDevice(pool->device));
   cudaStream_t st = pool->stream;
@@ -319,6 +328,7 @@ int32_t rank_impl(cook_pool* pool, int R, int J, const cook_tasks_soa* running, 
   double *d_dru_at, *d_pool_usage, *d_dru_task, *d_os_pm, *d_os_pc, *d_os_pg, *d_os_b;
   GridFlag* d_gf;
   QueueFilterArgs qa;
+  int64_t* d_off = nullptr;
   const int os_nb = (N + OS_TILE - 1) / OS_TILE;
   int64_t h2d = 0, d2h = 0;
   const cudaError_t carved = carve(pool->arena, st, pool->ev[8], &h2d, [&](Carve& c) {
@@ -358,6 +368,7 @@ int32_t rank_impl(cook_pool* pool, int R, int J, const cook_tasks_soa* running, 
     qa.ti_at = c.take<int32_t>(N + 1); qa.flag = c.take<uint8_t>(N + 1);
     qa.xc = c.take<double>(N + 1); qa.xm = c.take<double>(N + 1); qa.xg = c.take<double>(N + 1);
     qa.blk_cnt = c.take<int32_t>(N / CP_BLOCK + 2);
+    if (offensive) d_off = c.take<int64_t>(J + 1);
   });
   CK(pool, carved);
   CK(pool, cudaMemsetAsync(d_gf, 0, sizeof(GridFlag), st));
@@ -411,6 +422,11 @@ int32_t rank_impl(cook_pool* pool, int R, int J, const cook_tasks_soa* running, 
   }
   // at most J survivors: the caller's out_ranked_idx holds J, so no order can make the download overrun it
   compact(QueueSurvivors{qa}, N, qa.n_kept, qa.blk_cnt, qa.out_n, J, st, &nl);
+  // the queue's compaction is done with blk_cnt: the offensive one reuses it (nothing is offensive when the filter
+  // is off, and the count stays 0)
+  if (offensive && params->filter_offensive)
+    compact(QueueOffensive{qa, offensive->pslot, offensive->jid, d_off}, N, qa.n_kept, qa.blk_cnt, d_counters + 2, J,
+            st, &nl);
   if (out_dru) {
     scatter_dru_kernel<<<nb, TB, 0, st>>>(d_idx, d_dru_at, N, d_dru_task);
     nl++;
@@ -418,11 +434,15 @@ int32_t rank_impl(cook_pool* pool, int R, int J, const cook_tasks_soa* running, 
   CK(pool, cudaGetLastError());
   if (queue) *queue = RankQueue{d_out_ranked, qa.out_n};
   CK(pool, cudaEventRecord(pool->ev[10], st));
-  int32_t h_counters[2] = {0, 0};
-  CK(pool, download(h_counters, d_counters, 2, st, &d2h));
+  int32_t h_counters[3] = {0, 0, 0};   // [2]: offensive jobs
+  CK(pool, download(h_counters, d_counters, offensive ? 3 : 2, st, &d2h));
   CK(pool, cudaStreamSynchronize(st));
   const int32_t n_kept = h_counters[0], n_out = h_counters[1];
   if (n_out > 0 && out_ranked_idx) CK(pool, download(out_ranked_idx, d_out_ranked, n_out, st, &d2h));
+  if (offensive) {
+    *offensive->out_n = h_counters[2];
+    if (h_counters[2] > 0) CK(pool, download(offensive->out, d_off, h_counters[2], st, &d2h));
+  }
   if (out_order && n_kept > 0) CK(pool, download(out_order, d_out_order, n_kept, st, &d2h));
   if (out_dru) CK(pool, download(out_dru, d_dru_task, N, st, &d2h));
   CK(pool, cudaEventRecord(pool->ev[11], st));

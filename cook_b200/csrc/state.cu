@@ -21,6 +21,8 @@
 // Running rows carry their job's group list (a fourth arena, filled by running upserts and moved on the device
 // by a launch).  A group's cotasks: the live running rows with a known host expanded into one entry per group,
 // sorted by (group, task id).
+// Considerable jobs without a match: the live queue entries with their queue positions, their M0 columns gathered,
+// cook_match's considerable pass (match.cu) run on them; a consuming call retires the taken entries' generations.
 #include <algorithm>
 #include <map>
 #include <unordered_map>
@@ -217,6 +219,37 @@ struct QueueLive {
   __device__ bool keep(int k) const { const int s = q_slot[k]; return live[s] && gen[s] == q_gen[k]; }
   __device__ void emit(int k, int d) const { m_slot[d] = q_slot[k]; }
 };
+
+// ---- considerable: the live queue entries with their queue positions
+struct QueueLivePos {
+  QueueLive q; int32_t* qpos;
+  __device__ bool keep(int k) const { return q.keep(k); }
+  __device__ void emit(int k, int d) const { q.emit(k, d); qpos[d] = k; }
+};
+// row d of a considerable call is slot m_slot[d]: the columns M0 reads (a null mask is not gathered)
+__global__ void cons_rows_kernel(void* const* col, const int32_t* m_slot, int n, int32_t* ranked, int32_t* user,
+                                 double* cpus, double* mem, double* gpus, uint8_t* allowed, uint8_t* plugin) {
+  const int d = blockIdx.x * blockDim.x + threadIdx.x;
+  if (d >= n) return;
+  const int s = m_slot[d];
+  ranked[d] = d;
+  user[d] = static_cast<const int32_t*>(col[P_USER])[s];
+  cpus[d] = static_cast<const double*>(col[P_CPUS])[s];
+  mem[d] = static_cast<const double*>(col[P_MEM])[s];
+  gpus[d] = static_cast<const double*>(col[P_GPUS])[s];
+  if (allowed) allowed[d] = static_cast<const uint8_t*>(col[P_ALLOWED])[s];
+  if (plugin) plugin[d] = static_cast<const uint8_t*>(col[P_PLUGIN])[s];
+}
+// the k-th considerable job (row row[k] < *n): its job id and, with `consume`, its queue entry retired by writing the
+// rank-time generation minus one: a slot's generation only grows, so the entry stays stale until the next rank
+__global__ void cons_take_kernel(const int32_t* row, const int32_t* n, const int32_t* qpos, const int64_t* q_jid,
+                                 uint32_t* q_gen, int consume, int64_t* out) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= *n) return;
+  const int q = qpos[row[k]];
+  out[k] = q_jid[q];
+  if (consume) q_gen[q] -= 1u;
+}
 
 // row d of the match is slot m_slot[d]: its columns into the plan's
 __global__ void fill_rows_kernel(MatchRows r, void* const* col, const int32_t* m_slot, int n) {
@@ -1449,19 +1482,27 @@ extern "C" int32_t cook_state_cotasks(cook_pool* pool, int32_t n_groups, const i
                  out_cot_hostname_id, out_cot_attr_val, out_n);
 }
 
-extern "C" int32_t cook_state_rank(cook_pool* pool, const cook_user_table* users, const cook_pool_quota* pool_quota,
-                                   const cook_pool_quota* group_quota, const double* group_usage,
-                                   const cook_rank_params* params, int64_t* out_ranked_job_id, int32_t* out_n) {
+namespace {
+
+// cook_state_rank, and with `offensive` cook_state_rank_offensive: the jobs the rank drops as offensive, as job ids
+int32_t state_rank(cook_pool* pool, const char* who, bool offensive, const cook_user_table* users,
+                   const cook_pool_quota* pool_quota, const cook_pool_quota* group_quota, const double* group_usage,
+                   const cook_rank_params* params, int64_t* out_ranked_job_id, int32_t* out_n, int64_t* out_off,
+                   int32_t off_cap, int32_t* out_n_off) {
   if (!pool) return COOK_E_BADARG;
-  if (!users || !params || !out_n) return set_err(pool, COOK_E_BADARG, "cook_state_rank: null argument");
+  if (!users || !params || !out_n || (offensive && (!out_off || !out_n_off)))
+    return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
   *out_n = 0;
+  if (offensive) *out_n_off = 0;
   CK(pool, cudaSetDevice(pool->device));
   PoolState* S = state_of(pool, true);
-  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_rank: out of device memory");
+  if (!S) return set_err(pool, COOK_E_OOM, "%s: out of device memory", who);
   const int U = users->n_users;
-  if (U <= 0) return set_err(pool, COOK_E_BADARG, "cook_state_rank: bad sizes");
+  if (U <= 0) return set_err(pool, COOK_E_BADARG, "%s: bad sizes", who);
   if (std::max(count_max(S->users_p), count_max(S->users_r)) >= U)
-    return set_err(pool, COOK_E_BADARG, "cook_state_rank: a resident row's user code is >= n_users");
+    return set_err(pool, COOK_E_BADARG, "%s: a resident row's user code is >= n_users", who);
+  if (offensive && (int64_t)off_cap < (int64_t)S->pend.slot_of.size())
+    return set_err(pool, COOK_E_BADARG, "%s: offensive_cap < the live pending rows", who);
   cudaStream_t st = pool->stream;
   const int R = (int)S->run.slot_of.size(), J = (int)S->pend.slot_of.size();
   const size_t N = (size_t)R + J;
@@ -1486,8 +1527,9 @@ extern "C" int32_t cook_state_rank(cook_pool* pool, const cook_user_table* users
   }
   int32_t n = 0;
   RankQueue rq = {};
+  const RankOffensive ro{pslot, S->pend.at<int64_t>(P_JID), out_off, out_n_off};
   const int32_t rc = rank_impl(pool, R, J, nullptr, nullptr, &dt, users, pool_quota, group_quota, group_usage, params,
-                               nullptr, &n, nullptr, nullptr, nullptr, &rq);
+                               nullptr, &n, nullptr, nullptr, nullptr, &rq, offensive ? &ro : nullptr);
   if (rc != COOK_OK) return rc;
   cook_phase_stats& ps = pool->phase[COOK_PHASE_RANK];
   if (N > 0) ps.ms_device += ev_ms(pool->ev[7], pool->ev[23]);   // the gathering of the live rows
@@ -1517,8 +1559,6 @@ extern "C" int32_t cook_state_rank(cook_pool* pool, const cook_user_table* users
   *out_n = n;
   return COOK_OK;
 }
-
-namespace {
 
 // cook_state_match, and with `derived` cook_state_match_derived: the users' usage, the offers' run_* and the
 // groups' cot_* lists come from the live running rows, filled on the device into the columns the plan carved
@@ -1764,7 +1804,148 @@ int32_t state_rebalance(cook_pool* pool, const char* who, bool derived, const co
   return COOK_OK;
 }
 
+// cook_state_considerable: M0 over the live queue, the considerable pass cook_match runs (match.cu), without a plan
+int32_t considerable(cook_pool* pool, PoolState* S, const cook_user_table* users, const cook_pool_quota* pool_quota,
+                     const cook_considerable_params* prm, int64_t* out_job_id, int32_t* out_n) {
+  const char* who = "cook_state_considerable";
+  // ---- every check before any device work or output
+  if (!users || !prm || !out_job_id || !out_n) return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
+  if (!S || !S->ranked) return set_err(pool, COOK_E_BADARG, "%s: no cook_state_rank on this handle yet", who);
+  const int U = users->n_users, src = prm->usage_source;
+  if (U <= 0) return set_err(pool, COOK_E_BADARG, "%s: bad sizes", who);
+  if (src != COOK_USAGE_GIVEN && src != COOK_USAGE_DERIVED && src != COOK_USAGE_LAST_MATCH)
+    return set_err(pool, COOK_E_BADARG, "%s: unknown usage_source", who);
+  const double* quota[4] = {users->quota_count, users->quota_cpus, users->quota_mem, users->quota_gpus};
+  const double* given[4] = {users->usage_count, users->usage_cpus, users->usage_mem, users->usage_gpus};
+  for (int k = 0; k < 4; k++)
+    if (!quota[k] || (src == COOK_USAGE_GIVEN && !given[k]))
+      return set_err(pool, COOK_E_BADARG, "%s: null quota or (given usage) usage column", who);
+  if (count_max(S->users_p) >= U) return set_err(pool, COOK_E_BADARG, "%s: a pending row's user code is >= n_users", who);
+  if (src == COOK_USAGE_DERIVED && count_max(S->users_r) >= U)
+    return set_err(pool, COOK_E_BADARG, "%s: a live running row's user code is >= n_users", who);
+  const double* last[4] = {};
+  if (src == COOK_USAGE_LAST_MATCH && !match_last_usage(pool, U, last))
+    return set_err(pool, COOK_E_BADARG, "%s: LAST_MATCH without a match on this handle for these n_users", who);
+  *out_n = 0;
+  const int nq = S->n_q;
+  if (prm->num_considerable <= 0 || nq == 0) {
+    pool->phase[COOK_PHASE_CONSIDERABLE] = cook_phase_stats{};
+    return COOK_OK;
+  }
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  const bool masks = !prm->quota_only;
+  const bool al = masks && S->nflag[F_NOT_ALLOWED] > 0, pl = masks && S->nflag[F_NOT_PLUGIN] > 0;
+  const int R = (int)S->run.slot_of.size();
+  const int NC = std::min(prm->num_considerable, nq);
+  const int32_t* tokens = prm->enforce_rate_limit ? users->tokens : nullptr;
+  // ---- one carve, sized by the queue: the rows, M0's scratch, the user columns (uploaded), the derived usage
+  ConsRows r;
+  r.n_users = U;
+  int32_t *m_slot = nullptr, *qpos = nullptr, *blk = nullptr;
+  int64_t* d_jid = nullptr;
+  double* usage = nullptr;
+  UsageFold f;
+  f.R = R; f.U = U;
+  const bool fold = src == COOK_USAGE_DERIVED && R > 0;
+  int64_t h2d = 0, d2h = 0;
+  CK(pool, carve(S->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+    m_slot = c.take<int32_t>(nq); qpos = c.take<int32_t>(nq);
+    blk = c.take<int32_t>((size_t)nq / CP_BLOCK + 2);
+    r.ranked = c.take<int32_t>(nq); r.user = c.take<int32_t>(nq);
+    r.cpus = c.take<double>(nq); r.mem = c.take<double>(nq); r.gpus = c.take<double>(nq);
+    r.allowed = al ? c.take<uint8_t>(nq) : nullptr;
+    r.plugin = pl ? c.take<uint8_t>(nq) : nullptr;
+    r.pos = c.take<int32_t>(nq + 1); r.tmp = c.take<int32_t>(nq + 1);
+    r.seg_s = c.take<int32_t>(U + 1); r.seg_e = c.take<int32_t>(U + 1);
+    r.keep = c.take<uint8_t>(nq + 1);
+    r.gf = c.take<GridFlag>(1);
+    r.out_row = c.take<int32_t>(NC);
+    d_jid = c.take<int64_t>(NC);
+    for (int k = 0; k < 4; k++) r.quota[k] = c.up(quota[k], U);
+    if (tokens) r.tokens = c.up(tokens, U);
+    if (src == COOK_USAGE_GIVEN) {
+      for (int k = 0; k < 4; k++) r.usage[k] = c.up(given[k], U);
+    } else if (src == COOK_USAGE_DERIVED) {
+      usage = c.take<double>(4 * (size_t)U);
+      if (fold) f.take(c, S->run.hw);
+    }
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  int nl = 0;
+  // ---- the live queue with its positions, its length downloaded
+  const QueueLive ql{S->q_slot, S->q_gen, S->pend.at<uint8_t>(P_LIVE), S->pend.at<uint32_t>(P_GEN), m_slot};
+  compact(QueueLivePos{ql, qpos}, nq, nullptr, blk, S->counters + 2, nq, st, &nl);
+  CK(pool, cudaGetLastError());
+  int32_t n = 0;
+  CK(pool, download(&n, S->counters + 2, 1, st, &d2h));
+  CK(pool, cudaStreamSynchronize(st));
+  int32_t n_out = 0;
+  if (n > 0) {
+    // ---- the rows' columns, the usage, M0, the ids (and the consumption)
+    cons_rows_kernel<<<(n + 255) / 256, 256, 0, st>>>(S->pend.d_col, m_slot, n, writable(r.ranked), writable(r.user),
+                                                      writable(r.cpus), writable(r.mem), writable(r.gpus),
+                                                      writable(r.allowed), writable(r.plugin));
+    nl++;
+    if (src == COOK_USAGE_DERIVED) {
+      if (fold) {
+        f.a.user_out = usage;
+        CK(pool, f.run(S, st, &nl));
+      } else {
+        CK(pool, cudaMemsetAsync(usage, 0, sizeof(double) * 4 * (size_t)U, st));
+      }
+      for (int k = 0; k < 4; k++) r.usage[k] = usage + (size_t)k * U;
+    } else if (src == COOK_USAGE_LAST_MATCH) {
+      for (int k = 0; k < 4; k++) r.usage[k] = last[k];
+    }
+    r.n = n;
+    r.enforce_rate_limit = prm->enforce_rate_limit;
+    r.pool_q = pool_quota ? *pool_quota : cook_pool_quota{0, 0, 0, 0, 0};
+    r.num_considerable = NC;
+    r.out_n = S->counters + 4;
+    CK(pool, considerable_rows(r, st, &nl));
+    cons_take_kernel<<<(NC + 255) / 256, 256, 0, st>>>(r.out_row, r.out_n, qpos, S->q_jid, writable(S->q_gen),
+                                                       prm->consume ? 1 : 0, d_jid);
+    nl++;
+    CK(pool, cudaGetLastError());
+    CK(pool, cudaEventRecord(pool->ev[22], st));
+    CK(pool, download(&n_out, r.out_n, 1, st, &d2h));
+    CK(pool, cudaStreamSynchronize(st));
+    if (n_out > 0) CK(pool, download(out_job_id, d_jid, n_out, st, &d2h));
+  } else {
+    CK(pool, cudaEventRecord(pool->ev[22], st));
+  }
+  CK(pool, cudaEventRecord(pool->ev[23], st));
+  CK(pool, cudaStreamSynchronize(st));
+  record_phase(pool, COOK_PHASE_CONSIDERABLE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[23], h2d, d2h, nl);
+  *out_n = n_out;
+  return COOK_OK;
+}
+
 }  // namespace
+
+extern "C" int32_t cook_state_rank(cook_pool* pool, const cook_user_table* users, const cook_pool_quota* pool_quota,
+                                   const cook_pool_quota* group_quota, const double* group_usage,
+                                   const cook_rank_params* params, int64_t* out_ranked_job_id, int32_t* out_n) {
+  return state_rank(pool, "cook_state_rank", false, users, pool_quota, group_quota, group_usage, params,
+                    out_ranked_job_id, out_n, nullptr, 0, nullptr);
+}
+
+extern "C" int32_t cook_state_rank_offensive(cook_pool* pool, const cook_user_table* users,
+                                             const cook_pool_quota* pool_quota, const cook_pool_quota* group_quota,
+                                             const double* group_usage, const cook_rank_params* params,
+                                             int64_t* out_ranked_job_id, int32_t* out_n, int64_t* out_offensive_job_id,
+                                             int32_t offensive_cap, int32_t* out_n_offensive) {
+  return state_rank(pool, "cook_state_rank_offensive", true, users, pool_quota, group_quota, group_usage, params,
+                    out_ranked_job_id, out_n, out_offensive_job_id, offensive_cap, out_n_offensive);
+}
+
+extern "C" int32_t cook_state_considerable(cook_pool* pool, const cook_user_table* users,
+                                           const cook_pool_quota* pool_quota, const cook_considerable_params* params,
+                                           int64_t* out_job_id, int32_t* out_n) {
+  if (!pool) return COOK_E_BADARG;
+  return considerable(pool, static_cast<PoolState*>(pool->state), users, pool_quota, params, out_job_id, out_n);
+}
 
 extern "C" int32_t cook_state_match(cook_pool* pool, const cook_offers_soa* offers, const cook_groups* groups,
                                     const cook_user_table* users, const cook_pool_quota* pool_quota,

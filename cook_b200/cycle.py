@@ -251,3 +251,17 @@ def autoscalable_jobs(engine, queue_after_match, jobs, users, *, number_consider
                      pool_quota=pool_quota)
     skip = set(recent_synthetic_pod_jobs)
     return [int(j) for j in m["considerable"] if int(j) not in skip]
+
+
+def autoscalable_jobs_resident(engine, users, *, number_considerable, number_unmatched, max_jobs_for_autoscaling=1000,
+                               scale_factor=1.0, pool_quota=None, enforce_rate_limit=0, recent_synthetic_pod_jobs=()):
+    """autoscalable_jobs for a resident pool, after its cook_state_match(_derived) and the launches of the matched
+    jobs: the same selection by cook_state_considerable with quota_only over the resident queue (the launched jobs
+    have left it) and the usage the match read (COOK_USAGE_LAST_MATCH), so no job row or usage table crosses the bus.
+    The scaled maximum and the recent-synthetic-pod skip stay here.  Returns job ids."""
+    n = max_jobs_for_autoscaling_scaled(number_considerable, number_unmatched, max_jobs_for_autoscaling, scale_factor)
+    if n <= 0:
+        return []
+    prm = abi.ConsiderableParams(n, int(enforce_rate_limit), 1, abi.USAGE_LAST_MATCH, 0)
+    skip = set(recent_synthetic_pod_jobs)
+    return [int(j) for j in engine.state_considerable(users, prm, pool_quota=pool_quota) if int(j) not in skip]

@@ -63,7 +63,8 @@ def load_library(path=None):
                  "cook_comm_destroy", "cook_exchange_usage", "cook_exchange_usage_batch", "cook_rebalance_trace",
                  "cook_match_failures", "cook_state_apply", "cook_state_rank", "cook_state_match",
                  "cook_state_rebalance", "cook_state_launch", "cook_state_patch", "cook_state_usage",
-                 "cook_state_cotasks", "cook_state_match_derived", "cook_state_rebalance_derived"):
+                 "cook_state_cotasks", "cook_state_match_derived", "cook_state_rebalance_derived",
+                 "cook_state_considerable", "cook_state_rank_offensive"):
         getattr(lib, name).restype = C.c_int32
     for name, argtypes in abi.ARGTYPES.items():
         getattr(lib, name).argtypes = argtypes
@@ -260,16 +261,38 @@ class GpuEngine:
             self._err(rc)
         return off, host[:n.value], val[:n.value]
 
-    def state_rank(self, users, pool_quota=None, group_quota=None, group_usage=None, params=None):
-        """cook_state_rank: the live rows ranked; the queue stays on the device.  Returns its job ids."""
+    def state_rank(self, users, pool_quota=None, group_quota=None, group_usage=None, params=None, offensive=False):
+        """cook_state_rank: the live rows ranked; the queue stays on the device.  Returns its job ids.
+        offensive: cook_state_rank_offensive, returns (queue job ids, the job ids the rank dropped as offensive)."""
         pool_quota = pool_quota or abi.make_pool_quota(None)
         group_quota = group_quota or abi.make_pool_quota(None)
         params = params or abi.RankParams(100, 0, 0.0, 0.0)
         gu = np.ascontiguousarray(group_usage if group_usage is not None else np.zeros(4), np.float64)
-        out = np.zeros(max(len(getattr(self, "_state_pending_ids", ())), 1), np.int64)
+        n_live = len(getattr(self, "_state_pending_ids", ()))
+        out = np.zeros(max(n_live, 1), np.int64)
         n = C.c_int32(0)
-        rc = self.lib.cook_state_rank(self.pool, C.byref(users), C.byref(pool_quota), C.byref(group_quota),
-                                      abi.ptr(gu, abi.P_F64), C.byref(params), abi.ptr(out, abi.P_I64), C.byref(n))
+        args = (self.pool, C.byref(users), C.byref(pool_quota), C.byref(group_quota), abi.ptr(gu, abi.P_F64),
+                C.byref(params), abi.ptr(out, abi.P_I64), C.byref(n))
+        if not offensive:
+            rc = self.lib.cook_state_rank(*args)
+            if rc != 0:
+                self._err(rc)
+            return out[:n.value].copy()
+        off = np.zeros(max(n_live, 1), np.int64)
+        n_off = C.c_int32(0)
+        rc = self.lib.cook_state_rank_offensive(*args, abi.ptr(off, abi.P_I64), n_live, C.byref(n_off))
+        if rc != 0:
+            self._err(rc)
+        return out[:n.value].copy(), off[:n_off.value].copy()
+
+    def state_considerable(self, users, params, pool_quota=None):
+        """cook_state_considerable: M0 over the resident queue without a match (params: abi.ConsiderableParams).
+        Returns the job ids in take order; with params.consume they leave the queue until the next state_rank."""
+        pool_quota = pool_quota or abi.make_pool_quota(None)
+        out = np.zeros(max(int(params.num_considerable), 1), np.int64)
+        n = C.c_int32(0)
+        rc = self.lib.cook_state_considerable(self.pool, C.byref(users), C.byref(pool_quota), C.byref(params),
+                                              abi.ptr(out, abi.P_I64), C.byref(n))
         if rc != 0:
             self._err(rc)
         return out[:n.value].copy()

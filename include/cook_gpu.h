@@ -507,6 +507,19 @@ int32_t cook_state_rank(cook_pool* pool, const cook_user_table* users, const coo
                         const cook_pool_quota* group_quota, const double* group_usage,
                         const cook_rank_params* params, int64_t* out_ranked_job_id, int32_t* out_n);
 
+/* cook_state_rank plus the jobs filter-offensive-jobs (scheduler.clj:2198-2229) puts on offensive-jobs-ch: the jobs
+ * that survived the rank's quota filters (limit-over-quota, pool and group quota) and are offensive (mem >
+ * offensive_max_mem_mb or cpus > offensive_max_cpus), in rank order, as job ids in
+ * out_offensive_job_id[*out_n_offensive].  Empty when params->filter_offensive is 0; a job a quota cut first is not
+ * listed.  The queue, out_ranked_job_id and *out_n are bit-identical to cook_state_rank's.  COOK_E_BADARG, before
+ * any device work: every case cook_state_rank rejects, a NULL out_offensive_job_id or out_n_offensive, and
+ * offensive_cap < the number of live pending rows.  Transfers: cook_state_rank's, plus 4 bytes (the count, when a
+ * row is live) and 8 per offensive job down.  Statistics: cook_last_stats(COOK_PHASE_RANK).                     */
+int32_t cook_state_rank_offensive(cook_pool* pool, const cook_user_table* users, const cook_pool_quota* pool_quota,
+                                  const cook_pool_quota* group_quota, const double* group_usage,
+                                  const cook_rank_params* params, int64_t* out_ranked_job_id, int32_t* out_n,
+                                  int64_t* out_offensive_job_id, int32_t offensive_cap, int32_t* out_n_offensive);
+
 /* cook_match with ranked_idx = the resident queue minus every job removed or replaced since that
  * cook_state_rank, reading the rows' current columns (what cook_state_patch wrote since the rank counts).
  * Outputs as cook_match, with the job id of the k-th considerable job in out_considerable_job_id[k];
@@ -635,6 +648,45 @@ int32_t cook_state_rebalance_derived(cook_pool* pool, const cook_host_table* hos
                                      cook_decision* out_decisions, int64_t* out_decision_job_id,
                                      int64_t* out_victim_task_id, int32_t victim_cap, int32_t* out_n);
 
+/* M0 over the resident queue without a match: pending-jobs->considerable-jobs (scheduler.clj:729-762; the jobs
+ * handle-kubernetes-scheduler-pool :1749-1800 launches) or, with quota_only, filter-pending-jobs-for-quota
+ * (tools.clj:961-973; what handle-resource-offers-autoscaling-helper :1283-1335 takes).
+ *   Queue    the queue cook_state_match reads: the last cook_state_rank's, minus every entry whose slot was removed or
+ *            replaced since, and minus the entries an earlier consuming call took.  Each row's current allowed and
+ *            plugin_accept are read (cook_state_patch counts).
+ *   Result   out_job_id[*out_n] (room for num_considerable) in take order: bit-identical to the considerable set of
+ *            cook_match on host tables holding the same rows, in queue order, with an empty offer table (quota_only:
+ *            allowed and plugin_accept all ones).  Folds as there: per user a left fold in queue order, the pool
+ *            quota over users 0 .. n_users - 1 of the selected usage.  Does not depend on slot layout.
+ *   Usage    usage_source: COOK_USAGE_GIVEN reads users->usage_*; COOK_USAGE_DERIVED folds them on the device from
+ *            the live running rows (what cook_state_usage(n_users, ...) returns now; usage_* not read);
+ *            COOK_USAGE_LAST_MATCH takes the [4][n_users] usage the last cook_match / cook_state_match(_derived) on
+ *            this handle read (usage_* not read): the cycle-start usage the autoscaling helper reuses after the
+ *            match's launches.
+ *   Consume  consume != 0: the returned entries leave the queue until the next cook_state_rank, which brings back
+ *            those still pending; their rows stay live and unchanged (counts, usage, cotasks, cook_state_launch).
+ * Reads users' quota_* (and tokens when enforcing) always.  Builds no match plan: cook_match_failures,
+ * cook_exchange_usage(_batch) and COOK_USAGE_LAST_MATCH still refer to the last match.
+ * COOK_E_BADARG, before any device work with the queue unchanged and nothing written: no cook_state_rank yet; a NULL
+ * users, params, out_job_id, out_n or quota_* column (usage_* too for GIVEN); a live pending row's user code >=
+ * n_users (and a live running row's for DERIVED); LAST_MATCH with no match on the handle or one with another
+ * n_users; an unknown usage_source.  num_considerable <= 0 or an empty queue: *out_n = 0 without device work.
+ * Transfers exactly: up 32 * n_users (quotas) + 4 * n_users (tokens, when enforcing and given) + 32 * n_users (usage,
+ * GIVEN only); down 4 (the live queue's length) and, when that is not 0, 4 (*out_n) + 8 * *out_n.
+ * Statistics: cook_last_stats(COOK_PHASE_CONSIDERABLE); all zero after a call without device work.            */
+enum { COOK_USAGE_GIVEN = 0, COOK_USAGE_DERIVED = 1, COOK_USAGE_LAST_MATCH = 2 };
+typedef struct {
+  int32_t num_considerable;   /* take N; <= 0 => *out_n = 0, no device work                                        */
+  int32_t enforce_rate_limit; /* as cook_match_params                                                              */
+  int32_t quota_only;         /* 1: filter-pending-jobs-for-quota only (autoscaling): allowed and plugin_accept are
+                                 not read.  0: pending-jobs->considerable-jobs                                       */
+  int32_t usage_source;       /* COOK_USAGE_*: where users->usage_* come from                                      */
+  int32_t consume;            /* 1: the returned jobs leave the resident queue until the next cook_state_rank
+                                 (handle-kubernetes-scheduler-pool)                                                */
+} cook_considerable_params;
+int32_t cook_state_considerable(cook_pool* pool, const cook_user_table* users, const cook_pool_quota* pool_quota,
+                                const cook_considerable_params* params, int64_t* out_job_id, int32_t* out_n);
+
 /* ------------------------------------------------------------ phase timing */
 /* Device-side timing of the last call of each kind on this handle (CUDA events on the
  * pool's stream): what bench.py's `phases` block and roofline lines are computed from.
@@ -642,9 +694,11 @@ int32_t cook_state_rebalance_derived(cook_pool* pool, const cook_host_table* hos
  * scatter / move / compaction kernels).  COOK_PHASE_USAGE: the last cook_state_usage (upload of the
  * hostname list, the compaction, sorts and folds, the download of the sums).  COOK_PHASE_COTASKS: the last
  * cook_state_cotasks (upload of the host codes, attribute columns and group map, the compaction, expansion and
- * sort, the download of the lists; all zero after a call without device work). */
+ * sort, the download of the lists; all zero after a call without device work).  COOK_PHASE_CONSIDERABLE: the last
+ * cook_state_considerable (upload of the user columns, the queue compaction and gathers, the usage fold when derived,
+ * the considerable pass and the consumption, the download of the ids). */
 enum { COOK_PHASE_RANK = 0, COOK_PHASE_MATCH = 1, COOK_PHASE_REBALANCE = 2, COOK_PHASE_EXCHANGE = 3,
-       COOK_PHASE_STATE = 4, COOK_PHASE_USAGE = 5, COOK_PHASE_COTASKS = 6 };
+       COOK_PHASE_STATE = 4, COOK_PHASE_USAGE = 5, COOK_PHASE_COTASKS = 6, COOK_PHASE_CONSIDERABLE = 7 };
 typedef struct {
   double ms_h2d;      /* upload stage                                              */
   double ms_device;   /* kernels (for the exchange: delta kernels + the collective) */

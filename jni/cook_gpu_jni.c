@@ -222,6 +222,41 @@ JFN(jint, stateRank)(JNIEnv* env, jclass k, jlong pool, jint n_users, jobjectArr
   (*env)->SetIntArrayRegion(env, out_n, 0, 1, (jint*)&n);
   return rc;
 }
+/* stateRank plus the jobs the rank dropped as offensive (filter-offensive-jobs), as job ids in out_offensive_job_id
+ * (room for offensive_cap >= the live pending rows) and their number in out_n_offensive[0] */
+JFN(jint, stateRankOffensive)(JNIEnv* env, jclass k, jlong pool, jint n_users, jobjectArray users,
+                              jdoubleArray pool_quota, jdoubleArray group_quota, jobject group_usage,
+                              jint max_over_quota_jobs, jint filter_offensive, jdouble off_mem_mb, jdouble off_cpus,
+                              jobject out_ranked_job_id, jintArray out_n, jobject out_offensive_job_id,
+                              jint offensive_cap, jintArray out_n_offensive) {
+  cook_user_table u; cook_pool_quota pq, gq; cook_rank_params prm;
+  memset(&u, 0, sizeof(u));
+  users_from(env, n_users, users, &u); quota_from(env, pool_quota, &pq); quota_from(env, group_quota, &gq);
+  prm.max_over_quota_jobs = max_over_quota_jobs; prm.filter_offensive = filter_offensive;
+  prm.offensive_max_mem_mb = off_mem_mb; prm.offensive_max_cpus = off_cpus;
+  int32_t n = 0, n_off = 0;
+  jint rc = cook_state_rank_offensive((cook_pool*)(intptr_t)pool, &u, &pq, &gq, one(env, group_usage), &prm,
+                                      one(env, out_ranked_job_id), &n, one(env, out_offensive_job_id), offensive_cap,
+                                      &n_off);
+  (*env)->SetIntArrayRegion(env, out_n, 0, 1, (jint*)&n);
+  (*env)->SetIntArrayRegion(env, out_n_offensive, 0, 1, (jint*)&n_off);
+  return rc;
+}
+/* M0 over the resident queue without a match; iparams = {num_considerable, enforce_rate_limit, quota_only,
+ * usage_source, consume} (cook_considerable_params); the job ids go to out_job_id, their number to out_n[0] */
+JFN(jint, stateConsiderable)(JNIEnv* env, jclass k, jlong pool, jint n_users, jobjectArray users,
+                             jdoubleArray pool_quota, jintArray iparams, jobject out_job_id, jintArray out_n) {
+  cook_user_table u; cook_pool_quota pq; cook_considerable_params prm;
+  memset(&u, 0, sizeof(u));
+  users_from(env, n_users, users, &u); quota_from(env, pool_quota, &pq);
+  jint ip[5]; (*env)->GetIntArrayRegion(env, iparams, 0, 5, ip);
+  prm.num_considerable = ip[0]; prm.enforce_rate_limit = ip[1]; prm.quota_only = ip[2]; prm.usage_source = ip[3];
+  prm.consume = ip[4];
+  int32_t n = 0;
+  jint rc = cook_state_considerable((cook_pool*)(intptr_t)pool, &u, &pq, &prm, one(env, out_job_id), &n);
+  (*env)->SetIntArrayRegion(env, out_n, 0, 1, (jint*)&n);
+  return rc;
+}
 typedef int32_t (*state_match_fn)(cook_pool*, const cook_offers_soa*, const cook_groups*, const cook_user_table*,
                                   const cook_pool_quota*, const cook_match_params*, int64_t*, int32_t*, int32_t*, int32_t,
                                   uint8_t*, cook_match_stats*);

@@ -51,6 +51,15 @@ identical.  The placed jobs are then launched on their hosts and 3 % of the runn
   python tools/prof_state.py --derived --pool c2 --cycles 6
   python tools/prof_state.py --derived --pool c5 --c5-pool 5 --cycles 4
   python tools/prof_state.py --derived --c3-pool 0 --cycles 4      # a config-#3 pool with groups
+
+--considerable loads the pool's pending jobs and running tasks into a resident handle, ranks it, and per cycle runs
+cook_state_considerable (the users' usage given, all of the queue considerable) against cook_match on host tables
+holding the same rows in queue order with an empty offer table: the considerable set alone.  Per arm it prints the
+device time, the host wall time of the library call, the bytes up and down, and whether the two sets are identical;
+each cycle runs pending-jobs->considerable-jobs and, with quota_only, the autoscaling filter.
+
+  python tools/prof_state.py --considerable --pool c2 --cycles 5
+  python tools/prof_state.py --considerable --pool c5 --c5-pool 5 --cycles 5
 """
 import argparse
 import json
@@ -432,6 +441,57 @@ def launch_cycle(cycle, res, twin, job_id, lt, hosts, rest, match_args):
     return m1["considerable"][ok], offers.col("hostname_id")[m1["assign"][ok]].astype(np.int32)
 
 
+def considerable_prof(a):
+    t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
+    jobs, pc, rc, users = t["jobs"], t["cols"]["pending"], t["cols"]["running"], t["users"]
+    J = jobs.n
+    print(json.dumps({"card": card(), "pool": a.pool if a.pool == "c2" else f"c5/{a.c5_pool}", "jobs": J,
+                      "running": len(rc["task_id"]), "users": users.n_users}), flush=True)
+    store = Jobs(jobs, pc["priority"], pc["job_id"])
+    rows = np.arange(J)
+    res, host = GpuEngine(pool_name="resident"), GpuEngine(pool_name="host")
+    res.state_apply(abi.make_delta(reset=True, running=abi.make_tasks(**{k: np.asarray(v) for k, v in rc.items()}),
+                                   pending=store.soa(rows), pending_priority=store.prio, pending_job_id=store.jid))
+    q = res.state_rank(users)
+    pos = {int(j): i for i, j in enumerate(store.jid)}
+    ranked = np.array([pos[int(j)] for j in q], np.int32)
+    empty = abi.OffersSoA(n=0, hostname_id=np.zeros(1, np.int32), name_rank=np.zeros(1, np.int32), cpus=np.zeros(1),
+                          mem=np.zeros(1), run_cpus=np.zeros(1), run_mem=np.zeros(1), run_count=np.zeros(1, np.int32),
+                          n_attr_cols=0)
+    hj = store.soa(rows)
+    ones = np.ones(J, np.uint8)
+    plain = abi.JobsSoA(n=J, user=hj.col("user"), cpus=hj.col("cpus"), mem=hj.col("mem"), gpus=hj.col("gpus"),
+                        allowed=hj.col("allowed") if hj.col("allowed") is not None else ones,
+                        plugin_accept=hj.col("plugin_accept") if hj.col("plugin_accept") is not None else ones)
+    auto = abi.JobsSoA(n=J, user=hj.col("user"), cpus=hj.col("cpus"), mem=hj.col("mem"), gpus=hj.col("gpus"),
+                       allowed=ones, plugin_accept=ones)
+    nc = max(len(q), 1)
+    for cycle in range(a.cycles):
+        for quota_only in (0, 1):
+            prm = abi.ConsiderableParams(nc, 0, quota_only, abi.USAGE_GIVEN, 0)
+            w0 = time.perf_counter()
+            got = res.state_considerable(users, prm)
+            w_res = time.perf_counter() - w0
+            st = res.last_stats(abi.PHASE_CONSIDERABLE)
+            w0 = time.perf_counter()
+            mh = host.match(ranked, auto if quota_only else plain, empty, users, traces.match_params(nc))
+            w_host = time.perf_counter() - w0
+            hs = mh["stats"]
+            same = np.array_equal(got, store.jid[mh["considerable"]])
+            print(json.dumps({"cycle": cycle, "quota_only": quota_only, "considerable": len(got),
+                              "resident": {"ms_h2d": round(st["ms_h2d"], 3), "ms_device": round(st["ms_device"], 3),
+                                           "ms_d2h": round(st["ms_d2h"], 3), "wall_ms": round(1e3 * w_res, 3),
+                                           "h2d_bytes": st["h2d_bytes"], "d2h_bytes": st["d2h_bytes"],
+                                           "n_launches": st["n_launches"]},
+                              "host": {"ms_h2d": round(hs["ms_h2d"], 3), "ms_considerable": round(hs["ms_considerable"], 3),
+                                       "ms_d2h": round(hs["ms_d2h"], 3), "wall_ms": round(1e3 * w_host, 3),
+                                       "h2d_bytes": hs["h2d_bytes"], "d2h_bytes": hs["d2h_bytes"],
+                                       "n_launches": hs["n_launches"]},
+                              "identical": bool(same)}), flush=True)
+    res.close()
+    host.close()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--pool", choices=("c2", "c5"), default="c2")
@@ -447,7 +507,10 @@ def main():
                     help="--cotasks: a config-#3 pool (-1: the smaller c3-shaped pool); --derived: a config-#3 pool "
                          "instead of --pool")
     ap.add_argument("--derived", action="store_true")
+    ap.add_argument("--considerable", action="store_true")
     a = ap.parse_args()
+    if a.considerable:
+        return considerable_prof(a)
     if a.rebalance:
         return rebalance(a)
     if a.usage:
