@@ -210,6 +210,32 @@
           "cook_state_considerable")
   (let [lb (.asLongBuffer out)] (mapv #(.get lb (int %)) (range (aget out-n 0)))))
 
+;; cook_fp as 24 bytes of a little-endian direct buffer
+(defn- fp-at [^ByteBuffer b i] [(.getLong b (* 24 i)) (.getLong b (+ 8 (* 24 i))) (.getLong b (+ 16 (* 24 i)))])
+
+(defn audit-resident!
+  "Proves a resident pool equal to the database, or says where it is not (cook_state_digest, then cook_state_export
+   of the differing buckets).  `host-buckets` is {:pending [[sum xor n] ...] :running [...]}, the host's own bucket
+   fingerprints of its rows (the hash is stated in cook_gpu.h); `out`, `out-p`, `out-r` are the direct buffers of
+   Native/stateDigest.  Returns nil when every bucket agrees, else {:buckets [...] :consistent? bool}: the caller
+   exports those buckets (Native/stateExport with a mask of them), removes the exported ids it does not have and
+   upserts its own rows of those buckets in one apply!."
+  [handle n-buckets host-buckets ^ByteBuffer out ^ByteBuffer out-p ^ByteBuffer out-r]
+  (check! handle (Native/stateDigest handle n-buckets out out-p out-r) "cook_state_digest")
+  (let [differs? (fn [^ByteBuffer b want] (fn [i] (not= (fp-at b i) (nth want i))))
+        bad (into (sorted-set)
+                  (concat (filter (differs? out-p (:pending host-buckets)) (range n-buckets))
+                          (filter (differs? out-r (:running host-buckets)) (range n-buckets))))]
+    (when (seq bad)
+      {:buckets (vec bad) :consistent? (= 1 (.getInt out 104))})))
+
+(defn queue-resident
+  "The live queue of a resident pool as job ids (cook_state_queue): what the /queue endpoint reads between two ranks,
+   after the launches, removals, replacements and consumed jobs since the rank.  `out` holds `cap` longs."
+  [handle cap ^ByteBuffer out ^ints out-n]
+  (check! handle (Native/stateQueue handle cap out out-n) "cook_state_queue")
+  (let [lb (.asLongBuffer out)] (mapv #(.get lb (int %)) (range (aget out-n 0)))))
+
 (defn rebalance-derived!
   "cook_state_rebalance_derived: the rebalancer over the resident rows with the groups' cotask lists derived on the
    device over the host table in `args` (Native/stateRebalance's arguments after the handle)."

@@ -141,6 +141,7 @@ class PhaseStats(C.Structure):
 
 PHASE_RANK, PHASE_MATCH, PHASE_REBALANCE, PHASE_EXCHANGE, PHASE_STATE, PHASE_USAGE, PHASE_COTASKS = 0, 1, 2, 3, 4, 5, 6
 PHASE_CONSIDERABLE = 7
+PHASE_AUDIT = 8
 
 USAGE_GIVEN, USAGE_DERIVED, USAGE_LAST_MATCH = 0, 1, 2
 
@@ -175,6 +176,52 @@ def make_delta(reset=False, pending=None, pending_priority=None, pending_job_id=
                       n_running_rm=len(rrm), running_rm_task_id=rrm if len(rrm) else None,
                       running_hostname_id=running_hostname_id, running_group_off=running_group_off,
                       running_group_idx=running_group_idx)
+
+
+class Fp(C.Structure):
+    """cook_fp: the fingerprint of a set of rows."""
+    _fields_ = [("sum", C.c_uint64), ("xr", C.c_uint64), ("n", C.c_int64)]
+
+    def as_tuple(self):
+        return (self.sum, self.xr, self.n)
+
+
+FP_DTYPE = np.dtype([("sum", np.uint64), ("xr", np.uint64), ("n", np.int64)])   # a cook_fp array
+
+# COOK_AUDIT_*: the counts cook_state_digest recounts, by index
+AUDIT_NAMES = (["pending_rows", "running_rows", "entries_novel", "entries_attr", "entries_group", "entries_running_group"]
+               + ["flag_" + f for f in ("gpus", "ports", "not_allowed", "not_plugin", "gpu_model", "disk", "est_end_ms",
+                                        "ckpt_location", "reserved_host")]
+               + ["reserved_rows", "cot_rows", "cot_entries", "max_user_pending", "max_user_running",
+                  "max_group_pending", "max_group_running", "max_attr_col", "max_hostname_running"])
+AUDIT_N = len(AUDIT_NAMES)
+
+
+class StateDigest(C.Structure):
+    """cook_state_digest_out."""
+    _fields_ = [("pending", Fp), ("running", Fp), ("queue", Fp), ("entries", C.c_int64 * 4),
+                ("consistent", C.c_int32), ("first_mismatch", C.c_int32)]
+
+
+class JobsRows(_SoA):
+    """cook_jobs_rows: cook_jobs_soa's columns, writable."""
+    _fields_ = [(n, t) for n, t in JobsSoA._fields_ if n != "n"]
+
+
+class TasksRows(_SoA):
+    _fields_ = [(n, t) for n, t in TasksSoA._fields_ if n != "n"]
+
+
+class StateRows(_SoA):
+    """cook_state_rows: where cook_state_export writes the rows."""
+    _fields_ = [("pending", JobsRows), ("pending_priority", P_I32), ("pending_job_id", P_I64),
+                ("running", TasksRows), ("running_hostname_id", P_I32), ("running_group_off", P_I32),
+                ("running_group_idx", P_I32)]
+
+
+class StateSizes(C.Structure):
+    """cook_state_sizes: rows per table, entries per list (novel, attr, group, running group)."""
+    _fields_ = [("pending", C.c_int32), ("running", C.c_int32), ("entries", C.c_int32 * 4)]
 
 
 class RunningSoA(_SoA):
@@ -238,6 +285,11 @@ ARGTYPES = {
     "cook_state_rebalance_derived": _STATE_REBALANCE,
     "cook_state_considerable": [C.c_void_p, C.POINTER(UserTable), C.POINTER(PoolQuota), C.POINTER(ConsiderableParams),
                                 P_I64, P_I32],
+    "cook_state_digest": [C.c_void_p, C.c_int32, C.POINTER(StateDigest), C.POINTER(Fp), C.POINTER(Fp)],
+    "cook_state_counts_compare": [P_I64, P_I64, P_I32],
+    "cook_state_export": [C.c_void_p, C.c_int32, P_U8, C.POINTER(StateSizes), C.POINTER(StateRows),
+                          C.POINTER(StateSizes)],
+    "cook_state_queue": [C.c_void_p, C.c_int32, P_I64, P_I32],
     "cook_state_rank_offensive": [C.c_void_p, C.POINTER(UserTable), C.POINTER(PoolQuota), C.POINTER(PoolQuota), P_F64,
                                   C.POINTER(RankParams), P_I64, P_I32, P_I64, C.c_int32, P_I32],
 }

@@ -122,8 +122,8 @@ struct cook_pool {
   int sm_count = 0;
   cudaStream_t stream = nullptr;
   cudaEvent_t ev[24] = {};
-  cook_phase_stats phase[8] = {};        // last rank / match / rebalance / exchange / state-apply / usage / cotasks /
-                                         // considerable call
+  cook_phase_stats phase[9] = {};        // last rank / match / rebalance / exchange / state-apply / usage / cotasks /
+                                         // considerable / audit call
   double* xchg = nullptr;                // exchange buffers: [n_pad] local + [world * n_pad] gathered
   size_t xchg_cap = 0;
   Arena arena;

@@ -1980,3 +1980,551 @@ extern "C" int32_t cook_state_rebalance_derived(cook_pool* pool, const cook_host
   return state_rebalance(pool, "cook_state_rebalance_derived", true, hosts, groups, users, params, out_decisions,
                          out_decision_job_id, out_victim_task_id, victim_cap, out_n);
 }
+
+// ---- audit: the read side (cook_state_digest, cook_state_export, cook_state_queue).  The digest is one pass per
+// table: a thread hashes its slot's columns and short lists, a long list is read by the warp and absorbed by the
+// owning lane; fingerprints and counts are reduced per warp with shuffles, per block in shared memory, then one
+// atomic per block and word.  The export compacts the live (and selected) slots, sorts them by id, gathers the
+// requested columns and rebuilds each list as CSR with the match's own csr_gather_kernel.  All of it lives in
+// `scratch`: the queue arena and the match plan are only read.
+namespace {
+
+__device__ __forceinline__ uint64_t fp_mix(uint64_t z) {
+  z ^= z >> 30; z *= 0xbf58476d1ce4e5b9ULL;
+  z ^= z >> 27; z *= 0x94d049bb133111ebULL;
+  return z ^ (z >> 31);
+}
+__device__ __forceinline__ uint64_t fp_absorb(uint64_t h, uint64_t w) { return fp_mix((h ^ w) + 0x9e3779b97f4a7c15ULL); }
+__device__ __forceinline__ uint64_t fp_i32(int32_t x) { return (uint64_t)(int64_t)x; }
+
+// what a digest downloads: the fingerprints of the pending rows, the running rows and the queue, then the recount
+// (a maximum is kept as code + 1, so that zero is "none")
+struct AuditDev {
+  cook_fp fp[3];
+  long long c[COOK_AUDIT_N];
+};
+constexpr int AUDIT_SUMS_P = 4 + F_N, AUDIT_SUMS_R = 4, AUDIT_MAXS = 3;
+constexpr int AUDIT_SHORT = 8;        // a list up to this long is absorbed by its own thread
+constexpr int AUDIT_SHARED_BUCKETS = 1024;   // up to this many buckets are reduced per block in shared memory
+
+// the COOK_AUDIT_* index of a table pass's k-th sum and k-th maximum
+__device__ __forceinline__ int audit_sum_index(bool pend, int k) {
+  if (pend) return k == 0 ? (int)COOK_AUDIT_PENDING_ROWS : k < 4 ? COOK_AUDIT_ENTRIES + k - 1 : COOK_AUDIT_FLAGS + k - 4;
+  return k == 0 ? (int)COOK_AUDIT_RUNNING_ROWS : k == 1 ? COOK_AUDIT_ENTRIES + L_RGROUP
+         : k == 2 ? (int)COOK_AUDIT_COT_ROWS : (int)COOK_AUDIT_COT_ENTRIES;
+}
+__device__ __forceinline__ int audit_max_index(bool pend, int k) {   // user, group, then attribute column / hostname
+  if (pend) return k == 0 ? COOK_AUDIT_MAX_USER_PENDING : k == 1 ? COOK_AUDIT_MAX_GROUP_PENDING : COOK_AUDIT_MAX_ATTR_COL;
+  return k == 0 ? COOK_AUDIT_MAX_USER_RUNNING : k == 1 ? COOK_AUDIT_MAX_GROUP_RUNNING : COOK_AUDIT_MAX_HOSTNAME_RUNNING;
+}
+
+struct AuditArgs {
+  void* const* col;            // the table's columns
+  int n;                       // slots ever used
+  const int32_t* v0[3];        // the arenas of the table's lists
+  const int32_t* v1[3];        // non-null: (v0, v1) pairs
+  AuditDev* out;
+  cook_fp* bucket;             // [nb], null: no buckets
+  unsigned nb;
+  int sb;                      // nb when the block reduces the buckets in shared memory, else 0
+};
+
+__device__ __forceinline__ void fp_add(cook_fp* f, uint64_t sum, uint64_t xr, long long n) {
+  atomicAdd(reinterpret_cast<unsigned long long*>(&f->sum), (unsigned long long)sum);
+  atomicXor(reinterpret_cast<unsigned long long*>(&f->xr), (unsigned long long)xr);
+  atomicAdd(reinterpret_cast<unsigned long long*>(&f->n), (unsigned long long)n);
+}
+
+// thread per slot of the pending (PEND) or running table
+template <bool PEND>
+__global__ void __launch_bounds__(256) audit_table_kernel(AuditArgs a) {
+  extern __shared__ unsigned long long s_bkt[];   // [3 * a.sb]: sum, xor, n per bucket
+  __shared__ unsigned long long s_fp[3];
+  __shared__ int s_sum[AUDIT_SUMS_P], s_max[AUDIT_MAXS];
+  constexpr int NS = PEND ? AUDIT_SUMS_P : AUDIT_SUMS_R, NL = PEND ? 3 : 1;
+  if (threadIdx.x < 3) s_fp[threadIdx.x] = 0;
+  if (threadIdx.x < AUDIT_SUMS_P) s_sum[threadIdx.x] = 0;
+  if (threadIdx.x < AUDIT_MAXS) s_max[threadIdx.x] = 0;
+  for (int b = threadIdx.x; b < 3 * a.sb; b += blockDim.x) s_bkt[b] = 0;
+  __syncthreads();
+  const int i = blockIdx.x * blockDim.x + threadIdx.x, lane = threadIdx.x & 31;
+  void* const* c = a.col;
+  const bool live = i < a.n && static_cast<const uint8_t*>(c[PEND ? (int)P_LIVE : (int)R_LIVE])[i];
+  uint64_t h = 0, id = 0;
+  int sum[NS], mx[AUDIT_MAXS] = {0, 0, 0};
+#pragma unroll
+  for (int k = 0; k < NS; k++) sum[k] = 0;
+  bool cot = false;
+  if (live) {
+    sum[0] = 1;
+    const auto i32 = [&](int k) { return static_cast<const int32_t*>(c[k])[i]; };
+    const auto i64 = [&](int k) { return static_cast<const long long*>(c[k])[i]; };   // doubles: the bits as stored
+    const auto u8 = [&](int k) { return static_cast<const uint8_t*>(c[k])[i]; };
+    if (PEND) {
+      id = (uint64_t)i64(P_JID);
+      h = fp_absorb(1, id);
+      const int32_t user = i32(P_USER), ports = i32(P_PORTS), model = i32(P_GPU_MODEL), ckpt = i32(P_CKPT),
+                    reserved = i32(P_RESERVED);
+      const long long gpus = i64(P_GPUS), disk = i64(P_DISK_REQ), est = i64(P_EST);
+      const uint8_t allowed = u8(P_ALLOWED), plugin = u8(P_PLUGIN);
+      h = fp_absorb(h, fp_i32(user)); h = fp_absorb(h, fp_i32(i32(P_PRIO)));
+      h = fp_absorb(h, (uint64_t)i64(P_CPUS)); h = fp_absorb(h, (uint64_t)i64(P_MEM)); h = fp_absorb(h, (uint64_t)gpus);
+      h = fp_absorb(h, fp_i32(ports)); h = fp_absorb(h, allowed); h = fp_absorb(h, plugin);
+      h = fp_absorb(h, fp_i32(model)); h = fp_absorb(h, (uint64_t)disk); h = fp_absorb(h, fp_i32(i32(P_DISK_TYPE)));
+      h = fp_absorb(h, (uint64_t)est); h = fp_absorb(h, fp_i32(ckpt)); h = fp_absorb(h, fp_i32(reserved));
+      mx[0] = user + 1;
+      const bool f[F_N] = {__longlong_as_double(gpus) != 0.0, ports != 0, !allowed, !plugin, model != -1,
+                           __longlong_as_double(disk) >= 0.0, est != -1, ckpt != -1, reserved != -1};
+#pragma unroll
+      for (int k = 0; k < F_N; k++) sum[4 + k] = f[k] ? 1 : 0;
+    } else {
+      id = (uint64_t)i64(R_TID);
+      h = fp_absorb(2, id);
+      const int32_t user = i32(R_USER), host = i32(R_HOST);
+      h = fp_absorb(h, fp_i32(user)); h = fp_absorb(h, fp_i32(i32(R_PRIO))); h = fp_absorb(h, (uint64_t)i64(R_START));
+      h = fp_absorb(h, (uint64_t)i64(R_JID)); h = fp_absorb(h, (uint64_t)i64(R_CPUS)); h = fp_absorb(h, (uint64_t)i64(R_MEM));
+      h = fp_absorb(h, (uint64_t)i64(R_GPUS)); h = fp_absorb(h, fp_i32(host));
+      mx[0] = user + 1; mx[2] = host + 1;
+      cot = host != -1;
+    }
+  }
+  // the lists: length, then the entries in order
+#pragma unroll
+  for (int l = 0; l < NL; l++) {
+    const int oc = PEND ? (l == 0 ? (int)P_NOFF : l == 1 ? (int)P_AOFF : (int)P_GOFF) : (int)R_GOFF;
+    const int len = live ? static_cast<const int32_t*>(c[oc + 1])[i] : 0;
+    const int off = live ? static_cast<const int32_t*>(c[oc])[i] : 0;
+    const int32_t* v0 = a.v0[l];
+    const int32_t* v1 = a.v1[l];
+    int m = 0;   // the largest first word + 1
+    if (live) h = fp_absorb(h, fp_i32(len));
+    if (len <= AUDIT_SHORT)
+      for (int e = 0; e < len; e++) {
+        const int32_t w = v0[off + e];
+        h = fp_absorb(h, fp_i32(w));
+        m = max(m, w + 1);
+        if (v1) h = fp_absorb(h, fp_i32(v1[off + e]));
+      }
+    unsigned longer = __ballot_sync(FULL_MASK, len > AUDIT_SHORT);
+    while (longer) {   // the warp reads the list, its owner absorbs it
+      const int src = __ffs(longer) - 1;
+      longer &= longer - 1;
+      const int o = __shfl_sync(FULL_MASK, off, src), n = __shfl_sync(FULL_MASK, len, src);
+      for (int base = 0; base < n; base += 32) {
+        const int e = base + lane, cnt = min(32, n - base);
+        const int32_t x0 = e < n ? v0[o + e] : 0, x1 = v1 && e < n ? v1[o + e] : 0;
+        for (int k = 0; k < cnt; k++) {
+          const int32_t w0 = __shfl_sync(FULL_MASK, x0, k), w1 = __shfl_sync(FULL_MASK, x1, k);
+          if (lane == src) {
+            h = fp_absorb(h, fp_i32(w0));
+            m = max(m, w0 + 1);
+            if (v1) h = fp_absorb(h, fp_i32(w1));
+          }
+        }
+      }
+    }
+    sum[1 + l] = len;
+    if (PEND && l == 1) mx[2] = m;
+    if (PEND ? l == 2 : l == 0) mx[1] = m;
+    if (!PEND && cot && len > 0) { sum[2] = 1; sum[3] = len; }
+  }
+  // ---- the warp's fingerprint and counts, then the block's, then one atomic per word
+  uint64_t hs = live ? h : 0, hx = hs;
+  for (int o = 16; o > 0; o >>= 1) {
+    hs += __shfl_xor_sync(FULL_MASK, hs, o);
+    hx ^= __shfl_xor_sync(FULL_MASK, hx, o);
+  }
+  const int nlive = __reduce_add_sync(FULL_MASK, sum[0]);
+  if (lane == 0 && nlive) {
+    atomicAdd(&s_fp[0], (unsigned long long)hs);
+    atomicXor(&s_fp[1], (unsigned long long)hx);
+    atomicAdd(&s_fp[2], (unsigned long long)nlive);
+  }
+#pragma unroll
+  for (int k = 0; k < NS; k++) {
+    const int v = __reduce_add_sync(FULL_MASK, sum[k]);
+    if (lane == 0 && v) atomicAdd(&s_sum[k], v);
+  }
+#pragma unroll
+  for (int k = 0; k < AUDIT_MAXS; k++) {
+    const int v = __reduce_max_sync(FULL_MASK, mx[k]);
+    if (lane == 0 && v) atomicMax(&s_max[k], v);
+  }
+  if (live && a.nb) {
+    const unsigned b = (unsigned)fp_mix(id) & (a.nb - 1u);
+    if (a.sb) {
+      atomicAdd(&s_bkt[3 * b], (unsigned long long)h);
+      atomicXor(&s_bkt[3 * b + 1], (unsigned long long)h);
+      atomicAdd(&s_bkt[3 * b + 2], 1ULL);
+    } else {
+      fp_add(a.bucket + b, h, h, 1);
+    }
+  }
+  __syncthreads();
+  const int t = threadIdx.x;
+  if (t == 0 && s_fp[2]) fp_add(&a.out->fp[PEND ? 0 : 1], s_fp[0], s_fp[1], (long long)s_fp[2]);
+  if (t >= 32 && t < 32 + NS && s_sum[t - 32])
+    atomicAdd(reinterpret_cast<unsigned long long*>(&a.out->c[audit_sum_index(PEND, t - 32)]), (unsigned long long)s_sum[t - 32]);
+  if (t >= 64 && t < 64 + AUDIT_MAXS && s_max[t - 64])
+    atomicMax(&a.out->c[audit_max_index(PEND, t - 64)], (long long)s_max[t - 64]);
+  for (int b = t; b < a.sb; b += blockDim.x)
+    if (s_bkt[3 * b + 2]) fp_add(a.bucket + b, s_bkt[3 * b], s_bkt[3 * b + 1], (long long)s_bkt[3 * b + 2]);
+}
+
+// the live queue's job ids, in queue order
+struct QueueIds {
+  QueueLive q; const int64_t* q_jid; int64_t* out;
+  __device__ bool keep(int k) const { return q.keep(k); }
+  __device__ void emit(int k, int d) const { out[d] = q_jid[k]; }
+};
+// position d < *n of the live queue: absorb(absorb(3, d), job id)
+__global__ void audit_queue_kernel(const int64_t* ids, const int32_t* n, cook_fp* out) {
+  const int d = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool on = d < *n;
+  uint64_t hs = on ? fp_absorb(fp_absorb(3, (uint64_t)d), (uint64_t)ids[d]) : 0, hx = hs;
+  for (int o = 16; o > 0; o >>= 1) {
+    hs += __shfl_xor_sync(FULL_MASK, hs, o);
+    hx ^= __shfl_xor_sync(FULL_MASK, hx, o);
+  }
+  const int c = __reduce_add_sync(FULL_MASK, on ? 1 : 0);
+  if ((threadIdx.x & 31) == 0 && c) fp_add(out, hs, hx, c);
+}
+
+// the counts the host side keeps, in COOK_AUDIT_* order
+void host_counts(const PoolState* S, int64_t* c) {
+  c[COOK_AUDIT_PENDING_ROWS] = (int64_t)S->pend.slot_of.size();
+  c[COOK_AUDIT_RUNNING_ROWS] = (int64_t)S->run.slot_of.size();
+  for (int l = 0; l < L_N; l++) c[COOK_AUDIT_ENTRIES + l] = S->lists[l].live;
+  for (int f = 0; f < F_N; f++) c[COOK_AUDIT_FLAGS + f] = S->nflag[f];
+  c[COOK_AUDIT_RESERVED_ROWS] = (int64_t)S->reserved.size();
+  c[COOK_AUDIT_COT_ROWS] = S->cot_rows;
+  c[COOK_AUDIT_COT_ENTRIES] = S->cot_n;
+  c[COOK_AUDIT_MAX_USER_PENDING] = count_max(S->users_p);
+  c[COOK_AUDIT_MAX_USER_RUNNING] = count_max(S->users_r);
+  c[COOK_AUDIT_MAX_GROUP_PENDING] = count_max(S->groups);
+  c[COOK_AUDIT_MAX_GROUP_RUNNING] = count_max(S->groups_r);
+  c[COOK_AUDIT_MAX_ATTR_COL] = count_max(S->attr_cols);
+  c[COOK_AUDIT_MAX_HOSTNAME_RUNNING] = count_max(S->hosts_r);
+}
+
+bool buckets_ok(int32_t nb) { return nb >= 0 && nb <= 65536 && (nb & (nb - 1)) == 0; }
+
+int32_t digest(cook_pool* pool, PoolState* S, int nb, cook_state_digest_out* out, cook_fp* out_pb, cook_fp* out_rb) {
+  const char* who = "cook_state_digest";
+  if (!out) return set_err(pool, COOK_E_BADARG, "%s: null out", who);
+  if (!buckets_ok(nb)) return set_err(pool, COOK_E_BADARG, "%s: n_buckets is not 0 or a power of two up to 65536", who);
+  if (nb ? (!out_pb || !out_rb) : (out_pb || out_rb))
+    return set_err(pool, COOK_E_BADARG, "%s: the bucket outputs go with n_buckets > 0", who);
+  if (!S || S->pend.slot_of.size() + S->run.slot_of.size() == 0) {   // nothing live
+    memset(out, 0, sizeof(*out));
+    out->consistent = 1;
+    out->first_mismatch = -1;
+    if (nb) { memset(out_pb, 0, sizeof(cook_fp) * (size_t)nb); memset(out_rb, 0, sizeof(cook_fp) * (size_t)nb); }
+    pool->phase[COOK_PHASE_AUDIT] = cook_phase_stats{};
+    return COOK_OK;
+  }
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  const int nq = S->ranked ? S->n_q : 0;
+  AuditDev* dev = nullptr;
+  cook_fp* bkt = nullptr;
+  int64_t* ids = nullptr;
+  int32_t* blk = nullptr;
+  int64_t h2d = 0, d2h = 0;
+  CK(pool, carve(S->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+    dev = c.take<AuditDev>(1);
+    if (nb) bkt = c.take<cook_fp>(2 * (size_t)nb);
+    if (nq) { ids = c.take<int64_t>(nq); blk = c.take<int32_t>((size_t)nq / CP_BLOCK + 2); }
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  CK(pool, cudaMemsetAsync(dev, 0, sizeof(AuditDev), st));
+  if (nb) CK(pool, cudaMemsetAsync(bkt, 0, sizeof(cook_fp) * 2 * (size_t)nb, st));
+  int nl = 0;
+  AuditArgs a = {};
+  a.out = dev; a.nb = (unsigned)nb; a.sb = nb <= AUDIT_SHARED_BUCKETS ? nb : 0;
+  const size_t shm = sizeof(unsigned long long) * 3 * (size_t)a.sb;
+  if (S->pend.hw) {
+    a.col = S->pend.d_col; a.n = S->pend.hw; a.bucket = bkt;
+    for (int l = 0; l < 3; l++) { a.v0[l] = S->lists[l].v[0]; a.v1[l] = S->lists[l].v[1]; }
+    audit_table_kernel<true><<<(a.n + 255) / 256, 256, shm, st>>>(a);
+    nl++;
+  }
+  if (S->run.hw) {
+    a.col = S->run.d_col; a.n = S->run.hw; a.bucket = bkt ? bkt + nb : nullptr;
+    a.v0[0] = S->lists[L_RGROUP].v[0]; a.v1[0] = nullptr;
+    audit_table_kernel<false><<<(a.n + 255) / 256, 256, shm, st>>>(a);
+    nl++;
+  }
+  if (nq) {
+    const QueueLive ql{S->q_slot, S->q_gen, S->pend.at<uint8_t>(P_LIVE), S->pend.at<uint32_t>(P_GEN), nullptr};
+    compact(QueueIds{ql, S->q_jid, ids}, nq, nullptr, blk, S->counters + 5, nq, st, &nl);
+    audit_queue_kernel<<<(nq + 255) / 256, 256, 0, st>>>(ids, S->counters + 5, &dev->fp[2]);
+    nl++;
+  }
+  CK(pool, cudaGetLastError());
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  AuditDev got;
+  CK(pool, download(&got, dev, 1, st, &d2h));
+  if (nb) {
+    CK(pool, download(out_pb, bkt, (size_t)nb, st, &d2h));
+    CK(pool, download(out_rb, bkt + nb, (size_t)nb, st, &d2h));
+  }
+  CK(pool, cudaEventRecord(pool->ev[23], st));
+  CK(pool, cudaStreamSynchronize(st));
+  record_phase(pool, COOK_PHASE_AUDIT, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[23], h2d, d2h, nl);
+  // ---- the recount against the host side
+  int64_t hostc[COOK_AUDIT_N], devc[COOK_AUDIT_N];
+  host_counts(S, hostc);
+  for (int k = 0; k < COOK_AUDIT_N; k++) devc[k] = got.c[k] - (k >= COOK_AUDIT_MAX_USER_PENDING ? 1 : 0);
+  devc[COOK_AUDIT_RESERVED_ROWS] = devc[COOK_AUDIT_FLAGS + F_RESERVED];
+  out->pending = got.fp[0]; out->running = got.fp[1]; out->queue = got.fp[2];
+  for (int l = 0; l < L_N; l++) out->entries[l] = devc[COOK_AUDIT_ENTRIES + l];
+  cook_state_counts_compare(hostc, devc, &out->first_mismatch);
+  out->consistent = out->first_mismatch < 0 ? 1 : 0;
+  return COOK_OK;
+}
+
+// ---- export
+// the live slots of a table whose id's bucket is selected (mask null: all), with their ids
+struct SelectedRows {
+  const uint8_t* live; const int64_t* id; const uint8_t* mask; unsigned nb; int32_t* sel; int64_t* key;
+  __device__ bool keep(int i) const { return live[i] && (!mask || mask[(unsigned)fp_mix((uint64_t)id[i]) & (nb - 1u)]); }
+  __device__ void emit(int i, int d) const { sel[d] = i; key[d] = id[i]; }
+};
+struct ExportCols { char* dst[MAXC]; int sz[MAXC]; int nc; };
+// row p of the export is slot sel[ord[p]]: the requested data columns (a null dst is skipped)
+__global__ void export_rows_kernel(void* const* col, const int32_t* sel, const int32_t* ord, int n, int32_t* rowslot,
+                                   ExportCols c) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n) return;
+  const int s = sel[ord[p]];
+  rowslot[p] = s;
+#pragma unroll
+  for (int k = 0; k < MAXC; k++) {
+    if (k >= c.nc) break;
+    if (!c.dst[k]) continue;
+    if (c.sz[k] == 1) reinterpret_cast<uint8_t*>(c.dst[k])[p] = static_cast<const uint8_t*>(col[k])[s];
+    else if (c.sz[k] == 4) reinterpret_cast<int32_t*>(c.dst[k])[p] = static_cast<const int32_t*>(col[k])[s];
+    else reinterpret_cast<long long*>(c.dst[k])[p] = static_cast<const long long*>(col[k])[s];
+  }
+}
+__global__ void list_total_kernel(OrderScan<int, 1> os, int n, int32_t* out) { *out = os.at(0, n - 1); }
+
+int32_t export_rows(cook_pool* pool, PoolState* S, int nb, const uint8_t* mask, const cook_state_sizes* cap,
+                    const cook_state_rows* out, cook_state_sizes* out_n) {
+  const char* who = "cook_state_export";
+  const bool query = !out;
+  if (!out_n || (!query && !cap)) return set_err(pool, COOK_E_BADARG, "%s: null out_n or cap", who);
+  if (!buckets_ok(nb)) return set_err(pool, COOK_E_BADARG, "%s: n_buckets is not 0 or a power of two up to 65536", who);
+  if (mask && !nb) return set_err(pool, COOK_E_BADARG, "%s: a mask without buckets", who);
+  // ---- what goes where: table t's data column k to dst[t][k], list l (of table l == L_RGROUP) to loff / lv
+  void* dst[2][MAXC] = {};
+  int32_t* loff[L_N] = {};
+  int32_t* lv[L_N][2] = {};
+  if (!query) {
+    const cook_jobs_rows& p = out->pending;
+    const cook_tasks_rows& r = out->running;
+    void* pd[P_NDATA] = {p.user, out->pending_priority, out->pending_job_id, p.cpus, p.mem, p.gpus, p.ports, p.allowed,
+                         p.plugin_accept, p.gpu_model, p.disk_request, p.disk_type, p.est_end_ms, p.ckpt_location,
+                         p.reserved_host};
+    void* rd[R_NDATA] = {r.user, r.priority, r.start_time, r.task_id, r.job_id, r.cpus, r.mem, r.gpus,
+                         out->running_hostname_id};
+    std::copy(pd, pd + P_NDATA, dst[0]);
+    std::copy(rd, rd + R_NDATA, dst[1]);
+    loff[L_NOVEL] = p.novel_off; lv[L_NOVEL][0] = p.novel_host;
+    loff[L_ATTR] = p.attr_off; lv[L_ATTR][0] = p.attr_col; lv[L_ATTR][1] = p.attr_val;
+    loff[L_GROUP] = p.group_off; lv[L_GROUP][0] = p.group_idx;
+    loff[L_RGROUP] = out->running_group_off; lv[L_RGROUP][0] = out->running_group_idx;
+    for (int l = 0; l < L_N; l++)
+      if (loff[l] && (!lv[l][0] || (l == L_ATTR && !lv[l][1])))
+        return set_err(pool, COOK_E_BADARG, "%s: a list's offsets without its values", who);
+  }
+  // ---- the sizes the host side knows: exact without a mask, an upper bound with one
+  int64_t N[2] = {0, 0}, E[L_N] = {};
+  if (S) {
+    N[0] = (int64_t)S->pend.slot_of.size(); N[1] = (int64_t)S->run.slot_of.size();
+    for (int l = 0; l < L_N; l++) E[l] = S->lists[l].live;
+  }
+  const auto fits = [&](const int64_t* rows, const int64_t* entries) {
+    if (rows[0] > cap->pending || rows[1] > cap->running) return false;
+    for (int l = 0; l < L_N; l++) if (loff[l] && entries[l] > cap->entries[l]) return false;
+    return true;
+  };
+  if (!query && !mask && !fits(N, E)) return set_err(pool, COOK_E_BADARG, "%s: a capacity below the required size", who);
+  if (N[0] + N[1] == 0 || (query && !mask)) {   // no device work
+    if (N[0] + N[1] == 0) {
+      for (int l = 0; l < L_N; l++) if (loff[l]) loff[l][0] = 0;
+      memset(out_n, 0, sizeof(*out_n));
+    } else {
+      out_n->pending = (int32_t)N[0]; out_n->running = (int32_t)N[1];
+      for (int l = 0; l < L_N; l++) out_n->entries[l] = (int32_t)E[l];
+    }
+    pool->phase[COOK_PHASE_AUDIT] = cook_phase_stats{};
+    return COOK_OK;
+  }
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  Table* tbl[2] = {&S->pend, &S->run};
+  const int live_col[2] = {P_LIVE, R_LIVE}, id_col[2] = {P_JID, R_TID}, ndata[2] = {P_NDATA, R_NDATA};
+  const int* sz[2] = {P_SZ, R_SZ};
+  const int table_of[L_N] = {0, 0, 0, 1}, off_col[L_N] = {P_NOFF, P_AOFF, P_GOFF, R_GOFF};
+  int32_t *sel[2] = {}, *ord[2] = {}, *tmp[2] = {}, *rowslot[2] = {}, *blk = nullptr, *d_cnt = nullptr;
+  int64_t* key[2] = {};
+  ExportCols cols[2] = {};
+  int32_t* d_off[L_N] = {};
+  int32_t* d_v[L_N][2] = {};
+  const uint8_t* d_mask = nullptr;
+  OrderScan<int, 1> os;
+  int64_t h2d = 0, d2h = 0;
+  CK(pool, carve(S->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+    for (int t = 0; t < 2; t++) {
+      sel[t] = c.take<int32_t>(N[t]); key[t] = c.take<int64_t>(N[t]);
+      if (query) continue;
+      ord[t] = c.take<int32_t>(N[t]); tmp[t] = c.take<int32_t>(N[t]); rowslot[t] = c.take<int32_t>(N[t]);
+      cols[t].nc = ndata[t];
+      for (int k = 0; k < ndata[t]; k++) {
+        cols[t].sz[k] = sz[t][k];
+        cols[t].dst[k] = dst[t][k] ? c.take<char>((size_t)N[t] * sz[t][k]) : nullptr;
+      }
+    }
+    const int64_t nmax = std::max(N[0], N[1]);
+    blk = c.take<int32_t>((size_t)std::max(S->pend.hw, S->run.hw) / CP_BLOCK + 2);
+    os.part[0] = c.take<int32_t>(nmax);
+    os.tile[0] = c.take<int32_t>((nmax + OS_TILE - 1) / OS_TILE + 1);
+    d_cnt = c.take<int32_t>(2 + L_N);
+    for (int l = 0; l < L_N; l++) {
+      if (!loff[l]) continue;
+      d_off[l] = c.take<int32_t>(N[table_of[l]] + 1);
+      for (int i = 0; i < S->lists[l].k; i++) d_v[l][i] = c.take<int32_t>(std::max<int64_t>(E[l], 1));
+    }
+    if (mask) d_mask = c.up(mask, nb);
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  int nl = 0;
+  CK(pool, cudaMemsetAsync(d_cnt, 0, sizeof(int32_t) * (2 + L_N), st));
+  for (int t = 0; t < 2; t++)
+    if (N[t])
+      compact(SelectedRows{tbl[t]->at<uint8_t>(live_col[t]), tbl[t]->at<int64_t>(id_col[t]), d_mask, (unsigned)nb, sel[t],
+                           key[t]}, tbl[t]->hw, nullptr, blk, d_cnt + t, (int)N[t], st, &nl);
+  CK(pool, cudaGetLastError());
+  int32_t n[2] = {(int32_t)N[0], (int32_t)N[1]};
+  if (mask) {   // how many rows the mask selects: the sort and the scans are sized by it
+    CK(pool, download(n, d_cnt, 2, st, &d2h));
+    CK(pool, cudaStreamSynchronize(st));
+  }
+  for (int t = 0; t < 2; t++) {
+    if (query || !n[t]) continue;
+    CK(pool, csort::sort_indices(ord[t], tmp[t], n[t], LessKeyTid{nullptr, key[t]}, st, &nl));
+    export_rows_kernel<<<(n[t] + 255) / 256, 256, 0, st>>>(tbl[t]->d_col, sel[t], ord[t], n[t], rowslot[t], cols[t]);
+    nl++;
+  }
+  for (int l = 0; l < L_N; l++) {
+    const int t = table_of[l];
+    if (!n[t]) {
+      if (d_off[l]) CK(pool, cudaMemsetAsync(d_off[l], 0, sizeof(int32_t), st));
+      continue;
+    }
+    const int32_t* rs = query ? sel[t] : rowslot[t];
+    const int32_t* len = tbl[t]->at<int32_t>(off_col[l] + 1);
+    order_scan(os, RowLen{rs, len}, n[t], S->gf0, st, &nl);
+    list_total_kernel<<<1, 1, 0, st>>>(os, n[t], d_cnt + 2 + l);
+    nl++;
+    if (!d_off[l]) continue;
+    csr_gather_kernel<<<(n[t] + 7) / 8, 256, 0, st>>>(os, rs, n[t], tbl[t]->at<int32_t>(off_col[l]), len, S->lists[l].v[0],
+                                                       S->lists[l].v[1], d_off[l], d_v[l][0], d_v[l][1]);
+    nl++;
+  }
+  CK(pool, cudaGetLastError());
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  int32_t cnt[2 + L_N];
+  CK(pool, download(cnt, d_cnt, 2 + L_N, st, &d2h));
+  CK(pool, cudaStreamSynchronize(st));
+  const int64_t rows[2] = {cnt[0], cnt[1]};
+  int64_t entries[L_N];
+  for (int l = 0; l < L_N; l++) entries[l] = cnt[2 + l];
+  if (!query) {
+    if (!fits(rows, entries)) return set_err(pool, COOK_E_BADARG, "%s: a capacity below the required size", who);
+    for (int t = 0; t < 2; t++)
+      for (int k = 0; k < ndata[t]; k++)
+        if (dst[t][k] && rows[t])
+          CK(pool, download(static_cast<char*>(dst[t][k]), cols[t].dst[k], (size_t)rows[t] * sz[t][k], st, &d2h));
+    for (int l = 0; l < L_N; l++) {
+      if (!loff[l]) continue;
+      CK(pool, download(loff[l], d_off[l], (size_t)rows[table_of[l]] + 1, st, &d2h));
+      for (int i = 0; i < S->lists[l].k; i++)
+        if (entries[l]) CK(pool, download(lv[l][i], d_v[l][i], (size_t)entries[l], st, &d2h));
+    }
+  }
+  CK(pool, cudaEventRecord(pool->ev[23], st));
+  CK(pool, cudaStreamSynchronize(st));
+  record_phase(pool, COOK_PHASE_AUDIT, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[23], h2d, d2h, nl);
+  out_n->pending = cnt[0]; out_n->running = cnt[1];
+  for (int l = 0; l < L_N; l++) out_n->entries[l] = cnt[2 + l];
+  return COOK_OK;
+}
+
+int32_t live_queue(cook_pool* pool, PoolState* S, int cap, int64_t* out_job_id, int32_t* out_n) {
+  const char* who = "cook_state_queue";
+  if (!out_n) return set_err(pool, COOK_E_BADARG, "%s: null out_n", who);
+  if (!S || !S->ranked) return set_err(pool, COOK_E_BADARG, "%s: no cook_state_rank on this handle yet", who);
+  const int nq = S->n_q;
+  if (nq == 0) {
+    *out_n = 0;
+    pool->phase[COOK_PHASE_AUDIT] = cook_phase_stats{};
+    return COOK_OK;
+  }
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  int64_t* ids = nullptr;
+  int32_t* blk = nullptr;
+  int64_t h2d = 0, d2h = 0;
+  CK(pool, carve(S->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+    ids = c.take<int64_t>(nq);
+    blk = c.take<int32_t>((size_t)nq / CP_BLOCK + 2);
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  int nl = 0;
+  const QueueLive ql{S->q_slot, S->q_gen, S->pend.at<uint8_t>(P_LIVE), S->pend.at<uint32_t>(P_GEN), nullptr};
+  compact(QueueIds{ql, S->q_jid, ids}, nq, nullptr, blk, S->counters + 5, nq, st, &nl);
+  CK(pool, cudaGetLastError());
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  int32_t n = 0;
+  CK(pool, download(&n, S->counters + 5, 1, st, &d2h));
+  CK(pool, cudaStreamSynchronize(st));
+  if (out_job_id) {
+    if (cap < n) return set_err(pool, COOK_E_BADARG, "%s: cap < the live queue entries", who);
+    if (n > 0) CK(pool, download(out_job_id, ids, (size_t)n, st, &d2h));
+  }
+  CK(pool, cudaEventRecord(pool->ev[23], st));
+  CK(pool, cudaStreamSynchronize(st));
+  record_phase(pool, COOK_PHASE_AUDIT, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[23], h2d, d2h, nl);
+  *out_n = n;
+  return COOK_OK;
+}
+
+}  // namespace
+
+extern "C" int32_t cook_state_counts_compare(const int64_t* host, const int64_t* device, int32_t* out_first) {
+  if (!host || !device || !out_first) return COOK_E_BADARG;
+  *out_first = -1;
+  for (int k = 0; k < COOK_AUDIT_N; k++)
+    if (host[k] != device[k]) { *out_first = k; break; }
+  return COOK_OK;
+}
+
+extern "C" int32_t cook_state_digest(cook_pool* pool, int32_t n_buckets, cook_state_digest_out* out,
+                                     cook_fp* out_pending_bucket, cook_fp* out_running_bucket) {
+  if (!pool) return COOK_E_BADARG;
+  return digest(pool, static_cast<PoolState*>(pool->state), n_buckets, out, out_pending_bucket, out_running_bucket);
+}
+
+extern "C" int32_t cook_state_export(cook_pool* pool, int32_t n_buckets, const uint8_t* bucket_mask,
+                                     const cook_state_sizes* cap, const cook_state_rows* out, cook_state_sizes* out_n) {
+  if (!pool) return COOK_E_BADARG;
+  return export_rows(pool, static_cast<PoolState*>(pool->state), n_buckets, bucket_mask, cap, out, out_n);
+}
+
+extern "C" int32_t cook_state_queue(cook_pool* pool, int32_t cap, int64_t* out_job_id, int32_t* out_n) {
+  if (!pool) return COOK_E_BADARG;
+  return live_queue(pool, static_cast<PoolState*>(pool->state), cap, out_job_id, out_n);
+}

@@ -13,6 +13,8 @@ path end to end.  It computes nothing numeric: every placement decision is `engi
                         (:790-795) -> reservations released (:1050-1057) -> head-matched feedback
                         + num-considerable scale-back / reset (handle-fenzo-pool :1613-1651)
   summarize_failures    fenzo_utils.clj:45-89 shape from cook_match_failures' counters (8f-3)
+  resync                the audit of a resident pool fed by deltas: bucket fingerprints compared with the host's,
+                        the differing buckets exported, the repairing delta built
 """
 import numpy as np
 
@@ -265,3 +267,37 @@ def autoscalable_jobs_resident(engine, users, *, number_considerable, number_unm
     prm = abi.ConsiderableParams(n, int(enforce_rate_limit), 1, abi.USAGE_LAST_MATCH, 0)
     skip = set(recent_synthetic_pod_jobs)
     return [int(j) for j in engine.state_considerable(users, prm, pool_quota=pool_quota) if int(j) not in skip]
+
+
+def resync(engine, host_digest_buckets, rows_of_bucket):
+    """Audit a resident pool against the host's source of truth and build the delta that repairs it.
+
+    host_digest_buckets: {"pending": [(sum, xor, n)] * n_buckets, "running": likewise}, the host's own bucket
+    fingerprints (n_buckets a power of two).  rows_of_bucket(buckets) -> the host's rows of those buckets as the
+    keyword arguments of abi.make_delta (pending / pending_priority / pending_job_id / running / ...).
+    Returns (buckets, delta): the sorted differing buckets, and the abi.StateDelta that removes the device rows of
+    those buckets the host does not have and upserts the host's rows there; (,) and None when nothing differs.  The
+    caller applies it with engine.state_apply."""
+    nb = len(host_digest_buckets["pending"])
+    if nb == 0 or nb & (nb - 1) or len(host_digest_buckets["running"]) != nb:
+        raise ValueError("resync: the bucket lists need one power-of-two length")
+    dev = engine.state_digest(nb)
+    diff = set()
+    for table in ("pending", "running"):
+        d = dev[table + "_buckets"]
+        for b, want in enumerate(host_digest_buckets[table]):
+            if (int(d["sum"][b]), int(d["xr"][b]), int(d["n"][b])) != tuple(int(x) for x in want):
+                diff.add(b)
+    if not diff:
+        return [], None
+    buckets = sorted(diff)
+    mask = np.zeros(nb, np.uint8)
+    mask[buckets] = 1
+    held = engine.state_export(mask)
+    want = dict(rows_of_bucket(buckets))
+    wp, wr = want.get("pending_job_id"), want.get("running")
+    host_jobs = set(np.asarray(wp, np.int64).tolist()) if wp is not None else set()
+    host_tasks = set(wr.col("task_id").tolist()) if wr is not None and wr.n else set()
+    want["pending_rm"] = [j for j in held["pending_job_id"].tolist() if j not in host_jobs]
+    want["running_rm"] = [t for t in held["running"].col("task_id").tolist() if t not in host_tasks]
+    return buckets, abi.make_delta(**want)

@@ -64,7 +64,8 @@ def load_library(path=None):
                  "cook_match_failures", "cook_state_apply", "cook_state_rank", "cook_state_match",
                  "cook_state_rebalance", "cook_state_launch", "cook_state_patch", "cook_state_usage",
                  "cook_state_cotasks", "cook_state_match_derived", "cook_state_rebalance_derived",
-                 "cook_state_considerable", "cook_state_rank_offensive"):
+                 "cook_state_considerable", "cook_state_rank_offensive", "cook_state_digest",
+                 "cook_state_counts_compare", "cook_state_export", "cook_state_queue"):
         getattr(lib, name).restype = C.c_int32
     for name, argtypes in abi.ARGTYPES.items():
         getattr(lib, name).argtypes = argtypes
@@ -293,6 +294,76 @@ class GpuEngine:
         n = C.c_int32(0)
         rc = self.lib.cook_state_considerable(self.pool, C.byref(users), C.byref(pool_quota), C.byref(params),
                                               abi.ptr(out, abi.P_I64), C.byref(n))
+        if rc != 0:
+            self._err(rc)
+        return out[:n.value].copy()
+
+    def state_digest(self, n_buckets=0):
+        """cook_state_digest: the fingerprints of the live pending rows, the live running rows and the live queue as
+        (sum, xor, n) tuples, the live 'entries' per list, 'consistent' / 'first_mismatch' (an abi.AUDIT_NAMES name
+        or None) of the recount, and with n_buckets 'pending_buckets' / 'running_buckets' (abi.FP_DTYPE arrays)."""
+        nb = int(n_buckets)
+        out = abi.StateDigest()
+        pb, rb = np.zeros(max(nb, 1), abi.FP_DTYPE), np.zeros(max(nb, 1), abi.FP_DTYPE)
+        fp = C.POINTER(abi.Fp)
+        rc = self.lib.cook_state_digest(self.pool, nb, C.byref(out), pb.ctypes.data_as(fp) if nb else None,
+                                        rb.ctypes.data_as(fp) if nb else None)
+        if rc != 0:
+            self._err(rc)
+        return {"pending": out.pending.as_tuple(), "running": out.running.as_tuple(), "queue": out.queue.as_tuple(),
+                "entries": list(out.entries), "consistent": bool(out.consistent),
+                "first_mismatch": abi.AUDIT_NAMES[out.first_mismatch] if out.first_mismatch >= 0 else None,
+                "pending_buckets": pb[:nb], "running_buckets": rb[:nb]}
+
+    def state_export(self, bucket_mask=None):
+        """cook_state_export: the live rows (bucket_mask: a uint8 array of a power-of-two length, the rows whose
+        bucket is set) in ascending id, as the keyword arguments of abi.make_delta: pass them with reset=True to a
+        fresh handle for a copy, or as they are to repair those rows."""
+        mask = np.ascontiguousarray(bucket_mask, np.uint8) if bucket_mask is not None else None
+        args = (self.pool, len(mask) if mask is not None else 0, abi.ptr(mask, abi.P_U8) if mask is not None else None)
+        n = abi.StateSizes()
+        rc = self.lib.cook_state_export(*args, None, None, C.byref(n))
+        if rc != 0:
+            self._err(rc)
+        P, R, E = n.pending, n.running, list(n.entries)
+        dt = abi._NP
+
+        def cols(struct, rows, lists):
+            kw = {}
+            for name, ctype in struct._fields_:
+                if name.endswith("_off"):
+                    kw[name] = np.zeros(rows + 1, np.int32)
+                elif name in lists:
+                    kw[name] = np.zeros(max(lists[name], 1), np.int32)
+                else:
+                    kw[name] = np.zeros(max(rows, 1), dt[ctype])
+            return kw
+        pk = cols(abi.JobsRows, P, dict(novel_host=E[0], attr_col=E[1], attr_val=E[1], group_idx=E[2]))
+        rk = cols(abi.TasksRows, R, {})
+        prio, jid, host = np.zeros(max(P, 1), np.int32), np.zeros(max(P, 1), np.int64), np.zeros(max(R, 1), np.int32)
+        goff, gidx = np.zeros(R + 1, np.int32), np.zeros(max(E[3], 1), np.int32)
+        rows = abi.StateRows(pending=abi.JobsRows(**pk), pending_priority=prio, pending_job_id=jid,
+                             running=abi.TasksRows(**rk), running_hostname_id=host, running_group_off=goff,
+                             running_group_idx=gidx)
+        got = abi.StateSizes()
+        rc = self.lib.cook_state_export(*args, C.byref(n), C.byref(rows), C.byref(got))
+        if rc != 0:
+            self._err(rc)
+        assert (got.pending, got.running, list(got.entries)) == (P, R, E)
+        pk = {k: v if k.endswith("_off") or k in ("novel_host", "attr_col", "attr_val", "group_idx") else v[:P]
+              for k, v in pk.items()}
+        return dict(pending=abi.JobsSoA(n=P, **pk), pending_priority=prio[:P], pending_job_id=jid[:P],
+                    running=abi.TasksSoA(n=R, **{k: v[:R] for k, v in rk.items()}), running_hostname_id=host[:R],
+                    running_group_off=goff, running_group_idx=gidx)
+
+    def state_queue(self):
+        """cook_state_queue: the job ids cook_state_match would read now, in queue order."""
+        n = C.c_int32(0)
+        rc = self.lib.cook_state_queue(self.pool, 0, None, C.byref(n))
+        if rc != 0:
+            self._err(rc)
+        out = np.zeros(max(n.value, 1), np.int64)
+        rc = self.lib.cook_state_queue(self.pool, n.value, abi.ptr(out, abi.P_I64), C.byref(n))
         if rc != 0:
             self._err(rc)
         return out[:n.value].copy()

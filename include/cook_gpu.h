@@ -687,6 +687,121 @@ typedef struct {
 int32_t cook_state_considerable(cook_pool* pool, const cook_user_table* users, const cook_pool_quota* pool_quota,
                                 const cook_considerable_params* params, int64_t* out_job_id, int32_t* out_n);
 
+/* ---------------------------------------------------------- auditing a resident pool */
+/* The read side of the resident state: a fingerprint a host can restate from its own source of truth (the
+ * database the deltas came from), a bucketed form of it that localises a difference, the rows themselves in a
+ * form cook_state_apply takes back, and the live queue.  None of these calls changes anything resident, needs a
+ * cook_state_rank (the queue parts report empty) or touches the queue or the last match: cook_state_match,
+ * cook_match_failures, cook_exchange_usage(_batch) and COOK_USAGE_LAST_MATCH behave after them as before.
+ *
+ * Row hash (64 bit; all arithmetic mod 2^64):
+ *   mix(z)       = the splitmix64 finaliser: z ^= z >> 30; z *= 0xbf58476d1ce4e5b9; z ^= z >> 27;
+ *                  z *= 0x94d049bb133111eb; z ^= z >> 31
+ *   absorb(h, w) = mix((h ^ w) + 0x9e3779b97f4a7c15)
+ *   A row starts from its table's tag (1 pending, 2 running), absorbs its id (job id / task id), then every data
+ *   column as one 64-bit word each (int32 sign-extended, uint8 zero-extended, a double by its bit pattern as
+ *   stored, so -0.0 differs from 0.0; a column the delta left NULL by its documented absent value), then each
+ *   list: its length, then its entries in order (attribute-equals: column, then value; each sign-extended).
+ *     pending: user, priority, cpus, mem, gpus, ports, allowed, plugin_accept, gpu_model, disk_request, disk_type,
+ *              est_end_ms, ckpt_location, reserved_host; lists novel_host, (attr_col, attr_val), group_idx
+ *     running: user, priority, start_time, job_id, cpus, mem, gpus, running_hostname_id; list running_group_idx
+ *   Where a row is stored (slot, generation, list offsets) is layout and is not hashed.
+ * Set fingerprint: sum = the sum of the row hashes, xr = their xor, n = their number.  Both are commutative, so
+ *   the result does not depend on slot or arena layout, grid size or the order of atomics.
+ * Queue fingerprint: over the entries cook_state_match would read now, p the position among them:
+ *   row hash = absorb(absorb(3, p), job id).  Zero with n = 0 before any cook_state_rank.
+ * Buckets: n_buckets is 0 or a power of two up to 65536; bucket(id) = mix(id) & (n_buckets - 1).               */
+typedef struct { uint64_t sum, xr; int64_t n; } cook_fp;
+
+/* What the host side of the state mirrors of the device rows, recounted from them by cook_state_digest: live rows
+ * per table, live entries per list arena (+ 0 novel hosts, 1 attribute-equals, 2 pending groups, 3 running
+ * groups), pending rows holding a non-absent value per kind (+ 0 gpus, 1 ports, 2 not allowed, 3 not
+ * plugin-accepted, 4 gpu_model, 5 disk_request, 6 est_end_ms, 7 ckpt_location, 8 reserved_host), the reserved
+ * rows, the running rows with a known host and a group list and their entries, and the largest code per kind
+ * (-1: none).  first_mismatch is one of these.                                                                 */
+enum {
+  COOK_AUDIT_PENDING_ROWS = 0, COOK_AUDIT_RUNNING_ROWS = 1, COOK_AUDIT_ENTRIES = 2, COOK_AUDIT_FLAGS = 6,
+  COOK_AUDIT_RESERVED_ROWS = 15, COOK_AUDIT_COT_ROWS = 16, COOK_AUDIT_COT_ENTRIES = 17,
+  COOK_AUDIT_MAX_USER_PENDING = 18, COOK_AUDIT_MAX_USER_RUNNING = 19, COOK_AUDIT_MAX_GROUP_PENDING = 20,
+  COOK_AUDIT_MAX_GROUP_RUNNING = 21, COOK_AUDIT_MAX_ATTR_COL = 22, COOK_AUDIT_MAX_HOSTNAME_RUNNING = 23,
+  COOK_AUDIT_N = 24
+};
+typedef struct {
+  cook_fp pending, running;   /* the live rows of each table                                               */
+  cook_fp queue;              /* the live queue, order-sensitive                                           */
+  int64_t entries[4];         /* live list entries: novel hosts, attribute-equals, pending groups, running groups */
+  int32_t consistent;         /* 1: every host-side count equals its recount from the device rows          */
+  int32_t first_mismatch;     /* the first COOK_AUDIT_* count that differed, -1 when consistent            */
+} cook_state_digest_out;
+
+/* Fingerprints and recount in one pass per table.  out_pending_bucket / out_running_bucket [n_buckets] receive the
+ * fingerprint of each table's rows per bucket (their sums, xors and counts add up to the table's); both are
+ * required when n_buckets > 0.
+ * COOK_E_BADARG, before any device work with nothing written: a NULL out; n_buckets negative, not a power of two
+ * or above 65536; n_buckets > 0 with a NULL bucket output, or a bucket output with n_buckets == 0.
+ * No state, or no live row in either table: all zero, consistent = 1, no device work.
+ * Transfers exactly: up nothing; down 72 (the three fingerprints) + 8 * COOK_AUDIT_N (the recount) + 2 * 24 *
+ * n_buckets.  Statistics: cook_last_stats(COOK_PHASE_AUDIT).                                                   */
+int32_t cook_state_digest(cook_pool* pool, int32_t n_buckets, cook_state_digest_out* out,
+                          cook_fp* out_pending_bucket, cook_fp* out_running_bucket);
+
+/* The comparison cook_state_digest makes after its download: *out_first = the first index k < COOK_AUDIT_N with
+ * host[k] != device[k], or -1.  A pure host function.  COOK_E_BADARG on a NULL argument.                        */
+int32_t cook_state_counts_compare(const int64_t* host, const int64_t* device, int32_t* out_first);
+
+/* The rows as a delta: cook_state_delta's columns with writable pointers.  A NULL column is skipped; a list is
+ * written when its offsets column is given, and then needs its value column(s).                                 */
+typedef struct {
+  int32_t* user; double* cpus; double* mem; double* gpus; int32_t* ports; uint8_t* allowed; uint8_t* plugin_accept;
+  int32_t* novel_off; int32_t* novel_host; int32_t* gpu_model; double* disk_request; int32_t* disk_type;
+  int32_t* attr_off; int32_t* attr_col; int32_t* attr_val; int64_t* est_end_ms; int32_t* ckpt_location;
+  int32_t* reserved_host; int32_t* group_off; int32_t* group_idx;
+} cook_jobs_rows;
+typedef struct {
+  int32_t* user; int32_t* priority; int64_t* start_time; int64_t* task_id; int64_t* job_id;
+  double* cpus; double* mem; double* gpus;
+} cook_tasks_rows;
+typedef struct {
+  cook_jobs_rows pending;
+  int32_t* pending_priority;
+  int64_t* pending_job_id;
+  cook_tasks_rows running;
+  int32_t* running_hostname_id;
+  int32_t* running_group_off;
+  int32_t* running_group_idx;
+} cook_state_rows;
+typedef struct {
+  int32_t pending, running;   /* rows per table                                                             */
+  int32_t entries[4];         /* entries per list: novel hosts, attribute-equals, pending groups, running groups */
+} cook_state_sizes;
+
+/* Every live row or, with bucket_mask[n_buckets], those whose bucket b has bucket_mask[b] != 0: pending rows in
+ * ascending job id, running rows in ascending task id, the lists rebuilt as CSR over that order ([rows + 1]
+ * offsets).  *out_n receives the rows and entries; `cap` is the capacity of the columns of `out`.
+ * Round trip: the arrays, passed as one cook_state_delta with reset = 1 to a fresh handle, give a state with the
+ * same digest; without reset, to a handle that lacks or mis-holds those rows, they repair them.  Generations and
+ * the queue are not exported: repaired rows leave the queue until the next rank, as after any upsert.
+ * Size query: out == NULL writes only *out_n; without a mask from the host-side counts (no device work), with one
+ * by the count pass.
+ * COOK_E_BADARG with nothing written: a NULL out_n, or a NULL cap with out given; n_buckets as for
+ * cook_state_digest; a mask with n_buckets == 0; an offsets column without its value column(s); a capacity below
+ * the required size (without a mask before any device work, with one after the count pass).
+ * No state, or no live row in either table: *out_n all zero, each given offsets column gets its one 0, no device
+ * work.
+ * Transfers exactly (when there is device work): up n_buckets bytes with a mask, else nothing; down 24 (the
+ * counts) + 8 with a mask (the row counts, ahead of the sort) and, unless a size query, for each non-NULL column
+ * its element size times the rows, per given list 4 * (rows + 1) for the offsets and 4 (attribute-equals 8) per
+ * entry.  Statistics: cook_last_stats(COOK_PHASE_AUDIT).                                                        */
+int32_t cook_state_export(cook_pool* pool, int32_t n_buckets, const uint8_t* bucket_mask,
+                          const cook_state_sizes* cap, const cook_state_rows* out, cook_state_sizes* out_n);
+
+/* The live queue now: the job ids cook_state_match would read, in order (the last cook_state_rank's queue minus
+ * the launched, removed, replaced and consumed jobs).  out_job_id == NULL is a size query: only *out_n.
+ * COOK_E_BADARG with nothing written: before any cook_state_rank, a NULL out_n, cap < the live entries.
+ * Transfers exactly: down 4 (the length; nothing for an empty ranked queue: no device work) + 8 * *out_n unless a
+ * size query.  Statistics: cook_last_stats(COOK_PHASE_AUDIT).                                                   */
+int32_t cook_state_queue(cook_pool* pool, int32_t cap, int64_t* out_job_id, int32_t* out_n);
+
 /* ------------------------------------------------------------ phase timing */
 /* Device-side timing of the last call of each kind on this handle (CUDA events on the
  * pool's stream): what bench.py's `phases` block and roofline lines are computed from.
@@ -696,9 +811,13 @@ int32_t cook_state_considerable(cook_pool* pool, const cook_user_table* users, c
  * cook_state_cotasks (upload of the host codes, attribute columns and group map, the compaction, expansion and
  * sort, the download of the lists; all zero after a call without device work).  COOK_PHASE_CONSIDERABLE: the last
  * cook_state_considerable (upload of the user columns, the queue compaction and gathers, the usage fold when derived,
- * the considerable pass and the consumption, the download of the ids). */
+ * the considerable pass and the consumption, the download of the ids).  COOK_PHASE_AUDIT: the last
+ * cook_state_digest, cook_state_export or cook_state_queue (upload of the bucket mask, the passes over the tables,
+ * the compaction, sort and gathers, the download of the fingerprints, rows or ids; all zero after a call without
+ * device work). */
 enum { COOK_PHASE_RANK = 0, COOK_PHASE_MATCH = 1, COOK_PHASE_REBALANCE = 2, COOK_PHASE_EXCHANGE = 3,
-       COOK_PHASE_STATE = 4, COOK_PHASE_USAGE = 5, COOK_PHASE_COTASKS = 6, COOK_PHASE_CONSIDERABLE = 7 };
+       COOK_PHASE_STATE = 4, COOK_PHASE_USAGE = 5, COOK_PHASE_COTASKS = 6, COOK_PHASE_CONSIDERABLE = 7,
+       COOK_PHASE_AUDIT = 8 };
 typedef struct {
   double ms_h2d;      /* upload stage                                              */
   double ms_device;   /* kernels (for the exchange: delta kernels + the collective) */

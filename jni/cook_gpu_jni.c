@@ -257,6 +257,38 @@ JFN(jint, stateConsiderable)(JNIEnv* env, jclass k, jlong pool, jint n_users, jo
   (*env)->SetIntArrayRegion(env, out_n, 0, 1, (jint*)&n);
   return rc;
 }
+/* the fingerprints and the recount of the resident rows: out_digest is a direct buffer of sizeof(cook_state_digest_out),
+ * out_pending_bucket / out_running_bucket direct buffers of n_buckets cook_fp each (null when n_buckets == 0) */
+JFN(jint, stateDigest)(JNIEnv* env, jclass k, jlong pool, jint n_buckets, jobject out_digest, jobject out_pending_bucket,
+                       jobject out_running_bucket) {
+  return cook_state_digest((cook_pool*)(intptr_t)pool, n_buckets, (cook_state_digest_out*)one(env, out_digest),
+                           (cook_fp*)one(env, out_pending_bucket), (cook_fp*)one(env, out_running_bucket));
+}
+/* the live rows (bucket_mask: those of the selected buckets) as a delta's arrays.  cols: 33 direct buffers in the field
+ * order of cook_state_rows (the 20 of cook_jobs_rows, pending_priority, pending_job_id, the 8 of cook_tasks_rows,
+ * running_hostname_id, running_group_off, running_group_idx), a null element skips the column; a null `cols` asks for
+ * the sizes.  cap and out_n hold {pending, running, entries[4]} */
+JFN(jint, stateExport)(JNIEnv* env, jclass k, jlong pool, jint n_buckets, jobject bucket_mask, jintArray cap,
+                       jobjectArray cols, jintArray out_n) {
+  cook_state_rows rows; cook_state_sizes c, n;
+  void** field = (void**)&rows;   /* cook_state_rows holds nothing but pointers */
+  memset(&rows, 0, sizeof(rows)); memset(&n, 0, sizeof(n));
+  if (cols)
+    for (int i = 0; i < (int)(sizeof(rows) / sizeof(void*)); i++)
+      field[i] = one(env, (*env)->GetObjectArrayElement(env, cols, i));
+  if (cap) (*env)->GetIntArrayRegion(env, cap, 0, 6, (jint*)&c);
+  jint rc = cook_state_export((cook_pool*)(intptr_t)pool, n_buckets, (const uint8_t*)one(env, bucket_mask), cap ? &c : NULL,
+                              cols ? &rows : NULL, &n);
+  if (rc == COOK_OK) (*env)->SetIntArrayRegion(env, out_n, 0, 6, (jint*)&n);
+  return rc;
+}
+/* the live queue as job ids (a null out_job_id asks for the length) */
+JFN(jint, stateQueue)(JNIEnv* env, jclass k, jlong pool, jint cap, jobject out_job_id, jintArray out_n) {
+  int32_t n = 0;
+  jint rc = cook_state_queue((cook_pool*)(intptr_t)pool, cap, one(env, out_job_id), &n);
+  if (rc == COOK_OK) (*env)->SetIntArrayRegion(env, out_n, 0, 1, (jint*)&n);
+  return rc;
+}
 typedef int32_t (*state_match_fn)(cook_pool*, const cook_offers_soa*, const cook_groups*, const cook_user_table*,
                                   const cook_pool_quota*, const cook_match_params*, int64_t*, int32_t*, int32_t*, int32_t,
                                   uint8_t*, cook_match_stats*);

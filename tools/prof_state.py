@@ -60,6 +60,16 @@ each cycle runs pending-jobs->considerable-jobs and, with quota_only, the autosc
 
   python tools/prof_state.py --considerable --pool c2 --cycles 5
   python tools/prof_state.py --considerable --pool c5 --c5-pool 5 --cycles 5
+
+--audit loads the pool into a resident handle, churns it for --cycles batches (3 % of the running tasks finish, one
+pending job in a hundred is replaced, one in a hundred removed) and ranks it.  It then times, --reps times each after a
+warm-up call: cook_state_digest without buckets and with 4096, the full cook_state_export, the export of 4 of 4096
+buckets, and cook_state_queue.  Per call it prints the median, least and largest device time, download time and host
+wall time, the bytes down, and (digest) the rate against the bytes the pass must read: the live rows' hashed columns,
+live flags, list ranges and list entries.
+
+  python tools/prof_state.py --audit --pool c2
+  python tools/prof_state.py --audit --pool c5 --c5-pool 5
 """
 import argparse
 import json
@@ -492,6 +502,60 @@ def considerable_prof(a):
     host.close()
 
 
+def audit_prof(a):
+    t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
+    jobs, pc, rc, users = t["jobs"], t["cols"]["pending"], t["cols"]["running"], t["users"]
+    rng = np.random.default_rng(a.seed)
+    store = Jobs(jobs, pc["priority"], pc["job_id"])
+    run = {k: np.asarray(v) for k, v in rc.items()}
+    res = GpuEngine(pool_name="resident")
+    res.state_apply(abi.make_delta(reset=True, running=abi.make_tasks(**run), pending=store.soa(np.arange(jobs.n)),
+                                   pending_priority=store.prio, pending_job_id=store.jid))
+    alive, tids = np.ones(jobs.n, bool), run["task_id"].copy()
+    for _ in range(a.cycles):
+        live = np.flatnonzero(alive)
+        pick = rng.choice(live, max(2, len(live) // 50), replace=False)
+        rm, up = pick[:len(pick) // 2], pick[len(pick) // 2:]
+        fin = rng.choice(len(tids), len(tids) * 3 // 100, replace=False)
+        store.prio[up] = 90
+        res.state_apply(abi.make_delta(pending_rm=store.jid[rm], running_rm=tids[fin], pending=store.soa(up),
+                                       pending_priority=store.prio[up], pending_job_id=store.jid[up]))
+        alive[rm] = False
+        tids = np.delete(tids, fin)
+    q = res.state_rank(users)
+    d = res.state_digest()
+    P, Rn, E = d["pending"][2], d["running"][2], d["entries"]
+    must_read = P * (78 + 1 + 24) + 4 * E[0] + 8 * E[1] + 4 * E[2] + Rn * (60 + 1 + 8) + 4 * E[3]
+    print(json.dumps({"card": card(), "pool": a.pool if a.pool == "c2" else f"c5/{a.c5_pool}", "pending": P, "running": Rn,
+                      "entries": E, "queue": len(q), "consistent": d["consistent"], "digest_must_read_bytes": must_read,
+                      "reps": a.reps}), flush=True)
+    few = np.zeros(4096, np.uint8)
+    few[[1, 1000, 2000, 4000]] = 1
+    calls = (("digest", lambda: res.state_digest()), ("digest_4096_buckets", lambda: res.state_digest(4096)),
+             ("export_all", lambda: res.state_export()), ("export_4_of_4096_buckets", lambda: res.state_export(few)),
+             ("queue", lambda: res.state_queue()))
+    for name, call in calls:
+        call()
+        rows = []
+        for _ in range(a.reps):
+            w0 = time.perf_counter()
+            call()
+            rows.append((1e3 * (time.perf_counter() - w0), res.last_stats(abi.PHASE_AUDIT)))
+        st = rows[-1][1]
+
+        def spread(x):
+            return {"median": round(float(np.median(x)), 3), "min": round(float(np.min(x)), 3), "max": round(float(np.max(x)), 3)}
+
+        dev = [s["ms_device"] for _, s in rows]
+        out = {"call": name, "ms_device": spread(dev), "ms_d2h": spread([s["ms_d2h"] for _, s in rows]),
+               "wall_ms": spread([w for w, _ in rows]), "h2d_bytes": st["h2d_bytes"], "d2h_bytes": st["d2h_bytes"],
+               "n_launches": st["n_launches"]}
+        if name.startswith("digest"):
+            out["GBps_of_must_read_at_median"] = round(must_read / (np.median(dev) * 1e-3) / 1e9, 1)
+        print(json.dumps(out), flush=True)
+    res.close()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--pool", choices=("c2", "c5"), default="c2")
@@ -508,7 +572,11 @@ def main():
                          "instead of --pool")
     ap.add_argument("--derived", action="store_true")
     ap.add_argument("--considerable", action="store_true")
+    ap.add_argument("--audit", action="store_true")
+    ap.add_argument("--reps", type=int, default=20, help="--audit: timed calls per kind")
     a = ap.parse_args()
+    if a.audit:
+        return audit_prof(a)
     if a.considerable:
         return considerable_prof(a)
     if a.rebalance:
