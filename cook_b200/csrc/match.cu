@@ -464,7 +464,10 @@ struct EvalStatic {  // static VM table in shared memory (SoA), or null => globa
   const double* lc; const double* lm; const double* rc; const double* rm;
 };
 
-// per-CTA exchange buffer: every warp's per-lane partial lists of one row
+// per-CTA exchange buffer: every warp's per-lane partial lists of one row.  The sizes of EvalShared, SparseLive
+// and ResolverShared set the offer counts where match_run moves the static VM table and latest[] to global
+// memory; tests/match_edge_cases.py builds cases on either side of those counts from the sizes it records
+// (SMEM_STATIC_O, LATEST_O): change them together.
 struct EvalShared {
   double f[NW][TOPK][32];
   int32_t v[NW][TOPK][32];
