@@ -352,10 +352,21 @@ __device__ __forceinline__ double safe_rcp(double den) {
 }
 
 // FENZO 3a + 4 (see oracle): resource fit then cpuMemBinPacker fitness.
+// The usual case (both reciprocals usable) takes no branch between the two divisions, so their
+// dependent chains interleave: on the commit chain that is one 7-op f64 path instead of two 5-op ones
+// each fenced by a branch to the IEEE division.  Same operations, same results.
 __device__ __forceinline__ double fit_fitness(double jc, double jm, const VmState& st) {
   const bool no = (st.ac + jc > st.lc) | (st.am + jm > st.lm);
-  const double cpu_fit = div_y((jc + st.ac) + st.rc, st.lc + st.rc, st.yc);
-  const double mem_fit = div_y((jm + st.am) + st.rm, st.lm + st.rm, st.ym);
+  double cpu_fit, mem_fit;
+  if (st.yc != 0.0 && st.ym != 0.0) {
+    const double xc = (jc + st.ac) + st.rc, xm = (jm + st.am) + st.rm;
+    const double qc = xc * st.yc, qm = xm * st.ym;
+    cpu_fit = fma(fma(-(st.lc + st.rc), qc, xc), st.yc, qc);
+    mem_fit = fma(fma(-(st.lm + st.rm), qm, xm), st.ym, qm);
+  } else {
+    cpu_fit = div_y((jc + st.ac) + st.rc, st.lc + st.rc, st.yc);
+    mem_fit = div_y((jm + st.am) + st.rm, st.lm + st.rm, st.ym);
+  }
   return no ? 0.0 : (cpu_fit + mem_fit) * 0.5;
 }
 
@@ -734,6 +745,17 @@ struct Latest {
   __device__ __forceinline__ void set(int v, int e) const { if (g) g[v] = e; else s[v] = e; }
 };
 
+// Per-turn timeline of the PROF instantiation (COOK_PROF=1 with COOK_PROF_TRACE=<file>): null unless the
+// host armed it.  turn_trace[g] = TURN_WORDS stamps of queue entry g (clock64 of the resolver SM, so every
+// role of CTA 0 is on one clock); blk_trace[b] = when the driver saw every row of block b scored.
+constexpr int TURN_WORDS = 10;
+enum { TT_FREE = 0, TT_LAND, TT_READY, TT_SEEN, TT_DONE, TT_FENCE, TT_INFO, TT_K, TT_EVAL, TT_DEC };
+enum { TP_EXACT = 0, TP_ZTAKE = 1, TP_FALLBACK = 2, TP_GROUP = 3 };
+__device__ unsigned long long* g_turn_trace;
+__device__ int g_turn_cap;
+__device__ unsigned long long* g_blk_trace;
+__device__ int g_blk_cap;
+
 __device__ __forceinline__ void fence_cta() { asm volatile("fence.acq_rel.cta;" ::: "memory"); }
 // Readers of the resolver's shared flags: shared-memory loads of one warp complete in
 // program order, so polling needs no hardware fence - only the compiler must not move
@@ -1060,7 +1082,7 @@ __device__ __noinline__ int resolve_group_job(const MatchArgs& a, ResolverShared
 // ---- driver warp: feasibility stamps -> in-order queue
 // The resolver CTA runs the driver; every spec CTA runs a replica (REMOTE) that derives the same
 // queue from the same global inputs (stamps, block bounds, lo_g) and fills only its local ring.
-template <bool CONSTR, bool REMOTE>
+template <bool CONSTR, bool REMOTE, bool PROF = false>
 __device__ void driver_warp(const MatchArgs& a, ResolverShared& S) {
   const int lane = threadIdx.x & 31;
   int g = 0;
@@ -1097,6 +1119,7 @@ __device__ void driver_warp(const MatchArgs& a, ResolverShared& S) {
         __nanosleep(20);
       }
     }
+    if (PROF && lane == 0 && b < g_blk_cap) g_blk_trace[b] = (unsigned long long)clock64();
     dead = __shfl_sync(0xffffffffu, dead, 0);
     if (dead) {
       if (!REMOTE && lane == 0) {
@@ -1354,7 +1377,21 @@ __device__ void commit_warp(const MatchArgs& a, ResolverShared& S, const Latest 
     if (quit) break;
     const SpecOut* R = &S.res[slot];
     const int type = R->type;
-    if (PROF) prof[0] += (unsigned long long)(clock64() - t0);
+    const long long t_land = PROF ? clock64() : 0;
+    if (PROF) prof[0] += (unsigned long long)(t_land - t0);
+    // lane 0: this turn's row of the timeline
+    // (t_done is read right after the chain store: the row's other stamps may come back from local memory)
+    auto trace_turn = [&](long long t_ready, long long t_seen, long long t_eval, long long t_dec, long long t_fence,
+                          long long t_done, unsigned long long info, int key) {
+      if (PROF && lane == 0 && g < g_turn_cap) {
+        unsigned long long* p = g_turn_trace + (size_t)g * TURN_WORDS;
+        p[TT_FREE] = (unsigned long long)t0; p[TT_LAND] = (unsigned long long)t_land;
+        p[TT_READY] = (unsigned long long)t_ready; p[TT_SEEN] = (unsigned long long)t_seen;
+        p[TT_DONE] = (unsigned long long)t_done; p[TT_FENCE] = (unsigned long long)t_fence;
+        p[TT_INFO] = info; p[TT_K] = (unsigned long long)(long long)key;
+        p[TT_EVAL] = (unsigned long long)t_eval; p[TT_DEC] = (unsigned long long)t_dec;
+      }
+    };
     if (type == Q_EXIT) {
       while (chain_gdone(S.chain) != g) __nanosleep(20);
       if (lane == 0) a.stats[14] = (unsigned long long)(clock64() - t_start);
@@ -1402,9 +1439,14 @@ __device__ void commit_warp(const MatchArgs& a, ResolverShared& S, const Latest 
         __stcg(a.lo_g + b + 1, c);   // the spec CTAs' driver replicas read the block's lo from here
         fence_cta();
         S.bk_known = b + 3;
+        const long long t_fence = PROF ? clock64() : 0;
         __threadfence();
         asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(a.published), "r"((unsigned)(b + 1)) : "memory");
         S.chain = chain_pack(g + 1, c);
+        if (PROF) {
+          const long long t_done = clock64();
+          trace_turn(t_land, t4, 0, 0, t_fence, t_done, 1ull | ((unsigned long long)b << 32), c - lo);
+        }
         if (PROF && S.bk_ring[b & 7] < a.n_cons / 4) a.stats[15] = (unsigned long long)(clock64() - t_start);  // timeline: end of the first quarter
       }
       __syncwarp();
@@ -1454,6 +1496,8 @@ __device__ void commit_warp(const MatchArgs& a, ResolverShared& S, const Latest 
     bool more = false, have = false;
     int c_seen = s;
     long long t1 = PROF ? clock64() : 0;
+    long long t_ready = 0, t_seen = 0;               // PROF: end of the (first) first look, turn observed
+    unsigned n_fold = 0, n_rel = 0, slow = 0;        // PROF: entries folded one by one, relooks, slow turn
     unsigned long long w;
     int c = 0;
   relook:
@@ -1491,12 +1535,14 @@ __device__ void commit_warp(const MatchArgs& a, ResolverShared& S, const Latest 
         }
         have = true;
         if (mine) n_slow_turn++;
+        if (PROF && t_ready == 0) { t_ready = clock64(); slow = mine ? 1u : 0u; }
         continue;
       }
       if (mine && c_now <= c_seen + 1) { c = c_now; break; }
       if (c_now > c_seen) {
         // (b) one more entry, not the last before the turn: every lane evaluates it (uniform)
         // and the list is updated without a warp collective
+        if (PROF) n_fold++;
         int nvm, kk;
         const VmState ne = load_log<CONSTR>(S, c_seen, nvm, kk);
         const double nf = eval_res<CONSTR>(a, r, nvm, ne, grp, CONSTR ? sb_shared(sbw, nvm) : true);
@@ -1536,6 +1582,7 @@ __device__ void commit_warp(const MatchArgs& a, ResolverShared& S, const Latest 
     }
     long long t2 = PROF ? clock64() : 0;
     if (PROF) prof[1] += (unsigned long long)(t2 - t1);
+    if (PROF && t_seen == 0) t_seen = t2;   // a relook after this point belongs to the turn
     // ---- the turn: c == c_seen (nothing new) or c == c_seen + 1 (one new entry)
     VmState ne;
     ne.ac = ne.am = ne.lc = ne.lm = ne.rc = ne.rm = ne.yc = ne.ym = 0.0; ne.an = ne.pu = 0;
@@ -1555,6 +1602,7 @@ __device__ void commit_warp(const MatchArgs& a, ResolverShared& S, const Latest 
       // lanes' items again at the current version; the list is exact again afterwards
       have = false;
       n_relook++;
+      if (PROF) n_rel++;
       goto relook;
     }
     const double pf = first ? (d > 0 ? tf[0] : 0.0) : (d > 1 ? tf[1] : 0.0);
@@ -1569,6 +1617,10 @@ __device__ void commit_warp(const MatchArgs& a, ResolverShared& S, const Latest 
     // everything known is worse than the bound, the bound is a real VM and nothing touched it
     // since s: it is the best VM outside the set, hence the winner
     const bool take_z = !exact && known && R->z_real != 0 && ne_vm != r_zv && latest.get(r_zv) < s;
+    // PROF: stamps taken under a predicate computed from the value, so they wait for it
+    long long t_eval = 0, t_dec = 0;
+    if (PROF && __double_as_longlong(nf) != 0x7ff8deadbeef0000ll) t_eval = clock64();
+    if (PROF && (__double_as_longlong(wf) != 0x7ff8deadbeef0000ll || take_z)) t_dec = clock64();
     int wv = -1;
     auto append = [&](int vm, VmState st) {  // lane 0: the placement becomes log entry c
       st.ac = st.ac + r.c; st.am = st.am + r.m; st.an += 1; st.pu += r.ports;
@@ -1578,9 +1630,11 @@ __device__ void commit_warp(const MatchArgs& a, ResolverShared& S, const Latest 
       fence_cta();
       S.chain = chain_pack(g + 1, c + 1);
     };
+    bool wv_group = false;  // PROF: the group path was taken
     if (grp && group_version(a, r.j) != R->gver) {
       // a member of one of the job's groups was placed since the result was computed: the group
       // constraints it was filtered with are stale => exact full scan against the live state
+      if (PROF) wv_group = true;
       const QEntry q2 = qe;
       VmState ws;
       wv = resolve_group_job<CONSTR>(a, S, latest, q2, ws);  // uniform across lanes
@@ -1620,6 +1674,13 @@ __device__ void commit_warp(const MatchArgs& a, ResolverShared& S, const Latest 
         else S.chain = chain_pack(g + 1, c);
       }
       if (got) wv = 0;
+    }
+    if (PROF) {
+      const long long t_done = clock64();
+      const unsigned path = wv_group ? TP_GROUP : take_z ? TP_ZTAKE : exact ? TP_EXACT : TP_FALLBACK;
+      trace_turn(t_ready, t_seen, t_eval, t_dec, 0, t_done, (unsigned long long)(path << 4 | min(n_rel, 15u) << 8 | min(n_fold, 255u) << 12 |
+                                                          slow << 20 | (wv >= 0 ? 1u : 0u) << 21) |
+                                         ((unsigned long long)qe.blk << 32), k);
     }
     if (wv >= 0) n_matched++;
     __syncwarp();
@@ -1665,7 +1726,7 @@ __global__ void __launch_bounds__(RES_THREADS, 1) match_kernel(MatchArgs a) {
     if (blockIdx.x == 0) {
       // warps 0..3 sit on different schedulers (warp id mod 4): one commit warp each
       if (warp < NCW) commit_warp<CONSTR, PROF>(a, S, latest, warp, sbw_base + (size_t)warp * a.sb_words);
-      else if (warp == NCW) driver_warp<CONSTR, false>(a, S);
+      else if (warp == NCW) driver_warp<CONSTR, false, PROF>(a, S);
       else if (warp == NCW + 1) publisher_warp<CONSTR>(a, S);
       else if (warp == NCW + 2) fetcher_warp(a, S);
     } else {
@@ -2620,6 +2681,17 @@ int32_t match_run(cook_pool* pool, int32_t* out_considerable, int64_t* out_job_i
   int n_used = 0;
   unsigned long long hstats[32] = {0};
   const bool prof_on = getenv("COOK_PROF") != nullptr;
+  const char* trace_path = prof_on ? getenv("COOK_PROF_TRACE") : nullptr;
+  // The timeline's pointers are device globals of this module: PROF runs go one at a time per process, so
+  // that two pools on one device do not arm them over each other.  The buffer is freed on every return.
+  static std::mutex prof_mu;
+  std::unique_lock<std::mutex> prof_lock(prof_mu, std::defer_lock);
+  if (prof_on) prof_lock.lock();
+  struct TraceBuf {
+    unsigned long long* p = nullptr;
+    ~TraceBuf() { if (p) cudaFree(p); }
+  } trace;
+  int trace_caps[2] = {0, 0};
   CK(pool, cudaEventRecord(pool->ev[5], st));
   if (n_cons > 0) {
     if (O == 0) {
@@ -2688,6 +2760,22 @@ int32_t match_run(cook_pool* pool, int32_t* out_considerable, int64_t* out_job_i
       n_spec = std::max(1, std::min(n_spec, std::min(MAX_SPEC_CTAS, std::max(1, grid / 8))));
       n_spec = std::min(n_spec, grid - 2);
       ma.n_spec = n_spec;
+      if (prof_on) {  // per-turn timeline: armed only when a file asks for it
+        int caps[2] = {0, 0};
+        if (trace_path) {
+          caps[0] = n_cons + mp->max_blocks + 8;
+          caps[1] = mp->max_blocks + 8;
+          CK(pool, cudaMalloc(&trace.p, sizeof(unsigned long long) * ((size_t)caps[0] * TURN_WORDS + caps[1])));
+          CK(pool, cudaMemsetAsync(trace.p, 0, sizeof(unsigned long long) * ((size_t)caps[0] * TURN_WORDS + caps[1]), st));
+        }
+        unsigned long long* d_blk = trace.p ? trace.p + (size_t)caps[0] * TURN_WORDS : nullptr;
+        CK(pool, cudaMemcpyToSymbolAsync(g_turn_trace, &trace.p, sizeof(trace.p), 0, cudaMemcpyHostToDevice, st));
+        CK(pool, cudaMemcpyToSymbolAsync(g_blk_trace, &d_blk, sizeof(d_blk), 0, cudaMemcpyHostToDevice, st));
+        CK(pool, cudaMemcpyToSymbolAsync(g_turn_cap, &caps[0], sizeof(int), 0, cudaMemcpyHostToDevice, st));
+        CK(pool, cudaMemcpyToSymbolAsync(g_blk_cap, &caps[1], sizeof(int), 0, cudaMemcpyHostToDevice, st));
+        CK(pool, cudaStreamSynchronize(st));   // the caps live on this stack frame
+        trace_caps[0] = caps[0]; trace_caps[1] = caps[1];
+      }
       void* kargs[] = {&ma};
       CK(pool, cudaLaunchCooperativeKernel(kfn, dim3(grid), dim3(RES_THREADS), kargs, smem, st));
       launches++;
@@ -2724,6 +2812,18 @@ int32_t match_run(cook_pool* pool, int32_t* out_considerable, int64_t* out_job_i
                           "c_end_block", "c_fallback", "res_total", "res_q1_done", "eval_work", "eval_wait",
                           "eval_loop", "eval_sync", "eval_merge", "eval_work_q1", "eval_rowslots_q1", "blocks", "z_takes", "relooks", "rows_pretest_ei0"};
     for (int i = 0; i < 27; i++) fprintf(stderr, "[cook_prof] %-14s %llu\n", nm[i], hstats[i]);
+  }
+  if (trace.p) {
+    // header (8 x i64): magic, turn rows, block rows, words per turn row, resolver clocks, n_cons, matched, 0
+    const size_t nw = (size_t)trace_caps[0] * TURN_WORDS + trace_caps[1];
+    std::vector<unsigned long long> h(8 + nw);
+    h[0] = 0x314e5254ull; h[1] = trace_caps[0]; h[2] = trace_caps[1]; h[3] = TURN_WORDS;
+    h[4] = hstats[14]; h[5] = (unsigned long long)n_cons; h[6] = hstats[3]; h[7] = 0;
+    CK(pool, cudaMemcpy(h.data() + 8, trace.p, nw * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    if (FILE* f = fopen(trace_path, "wb")) {
+      fwrite(h.data(), sizeof(unsigned long long), h.size(), f);
+      fclose(f);
+    }
   }
   mp->last_n_cons = n_cons;
   record_phase(pool, COOK_PHASE_MATCH, uploaded ? pool->ev[0] : nullptr, pool->ev[1], pool->ev[3], pool->ev[4],
