@@ -274,24 +274,54 @@ def ptr(arr, ctype):
     return arr.ctypes.data_as(ctype)
 
 
-_STATE_MATCH = [C.c_void_p, C.POINTER(OffersSoA), C.POINTER(Groups), C.POINTER(UserTable), C.POINTER(PoolQuota),
-                C.POINTER(MatchParams), P_I64, P_I32, P_I32, C.c_int32, P_U8, C.POINTER(MatchStats)]
-_STATE_REBALANCE = [C.c_void_p, C.POINTER(HostTable), C.POINTER(Groups), C.POINTER(UserTable),
-                    C.POINTER(RebalanceParams), C.POINTER(Decision), P_I64, P_I64, C.c_int32, C.POINTER(C.c_int32)]
-# ctypes argument types of the entry points that declare them (engine.load_library sets them); the derived calls
-# take exactly cook_state_match's and cook_state_rebalance's arguments
+_H = C.c_void_p                   # an opaque handle (cook_ctx*, cook_pool*) or a void*
+_P = C.POINTER
+_I32 = C.c_int32
+_STATE_MATCH = [_H, _P(OffersSoA), _P(Groups), _P(UserTable), _P(PoolQuota), _P(MatchParams), P_I64, P_I32, P_I32,
+                _I32, P_U8, _P(MatchStats)]
+_STATE_REBALANCE = [_H, _P(HostTable), _P(Groups), _P(UserTable), _P(RebalanceParams), _P(Decision), P_I64, P_I64,
+                    _I32, P_I32]
+_REBALANCE = [_H, _P(RunningSoA), _P(JobsSoA), P_I64, P_I32, _P(HostTable), _P(Groups), _P(UserTable),
+              _P(RebalanceParams), _P(Decision), P_I32, P_I32]
+_STATE_RANK = [_H, _P(UserTable), _P(PoolQuota), _P(PoolQuota), P_F64, _P(RankParams), P_I64, P_I32]
+# ctypes argument types of every int32_t entry point of include/cook_gpu.h; engine.load_library sets them, and
+# restype c_int32, on each.  The derived calls take exactly cook_state_match's and cook_state_rebalance's arguments.
 ARGTYPES = {
+    "cook_gpu_init": [_P(GpuConfig), _P(_H)],
+    "cook_gpu_shutdown": [_H],
+    "cook_pool_open": [_H, C.c_char_p, _I32, _I32, _P(_H)],
+    "cook_pool_close": [_H],
+    "cook_last_error": [_H, C.c_char_p, _I32],
+    "cook_rank": [_H, _P(TasksSoA), _P(TasksSoA), _P(UserTable), _P(PoolQuota), _P(PoolQuota), P_F64, _P(RankParams),
+                  P_I32, P_I32, P_F64, P_I32, P_I32],
+    "cook_match": [_H, P_I32, _I32, _P(JobsSoA), _P(OffersSoA), _P(Groups), _P(UserTable), _P(PoolQuota),
+                   _P(MatchParams), P_I32, P_I32, P_I32, _I32, P_U8, _P(MatchStats)],
+    "cook_match_failures": [_H, P_I32, _I32, _P(FailureCounts)],
+    "cook_rebalance": _REBALANCE,
+    "cook_rebalance_trace": _REBALANCE + [_P(RebTrace)],
+    "cook_state_apply": [_H, _P(StateDelta)],
+    "cook_state_launch": [_H, _I32, P_I64, P_I64, P_I64, P_I32],
+    "cook_state_patch": [_H, _I32, P_I64, P_U8, P_U8, P_I32, _I32],
+    "cook_state_rank": _STATE_RANK,
+    "cook_state_rank_offensive": _STATE_RANK + [P_I64, _I32, P_I32],
+    "cook_state_match": _STATE_MATCH,
+    "cook_state_rebalance": _STATE_REBALANCE,
+    "cook_state_usage": [_H, _I32, P_F64, P_F64, _I32, P_I32, P_F64, P_F64, P_I32],
+    "cook_state_cotasks": [_H, _I32, P_I32, _P(HostTable), _I32, P_I32, P_I32, P_I32, P_I32],
     "cook_state_match_derived": _STATE_MATCH,
     "cook_state_rebalance_derived": _STATE_REBALANCE,
-    "cook_state_considerable": [C.c_void_p, C.POINTER(UserTable), C.POINTER(PoolQuota), C.POINTER(ConsiderableParams),
-                                P_I64, P_I32],
-    "cook_state_digest": [C.c_void_p, C.c_int32, C.POINTER(StateDigest), C.POINTER(Fp), C.POINTER(Fp)],
+    "cook_state_considerable": [_H, _P(UserTable), _P(PoolQuota), _P(ConsiderableParams), P_I64, P_I32],
+    "cook_state_digest": [_H, _I32, _P(StateDigest), _P(Fp), _P(Fp)],
     "cook_state_counts_compare": [P_I64, P_I64, P_I32],
-    "cook_state_export": [C.c_void_p, C.c_int32, P_U8, C.POINTER(StateSizes), C.POINTER(StateRows),
-                          C.POINTER(StateSizes)],
-    "cook_state_queue": [C.c_void_p, C.c_int32, P_I64, P_I32],
-    "cook_state_rank_offensive": [C.c_void_p, C.POINTER(UserTable), C.POINTER(PoolQuota), C.POINTER(PoolQuota), P_F64,
-                                  C.POINTER(RankParams), P_I64, P_I32, P_I64, C.c_int32, P_I32],
+    "cook_state_export": [_H, _I32, P_U8, _P(StateSizes), _P(StateRows), _P(StateSizes)],
+    "cook_state_queue": [_H, _I32, P_I64, P_I32],
+    "cook_last_stats": [_H, _I32, _P(PhaseStats)],
+    "cook_allgather_usage": [_H, _H, P_F64, P_F64, C.c_int64],
+    "cook_comm_unique_id": [P_U8],
+    "cook_comm_init": [P_U8, _I32, _I32, _I32, _P(_H)],
+    "cook_comm_destroy": [_H],
+    "cook_exchange_usage": [_H, _H, _I32, _I32, P_F64],
+    "cook_exchange_usage_batch": [_P(_H), _I32, _H, _I32, _I32, _I32, P_F64],
 }
 
 

@@ -57,18 +57,9 @@ def load_library(path=None):
             "(nvcc, sm_90a). There is no CPU fallback.")
     lib = C.CDLL(path)
     lib.cook_gpu_version.restype = C.c_char_p
-    for name in ("cook_gpu_init", "cook_gpu_shutdown", "cook_pool_open", "cook_pool_close",
-                 "cook_last_error", "cook_rank", "cook_match", "cook_rebalance",
-                 "cook_allgather_usage", "cook_last_stats", "cook_comm_unique_id", "cook_comm_init",
-                 "cook_comm_destroy", "cook_exchange_usage", "cook_exchange_usage_batch", "cook_rebalance_trace",
-                 "cook_match_failures", "cook_state_apply", "cook_state_rank", "cook_state_match",
-                 "cook_state_rebalance", "cook_state_launch", "cook_state_patch", "cook_state_usage",
-                 "cook_state_cotasks", "cook_state_match_derived", "cook_state_rebalance_derived",
-                 "cook_state_considerable", "cook_state_rank_offensive", "cook_state_digest",
-                 "cook_state_counts_compare", "cook_state_export", "cook_state_queue"):
-        getattr(lib, name).restype = C.c_int32
     for name, argtypes in abi.ARGTYPES.items():
-        getattr(lib, name).argtypes = argtypes
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = C.c_int32, argtypes
     return lib
 
 

@@ -211,14 +211,14 @@ def test_rebalance_trace_equals_oracle(gpu, oracle, name, regime):
 @pytest.mark.parametrize("name,regime", STATE, ids=ids(STATE))
 def test_state_rebalance_equals_oracle(oracle, name, regime):
     """The same rows through the resident state: victims as task ids, a synthetic one as -1 - e."""
-    from test_state_rebalance import RPool, rows_of
+    from resident_model import Pool, rows_of
     r, codes = CASES[name](regime)
     pend, run = rows_of(r, codes)
-    p = RPool(r, codes)
+    p = Pool.of_rebalance(r, codes)
     try:
         p.apply(up=sorted(pend.items()), run_up=list(run.values()))
-        assert p.rank() == [int(j) for j in r["pending_job_id"]]
-        got = p.check(oracle)
+        assert p.rank().tolist() == [int(j) for j in r["pending_job_id"]]
+        got = p.check_rebalance(oracle)
         want = oracle.rebalance(*_args(r))
         tid = [t["task_id"] for t in r["case"].tasks]
         R = len(tid)

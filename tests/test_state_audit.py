@@ -10,8 +10,6 @@ divergence drill repaired by cycle.resync; the edges, errors and transfer formul
 """
 import ctypes as C
 import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -19,14 +17,8 @@ import pytest
 import state_digest_ref as R
 from cook_b200 import abi, cycle, engine, traces
 from cook_b200.engine import CookError, GpuEngine
+from resident_model import OPTIONAL, START, pending_kw, pool_rows, rebalance_trace, rows_of, running_kw
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-START = 1_700_000_000_000
-OPTIONAL = ("gpus", "ports", "allowed", "plugin_accept", "gpu_model", "disk_request", "disk_type", "est_end_ms",
-            "ckpt_location", "reserved_host")
-DT = dict(cpus=np.float64, mem=np.float64, gpus=np.float64, ports=np.int32, allowed=np.uint8, plugin_accept=np.uint8,
-          gpu_model=np.int32, disk_request=np.float64, disk_type=np.int32, est_end_ms=np.int64, ckpt_location=np.int32,
-          reserved_host=np.int32)
 
 # two pending and two running rows whose hashes an independent C program computed from the header's definition
 PEND_A = dict(user=3, priority=50, cpus=1.5, mem=2048.0)
@@ -48,56 +40,6 @@ def test_hash_pinned():
     assert R.queue_fingerprint([1001, -7]) == (0x78510fc1fc93719c, 0x782c8fb9f34c8d5a, 2)
     assert R.queue_fingerprint([]) == (0, 0, 0)
     assert R.bucket(1001, 16) == 3 and R.bucket(-7, 65536) == 63219
-
-
-def test_layouts_and_prototypes(tmp_path):
-    cc = shutil.which("cc") or shutil.which("gcc")
-    if cc is None:
-        pytest.skip("no C compiler")
-    structs = [("cook_fp", abi.Fp), ("cook_state_digest_out", abi.StateDigest), ("cook_jobs_rows", abi.JobsRows),
-               ("cook_tasks_rows", abi.TasksRows), ("cook_state_rows", abi.StateRows), ("cook_state_sizes", abi.StateSizes)]
-    lines, want = [], []
-    for name, cls in structs:
-        lines.append(f'  printf("%zu\\n", sizeof({name}));')
-        want.append(C.sizeof(cls))
-        for f, _ in cls._fields_:
-            lines.append(f'  printf("%zu\\n", offsetof({name}, {f}));')
-            want.append(getattr(cls, f).offset)
-    lines.append('  printf("%d\\n%d\\n", (int)COOK_PHASE_AUDIT, (int)COOK_AUDIT_N);')
-    want += [abi.PHASE_AUDIT, abi.AUDIT_N]
-    # the prototypes: assigning each function to a pointer of the mirrored type fails to compile when they differ
-    protos = ('  int32_t (*d)(cook_pool*, int32_t, cook_state_digest_out*, cook_fp*, cook_fp*) = cook_state_digest;\n'
-              '  int32_t (*e)(cook_pool*, int32_t, const uint8_t*, const cook_state_sizes*, const cook_state_rows*,\n'
-              '               cook_state_sizes*) = cook_state_export;\n'
-              '  int32_t (*q)(cook_pool*, int32_t, int64_t*, int32_t*) = cook_state_queue;\n'
-              '  int32_t (*c)(const int64_t*, const int64_t*, int32_t*) = cook_state_counts_compare;\n'
-              '  (void)d; (void)e; (void)q; (void)c;\n')
-    src = tmp_path / "layout.c"
-    src.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "cook_gpu.h"\nint main(void) {\n' + protos +
-                   "\n".join(lines) + "\n  return 0;\n}\n")
-    obj = tmp_path / "layout.o"
-    subprocess.check_call([cc, "-Werror", "-I", os.path.join(ROOT, "include"), "-c", str(src), "-o", str(obj)])
-    # sizes and offsets are compile-time constants: a second unit without the function references links and runs
-    src2 = tmp_path / "sizes.c"
-    src2.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "cook_gpu.h"\nint main(void) {\n' +
-                    "\n".join(lines) + "\n  return 0;\n}\n")
-    exe = tmp_path / "sizes"
-    subprocess.check_call([cc, "-I", os.path.join(ROOT, "include"), str(src2), "-o", str(exe)])
-    assert [int(x) for x in subprocess.check_output([str(exe)]).split()] == want
-    assert abi.PHASE_AUDIT == 8 and [n for n, _ in abi.JobsRows._fields_] == [n for n, _ in abi.JobsSoA._fields_][1:]
-    assert C.sizeof(abi.Fp) == abi.FP_DTYPE.itemsize == 24
-
-
-def test_symbols_exported():
-    hdr = open(os.path.join(ROOT, "include", "cook_gpu.h")).read()
-    for name in ("cook_state_digest", "cook_state_export", "cook_state_queue"):
-        assert f"int32_t {name}(cook_pool* pool" in hdr
-    if not os.path.exists(engine.LIB_PATH):
-        pytest.skip("libcookgpu.so not built")
-    lib = engine.load_library()
-    for name in ("cook_state_digest", "cook_state_export", "cook_state_queue", "cook_state_counts_compare"):
-        assert hasattr(lib, name)
-    assert all(callable(getattr(GpuEngine, m)) for m in ("state_digest", "state_export", "state_queue"))
 
 
 def test_counts_compare():
@@ -182,37 +124,6 @@ def test_fingerprint_properties():
 
 
 # ---- rows <-> deltas -------------------------------------------------------------------------------------------
-def pending_kw(rows, drop=()):
-    """make_delta's pending arguments of [(job id, row)]; the columns and lists in `drop` are passed as NULL."""
-    n = len(rows)
-    kw = dict(user=np.array([r["user"] for _, r in rows], np.int32), cpus=np.array([r["cpus"] for _, r in rows]),
-              mem=np.array([r["mem"] for _, r in rows]))
-    for c in OPTIONAL:
-        if c not in drop:
-            kw[c] = np.array([r[c] for _, r in rows], DT[c])
-    if "novel" not in drop:
-        kw["novel_off"], kw["novel_host"] = abi.csr([r["novel"] for _, r in rows])
-    if "attr" not in drop:
-        kw["attr_off"], kw["attr_col"] = abi.csr([[c for c, _ in r["attr"]] for _, r in rows])
-        kw["attr_val"] = abi.csr([[v for _, v in r["attr"]] for _, r in rows])[1]
-    if "groups" not in drop:
-        kw["group_off"], kw["group_idx"] = abi.csr([r["groups"] for _, r in rows])
-    return dict(pending=abi.JobsSoA(n=n, **kw), pending_priority=np.array([r["priority"] for _, r in rows], np.int32),
-                pending_job_id=np.array([j for j, _ in rows], np.int64))
-
-
-def running_kw(rows, hosts=True, lists=True, gpus=True):
-    t = {k: np.array([r[k] for r in rows], np.int64 if k in ("start_time", "task_id", "job_id") else
-                     np.int32 if k in ("user", "priority") else np.float64)
-         for k in ("user", "priority", "start_time", "task_id", "job_id", "cpus", "mem")}
-    kw = dict(running=abi.TasksSoA(n=len(rows), gpus=np.array([r["gpus"] for r in rows]) if gpus else None, **t))
-    if hosts:
-        kw["running_hostname_id"] = np.array([r["host"] for r in rows], np.int32)
-    if lists:
-        kw["running_group_off"], kw["running_group_idx"] = abi.csr([r["groups"] for r in rows])
-    return kw
-
-
 def without(row, drop):
     """The row a delta stores when the columns and lists in `drop` are NULL."""
     row = dict(row)
@@ -418,7 +329,6 @@ def test_resync_on_models():
 def c3_rows(seed, n_jobs=1500, n_running=500, rng=None):
     """A config-#3 pool as model rows: every pending column and list in use, amounts on and off the 2^-10 grid,
     running rows with hosts and group lists."""
-    from test_state_resident import pool_rows
     t = traces.gen_c3_pool(seed, n_jobs=n_jobs, n_offers=160, n_users=24, n_running=n_running)
     rng = rng or np.random.default_rng(seed)
     pend, run = pool_rows(t)
@@ -519,7 +429,6 @@ def test_layout_independence():
 def test_round_trip_rank_match_rebalance():
     """export -> a reset delta on a fresh handle -> equal digest; then rank and a config-#3 match with groups, and a
     config-#4 rebalance, bit-identical on the two handles."""
-    from test_state_rebalance import _pool, rows_of
     t, pend, run = c3_rows(41)
     a, b = Twin("orig"), Twin("copy")
     try:
@@ -538,7 +447,7 @@ def test_round_trip_rank_match_rebalance():
         for k in ("considerable", "assign", "ports", "fail"):
             assert np.array_equal(ma[k], mb[k]), k
         assert (ma["assign"] >= 0).any()
-        r, codes = _pool(23, True)
+        r, codes = rebalance_trace(23, True)
         rp, rr = rows_of(r, codes)
         a.apply(reset=True, up=[(j, dict(R.ABSENT, **x)) for j, x in sorted(rp.items())],
                 run_up=[dict(x, groups=[]) for x in rr.values()])

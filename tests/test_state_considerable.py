@@ -11,10 +11,6 @@ and transfers.
 """
 import ctypes as C
 import itertools
-import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -22,75 +18,13 @@ import pytest
 import considerable_ref as CR
 from cook_b200 import abi, cycle, engine, traces
 from cook_b200.engine import CookError, GpuEngine
+from resident_model import START, USAGE_FIELDS, Pool, c2, c3, churn, delta, drop_all_but, host_inputs, pool_rows
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-HDR = os.path.join(ROOT, "include", "cook_gpu.h")
 KEYS = ("count", "cpus", "mem", "gpus")
 QUOTA_FIELDS = ("quota_count", "quota_cpus", "quota_mem", "quota_gpus")
-USAGE_FIELDS = ("usage_count", "usage_cpus", "usage_mem", "usage_gpus")
-NEW = ("cook_state_considerable", "cook_state_rank_offensive")
 
 
 # ---- CPU -------------------------------------------------------------------------------------------------
-def _prototype(hdr, name):
-    m = re.search(r"int32_t\s+" + name + r"\s*\(([^)]*)\)\s*;", hdr)
-    assert m, name
-    return [" ".join(p.split()) for p in m.group(1).split(",")]
-
-
-def test_entries_exported():
-    hdr = open(HDR).read()
-    for name in NEW:
-        _prototype(hdr, name)
-    if not os.path.exists(engine.LIB_PATH):
-        pytest.skip("libcookgpu.so not built")
-    lib = engine.load_library()
-    for name in NEW:
-        assert hasattr(lib, name), name
-        assert getattr(lib, name).restype is C.c_int32
-        assert getattr(lib, name).argtypes == abi.ARGTYPES[name]
-
-
-# ctypes -> the C spelling the header uses
-_C_OF = {C.c_void_p: "cook_pool*", C.c_int32: "int32_t", abi.P_I64: "int64_t*", abi.P_I32: "int32_t*",
-         abi.P_F64: "const double*", C.POINTER(abi.UserTable): "const cook_user_table*",
-         C.POINTER(abi.PoolQuota): "const cook_pool_quota*", C.POINTER(abi.RankParams): "const cook_rank_params*",
-         C.POINTER(abi.ConsiderableParams): "const cook_considerable_params*"}
-_C_FIELD = {C.c_int32: "int32_t"}
-
-
-def test_layout_and_prototypes_compile(tmp_path):
-    cc = shutil.which("cc") or shutil.which("gcc")
-    if cc is None:
-        pytest.skip("no C compiler")
-    P = abi.ConsiderableParams
-    lines = ['#include <stddef.h>', '#include "cook_gpu.h"',
-             f'_Static_assert(sizeof(cook_considerable_params) == {C.sizeof(P)}, "size");']
-    for name, ct in P._fields_:
-        assert ct in _C_FIELD
-        lines.append(f'_Static_assert(offsetof(cook_considerable_params, {name}) == {getattr(P, name).offset}, "{name}");')
-        lines.append(f'_Static_assert(__builtin_types_compatible_p(__typeof__(((cook_considerable_params*)0)->{name}), '
-                     f'{_C_FIELD[ct]}), "{name} type");')
-    for fn in NEW:
-        args = ", ".join(_C_OF[t] for t in abi.ARGTYPES[fn])
-        lines.append(f'_Static_assert(__builtin_types_compatible_p(__typeof__({fn}), int32_t ({args})), "{fn}");')
-    lines.append('_Static_assert(COOK_PHASE_CONSIDERABLE == %d, "phase");' % abi.PHASE_CONSIDERABLE)
-    lines.append('_Static_assert(COOK_USAGE_GIVEN == %d && COOK_USAGE_DERIVED == %d && COOK_USAGE_LAST_MATCH == %d, '
-                 '"usage sources");' % (abi.USAGE_GIVEN, abi.USAGE_DERIVED, abi.USAGE_LAST_MATCH))
-    lines.append('int main(void) { return 0; }')
-    src = tmp_path / "layout.c"
-    src.write_text("\n".join(lines) + "\n")
-    subprocess.check_call([cc, "-std=gnu11", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(tmp_path / "l")])
-
-
-def test_phase_code():
-    assert abi.PHASE_CONSIDERABLE == 7
-    hdr = open(HDR).read()
-    assert re.search(r"COOK_PHASE_CONSIDERABLE\s*=\s*7", hdr)
-    # one more than the last phase before it
-    assert abi.PHASE_CONSIDERABLE == abi.PHASE_COTASKS + 1
-
-
 class RefEngine:
     """considerable_ref behind the `match` call shape the K14 / K9 cases use (considerable set only)."""
 
@@ -181,57 +115,39 @@ def _quota_users(base, rng):
 POOL_Q = {"count": 900.0, "cpus": 3000.0, "mem": 1e7, "gpus": 1e9}
 
 
-class Pool:
+def new_pool(t, users):
     """A resident handle (`gpu`), a host-table handle (`ref`) and the model of the rows."""
+    return Pool.of_trace(t, users=users, name="considerable")
 
-    def __init__(self, t, users):
-        from test_state_resident import Model
-        self.t, self.users, self.offers = t, users, t["offers"]
-        self.gpu, self.ref, self.m = GpuEngine(pool_name="considerable"), GpuEngine(pool_name="host"), Model()
-        self.queue, self.gone = [], set()
 
-    def close(self):
-        self.gpu.close()
-        self.ref.close()
+def usage_of(p):
+    return p.gpu.state_usage(p.users.n_users)["user"]
 
-    def apply(self, up=(), rm=(), run_up=(), run_rm=(), reset=False):
-        from test_state_resident import delta
-        self.gpu.state_apply(delta(reset, up, rm, run_up, run_rm))
-        self.m.apply(up, rm, run_up, run_rm, reset)
-        self.gone |= set(rm) | {j for j, _ in up}
 
-    def rank(self, **kw):
-        q = self.gpu.state_rank(self.users, **kw)
-        self.queue, self.gone = q.tolist(), set()
-        return q
-
-    def usage(self):
-        return self.gpu.state_usage(self.users.n_users)["user"]
-
-    def host_considerable(self, prm, usage, pool_q=None):
-        """cook_match on the model's tables, the live queue, an empty offer table; and considerable_ref."""
-        _, _, jobs, jid = self.m.tables()
-        pos = {j: i for i, j in enumerate(jid.tolist())}
-        ranked = np.array([pos[j] for j in self.queue if j not in self.gone], np.int32)
-        J = jobs.n
-        ones = np.ones(J, np.uint8)
-        al = ones if prm.quota_only else np.array([self.m.pend[j]["allowed"] for j in jid.tolist()], np.uint8)
-        pa = ones if prm.quota_only else np.array([self.m.pend[j]["plugin_accept"] for j in jid.tolist()], np.uint8)
-        plain = abi.JobsSoA(n=J, user=jobs.col("user"), cpus=jobs.col("cpus"), mem=jobs.col("mem"),
-                            gpus=jobs.col("gpus"), allowed=al, plugin_accept=pa)
-        users = _usage_users(self.users, usage)
-        if len(ranked) == 0:
-            return [], []
-        mp = traces.match_params(prm.num_considerable, enforce_rate_limit=prm.enforce_rate_limit)
-        pq = abi.make_pool_quota(pool_q) if pool_q else None
-        want = self.ref.match(ranked, plain, _empty_offers(), users, mp, pool_quota=pq)["considerable"]
-        quota = {k: self.users.col(f) for k, f in zip(KEYS, QUOTA_FIELDS)}
-        gpus = jobs.col("gpus") if jobs.col("gpus") is not None else np.zeros(J)   # an all-zero column is absent
-        ref = CR.considerable(ranked.tolist(), jobs.col("user"), jobs.col("cpus"), jobs.col("mem"), gpus,
-                              quota, usage, prm.num_considerable, tokens=self.users.col("tokens"),
-                              enforce_rate_limit=prm.enforce_rate_limit, pool_quota=pool_q, allowed=al,
-                              plugin_accept=pa)
-        return jid[want].tolist(), jid[np.array(ref, np.int64)].tolist() if ref else []
+def host_considerable(p, prm, usage, pool_q=None):
+    """cook_match on the model's tables, the live queue, an empty offer table; and considerable_ref."""
+    _, _, jobs, jid = p.tables()
+    pos = {j: i for i, j in enumerate(jid.tolist())}
+    ranked = np.array([pos[j] for j in p.live_queue()], np.int32)
+    J = jobs.n
+    ones = np.ones(J, np.uint8)
+    al = ones if prm.quota_only else np.array([p.pend[j]["allowed"] for j in jid.tolist()], np.uint8)
+    pa = ones if prm.quota_only else np.array([p.pend[j]["plugin_accept"] for j in jid.tolist()], np.uint8)
+    plain = abi.JobsSoA(n=J, user=jobs.col("user"), cpus=jobs.col("cpus"), mem=jobs.col("mem"),
+                        gpus=jobs.col("gpus"), allowed=al, plugin_accept=pa)
+    users = _usage_users(p.users, usage)
+    if len(ranked) == 0:
+        return [], []
+    mp = traces.match_params(prm.num_considerable, enforce_rate_limit=prm.enforce_rate_limit)
+    pq = abi.make_pool_quota(pool_q) if pool_q else None
+    want = p.ref.match(ranked, plain, _empty_offers(), users, mp, pool_quota=pq)["considerable"]
+    quota = {k: p.users.col(f) for k, f in zip(KEYS, QUOTA_FIELDS)}
+    gpus = jobs.col("gpus") if jobs.col("gpus") is not None else np.zeros(J)   # an all-zero column is absent
+    ref = CR.considerable(ranked.tolist(), jobs.col("user"), jobs.col("cpus"), jobs.col("mem"), gpus,
+                          quota, usage, prm.num_considerable, tokens=p.users.col("tokens"),
+                          enforce_rate_limit=prm.enforce_rate_limit, pool_quota=pool_q, allowed=al,
+                          plugin_accept=pa)
+    return jid[want].tolist(), jid[np.array(ref, np.int64)].tolist() if ref else []
 
 
 def _combos():
@@ -241,7 +157,7 @@ def _combos():
 
 def _match_derived(p, nc=400):
     """A derived match on the resident handle; returns it and the usage it read (cook_state_usage before it)."""
-    usage = p.usage()
+    usage = usage_of(p)
     users = _with(p.users, **{f: None for f in USAGE_FIELDS})
     offers = _with_offers(p.offers)
     got = p.gpu.state_match(offers, users, traces.match_params(nc), derived=True)
@@ -268,7 +184,7 @@ def _check(p, prm, usage, pool_q, given=None):
         users = _with(p.users, **{f: None for f in USAGE_FIELDS})
     pq = abi.make_pool_quota(pool_q) if pool_q else None
     got = p.gpu.state_considerable(users, prm, pool_quota=pq).tolist()
-    want, ref = p.host_considerable(prm, given if given is not None else usage, pool_q)
+    want, ref = host_considerable(p, prm, given if given is not None else usage, pool_q)
     assert got == want, "resident considerable != cook_match on host tables"
     assert got == ref, "resident considerable != considerable_ref"
     return got
@@ -278,10 +194,9 @@ def _check(p, prm, usage, pool_q, given=None):
 @pytest.mark.gpu
 @pytest.mark.parametrize("kind", ["c2", "c2_offgrid", "c3"])
 def test_churn_equivalence(kind):
-    from test_state_resident import _c2, _c3, _churn, pool_rows
-    t = {"c2": lambda: _c2(11), "c2_offgrid": lambda: _c2(12, cpus=(0.1, 0.5, 1.0, 2.7)), "c3": lambda: _c3(13)}[kind]()
+    t = {"c2": lambda: c2(11), "c2_offgrid": lambda: c2(12, cpus=(0.1, 0.5, 1.0, 2.7)), "c3": lambda: c3(13)}[kind]()
     rng = np.random.default_rng(7)
-    p = Pool(t, _quota_users(t["users"], rng))
+    p = new_pool(t, _quota_users(t["users"], rng))
     combos = _combos()
     try:
         pend, run = pool_rows(t)
@@ -294,21 +209,21 @@ def test_churn_equivalence(kind):
         for batch in range(9):
             p.rank()
             got, last = _match_derived(p)
-            now = p.usage()
+            now = usage_of(p)
             given = _given_usage(p, rng)
             for _ in range(8):
                 qo, src, enf, pq, nc = combos[k % len(combos)]
                 k += 1
-                n_live = len([j for j in p.queue if j not in p.gone])
+                n_live = len(p.live_queue())
                 prm = _params(n_live + 37 if nc < 0 else nc, enf, qo, src)
                 usage = {abi.USAGE_GIVEN: given, abi.USAGE_DERIVED: now, abi.USAGE_LAST_MATCH: last}[src]
                 _check(p, prm, usage, pq, given=given if src == abi.USAGE_GIVEN else None)
             launched = [int(j) for j, a in zip(got["considerable"], got["assign"]) if a >= 0][:40]
-            up, rm, run_up, run_rm = _churn(p, rng, reserve, t_next, launched)
+            up, rm, run_up, run_rm = churn(p, rng, reserve, t_next, launched)
             p.apply(up, rm, run_up, run_rm)
             # between rank and the next calls the queue loses what the churn removed or replaced
             prm = _params(1000, 1, 0, abi.USAGE_DERIVED)
-            _check(p, prm, p.usage(), POOL_Q)
+            _check(p, prm, usage_of(p), POOL_Q)
         assert k >= len(combos)
     finally:
         p.close()
@@ -316,13 +231,12 @@ def test_churn_equivalence(kind):
 
 @pytest.mark.gpu
 def test_layout_independence():
-    from test_state_resident import _c2, pool_rows
-    t = _c2(21, cpus=(0.1, 0.5, 1.0, 2.0))
+    t = c2(21, cpus=(0.1, 0.5, 1.0, 2.0))
     rng = np.random.default_rng(4)
     users = _quota_users(t["users"], rng)
     pend, run = pool_rows(t)
     items = sorted(pend.items())
-    a, b = Pool(t, users), Pool(t, users)
+    a, b = new_pool(t, users), new_pool(t, users)
     try:
         a.apply(up=items, run_up=list(run.values()))
         junk = [(10 ** 11 + i, items[i][1]) for i in range(500)]
@@ -344,10 +258,9 @@ def test_layout_independence():
 
 @pytest.mark.gpu
 def test_autoscaling_after_match():
-    from test_state_resident import _c2, pool_rows
-    t = _c2(31)
+    t = c2(31)
     rng = np.random.default_rng(9)
-    p = Pool(t, _quota_users(t["users"], rng))
+    p = new_pool(t, _quota_users(t["users"], rng))
     try:
         pend, run = pool_rows(t)
         p.apply(up=sorted(pend.items()), run_up=list(run.values()))
@@ -355,11 +268,11 @@ def test_autoscaling_after_match():
         got, usage = _match_derived(p, nc=300)
         placed = [(int(j), int(a)) for j, a in zip(got["considerable"], got["assign"]) if a >= 0]
         assert placed
-        _, _, jobs, jid = p.m.tables()
+        _, _, jobs, jid = p.tables()
         pos = {j: i for i, j in enumerate(jid.tolist())}
         hid = p.offers.col("hostname_id")
-        p.gpu.state_launch([j for j, _ in placed], [5 * 10 ** 9 + i for i in range(len(placed))],
-                           np.full(len(placed), 1_700_000_000_000, np.int64), [int(hid[a]) for _, a in placed])
+        p.launch([j for j, _ in placed], [5 * 10 ** 9 + i for i in range(len(placed))],
+                 np.full(len(placed), START, np.int64), [int(hid[a]) for _, a in placed])
         gone = {j for j, _ in placed}
         queue_after = np.array([pos[j] for j in p.queue if j not in gone], np.int32)
         n_cons = len(got["considerable"])
@@ -388,22 +301,15 @@ def _hosted(run, hid):
 
 
 def _apply_hosted(p, items, run_rows):
-    from test_state_resident import jobs_soa, tasks_soa
-    pj, pp, jid = jobs_soa(items)
-    p.gpu.state_apply(abi.make_delta(reset=True, pending=pj, pending_priority=pp, pending_job_id=jid,
-                                     running=tasks_soa(run_rows),
-                                     running_hostname_id=np.array([r["host"] for r in run_rows], np.int32)))
-    p.m.apply(items, (), run_rows, (), True)
+    p.apply(items, (), run_rows, (), True, hosts=True)
 
 
 @pytest.mark.gpu
 def test_consume():
-    from test_state_derived import host_inputs
-    from test_state_resident import _c2, pool_rows
-    t = _c2(41)
+    t = c2(41)
     rng = np.random.default_rng(2)
     users = _quota_users(t["users"], rng)
-    p, twin = Pool(t, users), Pool(t, users)
+    p, twin = new_pool(t, users), new_pool(t, users)
     try:
         pend, run = pool_rows(t)
         items = sorted(pend.items())
@@ -428,13 +334,13 @@ def test_consume():
         for x, y in zip(cot0, p.gpu.state_cotasks(4)):
             assert np.array_equal(x, y)
         # a second call takes the next jobs: the host tables' queue leaves out the consumed ones
-        second = _check(p, _params(150, source=abi.USAGE_DERIVED, consume=1), p.usage(), None)
+        second = _check(p, _params(150, source=abi.USAGE_DERIVED, consume=1), usage_of(p), None)
         assert len(second) == 150 and not set(second) & set(first)
         p.gone |= set(second)
         taken = set(first) | set(second)
         # a patch does not bring an entry back
         p.gpu.state_patch(first[:50], allowed=np.ones(50, np.uint8))
-        third = _check(p, _params(1000, source=abi.USAGE_DERIVED), p.usage(), POOL_Q)
+        third = _check(p, _params(1000, source=abi.USAGE_DERIVED), usage_of(p), POOL_Q)
         assert not set(third) & taken
         # the twin removes the taken jobs after the same rank: its queue is the original one minus them
         twin.apply(rm=sorted(taken))
@@ -444,10 +350,10 @@ def test_consume():
         mt = twin.gpu.state_match(_with_offers(p.offers), du, prm, derived=True)
         for k in ("considerable", "assign", "ports", "fail"):
             assert np.array_equal(m[k], mt[k]), k
-        _, _, jobs, jid = p.m.tables()
+        _, _, jobs, jid = p.tables()
         pos = {j: i for i, j in enumerate(jid.tolist())}
         ranked = np.array([pos[j] for j in p.queue if j not in p.gone], np.int32)
-        ho, hu, _ = host_inputs(list(p.m.run.values()), p.offers, users, None)
+        ho, hu, _ = host_inputs(list(p.run.values()), p.offers, users, None)
         want = p.ref.match(ranked, jobs, ho, hu, prm)
         assert np.array_equal(m["considerable"], jid[want["considerable"]])
         assert np.array_equal(m["assign"], want["assign"])
@@ -463,18 +369,14 @@ def test_consume():
             assert np.array_equal(p.gpu.state_considerable(du, prm), twin.gpu.state_considerable(du, prm))
         # launching a consumed job works
         tids = [7 * 10 ** 9 + i for i in range(3)]
-        p.gpu.state_launch(first[:3], tids, np.full(3, 1, np.int64), [int(hn[0])] * 3)
-        new_rows = [dict(user=p.m.pend[j]["user"], priority=p.m.pend[j]["priority"], start_time=1, task_id=tid, job_id=j,
-                         cpus=p.m.pend[j]["cpus"], mem=p.m.pend[j]["mem"], gpus=p.m.pend[j]["gpus"], host=int(hn[0]))
-                    for j, tid in zip(first[:3], tids)]
-        p.m.apply((), first[:3], new_rows, ())
+        p.launch(first[:3], tids, np.full(3, 1, np.int64), [int(hn[0])] * 3)
         u2 = p.gpu.state_usage(nu)["user"]
         assert sum(u2["count"]) == sum(usage0["user"]["count"]) + 3
         # the next rank brings back every consumed job still pending
         q = p.rank()
         assert (taken - set(first[:3])) <= set(q.tolist())
         assert not set(first[:3]) & set(q.tolist())
-        _check(p, _params(len(q) + 10, source=abi.USAGE_DERIVED), p.usage(), None)
+        _check(p, _params(len(q) + 10, source=abi.USAGE_DERIVED), usage_of(p), None)
     finally:
         p.close()
         twin.close()
@@ -484,7 +386,7 @@ def _hosts_of(p):
     """A host table over the offers (every running row's host must be listed)."""
     o = p.offers
     hid = list(o.col("hostname_id"))
-    extra = sorted({int(r["host"]) for r in p.m.run.values() if "host" in r} - set(int(h) for h in hid))
+    extra = sorted({int(r["host"]) for r in p.run.values() if "host" in r} - set(int(h) for h in hid))
     codes = np.array(hid + extra, np.int32)
     H = len(codes)
     return abi.HostTable(n=H, hostname_id=codes, name_rank=np.argsort(np.argsort(codes)).astype(np.int32),
@@ -494,9 +396,8 @@ def _hosts_of(p):
 
 @pytest.mark.gpu
 def test_plan_untouched():
-    from test_state_resident import _c2, pool_rows
-    t = _c2(51)
-    p = Pool(t, _quota_users(t["users"], np.random.default_rng(1)))
+    t = c2(51)
+    p = new_pool(t, _quota_users(t["users"], np.random.default_rng(1)))
     try:
         pend, run = pool_rows(t)
         p.apply(up=sorted(pend.items()), run_up=list(run.values()))
@@ -518,17 +419,16 @@ def test_plan_untouched():
 
 @pytest.mark.gpu
 def test_offensive():
-    from test_state_resident import _c2, pool_rows
-    t = _c2(61)
+    t = c2(61)
     base = t["users"]
     pend, run = pool_rows(t)
     items = sorted(pend.items())
-    a, b = Pool(t, base), Pool(t, base)
+    a, b = new_pool(t, base), new_pool(t, base)
     try:
         for p in (a, b):
             p.apply(up=items, run_up=list(run.values()))
-        _, pending, jobs, jid = a.m.tables()
-        running = a.m.tables()[0]
+        _, pending, jobs, jid = a.tables()
+        running = a.tables()[0]
         cpus, mem = jobs.col("cpus"), jobs.col("mem")
         caps = (float(np.quantile(mem, 0.8)), float(np.quantile(cpus, 0.9)))
         # quotas above the running usage, that cut the queue part way (the pool quota counts the running tasks)
@@ -576,7 +476,7 @@ def test_offensive_quota_cuts_first():
     try:
         rows = [(i + 1, dict(user=0, priority=50, cpus=c, mem=m)) for i, (c, m) in
                 enumerate([(1.0, 100.0), (1.0, 5000.0), (1.0, 100.0), (1.0, 9000.0), (1.0, 100.0)])]
-        e.state_apply(_resident_delta(rows))
+        e.state_apply(delta(True, rows, drop=drop_all_but("gpus")))
         users = abi.make_users(1)
         prm = abi.RankParams(100, 1, 1000.0, 10.0)
         q, off = e.state_rank(users, params=prm, offensive=True)
@@ -588,16 +488,6 @@ def test_offensive_quota_cuts_first():
         e.close()
 
 
-def _resident_delta(rows):
-    """A delta of pending rows [(job id, {user, priority, cpus, mem[, gpus]})]."""
-    n = len(rows)
-    jobs = abi.JobsSoA(n=n, user=np.array([r["user"] for _, r in rows], np.int32),
-                       cpus=np.array([r["cpus"] for _, r in rows], float), mem=np.array([r["mem"] for _, r in rows], float),
-                       gpus=np.array([r.get("gpus", 0.0) for _, r in rows], float))
-    return abi.make_delta(reset=True, pending=jobs, pending_priority=np.array([r["priority"] for _, r in rows], np.int32),
-                          pending_job_id=np.array([j for j, _ in rows], np.int64))
-
-
 @pytest.mark.gpu
 def test_filter_offensive_jobs_reference():
     """test-filter-offensive-jobs (reference scheduler test :857-888) through resident deltas: with caps of 10 GB
@@ -606,7 +496,7 @@ def test_filter_offensive_jobs_reference():
     try:
         shapes = [(10.0, 10 * 1024.0), (30.0, 10 * 1024.0), (10.0, 12 * 1024.0), (5.0, 1024.0)]
         rows = [(100 + i, dict(user=0, priority=50 - i, cpus=c, mem=m)) for i, (c, m) in enumerate(shapes)]
-        e.state_apply(_resident_delta(rows))
+        e.state_apply(delta(True, rows, drop=drop_all_but("gpus")))
         q, off = e.state_rank(abi.make_users(1), params=abi.RankParams(100, 1, 10 * 1024.0, 20.0), offensive=True)
         assert q.tolist() == [100, 103]
         assert off.tolist() == [101, 102]
@@ -630,7 +520,7 @@ def test_k14_resident(monkeypatch):
             rows = [(int(j) + 1, dict(user=int(jobs.col("user")[j]), priority=50 + J - int(j),
                                       cpus=float(jobs.col("cpus")[j]), mem=float(jobs.col("mem")[j]),
                                       gpus=float(jobs.col("gpus")[j]))) for j in range(J)]
-            self.e.state_apply(_resident_delta(rows))
+            self.e.state_apply(delta(True, rows, drop=drop_all_but("gpus")))
             self.e.state_patch(np.arange(1, J + 1), plugin_accept=jobs.col("plugin_accept"))
             q = self.e.state_rank(abi.make_users(nu))
             assert q.tolist() == list(range(1, J + 1))   # priorities put the queue in job order
@@ -647,10 +537,9 @@ def test_k14_resident(monkeypatch):
 
 @pytest.mark.gpu
 def test_errors_and_transfers():
-    from test_state_resident import _c2, pool_rows
-    t = _c2(71)
+    t = c2(71)
     users = _quota_users(t["users"], np.random.default_rng(3))
-    p = Pool(t, users)
+    p = new_pool(t, users)
     try:
         du = _with(users, **{f: None for f in USAGE_FIELDS})
         with pytest.raises(CookError):   # no rank yet

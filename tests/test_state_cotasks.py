@@ -10,50 +10,18 @@ errors and transfer accounting; K13's group answers through the resident path; a
 and a config-#4 rebalance fed from the derived lists against the oracle and the host-table calls.
 """
 import ctypes as C
-import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
 from cook_b200 import abi, engine, traces
-from cook_b200.engine import GpuEngine
 from cotask_ref import cotasks
+from resident_model import (K13, START, Pool, group_pool, group_row, jobs_soa, keyed, pool_rows, rebalance_trace, rows_of,
+                            task_of, tasks_soa)
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-START = 1_700_000_000_000
 
 
 # ---- CPU -------------------------------------------------------------------------------------------------
-def test_state_delta_layout_with_group_lists(tmp_path):
-    cc = shutil.which("cc") or shutil.which("gcc")
-    if cc is None:
-        pytest.skip("no C compiler")
-    fields = [n for n, _ in abi.StateDelta._fields_]
-    assert fields[-2:] == ["running_group_off", "running_group_idx"]
-    src = tmp_path / "layout.c"
-    src.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "cook_gpu.h"\nint main(void) {\n'
-                   '  printf("%zu\\n", sizeof(cook_state_delta));\n' +
-                   "".join(f'  printf("%zu\\n", offsetof(cook_state_delta, {n}));\n' for n in fields) +
-                   '  printf("%d\\n", (int)COOK_PHASE_COTASKS);\n  return 0;\n}\n')
-    exe = tmp_path / "layout"
-    subprocess.check_call([cc, "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    got = [int(x) for x in subprocess.check_output([str(exe)]).split()]
-    assert got[0] == C.sizeof(abi.StateDelta)
-    assert got[1:-1] == [getattr(abi.StateDelta, n).offset for n in fields]
-    assert got[-1] == abi.PHASE_COTASKS == 6
-
-
-def test_cotasks_exported():
-    hdr = open(os.path.join(ROOT, "include", "cook_gpu.h")).read()
-    assert "int32_t cook_state_cotasks(cook_pool* pool" in hdr
-    if not os.path.exists(engine.LIB_PATH):
-        pytest.skip("libcookgpu.so not built")
-    assert hasattr(engine.load_library(), "cook_state_cotasks")
-    assert callable(GpuEngine.state_cotasks)
-
-
 def test_restatement_hand_built():
     rows = [dict(task_id=9, host=7, groups=[1]), dict(task_id=3, host=5, groups=[1, 0]),
             dict(task_id=4, host=-1, groups=[0, 1]), dict(task_id=6, host=8, groups=[1]),
@@ -94,79 +62,24 @@ def expected_bytes(G, attr_col, hosts, n):
     return 4 * H * (1 + D) + 4 * G, 4 * (G + 1) + 8 * n
 
 
-def tasks_of(rows):
-    n = len(rows)
-    return abi.make_tasks(user=np.array([r["user"] for r in rows], np.int32), priority=np.full(n, 50, np.int32),
-                          start_time=np.full(n, START, np.int64), task_id=np.array([r["task_id"] for r in rows], np.int64),
-                          job_id=np.array([r["job_id"] for r in rows], np.int64), cpus=np.ones(n), mem=np.full(n, 64.0))
-
-
-def jobs_of(rows):
-    n = len(rows)
-    off, idx = abi.csr([r["groups"] for r in rows])
-    return abi.JobsSoA(n=n, user=np.array([r["user"] for r in rows], np.int32), cpus=np.ones(n), mem=np.full(n, 64.0),
-                       group_off=off, group_idx=idx)
-
-
-class Handle:
-    """A resident handle and the rows it should hold: running {task id: row(user, job_id, host, groups)}, pending
-    {job id: row(user, groups)}."""
-
-    def __init__(self, name="cotasks"):
-        self.e = GpuEngine(pool_name=name)
-        self.run, self.pend = {}, {}
-
-    def close(self):
-        self.e.close()
-
-    def apply(self, up=(), rm=(), pend_up=(), pend_rm=(), reset=False, lists=True, hosts=True):
-        up = [dict(r, groups=r["groups"] if lists else [], host=r["host"] if hosts else -1) for r in up]
-        kw = {}
-        if up:
-            kw = dict(running=tasks_of(up), running_hostname_id=np.array([r["host"] for r in up], np.int32) if hosts else None)
-            if lists:
-                kw["running_group_off"], kw["running_group_idx"] = abi.csr([r["groups"] for r in up])
-        pend_up = list(pend_up)
-        if pend_up:
-            kw.update(pending=jobs_of(pend_up), pending_priority=np.full(len(pend_up), 50, np.int32),
-                      pending_job_id=np.array([p["job_id"] for p in pend_up], np.int64))
-        self.e.state_apply(abi.make_delta(reset=reset, running_rm=list(rm), pending_rm=list(pend_rm), **kw))
-        if reset:
-            self.run, self.pend = {}, {}
-        for t in rm:
-            del self.run[t]
-        for j in pend_rm:
-            del self.pend[j]
-        for r in up:
-            self.run[r["task_id"]] = r
-        for p in pend_up:
-            self.pend[p["job_id"]] = p
-
-    def launch(self, job_ids, task_ids, hosts=None):
-        self.e.state_launch(job_ids, task_ids, np.full(len(job_ids), START, np.int64), hosts)
-        for i, (j, t) in enumerate(zip(job_ids, task_ids)):
-            p = self.pend.pop(int(j))
-            self.run[int(t)] = dict(user=p["user"], job_id=int(j), task_id=int(t), groups=list(p["groups"]),
-                                    host=int(hosts[i]) if hosts is not None else -1)
-
-    def check(self, G, attr_col=None, hosts=None):
-        got = self.e.state_cotasks(G, attr_col, hosts)
-        want = ref_of(self.run.values(), G, attr_col, hosts)
-        assert got[0].tolist() == want[0] and got[1].tolist() == want[1] and got[2].tolist() == want[2]
-        st = self.e.last_stats(abi.PHASE_COTASKS)
-        assert (st["h2d_bytes"], st["d2h_bytes"]) == expected_bytes(G, attr_col, hosts, len(want[1]))
-        return got
+def check(h, G, attr_col=None, hosts=None):
+    got = h.gpu.state_cotasks(G, attr_col, hosts)
+    want = ref_of(h.run.values(), G, attr_col, hosts)
+    assert got[0].tolist() == want[0] and got[1].tolist() == want[1] and got[2].tolist() == want[2]
+    st = h.gpu.last_stats(abi.PHASE_COTASKS)
+    assert (st["h2d_bytes"], st["d2h_bytes"]) == expected_bytes(G, attr_col, hosts, len(want[1]))
+    return got
 
 
 def random_running(rng, n, tid0, codes, G, U=8):
-    return [dict(user=int(rng.integers(U)), task_id=tid0 + 3 * i, job_id=10 ** 9 + tid0 + 3 * i,
+    return [group_row(user=int(rng.integers(U)), task_id=tid0 + 3 * i, job_id=10 ** 9 + tid0 + 3 * i,
                  host=int(rng.choice(codes)),
                  groups=[int(g) for g in rng.choice(G, int(rng.choice([0, 0, 1, 1, 1, 2, 3])), replace=False)])
             for i in range(n)]
 
 
 def random_pending(rng, n, jid0, G, U=8):
-    return [dict(user=int(rng.integers(U)), job_id=jid0 + 2 * i,
+    return [group_row(user=int(rng.integers(U)), job_id=jid0 + 2 * i,
                  groups=[int(g) for g in rng.choice(G, int(rng.choice([0, 0, 1, 1, 2])), replace=False)])
             for i in range(n)]
 
@@ -180,7 +93,7 @@ def test_churn_matches_the_restatement():
     hosts = host_table(listed, rng.integers(0, 6, (3, len(listed))))
     attr_col = rng.integers(-1, 3, G).astype(np.int32)
     codes = list(range(55)) + [-1] * 6
-    h = Handle()
+    h = group_pool("cotasks")
     nxt = {"t": 1_000, "j": 5_000_000}
 
     def fresh_run(n):
@@ -194,33 +107,34 @@ def test_churn_matches_the_restatement():
         return rows
 
     def check_all():
-        h.check(G, attr_col, hosts)
-        h.check(G)                                               # no table: every value 0
-        h.check(G, None, hosts)
+        check(h, G, attr_col, hosts)
+        check(h, G)                                               # no table: every value 0
+        check(h, G, None, hosts)
 
     try:
         check_all()                                              # no state yet
-        h.apply(up=fresh_run(700), pend_up=fresh_pend(600))
+        h.apply(run_up=fresh_run(700), up=keyed(fresh_pend(600)))
         check_all()
         for b in range(6):
             fin = [t for t in h.run if rng.random() < 0.05]
             again = [dict(r, host=int(rng.choice(codes)), groups=[int(rng.integers(G))])
                      for r in rng.choice(list(h.run.values()), 25, replace=False) if r["task_id"] not in fin]
-            h.apply(up=fresh_run(250) + again, rm=fin, lists=b % 3 != 1, hosts=b % 2 == 0, pend_up=fresh_pend(150))
+            h.apply(run_up=fresh_run(250) + again, up=keyed(fresh_pend(150)), run_rm=fin, lists=b % 3 != 1,
+                    hosts=b % 2 == 0)
             check_all()                                          # past 1024, then 2048 running slots
             launch = [int(j) for j in rng.choice(sorted(h.pend), 120, replace=False)]
             tids = [nxt["t"] + 3 * i for i in range(len(launch))]
             nxt["t"] += 3 * len(launch) + 3
             hn = np.array(rng.choice(codes, len(launch)), np.int32) if b % 2 else None
-            h.launch(launch, tids, hn)
+            h.launch(launch, tids, np.full(len(launch), START, np.int64), hn)
             check_all()
-        h.apply(rm=[t for t in h.run if rng.random() < 0.8])     # dead entries outnumber live: compaction
+        h.apply(run_rm=[t for t in h.run if rng.random() < 0.8])     # dead entries outnumber live: compaction
         check_all()
-        h.apply(up=fresh_run(400))                               # the freed slots are taken again
+        h.apply(run_up=fresh_run(400))                               # the freed slots are taken again
         check_all()
-        h.apply(reset=True, up=fresh_run(900), pend_up=fresh_pend(50))
+        h.apply(reset=True, run_up=fresh_run(900), up=keyed(fresh_pend(50)))
         check_all()
-        h.apply(rm=list(h.run))
+        h.apply(run_rm=list(h.run))
         check_all()                                              # no live row: empty lists
     finally:
         h.close()
@@ -235,15 +149,15 @@ def test_layout_independence():
     hosts = host_table(np.arange(25, dtype=np.int32), rng.integers(0, 5, (2, 25)))
     attr_col = rng.integers(-1, 2, G).astype(np.int32)
     rows = random_running(rng, 1500, 10, codes, G)
-    a, b = Handle("a"), Handle("b")
+    a, b = group_pool("a"), group_pool("b")
     try:
-        a.apply(up=sorted(rows, key=lambda r: r["task_id"]))
+        a.apply(run_up=sorted(rows, key=lambda r: r["task_id"]))
         junk = random_running(rng, 900, 10_000_000, codes, G)
-        b.apply(up=junk)
+        b.apply(run_up=junk)
         perm = [rows[i] for i in rng.permutation(len(rows))]
-        b.apply(up=perm[:700], rm=[r["task_id"] for r in junk[:600]])
-        b.apply(up=perm[700:], rm=[r["task_id"] for r in junk[600:]])
-        ga, gb = a.check(G, attr_col, hosts), b.check(G, attr_col, hosts)
+        b.apply(run_up=perm[:700], run_rm=[r["task_id"] for r in junk[:600]])
+        b.apply(run_up=perm[700:], run_rm=[r["task_id"] for r in junk[600:]])
+        ga, gb = check(a, G, attr_col, hosts), check(b, G, attr_col, hosts)
         assert all(np.array_equal(x, y) for x, y in zip(ga, gb))
         assert len(ga[1]) > 1000
     finally:
@@ -259,29 +173,28 @@ def test_launch_against_delta():
     G, codes = 30, list(range(20)) + [-1]
     hosts = host_table(np.arange(20, dtype=np.int32), rng.integers(0, 4, (2, 20)))
     attr_col = rng.integers(-1, 2, G).astype(np.int32)
-    a, b = Handle("launch"), Handle("delta")
+    a, b = group_pool("launch"), group_pool("delta")
     try:
         pend, run = random_pending(rng, 800, 1_000_000, G), random_running(rng, 300, 10, codes, G)
         for h in (a, b):
-            h.apply(up=run, pend_up=pend)
+            h.apply(up=keyed(pend), run_up=run)
         tid = 100_000
         for step in range(5):
             jobs = [int(j) for j in rng.choice(sorted(a.pend), 90, replace=False)]
             tids = [tid + 3 * i for i in range(len(jobs))]
             tid += 3 * len(jobs) + 3
             hn = np.array(rng.choice(codes, len(jobs)), np.int32) if step % 2 == 0 else None
-            a.launch(jobs, tids, hn)
-            st = a.e.last_stats(abi.PHASE_STATE)
+            a.launch(jobs, tids, np.full(len(jobs), START, np.int64), hn)
+            st = a.gpu.last_stats(abi.PHASE_STATE)
             assert st["h2d_bytes"] == len(jobs) * (4 + 4 + 8 + 8) + (4 * len(jobs) if hn is not None else 0)
-            tasks = [dict(user=b.pend[j]["user"], job_id=j, task_id=t, groups=b.pend[j]["groups"],
-                          host=int(hn[i]) if hn is not None else -1) for i, (j, t) in enumerate(zip(jobs, tids))]
-            b.apply(up=tasks, pend_rm=jobs, hosts=hn is not None)
+            tasks = [task_of(b.pend[j], j, t, START, hn[i] if hn is not None else -1) for i, (j, t) in enumerate(zip(jobs, tids))]
+            b.apply(rm=jobs, run_up=tasks, hosts=hn is not None)
             fin = [t for t in a.run if rng.random() < 0.3]       # the running arena compacts on both
             for h in (a, b):
-                h.apply(rm=fin)
-            ga, gb = a.check(G, attr_col, hosts), b.check(G, attr_col, hosts)
+                h.apply(run_rm=fin)
+            ga, gb = check(a, G, attr_col, hosts), check(b, G, attr_col, hosts)
             assert all(np.array_equal(x, y) for x, y in zip(ga, gb))
-            assert np.array_equal(a.e.state_rank(abi.make_users(8)), b.e.state_rank(abi.make_users(8)))
+            assert np.array_equal(a.gpu.state_rank(abi.make_users(8)), b.gpu.state_rank(abi.make_users(8)))
     finally:
         a.close()
         b.close()
@@ -290,30 +203,30 @@ def test_launch_against_delta():
 # ---- GPU: edges, errors --------------------------------------------------------------------------------------
 @pytest.mark.gpu
 def test_edges():
-    h = Handle()
+    h = group_pool("cotasks")
     try:
         hosts = host_table([5, 7], [[11, 12], [21, 22]])
-        rows = [dict(user=0, task_id=10, job_id=1, host=-1, groups=[0, 1]),     # no host: not a cotask
-                dict(user=0, task_id=30, job_id=2, host=9, groups=[1]),         # unlisted host: kept, attribute 0
-                dict(user=1, task_id=20, job_id=3, host=7, groups=[1, 3]),
-                dict(user=1, task_id=40, job_id=4, host=5, groups=[0])]
-        h.apply(up=rows)
-        off, hn, av = h.check(5, np.array([1, 0, -1, -1, 0], np.int32), hosts)
+        rows = [group_row(user=0, task_id=10, job_id=1, host=-1, groups=[0, 1]),     # no host: not a cotask
+                group_row(user=0, task_id=30, job_id=2, host=9, groups=[1]),         # unlisted host: kept, attribute 0
+                group_row(user=1, task_id=20, job_id=3, host=7, groups=[1, 3]),
+                group_row(user=1, task_id=40, job_id=4, host=5, groups=[0])]
+        h.apply(run_up=rows)
+        off, hn, av = check(h, 5, np.array([1, 0, -1, -1, 0], np.int32), hosts)
         assert off.tolist() == [0, 1, 3, 3, 4, 4]                              # groups 2 and 4: empty
         assert hn.tolist() == [5, 7, 9, 7] and av.tolist() == [21, 12, 0, 0]
-        assert h.check(5, np.array([-1] * 5, np.int32), hosts)[2].tolist() == [0, 0, 0, 0]
-        assert h.check(9)[0].tolist() == [0, 1, 3, 3, 4, 4, 4, 4, 4, 4]       # more groups than codes
-        lib, pool = h.e.lib, h.e.pool
+        assert check(h, 5, np.array([-1] * 5, np.int32), hosts)[2].tolist() == [0, 0, 0, 0]
+        assert check(h, 9)[0].tolist() == [0, 1, 3, 3, 4, 4, 4, 4, 4, 4]       # more groups than codes
+        lib, pool = h.gpu.lib, h.gpu.pool
         n = C.c_int32(-7)
         assert lib.cook_state_cotasks(pool, 5, None, None, 0, None, None, None, C.byref(n)) == abi.COOK_OK
         assert n.value == 4                                                    # the size query is exact
         n = C.c_int32(-7)
         assert lib.cook_state_cotasks(pool, 5, None, C.byref(hosts), 0, None, None, None, C.byref(n)) == abi.COOK_OK
-        assert n.value == 4 and h.e.last_stats(abi.PHASE_COTASKS)["h2d_bytes"] == 0
-        h.apply(rm=[20, 30, 40])
-        assert h.check(5, np.array([1, 0, -1, -1, 0], np.int32), hosts)[0].tolist() == [0] * 6
-        h.apply(up=[dict(user=0, task_id=50, job_id=5, host=-1, groups=[4])], hosts=False)
-        assert h.check(5)[0].tolist() == [0] * 6                               # grouped rows, none with a host
+        assert n.value == 4 and h.gpu.last_stats(abi.PHASE_COTASKS)["h2d_bytes"] == 0
+        h.apply(run_rm=[20, 30, 40])
+        assert check(h, 5, np.array([1, 0, -1, -1, 0], np.int32), hosts)[0].tolist() == [0] * 6
+        h.apply(run_up=[group_row(user=0, task_id=50, job_id=5, host=-1, groups=[4])], hosts=False)
+        assert check(h, 5)[0].tolist() == [0] * 6                               # grouped rows, none with a host
     finally:
         h.close()
 
@@ -321,14 +234,14 @@ def test_edges():
 @pytest.mark.gpu
 def test_errors_write_nothing():
     rng = np.random.default_rng(11)
-    h = Handle()
+    h = group_pool("cotasks")
     try:
-        h.apply(up=random_running(rng, 200, 10, list(range(10)), 6))
+        h.apply(run_up=random_running(rng, 200, 10, list(range(10)), 6))
         hosts = host_table(np.arange(10, dtype=np.int32), rng.integers(1, 5, (2, 10)))
         ac = np.array([0, 1, -1, 0, 1, -1], np.int32)
-        want = h.check(6, ac, hosts)
+        want = check(h, 6, ac, hosts)
         N = len(want[1])
-        lib, pool = h.e.lib, h.e.pool
+        lib, pool = h.gpu.lib, h.gpu.pool
         P = abi.P_I32
         off, hn, av = np.full(7, -9, np.int32), np.full(N + 4, -9, np.int32), np.full(N + 4, -9, np.int32)
         n = C.c_int32(-9)
@@ -362,88 +275,41 @@ def test_errors_write_nothing():
         ]
         assert cases == [abi.COOK_E_BADARG] * len(cases)
         assert n.value == -9 and (off == -9).all() and (hn == -9).all() and (av == -9).all()
-        got = h.check(6, ac, hosts)                        # the handle is unchanged
+        got = check(h, 6, ac, hosts)                        # the handle is unchanged
         assert all(np.array_equal(x, y) for x, y in zip(got, want))
-        bad = dict(running=tasks_of([dict(user=0, task_id=1, job_id=1)]))
+        bad = dict(running=tasks_soa([group_row(user=0, task_id=1, job_id=1)]))
         for o, i in (([1, 1], [1]), ([0, -1], [1]), ([0, 1], [-1])):   # malformed CSR, negative group code
             with pytest.raises(engine.CookError):
-                h.e.state_apply(abi.make_delta(running_group_off=np.array(o, np.int32),
+                h.gpu.state_apply(abi.make_delta(running_group_off=np.array(o, np.int32),
                                                running_group_idx=np.array(i, np.int32), **bad))
-        got = h.check(6, ac, hosts)
+        got = check(h, 6, ac, hosts)
         assert all(np.array_equal(x, y) for x, y in zip(got, want))
     finally:
         h.close()
 
 
 # ---- GPU: K13 through the resident path --------------------------------------------------------------------
-class K13:
-    """One pool through the resident cycle: jobs submitted as pending rows, ranked, matched with cotasks derived
-    from the running rows an earlier launch created, and the placed jobs launched on the hosts the match chose."""
-
-    def __init__(self, oracle, groups):
-        self.o, self.e = oracle, Handle("k13")
-        self.kind = np.array([g["kind"] for g in groups], np.int32)
-        self.col = np.array([g.get("col", -1) for g in groups], np.int32)
-        self.minimum = np.array([g.get("minimum", 0) for g in groups], np.int32)
-        self.users, self.code, self.jid, self.tid = abi.make_users(1), {}, 1000, 50
-
-    def close(self):
-        self.e.close()
-
-    def offers(self, spec, n_attr_cols=1):
-        for o in spec:
-            self.code.setdefault(o["host"], len(self.code))
-        O = len(spec)
-        attr = np.zeros((n_attr_cols, O), np.int32)
-        for i, o in enumerate(spec):
-            for c, v in o.get("attrs", {}).items():
-                attr[c, i] = v
-        order = sorted(range(O), key=lambda i: spec[i]["host"])
-        rank = np.zeros(O, np.int32)
-        rank[order] = np.arange(O, dtype=np.int32)
-        return abi.OffersSoA(n=O, hostname_id=np.array([self.code[o["host"]] for o in spec], np.int32), name_rank=rank,
-                             cpus=np.array([o["cpus"] for o in spec]), mem=np.array([o.get("mem", 100000.0) for o in spec]),
-                             run_cpus=np.zeros(O), run_mem=np.zeros(O), run_count=np.zeros(O, np.int32),
-                             n_attr_cols=n_attr_cols, attr=attr.reshape(-1))
-
-    def submit(self, n, group=0):
-        rows = [dict(user=0, job_id=self.jid + 2 * i, groups=[group]) for i in range(n)]
-        self.jid += 2 * n
-        self.e.apply(pend_up=rows)
-
-    def groups(self, cot):
-        vals = [np.asarray(x if len(x) else [0], np.int32) for x in cot[1:]]   # empty: a valid pointer all the same
-        return abi.Groups(n_groups=len(self.kind), kind=self.kind, attr_col=self.col, minimum=self.minimum,
-                          cot_off=np.asarray(cot[0], np.int32), cot_hostname_id=vals[0], cot_attr_val=vals[1])
-
-    def cycle(self, spec):
-        """Rank, derive, match; the same match by the oracle on host tables with host-built lists.  Launches what
-        was placed and returns the assignment as offer host names (None: unplaced)."""
-        offers = self.offers(spec)
-        q = self.e.e.state_rank(self.users)
-        G = len(self.kind)
-        cot = self.e.check(G, self.col, offers)
-        want = ref_of(self.e.run.values(), G, self.col, offers)
-        prm = traces.match_params(len(q))
-        m = self.e.e.state_match(offers, self.users, prm, groups=self.groups(cot))
-        ids = sorted(self.e.pend)
-        pos = {j: i for i, j in enumerate(ids)}
-        jobs = jobs_of([self.e.pend[j] for j in ids])
-        ranked = np.array([pos[j] for j in q], np.int32)
-        om = self.o.match(ranked, jobs, offers, self.users, prm, groups=self.groups(want))
-        assert np.array_equal(m["considerable"], np.array(ids)[om["considerable"]]) and np.array_equal(m["assign"], om["assign"])
-        k = np.arange(len(m["considerable"]), dtype=np.int32)
-        fg, fo = self.e.e.match_failures(k), self.o.match_failures(ranked, jobs, offers, self.users, prm, k,
-                                                                   groups=self.groups(want))
-        grp = slice(abi.FAILC_N - 3, abi.FAILC_N)   # unique, balanced, attribute-equals
-        assert [(f["n_vms"], f["counts"][grp]) for f in fg] == [(f["n_vms"], f["counts"][grp]) for f in fo]
-        placed = m["assign"] >= 0
-        jl = m["considerable"][placed].tolist()
-        tids = [self.tid + 3 * i for i in range(len(jl))]
-        self.tid += 3 * len(jl) + 3
-        hn = offers.col("hostname_id")[m["assign"][placed]]
-        self.e.launch(jl, tids, hn)
-        return [spec[a]["host"] if a >= 0 else None for a in m["assign"]]
+def k13_cycle(p, spec):
+    """Rank, derive, match; the same match by the oracle on host tables with host-built lists.  Launches what was
+    placed and returns the assignment as offer host names (None: unplaced)."""
+    offers = p.offers(spec)
+    q = p.e.gpu.state_rank(p.users)
+    G = len(p.kind)
+    cot = check(p.e, G, p.col, offers)
+    want = ref_of(p.e.run.values(), G, p.col, offers)
+    prm = traces.match_params(len(q))
+    m = p.e.gpu.state_match(offers, p.users, prm, groups=p.groups(cot))
+    ids, jobs = p.jobs()
+    pos = {j: i for i, j in enumerate(ids)}
+    ranked = np.array([pos[j] for j in q], np.int32)
+    om = p.o.match(ranked, jobs, offers, p.users, prm, groups=p.groups(want))
+    assert np.array_equal(m["considerable"], np.array(ids)[om["considerable"]]) and np.array_equal(m["assign"], om["assign"])
+    k = np.arange(len(m["considerable"]), dtype=np.int32)
+    fg, fo = p.e.gpu.match_failures(k), p.o.match_failures(ranked, jobs, offers, p.users, prm, k, groups=p.groups(want))
+    grp = slice(abi.FAILC_N - 3, abi.FAILC_N)   # unique, balanced, attribute-equals
+    assert [(f["n_vms"], f["counts"][grp]) for f in fg] == [(f["n_vms"], f["counts"][grp]) for f in fo]
+    p.launch_placed(m, offers)
+    return [spec[a]["host"] if a >= 0 else None for a in m["assign"]]
 
 
 @pytest.mark.gpu
@@ -452,10 +318,10 @@ def test_k13_unique_across_cycles(oracle):
     try:
         host = [dict(host="test-host", cpus=100.0)]
         p.submit(1)
-        assert p.cycle(host) == ["test-host"]
+        assert k13_cycle(p, host) == ["test-host"]
         p.submit(1)                                        # its cotask now runs on the only host: 0 placed
-        assert p.cycle(host) == [None]
-        assert p.e.e.state_cotasks(1)[1].tolist() == [0]
+        assert k13_cycle(p, host) == [None]
+        assert p.e.gpu.state_cotasks(1)[1].tolist() == [0]
     finally:
         p.close()
 
@@ -465,7 +331,7 @@ def test_k13_unique_same_cycle(oracle):
     p = K13(oracle, [dict(kind=abi.GROUP_UNIQUE)])
     try:
         p.submit(2)
-        assert p.cycle([dict(host="test-host", cpus=100.0)]) == ["test-host", None]
+        assert k13_cycle(p, [dict(host="test-host", cpus=100.0)]) == ["test-host", None]
     finally:
         p.close()
 
@@ -476,9 +342,9 @@ def test_k13_balanced(oracle):
     try:
         hosts = [dict(host=h, cpus=100.0, attrs={0: i + 1}) for i, h in enumerate(["straw", "sticks", "bricks"])]
         p.submit(3)
-        first = p.cycle(hosts)
+        first = k13_cycle(p, hosts)
         p.submit(6)
-        second = p.cycle(hosts)
+        second = k13_cycle(p, hosts)
         assert None not in first + second
         assert sorted(np.unique(first + second, return_counts=True)[1].tolist()) == [3, 3, 3]
     finally:
@@ -492,12 +358,12 @@ def test_k13_attribute_equals(oracle):
     try:
         east = dict(host="first-east-host", cpus=1.0, attrs={0: EAST})
         p.submit(1)
-        assert p.cycle([east]) == ["first-east-host"]
+        assert k13_cycle(p, [east]) == ["first-east-host"]
         # the cotask's host stays in the offer table, full; 20 one-cpu west offers and a 5-cpu east offer
         offers = [dict(east, cpus=0.5)] + [dict(host=f"west-{i:02d}", cpus=1.0, attrs={0: WEST}) for i in range(20)]
         offers.append(dict(host="east-big", cpus=5.0, attrs={0: EAST}))
         p.submit(20)
-        got = p.cycle(offers)
+        got = k13_cycle(p, offers)
         assert got.count("east-big") == 5 and got.count(None) == 15
     finally:
         p.close()
@@ -506,7 +372,6 @@ def test_k13_attribute_equals(oracle):
 # ---- GPU: config-#3 match cycles and a config-#4 rebalance -------------------------------------------------------
 @pytest.mark.gpu
 def test_c3_cycles_against_the_oracle(oracle):
-    from test_state_resident import Model, pool_rows, jobs_soa, tasks_soa
     t = traces.gen_c3_pool(17, n_jobs=2500, n_offers=160, n_users=24, n_running=500)
     rng = np.random.default_rng(19)
     g0, offers, users = t["groups"], t["offers"], t["users"]
@@ -519,18 +384,8 @@ def test_c3_cycles_against_the_oracle(oracle):
     items = sorted(pend.items())
     cut = int(len(items) * 0.7)
     reserve = items[cut:]
-    e, ref, m = GpuEngine(pool_name="c3"), GpuEngine(pool_name="host"), Model()
-
-    def apply(up=(), rm=(), run_up=(), run_rm=(), reset=False):
-        up, run_up = list(up), list(run_up)
-        pj, pp, jid = jobs_soa(up) if up else (None, None, None)
-        kw = {}
-        if run_up:
-            kw = dict(running=tasks_soa(run_up), running_hostname_id=np.array([r["host"] for r in run_up], np.int32))
-            kw["running_group_off"], kw["running_group_idx"] = abi.csr([r["groups"] for r in run_up])
-        e.state_apply(abi.make_delta(reset=reset, pending=pj, pending_priority=pp, pending_job_id=jid,
-                                     pending_rm=list(rm), running_rm=list(run_rm), **kw))
-        m.apply(up, rm, run_up, run_rm, reset)
+    m = Pool("c3", send_hosts=True, send_lists=True)
+    e, ref, apply = m.gpu, m.ref, m.apply
 
     prm = traces.match_params(1000, host_lifetime_mins=t.get("host_lifetime_mins", 0))
     max_ports = int(t["jobs"].col("ports").max())
@@ -567,11 +422,7 @@ def test_c3_cycles_against_the_oracle(oracle):
             tids = [tid + 3 * i for i in range(len(jl))]
             tid += 3 * len(jl) + 3
             hosts = hn[got["assign"][placed]].astype(np.int32)
-            e.state_launch(jl, tids, np.full(len(jl), START, np.int64), hosts)
-            m.apply(d_rm=jl, r_up=[dict(user=m.pend[j]["user"], priority=m.pend[j]["priority"], start_time=START,
-                                        task_id=t_, job_id=j, cpus=m.pend[j]["cpus"], mem=m.pend[j]["mem"],
-                                        gpus=m.pend[j]["gpus"], host=int(h), groups=list(m.pend[j]["groups"]))
-                                   for j, t_, h in zip(jl, tids, hosts)])
+            m.launch(jl, tids, np.full(len(jl), START, np.int64), hosts)
             fin = [x for x in m.run if rng.random() < 0.03]
             new = [reserve.pop() for _ in range(min(len(reserve), len(fin) + 20))]
             for _, r in new[:10]:                           # new members of existing groups
@@ -579,21 +430,18 @@ def test_c3_cycles_against_the_oracle(oracle):
             apply(up=new, run_rm=fin)
         assert n_cot > 50
     finally:
-        e.close()
-        ref.close()
+        m.close()
 
 
 @pytest.mark.gpu
 def test_c4_rebalance_from_derived_lists(oracle):
-    from test_state_rebalance import RPool, _pool, rows_of
-    from test_state_resident import jobs_soa, tasks_soa
-    r, codes = _pool(23, True)
+    r, codes = rebalance_trace(23, True)
     rng = np.random.default_rng(29)
     G, g0, hosts = r["groups"].n_groups, r["groups"], r["hosts"]
     pend, run = rows_of(r, codes)
     for row in run.values():
         row["groups"] = [int(rng.integers(G))] if rng.random() < 0.2 else []
-    p = RPool(r, codes)
+    p = Pool.of_rebalance(r, codes)
     try:
         run_up = list(run.values())
         pj, pp, jid = jobs_soa(sorted(pend.items()))
@@ -609,6 +457,6 @@ def test_c4_rebalance_from_derived_lists(oracle):
         assert [x.tolist() for x in cot] == list(want) and len(want[1]) > 300
         p.groups = abi.Groups(n_groups=G, kind=g0.col("kind"), attr_col=acol, minimum=g0.col("minimum"),
                               cot_off=cot[0], cot_hostname_id=cot[1], cot_attr_val=cot[2])
-        p.check(oracle)
+        p.check_rebalance(oracle)
     finally:
         p.close()

@@ -10,105 +10,27 @@ download formula) and against the oracle on host tables built from a model; conf
 group cases; a config-#4 rebalance; freshness after launches; slot-layout independence; errors and edges.
 """
 import ctypes as C
-import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
 import fold_ref as F
-from cook_b200 import abi, engine, traces
+from cook_b200 import abi, traces
 from cook_b200.engine import CookError, GpuEngine
 from cotask_ref import cotasks
+from resident_model import (COT_FIELDS, K13, RUN_FIELDS, START, USAGE_FIELDS, Pool, decisions_eq, drop_all_but, fed_tables,
+                            host_inputs, jobs_soa, keyed, pending_rows, pool_rows, random_rows, rebalance_trace, rows_of,
+                            tasks_soa, with_fields)
 from usage_ref import KEYS, running_usage
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-START = 1_700_000_000_000
-USAGE_FIELDS = ("usage_count", "usage_cpus", "usage_mem", "usage_gpus")
-RUN_FIELDS = ("run_cpus", "run_mem", "run_count")
-COT_FIELDS = ("cot_off", "cot_hostname_id", "cot_attr_val")
-
-
-# ---- CPU -------------------------------------------------------------------------------------------------
-def _prototype(hdr, name):
-    m = re.search(r"int32_t\s+" + name + r"\s*\(([^)]*)\)\s*;", hdr)
-    assert m, name
-    return [" ".join(p.split()) for p in m.group(1).split(",")]
-
-
-def test_derived_entries_declared_and_exported():
-    hdr = open(os.path.join(ROOT, "include", "cook_gpu.h")).read()
-    for plain in ("cook_state_match", "cook_state_rebalance"):
-        # the same arguments, names included
-        assert _prototype(hdr, plain + "_derived") == _prototype(hdr, plain)
-    assert "derived" in GpuEngine.state_match.__code__.co_varnames
-    assert "derived" in GpuEngine.state_rebalance.__code__.co_varnames
-    if not os.path.exists(engine.LIB_PATH):
-        pytest.skip("libcookgpu.so not built")
-    lib = engine.load_library()
-    for name in ("cook_state_match_derived", "cook_state_rebalance_derived"):
-        assert hasattr(lib, name), name
-        assert getattr(lib, name).restype is C.c_int32
-
-
-def test_derived_prototypes_compile_as_the_plain_ones(tmp_path):
-    cc = shutil.which("cc") or shutil.which("gcc")
-    if cc is None:
-        pytest.skip("no C compiler")
-    src = tmp_path / "proto.c"
-    src.write_text('#include "cook_gpu.h"\n'
-                   '_Static_assert(__builtin_types_compatible_p(__typeof__(cook_state_match),\n'
-                   '               __typeof__(cook_state_match_derived)), "match");\n'
-                   '_Static_assert(__builtin_types_compatible_p(__typeof__(cook_state_rebalance),\n'
-                   '               __typeof__(cook_state_rebalance_derived)), "rebalance");\n'
-                   'int main(void) { return 0; }\n')
-    subprocess.check_call([cc, "-std=gnu11", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(tmp_path / "p")])
-
-
-# C parameter types of the header -> the ctypes abi.ARGTYPES must hold
-_CTYPE = {"cook_pool*": C.c_void_p, "const cook_offers_soa*": C.POINTER(abi.OffersSoA),
-          "const cook_groups*": C.POINTER(abi.Groups), "const cook_user_table*": C.POINTER(abi.UserTable),
-          "const cook_pool_quota*": C.POINTER(abi.PoolQuota), "const cook_match_params*": C.POINTER(abi.MatchParams),
-          "int64_t*": abi.P_I64, "int32_t*": abi.P_I32, "int32_t": C.c_int32, "uint8_t*": abi.P_U8,
-          "cook_match_stats*": C.POINTER(abi.MatchStats), "const cook_host_table*": C.POINTER(abi.HostTable),
-          "const cook_rebalance_params*": C.POINTER(abi.RebalanceParams), "cook_decision*": C.POINTER(abi.Decision)}
-
-
-def test_ctypes_signatures_match_the_header():
-    hdr = open(os.path.join(ROOT, "include", "cook_gpu.h")).read()
-    for name in ("cook_state_match_derived", "cook_state_rebalance_derived"):
-        types = [re.sub(r"\s*\w+$", "", p).replace(" *", "*") for p in _prototype(hdr, name)]
-        assert abi.ARGTYPES[name] == [_CTYPE[t] for t in types], name
 
 
 # ---- GPU helpers -------------------------------------------------------------------------------------------
-def with_fields(s, **over):
-    """A copy of the SoA struct `s` with fields replaced (None: NULL)."""
-    kw = {}
-    for n, t in s._fields_:
-        kw[n] = s.col(n) if t in (abi.P_I32, abi.P_I64, abi.P_F64, abi.P_U8) else getattr(s, n)
-    kw.update(over)
-    return type(s)(**kw)
-
-
 def derived_inputs(offers, users, groups):
     """The tables of a derived call: the fields it derives are NULL."""
     users = with_fields(users, **{f: None for f in USAGE_FIELDS})
     offers = with_fields(offers, **{f: None for f in RUN_FIELDS})
     groups = with_fields(groups, **{f: None for f in COT_FIELDS}) if groups is not None else None
-    return offers, users, groups
-
-
-def fed_tables(offers, users, groups, usage, cot):
-    """The tables of a sequenced call: usage (state_usage's dict) and cot (state_cotasks' triple) filled in."""
-    users = with_fields(users, **{f: usage["user"][k] for f, k in zip(USAGE_FIELDS, KEYS)})
-    offers = with_fields(offers, run_cpus=usage["run_cpus"], run_mem=usage["run_mem"], run_count=usage["run_count"])
-    if groups is not None and cot is not None:
-        groups = with_fields(groups, cot_off=np.asarray(cot[0], np.int32),
-                             cot_hostname_id=np.asarray(cot[1] if len(cot[1]) else [0], np.int32),
-                             cot_attr_val=np.asarray(cot[2] if len(cot[2]) else [0], np.int32))
     return offers, users, groups
 
 
@@ -119,18 +41,6 @@ def sequenced_inputs(e, offers, users, groups):
     if groups is not None and groups.n_groups:
         cot = e.state_cotasks(groups.n_groups, groups.col("attr_col"), offers)
     return fed_tables(offers, users, groups, usage, cot), usage, cot
-
-
-def host_inputs(run_rows, offers, users, groups):
-    """The same tables from a model's running rows (usage_ref / cotask_ref restatements)."""
-    hn = offers.col("hostname_id") if offers.n else np.zeros(0, np.int32)
-    usage = running_usage(run_rows, users.n_users, hn)
-    cot = None
-    if groups is not None and groups.n_groups:
-        at = offers.col("attr")
-        cot = cotasks(run_rows, groups.n_groups, groups.col("attr_col"), hn,
-                      at.reshape(offers.n_attr_cols, offers.n) if at is not None and offers.n else None)
-    return fed_tables(offers, users, groups, usage, cot)
 
 
 def saved_up(G, O, U, n_cot, grouped):
@@ -165,50 +75,24 @@ def compare(e, offers, users, prm, groups=None, max_ports=0, grouped=False):
     return got, (so, su, sg)
 
 
-def oracle_check(oracle, got, run_rows, jobs, jid, ranked, offers, users, prm, groups=None, max_ports=0):
+def oracle_check(oracle, got, run_rows, jobs, jid, ranked_, offers, users, prm, groups=None, max_ports=0):
     ho, hu, hg = host_inputs(run_rows, offers, users, groups)
-    om = oracle.match(ranked, jobs, ho, hu, prm, groups=hg, max_ports=max_ports)
+    om = oracle.match(ranked_, jobs, ho, hu, prm, groups=hg, max_ports=max_ports)
     assert np.array_equal(got["considerable"], jid[om["considerable"]])
     assert np.array_equal(got["assign"], om["assign"])
 
 
-class Pool:
-    """A resident handle and a model of its rows: pending {job id: row}, running {task id: row with host, groups}."""
+def new_pool(name):
+    """A resident handle whose running upserts carry hosts and group lists, and the model of its rows."""
+    return Pool(name, send_hosts=True, send_lists=True)
 
-    def __init__(self, name="derived"):
-        from test_state_resident import Model
-        self.e, self.m = GpuEngine(pool_name=name), Model()
 
-    def close(self):
-        self.e.close()
+def grouped(p):
+    return any(r["groups"] for r in p.pend.values())
 
-    def apply(self, up=(), rm=(), run_up=(), run_rm=(), reset=False):
-        from test_state_resident import jobs_soa, tasks_soa
-        up, run_up = list(up), list(run_up)
-        pj, pp, jid = jobs_soa(up) if up else (None, None, None)
-        kw = {}
-        if run_up:
-            kw = dict(running=tasks_soa(run_up), running_hostname_id=np.array([r["host"] for r in run_up], np.int32))
-            kw["running_group_off"], kw["running_group_idx"] = abi.csr([r.get("groups", []) for r in run_up])
-        self.e.state_apply(abi.make_delta(reset=reset, pending=pj, pending_priority=pp, pending_job_id=jid,
-                                          pending_rm=list(rm), running_rm=list(run_rm), **kw))
-        self.m.apply(up, rm, run_up, run_rm, reset)
 
-    def launch(self, jobs, tids, hosts=None):
-        self.e.state_launch(jobs, tids, np.full(len(jobs), START, np.int64), hosts)
-        p = self.m.pend
-        rows = [dict(user=p[j]["user"], priority=p[j]["priority"], start_time=START, task_id=t, job_id=j,
-                     cpus=p[j]["cpus"], mem=p[j]["mem"], gpus=p[j]["gpus"], groups=list(p[j]["groups"]),
-                     host=int(hosts[i]) if hosts is not None else -1) for i, (j, t) in enumerate(zip(jobs, tids))]
-        self.m.apply(d_rm=list(jobs), r_up=rows)
-
-    def grouped(self):
-        return any(r["groups"] for r in self.m.pend.values())
-
-    def ranked(self, q):
-        _, _, jobs, jid = self.m.tables()
-        pos = {j: i for i, j in enumerate(jid.tolist())}
-        return jobs, jid, np.array([pos[j] for j in q.tolist() if j in pos], np.int32)
+def live_positions(p, q):
+    return p.ranked([j for j in q.tolist() if j in p.pend])
 
 
 def _hosts_for(rng, run, codes, unlisted=(), none=0.05):
@@ -221,7 +105,6 @@ def _hosts_for(rng, run, codes, unlisted=(), none=0.05):
 @pytest.mark.gpu
 @pytest.mark.parametrize("regime", ["grid", "off"])
 def test_c2_churn(regime, oracle):
-    from test_state_resident import pool_rows
     cpus = (0.5, 1, 2, 4, 8) if regime == "grid" else (0.1, 0.5, 1.0, 2.0)
     t = traces.gen_pool(41 if regime == "grid" else 43, 3000, 200, 30, 600, cpus_choices=cpus)
     rng = np.random.default_rng(7)
@@ -240,7 +123,7 @@ def test_c2_churn(regime, oracle):
     cut = int(len(items) * 0.6)
     reserve = items[cut:]
     prm = traces.match_params(1000)
-    p = Pool("c2")
+    p = new_pool("c2")
     tid = [10 ** 9]
 
     def tids(n):
@@ -251,37 +134,35 @@ def test_c2_churn(regime, oracle):
     try:
         p.apply(up=items[:cut], run_up=list(run.values()), reset=True)
         for cycle in range(7):
-            q = p.e.state_rank(users)
-            got, _ = compare(p.e, offers, users, prm)
-            jobs, jid, ranked = p.ranked(q)
+            q = p.gpu.state_rank(users)
+            got, _ = compare(p.gpu, offers, users, prm)
+            jobs, jid, ranked_ = live_positions(p, q)
             if cycle % 2 == 0:
-                oracle_check(oracle, got, p.m.run.values(), jobs, jid, ranked, offers, users, prm)
-            cnt = running_usage(p.m.run.values(), U)["user"]["count"]
+                oracle_check(oracle, got, p.run.values(), jobs, jid, ranked_, offers, users, prm)
+            cnt = running_usage(p.run.values(), U)["user"]["count"]
             assert (cnt == 0).any()
             placed = got["assign"] >= 0
             jl = got["considerable"][placed].tolist()[:60]
             assert jl
             hn = codes[got["assign"][placed][:len(jl)]].astype(np.int32) if cycle % 3 != 1 else None
-            p.launch(jl, tids(len(jl)), hn)                    # launches with and without hosts
-            fin = [x for x in p.m.run if rng.random() < 0.04]
+            p.launch(jl, tids(len(jl)), np.full(len(jl), START, np.int64), hn)                    # launches with and without hosts
+            fin = [x for x in p.run if rng.random() < 0.04]
             new = [reserve.pop() for _ in range(min(len(reserve), 80))]
             p.apply(up=new, run_rm=fin)                          # finishes and submissions
-            live = sorted(p.m.pend)
+            live = sorted(p.pend)
             flip = [int(j) for j in rng.choice(live, 30, replace=False)]
-            p.e.state_patch(flip, allowed=np.zeros(30, np.uint8))   # patches keep the queue
-            for j in flip:
-                p.m.pend[j] = dict(p.m.pend[j], allowed=0)
+            p.patch(flip, allowed=np.zeros(30, np.uint8))        # patches keep the queue
             if cycle == 2:                                       # growth: past the running table's capacity
                 more = [dict(r, task_id=r["task_id"] + 5 * 10 ** 8, job_id=r["job_id"] + 5 * 10 ** 8)
-                        for r in list(p.m.run.values())[:700]]
+                        for r in list(p.run.values())[:700]]
                 p.apply(run_up=more)
             if cycle == 4:                                       # a reset with the same rows, then compaction
-                p.apply(up=sorted(p.m.pend.items()), run_up=list(p.m.run.values()), reset=True)
-                p.apply(run_rm=[x for x in p.m.run if rng.random() < 0.7])
-        q = p.e.state_rank(users)
-        got, _ = compare(p.e, offers, users, prm)
-        jobs, jid, ranked = p.ranked(q)
-        oracle_check(oracle, got, p.m.run.values(), jobs, jid, ranked, offers, users, prm)
+                p.apply(up=sorted(p.pend.items()), run_up=list(p.run.values()), reset=True)
+                p.apply(run_rm=[x for x in p.run if rng.random() < 0.7])
+        q = p.gpu.state_rank(users)
+        got, _ = compare(p.gpu, offers, users, prm)
+        jobs, jid, ranked_ = live_positions(p, q)
+        oracle_check(oracle, got, p.run.values(), jobs, jid, ranked_, offers, users, prm)
     finally:
         p.close()
 
@@ -289,7 +170,6 @@ def test_c2_churn(regime, oracle):
 # ---- GPU: config-#3 cycles with groups, K13 --------------------------------------------------------------------
 @pytest.mark.gpu
 def test_c3_cycles_with_groups(oracle):
-    from test_state_resident import pool_rows
     t = traces.gen_c3_pool(17, n_jobs=2500, n_offers=160, n_users=24, n_running=500)
     rng = np.random.default_rng(19)
     g0, offers, users = t["groups"], t["offers"], t["users"]
@@ -304,23 +184,24 @@ def test_c3_cycles_with_groups(oracle):
     reserve = items[cut:]
     prm = traces.match_params(1000, host_lifetime_mins=t.get("host_lifetime_mins", 0))
     max_ports = int(t["jobs"].col("ports").max())
-    p = Pool("c3")
+    p = new_pool("c3")
     tid = 10 ** 9
     try:
         p.apply(up=items[:cut], run_up=list(run.values()), reset=True)
         n_cot = 0
         for cycle in range(5):
-            q = p.e.state_rank(users)
-            got, (so, su, sg) = compare(p.e, offers, users, prm, groups=g0, max_ports=max_ports, grouped=p.grouped())
+            q = p.gpu.state_rank(users)
+            got, (so, su, sg) = compare(p.gpu, offers, users, prm, groups=g0, max_ports=max_ports, grouped=grouped(p))
             n_cot = max(n_cot, int(sg.col("cot_off")[-1]))
-            jobs, jid, ranked = p.ranked(q)
-            oracle_check(oracle, got, p.m.run.values(), jobs, jid, ranked, offers, users, prm, g0, max_ports)
+            jobs, jid, ranked_ = live_positions(p, q)
+            oracle_check(oracle, got, p.run.values(), jobs, jid, ranked_, offers, users, prm, g0, max_ports)
             placed = got["assign"] >= 0
             jl = got["considerable"][placed].tolist()
             assert jl
-            p.launch(jl, [tid + 3 * i for i in range(len(jl))], hn[got["assign"][placed]].astype(np.int32))
+            p.launch(jl, [tid + 3 * i for i in range(len(jl))], np.full(len(jl), START, np.int64),
+                     hn[got["assign"][placed]].astype(np.int32))
             tid += 3 * len(jl) + 3
-            fin = [x for x in p.m.run if rng.random() < 0.03]
+            fin = [x for x in p.run if rng.random() < 0.03]
             new = [reserve.pop() for _ in range(min(len(reserve), len(fin) + 20))]
             for _, r in new[:10]:
                 r["groups"] = sorted({*r["groups"], int(rng.integers(G))})
@@ -330,77 +211,62 @@ def test_c3_cycles_with_groups(oracle):
         p.close()
 
 
-class K13D:
-    """K13's group cases through the derived call: each cycle's derived match equals the sequenced one and the
-    oracle on host-built lists (failure counts included), then its placements are launched."""
-
-    def __init__(self, oracle, groups):
-        from test_state_cotasks import K13
-        self.k = K13(oracle, groups)
-
-    def close(self):
-        self.k.close()
-
-    def cycle(self, spec):
-        k = self.k
-        offers = k.offers(spec)
-        q = k.e.e.state_rank(k.users)
-        G = len(k.kind)
-        groups = abi.Groups(n_groups=G, kind=k.kind, attr_col=k.col, minimum=k.minimum)
-        prm = traces.match_params(len(q))
-        m, _ = compare(k.e.e, offers, k.users, prm, groups=groups, grouped=True)
-        ids = sorted(k.e.pend)
-        pos = {j: i for i, j in enumerate(ids)}
-        jobs = __import__("test_state_cotasks").jobs_of([k.e.pend[j] for j in ids])
-        ranked = np.array([pos[j] for j in q], np.int32)
-        hc = cotasks(k.e.run.values(), G, k.col, offers.col("hostname_id"), offers.col("attr").reshape(1, offers.n))
-        hg = fed_tables(offers, k.users, groups, running_usage([], 1), hc)[2]
-        om = k.o.match(ranked, jobs, offers, k.users, prm, groups=hg)
-        assert np.array_equal(m["considerable"], np.array(ids)[om["considerable"]])
-        assert np.array_equal(m["assign"], om["assign"])
-        kk = np.arange(len(m["considerable"]), dtype=np.int32)
-        fg, fo = k.e.e.match_failures(kk), k.o.match_failures(ranked, jobs, offers, k.users, prm, kk, groups=hg)
-        grp = slice(abi.FAILC_N - 3, abi.FAILC_N)
-        assert [(f["n_vms"], f["counts"][grp]) for f in fg] == [(f["n_vms"], f["counts"][grp]) for f in fo]
-        placed = m["assign"] >= 0
-        jl = m["considerable"][placed].tolist()
-        tids = [k.tid + 3 * i for i in range(len(jl))]
-        k.tid += 3 * len(jl) + 3
-        k.e.launch(jl, tids, offers.col("hostname_id")[m["assign"][placed]])
-        return [spec[a]["host"] if a >= 0 else None for a in m["assign"]]
+def derived_cycle(k, spec):
+    """K13's group cases through the derived call: the cycle's derived match equals the sequenced one and the oracle
+    on host-built lists (failure counts included), then its placements are launched."""
+    offers = k.offers(spec)
+    q = k.e.gpu.state_rank(k.users)
+    G = len(k.kind)
+    groups = abi.Groups(n_groups=G, kind=k.kind, attr_col=k.col, minimum=k.minimum)
+    prm = traces.match_params(len(q))
+    m, _ = compare(k.e.gpu, offers, k.users, prm, groups=groups, grouped=True)
+    ids, jobs = k.jobs()
+    pos = {j: i for i, j in enumerate(ids)}
+    ranked = np.array([pos[j] for j in q], np.int32)
+    hc = cotasks(k.e.run.values(), G, k.col, offers.col("hostname_id"), offers.col("attr").reshape(1, offers.n))
+    hg = fed_tables(offers, k.users, groups, running_usage([], 1), hc)[2]
+    om = k.o.match(ranked, jobs, offers, k.users, prm, groups=hg)
+    assert np.array_equal(m["considerable"], np.array(ids)[om["considerable"]])
+    assert np.array_equal(m["assign"], om["assign"])
+    kk = np.arange(len(m["considerable"]), dtype=np.int32)
+    fg, fo = k.e.gpu.match_failures(kk), k.o.match_failures(ranked, jobs, offers, k.users, prm, kk, groups=hg)
+    grp = slice(abi.FAILC_N - 3, abi.FAILC_N)
+    assert [(f["n_vms"], f["counts"][grp]) for f in fg] == [(f["n_vms"], f["counts"][grp]) for f in fo]
+    k.launch_placed(m, offers)
+    return [spec[a]["host"] if a >= 0 else None for a in m["assign"]]
 
 
 @pytest.mark.gpu
 def test_k13_groups_through_the_derived_call(oracle):
-    p = K13D(oracle, [dict(kind=abi.GROUP_UNIQUE)])
+    p = K13(oracle, [dict(kind=abi.GROUP_UNIQUE)])
     try:
         host = [dict(host="test-host", cpus=100.0)]
-        p.k.submit(1)
-        assert p.cycle(host) == ["test-host"]
-        p.k.submit(2)                                   # its cotask runs on the only host
-        assert p.cycle(host) == [None, None]
+        p.submit(1)
+        assert derived_cycle(p, host) == ["test-host"]
+        p.submit(2)                                   # its cotask runs on the only host
+        assert derived_cycle(p, host) == [None, None]
     finally:
         p.close()
-    p = K13D(oracle, [dict(kind=abi.GROUP_BALANCED, col=0, minimum=3)])
+    p = K13(oracle, [dict(kind=abi.GROUP_BALANCED, col=0, minimum=3)])
     try:
         hosts = [dict(host=h, cpus=100.0, attrs={0: i + 1}) for i, h in enumerate(["straw", "sticks", "bricks"])]
-        p.k.submit(3)
-        first = p.cycle(hosts)
-        p.k.submit(6)
-        second = p.cycle(hosts)
+        p.submit(3)
+        first = derived_cycle(p, hosts)
+        p.submit(6)
+        second = derived_cycle(p, hosts)
         assert None not in first + second
         assert sorted(np.unique(first + second, return_counts=True)[1].tolist()) == [3, 3, 3]
     finally:
         p.close()
-    p = K13D(oracle, [dict(kind=abi.GROUP_ATTR_EQUALS, col=0)])
+    p = K13(oracle, [dict(kind=abi.GROUP_ATTR_EQUALS, col=0)])
     try:
         east = dict(host="first-east-host", cpus=1.0, attrs={0: 1})
-        p.k.submit(1)
-        assert p.cycle([east]) == ["first-east-host"]
+        p.submit(1)
+        assert derived_cycle(p, [east]) == ["first-east-host"]
         offers = [dict(east, cpus=0.5)] + [dict(host=f"west-{i:02d}", cpus=1.0, attrs={0: 2}) for i in range(20)]
         offers.append(dict(host="east-big", cpus=5.0, attrs={0: 1}))
-        p.k.submit(20)
-        got = p.cycle(offers)
+        p.submit(20)
+        got = derived_cycle(p, offers)
         assert got.count("east-big") == 5 and got.count(None) == 15
     finally:
         p.close()
@@ -409,15 +275,13 @@ def test_k13_groups_through_the_derived_call(oracle):
 # ---- GPU: config-#4 rebalance -----------------------------------------------------------------------------------
 @pytest.mark.gpu
 def test_c4_rebalance_derived(oracle):
-    from test_state_rebalance import RPool, _pool, decisions_eq, rows_of
-    from test_state_resident import jobs_soa, tasks_soa
-    r, codes = _pool(23, True)
+    r, codes = rebalance_trace(23, True)
     rng = np.random.default_rng(29)
     G, g0, hosts = r["groups"].n_groups, r["groups"], r["hosts"]
     pend, run = rows_of(r, codes)
     for row in run.values():
         row["groups"] = [int(rng.integers(G))] if rng.random() < 0.2 else []
-    p = RPool(r, codes)
+    p = Pool.of_rebalance(r, codes)
     try:
         run_up = list(run.values())
         pj, pp, jid = jobs_soa(sorted(pend.items()))
@@ -432,14 +296,14 @@ def test_c4_rebalance_derived(oracle):
             cot = p.gpu.state_cotasks(G, acol, hosts)
             assert len(cot[1]) > 300
             p.groups = with_fields(g0, cot_off=cot[0], cot_hostname_id=cot[1], cot_attr_val=cot[2])
-            want = p.gpu.state_rebalance(hosts, p.users, p.params, groups=p.groups)
+            want = p.gpu.state_rebalance(hosts, p.users, p.rparams, groups=p.groups)
             sw = p.gpu.last_stats(abi.PHASE_REBALANCE)
-            got = p.gpu.state_rebalance(hosts, p.users, p.params, groups=with_fields(g0, **{f: None for f in COT_FIELDS}),
+            got = p.gpu.state_rebalance(hosts, p.users, p.rparams, groups=with_fields(g0, **{f: None for f in COT_FIELDS}),
                                         derived=True)
             sd = p.gpu.last_stats(abi.PHASE_REBALANCE)
             decisions_eq(got, want)
             assert got
-            decisions_eq(got, p.want(oracle))
+            decisions_eq(got, p.want_rebalance(oracle))
             assert sd["h2d_bytes"] == sw["h2d_bytes"] - (4 * (G + 1) + 8 * len(cot[1]))
             assert sd["d2h_bytes"] == sw["d2h_bytes"]
             fin = [t for t in p.run if rng.random() < 0.1]       # finishes move the lists between steps
@@ -453,18 +317,17 @@ def test_c4_rebalance_derived(oracle):
 def test_freshness_after_launches(oracle):
     """After each cycle's launches the derived match sees the launched tasks: it equals a sequenced match fed with
     freshly derived inputs, while a match fed with the previous cycle's arrays differs on the same inputs."""
-    from test_state_usage import Handle, pending_rows, random_rows
     rng = np.random.default_rng(51)
     U, O, J = 10, 40, 500
     codes = (100 + np.arange(O)).astype(np.int32)
-    h = Handle("fresh")
+    h = Pool("fresh", drop=drop_all_but("gpus", "novel"), send_hosts=True)
     pend = pending_rows(rng, "grid", J, U, 1_000_000, codes.tolist())
     for x in pend:
         x["gpus"], x["novel"] = 0.0, []
     run = random_rows(rng, "grid", 300, U, 10, codes.tolist() + [-1])
     for x in run:
         x["gpus"] = 0.0
-    h.apply(up=run, pend_up=pend)
+    h.apply(up=keyed(pend), run_up=run)
     cnt0 = np.bincount([x["user"] for x in run], minlength=U).astype(float)
     quota = {"count": cnt0 + 30.0, "cpus": np.full(U, 1e9), "mem": np.full(U, 1e12), "gpus": np.full(U, 1e9)}
     users = abi.make_users(U, quota=quota, div_cpus=np.full(U, 40.0), div_mem=np.full(U, 81920.0), div_gpus=np.ones(U))
@@ -475,21 +338,21 @@ def test_freshness_after_launches(oracle):
     tid = 10_000_000
     try:
         for cycle in range(4):
-            h.e.state_rank(users)
-            got, (so, su, _) = compare(h.e, offers, users, prm)
+            h.gpu.state_rank(users)
+            got, (so, su, _) = compare(h.gpu, offers, users, prm)
             want = running_usage(h.run.values(), U, codes)
             for f, k in zip(USAGE_FIELDS, KEYS):
                 assert F.same_bits(su.col(f), want["user"][k])
             assert 0 < len(got["considerable"]) < len(h.pend)
             if stale is not None:
-                old = h.e.state_match(stale[0], stale[1], prm)
+                old = h.gpu.state_match(stale[0], stale[1], prm)
                 differs |= not np.array_equal(old["considerable"], got["considerable"])
             stale = (so, su)
             placed = got["assign"] >= 0
             jl = got["considerable"][placed]
             tids = tid + 2 * np.arange(len(jl), dtype=np.int64)
             tid += 2 * len(jl) + 2
-            h.launch(jl.tolist(), tids.tolist(), codes[got["assign"][placed]])
+            h.launch(jl.tolist(), tids.tolist(), np.full(len(jl), START, np.int64), codes[got["assign"][placed]])
         assert differs
     finally:
         h.close()
@@ -497,7 +360,6 @@ def test_freshness_after_launches(oracle):
 
 @pytest.mark.gpu
 def test_layout_independence():
-    from test_state_resident import pool_rows
     t = traces.gen_c3_pool(31, n_jobs=1500, n_offers=120, n_users=20, n_running=600)
     rng = np.random.default_rng(33)
     g0, offers, users = t["groups"], t["offers"], t["users"]
@@ -509,7 +371,7 @@ def test_layout_independence():
     items, rr = sorted(pend.items()), list(run.values())
     prm = traces.match_params(1000)
     max_ports = int(t["jobs"].col("ports").max())
-    a, b = Pool("a"), Pool("b")
+    a, b = new_pool("a"), new_pool("b")
     try:
         a.apply(up=items, run_up=sorted(rr, key=lambda r: r["task_id"]))
         junk = [dict(r, task_id=r["task_id"] + 10 ** 10, job_id=r["job_id"] + 10 ** 10) for r in rr[:400]]
@@ -520,9 +382,9 @@ def test_layout_independence():
         b.apply(run_up=perm[300:])
         out = []
         for p in (a, b):
-            p.e.state_rank(users)
+            p.gpu.state_rank(users)
             do, du, dg = derived_inputs(offers, users, g0)
-            out.append(p.e.state_match(do, du, prm, groups=dg, max_ports=max_ports, derived=True))
+            out.append(p.gpu.state_match(do, du, prm, groups=dg, max_ports=max_ports, derived=True))
         for k in ("considerable", "assign", "ports", "fail"):
             assert np.array_equal(out[0][k], out[1][k]), k
         assert (out[0]["assign"] >= 0).sum() > 0
@@ -535,7 +397,6 @@ def test_layout_independence():
 @pytest.mark.parametrize("scale", [1, 6])
 def test_transfer_accounting(scale):
     """h2d = the sequenced match's minus exactly 32 U + 20 O + 4 (G + 1) + 8 max(1, N); d2h equal (compare())."""
-    from test_state_resident import pool_rows
     t = traces.gen_c3_pool(61 + scale, n_jobs=500 * scale, n_offers=40 * scale, n_users=8 * scale, n_running=200 * scale)
     rng = np.random.default_rng(scale)
     g0, offers, users = t["groups"], t["offers"], t["users"]
@@ -543,13 +404,13 @@ def test_transfer_accounting(scale):
     _hosts_for(rng, run, offers.col("hostname_id"))
     for r in run.values():
         r["groups"] = [int(rng.integers(g0.n_groups))] if rng.random() < 0.3 else []
-    p = Pool("acct")
+    p = new_pool("acct")
     try:
         p.apply(up=sorted(pend.items()), run_up=list(run.values()))
-        p.e.state_rank(users)
-        got, (_, _, sg) = compare(p.e, offers, users, traces.match_params(1000), groups=g0,
-                                  max_ports=int(t["jobs"].col("ports").max()), grouped=p.grouped())
-        assert p.grouped() and int(sg.col("cot_off")[-1]) > 0 and len(got["considerable"]) > 0
+        p.gpu.state_rank(users)
+        got, (_, _, sg) = compare(p.gpu, offers, users, traces.match_params(1000), groups=g0,
+                                  max_ports=int(t["jobs"].col("ports").max()), grouped=grouped(p))
+        assert grouped(p) and int(sg.col("cot_off")[-1]) > 0 and len(got["considerable"]) > 0
         assert got["stats"]["ms_h2d"] > 0.0 and got["stats"]["n_launches"] > 0
     finally:
         p.close()
@@ -558,7 +419,6 @@ def test_transfer_accounting(scale):
 # ---- GPU: errors and edges -------------------------------------------------------------------------------------
 def _small(rng, n_run=120, G=4):
     t = traces.gen_c3_pool(71, n_jobs=300, n_offers=30, n_users=6, n_running=n_run)
-    from test_state_resident import pool_rows
     pend, run = pool_rows(t)
     _hosts_for(rng, run, t["offers"].col("hostname_id"))
     for r in run.values():
@@ -574,12 +434,12 @@ def test_errors_write_nothing():
     t, pend, run, groups = _small(rng)
     offers, users = t["offers"], t["users"]
     prm = traces.match_params(1000)
-    p = Pool("errors")
+    p = new_pool("errors")
     try:
         p.apply(up=sorted(pend.items()), run_up=list(run.values()))
-        p.e.state_rank(users)
-        before, _ = compare(p.e, offers, users, prm, groups=groups, grouped=p.grouped())
-        lib, pool = p.e.lib, p.e.pool
+        p.gpu.state_rank(users)
+        before, _ = compare(p.gpu, offers, users, prm, groups=groups, grouped=grouped(p))
+        lib, pool = p.gpu.lib, p.gpu.pool
         do, du, dg = derived_inputs(offers, users, groups)
         O = offers.n
         hn = offers.col("hostname_id")
@@ -610,7 +470,7 @@ def test_errors_write_nothing():
         assert (cons == -7).all() and (assign == -7).all() and (ports == -7).all() and (fail == 7).all()
         assert lib.cook_state_match_derived(pool, None, None, None, None, None, None, None, None, 0, None, None) == \
             abi.COOK_E_BADARG
-        after, _ = compare(p.e, offers, users, prm, groups=groups, grouped=p.grouped())   # unaffected
+        after, _ = compare(p.gpu, offers, users, prm, groups=groups, grouped=grouped(p))   # unaffected
         for key in ("considerable", "assign", "ports", "fail"):
             assert np.array_equal(after[key], before[key])
         # the rebalance's own cases; GPU DRU mode is unsupported
@@ -643,47 +503,47 @@ def test_edges(oracle):
     t, pend, run, groups = _small(rng)
     offers, users = t["offers"], t["users"]
     prm = traces.match_params(1000)
-    p = Pool("edges")
+    p = new_pool("edges")
     try:
         items = sorted(pend.items())
         p.apply(up=items)                                  # no live running row
-        p.e.state_rank(users)
-        got, (so, su, sg) = compare(p.e, offers, users, prm, groups=groups, grouped=p.grouped())
+        p.gpu.state_rank(users)
+        got, (so, su, sg) = compare(p.gpu, offers, users, prm, groups=groups, grouped=grouped(p))
         assert all((su.col(f) == 0).all() for f in USAGE_FIELDS) and (sg.col("cot_off") == 0).all()
-        n0 = p.e.last_stats(abi.PHASE_MATCH)["n_launches"]
+        n0 = p.gpu.last_stats(abi.PHASE_MATCH)["n_launches"]
         zo, zu, zg = fed_tables(offers, users, groups, running_usage([], users.n_users, offers.col("hostname_id")),
                                 ([0] * (groups.n_groups + 1), [], []))
-        plain = p.e.state_match(zo, zu, prm, groups=zg)
-        assert p.e.last_stats(abi.PHASE_MATCH)["n_launches"] == n0   # no derivation kernel: the same launches
+        plain = p.gpu.state_match(zo, zu, prm, groups=zg)
+        assert p.gpu.last_stats(abi.PHASE_MATCH)["n_launches"] == n0   # no derivation kernel: the same launches
         assert np.array_equal(plain["assign"], got["assign"])
         # no groups; groups without a running row that has both a host and a group
         rows = list(run.values())
         p.apply(run_up=[dict(r, groups=[]) for r in rows[:40]] + [dict(r, host=-1) for r in rows[40:80]])
-        p.e.state_rank(users)
-        compare(p.e, offers, users, prm, grouped=p.grouped())
-        _, (_, _, sg) = compare(p.e, offers, users, prm, groups=groups, grouped=p.grouped())
+        p.gpu.state_rank(users)
+        compare(p.gpu, offers, users, prm, grouped=grouped(p))
+        _, (_, _, sg) = compare(p.gpu, offers, users, prm, groups=groups, grouped=grouped(p))
         assert (sg.col("cot_off") == 0).all()
         # running rows on hosts without an offer this cycle, and with host -1
         p.apply(run_up=[dict(r, host=7777) for r in rows[80:]])
-        p.e.state_rank(users)
-        got, _ = compare(p.e, offers, users, prm, groups=groups, grouped=p.grouped())
-        jobs, jid, ranked = p.ranked(p.e.state_rank(users))
-        oracle_check(oracle, got, p.m.run.values(), jobs, jid, ranked, offers, users, prm, groups)
+        p.gpu.state_rank(users)
+        got, _ = compare(p.gpu, offers, users, prm, groups=groups, grouped=grouped(p))
+        jobs, jid, ranked_ = live_positions(p, p.gpu.state_rank(users))
+        oracle_check(oracle, got, p.run.values(), jobs, jid, ranked_, offers, users, prm, groups)
         # offers->n == 0: as cook_state_match
         empty = abi.OffersSoA(n=0, hostname_id=np.zeros(1, np.int32), name_rank=np.zeros(1, np.int32),
                               cpus=np.zeros(1), mem=np.zeros(1), run_cpus=np.zeros(1), run_mem=np.zeros(1),
                               run_count=np.zeros(1, np.int32), n_attr_cols=offers.n_attr_cols, attr=np.zeros(4, np.int32))
-        got, _ = compare(p.e, empty, users, prm, groups=groups, grouped=p.grouped())
+        got, _ = compare(p.gpu, empty, users, prm, groups=groups, grouped=grouped(p))
         assert (got["fail"] == abi.FAIL_NO_OFFERS).all() and len(got["fail"]) > 0
         # no live queue row: returns before any device work, as cook_state_match does
-        p.apply(rm=sorted(p.m.pend))
-        got, _ = compare(p.e, offers, users, prm, groups=groups, grouped=p.grouped())
+        p.apply(rm=sorted(p.pend))
+        got, _ = compare(p.gpu, offers, users, prm, groups=groups, grouped=grouped(p))
         assert len(got["considerable"]) == 0
-        q = Pool("fresh")
+        q = new_pool("fresh")
         try:
             do, du, dg = derived_inputs(offers, users, groups)
             with pytest.raises(CookError):                 # no rank on a fresh handle
-                q.e.state_match(do, du, prm, groups=dg, derived=True)
+                q.gpu.state_match(do, du, prm, groups=dg, derived=True)
         finally:
             q.close()
     finally:

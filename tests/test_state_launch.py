@@ -6,27 +6,13 @@ tables built from it (and rank the oracle).  A launch must leave exactly the sta
 patch must keep the job in the ranked queue where an upsert drops it.  Plus the match's column-presence switch, slot
 layout, the rebalancer's view of launched tasks, upload accounting and the all-or-nothing errors.
 """
-import ctypes as C
-import os
-
 import numpy as np
 import pytest
 
-from cook_b200 import abi, engine, traces
-from cook_b200.engine import CookError, GpuEngine
-from test_state_rebalance import RPool, _pool, decisions_eq, rdelta, rows_of
-from test_state_resident import Model, _c2, _c3, _churn, pool_rows
-
-START = 1_700_000_000_000
-
-
-def test_launch_patch_symbols_exported():
-    if not os.path.exists(engine.LIB_PATH):
-        pytest.skip("libcookgpu.so not built")
-    lib = engine.load_library()
-    for name in ("cook_state_launch", "cook_state_patch"):
-        assert hasattr(lib, name), name
-    assert callable(GpuEngine.state_launch) and callable(GpuEngine.state_patch)
+from cook_b200 import abi
+from cook_b200.engine import CookError
+from resident_model import (START, Pool, c2, c3, churn, decisions_eq, pool_rows, rebalance_trace, rows_of,
+                            task_of, with_fields)
 
 
 def hosts_of(offers):
@@ -39,118 +25,64 @@ def hosts_of(offers):
 
 def with_reserved(offers, idx):
     """The offers with `reserved` set on the offer indices idx."""
-    kw = {n: offers.col(n) for n, _ in offers._fields_ if offers.col(n) is not None}
     res = np.zeros(offers.n, np.uint8)
     res[list(idx)] = 1
-    kw.update(n=offers.n, n_attr_cols=offers.n_attr_cols, reserved=res)
-    return abi.OffersSoA(**kw)
-
-
-def task_of(row, job_id, task_id, start, host):
-    return dict(user=row["user"], priority=row["priority"], start_time=int(start), task_id=int(task_id),
-                job_id=int(job_id), cpus=row["cpus"], mem=row["mem"], gpus=row["gpus"], host=int(host))
+    return with_fields(offers, reserved=res)
 
 
 class Twin:
-    """A (launches and patches by id), B (the same as deltas), the host-table handle and the model."""
+    """A (launches and patches by id) and B (the same changes as deltas), each with its host-table handle and model."""
 
     def __init__(self, t, groups=None):
-        self.t, self.users, self.offers, self.groups = t, t["users"], t["offers"], groups
+        self.a = Pool.of_trace(t, groups, name="launch", send_hosts=True)
+        self.b = Pool.of_trace(t, groups, name="delta", send_hosts=True, ref=self.a.ref)
         self.hosts = hosts_of(t["offers"])
-        self.params = traces.match_params(min(1000, t["jobs"].n), host_lifetime_mins=t.get("host_lifetime_mins", 0))
         self.rparams = abi.RebalanceParams(32, 0.0, 0.0, 0)
-        self.max_ports = int(t["jobs"].col("ports").max()) if t["jobs"].col("ports") is not None else 0
-        self.a, self.b, self.ref = GpuEngine(pool_name="launch"), GpuEngine(pool_name="delta"), GpuEngine(pool_name="host")
-        self.m = Model()
-        self.queue, self.gone = [], {"a": set(), "b": set()}
 
     def close(self):
-        for e in (self.a, self.b, self.ref):
-            e.close()
+        self.a.close()
+        self.b.close()
 
     def apply(self, up=(), rm=(), run_up=(), run_rm=(), reset=False):
-        up, run_up = list(up), list(run_up)
-        for e in (self.a, self.b):
-            e.state_apply(rdelta(reset, up, rm, run_up, run_rm))
-        self.m.apply(up, rm, run_up, run_rm, reset)
-        for g in self.gone.values():
-            g |= set(rm) | {j for j, _ in up} | (set(self.queue) if reset else set())
+        for p in (self.a, self.b):
+            p.apply(up, rm, run_up, run_rm, reset)
 
     def launch(self, jobs, tids, starts, hosts=None):
         """A: cook_state_launch; B: the batch pending_rm = jobs plus the running upserts built from the rows."""
-        tasks = [task_of(self.m.pend[j], j, t, s, -1 if hosts is None else h)
+        tasks = [task_of(self.b.pend[j], j, t, s, -1 if hosts is None else h)
                  for j, t, s, h in zip(jobs, tids, starts, hosts if hosts is not None else [None] * len(jobs))]
-        self.a.state_launch(jobs, tids, starts, hosts)
-        self.b.state_apply(rdelta(rm=jobs, run_up=tasks, with_hosts=hosts is not None))
-        self.m.apply(d_rm=jobs, r_up=tasks)
-        for g in self.gone.values():
-            g |= set(jobs)
+        self.a.launch(jobs, tids, starts, hosts)
+        self.b.apply(rm=jobs, run_up=tasks, hosts=hosts is not None)
         return tasks
 
     def patch(self, jobs, allowed=None, plugin_accept=None, reserved_host=None, clear=False, upsert_b=True):
         """A: cook_state_patch.  B (upsert_b): the same columns as pending upserts, which drop the jobs from the
         queue; else B is patched too."""
-        if clear:
-            for r in self.m.pend.values():
-                r["reserved_host"] = -1
-        cols = {"allowed": allowed, "plugin_accept": plugin_accept, "reserved_host": reserved_host}
-        for k, j in enumerate(jobs):
-            self.m.pend[j] = dict(self.m.pend[j], **{c: int(v[k]) for c, v in cols.items() if v is not None})
-        self.a.state_patch(jobs, allowed, plugin_accept, reserved_host, clear)
+        cols = dict(allowed=allowed, plugin_accept=plugin_accept, reserved_host=reserved_host)
+        self.a.patch(jobs, clear, **cols)
         if upsert_b:
             if clear:
-                self.b.state_patch([], clear_reservations=True)
-            self.b.state_apply(rdelta(up=[(j, self.m.pend[j]) for j in jobs]))
-            self.gone["b"] |= set(jobs)
+                self.b.patch([], clear=True)
+            self.b.apply(up=[(j, self.a.pend[j]) for j in jobs])
         else:
-            self.b.state_patch(jobs, allowed, plugin_accept, reserved_host, clear)
+            self.b.patch(jobs, clear, **cols)
 
     def rank(self, oracle=None):
-        qa, qb = self.a.state_rank(self.users), self.b.state_rank(self.users)
+        qa, qb = self.a.check_rank(oracle), self.b.rank()
         assert np.array_equal(qa, qb), "launch handle and delta twin rank differently"
-        running, pending, _, jid = self.m.tables()
-        host = self.ref.rank(running if running.n else None, pending, self.users)
-        assert np.array_equal(qa, jid[host["ranked"]]), "resident rank != cook_rank on the same rows"
-        if oracle is not None and pending.n:
-            o = oracle.rank(running if running.n else None, pending, self.users)
-            assert np.array_equal(qa, jid[o["ranked"]]), "resident rank != oracle"
-        self.queue, self.gone = qa.tolist(), {"a": set(), "b": set()}
         return qa
-
-    def _match_one(self, e, gone, offers):
-        got = e.state_match(offers, self.users, self.params, groups=self.groups, max_ports=self.max_ports)
-        _, _, jobs, jid = self.m.tables()
-        pos = {j: i for i, j in enumerate(jid.tolist())}
-        ranked = np.array([pos[j] for j in self.queue if j not in gone], np.int32)
-        if len(ranked) == 0:
-            assert len(got["considerable"]) == 0
-            return got
-        want = self.ref.match(ranked, jobs, offers, self.users, self.params, groups=self.groups,
-                              max_ports=self.max_ports)
-        assert np.array_equal(got["considerable"], jid[want["considerable"]]), "considerable"
-        for k in ("assign", "ports", "fail"):
-            assert np.array_equal(got[k], want[k]), k
-        n = len(got["considerable"])
-        if n:
-            k = np.unique(np.linspace(0, n - 1, min(n, 16)).astype(np.int32))
-            assert e.match_failures(k) == self.ref.match_failures(k)
-        nu = self.users.n_users
-        assert np.array_equal(e.exchange_usage(nu), self.ref.exchange_usage(nu))
-        return got
 
     def match(self, offers=None, same=True):
         """Both handles against the host-table path on the model; `same`: A and B must also agree."""
-        offers = offers if offers is not None else self.offers
-        ga = self._match_one(self.a, self.gone["a"], offers)
-        gb = self._match_one(self.b, self.gone["b"], offers)
+        ga, gb = self.a.check_match(offers=offers), self.b.check_match(offers=offers)
         if same:
             for k in ("considerable", "assign", "ports", "fail"):
                 assert np.array_equal(ga[k], gb[k]), k
         return ga, gb
 
     def rebalance(self):
-        ra = self.a.state_rebalance(self.hosts, self.users, self.rparams, groups=self.groups)
-        rb = self.b.state_rebalance(self.hosts, self.users, self.rparams, groups=self.groups)
+        ra = self.a.gpu.state_rebalance(self.hosts, self.a.users, self.rparams, groups=self.a.groups)
+        rb = self.b.gpu.state_rebalance(self.hosts, self.b.users, self.rparams, groups=self.b.groups)
         decisions_eq(ra, rb)
         return ra
 
@@ -170,7 +102,7 @@ def _load(t, frac=0.85, seed=1):
 @pytest.mark.gpu
 @pytest.mark.parametrize("kind", ["c2", "c3"])
 def test_launch_equivalence(kind, oracle):
-    t = _c2(11) if kind == "c2" else _c3(13)
+    t = c2(11) if kind == "c2" else c3(13)
     p = Twin(t, t.get("groups"))
     try:
         first, reserve, run = _load(t)
@@ -186,7 +118,7 @@ def test_launch_equivalence(kind, oracle):
                 ga, _ = p.match()
                 placed = [(int(j), int(a)) for j, a in zip(ga["considerable"], ga["assign"]) if a >= 0][:60]
                 launched = [j for j, _ in placed]
-                up, rm, run_up, run_rm = _churn(p, rng, reserve, t_next, launched)
+                up, rm, run_up, run_rm = churn(p.a, rng, reserve, t_next, launched)
                 # _churn's launches: the first len(launched) removals and every running upsert
                 assert rm[:len(launched)] == launched and len(run_up) == len(launched)
                 p.launch(launched, [r["task_id"] for r in run_up], [r["start_time"] for r in run_up],
@@ -195,7 +127,7 @@ def test_launch_equivalence(kind, oracle):
                 p.apply(up, rm[len(launched):], (), run_rm)
                 p.rebalance()
             if cycle == 3:                            # new leadership
-                p.apply(up=sorted(p.m.pend.items()), run_up=list(p.m.run.values()), reset=True)
+                p.apply(up=sorted(p.a.pend.items()), run_up=list(p.a.run.values()), reset=True)
         p.rank(oracle)
         p.match()
         p.rebalance()
@@ -206,7 +138,7 @@ def test_launch_equivalence(kind, oracle):
 
 @pytest.mark.gpu
 def test_patch_keeps_queue():
-    t = _c3(17)
+    t = c3(17)
     p = Twin(t, t["groups"])
     try:
         first, _, run = _load(t, frac=1.0)
@@ -244,7 +176,7 @@ def test_patch_keeps_queue():
 
 @pytest.mark.gpu
 def test_reservation_map_replacement():
-    t = _c3(19)
+    t = c3(19)
     p = Twin(t, t["groups"])
     try:
         first, _, run = _load(t, frac=1.0)
@@ -254,18 +186,18 @@ def test_reservation_map_replacement():
         set1, set2 = q[0:40:2], q[1:41:2]
         h1, h2 = hn[np.arange(20)], hn[np.arange(20, 40)]
         p.patch(set1, reserved_host=h1, clear=True, upsert_b=False)
-        n1 = sum(r["reserved_host"] != -1 for r in p.m.pend.values())
+        n1 = sum(r["reserved_host"] != -1 for r in p.a.pend.values())
         p.patch(set2, reserved_host=h2, clear=True, upsert_b=False)
-        st = p.a.last_stats(abi.PHASE_STATE)
+        st = p.a.gpu.last_stats(abi.PHASE_STATE)
         assert st["h2d_bytes"] == 4 * n1 + len(set2) * (4 + 4)
-        assert all(p.m.pend[j]["reserved_host"] == -1 for j in set1)
+        assert all(p.a.pend[j]["reserved_host"] == -1 for j in set1)
         # every host of both sets is reserved: set 1's hosts now take no job at all, set 2's only their own
         ga, _ = p.match(offers=with_reserved(t["offers"], range(40)))
         for j, a in zip(ga["considerable"].tolist(), ga["assign"].tolist()):
-            assert a < 0 or a >= 40 or (20 <= a < 40 and p.m.pend[j]["reserved_host"] == hn[a]), (j, a)
+            assert a < 0 or a >= 40 or (20 <= a < 40 and p.a.pend[j]["reserved_host"] == hn[a]), (j, a)
         # the second set's jobs without reservation again: a clear with an empty batch
         p.patch([], clear=True, upsert_b=False)
-        assert p.a.last_stats(abi.PHASE_STATE)["h2d_bytes"] == 4 * len(set2)
+        assert p.a.gpu.last_stats(abi.PHASE_STATE)["h2d_bytes"] == 4 * len(set2)
         p.match()
     finally:
         p.close()
@@ -273,7 +205,7 @@ def test_reservation_map_replacement():
 
 @pytest.mark.gpu
 def test_presence_switch():
-    t = _c2(23)                                       # no job holds a reservation, a disallow or a plugin veto
+    t = c2(23)                                       # no job holds a reservation, a disallow or a plugin veto
     p = Twin(t)
     try:
         first, _, run = _load(t, frac=1.0)
@@ -307,7 +239,7 @@ def test_presence_switch():
 
 @pytest.mark.gpu
 def test_launch_layout():
-    t = _c3(29)
+    t = c3(29)
     p = Twin(t, t["groups"])
     try:
         first, reserve, run = _load(t, frac=0.6)
@@ -327,7 +259,7 @@ def test_launch_layout():
         jobs = [j for j, _ in long_rows[:300]]
         tids = [5 * 10 ** 9 + 3 * k for k in range(300)]
         p.launch(jobs, tids, [START + k for k in range(300)], [int(hn[k % len(hn)]) for k in range(300)])
-        st = p.a.last_stats(abi.PHASE_STATE)
+        st = p.a.gpu.last_stats(abi.PHASE_STATE)
         assert st["n_launches"] > 2, "the launch compacted no list arena"
         p.match()
         p.rank()
@@ -344,26 +276,15 @@ def test_launch_layout():
         p.close()
 
 
-class LRPool(RPool):
-    """RPool plus launches by job id."""
-
-    def launch(self, jobs, tids, starts, hosts=None):
-        self.gpu.state_launch(jobs, tids, starts, hosts)
-        for k, j in enumerate(jobs):
-            row = self.pend.pop(j)
-            self.run[tids[k]] = task_of(row, j, tids[k], starts[k], -1 if hosts is None else hosts[k])
-        self.gone |= set(jobs)
-
-
 @pytest.mark.gpu
 def test_rebalance_after_launch(oracle):
-    r, codes = _pool(121, True)
+    r, codes = rebalance_trace(121, True)
     pend, run = rows_of(r, codes)
-    p = LRPool(r, codes)
+    p = Pool.of_rebalance(r, codes)
     try:
         p.apply(up=sorted(pend.items()), run_up=list(run.values()))
         p.rank()
-        before = p.check()
+        before = p.check_rebalance()
         # new jobs of the victims' user start on the hosts the walk preempts on, later than all its tasks: the
         # walk should now take some of them
         u = min(p.run[v]["user"] for d in before for v in d["victims"] if v >= 0)
@@ -373,7 +294,7 @@ def test_rebalance_after_launch(oracle):
         hosts = [int(codes[before[k % len(before)]["host"]]) for k in range(len(jobs))]
         p.launch(jobs, tids, [START + 10 ** 6 + k for k in range(len(jobs))], hosts)
         p.rank()
-        got = p.check(oracle)
+        got = p.check_rebalance(oracle)
         victims = {v for d in got for v in d["victims"]}
         assert victims & set(tids), "no launched task was chosen as a victim"
         # a launch with no host leaves a running row the rebalancer cannot place
@@ -381,7 +302,7 @@ def test_rebalance_after_launch(oracle):
         p.launch([j], [9 * 10 ** 9 + 999], [START])
         p.rank()
         with pytest.raises(CookError) as e:
-            p.gpu.state_rebalance(p.hosts, p.users, p.params, groups=p.groups)
+            p.gpu.state_rebalance(p.hosts, p.users, p.rparams, groups=p.groups)
         assert e.value.code == abi.COOK_E_BADARG
     finally:
         p.close()
@@ -390,7 +311,7 @@ def test_rebalance_after_launch(oracle):
 @pytest.mark.gpu
 @pytest.mark.parametrize("n", [7, 300])
 def test_accounting(n):
-    t = _c2(31)
+    t = c2(31)
     p = Twin(t)
     try:
         first, reserve, run = _load(t, frac=0.7)
@@ -400,7 +321,7 @@ def test_accounting(n):
         for k, (js, hosts) in enumerate(((jobs[:n], [int(hn[i % len(hn)]) for i in range(n)]), (jobs[n:], None))):
             tids = [7 * 10 ** 9 + 10 * k * n + i for i in range(n)]
             p.launch(js, tids, [START + i for i in range(n)], hosts)
-            a, b = p.a.last_stats(abi.PHASE_STATE), p.b.last_stats(abi.PHASE_STATE)
+            a, b = p.a.gpu.last_stats(abi.PHASE_STATE), p.b.gpu.last_stats(abi.PHASE_STATE)
             assert a["h2d_bytes"] == n * (4 + 4 + 8 + 8) + (4 * n if hosts else 0)
             # the delta: the task rows (8 columns, 56 B), a slot per removal and per upsert
             assert b["h2d_bytes"] == n * (56 + 4 + 4) + (4 * n if hosts else 0)
@@ -411,9 +332,9 @@ def test_accounting(n):
         for cols, size in (({"allowed": z8}, 5), ({"plugin_accept": z8, "reserved_host": z32}, 9),
                            ({"allowed": z8, "plugin_accept": z8, "reserved_host": codes}, 10), ({}, 0)):
             p.patch(rest, upsert_b=False, **cols)
-            assert p.a.last_stats(abi.PHASE_STATE)["h2d_bytes"] == n * size
+            assert p.a.gpu.last_stats(abi.PHASE_STATE)["h2d_bytes"] == n * size
         p.patch([], clear=True, upsert_b=False)        # n reservations from the third patch
-        assert p.a.last_stats(abi.PHASE_STATE)["h2d_bytes"] == 4 * n
+        assert p.a.gpu.last_stats(abi.PHASE_STATE)["h2d_bytes"] == 4 * n
         p.rank()
         p.match()
     finally:
@@ -422,14 +343,14 @@ def test_accounting(n):
 
 @pytest.mark.gpu
 def test_errors():
-    t = _c3(37)
+    t = c3(37)
     p = Twin(t, t["groups"])
     try:
         first, _, run = _load(t, frac=1.0)
         p.apply(up=first, run_up=run)
         p.rank()
         ids = [j for j, _ in first]
-        live_tid = next(iter(p.m.run))
+        live_tid = next(iter(p.a.run))
         gone = ids[0]
         p.launch([gone], [10 ** 10], [START], [int(t["offers"].col("hostname_id")[0])])   # no longer pending
         p.rank()
@@ -446,36 +367,36 @@ def test_errors():
         def raw_launch(n, jid, tid, st, hn=None):
             arr = [np.ascontiguousarray(x, np.int64) if x is not None else None for x in (jid, tid, st)]
             h = np.ascontiguousarray(hn, np.int32) if hn is not None else None
-            rc = p.a.lib.cook_state_launch(p.a.pool, int(n), *[abi.ptr(x, abi.P_I64) if x is not None else None for x in arr],
+            rc = p.a.gpu.lib.cook_state_launch(p.a.gpu.pool, int(n), *[abi.ptr(x, abi.P_I64) if x is not None else None for x in arr],
                                            abi.ptr(h, abi.P_I32) if h is not None else None)
             if rc != 0:
-                p.a._err(rc)
+                p.a.gpu._err(rc)
 
         def raw_patch(n, jid, rh=None):
             j = np.ascontiguousarray(jid, np.int64) if jid is not None else None
             h = np.ascontiguousarray(rh, np.int32) if rh is not None else None
-            rc = p.a.lib.cook_state_patch(p.a.pool, int(n), abi.ptr(j, abi.P_I64) if j is not None else None, None,
+            rc = p.a.gpu.lib.cook_state_patch(p.a.gpu.pool, int(n), abi.ptr(j, abi.P_I64) if j is not None else None, None,
                                           None, abi.ptr(h, abi.P_I32) if h is not None else None, 0)
             if rc != 0:
-                p.a._err(rc)
+                p.a.gpu._err(rc)
 
         j1, j2 = ids[1], ids[2]
         fails(lambda: raw_launch(-1, [j1], [1], [1]))                                  # n < 0
         fails(lambda: raw_launch(1, None, [1], [1]))                                   # null required columns
         fails(lambda: raw_launch(1, [j1], None, [1]))
         fails(lambda: raw_launch(1, [j1], [1], None))
-        fails(lambda: p.a.state_launch([j1, 10 ** 13], [1, 2], [1, 1]))               # unknown job id
-        fails(lambda: p.a.state_launch([j1, gone], [1, 2], [1, 1]))                   # not live
-        fails(lambda: p.a.state_launch([j1, j1], [1, 2], [1, 1]))                     # job id twice
-        fails(lambda: p.a.state_launch([j1, j2], [3, 3], [1, 1]))                     # task id twice
-        fails(lambda: p.a.state_launch([j1, j2], [3, live_tid], [1, 1]))              # task id already live
-        fails(lambda: p.a.state_launch([j1, j2], [3, 4], [1, 1], [0, -2]))            # hostname code below -1
+        fails(lambda: p.a.gpu.state_launch([j1, 10 ** 13], [1, 2], [1, 1]))               # unknown job id
+        fails(lambda: p.a.gpu.state_launch([j1, gone], [1, 2], [1, 1]))                   # not live
+        fails(lambda: p.a.gpu.state_launch([j1, j1], [1, 2], [1, 1]))                     # job id twice
+        fails(lambda: p.a.gpu.state_launch([j1, j2], [3, 3], [1, 1]))                     # task id twice
+        fails(lambda: p.a.gpu.state_launch([j1, j2], [3, live_tid], [1, 1]))              # task id already live
+        fails(lambda: p.a.gpu.state_launch([j1, j2], [3, 4], [1, 1], [0, -2]))            # hostname code below -1
         fails(lambda: raw_patch(-1, [j1]))                                             # n < 0
         fails(lambda: raw_patch(1, None))                                              # null job_id
-        fails(lambda: p.a.state_patch([j1, 10 ** 13], allowed=[0, 0]))               # unknown job id
-        fails(lambda: p.a.state_patch([j1, gone], allowed=[0, 0]))                    # not live
-        fails(lambda: p.a.state_patch([j1, j1], allowed=[0, 0]))                      # job id twice
+        fails(lambda: p.a.gpu.state_patch([j1, 10 ** 13], allowed=[0, 0]))               # unknown job id
+        fails(lambda: p.a.gpu.state_patch([j1, gone], allowed=[0, 0]))                    # not live
+        fails(lambda: p.a.gpu.state_patch([j1, j1], allowed=[0, 0]))                      # job id twice
         fails(lambda: raw_patch(2, [j1, j2], [3, -2]))                                 # reserved_host below -1
-        fails(lambda: p.a.state_patch([j1, j2], reserved_host=[3, -2], clear_reservations=True))
+        fails(lambda: p.a.gpu.state_patch([j1, j2], reserved_host=[3, -2], clear_reservations=True))
     finally:
         p.close()

@@ -7,162 +7,21 @@ stream of deltas, whatever the slot layout.  Plus: the state is left as it was, 
 errors.  Host codes are a permuted, non-contiguous set, so a host's index differs from its code.
 """
 import ctypes as C
-import os
 
 import numpy as np
 import pytest
 
-from cook_b200 import abi, engine, traces
+from cook_b200 import abi, traces
 from cook_b200.engine import CookError, GpuEngine
-from test_state_resident import DEFAULTS, _lists, jobs_soa, pool_rows, tasks_soa
-
-RUN_KEYS = ("user", "priority", "start_time", "task_id", "job_id", "cpus", "mem", "gpus")
-
-
-def test_state_rebalance_symbol_exported():
-    if not os.path.exists(engine.LIB_PATH):
-        pytest.skip("libcookgpu.so not built")
-    assert hasattr(engine.load_library(), "cook_state_rebalance")
-
-
-def remap_hosts(r, seed):
-    """The gen_rebalance dict `r` with hostname codes 3 * perm + 7: the host table, novel-host lists and
-    cotask hosts carry codes; running tasks keep their table index.  Returns the code of each index."""
-    H = r["hosts"].n
-    codes = (3 * np.random.default_rng(seed).permutation(H) + 7).astype(np.int32)
-    h = r["hosts"]
-    kw = {n: h.col(n) for n, _ in h._fields_ if h.col(n) is not None}
-    kw.update(n=H, n_attr_cols=h.n_attr_cols, hostname_id=codes)
-    r["hosts"] = abi.HostTable(**kw)
-    j = r["pending"]
-    if j.col("novel_off") is not None and j.col("novel_off")[-1] > 0:
-        kw = {n: j.col(n) for n, _ in j._fields_ if j.col(n) is not None}
-        kw.update(n=j.n, novel_host=codes[j.col("novel_host")])
-        r["pending"] = abi.JobsSoA(**kw)
-    g = r["groups"]
-    if g is not None:
-        kw = {n: g.col(n) for n, _ in g._fields_ if g.col(n) is not None}
-        kw.update(n_groups=g.n_groups, cot_hostname_id=codes[g.col("cot_hostname_id")] if g.col("cot_off")[-1] else
-                  g.col("cot_hostname_id"))
-        r["groups"] = abi.Groups(**kw)
-    return codes
-
-
-def rows_of(r, codes):
-    """The pool's pending jobs {job_id: row} and running tasks {task_id: row (with its hostname code)}."""
-    j = r["pending"]
-    nov, att, grp = _lists(j, "novel_off", "novel_host"), _lists(j, "attr_off", "attr_col", "attr_val"), \
-        _lists(j, "group_off", "group_idx")
-    pend = {}
-    for i in range(j.n):
-        row = dict(DEFAULTS, user=int(j.col("user")[i]), priority=int(r["pending_priority"][i]),
-                   cpus=float(j.col("cpus")[i]), mem=float(j.col("mem")[i]))
-        if j.col("ckpt_location") is not None:
-            row["ckpt_location"] = int(j.col("ckpt_location")[i])
-        row["novel"], row["attr"], row["groups"] = nov[i], att[i], grp[i]
-        pend[int(r["pending_job_id"][i])] = row
-    t = r["running"].col("t")
-    host = r["running"].col("host")
-    run = {}
-    for i in range(t.n):
-        row = {k: t.col(k)[i].item() for k in RUN_KEYS}
-        row["host"] = int(codes[host[i]])
-        run[row["task_id"]] = row
-    return pend, run
-
-
-def rdelta(reset=False, up=(), rm=(), run_up=(), run_rm=(), with_hosts=True):
-    up, run_up = list(up), list(run_up)
-    pend, prio, jid = jobs_soa(up) if up else (None, None, None)
-    hn = np.array([r["host"] for r in run_up], np.int32) if run_up and with_hosts else None
-    return abi.make_delta(reset=reset, pending=pend, pending_priority=prio, pending_job_id=jid, pending_rm=list(rm),
-                          running=tasks_soa(run_up) if run_up else None, running_rm=list(run_rm),
-                          running_hostname_id=hn)
-
-
-def decisions_eq(got, want):
-    keys = ("job_id", "pending_idx", "host", "victims", "dru", "mem", "cpus", "gpus")
-    assert [tuple(d[k] for k in keys) for d in got] == [tuple(d[k] for k in keys) for d in want]
-
-
-class RPool:
-    """A rebalance pool: the handle under test, a host-table handle, and the model."""
-
-    def __init__(self, r, codes, dru_mode=0):
-        self.r, self.codes = r, codes
-        self.idx = {int(c): i for i, c in enumerate(codes)}
-        self.users, self.hosts, self.groups, self.params = r["users"], r["hosts"], r["groups"], r["params"]
-        self.gpu, self.ref = GpuEngine(pool_name="state", dru_mode=dru_mode), GpuEngine(pool_name="host")
-        self.pend, self.run = {}, {}
-        self.queue, self.gone = [], set()
-
-    def close(self):
-        self.gpu.close()
-        self.ref.close()
-
-    def apply(self, up=(), rm=(), run_up=(), run_rm=(), reset=False):
-        up, run_up = list(up), list(run_up)
-        self.gpu.state_apply(rdelta(reset, up, rm, run_up, run_rm))
-        if reset:
-            self.pend, self.run = {}, {}
-            self.gone |= set(self.queue)
-        for j in rm:
-            del self.pend[j]
-        for t in run_rm:
-            del self.run[t]
-        for j, row in up:
-            self.pend[j] = row
-        for row in run_up:
-            self.run[row["task_id"]] = row
-        self.gone |= set(rm) | {j for j, _ in up}
-
-    def rank(self):
-        self.queue, self.gone = self.gpu.state_rank(self.users).tolist(), set()
-        return self.queue
-
-    def taken(self):
-        return [j for j in self.queue if j not in self.gone and self.pend[j]["allowed"]][:self.params.max_preemption]
-
-    def tables(self):
-        """cook_rebalance's host tables of the same rows, and the task id of each running index."""
-        rows = [self.run[t] for t in sorted(self.run)]
-        running = abi.RunningSoA(t=tasks_soa(rows), host=np.array([self.idx[r["host"]] for r in rows], np.int32))
-        take = self.taken()
-        jobs, prio, jid = jobs_soa([(j, self.pend[j]) for j in take])
-        return running, jobs, jid, prio, np.array([r["task_id"] for r in rows], np.int64)
-
-    def want(self, engine_):
-        running, jobs, jid, prio, tids = self.tables()
-        if jobs.n == 0:
-            return []
-        out = engine_.rebalance(running, jobs, jid, prio, self.hosts, self.users, self.params, groups=self.groups)
-        R = len(tids)
-        for d in out:
-            d["job_id"] = int(jid[d["pending_idx"]])
-            d["victims"] = [int(tids[v]) if v < R else -1 - (v - R) for v in d["victims"]]
-        return out
-
-    def check(self, oracle=None):
-        got = self.gpu.state_rebalance(self.hosts, self.users, self.params, groups=self.groups)
-        decisions_eq(got, self.want(self.ref))
-        if oracle is not None:
-            decisions_eq(got, self.want(oracle))
-        return got
-
-
-def _pool(seed, constraints, n_running=3000, n_pending=300, n_hosts=200, n_users=40, mp=24):
-    r = traces.gen_rebalance(seed, n_running, n_pending, n_hosts, n_users, max_preemption=mp,
-                             constraints=constraints)
-    codes = remap_hosts(r, seed + 1)
-    return r, codes
+from resident_model import Pool, decisions_eq, delta, nb, pool_rows, rebalance_trace, remap_hosts, rows_of
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("constraints", [False, True])
 def test_equivalence_over_deltas(constraints, oracle):
-    r, codes = _pool(71 if constraints else 73, constraints)
+    r, codes = rebalance_trace(71 if constraints else 73, constraints)
     pend, run = rows_of(r, codes)
-    p = RPool(r, codes)
+    p = Pool.of_rebalance(r, codes)
     rng = np.random.default_rng(9)
     try:
         items = sorted(pend.items())
@@ -181,7 +40,7 @@ def test_equivalence_over_deltas(constraints, oracle):
             ups = [(flip, dict(p.pend[flip], allowed=1 - p.pend[flip]["allowed"])),
                    (prio, dict(p.pend[prio], priority=int(rng.choice([10, 50, 90]))))]
             p.apply(up=ups, rm=kill)
-            got = p.check(oracle if cycle % 2 == 0 else None)
+            got = p.check_rebalance(oracle if cycle % 2 == 0 else None)
             many_victims = max([many_victims] + [len(d["victims"]) for d in got])
             removed_ahead += len(got) > 0
             # churn: the victims die, some tasks finish, some jobs start on random hosts, new jobs arrive,
@@ -210,7 +69,7 @@ def test_equivalence_over_deltas(constraints, oracle):
 
 @pytest.mark.gpu
 def test_layout_independence():
-    r, codes = _pool(81, True)
+    r, codes = rebalance_trace(81, True)
     pend, run = rows_of(r, codes)
     for k, t in enumerate(sorted(run)):              # off the binary grid: the serial folds run
         if k % 3 == 0:
@@ -219,7 +78,7 @@ def test_layout_independence():
         if k % 4 == 0:
             pend[j]["cpus"] += 0.1
     items = sorted(pend.items())
-    a, b = RPool(r, codes), RPool(r, codes)
+    a, b = Pool.of_rebalance(r, codes), Pool.of_rebalance(r, codes)
     rng = np.random.default_rng(4)
     try:
         a.apply(up=items, run_up=[run[t] for t in sorted(run)])
@@ -231,8 +90,8 @@ def test_layout_independence():
         rr = list(run.values())
         b.apply(up=[items[i] for i in perm[: len(perm) // 2]], run_up=[rr[i] for i in rng.permutation(len(rr))])
         b.apply(up=[items[i] for i in perm[len(perm) // 2:]])
-        assert a.rank() == b.rank()
-        ga, gb = a.check(), b.check()
+        assert a.rank().tolist() == b.rank().tolist()
+        ga, gb = a.check_rebalance(), b.check_rebalance()
         assert len(ga) > 0
         decisions_eq(ga, gb)
     finally:
@@ -246,11 +105,11 @@ def test_stated_size_c4_pool3():
     assert (r["running"].col("t").n, r["params"].max_preemption) == (40_000, 128)
     codes = remap_hosts(r, 5)
     pend, run = rows_of(r, codes)
-    p = RPool(r, codes)
+    p = Pool.of_rebalance(r, codes)
     try:
         p.apply(up=sorted(pend.items()), run_up=list(run.values()))
         p.rank()
-        got = p.check()
+        got = p.check_rebalance()
         assert len(got) > 0
     finally:
         p.close()
@@ -279,7 +138,7 @@ def test_state_untouched():
     mp = int(t["jobs"].col("ports").max()) if t["jobs"].col("ports") is not None else 0
     a, b = GpuEngine(pool_name="a"), GpuEngine(pool_name="b")
     try:
-        d = rdelta(up=sorted(pend.items()), run_up=list(run.values()))
+        d = delta(up=sorted(pend.items()), run_up=list(run.values()), hosts=True)
         for e in (a, b):
             e.state_apply(d)
         qa, qb = a.state_rank(t["users"]), b.state_rank(t["users"])
@@ -295,22 +154,18 @@ def test_state_untouched():
         b.close()
 
 
-def _nb(*arrays):
-    return sum(a.nbytes for a in arrays if isinstance(a, np.ndarray))
-
-
 @pytest.mark.gpu
 def test_accounting():
-    r, codes = _pool(101, True, n_running=2000, n_pending=200, n_hosts=150, n_users=30, mp=16)
+    r, codes = rebalance_trace(101, True, n_running=2000, n_pending=200, n_hosts=150, n_users=30, mp=16)
     pend, run = rows_of(r, codes)
     h, u, g = r["hosts"], r["users"], r["groups"]
-    want = _nb(*[h.col(n) for n, _ in h._fields_])
-    want += _nb(*[u.col(n) for n in ("name_rank", "div_mem", "div_cpus", "quota_count", "quota_cpus", "quota_mem",
+    want = nb(*[h.col(n) for n, _ in h._fields_])
+    want += nb(*[u.col(n) for n in ("name_rank", "div_mem", "div_cpus", "quota_count", "quota_cpus", "quota_mem",
                                       "quota_gpus")])
-    want += _nb(*[g.col(n) for n, _ in g._fields_])
+    want += nb(*[g.col(n) for n, _ in g._fields_])
     got = []
     for scale in (1, 2):                             # the same rows, and as many again under new ids
-        p = RPool(r, codes)
+        p = Pool.of_rebalance(r, codes)
         try:
             up = sorted(pend.items())
             rr = list(run.values())
@@ -319,7 +174,7 @@ def test_accounting():
                 rr += [dict(row, task_id=row["task_id"] + 10 ** 10) for row in rr]
             p.apply(up=up, run_up=rr)
             p.rank()
-            p.check()
+            p.check_rebalance()
             st = p.gpu.last_stats(abi.PHASE_REBALANCE)
             assert st["n_launches"] > 0
             got.append(st["h2d_bytes"])
@@ -330,10 +185,10 @@ def test_accounting():
 
 @pytest.mark.gpu
 def test_errors():
-    r, codes = _pool(111, True, mp=16)
+    r, codes = rebalance_trace(111, True, mp=16)
     pend, run = rows_of(r, codes)
     items = sorted(pend.items())
-    p = RPool(r, codes)
+    p = Pool.of_rebalance(r, codes)
     try:
         p.apply(up=items, run_up=list(run.values()))
 
@@ -342,9 +197,9 @@ def test_errors():
                 fn()
             return e.value.code
 
-        reb = lambda hosts=p.hosts, groups=p.groups: p.gpu.state_rebalance(hosts, p.users, p.params, groups=groups)
+        reb = lambda hosts=p.hosts, groups=p.groups: p.gpu.state_rebalance(hosts, p.users, p.rparams, groups=groups)
         assert code_of(reb) == abi.COOK_E_BADARG                 # no rank yet
-        q0 = p.rank()
+        q0 = p.rank().tolist()
         r0 = reb()
         assert len(r0) > 0
 
@@ -353,16 +208,16 @@ def test_errors():
             if undo:
                 undo()
             assert reb() == r0
-            assert p.rank() == q0
+            assert p.rank().tolist() == q0
             assert reb() == r0
 
-        R, MP = len(p.run), p.params.max_preemption
+        R, MP = len(p.run), p.rparams.max_preemption
 
         def raw(cap, dec=True):
             out = (abi.Decision * MP)()
             jid, vict, n = np.zeros(MP, np.int64), np.zeros(max(cap, 1), np.int64), C.c_int32(0)
             rc = p.gpu.lib.cook_state_rebalance(p.gpu.pool, C.byref(p.hosts), C.byref(p.groups), C.byref(p.users),
-                                                C.byref(p.params), out if dec else None, abi.ptr(jid, abi.P_I64),
+                                                C.byref(p.rparams), out if dec else None, abi.ptr(jid, abi.P_I64),
                                                 abi.ptr(vict, abi.P_I64), int(cap), C.byref(n))
             if rc != 0:
                 p.gpu._err(rc)
@@ -371,10 +226,10 @@ def test_errors():
         fails(lambda: raw(R + MP - 1))                             # victim_cap below the bound
         raw(R + MP)
         task = dict(next(iter(p.run.values())), task_id=10 ** 13)
-        p.gpu.state_apply(rdelta(run_up=[task], with_hosts=False))  # host unknown (-1)
-        fails(reb, undo=lambda: p.gpu.state_apply(rdelta(run_rm=[10 ** 13])))
-        p.gpu.state_apply(rdelta(run_up=[dict(task, host=int(codes.max()) + 1)]))   # a code not in the table
-        fails(reb, undo=lambda: p.gpu.state_apply(rdelta(run_rm=[10 ** 13])))
+        p.gpu.state_apply(delta(run_up=[task]))  # host unknown (-1)
+        fails(reb, undo=lambda: p.gpu.state_apply(delta(run_rm=[10 ** 13])))
+        p.gpu.state_apply(delta(run_up=[dict(task, host=int(codes.max()) + 1)], hosts=True))   # a code not in the table
+        fails(reb, undo=lambda: p.gpu.state_apply(delta(run_rm=[10 ** 13])))
         hn = p.hosts.col("hostname_id").copy()
         hn[1] = hn[0]
         kw = {n: p.hosts.col(n) for n, _ in p.hosts._fields_ if p.hosts.col(n) is not None}
@@ -384,12 +239,12 @@ def test_errors():
                     dict(items[0][1], groups=[p.groups.n_groups]),
                     dict(items[0][1], attr=[(p.hosts.n_attr_cols, 1)])]
         for row in bad_rows:
-            p.gpu.state_apply(rdelta(up=[(10 ** 13, row)]))
-            fails(reb, undo=lambda: p.gpu.state_apply(rdelta(rm=[10 ** 13])))
+            p.gpu.state_apply(delta(up=[(10 ** 13, row)]))
+            fails(reb, undo=lambda: p.gpu.state_apply(delta(rm=[10 ** 13])))
         g = GpuEngine(pool_name="gpu-dru", dru_mode=1)              # GPU DRU mode
         try:
             with pytest.raises(CookError) as e:
-                g.state_rebalance(p.hosts, p.users, p.params)
+                g.state_rebalance(p.hosts, p.users, p.rparams)
             assert e.value.code == abi.COOK_E_UNSUPPORTED_CONSTRAINT
         finally:
             g.close()

@@ -8,49 +8,13 @@ hosts, finishes, a reset, capacity doubling, arena compaction) on and off the gr
 both paths; independence from the slot layout; the host edges; a resident match fed from the derived columns
 against cook_match and the oracle on host tables; the errors and the upload accounting.
 """
-import os
-
 import numpy as np
 import pytest
 
 import fold_ref as F
 from cook_b200 import abi, engine
+from resident_model import START, Pool, amounts, drop_all_but, keyed, pending_rows, random_rows, tasks_soa
 from usage_ref import KEYS, aggregate_quota_groups, running_usage
-
-BIG = 2.0 ** 35   # mixed: on the grid, but a user of 256 rows or more passes 2^43
-
-
-# ---- tables --------------------------------------------------------------------------------------------
-def amounts(rng, regime, n, big=None):
-    """cpus, mem, gpus of n rows.  grid: halves and 512 MiB steps; off: tenths and sevenths; mixed: grid, the
-    rows of `big` carry mem just under 2^35 with 2^-10 parts."""
-    if regime == "off":
-        cpus = rng.choice(np.array([0.1, 0.3, 0.7, 1.1]), n)
-        mem = rng.integers(1, 40000, n) / 7.0
-        gpus = rng.choice(np.array([0.0, 0.0, 0.1, 1.0]), n)
-    else:
-        cpus = rng.choice(np.array([0.5, 1.0, 2.0, 4.0]), n)
-        mem = 512.0 * rng.integers(1, 65, n)
-        gpus = rng.choice(np.array([0.0, 0.0, 1.0, 2.0]), n)
-        if regime == "mixed" and big is not None and big.any():
-            mem[big] = BIG - F.GRID * rng.integers(1, 2 ** 20, int(big.sum()))
-    return cpus.astype(np.float64), mem.astype(np.float64), gpus.astype(np.float64)
-
-
-def zipf_users(rng, n, U):
-    """A third of the rows belong to user 0, the rest spread over the others."""
-    u = rng.integers(1, U, n).astype(np.int32)
-    u[rng.random(n) < 1.0 / 3.0] = 0
-    return u
-
-
-def random_rows(rng, regime, n, U, tid0, hosts):
-    user = zipf_users(rng, n, U)
-    cpus, mem, gpus = amounts(rng, regime, n, user == 0)
-    tid = tid0 + 2 * rng.permutation(n).astype(np.int64)
-    return [dict(user=int(user[i]), task_id=int(tid[i]), cpus=float(cpus[i]), mem=float(mem[i]), gpus=float(gpus[i]),
-                 host=int(rng.choice(hosts))) for i in range(n)]
-
 
 def plain_fold(rows, key, order):
     """The sum of `key` over rows in `order` (a list of rows), one float addition each."""
@@ -117,91 +81,24 @@ def test_aggregate_quota_groups_known_answer():
     assert got["s"].tolist() == [300.0, 30.0, 3.0, 0.0]
 
 
-def test_usage_exported_and_phase():
-    assert abi.PHASE_USAGE == 5
-    hdr = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "include", "cook_gpu.h")).read()
-    assert "int32_t cook_state_usage(cook_pool* pool" in hdr and "COOK_PHASE_USAGE = 5" in hdr
-    if not os.path.exists(engine.LIB_PATH):
-        pytest.skip("libcookgpu.so not built")
-    assert hasattr(engine.load_library(), "cook_state_usage")
-
-
 # ---- GPU -------------------------------------------------------------------------------------------------
-def run_delta(rows, hosts=True):
-    n = len(rows)
-    t = abi.make_tasks(user=np.array([r["user"] for r in rows], np.int32), priority=np.full(n, 50, np.int32),
-                       start_time=np.full(n, 1_700_000_000_000, np.int64),
-                       task_id=np.array([r["task_id"] for r in rows], np.int64),
-                       job_id=np.array([r.get("job_id", r["task_id"] + 1) for r in rows], np.int64),
-                       cpus=np.array([r["cpus"] for r in rows]), mem=np.array([r["mem"] for r in rows]),
-                       gpus=np.array([r["gpus"] for r in rows]))
-    return t, (np.array([r["host"] for r in rows], np.int32) if hosts else None)
+def new_handle(name="usage"):
+    """A resident handle whose pending upserts carry user, amounts and novel hosts only, and its model."""
+    return Pool(name, drop=drop_all_but("gpus", "novel"), send_hosts=True)
 
 
-class Handle:
-    """A resident handle and the running rows it should hold."""
-
-    def __init__(self, name="usage"):
-        self.e = engine.GpuEngine(pool_name=name)
-        self.run, self.pend = {}, {}
-
-    def close(self):
-        self.e.close()
-
-    def apply(self, up=(), rm=(), hosts=True, reset=False, pend_up=(), pend_rm=()):
-        up = list(up)
-        if not hosts:
-            up = [dict(r, host=-1) for r in up]
-        t, hn = run_delta(up, hosts) if up else (None, None)
-        kw = {}
-        if pend_up:
-            n = len(pend_up)
-            off, nov = abi.csr([p["novel"] for p in pend_up])
-            kw = dict(pending=abi.JobsSoA(n=n, user=np.array([p["user"] for p in pend_up], np.int32),
-                                          cpus=np.array([p["cpus"] for p in pend_up]),
-                                          mem=np.array([p["mem"] for p in pend_up]),
-                                          gpus=np.array([p["gpus"] for p in pend_up]), novel_off=off, novel_host=nov),
-                      pending_priority=np.full(n, 50, np.int32),
-                      pending_job_id=np.array([p["job_id"] for p in pend_up], np.int64))
-        self.e.state_apply(abi.make_delta(reset=reset, running=t, running_rm=list(rm), running_hostname_id=hn,
-                                          pending_rm=list(pend_rm), **kw))
-        if reset:
-            self.run, self.pend = {}, {}
-        for tid in rm:
-            del self.run[tid]
-        for j in pend_rm:
-            del self.pend[j]
-        for r in up:
-            self.run[r["task_id"]] = r
-        for p in pend_up:
-            self.pend[p["job_id"]] = p
-
-    def launch(self, job_ids, task_ids, hosts=None):
-        self.e.state_launch(job_ids, task_ids, np.full(len(job_ids), 1_700_000_000_000, np.int64), hosts)
-        for i, (j, t) in enumerate(zip(job_ids, task_ids)):
-            p = self.pend.pop(int(j))
-            self.run[int(t)] = dict(user=p["user"], task_id=int(t), job_id=int(j), cpus=p["cpus"], mem=p["mem"], gpus=p["gpus"],
-                                    host=int(hosts[i]) if hosts is not None else -1)
-
-    def check(self, U, listed):
-        got = self.e.state_usage(U, listed)
-        want = running_usage(self.run.values(), U, listed)
-        for k in KEYS:
-            assert F.same_bits(got["user"][k], want["user"][k]), k
-        assert F.same_bits(got["pool"], want["pool"])
-        assert F.same_bits(got["run_cpus"], want["run_cpus"]) and F.same_bits(got["run_mem"], want["run_mem"])
-        assert np.array_equal(got["run_count"], want["run_count"])
-        st = self.e.last_stats(abi.PHASE_USAGE)
-        assert st["h2d_bytes"] == (4 * len(listed) if self.run else 0)
-        assert st["d2h_bytes"] == (32 * U + 32 + 20 * len(listed) if self.run else 0)
-        return got
-
-
-def pending_rows(rng, regime, n, U, jid0, codes):
-    user = zipf_users(rng, n, U)
-    cpus, mem, gpus = amounts(rng, regime, n, user == 0)
-    return [dict(job_id=jid0 + 2 * i, user=int(user[i]), cpus=float(cpus[i]), mem=float(mem[i]), gpus=float(gpus[i]),
-                 novel=[int(x) for x in rng.choice(codes, int(rng.integers(1, 4)), replace=False)]) for i in range(n)]
+def check(h, U, listed):
+    got = h.gpu.state_usage(U, listed)
+    want = running_usage(h.run.values(), U, listed)
+    for k in KEYS:
+        assert F.same_bits(got["user"][k], want["user"][k]), k
+    assert F.same_bits(got["pool"], want["pool"])
+    assert F.same_bits(got["run_cpus"], want["run_cpus"]) and F.same_bits(got["run_mem"], want["run_mem"])
+    assert np.array_equal(got["run_count"], want["run_count"])
+    st = h.gpu.last_stats(abi.PHASE_USAGE)
+    assert st["h2d_bytes"] == (4 * len(listed) if h.run else 0)
+    assert st["d2h_bytes"] == (32 * U + 32 + 20 * len(listed) if h.run else 0)
+    return got
 
 
 @pytest.mark.gpu
@@ -211,7 +108,7 @@ def test_churn_matches_the_fold(regime):
     U, codes = 40, list(range(60))
     listed = np.array(rng.permutation(list(range(50)) + [200, 201, 202]), np.int32)   # 50..59 unlisted, 200.. empty
     hosts = codes + [7] * 30 + [-1] * 5   # host 7 carries more than 64 rows
-    h = Handle()
+    h = new_handle()
     tid, jid = [1_000], [5_000_000]
 
     def fresh_rows(n):
@@ -222,32 +119,32 @@ def test_churn_matches_the_fold(regime):
     def fresh_jobs(n):
         rows = pending_rows(rng, regime, n, U, jid[0], codes)
         jid[0] += 2 * n + 2
-        return rows
+        return keyed(rows)
 
     try:
-        h.check(U, listed)                                        # an empty handle: zeros
-        h.apply(up=fresh_rows(700), pend_up=fresh_jobs(600))
-        h.check(U, listed)
+        check(h, U, listed)                                        # an empty handle: zeros
+        h.apply(run_up=fresh_rows(700), up=fresh_jobs(600))
+        check(h, U, listed)
         for b in range(6):
             fin = [t for t in h.run if rng.random() < 0.05]
-            h.apply(up=fresh_rows(250), rm=fin, hosts=b % 2 == 0, pend_up=fresh_jobs(150))   # past 1024, then 2048
-            h.check(U, listed)
+            h.apply(run_up=fresh_rows(250), up=fresh_jobs(150), run_rm=fin, hosts=b % 2 == 0)   # past 1024, then 2048
+            check(h, U, listed)
             launch = list(rng.choice(sorted(h.pend), 120, replace=False))
             tids = [tid[0] + 2 * i for i in range(len(launch))]
             tid[0] += 2 * len(launch) + 2
             hn = np.array(rng.choice(hosts, len(launch)), np.int32) if b % 2 else None
-            h.launch(launch, tids, hn)                            # lists leave with the rows: arena compaction
-            h.check(U, listed)
-        h.apply(reset=True, up=fresh_rows(900), pend_up=fresh_jobs(50))
-        got = h.check(U, listed)
+            h.launch(launch, tids, np.full(len(launch), START, np.int64), hn)                           # lists leave with the rows: arena compaction
+            check(h, U, listed)
+        h.apply(reset=True, run_up=fresh_rows(900), up=fresh_jobs(50))
+        got = check(h, U, listed)
         if regime == "mixed":   # both paths in one call: user 0 passes 2^43, the others stay exact
             assert got["user"]["mem"][0] > 2.0 ** 43 and got["user"]["mem"][1:].max() < 2.0 ** 30
             mine = [r["mem"] for r in sorted(h.run.values(), key=lambda r: r["task_id"]) if r["user"] == 0]
             assert F.association_sensitive(mine)
-        h.apply(rm=list(h.run)[:300])
-        h.check(U, listed)
-        h.apply(rm=list(h.run))
-        h.check(U, listed)                                        # no live row: zeros again
+        h.apply(run_rm=list(h.run)[:300])
+        check(h, U, listed)
+        h.apply(run_rm=list(h.run))
+        check(h, U, listed)                                        # no live row: zeros again
     finally:
         h.close()
 
@@ -261,15 +158,15 @@ def test_layout_independence(regime):
     U, hosts = 30, list(range(40)) + [-1]
     rows = random_rows(rng, regime, 1500, U, 10, hosts)
     listed = np.array(rng.permutation(40), np.int32)
-    a, b = Handle("a"), Handle("b")
+    a, b = new_handle("a"), new_handle("b")
     try:
-        a.apply(up=sorted(rows, key=lambda r: r["task_id"]))
+        a.apply(run_up=sorted(rows, key=lambda r: r["task_id"]))
         junk = random_rows(rng, regime, 800, U, 10_000_000, hosts)
-        b.apply(up=junk)
+        b.apply(run_up=junk)
         perm = [rows[i] for i in rng.permutation(len(rows))]
-        b.apply(up=perm[:600], rm=[r["task_id"] for r in junk[:500]])
-        b.apply(up=perm[600:], rm=[r["task_id"] for r in junk[500:]])
-        ga, gb = a.check(U, listed), b.check(U, listed)
+        b.apply(run_up=perm[:600], run_rm=[r["task_id"] for r in junk[:500]])
+        b.apply(run_up=perm[600:], run_rm=[r["task_id"] for r in junk[500:]])
+        ga, gb = check(a, U, listed), check(b, U, listed)
         for k in KEYS:
             assert F.same_bits(ga["user"][k], gb["user"][k])
         for k in ("pool", "run_cpus", "run_mem"):
@@ -288,21 +185,21 @@ def test_layout_independence(regime):
 def test_host_edges():
     rng = np.random.default_rng(31)
     U = 5
-    h = Handle()
+    h = new_handle()
     try:
-        assert np.all(h.check(U, np.array([3, 9], np.int32))["run_count"] == 0)
+        assert np.all(check(h, U, np.array([3, 9], np.int32))["run_count"] == 0)
         # host 3: 3000 rows (past two sort tiles); host 4: 65; rows with -1 and with codes 8, 1000 not listed
         hosts = [3] * 3000 + [4] * 65 + [-1] * 40 + [8] * 30 + [1000] * 10 + [5]
         rows = random_rows(rng, "off", len(hosts), U, 100, [0])
         for r, c in zip(rows, hosts):
             r["host"] = c
-        h.apply(up=rows)
-        got = h.check(U, np.array([4, 3, 77, 5, 2], np.int32))   # 77 and 2: listed, no rows
+        h.apply(run_up=rows)
+        got = check(h, U, np.array([4, 3, 77, 5, 2], np.int32))   # 77 and 2: listed, no rows
         assert got["run_count"].tolist() == [65, 3000, 0, 1, 0]
         assert got["run_cpus"][2] == 0.0 and got["run_mem"][4] == 0.0
         assert got["pool"][0] == float(len(rows))
-        h.check(U, np.zeros(0, np.int32))                         # no host list
-        h.check(U, np.array([1000], np.int32))
+        check(h, U, np.zeros(0, np.int32))                         # no host list
+        check(h, U, np.array([1000], np.int32))
     finally:
         h.close()
 
@@ -310,12 +207,12 @@ def test_host_edges():
 @pytest.mark.gpu
 def test_errors_leave_the_handle_unchanged():
     rng = np.random.default_rng(41)
-    h = Handle()
+    h = new_handle()
     try:
-        h.apply(up=random_rows(rng, "off", 300, 6, 100, list(range(10))))
+        h.apply(run_up=random_rows(rng, "off", 300, 6, 100, list(range(10))))
         listed = np.arange(10, dtype=np.int32)
-        before = h.check(6, listed)
-        lib, pool = h.e.lib, h.e.pool
+        before = check(h, 6, listed)
+        lib, pool = h.gpu.lib, h.gpu.pool
         out = np.zeros(64)
         codes = np.array([1, 2, 1], np.int32)
         neg = np.array([1, -2], np.int32)
@@ -332,7 +229,7 @@ def test_errors_leave_the_handle_unchanged():
             assert rc == abi.COOK_E_BADARG
         assert lib.cook_state_usage(pool, 0, None, abi.ptr(out, P), 0, None, None, None, None) == abi.COOK_OK
         assert F.same_bits(out[:4], before["pool"])               # n_users is not read without out_user_usage
-        after = h.check(6, listed)
+        after = check(h, 6, listed)
         for k in KEYS:
             assert F.same_bits(after["user"][k], before["user"][k])
         assert F.same_bits(after["run_mem"], before["run_mem"])
@@ -349,7 +246,7 @@ def test_resident_match_fed_from_state_usage(oracle):
     rng = np.random.default_rng(51)
     U, O, J = 10, 40, 500
     codes = (100 + np.arange(O)).astype(np.int32)
-    h, ref = Handle("resident"), engine.GpuEngine(pool_name="host")
+    h, ref = new_handle("resident"), engine.GpuEngine(pool_name="host")
     pend = pending_rows(rng, "grid", J, U, 1_000_000, codes.tolist())
     for p in pend:
         p["gpus"] = 0.0
@@ -357,7 +254,7 @@ def test_resident_match_fed_from_state_usage(oracle):
     run = random_rows(rng, "grid", 300, U, 10, codes.tolist() + [-1])
     for r in run:
         r["gpus"] = 0.0
-    h.apply(up=run, pend_up=pend)
+    h.apply(up=keyed(pend), run_up=run)
     cnt0 = np.bincount([r["user"] for r in run], minlength=U).astype(float)
     quota = {"count": cnt0 + 30.0, "cpus": np.full(U, 1e9), "mem": np.full(U, 1e12), "gpus": np.full(U, 1e9)}
     lease_c, lease_m = np.full(O, 12.0), np.full(O, 32768.0)
@@ -377,12 +274,12 @@ def test_resident_match_fed_from_state_usage(oracle):
     next_tid = 10_000_000
     try:
         for cycle in range(4):
-            got = h.e.state_usage(U, codes)
+            got = h.gpu.state_usage(U, codes)
             want = running_usage(h.run.values(), U, codes)
             users, offers = tables(got)
             users_h, offers_h = tables(want)
-            q = h.e.state_rank(users)
-            m = h.e.state_match(offers, users, params)
+            q = h.gpu.state_rank(users)
+            m = h.gpu.state_match(offers, users, params)
             # host arm: the same rows as host tables, sorted by id
             jids = np.array(sorted(h.pend), np.int64)
             pr = [h.pend[j] for j in jids]
@@ -393,7 +290,7 @@ def test_resident_match_fed_from_state_usage(oracle):
                                 start_time=np.full(len(pr), abi.INT64_MAX), task_id=np.full(len(pr), -1, np.int64),
                                 job_id=jids, cpus=jobs.col("cpus"), mem=jobs.col("mem"))
             rr = sorted(h.run.values(), key=lambda r: r["task_id"])
-            rt = run_delta(rr)[0]
+            rt = tasks_soa(rr)
             hr = ref.rank(rt, pt, users_h)
             assert np.array_equal(q, jids[hr["ranked"]])
             hm = ref.match(hr["ranked"], jobs, offers_h, users_h, params)
@@ -414,7 +311,7 @@ def test_resident_match_fed_from_state_usage(oracle):
             assert len(jl) > 0
             tids = next_tid + 2 * np.arange(len(jl), dtype=np.int64)
             next_tid += 2 * len(jl) + 2
-            h.launch(jl.tolist(), tids.tolist(), codes[m["assign"][placed]])
+            h.launch(jl.tolist(), tids.tolist(), np.full(len(jl), START, np.int64), codes[m["assign"][placed]])
         assert differs
     finally:
         h.close()
