@@ -8,6 +8,7 @@
 ;;   :2262-2284 rank-jobs, resident pool     -> (rank-resident! ...)                [cook_state_rank_offensive]
 ;;   :1749-1800 Kubernetes-scheduler pool    -> (kubernetes-considerable! ...)      [cook_state_considerable]
 ;;   :1283-1335 autoscaling helper           -> (autoscalable-jobs! ...)            [cook_state_considerable]
+;;   monitor.clj:177-207 set-stats-counters! -> (monitor-resident! ...)             [cook_state_user_stats]
 ;; selected per pool with {:scheduler-config {:scheduler "gpu"}} next to "fenzo" / "kubernetes"
 ;; (config.clj:110-122, make-pool-handler :2425-2466).  Everything numeric happens in libcookgpu;
 ;; this namespace marshals columns and keeps the state Fenzo kept (cook_b200/cycle.py is the same
@@ -209,6 +210,43 @@
                         (concat args [(int-array [n (if enforce-rate-limit? 1 0) 1 2 0]) out out-n]))
           "cook_state_considerable")
   (let [lb (.asLongBuffer out)] (mapv #(.get lb (int %)) (range (aget out-n 0)))))
+
+;; cook_state_user_stats' states (COOK_STATS_*) and user counts (COOK_USERS_*), by index
+(def ^:private stat-states ["running" "waiting" "starved" "waiting-under-quota"])
+(def ^:private user-counts ["total" "starved" "waiting-under-quota" "hungry" "satisfied"])
+
+(defn monitor-resident!
+  "set-stats-counters! (monitor.clj:177-207) for one pool or quota-group name from its resident handles (the pool's
+   own, or every pool the quota grouping maps to the name; one device): cook_state_user_stats, then the per-user and
+   \"all\" counters through `set-user-counter!` (fn [state user type amount]) and the user counts through
+   `set-total-counter!` (fn [state n]), the monitor's own setters, which clear stale users and feed Prometheus.
+   `args` are Native/stateUserStats' n_users, users and quota_rest_ok; `names` maps user codes to names; `quota-extra`
+   (fn [code]) gives a waiting-under-quota user's other quota keys ({\"gpus\" x \"launch-rate-saved\" y ...}), which
+   the reference's merges pass through.  Out buffers are direct, n_users = (count names)."
+  [handles args names quota-extra set-user-counter! set-total-counter!]
+  (let [u (count names)
+        jobs (direct (* 32 u)) cpus (direct (* 32 u)) mem (direct (* 32 u)) member (direct u)
+        all-jobs (direct 32) all-cpus (direct 32) all-mem (direct 32) counts (direct 40)]
+    (check! (first handles)
+            (apply #(Native/stateUserStats (long-array handles) %&)
+                   (concat args [jobs cpus mem member all-jobs all-cpus all-mem counts nil]))
+            "cook_state_user_stats")
+    (doseq [[s state] (map-indexed vector stat-states)]
+      (let [in (filter #(bit-test (.get ^ByteBuffer member (int %)) s) (range u))
+            at (fn [^ByteBuffer b i] (.getDouble b (* 8 (+ (* s u) i))))
+            stats (into {} (for [i in]
+                             [(names i) (merge (when (= s 3) (quota-extra i))
+                                               {"jobs" (.getLong ^ByteBuffer jobs (* 8 (+ (* s u) i)))
+                                                "cpus" (at cpus i) "mem" (at mem i)})]))
+            all (if (seq in)
+                  (merge (apply merge-with + (map #(dissoc (stats (names %)) "jobs" "cpus" "mem") in))
+                         {"jobs" (.getLong ^ByteBuffer all-jobs (* 8 s)) "cpus" (.getDouble ^ByteBuffer all-cpus (* 8 s))
+                          "mem" (.getDouble ^ByteBuffer all-mem (* 8 s))})
+                  {"cpus" 0 "mem" 0 "jobs" 0})]
+        (doseq [[user m] (assoc stats "all" all) [type amount] m]
+          (set-user-counter! state user type amount))))
+    (doseq [[i c] (map-indexed vector user-counts)]
+      (set-total-counter! c (.getLong ^ByteBuffer counts (* 8 i))))))
 
 ;; cook_fp as 24 bytes of a little-endian direct buffer
 (defn- fp-at [^ByteBuffer b i] [(.getLong b (* 24 i)) (.getLong b (+ 8 (* 24 i))) (.getLong b (+ 16 (* 24 i)))])

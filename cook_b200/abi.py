@@ -143,6 +143,10 @@ PHASE_RANK, PHASE_MATCH, PHASE_REBALANCE, PHASE_EXCHANGE, PHASE_STATE, PHASE_USA
 PHASE_CONSIDERABLE = 7
 PHASE_AUDIT = 8
 
+# cook_state_user_stats: the state rows of its [4][n_users] outputs and the order of its user counts
+STATS_RUNNING, STATS_WAITING, STATS_STARVED, STATS_WUQ = 0, 1, 2, 3
+USERS_TOTAL, USERS_STARVED, USERS_WUQ, USERS_HUNGRY, USERS_SATISFIED, USERS_N = 0, 1, 2, 3, 4, 5
+
 USAGE_GIVEN, USAGE_DERIVED, USAGE_LAST_MATCH = 0, 1, 2
 
 
@@ -315,6 +319,8 @@ ARGTYPES = {
     "cook_state_counts_compare": [P_I64, P_I64, P_I32],
     "cook_state_export": [_H, _I32, P_U8, _P(StateSizes), _P(StateRows), _P(StateSizes)],
     "cook_state_queue": [_H, _I32, P_I64, P_I32],
+    "cook_state_user_stats": [_P(_H), _I32, _P(UserTable), P_U8, P_I64, P_F64, P_F64, P_U8, P_I64, P_F64, P_F64, P_I64,
+                              _P(PhaseStats)],
     "cook_last_stats": [_H, _I32, _P(PhaseStats)],
     "cook_allgather_usage": [_H, _H, P_F64, P_F64, C.c_int64],
     "cook_comm_unique_id": [P_U8],

@@ -314,32 +314,39 @@ __global__ void reb_pending_kernel(RebRows r, void* const* col, const int32_t* m
   writable(o.ckpt_location)[d] = static_cast<const int32_t*>(col[P_CKPT])[s];
 }
 
-// ---- running usage: the live running rows, dense in slot order; host = the index of the row's hostname
-// code in the caller's list, or H when the row's host is -1 or not listed (a segment no output reads)
+// ---- usage folds: a table's live rows, dense in slot order, each handle's after those of the handles before it
+// (base).  The table's columns by index: the running rows (user, task id, amounts, hostname code) or the pending
+// rows (user, job id, amounts; no host).  host = the index of the row's hostname code in the caller's list, or H
+// when the row's host is -1 or not listed (a segment no output reads)
+struct TableCols { int live, user, id, amt[3], host; };
+constexpr TableCols RUN_COLS = {R_LIVE, R_USER, R_TID, {R_CPUS, R_MEM, R_GPUS}, R_HOST};
+constexpr TableCols PEND_COLS = {P_LIVE, P_USER, P_JID, {P_CPUS, P_MEM, P_GPUS}, -1};
 struct UsageRows {
-  void* const* col;
-  int32_t* user; int64_t* tid; int32_t* host; double* amt[3];   // host null: no host list
+  void* const* col; TableCols c; int base;
+  int32_t* user; int64_t* id; int32_t* host; double* amt[3];   // host null: no host list
   const int32_t* host_of; int32_t n_codes, H;
-  __device__ bool keep(int i) const { return static_cast<const uint8_t*>(col[R_LIVE])[i]; }
+  __device__ bool keep(int i) const { return static_cast<const uint8_t*>(col[c.live])[i]; }
   __device__ void emit(int i, int d) const {
-    user[d] = static_cast<const int32_t*>(col[R_USER])[i];
-    tid[d] = static_cast<const int64_t*>(col[R_TID])[i];
-    amt[0][d] = static_cast<const double*>(col[R_CPUS])[i];
-    amt[1][d] = static_cast<const double*>(col[R_MEM])[i];
-    amt[2][d] = static_cast<const double*>(col[R_GPUS])[i];
+    d += base;
+    user[d] = static_cast<const int32_t*>(col[c.user])[i];
+    id[d] = static_cast<const int64_t*>(col[c.id])[i];
+#pragma unroll
+    for (int k = 0; k < 3; k++) amt[k][d] = static_cast<const double*>(col[c.amt[k]])[i];
     if (host) {
-      const int32_t code = static_cast<const int32_t*>(col[R_HOST])[i];
+      const int32_t code = static_cast<const int32_t*>(col[c.host])[i];
       const int32_t h = code >= 0 && code < n_codes ? host_of[code] : -1;
       host[d] = h < 0 ? H : h;
     }
   }
 };
-// (key, task id); key null: task id alone.  Task ids are unique among live rows, so the order is total.
+// (key, task id, dense index); key null: task id alone.  Task ids are unique among one handle's live rows; an id
+// that several handles hold goes in handle order, which the dense index keeps.
 struct LessKeyTid {
   const int32_t* key; const int64_t* tid;
   __device__ bool operator()(int32_t a, int32_t b) const {
     if (key && key[a] != key[b]) return key[a] < key[b];
-    return tid[a] < tid[b];
+    if (tid[a] != tid[b]) return tid[a] < tid[b];
+    return a < b;
   }
 };
 struct LoadSorted {   // the order-wide scan's addends: cpus, mem, gpus of the row at position p
@@ -395,6 +402,92 @@ __global__ void __launch_bounds__(128) usage_fold_kernel(UsageArgs a) {
     a.host_count[g] = e - s; a.host_cpus[g] = acc[0]; a.host_mem[g] = acc[1];
   } else {
     a.pool_out[0] = (double)(e - s); a.pool_out[1] = acc[0]; a.pool_out[2] = acc[1]; a.pool_out[3] = acc[2];
+  }
+}
+
+// ---- the monitor's user stats (set-stats-counters!, monitor.clj:177-207) from the running and waiting folds
+struct StatsArgs {
+  const double* run; const double* wait;   // [4][U] count, cpus, mem, gpus: the two usage folds
+  const double *div_cpus, *div_mem, *q_count, *q_cpus, *q_mem;
+  const uint8_t* rest_ok;                  // null: every user's other quota keys are > 0
+  int U;
+  int64_t* jobs; double* cpus; double* mem;   // [4][U] by COOK_STATS_*
+  uint8_t* member;                            // [U] bit s: the user is in state s
+};
+// Thread per user.  Starved (get-starved-job-stats :69-90): every share key above the running amount; values
+// (merge-with min waiting (merge-with - share running)), where :jobs is only in the running map and passes the
+// subtraction.  Waiting under quota (:92-116): every quota key above the running amount; values min(max(quota -
+// running, 0), waiting).  An absent running map reads 0.0, which leaves every subtraction exact.
+__global__ void user_stats_kernel(StatsArgs a) {
+  const int u = blockIdx.x * blockDim.x + threadIdx.x;
+  if (u >= a.U) return;
+  const int U = a.U;
+  const double rj = a.run[u], rc = a.run[U + u], rm = a.run[2 * U + u];
+  const double wj = a.wait[u], wc = a.wait[U + u], wm = a.wait[2 * U + u];
+  const bool running = rj > 0.0, waiting = wj > 0.0;
+  int64_t j[4] = {(int64_t)rj, (int64_t)wj, 0, 0};
+  double c[4] = {rc, wc, 0.0, 0.0}, m[4] = {rm, wm, 0.0, 0.0};
+  int bits = (running ? 1 << COOK_STATS_RUNNING : 0) | (waiting ? 1 << COOK_STATS_WAITING : 0);
+  if (waiting) {
+    const double sc = a.div_cpus[u], sm = a.div_mem[u];
+    if (rc < sc && rm < sm) {
+      bits |= 1 << COOK_STATS_STARVED;
+      j[COOK_STATS_STARVED] = running ? min(j[0], j[1]) : j[1];
+      c[COOK_STATS_STARVED] = fmin(wc, sc - rc);
+      m[COOK_STATS_STARVED] = fmin(wm, sm - rm);
+    }
+    const double qj = a.q_count[u], qc = a.q_cpus[u], qm = a.q_mem[u];
+    if (rj < qj && rc < qc && rm < qm && (!a.rest_ok || a.rest_ok[u])) {
+      bits |= 1 << COOK_STATS_WUQ;
+      j[COOK_STATS_WUQ] = (int64_t)fmin(wj, fmax(qj - rj, 0.0));
+      c[COOK_STATS_WUQ] = fmin(wc, fmax(qc - rc, 0.0));
+      m[COOK_STATS_WUQ] = fmin(wm, fmax(qm - rm, 0.0));
+    }
+  }
+#pragma unroll
+  for (int s = 0; s < 4; s++) {
+    a.jobs[(size_t)s * U + u] = j[s]; a.cpus[(size_t)s * U + u] = c[s]; a.mem[(size_t)s * U + u] = m[s];
+  }
+  a.member[u] = (uint8_t)bits;
+}
+
+struct StatsTotals { int64_t jobs[4]; double cpus[4]; double mem[4]; int64_t users[COOK_USERS_N]; };
+__device__ __forceinline__ long long warp_sum_ll(long long x) {
+  for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(FULL_MASK, x, o);
+  return x;
+}
+// One block, warp s per state: the "all" entry (add-aggregated-stats :59-67), a left fold of cpus and mem over the
+// state's users in ascending user code (association-free when all 4 * U values are on the grid), jobs an integer sum;
+// then the five user counts.
+__global__ void __launch_bounds__(128) user_stats_totals_kernel(const int64_t* jobs, const double* cpus,
+                                                                const double* mem, const uint8_t* member, int U,
+                                                                const GridFlag* gf, StatsTotals* out) {
+  __shared__ double stage[4][2][32];
+  __shared__ long long n_in[4];
+  const int s = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const size_t o = (size_t)s * U;
+  double acc[2] = {0.0, 0.0};
+  warp_fold_sum<2, 4>(acc, U, grid_exact(gf, U), [&](int u, double (&x)[2]) {
+    if (!((member[u] >> s) & 1)) return false;
+    x[0] = cpus[o + u]; x[1] = mem[o + u];
+    return true;
+  }, stage[s]);
+  long long nj = 0, nm = 0, nt = 0, nsat = 0;
+  for (int u = lane; u < U; u += 32) {
+    const int b = member[u];
+    if ((b >> s) & 1) { nj += jobs[o + u]; nm++; }
+    nt += (b & 3) != 0;   // running or waiting
+    nsat += (b & 3) == 1; // running, not waiting
+  }
+  nj = warp_sum_ll(nj); nm = warp_sum_ll(nm); nt = warp_sum_ll(nt); nsat = warp_sum_ll(nsat);
+  if (lane == 0) { out->jobs[s] = nj; out->cpus[s] = acc[0]; out->mem[s] = acc[1]; n_in[s] = nm; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    out->users[COOK_USERS_TOTAL] = nt;
+    out->users[COOK_USERS_STARVED] = n_in[COOK_STATS_STARVED];
+    out->users[COOK_USERS_WUQ] = n_in[COOK_STATS_WUQ];
+    out->users[COOK_USERS_HUNGRY] = n_in[COOK_STATS_WAITING] - n_in[COOK_STATS_STARVED];
+    out->users[COOK_USERS_SATISFIED] = nsat;
   }
 }
 
@@ -1098,19 +1191,21 @@ cudaError_t map_hosts(int32_t* host_of, int32_t n_codes, const int32_t* d_codes,
   return cudaGetLastError();
 }
 
-// The running usage of R live rows, each sum a left fold in ascending task id: per user (U > 0), per listed host
-// (H > 0) and of the pool.  The caller sets rows.host_of / rows.n_codes (H > 0) and the destinations
-// a.user_out [4][U], a.host_cpus / host_mem / host_count [H] and a.pool_out [4] of the sums it asked for.
+// The usage of R live rows of one or more handles, each sum a left fold in ascending id: per user (U > 0), per
+// listed host (H > 0, running rows only) and of the pool.  The running rows by task id, or (pending) the pending rows
+// by job id; an id several handles hold, in handle order.  The caller sets rows.host_of / rows.n_codes (H > 0) and
+// the destinations a.user_out [4][U], a.host_cpus / host_mem / host_count [H] and a.pool_out [4] of the sums it
+// asked for.  take's hw: the largest slot high-water mark of the table among the handles.
 struct UsageFold {
   int R = 0, U = 0, H = 0;
-  bool pool = false;
+  bool pool = false, pending = false;
   UsageRows rows = {};
   UsageArgs a = {};
   int32_t *blk = nullptr, *tmp = nullptr;
   GridFlag* gf = nullptr;
 
   void take(Carve& c, int hw) {
-    rows.user = c.take<int32_t>(R); rows.tid = c.take<int64_t>(R);
+    rows.user = c.take<int32_t>(R); rows.id = c.take<int64_t>(R);
     for (int k = 0; k < 3; k++) rows.amt[k] = c.take<double>(R);
     blk = c.take<int32_t>((size_t)hw / CP_BLOCK + 2);
     tmp = c.take<int32_t>(R);
@@ -1134,19 +1229,28 @@ struct UsageFold {
     if (pool) segs(a.seg[US_POOL], 1, false);
   }
 
-  // the live rows, the grid check, the orders with their segments and (on the grid) order-wide scans, the folds
-  cudaError_t run(const PoolState* S, cudaStream_t st, int* nl) {
-    rows.col = S->run.d_col; rows.H = H;
+  // the live rows of handles S[0, n) (their counts in S[0]'s counters), the grid check, the orders with their
+  // segments and (on the grid) order-wide scans, the folds
+  cudaError_t run(const PoolState* const* S, int n, cudaStream_t st, int* nl) {
+    rows.c = pending ? PEND_COLS : RUN_COLS; rows.H = H;
     cudaError_t e = cudaMemsetAsync(gf, 0, sizeof(GridFlag), st);
     if (e != cudaSuccess) return e;
-    compact(rows, S->run.hw, nullptr, blk, S->counters, R, st, nl);
+    rows.base = 0;
+    for (int k = 0; k < n; k++) {
+      const Table& t = pending ? S[k]->pend : S[k]->run;
+      const int live = (int)t.slot_of.size();
+      if (!live) continue;
+      rows.col = t.d_col;
+      compact(rows, t.hw, nullptr, blk, S[0]->counters + (pending ? 1 : 0), live, st, nl);
+      rows.base += live;
+    }
     grid_check_kernel<<<(R + 255) / 256, 256, 0, st>>>(rows.amt[0], rows.amt[1], rows.amt[2], R, gf);
     (*nl)++;
     const int32_t* key[US_N] = {rows.user, rows.host, nullptr};
     for (int k = 0; k < US_N; k++) {
       UsageSegs& q = a.seg[k];
       if (!q.n) continue;
-      if ((e = csort::sort_indices(writable(q.ord), tmp, R, LessKeyTid{key[k], rows.tid}, st, nl)) != cudaSuccess) return e;
+      if ((e = csort::sort_indices(writable(q.ord), tmp, R, LessKeyTid{key[k], rows.id}, st, nl)) != cudaSuccess) return e;
       if (!q.start) continue;
       // +1: the hosts' segment H holds the rows no listed host carries
       if ((e = cudaMemsetAsync(writable(q.start), 0, sizeof(int32_t) * (q.n + 1), st)) != cudaSuccess) return e;
@@ -1254,7 +1358,7 @@ int32_t usage(cook_pool* pool, PoolState* S, int U, double* out_user, double* ou
     CK(pool, map_hosts(host_of, n_codes, d_codes, H, st, &nl));
     f.rows.host_of = host_of; f.rows.n_codes = n_codes;
   }
-  CK(pool, f.run(S, st, &nl));
+  CK(pool, f.run(&S, 1, st, &nl));
   CK(pool, cudaEventRecord(pool->ev[22], st));
   if (users) CK(pool, download(out_user, a.user_out, 4 * (size_t)U, st, &d2h));
   if (out_pool) CK(pool, download(out_pool, a.pool_out, 4, st, &d2h));
@@ -1398,7 +1502,7 @@ int32_t derive_match(cook_pool* pool, PoolState* S, const MatchRows& rows, int U
   }
   f.a.user_out = rows.usage;
   f.a.host_cpus = rows.run_cpus; f.a.host_mem = rows.run_mem; f.a.host_count = rows.run_count;
-  CK(pool, f.run(S, st, nl));
+  CK(pool, f.run(&S, 1, st, nl));
   if (!entries) return COOK_OK;
   l.a.host_of = O > 0 ? host_of : nullptr; l.a.n_codes = n_codes;
   l.a.attr = rows.attr; l.a.H = O;
@@ -1890,7 +1994,7 @@ int32_t considerable(cook_pool* pool, PoolState* S, const cook_user_table* users
     if (src == COOK_USAGE_DERIVED) {
       if (fold) {
         f.a.user_out = usage;
-        CK(pool, f.run(S, st, &nl));
+        CK(pool, f.run(&S, 1, st, &nl));
       } else {
         CK(pool, cudaMemsetAsync(usage, 0, sizeof(double) * 4 * (size_t)U, st));
       }
@@ -1922,7 +2026,124 @@ int32_t considerable(cook_pool* pool, PoolState* S, const cook_user_table* users
   return COOK_OK;
 }
 
+// cook_state_user_stats: the running and waiting folds per user over the union of the handles' live rows, classified
+int32_t user_stats(cook_pool* const* pools, int n, const cook_user_table* users, const uint8_t* rest_ok,
+                   int64_t* out_jobs, double* out_cpus, double* out_mem, uint8_t* out_member, int64_t* out_all_jobs,
+                   double* out_all_cpus, double* out_all_mem, int64_t* out_users, cook_phase_stats* out_stats) {
+  const char* who = "cook_state_user_stats";
+  // ---- every check before any device work or output
+  if (!pools || n <= 0 || !pools[0]) return COOK_E_BADARG;
+  cook_pool* pool = pools[0];
+  std::vector<const PoolState*> S;
+  int R = 0, J = 0, hw_r = 0, hw_p = 0;
+  for (int k = 0; k < n; k++) {
+    if (!pools[k]) return set_err(pool, COOK_E_BADARG, "%s: a NULL handle", who);
+    if (std::find(pools, pools + k, pools[k]) != pools + k)
+      return set_err(pool, COOK_E_BADARG, "%s: a handle listed twice", who);
+    if (pools[k]->device != pool->device) return set_err(pool, COOK_E_BADARG, "%s: handles on different devices", who);
+  }
+  if (!users || !out_jobs || !out_cpus || !out_mem || !out_member || !out_all_jobs || !out_all_cpus || !out_all_mem ||
+      !out_users)
+    return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
+  const double* ucol[5] = {users->div_cpus, users->div_mem, users->quota_count, users->quota_cpus, users->quota_mem};
+  for (const double* c : ucol)
+    if (!c) return set_err(pool, COOK_E_BADARG, "%s: null div_cpus, div_mem, quota_count, quota_cpus or quota_mem", who);
+  const int U = users->n_users;
+  if (U <= 0) return set_err(pool, COOK_E_BADARG, "%s: n_users <= 0", who);
+  for (int k = 0; k < n; k++) {
+    const PoolState* s = static_cast<const PoolState*>(pools[k]->state);
+    if (!s) continue;
+    if (std::max(count_max(s->users_p), count_max(s->users_r)) >= U)
+      return set_err(pool, COOK_E_BADARG, "%s: a live row's user code is >= n_users", who);
+    S.push_back(s);
+    R += (int)s->run.slot_of.size(); J += (int)s->pend.slot_of.size();
+    hw_r = std::max(hw_r, s->run.hw); hw_p = std::max(hw_p, s->pend.hw);
+  }
+  if (R + J == 0) {   // no live row: every state is empty, without device work
+    memset(out_jobs, 0, sizeof(int64_t) * 4 * (size_t)U);
+    memset(out_cpus, 0, sizeof(double) * 4 * (size_t)U);
+    memset(out_mem, 0, sizeof(double) * 4 * (size_t)U);
+    memset(out_member, 0, (size_t)U);
+    memset(out_all_jobs, 0, sizeof(int64_t) * 4);
+    memset(out_all_cpus, 0, sizeof(double) * 4);
+    memset(out_all_mem, 0, sizeof(double) * 4);
+    memset(out_users, 0, sizeof(int64_t) * COOK_USERS_N);
+    if (out_stats) *out_stats = cook_phase_stats{};
+    return COOK_OK;
+  }
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S0 = state_of(pool, true);   // pools[0]'s scratch and counters, even when it holds no row
+  if (!S0) return set_err(pool, COOK_E_OOM, "%s: out of device memory", who);
+  if (S.empty() || S[0] != S0) S.insert(S.begin(), S0);   // S[0] owns the counters the compactions write
+  cudaStream_t st = pool->stream;
+  // ---- one carve: the two folds, the user columns (uploaded), the per-state columns and the totals
+  UsageFold fr, fw;
+  fr.R = R; fr.U = U;
+  fw.R = J; fw.U = U; fw.pending = true;
+  StatsArgs a = {};
+  a.U = U;
+  GridFlag* gf = nullptr;
+  StatsTotals* tot = nullptr;
+  double *run = nullptr, *wait = nullptr;
+  int64_t h2d = 0, d2h = 0;
+  CK(pool, carve(S0->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+    if (R) fr.take(c, hw_r);
+    if (J) fw.take(c, hw_p);
+    run = c.take<double>(4 * (size_t)U); wait = c.take<double>(4 * (size_t)U);
+    a.jobs = c.take<int64_t>(4 * (size_t)U); a.cpus = c.take<double>(4 * (size_t)U);
+    a.mem = c.take<double>(4 * (size_t)U); a.member = c.take<uint8_t>(U);
+    gf = c.take<GridFlag>(1);
+    tot = c.take<StatsTotals>(1);
+    a.div_cpus = c.up(ucol[0], U); a.div_mem = c.up(ucol[1], U);
+    a.q_count = c.up(ucol[2], U); a.q_cpus = c.up(ucol[3], U); a.q_mem = c.up(ucol[4], U);
+    a.rest_ok = c.up(rest_ok, U);
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  int nl = 0;
+  const PoolState* const* list = S.data();
+  const int ns = (int)S.size();
+  fr.a.user_out = run; fw.a.user_out = wait;
+  if (R) CK(pool, fr.run(list, ns, st, &nl));
+  else CK(pool, cudaMemsetAsync(run, 0, sizeof(double) * 4 * (size_t)U, st));
+  if (J) CK(pool, fw.run(list, ns, st, &nl));
+  else CK(pool, cudaMemsetAsync(wait, 0, sizeof(double) * 4 * (size_t)U, st));
+  a.run = run; a.wait = wait;
+  user_stats_kernel<<<(U + 255) / 256, 256, 0, st>>>(a);
+  CK(pool, cudaMemsetAsync(gf, 0, sizeof(GridFlag), st));
+  grid_check_kernel<<<(4 * U + 255) / 256, 256, 0, st>>>(a.cpus, a.mem, nullptr, 4 * U, gf);
+  user_stats_totals_kernel<<<1, 128, 0, st>>>(a.jobs, a.cpus, a.mem, a.member, U, gf, tot);
+  nl += 3;
+  CK(pool, cudaGetLastError());
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  StatsTotals t;
+  CK(pool, download(out_jobs, a.jobs, 4 * (size_t)U, st, &d2h));
+  CK(pool, download(out_cpus, a.cpus, 4 * (size_t)U, st, &d2h));
+  CK(pool, download(out_mem, a.mem, 4 * (size_t)U, st, &d2h));
+  CK(pool, download(out_member, a.member, U, st, &d2h));
+  CK(pool, download(&t, tot, 1, st, &d2h));
+  CK(pool, cudaEventRecord(pool->ev[23], st));
+  CK(pool, cudaStreamSynchronize(st));
+  memcpy(out_all_jobs, t.jobs, sizeof t.jobs);
+  memcpy(out_all_cpus, t.cpus, sizeof t.cpus);
+  memcpy(out_all_mem, t.mem, sizeof t.mem);
+  memcpy(out_users, t.users, sizeof t.users);
+  // the call's own statistics: no cook_last_stats slot is written
+  if (out_stats)
+    *out_stats = {ev_ms(pool->ev[20], pool->ev[21]), ev_ms(pool->ev[21], pool->ev[22]), ev_ms(pool->ev[22], pool->ev[23]),
+                  h2d, d2h, nl, 0};
+  return COOK_OK;
+}
+
 }  // namespace
+
+extern "C" int32_t cook_state_user_stats(cook_pool* const* pools, int32_t n_pools, const cook_user_table* users,
+                                         const uint8_t* quota_rest_ok, int64_t* out_jobs, double* out_cpus,
+                                         double* out_mem, uint8_t* out_member, int64_t* out_all_jobs,
+                                         double* out_all_cpus, double* out_all_mem, int64_t* out_users,
+                                         cook_phase_stats* out_stats) {
+  return user_stats(pools, n_pools, users, quota_rest_ok, out_jobs, out_cpus, out_mem, out_member, out_all_jobs,
+                    out_all_cpus, out_all_mem, out_users, out_stats);
+}
 
 extern "C" int32_t cook_state_rank(cook_pool* pool, const cook_user_table* users, const cook_pool_quota* pool_quota,
                                    const cook_pool_quota* group_quota, const double* group_usage,

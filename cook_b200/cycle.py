@@ -15,10 +15,13 @@ path end to end.  It computes nothing numeric: every placement decision is `engi
   summarize_failures    fenzo_utils.clj:45-89 shape from cook_match_failures' counters (8f-3)
   resync                the audit of a resident pool fed by deltas: bucket fingerprints compared with the host's,
                         the differing buckets exported, the repairing delta built
+  monitor_stats         the counters set-stats-counters! (monitor.clj:177-207) sets, from cook_state_user_stats
+  queue_lengths         jobs->queue-lengths (queue_limit.clj:64-90), from single-pool cook_state_user_stats calls
 """
 import numpy as np
 
 from . import abi, traces
+from .engine import STATS_KEYS
 
 CONSTRAINT_NAMES = [  # Cook's evaluation order (constraints.clj:459-495; defrecord class names)
     "checkpoint_locality_constraint", "estimated_completion_constraint", "user_defined_constraint",
@@ -301,3 +304,59 @@ def resync(engine, host_digest_buckets, rows_of_bucket):
     want["pending_rm"] = [j for j in held["pending_job_id"].tolist() if j not in host_jobs]
     want["running_rm"] = [t for t in held["running"].col("task_id").tolist() if t not in host_tasks]
     return buckets, abi.make_delta(**want)
+
+
+# ---- the monitor's user stats and the queue lengths from resident pools (SURVEY §8f-1) --------------------------
+LONG_MAX = 2 ** 63 - 1
+
+
+def counter_value(x):
+    """What set-counter! (monitor.clj:118-123) stores: (long (min value Long/MAX_VALUE)), saturating at
+    Long/MAX_VALUE and truncating toward zero."""
+    if isinstance(x, (int, np.integer)):
+        return min(int(x), LONG_MAX)
+    x = float(x)
+    return LONG_MAX if x >= 2.0 ** 63 else int(x)
+
+
+def monitor_stats(stats, user_names, quota_extra=None):
+    """The counters set-stats-counters! sets for one pool or quota-group name, from engine.state_user_stats over its
+    handles: {state: {user name: {"jobs", "cpus", "mem", ...}}} for each of engine.STATS_KEYS, each with its "all"
+    entry (add-aggregated-stats: {"cpus" 0 "mem" 0 "jobs" 0} when nobody is in the state), and "users": the five user
+    counts.  Every value is the one set-counter! stores.
+    quota_extra: per user code, the keys of the user's quota map beyond count, cpus and mem (gpus, the launch rates)
+    by counter name.  A waiting-under-quota user's map carries them unchanged (the merges pass them through), and the
+    state's "all" entry sums them over its users in ascending user code."""
+    out = {}
+    for s, state in enumerate(STATS_KEYS):
+        users = np.flatnonzero((stats["member"] >> s) & 1)
+        m = {}
+        for u in users:
+            e = {"jobs": int(stats["jobs"][s, u]), "cpus": float(stats["cpus"][s, u]), "mem": float(stats["mem"][s, u])}
+            if s == abi.STATS_WUQ and quota_extra is not None:
+                e.update({k: v for k, v in quota_extra[u].items() if k not in e})
+            m[user_names[u]] = e
+        if m:
+            total = dict(zip(("jobs", "cpus", "mem"), stats["all"][state]))
+            for e in m.values():
+                for k, v in e.items():
+                    if k not in ("jobs", "cpus", "mem"):
+                        total[k] = total[k] + v if k in total else v
+            m["all"] = total
+        else:
+            m["all"] = {"cpus": 0, "mem": 0, "jobs": 0}
+        out[state] = {name: {k: counter_value(v) for k, v in e.items()} for name, e in m.items()}
+    out["users"] = dict(stats["users"])
+    return out
+
+
+def queue_lengths(pool_stats, user_names):
+    """jobs->queue-lengths from {pool name: engine.state_user_stats of that pool alone}: {"pool->queue-length":
+    {pool: pending jobs}, "pool->user->queue-length": {pool: {user name: pending jobs}}}.  As group-by, a pool or user
+    without a pending job has no entry."""
+    per = {}
+    for pool, st in pool_stats.items():
+        w = np.flatnonzero((st["member"] >> abi.STATS_WAITING) & 1)
+        if len(w):
+            per[pool] = {user_names[u]: int(st["jobs"][abi.STATS_WAITING, u]) for u in w}
+    return {"pool->queue-length": {p: sum(m.values()) for p, m in per.items()}, "pool->user->queue-length": per}

@@ -466,6 +466,40 @@ def exchange_usage_batch(engines, n_users_pad, n_slots=None, comm=None, world=1)
     return out.reshape(world, n_slots, n_users_pad, 4)
 
 
+STATS_KEYS = ("running", "waiting", "starved", "waiting-under-quota")   # by abi.STATS_*
+USER_COUNTS = ("total", "starved", "waiting-under-quota", "hungry", "satisfied")   # by abi.USERS_*
+
+
+def state_user_stats(engines, users, quota_rest_ok=None):
+    """cook_state_user_stats over the live rows of `engines` (one pool, or the pools of a quota group; one device, the
+    work on engines[0]'s stream).  quota_rest_ok: per user code, whether the user's other quota keys are all > 0
+    (None: all).  Returns 'jobs' (int64), 'cpus' and 'mem' as [4, n_users] arrays by abi.STATS_*, 'member' [n_users]
+    (bit s: the user is in state s), 'all' {state: (jobs, cpus, mem)} and 'users' {count name: n}, keyed by
+    STATS_KEYS and USER_COUNTS, and 'stats', the call's own phase statistics (abi.PhaseStats.as_dict())."""
+    if not engines:
+        raise ValueError("state_user_stats: at least one handle")
+    U = int(users.n_users)
+    ok = np.ascontiguousarray(quota_rest_ok, np.uint8) if quota_rest_ok is not None else None
+    if ok is not None and len(ok) != U:
+        raise ValueError("state_user_stats: quota_rest_ok needs one flag per user")
+    n = max(U, 1)
+    jobs, cpus, mem = np.zeros((4, n), np.int64), np.zeros((4, n)), np.zeros((4, n))
+    member = np.zeros(n, np.uint8)
+    aj, ac, am = np.zeros(4, np.int64), np.zeros(4), np.zeros(4)
+    counts = np.zeros(abi.USERS_N, np.int64)
+    st = abi.PhaseStats()
+    handles = (C.c_void_p * len(engines))(*[e.pool for e in engines])
+    rc = engines[0].lib.cook_state_user_stats(
+        handles, len(engines), C.byref(users), abi.ptr(ok, abi.P_U8) if ok is not None else None,
+        abi.ptr(jobs, abi.P_I64), abi.ptr(cpus, abi.P_F64), abi.ptr(mem, abi.P_F64), abi.ptr(member, abi.P_U8),
+        abi.ptr(aj, abi.P_I64), abi.ptr(ac, abi.P_F64), abi.ptr(am, abi.P_F64), abi.ptr(counts, abi.P_I64), C.byref(st))
+    if rc != 0:
+        engines[0]._err(rc)
+    return {"jobs": jobs[:, :U], "cpus": cpus[:, :U], "mem": mem[:, :U], "member": member[:U],
+            "all": {k: (int(aj[s]), float(ac[s]), float(am[s])) for s, k in enumerate(STATS_KEYS)},
+            "users": {k: int(counts[i]) for i, k in enumerate(USER_COUNTS)}, "stats": st.as_dict()}
+
+
 def comm_unique_id(lib):
     buf = (C.c_uint8 * 128)()
     rc = lib.cook_comm_unique_id(buf)

@@ -814,7 +814,7 @@ int32_t cook_state_queue(cook_pool* pool, int32_t cap, int64_t* out_job_id, int3
  * the considerable pass and the consumption, the download of the ids).  COOK_PHASE_AUDIT: the last
  * cook_state_digest, cook_state_export or cook_state_queue (upload of the bucket mask, the passes over the tables,
  * the compaction, sort and gathers, the download of the fingerprints, rows or ids; all zero after a call without
- * device work). */
+ * device work).  cook_state_user_stats reports through its own out_stats argument. */
 enum { COOK_PHASE_RANK = 0, COOK_PHASE_MATCH = 1, COOK_PHASE_REBALANCE = 2, COOK_PHASE_EXCHANGE = 3,
        COOK_PHASE_STATE = 4, COOK_PHASE_USAGE = 5, COOK_PHASE_COTASKS = 6, COOK_PHASE_CONSIDERABLE = 7,
        COOK_PHASE_AUDIT = 8 };
@@ -828,6 +828,57 @@ typedef struct {
   int32_t reserved0;
 } cook_phase_stats;
 int32_t cook_last_stats(cook_pool* pool, int32_t phase, cook_phase_stats* out);
+
+/* ------------------------------------------------------ the monitor over resident pools */
+/* The monitor's per-user stats and user counts (set-stats-counters!, monitor.clj:177-207) read from the live rows of
+ * one pool or of a quota group, and the queue lengths (jobs->queue-lengths, queue_limit.clj:64-90) as the waiting
+ * state of single-pool calls.
+ *   Rows     the union of the live rows of pools[0, n_pools): one handle gives a pool's stats; the handles of the pools
+ *            a quota-group name maps to give that name's (job-ent-in-pool :35-38).  The handles follow
+ *            cook_exchange_usage_batch's rules: one device, idle, each call serialised with each of them by the
+ *            caller; the work runs on pools[0]'s stream and scratch.
+ *   Folds    get-job-stats (:40-57) per user, each sum a left fold in a fixed order (DESIGN.md §2): waiting over the
+ *            live pending rows in ascending job id, running over the live running rows in ascending task id; an id
+ *            several handles hold, in the order of pools.  jobs is the number of rows.
+ *   Outputs  for each state s (COOK_STATS_*) and user code u < n_users, out_jobs / out_cpus / out_mem[s * n_users +
+ *            u]; bit s of out_member[u] says whether u is in state s.  A user outside a state has zeros there.
+ *     running  the user has a live running row: their running fold.
+ *     waiting  the user has a live pending row: their waiting fold.
+ *     starved  (waiting users, get-starved-job-stats :69-90) run_cpus < share_cpus and run_mem < share_mem, the shares
+ *              being users->div_cpus / div_mem filled as share/get-shares fills them (the user's share, else the
+ *              default user's, else Double/MAX_VALUE); a user with no running row has usage 0.0.  cpus = min(share -
+ *              run, wait), mem likewise; jobs = min(run_jobs, wait_jobs) when the user runs, else wait_jobs: :jobs is
+ *              only in the running map, so (merge-with - share running) passes it through unchanged.
+ *     wuq      (waiting users, get-waiting-under-quota-job-stats :92-116) run_jobs < quota_count, run_cpus <
+ *              quota_cpus, run_mem < quota_mem and quota_rest_ok[u] != 0: the caller's verdict that every other key
+ *              of the user's quota map is > 0.0 (gpus always, plus the default user's :launch-rate-* for users
+ *              without a quota of their own, quota.clj:82-111, 272-295); NULL means all 1.  jobs, cpus, mem =
+ *              min(max(quota - run, 0), wait), quota_count an integral value.  The map's other keys pass through
+ *              from the quota unchanged; they are host values and not computed here.
+ *   Totals   out_all_jobs / _cpus / _mem[s]: the "all" entry of state s (add-aggregated-stats :59-67), a left fold
+ *            over the state's users in ascending user code (any association only where the grid rule holds).
+ *            out_users[COOK_USERS_*]: total = |running u waiting|, starved, wuq, hungry = waiting - starved,
+ *            satisfied = running - waiting.
+ * Changes nothing resident: no row, queue, match plan or COOK_USAGE_LAST_MATCH usage.
+ * COOK_E_BADARG, before any device work and with nothing written: a NULL pools, users or out_* array; n_pools <= 0;
+ * a NULL handle, a handle listed twice or one on another device than pools[0]; n_users <= 0; a NULL div_cpus, div_mem,
+ * quota_count, quota_cpus or quota_mem; a live row's user code >= n_users.  A quota group whose pools sit on
+ * different GPUs is served by one call per device and the host's addition of the folds.
+ * No live row in any handle: every output zero, no device work.
+ * Transfers exactly: up 40 * n_users (the five user columns) + n_users (quota_rest_ok, when given); down 97 * n_users
+ * (the three [4][n_users] arrays and out_member) + 136 (the totals).
+ * Statistics: out_stats (may be NULL) receives the call's own cook_phase_stats: upload of the user columns, the
+ * compactions, sorts and folds of both tables, the classification and totals, the download; all zero after a call
+ * without device work.  No cook_last_stats slot is written, so every phase reports its own calls as before.
+ * Outputs are plain caller arrays, like cook_state_usage's, rather than one result struct: every struct of this
+ * header has a field-for-field ctypes mirror (cook_b200/abi.py), and arrays need none.                          */
+enum { COOK_STATS_RUNNING = 0, COOK_STATS_WAITING = 1, COOK_STATS_STARVED = 2, COOK_STATS_WUQ = 3 };
+enum { COOK_USERS_TOTAL = 0, COOK_USERS_STARVED = 1, COOK_USERS_WUQ = 2, COOK_USERS_HUNGRY = 3,
+       COOK_USERS_SATISFIED = 4, COOK_USERS_N = 5 };
+int32_t cook_state_user_stats(cook_pool* const* pools, int32_t n_pools, const cook_user_table* users,
+                              const uint8_t* quota_rest_ok, int64_t* out_jobs, double* out_cpus, double* out_mem,
+                              uint8_t* out_member, int64_t* out_all_jobs, double* out_all_cpus, double* out_all_mem,
+                              int64_t* out_users, cook_phase_stats* out_stats);
 
 /* ----------------------------------------------------------------- multi-GPU */
 /* §8e: after a pool's match round every rank contributes its pools' usage

@@ -257,6 +257,27 @@ JFN(jint, stateConsiderable)(JNIEnv* env, jclass k, jlong pool, jint n_users, jo
   (*env)->SetIntArrayRegion(env, out_n, 0, 1, (jint*)&n);
   return rc;
 }
+/* the monitor's user stats over the live rows of `pools` (a long[] of handles: one pool, or a quota group's pools);
+ * out_jobs / out_cpus / out_mem hold [4][n_users] values, out_member n_users bytes, out_all_jobs / _cpus / _mem 4
+ * values, out_users COOK_USERS_N longs, out_stats sizeof(cook_phase_stats) bytes; quota_rest_ok and out_stats may
+ * be null.  More than 64 handles is COOK_E_BADARG: a quota group's stats over a subset of its pools would be wrong */
+JFN(jint, stateUserStats)(JNIEnv* env, jclass k, jlongArray pools, jint n_users, jobjectArray users,
+                          jobject quota_rest_ok, jobject out_jobs, jobject out_cpus, jobject out_mem, jobject out_member,
+                          jobject out_all_jobs, jobject out_all_cpus, jobject out_all_mem, jobject out_users,
+                          jobject out_stats) {
+  cook_user_table u;
+  memset(&u, 0, sizeof(u));
+  users_from(env, n_users, users, &u);
+  jsize n = (*env)->GetArrayLength(env, pools);
+  if (n > 64) return COOK_E_BADARG;
+  jlong* h = (*env)->GetLongArrayElements(env, pools, NULL);
+  cook_pool* p[64];
+  for (jsize i = 0; i < n; i++) p[i] = (cook_pool*)(intptr_t)h[i];
+  (*env)->ReleaseLongArrayElements(env, pools, h, JNI_ABORT);
+  return cook_state_user_stats(p, (int32_t)n, &u, one(env, quota_rest_ok), one(env, out_jobs), one(env, out_cpus),
+                               one(env, out_mem), one(env, out_member), one(env, out_all_jobs), one(env, out_all_cpus),
+                               one(env, out_all_mem), one(env, out_users), one(env, out_stats));
+}
 /* the fingerprints and the recount of the resident rows: out_digest is a direct buffer of sizeof(cook_state_digest_out),
  * out_pending_bucket / out_running_bucket direct buffers of n_buckets cook_fp each (null when n_buckets == 0) */
 JFN(jint, stateDigest)(JNIEnv* env, jclass k, jlong pool, jint n_buckets, jobject out_digest, jobject out_pending_bucket,

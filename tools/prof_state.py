@@ -70,6 +70,16 @@ live flags, list ranges and list entries.
 
   python tools/prof_state.py --audit --pool c2
   python tools/prof_state.py --audit --pool c5 --c5-pool 5
+
+--user-stats loads the pool's pending jobs and running tasks (or, with --c3-group N, config-#3 pools 0 .. N-1 into one
+handle each) and per cycle runs cook_state_user_stats over the handles, users' shares and quotas set around their
+running usage, on the grid and off it (cpus + 0.1, mem / 3).  It prints the call's device time, wall time, bytes and
+launches, the wall time of the same folds and classification in single-threaded numpy (what a shim runs without the
+call), and whether the two agree to the bit.
+
+  python tools/prof_state.py --user-stats --pool c2 --cycles 5
+  python tools/prof_state.py --user-stats --pool c5 --c5-pool 5 --cycles 5
+  python tools/prof_state.py --user-stats --c3-group 4 --cycles 5
 """
 import argparse
 import json
@@ -118,7 +128,8 @@ class Jobs:
 
 def card():
     try:
-        out = subprocess.check_output(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], text=True)
+        out = subprocess.check_output(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm",
+                                       "--format=csv,noheader"], text=True)
         return out.strip().splitlines()[0]
     except Exception as e:   # noqa: BLE001
         return f"unknown ({e})"
@@ -222,6 +233,102 @@ def usage(a):
                                               "d2h_bytes": st["d2h_bytes"], "n_launches": st["n_launches"]},
                               "host_fold_wall_ms": round(1e3 * w_host, 3), "identical": bool(same)}), flush=True)
         e.close()
+
+
+def host_user_stats(tables, U, t):
+    """What a shim computes without cook_state_user_stats, single-threaded numpy: per table the rows of every pool
+    sorted by (user, id) (stable: an id two pools hold in pool order) and summed per user with np.add.at, which adds in
+    index order, so each sum is the left fold; the states as cook_state_user_stats classifies them; each "all" entry a
+    cumulative sum over the state's users in ascending code."""
+    folds = []
+    for rows in tables:   # running, then waiting: (user, id, cpus, mem) concatenated in pool order
+        u, i, c, m = (np.concatenate([r[k] for r in rows]) for k in range(4))
+        o = np.lexsort((i, u))
+        f = np.zeros((3, U))
+        np.add.at(f[0], u[o], 1.0)
+        np.add.at(f[1], u[o], c[o])
+        np.add.at(f[2], u[o], m[o])
+        folds.append(f)
+    (rj, rc, rm), (wj, wc, wm) = folds
+    waiting = wj > 0
+    starved = waiting & (rc < t["div_cpus"]) & (rm < t["div_mem"])
+    wuq = waiting & (rj < t["quota_count"]) & (rc < t["quota_cpus"]) & (rm < t["quota_mem"]) & (t["rest_ok"] > 0)
+    member = ((rj > 0).astype(np.uint8) | waiting.astype(np.uint8) << 1 | starved.astype(np.uint8) << 2 |
+              wuq.astype(np.uint8) << 3)
+    sel = [rj > 0, waiting, starved, wuq]
+    jobs = np.stack([rj, wj, np.where(rj > 0, np.minimum(rj, wj), wj),
+                     np.minimum(wj, np.maximum(t["quota_count"] - rj, 0.0))]).astype(np.int64)
+    cpus = np.stack([rc, wc, np.minimum(wc, t["div_cpus"] - rc), np.minimum(wc, np.maximum(t["quota_cpus"] - rc, 0.0))])
+    mem = np.stack([rm, wm, np.minimum(wm, t["div_mem"] - rm), np.minimum(wm, np.maximum(t["quota_mem"] - rm, 0.0))])
+    for s in range(4):
+        for a in (jobs, cpus, mem):
+            a[s][~sel[s]] = 0
+    last = lambda x: float(np.cumsum(x)[-1]) if len(x) else 0.0
+    tot = [(int(jobs[s][sel[s]].sum()), last(cpus[s][sel[s]]), last(mem[s][sel[s]])) for s in range(4)]
+    users = [int((sel[0] | sel[1]).sum()), int(starved.sum()), int(wuq.sum()), int(waiting.sum() - starved.sum()),
+             int((sel[0] & ~waiting).sum())]
+    return jobs, cpus, mem, member, tot, users
+
+
+def user_stats_prof(a):
+    """--user-stats: cook_state_user_stats against host_user_stats on one pool (--pool) or a quota group of config-#3
+    pools (--c3-group N: pools 0 .. N-1, one handle each), on the grid and off it (cpus + 0.1, mem / 3)."""
+    from cook_b200.engine import state_user_stats
+    if a.c3_group > 0:
+        ts = [traces.gen_config_pool("c3", p) for p in range(a.c3_group)]
+        name = f"c3/0-{a.c3_group - 1}"
+    else:
+        ts = [traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)]
+        name = a.pool if a.pool == "c2" else f"c5/{a.c5_pool}"
+    U = max(t["users"].n_users for t in ts)
+    rng = np.random.default_rng(a.seed)
+    pend = [(t["cols"]["pending"]["user"].astype(np.int32), t["cols"]["pending"]["job_id"].astype(np.int64),
+             t["jobs"].col("cpus"), t["jobs"].col("mem")) for t in ts]
+    run = [tuple(np.asarray(t["cols"]["running"][k]) for k in ("user", "task_id", "cpus", "mem")) for t in ts]
+    print(json.dumps({"card": card(), "pool": name, "pending": sum(len(p[0]) for p in pend),
+                      "running": sum(len(r[0]) for r in run), "users": U}), flush=True)
+    used = np.zeros(U)
+    for r in run:
+        np.add.at(used, r[0], r[2])
+    # shares and quotas around the running usage, so that every state is populated
+    tab = dict(div_cpus=np.where(rng.random(U) < 0.3, np.finfo(np.float64).max, used + rng.choice([-1.0, 4.0], U)),
+               div_mem=np.full(U, np.finfo(np.float64).max), quota_count=rng.integers(0, 500, U).astype(float),
+               quota_cpus=used + rng.choice([-1.0, 8.0], U), quota_mem=np.full(U, np.finfo(np.float64).max),
+               rest_ok=(rng.random(U) < 0.9).astype(np.uint8))
+    users = abi.make_users(U, div_cpus=tab["div_cpus"], div_mem=tab["div_mem"],
+                           quota={"count": tab["quota_count"], "cpus": tab["quota_cpus"], "mem": tab["quota_mem"]})
+    for regime in ("grid", "off"):
+        off = (lambda c, m: (c + 0.1, m / 3.0)) if regime == "off" else (lambda c, m: (c, m))
+        tp = [(u, i) + off(c, m) for u, i, c, m in pend]
+        tr = [(u, i) + off(c, m) for u, i, c, m in run]
+        engines = [GpuEngine(pool_name=f"stats{k}") for k in range(len(ts))]
+        for e, p, r in zip(engines, tp, tr):
+            n = len(p[0])
+            e.state_apply(abi.make_delta(
+                reset=True, pending=abi.JobsSoA(n=n, user=p[0], cpus=p[2], mem=p[3]), pending_priority=np.full(n, 50, np.int32),
+                pending_job_id=p[1], running=abi.make_tasks(r[0], np.full(len(r[0]), 50, np.int32),
+                                                           np.zeros(len(r[0]), np.int64), r[1], r[1] + 1, r[2], r[3])))
+        for cycle in range(a.cycles):
+            w0 = time.perf_counter()
+            got = state_user_stats(engines, users, tab["rest_ok"])
+            w_dev = time.perf_counter() - w0
+            st = got["stats"]
+            w0 = time.perf_counter()
+            jobs, cpus, mem, member, tot, cnt = host_user_stats([tr, tp], U, tab)
+            w_host = time.perf_counter() - w0
+            bits = lambda x, y: np.array_equal(np.asarray(x).view(np.uint64), np.asarray(y).view(np.uint64))
+            same = (np.array_equal(got["jobs"], jobs) and bits(got["cpus"], cpus) and bits(got["mem"], mem) and
+                    np.array_equal(got["member"], member) and list(got["users"].values()) == cnt and
+                    all(got["all"][k][0] == tot[s][0] and bits(np.array(got["all"][k][1:]), np.array(tot[s][1:]))
+                        for s, k in enumerate(got["all"])))
+            print(json.dumps({"regime": regime, "cycle": cycle,
+                              "user_stats": {**{k: round(st[k], 3) for k in ("ms_h2d", "ms_device", "ms_d2h")},
+                                             "wall_ms": round(1e3 * w_dev, 3), "h2d_bytes": st["h2d_bytes"],
+                                             "d2h_bytes": st["d2h_bytes"], "n_launches": st["n_launches"]},
+                              "numpy_wall_ms": round(1e3 * w_host, 3), "users": got["users"],
+                              "identical": bool(same)}), flush=True)
+        for e in engines:
+            e.close()
 
 
 def host_cotasks(tid, host, gidx, goff, G, acol, codes, attr):
@@ -573,10 +680,14 @@ def main():
     ap.add_argument("--derived", action="store_true")
     ap.add_argument("--considerable", action="store_true")
     ap.add_argument("--audit", action="store_true")
+    ap.add_argument("--user-stats", action="store_true")
+    ap.add_argument("--c3-group", type=int, default=0, help="--user-stats: a quota group of config-#3 pools 0 .. N-1")
     ap.add_argument("--reps", type=int, default=20, help="--audit: timed calls per kind")
     a = ap.parse_args()
     if a.audit:
         return audit_prof(a)
+    if a.user_stats:
+        return user_stats_prof(a)
     if a.considerable:
         return considerable_prof(a)
     if a.rebalance:
