@@ -188,11 +188,13 @@ struct RankOffensive {
   int64_t* out;
   int32_t* out_n;
 };
+// `d_pool_usage` (if given): the pool quota filter's start, [4] on the device (count, cpus, mem, gpus), in place of
+// the fold of the R running rows in input order.
 int32_t rank_impl(cook_pool* pool, int R, int J, const cook_tasks_soa* running, const cook_tasks_soa* pending,
                   const TaskCols* dev, const cook_user_table* users, const cook_pool_quota* pool_quota,
                   const cook_pool_quota* group_quota, const double* group_usage, const cook_rank_params* params,
                   int32_t* out_ranked_idx, int32_t* out_n, double* out_dru, int32_t* out_order, int32_t* out_order_n,
-                  RankQueue* queue, const RankOffensive* offensive = nullptr);
+                  RankQueue* queue, const RankOffensive* offensive = nullptr, const double* d_pool_usage = nullptr);
 
 // The running-side inputs of a match or rebalance that the resident state derives on the device after the build:
 // carved, not uploaded.  usage: the users' usage_* as one [4][n_users] block (count, cpus, mem, gpus); run: the

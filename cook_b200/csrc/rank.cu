@@ -306,7 +306,7 @@ int32_t rank_impl(cook_pool* pool, int R, int J, const cook_tasks_soa* running, 
                   const TaskCols* dev, const cook_user_table* users, const cook_pool_quota* pool_quota,
                   const cook_pool_quota* group_quota, const double* group_usage, const cook_rank_params* params,
                   int32_t* out_ranked_idx, int32_t* out_n, double* out_dru, int32_t* out_order, int32_t* out_order_n,
-                  RankQueue* queue, const RankOffensive* offensive) {
+                  RankQueue* queue, const RankOffensive* offensive, const double* d_pool_usage) {
   if (!users || !params || !out_n) return set_err(pool, COOK_E_BADARG, "cook_rank: null argument");
   const int N = R + J, U = users->n_users;
   if (R < 0 || J < 0 || U <= 0) return set_err(pool, COOK_E_BADARG, "cook_rank: bad sizes");
@@ -325,7 +325,7 @@ int32_t rank_impl(cook_pool* pool, int R, int J, const cook_tasks_soa* running, 
   int32_t *d_idx, *d_tmp, *d_user_at, *d_pos, *d_out_order, *d_out_ranked, *d_seg_start, *d_seg_end, *d_counters;
   int64_t* d_tie;
   int32_t *d_os_pv, *d_os_bv;
-  double *d_dru_at, *d_pool_usage, *d_dru_task, *d_os_pm, *d_os_pc, *d_os_pg, *d_os_b;
+  double *d_dru_at, *d_quota_usage, *d_dru_task, *d_os_pm, *d_os_pc, *d_os_pg, *d_os_b;
   GridFlag* d_gf;
   QueueFilterArgs qa;
   int64_t* d_off = nullptr;
@@ -358,7 +358,7 @@ int32_t rank_impl(cook_pool* pool, int R, int J, const cook_tasks_soa* running, 
     d_tie = c.take<int64_t>(N + 1);
     d_seg_start = c.take<int32_t>(U);
     d_seg_end = c.take<int32_t>(U);
-    d_pool_usage = c.take<double>(8);
+    d_quota_usage = c.take<double>(8);   // [0, 4): the pool's running usage (unless given), [4, 8): the group's
     d_counters = c.take<int32_t>(8);  // [0]=n_kept [1]=n_out
     d_dru_task = c.take<double>(N + 1);
     d_gf = c.take<GridFlag>(1);
@@ -411,13 +411,16 @@ int32_t rank_impl(cook_pool* pool, int R, int J, const cook_tasks_soa* running, 
   qf_gather_kernel<<<qnb, QF_TB, 0, st>>>(qa);
   nl++;
   if (pool_quota && pool_quota->enabled) {
-    pool_usage_kernel<<<1, 32, 0, st>>>(t.cpus, t.mem, t.gpus, R, d_pool_usage, d_gf);
-    qf_quota_kernel<<<1, QF_CH, 0, st>>>(qa, *pool_quota, d_pool_usage, d_gf);
-    nl += 2;
+    if (!d_pool_usage) {
+      pool_usage_kernel<<<1, 32, 0, st>>>(t.cpus, t.mem, t.gpus, R, d_quota_usage, d_gf);
+      nl++;
+    }
+    qf_quota_kernel<<<1, QF_CH, 0, st>>>(qa, *pool_quota, d_pool_usage ? d_pool_usage : d_quota_usage, d_gf);
+    nl++;
   }
   if (group_quota && group_usage && group_quota->enabled) {
-    CK(pool, cudaMemcpyAsync(d_pool_usage + 4, group_usage, sizeof(double) * 4, cudaMemcpyHostToDevice, st));
-    qf_quota_kernel<<<1, QF_CH, 0, st>>>(qa, *group_quota, d_pool_usage + 4, d_gf);
+    CK(pool, cudaMemcpyAsync(d_quota_usage + 4, group_usage, sizeof(double) * 4, cudaMemcpyHostToDevice, st));
+    qf_quota_kernel<<<1, QF_CH, 0, st>>>(qa, *group_quota, d_quota_usage + 4, d_gf);
     nl++;
   }
   // at most J survivors: the caller's out_ranked_idx holds J, so no order can make the download overrun it

@@ -1615,6 +1615,10 @@ int32_t state_rank(cook_pool* pool, const char* who, bool offensive, const cook_
   int nl = 0;
   TaskCols dt = {};
   int32_t* pslot = nullptr;
+  // the pool quota's start: the live running rows folded in ascending task id, cook_state_usage's pool total, not
+  // the dense columns' slot order
+  UsageFold pf;
+  const bool pool_fold = pool_quota && pool_quota->enabled && R > 0;
   if (N > 0) {
     int32_t* blk = nullptr;
     CK(pool, carve(S->scratch, st, nullptr, nullptr, [&](Carve& c) {
@@ -1623,9 +1627,15 @@ int32_t state_rank(cook_pool* pool, const char* who, bool offensive, const cook_
       dt.cpus = c.take<double>(N); dt.mem = c.take<double>(N); dt.gpus = c.take<double>(N);
       pslot = c.take<int32_t>(J);
       blk = c.take<int32_t>((size_t)std::max(S->pend.hw, S->run.hw) / CP_BLOCK + 2);
+      if (pool_fold) {
+        pf.R = R; pf.pool = true;
+        pf.take(c, S->run.hw);
+        pf.a.pool_out = c.take<double>(4);
+      }
     }));
     if (R) compact(RunningRows{S->run.d_col, dt}, S->run.hw, nullptr, blk, S->counters, R, st, &nl);
     if (J) compact(PendingRows{S->pend.d_col, dt, pslot, R}, S->pend.hw, nullptr, blk, S->counters + 1, J, st, &nl);
+    if (pool_fold) CK(pool, pf.run(&S, 1, st, &nl));
     CK(pool, cudaGetLastError());
     CK(pool, cudaEventRecord(pool->ev[23], st));
   }
@@ -1633,10 +1643,11 @@ int32_t state_rank(cook_pool* pool, const char* who, bool offensive, const cook_
   RankQueue rq = {};
   const RankOffensive ro{pslot, S->pend.at<int64_t>(P_JID), out_off, out_n_off};
   const int32_t rc = rank_impl(pool, R, J, nullptr, nullptr, &dt, users, pool_quota, group_quota, group_usage, params,
-                               nullptr, &n, nullptr, nullptr, nullptr, &rq, offensive ? &ro : nullptr);
+                               nullptr, &n, nullptr, nullptr, nullptr, &rq, offensive ? &ro : nullptr,
+                               pool_fold ? pf.a.pool_out : nullptr);
   if (rc != COOK_OK) return rc;
   cook_phase_stats& ps = pool->phase[COOK_PHASE_RANK];
-  if (N > 0) ps.ms_device += ev_ms(pool->ev[7], pool->ev[23]);   // the gathering of the live rows
+  if (N > 0) ps.ms_device += ev_ms(pool->ev[7], pool->ev[23]);   // the gathering of the live rows and the pool fold
   if (J > 0) {   // the ranked list as (slot, generation) pairs, while it is still in the pool's arena
     int32_t* q_slot = nullptr; uint32_t* q_gen = nullptr; int64_t* q_jid = nullptr;
     CK(pool, carve(S->queue, st, nullptr, nullptr, [&](Carve& c) {

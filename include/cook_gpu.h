@@ -501,8 +501,10 @@ int32_t cook_state_patch(cook_pool* pool, int32_t n, const int64_t* job_id, cons
 /* cook_rank over the live rows (running = live running tasks, pending = live pending jobs).  The ranked
  * queue stays on the device as the handle's resident queue; out_ranked_job_id[<= #pending] (may be
  * NULL) receives it as job ids, *out_n its length.  Rank is a total order on (user, -priority, start,
- * task id, job id) over unique ids, so the result does not depend on where rows are stored.  Uploads
- * only the user table's rank columns; cook_last_stats(COOK_PHASE_RANK) as after cook_rank.          */
+ * task id, job id) over unique ids, and the pool quota's start value (the pool's running usage) is the
+ * live running rows folded in ascending task id, equal to cook_state_usage's pool total bit for bit, so
+ * the result does not depend on where rows are stored.  Uploads only the user table's rank columns;
+ * cook_last_stats(COOK_PHASE_RANK) as after cook_rank.                                             */
 int32_t cook_state_rank(cook_pool* pool, const cook_user_table* users, const cook_pool_quota* pool_quota,
                         const cook_pool_quota* group_quota, const double* group_usage,
                         const cook_rank_params* params, int64_t* out_ranked_job_id, int32_t* out_n);

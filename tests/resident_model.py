@@ -414,16 +414,23 @@ class Pool:
         return running, jobs, jid, prio, np.array([r["task_id"] for r in rows], np.int64)
 
     # -- the resident calls against the host-table calls --------------------------------------------------------------
-    def check_rank(self, oracle=None):
-        """state_rank, equal to cook_rank on the model's tables (and the oracle's rank)."""
-        q = self.rank()
+    def check_rank(self, oracle=None, **kw):
+        """state_rank, equal to cook_rank on the model's tables (and the oracle's rank).  kw: pool_quota,
+        group_quota, group_usage and params, passed to all three."""
+        q = self.rank(**kw)
         running, pending, _, jid = self.tables()
-        host = self.ref.rank(running if running.n else None, pending, self.users)
+        host = self.ref.rank(running if running.n else None, pending, self.users, **kw)
         assert np.array_equal(q, jid[host["ranked"]]), "resident rank != cook_rank on the same rows"
         if oracle is not None and pending.n:
-            o = oracle.rank(running if running.n else None, pending, self.users)
+            o = oracle.rank(running if running.n else None, pending, self.users, **kw)
             assert np.array_equal(q, jid[o["ranked"]]), "resident rank != oracle"
         return q
+
+    def quota_at(self, queue, key, k):
+        """The pool quota on the last bit of the rank's fold: the `key` requests of the first k jobs of `queue` (job
+        ids) folded on from the model's running usage, itself a left fold in ascending task id."""
+        start = F.left_total([self.run[t][key] for t in sorted(self.run)])
+        return F.left_total([self.pend[j][key] for j in queue[:k]], start)
 
     def check_match(self, offers=None):
         """state_match, equal to cook_match on the model's tables over the live queue, failure counts and the usage

@@ -10,7 +10,9 @@ import pytest
 
 from cook_b200 import abi, traces
 from cook_b200.engine import CookError
-from resident_model import Pool, c2, c3, churn, delta, nb, pool_rows
+import fold_ref as F
+import rank_quota_cases as Q
+from resident_model import START, Pool, c2, c3, churn, delta, drop_all_but, nb, pool_rows
 
 pytestmark = pytest.mark.gpu
 
@@ -49,7 +51,7 @@ def test_equivalence_random_deltas(kind, oracle):
         p.close()
 
 
-def test_layout_independence():
+def test_layout_independence(oracle):
     t = c2(21, cpus=(0.1, 0.5, 1.0, 2.0))           # off the binary grid: the serial folds run
     pend, run = pool_rows(t)
     items = sorted(pend.items())
@@ -69,9 +71,68 @@ def test_layout_independence():
         ma, mb = a.check_match(), b.check_match()
         for k in ("considerable", "assign", "ports", "fail"):
             assert np.array_equal(ma[k], mb[k]), k
+        # a pool quota on the last bit of the running fold: the same cut on both layouts, the oracle's
+        q = qa.tolist()
+        for k in (37, F.QF_CH + 1):
+            at = a.quota_at(q, "cpus", k)
+            for quota, n in ((at, k), (np.nextafter(at, -np.inf), k - 1)):
+                pq = Q.pool_quota("cpus", quota)
+                ra, rb = a.check_rank(oracle, pool_quota=pq), b.check_rank(oracle, pool_quota=pq)
+                assert len(ra) == n and np.array_equal(ra, rb), (k, quota)
+        ma, mb = a.check_match(), b.check_match()
+        for k in ("considerable", "assign", "ports", "fail"):
+            assert np.array_equal(ma[k], mb[k]), k
     finally:
         a.close()
         b.close()
+
+
+def test_pool_quota_through_churn(oracle):
+    """Slot orders that churn leaves: running rows removed and upserted again (they refill the freed slots last in,
+    first out), growth past a capacity doubling, launches into freed running slots.  After every step the rank with
+    a pool quota on the last bit of the model's running fold (off the grid) equals cook_rank's and the oracle's on
+    task-id tables, and the match over that queue equals cook_match's."""
+    c = Q.build("off")
+    run = c["run"]
+    rng = np.random.default_rng(17)
+    order = rng.permutation(len(run))
+    first, later = order[:700], order[700:]          # 700 rows fit the first 1024 slots; 1200 do not
+    p = Pool("quota-churn", drop=drop_all_but("gpus"), users=c["users"], offers=Q.offers(),
+             params=traces.match_params(300))
+    try:
+        def check(k):
+            q = p.check_rank(oracle).tolist()
+            for col in ("cpus", "mem"):
+                at = p.quota_at(q, col, k)
+                for quota, n in ((at, k), (np.nextafter(at, -np.inf), k - 1)):
+                    assert len(p.check_rank(oracle, pool_quota=Q.pool_quota(col, quota))) == n, (col, k, quota)
+            p.check_match()
+
+        def reinsert(n):
+            tids = [int(t) for t in rng.choice(sorted(p.run), n, replace=False)]
+            rows = [p.run[t] for t in tids]
+            p.apply(run_rm=tids)
+            p.apply(run_up=[rows[i] for i in rng.permutation(n)])
+
+        def launch(n, tid0):
+            p.apply(run_rm=[int(t) for t in rng.choice(sorted(p.run), n, replace=False)])
+            jobs = [int(j) for j in rng.choice(sorted(p.pend), n, replace=False)]
+            tids = tid0 + 4 * rng.permutation(n)      # even: the case's task ids are odd
+            p.launch(jobs, tids, START + rng.integers(0, 10 ** 6, n))
+
+        p.apply(up=c["pend"], run_up=[run[i] for i in first])
+        check(37)
+        reinsert(200)
+        check(F.QF_CH)
+        p.apply(run_up=[run[i] for i in later])
+        check(F.QF_CH + 1)
+        launch(150, 2 * 10 ** 7)
+        check(37)
+        reinsert(300)
+        launch(100, 10 ** 8)
+        check(F.QF_CH)
+    finally:
+        p.close()
 
 
 def test_growth_and_compaction():

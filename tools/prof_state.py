@@ -71,6 +71,15 @@ live flags, list ranges and list entries.
   python tools/prof_state.py --audit --pool c2
   python tools/prof_state.py --audit --pool c5 --c5-pool 5
 
+--rank-quota loads the pool's pending jobs and running tasks into a resident handle, on the grid and off it (running
+cpus + 0.1, mem / 3), and times cook_state_rank --reps times each after a warm-up call: without a quota and with a pool
+quota that cuts the queue half way (its start the running usage, folded in ascending task id).  Per kind it prints
+the median and least device time and host wall time, the bytes up and down and the launches; COOK_GPU_LIB names
+another build of the library to time the same calls on.
+
+  python tools/prof_state.py --rank-quota --pool c2
+  python tools/prof_state.py --rank-quota --pool c5 --c5-pool 5
+
 --user-stats loads the pool's pending jobs and running tasks (or, with --c3-group N, config-#3 pools 0 .. N-1 into one
 handle each) and per cycle runs cook_state_user_stats over the handles, users' shares and quotas set around their
 running usage, on the grid and off it (cpus + 0.1, mem / 3).  It prints the call's device time, wall time, bytes and
@@ -663,6 +672,45 @@ def audit_prof(a):
     res.close()
 
 
+def rank_quota_prof(a):
+    t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
+    pc, rc0, users = t["cols"]["pending"], t["cols"]["running"], t["users"]
+    jobs = t["jobs"]
+    J, R = jobs.n, len(rc0["task_id"])
+    print(json.dumps({"card": card(), "pool": a.pool if a.pool == "c2" else f"c5/{a.c5_pool}", "pending": J,
+                      "running": R, "lib": os.environ.get("COOK_GPU_LIB", "in-tree")}), flush=True)
+    pend = dict(pending=Jobs(jobs, pc["priority"], pc["job_id"]).soa(np.arange(J)), pending_priority=pc["priority"],
+                pending_job_id=pc["job_id"])
+    for regime in ("grid", "off"):
+        run = {k: np.asarray(v).copy() for k, v in rc0.items()}
+        if regime == "off":
+            run["cpus"] = run["cpus"] + 0.1
+            run["mem"] = run["mem"] / 3.0
+        e = GpuEngine(pool_name="rank-quota")
+        e.state_apply(abi.make_delta(reset=True, running=abi.make_tasks(**run), **pend))
+        total = e.state_usage(users.n_users)["pool"]
+        q = e.state_rank(users)
+        half = float(np.sum(jobs.col("cpus")[np.searchsorted(pc["job_id"], q[:len(q) // 2])]))
+        pq = abi.make_pool_quota({"count": 1e18, "cpus": total[1] + half, "mem": 1e18, "gpus": 1e18})
+        for kind, kw in (("no_quota", {}), ("pool_quota", dict(pool_quota=pq))):
+            dev, wall = [], []
+            n = 0
+            for rep in range(a.reps + 1):
+                w0 = time.perf_counter()
+                n = len(e.state_rank(users, **kw))
+                w = time.perf_counter() - w0
+                st = e.last_stats(abi.PHASE_RANK)
+                if rep:
+                    dev.append(st["ms_device"])
+                    wall.append(1e3 * w)
+            print(json.dumps({"regime": regime, "kind": kind, "queue": n,
+                              "ms_device_median": round(float(np.median(dev)), 3), "ms_device_min": round(min(dev), 3),
+                              "wall_ms_median": round(float(np.median(wall)), 3), "wall_ms_min": round(min(wall), 3),
+                              "h2d_bytes": st["h2d_bytes"], "d2h_bytes": st["d2h_bytes"],
+                              "n_launches": st["n_launches"]}), flush=True)
+        e.close()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--pool", choices=("c2", "c5"), default="c2")
@@ -682,8 +730,11 @@ def main():
     ap.add_argument("--audit", action="store_true")
     ap.add_argument("--user-stats", action="store_true")
     ap.add_argument("--c3-group", type=int, default=0, help="--user-stats: a quota group of config-#3 pools 0 .. N-1")
-    ap.add_argument("--reps", type=int, default=20, help="--audit: timed calls per kind")
+    ap.add_argument("--rank-quota", action="store_true")
+    ap.add_argument("--reps", type=int, default=20, help="--audit, --rank-quota: timed calls per kind")
     a = ap.parse_args()
+    if a.rank_quota:
+        return rank_quota_prof(a)
     if a.audit:
         return audit_prof(a)
     if a.user_stats:
