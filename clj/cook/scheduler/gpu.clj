@@ -280,6 +280,34 @@
   [handle args]
   (check! handle (apply #(Native/stateRebalanceDerived handle %&) args) "cook_state_rebalance_derived"))
 
+(defn offers-add!
+  "cook_state_offers_add: the offers that arrived since the last cycle (cc/pending-offers), each once, stamped with
+   the cycle's time.  `args` are Native/stateOffersAdd's arguments after the handle."
+  [handle args]
+  (check! handle (apply #(Native/stateOffersAdd handle %&) args) "cook_state_offers_add"))
+
+(defn match-offers!
+  "handle-fenzo-pool's match for a \"gpu\" pool whose offers are resident (cook_state_match_offers): expiry after
+   offer-incubate-time-ms, the merge per hostname, the derived match and the consumption, in one call.  `args` are
+   Native/stateMatchOffers' arguments after the handle; `offer-id->offer` resolves an offer id, `out-gone-id`,
+   `out-gone-fate` and `out-n-gone` are its gone buffers.  Returns {:used {hostname-code [offers]} :expired [offers]
+   :single-shot [offers]}: the caller launches each placement on the :used offers of its host (the match's
+   :leases), declines :expired (the lease reject action, scheduler.clj:2315-2323) and forgets :single-shot."
+  [handle args offer-id->offer ^ByteBuffer out-gone-id ^ByteBuffer out-gone-fate ^ints out-n-gone]
+  (check! handle (apply #(Native/stateMatchOffers handle %&) args) "cook_state_match_offers")
+  (let [ids (.asLongBuffer out-gone-id)
+        gone (for [i (range (aget out-n-gone 0))]
+               [(offer-id->offer (.get ids (int i))) (.get out-gone-fate (int i))])]
+    {:used (->> gone (filter #(= 1 (second %))) (map first) (group-by :hostname-code))
+     :expired (->> gone (filter #(= 2 (second %))) (mapv first))
+     :single-shot (->> gone (filter #(= 3 (second %))) (mapv first))}))
+
+(defn rebalance-offers!
+  "cook_state_rebalance_offers: rebalance-derived! with each host's spare resources (view-incubating-offers) folded
+   from the live offers on the device; the host table's spare columns may be nil."
+  [handle args]
+  (check! handle (apply #(Native/stateRebalanceOffers handle %&) args) "cook_state_rebalance_offers"))
+
 (defn exchange-usage!
   "§8e: after a pool's match round; `comm` from Native/commInit (rank 0's Native/commUniqueId bytes travel
    over Cook's own control plane).  Returns the [world n-pad] table as a DoubleBuffer."

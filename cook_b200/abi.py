@@ -148,6 +148,8 @@ STATS_RUNNING, STATS_WAITING, STATS_STARVED, STATS_WUQ = 0, 1, 2, 3
 USERS_TOTAL, USERS_STARVED, USERS_WUQ, USERS_HUNGRY, USERS_SATISFIED, USERS_N = 0, 1, 2, 3, 4, 5
 
 USAGE_GIVEN, USAGE_DERIVED, USAGE_LAST_MATCH = 0, 1, 2
+# cook_state_match_offers: why an offer left the live set
+OFFER_USED, OFFER_EXPIRED, OFFER_SINGLE_SHOT = 1, 2, 3
 
 
 class ConsiderableParams(C.Structure):
@@ -319,6 +321,10 @@ ARGTYPES = {
     "cook_state_counts_compare": [P_I64, P_I64, P_I32],
     "cook_state_export": [_H, _I32, P_U8, _P(StateSizes), _P(StateRows), _P(StateSizes)],
     "cook_state_queue": [_H, _I32, P_I64, P_I32],
+    "cook_state_offers_add": [_H, _P(OffersSoA), P_I64, P_U8, P_F64, C.c_char_p, P_I32, C.c_int64],
+    "cook_state_match_offers": [_H, C.c_int64, C.c_int64, _P(Groups), _P(UserTable), _P(PoolQuota), _P(MatchParams),
+                                P_I64, P_I32, P_I32, _I32, P_U8, P_I64, P_U8, _I32, P_I32, _P(MatchStats)],
+    "cook_state_rebalance_offers": _STATE_REBALANCE,
     "cook_state_user_stats": [_P(_H), _I32, _P(UserTable), P_U8, P_I64, P_F64, P_F64, P_U8, P_I64, P_F64, P_F64, P_I64,
                               _P(PhaseStats)],
     "cook_last_stats": [_H, _I32, _P(PhaseStats)],

@@ -199,9 +199,9 @@ int32_t rank_impl(cook_pool* pool, int R, int J, const cook_tasks_soa* running, 
 // The running-side inputs of a match or rebalance that the resident state derives on the device after the build:
 // carved, not uploaded.  usage: the users' usage_* as one [4][n_users] block (count, cpus, mem, gpus); run: the
 // offers' run_cpus, run_mem and run_count; cot: the groups' cot_* lists, sized for n_cot entries (carved where
-// the plan reads the lists).
+// the plan reads the lists); spare: a rebalance's has_spare / spare_* per host (carved zeroed).
 struct Derived {
-  bool usage = false, run = false, cot = false;
+  bool usage = false, run = false, cot = false, spare = false;
   int64_t n_cot = 0;
 };
 
@@ -217,6 +217,34 @@ struct JobShape {
   bool job_ids = false;           // carve a job id per row, and report the considerable jobs by job id
   Derived dev;                    // the users', offers' and groups' columns the caller fills on the device
 };
+// match.cu: what a match's plan needs to know about its offers before it carves their columns.  `host`: a host
+// table, uploaded as given (cook_match, cook_state_match).  Null: O VMs in the order the plan tries them (the
+// permutation is the identity), hostname_id[O] uploaded, and the columns flagged here carved for the caller to
+// fill on the device (cook_state_match_offers).  Either way the flags and sizes say which columns the plan has,
+// and they alone pick the matcher kernel.
+struct OfferShape {
+  int O = 0;
+  const cook_offers_soa* host = nullptr;
+  const int32_t* hostname_id = nullptr;
+  bool ports = false, is_k8s = false, location = false, gpu = false, disk = false, max_tasks = false,
+       num_tasks = false, host_start = false, reserved = false;
+  int64_t n_ports = 0, n_gpu = 0, n_disk = 0;   // CSR entries of the port ranges and the gpu and disk maps
+  int n_attr_cols = 0;                          // 0: no attribute matrix
+};
+OfferShape host_offer_shape(const cook_offers_soa* offers);
+// The offer columns of a plan built from an OfferShape without `host`, for the caller to fill (null: not carved).
+struct OfferCols {
+  int32_t* perm;
+  double* cpus; double* mem;
+  int32_t* port_off; int32_t* port_begin; int32_t* port_end;
+  uint8_t* is_k8s; int32_t* location;
+  int32_t* gpu_off; int32_t* gpu_model; double* gpu_count;
+  int32_t* disk_off; int32_t* disk_type; double* disk_space;
+  int32_t* max_tasks; int32_t* num_tasks; int64_t* host_start;
+  int32_t* attr;   // [n_attr_cols][O]
+  uint8_t* reserved;
+};
+
 // The carved rows of a plan whose columns the caller writes: row d is ranked[d] = d.
 // The columns of shape.dev, null where not carved: usage [4][n_users]; run_* [offers->n] by input index;
 // cot_off [n_groups + 1], cot_host / cot_attr [max(1, n_cot)].  What a derivation reads from the plan's uploads:
@@ -230,6 +258,7 @@ struct MatchRows {
   double* run_cpus; double* run_mem; int32_t* run_count;
   int32_t* cot_off; int32_t* cot_host; int32_t* cot_attr;
   const int32_t* hostname_id; const int32_t* attr; const int32_t* gcol;
+  OfferCols oc;   // the offer columns to fill (all null when the shape has a host table)
 };
 // The checks of a match's offers, groups, users, params and sizes, with `who` in the messages.  The offer
 // and group tables are checked when `tables`; `novel` and `grouped`: some job has novel-host or group lists.
@@ -240,7 +269,7 @@ int32_t check_match_inputs(cook_pool* pool, const char* who, const cook_offers_s
 // The pool's match plan is built for n_ranked rows of the jobs `sh` describes (ranked_idx: uploaded, null:
 // the caller writes *rows before the run), then run.  A failed build leaves no valid plan.
 int32_t match_build(cook_pool* pool, const int32_t* ranked_idx, int32_t n_ranked, const JobShape& sh,
-                    const cook_offers_soa* offers, const cook_groups* groups, const cook_user_table* users,
+                    const OfferShape& osh, const cook_groups* groups, const cook_user_table* users,
                     const cook_pool_quota* pool_quota, const cook_match_params* params, int32_t max_ports,
                     MatchRows* rows);
 int32_t match_run(cook_pool* pool, int32_t* out_considerable, int64_t* out_job_id, int32_t* out_assign,
@@ -285,7 +314,7 @@ struct RebShape {
   const int64_t* job_id = nullptr;
   const int32_t* priority = nullptr;
   int64_t n_novel = 0, n_attr = 0, n_group = 0;   // caller-written rows: entries each list may hold (0: no list)
-  Derived dev;                                    // caller-written rows: only .cot applies
+  Derived dev;                                    // caller-written rows: .cot and .spare apply
 };
 // The carved rows a caller writes before the run: running task r < R (host: index into the host table) and
 // pending job p < P, with the pending lists the shape asked for.
@@ -299,6 +328,7 @@ struct RebRows {
   const int32_t* attr;          // its [n_attr_cols][hosts->n] attribute matrix (null: none uploaded)
   const int32_t* gcol;          // the groups' attr_col, uploaded (null: none)
   int32_t* cot_off; int32_t* cot_host; int32_t* cot_attr;   // sh.dev.cot and the walk reads the lists, else null
+  uint8_t* has_spare; double* spare_cpus; double* spare_mem; double* spare_gpus;   // sh.dev.spare, else null
 };
 struct RebPlan;
 struct RebPlanFree { void operator()(RebPlan* p) const; };

@@ -2382,20 +2382,45 @@ static T* job_col(Carve& c, const JobShape& sh, const T* col, size_t n) {
   return d;
 }
 
+OfferShape host_offer_shape(const cook_offers_soa* offers) {
+  OfferShape s;
+  const int O = offers->n;
+  s.O = O;
+  s.host = offers;
+  s.hostname_id = offers->hostname_id;
+  s.ports = offers->port_off; s.n_ports = s.ports ? offers->port_off[O] : 0;
+  s.is_k8s = offers->is_k8s; s.location = offers->location;
+  s.gpu = offers->gpu_off; s.n_gpu = s.gpu ? offers->gpu_off[O] : 0;
+  s.disk = offers->disk_off; s.n_disk = s.disk ? offers->disk_off[O] : 0;
+  s.max_tasks = offers->max_tasks; s.num_tasks = offers->num_tasks; s.host_start = offers->host_start_time;
+  s.reserved = offers->reserved;
+  s.n_attr_cols = offers->attr ? offers->n_attr_cols : 0;
+  return s;
+}
+
+// An offer column of the plan: the host table's, uploaded, or carved for the caller when the shape has it.
+template <class T>
+static T* offer_col(Carve& c, const OfferShape& osh, const T* col, bool has, size_t n) {
+  if (osh.host) return c.up(col, n);
+  return has ? c.take<T>(n ? n : 1) : nullptr;
+}
+
 int32_t match_build(cook_pool* pool, const int32_t* ranked_idx, int32_t n_ranked, const JobShape& sh,
-                    const cook_offers_soa* offers, const cook_groups* groups, const cook_user_table* users,
+                    const OfferShape& osh, const cook_groups* groups, const cook_user_table* users,
                     const cook_pool_quota* pool_quota, const cook_match_params* params, int32_t max_ports,
                     MatchRows* rows) {
   cudaStream_t st = pool->stream;
   MatchPlan* mp = plan_of(pool);
   Arena& ar = mp->arena;
   const JobDev& jc = sh.cols;
-  const int J = sh.J, O = offers->n, U = users->n_users, NC = params->num_considerable;
+  const int J = sh.J, O = osh.O, U = users->n_users, NC = params->num_considerable;
+  const cook_offers_soa none = {};
+  const cook_offers_soa* offers = osh.host ? osh.host : &none;
   mp->valid = false;
-  // host-side prep: offers sorted by hostname rank (tie-break order)
-  std::vector<int32_t> perm(O, -1);
+  // host-side prep: offers sorted by hostname rank (tie-break order); without a host table the VMs come in it
+  std::vector<int32_t> perm(osh.host ? O : 0, -1);
   bool dense = true;  // name_rank is normally a permutation of 0..O-1: invert it directly
-  for (int i = 0; i < O && dense; i++) {
+  for (int i = 0; i < (int)perm.size() && dense; i++) {
     const int32_t r = offers->name_rank[i];
     if (r < 0 || r >= O || perm[r] >= 0) dense = false; else perm[r] = i;
   }
@@ -2411,8 +2436,8 @@ int32_t match_build(cook_pool* pool, const int32_t* ranked_idx, int32_t n_ranked
   // The cpu+mem-only kernel is used when no constraint column can affect a
   // placement (all-zero ports/gpus columns count as absent).
   const bool constr_eff = jc.novel_off || jc.gpu_model || jc.disk_request || jc.attr_off || jc.est_end_ms ||
-                          jc.ckpt_location || jc.reserved_host || grouped || offers->is_k8s || offers->max_tasks ||
-                          offers->reserved || offers->gpu_off || sh.any_gpus_ports;
+                          jc.ckpt_location || jc.reserved_host || grouped || osh.is_k8s || osh.max_tasks ||
+                          osh.reserved || osh.gpu || sh.any_gpus_ports;
 
   // blocks: B jobs at the start, then sized by the resolver to ~btarget placements per block
   int B = 64, bmin = 64, bmax = MAXB, btarget = 32;
@@ -2439,7 +2464,8 @@ int32_t match_build(cook_pool* pool, const int32_t* ranked_idx, int32_t n_ranked
   memset(&of, 0, sizeof(of));
   memset(&gr, 0, sizeof(gr));
   of.O = O;
-  of.n_attr_cols = offers->attr ? offers->n_attr_cols : 0;
+  of.n_attr_cols = osh.n_attr_cols;
+  OfferCols oc = {};
   mp->h2d_bytes = 0;
   const cudaError_t carved = carve(ar, st, nullptr, &mp->h2d_bytes, [&](Carve& c) {
     ranked = c.take<int32_t>(n_ranked ? n_ranked : 1);
@@ -2474,38 +2500,49 @@ int32_t match_build(cook_pool* pool, const int32_t* ranked_idx, int32_t n_ranked
     mp->d_job_id = sh.job_ids ? c.take<int64_t>(J + 1) : nullptr;
     mp->d_cons_jid = sh.job_ids ? c.take<int64_t>(NC + 1) : nullptr;
 
-    mp->d_perm = c.up(perm.data(), O); of.perm = mp->d_perm;
-    mp->d_oc = c.up(offers->cpus, O); mp->d_om = c.up(offers->mem, O);
+    mp->d_perm = offer_col(c, osh, perm.data(), true, O); of.perm = mp->d_perm;
+    mp->d_oc = offer_col(c, osh, offers->cpus, true, O); mp->d_om = offer_col(c, osh, offers->mem, true, O);
     if (sh.dev.run) {
       mp->d_orc = c.take<double>(O ? O : 1); mp->d_orm = c.take<double>(O ? O : 1);
     } else {
       mp->d_orc = c.up(offers->run_cpus, O); mp->d_orm = c.up(offers->run_mem, O);
     }
     mp->d_vs = c.take<VmStatic>(O + 1); of.vs = mp->d_vs;
-    of.hostname_id = c.up(offers->hostname_id, O);
+    of.hostname_id = c.up(osh.hostname_id, O);
     of.run_count = sh.dev.run ? c.take<int32_t>(O ? O : 1) : c.up(offers->run_count, O);
     mp->d_ports_total = nullptr;
-    if (offers->port_off) {
-      const int np = std::max(1, offers->port_off[O]);
-      of.port_off = c.up(offers->port_off, O + 1);
-      of.port_begin = c.up(offers->port_begin, np); of.port_end = c.up(offers->port_end, np);
+    if (osh.ports) {
+      const int np = std::max<int64_t>(1, osh.n_ports);
+      of.port_off = offer_col(c, osh, offers->port_off, true, O + 1);
+      of.port_begin = offer_col(c, osh, offers->port_begin, true, np);
+      of.port_end = offer_col(c, osh, offers->port_end, true, np);
       mp->d_ports_total = c.take<int32_t>(O + 1); of.ports_total = mp->d_ports_total;
     }
-    of.is_k8s = c.up(offers->is_k8s, O); of.reserved = c.up(offers->reserved, O);
-    of.location = c.up(offers->location, O);
-    if (offers->gpu_off) {
-      const int ng = std::max(1, offers->gpu_off[O]);
-      of.gpu_off = c.up(offers->gpu_off, O + 1);
-      of.gpu_model = c.up(offers->gpu_model, ng); of.gpu_count = c.up(offers->gpu_count, ng);
+    of.is_k8s = offer_col(c, osh, offers->is_k8s, osh.is_k8s, O);
+    of.reserved = offer_col(c, osh, offers->reserved, osh.reserved, O);
+    of.location = offer_col(c, osh, offers->location, osh.location, O);
+    if (osh.gpu) {
+      const int ng = std::max<int64_t>(1, osh.n_gpu);
+      of.gpu_off = offer_col(c, osh, offers->gpu_off, true, O + 1);
+      of.gpu_model = offer_col(c, osh, offers->gpu_model, true, ng);
+      of.gpu_count = offer_col(c, osh, offers->gpu_count, true, ng);
     }
-    if (offers->disk_off) {
-      const int nd = std::max(1, offers->disk_off[O]);
-      of.disk_off = c.up(offers->disk_off, O + 1);
-      of.disk_type = c.up(offers->disk_type, nd); of.disk_space = c.up(offers->disk_space, nd);
+    if (osh.disk) {
+      const int nd = std::max<int64_t>(1, osh.n_disk);
+      of.disk_off = offer_col(c, osh, offers->disk_off, true, O + 1);
+      of.disk_type = offer_col(c, osh, offers->disk_type, true, nd);
+      of.disk_space = offer_col(c, osh, offers->disk_space, true, nd);
     }
-    of.max_tasks = c.up(offers->max_tasks, O); of.num_tasks = c.up(offers->num_tasks, O);
-    of.host_start = c.up(offers->host_start_time, O);
-    if (of.n_attr_cols > 0) of.attr = c.up(offers->attr, (size_t)of.n_attr_cols * O);
+    of.max_tasks = offer_col(c, osh, offers->max_tasks, osh.max_tasks, O);
+    of.num_tasks = offer_col(c, osh, offers->num_tasks, osh.num_tasks, O);
+    of.host_start = offer_col(c, osh, offers->host_start_time, osh.host_start, O);
+    if (of.n_attr_cols > 0) of.attr = offer_col(c, osh, offers->attr, true, (size_t)of.n_attr_cols * O);
+    if (!osh.host)
+      oc = OfferCols{mp->d_perm, mp->d_oc, mp->d_om, writable(of.port_off), writable(of.port_begin),
+                     writable(of.port_end), writable(of.is_k8s), writable(of.location), writable(of.gpu_off),
+                     writable(of.gpu_model), writable(of.gpu_count), writable(of.disk_off), writable(of.disk_type),
+                     writable(of.disk_space), writable(of.max_tasks), writable(of.num_tasks),
+                     writable(of.host_start), writable(of.attr), writable(of.reserved)};
     mp->d_vc = c.take<VmCons>(O + 1);
     mp->d_attr_v = c.take<int32_t>((size_t)of.n_attr_cols * O + 1);
     of.vc = mp->d_vc; of.attr_v = mp->d_attr_v;
@@ -2615,7 +2652,7 @@ int32_t match_build(cook_pool* pool, const int32_t* ranked_idx, int32_t n_ranked
     *rows = MatchRows{jb, ranked, mp->d_job_id, usage, run ? mp->d_orc : nullptr, run ? mp->d_orm : nullptr,
                       run ? writable(of.run_count) : nullptr, cot ? writable(gr.cot_off) : nullptr,
                       cot ? writable(gr.cot_host) : nullptr, cot ? writable(gr.cot_attr) : nullptr, of.hostname_id,
-                      of.attr, gr.attr_col};
+                      of.attr, gr.attr_col, oc};
   }
   return COOK_OK;
 }
@@ -2964,7 +3001,8 @@ extern "C" int32_t cook_match(cook_pool* pool, const int32_t* ranked_idx, int32_
     JobShape sh;
     rc = host_shape(pool, jobs, groups ? groups->n_groups : 0, &sh);
     if (rc == COOK_OK)
-      rc = match_build(pool, ranked_idx, n_ranked, sh, offers, groups, users, pool_quota, params, max_ports, nullptr);
+      rc = match_build(pool, ranked_idx, n_ranked, sh, host_offer_shape(offers), groups, users, pool_quota, params,
+                       max_ports, nullptr);
     if (rc != COOK_OK) return rc;
   }
   return match_run(pool, out_considerable, nullptr, out_assign, out_ports, out_fail_reason, out_stats, !reuse,

@@ -1073,8 +1073,11 @@ static int32_t build(cook_pool* pool, const RebShape& sh, const cook_host_table*
     q.d_qg = c.up(users->quota_gpus, U);
 
     hc.hostname_id = c.up(hosts->hostname_id, H); hc.name_rank = c.up(hosts->name_rank, H);
-    hc.has_spare = c.part(hosts->has_spare, H, H + 1, true); hc.spare_cpus = c.part(hosts->spare_cpus, H, H + 1, true);
-    hc.spare_mem = c.part(hosts->spare_mem, H, H + 1, true); hc.spare_gpus = c.part(hosts->spare_gpus, H, H + 1, true);
+    const bool ds = sh.dev.spare;   // derived by the caller on the device: carved zeroed, not uploaded
+    hc.has_spare = c.part(ds ? nullptr : hosts->has_spare, H, H + 1, true);
+    hc.spare_cpus = c.part(ds ? nullptr : hosts->spare_cpus, H, H + 1, true);
+    hc.spare_mem = c.part(ds ? nullptr : hosts->spare_mem, H, H + 1, true);
+    hc.spare_gpus = c.part(ds ? nullptr : hosts->spare_gpus, H, H + 1, true);
     hc.is_k8s = c.up(hosts->is_k8s, H);
     hc.location = c.up(hosts->location, H);
     if (hosts->gpu_off) {
@@ -1336,6 +1339,11 @@ int32_t rebalance_build(cook_pool* pool, const RebShape& sh, const cook_host_tab
   rows->cot_off = cot ? writable(q.gc.cot_off) : nullptr;
   rows->cot_host = cot ? writable(q.gc.cot_host) : nullptr;
   rows->cot_attr = cot ? writable(q.gc.cot_attr) : nullptr;
+  const bool sp = sh.dev.spare;
+  rows->has_spare = sp ? q.hc.has_spare : nullptr;
+  rows->spare_cpus = sp ? q.hc.spare_cpus : nullptr;
+  rows->spare_mem = sp ? q.hc.spare_mem : nullptr;
+  rows->spare_gpus = sp ? q.hc.spare_gpus : nullptr;
   return COOK_OK;
 }
 

@@ -44,8 +44,19 @@ enum RCol { R_USER, R_PRIO, R_START, R_TID, R_JID, R_CPUS, R_MEM, R_GPUS, R_HOST
             R_GOFF, R_GLEN, R_NCOL };
 constexpr int R_SZ[R_NCOL] = {4, 4, 8, 8, 8, 8, 8, 8, 4, 1, 4, 4, 4};
 
+// The live offers (leases): one row per offer as it arrived, before any merge.  Data columns first, then the live
+// flag and generation, then the (off, len) pairs of the offer's four lists.
+enum OCol {
+  O_CODE, O_CPUS, O_MEM, O_GPUS, O_K8S, O_LOC, O_MAXT, O_NUMT, O_START, O_SEQ, O_NDATA,
+  O_LIVE = O_NDATA, O_GEN, O_POFF, O_PLEN, O_GOFF, O_GLEN, O_DOFF, O_DLEN, O_AOFF, O_ALEN, O_NCOL
+};
+constexpr int O_SZ[O_NCOL] = {4, 8, 8, 8, 1, 4, 4, 4, 8, 8, 1, 4, 4, 4, 4, 4, 4, 4, 4, 4};
+
 // the pending rows' three lists, then the running rows' group list
 enum { L_NOVEL = 0, L_ATTR = 1, L_GROUP = 2, L_RGROUP = 3, L_N };
+// the offers' port ranges (begin, end), gpu map (model, count), disk map (type, MiB) and attribute values (one per
+// column of the offer's row)
+enum { OL_PORT = 0, OL_GPU = 1, OL_DISK = 2, OL_ATTR = 3, OL_N };
 
 // ---- scatter: row i of a batch to slot[i].  Upserts write the columns (a null source writes the
 // column's absent value) and the rows' list ranges; removals clear the live flag.  Both bump the
@@ -59,10 +70,10 @@ struct ScatterArgs {
   const int32_t* slot;
   uint8_t* live;           // null: a patch
   uint32_t* gen;
-  int32_t* loff[3];        // per-slot list range; null: the table has no lists
-  int32_t* llen[3];
-  const int32_t* doff[3];  // the batch's CSR offsets (null: empty lists)
-  int32_t tail[3];         // where the batch's lists were appended
+  int32_t* loff[4];        // per-slot list range; null: the table has no lists
+  int32_t* llen[4];
+  const int32_t* doff[4];  // the batch's CSR offsets (null: empty lists)
+  int32_t tail[4];         // where the batch's lists were appended
 };
 
 __global__ void scatter_kernel(ScatterArgs a) {
@@ -81,7 +92,7 @@ __global__ void scatter_kernel(ScatterArgs a) {
   a.live[s] = a.upsert ? 1 : 0;
   a.gen[s] += 1u;
 #pragma unroll
-  for (int l = 0; l < 3; l++)
+  for (int l = 0; l < 4; l++)
     if (a.loff[l]) {
       const bool has = a.upsert && a.doff[l];
       const int o = has ? a.doff[l][i] : 0;
@@ -125,8 +136,9 @@ struct RowLen {    // the match's row p is slot m_slot[p]
 };
 
 // warp per live slot: its list moves to the exclusive scan of the live lengths in the new arena
+template <class T1>
 __global__ void list_compact_kernel(OrderScan<int, 1> os, const uint8_t* live, int32_t* off, const int32_t* len, int n,
-                                    const int32_t* src0, const int32_t* src1, int32_t* dst0, int32_t* dst1) {
+                                    const int32_t* src0, const T1* src1, int32_t* dst0, T1* dst1) {
   const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (w >= n || !live[w]) return;
   const int l = len[w], start = os.at(0, w) - l, o = off[w];
@@ -154,9 +166,10 @@ __global__ void launch_lists_kernel(OrderScan<int, 1> os, const int32_t* pslot, 
 }
 
 // warp per match row: the row's list into the dense CSR (doff[n + 1], values) cook_match reads
+template <class T1>
 __global__ void csr_gather_kernel(OrderScan<int, 1> os, const int32_t* m_slot, int n, const int32_t* off,
-                                  const int32_t* len, const int32_t* src0, const int32_t* src1, int32_t* doff,
-                                  int32_t* dst0, int32_t* dst1) {
+                                  const int32_t* len, const int32_t* src0, const T1* src1, int32_t* doff,
+                                  int32_t* dst0, T1* dst1) {
   const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (w >= n) return;
   const int s = m_slot[w], l = len[s], end = os.at(0, w), start = end - l, o = off[s];
@@ -560,7 +573,8 @@ struct Table {
   void* col[P_NCOL] = {};
   void** d_col = nullptr;        // the column pointers on the device (for the gather kernels)
   int32_t cap = 0, hw = 0;       // slots allocated, slots ever used
-  int nlist = 0, lcol[3] = {};   // the per-slot (off, len) column pairs of the table's lists: off at lcol[l]
+  int nlist = 0, lcol[4] = {};   // the per-slot (off, len) column pairs of the table's lists: off at lcol[l]
+  int live_col = 0;
   std::unordered_map<int64_t, int32_t> slot_of;
   std::vector<int32_t> free;
 
@@ -606,6 +620,7 @@ struct Table {
 
 struct ListArena {
   int k = 1;                      // value arrays: 2 for (attribute column, value)
+  int esz1 = 4;                   // bytes per entry of v[1]: 8 when it holds doubles (an offer's gpu or disk map)
   int32_t* v[2] = {};
   int32_t* alt[2] = {};           // compaction target, same capacity
   int64_t cap = 0, tail = 0, live = 0;
@@ -614,8 +629,9 @@ struct ListArena {
     const int64_t ncap = std::max<int64_t>(n, std::max<int64_t>(2 * cap, 4096));
     for (int i = 0; i < k; i++) {
       int32_t* p = nullptr;
-      cudaError_t e = cudaMalloc(&p, sizeof(int32_t) * ncap);
-      if (e == cudaSuccess && tail) e = cudaMemcpyAsync(p, v[i], sizeof(int32_t) * tail, cudaMemcpyDeviceToDevice, st);
+      const size_t es = i ? esz1 : sizeof(int32_t);
+      cudaError_t e = cudaMalloc(&p, es * ncap);
+      if (e == cudaSuccess && tail) e = cudaMemcpyAsync(p, v[i], es * tail, cudaMemcpyDeviceToDevice, st);
       if (e == cudaSuccess) e = cudaStreamSynchronize(st);
       if (e != cudaSuccess) { if (p) cudaFree(p); return e; }
       if (v[i]) cudaFree(v[i]);
@@ -637,12 +653,38 @@ void count_add(std::map<int32_t, int64_t>& m, int32_t code, int64_t d) {
 }
 int32_t count_max(const std::map<int32_t, int64_t>& m) { return m.empty() ? -1 : m.rbegin()->first; }
 
+// What the host keeps of one live offer, by offer slot.
+struct OfferInfo {
+  int64_t id = 0, seq = 0, received = 0;
+  int32_t code = 0;
+  int32_t len[4] = {0, 0, 0, 0};   // ports, gpu map, disk map, attribute columns
+  bool single_shot = false, k8s = false, max_tasks = false;
+};
+// A hostname code: its name, and its live offers in arrival order (seq, slot).  A code with a live offer is a VM.
+struct OfferHost {
+  std::string name;
+  std::map<int64_t, int32_t> live;
+};
+
 struct PoolState {
   Table pend, run;
+  // ---- the live offers (cook_state_offers_add, cook_state_match_offers)
+  Table offer;
+  std::vector<OfferInfo> oinfo;                  // by offer slot
+  std::unordered_map<int32_t, OfferHost> ohost;  // by hostname code, every code the handle has a name for
+  std::map<std::string, int32_t> code_of_name;   // every name the handle knows (byte order)
+  std::map<std::string, int32_t> vm_names;       // the names of the VMs (hosts with a live offer), in byte order
+  std::map<std::pair<int64_t, int64_t>, int32_t> by_time;   // (received, seq) -> slot: expiry walks this
+  std::map<int64_t, int32_t> single_shot;        // seq -> slot of the live single-shot offers
+  std::map<int32_t, int64_t> owidth;             // attribute-row width -> live offers
+  int64_t next_seq = 0;
+  int64_t o_ports = 0;                           // port ranges over the live offers
+  int64_t vm_gpu = 0, vm_disk = 0, vm_k8s = 0, vm_maxt = 0;   // over the VMs' newest offers: map entries, flags
   std::vector<PendingInfo> pinfo;    // by pending slot
   std::vector<int32_t> ruser, rhost; // by running slot
   std::vector<std::vector<int32_t>> rgroups;   // by running slot: its group list
   ListArena lists[L_N];
+  ListArena olists[OL_N];
   std::map<int32_t, int64_t> users_p, users_r, attr_cols, groups;   // code -> live uses
   std::map<int32_t, int64_t> hosts_r;                               // running rows' hostname codes (-1 too)
   std::map<int32_t, int64_t> groups_r;                              // running rows' group codes
@@ -652,6 +694,7 @@ struct PoolState {
   Arena stage;                        // one batch's uploads
   Arena scratch;                      // one call's device buffers
   Arena derive;                       // a derived match's or rebalance's running-side scratch (scratch is live then)
+  Arena omerge;                       // a match's merge of the live offers
   Arena queue;                        // the ranked queue, carved by rank only: it lives until the match
   int32_t* counters = nullptr;        // [0] running rows, [1] pending rows, [2] live queue entries
   GridFlag* gf0 = nullptr;            // stays zero: integer scans are always exact
@@ -664,12 +707,19 @@ struct PoolState {
     run.ncol = R_NCOL; run.sz = R_SZ;
     pend.nlist = 3; pend.lcol[L_NOVEL] = P_NOFF; pend.lcol[L_ATTR] = P_AOFF; pend.lcol[L_GROUP] = P_GOFF;
     run.nlist = 1; run.lcol[0] = R_GOFF;
+    pend.live_col = P_LIVE; run.live_col = R_LIVE;
+    offer.ncol = O_NCOL; offer.sz = O_SZ; offer.live_col = O_LIVE;
+    offer.nlist = 4;
+    for (int l = 0; l < 4; l++) offer.lcol[l] = O_POFF + 2 * l;
     lists[L_ATTR].k = 2;
+    olists[OL_PORT].k = olists[OL_GPU].k = olists[OL_DISK].k = 2;
+    olists[OL_GPU].esz1 = olists[OL_DISK].esz1 = 8;
   }
   void release() {
-    pend.release(); run.release();
+    pend.release(); run.release(); offer.release();
     for (auto& l : lists) l.release();
-    stage.release(); scratch.release(); derive.release(); queue.release();
+    for (auto& l : olists) l.release();
+    stage.release(); scratch.release(); derive.release(); queue.release(); omerge.release();
     if (counters) cudaFree(counters);
     if (gf0) cudaFree(gf0);
   }
@@ -773,26 +823,30 @@ void gather_lists(const PoolState* S, const JobDev& o, const int32_t* m_slot, in
 
 // compaction of every list arena whose dead entries outnumber its live ones
 int32_t compact_lists(cook_pool* pool, PoolState* S, cudaStream_t st, int* nl) {
-  for (int l = 0; l < L_N; l++) {
-    ListArena& A = S->lists[l];
+  for (int l = 0; l < L_N + OL_N; l++) {
+    ListArena& A = l < L_N ? S->lists[l] : S->olists[l - L_N];
     if (A.tail - A.live <= A.live) continue;
-    const bool run = l == L_RGROUP;
-    const Table& t = run ? S->run : S->pend;
-    const int n = t.hw, oc = t.lcol[run ? 0 : l];
+    const Table& t = l == L_RGROUP ? S->run : l >= L_N ? S->offer : S->pend;
+    const int n = t.hw, oc = t.lcol[l == L_RGROUP ? 0 : l >= L_N ? l - L_N : l];
     if (A.live > 0 && n > 0) {
       for (int i = 0; i < A.k; i++)
-        if (!A.alt[i]) CK(pool, cudaMalloc(&A.alt[i], sizeof(int32_t) * std::max<int64_t>(A.cap, 1)));
+        if (!A.alt[i]) CK(pool, cudaMalloc(&A.alt[i], (i ? A.esz1 : sizeof(int32_t)) * std::max<int64_t>(A.cap, 1)));
       OrderScan<int, 1> os;
       CK(pool, carve(S->scratch, st, nullptr, nullptr, [&](Carve& c) {
         os.part[0] = c.take<int32_t>(n);
         os.tile[0] = c.take<int32_t>((n + OS_TILE - 1) / OS_TILE + 1);
       }));
-      const uint8_t* live = static_cast<const uint8_t*>(t.col[run ? (int)R_LIVE : (int)P_LIVE]);
+      const uint8_t* live = static_cast<const uint8_t*>(t.col[t.live_col]);
       int32_t* off = static_cast<int32_t*>(t.col[oc]);
       const int32_t* len = static_cast<const int32_t*>(t.col[oc + 1]);
       order_scan(os, SlotLen{live, len}, n, S->gf0, st, nl);
-      list_compact_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, live, off, len, n, A.v[0], A.v[1], A.alt[0],
-                                                       A.k > 1 ? A.alt[1] : nullptr);
+      if (A.esz1 == 8)
+        list_compact_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, live, off, len, n, A.v[0],
+                                                         reinterpret_cast<const double*>(A.v[1]), A.alt[0],
+                                                         reinterpret_cast<double*>(A.alt[1]));
+      else
+        list_compact_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, live, off, len, n, A.v[0], A.v[1], A.alt[0],
+                                                         A.k > 1 ? A.alt[1] : nullptr);
       (*nl)++;
       CK(pool, cudaGetLastError());
       for (int i = 0; i < A.k; i++) std::swap(A.v[i], A.alt[i]);
@@ -821,6 +875,8 @@ void scatter(ScatterArgs& a, Table& t, int n, int upsert, int live_col, const in
   scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(a);
   (*nl)++;
 }
+
+void offers_drop(PoolState* S);
 
 int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
   const cook_jobs_soa& P = d->pending;
@@ -883,6 +939,8 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
     S->reserved.clear();
     for (auto& f : S->nflag) f = 0;
     for (auto& l : S->lists) l.tail = l.live = 0;
+    if (S->offer.hw) CK(pool, cudaMemsetAsync(S->offer.col[O_LIVE], 0, (size_t)S->offer.hw, st));
+    offers_drop(S);
   }
   std::vector<int32_t> prm_slot(npr), pup_slot(np), rrm_slot(nrr), rup_slot(nr);
   for (int i = 0; i < npr; i++) {
@@ -1537,6 +1595,425 @@ int32_t derive_rebalance(cook_pool* pool, PoolState* S, const RebRows& rows, con
   return COOK_OK;
 }
 
+// ---- the live offers (Fenzo's leases): added once as they arrive, expired, merged per hostname and consumed here
+// the live offers, dense, with their VM (host_of their hostname code) and arrival sequence
+struct OfferRows {
+  void* const* col; const int32_t* host_of; int32_t* vm; int64_t* seq; int32_t* slot;
+  __device__ bool keep(int i) const { return static_cast<const uint8_t*>(col[O_LIVE])[i]; }
+  __device__ void emit(int i, int d) const {
+    slot[d] = i;
+    vm[d] = host_of[static_cast<const int32_t*>(col[O_CODE])[i]];
+    seq[d] = static_cast<const int64_t*>(col[O_SEQ])[i];
+  }
+};
+// position p of the (VM, sequence) order: its slot, and the VMs' segments [start, end)
+__global__ void offer_order_kernel(const int32_t* ord, const int32_t* vm, const int32_t* slot, int n, int32_t* ss,
+                                   int32_t* start, int32_t* end) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n) return;
+  ss[p] = slot[ord[p]];
+  mark_segment(p, n, SortedKey{ord, nullptr, vm}, start, end);
+}
+struct MergeArgs {
+  void* const* col; const int32_t* ss; const int32_t* start; const int32_t* end; int O;
+  OrderScan<int, 1> ports;   // the port ranges' scan over the order (when the plan has ports)
+  const int32_t* attr_arena; // the offers' attribute rows
+  OfferCols oc; int n_attr_cols;
+  int32_t* newest;           // [O] the slot of each VM's newest offer
+};
+// thread per VM: cpus and mem as left folds over its offers in arrival order, every other column from its newest
+__global__ void offer_merge_kernel(MergeArgs a) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= a.O) return;
+  const double* oc = static_cast<const double*>(a.col[O_CPUS]);
+  const double* om = static_cast<const double*>(a.col[O_MEM]);
+  const int s = a.start[v], e = a.end[v];
+  double cpus = 0.0, mem = 0.0;
+  for (int p = s; p < e; p++) {
+    const int i = a.ss[p];
+    cpus = cpus + oc[i];
+    mem = mem + om[i];
+  }
+  const int i = a.ss[e - 1];
+  a.oc.perm[v] = v;
+  a.oc.cpus[v] = cpus;
+  a.oc.mem[v] = mem;
+  a.newest[v] = i;
+  if (a.oc.port_off) {
+    a.oc.port_off[v + 1] = a.ports.at(0, e - 1);
+    if (v == 0) a.oc.port_off[0] = 0;
+  }
+  if (a.oc.is_k8s) a.oc.is_k8s[v] = static_cast<const uint8_t*>(a.col[O_K8S])[i];
+  if (a.oc.location) a.oc.location[v] = static_cast<const int32_t*>(a.col[O_LOC])[i];
+  if (a.oc.max_tasks) a.oc.max_tasks[v] = static_cast<const int32_t*>(a.col[O_MAXT])[i];
+  if (a.oc.num_tasks) a.oc.num_tasks[v] = static_cast<const int32_t*>(a.col[O_NUMT])[i];
+  if (a.oc.host_start) a.oc.host_start[v] = static_cast<const int64_t*>(a.col[O_START])[i];
+  if (a.oc.reserved) a.oc.reserved[v] = 0;
+  const int ao = static_cast<const int32_t*>(a.col[O_AOFF])[i], al = static_cast<const int32_t*>(a.col[O_ALEN])[i];
+  for (int c = 0; c < a.n_attr_cols; c++) a.oc.attr[(size_t)c * a.O + v] = c < al ? a.attr_arena[ao + c] : 0;
+}
+// thread per host of a rebalance's table: the spare resources of its live offers (view-incubating-offers), cpus, mem
+// and the offers' "gpus" as left folds in arrival order; a host without a live offer keeps has_spare 0
+__global__ void offer_spare_kernel(void* const* col, const int32_t* ss, const int32_t* start, const int32_t* end, int H,
+                                   uint8_t* has, double* sc, double* sm, double* sg) {
+  const int h = blockIdx.x * blockDim.x + threadIdx.x;
+  if (h >= H || start[h] >= end[h]) return;
+  const double* oc = static_cast<const double*>(col[O_CPUS]);
+  const double* om = static_cast<const double*>(col[O_MEM]);
+  const double* og = static_cast<const double*>(col[O_GPUS]);
+  double c = 0.0, m = 0.0, g = 0.0;
+  for (int p = start[h]; p < end[h]; p++) {
+    const int i = ss[p];
+    c = c + oc[i];
+    m = m + om[i];
+    g = g + og[i];
+  }
+  has[h] = 1; sc[h] = c; sm[h] = m; sg[h] = g;
+}
+
+// the hosts some live pending row has as reserved_host: pending slots pslot[0, n)
+__global__ void offer_reserved_kernel(const int32_t* pslot, int n, const int32_t* reserved_host, const int32_t* host_of,
+                                      int32_t n_codes, uint8_t* reserved) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const int32_t c = reserved_host[pslot[k]];
+  if (c >= 0 && c < n_codes && host_of[c] >= 0) reserved[host_of[c]] = 1;
+}
+
+// One cook_state_match_offers: the check table it starts from, the VMs and the plan's offer shape after the expiry,
+// the offers that left (slot, fate, sequence), the uploads and launches of the expiry and the consumption.
+struct OfferPass {
+  int64_t now_ms = 0, incubate_ms = 0;
+  int32_t dummy = 0;
+  cook_offers_soa check = {};   // what the checks read before the expiry: no column is uploaded from it
+  std::vector<int32_t> codes;   // the VMs' hostname codes in name order
+  int32_t n_codes = 0;
+  OfferShape osh;
+  std::vector<std::pair<int64_t, std::pair<int64_t, uint8_t>>> gone;   // (seq, (id, fate))
+  int64_t h2d = 0;
+  int nl = 0;
+};
+
+// a hostname code's newest live offer enters (+1) or leaves (-1) the VM counts
+void vm_touch(PoolState* S, OfferHost& h, int64_t sign) {
+  if (h.live.empty()) return;
+  const OfferInfo& oi = S->oinfo[h.live.rbegin()->second];
+  S->vm_gpu += sign * oi.len[OL_GPU];
+  S->vm_disk += sign * oi.len[OL_DISK];
+  S->vm_k8s += sign * (oi.k8s ? 1 : 0);
+  S->vm_maxt += sign * (oi.max_tasks ? 1 : 0);
+}
+
+// offer slot s enters (+1) or leaves (-1) the host-side bookkeeping
+void offer_count(PoolState* S, int32_t s, int64_t sign) {
+  const OfferInfo& oi = S->oinfo[s];
+  OfferHost& h = S->ohost[oi.code];
+  vm_touch(S, h, -1);
+  if (sign > 0) {
+    if (h.live.empty()) S->vm_names.emplace(h.name, oi.code);
+    h.live.emplace(oi.seq, s);
+    S->by_time.emplace(std::make_pair(oi.received, oi.seq), s);
+    if (oi.single_shot) S->single_shot.emplace(oi.seq, s);
+  } else {
+    h.live.erase(oi.seq);
+    if (h.live.empty()) S->vm_names.erase(h.name);
+    S->by_time.erase(std::make_pair(oi.received, oi.seq));
+    S->single_shot.erase(oi.seq);
+  }
+  vm_touch(S, h, +1);
+  S->o_ports += sign * oi.len[OL_PORT];
+  for (int l = 0; l < OL_N; l++) S->olists[l].live += sign * oi.len[l];
+  count_add(S->owidth, oi.len[OL_ATTR], sign);
+}
+
+// slots leave: the host side, then one removal scatter (its upload and launch into *h2d, *nl)
+int32_t offers_remove(cook_pool* pool, PoolState* S, const std::vector<int32_t>& slots, int64_t* h2d, int* nl) {
+  if (slots.empty()) return COOK_OK;
+  for (int32_t s : slots) {
+    offer_count(S, s, -1);
+    S->offer.slot_of.erase(S->oinfo[s].id);
+    S->offer.free.push_back(s);
+  }
+  cudaStream_t st = pool->stream;
+  ScatterArgs a;
+  memset(&a, 0, sizeof(a));
+  CK(pool, carve(S->stage, st, nullptr, h2d, [&](Carve& c) { a.slot = c.up(slots.data(), slots.size()); }));
+  scatter(a, S->offer, (int)slots.size(), 0, O_LIVE, nullptr, st, nl);
+  CK(pool, cudaGetLastError());
+  return COOK_OK;
+}
+
+// drop every live offer (a reset); the names stay known
+void offers_drop(PoolState* S) {
+  for (auto& kv : S->ohost) kv.second.live.clear();
+  S->offer.slot_of.clear(); S->offer.free.clear(); S->offer.hw = 0;
+  S->vm_names.clear(); S->by_time.clear(); S->single_shot.clear(); S->owidth.clear();
+  S->o_ports = S->vm_gpu = S->vm_disk = S->vm_k8s = S->vm_maxt = 0;
+  for (auto& l : S->olists) l.tail = l.live = 0;
+}
+
+int32_t offers_add(cook_pool* pool, PoolState* S, const cook_offers_soa* o, const int64_t* id, const uint8_t* single,
+                   const double* gpus, const char* name, const int32_t* name_off, int64_t now_ms) {
+  const char* who = "cook_state_offers_add";
+  if (!o) return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
+  const int n = o->n;
+  if (n < 0 || o->n_attr_cols < 0) return set_err(pool, COOK_E_BADARG, "%s: bad sizes", who);
+  if (n == 0) {
+    pool->phase[COOK_PHASE_STATE] = {};
+    return COOK_OK;
+  }
+  if (!id || !o->hostname_id || !o->cpus || !o->mem || (o->n_attr_cols > 0 && !o->attr))
+    return set_err(pool, COOK_E_BADARG, "%s: offers need offer_id, hostname_id, cpus and mem", who);
+  const int32_t* gpu_cnt = reinterpret_cast<const int32_t*>(o->gpu_count);
+  const int32_t* disk_sp = reinterpret_cast<const int32_t*>(o->disk_space);
+  if (!csr_ok(o->port_off, n, o->port_begin, o->port_end, true) || !csr_ok(o->gpu_off, n, o->gpu_model, gpu_cnt, true) ||
+      !csr_ok(o->disk_off, n, o->disk_type, disk_sp, true) ||
+      (name_off && !csr_ok(name_off, n, reinterpret_cast<const int32_t*>(name), nullptr, false)))
+    return set_err(pool, COOK_E_BADARG, "%s: malformed CSR offsets", who);
+  // ids, codes and names, all before any change
+  std::unordered_set<int64_t> seen;
+  seen.reserve((size_t)n);
+  std::unordered_map<int32_t, std::string> batch_name;   // code -> name given in this batch
+  std::unordered_map<std::string, int32_t> batch_code;   // name -> code given in this batch
+  for (int i = 0; i < n; i++) {
+    if (!seen.insert(id[i]).second || S->offer.slot_of.count(id[i]))
+      return set_err(pool, COOK_E_BADARG, "%s: an offer id is live already or twice in the batch", who);
+    const int32_t code = o->hostname_id[i];
+    if (code < 0) return set_err(pool, COOK_E_BADARG, "%s: a negative hostname code", who);
+    const int len = name_off ? name_off[i + 1] - name_off[i] : 0;
+    if (!len) continue;
+    const std::string nm(name + name_off[i], (size_t)len);
+    auto h = S->ohost.find(code);
+    auto k = S->code_of_name.find(nm);
+    auto bn = batch_name.find(code);
+    auto bc = batch_code.find(nm);
+    if ((h != S->ohost.end() && h->second.name != nm) || (k != S->code_of_name.end() && k->second != code) ||
+        (bn != batch_name.end() && bn->second != nm) || (bc != batch_code.end() && bc->second != code))
+      return set_err(pool, COOK_E_BADARG, "%s: a hostname code with two names or a name with two codes", who);
+    batch_name.emplace(code, nm);
+    batch_code.emplace(nm, code);
+  }
+  for (int i = 0; i < n; i++) {
+    const int32_t code = o->hostname_id[i];
+    if (!S->ohost.count(code) && !batch_name.count(code))
+      return set_err(pool, COOK_E_BADARG, "%s: a new hostname code without a name", who);
+  }
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  // ---- the host side, O(batch)
+  for (const auto& kv : batch_name) {
+    if (S->ohost.count(kv.first)) continue;
+    S->ohost[kv.first].name = kv.second;
+    S->code_of_name.emplace(kv.second, kv.first);
+  }
+  const int W = o->n_attr_cols;
+  std::vector<int32_t> slot(n);
+  std::vector<int64_t> seq(n);
+  for (int i = 0; i < n; i++) {
+    const int32_t s = S->offer.take_slot();
+    S->offer.slot_of.emplace(id[i], s);
+    if ((size_t)s >= S->oinfo.size()) S->oinfo.resize(std::max<size_t>(s + 1, 2 * S->oinfo.size()));
+    OfferInfo& oi = S->oinfo[s];
+    oi.id = id[i]; oi.seq = seq[i] = S->next_seq++; oi.received = now_ms; oi.code = o->hostname_id[i];
+    oi.len[OL_PORT] = o->port_off ? o->port_off[i + 1] - o->port_off[i] : 0;
+    oi.len[OL_GPU] = o->gpu_off ? o->gpu_off[i + 1] - o->gpu_off[i] : 0;
+    oi.len[OL_DISK] = o->disk_off ? o->disk_off[i + 1] - o->disk_off[i] : 0;
+    oi.len[OL_ATTR] = W;
+    oi.single_shot = single && single[i];
+    oi.k8s = o->is_k8s && o->is_k8s[i];
+    oi.max_tasks = o->max_tasks && o->max_tasks[i] != -1;
+    offer_count(S, s, +1);
+    slot[i] = s;
+  }
+  // the attribute rows, row-major: row i's W values at i * W
+  std::vector<int32_t> attr_rows((size_t)n * W), attr_off(W ? n + 1 : 0);
+  for (int i = 0; i < n && W; i++) {
+    for (int c = 0; c < W; c++) attr_rows[(size_t)i * W + c] = o->attr[(size_t)c * n + i];
+    attr_off[i] = i * W;
+  }
+  if (W) attr_off[n] = n * W;
+  // ---- device: capacity, the upload, the scatter
+  CK(pool, S->offer.grow(S->offer.hw, st));
+  const int32_t* loff[OL_N] = {o->port_off, o->gpu_off, o->disk_off, W ? attr_off.data() : nullptr};
+  const int32_t* lv0[OL_N] = {o->port_begin, o->gpu_model, o->disk_type, attr_rows.data()};
+  const void* lv1[OL_N] = {o->port_end, o->gpu_count, o->disk_space, nullptr};
+  int32_t tail0[OL_N];
+  int64_t nv[OL_N];
+  for (int l = 0; l < OL_N; l++) {
+    ListArena& A = S->olists[l];
+    tail0[l] = (int32_t)A.tail;
+    nv[l] = loff[l] ? loff[l][n] : 0;
+    CK(pool, A.grow(A.tail + nv[l], st));
+    A.tail += nv[l];
+  }
+  ScatterArgs a;
+  memset(&a, 0, sizeof(a));
+  int64_t h2d = 0;
+  CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
+    const void* src[O_NDATA] = {o->hostname_id, o->cpus, o->mem, gpus, o->is_k8s, o->location, o->max_tasks,
+                                o->num_tasks, o->host_start_time, seq.data()};
+    const long long dflt[O_NDATA] = {0, 0, 0, 0, 0, -1, -1, 0, -1, 0};
+    for (int k = 0; k < O_NDATA; k++) {
+      const char* up = nullptr;
+      if (O_SZ[k] == 1) up = reinterpret_cast<const char*>(c.up(static_cast<const uint8_t*>(src[k]), n));
+      else if (O_SZ[k] == 4) up = reinterpret_cast<const char*>(c.up(static_cast<const int32_t*>(src[k]), n));
+      else up = reinterpret_cast<const char*>(c.up(static_cast<const int64_t*>(src[k]), n));
+      a.c[k] = ScatterCol{static_cast<char*>(S->offer.col[k]), up, dflt[k], O_SZ[k]};
+    }
+    a.nc = O_NDATA;
+    a.slot = c.up(slot.data(), n);
+    for (int l = 0; l < OL_N; l++) {
+      a.doff[l] = c.up(loff[l], n + 1);
+      if (!c.base || !nv[l]) continue;
+      ListArena& A = S->olists[l];
+      c.copy(A.v[0] + tail0[l], lv0[l], nv[l]);
+      if (A.k > 1 && A.esz1 == 8)
+        c.copy(reinterpret_cast<double*>(A.v[1]) + tail0[l], static_cast<const double*>(lv1[l]), nv[l]);
+      else if (A.k > 1)
+        c.copy(A.v[1] + tail0[l], static_cast<const int32_t*>(lv1[l]), nv[l]);
+    }
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  int nl = 0;
+  scatter(a, S->offer, n, 1, O_LIVE, tail0, st, &nl);
+  CK(pool, cudaGetLastError());
+  int32_t rc = compact_lists(pool, S, st, &nl);
+  if (rc != COOK_OK) return rc;
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  CK(pool, cudaStreamSynchronize(st));
+  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
+  return COOK_OK;
+}
+
+// step (a) and the plan's offer shape: the offers received incubate_ms or more before now_ms leave, then the VMs are
+// the hostname codes with a live offer, in name order.  Runs after every check of the match.
+int32_t offers_expire(cook_pool* pool, PoolState* S, OfferPass* op, const cook_groups* groups) {
+  std::vector<int32_t> old;
+  for (auto it = S->by_time.begin(); it != S->by_time.end() && op->now_ms - it->first.first >= op->incubate_ms; ++it) {
+    old.push_back(it->second);
+    const OfferInfo& oi = S->oinfo[it->second];
+    op->gone.push_back({oi.seq, {oi.id, (uint8_t)COOK_OFFER_EXPIRED}});
+  }
+  const int32_t rc = offers_remove(pool, S, old, &op->h2d, &op->nl);
+  if (rc != COOK_OK) return rc;
+  op->codes.clear();
+  op->codes.reserve(S->vm_names.size());
+  op->n_codes = 0;
+  for (const auto& kv : S->vm_names) {
+    op->codes.push_back(kv.second);
+    op->n_codes = std::max(op->n_codes, kv.second + 1);
+  }
+  OfferShape& sh = op->osh;
+  sh = OfferShape();
+  sh.O = (int)op->codes.size();
+  sh.hostname_id = op->codes.data();
+  sh.ports = S->o_ports > 0; sh.n_ports = S->o_ports;
+  sh.gpu = S->vm_gpu > 0; sh.n_gpu = S->vm_gpu;
+  sh.disk = S->vm_disk > 0; sh.n_disk = S->vm_disk;
+  sh.is_k8s = S->vm_k8s > 0;
+  sh.max_tasks = S->vm_maxt > 0;
+  sh.location = sh.num_tasks = sh.host_start = true;
+  sh.reserved = S->nflag[F_RESERVED] > 0;
+  int w = std::max<int>(count_max(S->owidth), count_max(S->attr_cols) + 1);
+  for (int g = 0; groups && groups->attr_col && g < groups->n_groups; g++) w = std::max(w, groups->attr_col[g] + 1);
+  sh.n_attr_cols = std::max(w, 0);
+  return COOK_OK;
+}
+
+// step (b): the VMs' columns into the plan's, from the live offers
+int32_t offers_merge(cook_pool* pool, PoolState* S, OfferPass& op, const MatchRows& rows, int* nl) {
+  const int O = op.osh.O, L = (int)S->offer.slot_of.size();
+  if (O == 0) return COOK_OK;
+  cudaStream_t st = pool->stream;
+  const OfferCols& oc = rows.oc;
+  std::vector<int32_t> rslots(S->reserved.begin(), S->reserved.end());
+  int32_t *host_of = nullptr, *vm = nullptr, *slot = nullptr, *ord = nullptr, *tmp = nullptr, *ss = nullptr;
+  int32_t *start = nullptr, *end = nullptr, *blk = nullptr, *ldoff = nullptr, *newest = nullptr, *d_rslots = nullptr;
+  int64_t* seq = nullptr;
+  OrderScan<int, 1> osp, osg, osd;
+  int64_t h2d = 0;
+  CK(pool, carve(S->omerge, st, nullptr, &h2d, [&](Carve& c) {
+    host_of = c.take<int32_t>(op.n_codes);
+    vm = c.take<int32_t>(L); seq = c.take<int64_t>(L); slot = c.take<int32_t>(L);
+    ord = c.take<int32_t>(L); tmp = c.take<int32_t>(L); ss = c.take<int32_t>(L);
+    start = c.take<int32_t>(O); end = c.take<int32_t>(O); newest = c.take<int32_t>(O);
+    blk = c.take<int32_t>((size_t)S->offer.hw / CP_BLOCK + 2);
+    const auto scan = [&](OrderScan<int, 1>& os, int n) {
+      os.part[0] = c.take<int32_t>(n);
+      os.tile[0] = c.take<int32_t>((n + OS_TILE - 1) / OS_TILE + 1);
+    };
+    if (oc.port_off) { scan(osp, L); ldoff = c.take<int32_t>(L + 1); }
+    if (oc.gpu_off) scan(osg, O);
+    if (oc.disk_off) scan(osd, O);
+    if (oc.reserved && !rslots.empty()) d_rslots = c.up(rslots.data(), rslots.size());
+  }));
+  CK(pool, map_hosts(host_of, op.n_codes, rows.hostname_id, O, st, nl));
+  compact(OfferRows{S->offer.d_col, host_of, vm, seq, slot}, S->offer.hw, nullptr, blk, S->counters + 4, L, st, nl);
+  CK(pool, csort::sort_indices(ord, tmp, L, LessKeyTid{vm, seq}, st, nl));
+  offer_order_kernel<<<(L + 255) / 256, 256, 0, st>>>(ord, vm, slot, L, ss, start, end);
+  (*nl)++;
+  const ListArena* A = S->olists;
+  if (oc.port_off) {
+    const int32_t* plen = S->offer.at<int32_t>(O_PLEN);
+    order_scan(osp, RowLen{ss, plen}, L, S->gf0, st, nl);
+    csr_gather_kernel<<<(L + 7) / 8, 256, 0, st>>>(osp, ss, L, S->offer.at<int32_t>(O_POFF), plen, A[OL_PORT].v[0],
+                                                   A[OL_PORT].v[1], ldoff, oc.port_begin, oc.port_end);
+    (*nl)++;
+  }
+  MergeArgs ma = {S->offer.d_col, ss, start, end, O, osp, A[OL_ATTR].v[0], oc, op.osh.n_attr_cols, newest};
+  offer_merge_kernel<<<(O + 127) / 128, 128, 0, st>>>(ma);
+  (*nl)++;
+  const int lists[2] = {OL_GPU, OL_DISK};
+  for (int l : lists) {
+    int32_t* doff = l == OL_GPU ? oc.gpu_off : oc.disk_off;
+    if (!doff) continue;
+    OrderScan<int, 1>& os = l == OL_GPU ? osg : osd;
+    const int32_t* len = S->offer.at<int32_t>(O_POFF + 2 * l + 1);
+    order_scan(os, RowLen{newest, len}, O, S->gf0, st, nl);
+    csr_gather_kernel<<<(O + 7) / 8, 256, 0, st>>>(os, newest, O, S->offer.at<int32_t>(O_POFF + 2 * l), len, A[l].v[0],
+                                                   reinterpret_cast<const double*>(A[l].v[1]), doff,
+                                                   l == OL_GPU ? oc.gpu_model : oc.disk_type,
+                                                   l == OL_GPU ? oc.gpu_count : oc.disk_space);
+    (*nl)++;
+  }
+  if (d_rslots) {
+    const int nr = (int)rslots.size();
+    offer_reserved_kernel<<<(nr + 255) / 256, 256, 0, st>>>(d_rslots, nr, S->pend.at<int32_t>(P_RESERVED), host_of,
+                                                            op.n_codes, oc.reserved);
+    (*nl)++;
+  }
+  CK(pool, cudaGetLastError());
+  op.h2d += h2d;
+  return COOK_OK;
+}
+
+// a rebalance's has_spare / spare_* (rows carved them zeroed) from the live offers, at each host's table index through
+// host_of (every live offer's code is in the table: checked by the caller)
+int32_t offers_spare(cook_pool* pool, PoolState* S, const RebRows& rows, const int32_t* host_of, int H, int* nl) {
+  const int L = (int)S->offer.slot_of.size();
+  if (L == 0) return COOK_OK;
+  cudaStream_t st = pool->stream;
+  int32_t *vm = nullptr, *slot = nullptr, *ord = nullptr, *tmp = nullptr, *ss = nullptr, *start = nullptr;
+  int32_t *end = nullptr, *blk = nullptr;
+  int64_t* seq = nullptr;
+  CK(pool, carve(S->omerge, st, nullptr, nullptr, [&](Carve& c) {
+    vm = c.take<int32_t>(L); seq = c.take<int64_t>(L); slot = c.take<int32_t>(L);
+    ord = c.take<int32_t>(L); tmp = c.take<int32_t>(L); ss = c.take<int32_t>(L);
+    start = c.take<int32_t>(H); end = c.take<int32_t>(H);
+    blk = c.take<int32_t>((size_t)S->offer.hw / CP_BLOCK + 2);
+  }));
+  CK(pool, cudaMemsetAsync(start, 0, sizeof(int32_t) * (size_t)H, st));
+  CK(pool, cudaMemsetAsync(end, 0, sizeof(int32_t) * (size_t)H, st));
+  compact(OfferRows{S->offer.d_col, host_of, vm, seq, slot}, S->offer.hw, nullptr, blk, S->counters + 4, L, st, nl);
+  CK(pool, csort::sort_indices(ord, tmp, L, LessKeyTid{vm, seq}, st, nl));
+  offer_order_kernel<<<(L + 255) / 256, 256, 0, st>>>(ord, vm, slot, L, ss, start, end);
+  offer_spare_kernel<<<(H + 127) / 128, 128, 0, st>>>(S->offer.d_col, ss, start, end, H, rows.has_spare, rows.spare_cpus,
+                                                      rows.spare_mem, rows.spare_gpus);
+  *nl += 2;
+  CK(pool, cudaGetLastError());
+  return COOK_OK;
+}
+
 }  // namespace
 
 extern "C" int32_t cook_state_apply(cook_pool* pool, const cook_state_delta* delta) {
@@ -1677,10 +2154,13 @@ int32_t state_rank(cook_pool* pool, const char* who, bool offensive, const cook_
 
 // cook_state_match, and with `derived` cook_state_match_derived: the users' usage, the offers' run_* and the
 // groups' cot_* lists come from the live running rows, filled on the device into the columns the plan carved
+// With `op` (cook_state_match_offers, derived): the offer table is the live offers merged per hostname after the
+// expiry, which runs once every check has passed; offers is op->check until then.
 int32_t state_match(cook_pool* pool, const char* who, bool derived, const cook_offers_soa* offers,
                     const cook_groups* groups, const cook_user_table* users, const cook_pool_quota* pool_quota,
                     const cook_match_params* params, int64_t* out_considerable_job_id, int32_t* out_assign,
-                    int32_t* out_ports, int32_t max_ports, uint8_t* out_fail_reason, cook_match_stats* out_stats) {
+                    int32_t* out_ports, int32_t max_ports, uint8_t* out_fail_reason, cook_match_stats* out_stats,
+                    OfferPass* op = nullptr) {
   if (!pool) return COOK_E_BADARG;
   if (!offers || !users || !params || !out_considerable_job_id || !out_assign)
     return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
@@ -1724,14 +2204,14 @@ int32_t state_match(cook_pool* pool, const char* who, bool derived, const cook_o
   if (G > 0 && count_max(S->groups) >= G)
     return set_err(pool, COOK_E_BADARG, "%s: a pending row's group code is >= n_groups", who);
   // ---- what the derivation reads, checked from the host-side counts and the offer and group tables
-  const int O = offers->n;
+  int O = offers->n;
   int32_t n_codes = 0;
   if (derived) {
     if (count_max(S->users_r) >= U)
       return set_err(pool, COOK_E_BADARG, "%s: a live running row's user code is >= n_users", who);
     if (n > 0) {
       if (O > 0 && !offers->hostname_id) return set_err(pool, COOK_E_BADARG, "%s: null offers->hostname_id", who);
-      if (!host_codes(offers->hostname_id, O, &n_codes))
+      if (!op && !host_codes(offers->hostname_id, O, &n_codes))
         return set_err(pool, COOK_E_BADARG, "%s: an offers->hostname_id is negative or twice in the table", who);
       if (G > 0) {
         if (count_max(S->groups_r) >= G)
@@ -1749,6 +2229,14 @@ int32_t state_match(cook_pool* pool, const char* who, bool derived, const cook_o
     }
   }
   if (out_stats) memset(out_stats, 0, sizeof(*out_stats));
+  if (op) {
+    CK(pool, cudaSetDevice(pool->device));
+    rc = offers_expire(pool, S, op, groups);
+    if (rc != COOK_OK) return rc;
+    O = op->osh.O;
+    n_codes = op->n_codes;
+    if (n == 0) pool->phase[COOK_PHASE_MATCH] = {};   // this call's own removals are all it reports
+  }
   if (n == 0) return COOK_OK;
   // ---- what the rows hold, from the host-side counts: the resident columns of the kinds some live row
   // holds a non-absent value of
@@ -1782,12 +2270,17 @@ int32_t state_match(cook_pool* pool, const char* who, bool derived, const cook_o
   // ---- the plan, the gathers into the job columns it carved, the derived columns, the run
   CK(pool, cudaEventRecord(pool->ev[0], st));
   MatchRows rows;
-  rc = match_build(pool, nullptr, n, sh, offers, groups, users, pool_quota, params, max_ports, &rows);
+  rc = match_build(pool, nullptr, n, sh, op ? op->osh : host_offer_shape(offers), groups, users, pool_quota, params,
+                   max_ports, &rows);
   if (rc != COOK_OK) return rc;
   fill_rows_kernel<<<(n + 255) / 256, 256, 0, st>>>(rows, S->pend.d_col, m_slot, n);
   nl++;
   gather_lists(S, rows.jb, m_slot, n, os, st, &nl);
   CK(pool, cudaGetLastError());
+  if (op) {
+    rc = offers_merge(pool, S, *op, rows, &nl);
+    if (rc != COOK_OK) return rc;
+  }
   if (derived) {
     rc = derive_match(pool, S, rows, U, O, n_codes, G, groups ? groups->attr_col : nullptr, &nl);
     if (rc != COOK_OK) return rc;
@@ -1802,12 +2295,88 @@ int32_t state_match(cook_pool* pool, const char* who, bool derived, const cook_o
   return COOK_OK;
 }
 
+// cook_state_match_offers: (a) expiry and (b) the merge inside state_match, (c) its match, (d) the consumption
+int32_t match_offers(cook_pool* pool, int64_t now_ms, int64_t incubate_ms, const cook_groups* groups,
+                     const cook_user_table* users, const cook_pool_quota* pool_quota, const cook_match_params* params,
+                     int64_t* out_job_id, int32_t* out_assign, int32_t* out_ports, int32_t max_ports,
+                     uint8_t* out_fail_reason, int64_t* out_gone_id, uint8_t* out_gone_fate, int32_t gone_cap,
+                     int32_t* out_n_gone, cook_match_stats* out_stats) {
+  const char* who = "cook_state_match_offers";
+  if (!pool) return COOK_E_BADARG;
+  if (!users || !params || !out_job_id || !out_assign || !out_gone_id || !out_gone_fate || !out_n_gone)
+    return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
+  if (incubate_ms <= 0) return set_err(pool, COOK_E_BADARG, "%s: incubate_ms <= 0", who);
+  PoolState* S = static_cast<PoolState*>(pool->state);
+  if ((int64_t)gone_cap < (S ? (int64_t)S->offer.slot_of.size() : 0))
+    return set_err(pool, COOK_E_BADARG, "%s: gone_cap < the live offers", who);
+  if (groups && groups->attr_col)
+    for (int g = 0; g < groups->n_groups; g++)
+      if (groups->attr_col[g] < -1) return set_err(pool, COOK_E_BADARG, "%s: groups->attr_col < -1", who);
+  *out_n_gone = 0;
+  OfferPass op;
+  op.now_ms = now_ms; op.incubate_ms = incubate_ms;
+  // the checks read a table as wide as every column a pending row or group names, with a code for every VM
+  op.check.n = S ? (int)S->vm_names.size() : 0;
+  op.check.hostname_id = op.check.name_rank = op.check.attr = &op.dummy;
+  int w = S ? count_max(S->attr_cols) + 1 : 0;
+  for (int g = 0; groups && groups->attr_col && g < groups->n_groups; g++) w = std::max(w, groups->attr_col[g] + 1);
+  op.check.n_attr_cols = w;
+  // the offers that left, in arrival order; also after a failure past the expiry, so no removed offer goes unreported
+  const auto report = [&]() {
+    std::sort(op.gone.begin(), op.gone.end());
+    for (size_t i = 0; i < op.gone.size(); i++) {
+      out_gone_id[i] = op.gone[i].second.first;
+      out_gone_fate[i] = op.gone[i].second.second;
+    }
+    *out_n_gone = (int32_t)op.gone.size();
+  };
+  cook_match_stats ms;
+  int32_t rc = state_match(pool, who, true, &op.check, groups, users, pool_quota, params, out_job_id, out_assign,
+                           out_ports, max_ports, out_fail_reason, &ms, &op);
+  if (rc != COOK_OK) {
+    report();
+    return rc;
+  }
+  // (d) every offer of a host with an assignment, then every remaining single-shot offer
+  std::vector<int32_t> used;
+  std::unordered_set<int32_t> hit;
+  for (int k = 0; k < ms.n_considerable; k++) {
+    if (out_assign[k] < 0) continue;
+    const int32_t code = op.codes[out_assign[k]];
+    out_assign[k] = code;
+    if (!hit.insert(code).second) continue;
+    for (const auto& kv : S->ohost[code].live) {
+      used.push_back(kv.second);
+      op.gone.push_back({kv.first, {S->oinfo[kv.second].id, (uint8_t)COOK_OFFER_USED}});
+    }
+  }
+  for (const auto& kv : S->single_shot) {
+    if (hit.count(S->oinfo[kv.second].code)) continue;
+    used.push_back(kv.second);
+    op.gone.push_back({kv.first, {S->oinfo[kv.second].id, (uint8_t)COOK_OFFER_SINGLE_SHOT}});
+  }
+  cudaStream_t st = pool->stream;
+  rc = offers_remove(pool, S, used, &op.h2d, &op.nl);
+  if (rc == COOK_OK) rc = compact_lists(pool, S, st, &op.nl);
+  if (rc == COOK_OK && cudaStreamSynchronize(st) != cudaSuccess)
+    rc = set_err(pool, COOK_E_CUDA, "%s: %s", who, cudaGetErrorString(cudaGetLastError()));
+  report();
+  if (rc != COOK_OK) return rc;
+  ms.h2d_bytes += op.h2d;
+  ms.n_launches += op.nl;
+  cook_phase_stats& ps = pool->phase[COOK_PHASE_MATCH];
+  ps.h2d_bytes += op.h2d;
+  ps.n_launches += op.nl;
+  if (out_stats) *out_stats = ms;
+  return COOK_OK;
+}
+
 // cook_state_rebalance, and with `derived` cook_state_rebalance_derived: the groups' cot_* lists come from the live
 // running rows over `hosts`, filled on the device into the lists the build carved
 int32_t state_rebalance(cook_pool* pool, const char* who, bool derived, const cook_host_table* hosts,
                         const cook_groups* groups, const cook_user_table* users, const cook_rebalance_params* params,
                         cook_decision* out_decisions, int64_t* out_decision_job_id, int64_t* out_victim_task_id,
-                        int32_t victim_cap, int32_t* out_n) {
+                        int32_t victim_cap, int32_t* out_n, bool offers = false) {
   if (!pool) return COOK_E_BADARG;
   if (!hosts || !users || !params || !out_decisions || !out_decision_job_id || !out_victim_task_id || !out_n)
     return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
@@ -1836,6 +2405,10 @@ int32_t state_rebalance(cook_pool* pool, const char* who, bool derived, const co
   for (const auto& kv : S->hosts_r)
     if (!codes.count(kv.first))
       return set_err(pool, COOK_E_BADARG, "%s: a running row's host is unknown or not in the host table", who);
+  if (offers)
+    for (const auto& kv : S->vm_names)
+      if (!codes.count(kv.second))
+        return set_err(pool, COOK_E_BADARG, "%s: a host with a live offer is not in the host table", who);
   if (std::max(count_max(S->users_p), count_max(S->users_r)) >= users->n_users)
     return set_err(pool, COOK_E_BADARG, "%s: a resident row's user code is >= n_users", who);
   const int G = groups ? groups->n_groups : 0;
@@ -1890,14 +2463,22 @@ int32_t state_rebalance(cook_pool* pool, const char* who, bool derived, const co
   sh.n_novel = S->lists[L_NOVEL].live; sh.n_attr = S->lists[L_ATTR].live; sh.n_group = S->lists[L_GROUP].live;
   sh.dev.cot = derived;
   sh.dev.n_cot = S->cot_n;
+  sh.dev.spare = offers;
   RebPlanPtr plan;
   RebRows rows;
   int32_t rc = rebalance_build(pool, sh, hosts, groups, users, params, &plan, &rows);
   if (rc != COOK_OK) return rc;
   CK(pool, cudaEventRecord(pool->ev[22], st));
-  if (R > 0) {
+  const bool spare = offers && !S->offer.slot_of.empty();
+  if (R > 0 || spare) {
     host_map_kernel<<<(H + 255) / 256, 256, 0, st>>>(rows.hostname_id, H, host_of);
     nl++;
+  }
+  if (spare) {
+    rc = offers_spare(pool, S, rows, host_of, H, &nl);
+    if (rc != COOK_OK) return rc;
+  }
+  if (R > 0) {
     compact(RebRunningRows{RunningRows{S->run.d_col, rows.t}, writable(rows.host), host_of}, S->run.hw, nullptr, blk,
             S->counters, R, st, &nl);
   }
@@ -2195,6 +2776,36 @@ extern "C" int32_t cook_state_match_derived(cook_pool* pool, const cook_offers_s
                                             uint8_t* out_fail_reason, cook_match_stats* out_stats) {
   return state_match(pool, "cook_state_match_derived", true, offers, groups, users, pool_quota, params,
                      out_considerable_job_id, out_assign, out_ports, max_ports, out_fail_reason, out_stats);
+}
+
+extern "C" int32_t cook_state_offers_add(cook_pool* pool, const cook_offers_soa* offers, const int64_t* offer_id,
+                                         const uint8_t* single_shot, const double* offer_gpus, const char* hostname,
+                                         const int32_t* hostname_off, int64_t now_ms) {
+  if (!pool) return COOK_E_BADARG;
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_offers_add: out of device memory");
+  return offers_add(pool, S, offers, offer_id, single_shot, offer_gpus, hostname, hostname_off, now_ms);
+}
+
+extern "C" int32_t cook_state_match_offers(cook_pool* pool, int64_t now_ms, int64_t incubate_ms,
+                                           const cook_groups* groups, const cook_user_table* users,
+                                           const cook_pool_quota* pool_quota, const cook_match_params* params,
+                                           int64_t* out_considerable_job_id, int32_t* out_assign_hostname_id,
+                                           int32_t* out_ports, int32_t max_ports, uint8_t* out_fail_reason,
+                                           int64_t* out_gone_offer_id, uint8_t* out_gone_fate, int32_t gone_cap,
+                                           int32_t* out_n_gone, cook_match_stats* out_stats) {
+  return match_offers(pool, now_ms, incubate_ms, groups, users, pool_quota, params, out_considerable_job_id,
+                      out_assign_hostname_id, out_ports, max_ports, out_fail_reason, out_gone_offer_id, out_gone_fate,
+                      gone_cap, out_n_gone, out_stats);
+}
+
+extern "C" int32_t cook_state_rebalance_offers(cook_pool* pool, const cook_host_table* hosts, const cook_groups* groups,
+                                               const cook_user_table* users, const cook_rebalance_params* params,
+                                               cook_decision* out_decisions, int64_t* out_decision_job_id,
+                                               int64_t* out_victim_task_id, int32_t victim_cap, int32_t* out_n) {
+  return state_rebalance(pool, "cook_state_rebalance_offers", true, hosts, groups, users, params, out_decisions,
+                         out_decision_job_id, out_victim_task_id, victim_cap, out_n, true);
 }
 
 extern "C" int32_t cook_state_rebalance(cook_pool* pool, const cook_host_table* hosts, const cook_groups* groups,

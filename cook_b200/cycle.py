@@ -11,7 +11,9 @@ path end to end.  It computes nothing numeric: every placement decision is `engi
   PoolCycle             handle-resource-offers! (:1339-1535): considerable jobs -> match ->
                         per-cluster launch-rate filter (:887-924) -> matched jobs leave the queue
                         (:790-795) -> reservations released (:1050-1057) -> head-matched feedback
-                        + num-considerable scale-back / reset (handle-fenzo-pool :1613-1651)
+                        + num-considerable scale-back / reset (handle-fenzo-pool :1613-1651); its resident
+                        form takes the offers the library keeps (cook_state_match_offers) and turns the
+                        offers that left into the matches' leases, the declines and the dropped ones
   summarize_failures    fenzo_utils.clj:45-89 shape from cook_match_failures' counters (8f-3)
   resync                the audit of a resident pool fed by deltas: bucket fingerprints compared with the host's,
                         the differing buckets exported, the repairing delta built
@@ -113,6 +115,7 @@ class PoolCycle:
         self.job_reserved_host = {}     # job index -> hostname id
         self.launched_jobs = set()
         self.unmatched_cycles = {}      # job -> consecutive cycles considered but unmatched (:1400-1470)
+        self.offer_host = {}            # resident pools: live offer id -> hostname code
 
     # ---- M6 ------------------------------------------------------------------------------------
     def handle_resource_offers(self, queue, jobs, offers, users, *, num_considerable=None, groups=None,
@@ -174,6 +177,61 @@ class PoolCycle:
         return self._finish(queue, matches, matched_jobs, {mt["offer"] for mt in matches},
                             no_matches or matched_head, len(cons), nc, considerable=[int(c) for c in cons],
                             fail=m["fail"])
+
+    # ---- M5 + M6 for a resident pool: the offers live in the library (cook_state_offers_add / _match_offers) ----
+    def add_offers(self, offers, offer_id, now_ms, **kw):
+        """cook_state_offers_add (engine.state_offers_add's keywords), remembering each offer's hostname code: the
+        match reports the offers that left by id."""
+        self.eng.state_offers_add(offers, offer_id, now_ms, **kw)
+        self.offer_host.update(zip(np.asarray(offer_id).tolist(), offers.col("hostname_id").tolist()))
+
+    def handle_resource_offers_resident(self, now_ms, users, *, num_considerable=None, groups=None, pool_quota=None,
+                                        max_ports=0, host_lifetime_mins=0, enforce_rate_limit=0, cluster_of_host=None,
+                                        cluster_tokens=None, cluster_enforce=None):
+        """One cycle of a resident pool (after its deltas and cook_state_rank): cook_state_match_offers with the
+        pool's incubation time, then the reference's shape of the result.  Returns handle_resource_offers' dict, with
+        job ids for jobs and hostname codes for hosts, where each match is {hostname_id, leases (the USED offer ids of
+        the host, for launch-tasks), jobs, ports}, plus 'decline' (the EXPIRED offer ids: the lease reject action),
+        'dropped' (the SINGLE_SHOT ones) and 'unlaunched' (the leases of the matches the launch-rate filter dropped;
+        they are consumed, so the caller declines them too).  cluster_of_host: hostname code -> compute cluster."""
+        nc = self.num_considerable if num_considerable is None else num_considerable
+        prm = traces.match_params(max(nc, 0), enforce_rate_limit=enforce_rate_limit,
+                                  host_lifetime_mins=host_lifetime_mins)
+        m = self.eng.state_match_offers(now_ms, self.offers.incubate_ms, users, prm, groups=groups,
+                                        pool_quota=pool_quota, max_ports=max_ports)
+        leases, decline, dropped = {}, [], []
+        for oid, fate in m["gone"]:
+            code = self.offer_host.pop(oid)
+            if fate == abi.OFFER_USED:
+                leases.setdefault(code, []).append(oid)
+            elif fate == abi.OFFER_EXPIRED:
+                decline.append(oid)
+            else:
+                dropped.append(oid)
+        cons, assign = m["considerable"], m["assign"]
+        by_host = {}
+        for k in range(len(cons)):
+            if assign[k] >= 0:
+                by_host.setdefault(int(assign[k]), []).append(k)
+        matches = [{"hostname_id": h, "leases": leases[h], "jobs": [int(cons[k]) for k in ks],
+                    "ports": {int(cons[k]): [int(p) for p in m["ports"][k] if p >= 0] for k in ks}}
+                   for h, ks in by_host.items()]
+        unlaunched = []
+        if cluster_of_host is not None and cluster_tokens is not None:   # filter-matches-for-ratelimit (:887-924)
+            def skipped(h):
+                c = cluster_of_host[h]
+                enf = True if cluster_enforce is None else bool(cluster_enforce.get(c, False))
+                return enf and cluster_tokens.get(c, 0) < 0
+            unlaunched = [l for mt in matches if skipped(mt["hostname_id"]) for l in mt["leases"]]
+            matches = [mt for mt in matches if not skipped(mt["hostname_id"])]
+        matched_jobs = {j for mt in matches for j in mt["jobs"]}
+        head = int(cons[0]) if len(cons) else None
+        ok = len(matches) == 0 or (head is not None and head in matched_jobs)
+        r = self._finish(np.zeros(0, np.int32), matches, matched_jobs, {mt["hostname_id"] for mt in matches}, ok,
+                         len(cons), nc, considerable=[int(c) for c in cons], fail=m["fail"])
+        del r["queue"]   # the queue is the resident one: the launches take the matched jobs out of it
+        r.update(decline=decline, dropped=dropped, unlaunched=unlaunched, stats=m["stats"])
+        return r
 
     def _finish(self, queue, matches, matched_jobs, used_offers, ok, n_considerable, nc, considerable=(), fail=None):
         if matches:

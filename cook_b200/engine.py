@@ -157,6 +157,7 @@ class GpuEngine:
         live = getattr(self, "_state_pending_ids", set())
         if delta.reset:
             live = set()
+            self._state_offer_ids = set()
         rm = delta.col("pending_rm_job_id")
         live.difference_update(rm.tolist() if rm is not None else [])
         up = delta.col("pending_job_id")
@@ -382,18 +383,73 @@ class GpuEngine:
                 "ports": ports[:n * max(max_ports, 1)].reshape(n, max(max_ports, 1)).copy(),
                 "fail": fail[:n].copy(), "stats": stats.as_dict()}
 
-    def state_rebalance(self, hosts, users, params, groups=None, derived=False):
+    def state_offers_add(self, offers, offer_id, now_ms, single_shot=None, offer_gpus=None, hostnames=None):
+        """cook_state_offers_add: one row per arriving offer (an abi.OffersSoA, not merged), stamped now_ms.
+        hostnames: each row's hostname (str or bytes; "" or None for a code the handle already knows)."""
+        ids = np.ascontiguousarray(offer_id, np.int64)
+        ss = np.ascontiguousarray(single_shot, np.uint8) if single_shot is not None else None
+        og = np.ascontiguousarray(offer_gpus, np.float64) if offer_gpus is not None else None
+        blob, off = b"", None
+        if hostnames is not None:
+            parts = [h.encode() if isinstance(h, str) else bytes(h or b"") for h in hostnames]
+            blob = b"".join(parts)
+            off = np.zeros(len(parts) + 1, np.int32)
+            off[1:] = np.cumsum([len(b) for b in parts])
+        rc = self.lib.cook_state_offers_add(self.pool, C.byref(offers), abi.ptr(ids, abi.P_I64),
+                                            abi.ptr(ss, abi.P_U8) if ss is not None else None,
+                                            abi.ptr(og, abi.P_F64) if og is not None else None,
+                                            blob or None, abi.ptr(off, abi.P_I32) if off is not None else None,
+                                            C.c_int64(int(now_ms)))
+        if rc != 0:
+            self._err(rc)
+        live = getattr(self, "_state_offer_ids", set())
+        live.update(ids.tolist())
+        self._state_offer_ids = live
+
+    def state_match_offers(self, now_ms, incubate_ms, users, params, groups=None, pool_quota=None, max_ports=0,
+                           gone_cap=None):
+        """cook_state_match_offers: expiry, the merge of the live offers per hostname, the match over the resident
+        queue, the consumption.  'considerable' holds job ids, 'assign' hostname codes (-1: unplaced); 'gone' lists
+        (offer id, fate) in arrival order."""
+        pool_quota = pool_quota or abi.make_pool_quota(None)
+        k = max(params.num_considerable, 1)
+        cons = np.full(k, -1, np.int64)
+        _, assign, ports, fail, stats = _CallShapes.match_buffers(params, max_ports)
+        live = getattr(self, "_state_offer_ids", set())
+        cap = len(live) if gone_cap is None else gone_cap
+        gid = np.full(max(cap, 1), -1, np.int64)
+        gfate = np.zeros(max(cap, 1), np.uint8)
+        ng = C.c_int32(0)
+        rc = self.lib.cook_state_match_offers(self.pool, C.c_int64(int(now_ms)), C.c_int64(int(incubate_ms)),
+                                              C.byref(groups) if groups is not None else None, C.byref(users),
+                                              C.byref(pool_quota), C.byref(params), abi.ptr(cons, abi.P_I64),
+                                              abi.ptr(assign, abi.P_I32),
+                                              abi.ptr(ports, abi.P_I32) if max_ports > 0 else None, int(max_ports),
+                                              abi.ptr(fail, abi.P_U8), abi.ptr(gid, abi.P_I64),
+                                              abi.ptr(gfate, abi.P_U8), int(cap), C.byref(ng), C.byref(stats))
+        if rc != 0:
+            self._err(rc)
+        n = stats.n_considerable
+        gone = list(zip(gid[:ng.value].tolist(), gfate[:ng.value].tolist()))
+        live.difference_update(g for g, _ in gone)
+        return {"considerable": cons[:n].copy(), "assign": assign[:n].copy(),
+                "ports": ports[:n * max(max_ports, 1)].reshape(n, max(max_ports, 1)).copy(),
+                "fail": fail[:n].copy(), "gone": gone, "stats": stats.as_dict()}
+
+    def state_rebalance(self, hosts, users, params, groups=None, derived=False, offers=False):
         """cook_state_rebalance: the rebalancer over the live running tasks and the first allowed jobs of the
         resident queue.  As rebalance(), plus each decision's 'job_id'; 'victims' are task ids (the task
         of the job an earlier decision e placed: -1 - e).  derived: cook_state_rebalance_derived, the groups'
-        cot_* read from the resident running rows over `hosts` on the device (those fields are ignored)."""
+        cot_* read from the resident running rows over `hosts` on the device (those fields are ignored).  offers:
+        cook_state_rebalance_offers, the derived call with the hosts' spare resources from the live offers."""
         mp = max(params.max_preemption, 1)
         dec = (abi.Decision * mp)()
         jid = np.full(mp, -1, np.int64)
         cap = len(getattr(self, "_state_running_ids", ())) + mp
         vict = np.full(cap, -1, np.int64)
         n = C.c_int32(0)
-        fn = self.lib.cook_state_rebalance_derived if derived else self.lib.cook_state_rebalance
+        fn = (self.lib.cook_state_rebalance_offers if offers else
+              self.lib.cook_state_rebalance_derived if derived else self.lib.cook_state_rebalance)
         rc = fn(self.pool, C.byref(hosts), C.byref(groups) if groups is not None else None, C.byref(users),
                 C.byref(params), dec, abi.ptr(jid, abi.P_I64), abi.ptr(vict, abi.P_I64), int(cap), C.byref(n))
         if rc != 0:

@@ -650,6 +650,71 @@ int32_t cook_state_rebalance_derived(cook_pool* pool, const cook_host_table* hos
                                      cook_decision* out_decisions, int64_t* out_decision_job_id,
                                      int64_t* out_victim_task_id, int32_t victim_cap, int32_t* out_n);
 
+/* The live offers: Fenzo's leases (scheduler.clj:617-687, :2301-2324), kept on the device between match cycles.
+ * cook_state_offers_add takes one row per offer as it arrives, not merged: offers->n rows of hostname_id, cpus, mem,
+ * the port CSR, is_k8s, location, the gpu and disk maps, max_tasks, num_tasks, host_start_time and n_attr_cols / attr
+ * (columns past a row's n_attr_cols are absent, 0); name_rank, run_* and reserved are not read.  A NULL column takes
+ * its absent value (is_k8s 0, location -1, max_tasks -1, num_tasks 0, host_start_time -1, empty lists).
+ * offer_id[n] names each offer; single_shot[n] (NULL: none) marks offers that never outlive a match attempt
+ * (Kubernetes, :674-678); offer_gpus[n] is the lease's "gpus" scalar (NULL: 0).  hostname / hostname_off[n + 1]: each
+ * row's hostname bytes as a CSR (NULL hostname_off: all empty); a row may give an empty name when the handle already
+ * knows its code.  Every row is stamped received = now_ms and takes the next arrival number (calls in sequence,
+ * rows in order).
+ * COOK_E_BADARG with nothing changed: an offer id that is live or twice in the batch, a negative code, a new code
+ * without a name, a code whose name differs from the one the handle holds, two codes with one name, a malformed CSR.
+ * cook_state_apply with reset drops the live offers (the names stay known).  Uploads: the non-NULL columns, the
+ * lists with their offsets, 8 bytes (arrival number) plus 4 (slot) per row, and the attribute rows as one more list
+ * (4 * n_attr_cols values and 4 bytes of offset per row); statistics: cook_last_stats(COOK_PHASE_STATE). */
+int32_t cook_state_offers_add(cook_pool* pool, const cook_offers_soa* offers, const int64_t* offer_id,
+                              const uint8_t* single_shot, const double* offer_gpus, const char* hostname,
+                              const int32_t* hostname_off, int64_t now_ms);
+
+/* One Fenzo scheduleOnce over the resident queue and the live offers, in four steps:
+ *   (a) expiry       offers with now_ms - received >= incubate_ms leave, fate COOK_OFFER_EXPIRED.  The boundary is
+ *                    this library's rule (Fenzo's own is not in the reference); a shim converts
+ *                    offer-incubate-time-ms as max(seconds, 1) * 1000.
+ *   (b) merge        one VM per hostname with a live offer, VMs in memcmp order of the hostname bytes (the equal
+ *                    fitness tie-break).  cpus and mem are left folds over the host's offers in arrival order, port
+ *                    ranges concatenated in arrival order, every other column from the host's newest offer.  The
+ *                    attribute matrix is as wide as the widest live offer row, the largest column a pending row
+ *                    names and the largest group attr_col, whichever is largest.  reserved marks the hosts some
+ *                    live pending row has as reserved_host (present when some row has one).  is_k8s, max_tasks and
+ *                    the gpu and disk maps are present when some VM's value is not absent, the port lists when some
+ *                    live offer has a range; location, num_tasks and host_start_time always.
+ *   (c) match        cook_state_match_derived over that table; out_assign_hostname_id gets the VM's hostname code
+ *                    or -1.  cook_match_failures, cook_exchange_usage(_batch) and COOK_USAGE_LAST_MATCH then refer
+ *                    to this round.
+ *   (d) consumption  every offer of a host with an assignment leaves, fate COOK_OFFER_USED; every remaining
+ *                    single-shot offer leaves, fate COOK_OFFER_SINGLE_SHOT.
+ * (a) and (d) also run when no queue row is left.  out_gone_offer_id / out_gone_fate [*out_n_gone]: the offers that
+ * left, in arrival order; gone_cap must be at least the live offers before the call.  An error returned after the
+ * expiry still writes the offers that had left by then.
+ * COOK_E_BADARG before any device work or offer change: every case of cook_state_match_derived, incubate_ms <= 0,
+ * gone_cap too small, a NULL gone output, params->reuse_resident.
+ * Transfers: up = cook_state_match_derived's over the merged table, without that table's columns, plus 4 bytes per VM
+ * (its hostname code), 4 per reserved pending row (when the table has reserved) and 4 per offer that left; down =
+ * cook_state_match_derived's.  Statistics: stats and cook_last_stats(COOK_PHASE_MATCH). */
+enum { COOK_OFFER_USED = 1, COOK_OFFER_EXPIRED = 2, COOK_OFFER_SINGLE_SHOT = 3 };
+int32_t cook_state_match_offers(cook_pool* pool, int64_t now_ms, int64_t incubate_ms, const cook_groups* groups,
+                                const cook_user_table* users, const cook_pool_quota* pool_quota,
+                                const cook_match_params* params, int64_t* out_considerable_job_id,
+                                int32_t* out_assign_hostname_id, int32_t* out_ports, int32_t max_ports,
+                                uint8_t* out_fail_reason, int64_t* out_gone_offer_id, uint8_t* out_gone_fate,
+                                int32_t gone_cap, int32_t* out_n_gone, cook_match_stats* out_stats);
+
+/* cook_state_rebalance_derived with hosts->has_spare / spare_cpus / spare_mem / spare_gpus (not read, may be NULL)
+ * derived from the live offers as view-incubating-offers (scheduler.clj:1537-1546) gives them: has_spare is set for a
+ * host with at least one live offer, and the spare values are left folds in arrival order of its offers' cpus, mem
+ * and offer_gpus.  Nothing expires here (getVmCurrentStates does not expire either); the attributes still come from
+ * the caller's table (the agent-attributes cache).
+ * COOK_E_BADARG, before any device work: every case of cook_state_rebalance_derived, and a host with a live offer
+ * that is not in `hosts`.  Transfers: cook_state_rebalance_derived's minus 25 bytes per host (the spare columns).
+ * Statistics: cook_last_stats(COOK_PHASE_REBALANCE). */
+int32_t cook_state_rebalance_offers(cook_pool* pool, const cook_host_table* hosts, const cook_groups* groups,
+                                    const cook_user_table* users, const cook_rebalance_params* params,
+                                    cook_decision* out_decisions, int64_t* out_decision_job_id,
+                                    int64_t* out_victim_task_id, int32_t victim_cap, int32_t* out_n);
+
 /* M0 over the resident queue without a match: pending-jobs->considerable-jobs (scheduler.clj:729-762; the jobs
  * handle-kubernetes-scheduler-pool :1749-1800 launches) or, with quota_only, filter-pending-jobs-for-quota
  * (tools.clj:961-973; what handle-resource-offers-autoscaling-helper :1283-1335 takes).

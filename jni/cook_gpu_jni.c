@@ -348,6 +348,42 @@ JFN(jint, stateMatchDerived)(JNIEnv* env, jclass k, jlong pool, jint n_offers, j
                      max_ports, out_fail, out_stats);
 }
 
+/* the offers that arrived, one row each (offers in cook_offers_soa field order; name_rank, run_* and reserved are not
+ * read), their ids, single-shot flags, "gpus" scalars and hostname bytes as a CSR (null hostname_off: all empty) */
+JFN(jint, stateOffersAdd)(JNIEnv* env, jclass k, jlong pool, jint n_offers, jint n_attr_cols, jobjectArray offers,
+                          jobject offer_id, jobject single_shot, jobject offer_gpus, jobject hostname,
+                          jobject hostname_off, jlong now_ms) {
+  cook_offers_soa o;
+  memset(&o, 0, sizeof(o));
+  offers_from(env, n_offers, n_attr_cols, offers, &o);
+  return cook_state_offers_add((cook_pool*)(intptr_t)pool, &o, one(env, offer_id), one(env, single_shot),
+                               one(env, offer_gpus), one(env, hostname), one(env, hostname_off), now_ms);
+}
+/* expiry, the merge of the live offers, the derived match, consumption; out_assign gets hostname codes and
+ * out_gone_offer_id / out_gone_fate (gone_cap entries each) the offers that left, their count in out_n_gone[0] */
+JFN(jint, stateMatchOffers)(JNIEnv* env, jclass k, jlong pool, jlong now_ms, jlong incubate_ms, jint n_groups,
+                            jobjectArray groups, jint n_users, jobjectArray users, jdoubleArray pool_quota,
+                            jintArray iparams, jdouble good_enough_fitness, jobject out_considerable_job_id,
+                            jobject out_assign, jobject out_ports, jint max_ports, jobject out_fail,
+                            jobject out_gone_offer_id, jobject out_gone_fate, jint gone_cap, jintArray out_n_gone,
+                            jobject out_stats) {
+  cook_groups g; cook_user_table u; cook_pool_quota pq; cook_match_params prm;
+  memset(&g, 0, sizeof(g)); memset(&u, 0, sizeof(u));
+  int have_g = groups_from(env, n_groups, groups, &g);
+  users_from(env, n_users, users, &u); quota_from(env, pool_quota, &pq);
+  jint ip[6]; (*env)->GetIntArrayRegion(env, iparams, 0, 6, ip);
+  memset(&prm, 0, sizeof(prm));
+  prm.num_considerable = ip[0]; prm.enforce_rate_limit = ip[1]; prm.host_lifetime_mins = ip[2]; prm.fitness_kind = ip[3];
+  prm.good_enough_fitness = good_enough_fitness; prm.reuse_resident = ip[4]; prm.max_ctas = ip[5];
+  int32_t n_gone = 0;
+  jint rc = cook_state_match_offers((cook_pool*)(intptr_t)pool, now_ms, incubate_ms, have_g ? &g : NULL, &u, &pq, &prm,
+                                    one(env, out_considerable_job_id), one(env, out_assign), one(env, out_ports),
+                                    max_ports, one(env, out_fail), one(env, out_gone_offer_id), one(env, out_gone_fate),
+                                    gone_cap, &n_gone, (cook_match_stats*)one(env, out_stats));
+  (*env)->SetIntArrayRegion(env, out_n_gone, 0, 1, (jint*)&n_gone);
+  return rc;
+}
+
 /* the rebalancer over the resident rows; out_victim_task_id holds victim_cap task ids */
 typedef int32_t (*state_rebalance_fn)(cook_pool*, const cook_host_table*, const cook_groups*, const cook_user_table*,
                                       const cook_rebalance_params*, cook_decision*, int64_t*, int64_t*, int32_t, int32_t*);
@@ -384,6 +420,16 @@ JFN(jint, stateRebalanceDerived)(JNIEnv* env, jclass k, jlong pool, jint n_hosts
                                  jobject out_decisions, jobject out_decision_job_id, jobject out_victim_task_id,
                                  jint victim_cap, jintArray out_n) {
   return state_rebalance(cook_state_rebalance_derived, env, pool, n_hosts, n_attr_cols, hosts, n_groups, groups, n_users,
+                         users, max_preemption, min_dru_diff, safe_dru_threshold, host_lifetime_mins, out_decisions,
+                         out_decision_job_id, out_victim_task_id, victim_cap, out_n);
+}
+/* stateRebalanceDerived with the hosts' spare columns derived from the live offers (those columns are not read) */
+JFN(jint, stateRebalanceOffers)(JNIEnv* env, jclass k, jlong pool, jint n_hosts, jint n_attr_cols, jobjectArray hosts,
+                                jint n_groups, jobjectArray groups, jint n_users, jobjectArray users, jint max_preemption,
+                                jdouble min_dru_diff, jdouble safe_dru_threshold, jint host_lifetime_mins,
+                                jobject out_decisions, jobject out_decision_job_id, jobject out_victim_task_id,
+                                jint victim_cap, jintArray out_n) {
+  return state_rebalance(cook_state_rebalance_offers, env, pool, n_hosts, n_attr_cols, hosts, n_groups, groups, n_users,
                          users, max_preemption, min_dru_diff, safe_dru_threshold, host_lifetime_mins, out_decisions,
                          out_decision_job_id, out_victim_task_id, victim_cap, out_n);
 }

@@ -16,6 +16,15 @@ the same rows (the queue's first max_preemption jobs): device time, wall time, b
 
   python tools/prof_state.py --rebalance --c4-pool 0 --cycles 5
 
+--offers feeds one offer stream (40 % of the hosts offer each cycle, some in two or three leases, 15 s incubation)
+to two resident handles holding the same rows: one keeps the offers itself (cook_state_offers_add, then
+cook_state_match_offers), the other gets the host's lease cache (cycle.OfferCache, offers_from_cache, then
+cook_state_match_derived).  Per cycle it prints each arm's wall time, device time and bytes, and whether the
+placements are identical.
+
+  python tools/prof_state.py --offers --cycles 8
+  python tools/prof_state.py --offers --c3-pool 0 --cycles 6
+
 --launch runs the same cycles on two resident handles instead of the host arm.  Each cycle's launches go to one
 handle through cook_state_launch (job ids, task ids, start times, the hosts the match chose) and to its twin through
 the equivalent cook_state_apply batch (the jobs' removal plus their task rows); the rest of the batch goes to both
@@ -535,6 +544,96 @@ def derived_prof(a):
     e.close()
 
 
+def offers_prof(a):
+    """--offers: the same offer stream through the library's live offers (cook_state_offers_add +
+    cook_state_match_offers) and through the host's lease cache (cycle.OfferCache, offers_from_cache and
+    cook_state_match_derived), on two resident handles holding the same rows."""
+    from cook_b200.cycle import OfferCache, offers_from_cache
+    if a.c3_pool >= 0:
+        t, name = traces.gen_config_pool("c3", a.c3_pool), f"c3/{a.c3_pool}"
+    else:
+        t, name = traces.gen_c2(), "c2"
+    jobs, pc, rc = t["jobs"], t["cols"]["pending"], t["cols"]["running"]
+    users, tmpl = t["users"], t["offers"]
+    codes = tmpl.col("hostname_id").astype(np.int32)
+    names = {int(c): f"node-{int(c):07d}" for c in codes}
+    code_of = {n: c for c, n in names.items()}
+    U, R, O = users.n_users, len(rc["task_id"]), tmpl.n
+    rng = np.random.default_rng(a.seed)
+    host = codes[rng.integers(0, O, R)].astype(np.int32)
+    print(json.dumps({"card": card(), "pool": name, "jobs": jobs.n, "running": R, "hosts": O, "users": U}), flush=True)
+    store = Jobs(jobs, pc["priority"], pc["job_id"])
+    arms = {k: GpuEngine(pool_name=k) for k in ("resident", "cache")}
+    # the leases carry cpus, mem and hostnames only (what offers_from_cache merges), and no job holds a reservation;
+    # the cache arm's table is as wide as the attribute columns the jobs name, as the library's is
+    pend = _with(store.soa(np.arange(jobs.n)), reserved_host=None)
+    ac = jobs.col("attr_col")
+    W = int(ac.max()) + 1 if ac is not None and len(ac) else 0
+    for e in arms.values():
+        e.state_apply(abi.make_delta(reset=True, running=abi.make_tasks(**rc), running_hostname_id=host,
+                                     pending=pend, pending_priority=store.prio, pending_job_id=store.jid))
+    params = traces.match_params(min(jobs.n, 20_000))
+    d_users = _with(users, usage_count=None, usage_cpus=None, usage_mem=None, usage_gpus=None)
+    cache, incubate, lid = OfferCache(incubate_ms=15_000), 15_000, 0
+    next_tid = int(max(rc["task_id"])) + 10 if R else 10
+    now = 1_700_000_000_000
+    cpus0, mem0 = tmpl.col("cpus"), tmpl.col("mem")
+    for cycle in range(a.cycles):
+        now += 5_000
+        leases = []   # 40 % of the hosts offer again, some in two or three leases (cpus and mem in halves)
+        for h in rng.choice(O, int(O * 0.4), replace=False).tolist():
+            k = int(rng.choice([1, 1, 1, 2, 3]))
+            for _ in range(k):
+                leases.append({"id": lid, "hostname": names[int(codes[h])], "code": int(codes[h]),
+                               "cpus": float(np.floor(2 * cpus0[h] / k) / 2), "mem": float(np.floor(mem0[h] / k))})
+                lid += 1
+        n = len(leases)
+        soa = abi.OffersSoA(n=n, n_attr_cols=0, hostname_id=np.array([l["code"] for l in leases], np.int32),
+                            cpus=np.array([l["cpus"] for l in leases]), mem=np.array([l["mem"] for l in leases]))
+        ids = np.array([l["id"] for l in leases], np.int64)
+        for e in arms.values():
+            e.state_rank(users)
+        # ---- resident offers
+        e = arms["resident"]
+        w0 = time.perf_counter()
+        e.state_offers_add(soa, ids, now, hostnames=[l["hostname"] for l in leases])
+        add_stats = e.last_stats(abi.PHASE_STATE)
+        mr = e.state_match_offers(now, incubate, d_users, params)
+        wall_r = time.perf_counter() - w0
+        sr = mr["stats"]
+        # ---- the host's lease cache
+        e = arms["cache"]
+        w0 = time.perf_counter()
+        cache.add(leases, now)
+        cache.expire(now)
+        vm, table = offers_from_cache(cache, code_of)
+        if W:
+            table = _with(table, n_attr_cols=W, attr=np.zeros(W * table.n, np.int32))
+        mc = e.state_match(_with(table, run_cpus=None, run_mem=None, run_count=None), d_users, params, derived=True)
+        assign_codes = np.where(mc["assign"] >= 0, table.col("hostname_id")[np.maximum(mc["assign"], 0)], -1)
+        cache.after_match({names[int(c)] for c in assign_codes if c >= 0})
+        wall_c = time.perf_counter() - w0
+        sc = mc["stats"]
+        same = np.array_equal(mr["considerable"], mc["considerable"]) and np.array_equal(mr["assign"], assign_codes)
+        dev = lambda s: round(s["ms_considerable"] + s["ms_match"] + s["ms_h2d"] + s["ms_d2h"], 3)
+        print(json.dumps({"cycle": cycle, "offers_added": n, "vms": int(table.n), "placed": int((mr["assign"] >= 0).sum()),
+                          "resident": {"wall_ms": round(1e3 * wall_r, 3),
+                                       "device_ms": round(dev(sr) + add_stats["ms_h2d"] + add_stats["ms_device"], 3),
+                                       "h2d_bytes": sr["h2d_bytes"] + add_stats["h2d_bytes"], "d2h_bytes": sr["d2h_bytes"]},
+                          "cache": {"wall_ms": round(1e3 * wall_c, 3), "device_ms": dev(sc), "h2d_bytes": sc["h2d_bytes"],
+                                    "d2h_bytes": sc["d2h_bytes"]},
+                          "identical": bool(same)}), flush=True)
+        # ---- both arms launch the placements on the chosen hosts
+        ok = mr["assign"] >= 0
+        jl = mr["considerable"][ok]
+        tl = next_tid + 2 * np.arange(len(jl), dtype=np.int64)
+        next_tid += 2 * len(jl) + 2
+        for e in arms.values():
+            e.state_launch(jl, tl, np.full(len(jl), now, np.int64), mr["assign"][ok].astype(np.int32))
+    for e in arms.values():
+        e.close()
+
+
 def launch_cycle(cycle, res, twin, job_id, lt, hosts, rest, match_args):
     """One cycle of --launch: the launches by id on `res` and as a delta on `twin`, the rest of the batch on both,
     then rank and match on both.  Returns the jobs the match placed and their hosts' codes."""
@@ -726,6 +825,7 @@ def main():
                     help="--cotasks: a config-#3 pool (-1: the smaller c3-shaped pool); --derived: a config-#3 pool "
                          "instead of --pool")
     ap.add_argument("--derived", action="store_true")
+    ap.add_argument("--offers", action="store_true", help="live offers against the host's lease cache (C2 or --c3-pool)")
     ap.add_argument("--considerable", action="store_true")
     ap.add_argument("--audit", action="store_true")
     ap.add_argument("--user-stats", action="store_true")
@@ -749,6 +849,8 @@ def main():
         return cotasks_prof(a)
     if a.derived:
         return derived_prof(a)
+    if a.offers:
+        return offers_prof(a)
     t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
     jobs, pc, rc = t["jobs"], t["cols"]["pending"], t["cols"]["running"]
     J = jobs.n

@@ -5,7 +5,7 @@
 # every reported hazard is listed by source line in the log).
 mkdir -p gpurun_out/san
 K1='rank_and_match_parity_random or constraint_kernel or rank_golden or quota_and_rate'
-K2='rebalanc or next_state or pending_job or below_quota or off_grid or placement_failure or exchange_device'
+K2='rebalanc or next_state or pending_job or below_quota or off_grid or placement_failure or exchange_device or state_offers'
 timeout 1500 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests -m gpu -x -q -k "$K1" > gpurun_out/san/memcheck_rank_match.log 2>&1
 echo "memcheck rank+match rc=$?"; grep -E "ERROR SUMMARY|passed|failed" gpurun_out/san/memcheck_rank_match.log | tail -3
 timeout 1500 compute-sanitizer --tool memcheck --error-exitcode 9 python -m pytest tests -m gpu -x -q -k "$K2" > gpurun_out/san/memcheck_rebalance_misc.log 2>&1
