@@ -9,6 +9,9 @@
 ;;   :1749-1800 Kubernetes-scheduler pool    -> (kubernetes-considerable! ...)      [cook_state_considerable]
 ;;   :1283-1335 autoscaling helper           -> (autoscalable-jobs! ...)            [cook_state_considerable]
 ;;   monitor.clj:177-207 set-stats-counters! -> (monitor-resident! ...)             [cook_state_user_stats]
+;;   :1888-2016 the three killers            -> (sweep! ...), fed by task-facts! / finish! / group-runtimes!
+;;                                              [cook_state_sweep, cook_state_task_facts, cook_state_finish,
+;;                                               cook_state_group_runtimes]
 ;; selected per pool with {:scheduler-config {:scheduler "gpu"}} next to "fenzo" / "kubernetes"
 ;; (config.clj:110-122, make-pool-handler :2425-2466).  Everything numeric happens in libcookgpu;
 ;; this namespace marshals columns and keeps the state Fenzo kept (cook_b200/cycle.py is the same
@@ -322,3 +325,64 @@
   (check! (first handles) (Native/exchangeUsageBatch (long-array handles) comm world n-pad n-slots out)
           "cook_exchange_usage_batch")
   (.asDoubleBuffer ^ByteBuffer out))
+
+;; ---------------------------------------------------------------------------------------------
+;; the periodic killers over resident pools (cancelled-task-killer, lingering-task-killer, straggler-handler)
+(defn- longs-buf ^ByteBuffer [xs]
+  (let [b (direct (* 8 (count xs)))] (doseq [[i x] (map-indexed vector xs)] (.putLong b (int (* 8 i)) (long x))) b))
+(defn- ints-buf ^ByteBuffer [xs]
+  (let [b (direct (* 4 (count xs)))] (doseq [[i x] (map-indexed vector xs)] (.putInt b (int (* 4 i)) (int x))) b))
+(defn- bytes-buf ^ByteBuffer [xs]
+  (let [b (direct (count xs))] (doseq [[i x] (map-indexed vector xs)] (.put b (int i) (byte (if x 1 0)))) b))
+(defn- doubles-buf ^ByteBuffer [xs]
+  (let [b (direct (* 8 (count xs)))] (doseq [[i x] (map-indexed vector xs)] (.putDouble b (int (* 8 i)) (double x))) b))
+
+(defn task-facts!
+  "The killers' facts of live running instances, from the tx-report tap: `facts` is [{:task-id :max-runtime-ms
+   (-1: the job has none) :cancelled? :unknown?}]; every row must carry all three."
+  [handle facts]
+  (check! handle (Native/stateTaskFacts handle (count facts) (longs-buf (map :task-id facts))
+                                        (longs-buf (map :max-runtime-ms facts)) (bytes-buf (map :cancelled? facts))
+                                        (bytes-buf (map :unknown? facts)))
+          "cook_state_task_facts"))
+
+(defn finish!
+  "Status updates of instances that left running or unknown: [{:task-id :end-ms :success?}].  The rows leave as a
+   removal delta takes them; a success leaves its runtime per group for the straggler handler."
+  [handle done]
+  (check! handle (Native/stateFinish handle (count done) (longs-buf (map :task-id done)) (longs-buf (map :end-ms done))
+                                     (bytes-buf (map :success? done)))
+          "cook_state_finish"))
+
+(defn group-runtimes!
+  "After a reset or a leadership change: the successes of the tracked groups' jobs that finished before their rows
+   were resident, [[group-code runtime-seconds]], and the group codes no longer tracked."
+  [handle seeds forget]
+  (check! handle (Native/stateGroupRuntimes handle (count seeds) (ints-buf (map first seeds)) (ints-buf (map second seeds))
+                                            (count forget) (ints-buf forget))
+          "cook_state_group_runtimes"))
+
+(defn sweep!
+  "One trigger of a killer over `handles` (one device): `kinds` a subset of #{:linger :cancel :straggler}; `groups`
+   [{:kind :none|:quantile-deviation :quantile :multiplier :n-jobs}] by group code; `n-rows` / `n-entries` the live
+   running rows and their group entries (the shim's counts).  Returns {:linger [[task-id handle-index]] :cancel [...]
+   :straggler [[group task-id handle-index]]}, each to be killed with :max-runtime-exceeded, :reason-killed-by-user and
+   :straggler by the shim as the reference does.  The timeouts are derived from the hours as kill-lingering-tasks does."
+  [handles kinds now-ms default-timeout-ms max-timeout-ms groups n-rows n-entries]
+  (let [want (fn [k n bytes] (when (kinds k) (direct (* bytes (max 1 n)))))
+        lists [(want :linger n-rows 8) (want :linger n-rows 4) (want :cancel n-rows 8) (want :cancel n-rows 4)
+               (want :straggler n-entries 4) (want :straggler n-entries 8) (want :straggler n-entries 4)]
+        out-n (int-array 3)
+        gcols (object-array [(ints-buf (map #(if (= :quantile-deviation (:kind %)) 1 0) groups))
+                             (doubles-buf (map #(:quantile % 0.0) groups)) (doubles-buf (map #(:multiplier % 0.0) groups))
+                             (ints-buf (map :n-jobs groups))])]
+    (check! (first handles)
+            (Native/stateSweep (long-array handles) (long-array [now-ms default-timeout-ms max-timeout-ms])
+                               (count groups) gcols (int-array [n-rows n-entries]) (object-array lists) out-n nil)
+            "cook_state_sweep")
+    (let [l (fn [^ByteBuffer b i w] (if (= w 8) (.getLong b (int (* 8 i))) (.getInt b (int (* 4 i)))))
+          rows (fn [n cols] (vec (for [i (range n)] (mapv (fn [[b w]] (l b i w)) cols))))]
+      (cond-> {}
+        (kinds :linger) (assoc :linger (rows (aget out-n 0) [[(lists 0) 8] [(lists 1) 4]]))
+        (kinds :cancel) (assoc :cancel (rows (aget out-n 1) [[(lists 2) 8] [(lists 3) 4]]))
+        (kinds :straggler) (assoc :straggler (rows (aget out-n 2) [[(lists 4) 4] [(lists 5) 8] [(lists 6) 4]]))))))

@@ -148,6 +148,8 @@ STATS_RUNNING, STATS_WAITING, STATS_STARVED, STATS_WUQ = 0, 1, 2, 3
 USERS_TOTAL, USERS_STARVED, USERS_WUQ, USERS_HUNGRY, USERS_SATISFIED, USERS_N = 0, 1, 2, 3, 4, 5
 
 USAGE_GIVEN, USAGE_DERIVED, USAGE_LAST_MATCH = 0, 1, 2
+# cook_state_sweep: a group's straggler handling
+SWEEP_NONE, SWEEP_QUANTILE_DEVIATION = 0, 1
 # cook_state_match_offers: why an offer left the live set
 OFFER_USED, OFFER_EXPIRED, OFFER_SINGLE_SHOT = 1, 2, 3
 
@@ -327,6 +329,11 @@ ARGTYPES = {
     "cook_state_rebalance_offers": _STATE_REBALANCE,
     "cook_state_user_stats": [_P(_H), _I32, _P(UserTable), P_U8, P_I64, P_F64, P_F64, P_U8, P_I64, P_F64, P_F64, P_I64,
                               _P(PhaseStats)],
+    "cook_state_task_facts": [_H, _I32, P_I64, P_I64, P_U8, P_U8],
+    "cook_state_finish": [_H, _I32, P_I64, P_I64, P_U8],
+    "cook_state_group_runtimes": [_H, _I32, P_I32, P_I32, _I32, P_I32],
+    "cook_state_sweep": [_P(_H), _I32, C.c_int64, C.c_int64, C.c_int64, _I32, P_I32, P_F64, P_F64, P_I32, _I32, P_I64,
+                         P_I32, P_I32, P_I64, P_I32, P_I32, _I32, P_I32, P_I64, P_I32, P_I32, _P(PhaseStats)],
     "cook_last_stats": [_H, _I32, _P(PhaseStats)],
     "cook_allgather_usage": [_H, _H, P_F64, P_F64, C.c_int64],
     "cook_comm_unique_id": [P_U8],

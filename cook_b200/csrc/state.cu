@@ -40,9 +40,12 @@ enum PCol {
   P_LIVE = P_NDATA, P_GEN, P_NOFF, P_NLEN, P_AOFF, P_ALEN, P_GOFF, P_GLEN, P_NCOL
 };
 constexpr int P_SZ[P_NCOL] = {4, 4, 8, 8, 8, 8, 4, 1, 1, 4, 8, 4, 8, 4, 4, 1, 4, 4, 4, 4, 4, 4, 4};
+// R_MAXRT and R_FACTS are the facts cook_state_task_facts writes: the job's max-runtime (-1: none) and the
+// RF_* bits.  Every upsert and launch writes their absent values.
 enum RCol { R_USER, R_PRIO, R_START, R_TID, R_JID, R_CPUS, R_MEM, R_GPUS, R_HOST, R_NDATA, R_LIVE = R_NDATA, R_GEN,
-            R_GOFF, R_GLEN, R_NCOL };
-constexpr int R_SZ[R_NCOL] = {4, 4, 8, 8, 8, 8, 8, 8, 4, 1, 4, 4, 4};
+            R_GOFF, R_GLEN, R_MAXRT, R_FACTS, R_NCOL };
+constexpr int R_SZ[R_NCOL] = {4, 4, 8, 8, 8, 8, 8, 8, 4, 1, 4, 4, 4, 8, 1};
+enum { RF_CANCELLED = 1, RF_UNKNOWN = 2 };
 
 // The live offers (leases): one row per offer as it arrived, before any merge.  Data columns first, then the live
 // flag and generation, then the (off, len) pairs of the offer's four lists.
@@ -123,6 +126,8 @@ __global__ void launch_kernel(const int32_t* pslot, const int32_t* rslot, const 
   static_cast<uint32_t*>(rc[R_GEN])[r] += 1u;
   static_cast<int32_t*>(rc[R_GOFF])[r] = rtail;
   static_cast<int32_t*>(rc[R_GLEN])[r] = 0;
+  static_cast<int64_t*>(rc[R_MAXRT])[r] = -1;
+  static_cast<uint8_t*>(rc[R_FACTS])[r] = 0;
 }
 
 // ---- list lengths for the order-wide scan (integer sums: any association is exact)
@@ -647,6 +652,46 @@ struct ListArena {
   }
 };
 
+// The successful runtimes the straggler sweep measures against: an append-only SoA of (group code, whole seconds)
+// with a live flag, compacted (compact_records) once its dead records outnumber the live ones.
+struct Records {
+  int32_t* grp = nullptr; int32_t* rt = nullptr; uint8_t* live = nullptr;
+  int32_t* alt_grp = nullptr; int32_t* alt_rt = nullptr; uint8_t* alt_live = nullptr;   // compaction target
+  int64_t cap = 0, tail = 0, n_live = 0;
+  void free_all() {
+    for (void* p : {(void*)grp, (void*)rt, (void*)live, (void*)alt_grp, (void*)alt_rt, (void*)alt_live})
+      if (p) cudaFree(p);
+    grp = rt = alt_grp = alt_rt = nullptr;
+    live = alt_live = nullptr;
+  }
+  // capacity >= n: new columns holding the first `tail` records, both sets
+  cudaError_t grow(int64_t n, cudaStream_t st) {
+    if (n <= cap) return cudaSuccess;
+    const int64_t ncap = std::max<int64_t>(n, std::max<int64_t>(2 * cap, 4096));
+    int32_t *g = nullptr, *r = nullptr, *ag = nullptr, *ar = nullptr;
+    uint8_t *l = nullptr, *al = nullptr;
+    cudaError_t e = cudaMalloc(&g, 4 * ncap);
+    if (e == cudaSuccess) e = cudaMalloc(&r, 4 * ncap);
+    if (e == cudaSuccess) e = cudaMalloc(&l, ncap);
+    if (e == cudaSuccess) e = cudaMalloc(&ag, 4 * ncap);
+    if (e == cudaSuccess) e = cudaMalloc(&ar, 4 * ncap);
+    if (e == cudaSuccess) e = cudaMalloc(&al, ncap);
+    if (e == cudaSuccess && tail) e = cudaMemcpyAsync(g, grp, 4 * tail, cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess && tail) e = cudaMemcpyAsync(r, rt, 4 * tail, cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess && tail) e = cudaMemcpyAsync(l, live, tail, cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) {
+      for (void* p : {(void*)g, (void*)r, (void*)l, (void*)ag, (void*)ar, (void*)al}) if (p) cudaFree(p);
+      return e;
+    }
+    free_all();
+    grp = g; rt = r; live = l; alt_grp = ag; alt_rt = ar; alt_live = al;
+    cap = ncap;
+    return cudaSuccess;
+  }
+  void release() { free_all(); cap = tail = n_live = 0; }
+};
+
 void count_add(std::map<int32_t, int64_t>& m, int32_t code, int64_t d) {
   auto it = m.emplace(code, 0).first;
   if ((it->second += d) == 0) m.erase(it);
@@ -683,6 +728,11 @@ struct PoolState {
   std::vector<PendingInfo> pinfo;    // by pending slot
   std::vector<int32_t> ruser, rhost; // by running slot
   std::vector<std::vector<int32_t>> rgroups;   // by running slot: its group list
+  std::vector<int64_t> rstart;                 // by running slot: its start time (cook_state_finish's checks)
+  std::vector<uint8_t> rfacts;                 // by running slot: its RF_* bits
+  int64_t grp_rows = 0;                        // live running rows with a group list
+  Records rec;                                 // the successful runtimes per group
+  std::map<int32_t, int64_t> rec_groups;       // group code -> live records
   ListArena lists[L_N];
   ListArena olists[OL_N];
   std::map<int32_t, int64_t> users_p, users_r, attr_cols, groups;   // code -> live uses
@@ -716,7 +766,7 @@ struct PoolState {
     olists[OL_GPU].esz1 = olists[OL_DISK].esz1 = 8;
   }
   void release() {
-    pend.release(); run.release(); offer.release();
+    pend.release(); run.release(); offer.release(); rec.release();
     for (auto& l : lists) l.release();
     for (auto& l : olists) l.release();
     stage.release(); scratch.release(); derive.release(); queue.release(); omerge.release();
@@ -741,6 +791,7 @@ struct PoolState {
     const std::vector<int32_t>& g = rgroups[slot];
     for (int32_t c : g) count_add(groups_r, c, sign);
     lists[L_RGROUP].live += sign * (int64_t)g.size();
+    if (!g.empty()) grp_rows += sign;
     if (rhost[slot] != -1 && !g.empty()) {
       cot_rows += sign;
       cot_n += sign * (int64_t)g.size();
@@ -749,7 +800,7 @@ struct PoolState {
   void running_room(int32_t slot) {
     if ((size_t)slot < ruser.size()) return;
     const size_t n = std::max<size_t>(slot + 1, 2 * ruser.size());
-    ruser.resize(n); rhost.resize(n); rgroups.resize(n);
+    ruser.resize(n); rhost.resize(n); rgroups.resize(n); rstart.resize(n); rfacts.resize(n);
   }
   // a live pending slot's flag f after a patch of its column
   void set_flag(int32_t slot, int f, bool on) {
@@ -935,7 +986,9 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
     }
     S->users_p.clear(); S->users_r.clear(); S->attr_cols.clear(); S->groups.clear(); S->hosts_r.clear();
     S->groups_r.clear();
-    S->cot_rows = S->cot_n = 0;
+    S->cot_rows = S->cot_n = S->grp_rows = 0;
+    S->rec.tail = S->rec.n_live = 0;
+    S->rec_groups.clear();
     S->reserved.clear();
     for (auto& f : S->nflag) f = 0;
     for (auto& l : S->lists) l.tail = l.live = 0;
@@ -996,6 +1049,8 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
     S->ruser[s] = T.user[i];
     S->rhost[s] = d->running_hostname_id ? d->running_hostname_id[i] : -1;
     S->rgroups[s].assign(rgo ? d->running_group_idx + rgo[i] : nullptr, rgo ? d->running_group_idx + rgo[i + 1] : nullptr);
+    S->rstart[s] = T.start_time[i];
+    S->rfacts[s] = 0;
     S->add_running(s, +1);
     rup_slot[i] = s;
   }
@@ -1052,7 +1107,9 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
                                       : reinterpret_cast<const char*>(c.up(static_cast<const int64_t*>(src[k]), nr));
         ru.c[k] = ScatterCol{static_cast<char*>(S->run.col[k]), up, dflt[k], R_SZ[k]};
       }
-      ru.nc = R_NDATA;
+      ru.c[R_NDATA] = ScatterCol{static_cast<char*>(S->run.col[R_MAXRT]), nullptr, -1, R_SZ[R_MAXRT]};
+      ru.c[R_NDATA + 1] = ScatterCol{static_cast<char*>(S->run.col[R_FACTS]), nullptr, 0, R_SZ[R_FACTS]};
+      ru.nc = R_NDATA + 2;
       ru.slot = c.up(rup_slot.data(), nr);
       ru.doff[0] = c.up(rgo, nr + 1);
       if (c.base && radd) c.copy(RG.v[0] + rtail0, d->running_group_idx, radd);
@@ -1124,6 +1181,8 @@ int32_t launch(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, cons
     S->ruser[r] = S->pinfo[pslot[i]].user;
     S->rhost[r] = hostname_id ? hostname_id[i] : -1;
     S->rgroups[r] = S->pinfo[pslot[i]].groups;
+    S->rstart[r] = start_time[i];
+    S->rfacts[r] = 0;
     S->add_running(r, +1);
     ng += (int64_t)S->rgroups[r].size();
     rslot[i] = r;
@@ -2822,6 +2881,588 @@ extern "C" int32_t cook_state_rebalance_derived(cook_pool* pool, const cook_host
                                                 int64_t* out_victim_task_id, int32_t victim_cap, int32_t* out_n) {
   return state_rebalance(pool, "cook_state_rebalance_derived", true, hosts, groups, users, params, out_decisions,
                          out_decision_job_id, out_victim_task_id, victim_cap, out_n);
+}
+
+// ---- the periodic killers (cook_state_task_facts, cook_state_finish, cook_state_group_runtimes, cook_state_sweep).
+// Lingering and cancelled: the live running rows of the handles compacted into one dense range, sorted by (task id,
+// handle), then one stable compaction per list in that order.  Stragglers: the live records of the checked groups
+// sorted by (group, runtime) and cut into segments, one limit per group; the running rows' group lists expanded into
+// (group, task id, runtime) entries, sorted by (group, task id, handle), and compacted by their group's limit.
+namespace {
+
+// warp per finished row w: a successful row's group list becomes records (group, whole seconds since its start) at
+// the record table's tail plus the exclusive scan of the successful rows' list lengths
+struct FinishLen {
+  const int32_t* slot; const uint8_t* ok; const int32_t* len;
+  __device__ void operator()(int p, int (&x)[1]) const { x[0] = ok[p] ? len[slot[p]] : 0; }
+};
+__global__ void finish_records_kernel(OrderScan<int, 1> os, const int32_t* slot, const uint8_t* ok, const int64_t* end,
+                                      int n, void* const* rc, const int32_t* arena, int32_t* r_grp, int32_t* r_rt,
+                                      uint8_t* r_live, int32_t tail) {
+  const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (w >= n || !ok[w]) return;
+  const int s = slot[w];
+  const int l = static_cast<const int32_t*>(rc[R_GLEN])[s], o = static_cast<const int32_t*>(rc[R_GOFF])[s];
+  const int start = tail + os.at(0, w) - l;
+  const int32_t rt = (int32_t)((end[w] - static_cast<const int64_t*>(rc[R_START])[s]) / 1000);
+  for (int i = lane; i < l; i += 32) {
+    r_grp[start + i] = arena[o + i];
+    r_rt[start + i] = rt;
+    r_live[start + i] = 1;
+  }
+}
+
+// thread per record: a live record of a group in forget[0, n) (ascending) leaves
+__global__ void forget_records_kernel(const int32_t* grp, uint8_t* live, int n_rec, const int32_t* forget, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_rec || !live[i]) return;
+  const int32_t g = grp[i];
+  int lo = 0, hi = n;
+  while (lo < hi) {
+    const int m = (lo + hi) >> 1;
+    if (forget[m] < g) lo = m + 1;
+    else hi = m;
+  }
+  if (lo < n && forget[lo] == g) live[i] = 0;
+}
+
+struct RecordKeep {   // the record table's compaction
+  const int32_t* grp; const int32_t* rt; const uint8_t* live; int32_t* d_grp; int32_t* d_rt; uint8_t* d_live;
+  __device__ bool keep(int i) const { return live[i]; }
+  __device__ void emit(int i, int d) const { d_grp[d] = grp[i]; d_rt[d] = rt[i]; d_live[d] = 1; }
+};
+
+// the arena rule on the record table: compacted once its dead records outnumber the live ones
+int32_t compact_records(cook_pool* pool, PoolState* S, cudaStream_t st, int* nl) {
+  Records& R = S->rec;
+  if (R.tail - R.n_live <= R.n_live) return COOK_OK;
+  if (R.n_live > 0) {
+    int32_t* blk = nullptr;
+    CK(pool, carve(S->scratch, st, nullptr, nullptr, [&](Carve& c) { blk = c.take<int32_t>((size_t)R.tail / CP_BLOCK + 2); }));
+    compact(RecordKeep{R.grp, R.rt, R.live, R.alt_grp, R.alt_rt, R.alt_live}, (int)R.tail, nullptr, blk, S->counters + 6,
+            (int)R.n_live, st, nl);
+    CK(pool, cudaGetLastError());
+    std::swap(R.grp, R.alt_grp); std::swap(R.rt, R.alt_rt); std::swap(R.live, R.alt_live);
+  }
+  R.tail = R.n_live;
+  return COOK_OK;
+}
+
+// the slots of n distinct live running task ids, or why not
+const char* running_slots(const PoolState* S, int n, const int64_t* task_id, std::vector<int32_t>* slot) {
+  std::unordered_set<int64_t> seen;
+  seen.reserve((size_t)n);
+  slot->resize(n);
+  for (int i = 0; i < n; i++) {
+    if (!seen.insert(task_id[i]).second) return "task id twice";
+    auto it = S->run.slot_of.find(task_id[i]);
+    if (it == S->run.slot_of.end()) return "unknown task id";
+    (*slot)[i] = it->second;
+  }
+  return nullptr;
+}
+
+int32_t task_facts(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, const int64_t* max_runtime_ms,
+                   const uint8_t* cancelled, const uint8_t* unknown) {
+  const char* who = "cook_state_task_facts";
+  if (n < 0) return set_err(pool, COOK_E_BADARG, "%s: n < 0", who);
+  if (n && !task_id) return set_err(pool, COOK_E_BADARG, "%s: null task_id", who);
+  for (int i = 0; max_runtime_ms && i < n; i++)
+    if (max_runtime_ms[i] < -1) return set_err(pool, COOK_E_BADARG, "%s: a max_runtime_ms below -1", who);
+  std::vector<int32_t> slot;
+  if (const char* why = running_slots(S, n, task_id, &slot)) return set_err(pool, COOK_E_BADARG, "%s: %s", who, why);
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  // ---- host side: each row's bits, the given ones replaced
+  const bool bits = cancelled || unknown;
+  std::vector<uint8_t> facts(bits ? n : 0);
+  for (int i = 0; bits && i < n; i++) {
+    uint8_t& f = S->rfacts[slot[i]];
+    if (cancelled) f = (uint8_t)((f & ~RF_CANCELLED) | (cancelled[i] ? RF_CANCELLED : 0));
+    if (unknown) f = (uint8_t)((f & ~RF_UNKNOWN) | (unknown[i] ? RF_UNKNOWN : 0));
+    facts[i] = f;
+  }
+  // ---- device: a patch scatter (live flag and generation kept)
+  const bool cols = n && (max_runtime_ms || bits);
+  ScatterArgs pa;
+  memset(&pa, 0, sizeof(pa));
+  int64_t h2d = 0;
+  CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
+    if (!cols) return;
+    pa.slot = c.up(slot.data(), n);
+    if (max_runtime_ms) pa.c[pa.nc++] = ScatterCol{static_cast<char*>(S->run.col[R_MAXRT]),
+                                                   reinterpret_cast<const char*>(c.up(max_runtime_ms, n)), -1, 8};
+    if (bits) pa.c[pa.nc++] = ScatterCol{static_cast<char*>(S->run.col[R_FACTS]),
+                                         reinterpret_cast<const char*>(c.up(facts.data(), n)), 0, 1};
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  int nl = 0;
+  scatter(pa, S->run, cols ? n : 0, 0, -1, nullptr, st, &nl);
+  CK(pool, cudaGetLastError());
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  CK(pool, cudaStreamSynchronize(st));
+  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
+  return COOK_OK;
+}
+
+// running_rm_task_id = task_id, plus one record per group of each successful row
+int32_t finish(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, const int64_t* end_time_ms,
+               const uint8_t* success) {
+  const char* who = "cook_state_finish";
+  if (n < 0) return set_err(pool, COOK_E_BADARG, "%s: n < 0", who);
+  if (n && !task_id) return set_err(pool, COOK_E_BADARG, "%s: null task_id", who);
+  if (n && success && !end_time_ms) return set_err(pool, COOK_E_BADARG, "%s: success without end_time_ms", who);
+  std::vector<int32_t> slot;
+  if (const char* why = running_slots(S, n, task_id, &slot)) return set_err(pool, COOK_E_BADARG, "%s: %s", who, why);
+  int64_t nrec = 0;   // the records the successful rows append
+  for (int i = 0; success && i < n; i++) {
+    if (!success[i]) continue;
+    const int32_t s = slot[i];
+    if (end_time_ms[i] < S->rstart[s]) return set_err(pool, COOK_E_BADARG, "%s: a success that ends before its start", who);
+    if ((end_time_ms[i] - S->rstart[s]) / 1000 > INT32_MAX)
+      return set_err(pool, COOK_E_BADARG, "%s: a runtime of 2^31 s or more", who);
+    nrec += (int64_t)S->rgroups[s].size();
+  }
+  if (S->rec.tail + nrec > INT32_MAX) return set_err(pool, COOK_E_TOO_LARGE, "%s: more than 2^31 - 1 records", who);
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  // ---- host side: cook_state_apply's removals, then the records' counts
+  for (int i = 0; i < n; i++) {
+    const int32_t s = slot[i];
+    S->run.slot_of.erase(task_id[i]);
+    S->add_running(s, -1);
+    S->run.free.push_back(s);
+    if (success && success[i])
+      for (int32_t g : S->rgroups[s]) count_add(S->rec_groups, g, +1);
+  }
+  // ---- device: the records (read before the removal empties the rows' lists), the removal, the arena rules
+  Records& RC = S->rec;
+  const int32_t rtail = (int32_t)RC.tail;
+  CK(pool, RC.grow(RC.tail + nrec, st));
+  RC.tail += nrec;
+  RC.n_live += nrec;
+  const int32_t rgtail = (int32_t)S->lists[L_RGROUP].tail;
+  const int32_t* d_slot = nullptr;
+  const uint8_t* d_ok = nullptr;
+  const int64_t* d_end = nullptr;
+  OrderScan<int, 1> os;
+  int64_t h2d = 0;
+  CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
+    if (!n) return;
+    d_slot = c.up(slot.data(), n);
+    if (success) { d_ok = c.up(success, n); d_end = c.up(end_time_ms, n); }
+    if (nrec) {   // device-only buffers: nothing uploaded
+      os.part[0] = c.take<int32_t>(n);
+      os.tile[0] = c.take<int32_t>((n + OS_TILE - 1) / OS_TILE + 1);
+    }
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  int nl = 0;
+  if (nrec) {
+    order_scan(os, FinishLen{d_slot, d_ok, S->run.at<int32_t>(R_GLEN)}, n, S->gf0, st, &nl);
+    finish_records_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, d_slot, d_ok, d_end, n, S->run.d_col,
+                                                       S->lists[L_RGROUP].v[0], RC.grp, RC.rt, RC.live, rtail);
+    nl++;
+  }
+  if (n) {
+    ScatterArgs rr;
+    memset(&rr, 0, sizeof(rr));
+    rr.slot = d_slot;
+    scatter(rr, S->run, n, 0, R_LIVE, &rgtail, st, &nl);
+  }
+  CK(pool, cudaGetLastError());
+  int32_t rc = compact_lists(pool, S, st, &nl);
+  if (rc == COOK_OK) rc = compact_records(pool, S, st, &nl);
+  if (rc != COOK_OK) return rc;
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  CK(pool, cudaStreamSynchronize(st));
+  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
+  return COOK_OK;
+}
+
+// the records of the forgotten groups leave, then the seeds are appended
+int32_t group_runtimes(cook_pool* pool, PoolState* S, int n_add, const int32_t* group, const int32_t* runtime_s,
+                       int n_forget, const int32_t* forget_group) {
+  const char* who = "cook_state_group_runtimes";
+  if (n_add < 0 || n_forget < 0) return set_err(pool, COOK_E_BADARG, "%s: a negative size", who);
+  if ((n_add && (!group || !runtime_s)) || (n_forget && !forget_group))
+    return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
+  if (!idx_in_range(group, n_add, 0, INT32_MAX) || !idx_in_range(forget_group, n_forget, 0, INT32_MAX))
+    return set_err(pool, COOK_E_BADARG, "%s: a negative group code", who);
+  if (!idx_in_range(runtime_s, n_add, 0, INT32_MAX)) return set_err(pool, COOK_E_BADARG, "%s: a negative runtime", who);
+  Records& RC = S->rec;
+  if (RC.tail + n_add > INT32_MAX) return set_err(pool, COOK_E_TOO_LARGE, "%s: more than 2^31 - 1 records", who);
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  // ---- host side
+  std::vector<int32_t> forget(forget_group, forget_group + n_forget);
+  std::sort(forget.begin(), forget.end());
+  forget.erase(std::unique(forget.begin(), forget.end()), forget.end());
+  for (int32_t g : forget) {
+    auto it = S->rec_groups.find(g);
+    if (it == S->rec_groups.end()) continue;
+    RC.n_live -= it->second;
+    S->rec_groups.erase(it);
+  }
+  for (int i = 0; i < n_add; i++) count_add(S->rec_groups, group[i], +1);
+  // ---- device
+  const int32_t tail0 = (int32_t)RC.tail;
+  CK(pool, RC.grow(RC.tail + n_add, st));
+  const int nf = (int)forget.size();
+  const int32_t* d_forget = nullptr;
+  int64_t h2d = 0;
+  CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
+    if (nf) d_forget = c.up(forget.data(), nf);
+    if (c.base && n_add) {
+      c.copy(RC.grp + tail0, group, n_add);
+      c.copy(RC.rt + tail0, runtime_s, n_add);
+    }
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  int nl = 0;
+  if (nf && tail0) {
+    forget_records_kernel<<<(tail0 + 255) / 256, 256, 0, st>>>(RC.grp, RC.live, tail0, d_forget, nf);
+    nl++;
+  }
+  if (n_add) CK(pool, cudaMemsetAsync(RC.live + tail0, 1, (size_t)n_add, st));
+  RC.tail += n_add;
+  RC.n_live += n_add;
+  CK(pool, cudaGetLastError());
+  int32_t rc = compact_records(pool, S, st, &nl);
+  if (rc != COOK_OK) return rc;
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  CK(pool, cudaStreamSynchronize(st));
+  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
+  return COOK_OK;
+}
+
+// ---- cook_state_sweep
+// every live running row of one handle, dense after those of the handles before it (base)
+struct SweepRows {
+  void* const* col; int base; int32_t pool;
+  int64_t* tid; int32_t* pidx; int64_t* start; int64_t* maxrt; uint8_t* facts;
+  __device__ bool keep(int i) const { return static_cast<const uint8_t*>(col[R_LIVE])[i]; }
+  __device__ void emit(int i, int d) const {
+    d += base;
+    tid[d] = static_cast<const int64_t*>(col[R_TID])[i];
+    pidx[d] = pool;
+    start[d] = static_cast<const int64_t*>(col[R_START])[i];
+    maxrt[d] = static_cast<const int64_t*>(col[R_MAXRT])[i];
+    facts[d] = static_cast<const uint8_t*>(col[R_FACTS])[i];
+  }
+};
+// position p of the (task id, handle) order: lingering, now - start > min(max-runtime or the default, max timeout), or
+// (cancelled) the cancelled bit
+struct KillSel {
+  const int32_t* ord; const int64_t* tid; const int32_t* pidx; const int64_t* start; const int64_t* maxrt;
+  const uint8_t* facts; int64_t now, dflt, cap; bool cancelled;
+  int64_t* o_tid; int32_t* o_pool;
+  __device__ bool keep(int p) const {
+    const int i = ord[p];
+    if (cancelled) return facts[i] & RF_CANCELLED;
+    const int64_t m = maxrt[i] < 0 ? dflt : maxrt[i];
+    return now - start[i] > (m < cap ? m : cap);
+  }
+  __device__ void emit(int p, int d) const { const int i = ord[p]; o_tid[d] = tid[i]; o_pool[d] = pidx[i]; }
+};
+// the live records of one handle whose group is checked, dense after the handles before it
+struct SweepRecords {
+  const int32_t* grp; const int32_t* rt; const uint8_t* live; const int32_t* kind; int base;
+  int32_t* d_grp; int64_t* d_rt;
+  __device__ bool keep(int i) const { return live[i] && kind[grp[i]] == COOK_SWEEP_QUANTILE_DEVIATION; }
+  __device__ void emit(int i, int d) const { d_grp[base + d] = grp[i]; d_rt[base + d] = rt[i]; }
+};
+// thread per group: idx = (int)((n_jobs - 1) * quantile); with more than idx successes the limit is the idx-th
+// smallest runtime times the multiplier, else (or unchecked, or idx < 0) +inf
+__global__ void straggler_limit_kernel(const int32_t* kind, const double* quantile, const double* multiplier,
+                                       const int32_t* n_jobs, const int32_t* seg_start, const int32_t* seg_end,
+                                       const int32_t* ord, const int64_t* rt, int G, double* limit) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= G) return;
+  double lim = INFINITY;
+  if (kind[g] == COOK_SWEEP_QUANTILE_DEVIATION) {
+    const int idx = (int)((double)(n_jobs[g] - 1) * quantile[g]);
+    if (idx >= 0 && seg_end[g] - seg_start[g] > idx) lim = (double)rt[ord[seg_start[g] + idx]] * multiplier[g];
+  }
+  limit[g] = lim;
+}
+struct GroupedRows {   // one handle's live running rows with a group list, by slot
+  const uint8_t* live; const int32_t* len; int32_t* slot;
+  __device__ bool keep(int i) const { return live[i] && len[i] > 0; }
+  __device__ void emit(int i, int d) const { slot[d] = i; }
+};
+struct ExpandArgs {
+  OrderScan<int, 1> os;   // inclusive scan of the rows' list lengths
+  const int32_t* slot; int K, ebase; int32_t pool;
+  void* const* col; const int32_t* arena; const int32_t* kind; int64_t now;
+  int32_t* e_grp; int64_t* e_tid; int32_t* e_pool;
+  int64_t* e_rt;          // whole seconds run; -1: not judged (status unknown, or the group is not checked)
+  int32_t* bad;           // set by a judged entry that starts after now
+};
+// thread per row: one entry per group of its list, at ebase plus where the scan puts the row
+__global__ void straggler_expand_kernel(ExpandArgs a) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= a.K) return;
+  const int s = a.slot[k];
+  const int l = static_cast<const int32_t*>(a.col[R_GLEN])[s], o = static_cast<const int32_t*>(a.col[R_GOFF])[s];
+  const int base = a.ebase + a.os.at(0, k) - l;
+  const bool running = !(static_cast<const uint8_t*>(a.col[R_FACTS])[s] & RF_UNKNOWN);
+  const int64_t t = static_cast<const int64_t*>(a.col[R_TID])[s], st = static_cast<const int64_t*>(a.col[R_START])[s];
+  for (int i = 0; i < l; i++) {
+    const int32_t g = a.arena[o + i];
+    const bool judged = running && a.kind[g] == COOK_SWEEP_QUANTILE_DEVIATION;
+    if (judged && st > a.now) *a.bad = 1;
+    a.e_grp[base + i] = g;
+    a.e_tid[base + i] = t;
+    a.e_pool[base + i] = a.pool;
+    a.e_rt[base + i] = judged ? (a.now - st) / 1000 : -1;
+  }
+}
+// position p of the (group, task id, handle) order: a judged entry past its group's limit
+struct StragglerSel {
+  const int32_t* ord; const int32_t* e_grp; const int64_t* e_tid; const int32_t* e_pool; const int64_t* e_rt;
+  const double* limit; int32_t* o_grp; int64_t* o_tid; int32_t* o_pool;
+  __device__ bool keep(int p) const { const int i = ord[p]; return e_rt[i] >= 0 && (double)e_rt[i] > limit[e_grp[i]]; }
+  __device__ void emit(int p, int d) const {
+    const int i = ord[p];
+    o_grp[d] = e_grp[i]; o_tid[d] = e_tid[i]; o_pool[d] = e_pool[i];
+  }
+};
+
+int32_t sweep(cook_pool* const* pools, int n, int64_t now, int64_t dflt, int64_t max_to, int G, const int32_t* kind,
+              const double* quantile, const double* multiplier, const int32_t* n_jobs, int32_t row_cap, int64_t* l_tid,
+              int32_t* l_pool, int32_t* l_n, int64_t* c_tid, int32_t* c_pool, int32_t* c_n, int32_t entry_cap,
+              int32_t* s_grp, int64_t* s_tid, int32_t* s_pool, int32_t* s_n, cook_phase_stats* out_stats) {
+  const char* who = "cook_state_sweep";
+  // ---- every check before any device work or output
+  if (!pools || n <= 0 || !pools[0]) return COOK_E_BADARG;
+  cook_pool* pool = pools[0];
+  for (int k = 0; k < n; k++) {
+    if (!pools[k]) return set_err(pool, COOK_E_BADARG, "%s: a NULL handle", who);
+    if (std::find(pools, pools + k, pools[k]) != pools + k)
+      return set_err(pool, COOK_E_BADARG, "%s: a handle listed twice", who);
+    if (pools[k]->device != pool->device) return set_err(pool, COOK_E_BADARG, "%s: handles on different devices", who);
+  }
+  const bool linger = l_tid != nullptr, cancel = c_tid != nullptr, strag = s_tid != nullptr;
+  if ((linger && (!l_pool || !l_n)) || (cancel && (!c_pool || !c_n)) || (strag && (!s_grp || !s_pool || !s_n)))
+    return set_err(pool, COOK_E_BADARG, "%s: a list without its pool column or count", who);
+  if (G < 0) return set_err(pool, COOK_E_BADARG, "%s: n_groups < 0", who);
+  if (strag && G > 0 && (!kind || !quantile || !multiplier || !n_jobs))
+    return set_err(pool, COOK_E_BADARG, "%s: null group_kind, quantile, multiplier or n_jobs", who);
+  for (int g = 0; strag && g < G; g++) {
+    if (kind[g] != COOK_SWEEP_NONE && kind[g] != COOK_SWEEP_QUANTILE_DEVIATION)
+      return set_err(pool, COOK_E_BADARG, "%s: an unknown group kind", who);
+    if (kind[g] == COOK_SWEEP_QUANTILE_DEVIATION && !(quantile[g] >= 0.0 && quantile[g] <= 1.0))
+      return set_err(pool, COOK_E_BADARG, "%s: a quantile outside [0, 1]", who);
+    if (n_jobs[g] < 0) return set_err(pool, COOK_E_BADARG, "%s: a negative n_jobs", who);
+  }
+  // the handles with rows, their pool index; sizes from the host-side counts
+  std::vector<std::pair<const PoolState*, int32_t>> hs;
+  int64_t R = 0, N = 0, M = 0, K = 0;
+  int hw = 0, kmax = 0;
+  for (int k = 0; k < n; k++) {
+    const PoolState* s = static_cast<const PoolState*>(pools[k]->state);
+    if (!s) continue;
+    if (strag && (count_max(s->groups_r) >= G || count_max(s->rec_groups) >= G))
+      return set_err(pool, COOK_E_BADARG, "%s: a live group code >= n_groups", who);
+    hs.push_back({s, k});
+    R += (int64_t)s->run.slot_of.size();
+    N += s->lists[L_RGROUP].live;
+    K += s->grp_rows;
+    kmax = std::max<int>(kmax, (int)s->grp_rows);
+    hw = std::max({hw, s->run.hw, (int)s->rec.tail});
+    for (const auto& kv : s->rec_groups)
+      if (strag && kind[kv.first] == COOK_SWEEP_QUANTILE_DEVIATION) M += kv.second;
+  }
+  if (R > INT32_MAX || N > INT32_MAX) return set_err(pool, COOK_E_TOO_LARGE, "%s: more than 2^31 - 1 rows", who);
+  if ((linger || cancel) && row_cap < R) return set_err(pool, COOK_E_BADARG, "%s: row_cap < the live running rows", who);
+  if (strag && entry_cap < N) return set_err(pool, COOK_E_BADARG, "%s: entry_cap < the live group entries", who);
+  const bool rows = (linger || cancel) && R > 0, groups = strag && N > 0;
+  if (!rows && !groups) {   // nothing to judge: empty lists, no device work
+    if (linger) *l_n = 0;
+    if (cancel) *c_n = 0;
+    if (strag) *s_n = 0;
+    if (out_stats) *out_stats = cook_phase_stats{};
+    return COOK_OK;
+  }
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S0 = state_of(pool, true);   // pools[0]'s scratch, even when it holds no row
+  if (!S0) return set_err(pool, COOK_E_OOM, "%s: out of device memory", who);
+  cudaStream_t st = pool->stream;
+  hw = std::max({hw, (int)R, (int)N});
+  // ---- one carve
+  int32_t *cnt = nullptr, *blk = nullptr, *ord = nullptr, *tmp = nullptr, *pidx = nullptr;
+  int64_t *tid = nullptr, *start = nullptr, *maxrt = nullptr;
+  uint8_t* facts = nullptr;
+  int64_t *o_ltid = nullptr, *o_ctid = nullptr, *o_stid = nullptr;
+  int32_t *o_lpool = nullptr, *o_cpool = nullptr, *o_sgrp = nullptr, *o_spool = nullptr;
+  const int32_t *d_kind = nullptr, *d_nj = nullptr;
+  const double *d_q = nullptr, *d_m = nullptr;
+  int32_t *r_grp = nullptr, *r_ord = nullptr, *r_tmp = nullptr, *seg_s = nullptr, *seg_e = nullptr, *slot = nullptr;
+  int64_t* r_rt = nullptr;
+  double* limit = nullptr;
+  OrderScan<int, 1> os;
+  int32_t *e_grp = nullptr, *e_pool = nullptr, *e_ord = nullptr, *e_tmp = nullptr;
+  int64_t *e_tid = nullptr, *e_rt = nullptr;
+  int64_t h2d = 0, d2h = 0;
+  CK(pool, carve(S0->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+    cnt = c.take<int32_t>(5);   // lingering, cancelled, stragglers, start after now, the compactions' own
+    blk = c.take<int32_t>((size_t)hw / CP_BLOCK + 2);
+    if (rows) {
+      tid = c.take<int64_t>(R); pidx = c.take<int32_t>(R); start = c.take<int64_t>(R); maxrt = c.take<int64_t>(R);
+      facts = c.take<uint8_t>(R); ord = c.take<int32_t>(R); tmp = c.take<int32_t>(R);
+      if (linger) { o_ltid = c.take<int64_t>(R); o_lpool = c.take<int32_t>(R); }
+      if (cancel) { o_ctid = c.take<int64_t>(R); o_cpool = c.take<int32_t>(R); }
+    }
+    if (groups) {
+      d_kind = c.up(kind, G); d_q = c.up(quantile, G); d_m = c.up(multiplier, G); d_nj = c.up(n_jobs, G);
+      r_grp = c.take<int32_t>(M); r_rt = c.take<int64_t>(M); r_ord = c.take<int32_t>(M); r_tmp = c.take<int32_t>(M);
+      seg_s = c.take<int32_t>(G); seg_e = c.take<int32_t>(G); limit = c.take<double>(G);
+      slot = c.take<int32_t>(K);
+      os.part[0] = c.take<int32_t>(kmax);
+      os.tile[0] = c.take<int32_t>((kmax + OS_TILE - 1) / OS_TILE + 1);
+      e_grp = c.take<int32_t>(N); e_tid = c.take<int64_t>(N); e_pool = c.take<int32_t>(N); e_rt = c.take<int64_t>(N);
+      e_ord = c.take<int32_t>(N); e_tmp = c.take<int32_t>(N);
+      o_sgrp = c.take<int32_t>(N); o_stid = c.take<int64_t>(N); o_spool = c.take<int32_t>(N);
+    }
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  CK(pool, cudaMemsetAsync(cnt, 0, sizeof(int32_t) * 5, st));
+  int nl = 0;
+  if (rows) {
+    int base = 0;
+    for (const auto& h : hs) {
+      const Table& t = h.first->run;
+      const int live = (int)t.slot_of.size();
+      if (!live) continue;
+      compact(SweepRows{t.d_col, base, h.second, tid, pidx, start, maxrt, facts}, t.hw, nullptr, blk, cnt + 4, live, st,
+              &nl);
+      base += live;
+    }
+    CK(pool, csort::sort_indices(ord, tmp, (int)R, LessKeyTid{nullptr, tid}, st, &nl));
+    if (linger)
+      compact(KillSel{ord, tid, pidx, start, maxrt, facts, now, dflt, max_to, false, o_ltid, o_lpool}, (int)R, nullptr,
+              blk, cnt + 0, (int)R, st, &nl);
+    if (cancel)
+      compact(KillSel{ord, tid, pidx, start, maxrt, facts, now, dflt, max_to, true, o_ctid, o_cpool}, (int)R, nullptr,
+              blk, cnt + 1, (int)R, st, &nl);
+  }
+  if (groups) {
+    // the limits, from the checked groups' records
+    CK(pool, cudaMemsetAsync(seg_s, 0, sizeof(int32_t) * (size_t)G, st));
+    CK(pool, cudaMemsetAsync(seg_e, 0, sizeof(int32_t) * (size_t)G, st));
+    if (M > 0) {
+      int base = 0;
+      for (const auto& h : hs) {
+        const Records& rc = h.first->rec;
+        int64_t mk = 0;
+        for (const auto& kv : h.first->rec_groups)
+          if (kind[kv.first] == COOK_SWEEP_QUANTILE_DEVIATION) mk += kv.second;
+        if (!mk) continue;
+        compact(SweepRecords{rc.grp, rc.rt, rc.live, d_kind, base, r_grp, r_rt}, (int)rc.tail, nullptr, blk, cnt + 4,
+                (int)mk, st, &nl);
+        base += (int)mk;
+      }
+      CK(pool, csort::sort_indices(r_ord, r_tmp, (int)M, LessKeyTid{r_grp, r_rt}, st, &nl));
+      seg_bounds_kernel<<<((int)M + 255) / 256, 256, 0, st>>>(SortedKey{r_ord, nullptr, r_grp}, (int)M, seg_s, seg_e,
+                                                              nullptr);
+      nl++;
+    }
+    straggler_limit_kernel<<<(G + 255) / 256, 256, 0, st>>>(d_kind, d_q, d_m, d_nj, seg_s, seg_e, r_ord, r_rt, G, limit);
+    nl++;
+    // the entries, handle by handle
+    int kbase = 0, ebase = 0;
+    for (const auto& h : hs) {
+      const PoolState* s = h.first;
+      const int Kk = (int)s->grp_rows;
+      if (!Kk) continue;
+      const int32_t* glen = s->run.at<int32_t>(R_GLEN);
+      compact(GroupedRows{s->run.at<uint8_t>(R_LIVE), glen, slot + kbase}, s->run.hw, nullptr, blk, cnt + 4, Kk, st, &nl);
+      order_scan(os, RowLen{slot + kbase, glen}, Kk, S0->gf0, st, &nl);
+      ExpandArgs a = {os, slot + kbase, Kk, ebase, h.second, s->run.d_col, s->lists[L_RGROUP].v[0], d_kind, now,
+                      e_grp, e_tid, e_pool, e_rt, cnt + 3};
+      straggler_expand_kernel<<<(Kk + 255) / 256, 256, 0, st>>>(a);
+      nl++;
+      kbase += Kk;
+      ebase += (int)s->lists[L_RGROUP].live;
+    }
+    CK(pool, csort::sort_indices(e_ord, e_tmp, (int)N, LessKeyTid{e_grp, e_tid}, st, &nl));
+    compact(StragglerSel{e_ord, e_grp, e_tid, e_pool, e_rt, limit, o_sgrp, o_stid, o_spool}, (int)N, nullptr, blk,
+            cnt + 2, (int)N, st, &nl);
+  }
+  CK(pool, cudaGetLastError());
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  int32_t got[4];
+  CK(pool, download(got, cnt, 4, st, &d2h));
+  CK(pool, cudaStreamSynchronize(st));
+  if (got[3]) return set_err(pool, COOK_E_BADARG, "%s: a running task of a checked group starts after now_ms", who);
+  if (rows && linger && got[0]) {
+    CK(pool, download(l_tid, o_ltid, got[0], st, &d2h));
+    CK(pool, download(l_pool, o_lpool, got[0], st, &d2h));
+  }
+  if (rows && cancel && got[1]) {
+    CK(pool, download(c_tid, o_ctid, got[1], st, &d2h));
+    CK(pool, download(c_pool, o_cpool, got[1], st, &d2h));
+  }
+  if (groups && got[2]) {
+    CK(pool, download(s_grp, o_sgrp, got[2], st, &d2h));
+    CK(pool, download(s_tid, o_stid, got[2], st, &d2h));
+    CK(pool, download(s_pool, o_spool, got[2], st, &d2h));
+  }
+  CK(pool, cudaEventRecord(pool->ev[23], st));
+  CK(pool, cudaStreamSynchronize(st));
+  if (linger) *l_n = got[0];
+  if (cancel) *c_n = got[1];
+  if (strag) *s_n = got[2];
+  if (out_stats)
+    *out_stats = {ev_ms(pool->ev[20], pool->ev[21]), ev_ms(pool->ev[21], pool->ev[22]), ev_ms(pool->ev[22], pool->ev[23]),
+                  h2d, d2h, nl, 0};
+  return COOK_OK;
+}
+
+}  // namespace
+
+extern "C" int32_t cook_state_task_facts(cook_pool* pool, int32_t n, const int64_t* task_id,
+                                         const int64_t* max_runtime_ms, const uint8_t* cancelled,
+                                         const uint8_t* unknown) {
+  if (!pool) return COOK_E_BADARG;
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_task_facts: out of device memory");
+  return task_facts(pool, S, n, task_id, max_runtime_ms, cancelled, unknown);
+}
+
+extern "C" int32_t cook_state_finish(cook_pool* pool, int32_t n, const int64_t* task_id, const int64_t* end_time_ms,
+                                     const uint8_t* success) {
+  if (!pool) return COOK_E_BADARG;
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_finish: out of device memory");
+  return finish(pool, S, n, task_id, end_time_ms, success);
+}
+
+extern "C" int32_t cook_state_group_runtimes(cook_pool* pool, int32_t n_add, const int32_t* group,
+                                             const int32_t* runtime_s, int32_t n_forget, const int32_t* forget_group) {
+  if (!pool) return COOK_E_BADARG;
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_group_runtimes: out of device memory");
+  return group_runtimes(pool, S, n_add, group, runtime_s, n_forget, forget_group);
+}
+
+extern "C" int32_t cook_state_sweep(cook_pool* const* pools, int32_t n_pools, int64_t now_ms,
+                                    int64_t default_timeout_ms, int64_t max_timeout_ms, int32_t n_groups,
+                                    const int32_t* group_kind, const double* quantile, const double* multiplier,
+                                    const int32_t* n_jobs, int32_t row_cap, int64_t* out_linger_task_id,
+                                    int32_t* out_linger_pool, int32_t* out_n_linger, int64_t* out_cancel_task_id,
+                                    int32_t* out_cancel_pool, int32_t* out_n_cancel, int32_t entry_cap,
+                                    int32_t* out_straggler_group, int64_t* out_straggler_task_id,
+                                    int32_t* out_straggler_pool, int32_t* out_n_straggler,
+                                    cook_phase_stats* out_stats) {
+  return sweep(pools, n_pools, now_ms, default_timeout_ms, max_timeout_ms, n_groups, group_kind, quantile, multiplier,
+               n_jobs, row_cap, out_linger_task_id, out_linger_pool, out_n_linger, out_cancel_task_id, out_cancel_pool,
+               out_n_cancel, entry_cap, out_straggler_group, out_straggler_task_id, out_straggler_pool, out_n_straggler,
+               out_stats);
 }
 
 // ---- audit: the read side (cook_state_digest, cook_state_export, cook_state_queue).  The digest is one pass per

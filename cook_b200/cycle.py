@@ -418,3 +418,30 @@ def queue_lengths(pool_stats, user_names):
         if len(w):
             per[pool] = {user_names[u]: int(st["jobs"][abi.STATS_WAITING, u]) for u in w}
     return {"pool->queue-length": {p: sum(m.values()) for p, m in per.items()}, "pool->user->queue-length": per}
+
+
+# ---- the periodic killers over resident pools --------------------------------------------------------------------
+KILL_REASONS = {"linger": "max-runtime-exceeded", "straggler": "straggler", "cancel": "reason-killed-by-user"}
+
+
+def lingering_timeouts_ms(timeout_hours=48, max_timeout_hours=None, default_timeout_hours=None):
+    """kill-lingering-tasks' (scheduler.clj:1912-1918) default and max timeouts in ms: each falls back to
+    timeout-hours (48 in lingering-task-killer)."""
+    dflt = default_timeout_hours if default_timeout_hours is not None else timeout_hours
+    mx = max_timeout_hours if max_timeout_hours is not None else timeout_hours
+    return int(dflt * 3_600_000), int(mx * 3_600_000)
+
+
+def kill_lists(engines, now_ms, default_timeout_ms, max_timeout_ms, groups=None,
+               lists=("linger", "cancel", "straggler")):
+    """One trigger of the killers over resident pools (engine.state_sweep): [(reason, task id, engine index, group or
+    None)] in the sweep's orders, lingering first, then stragglers, then cancelled.  The status updates of the killed
+    tasks come back through the tap and go to engine.state_finish."""
+    from .engine import state_sweep
+    got = state_sweep(engines, now_ms, default_timeout_ms, max_timeout_ms, groups, lists)
+    out = []
+    for k in ("linger", "straggler", "cancel"):
+        for x in got[k] or ():
+            g, (t, p) = (x[0], x[1:]) if k == "straggler" else (None, x)
+            out.append((KILL_REASONS[k], t, p, g))
+    return out

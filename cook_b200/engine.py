@@ -172,6 +172,21 @@ class GpuEngine:
         tid = delta.col("running").col("task_id") if delta.running.n else None
         run.update(tid.tolist() if tid is not None else [])
         self._state_running_ids = run
+        # and the length of each live row's group list: they size state_sweep's straggler entries
+        png, rng_ = self._group_lengths()
+        if delta.reset:
+            png.clear()
+            rng_.clear()
+        for j in (rm.tolist() if (rm := delta.col("pending_rm_job_id")) is not None else []):
+            png.pop(j, None)
+        for t in (rm.tolist() if (rm := delta.col("running_rm_task_id")) is not None else []):
+            rng_.pop(t, None)
+        if up is not None:
+            off = delta.col("pending").col("group_off")
+            png.update(zip(up.tolist(), np.diff(off).tolist() if off is not None else [0] * len(up)))
+        if tid is not None:
+            off = delta.col("running_group_off")
+            rng_.update(zip(tid.tolist(), np.diff(off).tolist() if off is not None else [0] * len(tid)))
 
     def state_launch(self, job_id, task_id, start_time, hostname_id=None):
         """cook_state_launch: live pending job job_id[i] becomes running task task_id[i] (started at
@@ -192,6 +207,62 @@ class GpuEngine:
         run = getattr(self, "_state_running_ids", set())
         run.update(tid.tolist())
         self._state_running_ids = run
+        png, rng_ = self._group_lengths()
+        rng_.update((t, png.pop(j, 0)) for j, t in zip(jid.tolist(), tid.tolist()))
+
+    def _group_lengths(self):
+        """{job id: group list length} of the live pending rows and {task id: length} of the live running rows."""
+        if not hasattr(self, "_state_group_len"):
+            self._state_group_len = ({}, {})
+        return self._state_group_len
+
+    def state_task_facts(self, task_id, max_runtime_ms=None, cancelled=None, unknown=None):
+        """cook_state_task_facts: the killers' facts of live running tasks (None: unchanged): the job's max-runtime in
+        ms (-1: none), the cancelled flag, and whether the status is unknown rather than running."""
+        tid = np.ascontiguousarray(task_id, np.int64)
+        cols = [np.ascontiguousarray(c, dt) if c is not None else None
+                for c, dt in ((max_runtime_ms, np.int64), (cancelled, np.uint8), (unknown, np.uint8))]
+        if any(c is not None and len(c) != len(tid) for c in cols):
+            raise ValueError("state_task_facts: a column's length differs from task_id's")
+        mr, ca, un = cols
+        rc = self.lib.cook_state_task_facts(self.pool, len(tid), abi.ptr(tid, abi.P_I64),
+                                            abi.ptr(mr, abi.P_I64) if mr is not None else None,
+                                            abi.ptr(ca, abi.P_U8) if ca is not None else None,
+                                            abi.ptr(un, abi.P_U8) if un is not None else None)
+        if rc != 0:
+            self._err(rc)
+
+    def state_finish(self, task_id, end_time_ms=None, success=None):
+        """cook_state_finish: the tasks leave as a removal delta would take them; each successful one leaves a runtime
+        record per group of its list (success None: none succeeded)."""
+        tid = np.ascontiguousarray(task_id, np.int64)
+        end = np.ascontiguousarray(end_time_ms, np.int64) if end_time_ms is not None else None
+        ok = np.ascontiguousarray(success, np.uint8) if success is not None else None
+        if any(c is not None and len(c) != len(tid) for c in (end, ok)):
+            raise ValueError("state_finish: end_time_ms or success differs in length from task_id")
+        rc = self.lib.cook_state_finish(self.pool, len(tid), abi.ptr(tid, abi.P_I64),
+                                        abi.ptr(end, abi.P_I64) if end is not None else None,
+                                        abi.ptr(ok, abi.P_U8) if ok is not None else None)
+        if rc != 0:
+            self._err(rc)
+        getattr(self, "_state_running_ids", set()).difference_update(tid.tolist())
+        rng_ = self._group_lengths()[1]
+        for t in tid.tolist():
+            rng_.pop(t, None)
+
+    def state_group_runtimes(self, group=(), runtime_s=(), forget=()):
+        """cook_state_group_runtimes: the records of the groups in `forget` leave, then (group[i], runtime_s[i]) are
+        appended."""
+        g = np.ascontiguousarray(group, np.int32)
+        r = np.ascontiguousarray(runtime_s, np.int32)
+        f = np.ascontiguousarray(forget, np.int32)
+        if len(g) != len(r):
+            raise ValueError("state_group_runtimes: group and runtime_s differ in length")
+        rc = self.lib.cook_state_group_runtimes(self.pool, len(g), abi.ptr(g, abi.P_I32) if len(g) else None,
+                                                abi.ptr(r, abi.P_I32) if len(r) else None, len(f),
+                                                abi.ptr(f, abi.P_I32) if len(f) else None)
+        if rc != 0:
+            self._err(rc)
 
     def state_patch(self, job_id, allowed=None, plugin_accept=None, reserved_host=None, clear_reservations=False):
         """cook_state_patch: the given match-time columns of live pending jobs, in place (None: unchanged).
@@ -520,6 +591,55 @@ def exchange_usage_batch(engines, n_users_pad, n_slots=None, comm=None, world=1)
     if rc != 0:
         engines[0]._err(rc)
     return out.reshape(world, n_slots, n_users_pad, 4)
+
+
+def state_sweep(engines, now_ms, default_timeout_ms, max_timeout_ms, groups=None, lists=("linger", "cancel", "straggler")):
+    """cook_state_sweep over the live running rows of `engines` (one device, the work on engines[0]'s stream).
+    groups: {"kind", "quantile", "multiplier", "n_jobs"} arrays by group code (None: no group).  lists: which of
+    "linger", "cancel" and "straggler" to sweep.  Returns 'linger' and 'cancel' as [(task id, engine index)],
+    'straggler' as [(group, task id, engine index)] (a list not asked for: None), and 'stats' (the call's own)."""
+    if not engines:
+        raise ValueError("state_sweep: at least one handle")
+    g = groups or {}
+    G = len(g.get("kind", ()))
+    kind = np.ascontiguousarray(g.get("kind", ()), np.int32)
+    q = np.ascontiguousarray(g.get("quantile", ()), np.float64)
+    m = np.ascontiguousarray(g.get("multiplier", ()), np.float64)
+    nj = np.ascontiguousarray(g.get("n_jobs", ()), np.int32)
+    if not len(kind) == len(q) == len(m) == len(nj):
+        raise ValueError("state_sweep: the group columns differ in length")
+    R = sum(len(getattr(e, "_state_running_ids", ())) for e in engines)
+    N = sum(sum(e._group_lengths()[1].values()) for e in engines)
+    out = {}
+    for k, n_cols, cap in (("linger", 2, R), ("cancel", 2, R), ("straggler", 3, N)):
+        if k in lists:
+            cols = ([np.zeros(max(cap, 1), np.int32)] if n_cols == 3 else []) + [np.zeros(max(cap, 1), np.int64),
+                                                                              np.zeros(max(cap, 1), np.int32)]
+            out[k] = (cols, C.c_int32(0))
+    def arg(k, i):
+        if k not in out:
+            return None
+        a = out[k][0][i]
+        return abi.ptr(a, abi.P_I64 if a.dtype == np.int64 else abi.P_I32)
+    cnt = lambda k: C.byref(out[k][1]) if k in out else None
+    st = abi.PhaseStats()
+    handles = (C.c_void_p * len(engines))(*[e.pool for e in engines])
+    rc = engines[0].lib.cook_state_sweep(
+        handles, len(engines), int(now_ms), int(default_timeout_ms), int(max_timeout_ms), G,
+        abi.ptr(kind, abi.P_I32) if G else None, abi.ptr(q, abi.P_F64) if G else None,
+        abi.ptr(m, abi.P_F64) if G else None, abi.ptr(nj, abi.P_I32) if G else None, R, arg("linger", 0),
+        arg("linger", 1), cnt("linger"), arg("cancel", 0), arg("cancel", 1), cnt("cancel"), N, arg("straggler", 0),
+        arg("straggler", 1), arg("straggler", 2), cnt("straggler"), C.byref(st))
+    if rc != 0:
+        engines[0]._err(rc)
+    res = {"stats": st.as_dict()}
+    for k in ("linger", "cancel", "straggler"):
+        if k not in out:
+            res[k] = None
+            continue
+        cols, n = out[k]
+        res[k] = list(zip(*[c[:n.value].tolist() for c in cols]))
+    return res
 
 
 STATS_KEYS = ("running", "waiting", "starved", "waiting-under-quota")   # by abi.STATS_*

@@ -872,8 +872,8 @@ int32_t cook_state_queue(cook_pool* pool, int32_t cap, int64_t* out_job_id, int3
 /* ------------------------------------------------------------ phase timing */
 /* Device-side timing of the last call of each kind on this handle (CUDA events on the
  * pool's stream): what bench.py's `phases` block and roofline lines are computed from.
- * COOK_PHASE_STATE: the last cook_state_apply, cook_state_launch or cook_state_patch (upload, then the
- * scatter / move / compaction kernels).  COOK_PHASE_USAGE: the last cook_state_usage (upload of the
+ * COOK_PHASE_STATE: the last cook_state_apply, cook_state_launch, cook_state_patch, cook_state_task_facts,
+ * cook_state_finish or cook_state_group_runtimes (upload, then the scatter / move / record / compaction kernels).  COOK_PHASE_USAGE: the last cook_state_usage (upload of the
  * hostname list, the compaction, sorts and folds, the download of the sums).  COOK_PHASE_COTASKS: the last
  * cook_state_cotasks (upload of the host codes, attribute columns and group map, the compaction, expansion and
  * sort, the download of the lists; all zero after a call without device work).  COOK_PHASE_CONSIDERABLE: the last
@@ -946,6 +946,88 @@ int32_t cook_state_user_stats(cook_pool* const* pools, int32_t n_pools, const co
                               const uint8_t* quota_rest_ok, int64_t* out_jobs, double* out_cpus, double* out_mem,
                               uint8_t* out_member, int64_t* out_all_jobs, double* out_all_cpus, double* out_all_mem,
                               int64_t* out_users, cook_phase_stats* out_stats);
+
+/* ------------------------------------------ the periodic killers over resident pools */
+/* What the cancelled-task killer (killable-cancelled-tasks, scheduler.clj:1988-2016), the lingering-task killer
+ * (get-lingering-tasks :1888-1953) and the straggler handler (handle-stragglers :1955-1986, find-stragglers
+ * :quantile-deviation, group.clj:17-45) read, kept on the resident rows, and the three lists swept on the device.
+ * All times are ms since the epoch, as cook_tasks_soa.start_time.
+ *
+ * Facts on live running rows, by task id: max_runtime_ms[i] (the job's :job/max-runtime, -1: none), cancelled[i]
+ * (:instance/cancelled) and unknown[i] (status unknown rather than running); a NULL column is left unchanged.  Like
+ * cook_state_patch, the row keeps its live flag and generation.  Every running upsert of cook_state_apply and every
+ * cook_state_launch writes the absent facts (no max-runtime, not cancelled, running), so an upsert of a known running id
+ * resets them.  The facts are not part of cook_state_digest or cook_state_export: after a resync the caller sends them
+ * again.
+ * COOK_E_BADARG, before any change: n < 0; a NULL task_id while n > 0; a task id that is not live or appears twice;
+ * a max_runtime_ms below -1.  Uploads exactly, when n > 0 and some column is given: n * (4 + [max_runtime_ms] 8 +
+ * [cancelled or unknown] 1) bytes.  Statistics: cook_last_stats(COOK_PHASE_STATE).                                */
+int32_t cook_state_task_facts(cook_pool* pool, int32_t n, const int64_t* task_id, const int64_t* max_runtime_ms,
+                              const uint8_t* cancelled, const uint8_t* unknown);
+
+/* Finished tasks by id.  Leaves exactly the state cook_state_apply with running_rm_task_id = task_id leaves for every
+ * other call (rows, list arenas, counts, digest, export, queue).  In addition, each row with success[i] != 0 appends one
+ * runtime record (group code, runtime_s) per entry of its group list to the handle's record table, runtime_s =
+ * (end_time_ms[i] - start) / 1000 truncated (Joda's in-seconds of the interval), computed on the device from the row's
+ * start time.  success NULL: no row succeeded (end_time_ms may then be NULL).  A reset through cook_state_apply drops
+ * every record; cook_state_digest and cook_state_export do not cover them: after a resync the caller seeds them again
+ * (cook_state_group_runtimes).
+ * COOK_E_BADARG, before any change: n < 0; a NULL task_id while n > 0; success without end_time_ms; a task id that is
+ * not live or appears twice; a successful row whose end is before its start (the reference's interval throws; this
+ * error is ours) or whose runtime is 2^31 s or more.  COOK_E_TOO_LARGE: more than 2^31 - 1 records.
+ * Uploads exactly, when n > 0: 4 * n (the slots) + 9 * n when success is given (success, end_time_ms).
+ * Statistics: cook_last_stats(COOK_PHASE_STATE).                                                                  */
+int32_t cook_state_finish(cook_pool* pool, int32_t n, const int64_t* task_id, const int64_t* end_time_ms,
+                          const uint8_t* success);
+
+/* The record table by hand: first every record of the groups forget_group[0, n_forget) leaves (groups the caller no
+ * longer tracks), then n_add records (group[i], runtime_s[i]) are appended: the successes that finished before the
+ * rows were resident (after a reset or a leadership change).
+ * COOK_E_BADARG, before any change: a negative size; a NULL array with its size > 0; a negative group code or
+ * runtime.  COOK_E_TOO_LARGE: more than 2^31 - 1 records.  Uploads exactly 4 * (the distinct codes of forget_group)
+ * + 8 * n_add bytes.  Statistics: cook_last_stats(COOK_PHASE_STATE).                                           */
+int32_t cook_state_group_runtimes(cook_pool* pool, int32_t n_add, const int32_t* group, const int32_t* runtime_s,
+                                  int32_t n_forget, const int32_t* forget_group);
+
+/* The three kill lists over the union of the live running rows of pools[0, n_pools): the handles follow
+ * cook_state_user_stats' rules (one device, idle, the work on pools[0]'s stream and scratch).  Each list comes with
+ * the index in pools of the handle that holds the row.  A NULL task-id array skips that sweep and its kernels.
+ *   Lingering  (out_linger_*) every row, running or unknown, with now_ms - start > min(max_runtime, max_timeout_ms),
+ *              max_runtime the row's max_runtime_ms or default_timeout_ms when it has none; int64, strict (a row whose
+ *              boundary equals now_ms is not lingering).  The caller derives both timeouts from its hours as
+ *              kill-lingering-tasks does (:1912-1918).
+ *   Cancelled  (out_cancel_*) every row with the cancelled fact, running or unknown.
+ *   Stragglers (out_straggler_*) for each group g < n_groups with group_kind[g] == COOK_SWEEP_QUANTILE_DEVIATION:
+ *              idx = (int)((double)(n_jobs[g] - 1) * quantile[g]) (truncated toward zero; n_jobs[g] counts the group's
+ *              jobs in every state); when the group has more than idx live records, limit = (double)(its idx-th
+ *              smallest runtime_s) * multiplier[g], and every row of status running (not unknown) with g in its group
+ *              list and (double)((now_ms - start) / 1000) > limit is a straggler of g.  A row in several groups is
+ *              judged once per group.  COOK_SWEEP_NONE yields nothing; so does idx < 0 (n_jobs 0 with quantile 1,
+ *              where the reference's nth throws).
+ * Orders (the reference returns sets): lingering and cancelled by ascending task id, a task id several handles hold
+ * by pool index; stragglers by ascending (group, task id, pool index).  *out_n_* gets each list's length.
+ * Capacities: row_cap >= the live running rows (lingering, cancelled), entry_cap >= the live running rows' group
+ * entries (stragglers).  Changes nothing resident.
+ * COOK_E_BADARG, before any device work and with nothing written: cook_state_user_stats' handle cases; a list without
+ * its pool column or count; n_groups < 0; (stragglers) a NULL group_kind, quantile, multiplier or n_jobs with
+ * n_groups > 0, an unknown kind, a quantile outside [0, 1] for a checked group, a negative n_jobs, a live running
+ * row's group or a record's group >= n_groups; a capacity below the required size.  COOK_E_BADARG after the sweep
+ * and with nothing written: a running row of a checked group that starts after now_ms (the reference's interval
+ * throws and aborts the sweep; this error is ours).
+ * No live row to judge: empty lists without device work.
+ * Transfers exactly: up 24 * n_groups (the four group columns) when the stragglers are swept over some group entry;
+ * down 16 (the counts) + 12 per lingering and per cancelled row + 16 per straggler.  Nothing that scales with the
+ * running table crosses the bus.
+ * Statistics: out_stats (may be NULL), as cook_state_user_stats; no cook_last_stats slot is written.  The parameters
+ * are plain arguments, like cook_state_user_stats' outputs: every struct of this header has a ctypes mirror. */
+enum { COOK_SWEEP_NONE = 0, COOK_SWEEP_QUANTILE_DEVIATION = 1 };
+int32_t cook_state_sweep(cook_pool* const* pools, int32_t n_pools, int64_t now_ms, int64_t default_timeout_ms,
+                         int64_t max_timeout_ms, int32_t n_groups, const int32_t* group_kind, const double* quantile,
+                         const double* multiplier, const int32_t* n_jobs, int32_t row_cap, int64_t* out_linger_task_id,
+                         int32_t* out_linger_pool, int32_t* out_n_linger, int64_t* out_cancel_task_id,
+                         int32_t* out_cancel_pool, int32_t* out_n_cancel, int32_t entry_cap,
+                         int32_t* out_straggler_group, int64_t* out_straggler_task_id, int32_t* out_straggler_pool,
+                         int32_t* out_n_straggler, cook_phase_stats* out_stats);
 
 /* ----------------------------------------------------------------- multi-GPU */
 /* §8e: after a pool's match round every rank contributes its pools' usage

@@ -278,6 +278,47 @@ JFN(jint, stateUserStats)(JNIEnv* env, jclass k, jlongArray pools, jint n_users,
                                one(env, out_mem), one(env, out_member), one(env, out_all_jobs), one(env, out_all_cpus),
                                one(env, out_all_mem), one(env, out_users), one(env, out_stats));
 }
+/* the killers' facts of live running tasks: task_id n longs, max_runtime_ms n longs, cancelled / unknown n bytes (each
+ * but task_id may be null: unchanged) */
+JFN(jint, stateTaskFacts)(JNIEnv* env, jclass k, jlong pool, jint n, jobject task_id, jobject max_runtime_ms,
+                          jobject cancelled, jobject unknown) {
+  return cook_state_task_facts((cook_pool*)(intptr_t)pool, n, one(env, task_id), one(env, max_runtime_ms),
+                               one(env, cancelled), one(env, unknown));
+}
+/* finished tasks: task_id and end_time_ms n longs, success n bytes (null: none succeeded) */
+JFN(jint, stateFinish)(JNIEnv* env, jclass k, jlong pool, jint n, jobject task_id, jobject end_time_ms,
+                       jobject success) {
+  return cook_state_finish((cook_pool*)(intptr_t)pool, n, one(env, task_id), one(env, end_time_ms), one(env, success));
+}
+/* records by hand: (group, runtime_s) n_add ints each, then forget_group n_forget ints */
+JFN(jint, stateGroupRuntimes)(JNIEnv* env, jclass k, jlong pool, jint n_add, jobject group, jobject runtime_s,
+                              jint n_forget, jobject forget_group) {
+  return cook_state_group_runtimes((cook_pool*)(intptr_t)pool, n_add, one(env, group), one(env, runtime_s), n_forget,
+                                   one(env, forget_group));
+}
+/* the three kill lists over `pools` (a long[] of handles on one device, at most 64); times = {now_ms,
+ * default_timeout_ms, max_timeout_ms}; groups: the four group columns (kind, quantile, multiplier, n_jobs), n_groups
+ * values each; lists: {linger task id, linger pool, cancel task id, cancel pool, straggler group, straggler task id,
+ * straggler pool} (a null task id skips that sweep); caps = {row_cap, entry_cap}; out_n gets the three lengths */
+JFN(jint, stateSweep)(JNIEnv* env, jclass k, jlongArray pools, jlongArray times, jint n_groups, jobjectArray groups,
+                      jintArray caps, jobjectArray lists, jintArray out_n, jobject out_stats) {
+  jsize n = (*env)->GetArrayLength(env, pools);
+  if (n > 64) return COOK_E_BADARG;
+  jlong* h = (*env)->GetLongArrayElements(env, pools, NULL);
+  cook_pool* p[64];
+  for (jsize i = 0; i < n; i++) p[i] = (cook_pool*)(intptr_t)h[i];
+  (*env)->ReleaseLongArrayElements(env, pools, h, JNI_ABORT);
+  jlong t[3]; (*env)->GetLongArrayRegion(env, times, 0, 3, t);
+  jint c[2]; (*env)->GetIntArrayRegion(env, caps, 0, 2, c);
+  int32_t nl = 0, nc = 0, ns = 0;
+  jint rc = cook_state_sweep(p, (int32_t)n, t[0], t[1], t[2], n_groups, buf(env, groups, 0), buf(env, groups, 1),
+                             buf(env, groups, 2), buf(env, groups, 3), c[0], buf(env, lists, 0), buf(env, lists, 1),
+                             &nl, buf(env, lists, 2), buf(env, lists, 3), &nc, c[1], buf(env, lists, 4),
+                             buf(env, lists, 5), buf(env, lists, 6), &ns, one(env, out_stats));
+  jint got[3] = {nl, nc, ns};
+  (*env)->SetIntArrayRegion(env, out_n, 0, 3, got);
+  return rc;
+}
 /* the fingerprints and the recount of the resident rows: out_digest is a direct buffer of sizeof(cook_state_digest_out),
  * out_pending_bucket / out_running_bucket direct buffers of n_buckets cook_fp each (null when n_buckets == 0) */
 JFN(jint, stateDigest)(JNIEnv* env, jclass k, jlong pool, jint n_buckets, jobject out_digest, jobject out_pending_bucket,

@@ -25,6 +25,14 @@ placements are identical.
   python tools/prof_state.py --offers --cycles 8
   python tools/prof_state.py --offers --c3-pool 0 --cycles 6
 
+--sweeps loads a running table (C2's, or config-#5 pool --c5-pool with --pool c5) into a resident handle, gives
+about 20 % of its rows group lists, a few thousand successful runtimes, max-runtimes, cancelled and unknown facts,
+and times cook_state_sweep per list and for all three against a numpy restatement over a host mirror of the same
+rows (median of --reps calls): device time, wall time, bytes, launches, and whether the lists are identical.
+
+  python tools/prof_state.py --sweeps --pool c2 --reps 30
+  python tools/prof_state.py --sweeps --pool c5 --c5-pool 5 --reps 30
+
 --launch runs the same cycles on two resident handles instead of the host arm.  Each cycle's launches go to one
 handle through cook_state_launch (job ids, task ids, start times, the hosts the match chose) and to its twin through
 the equivalent cook_state_apply batch (the jobs' removal plus their task rows); the rest of the batch goes to both
@@ -109,7 +117,7 @@ import time
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from cook_b200 import abi, traces  # noqa: E402
+from cook_b200 import abi, engine, traces  # noqa: E402
 from cook_b200.engine import GpuEngine  # noqa: E402
 
 COLS = ("user", "cpus", "mem", "gpus", "ports", "allowed", "plugin_accept", "gpu_model", "disk_request", "disk_type",
@@ -771,6 +779,96 @@ def audit_prof(a):
     res.close()
 
 
+def host_sweeps(m, now, dflt, mx, gp, lists):
+    """The three lists in numpy over the host mirror m (the columns of the handle's rows and records)."""
+    out = {}
+    if "linger" in lists:
+        lim = np.minimum(np.where(m["maxrt"] < 0, dflt, m["maxrt"]), mx)
+        k = np.flatnonzero(now - m["start"] > lim)
+        out["linger"] = np.sort(m["tid"][k])
+    if "cancel" in lists:
+        out["cancel"] = np.sort(m["tid"][m["cancelled"]])
+    if "straggler" in lists:
+        G = len(gp["kind"])
+        chk = gp["kind"] == abi.SWEEP_QUANTILE_DEVIATION
+        rg, rt = m["rec_group"], m["rec_rt"]
+        keep = chk[rg]
+        rg, rt = rg[keep], rt[keep]
+        o = np.lexsort((rt, rg))
+        rg, rt = rg[o], rt[o]
+        cnt = np.bincount(rg, minlength=G)
+        first = np.concatenate(([0], np.cumsum(cnt)[:-1]))
+        idx = ((gp["n_jobs"] - 1).astype(np.float64) * gp["quantile"]).astype(np.int64)
+        ok = chk & (idx >= 0) & (cnt > idx)
+        limit = np.full(G, np.inf)
+        limit[ok] = rt[first[ok] + idx[ok]].astype(np.float64) * gp["multiplier"][ok]
+        eg, row = m["e_group"], m["e_row"]
+        run = ~m["unknown"][row] & chk[eg]
+        secs = (now - m["start"][row]) // 1000
+        hit = run & (secs.astype(np.float64) > limit[eg])
+        g, t = eg[hit], m["tid"][row[hit]]
+        o = np.lexsort((t, g))
+        out["straggler"] = (g[o], t[o])
+    return out
+
+
+def sweeps_prof(a):
+    t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
+    rc = {k: np.asarray(v).copy() for k, v in t["cols"]["running"].items()}
+    rng = np.random.default_rng(a.seed)
+    n, G = len(rc["task_id"]), 400
+    glen = np.where(rng.random(n) < 0.2, rng.integers(1, 3, n), 0)
+    goff = np.concatenate(([0], np.cumsum(glen))).astype(np.int32)
+    gidx = rng.integers(0, G, int(goff[-1])).astype(np.int32)
+    now = int(rc["start_time"].max()) + 3_600_000
+    rc["start_time"] = now - rng.integers(1000, 48 * 3_600_000, n)
+    e = GpuEngine(pool_name="sweeps")
+    e.state_apply(abi.make_delta(reset=True, running=abi.make_tasks(**rc), running_group_off=goff,
+                                 running_group_idx=gidx))
+    tid = rc["task_id"].astype(np.int64)
+    maxrt = np.where(rng.random(n) < 0.1, rng.integers(3_600_000, 30 * 3_600_000, n), -1).astype(np.int64)
+    canc, unk = rng.random(n) < 0.02, rng.random(n) < 0.05
+    e.state_task_facts(tid, maxrt, canc, unk)
+    n_rec = 4000
+    rec_group = rng.integers(0, G, n_rec).astype(np.int32)
+    rec_rt = rng.integers(600, 20 * 3600, n_rec).astype(np.int32)
+    e.state_group_runtimes(rec_group, rec_rt)
+    gp = {"kind": np.where(rng.random(G) < 0.8, abi.SWEEP_QUANTILE_DEVIATION, abi.SWEEP_NONE).astype(np.int32),
+          "quantile": rng.choice([0.25, 0.5, 0.9], G), "multiplier": rng.choice([1.5, 2.0, 3.0], G),
+          "n_jobs": rng.integers(5, 40, G).astype(np.int32)}
+    mirror = {"tid": tid, "start": rc["start_time"].astype(np.int64), "maxrt": maxrt, "cancelled": canc,
+              "unknown": unk, "rec_group": rec_group, "rec_rt": rec_rt, "e_group": gidx,
+              "e_row": np.repeat(np.arange(n), glen)}
+    dflt, mx = 24 * 3_600_000, 36 * 3_600_000
+    print(json.dumps({"card": card(), "pool": a.pool if a.pool == "c2" else f"c5/{a.c5_pool}", "running": n,
+                      "grouped_rows": int((glen > 0).sum()), "group_entries": int(goff[-1]), "records": n_rec,
+                      "groups": G}), flush=True)
+    for lists in (("linger",), ("cancel",), ("straggler",), ("linger", "cancel", "straggler")):
+        got = None
+        for _ in range(3):   # warm-up: the carves and the first launches
+            got = engine.state_sweep([e], now, dflt, mx, gp, lists)
+        dev, wall, host = [], [], []
+        for _ in range(a.reps):
+            w0 = time.perf_counter()
+            got = engine.state_sweep([e], now, dflt, mx, gp, lists)
+            wall.append(time.perf_counter() - w0)
+            dev.append(got["stats"]["ms_h2d"] + got["stats"]["ms_device"] + got["stats"]["ms_d2h"])
+            w0 = time.perf_counter()
+            want = host_sweeps(mirror, now, dflt, mx, gp, lists)
+            host.append(time.perf_counter() - w0)
+        same = all(np.array_equal([x[0] for x in got[k]], want[k]) for k in ("linger", "cancel") if k in lists)
+        if "straggler" in lists:
+            same = same and np.array_equal([x[0] for x in got["straggler"]], want["straggler"][0]) and \
+                np.array_equal([x[1] for x in got["straggler"]], want["straggler"][1])
+        st = got["stats"]
+        print(json.dumps({"lists": "+".join(lists), "n": {k: len(got[k]) for k in lists},
+                          "device_ms": round(float(np.median(dev)), 4), "wall_ms": round(1e3 * float(np.median(wall)), 4),
+                          "h2d_bytes": st["h2d_bytes"], "d2h_bytes": st["d2h_bytes"], "n_launches": st["n_launches"],
+                          "numpy_wall_ms": round(1e3 * float(np.median(host)), 4), "identical": bool(same)}),
+              flush=True)
+    e.close()
+
+
 def rank_quota_prof(a):
     t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
     pc, rc0, users = t["cols"]["pending"], t["cols"]["running"], t["users"]
@@ -831,8 +929,11 @@ def main():
     ap.add_argument("--user-stats", action="store_true")
     ap.add_argument("--c3-group", type=int, default=0, help="--user-stats: a quota group of config-#3 pools 0 .. N-1")
     ap.add_argument("--rank-quota", action="store_true")
-    ap.add_argument("--reps", type=int, default=20, help="--audit, --rank-quota: timed calls per kind")
+    ap.add_argument("--sweeps", action="store_true", help="cook_state_sweep against numpy over a host mirror")
+    ap.add_argument("--reps", type=int, default=20, help="--audit, --rank-quota, --sweeps: timed calls per kind")
     a = ap.parse_args()
+    if a.sweeps:
+        return sweeps_prof(a)
     if a.rank_quota:
         return rank_quota_prof(a)
     if a.audit:
