@@ -12,6 +12,7 @@
 ;;   :1888-2016 the three killers            -> (sweep! ...), fed by task-facts! / finish! / group-runtimes!
 ;;                                              [cook_state_sweep, cook_state_task_facts, cook_state_finish,
 ;;                                               cook_state_group_runtimes]
+;;   unscheduled.clj:172-200 reasons      -> (unscheduled! ...) + cycle.py's unscheduled_reasons  [cook_state_unscheduled]
 ;; selected per pool with {:scheduler-config {:scheduler "gpu"}} next to "fenzo" / "kubernetes"
 ;; (config.clj:110-122, make-pool-handler :2425-2466).  Everything numeric happens in libcookgpu;
 ;; this namespace marshals columns and keeps the state Fenzo kept (cook_b200/cycle.py is the same
@@ -386,3 +387,26 @@
         (kinds :linger) (assoc :linger (rows (aget out-n 0) [[(lists 0) 8] [(lists 1) 4]]))
         (kinds :cancel) (assoc :cancel (rows (aget out-n 1) [[(lists 2) 8] [(lists 3) 4]]))
         (kinds :straggler) (assoc :straggler (rows (aget out-n 2) [[(lists 4) 4] [(lists 5) 8] [(lists 6) 4]]))))))
+
+;; ---------------------------------------------------------------------------------------------
+;; /unscheduled_jobs over a resident pool: the device half of reasons (unscheduled.clj:172-200)
+(def ^:const unsched-ahead 10)
+
+(defn unscheduled!
+  "The queried job ids of one pool's handle: [{:status (:absent :waiting :running) :usage {:count :cpus :mem :gpus}
+   (waiting: the user's running jobs plus the job) :position :ahead [job ids] :plugin-deferred?}] by query.  The
+   handler compares :usage with the user's quota and share in the pool (strict >, only the keys present) and assembles
+   the reasons in the reference's order, as cook_b200/cycle.py's unscheduled_reasons does."
+  [handle job-ids]
+  (let [n (count job-ids)
+        st (direct (max 1 n)) us (direct (* 32 (max 1 n))) pos (direct (* 4 (max 1 n))) na (direct (* 4 (max 1 n)))
+        ah (direct (* 8 unsched-ahead (max 1 n))) pl (direct (max 1 n))]
+    (check! handle (Native/stateUnscheduled handle n (longs-buf job-ids) st us pos na ah pl nil)
+            "cook_state_unscheduled")
+    (vec (for [i (range n)]
+           (let [k (.getInt ^ByteBuffer na (int (* 4 i)))]
+             {:status ([:absent :waiting :running] (.get ^ByteBuffer st (int i)))
+              :usage (zipmap [:count :cpus :mem :gpus] (for [c (range 4)] (.getDouble ^ByteBuffer us (int (* 8 (+ (* 4 i) c))))))
+              :position (.getInt ^ByteBuffer pos (int (* 4 i)))
+              :ahead (vec (for [j (range k)] (.getLong ^ByteBuffer ah (int (* 8 (+ (* unsched-ahead i) j))))))
+              :plugin-deferred? (= 1 (.get ^ByteBuffer pl (int i)))})))))

@@ -152,6 +152,8 @@ USAGE_GIVEN, USAGE_DERIVED, USAGE_LAST_MATCH = 0, 1, 2
 SWEEP_NONE, SWEEP_QUANTILE_DEVIATION = 0, 1
 # cook_state_match_offers: why an offer left the live set
 OFFER_USED, OFFER_EXPIRED, OFFER_SINGLE_SHOT = 1, 2, 3
+# cook_state_unscheduled: a queried job's status, and the most job ids ahead it returns
+UNSCHED_ABSENT, UNSCHED_WAITING, UNSCHED_RUNNING, UNSCHED_AHEAD = 0, 1, 2, 10
 
 
 class ConsiderableParams(C.Structure):
@@ -334,6 +336,7 @@ ARGTYPES = {
     "cook_state_group_runtimes": [_H, _I32, P_I32, P_I32, _I32, P_I32],
     "cook_state_sweep": [_P(_H), _I32, C.c_int64, C.c_int64, C.c_int64, _I32, P_I32, P_F64, P_F64, P_I32, _I32, P_I64,
                          P_I32, P_I32, P_I64, P_I32, P_I32, _I32, P_I32, P_I64, P_I32, P_I32, _P(PhaseStats)],
+    "cook_state_unscheduled": [_H, _I32, P_I64, P_U8, P_F64, P_I32, P_I32, P_I64, P_U8, _P(PhaseStats)],
     "cook_last_stats": [_H, _I32, _P(PhaseStats)],
     "cook_allgather_usage": [_H, _H, P_F64, P_F64, C.c_int64],
     "cook_comm_unique_id": [P_U8],

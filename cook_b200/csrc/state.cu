@@ -730,6 +730,8 @@ struct PoolState {
   std::vector<std::vector<int32_t>> rgroups;   // by running slot: its group list
   std::vector<int64_t> rstart;                 // by running slot: its start time (cook_state_finish's checks)
   std::vector<uint8_t> rfacts;                 // by running slot: its RF_* bits
+  std::vector<int64_t> rjid, rtid;             // by running slot: its job id and task id
+  std::unordered_map<int64_t, std::vector<int32_t>> jobs_r;   // job id -> its live running slots (cook_state_unscheduled)
   int64_t grp_rows = 0;                        // live running rows with a group list
   Records rec;                                 // the successful runtimes per group
   std::map<int32_t, int64_t> rec_groups;       // group code -> live records
@@ -796,11 +798,19 @@ struct PoolState {
       cot_rows += sign;
       cot_n += sign * (int64_t)g.size();
     }
+    if (sign > 0) {
+      jobs_r[rjid[slot]].push_back(slot);
+    } else {
+      auto it = jobs_r.find(rjid[slot]);
+      std::vector<int32_t>& v = it->second;
+      v.erase(std::find(v.begin(), v.end(), slot));
+      if (v.empty()) jobs_r.erase(it);
+    }
   }
   void running_room(int32_t slot) {
     if ((size_t)slot < ruser.size()) return;
     const size_t n = std::max<size_t>(slot + 1, 2 * ruser.size());
-    ruser.resize(n); rhost.resize(n); rgroups.resize(n); rstart.resize(n); rfacts.resize(n);
+    ruser.resize(n); rhost.resize(n); rgroups.resize(n); rstart.resize(n); rfacts.resize(n); rjid.resize(n); rtid.resize(n);
   }
   // a live pending slot's flag f after a patch of its column
   void set_flag(int32_t slot, int f, bool on) {
@@ -986,6 +996,7 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
     }
     S->users_p.clear(); S->users_r.clear(); S->attr_cols.clear(); S->groups.clear(); S->hosts_r.clear();
     S->groups_r.clear();
+    S->jobs_r.clear();
     S->cot_rows = S->cot_n = S->grp_rows = 0;
     S->rec.tail = S->rec.n_live = 0;
     S->rec_groups.clear();
@@ -1051,6 +1062,7 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
     S->rgroups[s].assign(rgo ? d->running_group_idx + rgo[i] : nullptr, rgo ? d->running_group_idx + rgo[i + 1] : nullptr);
     S->rstart[s] = T.start_time[i];
     S->rfacts[s] = 0;
+    S->rjid[s] = T.job_id[i]; S->rtid[s] = T.task_id[i];
     S->add_running(s, +1);
     rup_slot[i] = s;
   }
@@ -1183,6 +1195,7 @@ int32_t launch(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, cons
     S->rgroups[r] = S->pinfo[pslot[i]].groups;
     S->rstart[r] = start_time[i];
     S->rfacts[r] = 0;
+    S->rjid[r] = job_id[i]; S->rtid[r] = task_id[i];
     S->add_running(r, +1);
     ng += (int64_t)S->rgroups[r].size();
     rslot[i] = r;
@@ -3463,6 +3476,294 @@ extern "C" int32_t cook_state_sweep(cook_pool* const* pools, int32_t n_pools, in
                n_jobs, row_cap, out_linger_task_id, out_linger_pool, out_n_linger, out_cancel_task_id, out_cancel_pool,
                out_n_cancel, entry_cap, out_straggler_group, out_straggler_task_id, out_straggler_pool, out_n_straggler,
                out_stats);
+}
+
+// ---- why a job is not scheduled (/unscheduled_jobs, unscheduled.clj:172-200): each queried job's status, its user's
+// running usage plus the job, its place among its user's entries and the jobs ahead, and its plugin flag.  The host
+// resolves each queried id to its row (a pending slot, or the running row of the job with the greatest task id) and
+// its user; the device takes the live rows of the queried users, keeps one running row per (user, job), folds the
+// users' usage over those in ascending task id and orders the users' entries as rank does.
+namespace {
+
+// the queried users: umap[user code] = its index k in quser, -1 for any other code; rank[k] = k (LessUserTask's name
+// ranks: users in index order, and index nU last)
+__global__ void unsched_users_kernel(const int32_t* quser, int nU, int32_t* umap, int32_t* rank) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k > nU) return;
+  rank[k] = k;
+  if (k < nU) umap[quser[k]] = k;
+}
+
+// The entries: the queried users' live running rows dense in [0, R), their live pending rows in [R, R + J), as rank's
+// task columns plus each entry's slot.  key: a pending entry's user index; the running entries' is written by
+// unsched_rep_kernel.  ru: a running entry's user index.
+struct UnschedCols {
+  int32_t* key; int32_t* ru; int32_t* prio; int64_t* start; int64_t* tid; int64_t* jid; int32_t* slot;
+  double* amt[3];   // [R]: the running entries' cpus, mem, gpus
+};
+struct UnschedRunRows {
+  void* const* col; const int32_t* umap; UnschedCols o;
+  __device__ bool keep(int i) const {
+    return static_cast<const uint8_t*>(col[R_LIVE])[i] && umap[static_cast<const int32_t*>(col[R_USER])[i]] >= 0;
+  }
+  __device__ void emit(int i, int d) const {
+    o.ru[d] = umap[static_cast<const int32_t*>(col[R_USER])[i]];
+    o.prio[d] = static_cast<const int32_t*>(col[R_PRIO])[i];
+    o.start[d] = static_cast<const int64_t*>(col[R_START])[i];
+    o.tid[d] = static_cast<const int64_t*>(col[R_TID])[i];
+    o.jid[d] = static_cast<const int64_t*>(col[R_JID])[i];
+    o.slot[d] = i;
+    o.amt[0][d] = static_cast<const double*>(col[R_CPUS])[i];
+    o.amt[1][d] = static_cast<const double*>(col[R_MEM])[i];
+    o.amt[2][d] = static_cast<const double*>(col[R_GPUS])[i];
+  }
+};
+struct UnschedPendRows {
+  void* const* col; const int32_t* umap; UnschedCols o; int R;
+  __device__ bool keep(int i) const {
+    return static_cast<const uint8_t*>(col[P_LIVE])[i] && umap[static_cast<const int32_t*>(col[P_USER])[i]] >= 0;
+  }
+  __device__ void emit(int i, int d) const {
+    d += R;
+    o.key[d] = umap[static_cast<const int32_t*>(col[P_USER])[i]];
+    o.prio[d] = static_cast<const int32_t*>(col[P_PRIO])[i];
+    o.start[d] = INT64_MAX;   // a pending job's synthetic task (tools.clj:582-588)
+    o.tid[d] = -1;
+    o.jid[d] = static_cast<const int64_t*>(col[P_JID])[i];
+    o.slot[d] = i;
+  }
+};
+// (user, job id, task id, dense index): a (user, job)'s running rows together, its greatest task id last
+struct LessUserJobTask {
+  const int32_t* u; const int64_t* jid; const int64_t* tid;
+  __device__ bool operator()(int32_t a, int32_t b) const {
+    if (u[a] != u[b]) return u[a] < u[b];
+    if (jid[a] != jid[b]) return jid[a] < jid[b];
+    if (tid[a] != tid[b]) return tid[a] < tid[b];
+    return a < b;
+  }
+};
+// The representative of each (user, job) is its last running row in that order: it keeps its user index as key, the
+// other rows get nU, a segment after every user's that no output reads.
+__global__ void unsched_rep_kernel(const int32_t* ord, int R, const int32_t* ru, const int64_t* jid, int nU,
+                                   int32_t* key) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= R) return;
+  const int i = ord[p];
+  bool rep = p == R - 1;
+  if (!rep) {
+    const int n = ord[p + 1];
+    rep = ru[n] != ru[i] || jid[n] != jid[i];
+  }
+  key[i] = rep ? ru[i] : nU;
+}
+// slot -> position in the entries' order, for the running representatives (rpos) and the pending rows (ppos)
+__global__ void unsched_pos_kernel(const int32_t* ord, int E, int R, const int32_t* key, const int32_t* slot, int nU,
+                                   int32_t* rpos, int32_t* ppos) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= E) return;
+  const int i = ord[p];
+  if (key[i] == nU) return;
+  (i < R ? rpos : ppos)[slot[i]] = p;
+}
+
+struct UnschedArgs {
+  const int32_t* qkey; int Q;   // per query: its pending slot, -2 - its running slot, or -1 (absent)
+  const int32_t *ord, *key, *ostart, *rpos, *ppos; const int64_t* jid;
+  const double* user_out; int nU;   // [4][nU]: count, cpus, mem, gpus of each user's running jobs
+  void* const* pcol;
+  double* usage; int32_t* pos; int32_t* n_ahead; int64_t* ahead; uint8_t* plugin;
+};
+// Thread per query: the position of its entry in its user's segment, the first min(position, AHEAD) entries' job
+// ids (0 past them), and for a waiting job the usage fold continued by the job and the plugin flag.
+__global__ void unsched_query_kernel(UnschedArgs a) {
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= a.Q) return;
+  const int k = a.qkey[q];
+  double u4[4] = {0.0, 0.0, 0.0, 0.0};
+  int pos = -1, na = 0;
+  uint8_t pl = 0;
+  int64_t* ahead = a.ahead + (size_t)q * COOK_UNSCHED_AHEAD;
+  if (k != -1) {
+    const bool wait = k >= 0;
+    const int p = wait ? a.ppos[k] : a.rpos[-2 - k];
+    const int u = a.key[a.ord[p]], s0 = a.ostart[u];
+    pos = p - s0;
+    na = min(pos, (int)COOK_UNSCHED_AHEAD);
+    for (int j = 0; j < na; j++) ahead[j] = a.jid[a.ord[s0 + j]];
+    if (wait) {
+      const int nU = a.nU;
+      u4[0] = a.user_out[u] + 1.0;
+      u4[1] = a.user_out[nU + u] + static_cast<const double*>(a.pcol[P_CPUS])[k];
+      u4[2] = a.user_out[2 * nU + u] + static_cast<const double*>(a.pcol[P_MEM])[k];
+      u4[3] = a.user_out[3 * nU + u] + static_cast<const double*>(a.pcol[P_GPUS])[k];
+      pl = static_cast<const uint8_t*>(a.pcol[P_PLUGIN])[k] == 0;
+    }
+  }
+  for (int j = na; j < COOK_UNSCHED_AHEAD; j++) ahead[j] = 0;
+#pragma unroll
+  for (int c = 0; c < 4; c++) a.usage[4 * (size_t)q + c] = u4[c];
+  a.pos[q] = pos; a.n_ahead[q] = na; a.plugin[q] = pl;
+}
+
+int32_t unscheduled(cook_pool* pool, int n, const int64_t* job_id, uint8_t* out_status, double* out_usage,
+                    int32_t* out_position, int32_t* out_n_ahead, int64_t* out_ahead, uint8_t* out_plugin,
+                    cook_phase_stats* out_stats) {
+  const char* who = "cook_state_unscheduled";
+  // ---- every check before any device work or output
+  if (n < 0) return pool ? set_err(pool, COOK_E_BADARG, "%s: n < 0", who) : COOK_E_BADARG;
+  if (n == 0) {
+    if (out_stats) *out_stats = cook_phase_stats{};
+    return COOK_OK;
+  }
+  if (!pool) return COOK_E_BADARG;
+  if (!job_id || !out_status || !out_usage || !out_position || !out_n_ahead || !out_ahead || !out_plugin)
+    return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
+  // ---- host: each query's row and user, the queried users and their rows' counts, O(n log n)
+  PoolState* S = state_of(pool, false);
+  std::vector<int32_t> qkey(n, -1), qu(n, -1), quser;
+  for (int i = 0; S && i < n; i++) {
+    auto p = S->pend.slot_of.find(job_id[i]);
+    if (p != S->pend.slot_of.end()) {
+      qkey[i] = p->second;
+      qu[i] = S->pinfo[p->second].user;
+      continue;
+    }
+    auto r = S->jobs_r.find(job_id[i]);
+    if (r == S->jobs_r.end()) continue;
+    int32_t best = r->second[0];
+    for (int32_t s : r->second) if (S->rtid[s] > S->rtid[best]) best = s;
+    qkey[i] = -2 - best;
+    qu[i] = S->ruser[best];
+  }
+  for (int i = 0; i < n; i++) {
+    out_status[i] = qkey[i] == -1 ? COOK_UNSCHED_ABSENT : qkey[i] >= 0 ? COOK_UNSCHED_WAITING : COOK_UNSCHED_RUNNING;
+    if (qu[i] >= 0) quser.push_back(qu[i]);
+  }
+  std::sort(quser.begin(), quser.end());
+  quser.erase(std::unique(quser.begin(), quser.end()), quser.end());
+  const int nU = (int)quser.size();
+  if (nU == 0) {   // no queried job in the handle: without device work
+    memset(out_usage, 0, sizeof(double) * 4 * (size_t)n);
+    for (int i = 0; i < n; i++) out_position[i] = -1;
+    memset(out_n_ahead, 0, sizeof(int32_t) * (size_t)n);
+    memset(out_ahead, 0, sizeof(int64_t) * COOK_UNSCHED_AHEAD * (size_t)n);
+    memset(out_plugin, 0, (size_t)n);
+    if (out_stats) *out_stats = cook_phase_stats{};
+    return COOK_OK;
+  }
+  int R = 0, J = 0;
+  for (int32_t u : quser) {
+    auto r = S->users_r.find(u);
+    if (r != S->users_r.end()) R += (int)r->second;
+    auto p = S->users_p.find(u);
+    if (p != S->users_p.end()) J += (int)p->second;
+  }
+  const int E = R + J;
+  const int n_codes = std::max(count_max(S->users_p), count_max(S->users_r)) + 1;
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  // ---- one carve: the maps, the entries, the three orders, the fold, the outputs; up the users and the query keys
+  UnschedCols o = {};
+  int32_t *umap = nullptr, *rank = nullptr, *blk = nullptr, *cnt = nullptr, *ord1 = nullptr, *ord3 = nullptr;
+  int32_t *tmp = nullptr, *ostart = nullptr, *oend = nullptr, *rpos = nullptr, *ppos = nullptr;
+  const int32_t *d_quser = nullptr, *d_qkey = nullptr;
+  GridFlag* gf = nullptr;
+  UsageArgs f = {};
+  UsageSegs& us = f.seg[US_USER];
+  UnschedArgs a = {};
+  const int hw = std::max(S->run.hw, S->pend.hw);
+  int64_t h2d = 0, d2h = 0;
+  CK(pool, carve(S->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+    umap = c.take<int32_t>(n_codes); rank = c.take<int32_t>(nU + 1);
+    blk = c.take<int32_t>((size_t)hw / CP_BLOCK + 2); cnt = c.take<int32_t>(2);
+    o.key = c.take<int32_t>(E); o.prio = c.take<int32_t>(E); o.start = c.take<int64_t>(E);
+    o.tid = c.take<int64_t>(E); o.jid = c.take<int64_t>(E); o.slot = c.take<int32_t>(E);
+    ord3 = c.take<int32_t>(E); tmp = c.take<int32_t>(E);
+    ostart = c.take<int32_t>(nU + 2); oend = c.take<int32_t>(nU + 2);
+    rpos = c.take<int32_t>(std::max(S->run.hw, 1)); ppos = c.take<int32_t>(std::max(S->pend.hw, 1));
+    f.user_out = c.take<double>(4 * (size_t)nU);
+    if (R) {
+      o.ru = c.take<int32_t>(R);
+      for (int k = 0; k < 3; k++) o.amt[k] = c.take<double>(R);
+      ord1 = c.take<int32_t>(R);
+      gf = c.take<GridFlag>(1);
+      us.ord = c.take<int32_t>(R);
+      us.start = c.take<int32_t>(nU + 2); us.end = c.take<int32_t>(nU + 2);
+      for (int k = 0; k < 3; k++) {
+        us.os.part[k] = c.take<double>(R);
+        us.os.tile[k] = c.take<double>(R / OS_TILE + 2);
+      }
+    }
+    a.usage = c.take<double>(4 * (size_t)n); a.pos = c.take<int32_t>(n); a.n_ahead = c.take<int32_t>(n);
+    a.ahead = c.take<int64_t>(COOK_UNSCHED_AHEAD * (size_t)n); a.plugin = c.take<uint8_t>(n);
+    d_quser = c.up(quser.data(), nU);
+    d_qkey = c.up(qkey.data(), n);
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  int nl = 0;
+  CK(pool, cudaMemsetAsync(umap, 0xff, sizeof(int32_t) * (size_t)n_codes, st));
+  unsched_users_kernel<<<(nU + 256) / 256, 256, 0, st>>>(d_quser, nU, umap, rank);
+  nl++;
+  // the entries
+  if (R) compact(UnschedRunRows{S->run.d_col, umap, o}, S->run.hw, nullptr, blk, cnt, R, st, &nl);
+  if (J) compact(UnschedPendRows{S->pend.d_col, umap, o, R}, S->pend.hw, nullptr, blk, cnt + 1, J, st, &nl);
+  // one running row per (user, job), then the users' folds over them in ascending task id (usage_fold_kernel)
+  if (R) {
+    CK(pool, csort::sort_indices(ord1, tmp, R, LessUserJobTask{o.ru, o.jid, o.tid}, st, &nl));
+    unsched_rep_kernel<<<(R + 255) / 256, 256, 0, st>>>(ord1, R, o.ru, o.jid, nU, o.key);
+    CK(pool, cudaMemsetAsync(gf, 0, sizeof(GridFlag), st));
+    grid_check_kernel<<<(R + 255) / 256, 256, 0, st>>>(o.amt[0], o.amt[1], o.amt[2], R, gf);
+    nl += 2;
+    CK(pool, csort::sort_indices(writable(us.ord), tmp, R, LessKeyTid{o.key, o.tid}, st, &nl));
+    CK(pool, cudaMemsetAsync(writable(us.start), 0, sizeof(int32_t) * (nU + 1), st));
+    CK(pool, cudaMemsetAsync(writable(us.end), 0, sizeof(int32_t) * (nU + 1), st));
+    seg_bounds_kernel<<<(R + 255) / 256, 256, 0, st>>>(SortedKey{us.ord, nullptr, o.key}, R, writable(us.start),
+                                                       writable(us.end), nullptr);
+    nl++;
+    order_scan(us.os, LoadSorted{us.ord, {o.amt[0], o.amt[1], o.amt[2]}}, R, gf, st, &nl);
+    us.scan = 1; us.n = nU;
+    for (int k = 0; k < 3; k++) f.amt[k] = o.amt[k];
+    f.gf = gf; f.R = R; f.U = nU;
+    usage_fold_kernel<<<(nU + 3) / 4, 128, 0, st>>>(f);
+    nl++;
+  } else {
+    CK(pool, cudaMemsetAsync(f.user_out, 0, sizeof(double) * 4 * (size_t)nU, st));
+  }
+  // the users' entries in rank's same-user order, each entry's position by slot, then the queries
+  CK(pool, csort::sort_indices(ord3, tmp, E, LessUserTask{o.key, o.prio, o.start, o.tid, o.jid, rank}, st, &nl));
+  CK(pool, cudaMemsetAsync(ostart, 0, sizeof(int32_t) * (nU + 1), st));
+  seg_bounds_kernel<<<(E + 255) / 256, 256, 0, st>>>(SortedKey{ord3, nullptr, o.key}, E, ostart, oend, nullptr);
+  unsched_pos_kernel<<<(E + 255) / 256, 256, 0, st>>>(ord3, E, R, o.key, o.slot, nU, rpos, ppos);
+  a.qkey = d_qkey; a.Q = n;
+  a.ord = ord3; a.key = o.key; a.ostart = ostart; a.rpos = rpos; a.ppos = ppos; a.jid = o.jid;
+  a.user_out = f.user_out; a.nU = nU; a.pcol = S->pend.d_col;
+  unsched_query_kernel<<<(n + 127) / 128, 128, 0, st>>>(a);
+  nl += 3;
+  CK(pool, cudaGetLastError());
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  CK(pool, download(out_usage, a.usage, 4 * (size_t)n, st, &d2h));
+  CK(pool, download(out_position, a.pos, n, st, &d2h));
+  CK(pool, download(out_n_ahead, a.n_ahead, n, st, &d2h));
+  CK(pool, download(out_ahead, a.ahead, COOK_UNSCHED_AHEAD * (size_t)n, st, &d2h));
+  CK(pool, download(out_plugin, a.plugin, n, st, &d2h));
+  CK(pool, cudaEventRecord(pool->ev[23], st));
+  CK(pool, cudaStreamSynchronize(st));
+  // the call's own statistics: no cook_last_stats slot is written
+  if (out_stats)
+    *out_stats = {ev_ms(pool->ev[20], pool->ev[21]), ev_ms(pool->ev[21], pool->ev[22]), ev_ms(pool->ev[22], pool->ev[23]),
+                  h2d, d2h, nl, 0};
+  return COOK_OK;
+}
+
+}  // namespace
+
+extern "C" int32_t cook_state_unscheduled(cook_pool* pool, int32_t n, const int64_t* job_id, uint8_t* out_status,
+                                          double* out_usage, int32_t* out_position, int32_t* out_n_ahead,
+                                          int64_t* out_ahead_job_id, uint8_t* out_plugin_deferred,
+                                          cook_phase_stats* out_stats) {
+  return unscheduled(pool, n, job_id, out_status, out_usage, out_position, out_n_ahead, out_ahead_job_id,
+                     out_plugin_deferred, out_stats);
 }
 
 // ---- audit: the read side (cook_state_digest, cook_state_export, cook_state_queue).  The digest is one pass per

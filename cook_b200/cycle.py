@@ -19,6 +19,8 @@ path end to end.  It computes nothing numeric: every placement decision is `engi
                         the differing buckets exported, the repairing delta built
   monitor_stats         the counters set-stats-counters! (monitor.clj:177-207) sets, from cook_state_user_stats
   queue_lengths         jobs->queue-lengths (queue_limit.clj:64-90), from single-pool cook_state_user_stats calls
+  unscheduled_reasons   reasons (unscheduled.clj:172-200) of a resident pool's job from cook_state_unscheduled and the
+                        host's limit maps and facts; Investigations, the host half of record-placement-failures!
 """
 import numpy as np
 
@@ -444,4 +446,98 @@ def kill_lists(engines, now_ms, default_timeout_ms, max_timeout_ms, groups=None,
         for x in got[k] or ():
             g, (t, p) = (x[0], x[1:]) if k == "straggler" else (None, x)
             out.append((KILL_REASONS[k], t, p, g))
+    return out
+
+
+# ---- why a resident pool's job is not scheduled (/unscheduled_jobs, unscheduled.clj:172-200) -----------------------
+CONSTRAINT_MESSAGES = {   # constraint-name->message (unscheduled.clj:71-75), key spellings as the reference has them
+    "novel_host_constraint": "Job already ran on this host.",
+    "gpu_host_constraint": "Host has no GPU support.",
+    "non_gpu_host_constraint": "Host is reserved for jobs that need GPU support.",
+    "attribute-equals-host-placement-group-constraint": "Host had a different attribute than other jobs in the group."}
+USAGE_KEYS = ("count", "cpus", "mem", "gpus")   # cook_state_unscheduled's usage columns
+
+
+def fenzo_failures_for_user(summary):
+    """fenzo-failures-for-user (:77-90): a placement-failure summary -> [{reason, host_count}], resources first; a
+    constraint the message table lacks is shown by its name."""
+    return ([{"reason": f"Not enough {k} available.", "host_count": v} for k, v in summary.get("resources", {}).items()] +
+            [{"reason": CONSTRAINT_MESSAGES.get(k, k), "host_count": v}
+             for k, v in summary.get("constraints", {}).items()])
+
+
+def exceeded(limits, usage):
+    """how-job-would-exceed-resource-limits (:37-52) on the device's usage including the job: {key: {limit, usage}}
+    for the keys of `limits` (in their order) whose usage is strictly above the limit; a key the usage lacks reads 0."""
+    got = dict(zip(USAGE_KEYS, (float(x) for x in usage)))
+    return {k: {"limit": v, "usage": got.get(k)} for k, v in limits.items() if got.get(k, 0) > v}
+
+
+class Investigations:
+    """The host half of record-placement-failures! (fenzo_utils.clj:47-89) for a resident pool: the jobs under
+    investigation and the last placement-failure summary of each job."""
+
+    def __init__(self):
+        self.marked, self.summary = set(), {}
+
+    def investigate(self, job_id):
+        """check-fenzo-placement's mark: the next match that leaves the job unplaced records why."""
+        self.marked.add(int(job_id))
+
+    def record(self, engine, match):
+        """After a resident match (engine.state_match_offers' or state_match's result, on the same handle before its
+        next match): the marked considerable jobs left unplaced get cook_match_failures' summary; a non-empty one is
+        stored and ends the investigation, an empty one (ports only) leaves the job under investigation."""
+        cons, assign = match["considerable"], match["assign"]
+        ks = [k for k in range(len(cons)) if assign[k] < 0 and int(cons[k]) in self.marked]
+        if not ks:
+            return
+        for k, f in zip(ks, engine.match_failures(ks)):
+            s = summarize_failures(f["counts"])
+            if s:
+                j = int(cons[k])
+                self.summary[j] = s
+                self.marked.discard(j)
+
+
+def unscheduled_reasons(answer, i, *, job_state="completed", quota=None, share=None, attempts_consumed=0,
+                        max_retries=None, enforcing_rate_limit=False, num_rate_limited=0, plugin="", plugin_message=None,
+                        investigations=None, job_of=None):
+    """reasons (:172-200) for query i of engine.state_unscheduled's `answer`: [[message, data]] in the reference's
+    order.  The host facts: job_state (a job the handle does not hold: "running" or "completed"), the user's quota and
+    share maps in this pool, attempts consumed and max retries, whether the launch rate limit is enforced and the
+    user's rate-limited count summed over pools, the launch plugin's name and message, the pool's Investigations (the
+    job is marked) and job_of (job id -> what the answer shows, e.g. its uuid; default the id)."""
+    status = int(answer["status"][i])
+    if status == abi.UNSCHED_RUNNING or (status == abi.UNSCHED_ABSENT and job_state == "running"):
+        return [["The job is running now.", {}]]
+    if status == abi.UNSCHED_ABSENT:
+        return [["The job already completed.", {}]]
+    job_of = job_of or (lambda j: j)
+    usage = answer["usage"][i]
+    out = []
+    if max_retries is not None and attempts_consumed >= max_retries:
+        out.append(["Job has exhausted its maximum number of retries.",
+                    {"max-retries": max_retries, "instance-count": attempts_consumed}])
+    for limits, msg in ((quota, "The job would cause you to exceed resource quotas."),
+                        (share, "The job would cause you to exceed resource shares.")):
+        ways = exceeded(limits or {}, usage)
+        if ways:
+            out.append([msg, ways])
+    if enforcing_rate_limit and num_rate_limited > 0:
+        out.append(["You are currently rate limited on how many jobs you launch per minute.",
+                    {"num-ratelimited": num_rate_limited}])
+    if answer["plugin_deferred"][i]:
+        out.append(["The launch filter plugin is blocking the job launch.", {"plugin": plugin, "message": plugin_message}])
+    pos, ahead = int(answer["position"][i]), answer["ahead"][i]
+    if ahead:
+        out.append([f"You have {pos} other jobs ahead in the queue.", {"jobs": [job_of(j) for j in ahead]}])
+    inv = investigations if investigations is not None else Investigations()
+    j = int(answer["job_id"][i])
+    inv.investigate(j)   # check-fenzo-placement (:92-108) marks the job whether or not a summary is stored
+    if j in inv.summary:
+        out.append(["The job couldn't be placed on any available hosts.",
+                    {"reasons": fenzo_failures_for_user(inv.summary[j])}])
+    else:
+        out.append(["The job is now under investigation. Check back in a minute for more details!", {}])
     return out

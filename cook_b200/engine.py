@@ -507,6 +507,29 @@ class GpuEngine:
                 "ports": ports[:n * max(max_ports, 1)].reshape(n, max(max_ports, 1)).copy(),
                 "fail": fail[:n].copy(), "gone": gone, "stats": stats.as_dict()}
 
+    def state_unscheduled(self, job_id):
+        """cook_state_unscheduled: per queried job id, 'status' (abi.UNSCHED_*), 'usage' [n, 4] (count, cpus, mem, gpus of
+        the user's running jobs plus the job; WAITING only), 'position' (-1: neither waiting nor running), 'ahead' (a
+        list per query of the job ids of the first min(position, abi.UNSCHED_AHEAD) entries ahead), 'plugin_deferred',
+        and 'stats', the call's own phase statistics.  Changes nothing on the handle."""
+        jid = np.ascontiguousarray(job_id, np.int64)
+        n = len(jid)
+        m = max(n, 1)
+        status, plugin = np.zeros(m, np.uint8), np.zeros(m, np.uint8)
+        usage = np.zeros((m, 4))
+        pos, na = np.zeros(m, np.int32), np.zeros(m, np.int32)
+        ahead = np.zeros((m, abi.UNSCHED_AHEAD), np.int64)
+        st = abi.PhaseStats()
+        rc = self.lib.cook_state_unscheduled(self.pool, n, abi.ptr(jid, abi.P_I64) if n else None,
+                                             abi.ptr(status, abi.P_U8), abi.ptr(usage, abi.P_F64),
+                                             abi.ptr(pos, abi.P_I32), abi.ptr(na, abi.P_I32),
+                                             abi.ptr(ahead, abi.P_I64), abi.ptr(plugin, abi.P_U8), C.byref(st))
+        if rc != 0:
+            self._err(rc)
+        return {"job_id": jid, "status": status[:n], "usage": usage[:n], "position": pos[:n],
+                "ahead": [ahead[i, :na[i]].tolist() for i in range(n)], "ahead_raw": ahead[:n],
+                "plugin_deferred": plugin[:n], "stats": st.as_dict()}
+
     def state_rebalance(self, hosts, users, params, groups=None, derived=False, offers=False):
         """cook_state_rebalance: the rebalancer over the live running tasks and the first allowed jobs of the
         resident queue.  As rebalance(), plus each decision's 'job_id'; 'victims' are task ids (the task

@@ -1029,6 +1029,37 @@ int32_t cook_state_sweep(cook_pool* const* pools, int32_t n_pools, int64_t now_m
                          int32_t* out_straggler_group, int64_t* out_straggler_task_id, int32_t* out_straggler_pool,
                          int32_t* out_n_straggler, cook_phase_stats* out_stats);
 
+/* ------------------------------------------------ why a resident pool's job is not scheduled */
+/* The device half of /unscheduled_jobs (reasons, unscheduled.clj:172-200) for n queried job ids of one handle; the
+ * caller compares the usage with the user's quota and share maps and assembles the reasons (cycle.unscheduled_reasons).
+ * For each job_id[i], answered independently of repeats:
+ *   out_status[i]    COOK_UNSCHED_WAITING when a live pending row holds the id; else COOK_UNSCHED_RUNNING when a live
+ *                    running row carries it as its job id; else COOK_UNSCHED_ABSENT (completed, or another pool's).
+ * The user's running jobs are the distinct job ids of the user's live running rows (running and unknown alike), each
+ * represented by its row with the greatest task id.  The job's user is its pending row's, or (RUNNING) that of the
+ * job's live running row with the greatest task id.
+ *   out_usage[4i..4i+3]  (WAITING) count, cpus, mem, gpus: a left fold over the user's running jobs' representatives in
+ *                    ascending task id (count 1.0 each, cook_state_usage's fold when every job has one row), then plus
+ *                    the job (count 1.0, its cpus, mem, gpus); zeros otherwise.
+ *   out_position[i]  (WAITING, RUNNING) the number of the user's entries before the job's own, where the entries are
+ *                    the representatives and the user's live pending rows in the same-user task order of cook_state_rank
+ *                    (-priority, start (pending INT64_MAX), task id (pending -1), job id); -1 otherwise.  A job with a
+ *                    pending row and running rows is WAITING, and its running rows still count.
+ *   out_ahead_job_id[COOK_UNSCHED_AHEAD*i ..]  the job ids of the first out_n_ahead[i] = min(position, COOK_UNSCHED_AHEAD)
+ *                    entries in that order, 0 after them.
+ *   out_plugin_deferred[i]  (WAITING) 1 when the row's plugin_accept is 0; 0 otherwise.
+ * No submit-time window and no cap on the waiting jobs: every live row counts.  Changes nothing resident (rows, queue,
+ * match plan, COOK_USAGE_LAST_MATCH).
+ * COOK_E_BADARG, before any device work and with nothing written: n < 0; a NULL handle, job_id or output (but
+ * out_stats) while n > 0.  n == 0, or no queried job in the handle: no device work (statistics zero).
+ * Transfers exactly, otherwise: up 4 * (the distinct users of the queried jobs found) + 4 * n; down 121 * n (usage 32,
+ * position 4, count 4, ahead 80, plugin 1).  Nothing that scales with the tables crosses the bus.
+ * Statistics: out_stats (may be NULL), as cook_state_user_stats; no cook_last_stats slot is written.             */
+enum { COOK_UNSCHED_ABSENT = 0, COOK_UNSCHED_WAITING = 1, COOK_UNSCHED_RUNNING = 2, COOK_UNSCHED_AHEAD = 10 };
+int32_t cook_state_unscheduled(cook_pool* pool, int32_t n, const int64_t* job_id, uint8_t* out_status,
+                               double* out_usage, int32_t* out_position, int32_t* out_n_ahead,
+                               int64_t* out_ahead_job_id, uint8_t* out_plugin_deferred, cook_phase_stats* out_stats);
+
 /* ----------------------------------------------------------------- multi-GPU */
 /* §8e: after a pool's match round every rank contributes its pools' usage
  * deltas {count,cpus,mem,gpus} per user; one ncclAllGather over NVLink makes

@@ -319,6 +319,16 @@ JFN(jint, stateSweep)(JNIEnv* env, jclass k, jlongArray pools, jlongArray times,
   (*env)->SetIntArrayRegion(env, out_n, 0, 3, got);
   return rc;
 }
+/* why queried jobs are not scheduled: job_id n longs; outputs direct buffers of n bytes (status), 4n doubles (usage),
+ * n ints (position, n_ahead), COOK_UNSCHED_AHEAD*n longs (ahead job ids), n bytes (plugin deferred); out_stats may be
+ * null */
+JFN(jint, stateUnscheduled)(JNIEnv* env, jclass k, jlong pool, jint n, jobject job_id, jobject out_status,
+                            jobject out_usage, jobject out_position, jobject out_n_ahead, jobject out_ahead_job_id,
+                            jobject out_plugin_deferred, jobject out_stats) {
+  return cook_state_unscheduled((cook_pool*)(intptr_t)pool, n, one(env, job_id), one(env, out_status),
+                                one(env, out_usage), one(env, out_position), one(env, out_n_ahead),
+                                one(env, out_ahead_job_id), one(env, out_plugin_deferred), one(env, out_stats));
+}
 /* the fingerprints and the recount of the resident rows: out_digest is a direct buffer of sizeof(cook_state_digest_out),
  * out_pending_bucket / out_running_bucket direct buffers of n_buckets cook_fp each (null when n_buckets == 0) */
 JFN(jint, stateDigest)(JNIEnv* env, jclass k, jlong pool, jint n_buckets, jobject out_digest, jobject out_pending_bucket,

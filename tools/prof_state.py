@@ -32,6 +32,10 @@ rows (median of --reps calls): device time, wall time, bytes, launches, and whet
 
   python tools/prof_state.py --sweeps --pool c2 --reps 30
   python tools/prof_state.py --sweeps --pool c5 --c5-pool 5 --reps 30
+--unscheduled loads C2 (or config-#5 pool --c5-pool with --pool c5) into a resident handle, on the grid and off it,
+and times cook_state_unscheduled for one job, 1000 jobs and every waiting job of the user with the most, against numpy
+over a host mirror, with the answers compared bit for bit:
+  python tools/prof_state.py --unscheduled --pool c2 --reps 20
 
 --launch runs the same cycles on two resident handles instead of the host arm.  Each cycle's launches go to one
 handle through cook_state_launch (job ids, task ids, start times, the hosts the match chose) and to its twin through
@@ -869,6 +873,115 @@ def sweeps_prof(a):
     e.close()
 
 
+def host_unscheduled(m, q):
+    """numpy over a host mirror of the rows: cook_state_unscheduled's answers (status, usage, position, ahead)."""
+    pj = m["p_pos"]
+    rpos = m["r_of_job"]
+    out = []
+    per_user = {}
+    for j in q.tolist():
+        if j in pj:
+            st, i = 1, pj[j]
+            u = int(m["p_user"][i])
+        elif j in rpos:
+            st, i = 2, rpos[j]
+            u = int(m["r_user"][i])
+        else:
+            out.append((0, (0.0,) * 4, -1, []))
+            continue
+        if u not in per_user:
+            ri = np.flatnonzero(m["r_user"] == u)
+            ri = ri[np.lexsort((m["r_tid"][ri], m["r_jid"][ri]))]
+            last = np.ones(len(ri), bool)
+            last[:-1] = m["r_jid"][ri[1:]] != m["r_jid"][ri[:-1]]
+            ri = ri[last]                                       # one row per job: its greatest task id
+            ri = ri[np.argsort(m["r_tid"][ri], kind="stable")]   # the fold order
+            fold = (float(len(ri)),) + tuple(float(np.cumsum(m["r_" + c][ri])[-1]) if len(ri) else 0.0
+                                             for c in ("cpus", "mem", "gpus"))
+            pi = np.flatnonzero(m["p_user"] == u)
+            key = (np.concatenate([m["r_jid"][ri], m["p_jid"][pi]]),
+                   np.concatenate([m["r_tid"][ri], np.full(len(pi), -1)]),
+                   np.concatenate([m["r_start"][ri], np.full(len(pi), np.iinfo(np.int64).max)]),
+                   -np.concatenate([m["r_prio"][ri], m["p_prio"][pi]]))
+            order = np.lexsort(key)
+            ids = key[0][order]
+            run_at = {int(t): k for k, t in enumerate(np.concatenate([m["r_tid"][ri], np.full(len(pi), -1)])[order])
+                      if t >= 0}
+            pend_at = {int(x): k for k, (x, t) in enumerate(zip(ids, key[1][order])) if t < 0}
+            per_user[u] = (fold, ids, run_at, pend_at)
+        fold, ids, run_at, pend_at = per_user[u]
+        pos = pend_at[j] if st == 1 else run_at[int(m["r_tid"][i])]
+        usage = (0.0,) * 4
+        if st == 1:
+            usage = (fold[0] + 1.0, fold[1] + m["p_cpus"][i], fold[2] + m["p_mem"][i], fold[3] + m["p_gpus"][i])
+        out.append((st, usage, pos, ids[:min(pos, 10)].tolist()))
+    return out
+
+
+def unscheduled_prof(a):
+    """cook_state_unscheduled over a resident pool (C2, or config-#5 pool --c5-pool), on the grid and off it, for one
+    job, 1000 jobs and every waiting job of the user with the most, against numpy over a host mirror."""
+    t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
+    jobs, pc, rc0 = t["jobs"], t["cols"]["pending"], t["cols"]["running"]
+    J, R = jobs.n, len(rc0["task_id"])
+    print(json.dumps({"card": card(), "pool": a.pool if a.pool == "c2" else f"c5/{a.c5_pool}", "pending": J,
+                      "running": R}), flush=True)
+    rng = np.random.default_rng(a.seed)
+    for regime in ("grid", "off"):
+        run = {k: np.asarray(v).copy() for k, v in rc0.items()}
+        cols = {c: np.asarray(jobs.col(c) if jobs.col(c) is not None else np.zeros(J)).astype(np.float64)
+                for c in ("cpus", "mem", "gpus")}
+        if regime == "off":
+            run["cpus"] = run["cpus"] + 0.1
+            run["mem"] = run["mem"] / 3.0
+            cols["cpus"] = cols["cpus"] + 0.1
+        soa = Jobs(jobs, pc["priority"], pc["job_id"]).soa(np.arange(J))
+        soa = abi.JobsSoA(**{n: soa.col(n) if tp in abi._NP else getattr(soa, n) for n, tp in soa._fields_
+                             if n not in ("cpus",)}, cpus=cols["cpus"]) if regime == "off" else soa
+        e = GpuEngine(pool_name="unscheduled")
+        e.state_apply(abi.make_delta(reset=True, running=abi.make_tasks(**run), pending=soa,
+                                     pending_priority=pc["priority"], pending_job_id=pc["job_id"]))
+        m = {"p_user": np.asarray(pc["user"]), "p_prio": np.asarray(pc["priority"]), "p_jid": np.asarray(pc["job_id"]),
+             "p_cpus": cols["cpus"], "p_mem": cols["mem"], "p_gpus": cols["gpus"],
+             "r_user": np.asarray(run["user"]), "r_prio": np.asarray(run["priority"]),
+             "r_start": np.asarray(run["start_time"]), "r_tid": np.asarray(run["task_id"]),
+             "r_jid": np.asarray(run["job_id"]), "r_cpus": np.asarray(run["cpus"], np.float64),
+             "r_mem": np.asarray(run["mem"], np.float64),
+             "r_gpus": np.asarray(run["gpus"] if "gpus" in run else np.zeros(R), np.float64)}
+        m["p_pos"] = {int(j): i for i, j in enumerate(m["p_jid"])}
+        m["r_of_job"] = {}
+        for i in np.argsort(m["r_tid"]):
+            m["r_of_job"][int(m["r_jid"][i])] = int(i)
+        heavy = int(np.bincount(m["p_user"]).argmax())
+        sizes = {"1": rng.choice(m["p_jid"], 1), "1000": np.concatenate([rng.choice(m["p_jid"], 900),
+                                                                         rng.choice(m["r_jid"], 100)]),
+                 "heaviest_user": m["p_jid"][m["p_user"] == heavy]}
+        for name, q in sizes.items():
+            q = np.asarray(q, np.int64)
+            for _ in range(3):   # warm-up: the carves and the first launches
+                got = e.state_unscheduled(q)
+            dev, wall, host, same = [], [], [], True
+            for _ in range(a.reps):
+                w0 = time.perf_counter()
+                got = e.state_unscheduled(q)
+                wall.append(time.perf_counter() - w0)
+                st = got["stats"]
+                dev.append(st["ms_h2d"] + st["ms_device"] + st["ms_d2h"])
+                w0 = time.perf_counter()
+                want = host_unscheduled(m, q)
+                host.append(time.perf_counter() - w0)
+                same = same and all(
+                    int(got["status"][i]) == w[0] and np.array_equal(got["usage"][i].view(np.int64),
+                                                                     np.array(w[1], np.float64).view(np.int64))
+                    and int(got["position"][i]) == w[2] and got["ahead"][i] == w[3] for i, w in enumerate(want))
+            print(json.dumps({"regime": regime, "queries": name, "n": len(q),
+                              "device_ms": round(float(np.median(dev)), 4), "wall_ms": round(1e3 * float(np.median(wall)), 4),
+                              "h2d_bytes": st["h2d_bytes"], "d2h_bytes": st["d2h_bytes"], "n_launches": st["n_launches"],
+                              "numpy_wall_ms": round(1e3 * float(np.median(host)), 4), "identical": bool(same)}),
+                  flush=True)
+        e.close()
+
+
 def rank_quota_prof(a):
     t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
     pc, rc0, users = t["cols"]["pending"], t["cols"]["running"], t["users"]
@@ -931,7 +1044,10 @@ def main():
     ap.add_argument("--rank-quota", action="store_true")
     ap.add_argument("--sweeps", action="store_true", help="cook_state_sweep against numpy over a host mirror")
     ap.add_argument("--reps", type=int, default=20, help="--audit, --rank-quota, --sweeps: timed calls per kind")
+    ap.add_argument("--unscheduled", action="store_true", help="cook_state_unscheduled against numpy over a host mirror")
     a = ap.parse_args()
+    if a.unscheduled:
+        return unscheduled_prof(a)
     if a.sweeps:
         return sweeps_prof(a)
     if a.rank_quota:
