@@ -13,6 +13,7 @@
 ;;                                              [cook_state_sweep, cook_state_task_facts, cook_state_finish,
 ;;                                               cook_state_group_runtimes]
 ;;   unscheduled.clj:172-200 reasons      -> (unscheduled! ...) + cycle.py's unscheduled_reasons  [cook_state_unscheduled]
+;;   api.clj:2946-2969 get-user-usage       -> (user-usage! ...) + cycle.py's usage_response  [cook_state_user_usage]
 ;; selected per pool with {:scheduler-config {:scheduler "gpu"}} next to "fenzo" / "kubernetes"
 ;; (config.clj:110-122, make-pool-handler :2425-2466).  Everything numeric happens in libcookgpu;
 ;; this namespace marshals columns and keeps the state Fenzo kept (cook_b200/cycle.py is the same
@@ -410,3 +411,33 @@
               :position (.getInt ^ByteBuffer pos (int (* 4 i)))
               :ahead (vec (for [j (range k)] (.getLong ^ByteBuffer ah (int (* 8 (+ (* unsched-ahead i) j))))))
               :plugin-deferred? (= 1 (.get ^ByteBuffer pl (int i)))})))))
+
+;; ---------------------------------------------------------------------------------------------
+;; /usage over resident pools: the device half of get-user-usage (api.clj:2946-2969)
+(defn user-usage!
+  "The running usage of the user codes `users` (nil: every user) over `handles` (one device; a pool per handle).
+   `n-rows` is the live running rows over the handles (the shim's count, which bounds the queried users' rows).
+   Returns [{:user :scope (-1 or the handle index) :group (-2 total, -1 ungrouped, else the group code) :jobs :cpus :mem
+   :gpus :job-ids (group segments with by-group?)}] in (user, scope, group) order; the handler builds the reference's
+   response (zero maps, pool names, group uuids and names, job uuids) as cook_b200/cycle.py's usage_response does."
+  [handles users per-pool? by-group? n-rows]
+  (let [L (* (if per-pool? 2 1) (if by-group? 2 1))
+        seg-cap (* L n-rows) job-cap (if by-group? (* (if per-pool? 2 1) n-rows) 0)
+        m (max 1 seg-cap)
+        segs [(direct (* 4 m)) (direct (* 4 m)) (direct (* 4 m)) (direct (* 8 m)) (direct (* 8 m)) (direct (* 8 m))
+              (direct (* 8 m)) (when by-group? (direct (* 4 m)))]
+        jids (when by-group? (direct (* 8 (max 1 job-cap))))
+        out-n (int-array 2)]
+    (check! (first handles)
+            (Native/stateUserUsage (long-array handles) (count users) (when users (ints-buf users)) (if per-pool? 1 0)
+                                   (if by-group? 1 0) (int-array [seg-cap job-cap]) (object-array segs) jids out-n nil)
+            "cook_state_user_usage")
+    (let [i32 (fn [^ByteBuffer b d] (.getInt b (int (* 4 d))))
+          f64 (fn [^ByteBuffer b d] (.getDouble b (int (* 8 d))))]
+      (vec (for [d (range (aget out-n 0))]
+             (let [g (i32 (segs 2) d) jobs (.getLong ^ByteBuffer (segs 3) (int (* 8 d)))]
+               (cond-> {:user (i32 (segs 0) d) :scope (i32 (segs 1) d) :group g :jobs jobs
+                        :cpus (f64 (segs 4) d) :mem (f64 (segs 5) d) :gpus (f64 (segs 6) d)}
+                 (and by-group? (not= g -2))
+                 (assoc :job-ids (let [o (i32 (segs 7) d)]
+                                   (vec (for [j (range jobs)] (.getLong ^ByteBuffer jids (int (* 8 (+ o j))))))))))))))))

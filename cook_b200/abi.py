@@ -154,6 +154,8 @@ SWEEP_NONE, SWEEP_QUANTILE_DEVIATION = 0, 1
 OFFER_USED, OFFER_EXPIRED, OFFER_SINGLE_SHOT = 1, 2, 3
 # cook_state_unscheduled: a queried job's status, and the most job ids ahead it returns
 UNSCHED_ABSENT, UNSCHED_WAITING, UNSCHED_RUNNING, UNSCHED_AHEAD = 0, 1, 2, 10
+# cook_state_user_usage: a segment's group when it is the scope's total, or its jobs without a group
+UU_TOTAL, UU_UNGROUPED = -2, -1
 
 
 class ConsiderableParams(C.Structure):
@@ -337,6 +339,8 @@ ARGTYPES = {
     "cook_state_sweep": [_P(_H), _I32, C.c_int64, C.c_int64, C.c_int64, _I32, P_I32, P_F64, P_F64, P_I32, _I32, P_I64,
                          P_I32, P_I32, P_I64, P_I32, P_I32, _I32, P_I32, P_I64, P_I32, P_I32, _P(PhaseStats)],
     "cook_state_unscheduled": [_H, _I32, P_I64, P_U8, P_F64, P_I32, P_I32, P_I64, P_U8, _P(PhaseStats)],
+    "cook_state_user_usage": [_P(_H), _I32, P_I32, _I32, _I32, _I32, _I32, P_I32, P_I32, P_I32, P_I64, P_F64, P_F64,
+                              P_F64, P_I32, _I32, P_I64, P_I32, P_I32, _P(PhaseStats)],
     "cook_last_stats": [_H, _I32, _P(PhaseStats)],
     "cook_allgather_usage": [_H, _H, P_F64, P_F64, C.c_int64],
     "cook_comm_unique_id": [P_U8],

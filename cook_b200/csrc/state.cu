@@ -3766,6 +3766,331 @@ extern "C" int32_t cook_state_unscheduled(cook_pool* pool, int32_t n, const int6
                      out_plugin_deferred, out_stats);
 }
 
+// ---- the running usage of users (/usage, get-user-usage api.clj:2946-2969): per (user, scope, group) segment the
+// number of running jobs and the left folds of cpus, mem and gpus over one representative per running job, and each
+// group segment's job ids.  The host sizes every buffer from its per-user counts; the device takes the queried users'
+// live running rows of every handle, keeps each (handle, job)'s row with the greatest task id, expands each
+// representative into one entry per level the call asks for, sorts the entries once by (segment, task id, dense
+// index) and folds each segment as usage_fold_kernel does.
+namespace {
+
+constexpr int32_t UU_DEAD = INT32_MAX;   // the user of an entry whose row is not its job's representative: sorts last
+
+__global__ void uu_users_kernel(const int32_t* quser, int nU, int32_t n_codes, uint8_t* umap) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < nU && quser[k] < n_codes) umap[quser[k]] = 1;
+}
+
+// one handle's live running rows of the queried users (umap null: every user), dense after the handles before it
+struct UURows {
+  void* const* col; const uint8_t* umap; int base; int32_t pool; const int32_t* arena;
+  int32_t* user; int64_t* jid; int64_t* tid; int32_t* pidx; int32_t* grp; double* amt[3];
+  __device__ bool keep(int i) const {
+    return static_cast<const uint8_t*>(col[R_LIVE])[i] && (!umap || umap[static_cast<const int32_t*>(col[R_USER])[i]]);
+  }
+  __device__ void emit(int i, int d) const {
+    d += base;
+    user[d] = static_cast<const int32_t*>(col[R_USER])[i];
+    jid[d] = static_cast<const int64_t*>(col[R_JID])[i];
+    tid[d] = static_cast<const int64_t*>(col[R_TID])[i];
+    pidx[d] = pool;
+    const int32_t len = static_cast<const int32_t*>(col[R_GLEN])[i];
+    grp[d] = len > 0 ? arena[static_cast<const int32_t*>(col[R_GOFF])[i]] : COOK_UU_UNGROUPED;
+    amt[0][d] = static_cast<const double*>(col[R_CPUS])[i];
+    amt[1][d] = static_cast<const double*>(col[R_MEM])[i];
+    amt[2][d] = static_cast<const double*>(col[R_GPUS])[i];
+  }
+};
+// (handle, job id, task id, dense index): a (handle, job)'s rows together, its greatest task id last
+struct LessPoolJobTask {
+  const int32_t* pidx; const int64_t* jid; const int64_t* tid;
+  __device__ bool operator()(int32_t a, int32_t b) const {
+    if (pidx[a] != pidx[b]) return pidx[a] < pidx[b];
+    if (jid[a] != jid[b]) return jid[a] < jid[b];
+    if (tid[a] != tid[b]) return tid[a] < tid[b];
+    return a < b;
+  }
+};
+__global__ void uu_rep_kernel(const int32_t* ord, int R, const int32_t* pidx, const int64_t* jid, uint8_t* rep) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= R) return;
+  const int i = ord[p];
+  bool last = p == R - 1;
+  if (!last) {
+    const int n = ord[p + 1];
+    last = pidx[n] != pidx[i] || jid[n] != jid[i];
+  }
+  rep[i] = last;
+}
+
+// The entries: entry l * R + i is row i at level l.  Bit 0 of the level's code scopes the entry to its handle, bit 1
+// keys it by its group (per_pool: codes 0 .. L - 1; else 0 and, by_group, 2).  A row that is not a representative
+// gives entries of user UU_DEAD.
+struct UUKey {
+  int32_t* user; int32_t* scope; int32_t* grp;
+  __device__ bool same(int a, int b) const { return user[a] == user[b] && scope[a] == scope[b] && grp[a] == grp[b]; }
+};
+__global__ void uu_expand_kernel(int R, int E, int per_pool, const uint8_t* rep, const int32_t* user,
+                                 const int32_t* pidx, const int32_t* grp, UUKey k, int32_t* row) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  if (x >= E) return;
+  const int l = x / R, i = x - l * R, code = per_pool ? l : l << 1;
+  k.user[x] = rep[i] ? user[i] : UU_DEAD;
+  k.scope[x] = code & 1 ? pidx[i] : -1;
+  k.grp[x] = code & 2 ? grp[i] : COOK_UU_TOTAL;
+  row[x] = i;
+}
+// (user, scope, group, task id, dense index): the segments in the output order, each in its fold order
+struct LessSegTid {
+  UUKey k; const int32_t* row; const int64_t* tid;
+  __device__ bool operator()(int32_t a, int32_t b) const {
+    if (k.user[a] != k.user[b]) return k.user[a] < k.user[b];
+    if (k.scope[a] != k.scope[b]) return k.scope[a] < k.scope[b];
+    if (k.grp[a] != k.grp[b]) return k.grp[a] < k.grp[b];
+    const int ra = row[a], rb = row[b];
+    if (tid[ra] != tid[rb]) return tid[ra] < tid[rb];
+    if (ra != rb) return ra < rb;
+    return a < b;
+  }
+};
+// the last position of each segment of the sorted entries: end[d] = one past segment d's last, segment d starting
+// where segment d - 1 ends
+struct UUSegEnds {
+  const int32_t* ord; UUKey k; int E; int32_t* end;
+  __device__ bool keep(int p) const {
+    const int i = ord[p];
+    return k.user[i] != UU_DEAD && (p == E - 1 || !k.same(i, ord[p + 1]));
+  }
+  __device__ void emit(int p, int d) const { end[d] = p + 1; }
+};
+// the group segments' job ids in segment order; head_off[p] of a segment's first position p: its first list index
+struct UUListed {
+  const int32_t* ord; UUKey k; const int32_t* row; const int64_t* jid; int64_t* o_jid; int32_t* head_off;
+  __device__ bool keep(int p) const {
+    const int i = ord[p];
+    return k.user[i] != UU_DEAD && k.grp[i] != COOK_UU_TOTAL;
+  }
+  __device__ void emit(int p, int d) const {
+    const int i = ord[p];
+    o_jid[d] = jid[row[i]];
+    if (p == 0 || !k.same(i, ord[p - 1])) head_off[p] = d;
+  }
+};
+struct UULoad {   // the order-wide scan's addends: cpus, mem, gpus of the entry at position p
+  const int32_t* ord; const int32_t* row; const double* amt[3];
+  __device__ void operator()(int p, double (&x)[3]) const {
+    const int r = row[ord[p]];
+    x[0] = amt[0][r]; x[1] = amt[1][r]; x[2] = amt[2][r];
+  }
+};
+struct UUFoldArgs {
+  const int32_t* ord; const int32_t* row; UUKey k; const double* amt[3];
+  const int32_t* end; const int32_t* n_seg; const int32_t* head_off;   // head_off null: no lists
+  OrderScan<double, 3> os; const GridFlag* gf; int E;
+  int32_t *o_user, *o_scope, *o_grp, *o_off; int64_t* o_jobs; double* o_amt[3];
+};
+// Warp per segment, grid-stride: the left fold of cpus, mem and gpus in ascending (task id, dense index).  The whole
+// order on the grid: the two ends of the order-wide scan; else warp_fold_sum, association-free when the segment alone
+// is on the grid, else the serial chain.
+__global__ void __launch_bounds__(128) uu_fold_kernel(UUFoldArgs a) {
+  __shared__ double stage[4][3][32];
+  const int n = *a.n_seg, nw = gridDim.x * (blockDim.x >> 5);
+  const bool scan = grid_exact(a.gf, a.E);
+  for (int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; g < n; g += nw) {
+    const int s = g ? a.end[g - 1] : 0, e = a.end[g];
+    double acc[3] = {0.0, 0.0, 0.0};
+    if (scan) {
+#pragma unroll
+      for (int k = 0; k < 3; k++) acc[k] = a.os.segment_sum(k, e - 1, s);
+    } else {
+      warp_fold_sum<3, 4>(acc, e - s, grid_exact(a.gf, e - s), [&](int k, double (&x)[3]) {
+        const int r = a.row[a.ord[s + k]];
+        x[0] = a.amt[0][r]; x[1] = a.amt[1][r]; x[2] = a.amt[2][r];
+        return true;
+      }, stage[threadIdx.x >> 5]);
+    }
+    if (threadIdx.x & 31) continue;
+    const int i = a.ord[s];
+    a.o_user[g] = a.k.user[i]; a.o_scope[g] = a.k.scope[i]; a.o_grp[g] = a.k.grp[i];
+    a.o_jobs[g] = e - s;
+#pragma unroll
+    for (int k = 0; k < 3; k++) a.o_amt[k][g] = acc[k];
+    if (a.head_off) a.o_off[g] = a.k.grp[i] == COOK_UU_TOTAL ? -1 : a.head_off[s];
+  }
+}
+
+int32_t user_usage(cook_pool* const* pools, int n, const int32_t* user, int nU, int per_pool, int by_group,
+                   int seg_cap, int32_t* o_user, int32_t* o_scope, int32_t* o_group, int64_t* o_jobs, double* o_cpus,
+                   double* o_mem, double* o_gpus, int32_t* o_off, int job_cap, int64_t* o_jid, int32_t* o_nseg,
+                   int32_t* o_njob, cook_phase_stats* out_stats) {
+  const char* who = "cook_state_user_usage";
+  // ---- every check before any device work or output
+  if (!pools || n <= 0 || !pools[0]) return COOK_E_BADARG;
+  cook_pool* pool = pools[0];
+  for (int k = 0; k < n; k++) {
+    if (!pools[k]) return set_err(pool, COOK_E_BADARG, "%s: a NULL handle", who);
+    if (std::find(pools, pools + k, pools[k]) != pools + k)
+      return set_err(pool, COOK_E_BADARG, "%s: a handle listed twice", who);
+    if (pools[k]->device != pool->device) return set_err(pool, COOK_E_BADARG, "%s: handles on different devices", who);
+  }
+  const bool pp = per_pool != 0, bg = by_group != 0;
+  if (!o_user || !o_scope || !o_group || !o_jobs || !o_cpus || !o_mem || !o_gpus || !o_nseg || !o_njob ||
+      (bg && (!o_off || !o_jid)))
+    return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
+  if (user ? nU < 0 : nU != 0) return set_err(pool, COOK_E_BADARG, "%s: n_users < 0, or n_users without user", who);
+  std::vector<int32_t> q(user, user + (user ? nU : 0));
+  std::sort(q.begin(), q.end());
+  if (!q.empty() && q[0] < 0) return set_err(pool, COOK_E_BADARG, "%s: a negative user code", who);
+  if (std::adjacent_find(q.begin(), q.end()) != q.end()) return set_err(pool, COOK_E_BADARG, "%s: a user code twice", who);
+  // the handles with rows of the queried users, their pool index and row count; sizes from the host-side counts
+  struct Src { const PoolState* s; int32_t k; int live; };
+  std::vector<Src> hs;
+  int64_t R = 0;
+  int hw = 0;
+  int32_t n_codes = 0;
+  for (int k = 0; k < n; k++) {
+    const PoolState* s = static_cast<const PoolState*>(pools[k]->state);
+    if (!s) continue;
+    int64_t r = 0;
+    if (!user) {
+      r = (int64_t)s->run.slot_of.size();
+    } else {
+      for (int32_t u : q) {
+        auto it = s->users_r.find(u);
+        if (it != s->users_r.end()) r += it->second;
+      }
+    }
+    if (!r) continue;
+    hs.push_back({s, k, (int)r});
+    R += r;
+    hw = std::max(hw, s->run.hw);
+    n_codes = std::max(n_codes, count_max(s->users_r) + 1);
+  }
+  const int L = (1 + pp) * (1 + bg);
+  if (R * L > INT32_MAX) return set_err(pool, COOK_E_TOO_LARGE, "%s: more than 2^31 - 1 entries", who);
+  if (seg_cap < R * L) return set_err(pool, COOK_E_BADARG, "%s: seg_cap below the queried users' rows' bound", who);
+  if (bg && job_cap < R * (1 + pp))
+    return set_err(pool, COOK_E_BADARG, "%s: job_cap below the queried users' rows' bound", who);
+  if (R == 0) {   // no row to read: empty results without device work
+    *o_nseg = 0;
+    *o_njob = 0;
+    if (out_stats) *out_stats = cook_phase_stats{};
+    return COOK_OK;
+  }
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S0 = state_of(pool, true);   // pools[0]'s scratch, even when it holds no row
+  if (!S0) return set_err(pool, COOK_E_OOM, "%s: out of device memory", who);
+  cudaStream_t st = pool->stream;
+  const int Rn = (int)R, E = Rn * L, J = bg ? Rn * (1 + pp) : 0;
+  hw = std::max(hw, E);
+  // ---- one carve: the rows, the representatives, the entries and their order, the folds, the outputs
+  int32_t *cnt = nullptr, *blk = nullptr, *ord1 = nullptr, *tmp = nullptr, *ord = nullptr, *end = nullptr;
+  int32_t *r_user = nullptr, *r_pidx = nullptr, *r_grp = nullptr, *row = nullptr, *head_off = nullptr;
+  int64_t *r_jid = nullptr, *r_tid = nullptr, *d_jid = nullptr;
+  double* amt[3] = {};
+  uint8_t *umap = nullptr, *rep = nullptr;
+  const int32_t* d_q = nullptr;
+  GridFlag* gf = nullptr;
+  UUKey key = {};
+  UUFoldArgs a = {};
+  int64_t h2d = 0, d2h = 0;
+  CK(pool, carve(S0->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+    cnt = c.take<int32_t>(3);   // segments, listed jobs, the row compactions' own
+    blk = c.take<int32_t>((size_t)hw / CP_BLOCK + 2);
+    if (user) umap = c.take<uint8_t>(n_codes);
+    r_user = c.take<int32_t>(Rn); r_pidx = c.take<int32_t>(Rn); r_grp = c.take<int32_t>(Rn);
+    r_jid = c.take<int64_t>(Rn); r_tid = c.take<int64_t>(Rn);
+    for (int k = 0; k < 3; k++) amt[k] = c.take<double>(Rn);
+    rep = c.take<uint8_t>(Rn); ord1 = c.take<int32_t>(Rn);
+    gf = c.take<GridFlag>(1);
+    key.user = c.take<int32_t>(E); key.scope = c.take<int32_t>(E); key.grp = c.take<int32_t>(E);
+    row = c.take<int32_t>(E); ord = c.take<int32_t>(E); tmp = c.take<int32_t>(E); end = c.take<int32_t>(E);
+    for (int k = 0; k < 3; k++) {
+      a.os.part[k] = c.take<double>(E);
+      a.os.tile[k] = c.take<double>(E / OS_TILE + 2);
+    }
+    a.o_user = c.take<int32_t>(E); a.o_scope = c.take<int32_t>(E); a.o_grp = c.take<int32_t>(E);
+    a.o_jobs = c.take<int64_t>(E);
+    for (int k = 0; k < 3; k++) a.o_amt[k] = c.take<double>(E);
+    if (bg) {
+      a.o_off = c.take<int32_t>(E); head_off = c.take<int32_t>(E);
+      d_jid = c.take<int64_t>(J);
+    }
+    if (user) d_q = c.up(q.data(), nU);
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  CK(pool, cudaMemsetAsync(cnt, 0, sizeof(int32_t) * 3, st));
+  CK(pool, cudaMemsetAsync(gf, 0, sizeof(GridFlag), st));
+  int nl = 0;
+  if (user) {
+    CK(pool, cudaMemsetAsync(umap, 0, (size_t)n_codes, st));
+    uu_users_kernel<<<(nU + 255) / 256, 256, 0, st>>>(d_q, nU, n_codes, umap);
+    nl++;
+  }
+  int base = 0;
+  for (const Src& h : hs) {
+    compact(UURows{h.s->run.d_col, umap, base, h.k, h.s->lists[L_RGROUP].v[0], r_user, r_jid, r_tid, r_pidx, r_grp,
+                   {amt[0], amt[1], amt[2]}},
+            h.s->run.hw, nullptr, blk, cnt + 2, h.live, st, &nl);
+    base += h.live;
+  }
+  grid_check_kernel<<<(Rn + 255) / 256, 256, 0, st>>>(amt[0], amt[1], amt[2], Rn, gf);
+  nl++;
+  // one representative per (handle, job), then every level's entries in one (segment, task id) order
+  CK(pool, csort::sort_indices(ord1, tmp, Rn, LessPoolJobTask{r_pidx, r_jid, r_tid}, st, &nl));
+  uu_rep_kernel<<<(Rn + 255) / 256, 256, 0, st>>>(ord1, Rn, r_pidx, r_jid, rep);
+  uu_expand_kernel<<<(E + 255) / 256, 256, 0, st>>>(Rn, E, pp, rep, r_user, r_pidx, r_grp, key, row);
+  nl += 2;
+  CK(pool, csort::sort_indices(ord, tmp, E, LessSegTid{key, row, r_tid}, st, &nl));
+  compact(UUSegEnds{ord, key, E, end}, E, nullptr, blk, cnt + 0, E, st, &nl);
+  if (bg) compact(UUListed{ord, key, row, r_jid, d_jid, head_off}, E, nullptr, blk, cnt + 1, J, st, &nl);
+  order_scan(a.os, UULoad{ord, row, {amt[0], amt[1], amt[2]}}, E, gf, st, &nl);
+  a.ord = ord; a.row = row; a.k = key;
+  for (int k = 0; k < 3; k++) a.amt[k] = amt[k];
+  a.end = end; a.n_seg = cnt; a.head_off = head_off; a.gf = gf; a.E = E;
+  uu_fold_kernel<<<std::min((E + 3) / 4, 4096), 128, 0, st>>>(a);
+  nl++;
+  CK(pool, cudaGetLastError());
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  int32_t got[2];
+  CK(pool, download(got, cnt, 2, st, &d2h));
+  CK(pool, cudaStreamSynchronize(st));
+  const int ns = got[0], nj = bg ? got[1] : 0;
+  CK(pool, download(o_user, a.o_user, ns, st, &d2h));
+  CK(pool, download(o_scope, a.o_scope, ns, st, &d2h));
+  CK(pool, download(o_group, a.o_grp, ns, st, &d2h));
+  CK(pool, download(o_jobs, a.o_jobs, ns, st, &d2h));
+  CK(pool, download(o_cpus, a.o_amt[0], ns, st, &d2h));
+  CK(pool, download(o_mem, a.o_amt[1], ns, st, &d2h));
+  CK(pool, download(o_gpus, a.o_amt[2], ns, st, &d2h));
+  if (bg) {
+    CK(pool, download(o_off, a.o_off, ns, st, &d2h));
+    CK(pool, download(o_jid, d_jid, nj, st, &d2h));
+  }
+  CK(pool, cudaEventRecord(pool->ev[23], st));
+  CK(pool, cudaStreamSynchronize(st));
+  *o_nseg = ns;
+  *o_njob = nj;
+  // the call's own statistics: no cook_last_stats slot is written
+  if (out_stats)
+    *out_stats = {ev_ms(pool->ev[20], pool->ev[21]), ev_ms(pool->ev[21], pool->ev[22]), ev_ms(pool->ev[22], pool->ev[23]),
+                  h2d, d2h, nl, 0};
+  return COOK_OK;
+}
+
+}  // namespace
+
+extern "C" int32_t cook_state_user_usage(cook_pool* const* pools, int32_t n_pools, const int32_t* user,
+                                         int32_t n_users, int32_t per_pool, int32_t by_group, int32_t seg_cap,
+                                         int32_t* out_user, int32_t* out_scope, int32_t* out_group, int64_t* out_jobs,
+                                         double* out_cpus, double* out_mem, double* out_gpus, int32_t* out_list_off,
+                                         int32_t job_cap, int64_t* out_job_id, int32_t* out_n_seg,
+                                         int32_t* out_n_job, cook_phase_stats* out_stats) {
+  return user_usage(pools, n_pools, user, n_users, per_pool, by_group, seg_cap, out_user, out_scope, out_group,
+                    out_jobs, out_cpus, out_mem, out_gpus, out_list_off, job_cap, out_job_id, out_n_seg, out_n_job,
+                    out_stats);
+}
+
 // ---- audit: the read side (cook_state_digest, cook_state_export, cook_state_queue).  The digest is one pass per
 // table: a thread hashes its slot's columns and short lists, a long list is read by the warp and absorbed by the
 // owning lane; fingerprints and counts are reduced per warp with shuffles, per block in shared memory, then one

@@ -21,6 +21,7 @@ path end to end.  It computes nothing numeric: every placement decision is `engi
   queue_lengths         jobs->queue-lengths (queue_limit.clj:64-90), from single-pool cook_state_user_stats calls
   unscheduled_reasons   reasons (unscheduled.clj:172-200) of a resident pool's job from cook_state_unscheduled and the
                         host's limit maps and facts; Investigations, the host half of record-placement-failures!
+  usage_response        the body of GET /usage (get-user-usage, api.clj:2946-2969) from cook_state_user_usage answers
 """
 import numpy as np
 
@@ -541,3 +542,65 @@ def unscheduled_reasons(answer, i, *, job_state="completed", quota=None, share=N
     else:
         out.append(["The job is now under investigation. Check back in a minute for more details!", {}])
     return out
+
+
+# ---- users' running usage (GET /usage, get-user-usage api.clj:2946-2969) -----------------------------------------
+def _usage_map(v):
+    """{cpus mem gpus jobs} of (jobs, cpus, mem, gpus); None: the reference's zero-usage."""
+    return {"cpus": 0.0, "mem": 0.0, "gpus": 0.0, "jobs": 0} if v is None else \
+        {"cpus": v[1], "mem": v[2], "gpus": v[3], "jobs": v[0]}
+
+
+def _add(a, b):
+    return b if a is None else tuple(x + y for x, y in zip(a, b))
+
+
+def usage_response(answers, *, user=None, pool=None, pools=(), group_breakdown=False, job_uuid=None, group_info=None,
+                   user_name=None):
+    """The body of GET /usage from engine.state_user_usage answers, in the reference's shape (usage, user-usage and
+    no-usage-map, api.clj:2894-2944).  answers: [(answer, names)], one per device, each over handles whose pool names
+    are `names` in handle order, asked with by_group = group_breakdown and per_pool = (pool is None and pools).  With
+    a `pool` (the parameter or header), the answers cover that pool's handle alone and the response has no "pools".
+    user: the queried user code, else {"users": {name: usage}} over the users that run a job.  pools: every pool name
+    in the database (the zero maps; empty: no pools).  job_uuid(job id), group_info(group code) -> (uuid, name) and
+    user_name(code) give what the response shows (default: the codes, a None name).  The device folds are exact; the
+    totals of several devices are added here in device order."""
+    job_of = job_uuid or (lambda j: j)
+    info = group_info or (lambda g: (g, None))
+    name_of = user_name or (lambda u: u)
+    per_pool = pool is None and len(pools) > 0
+    acc = {}   # user -> scope name (None: every pool) -> {"total": usage, "groups": {group: [usage, job ids]}}
+    for ans, names in answers:
+        for d in range(len(ans["user"])):
+            sc, g = int(ans["scope"][d]), int(ans["group"][d])
+            slot = acc.setdefault(int(ans["user"][d]), {}).setdefault(None if sc < 0 else names[sc],
+                                                                       {"total": None, "groups": {}})
+            v = (int(ans["jobs"][d]), float(ans["cpus"][d]), float(ans["mem"][d]), float(ans["gpus"][d]))
+            if g == abi.UU_TOTAL:
+                slot["total"] = _add(slot["total"], v)
+            else:
+                cur = slot["groups"].setdefault(g, [None, []])
+                cur[0] = _add(cur[0], v)
+                cur[1] += ans["lists"][d]
+
+    def user_usage(slot):
+        out = {"total_usage": _usage_map(slot and slot["total"])}
+        if group_breakdown:
+            groups = slot["groups"] if slot else {}
+            out["grouped"] = [{"group": {"uuid": info(g)[0], "name": info(g)[1],
+                                         "running_jobs": [job_of(j) for j in js]}, "usage": _usage_map(v)}
+                              for g, (v, js) in sorted(groups.items()) if g >= 0]
+            v, js = groups.get(abi.UU_UNGROUPED, (None, []))
+            out["ungrouped"] = {"running_jobs": [job_of(j) for j in js], "usage": _usage_map(v)}
+        return out
+
+    def usage(u):
+        per = acc.get(u, {})
+        out = user_usage(per.get(None))
+        if per_pool:
+            out["pools"] = {p: user_usage(per.get(p)) for p in list(pools) + [p for p in per if p is not None and p not in pools]}
+        return out
+
+    if user is not None:
+        return usage(int(user))
+    return {"users": {name_of(u): usage(u) for u in sorted(acc)}}

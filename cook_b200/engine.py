@@ -665,6 +665,45 @@ def state_sweep(engines, now_ms, default_timeout_ms, max_timeout_ms, groups=None
     return res
 
 
+def state_user_usage(engines, users=None, per_pool=False, by_group=False):
+    """cook_state_user_usage over the live running rows of `engines` (one device, the work on engines[0]'s stream) for
+    the user codes `users` (None: every user).  Returns the segments as numpy columns 'user', 'scope' (-1: every
+    handle, else the engine index), 'group' (abi.UU_TOTAL, abi.UU_UNGROUPED or a group code), 'jobs' (int64), 'cpus',
+    'mem', 'gpus', and with by_group 'list_off' and 'job_id' (the group segments' job ids, in segment order), plus
+    'lists' (per segment its job ids, None for a total) and 'stats', the call's own phase statistics.  The capacities
+    are sized from the engines' live running ids."""
+    if not engines:
+        raise ValueError("state_user_usage: at least one handle")
+    q = np.ascontiguousarray(users if users is not None else (), np.int32)
+    R = sum(len(getattr(e, "_state_running_ids", ())) for e in engines)
+    L = (1 + bool(per_pool)) * (1 + bool(by_group))
+    seg_cap, job_cap = R * L, R * (1 + bool(per_pool)) if by_group else 0
+    m = max(seg_cap, 1)
+    u, sc, g, off = (np.zeros(m, np.int32) for _ in range(4))
+    jobs = np.zeros(m, np.int64)
+    cpus, mem, gpus = np.zeros(m), np.zeros(m), np.zeros(m)
+    jid = np.zeros(max(job_cap, 1), np.int64)
+    n_seg, n_job = C.c_int32(0), C.c_int32(0)
+    st = abi.PhaseStats()
+    handles = (C.c_void_p * len(engines))(*[e.pool for e in engines])
+    rc = engines[0].lib.cook_state_user_usage(
+        handles, len(engines), abi.ptr(q, abi.P_I32) if users is not None else None, len(q), int(bool(per_pool)),
+        int(bool(by_group)), seg_cap, abi.ptr(u, abi.P_I32), abi.ptr(sc, abi.P_I32), abi.ptr(g, abi.P_I32),
+        abi.ptr(jobs, abi.P_I64), abi.ptr(cpus, abi.P_F64), abi.ptr(mem, abi.P_F64), abi.ptr(gpus, abi.P_F64),
+        abi.ptr(off, abi.P_I32) if by_group else None, job_cap, abi.ptr(jid, abi.P_I64) if by_group else None,
+        C.byref(n_seg), C.byref(n_job), C.byref(st))
+    if rc != 0:
+        engines[0]._err(rc)
+    n, nj = n_seg.value, n_job.value
+    out = {"user": u[:n], "scope": sc[:n], "group": g[:n], "jobs": jobs[:n], "cpus": cpus[:n], "mem": mem[:n],
+           "gpus": gpus[:n], "stats": st.as_dict()}
+    if by_group:
+        out["list_off"], out["job_id"] = off[:n], jid[:nj]
+    out["lists"] = [None if not by_group or out["group"][d] == abi.UU_TOTAL else
+                    jid[off[d]:off[d] + jobs[d]].tolist() for d in range(n)]
+    return out
+
+
 STATS_KEYS = ("running", "waiting", "starved", "waiting-under-quota")   # by abi.STATS_*
 USER_COUNTS = ("total", "starved", "waiting-under-quota", "hungry", "satisfied")   # by abi.USERS_*
 

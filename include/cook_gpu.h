@@ -1060,6 +1060,44 @@ int32_t cook_state_unscheduled(cook_pool* pool, int32_t n, const int64_t* job_id
                                double* out_usage, int32_t* out_position, int32_t* out_n_ahead,
                                int64_t* out_ahead_job_id, uint8_t* out_plugin_deferred, cook_phase_stats* out_stats);
 
+/* ------------------------------------------------------------- users' running usage over resident pools */
+/* The device half of GET /usage (get-user-usage, api.clj:2946-2969; user-usage :2894-2915) over the union of the live
+ * running rows of pools[0, n_pools), for the user codes user[0, n_users) or, with user NULL (n_users 0), every user.
+ * Each handle is one pool; the handles follow cook_state_user_stats' rules (one device, idle, the work on pools[0]'s
+ * stream and scratch).  Pools on different GPUs: one call per device and the host's addition.  Fixed choices:
+ *   Jobs      a running job is a distinct (handle, job id) over the live running rows, running and status-unknown
+ *             alike; its representative is its row with the greatest task id (cook_state_unscheduled's rule).
+ *   Order     every fold is a left fold from +0.0 over the segment's representatives in ascending (task id, pool
+ *             index); jobs is an integer count; the job lists come in the same order.
+ *   Group     a job's group is the first entry of its representative's running group list, as the delta or the
+ *             launch gave it; an empty list is ungrouped.  The reference's "first of a set" is the caller's order.
+ *   Segments  (user, scope, group): scope -1 is all the handles, p (per_pool != 0 only) handle p; group
+ *             COOK_UU_TOTAL the scope's total, COOK_UU_UNGROUPED the jobs without a group, g >= 0 (by_group != 0 only)
+ *             group code g.  A segment is emitted only when it holds a job (the host builds the zero maps), in
+ *             ascending (user, scope, group): -1 before the handles, COOK_UU_TOTAL, COOK_UU_UNGROUPED, then codes.
+ *   Outputs   per segment d < *out_n_seg: out_user, out_scope, out_group, out_jobs, out_cpus, out_mem, out_gpus; with
+ *             by_group, out_list_off[d] (-1 for a total) is where the segment's out_jobs[d] job ids start in
+ *             out_job_id[0, *out_n_job), segments in order.  Without by_group, out_list_off and out_job_id are not
+ *             read and *out_n_job = 0.
+ *   Sizes     with R_q the live running rows of the queried users over the handles (the library's host-side
+ *             counts): seg_cap >= R_q * (1 + per_pool) * (1 + by_group), and with by_group job_cap >=
+ *             R_q * (1 + per_pool).
+ * Changes nothing resident (rows, queue, match plan, COOK_USAGE_LAST_MATCH).
+ * COOK_E_BADARG, before any device work and with nothing written: cook_state_user_stats' handle cases; a NULL output
+ * (out_list_off and out_job_id only with by_group; out_stats may be NULL); n_users < 0, or n_users != 0 with user
+ * NULL; a negative user code or one listed twice; a capacity below its bound.  COOK_E_TOO_LARGE: R_q * (1 + per_pool)
+ * * (1 + by_group) >= 2^31.  R_q == 0: empty results without device work (statistics zero).
+ * Transfers exactly, otherwise: up 4 * n_users; down 8 (the counts) + (44 + 4 * by_group) * *out_n_seg + 8 *
+ * *out_n_job.  Nothing that scales with the tables crosses the bus.
+ * Statistics: out_stats (may be NULL), as cook_state_user_stats; no cook_last_stats slot is written.  The outputs are
+ * plain arrays, like cook_state_user_stats' outputs: every struct of this header has a ctypes mirror. */
+enum { COOK_UU_TOTAL = -2, COOK_UU_UNGROUPED = -1 };
+int32_t cook_state_user_usage(cook_pool* const* pools, int32_t n_pools, const int32_t* user, int32_t n_users,
+                              int32_t per_pool, int32_t by_group, int32_t seg_cap, int32_t* out_user,
+                              int32_t* out_scope, int32_t* out_group, int64_t* out_jobs, double* out_cpus,
+                              double* out_mem, double* out_gpus, int32_t* out_list_off, int32_t job_cap,
+                              int64_t* out_job_id, int32_t* out_n_seg, int32_t* out_n_job, cook_phase_stats* out_stats);
+
 /* ----------------------------------------------------------------- multi-GPU */
 /* §8e: after a pool's match round every rank contributes its pools' usage
  * deltas {count,cpus,mem,gpus} per user; one ncclAllGather over NVLink makes

@@ -319,6 +319,28 @@ JFN(jint, stateSweep)(JNIEnv* env, jclass k, jlongArray pools, jlongArray times,
   (*env)->SetIntArrayRegion(env, out_n, 0, 3, got);
   return rc;
 }
+/* users' running usage: user n_users ints (null: every user); caps [seg_cap, job_cap]; segs the direct buffers of
+ * user, scope, group (ints), jobs (longs), cpus, mem, gpus (doubles), list_off (ints; null without by_group); job_id
+ * job_cap longs (null without by_group); out_n gets [n_seg, n_job]; out_stats may be null */
+JFN(jint, stateUserUsage)(JNIEnv* env, jclass k, jlongArray pools, jint n_users, jobject user, jint per_pool,
+                          jint by_group, jintArray caps, jobjectArray segs, jobject job_id, jintArray out_n,
+                          jobject out_stats) {
+  jsize n = (*env)->GetArrayLength(env, pools);
+  if (n > 64) return COOK_E_BADARG;
+  jlong* h = (*env)->GetLongArrayElements(env, pools, NULL);
+  cook_pool* p[64];
+  for (jsize i = 0; i < n; i++) p[i] = (cook_pool*)(intptr_t)h[i];
+  (*env)->ReleaseLongArrayElements(env, pools, h, JNI_ABORT);
+  jint c[2]; (*env)->GetIntArrayRegion(env, caps, 0, 2, c);
+  int32_t ns = 0, nj = 0;
+  jint rc = cook_state_user_usage(p, (int32_t)n, one(env, user), n_users, per_pool, by_group, c[0], buf(env, segs, 0),
+                                  buf(env, segs, 1), buf(env, segs, 2), buf(env, segs, 3), buf(env, segs, 4),
+                                  buf(env, segs, 5), buf(env, segs, 6), buf(env, segs, 7), c[1], one(env, job_id), &ns,
+                                  &nj, one(env, out_stats));
+  jint got[2] = {ns, nj};
+  (*env)->SetIntArrayRegion(env, out_n, 0, 2, got);
+  return rc;
+}
 /* why queried jobs are not scheduled: job_id n longs; outputs direct buffers of n bytes (status), 4n doubles (usage),
  * n ints (position, n_ahead), COOK_UNSCHED_AHEAD*n longs (ahead job ids), n bytes (plugin deferred); out_stats may be
  * null */

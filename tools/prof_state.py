@@ -32,6 +32,10 @@ rows (median of --reps calls): device time, wall time, bytes, launches, and whet
 
   python tools/prof_state.py --sweeps --pool c2 --reps 30
   python tools/prof_state.py --sweeps --pool c5 --c5-pool 5 --reps 30
+--user-usage loads C2, config-#5 pool --c5-pool, or (--c3-group N) config-#3 pools 0 .. N-1 as N handles, on the grid and
+off it, and times cook_state_user_usage for the lightest user, the heaviest user and every user, with and without
+groups, against numpy over a host mirror:
+  python tools/prof_state.py --user-usage --pool c5 --reps 10
 --unscheduled loads C2 (or config-#5 pool --c5-pool with --pool c5) into a resident handle, on the grid and off it,
 and times cook_state_unscheduled for one job, 1000 jobs and every waiting job of the user with the most, against numpy
 over a host mirror, with the answers compared bit for bit:
@@ -982,6 +986,104 @@ def unscheduled_prof(a):
         e.close()
 
 
+def host_user_usage(m, users, per_pool, by_group):
+    """numpy over a host mirror of the running rows (every handle's, with its index): cook_state_user_usage's segments
+    [(user, scope, group, jobs, cpus, mem, gpus, job ids or None)], each fold sequential in (task id, handle)."""
+    i = np.arange(len(m["user"])) if users is None else np.flatnonzero(np.isin(m["user"], users))
+    i = i[np.lexsort((m["tid"][i], m["jid"][i], m["pidx"][i]))]
+    last = np.ones(len(i), bool)
+    last[:-1] = (m["jid"][i[1:]] != m["jid"][i[:-1]]) | (m["pidx"][i[1:]] != m["pidx"][i[:-1]])
+    i = i[last]                                          # one row per (handle, job): its greatest task id
+    i = i[np.lexsort((m["pidx"][i], m["tid"][i]))]       # the fold order
+    out = []
+    for sc in [False] + ([True] if per_pool else []):
+        for gr in [False] + ([True] if by_group else []):
+            scope = m["pidx"][i] if sc else np.full(len(i), -1)
+            group = m["grp"][i] if gr else np.full(len(i), -2)
+            k = np.lexsort((np.arange(len(i)), group, scope, m["user"][i]))
+            ii, key = i[k], np.stack([m["user"][i][k], scope[k], group[k]], 1)
+            cut = np.flatnonzero(np.any(key[1:] != key[:-1], 1)) + 1
+            for s, e in zip(np.concatenate([[0], cut]), np.concatenate([cut, [len(ii)]])):
+                seg = ii[s:e]
+                sums = [float(np.cumsum(m[c][seg])[-1]) for c in ("cpus", "mem", "gpus")]
+                out.append((int(key[s, 0]), int(key[s, 1]), int(key[s, 2]), e - s, *sums,
+                            m["jid"][seg].tolist() if gr else None))
+    return sorted(out, key=lambda x: x[:3])
+
+
+def user_usage_prof(a):
+    """cook_state_user_usage over resident pools (C2, config-#5 pool --c5-pool, or --c3-group N config-#3 pools as N
+    handles with per_pool), on the grid and off it, for the lightest user, the heaviest user and every user, with and
+    without groups, against numpy over a host mirror.  A third of the running rows get a group list of one or two
+    groups of 500."""
+    if a.c3_group > 0:
+        ts = [traces.gen_config_pool("c3", p) for p in range(a.c3_group)]
+        name = f"c3/0-{a.c3_group - 1}"
+    else:
+        ts = [traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)]
+        name = a.pool if a.pool == "c2" else f"c5/{a.c5_pool}"
+    rng = np.random.default_rng(a.seed)
+    runs = [{k: np.asarray(v).copy() for k, v in t["cols"]["running"].items()} for t in ts]
+    lists = [[[int(g) for g in rng.choice(500, int(rng.integers(1, 3)), replace=False)] if rng.random() < 1 / 3
+              else [] for _ in range(len(r["task_id"]))] for r in runs]
+    print(json.dumps({"card": card(), "pools": name, "handles": len(ts),
+                      "running": sum(len(r["task_id"]) for r in runs)}), flush=True)
+    per_pool = len(ts) > 1
+    for regime in ("grid", "off"):
+        es, m = [], {k: [] for k in ("user", "tid", "jid", "pidx", "grp", "cpus", "mem", "gpus")}
+        for p, (r0, gl) in enumerate(zip(runs, lists)):
+            r = dict(r0)
+            if regime == "off":
+                r["cpus"] = r["cpus"] + 0.1
+                r["mem"] = r["mem"] / 3.0
+            off, idx = abi.csr(gl)
+            e = GpuEngine(pool_name=f"user-usage-{p}")
+            e.state_apply(abi.make_delta(reset=True, running=abi.make_tasks(**r), running_group_off=off,
+                                         running_group_idx=idx))
+            es.append(e)
+            n = len(r["task_id"])
+            for k, src in (("user", r["user"]), ("tid", r["task_id"]), ("jid", r["job_id"]), ("cpus", r["cpus"]),
+                           ("mem", r["mem"]), ("gpus", r["gpus"] if "gpus" in r else np.zeros(n))):
+                m[k].append(np.asarray(src))
+            m["pidx"].append(np.full(n, p))
+            m["grp"].append(np.array([g[0] if g else -1 for g in gl]))
+        m = {k: np.concatenate(v) for k, v in m.items()}
+        for k in ("cpus", "mem", "gpus"):
+            m[k] = m[k].astype(np.float64)
+        cnt = np.bincount(m["user"])
+        users = {"light": [int(np.argmin(np.where(cnt > 0, cnt, cnt.max() + 1)))],
+                 "heaviest": [int(cnt.argmax())], "all": None}
+        for kind, q in users.items():
+            for bg in (False, True):
+                for _ in range(3):   # warm-up: the carves and the first launches
+                    got = engine.state_user_usage(es, q, per_pool, bg)
+                dev, wall, host, same = [], [], [], True
+                for _ in range(a.reps):
+                    w0 = time.perf_counter()
+                    got = engine.state_user_usage(es, q, per_pool, bg)
+                    wall.append(time.perf_counter() - w0)
+                    st = got["stats"]
+                    dev.append(st["ms_h2d"] + st["ms_device"] + st["ms_d2h"])
+                    w0 = time.perf_counter()
+                    want = host_user_usage(m, q, per_pool, bg)
+                    host.append(time.perf_counter() - w0)
+                    same = same and len(want) == len(got["user"]) and all(
+                        (int(got["user"][d]), int(got["scope"][d]), int(got["group"][d]), int(got["jobs"][d])) == w[:4]
+                        and np.array_equal(np.array([got[c][d] for c in ("cpus", "mem", "gpus")]).view(np.int64),
+                                           np.array(w[4:7], np.float64).view(np.int64)) and got["lists"][d] == w[7]
+                        for d, w in enumerate(want))
+                print(json.dumps({"regime": regime, "users": kind, "by_group": bg, "per_pool": per_pool,
+                                  "segments": len(got["user"]), "jobs": int(sum(got["jobs"][got["scope"] == -1][
+                                      got["group"][got["scope"] == -1] == abi.UU_TOTAL])),
+                                  "device_ms": round(float(np.median(dev)), 4),
+                                  "wall_ms": round(1e3 * float(np.median(wall)), 4), "h2d_bytes": st["h2d_bytes"],
+                                  "d2h_bytes": st["d2h_bytes"], "n_launches": st["n_launches"],
+                                  "numpy_wall_ms": round(1e3 * float(np.median(host)), 4), "identical": bool(same)}),
+                      flush=True)
+        for e in es:
+            e.close()
+
+
 def rank_quota_prof(a):
     t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
     pc, rc0, users = t["cols"]["pending"], t["cols"]["running"], t["users"]
@@ -1045,7 +1147,11 @@ def main():
     ap.add_argument("--sweeps", action="store_true", help="cook_state_sweep against numpy over a host mirror")
     ap.add_argument("--reps", type=int, default=20, help="--audit, --rank-quota, --sweeps: timed calls per kind")
     ap.add_argument("--unscheduled", action="store_true", help="cook_state_unscheduled against numpy over a host mirror")
+    ap.add_argument("--user-usage", action="store_true",
+                    help="cook_state_user_usage against numpy over a host mirror (--c3-group N: N config-#3 pools)")
     a = ap.parse_args()
+    if a.user_usage:
+        return user_usage_prof(a)
     if a.unscheduled:
         return unscheduled_prof(a)
     if a.sweeps:
