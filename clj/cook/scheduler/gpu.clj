@@ -14,6 +14,8 @@
 ;;                                               cook_state_group_runtimes]
 ;;   unscheduled.clj:172-200 reasons      -> (unscheduled! ...) + cycle.py's unscheduled_reasons  [cook_state_unscheduled]
 ;;   api.clj:2946-2969 get-user-usage       -> (user-usage! ...) + cycle.py's usage_response  [cook_state_user_usage]
+;;   api.clj:3150-3232 task-stats-handler   -> (instance-stats! ...) + cycle.py's instance_stats_response, fed by
+;;                                              task-reason! [cook_state_instance_stats, cook_state_task_reason]
 ;; selected per pool with {:scheduler-config {:scheduler "gpu"}} next to "fenzo" / "kubernetes"
 ;; (config.clj:110-122, make-pool-handler :2425-2466).  Everything numeric happens in libcookgpu;
 ;; this namespace marshals columns and keeps the state Fenzo kept (cook_b200/cycle.py is the same
@@ -348,6 +350,25 @@
                                         (bytes-buf (map :unknown? facts)))
           "cook_state_task_facts"))
 
+(defn task-reason!
+  "The reason fact of live running instances, from the tx-report tap: `reasons` is [{:task-id :reason-code}], the
+   code the :reason/code of the instance's :instance/reason (-1: none).  The tap forwards every :instance/reason datom
+   whose instance is running or unknown (a killer's reason written before the backend confirms the kill); an upsert or
+   a launch of the row writes -1."
+  [handle reasons]
+  (check! handle (Native/stateTaskReason handle (count reasons) (longs-buf (map :task-id reasons))
+                                         (ints-buf (map :reason-code reasons)))
+          "cook_state_task_reason"))
+
+(defn reason-datoms
+  "The tap's half of task-reason!: from a tx-report's datoms, the [{:task-id :reason-code}] of the asserted
+   :instance/reason values whose instance `running?` holds (running or unknown in the resident state).  `reason-attr`
+   is the attribute's entity id in the tx's db; `reason-code` maps a :reason entity id to its :reason/code."
+  [datoms reason-attr running? reason-code]
+  (vec (for [d datoms
+             :when (and (= reason-attr (.a d)) (.added d) (running? (.e d)))]
+         {:task-id (.e d) :reason-code (reason-code (.v d))})))
+
 (defn finish!
   "Status updates of instances that left running or unknown: [{:task-id :end-ms :success?}].  The rows leave as a
    removal delta takes them; a success leaves its runtime per group for the straggler handler."
@@ -441,3 +462,40 @@
                  (and by-group? (not= g -2))
                  (assoc :job-ids (let [o (i32 (segs 7) d)]
                                    (vec (for [j (range jobs)] (.getLong ^ByteBuffer jids (int (* 8 (+ o j))))))))))))))))
+
+;; ---------------------------------------------------------------------------------------------
+;; /stats/instances over resident pools: the device half of task-stats/get-stats (task_stats.clj), for status running
+;; or unknown without a name filter; the handler keeps the Datomic path for success, failed and a name filter, and
+;; for pools on several devices (percentiles do not compose from per-device summaries)
+(def ^:private instance-stats-leaders 10)
+(defn instance-stats!
+  "Instance stats over `handles` (one device): `status` :running or :unknown, the window [start-ms, end-ms), the
+   entity-id bounds [task-id-lo, task-id-hi) (d/entid-at of start - 1 h and end + 1 h), one `now-ms`.  `n-rows` is the
+   live running rows over the handles (the shim's count).  Returns {:segments [{:kind 0|1|2 (overall, reason, user and
+   reason) :user :reason (-1: none) :count :totals [run cpu mem] :percentiles [[p50 p75 p95 p99 p100] x3]}]
+   :leaders-cpu [[user total]] :leaders-mem [[user total]]}; the handler builds the response (user names, reason
+   strings, the nil reason's key) as cook_b200/cycle.py's instance_stats_response does."
+  [handles status now-ms start-ms end-ms task-id-lo task-id-hi n-rows]
+  (let [cap (+ 1 (* 2 n-rows))
+        segs [(direct (* 4 cap)) (direct (* 4 cap)) (direct (* 4 cap)) (direct (* 8 cap)) (direct (* 24 cap))
+              (direct (* 120 cap))]
+        leaders [(direct (* 4 2 instance-stats-leaders)) (direct (* 8 2 instance-stats-leaders))]
+        out-n (int-array 2)]
+    (check! (first handles)
+            (Native/stateInstanceStats (long-array handles) (long-array [now-ms start-ms end-ms task-id-lo task-id-hi])
+                                       (if (= status :unknown) 1 0) (int cap) (object-array segs)
+                                       (object-array leaders) out-n nil)
+            "cook_state_instance_stats")
+    (let [i32 (fn [^ByteBuffer b d] (.getInt b (int (* 4 d))))
+          f64 (fn [^ByteBuffer b d] (.getDouble b (int (* 8 d))))
+          lead (fn [k] (vec (for [i (range (aget out-n 1))]
+                              [(i32 (leaders 0) (+ (* k instance-stats-leaders) i))
+                               (f64 (leaders 1) (+ (* k instance-stats-leaders) i))])))]
+      {:segments (vec (for [d (range (aget out-n 0))]
+                        {:kind (i32 (segs 0) d) :user (i32 (segs 1) d) :reason (i32 (segs 2) d)
+                         :count (.getLong ^ByteBuffer (segs 3) (int (* 8 d)))
+                         :totals (vec (for [m (range 3)] (f64 (segs 4) (+ (* 3 d) m))))
+                         :percentiles (vec (for [m (range 3)]
+                                             (vec (for [j (range 5)] (f64 (segs 5) (+ (* 15 d) (* 5 m) j))))))}))
+       :leaders-cpu (lead 0)
+       :leaders-mem (lead 1)})))

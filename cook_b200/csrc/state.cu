@@ -41,10 +41,11 @@ enum PCol {
 };
 constexpr int P_SZ[P_NCOL] = {4, 4, 8, 8, 8, 8, 4, 1, 1, 4, 8, 4, 8, 4, 4, 1, 4, 4, 4, 4, 4, 4, 4};
 // R_MAXRT and R_FACTS are the facts cook_state_task_facts writes: the job's max-runtime (-1: none) and the
-// RF_* bits.  Every upsert and launch writes their absent values.
+// RF_* bits; R_REASON the fact cook_state_task_reason writes: the instance's reason code (-1: none).  Every upsert
+// and launch writes their absent values.
 enum RCol { R_USER, R_PRIO, R_START, R_TID, R_JID, R_CPUS, R_MEM, R_GPUS, R_HOST, R_NDATA, R_LIVE = R_NDATA, R_GEN,
-            R_GOFF, R_GLEN, R_MAXRT, R_FACTS, R_NCOL };
-constexpr int R_SZ[R_NCOL] = {4, 4, 8, 8, 8, 8, 8, 8, 4, 1, 4, 4, 4, 8, 1};
+            R_GOFF, R_GLEN, R_MAXRT, R_FACTS, R_REASON, R_NCOL };
+constexpr int R_SZ[R_NCOL] = {4, 4, 8, 8, 8, 8, 8, 8, 4, 1, 4, 4, 4, 8, 1, 4};
 enum { RF_CANCELLED = 1, RF_UNKNOWN = 2 };
 
 // The live offers (leases): one row per offer as it arrived, before any merge.  Data columns first, then the live
@@ -128,6 +129,7 @@ __global__ void launch_kernel(const int32_t* pslot, const int32_t* rslot, const 
   static_cast<int32_t*>(rc[R_GLEN])[r] = 0;
   static_cast<int64_t*>(rc[R_MAXRT])[r] = -1;
   static_cast<uint8_t*>(rc[R_FACTS])[r] = 0;
+  static_cast<int32_t*>(rc[R_REASON])[r] = -1;
 }
 
 // ---- list lengths for the order-wide scan (integer sums: any association is exact)
@@ -1121,7 +1123,8 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
       }
       ru.c[R_NDATA] = ScatterCol{static_cast<char*>(S->run.col[R_MAXRT]), nullptr, -1, R_SZ[R_MAXRT]};
       ru.c[R_NDATA + 1] = ScatterCol{static_cast<char*>(S->run.col[R_FACTS]), nullptr, 0, R_SZ[R_FACTS]};
-      ru.nc = R_NDATA + 2;
+      ru.c[R_NDATA + 2] = ScatterCol{static_cast<char*>(S->run.col[R_REASON]), nullptr, -1, R_SZ[R_REASON]};
+      ru.nc = R_NDATA + 3;
       ru.slot = c.up(rup_slot.data(), nr);
       ru.doff[0] = c.up(rgo, nr + 1);
       if (c.base && radd) c.copy(RG.v[0] + rtail0, d->running_group_idx, radd);
@@ -3018,6 +3021,35 @@ int32_t task_facts(cook_pool* pool, PoolState* S, int n, const int64_t* task_id,
   return COOK_OK;
 }
 
+// the reason code of each listed live running row, in place (live flag and generation kept)
+int32_t task_reason(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, const int32_t* reason_code) {
+  const char* who = "cook_state_task_reason";
+  if (n < 0) return set_err(pool, COOK_E_BADARG, "%s: n < 0", who);
+  if (n && (!task_id || !reason_code)) return set_err(pool, COOK_E_BADARG, "%s: null task_id or reason_code", who);
+  if (!idx_in_range(reason_code, n, -1, INT32_MAX)) return set_err(pool, COOK_E_BADARG, "%s: a reason code below -1", who);
+  std::vector<int32_t> slot;
+  if (const char* why = running_slots(S, n, task_id, &slot)) return set_err(pool, COOK_E_BADARG, "%s: %s", who, why);
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  ScatterArgs pa;
+  memset(&pa, 0, sizeof(pa));
+  int64_t h2d = 0;
+  CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
+    if (!n) return;
+    pa.slot = c.up(slot.data(), n);
+    pa.c[pa.nc++] = ScatterCol{static_cast<char*>(S->run.col[R_REASON]),
+                               reinterpret_cast<const char*>(c.up(reason_code, n)), -1, 4};
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  int nl = 0;
+  scatter(pa, S->run, n, 0, -1, nullptr, st, &nl);
+  CK(pool, cudaGetLastError());
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  CK(pool, cudaStreamSynchronize(st));
+  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
+  return COOK_OK;
+}
+
 // running_rm_task_id = task_id, plus one record per group of each successful row
 int32_t finish(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, const int64_t* end_time_ms,
                const uint8_t* success) {
@@ -3443,6 +3475,15 @@ extern "C" int32_t cook_state_task_facts(cook_pool* pool, int32_t n, const int64
   PoolState* S = state_of(pool, true);
   if (!S) return set_err(pool, COOK_E_OOM, "cook_state_task_facts: out of device memory");
   return task_facts(pool, S, n, task_id, max_runtime_ms, cancelled, unknown);
+}
+
+extern "C" int32_t cook_state_task_reason(cook_pool* pool, int32_t n, const int64_t* task_id,
+                                          const int32_t* reason_code) {
+  if (!pool) return COOK_E_BADARG;
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_task_reason: out of device memory");
+  return task_reason(pool, S, n, task_id, reason_code);
 }
 
 extern "C" int32_t cook_state_finish(cook_pool* pool, int32_t n, const int64_t* task_id, const int64_t* end_time_ms,
@@ -4089,6 +4130,383 @@ extern "C" int32_t cook_state_user_usage(cook_pool* const* pools, int32_t n_pool
   return user_usage(pools, n_pools, user, n_users, per_pool, by_group, seg_cap, out_user, out_scope, out_group,
                     out_jobs, out_cpus, out_mem, out_gpus, out_list_off, job_cap, out_job_id, out_n_seg, out_n_job,
                     out_stats);
+}
+
+// ---- instance stats (/stats/instances, task-stats/get-stats task_stats.clj): over the selected live running rows,
+// per segment (overall, per reason, per (user, reason)) the count, and per metric (run-time, cpu and mem seconds)
+// the left fold and the nearest-rank percentiles 50 75 95 99 100; and the ten users with the largest cpu and mem
+// totals.  The live rows of every handle are compacted into one range, the selection compacted from it with the
+// three metrics, then each selected row becomes one entry per level (overall, reason, (user, reason), user).  One
+// sort by (segment, task id, pool index) gives every segment's fold order; per metric, one sort of the first three
+// levels by (segment, value) gives the ranks.  The user level's folds feed the leaders and are not returned.
+namespace {
+
+constexpr int IS_LEVELS = 4, IS_USER = 3;   // the levels' kinds: COOK_IS_OVERALL, _REASON, _USER_REASON, then users
+__device__ __forceinline__ int is_pct(int j) { return j == 0 ? 50 : j == 1 ? 75 : j == 2 ? 95 : j == 3 ? 99 : 100; }
+
+// one handle's live running rows, dense after the handles before it
+struct ISRows {
+  void* const* col; int base; int32_t pool;
+  int32_t* user; int32_t* reason; int64_t* tid; int32_t* pidx; int64_t* start; double* cpus; double* mem;
+  uint8_t* facts;
+  __device__ bool keep(int i) const { return static_cast<const uint8_t*>(col[R_LIVE])[i]; }
+  __device__ void emit(int i, int d) const {
+    d += base;
+    user[d] = static_cast<const int32_t*>(col[R_USER])[i];
+    reason[d] = static_cast<const int32_t*>(col[R_REASON])[i];
+    tid[d] = static_cast<const int64_t*>(col[R_TID])[i];
+    pidx[d] = pool;
+    start[d] = static_cast<const int64_t*>(col[R_START])[i];
+    cpus[d] = static_cast<const double*>(col[R_CPUS])[i];
+    mem[d] = static_cast<const double*>(col[R_MEM])[i];
+    facts[d] = static_cast<const uint8_t*>(col[R_FACTS])[i];
+  }
+};
+// the selected rows: status, task id in [tid_lo, tid_hi), start in [start_ms, end_ms); their metrics with one now
+// (task->task-entry: run-time-seconds = (double) ms / 1000.0, times cpus and mem).  A selected row that starts after
+// now sets *bad.
+struct ISSel {
+  const int32_t* user; const int32_t* reason; const int64_t* tid; const int32_t* pidx; const int64_t* start;
+  const double* cpus; const double* mem; const uint8_t* facts;
+  int64_t now, start_ms, end_ms, tid_lo, tid_hi; int unknown;
+  int32_t* s_user; int32_t* s_reason; int64_t* s_tid; int32_t* s_pidx; double* met[3]; int32_t* bad;
+  __device__ bool keep(int i) const {
+    return ((facts[i] & RF_UNKNOWN) != 0) == (unknown != 0) && tid[i] >= tid_lo && tid[i] < tid_hi &&
+           start[i] >= start_ms && start[i] < end_ms;
+  }
+  __device__ void emit(int i, int d) const {
+    s_user[d] = user[i]; s_reason[d] = reason[i]; s_tid[d] = tid[i]; s_pidx[d] = pidx[i];
+    if (start[i] > now) *bad = 1;
+    const double rt = (double)(now - start[i]) / 1000.0;
+    met[0][d] = rt;
+    met[1][d] = rt * cpus[i];
+    met[2][d] = rt * mem[i];
+  }
+};
+
+// The entries: entry l * S + i is selected row i at level l, keyed (kind, user, reason); the segment of an entry is
+// its key.
+struct ISKey {
+  int32_t* kind; int32_t* user; int32_t* reason;
+  __device__ bool same(int a, int b) const { return kind[a] == kind[b] && user[a] == user[b] && reason[a] == reason[b]; }
+  __device__ int cmp(int a, int b) const {
+    if (kind[a] != kind[b]) return kind[a] < kind[b] ? -1 : 1;
+    if (user[a] != user[b]) return user[a] < user[b] ? -1 : 1;
+    if (reason[a] != reason[b]) return reason[a] < reason[b] ? -1 : 1;
+    return 0;
+  }
+};
+__global__ void is_expand_kernel(int S, const int32_t* user, const int32_t* reason, ISKey k, int32_t* row) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  if (x >= IS_LEVELS * S) return;
+  const int l = x / S, i = x - l * S;
+  k.kind[x] = l;
+  k.user[x] = l >= COOK_IS_USER_REASON ? user[i] : -1;
+  k.reason[x] = l == COOK_IS_REASON || l == COOK_IS_USER_REASON ? reason[i] : -1;
+  row[x] = i;
+}
+// (segment, task id, pool index, entry): the segments in the output order, each in its fold order
+struct LessSegTidPool {
+  ISKey k; const int32_t* row; const int64_t* tid; const int32_t* pidx;
+  __device__ bool operator()(int32_t a, int32_t b) const {
+    const int c = k.cmp(a, b);
+    if (c) return c < 0;
+    const int ra = row[a], rb = row[b];
+    if (tid[ra] != tid[rb]) return tid[ra] < tid[rb];
+    if (pidx[ra] != pidx[rb]) return pidx[ra] < pidx[rb];
+    return a < b;
+  }
+};
+// (segment, value, entry): the ranks of one metric; no value is NaN or -0.0, so equal values are equal bits
+struct LessSegValue {
+  ISKey k; const int32_t* row; const double* v;
+  __device__ bool operator()(int32_t a, int32_t b) const {
+    const int c = k.cmp(a, b);
+    if (c) return c < 0;
+    const double va = v[row[a]], vb = v[row[b]];
+    if (va != vb) return va < vb;
+    return a < b;
+  }
+};
+struct ISSegEnds {   // end[d] = one past segment d's last position, segment d starting where segment d - 1 ends
+  const int32_t* ord; ISKey k; int E; int32_t* end;
+  __device__ bool keep(int p) const { return p == E - 1 || !k.same(ord[p], ord[p + 1]); }
+  __device__ void emit(int p, int d) const { end[d] = p + 1; }
+};
+struct ISLoad {   // the order-wide scan's addends: the three metrics of the entry at position p
+  const int32_t* ord; const int32_t* row; const double* met[3];
+  __device__ void operator()(int p, double (&x)[3]) const {
+    const int r = row[ord[p]];
+    x[0] = met[0][r]; x[1] = met[1][r]; x[2] = met[2][r];
+  }
+};
+struct ISFoldArgs {
+  const int32_t* ord; const int32_t* row; ISKey k; const double* met[3];
+  const int32_t* end; const int32_t* n_seg;
+  OrderScan<double, 3> os; const GridFlag* gf; int E;
+  int32_t *o_kind, *o_user, *o_reason; int64_t* o_count; double* o_total;   // o_total [3 * segment + metric]
+};
+// Warp per segment, grid-stride: the left fold of the three metrics in ascending (task id, pool index), as
+// uu_fold_kernel folds: the two ends of the order-wide scan when the whole order is on the grid, else warp_fold_sum.
+__global__ void __launch_bounds__(128) is_fold_kernel(ISFoldArgs a) {
+  __shared__ double stage[4][3][32];
+  const int n = *a.n_seg, nw = gridDim.x * (blockDim.x >> 5);
+  const bool scan = grid_exact(a.gf, a.E);
+  for (int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; g < n; g += nw) {
+    const int s = g ? a.end[g - 1] : 0, e = a.end[g];
+    double acc[3] = {0.0, 0.0, 0.0};
+    if (scan) {
+#pragma unroll
+      for (int k = 0; k < 3; k++) acc[k] = a.os.segment_sum(k, e - 1, s);
+    } else {
+      warp_fold_sum<3, 4>(acc, e - s, grid_exact(a.gf, e - s), [&](int k, double (&x)[3]) {
+        const int r = a.row[a.ord[s + k]];
+        x[0] = a.met[0][r]; x[1] = a.met[1][r]; x[2] = a.met[2][r];
+        return true;
+      }, stage[threadIdx.x >> 5]);
+    }
+    if (threadIdx.x & 31) continue;
+    const int i = a.ord[s];
+    a.o_kind[g] = a.k.kind[i]; a.o_user[g] = a.k.user[i]; a.o_reason[g] = a.k.reason[i];
+    a.o_count[g] = e - s;
+#pragma unroll
+    for (int k = 0; k < 3; k++) a.o_total[3 * g + k] = acc[k];
+  }
+}
+// thread per (returned segment, metric): element ceil(p * n / 100) - 1 of the segment's ascending values
+// (percentile, task_stats.clj: p/100 is a ratio, so exact integer arithmetic).  The user segments come last and are
+// skipped.
+__global__ void is_pct_kernel(const int32_t* n_seg, const int32_t* end, const int32_t* o_kind, const int32_t* ord0,
+                              const int32_t* ord1, const int32_t* ord2, const int32_t* row, const double* m0,
+                              const double* m1, const double* m2, double* o_pct) {
+  const int n = *n_seg;
+  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < 3 * n; t += gridDim.x * blockDim.x) {
+    const int g = t / 3, m = t - 3 * g;
+    if (o_kind[g] == IS_USER) continue;
+    const int s = g ? end[g - 1] : 0;
+    const int64_t c = end[g] - s;
+    const int32_t* ord = m == 0 ? ord0 : m == 1 ? ord1 : ord2;
+    const double* v = m == 0 ? m0 : m == 1 ? m1 : m2;
+#pragma unroll
+    for (int j = 0; j < 5; j++) o_pct[15 * g + 5 * m + j] = v[row[ord[s + (int)((is_pct(j) * c + 99) / 100) - 1]]];
+  }
+}
+// block k (0: cpu seconds, 1: mem seconds): the first COOK_IS_LEADERS users in (total descending, user ascending)
+// order, one block-wide selection per place, each of the users after the previous pick.  The user segments are the
+// last ones, [n_ret, n_seg), in ascending user; block 0 writes n_ret and the leaders' number to counts[0, 2).
+__global__ void __launch_bounds__(256) is_leaders_kernel(const int32_t* n_seg, const int32_t* o_kind,
+                                                         const int32_t* o_user, const double* o_total,
+                                                         int32_t* l_user, double* l_total, int32_t* counts) {
+  __shared__ int s_ret;
+  __shared__ double s_v[8];
+  __shared__ int32_t s_u[8];
+  const int n = *n_seg, k = blockIdx.x + 1, lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  if (threadIdx.x == 0) {
+    int lo = 0, hi = n;   // the first user segment: kinds ascend
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (o_kind[mid] < IS_USER) lo = mid + 1;
+      else hi = mid;
+    }
+    s_ret = lo;
+  }
+  __syncthreads();
+  const int first = s_ret, U = n - first, L = min(U, COOK_IS_LEADERS);
+  double pv = 0.0;
+  int32_t pu = -1;
+  for (int r = 0; r < L; r++) {
+    double bv = -1.0;
+    int32_t bu = INT32_MAX;
+    for (int g = first + threadIdx.x; g < n; g += blockDim.x) {
+      const double v = o_total[3 * g + k];
+      const int32_t u = o_user[g];
+      const bool after = r == 0 || v < pv || (v == pv && u > pu);
+      if (after && (v > bv || (v == bv && u < bu))) { bv = v; bu = u; }
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+      const double v = __shfl_xor_sync(FULL_MASK, bv, o);
+      const int32_t u = __shfl_xor_sync(FULL_MASK, bu, o);
+      if (v > bv || (v == bv && u < bu)) { bv = v; bu = u; }
+    }
+    if (lane == 0) { s_v[w] = bv; s_u[w] = bu; }
+    __syncthreads();
+    bv = s_v[0]; bu = s_u[0];
+    for (int q = 1; q < 8; q++)
+      if (s_v[q] > bv || (s_v[q] == bv && s_u[q] < bu)) { bv = s_v[q]; bu = s_u[q]; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      l_user[blockIdx.x * COOK_IS_LEADERS + r] = bu;
+      l_total[blockIdx.x * COOK_IS_LEADERS + r] = bv;
+    }
+    pv = bv; pu = bu;
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    counts[0] = first;
+    counts[1] = L;
+  }
+}
+
+int32_t instance_stats(cook_pool* const* pools, int n, int64_t now, int32_t status, int64_t start_ms, int64_t end_ms,
+                       int64_t tid_lo, int64_t tid_hi, int32_t seg_cap, int32_t* o_kind, int32_t* o_user,
+                       int32_t* o_reason, int64_t* o_count, double* o_total, double* o_pct, int32_t* o_lead_user,
+                       double* o_lead_total, int32_t* o_nseg, int32_t* o_nlead, cook_phase_stats* out_stats) {
+  const char* who = "cook_state_instance_stats";
+  // ---- every check before any device work or output
+  if (!pools || n <= 0 || !pools[0]) return COOK_E_BADARG;
+  cook_pool* pool = pools[0];
+  for (int k = 0; k < n; k++) {
+    if (!pools[k]) return set_err(pool, COOK_E_BADARG, "%s: a NULL handle", who);
+    if (std::find(pools, pools + k, pools[k]) != pools + k)
+      return set_err(pool, COOK_E_BADARG, "%s: a handle listed twice", who);
+    if (pools[k]->device != pool->device) return set_err(pool, COOK_E_BADARG, "%s: handles on different devices", who);
+  }
+  if (status != COOK_IS_RUNNING && status != COOK_IS_UNKNOWN) return set_err(pool, COOK_E_BADARG, "%s: an unknown status", who);
+  if (end_ms <= start_ms) return set_err(pool, COOK_E_BADARG, "%s: end_ms <= start_ms", who);
+  if (!o_kind || !o_user || !o_reason || !o_count || !o_total || !o_pct || !o_lead_user || !o_lead_total || !o_nseg ||
+      !o_nlead)
+    return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
+  // the handles with rows and their pool index; sizes from the host-side counts
+  std::vector<std::pair<const PoolState*, int32_t>> hs;
+  int64_t R = 0;
+  int hw = 0;
+  for (int k = 0; k < n; k++) {
+    const PoolState* s = static_cast<const PoolState*>(pools[k]->state);
+    if (!s || s->run.slot_of.empty()) continue;
+    hs.push_back({s, k});
+    R += (int64_t)s->run.slot_of.size();
+    hw = std::max(hw, s->run.hw);
+  }
+  if (R * IS_LEVELS > INT32_MAX) return set_err(pool, COOK_E_TOO_LARGE, "%s: more than 2^31 - 1 entries", who);
+  if (seg_cap < 1 + 2 * R) return set_err(pool, COOK_E_BADARG, "%s: seg_cap below 1 + 2 * the live running rows", who);
+  if (R == 0) {   // no row to read: empty results without device work
+    *o_nseg = 0;
+    *o_nlead = 0;
+    if (out_stats) *out_stats = cook_phase_stats{};
+    return COOK_OK;
+  }
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S0 = state_of(pool, true);   // pools[0]'s scratch, even when it holds no row
+  if (!S0) return set_err(pool, COOK_E_OOM, "%s: out of device memory", who);
+  cudaStream_t st = pool->stream;
+  const int Rn = (int)R, Emax = IS_LEVELS * Rn;
+  hw = std::max(hw, Emax);
+  // ---- one carve, sized by the live rows: the rows, the selection, the entries and their orders, the outputs
+  int32_t *cnt = nullptr, *blk = nullptr, *a_user = nullptr, *a_reason = nullptr, *a_pidx = nullptr;
+  int64_t *a_tid = nullptr, *a_start = nullptr;
+  double *a_cpus = nullptr, *a_mem = nullptr;
+  uint8_t* a_facts = nullptr;
+  int32_t *s_user = nullptr, *s_reason = nullptr, *s_pidx = nullptr, *row = nullptr, *ord = nullptr, *tmp = nullptr;
+  int32_t *end = nullptr, *vord[3] = {}, *l_user = nullptr;
+  int64_t* s_tid = nullptr;
+  double *met[3] = {}, *pct = nullptr, *l_total = nullptr;
+  GridFlag* gf = nullptr;
+  ISKey key = {};
+  ISFoldArgs a = {};
+  int64_t h2d = 0, d2h = 0;
+  CK(pool, carve(S0->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+    cnt = c.take<int32_t>(6);   // selected, start after now, segments, returned segments, leaders, compactions' own
+    blk = c.take<int32_t>((size_t)hw / CP_BLOCK + 2);
+    a_user = c.take<int32_t>(Rn); a_reason = c.take<int32_t>(Rn); a_pidx = c.take<int32_t>(Rn);
+    a_tid = c.take<int64_t>(Rn); a_start = c.take<int64_t>(Rn);
+    a_cpus = c.take<double>(Rn); a_mem = c.take<double>(Rn); a_facts = c.take<uint8_t>(Rn);
+    s_user = c.take<int32_t>(Rn); s_reason = c.take<int32_t>(Rn); s_pidx = c.take<int32_t>(Rn);
+    s_tid = c.take<int64_t>(Rn);
+    for (int k = 0; k < 3; k++) met[k] = c.take<double>(Rn);
+    gf = c.take<GridFlag>(1);
+    key.kind = c.take<int32_t>(Emax); key.user = c.take<int32_t>(Emax); key.reason = c.take<int32_t>(Emax);
+    row = c.take<int32_t>(Emax); ord = c.take<int32_t>(Emax); tmp = c.take<int32_t>(Emax); end = c.take<int32_t>(Emax);
+    for (int k = 0; k < 3; k++) vord[k] = c.take<int32_t>(Emax);
+    for (int k = 0; k < 3; k++) {
+      a.os.part[k] = c.take<double>(Emax);
+      a.os.tile[k] = c.take<double>(Emax / OS_TILE + 2);
+    }
+    a.o_kind = c.take<int32_t>(Emax); a.o_user = c.take<int32_t>(Emax); a.o_reason = c.take<int32_t>(Emax);
+    a.o_count = c.take<int64_t>(Emax); a.o_total = c.take<double>(3 * (size_t)Emax);
+    pct = c.take<double>(15 * (size_t)Emax);
+    l_user = c.take<int32_t>(2 * COOK_IS_LEADERS); l_total = c.take<double>(2 * COOK_IS_LEADERS);
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  CK(pool, cudaMemsetAsync(cnt, 0, sizeof(int32_t) * 6, st));
+  CK(pool, cudaMemsetAsync(gf, 0, sizeof(GridFlag), st));
+  int nl = 0;
+  // ---- the selection and its metrics
+  int base = 0;
+  for (const auto& h : hs) {
+    const int live = (int)h.first->run.slot_of.size();
+    compact(ISRows{h.first->run.d_col, base, h.second, a_user, a_reason, a_tid, a_pidx, a_start, a_cpus, a_mem,
+                   a_facts},
+            h.first->run.hw, nullptr, blk, cnt + 5, live, st, &nl);
+    base += live;
+  }
+  compact(ISSel{a_user, a_reason, a_tid, a_pidx, a_start, a_cpus, a_mem, a_facts, now, start_ms, end_ms, tid_lo, tid_hi,
+                status == COOK_IS_UNKNOWN, s_user, s_reason, s_tid, s_pidx, {met[0], met[1], met[2]}, cnt + 1},
+          Rn, nullptr, blk, cnt + 0, Rn, st, &nl);
+  CK(pool, cudaGetLastError());
+  int32_t sel[2];
+  CK(pool, download(sel, cnt, 2, st, &d2h));
+  CK(pool, cudaStreamSynchronize(st));
+  if (sel[1]) return set_err(pool, COOK_E_BADARG, "%s: a selected task starts after now_ms", who);
+  const int S = sel[0], E = IS_LEVELS * S, E3 = 3 * S;
+  int32_t got[2] = {0, 0};
+  if (S > 0) {
+    // ---- the entries, the fold order and its segments, the folds
+    grid_check_kernel<<<(S + 255) / 256, 256, 0, st>>>(met[0], met[1], met[2], S, gf);
+    is_expand_kernel<<<(E + 255) / 256, 256, 0, st>>>(S, s_user, s_reason, key, row);
+    nl += 2;
+    CK(pool, csort::sort_indices(ord, tmp, E, LessSegTidPool{key, row, s_tid, s_pidx}, st, &nl));
+    compact(ISSegEnds{ord, key, E, end}, E, nullptr, blk, cnt + 2, E, st, &nl);
+    order_scan(a.os, ISLoad{ord, row, {met[0], met[1], met[2]}}, E, gf, st, &nl);
+    a.ord = ord; a.row = row; a.k = key;
+    for (int k = 0; k < 3; k++) a.met[k] = met[k];
+    a.end = end; a.n_seg = cnt + 2; a.gf = gf; a.E = E;
+    is_fold_kernel<<<std::min((E + 3) / 4, 4096), 128, 0, st>>>(a);
+    nl++;
+    // ---- the ranks: the three levels returned are entries [0, 3 S), whose segments lead the fold order's
+    for (int k = 0; k < 3; k++) CK(pool, csort::sort_indices(vord[k], tmp, E3, LessSegValue{key, row, met[k]}, st, &nl));
+    is_pct_kernel<<<std::min((3 * E + 255) / 256, 4096), 256, 0, st>>>(cnt + 2, end, a.o_kind, vord[0], vord[1], vord[2],
+                                                                      row, met[0], met[1], met[2], pct);
+    is_leaders_kernel<<<2, 256, 0, st>>>(cnt + 2, a.o_kind, a.o_user, a.o_total, l_user, l_total, cnt + 3);
+    nl += 2;
+    CK(pool, cudaGetLastError());
+    CK(pool, download(got, cnt + 3, 2, st, &d2h));
+    CK(pool, cudaStreamSynchronize(st));
+  }
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  const int ns = got[0], nlead = got[1];
+  if (ns) {
+    CK(pool, download(o_kind, a.o_kind, ns, st, &d2h));
+    CK(pool, download(o_user, a.o_user, ns, st, &d2h));
+    CK(pool, download(o_reason, a.o_reason, ns, st, &d2h));
+    CK(pool, download(o_count, a.o_count, ns, st, &d2h));
+    CK(pool, download(o_total, a.o_total, 3 * (size_t)ns, st, &d2h));
+    CK(pool, download(o_pct, pct, 15 * (size_t)ns, st, &d2h));
+  }
+  for (int k = 0; k < 2 && nlead; k++) {
+    CK(pool, download(o_lead_user + k * COOK_IS_LEADERS, l_user + k * COOK_IS_LEADERS, nlead, st, &d2h));
+    CK(pool, download(o_lead_total + k * COOK_IS_LEADERS, l_total + k * COOK_IS_LEADERS, nlead, st, &d2h));
+  }
+  CK(pool, cudaEventRecord(pool->ev[23], st));
+  CK(pool, cudaStreamSynchronize(st));
+  *o_nseg = ns;
+  *o_nlead = nlead;
+  // the call's own statistics: no cook_last_stats slot is written
+  if (out_stats)
+    *out_stats = {ev_ms(pool->ev[20], pool->ev[21]), ev_ms(pool->ev[21], pool->ev[22]), ev_ms(pool->ev[22], pool->ev[23]),
+                  h2d, d2h, nl, 0};
+  return COOK_OK;
+}
+
+}  // namespace
+
+extern "C" int32_t cook_state_instance_stats(cook_pool* const* pools, int32_t n_pools, int64_t now_ms, int32_t status,
+                                             int64_t start_ms, int64_t end_ms, int64_t task_id_lo, int64_t task_id_hi,
+                                             int32_t seg_cap, int32_t* out_kind, int32_t* out_user,
+                                             int32_t* out_reason, int64_t* out_count, double* out_total,
+                                             double* out_pct, int32_t* out_leader_user, double* out_leader_total,
+                                             int32_t* out_n_seg, int32_t* out_n_leader, cook_phase_stats* out_stats) {
+  return instance_stats(pools, n_pools, now_ms, status, start_ms, end_ms, task_id_lo, task_id_hi, seg_cap, out_kind,
+                        out_user, out_reason, out_count, out_total, out_pct, out_leader_user, out_leader_total,
+                        out_n_seg, out_n_leader, out_stats);
 }
 
 // ---- audit: the read side (cook_state_digest, cook_state_export, cook_state_queue).  The digest is one pass per

@@ -22,6 +22,8 @@ path end to end.  It computes nothing numeric: every placement decision is `engi
   unscheduled_reasons   reasons (unscheduled.clj:172-200) of a resident pool's job from cook_state_unscheduled and the
                         host's limit maps and facts; Investigations, the host half of record-placement-failures!
   usage_response        the body of GET /usage (get-user-usage, api.clj:2946-2969) from cook_state_user_usage answers
+  instance_stats_response  the body of GET /stats/instances (task-stats/get-stats) from a cook_state_instance_stats
+                        answer
 """
 import numpy as np
 
@@ -604,3 +606,40 @@ def usage_response(answers, *, user=None, pool=None, pools=(), group_breakdown=F
     if user is not None:
         return usage(int(user))
     return {"users": {name_of(u): usage(u) for u in sorted(acc)}}
+
+
+# ---- instance stats (GET /stats/instances, task-stats/get-stats task_stats.clj) ----------------------------------
+_IS_METRICS = ("run-time-seconds", "cpu-seconds", "mem-seconds")   # by abi.IS_RUN_TIME, IS_CPU, IS_MEM
+_IS_PCTS = (50, 75, 95, 99, 100)
+
+
+def instance_stats_response(answer, *, user_name=None, reason_string=None):
+    """The body of GET /stats/instances from an engine.state_instance_stats answer, in the reference's shape
+    (generate-all-stats): "overall" ({} when no instance is selected), "by-reason" {reason: stats},
+    "by-user-and-reason" {user: {reason: stats}} and "leaders" {"cpu-seconds" / "mem-seconds": {user: total}}, the
+    leaders in descending total.  stats = {"count", and per metric {"percentiles": {50 75 95 99 100}, "total"}}.
+    user_name(code) and reason_string(code >= 0) give what the response shows (default: the codes).  The nil reason
+    (code -1) is the key "", which is how the reference's JSON encoder writes a nil map key."""
+    name_of = user_name or (lambda u: u)
+    reason_of = reason_string or (lambda r: r)
+    key = lambda r: "" if r == -1 else reason_of(r)
+
+    def stats(d):
+        out = {"count": int(answer["count"][d])}
+        for m, k in enumerate(_IS_METRICS):
+            out[k] = {"percentiles": {p: float(answer["pct"][d][m][j]) for j, p in enumerate(_IS_PCTS)},
+                      "total": float(answer["total"][d][m])}
+        return out
+
+    out = {"by-reason": {}, "by-user-and-reason": {}, "leaders": {}, "overall": {}}
+    for d in range(len(answer["kind"])):
+        kind, u, r = int(answer["kind"][d]), int(answer["user"][d]), int(answer["reason"][d])
+        if kind == abi.IS_OVERALL:
+            out["overall"] = stats(d)
+        elif kind == abi.IS_REASON:
+            out["by-reason"][key(r)] = stats(d)
+        else:
+            out["by-user-and-reason"].setdefault(name_of(u), {})[key(r)] = stats(d)
+    out["leaders"] = {"cpu-seconds": {name_of(u): t for u, t in answer["leaders_cpu"]},
+                      "mem-seconds": {name_of(u): t for u, t in answer["leaders_mem"]}}
+    return out

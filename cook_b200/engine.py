@@ -232,6 +232,17 @@ class GpuEngine:
         if rc != 0:
             self._err(rc)
 
+    def state_task_reason(self, task_id, reason_code):
+        """cook_state_task_reason: the reason code of live running tasks (the caller's :reason/code dictionary, -1:
+        none), read by state_instance_stats."""
+        tid = np.ascontiguousarray(task_id, np.int64)
+        rc_ = np.ascontiguousarray(reason_code, np.int32)
+        if len(rc_) != len(tid):
+            raise ValueError("state_task_reason: reason_code differs in length from task_id")
+        rc = self.lib.cook_state_task_reason(self.pool, len(tid), abi.ptr(tid, abi.P_I64), abi.ptr(rc_, abi.P_I32))
+        if rc != 0:
+            self._err(rc)
+
     def state_finish(self, task_id, end_time_ms=None, success=None):
         """cook_state_finish: the tasks leave as a removal delta would take them; each successful one leaves a runtime
         record per group of its list (success None: none succeeded)."""
@@ -702,6 +713,37 @@ def state_user_usage(engines, users=None, per_pool=False, by_group=False):
     out["lists"] = [None if not by_group or out["group"][d] == abi.UU_TOTAL else
                     jid[off[d]:off[d] + jobs[d]].tolist() for d in range(n)]
     return out
+
+
+def state_instance_stats(engines, now_ms, status, start_ms, end_ms, task_id_lo=-(1 << 63), task_id_hi=(1 << 63) - 1):
+    """cook_state_instance_stats over the live running rows of `engines` (one device, the work on engines[0]'s stream):
+    the rows of `status` (abi.IS_RUNNING or abi.IS_UNKNOWN) with task_id_lo <= task id < task_id_hi and start_ms <=
+    start < end_ms.  Returns the segments as numpy columns 'kind', 'user', 'reason', 'count' (int64), 'total' [n, 3]
+    and 'pct' [n, 3, 5] (metrics by abi.IS_RUN_TIME / IS_CPU / IS_MEM, percentiles 50 75 95 99 100), the leaders
+    'leaders_cpu' and 'leaders_mem' as [(user, total)], and 'stats', the call's own phase statistics.  The segment
+    capacity is sized from the engines' live running ids."""
+    if not engines:
+        raise ValueError("state_instance_stats: at least one handle")
+    R = sum(len(getattr(e, "_state_running_ids", ())) for e in engines)
+    cap = 1 + 2 * R
+    kind, user, reason = (np.zeros(cap, np.int32) for _ in range(3))
+    count = np.zeros(cap, np.int64)
+    total, pct = np.zeros((cap, 3)), np.zeros((cap, 3, 5))
+    lu, lt = np.zeros(2 * abi.IS_LEADERS, np.int32), np.zeros(2 * abi.IS_LEADERS)
+    n_seg, n_lead = C.c_int32(0), C.c_int32(0)
+    st = abi.PhaseStats()
+    handles = (C.c_void_p * len(engines))(*[e.pool for e in engines])
+    rc = engines[0].lib.cook_state_instance_stats(
+        handles, len(engines), int(now_ms), int(status), int(start_ms), int(end_ms), int(task_id_lo), int(task_id_hi),
+        cap, abi.ptr(kind, abi.P_I32), abi.ptr(user, abi.P_I32), abi.ptr(reason, abi.P_I32), abi.ptr(count, abi.P_I64),
+        abi.ptr(total, abi.P_F64), abi.ptr(pct, abi.P_F64), abi.ptr(lu, abi.P_I32), abi.ptr(lt, abi.P_F64),
+        C.byref(n_seg), C.byref(n_lead), C.byref(st))
+    if rc != 0:
+        engines[0]._err(rc)
+    n, L = n_seg.value, n_lead.value
+    lead = lambda k: [(int(lu[k * abi.IS_LEADERS + i]), float(lt[k * abi.IS_LEADERS + i])) for i in range(L)]
+    return {"kind": kind[:n], "user": user[:n], "reason": reason[:n], "count": count[:n], "total": total[:n],
+            "pct": pct[:n], "leaders_cpu": lead(0), "leaders_mem": lead(1), "stats": st.as_dict()}
 
 
 STATS_KEYS = ("running", "waiting", "starved", "waiting-under-quota")   # by abi.STATS_*

@@ -873,7 +873,7 @@ int32_t cook_state_queue(cook_pool* pool, int32_t cap, int64_t* out_job_id, int3
 /* Device-side timing of the last call of each kind on this handle (CUDA events on the
  * pool's stream): what bench.py's `phases` block and roofline lines are computed from.
  * COOK_PHASE_STATE: the last cook_state_apply, cook_state_launch, cook_state_patch, cook_state_task_facts,
- * cook_state_finish or cook_state_group_runtimes (upload, then the scatter / move / record / compaction kernels).  COOK_PHASE_USAGE: the last cook_state_usage (upload of the
+ * cook_state_task_reason, cook_state_finish or cook_state_group_runtimes (upload, then the scatter / move / record / compaction kernels).  COOK_PHASE_USAGE: the last cook_state_usage (upload of the
  * hostname list, the compaction, sorts and folds, the download of the sums).  COOK_PHASE_COTASKS: the last
  * cook_state_cotasks (upload of the host codes, attribute columns and group map, the compaction, expansion and
  * sort, the download of the lists; all zero after a call without device work).  COOK_PHASE_CONSIDERABLE: the last
@@ -964,6 +964,18 @@ int32_t cook_state_user_stats(cook_pool* const* pools, int32_t n_pools, const co
  * [cancelled or unknown] 1) bytes.  Statistics: cook_last_stats(COOK_PHASE_STATE).                                */
 int32_t cook_state_task_facts(cook_pool* pool, int32_t n, const int64_t* task_id, const int64_t* max_runtime_ms,
                               const uint8_t* cancelled, const uint8_t* unknown);
+
+/* The reason fact of live running rows, by task id: reason_code[i] is the instance's :instance/reason as the caller's
+ * dictionary of :reason/code values, -1 for none.  A running or unknown instance carries one only when a killer wrote
+ * it before the backend confirmed the kill (:reason-killed-by-user from the cancelled-task killer, scheduler.clj:2012,
+ * and from the tx-report job-completion kill, :439); :instance/update-state writes none.  Written in place like
+ * cook_state_task_facts (live flag and generation kept); every running upsert of cook_state_apply and every
+ * cook_state_launch writes -1.  Not part of cook_state_digest or cook_state_export: after a resync the caller sends it
+ * again.  cook_state_instance_stats reads it.
+ * COOK_E_BADARG, before any change: n < 0; a NULL task_id or reason_code while n > 0; a task id that is not live or
+ * appears twice; a reason code below -1.  Uploads exactly 8 * n bytes (the slots and the codes).
+ * Statistics: cook_last_stats(COOK_PHASE_STATE).                                                                  */
+int32_t cook_state_task_reason(cook_pool* pool, int32_t n, const int64_t* task_id, const int32_t* reason_code);
 
 /* Finished tasks by id.  Leaves exactly the state cook_state_apply with running_rm_task_id = task_id leaves for every
  * other call (rows, list arenas, counts, digest, export, queue).  In addition, each row with success[i] != 0 appends one
@@ -1097,6 +1109,53 @@ int32_t cook_state_user_usage(cook_pool* const* pools, int32_t n_pools, const in
                               int32_t* out_scope, int32_t* out_group, int64_t* out_jobs, double* out_cpus,
                               double* out_mem, double* out_gpus, int32_t* out_list_off, int32_t job_cap,
                               int64_t* out_job_id, int32_t* out_n_seg, int32_t* out_n_job, cook_phase_stats* out_stats);
+
+/* ------------------------------------------------------- instance stats over resident pools */
+/* The device half of GET /stats/instances with status running or unknown and no name filter (task-stats/get-stats,
+ * task_stats.clj) over the union of the live running rows of pools[0, n_pools); the handles follow
+ * cook_state_user_stats' rules (one device, idle, the work on pools[0]'s stream and scratch).  Pools on several devices
+ * keep the Datomic path: percentiles do not compose from per-device summaries.
+ *   Selection  (get-tasks) a row is selected when its status is `status` (COOK_IS_RUNNING: without the unknown fact of
+ *              cook_state_task_facts; COOK_IS_UNKNOWN: with it), task_id_lo <= task id < task_id_hi (the caller's
+ *              d/entid-at of start - 1 h and end + 1 h; the bound is part of the reference's semantics) and
+ *              start_ms <= start < end_ms.
+ *   Entries    (task->task-entry) run_time = (double)(now_ms - start) / 1000.0, cpu = run_time * cpus, mem = run_time *
+ *              mem, each an f64 product; reason the row's cook_state_task_reason code (-1: none); user the row's.
+ *   Segments   (generate-all-stats) kind COOK_IS_OVERALL (user -1, reason -1), COOK_IS_REASON (user -1) and
+ *              COOK_IS_USER_REASON; only non-empty segments, in ascending (kind, user, reason), -1 first.  No selected
+ *              row: no segment (the reference's {} overall).
+ *   Outputs    per segment d < *out_n_seg: out_kind, out_user, out_reason, out_count (rows), and for metric m
+ *              (COOK_IS_RUN_TIME, COOK_IS_CPU, COOK_IS_MEM) out_total[3 * d + m] and out_pct[15 * d + 5 * m + j], the
+ *              nearest-rank percentiles p = 50, 75, 95, 99, 100: element ceil(p * n / 100) - 1 of the segment's n
+ *              values in ascending order.  Leaders: for k = 0 (cpu) and 1 (mem), out_leader_user / out_leader_total
+ *              [COOK_IS_LEADERS * k + i], i < *out_n_leader = min(COOK_IS_LEADERS, users selected): the users with the
+ *              largest per-user total of that metric, totals descending.
+ * Fixed choices:
+ *   Now      one now_ms for the whole call (the reference calls t/now per lazily realised entry).
+ *   Order    every total is a left fold from +0.0 in ascending (task id, pool index), a task id several handles hold by
+ *            pool index; a user's leader total is its own fold over all its selected rows, not a sum of its per-reason
+ *            totals.  The percentile sort is by value; equal values are equal bits (no value is -0.0 or NaN).
+ *   Ties     leaders of equal totals go by ascending user code (the reference's order is its user map's hash order).
+ * Sizes: seg_cap >= 1 + 2 * R, R the live running rows over the handles (the library's host-side counts).
+ * Changes nothing resident (rows, queue, match plan, COOK_USAGE_LAST_MATCH).
+ * COOK_E_BADARG, before any device work and with nothing written: cook_state_user_stats' handle cases; an unknown
+ * status; end_ms <= start_ms; a NULL output (out_stats may be NULL); seg_cap below its bound.  COOK_E_TOO_LARGE: 4 * R
+ * >= 2^31.  COOK_E_BADARG after the selection, with nothing written: a selected row that starts after now_ms (the
+ * reference's interval throws; this error is ours).  No live row: empty results without device work (statistics
+ * zero).
+ * Transfers exactly: up nothing; down 8 (the selection's count and flag), and when a row is selected 8 (the counts)
+ * + 164 * *out_n_seg (kind, user, reason, count, three totals, fifteen percentiles) + 24 * *out_n_leader.
+ * Statistics: out_stats (may be NULL), as cook_state_user_stats; no cook_last_stats slot is written.  The outputs are
+ * plain arrays, like cook_state_user_stats' outputs: every struct of this header has a ctypes mirror. */
+enum { COOK_IS_RUNNING = 0, COOK_IS_UNKNOWN = 1 };
+enum { COOK_IS_OVERALL = 0, COOK_IS_REASON = 1, COOK_IS_USER_REASON = 2 };
+enum { COOK_IS_RUN_TIME = 0, COOK_IS_CPU = 1, COOK_IS_MEM = 2, COOK_IS_LEADERS = 10 };
+int32_t cook_state_instance_stats(cook_pool* const* pools, int32_t n_pools, int64_t now_ms, int32_t status,
+                                  int64_t start_ms, int64_t end_ms, int64_t task_id_lo, int64_t task_id_hi,
+                                  int32_t seg_cap, int32_t* out_kind, int32_t* out_user, int32_t* out_reason,
+                                  int64_t* out_count, double* out_total, double* out_pct, int32_t* out_leader_user,
+                                  double* out_leader_total, int32_t* out_n_seg, int32_t* out_n_leader,
+                                  cook_phase_stats* out_stats);
 
 /* ----------------------------------------------------------------- multi-GPU */
 /* §8e: after a pool's match round every rank contributes its pools' usage

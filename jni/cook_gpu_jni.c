@@ -285,6 +285,10 @@ JFN(jint, stateTaskFacts)(JNIEnv* env, jclass k, jlong pool, jint n, jobject tas
   return cook_state_task_facts((cook_pool*)(intptr_t)pool, n, one(env, task_id), one(env, max_runtime_ms),
                                one(env, cancelled), one(env, unknown));
 }
+/* the reason fact of running tasks: task_id n longs, reason_code n ints (-1: none) */
+JFN(jint, stateTaskReason)(JNIEnv* env, jclass k, jlong pool, jint n, jobject task_id, jobject reason_code) {
+  return cook_state_task_reason((cook_pool*)(intptr_t)pool, n, one(env, task_id), one(env, reason_code));
+}
 /* finished tasks: task_id and end_time_ms n longs, success n bytes (null: none succeeded) */
 JFN(jint, stateFinish)(JNIEnv* env, jclass k, jlong pool, jint n, jobject task_id, jobject end_time_ms,
                        jobject success) {
@@ -338,6 +342,28 @@ JFN(jint, stateUserUsage)(JNIEnv* env, jclass k, jlongArray pools, jint n_users,
                                   buf(env, segs, 5), buf(env, segs, 6), buf(env, segs, 7), c[1], one(env, job_id), &ns,
                                   &nj, one(env, out_stats));
   jint got[2] = {ns, nj};
+  (*env)->SetIntArrayRegion(env, out_n, 0, 2, got);
+  return rc;
+}
+/* instance stats: times [now_ms, start_ms, end_ms, task_id_lo, task_id_hi]; segs the direct buffers of kind, user,
+ * reason (seg_cap ints), count (seg_cap longs), total (3 * seg_cap doubles), pct (15 * seg_cap doubles); leaders the
+ * direct buffers of user (2 * COOK_IS_LEADERS ints) and total (2 * COOK_IS_LEADERS doubles); out_n gets [n_seg,
+ * n_leader]; out_stats may be null */
+JFN(jint, stateInstanceStats)(JNIEnv* env, jclass k, jlongArray pools, jlongArray times, jint status, jint seg_cap,
+                              jobjectArray segs, jobjectArray leaders, jintArray out_n, jobject out_stats) {
+  jsize n = (*env)->GetArrayLength(env, pools);
+  if (n > 64) return COOK_E_BADARG;
+  jlong* h = (*env)->GetLongArrayElements(env, pools, NULL);
+  cook_pool* p[64];
+  for (jsize i = 0; i < n; i++) p[i] = (cook_pool*)(intptr_t)h[i];
+  (*env)->ReleaseLongArrayElements(env, pools, h, JNI_ABORT);
+  jlong t[5]; (*env)->GetLongArrayRegion(env, times, 0, 5, t);
+  int32_t ns = 0, nl = 0;
+  jint rc = cook_state_instance_stats(p, (int32_t)n, t[0], status, t[1], t[2], t[3], t[4], seg_cap, buf(env, segs, 0),
+                                      buf(env, segs, 1), buf(env, segs, 2), buf(env, segs, 3), buf(env, segs, 4),
+                                      buf(env, segs, 5), buf(env, leaders, 0), buf(env, leaders, 1), &ns, &nl,
+                                      one(env, out_stats));
+  jint got[2] = {ns, nl};
   (*env)->SetIntArrayRegion(env, out_n, 0, 2, got);
   return rc;
 }

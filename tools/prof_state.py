@@ -36,6 +36,10 @@ rows (median of --reps calls): device time, wall time, bytes, launches, and whet
 off it, and times cook_state_user_usage for the lightest user, the heaviest user and every user, with and without
 groups, against numpy over a host mirror:
   python tools/prof_state.py --user-usage --pool c5 --reps 10
+--instance-stats loads C2, config-#5 pool --c5-pool, or (--c3-group N) config-#3 pools 0 .. N-1 as N handles, a tenth
+of the rows with a reason and a twentieth unknown, and times cook_state_instance_stats for status running and unknown
+over a window covering every row, against numpy over a host mirror:
+  python tools/prof_state.py --instance-stats --pool c5 --reps 10
 --unscheduled loads C2 (or config-#5 pool --c5-pool with --pool c5) into a resident handle, on the grid and off it,
 and times cook_state_unscheduled for one job, 1000 jobs and every waiting job of the user with the most, against numpy
 over a host mirror, with the answers compared bit for bit:
@@ -1084,6 +1088,97 @@ def user_usage_prof(a):
             e.close()
 
 
+def host_instance_stats(m, now, unknown):
+    """numpy over a host mirror of the running rows (every handle's, with its index): cook_state_instance_stats'
+    segments [(kind, user, reason, count, totals, percentiles)] and leaders, each fold sequential in (task id, handle)
+    (np.cumsum), each percentile a nearest rank of np.sort."""
+    i = np.flatnonzero(m["unknown"] == unknown)
+    i = i[np.lexsort((m["pidx"][i], m["tid"][i]))]          # the fold order
+    rt = (now - m["start"][i]) / 1000.0
+    met = np.stack([rt, rt * m["cpus"][i], rt * m["mem"][i]])
+    ranks = lambda n: [(p * n + 99) // 100 - 1 for p in (50, 75, 95, 99, 100)]
+    out, lead = [], []
+    n = len(i)
+    for kind in range(4):
+        user = m["user"][i] if kind >= 2 else np.full(n, -1)
+        reason = m["reason"][i] if kind in (1, 2) else np.full(n, -1)
+        k = np.lexsort((np.arange(n), reason, user))
+        key = np.stack([user[k], reason[k]], 1)
+        cut = np.flatnonzero(np.any(key[1:] != key[:-1], 1)) + 1
+        for s, e in zip(np.concatenate([[0], cut]), np.concatenate([cut, [n]])):
+            seg = met[:, k[s:e]]
+            tot = [float(np.cumsum(seg[c])[-1]) for c in range(3)]
+            if kind == 3:
+                lead.append((int(key[s, 0]), tot))
+            else:
+                r = ranks(e - s)
+                out.append((kind, int(key[s, 0]), int(key[s, 1]), e - s, tot,
+                            [np.sort(seg[c])[r].tolist() for c in range(3)]))
+    lc = sorted(((u, t[1]) for u, t in lead), key=lambda x: (-x[1], x[0]))[:10]
+    lm = sorted(((u, t[2]) for u, t in lead), key=lambda x: (-x[1], x[0]))[:10]
+    return out, lc, lm
+
+
+def instance_stats_prof(a):
+    """cook_state_instance_stats over resident pools (C2, config-#5 pool --c5-pool, or --c3-group N config-#3 pools as N
+    handles) for status running and unknown over a window covering every row, against numpy over a host mirror.  A
+    tenth of the rows carry one of three reason codes, a twentieth are unknown."""
+    if a.c3_group > 0:
+        ts = [traces.gen_config_pool("c3", p) for p in range(a.c3_group)]
+        name = f"c3/0-{a.c3_group - 1}"
+    else:
+        ts = [traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)]
+        name = a.pool if a.pool == "c2" else f"c5/{a.c5_pool}"
+    rng = np.random.default_rng(a.seed)
+    es, m = [], {k: [] for k in ("user", "tid", "pidx", "start", "cpus", "mem", "reason", "unknown")}
+    for p, t in enumerate(ts):
+        r = {k: np.asarray(v).copy() for k, v in t["cols"]["running"].items()}
+        n = len(r["task_id"])
+        e = GpuEngine(pool_name=f"instance-stats-{p}")
+        e.state_apply(abi.make_delta(reset=True, running=abi.make_tasks(**r)))
+        reason = np.where(rng.random(n) < 0.1, rng.choice([1001, 1002, 2003], n), -1).astype(np.int32)
+        unknown = (rng.random(n) < 0.05).astype(np.uint8)
+        e.state_task_reason(r["task_id"], reason)
+        e.state_task_facts(r["task_id"], unknown=unknown)
+        es.append(e)
+        for k, src in (("user", r["user"]), ("tid", r["task_id"]), ("start", r["start_time"]), ("cpus", r["cpus"]),
+                       ("mem", r["mem"]), ("reason", reason), ("unknown", unknown)):
+            m[k].append(np.asarray(src))
+        m["pidx"].append(np.full(n, p))
+    m = {k: np.concatenate(v) for k, v in m.items()}
+    for k in ("cpus", "mem"):
+        m[k] = m[k].astype(np.float64)
+    now = int(m["start"].max()) + 1
+    lo, hi = int(m["start"].min()), now
+    print(json.dumps({"card": card(), "pools": name, "handles": len(ts), "running": int(len(m["tid"]))}), flush=True)
+    for status in (abi.IS_RUNNING, abi.IS_UNKNOWN):
+        for _ in range(3):   # warm-up: the carves and the first launches
+            got = engine.state_instance_stats(es, now, status, lo, hi)
+        dev, wall, host, same = [], [], [], True
+        for _ in range(a.reps):
+            w0 = time.perf_counter()
+            got = engine.state_instance_stats(es, now, status, lo, hi)
+            wall.append(time.perf_counter() - w0)
+            st = got["stats"]
+            dev.append(st["ms_h2d"] + st["ms_device"] + st["ms_d2h"])
+            w0 = time.perf_counter()
+            segs, lc, lm = host_instance_stats(m, now, status == abi.IS_UNKNOWN)
+            host.append(time.perf_counter() - w0)
+            f = lambda x: np.asarray(x, np.float64).view(np.int64).tolist()
+            same = same and len(segs) == len(got["kind"]) and all(
+                (int(got["kind"][d]), int(got["user"][d]), int(got["reason"][d]), int(got["count"][d])) == w[:4]
+                and f(got["total"][d]) == f(w[4]) and f(got["pct"][d]) == f(w[5]) for d, w in enumerate(segs)) and \
+                [(u, f([x])) for u, x in got["leaders_cpu"]] == [(u, f([x])) for u, x in lc] and \
+                [(u, f([x])) for u, x in got["leaders_mem"]] == [(u, f([x])) for u, x in lm]
+        print(json.dumps({"status": "unknown" if status == abi.IS_UNKNOWN else "running",
+                          "selected": int(got["count"][0]) if len(got["count"]) else 0, "segments": len(got["kind"]),
+                          "device_ms": round(float(np.median(dev)), 4), "wall_ms": round(1e3 * float(np.median(wall)), 4),
+                          "h2d_bytes": st["h2d_bytes"], "d2h_bytes": st["d2h_bytes"], "n_launches": st["n_launches"],
+                          "numpy_wall_ms": round(1e3 * float(np.median(host)), 4), "identical": bool(same)}), flush=True)
+    for e in es:
+        e.close()
+
+
 def rank_quota_prof(a):
     t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
     pc, rc0, users = t["cols"]["pending"], t["cols"]["running"], t["users"]
@@ -1149,7 +1244,11 @@ def main():
     ap.add_argument("--unscheduled", action="store_true", help="cook_state_unscheduled against numpy over a host mirror")
     ap.add_argument("--user-usage", action="store_true",
                     help="cook_state_user_usage against numpy over a host mirror (--c3-group N: N config-#3 pools)")
+    ap.add_argument("--instance-stats", action="store_true",
+                    help="cook_state_instance_stats against numpy over a host mirror (--c3-group N: N config-#3 pools)")
     a = ap.parse_args()
+    if a.instance_stats:
+        return instance_stats_prof(a)
     if a.user_usage:
         return user_usage_prof(a)
     if a.unscheduled:
