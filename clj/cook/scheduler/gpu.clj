@@ -15,7 +15,9 @@
 ;;   unscheduled.clj:172-200 reasons      -> (unscheduled! ...) + cycle.py's unscheduled_reasons  [cook_state_unscheduled]
 ;;   api.clj:2946-2969 get-user-usage       -> (user-usage! ...) + cycle.py's usage_response  [cook_state_user_usage]
 ;;   api.clj:3150-3232 task-stats-handler   -> (instance-stats! ...) + cycle.py's instance_stats_response, fed by
-;;                                              task-reason! [cook_state_instance_stats, cook_state_task_reason]
+;;                                              task-reason! [cook_state_instance_stats, cook_state_task_reason], and
+;;                                              for success / failed by history-seed!, finish-history! and
+;;                                              history-advance! [cook_state_history_*]
 ;; selected per pool with {:scheduler-config {:scheduler "gpu"}} next to "fenzo" / "kubernetes"
 ;; (config.clj:110-122, make-pool-handler :2425-2466).  Everything numeric happens in libcookgpu;
 ;; this namespace marshals columns and keeps the state Fenzo kept (cook_b200/cycle.py is the same
@@ -377,6 +379,36 @@
                                      (bytes-buf (map :success? done)))
           "cook_state_finish"))
 
+(defn finish-history!
+  "finish!, and while the handle's history is on, the rows that started at or after its horizon are kept as finished
+   instances for instance-stats!: [{:task-id :end-ms :success? :reason-code}], fed by the tap's terminal status datoms
+   (the status, the reason and the end time arrive in one transaction, scheduler.clj:274-292).  A :reason-code of nil
+   on every row keeps each row's reason fact (task-reason!, the previous-reason of scheduler.clj:281)."
+  [handle done]
+  (check! handle (Native/stateFinishHistory handle (count done) (longs-buf (map :task-id done))
+                                            (longs-buf (map :end-ms done)) (bytes-buf (map :success? done))
+                                            (when (some :reason-code done) (ints-buf (map #(or (:reason-code %) -1) done))))
+          "cook_state_finish_history"))
+
+(defn history-seed!
+  "At start-up and on a leadership change, after the reset and the load and before the tap resumes: the finished
+   instances of the pool with start >= since-ms, read once from Datomic, [{:task-id :user :start-ms :end-ms :cpus :mem
+   :success? :reason-code}].  Turns the history on at horizon since-ms."
+  [handle since-ms rows]
+  (check! handle (Native/stateHistorySeed handle (long since-ms) (count rows)
+                                          (object-array [(i64-col (map :task-id rows)) (i32-col (map :user rows))
+                                                         (i64-col (map :start-ms rows)) (i64-col (map :end-ms rows))
+                                                         (f64-col (map :cpus rows)) (f64-col (map :mem rows))
+                                                         (u8-col (map :success? rows))
+                                                         (i32-col (map #(or (:reason-code %) -1) rows))]))
+          "cook_state_history_seed"))
+
+(defn history-advance!
+  "Periodically, with now - retention (the shim's setting, default 32 days: every window task-stats-handler accepts
+   that ends by now): the horizon rises and the rows that started before it leave."
+  [handle since-ms]
+  (check! handle (Native/stateHistoryAdvance handle (long since-ms)) "cook_state_history_advance"))
+
 (defn group-runtimes!
   "After a reset or a leadership change: the successes of the tracked groups' jobs that finished before their rows
    were resident, [[group-code runtime-seconds]], and the group codes no longer tracked."
@@ -465,13 +497,17 @@
 
 ;; ---------------------------------------------------------------------------------------------
 ;; /stats/instances over resident pools: the device half of task-stats/get-stats (task_stats.clj), for status running
-;; or unknown without a name filter; the handler keeps the Datomic path for success, failed and a name filter, and
-;; for pools on several devices (percentiles do not compose from per-device summaries)
+;; or unknown (the running rows) and success or failed (the finished-instance histories) without a name filter; the
+;; handler keeps the Datomic path for a name filter, for pools on several devices (percentiles do not compose from
+;; per-device summaries) and for a window that starts before a history's horizon
 (def ^:private instance-stats-leaders 10)
 (defn instance-stats!
-  "Instance stats over `handles` (one device): `status` :running or :unknown, the window [start-ms, end-ms), the
-   entity-id bounds [task-id-lo, task-id-hi) (d/entid-at of start - 1 h and end + 1 h), one `now-ms`.  `n-rows` is the
-   live running rows over the handles (the shim's count).  Returns {:segments [{:kind 0|1|2 (overall, reason, user and
+  "Instance stats over `handles` (one device): `status` :running or :unknown (the live running rows, one `now-ms`) or
+   :success or :failed (the handles' histories, history-seed!; now-ms unused), the window [start-ms, end-ms), the
+   entity-id bounds [task-id-lo, task-id-hi) (d/entid-at of start - 1 h and end + 1 h).  `n-rows` sizes the segments:
+   the live running rows over the handles (the shim's count); for a history, a capacity the call may refuse with the
+   count it needs (cook_state_history_stats' COOK_E_TOO_LARGE), and the handler retries with that count.  A name
+   filter, pools on several devices, or a window before a history's horizon keep the Datomic path.  Returns {:segments [{:kind 0|1|2 (overall, reason, user and
    reason) :user :reason (-1: none) :count :totals [run cpu mem] :percentiles [[p50 p75 p95 p99 p100] x3]}]
    :leaders-cpu [[user total]] :leaders-mem [[user total]]}; the handler builds the response (user names, reason
    strings, the nil reason's key) as cook_b200/cycle.py's instance_stats_response does."
@@ -483,7 +519,8 @@
         out-n (int-array 2)]
     (check! (first handles)
             (Native/stateInstanceStats (long-array handles) (long-array [now-ms start-ms end-ms task-id-lo task-id-hi])
-                                       (if (= status :unknown) 1 0) (int cap) (object-array segs)
+                                       (case status :running 0 :unknown 1 :success 2 :failed 3) (int cap)
+                                       (object-array segs)
                                        (object-array leaders) out-n nil)
             "cook_state_instance_stats")
     (let [i32 (fn [^ByteBuffer b d] (.getInt b (int (* 4 d))))

@@ -156,8 +156,9 @@ OFFER_USED, OFFER_EXPIRED, OFFER_SINGLE_SHOT = 1, 2, 3
 UNSCHED_ABSENT, UNSCHED_WAITING, UNSCHED_RUNNING, UNSCHED_AHEAD = 0, 1, 2, 10
 # cook_state_user_usage: a segment's group when it is the scope's total, or its jobs without a group
 UU_TOTAL, UU_UNGROUPED = -2, -1
-# cook_state_instance_stats: the statuses, the segment kinds, the metrics and the leaders' places
-IS_RUNNING, IS_UNKNOWN = 0, 1
+# cook_state_instance_stats (running, unknown) and cook_state_history_stats (success, failed): the statuses, the
+# segment kinds, the metrics and the leaders' places
+IS_RUNNING, IS_UNKNOWN, IS_SUCCESS, IS_FAILED = 0, 1, 2, 3
 IS_OVERALL, IS_REASON, IS_USER_REASON = 0, 1, 2
 IS_RUN_TIME, IS_CPU, IS_MEM, IS_LEADERS = 0, 1, 2, 10
 
@@ -340,6 +341,9 @@ ARGTYPES = {
     "cook_state_task_facts": [_H, _I32, P_I64, P_I64, P_U8, P_U8],
     "cook_state_task_reason": [_H, _I32, P_I64, P_I32],
     "cook_state_finish": [_H, _I32, P_I64, P_I64, P_U8],
+    "cook_state_finish_history": [_H, _I32, P_I64, P_I64, P_U8, P_I32],
+    "cook_state_history_seed": [_H, C.c_int64, _I32, P_I64, P_I32, P_I64, P_I64, P_F64, P_F64, P_U8, P_I32],
+    "cook_state_history_advance": [_H, C.c_int64],
     "cook_state_group_runtimes": [_H, _I32, P_I32, P_I32, _I32, P_I32],
     "cook_state_sweep": [_P(_H), _I32, C.c_int64, C.c_int64, C.c_int64, _I32, P_I32, P_F64, P_F64, P_I32, _I32, P_I64,
                          P_I32, P_I32, P_I64, P_I32, P_I32, _I32, P_I32, P_I64, P_I32, P_I32, _P(PhaseStats)],
@@ -348,6 +352,8 @@ ARGTYPES = {
                               P_F64, P_I32, _I32, P_I64, P_I32, P_I32, _P(PhaseStats)],
     "cook_state_instance_stats": [_P(_H), _I32, C.c_int64, _I32, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _I32,
                                   P_I32, P_I32, P_I32, P_I64, P_F64, P_F64, P_I32, P_F64, P_I32, P_I32, _P(PhaseStats)],
+    "cook_state_history_stats": [_P(_H), _I32, _I32, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _I32, P_I32, P_I32,
+                                 P_I32, P_I64, P_F64, P_F64, P_I32, P_F64, P_I32, P_I32, _P(PhaseStats)],
     "cook_last_stats": [_H, _I32, _P(PhaseStats)],
     "cook_allgather_usage": [_H, _H, P_F64, P_F64, C.c_int64],
     "cook_comm_unique_id": [P_U8],

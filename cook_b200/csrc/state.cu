@@ -24,6 +24,7 @@
 // Considerable jobs without a match: the live queue entries with their queue positions, their M0 columns gathered,
 // cook_match's considerable pass (match.cu) run on them; a consuming call retires the taken entries' generations.
 #include <algorithm>
+#include <cmath>
 #include <map>
 #include <unordered_map>
 #include <unordered_set>
@@ -694,6 +695,59 @@ struct Records {
   void release() { free_all(); cap = tail = n_live = 0; }
 };
 
+// The finished instances (cook_state_history_*): 49 B per row in arrival order, dense in [0, tail); rows leave only by
+// a stable compaction (cook_state_history_advance).  Off until seeded; `since` is the horizon on start time.
+struct HistCols {
+  int64_t* tid = nullptr; int64_t* start = nullptr; int64_t* end = nullptr; double* cpus = nullptr; double* mem = nullptr;
+  int32_t* user = nullptr; int32_t* reason = nullptr; uint8_t* ok = nullptr;
+  cudaError_t alloc(int64_t n) {
+    cudaError_t e = cudaSuccess;
+    for (void** p : {(void**)&tid, (void**)&start, (void**)&end, (void**)&cpus, (void**)&mem})
+      if (e == cudaSuccess) e = cudaMalloc(p, 8 * n);
+    for (void** p : {(void**)&user, (void**)&reason}) if (e == cudaSuccess) e = cudaMalloc(p, 4 * n);
+    if (e == cudaSuccess) e = cudaMalloc(&ok, n);
+    if (e != cudaSuccess) free_all();
+    return e;
+  }
+  void free_all() {
+    for (void* p : {(void*)tid, (void*)start, (void*)end, (void*)cpus, (void*)mem, (void*)user, (void*)reason, (void*)ok})
+      if (p) cudaFree(p);
+    *this = HistCols{};
+  }
+};
+struct History {
+  HistCols c;
+  int64_t cap = 0, tail = 0, since = 0;
+  bool on = false;
+  // capacity >= n: new columns holding the first `tail` rows (device to device)
+  cudaError_t grow(int64_t n, cudaStream_t st) {
+    if (n <= cap) return cudaSuccess;
+    const int64_t ncap = std::max<int64_t>(n, std::max<int64_t>(2 * cap, 4096));
+    HistCols nc;
+    cudaError_t e = nc.alloc(ncap);
+    if (e == cudaSuccess && tail) e = copy_rows(nc, c, tail, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { nc.free_all(); return e; }
+    c.free_all();
+    c = nc;
+    cap = ncap;
+    return cudaSuccess;
+  }
+  static cudaError_t copy_rows(const HistCols& d, const HistCols& s, int64_t n, cudaStream_t st) {
+    const cudaMemcpyKind k = cudaMemcpyDeviceToDevice;
+    cudaError_t e = cudaMemcpyAsync(d.tid, s.tid, 8 * n, k, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d.start, s.start, 8 * n, k, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d.end, s.end, 8 * n, k, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d.cpus, s.cpus, 8 * n, k, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d.mem, s.mem, 8 * n, k, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d.user, s.user, 4 * n, k, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d.reason, s.reason, 4 * n, k, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d.ok, s.ok, n, k, st);
+    return e;
+  }
+  void release() { c.free_all(); cap = tail = since = 0; on = false; }
+};
+
 void count_add(std::map<int32_t, int64_t>& m, int32_t code, int64_t d) {
   auto it = m.emplace(code, 0).first;
   if ((it->second += d) == 0) m.erase(it);
@@ -737,6 +791,7 @@ struct PoolState {
   int64_t grp_rows = 0;                        // live running rows with a group list
   Records rec;                                 // the successful runtimes per group
   std::map<int32_t, int64_t> rec_groups;       // group code -> live records
+  History hist;                                // the finished instances
   ListArena lists[L_N];
   ListArena olists[OL_N];
   std::map<int32_t, int64_t> users_p, users_r, attr_cols, groups;   // code -> live uses
@@ -770,7 +825,7 @@ struct PoolState {
     olists[OL_GPU].esz1 = olists[OL_DISK].esz1 = 8;
   }
   void release() {
-    pend.release(); run.release(); offer.release(); rec.release();
+    pend.release(); run.release(); offer.release(); rec.release(); hist.release();
     for (auto& l : lists) l.release();
     for (auto& l : olists) l.release();
     stage.release(); scratch.release(); derive.release(); queue.release(); omerge.release();
@@ -1002,6 +1057,8 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
     S->cot_rows = S->cot_n = S->grp_rows = 0;
     S->rec.tail = S->rec.n_live = 0;
     S->rec_groups.clear();
+    S->hist.tail = S->hist.since = 0;
+    S->hist.on = false;
     S->reserved.clear();
     for (auto& f : S->nflag) f = 0;
     for (auto& l : S->lists) l.tail = l.live = 0;
@@ -2928,6 +2985,26 @@ __global__ void finish_records_kernel(OrderScan<int, 1> os, const int32_t* slot,
   }
 }
 
+// the history's append: finished row p whose running row starts at or after the horizon goes, in batch order, to the
+// table's tail; user, start, cpus and mem from the running row, the reason from the batch or else the row's fact
+struct HistAppend {
+  const int32_t* slot; const int64_t* end; const uint8_t* ok; const int32_t* reason; void* const* rc; int64_t since;
+  HistCols h; int64_t tail;
+  __device__ bool keep(int p) const { return static_cast<const int64_t*>(rc[R_START])[slot[p]] >= since; }
+  __device__ void emit(int p, int d) const {
+    const int s = slot[p];
+    const int64_t t = tail + d;
+    h.tid[t] = static_cast<const int64_t*>(rc[R_TID])[s];
+    h.user[t] = static_cast<const int32_t*>(rc[R_USER])[s];
+    h.start[t] = static_cast<const int64_t*>(rc[R_START])[s];
+    h.end[t] = end[p];
+    h.cpus[t] = static_cast<const double*>(rc[R_CPUS])[s];
+    h.mem[t] = static_cast<const double*>(rc[R_MEM])[s];
+    h.reason[t] = reason ? reason[p] : static_cast<const int32_t*>(rc[R_REASON])[s];
+    h.ok[t] = ok[p] ? 1 : 0;
+  }
+};
+
 // thread per record: a live record of a group in forget[0, n) (ascending) leaves
 __global__ void forget_records_kernel(const int32_t* grp, uint8_t* live, int n_rec, const int32_t* forget, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -3050,15 +3127,29 @@ int32_t task_reason(cook_pool* pool, PoolState* S, int n, const int64_t* task_id
   return COOK_OK;
 }
 
-// running_rm_task_id = task_id, plus one record per group of each successful row
+// What cook_state_finish_history adds to cook_state_finish: the rows' reason codes (NULL: each row's reason fact).
+struct FinishHistory { const int32_t* reason_code; };
+
+// running_rm_task_id = task_id, plus one record per group of each successful row; with `fh`, the rows that start at
+// or after the horizon of an enabled history are also appended to it
 int32_t finish(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, const int64_t* end_time_ms,
-               const uint8_t* success) {
-  const char* who = "cook_state_finish";
+               const uint8_t* success, const FinishHistory* fh = nullptr) {
+  const char* who = fh ? "cook_state_finish_history" : "cook_state_finish";
   if (n < 0) return set_err(pool, COOK_E_BADARG, "%s: n < 0", who);
   if (n && !task_id) return set_err(pool, COOK_E_BADARG, "%s: null task_id", who);
   if (n && success && !end_time_ms) return set_err(pool, COOK_E_BADARG, "%s: success without end_time_ms", who);
+  if (fh && n && (!end_time_ms || !success)) return set_err(pool, COOK_E_BADARG, "%s: null end_time_ms or success", who);
+  if (fh && !idx_in_range(fh->reason_code, n, -1, INT32_MAX))
+    return set_err(pool, COOK_E_BADARG, "%s: a reason code below -1", who);
   std::vector<int32_t> slot;
   if (const char* why = running_slots(S, n, task_id, &slot)) return set_err(pool, COOK_E_BADARG, "%s: %s", who, why);
+  History& H = S->hist;
+  int64_t nhist = 0;   // the rows the history appends
+  for (int i = 0; fh && i < n; i++) {
+    if (end_time_ms[i] < S->rstart[slot[i]]) return set_err(pool, COOK_E_BADARG, "%s: a row that ends before its start", who);
+    if (H.on && S->rstart[slot[i]] >= H.since) nhist++;
+  }
+  if (H.tail + nhist > INT32_MAX) return set_err(pool, COOK_E_TOO_LARGE, "%s: more than 2^31 - 1 history rows", who);
   int64_t nrec = 0;   // the records the successful rows append
   for (int i = 0; success && i < n; i++) {
     if (!success[i]) continue;
@@ -3086,10 +3177,15 @@ int32_t finish(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, con
   CK(pool, RC.grow(RC.tail + nrec, st));
   RC.tail += nrec;
   RC.n_live += nrec;
+  const int64_t htail = H.tail;
+  if (nhist) CK(pool, H.grow(H.tail + nhist, st));
+  H.tail += nhist;
   const int32_t rgtail = (int32_t)S->lists[L_RGROUP].tail;
   const int32_t* d_slot = nullptr;
   const uint8_t* d_ok = nullptr;
   const int64_t* d_end = nullptr;
+  const int32_t* d_reason = nullptr;
+  int32_t* hblk = nullptr;
   OrderScan<int, 1> os;
   int64_t h2d = 0;
   CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
@@ -3100,6 +3196,10 @@ int32_t finish(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, con
       os.part[0] = c.take<int32_t>(n);
       os.tile[0] = c.take<int32_t>((n + OS_TILE - 1) / OS_TILE + 1);
     }
+    if (nhist) {
+      d_reason = c.up(fh->reason_code, n);
+      hblk = c.take<int32_t>((size_t)n / CP_BLOCK + 2);
+    }
   }));
   CK(pool, cudaEventRecord(pool->ev[21], st));
   int nl = 0;
@@ -3109,6 +3209,9 @@ int32_t finish(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, con
                                                        S->lists[L_RGROUP].v[0], RC.grp, RC.rt, RC.live, rtail);
     nl++;
   }
+  if (nhist)   // read from the running rows before the removal
+    compact(HistAppend{d_slot, d_end, d_ok, d_reason, S->run.d_col, H.since, H.c, htail}, n, nullptr, hblk,
+            S->counters + 7, (int)nhist, st, &nl);
   if (n) {
     ScatterArgs rr;
     memset(&rr, 0, sizeof(rr));
@@ -3122,6 +3225,98 @@ int32_t finish(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, con
   CK(pool, cudaEventRecord(pool->ev[22], st));
   CK(pool, cudaStreamSynchronize(st));
   record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
+  return COOK_OK;
+}
+
+bool bad_amount(double x) { return !std::isfinite(x) || x < 0 || std::signbit(x); }
+
+// the history replaced by n rows at horizon since_ms, and on; the rows are copied straight into the table's columns
+int32_t history_seed(cook_pool* pool, PoolState* S, int64_t since_ms, int n, const int64_t* task_id,
+                     const int32_t* user, const int64_t* start_ms, const int64_t* end_ms, const double* cpus,
+                     const double* mem, const uint8_t* success, const int32_t* reason_code) {
+  const char* who = "cook_state_history_seed";
+  if (n < 0) return set_err(pool, COOK_E_BADARG, "%s: n < 0", who);
+  if (n && (!task_id || !user || !start_ms || !end_ms || !cpus || !mem || !success || !reason_code))
+    return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
+  if (!idx_in_range(user, n, 0, INT32_MAX)) return set_err(pool, COOK_E_BADARG, "%s: a negative user code", who);
+  if (!idx_in_range(reason_code, n, -1, INT32_MAX)) return set_err(pool, COOK_E_BADARG, "%s: a reason code below -1", who);
+  std::unordered_set<int64_t> seen;
+  seen.reserve((size_t)n);
+  for (int i = 0; i < n; i++) {
+    if (start_ms[i] < since_ms) return set_err(pool, COOK_E_BADARG, "%s: a row that starts before since_ms", who);
+    if (end_ms[i] < start_ms[i]) return set_err(pool, COOK_E_BADARG, "%s: a row that ends before its start", who);
+    if (bad_amount(cpus[i]) || bad_amount(mem[i]))
+      return set_err(pool, COOK_E_BADARG, "%s: cpus or mem negative, -0.0 or not finite", who);
+    if (!seen.insert(task_id[i]).second) return set_err(pool, COOK_E_BADARG, "%s: task id twice", who);
+    if (S->run.slot_of.count(task_id[i])) return set_err(pool, COOK_E_BADARG, "%s: a live running task id", who);
+  }
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  History& H = S->hist;
+  H.tail = 0;
+  H.since = since_ms;
+  H.on = true;
+  CK(pool, H.grow(n, st));
+  H.tail = n;
+  // straight into the table's columns: no staging buffer
+  CK(pool, cudaEventRecord(pool->ev[20], st));
+  Carve c;   // only its copy(): the bytes counted, the first error kept
+  c.st = st;
+  if (n) {
+    c.copy(H.c.tid, task_id, n); c.copy(H.c.user, user, n); c.copy(H.c.start, start_ms, n); c.copy(H.c.end, end_ms, n);
+    c.copy(H.c.cpus, cpus, n); c.copy(H.c.mem, mem, n); c.copy(H.c.ok, success, n); c.copy(H.c.reason, reason_code, n);
+  }
+  CK(pool, c.err);
+  const int64_t h2d = c.h2d;
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  CK(pool, cudaStreamSynchronize(st));
+  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, 0);
+  return COOK_OK;
+}
+
+struct HistKeep {   // the advance's compaction: the rows that start at or after the new horizon, in order
+  HistCols s, d; int64_t since;
+  __device__ bool keep(int i) const { return s.start[i] >= since; }
+  __device__ void emit(int i, int k) const {
+    d.tid[k] = s.tid[i]; d.user[k] = s.user[i]; d.start[k] = s.start[i]; d.end[k] = s.end[i];
+    d.cpus[k] = s.cpus[i]; d.mem[k] = s.mem[i]; d.reason[k] = s.reason[i]; d.ok[k] = s.ok[i];
+  }
+};
+
+// the horizon raised to since_ms: the rows that start before it leave in one compaction into new columns
+int32_t history_advance(cook_pool* pool, PoolState* S, int64_t since_ms) {
+  const char* who = "cook_state_history_advance";
+  History& H = S->hist;
+  if (!H.on) return set_err(pool, COOK_E_BADARG, "%s: history is off", who);
+  if (since_ms < H.since) return set_err(pool, COOK_E_BADARG, "%s: since_ms below the horizon", who);
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  int32_t* blk = nullptr;
+  const int T = (int)H.tail;
+  CK(pool, carve(S->scratch, st, pool->ev[20], nullptr, [&](Carve& c) {
+    if (T && since_ms > H.since) blk = c.take<int32_t>((size_t)T / CP_BLOCK + 2);
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  int nl = 0;
+  int64_t d2h = 0;
+  if (T && since_ms > H.since) {
+    HistCols nc;
+    CK(pool, nc.alloc(H.cap));
+    compact(HistKeep{H.c, nc, since_ms}, T, nullptr, blk, S->counters + 7, T, st, &nl);
+    int32_t kept = 0;
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = download(&kept, S->counters + 7, 1, st, &d2h);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { nc.free_all(); CK(pool, e); }
+    H.c.free_all();
+    H.c = nc;
+    H.tail = kept;
+  }
+  H.since = since_ms;
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  CK(pool, cudaStreamSynchronize(st));
+  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], 0, d2h, nl);
   return COOK_OK;
 }
 
@@ -3493,6 +3688,36 @@ extern "C" int32_t cook_state_finish(cook_pool* pool, int32_t n, const int64_t* 
   PoolState* S = state_of(pool, true);
   if (!S) return set_err(pool, COOK_E_OOM, "cook_state_finish: out of device memory");
   return finish(pool, S, n, task_id, end_time_ms, success);
+}
+
+extern "C" int32_t cook_state_finish_history(cook_pool* pool, int32_t n, const int64_t* task_id,
+                                             const int64_t* end_time_ms, const uint8_t* success,
+                                             const int32_t* reason_code) {
+  if (!pool) return COOK_E_BADARG;
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_finish_history: out of device memory");
+  const FinishHistory fh{reason_code};
+  return finish(pool, S, n, task_id, end_time_ms, success, &fh);
+}
+
+extern "C" int32_t cook_state_history_seed(cook_pool* pool, int64_t since_ms, int32_t n, const int64_t* task_id,
+                                           const int32_t* user, const int64_t* start_ms, const int64_t* end_ms,
+                                           const double* cpus, const double* mem, const uint8_t* success,
+                                           const int32_t* reason_code) {
+  if (!pool) return COOK_E_BADARG;
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_history_seed: out of device memory");
+  return history_seed(pool, S, since_ms, n, task_id, user, start_ms, end_ms, cpus, mem, success, reason_code);
+}
+
+extern "C" int32_t cook_state_history_advance(cook_pool* pool, int64_t since_ms) {
+  if (!pool) return COOK_E_BADARG;
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_history_advance: out of device memory");
+  return history_advance(pool, S, since_ms);
 }
 
 extern "C" int32_t cook_state_group_runtimes(cook_pool* pool, int32_t n_add, const int32_t* group,
@@ -4135,10 +4360,13 @@ extern "C" int32_t cook_state_user_usage(cook_pool* const* pools, int32_t n_pool
 // ---- instance stats (/stats/instances, task-stats/get-stats task_stats.clj): over the selected live running rows,
 // per segment (overall, per reason, per (user, reason)) the count, and per metric (run-time, cpu and mem seconds)
 // the left fold and the nearest-rank percentiles 50 75 95 99 100; and the ten users with the largest cpu and mem
-// totals.  The live rows of every handle are compacted into one range, the selection compacted from it with the
-// three metrics, then each selected row becomes one entry per level (overall, reason, (user, reason), user).  One
-// sort by (segment, task id, pool index) gives every segment's fold order; per metric, one sort of the first three
-// levels by (segment, value) gives the ranks.  The user level's folds feed the leaders and are not returned.
+// totals.  Two sources: the live running rows (cook_state_instance_stats: the live rows of every handle compacted
+// into one range, the selection compacted from it with the metrics at one now) and the finished rows
+// (cook_state_history_stats: the selection compacted straight from each handle's history table with end - start).
+// From the selected rows on, one pipeline (is_answer): each selected row becomes one entry per level (overall, reason,
+// (user, reason), user).  One sort by (segment, task id, pool index, table position) gives every segment's fold
+// order; per metric, one sort of the first three levels by (segment, value) gives the ranks.  The user level's folds
+// feed the leaders and are not returned.
 namespace {
 
 constexpr int IS_LEVELS = 4, IS_USER = 3;   // the levels' kinds: COOK_IS_OVERALL, _REASON, _USER_REASON, then users
@@ -4205,15 +4433,17 @@ __global__ void is_expand_kernel(int S, const int32_t* user, const int32_t* reas
   k.reason[x] = l == COOK_IS_REASON || l == COOK_IS_USER_REASON ? reason[i] : -1;
   row[x] = i;
 }
-// (segment, task id, pool index, entry): the segments in the output order, each in its fold order
+// (segment, task id, pool index, table position when given, entry): the segments in the output order, each in its
+// fold order
 struct LessSegTidPool {
-  ISKey k; const int32_t* row; const int64_t* tid; const int32_t* pidx;
+  ISKey k; const int32_t* row; const int64_t* tid; const int32_t* pidx; const int32_t* pos;
   __device__ bool operator()(int32_t a, int32_t b) const {
     const int c = k.cmp(a, b);
     if (c) return c < 0;
     const int ra = row[a], rb = row[b];
     if (tid[ra] != tid[rb]) return tid[ra] < tid[rb];
     if (pidx[ra] != pidx[rb]) return pidx[ra] < pidx[rb];
+    if (pos && pos[ra] != pos[rb]) return pos[ra] < pos[rb];
     return a < b;
   }
 };
@@ -4346,13 +4576,17 @@ __global__ void __launch_bounds__(256) is_leaders_kernel(const int32_t* n_seg, c
   }
 }
 
-int32_t instance_stats(cook_pool* const* pools, int n, int64_t now, int32_t status, int64_t start_ms, int64_t end_ms,
-                       int64_t tid_lo, int64_t tid_hi, int32_t seg_cap, int32_t* o_kind, int32_t* o_user,
-                       int32_t* o_reason, int64_t* o_count, double* o_total, double* o_pct, int32_t* o_lead_user,
-                       double* o_lead_total, int32_t* o_nseg, int32_t* o_nlead, cook_phase_stats* out_stats) {
-  const char* who = "cook_state_instance_stats";
-  // ---- every check before any device work or output
-  if (!pools || n <= 0 || !pools[0]) return COOK_E_BADARG;
+// The answer's outputs (cook_state_instance_stats' and cook_state_history_stats' out_* arguments).
+struct ISOut {
+  int32_t *kind, *user, *reason; int64_t* count; double *total, *pct; int32_t* lead_user; double* lead_total;
+  int32_t *n_seg, *n_lead;
+};
+bool is_out_null(const ISOut& o) {
+  return !o.kind || !o.user || !o.reason || !o.count || !o.total || !o.pct || !o.lead_user || !o.lead_total ||
+         !o.n_seg || !o.n_lead;
+}
+// cook_state_user_stats' handle rules: non-NULL, distinct, one device
+int32_t is_handles(cook_pool* const* pools, int n, const char* who) {
   cook_pool* pool = pools[0];
   for (int k = 0; k < n; k++) {
     if (!pools[k]) return set_err(pool, COOK_E_BADARG, "%s: a NULL handle", who);
@@ -4360,11 +4594,123 @@ int32_t instance_stats(cook_pool* const* pools, int n, int64_t now, int32_t stat
       return set_err(pool, COOK_E_BADARG, "%s: a handle listed twice", who);
     if (pools[k]->device != pool->device) return set_err(pool, COOK_E_BADARG, "%s: handles on different devices", who);
   }
+  return COOK_OK;
+}
+
+// The selected rows with their metrics, and the pipeline's device buffers, carved by take() for at most Smax rows.
+// cnt: [0] selected, [1] the source's flag, [2] segments, [3] returned segments, [4] leaders, [5] the compactions' own.
+struct ISPipe {
+  int32_t *cnt = nullptr, *blk = nullptr;
+  int32_t *s_user = nullptr, *s_reason = nullptr, *s_pidx = nullptr, *s_pos = nullptr;
+  int64_t* s_tid = nullptr;
+  double* met[3] = {};
+  GridFlag* gf = nullptr;
+  ISKey key = {};
+  int32_t *row = nullptr, *ord = nullptr, *tmp = nullptr, *end = nullptr, *vord[3] = {}, *l_user = nullptr;
+  double *pct = nullptr, *l_total = nullptr;
+  ISFoldArgs a = {};
+  // blk_n: the most items any compaction of the call runs over; pos: the selection carries table positions
+  void take(Carve& c, int Smax, int blk_n, bool pos) {
+    const int Emax = IS_LEVELS * Smax;
+    blk_n = std::max(blk_n, Emax);
+    cnt = c.take<int32_t>(6);
+    blk = c.take<int32_t>((size_t)blk_n / CP_BLOCK + 2);
+    s_user = c.take<int32_t>(Smax); s_reason = c.take<int32_t>(Smax); s_pidx = c.take<int32_t>(Smax);
+    if (pos) s_pos = c.take<int32_t>(Smax);
+    s_tid = c.take<int64_t>(Smax);
+    for (int k = 0; k < 3; k++) met[k] = c.take<double>(Smax);
+    gf = c.take<GridFlag>(1);
+    key.kind = c.take<int32_t>(Emax); key.user = c.take<int32_t>(Emax); key.reason = c.take<int32_t>(Emax);
+    row = c.take<int32_t>(Emax); ord = c.take<int32_t>(Emax); tmp = c.take<int32_t>(Emax); end = c.take<int32_t>(Emax);
+    for (int k = 0; k < 3; k++) vord[k] = c.take<int32_t>(Emax);
+    for (int k = 0; k < 3; k++) {
+      a.os.part[k] = c.take<double>(Emax);
+      a.os.tile[k] = c.take<double>(Emax / OS_TILE + 2);
+    }
+    a.o_kind = c.take<int32_t>(Emax); a.o_user = c.take<int32_t>(Emax); a.o_reason = c.take<int32_t>(Emax);
+    a.o_count = c.take<int64_t>(Emax); a.o_total = c.take<double>(3 * (size_t)Emax);
+    pct = c.take<double>(15 * (size_t)Emax);
+    l_user = c.take<int32_t>(2 * COOK_IS_LEADERS); l_total = c.take<double>(2 * COOK_IS_LEADERS);
+  }
+  cudaError_t clear(cudaStream_t st) const {
+    cudaError_t e = cudaMemsetAsync(cnt, 0, sizeof(int32_t) * 6, st);
+    return e == cudaSuccess ? cudaMemsetAsync(gf, 0, sizeof(GridFlag), st) : e;
+  }
+};
+
+// From S selected rows on: the entries, the fold order and its segments, the folds, the ranks and the leaders; then
+// ev[22], the downloads and ev[23].  More segments than seg_cap: only *o.n_seg is written, COOK_E_TOO_LARGE.
+int32_t is_answer(cook_pool* pool, cudaStream_t st, ISPipe& p, int S, int32_t seg_cap, const ISOut& o, int* nl,
+                  int64_t* d2h) {
+  const int E = IS_LEVELS * S, E3 = 3 * S;
+  int32_t got[2] = {0, 0};
+  ISFoldArgs& a = p.a;
+  if (S > 0) {
+    // ---- the entries, the fold order and its segments, the folds
+    grid_check_kernel<<<(S + 255) / 256, 256, 0, st>>>(p.met[0], p.met[1], p.met[2], S, p.gf);
+    is_expand_kernel<<<(E + 255) / 256, 256, 0, st>>>(S, p.s_user, p.s_reason, p.key, p.row);
+    *nl += 2;
+    CK(pool, csort::sort_indices(p.ord, p.tmp, E, LessSegTidPool{p.key, p.row, p.s_tid, p.s_pidx, p.s_pos}, st, nl));
+    compact(ISSegEnds{p.ord, p.key, E, p.end}, E, nullptr, p.blk, p.cnt + 2, E, st, nl);
+    order_scan(a.os, ISLoad{p.ord, p.row, {p.met[0], p.met[1], p.met[2]}}, E, p.gf, st, nl);
+    a.ord = p.ord; a.row = p.row; a.k = p.key;
+    for (int k = 0; k < 3; k++) a.met[k] = p.met[k];
+    a.end = p.end; a.n_seg = p.cnt + 2; a.gf = p.gf; a.E = E;
+    is_fold_kernel<<<std::min((E + 3) / 4, 4096), 128, 0, st>>>(a);
+    (*nl)++;
+    // ---- the ranks: the three levels returned are entries [0, 3 S), whose segments lead the fold order's
+    for (int k = 0; k < 3; k++)
+      CK(pool, csort::sort_indices(p.vord[k], p.tmp, E3, LessSegValue{p.key, p.row, p.met[k]}, st, nl));
+    is_pct_kernel<<<std::min((3 * E + 255) / 256, 4096), 256, 0, st>>>(p.cnt + 2, p.end, a.o_kind, p.vord[0], p.vord[1],
+                                                                      p.vord[2], p.row, p.met[0], p.met[1], p.met[2],
+                                                                      p.pct);
+    is_leaders_kernel<<<2, 256, 0, st>>>(p.cnt + 2, a.o_kind, a.o_user, a.o_total, p.l_user, p.l_total, p.cnt + 3);
+    *nl += 2;
+    CK(pool, cudaGetLastError());
+    CK(pool, download(got, p.cnt + 3, 2, st, d2h));
+    CK(pool, cudaStreamSynchronize(st));
+  }
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  const int ns = got[0], nlead = got[1];
+  if (ns > seg_cap) {
+    *o.n_seg = ns;
+    return set_err(pool, COOK_E_TOO_LARGE, "more segments than seg_cap: %d", ns);
+  }
+  if (ns) {
+    CK(pool, download(o.kind, a.o_kind, ns, st, d2h));
+    CK(pool, download(o.user, a.o_user, ns, st, d2h));
+    CK(pool, download(o.reason, a.o_reason, ns, st, d2h));
+    CK(pool, download(o.count, a.o_count, ns, st, d2h));
+    CK(pool, download(o.total, a.o_total, 3 * (size_t)ns, st, d2h));
+    CK(pool, download(o.pct, p.pct, 15 * (size_t)ns, st, d2h));
+  }
+  for (int k = 0; k < 2 && nlead; k++) {
+    CK(pool, download(o.lead_user + k * COOK_IS_LEADERS, p.l_user + k * COOK_IS_LEADERS, nlead, st, d2h));
+    CK(pool, download(o.lead_total + k * COOK_IS_LEADERS, p.l_total + k * COOK_IS_LEADERS, nlead, st, d2h));
+  }
+  CK(pool, cudaEventRecord(pool->ev[23], st));
+  CK(pool, cudaStreamSynchronize(st));
+  *o.n_seg = ns;
+  *o.n_lead = nlead;
+  return COOK_OK;
+}
+
+void is_empty(const ISOut& o, cook_phase_stats* out_stats) {
+  *o.n_seg = 0;
+  *o.n_lead = 0;
+  if (out_stats) *out_stats = cook_phase_stats{};
+}
+
+int32_t instance_stats(cook_pool* const* pools, int n, int64_t now, int32_t status, int64_t start_ms, int64_t end_ms,
+                       int64_t tid_lo, int64_t tid_hi, int32_t seg_cap, const ISOut& o, cook_phase_stats* out_stats) {
+  const char* who = "cook_state_instance_stats";
+  // ---- every check before any device work or output
+  if (!pools || n <= 0 || !pools[0]) return COOK_E_BADARG;
+  cook_pool* pool = pools[0];
+  if (int32_t rc = is_handles(pools, n, who)) return rc;
   if (status != COOK_IS_RUNNING && status != COOK_IS_UNKNOWN) return set_err(pool, COOK_E_BADARG, "%s: an unknown status", who);
   if (end_ms <= start_ms) return set_err(pool, COOK_E_BADARG, "%s: end_ms <= start_ms", who);
-  if (!o_kind || !o_user || !o_reason || !o_count || !o_total || !o_pct || !o_lead_user || !o_lead_total || !o_nseg ||
-      !o_nlead)
-    return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
+  if (is_out_null(o)) return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
   // the handles with rows and their pool index; sizes from the host-side counts
   std::vector<std::pair<const PoolState*, int32_t>> hs;
   int64_t R = 0;
@@ -4379,55 +4725,29 @@ int32_t instance_stats(cook_pool* const* pools, int n, int64_t now, int32_t stat
   if (R * IS_LEVELS > INT32_MAX) return set_err(pool, COOK_E_TOO_LARGE, "%s: more than 2^31 - 1 entries", who);
   if (seg_cap < 1 + 2 * R) return set_err(pool, COOK_E_BADARG, "%s: seg_cap below 1 + 2 * the live running rows", who);
   if (R == 0) {   // no row to read: empty results without device work
-    *o_nseg = 0;
-    *o_nlead = 0;
-    if (out_stats) *out_stats = cook_phase_stats{};
+    is_empty(o, out_stats);
     return COOK_OK;
   }
   CK(pool, cudaSetDevice(pool->device));
   PoolState* S0 = state_of(pool, true);   // pools[0]'s scratch, even when it holds no row
   if (!S0) return set_err(pool, COOK_E_OOM, "%s: out of device memory", who);
   cudaStream_t st = pool->stream;
-  const int Rn = (int)R, Emax = IS_LEVELS * Rn;
-  hw = std::max(hw, Emax);
-  // ---- one carve, sized by the live rows: the rows, the selection, the entries and their orders, the outputs
-  int32_t *cnt = nullptr, *blk = nullptr, *a_user = nullptr, *a_reason = nullptr, *a_pidx = nullptr;
+  const int Rn = (int)R;
+  // ---- one carve, sized by the live rows: the rows, then the selection and the pipeline's buffers
+  int32_t *a_user = nullptr, *a_reason = nullptr, *a_pidx = nullptr;
   int64_t *a_tid = nullptr, *a_start = nullptr;
   double *a_cpus = nullptr, *a_mem = nullptr;
   uint8_t* a_facts = nullptr;
-  int32_t *s_user = nullptr, *s_reason = nullptr, *s_pidx = nullptr, *row = nullptr, *ord = nullptr, *tmp = nullptr;
-  int32_t *end = nullptr, *vord[3] = {}, *l_user = nullptr;
-  int64_t* s_tid = nullptr;
-  double *met[3] = {}, *pct = nullptr, *l_total = nullptr;
-  GridFlag* gf = nullptr;
-  ISKey key = {};
-  ISFoldArgs a = {};
+  ISPipe p;
   int64_t h2d = 0, d2h = 0;
   CK(pool, carve(S0->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
-    cnt = c.take<int32_t>(6);   // selected, start after now, segments, returned segments, leaders, compactions' own
-    blk = c.take<int32_t>((size_t)hw / CP_BLOCK + 2);
     a_user = c.take<int32_t>(Rn); a_reason = c.take<int32_t>(Rn); a_pidx = c.take<int32_t>(Rn);
     a_tid = c.take<int64_t>(Rn); a_start = c.take<int64_t>(Rn);
     a_cpus = c.take<double>(Rn); a_mem = c.take<double>(Rn); a_facts = c.take<uint8_t>(Rn);
-    s_user = c.take<int32_t>(Rn); s_reason = c.take<int32_t>(Rn); s_pidx = c.take<int32_t>(Rn);
-    s_tid = c.take<int64_t>(Rn);
-    for (int k = 0; k < 3; k++) met[k] = c.take<double>(Rn);
-    gf = c.take<GridFlag>(1);
-    key.kind = c.take<int32_t>(Emax); key.user = c.take<int32_t>(Emax); key.reason = c.take<int32_t>(Emax);
-    row = c.take<int32_t>(Emax); ord = c.take<int32_t>(Emax); tmp = c.take<int32_t>(Emax); end = c.take<int32_t>(Emax);
-    for (int k = 0; k < 3; k++) vord[k] = c.take<int32_t>(Emax);
-    for (int k = 0; k < 3; k++) {
-      a.os.part[k] = c.take<double>(Emax);
-      a.os.tile[k] = c.take<double>(Emax / OS_TILE + 2);
-    }
-    a.o_kind = c.take<int32_t>(Emax); a.o_user = c.take<int32_t>(Emax); a.o_reason = c.take<int32_t>(Emax);
-    a.o_count = c.take<int64_t>(Emax); a.o_total = c.take<double>(3 * (size_t)Emax);
-    pct = c.take<double>(15 * (size_t)Emax);
-    l_user = c.take<int32_t>(2 * COOK_IS_LEADERS); l_total = c.take<double>(2 * COOK_IS_LEADERS);
+    p.take(c, Rn, hw, false);
   }));
   CK(pool, cudaEventRecord(pool->ev[21], st));
-  CK(pool, cudaMemsetAsync(cnt, 0, sizeof(int32_t) * 6, st));
-  CK(pool, cudaMemsetAsync(gf, 0, sizeof(GridFlag), st));
+  CK(pool, p.clear(st));
   int nl = 0;
   // ---- the selection and its metrics
   int base = 0;
@@ -4435,61 +4755,119 @@ int32_t instance_stats(cook_pool* const* pools, int n, int64_t now, int32_t stat
     const int live = (int)h.first->run.slot_of.size();
     compact(ISRows{h.first->run.d_col, base, h.second, a_user, a_reason, a_tid, a_pidx, a_start, a_cpus, a_mem,
                    a_facts},
-            h.first->run.hw, nullptr, blk, cnt + 5, live, st, &nl);
+            h.first->run.hw, nullptr, p.blk, p.cnt + 5, live, st, &nl);
     base += live;
   }
   compact(ISSel{a_user, a_reason, a_tid, a_pidx, a_start, a_cpus, a_mem, a_facts, now, start_ms, end_ms, tid_lo, tid_hi,
-                status == COOK_IS_UNKNOWN, s_user, s_reason, s_tid, s_pidx, {met[0], met[1], met[2]}, cnt + 1},
-          Rn, nullptr, blk, cnt + 0, Rn, st, &nl);
+                status == COOK_IS_UNKNOWN, p.s_user, p.s_reason, p.s_tid, p.s_pidx, {p.met[0], p.met[1], p.met[2]},
+                p.cnt + 1},
+          Rn, nullptr, p.blk, p.cnt + 0, Rn, st, &nl);
   CK(pool, cudaGetLastError());
   int32_t sel[2];
-  CK(pool, download(sel, cnt, 2, st, &d2h));
+  CK(pool, download(sel, p.cnt, 2, st, &d2h));
   CK(pool, cudaStreamSynchronize(st));
   if (sel[1]) return set_err(pool, COOK_E_BADARG, "%s: a selected task starts after now_ms", who);
-  const int S = sel[0], E = IS_LEVELS * S, E3 = 3 * S;
-  int32_t got[2] = {0, 0};
-  if (S > 0) {
-    // ---- the entries, the fold order and its segments, the folds
-    grid_check_kernel<<<(S + 255) / 256, 256, 0, st>>>(met[0], met[1], met[2], S, gf);
-    is_expand_kernel<<<(E + 255) / 256, 256, 0, st>>>(S, s_user, s_reason, key, row);
-    nl += 2;
-    CK(pool, csort::sort_indices(ord, tmp, E, LessSegTidPool{key, row, s_tid, s_pidx}, st, &nl));
-    compact(ISSegEnds{ord, key, E, end}, E, nullptr, blk, cnt + 2, E, st, &nl);
-    order_scan(a.os, ISLoad{ord, row, {met[0], met[1], met[2]}}, E, gf, st, &nl);
-    a.ord = ord; a.row = row; a.k = key;
-    for (int k = 0; k < 3; k++) a.met[k] = met[k];
-    a.end = end; a.n_seg = cnt + 2; a.gf = gf; a.E = E;
-    is_fold_kernel<<<std::min((E + 3) / 4, 4096), 128, 0, st>>>(a);
-    nl++;
-    // ---- the ranks: the three levels returned are entries [0, 3 S), whose segments lead the fold order's
-    for (int k = 0; k < 3; k++) CK(pool, csort::sort_indices(vord[k], tmp, E3, LessSegValue{key, row, met[k]}, st, &nl));
-    is_pct_kernel<<<std::min((3 * E + 255) / 256, 4096), 256, 0, st>>>(cnt + 2, end, a.o_kind, vord[0], vord[1], vord[2],
-                                                                      row, met[0], met[1], met[2], pct);
-    is_leaders_kernel<<<2, 256, 0, st>>>(cnt + 2, a.o_kind, a.o_user, a.o_total, l_user, l_total, cnt + 3);
-    nl += 2;
-    CK(pool, cudaGetLastError());
-    CK(pool, download(got, cnt + 3, 2, st, &d2h));
-    CK(pool, cudaStreamSynchronize(st));
-  }
-  CK(pool, cudaEventRecord(pool->ev[22], st));
-  const int ns = got[0], nlead = got[1];
-  if (ns) {
-    CK(pool, download(o_kind, a.o_kind, ns, st, &d2h));
-    CK(pool, download(o_user, a.o_user, ns, st, &d2h));
-    CK(pool, download(o_reason, a.o_reason, ns, st, &d2h));
-    CK(pool, download(o_count, a.o_count, ns, st, &d2h));
-    CK(pool, download(o_total, a.o_total, 3 * (size_t)ns, st, &d2h));
-    CK(pool, download(o_pct, pct, 15 * (size_t)ns, st, &d2h));
-  }
-  for (int k = 0; k < 2 && nlead; k++) {
-    CK(pool, download(o_lead_user + k * COOK_IS_LEADERS, l_user + k * COOK_IS_LEADERS, nlead, st, &d2h));
-    CK(pool, download(o_lead_total + k * COOK_IS_LEADERS, l_total + k * COOK_IS_LEADERS, nlead, st, &d2h));
-  }
-  CK(pool, cudaEventRecord(pool->ev[23], st));
-  CK(pool, cudaStreamSynchronize(st));
-  *o_nseg = ns;
-  *o_nlead = nlead;
+  if (int32_t rc = is_answer(pool, st, p, sel[0], seg_cap, o, &nl, &d2h)) return rc;
   // the call's own statistics: no cook_last_stats slot is written
+  if (out_stats)
+    *out_stats = {ev_ms(pool->ev[20], pool->ev[21]), ev_ms(pool->ev[21], pool->ev[22]), ev_ms(pool->ev[22], pool->ev[23]),
+                  h2d, d2h, nl, 0};
+  return COOK_OK;
+}
+
+// one handle's finished rows of the status with task id in [tid_lo, tid_hi) and start in [start_ms, end_ms), dense
+// after the handles before it, with their metrics (task-run-time with the instance's end: (double)(end - start) /
+// 1000.0, times cpus and mem) and table position
+struct HSSel {
+  HistCols h; int base; int32_t pool; int success;
+  int64_t start_ms, end_ms, tid_lo, tid_hi;
+  int32_t* s_user; int32_t* s_reason; int64_t* s_tid; int32_t* s_pidx; int32_t* s_pos; double* met[3];
+  __device__ bool keep(int i) const {
+    return (h.ok[i] != 0) == (success != 0) && h.tid[i] >= tid_lo && h.tid[i] < tid_hi && h.start[i] >= start_ms &&
+           h.start[i] < end_ms;
+  }
+  __device__ void emit(int i, int d) const {
+    d += base;
+    s_user[d] = h.user[i]; s_reason[d] = h.reason[i]; s_tid[d] = h.tid[i]; s_pidx[d] = pool; s_pos[d] = i;
+    const double rt = (double)(h.end[i] - h.start[i]) / 1000.0;
+    met[0][d] = rt;
+    met[1][d] = rt * h.cpus[i];
+    met[2][d] = rt * h.mem[i];
+  }
+};
+// the selected rows' count, *out += (integer adds: any order is exact)
+__global__ void hs_count_kernel(HSSel f, int n, int32_t* out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int c = __reduce_add_sync(FULL_MASK, (i < n && f.keep(i)) ? 1 : 0);
+  if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, c);
+}
+
+int32_t history_stats(cook_pool* const* pools, int n, int32_t status, int64_t start_ms, int64_t end_ms, int64_t tid_lo,
+                      int64_t tid_hi, int32_t seg_cap, const ISOut& o, cook_phase_stats* out_stats) {
+  const char* who = "cook_state_history_stats";
+  // ---- every check before any device work or output
+  if (!pools || n <= 0 || !pools[0]) return COOK_E_BADARG;
+  cook_pool* pool = pools[0];
+  if (int32_t rc = is_handles(pools, n, who)) return rc;
+  if (status != COOK_IS_SUCCESS && status != COOK_IS_FAILED) return set_err(pool, COOK_E_BADARG, "%s: an unknown status", who);
+  if (end_ms <= start_ms) return set_err(pool, COOK_E_BADARG, "%s: end_ms <= start_ms", who);
+  if (is_out_null(o)) return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
+  if (seg_cap < 0) return set_err(pool, COOK_E_BADARG, "%s: seg_cap < 0", who);
+  // the handles with rows and their pool index
+  std::vector<std::pair<const History*, int32_t>> hs;
+  int Tmax = 0;
+  for (int k = 0; k < n; k++) {
+    const PoolState* s = static_cast<const PoolState*>(pools[k]->state);
+    if (!s || !s->hist.on) return set_err(pool, COOK_E_BADARG, "%s: a handle whose history is off", who);
+    if (s->hist.since > start_ms) return set_err(pool, COOK_E_BADARG, "%s: start_ms before a handle's horizon", who);
+    if (!s->hist.tail) continue;
+    hs.push_back({&s->hist, k});
+    Tmax = std::max(Tmax, (int)s->hist.tail);
+  }
+  if (hs.empty()) {   // no row to read: empty results without device work
+    is_empty(o, out_stats);
+    return COOK_OK;
+  }
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S0 = state_of(pool, true);
+  if (!S0) return set_err(pool, COOK_E_OOM, "%s: out of device memory", who);
+  cudaStream_t st = pool->stream;
+  const int H = (int)hs.size();
+  const bool ok = status == COOK_IS_SUCCESS;
+  auto sel = [&](int j, int base, const ISPipe& p) {
+    return HSSel{hs[j].first->c, base, hs[j].second, ok, start_ms, end_ms, tid_lo, tid_hi,
+                 p.s_user, p.s_reason, p.s_tid, p.s_pidx, p.s_pos, {p.met[0], p.met[1], p.met[2]}};
+  };
+  // ---- the selection's size per handle, so that every buffer after it is sized by the selection
+  int32_t* hcnt = nullptr;
+  int64_t h2d = 0, d2h = 0;
+  CK(pool, carve(S0->scratch, st, pool->ev[20], &h2d, [&](Carve& c) { hcnt = c.take<int32_t>(H); }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  CK(pool, cudaMemsetAsync(hcnt, 0, sizeof(int32_t) * H, st));
+  int nl = 0;
+  for (int j = 0; j < H; j++) {
+    const int T = (int)hs[j].first->tail;
+    hs_count_kernel<<<(T + 255) / 256, 256, 0, st>>>(sel(j, 0, ISPipe{}), T, hcnt + j);
+    nl++;
+  }
+  CK(pool, cudaGetLastError());
+  std::vector<int32_t> cnt(H);
+  CK(pool, download(cnt.data(), hcnt, H, st, &d2h));
+  CK(pool, cudaStreamSynchronize(st));
+  int64_t S = 0;
+  for (int32_t c : cnt) S += c;
+  if (S * IS_LEVELS > INT32_MAX) return set_err(pool, COOK_E_TOO_LARGE, "%s: more than 2^31 - 1 entries", who);
+  // ---- the selection and its metrics, then the pipeline
+  ISPipe p;
+  CK(pool, carve(S0->scratch, st, nullptr, &h2d, [&](Carve& c) { p.take(c, (int)S, Tmax, true); }));
+  CK(pool, p.clear(st));
+  int base = 0;
+  for (int j = 0; j < H && S; j++) {
+    if (cnt[j]) compact(sel(j, base, p), (int)hs[j].first->tail, nullptr, p.blk, p.cnt + 5, cnt[j], st, &nl);
+    base += cnt[j];
+  }
+  CK(pool, cudaGetLastError());
+  if (int32_t rc = is_answer(pool, st, p, (int)S, seg_cap, o, &nl, &d2h)) return rc;
   if (out_stats)
     *out_stats = {ev_ms(pool->ev[20], pool->ev[21]), ev_ms(pool->ev[21], pool->ev[22]), ev_ms(pool->ev[22], pool->ev[23]),
                   h2d, d2h, nl, 0};
@@ -4504,9 +4882,22 @@ extern "C" int32_t cook_state_instance_stats(cook_pool* const* pools, int32_t n_
                                              int32_t* out_reason, int64_t* out_count, double* out_total,
                                              double* out_pct, int32_t* out_leader_user, double* out_leader_total,
                                              int32_t* out_n_seg, int32_t* out_n_leader, cook_phase_stats* out_stats) {
-  return instance_stats(pools, n_pools, now_ms, status, start_ms, end_ms, task_id_lo, task_id_hi, seg_cap, out_kind,
-                        out_user, out_reason, out_count, out_total, out_pct, out_leader_user, out_leader_total,
-                        out_n_seg, out_n_leader, out_stats);
+  return instance_stats(pools, n_pools, now_ms, status, start_ms, end_ms, task_id_lo, task_id_hi, seg_cap,
+                        ISOut{out_kind, out_user, out_reason, out_count, out_total, out_pct, out_leader_user,
+                              out_leader_total, out_n_seg, out_n_leader},
+                        out_stats);
+}
+
+extern "C" int32_t cook_state_history_stats(cook_pool* const* pools, int32_t n_pools, int32_t status, int64_t start_ms,
+                                            int64_t end_ms, int64_t task_id_lo, int64_t task_id_hi, int32_t seg_cap,
+                                            int32_t* out_kind, int32_t* out_user, int32_t* out_reason,
+                                            int64_t* out_count, double* out_total, double* out_pct,
+                                            int32_t* out_leader_user, double* out_leader_total, int32_t* out_n_seg,
+                                            int32_t* out_n_leader, cook_phase_stats* out_stats) {
+  return history_stats(pools, n_pools, status, start_ms, end_ms, task_id_lo, task_id_hi, seg_cap,
+                       ISOut{out_kind, out_user, out_reason, out_count, out_total, out_pct, out_leader_user,
+                             out_leader_total, out_n_seg, out_n_leader},
+                       out_stats);
 }
 
 // ---- audit: the read side (cook_state_digest, cook_state_export, cook_state_queue).  The digest is one pass per

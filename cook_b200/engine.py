@@ -261,6 +261,49 @@ class GpuEngine:
         for t in tid.tolist():
             rng_.pop(t, None)
 
+    def state_finish_history(self, task_id, end_time_ms, success, reason_code=None):
+        """cook_state_finish_history: state_finish, and while the history is on, the rows that start at or after its
+        horizon are appended to it (reason_code None: each row's reason fact)."""
+        tid = np.ascontiguousarray(task_id, np.int64)
+        end = np.ascontiguousarray(end_time_ms, np.int64)
+        ok = np.ascontiguousarray(success, np.uint8)
+        rs = np.ascontiguousarray(reason_code, np.int32) if reason_code is not None else None
+        if any(c is not None and len(c) != len(tid) for c in (end, ok, rs)):
+            raise ValueError("state_finish_history: a column differs in length from task_id")
+        rc = self.lib.cook_state_finish_history(self.pool, len(tid), abi.ptr(tid, abi.P_I64), abi.ptr(end, abi.P_I64),
+                                                abi.ptr(ok, abi.P_U8),
+                                                abi.ptr(rs, abi.P_I32) if rs is not None else None)
+        if rc != 0:
+            self._err(rc)
+        getattr(self, "_state_running_ids", set()).difference_update(tid.tolist())
+        rng_ = self._group_lengths()[1]
+        for t in tid.tolist():
+            rng_.pop(t, None)
+
+    def state_history_seed(self, since_ms, task_id=(), user=(), start_ms=(), end_ms=(), cpus=(), mem=(), success=(),
+                           reason_code=()):
+        """cook_state_history_seed: the history replaced by these finished rows at horizon since_ms, and on."""
+        tid = np.ascontiguousarray(task_id, np.int64)
+        cols = (np.ascontiguousarray(user, np.int32), np.ascontiguousarray(start_ms, np.int64),
+                np.ascontiguousarray(end_ms, np.int64), np.ascontiguousarray(cpus, np.float64),
+                np.ascontiguousarray(mem, np.float64), np.ascontiguousarray(success, np.uint8),
+                np.ascontiguousarray(reason_code, np.int32))
+        if any(len(c) != len(tid) for c in cols):
+            raise ValueError("state_history_seed: a column differs in length from task_id")
+        u, st_, en, cp, me, ok, rs = cols
+        rc = self.lib.cook_state_history_seed(self.pool, int(since_ms), len(tid), abi.ptr(tid, abi.P_I64),
+                                              abi.ptr(u, abi.P_I32), abi.ptr(st_, abi.P_I64), abi.ptr(en, abi.P_I64),
+                                              abi.ptr(cp, abi.P_F64), abi.ptr(me, abi.P_F64), abi.ptr(ok, abi.P_U8),
+                                              abi.ptr(rs, abi.P_I32))
+        if rc != 0:
+            self._err(rc)
+
+    def state_history_advance(self, since_ms):
+        """cook_state_history_advance: the horizon raised to since_ms; the rows that start before it leave."""
+        rc = self.lib.cook_state_history_advance(self.pool, int(since_ms))
+        if rc != 0:
+            self._err(rc)
+
     def state_group_runtimes(self, group=(), runtime_s=(), forget=()):
         """cook_state_group_runtimes: the records of the groups in `forget` leave, then (group[i], runtime_s[i]) are
         appended."""
@@ -715,6 +758,27 @@ def state_user_usage(engines, users=None, per_pool=False, by_group=False):
     return out
 
 
+def _is_answer(engines, call, cap):
+    """One cook_state_instance_stats or cook_state_history_stats call with segment capacity `cap`: call(handles,
+    outputs...) -> rc.  Returns (rc, the answer, or the segments needed when rc is COOK_E_TOO_LARGE)."""
+    kind, user, reason = (np.zeros(cap, np.int32) for _ in range(3))
+    count = np.zeros(cap, np.int64)
+    total, pct = np.zeros((cap, 3)), np.zeros((cap, 3, 5))
+    lu, lt = np.zeros(2 * abi.IS_LEADERS, np.int32), np.zeros(2 * abi.IS_LEADERS)
+    n_seg, n_lead = C.c_int32(0), C.c_int32(0)
+    st = abi.PhaseStats()
+    handles = (C.c_void_p * len(engines))(*[e.pool for e in engines])
+    rc = call(handles, cap, abi.ptr(kind, abi.P_I32), abi.ptr(user, abi.P_I32), abi.ptr(reason, abi.P_I32),
+              abi.ptr(count, abi.P_I64), abi.ptr(total, abi.P_F64), abi.ptr(pct, abi.P_F64), abi.ptr(lu, abi.P_I32),
+              abi.ptr(lt, abi.P_F64), C.byref(n_seg), C.byref(n_lead), C.byref(st))
+    if rc != 0:
+        return rc, n_seg.value
+    n, L = n_seg.value, n_lead.value
+    lead = lambda k: [(int(lu[k * abi.IS_LEADERS + i]), float(lt[k * abi.IS_LEADERS + i])) for i in range(L)]
+    return rc, {"kind": kind[:n], "user": user[:n], "reason": reason[:n], "count": count[:n], "total": total[:n],
+                "pct": pct[:n], "leaders_cpu": lead(0), "leaders_mem": lead(1), "stats": st.as_dict()}
+
+
 def state_instance_stats(engines, now_ms, status, start_ms, end_ms, task_id_lo=-(1 << 63), task_id_hi=(1 << 63) - 1):
     """cook_state_instance_stats over the live running rows of `engines` (one device, the work on engines[0]'s stream):
     the rows of `status` (abi.IS_RUNNING or abi.IS_UNKNOWN) with task_id_lo <= task id < task_id_hi and start_ms <=
@@ -725,25 +789,30 @@ def state_instance_stats(engines, now_ms, status, start_ms, end_ms, task_id_lo=-
     if not engines:
         raise ValueError("state_instance_stats: at least one handle")
     R = sum(len(getattr(e, "_state_running_ids", ())) for e in engines)
-    cap = 1 + 2 * R
-    kind, user, reason = (np.zeros(cap, np.int32) for _ in range(3))
-    count = np.zeros(cap, np.int64)
-    total, pct = np.zeros((cap, 3)), np.zeros((cap, 3, 5))
-    lu, lt = np.zeros(2 * abi.IS_LEADERS, np.int32), np.zeros(2 * abi.IS_LEADERS)
-    n_seg, n_lead = C.c_int32(0), C.c_int32(0)
-    st = abi.PhaseStats()
-    handles = (C.c_void_p * len(engines))(*[e.pool for e in engines])
-    rc = engines[0].lib.cook_state_instance_stats(
-        handles, len(engines), int(now_ms), int(status), int(start_ms), int(end_ms), int(task_id_lo), int(task_id_hi),
-        cap, abi.ptr(kind, abi.P_I32), abi.ptr(user, abi.P_I32), abi.ptr(reason, abi.P_I32), abi.ptr(count, abi.P_I64),
-        abi.ptr(total, abi.P_F64), abi.ptr(pct, abi.P_F64), abi.ptr(lu, abi.P_I32), abi.ptr(lt, abi.P_F64),
-        C.byref(n_seg), C.byref(n_lead), C.byref(st))
+    rc, out = _is_answer(engines, lambda h, cap, *o: engines[0].lib.cook_state_instance_stats(
+        h, len(engines), int(now_ms), int(status), int(start_ms), int(end_ms), int(task_id_lo), int(task_id_hi), cap,
+        *o), 1 + 2 * R)
     if rc != 0:
         engines[0]._err(rc)
-    n, L = n_seg.value, n_lead.value
-    lead = lambda k: [(int(lu[k * abi.IS_LEADERS + i]), float(lt[k * abi.IS_LEADERS + i])) for i in range(L)]
-    return {"kind": kind[:n], "user": user[:n], "reason": reason[:n], "count": count[:n], "total": total[:n],
-            "pct": pct[:n], "leaders_cpu": lead(0), "leaders_mem": lead(1), "stats": st.as_dict()}
+    return out
+
+
+def state_history_stats(engines, status, start_ms, end_ms, task_id_lo=-(1 << 63), task_id_hi=(1 << 63) - 1,
+                        seg_cap=16384):
+    """cook_state_history_stats over the finished rows of `engines`' histories (one device): the rows of `status`
+    (abi.IS_SUCCESS or abi.IS_FAILED) with task_id_lo <= task id < task_id_hi and start_ms <= start < end_ms.  Returns
+    state_instance_stats' answer shape, so cycle.instance_stats_response builds the response unchanged.  The call is
+    made with seg_cap segments first and, when more are needed, once more with the count it reports."""
+    if not engines:
+        raise ValueError("state_history_stats: at least one handle")
+    call = lambda h, cap, *o: engines[0].lib.cook_state_history_stats(
+        h, len(engines), int(status), int(start_ms), int(end_ms), int(task_id_lo), int(task_id_hi), cap, *o)
+    rc, out = _is_answer(engines, call, max(int(seg_cap), 1))
+    if rc == abi.COOK_E_TOO_LARGE and out > seg_cap:
+        rc, out = _is_answer(engines, call, out)
+    if rc != 0:
+        engines[0]._err(rc)
+    return out
 
 
 STATS_KEYS = ("running", "waiting", "starved", "waiting-under-quota")   # by abi.STATS_*

@@ -873,7 +873,8 @@ int32_t cook_state_queue(cook_pool* pool, int32_t cap, int64_t* out_job_id, int3
 /* Device-side timing of the last call of each kind on this handle (CUDA events on the
  * pool's stream): what bench.py's `phases` block and roofline lines are computed from.
  * COOK_PHASE_STATE: the last cook_state_apply, cook_state_launch, cook_state_patch, cook_state_task_facts,
- * cook_state_task_reason, cook_state_finish or cook_state_group_runtimes (upload, then the scatter / move / record / compaction kernels).  COOK_PHASE_USAGE: the last cook_state_usage (upload of the
+ * cook_state_task_reason, cook_state_finish, cook_state_finish_history, cook_state_history_seed,
+ * cook_state_history_advance or cook_state_group_runtimes (upload, then the scatter / move / record / compaction kernels).  COOK_PHASE_USAGE: the last cook_state_usage (upload of the
  * hostname list, the compaction, sorts and folds, the download of the sums).  COOK_PHASE_COTASKS: the last
  * cook_state_cotasks (upload of the host codes, attribute columns and group map, the compaction, expansion and
  * sort, the download of the lists; all zero after a call without device work).  COOK_PHASE_CONSIDERABLE: the last
@@ -991,6 +992,53 @@ int32_t cook_state_task_reason(cook_pool* pool, int32_t n, const int64_t* task_i
  * Statistics: cook_last_stats(COOK_PHASE_STATE).                                                                  */
 int32_t cook_state_finish(cook_pool* pool, int32_t n, const int64_t* task_id, const int64_t* end_time_ms,
                           const uint8_t* success);
+
+/* ------------------------------------------------------- finished-instance history */
+/* A handle's history: a device table of its finished instances, 49 B per row (task id i64, user i32, start and end
+ * i64 ms, cpus and mem f64, reason code i32 with -1 for none, success u8), in arrival order.  Capacity doubles with
+ * device-to-device copies; rows leave only by a stable compaction.  The history is off until seeded; while it is off,
+ * no other call changes its behaviour or cost.  The handle keeps a horizon since_ms: every finished instance of this
+ * pool whose start is >= since_ms is in the table, and a finishing row whose start is before it is not kept.  Not part
+ * of cook_state_digest or cook_state_export; a reset through cook_state_apply empties it and turns it off.
+ * cook_state_history_stats reads it.
+ * Fixed choices:
+ *   Horizon  on start time.  Rows with start < the horizon are neither kept nor selectable; a window before it is
+ *            refused (cook_state_history_stats), never answered partially.
+ *   Reason   a finished row's reason is the caller's final reason (reason_code) or, with reason_code NULL, the running
+ *            row's cook_state_task_reason fact.
+ *   Interval end before start is COOK_E_BADARG (the reference's interval throws; this error is ours).
+ *
+ * cook_state_history_seed: replaces the history with rows [0, n), sets the horizon to since_ms and turns the history
+ * on (the start-up and leadership-change path: the finished instances with start >= since_ms, read once).  n = 0
+ * starts an empty history at that horizon.
+ * COOK_E_BADARG, before any change: n < 0; a NULL array while n > 0; a row with start < since_ms or end < start; a
+ * negative user; a reason below -1; cpus or mem negative, -0.0 or not finite (the stats rely on equal values being
+ * equal bits); a task id listed twice, or live in the handle's running table.
+ * Uploads exactly 49 * n bytes, copied straight into the table.  Statistics: cook_last_stats(COOK_PHASE_STATE). */
+int32_t cook_state_history_seed(cook_pool* pool, int64_t since_ms, int32_t n, const int64_t* task_id,
+                                const int32_t* user, const int64_t* start_ms, const int64_t* end_ms, const double* cpus,
+                                const double* mem, const uint8_t* success, const int32_t* reason_code);
+
+/* Exactly cook_state_finish(pool, n, task_id, end_time_ms, success), straggler records included; in addition, while
+ * the history is on, each row whose start is >= the horizon is appended to it in batch order, on the device from the
+ * running row before its removal (user, start, cpus, mem), with end_time_ms[i], success[i] != 0 (1 success, 0 failed)
+ * and reason_code[i] (NULL: the running row's reason fact).  The append costs O(n), not O(history).  While the
+ * history is off this is cook_state_finish plus the checks below.
+ * COOK_E_BADARG, before any change: everything cook_state_finish rejects; a NULL end_time_ms or success while n > 0;
+ * any row, failed ones included, whose end is before its start; a reason below -1.  COOK_E_TOO_LARGE: more than
+ * 2^31 - 1 records, or history rows.
+ * Uploads exactly cook_state_finish's 13 * n, plus 4 * n (reason_code) when reason_code is given and a row is appended.
+ * Statistics: cook_last_stats(COOK_PHASE_STATE).                                                                  */
+int32_t cook_state_finish_history(cook_pool* pool, int32_t n, const int64_t* task_id, const int64_t* end_time_ms,
+                                  const uint8_t* success, const int32_t* reason_code);
+
+/* Raises the horizon to since_ms and drops the rows with start < since_ms in one stable device compaction (into new
+ * columns of the same capacity, the old ones then freed).  The caller calls it periodically with now - retention; the
+ * retention is the caller's configuration.
+ * COOK_E_BADARG: the history is off; since_ms below the current horizon.
+ * Uploads nothing; downloads 4 bytes (the rows kept) when the table holds a row and since_ms is above the horizon,
+ * else nothing.  Statistics: cook_last_stats(COOK_PHASE_STATE).                                                 */
+int32_t cook_state_history_advance(cook_pool* pool, int64_t since_ms);
 
 /* The record table by hand: first every record of the groups forget_group[0, n_forget) leaves (groups the caller no
  * longer tracks), then n_add records (group[i], runtime_s[i]) are appended: the successes that finished before the
@@ -1147,7 +1195,7 @@ int32_t cook_state_user_usage(cook_pool* const* pools, int32_t n_pools, const in
  * + 164 * *out_n_seg (kind, user, reason, count, three totals, fifteen percentiles) + 24 * *out_n_leader.
  * Statistics: out_stats (may be NULL), as cook_state_user_stats; no cook_last_stats slot is written.  The outputs are
  * plain arrays, like cook_state_user_stats' outputs: every struct of this header has a ctypes mirror. */
-enum { COOK_IS_RUNNING = 0, COOK_IS_UNKNOWN = 1 };
+enum { COOK_IS_RUNNING = 0, COOK_IS_UNKNOWN = 1, COOK_IS_SUCCESS = 2, COOK_IS_FAILED = 3 };
 enum { COOK_IS_OVERALL = 0, COOK_IS_REASON = 1, COOK_IS_USER_REASON = 2 };
 enum { COOK_IS_RUN_TIME = 0, COOK_IS_CPU = 1, COOK_IS_MEM = 2, COOK_IS_LEADERS = 10 };
 int32_t cook_state_instance_stats(cook_pool* const* pools, int32_t n_pools, int64_t now_ms, int32_t status,
@@ -1156,6 +1204,32 @@ int32_t cook_state_instance_stats(cook_pool* const* pools, int32_t n_pools, int6
                                   int64_t* out_count, double* out_total, double* out_pct, int32_t* out_leader_user,
                                   double* out_leader_total, int32_t* out_n_seg, int32_t* out_n_leader,
                                   cook_phase_stats* out_stats);
+
+/* The device half of GET /stats/instances with status success or failed and no name filter, over the union of the
+ * history tables (cook_state_history_seed) of pools[0, n_pools); the handles follow cook_state_user_stats' rules.
+ * Outputs, segments, fold order, percentiles, leaders and their tie rule are cook_state_instance_stats', with:
+ *   Selection  status COOK_IS_SUCCESS (the success flag set) or COOK_IS_FAILED (clear; only this call accepts the two),
+ *              task_id_lo <= task id < task_id_hi and start_ms <= start < end_ms.
+ *   Entries    run_time = (double)(end - start) / 1000.0 (task-run-time with the instance's end time), cpu = run_time *
+ *              cpus, mem = run_time * mem.  There is no now.
+ *   Order      every total is a left fold from +0.0 in ascending (task id, pool index, table position): the position
+ *              keeps the answer deterministic when one handle holds a task id twice (a caller's divergence, not
+ *              checked after the seed).  Leaders of equal totals go by ascending user code.
+ * Sizes follow the selection S, not the table: every buffer after a count pass is sized by S.
+ * COOK_E_BADARG, before any device work and with nothing written: cook_state_user_stats' handle cases; an unknown
+ * status; end_ms <= start_ms; a NULL output (out_stats may be NULL); seg_cap < 0; a handle whose history is off or
+ * whose horizon is > start_ms (the caller then keeps the Datomic path).  COOK_E_TOO_LARGE: 4 * S >= 2^31, with nothing
+ * written; more than seg_cap segments, with only *out_n_seg (the segments needed) written, so that the caller can
+ * retry with that capacity.  No handle holds a row: empty results without device work (statistics zero).
+ * Transfers exactly: up nothing; down 4 * H (the selected rows of each of the H handles holding a row), plus, when a
+ * row is selected, 8 (the counts), plus, when *out_n_seg <= seg_cap, 164 * *out_n_seg + 24 * *out_n_leader.
+ * Statistics: out_stats (may be NULL), as cook_state_instance_stats.  Changes nothing resident.                    */
+int32_t cook_state_history_stats(cook_pool* const* pools, int32_t n_pools, int32_t status, int64_t start_ms,
+                                 int64_t end_ms, int64_t task_id_lo, int64_t task_id_hi, int32_t seg_cap,
+                                 int32_t* out_kind, int32_t* out_user, int32_t* out_reason, int64_t* out_count,
+                                 double* out_total, double* out_pct, int32_t* out_leader_user,
+                                 double* out_leader_total, int32_t* out_n_seg, int32_t* out_n_leader,
+                                 cook_phase_stats* out_stats);
 
 /* ----------------------------------------------------------------- multi-GPU */
 /* §8e: after a pool's match round every rank contributes its pools' usage

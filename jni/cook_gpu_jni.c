@@ -345,6 +345,21 @@ JFN(jint, stateUserUsage)(JNIEnv* env, jclass k, jlongArray pools, jint n_users,
   (*env)->SetIntArrayRegion(env, out_n, 0, 2, got);
   return rc;
 }
+/* finished tasks with the history: as stateFinish, plus reason_code n ints (null: each row's reason fact) */
+JFN(jint, stateFinishHistory)(JNIEnv* env, jclass k, jlong pool, jint n, jobject task_id, jobject end_time_ms,
+                              jobject success, jobject reason_code) {
+  return cook_state_finish_history((cook_pool*)(intptr_t)pool, n, one(env, task_id), one(env, end_time_ms),
+                                   one(env, success), one(env, reason_code));
+}
+/* the history's seed: cols the direct buffers of task_id, user, start_ms, end_ms, cpus, mem, success, reason_code */
+JFN(jint, stateHistorySeed)(JNIEnv* env, jclass k, jlong pool, jlong since_ms, jint n, jobjectArray cols) {
+  return cook_state_history_seed((cook_pool*)(intptr_t)pool, since_ms, n, buf(env, cols, 0), buf(env, cols, 1),
+                                 buf(env, cols, 2), buf(env, cols, 3), buf(env, cols, 4), buf(env, cols, 5),
+                                 buf(env, cols, 6), buf(env, cols, 7));
+}
+JFN(jint, stateHistoryAdvance)(JNIEnv* env, jclass k, jlong pool, jlong since_ms) {
+  return cook_state_history_advance((cook_pool*)(intptr_t)pool, since_ms);
+}
 /* instance stats: times [now_ms, start_ms, end_ms, task_id_lo, task_id_hi]; segs the direct buffers of kind, user,
  * reason (seg_cap ints), count (seg_cap longs), total (3 * seg_cap doubles), pct (15 * seg_cap doubles); leaders the
  * direct buffers of user (2 * COOK_IS_LEADERS ints) and total (2 * COOK_IS_LEADERS doubles); out_n gets [n_seg,
@@ -359,10 +374,16 @@ JFN(jint, stateInstanceStats)(JNIEnv* env, jclass k, jlongArray pools, jlongArra
   (*env)->ReleaseLongArrayElements(env, pools, h, JNI_ABORT);
   jlong t[5]; (*env)->GetLongArrayRegion(env, times, 0, 5, t);
   int32_t ns = 0, nl = 0;
-  jint rc = cook_state_instance_stats(p, (int32_t)n, t[0], status, t[1], t[2], t[3], t[4], seg_cap, buf(env, segs, 0),
-                                      buf(env, segs, 1), buf(env, segs, 2), buf(env, segs, 3), buf(env, segs, 4),
-                                      buf(env, segs, 5), buf(env, leaders, 0), buf(env, leaders, 1), &ns, &nl,
-                                      one(env, out_stats));
+  /* COOK_IS_SUCCESS and COOK_IS_FAILED read the histories (now_ms unused) */
+  jint rc = status == COOK_IS_SUCCESS || status == COOK_IS_FAILED
+                ? cook_state_history_stats(p, (int32_t)n, status, t[1], t[2], t[3], t[4], seg_cap, buf(env, segs, 0),
+                                           buf(env, segs, 1), buf(env, segs, 2), buf(env, segs, 3), buf(env, segs, 4),
+                                           buf(env, segs, 5), buf(env, leaders, 0), buf(env, leaders, 1), &ns, &nl,
+                                           one(env, out_stats))
+                : cook_state_instance_stats(p, (int32_t)n, t[0], status, t[1], t[2], t[3], t[4], seg_cap,
+                                            buf(env, segs, 0), buf(env, segs, 1), buf(env, segs, 2), buf(env, segs, 3),
+                                            buf(env, segs, 4), buf(env, segs, 5), buf(env, leaders, 0),
+                                            buf(env, leaders, 1), &ns, &nl, one(env, out_stats));
   jint got[2] = {ns, nl};
   (*env)->SetIntArrayRegion(env, out_n, 0, 2, got);
   return rc;

@@ -40,6 +40,13 @@ groups, against numpy over a host mirror:
 of the rows with a reason and a twentieth unknown, and times cook_state_instance_stats for status running and unknown
 over a window covering every row, against numpy over a host mirror:
   python tools/prof_state.py --instance-stats --pool c5 --reps 10
+--history-stats seeds finished-instance histories over 31 days (--history-rows rows, C2's users and shapes on one
+handle, or with --c3-group N config-#3 pools' shapes as N handles) and times cook_state_history_stats for success and
+failed over a window covering every row and over the last day, against numpy over a host mirror; then a batch of 1000
+finishes through cook_state_finish_history against cook_state_finish, one advance dropping a day, and the device
+memory of the table and of the call's scratch:
+  python tools/prof_state.py --history-stats --history-rows 1000000 --reps 5
+  python tools/prof_state.py --history-stats --history-rows 10000000 --c3-group 4 --reps 3
 --unscheduled loads C2 (or config-#5 pool --c5-pool with --pool c5) into a resident handle, on the grid and off it,
 and times cook_state_unscheduled for one job, 1000 jobs and every waiting job of the user with the most, against numpy
 over a host mirror, with the answers compared bit for bit:
@@ -1179,6 +1186,127 @@ def instance_stats_prof(a):
         e.close()
 
 
+DAY_MS = 86_400_000
+
+
+def free_bytes():
+    import torch
+    torch.cuda.synchronize()
+    return int(torch.cuda.mem_get_info(0)[0])
+
+
+def history_stats_prof(a):
+    """cook_state_history_stats over seeded histories against numpy over a host mirror (host_instance_stats with each
+    row's start moved to -(end - start) and now = 0, so that its run time is end - start)."""
+    if a.c3_group > 0:
+        ts = [traces.gen_config_pool("c3", p) for p in range(a.c3_group)]
+        name = f"c3/0-{a.c3_group - 1}"
+    else:
+        ts = [traces.gen_c2()]
+        name = "c2"
+    rng = np.random.default_rng(a.seed)
+    H = len(ts)
+    per = a.history_rows // H
+    t_end = 1_700_000_000_000
+    since = t_end - 31 * DAY_MS
+    print(json.dumps({"card": card(), "pools": name, "handles": H, "rows": per * H}), flush=True)
+    es, m = [], {k: [] for k in ("user", "tid", "pidx", "start", "end", "cpus", "mem", "reason", "ok")}
+    f0 = free_bytes()
+    next_tid = 1
+    for p, t in enumerate(ts):
+        r = t["cols"]["running"]
+        k = rng.integers(0, len(r["task_id"]), per)   # C2's (or the pool's) users and shapes
+        start = np.sort(rng.integers(since, t_end, per))
+        cols = dict(task_id=np.arange(next_tid, next_tid + per, dtype=np.int64), user=np.asarray(r["user"])[k],
+                    start_ms=start, end_ms=start + rng.integers(0, 2 * 3_600_000, per),
+                    cpus=np.asarray(r["cpus"], np.float64)[k], mem=np.asarray(r["mem"], np.float64)[k],
+                    success=(rng.random(per) < 0.7).astype(np.uint8),
+                    reason_code=np.where(rng.random(per) < 0.3, rng.choice([1001, 2003, 3001], per), -1))
+        next_tid += per
+        e = GpuEngine(pool_name=f"history-stats-{p}")
+        e.state_history_seed(since, **cols)
+        es.append(e)
+        for mk, ck in (("user", "user"), ("tid", "task_id"), ("start", "start_ms"), ("end", "end_ms"),
+                       ("cpus", "cpus"), ("mem", "mem"), ("reason", "reason_code"), ("ok", "success")):
+            m[mk].append(np.asarray(cols[ck]))
+        m["pidx"].append(np.full(per, p))
+    table = f0 - free_bytes()
+    m = {k: np.concatenate(v) for k, v in m.items()}
+    f = lambda x: np.asarray(x, np.float64).view(np.int64).tolist()
+    for wname, lo, hi in (("all", since, t_end + 1), ("one day", t_end - DAY_MS, t_end + 1)):
+        for status in (abi.IS_SUCCESS, abi.IS_FAILED):
+            f1 = free_bytes()
+            for _ in range(2):   # warm-up: the carves and the first launches
+                got = engine.state_history_stats(es, status, lo, hi)
+            scratch = f1 - free_bytes()
+            sel = np.flatnonzero((m["start"] >= lo) & (m["start"] < hi))
+            mirror = {"user": m["user"][sel], "tid": m["tid"][sel], "pidx": m["pidx"][sel],
+                      "start": -(m["end"][sel] - m["start"][sel]), "cpus": m["cpus"][sel], "mem": m["mem"][sel],
+                      "reason": m["reason"][sel], "unknown": m["ok"][sel]}
+            dev, wall, host, same = [], [], [], True
+            for _ in range(a.reps):
+                w0 = time.perf_counter()
+                got = engine.state_history_stats(es, status, lo, hi)
+                wall.append(time.perf_counter() - w0)
+                st = got["stats"]
+                dev.append(st["ms_h2d"] + st["ms_device"] + st["ms_d2h"])
+            w0 = time.perf_counter()
+            segs, lc, lm = host_instance_stats(mirror, 0, int(status == abi.IS_SUCCESS))
+            host.append(time.perf_counter() - w0)
+            same = len(segs) == len(got["kind"]) and all(
+                (int(got["kind"][d]), int(got["user"][d]), int(got["reason"][d]), int(got["count"][d])) == w[:4]
+                and f(got["total"][d]) == f(w[4]) and f(got["pct"][d]) == f(w[5]) for d, w in enumerate(segs)) and \
+                [(u, f([x])) for u, x in got["leaders_cpu"]] == [(u, f([x])) for u, x in lc] and \
+                [(u, f([x])) for u, x in got["leaders_mem"]] == [(u, f([x])) for u, x in lm]
+            print(json.dumps({"window": wname, "status": "success" if status == abi.IS_SUCCESS else "failed",
+                              "selected": int(got["count"][0]) if len(got["count"]) else 0,
+                              "segments": len(got["kind"]), "device_ms": round(float(np.median(dev)), 4),
+                              "wall_ms": round(1e3 * float(np.median(wall)), 4), "h2d_bytes": st["h2d_bytes"],
+                              "d2h_bytes": st["d2h_bytes"], "n_launches": st["n_launches"],
+                              "numpy_wall_ms": round(1e3 * float(np.median(host)), 4), "identical": bool(same),
+                              "table_bytes": table, "scratch_bytes_grown": scratch}), flush=True)
+    # a batch of 1000 finishes over the history of handle 0: cook_state_finish_history against cook_state_finish on a
+    # twin without history, alternating
+    e, twin = es[0], GpuEngine(pool_name="history-twin")
+    t = ts[0]["cols"]["running"]
+    res = {"finish_history": [], "finish": []}
+    for rep in range(a.reps + 1):
+        tid = np.arange(next_tid, next_tid + 1000, dtype=np.int64)
+        next_tid += 1000
+        run = dict(task_id=tid, job_id=tid + 10 ** 9, user=np.asarray(t["user"])[:1000],
+                   priority=np.full(1000, 50, np.int32), start_time=np.full(1000, t_end - 1000, np.int64),
+                   cpus=np.asarray(t["cpus"], np.float64)[:1000], mem=np.asarray(t["mem"], np.float64)[:1000],
+                   gpus=np.zeros(1000))
+        for x in (e, twin):
+            x.state_apply(abi.make_delta(running=abi.make_tasks(**run)))
+        end = np.full(1000, t_end, np.int64)
+        ok = (np.arange(1000) % 2).astype(np.uint8)
+        for kind, fn in (("finish_history", lambda: e.state_finish_history(tid, end, ok, None)),
+                         ("finish", lambda: twin.state_finish(tid, end, ok))):
+            w0 = time.perf_counter()
+            fn()
+            w = time.perf_counter() - w0
+            st = (e if kind == "finish_history" else twin).last_stats(abi.PHASE_STATE)
+            if rep:
+                res[kind].append((st["ms_h2d"] + st["ms_device"], 1e3 * w, st["h2d_bytes"], st["n_launches"]))
+    for kind, v in res.items():
+        print(json.dumps({"call": kind, "batch": 1000, "history_rows": int(len(m["tid"]) // H),
+                          "device_ms": round(float(np.median([x[0] for x in v])), 4),
+                          "wall_ms": round(float(np.median([x[1] for x in v])), 4), "h2d_bytes": v[-1][2],
+                          "n_launches": v[-1][3]}), flush=True)
+    twin.close()
+    # one advance dropping a day
+    w0 = time.perf_counter()
+    e.state_history_advance(since + DAY_MS)
+    w = time.perf_counter() - w0
+    st = e.last_stats(abi.PHASE_STATE)
+    print(json.dumps({"call": "advance", "dropped_day": True, "device_ms": round(st["ms_device"], 4),
+                      "wall_ms": round(1e3 * w, 4), "d2h_bytes": st["d2h_bytes"], "n_launches": st["n_launches"]}),
+          flush=True)
+    for x in es:
+        x.close()
+
+
 def rank_quota_prof(a):
     t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
     pc, rc0, users = t["cols"]["pending"], t["cols"]["running"], t["users"]
@@ -1246,7 +1374,12 @@ def main():
                     help="cook_state_user_usage against numpy over a host mirror (--c3-group N: N config-#3 pools)")
     ap.add_argument("--instance-stats", action="store_true",
                     help="cook_state_instance_stats against numpy over a host mirror (--c3-group N: N config-#3 pools)")
+    ap.add_argument("--history-stats", action="store_true",
+                    help="cook_state_history_stats against numpy over a host mirror (--c3-group N: N config-#3 pools)")
+    ap.add_argument("--history-rows", type=int, default=1_000_000, help="--history-stats: the finished rows in all")
     a = ap.parse_args()
+    if a.history_stats:
+        return history_stats_prof(a)
     if a.instance_stats:
         return instance_stats_prof(a)
     if a.user_usage:
