@@ -18,6 +18,9 @@
 ;;                                              task-reason! [cook_state_instance_stats, cook_state_task_reason], and
 ;;                                              for success / failed by history-seed!, finish-history! and
 ;;                                              history-advance! [cook_state_history_*]
+;;   :1210-1280 handle-match-cycle-metrics and the unmatched tracking :1399-1486
+;;                                           -> (match-metrics! ...) + cycle.py's match_cycle_metrics_response, fed by
+;;                                              job-facts! [cook_state_match_metrics, cook_state_job_facts]
 ;; selected per pool with {:scheduler-config {:scheduler "gpu"}} next to "fenzo" / "kubernetes"
 ;; (config.clj:110-122, make-pool-handler :2425-2466).  Everything numeric happens in libcookgpu;
 ;; this namespace marshals columns and keeps the state Fenzo kept (cook_b200/cycle.py is the same
@@ -536,3 +539,63 @@
                                              (vec (for [j (range 5)] (f64 (segs 5) (+ (* 15 d) (* 5 m) j))))))}))
        :leaders-cpu (lead 0)
        :leaders-mem (lead 1)})))
+
+;; ---------------------------------------------------------------------------------------------
+;; the match-cycle metrics of a resident pool (handle-match-cycle-metrics scheduler.clj:1210-1280, the unmatched
+;; tracking :1399-1486), called after the match and before the launches
+(def ^:private jf-gpus 1) (def ^:private jf-disk 2) (def ^:private jf-disk-request 4) (def ^:private jf-disk-limit 8)
+(def ^:private jf-uris 16)
+(defn job-facts!
+  "The stats keys of live pending jobs, from the tx-report tap after each pending upsert (which clears them): `jobs` is
+   [{:job-id :resources (tools/job-ent->resources) :gpu-model (the job's COOK_GPU_MODEL or nil)}]; the model and disk
+   type names are coded through `gpu-models` and `disk-types` (dictionary)."
+  [handle gpu-models disk-types jobs]
+  (let [facts (for [{:keys [resources]} jobs
+                    :let [{:keys [gpus disk uris]} resources]]
+                (cond-> 0
+                  gpus (bit-or jf-gpus)
+                  disk (bit-or jf-disk)
+                  (some? (:request disk)) (bit-or jf-disk-request)
+                  (some? (:limit disk)) (bit-or jf-disk-limit)
+                  (seq uris) (bit-or jf-uris)))]
+    (check! handle (Native/stateJobFacts handle (count jobs) (longs-buf (map :job-id jobs))
+                                         (let [b (direct (count jobs))]
+                                           (doseq [[i f] (map-indexed vector facts)] (.put b (int i) (byte f))) b)
+                                         (ints-buf (map #(code! gpu-models (:gpu-model %)) jobs))
+                                         (doubles-buf (map #(or (get-in % [:resources :disk :request]) 0.0) jobs))
+                                         (doubles-buf (map #(or (get-in % [:resources :disk :limit]) 0.0) jobs))
+                                         (ints-buf (map #(code! disk-types (get-in % [:resources :disk :type])) jobs)))
+            "cook_state_job_facts")))
+
+(def ^:private mm-first 10)
+(defn match-metrics!
+  "The metrics of the last resident match on `handle`: `dropped` are the considerable positions whose matches
+   filter-matches-for-ratelimit dropped.  With more keys than `key-cap` the call reports the count and the round stays
+   uncounted, so this retries once with it.  Returns {:counts [considerable matched head-job-id head-matched uris
+   uris-position keys too-long first] :amounts [total-cpus total-mem p50 p95 p100 (cpus) p50 p95 p100 (mem)]
+   :rows [{:ints [job-id position user ports facts gpu-model disk-type] :amounts [cpus mem gpus disk-request
+   disk-limit]} x3 (head, largest by cpus, largest by mem)] :first [[job-id cycles]] :users [[considerable matched]]
+   :keys [[kind code total]]}; the handler builds the log maps and the warning as cook_b200/cycle.py's
+   match_cycle_metrics_response does."
+  [handle n-users dropped unmatched-warn-cycles key-cap]
+  (loop [cap (max 1 key-cap) tries 0]
+    (let [outs [(direct (* 8 9)) (direct (* 8 8)) (direct (* 8 21)) (direct (* 8 15)) (direct (* 8 mm-first))
+                (direct (* 4 mm-first)) (direct (* 4 n-users)) (direct (* 4 n-users)) (direct (* 4 cap))
+                (direct (* 4 cap)) (direct (* 8 cap))]
+          rc (Native/stateMatchMetrics handle n-users (count dropped) (when (seq dropped) (ints-buf dropped))
+                                       unmatched-warn-cycles cap (object-array outs) nil)
+          i64 (fn [^ByteBuffer b d] (.getLong b (int (* 8 d))))
+          i32 (fn [^ByteBuffer b d] (.getInt b (int (* 4 d))))
+          f64 (fn [^ByteBuffer b d] (.getDouble b (int (* 8 d))))
+          n-keys (i64 (outs 0) 6)]
+      (if (and (= rc -7) (zero? tries) (> n-keys cap))
+        (recur (int n-keys) 1)
+        (do
+          (check! handle rc "cook_state_match_metrics")
+          {:counts (vec (for [i (range 9)] (i64 (outs 0) i)))
+           :amounts (vec (for [i (range 8)] (f64 (outs 1) i)))
+           :rows (vec (for [r (range 3)] {:ints (vec (for [i (range 7)] (i64 (outs 2) (+ (* 7 r) i))))
+                                          :amounts (vec (for [i (range 5)] (f64 (outs 3) (+ (* 5 r) i))))}))
+           :first (vec (for [i (range (i64 (outs 0) 8))] [(i64 (outs 4) i) (i32 (outs 5) i)]))
+           :users (vec (for [u (range n-users)] [(i32 (outs 6) u) (i32 (outs 7) u)]))
+           :keys (vec (for [d (range n-keys)] [(i32 (outs 8) d) (i32 (outs 9) d) (f64 (outs 10) d)]))})))))

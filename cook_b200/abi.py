@@ -162,6 +162,17 @@ IS_RUNNING, IS_UNKNOWN, IS_SUCCESS, IS_FAILED = 0, 1, 2, 3
 IS_OVERALL, IS_REASON, IS_USER_REASON = 0, 1, 2
 IS_RUN_TIME, IS_CPU, IS_MEM, IS_LEADERS = 0, 1, 2, 10
 
+# cook_state_job_facts' bits and cook_state_match_metrics' key kinds and first-ten length
+JF_GPUS, JF_DISK, JF_DISK_REQUEST, JF_DISK_LIMIT, JF_URIS = 1, 2, 4, 8, 16
+MM_GPUS, MM_DISK_REQUEST, MM_DISK_LIMIT = 0, 1, 2
+MM_FIRST_N = 10
+
+MMC_CONSIDERABLE, MMC_MATCHED, MMC_HEAD_JOB_ID, MMC_HEAD_MATCHED, MMC_URIS, MMC_URIS_POSITION, MMC_KEYS = 0, 1, 2, 3, 4, 5, 6
+MMC_TOO_LONG, MMC_FIRST, MMC_N = 7, 8, 9
+MMA_TOTAL_CPUS, MMA_TOTAL_MEM, MMA_PCT_CPUS, MMA_PCT_MEM, MMA_N = 0, 1, 2, 5, 8
+MM_HEAD, MM_LARGEST_CPUS, MM_LARGEST_MEM, MM_ROWS = 0, 1, 2, 3
+MMR_INT = ("job_id", "position", "user", "ports", "facts", "gpu_model", "disk_type")    # by COOK_MMR_*, integers
+MMR_AMOUNT = ("cpus", "mem", "gpus", "disk_request", "disk_limit")                        # by COOK_MMR_*, amounts
 
 class ConsiderableParams(C.Structure):
     """cook_considerable_params: M0 over the resident queue (cook_state_considerable)."""
@@ -340,6 +351,9 @@ ARGTYPES = {
                               _P(PhaseStats)],
     "cook_state_task_facts": [_H, _I32, P_I64, P_I64, P_U8, P_U8],
     "cook_state_task_reason": [_H, _I32, P_I64, P_I32],
+    "cook_state_job_facts": [_H, _I32, P_I64, P_U8, P_I32, P_F64, P_F64, P_I32],
+    "cook_state_match_metrics": [_H, _I32, _I32, P_I32, _I32, _I32, P_I64, P_F64, P_I64, P_F64, P_I64, P_I32, P_I32,
+                                 P_I32, P_I32, P_I32, P_F64, _P(PhaseStats)],
     "cook_state_finish": [_H, _I32, P_I64, P_I64, P_U8],
     "cook_state_finish_history": [_H, _I32, P_I64, P_I64, P_U8, P_I32],
     "cook_state_history_seed": [_H, C.c_int64, _I32, P_I64, P_I32, P_I64, P_I64, P_F64, P_F64, P_U8, P_I32],

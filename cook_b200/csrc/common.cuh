@@ -274,6 +274,11 @@ int32_t match_build(cook_pool* pool, const int32_t* ranked_idx, int32_t n_ranked
                     MatchRows* rows);
 int32_t match_run(cook_pool* pool, int32_t* out_considerable, int64_t* out_job_id, int32_t* out_assign,
                   int32_t* out_ports, uint8_t* out_fail_reason, cook_match_stats* out_stats, bool uploaded, int max_ctas);
+// The number of match_run calls on the pool's plan so far, and the round of run number `run` while it is still the
+// plan's last (false after a later run or a failed build): its considerable jobs' rows (cons[k]: the row of the k-th
+// considerable job) and their assignments (-1: none), on the device.  cook_state_match_metrics reads them.
+uint64_t match_runs(cook_pool* pool);
+bool match_round(cook_pool* pool, uint64_t run, int32_t* n_cons, const int32_t** cons, const int32_t** assign);
 
 // match.cu: M0 (pending-jobs->considerable-jobs, filter-pending-jobs-for-quota) over n job rows already on the
 // device, by cook_match's own launches: the per-user folds in the order `ranked` gives, the pool-quota fold over

@@ -2357,6 +2357,7 @@ struct MatchPlan {
   int32_t bk_init[3] = {0, 0, 0};
   int64_t* d_job_id = nullptr;    // device-source plans: job id per row, and per considerable job
   int64_t* d_cons_jid = nullptr;
+  uint64_t runs = 0;              // match_run calls on this plan: what identifies a round (match_round)
 };
 
 static void plan_free(void* p) {
@@ -2662,6 +2663,7 @@ int32_t match_run(cook_pool* pool, int32_t* out_considerable, int64_t* out_job_i
                   int32_t* out_ports, uint8_t* out_fail_reason, cook_match_stats* out_stats, bool uploaded, int max_ctas) {
   MatchPlan* mp = plan_of(pool);
   mp->valid = true;   // the plan's inputs are complete: a caller that writes its rows did so before the run
+  mp->runs++;
   cudaStream_t st = pool->stream;
   const int O = mp->O, U = mp->U, max_ports = mp->max_ports;
   MatchArgs& ma = mp->ma;
@@ -2885,6 +2887,17 @@ int32_t match_run(cook_pool* pool, int32_t* out_considerable, int64_t* out_job_i
     out_stats->d2h_bytes = ps.d2h_bytes;
   }
   return COOK_OK;
+}
+
+uint64_t match_runs(cook_pool* pool) { return pool->match_plan ? static_cast<MatchPlan*>(pool->match_plan)->runs : 0; }
+
+bool match_round(cook_pool* pool, uint64_t run, int32_t* n_cons, const int32_t** cons, const int32_t** assign) {
+  const MatchPlan* mp = static_cast<const MatchPlan*>(pool->match_plan);
+  if (!mp || !mp->valid || mp->runs != run) return false;
+  *n_cons = mp->last_n_cons;
+  *cons = mp->d_cons;
+  *assign = mp->d_out_assign;
+  return true;
 }
 
 cudaError_t considerable_rows(const ConsRows& r, cudaStream_t st, int* launches) {

@@ -38,9 +38,13 @@ namespace {
 enum PCol {
   P_USER, P_PRIO, P_JID, P_CPUS, P_MEM, P_GPUS, P_PORTS, P_ALLOWED, P_PLUGIN, P_GPU_MODEL, P_DISK_REQ, P_DISK_TYPE,
   P_EST, P_CKPT, P_RESERVED, P_NDATA,   // the columns a delta row carries
-  P_LIVE = P_NDATA, P_GEN, P_NOFF, P_NLEN, P_AOFF, P_ALEN, P_GOFF, P_GLEN, P_NCOL
+  P_LIVE = P_NDATA, P_GEN, P_NOFF, P_NLEN, P_AOFF, P_ALEN, P_GOFF, P_GLEN,
+  P_JF, P_JF_GPU, P_JF_DREQ, P_JF_DLIM, P_JF_DTYPE, P_NCOL
 };
-constexpr int P_SZ[P_NCOL] = {4, 4, 8, 8, 8, 8, 4, 1, 1, 4, 8, 4, 8, 4, 4, 1, 4, 4, 4, 4, 4, 4, 4};
+constexpr int P_SZ[P_NCOL] = {4, 4, 8, 8, 8, 8, 4, 1, 1, 4, 8, 4, 8, 4, 4, 1, 4, 4, 4, 4, 4, 4, 4, 1, 4, 8, 8, 4};
+// P_JF .. P_JF_DTYPE are the job facts cook_state_job_facts writes (the stats keys of jobs->resource-maps): the
+// COOK_JF_* bits, then the gpu model, disk request, disk limit and disk type, each read only under its bit.  Every
+// pending upsert writes P_JF = 0, so the others need no reset.
 // R_MAXRT and R_FACTS are the facts cook_state_task_facts writes: the job's max-runtime (-1: none) and the
 // RF_* bits; R_REASON the fact cook_state_task_reason writes: the instance's reason code (-1: none).  Every upsert
 // and launch writes their absent values.
@@ -572,6 +576,8 @@ struct PendingInfo {
   int32_t user = 0;
   int32_t len[3] = {0, 0, 0};
   uint16_t flags = 0;
+  uint8_t jf = 0;            // the COOK_JF_* bits of the row's job facts
+  int64_t touched = 0;       // PoolState::pend_epoch when the slot was last upserted or removed
   std::vector<int32_t> groups, attr_cols;
 };
 
@@ -767,6 +773,23 @@ struct OfferHost {
   std::map<int64_t, int32_t> live;
 };
 
+// The last resident match round, as cook_state_match_metrics reads it: the match's rows as pending slots (its m_slot,
+// copied on the device), the pending epoch at the match and the plan run (match_runs) that holds the considerable jobs
+// and their assignments; and the unmatched counters, the last counted round's unmatched jobs as (job id ascending,
+// cycles), double-buffered.
+struct MetricsRound {
+  bool on = false, counted = false;
+  int32_t n_rows = 0;
+  int64_t epoch = 0;
+  uint64_t run = 0;
+  int32_t* slot = nullptr; int64_t slot_cap = 0;
+  int64_t* u_jid[2] = {}; int32_t* u_cyc[2] = {}; int64_t u_cap = 0; int cur = 0; int32_t u_n = 0;
+  void release() {
+    for (void* p : {(void*)slot, (void*)u_jid[0], (void*)u_jid[1], (void*)u_cyc[0], (void*)u_cyc[1]}) if (p) cudaFree(p);
+    *this = MetricsRound{};
+  }
+};
+
 struct PoolState {
   Table pend, run;
   // ---- the live offers (cook_state_offers_add, cook_state_match_offers)
@@ -799,6 +822,9 @@ struct PoolState {
   std::map<int32_t, int64_t> groups_r;                              // running rows' group codes
   int64_t cot_rows = 0, cot_n = 0;   // live running rows with a known host and a group list, and their entries
   int64_t nflag[F_N] = {};
+  int64_t jf_keyed = 0;               // live pending rows whose job facts hold a gpus or disk resource
+  int64_t pend_epoch = 0;             // counts the calls that upserted or removed a pending row
+  MetricsRound mm;
   std::unordered_set<int32_t> reserved;   // the live pending slots whose reserved_host is not -1
   Arena stage;                        // one batch's uploads
   Arena scratch;                      // one call's device buffers
@@ -829,6 +855,7 @@ struct PoolState {
     for (auto& l : lists) l.release();
     for (auto& l : olists) l.release();
     stage.release(); scratch.release(); derive.release(); queue.release(); omerge.release();
+    mm.release();
     if (counters) cudaFree(counters);
     if (gf0) cudaFree(gf0);
   }
@@ -838,6 +865,7 @@ struct PoolState {
     for (int32_t c : pi.attr_cols) count_add(attr_cols, c, sign);
     for (int l = 0; l < 3; l++) lists[l].live += sign * pi.len[l];
     for (int f = 0; f < F_N; f++) if ((pi.flags >> f) & 1) nflag[f] += sign;
+    if (pi.jf & (COOK_JF_GPUS | COOK_JF_DISK)) jf_keyed += sign;
     if ((pi.flags >> F_RESERVED) & 1) {
       if (sign > 0) reserved.insert(slot);
       else reserved.erase(slot);
@@ -1064,13 +1092,18 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
     for (auto& l : S->lists) l.tail = l.live = 0;
     if (S->offer.hw) CK(pool, cudaMemsetAsync(S->offer.col[O_LIVE], 0, (size_t)S->offer.hw, st));
     offers_drop(S);
+    S->jf_keyed = 0;
+    S->mm.on = false;
+    S->mm.u_n = 0;
   }
+  if (rs || np || npr) S->pend_epoch++;
   std::vector<int32_t> prm_slot(npr), pup_slot(np), rrm_slot(nrr), rup_slot(nr);
   for (int i = 0; i < npr; i++) {
     auto it = S->pend.slot_of.find(d->pending_rm_job_id[i]);
     const int32_t s = it->second;
     S->pend.slot_of.erase(it);
     S->add_pending(s, S->pinfo[s], -1);
+    S->pinfo[s].touched = S->pend_epoch;
     S->pend.free.push_back(s);
     prm_slot[i] = s;
   }
@@ -1101,6 +1134,8 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
                          P.ckpt_location && P.ckpt_location[i] != -1, P.reserved_host && P.reserved_host[i] != -1};
     pi.flags = 0;
     for (int k = 0; k < F_N; k++) if (f[k]) pi.flags |= (uint16_t)(1u << k);
+    pi.jf = 0;
+    pi.touched = S->pend_epoch;
     S->add_pending(s, pi, +1);
     pup_slot[i] = s;
   }
@@ -1159,7 +1194,8 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
         else up = reinterpret_cast<const char*>(c.up(static_cast<const int64_t*>(src[k]), np));
         pu.c[k] = ScatterCol{static_cast<char*>(S->pend.col[k]), up, dflt[k], P_SZ[k]};
       }
-      pu.nc = P_NDATA;
+      pu.c[P_NDATA] = ScatterCol{static_cast<char*>(S->pend.col[P_JF]), nullptr, 0, P_SZ[P_JF]};   // no job facts
+      pu.nc = P_NDATA + 1;
       pu.slot = c.up(pup_slot.data(), np);
       for (int l = 0; l < 3; l++) {
         pu.doff[l] = c.up(lists_off[l], np + 1);
@@ -1239,10 +1275,12 @@ int32_t launch(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, cons
   CK(pool, cudaSetDevice(pool->device));
   cudaStream_t st = pool->stream;
   // ---- host side, in cook_state_apply's order: the removals free their slots, then the tasks take theirs
+  if (n) S->pend_epoch++;
   for (int i = 0; i < n; i++) {
     const int32_t s = pslot[i];
     S->pend.slot_of.erase(job_id[i]);
     S->add_pending(s, S->pinfo[s], -1);
+    S->pinfo[s].touched = S->pend_epoch;
     S->pend.free.push_back(s);
   }
   int64_t ng = 0;   // group list entries that move with the jobs
@@ -2197,6 +2235,27 @@ extern "C" int32_t cook_state_cotasks(cook_pool* pool, int32_t n_groups, const i
 
 namespace {
 
+// The round a match leaves for cook_state_match_metrics: its n rows' slots, copied device to device (no launch and no
+// transfer between host and device), the pending epoch and the plan's run.
+int32_t mm_record(cook_pool* pool, PoolState* S, const int32_t* m_slot, int n) {
+  MetricsRound& R = S->mm;
+  if (n > R.slot_cap) {
+    const int64_t cap = std::max<int64_t>(n, 2 * R.slot_cap);
+    if (R.slot) cudaFree(R.slot);
+    R.slot = nullptr;
+    R.slot_cap = 0;
+    CK(pool, cudaMalloc(&R.slot, sizeof(int32_t) * cap));
+    R.slot_cap = cap;
+  }
+  if (n) CK(pool, cudaMemcpyAsync(R.slot, m_slot, sizeof(int32_t) * n, cudaMemcpyDeviceToDevice, pool->stream));
+  R.n_rows = n;
+  R.epoch = S->pend_epoch;
+  R.run = match_runs(pool);
+  R.on = true;
+  R.counted = false;
+  return COOK_OK;
+}
+
 // cook_state_rank, and with `offensive` cook_state_rank_offensive: the jobs the rank drops as offensive, as job ids
 int32_t state_rank(cook_pool* pool, const char* who, bool offensive, const cook_user_table* users,
                    const cook_pool_quota* pool_quota, const cook_pool_quota* group_quota, const double* group_usage,
@@ -2369,7 +2428,8 @@ int32_t state_match(cook_pool* pool, const char* who, bool derived, const cook_o
     n_codes = op->n_codes;
     if (n == 0) pool->phase[COOK_PHASE_MATCH] = {};   // this call's own removals are all it reports
   }
-  if (n == 0) return COOK_OK;
+  S->mm.on = false;
+  if (n == 0) return mm_record(pool, S, nullptr, 0);
   // ---- what the rows hold, from the host-side counts: the resident columns of the kinds some live row
   // holds a non-absent value of
   JobShape sh;
@@ -2419,6 +2479,8 @@ int32_t state_match(cook_pool* pool, const char* who, bool derived, const cook_o
   }
   rc = match_run(pool, nullptr, out_considerable_job_id, out_assign, out_ports, out_fail_reason, out_stats, true,
                  params->max_ctas);
+  if (rc != COOK_OK) return rc;
+  rc = mm_record(pool, S, m_slot, n);
   if (rc != COOK_OK) return rc;
   cook_phase_stats& ps = pool->phase[COOK_PHASE_MATCH];
   ps.n_launches += nl;
@@ -5446,4 +5508,513 @@ extern "C" int32_t cook_state_export(cook_pool* pool, int32_t n_buckets, const u
 extern "C" int32_t cook_state_queue(cook_pool* pool, int32_t cap, int64_t* out_job_id, int32_t* out_n) {
   if (!pool) return COOK_E_BADARG;
   return live_queue(pool, static_cast<PoolState*>(pool->state), cap, out_job_id, out_n);
+}
+
+// ---- match-cycle metrics (handle-match-cycle-metrics scheduler.clj:1210-1280 and the unmatched tracking :1399-1486)
+// over the last resident match round: the considerable rows gathered in take order with their job facts; per user
+// integer counts; cpus and mem folded in take order and sorted by (value, position) for the nearest-rank percentiles,
+// the last position of each order being the last maximal row; the keyed totals' entries sorted by (kind, code,
+// position) and folded per key; the unmatched cycles looked up by job id in the last counted round's sorted pairs.
+namespace {
+
+enum { MM_GPUS = 0, MM_DISK_REQ = 1, MM_DISK_LIM = 2, MM_KINDS = 3 };
+constexpr int MM_FIRST = COOK_MM_FIRST_N;
+// the result block the device writes and the call downloads in one copy, then spreads over the caller's arrays
+struct MMRow {
+  int64_t job_id; int32_t position, user; double cpus, mem, gpus; int32_t ports, facts, gpu_model, disk_type;
+  double disk_request, disk_limit;
+};
+struct MMOut {
+  int32_t n_considerable, n_matched; int64_t head_job_id; int32_t head_matched, n_uris, uris_position, n_keys;
+  double total_cpus, total_mem, pct_cpus[3], pct_mem[3];
+  MMRow row[COOK_MM_ROWS];
+  int32_t n_too_long, n_first; int64_t first_job_id[MM_FIRST]; int32_t first_cycles[MM_FIRST];
+};
+static_assert(sizeof(MMOut) == 440, "the result block's size is part of the transfer formula");
+// cnt: [0] matched after the drops, [1] rows with uris, [2] 1 + the position of one of them, [3] keys, [4] rows unmatched
+// too long, [5] key entries, [6] unmatched rows, [7] a dropped position that holds no assignment
+enum { MMC_MATCHED, MMC_URIS, MMC_URI_POS, MMC_KEYS, MMC_TOO_LONG, MMC_ENTRIES, MMC_UNMATCHED, MMC_BAD, MMC_N };
+
+struct MMCols {   // row k: the k-th considerable job
+  int32_t* slot; int32_t* user; int64_t* jid; double* cpus; double* mem; double* gpus; int32_t* ports; uint8_t* jf;
+  int32_t* gmodel; int32_t* dtype; double* dreq; double* dlim; uint8_t* matched; int32_t* cyc;
+};
+
+__global__ void mm_gather_kernel(void* const* col, const int32_t* rslot, const int32_t* cons, const int32_t* assign,
+                                 int N, MMCols r) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= N) return;
+  const int s = rslot[cons[k]];
+  const uint8_t jf = static_cast<const uint8_t*>(col[P_JF])[s];
+  r.slot[k] = s;
+  r.user[k] = static_cast<const int32_t*>(col[P_USER])[s];
+  r.jid[k] = static_cast<const int64_t*>(col[P_JID])[s];
+  r.cpus[k] = static_cast<const double*>(col[P_CPUS])[s];
+  r.mem[k] = static_cast<const double*>(col[P_MEM])[s];
+  r.gpus[k] = static_cast<const double*>(col[P_GPUS])[s];
+  r.ports[k] = static_cast<const int32_t*>(col[P_PORTS])[s];
+  r.jf[k] = jf;
+  r.gmodel[k] = jf & COOK_JF_GPUS ? static_cast<const int32_t*>(col[P_JF_GPU])[s] : -1;
+  r.dtype[k] = jf & COOK_JF_DISK ? static_cast<const int32_t*>(col[P_JF_DTYPE])[s] : -1;
+  r.dreq[k] = jf & COOK_JF_DISK_REQUEST ? static_cast<const double*>(col[P_JF_DREQ])[s] : 0.0;
+  r.dlim[k] = jf & COOK_JF_DISK_LIMIT ? static_cast<const double*>(col[P_JF_DLIM])[s] : 0.0;
+  r.matched[k] = assign[k] >= 0;
+}
+
+// the launch-rate filter's drops: their jobs count as unmatched; one that holds no assignment sets the flag
+__global__ void mm_drop_kernel(const int32_t* dropped, int D, const int32_t* assign, uint8_t* matched, int32_t* bad) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= D) return;
+  const int k = dropped[i];
+  if (assign[k] < 0) atomicOr(bad, 1);
+  matched[k] = 0;
+}
+
+// per row: its user's counts (a code >= U is skipped: the round is then refused), the matched and uris counts, and its
+// unmatched cycles: 0 when matched, else 1 + its cycles in the last counted round (u_jid ascending, u_n pairs)
+__global__ void mm_count_kernel(MMCols r, int N, int U, const int64_t* u_jid, const int32_t* u_cyc, int u_n,
+                                int32_t* ucons, int32_t* umat, int32_t* cnt) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  const unsigned act = __ballot_sync(FULL_MASK, k < N);
+  if (k >= N) return;
+  const int lane = threadIdx.x & 31;
+  const int u = r.user[k];
+  const bool m = r.matched[k];
+  const unsigned same = __match_any_sync(act, u);
+  const unsigned same_m = same & __ballot_sync(act, m);
+  if (u < U) {
+    if (lane == __ffs(same) - 1) atomicAdd(&ucons[u], __popc(same));
+    if (m && lane == __ffs(same_m) - 1) atomicAdd(&umat[u], __popc(same_m));
+  }
+  const unsigned mm = __ballot_sync(act, m);
+  if (lane == __ffs(act) - 1 && mm) atomicAdd(&cnt[MMC_MATCHED], __popc(mm));
+  if (r.jf[k] & COOK_JF_URIS) {
+    atomicAdd(&cnt[MMC_URIS], 1);
+    atomicMax(&cnt[MMC_URI_POS], k + 1);
+  }
+  int c = 0;
+  if (!m) {
+    const int64_t j = r.jid[k];
+    int lo = 0, hi = u_n;
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (u_jid[mid] < j) lo = mid + 1;
+      else hi = mid;
+    }
+    c = 1 + (lo < u_n && u_jid[lo] == j ? u_cyc[lo] : 0);
+  }
+  r.cyc[k] = c;
+}
+
+// entry e = kind * N + k: row k's key of that kind, when the row carries it
+struct MMKey {
+  const uint8_t* jf; const int32_t* gmodel; const int32_t* dtype; const double* dreq; const double* dlim; int N;
+  __device__ int kind(int e) const { return e / N; }
+  __device__ int row(int e) const { return e - (e / N) * N; }
+  __device__ int code(int e) const { return kind(e) == MM_GPUS ? gmodel[row(e)] : dtype[row(e)]; }
+  __device__ double value(int e, const double* gpus) const {
+    const int t = kind(e), k = row(e);
+    return t == MM_GPUS ? gpus[k] : t == MM_DISK_REQ ? dreq[k] : dlim[k];
+  }
+  __device__ bool present(int e) const {
+    const int t = kind(e);
+    return jf[row(e)] & (t == MM_GPUS ? COOK_JF_GPUS : t == MM_DISK_REQ ? COOK_JF_DISK_REQUEST : COOK_JF_DISK_LIMIT);
+  }
+  __device__ bool same(int a, int b) const { return kind(a) == kind(b) && code(a) == code(b); }
+};
+struct MMEntries {
+  MMKey key; int32_t* ent;
+  __device__ bool keep(int e) const { return key.present(e); }
+  __device__ void emit(int e, int d) const { ent[d] = e; }
+};
+struct LessKindCodePos {   // (kind, code, position): each key's entries in take order
+  MMKey key; const int32_t* ent;
+  __device__ bool operator()(int32_t a, int32_t b) const {
+    const int ea = ent[a], eb = ent[b];
+    const int ka = key.kind(ea), kb = key.kind(eb);
+    if (ka != kb) return ka < kb;
+    const int ca = key.code(ea), cb = key.code(eb);
+    if (ca != cb) return ca < cb;
+    return key.row(ea) < key.row(eb);
+  }
+};
+struct MMSegEnds {   // end[d] = one past key d's last position in the sorted entries
+  MMKey key; const int32_t* ent; const int32_t* ord; const int32_t* n; int32_t* end;
+  __device__ bool keep(int p) const { return p == *n - 1 || !key.same(ent[ord[p]], ent[ord[p + 1]]); }
+  __device__ void emit(int p, int d) const { end[d] = p + 1; }
+};
+// warp per key: the left fold of its entries' values in take order, on the grid or by the serial chain
+__global__ void __launch_bounds__(128) mm_key_fold_kernel(MMKey key, const double* gpus, const int32_t* ent,
+                                                          const int32_t* ord, const int32_t* end, const int32_t* n_keys,
+                                                          const GridFlag* gf, int32_t* o_kind, int32_t* o_code,
+                                                          double* o_total) {
+  __shared__ double stage[4][1][32];
+  const int n = *n_keys, nw = gridDim.x * (blockDim.x >> 5);
+  for (int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; g < n; g += nw) {
+    const int s = g ? end[g - 1] : 0, e = end[g];
+    double acc[1] = {0.0};
+    warp_fold_sum<1, 4>(acc, e - s, grid_exact(gf, e - s), [&](int i, double (&x)[1]) {
+      x[0] = key.value(ent[ord[s + i]], gpus);
+      return true;
+    }, stage[threadIdx.x >> 5]);
+    if (threadIdx.x & 31) continue;
+    const int e0 = ent[ord[s]];
+    o_kind[g] = key.kind(e0);
+    o_code[g] = key.code(e0);
+    o_total[g] = acc[0];
+  }
+}
+
+struct LessValuePos {   // (value, position): no amount is NaN, and -0.0 and 0.0 compare equal as in Clojure's compare
+  const double* v;
+  __device__ bool operator()(int32_t a, int32_t b) const { return v[a] != v[b] ? v[a] < v[b] : a < b; }
+};
+struct MMTooLong {   // rows unmatched for more than thr cycles, in take order: the first MM_FIRST recorded
+  const int32_t* cyc; const int64_t* jid; int thr; int64_t* f_jid; int32_t* f_cyc;
+  __device__ bool keep(int k) const { return cyc[k] > thr; }
+  __device__ void emit(int k, int d) const {
+    if (d < MM_FIRST) { f_jid[d] = jid[k]; f_cyc[d] = cyc[k]; }
+  }
+};
+struct MMUnmatched {   // the unmatched rows' (job id, cycles), in take order
+  const int32_t* cyc; const int64_t* jid; int64_t* o_jid; int32_t* o_cyc;
+  __device__ bool keep(int k) const { return cyc[k] > 0; }
+  __device__ void emit(int k, int d) const { o_jid[d] = jid[k]; o_cyc[d] = cyc[k]; }
+};
+struct LessJid {
+  const int64_t* jid;
+  __device__ bool operator()(int32_t a, int32_t b) const { return jid[a] < jid[b]; }
+};
+__global__ void mm_map_kernel(const int32_t* ord, int n, const int64_t* jid, const int32_t* cyc, int64_t* o_jid,
+                              int32_t* o_cyc) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  o_jid[i] = jid[ord[i]];
+  o_cyc[i] = cyc[ord[i]];
+}
+
+__device__ void mm_row(const MMCols& r, int k, MMRow* o) {
+  o->job_id = r.jid[k]; o->position = k; o->user = r.user[k];
+  o->cpus = r.cpus[k]; o->mem = r.mem[k]; o->gpus = r.gpus[k]; o->ports = r.ports[k]; o->facts = r.jf[k];
+  o->gpu_model = r.gmodel[k]; o->disk_type = r.dtype[k]; o->disk_request = r.dreq[k]; o->disk_limit = r.dlim[k];
+}
+// one warp: the cpus and mem totals (left folds in take order), then lane 0 writes the result block
+__global__ void __launch_bounds__(32) mm_finish_kernel(MMCols r, int N, const GridFlag* gf, const int32_t* ord_c,
+                                                       const int32_t* ord_m, const int32_t* cnt, const int64_t* f_jid,
+                                                       const int32_t* f_cyc, MMOut* o) {
+  __shared__ double stage[1][2][32];
+  double acc[2] = {0.0, 0.0};
+  warp_fold_sum<2, 4>(acc, N, grid_exact(gf, N), [&](int k, double (&x)[2]) {
+    x[0] = r.cpus[k]; x[1] = r.mem[k];
+    return true;
+  }, stage[0]);
+  if (threadIdx.x) return;
+  o->n_considerable = N;
+  o->n_matched = cnt[MMC_MATCHED];
+  o->head_job_id = r.jid[0];
+  o->head_matched = r.matched[0];
+  o->n_uris = cnt[MMC_URIS];
+  o->uris_position = cnt[MMC_URIS] == 1 ? cnt[MMC_URI_POS] - 1 : -1;
+  o->n_keys = cnt[MMC_KEYS];
+  o->total_cpus = acc[0];
+  o->total_mem = acc[1];
+  const int pcts[3] = {50, 95, 100};
+  for (int j = 0; j < 3; j++) {
+    const int p = (int)(((int64_t)pcts[j] * N + 99) / 100) - 1;
+    o->pct_cpus[j] = r.cpus[ord_c[p]];
+    o->pct_mem[j] = r.mem[ord_m[p]];
+  }
+  mm_row(r, 0, &o->row[COOK_MM_HEAD]);
+  mm_row(r, ord_c[N - 1], &o->row[COOK_MM_LARGEST_CPUS]);
+  mm_row(r, ord_m[N - 1], &o->row[COOK_MM_LARGEST_MEM]);
+  o->n_too_long = cnt[MMC_TOO_LONG];
+  o->n_first = min(cnt[MMC_TOO_LONG], MM_FIRST);
+  for (int i = 0; i < MM_FIRST; i++) {
+    o->first_job_id[i] = i < o->n_first ? f_jid[i] : -1;
+    o->first_cycles[i] = i < o->n_first ? f_cyc[i] : 0;
+  }
+}
+
+// capacity for n pairs in both halves of the counters, the current half's u_n pairs kept
+int32_t mm_counters_room(cook_pool* pool, MetricsRound& R, int64_t n, cudaStream_t st) {
+  if (n <= R.u_cap) return COOK_OK;
+  const int64_t cap = std::max<int64_t>(n, 2 * R.u_cap);
+  int64_t* j[2] = {};
+  int32_t* c[2] = {};
+  cudaError_t e = cudaSuccess;
+  for (int h = 0; h < 2 && e == cudaSuccess; h++) {
+    e = cudaMalloc(&j[h], sizeof(int64_t) * cap);
+    if (e == cudaSuccess) e = cudaMalloc(&c[h], sizeof(int32_t) * cap);
+  }
+  if (e == cudaSuccess && R.u_n) e = cudaMemcpyAsync(j[0], R.u_jid[R.cur], sizeof(int64_t) * R.u_n, cudaMemcpyDeviceToDevice, st);
+  if (e == cudaSuccess && R.u_n) e = cudaMemcpyAsync(c[0], R.u_cyc[R.cur], sizeof(int32_t) * R.u_n, cudaMemcpyDeviceToDevice, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (e != cudaSuccess) {
+    for (void* p : {(void*)j[0], (void*)j[1], (void*)c[0], (void*)c[1]}) if (p) cudaFree(p);
+    return set_err(pool, COOK_E_OOM, "cook_state_match_metrics: out of device memory");
+  }
+  for (int h = 0; h < 2; h++) {
+    if (R.u_jid[h]) cudaFree(R.u_jid[h]);
+    if (R.u_cyc[h]) cudaFree(R.u_cyc[h]);
+    R.u_jid[h] = j[h];
+    R.u_cyc[h] = c[h];
+  }
+  R.cur = 0;
+  R.u_cap = cap;
+  return COOK_OK;
+}
+
+int32_t job_facts(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, const uint8_t* flags,
+                  const int32_t* gpu_model, const double* disk_request, const double* disk_limit,
+                  const int32_t* disk_type) {
+  const char* who = "cook_state_job_facts";
+  if (n < 0) return set_err(pool, COOK_E_BADARG, "%s: n < 0", who);
+  if (n && !job_id) return set_err(pool, COOK_E_BADARG, "%s: null job_id", who);
+  const int all = COOK_JF_GPUS | COOK_JF_DISK | COOK_JF_DISK_REQUEST | COOK_JF_DISK_LIMIT | COOK_JF_URIS;
+  for (int i = 0; flags && i < n; i++) {
+    if (flags[i] & ~all) return set_err(pool, COOK_E_BADARG, "%s: an unknown flag bit", who);
+    if ((flags[i] & (COOK_JF_DISK_REQUEST | COOK_JF_DISK_LIMIT)) && !(flags[i] & COOK_JF_DISK))
+      return set_err(pool, COOK_E_BADARG, "%s: a disk request or limit without the disk flag", who);
+  }
+  if (!idx_in_range(gpu_model, n, -1, INT32_MAX) || !idx_in_range(disk_type, n, -1, INT32_MAX))
+    return set_err(pool, COOK_E_BADARG, "%s: a gpu model or disk type code below -1", who);
+  for (const double* v : {disk_request, disk_limit})
+    for (int i = 0; v && i < n; i++)
+      if (std::isnan(v[i])) return set_err(pool, COOK_E_BADARG, "%s: a NaN disk amount", who);
+  std::vector<int32_t> slot;
+  if (const char* why = pending_slots(S, n, job_id, &slot)) return set_err(pool, COOK_E_BADARG, "%s: %s", who, why);
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  // ---- host side: the rows' bits, for the count of rows with a keyed resource
+  for (int i = 0; flags && i < n; i++) {
+    PendingInfo& pi = S->pinfo[slot[i]];
+    S->jf_keyed -= (pi.jf & (COOK_JF_GPUS | COOK_JF_DISK)) ? 1 : 0;
+    pi.jf = flags[i];
+    S->jf_keyed += (pi.jf & (COOK_JF_GPUS | COOK_JF_DISK)) ? 1 : 0;
+  }
+  // ---- device: a patch scatter (live flag and generation kept)
+  const bool cols = n && (flags || gpu_model || disk_request || disk_limit || disk_type);
+  ScatterArgs pa;
+  memset(&pa, 0, sizeof(pa));
+  int64_t h2d = 0;
+  CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
+    if (!cols) return;
+    pa.slot = c.up(slot.data(), n);
+    const auto col = [&](int k, const char* src) {
+      pa.c[pa.nc++] = ScatterCol{static_cast<char*>(S->pend.col[k]), src, 0, P_SZ[k]};
+    };
+    if (flags) col(P_JF, reinterpret_cast<const char*>(c.up(flags, n)));
+    if (gpu_model) col(P_JF_GPU, reinterpret_cast<const char*>(c.up(gpu_model, n)));
+    if (disk_request) col(P_JF_DREQ, reinterpret_cast<const char*>(c.up(disk_request, n)));
+    if (disk_limit) col(P_JF_DLIM, reinterpret_cast<const char*>(c.up(disk_limit, n)));
+    if (disk_type) col(P_JF_DTYPE, reinterpret_cast<const char*>(c.up(disk_type, n)));
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  int nl = 0;
+  scatter(pa, S->pend, cols ? n : 0, 0, -1, nullptr, st, &nl);
+  CK(pool, cudaGetLastError());
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  CK(pool, cudaStreamSynchronize(st));
+  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
+  return COOK_OK;
+}
+
+// The caller's arrays of cook_state_match_metrics
+struct MMArrays {
+  int64_t* counts; double* amounts; int64_t* row_int; double* row_amount; int64_t* first_jid; int32_t* first_cyc;
+  int32_t* ucons; int32_t* umat; int32_t* kind; int32_t* code; double* total;
+  void put(const MMOut& o) const {
+    const int64_t c[COOK_MMC_N] = {o.n_considerable, o.n_matched, o.head_job_id, o.head_matched, o.n_uris,
+                                   o.uris_position, o.n_keys, o.n_too_long, o.n_first};
+    std::copy(c, c + COOK_MMC_N, counts);
+    const double a[COOK_MMA_N] = {o.total_cpus, o.total_mem, o.pct_cpus[0], o.pct_cpus[1], o.pct_cpus[2],
+                                  o.pct_mem[0], o.pct_mem[1], o.pct_mem[2]};
+    std::copy(a, a + COOK_MMA_N, amounts);
+    for (int r = 0; r < COOK_MM_ROWS; r++) {
+      const MMRow& w = o.row[r];
+      const int64_t ri[COOK_MMR_NI] = {w.job_id, w.position, w.user, w.ports, w.facts, w.gpu_model, w.disk_type};
+      const double ra[COOK_MMR_NF] = {w.cpus, w.mem, w.gpus, w.disk_request, w.disk_limit};
+      std::copy(ri, ri + COOK_MMR_NI, row_int + COOK_MMR_NI * r);
+      std::copy(ra, ra + COOK_MMR_NF, row_amount + COOK_MMR_NF * r);
+    }
+    std::copy(o.first_job_id, o.first_job_id + MM_FIRST, first_jid);
+    std::copy(o.first_cycles, o.first_cycles + MM_FIRST, first_cyc);
+  }
+};
+
+int32_t match_metrics(cook_pool* pool, PoolState* S, int32_t U, int32_t D, const int32_t* dropped, int32_t thr,
+                      int32_t key_cap, const MMArrays& out, cook_phase_stats* out_stats) {
+  const char* who = "cook_state_match_metrics";
+  int32_t *out_ucons = out.ucons, *out_umat = out.umat, *out_kind = out.kind, *out_code = out.code;
+  double* out_total = out.total;
+  // ---- every check the host can make, before any device work
+  if (!out.counts || !out.amounts || !out.row_int || !out.row_amount || !out.first_jid || !out.first_cyc || !out_ucons || !out_umat || !out_kind || !out_code || !out_total)
+    return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
+  if (U <= 0 || D < 0 || thr < 0 || key_cap < 0 || (D && !dropped))
+    return set_err(pool, COOK_E_BADARG, "%s: bad sizes or threshold", who);
+  if (!S || !S->mm.on) return set_err(pool, COOK_E_BADARG, "%s: no resident match round on this handle", who);
+  MetricsRound& R = S->mm;
+  if (R.counted) return set_err(pool, COOK_E_BADARG, "%s: the round has already been counted", who);
+  int32_t N = 0;
+  const int32_t *cons = nullptr, *assign = nullptr;
+  if (R.n_rows > 0 && !match_round(pool, R.run, &N, &cons, &assign))
+    return set_err(pool, COOK_E_BADARG, "%s: no resident match round on this handle (a later match ran)", who);
+  if (count_max(S->users_p) >= U) return set_err(pool, COOK_E_BADARG, "%s: a pending row's user code is >= n_users", who);
+  {
+    std::vector<uint8_t> seen(N, 0);
+    for (int i = 0; i < D; i++) {
+      if (dropped[i] < 0 || dropped[i] >= N) return set_err(pool, COOK_E_BADARG, "%s: a dropped position out of range", who);
+      if (seen[dropped[i]]++) return set_err(pool, COOK_E_BADARG, "%s: a dropped position twice", who);
+    }
+  }
+  if (out_stats) *out_stats = cook_phase_stats{};
+  if (N == 0) {   // an empty round: the counts, the counters zeroed, no device work
+    std::fill(out.counts, out.counts + COOK_MMC_N, 0);
+    out.counts[COOK_MMC_HEAD_JOB_ID] = out.counts[COOK_MMC_URIS_POSITION] = -1;
+    R.u_n = 0;
+    R.counted = true;
+    return COOK_OK;
+  }
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  if (int32_t rc = mm_counters_room(pool, R, N, st)) return rc;
+  const bool changed = S->pend_epoch != R.epoch;
+  const bool keyed = S->jf_keyed > 0;
+  const int E = keyed ? 3 * N : 0;
+  // ---- one carve: the rows, the orders, the entries, the counters' new pairs, the result block; up the drops
+  MMCols r = {};
+  int32_t *cnt = nullptr, *blk = nullptr, *ucons = nullptr, *umat = nullptr, *ord_c = nullptr, *ord_m = nullptr,
+          *tmp = nullptr, *ent = nullptr, *ord_e = nullptr, *end = nullptr, *o_kind = nullptr, *o_code = nullptr,
+          *f_cyc = nullptr, *n_cyc = nullptr, *ord_u = nullptr;
+  const int32_t* d_drop = nullptr;
+  int64_t *f_jid = nullptr, *n_jid = nullptr;
+  double* o_total = nullptr;
+  GridFlag* gf = nullptr;
+  MMOut* d_out = nullptr;
+  int64_t h2d = 0, d2h = 0;
+  CK(pool, carve(S->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+    r.slot = c.take<int32_t>(N); r.user = c.take<int32_t>(N); r.jid = c.take<int64_t>(N);
+    r.cpus = c.take<double>(N); r.mem = c.take<double>(N); r.gpus = c.take<double>(N); r.ports = c.take<int32_t>(N);
+    r.jf = c.take<uint8_t>(N); r.gmodel = c.take<int32_t>(N); r.dtype = c.take<int32_t>(N);
+    r.dreq = c.take<double>(N); r.dlim = c.take<double>(N); r.matched = c.take<uint8_t>(N); r.cyc = c.take<int32_t>(N);
+    cnt = c.take<int32_t>(MMC_N);
+    blk = c.take<int32_t>((size_t)std::max(N, E) / CP_BLOCK + 2);
+    ucons = c.take<int32_t>(U); umat = c.take<int32_t>(U);
+    ord_c = c.take<int32_t>(N); ord_m = c.take<int32_t>(N); tmp = c.take<int32_t>(std::max(N, E));
+    if (keyed) {
+      ent = c.take<int32_t>(E); ord_e = c.take<int32_t>(E); end = c.take<int32_t>(E);
+      o_kind = c.take<int32_t>(E); o_code = c.take<int32_t>(E); o_total = c.take<double>(E);
+    }
+    f_jid = c.take<int64_t>(MM_FIRST); f_cyc = c.take<int32_t>(MM_FIRST);
+    n_jid = c.take<int64_t>(N); n_cyc = c.take<int32_t>(N); ord_u = c.take<int32_t>(N);
+    gf = c.take<GridFlag>(2);
+    d_out = c.take<MMOut>(1);
+    d_drop = c.up(D ? dropped : nullptr, D);
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  CK(pool, cudaMemsetAsync(cnt, 0, sizeof(int32_t) * MMC_N, st));
+  CK(pool, cudaMemsetAsync(ucons, 0, sizeof(int32_t) * U, st));
+  CK(pool, cudaMemsetAsync(umat, 0, sizeof(int32_t) * U, st));
+  CK(pool, cudaMemsetAsync(gf, 0, sizeof(GridFlag) * 2, st));
+  int nl = 0;
+  // ---- the rows, the drops, the counts and cycles, the entries; the first-ten and the new pairs in take order
+  mm_gather_kernel<<<(N + 255) / 256, 256, 0, st>>>(S->pend.d_col, R.slot, cons, assign, N, r);
+  nl++;
+  if (D) {
+    mm_drop_kernel<<<(D + 255) / 256, 256, 0, st>>>(d_drop, D, assign, r.matched, cnt + MMC_BAD);
+    nl++;
+  }
+  mm_count_kernel<<<(N + 255) / 256, 256, 0, st>>>(r, N, U, R.u_jid[R.cur], R.u_cyc[R.cur], R.u_n, ucons, umat, cnt);
+  grid_check_kernel<<<(N + 255) / 256, 256, 0, st>>>(r.cpus, r.mem, nullptr, N, gf);
+  nl += 2;
+  const MMKey key{r.jf, r.gmodel, r.dtype, r.dreq, r.dlim, N};
+  if (keyed) {
+    grid_check_kernel<<<(N + 255) / 256, 256, 0, st>>>(r.gpus, r.dreq, r.dlim, N, gf + 1);
+    nl++;
+    compact(MMEntries{key, ent}, E, nullptr, blk, cnt + MMC_ENTRIES, E, st, &nl);
+  }
+  compact(MMTooLong{r.cyc, r.jid, thr, f_jid, f_cyc}, N, nullptr, blk, cnt + MMC_TOO_LONG, N, st, &nl);
+  compact(MMUnmatched{r.cyc, r.jid, n_jid, n_cyc}, N, nullptr, blk, cnt + MMC_UNMATCHED, N, st, &nl);
+  CK(pool, cudaGetLastError());
+  int32_t c0[MMC_N];
+  std::vector<int32_t> slots(changed ? N : 0);
+  CK(pool, download(c0, cnt, MMC_N, st, &d2h));
+  if (changed) CK(pool, download(slots.data(), r.slot, N, st, &d2h));
+  CK(pool, cudaStreamSynchronize(st));
+  // ---- the checks only the device could make, before anything is written
+  if (c0[MMC_BAD]) return set_err(pool, COOK_E_BADARG, "%s: a dropped position holds no assignment", who);
+  for (int k = 0; k < (int)slots.size(); k++)
+    if (S->pinfo[slots[k]].touched > R.epoch)
+      return set_err(pool, COOK_E_BADARG, "%s: a considerable row changed since the match", who);
+  // ---- the orders, the keyed totals, the counters' new pairs by job id, the result block
+  CK(pool, csort::sort_indices(ord_c, tmp, N, LessValuePos{r.cpus}, st, &nl));
+  CK(pool, csort::sort_indices(ord_m, tmp, N, LessValuePos{r.mem}, st, &nl));
+  const int ne = c0[MMC_ENTRIES], nu = c0[MMC_UNMATCHED];
+  if (ne) {
+    CK(pool, csort::sort_indices(ord_e, tmp, ne, LessKindCodePos{key, ent}, st, &nl));
+    compact(MMSegEnds{key, ent, ord_e, cnt + MMC_ENTRIES, end}, ne, nullptr, blk, cnt + MMC_KEYS, ne, st, &nl);
+    mm_key_fold_kernel<<<std::min((ne + 3) / 4, 4096), 128, 0, st>>>(key, r.gpus, ent, ord_e, end, cnt + MMC_KEYS, gf + 1,
+                                                                     o_kind, o_code, o_total);
+    nl++;
+  }
+  const int nxt = 1 - R.cur;
+  if (nu) {
+    CK(pool, csort::sort_indices(ord_u, tmp, nu, LessJid{n_jid}, st, &nl));
+    mm_map_kernel<<<(nu + 255) / 256, 256, 0, st>>>(ord_u, nu, n_jid, n_cyc, R.u_jid[nxt], R.u_cyc[nxt]);
+    nl++;
+  }
+  mm_finish_kernel<<<1, 32, 0, st>>>(r, N, gf, ord_c, ord_m, cnt, f_jid, f_cyc, d_out);
+  nl++;
+  CK(pool, cudaGetLastError());
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  MMOut res;
+  CK(pool, download(&res, d_out, 1, st, &d2h));
+  CK(pool, cudaStreamSynchronize(st));
+  if (res.n_keys > key_cap) {
+    out.counts[COOK_MMC_KEYS] = res.n_keys;
+    return set_err(pool, COOK_E_TOO_LARGE, "%s: more keys than key_cap: %d", who, res.n_keys);
+  }
+  CK(pool, download(out_ucons, ucons, U, st, &d2h));
+  CK(pool, download(out_umat, umat, U, st, &d2h));
+  if (res.n_keys) {
+    CK(pool, download(out_kind, o_kind, res.n_keys, st, &d2h));
+    CK(pool, download(out_code, o_code, res.n_keys, st, &d2h));
+    CK(pool, download(out_total, o_total, res.n_keys, st, &d2h));
+  }
+  CK(pool, cudaEventRecord(pool->ev[23], st));
+  CK(pool, cudaStreamSynchronize(st));
+  out.put(res);
+  R.cur = nxt;
+  R.u_n = nu;
+  R.counted = true;
+  if (out_stats)
+    *out_stats = {ev_ms(pool->ev[20], pool->ev[21]), ev_ms(pool->ev[21], pool->ev[22]), ev_ms(pool->ev[22], pool->ev[23]),
+                  h2d, d2h, nl, 0};
+  return COOK_OK;
+}
+
+}  // namespace
+
+extern "C" int32_t cook_state_job_facts(cook_pool* pool, int32_t n, const int64_t* job_id, const uint8_t* flags,
+                                        const int32_t* gpu_model, const double* disk_request, const double* disk_limit,
+                                        const int32_t* disk_type) {
+  if (!pool) return COOK_E_BADARG;
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_job_facts: out of device memory");
+  return job_facts(pool, S, n, job_id, flags, gpu_model, disk_request, disk_limit, disk_type);
+}
+
+extern "C" int32_t cook_state_match_metrics(cook_pool* pool, int32_t n_users, int32_t n_dropped, const int32_t* dropped,
+                                            int32_t unmatched_warn_cycles, int32_t key_cap, int64_t* out_counts,
+                                            double* out_amounts, int64_t* out_row_int, double* out_row_amount,
+                                            int64_t* out_first_job_id, int32_t* out_first_cycles,
+                                            int32_t* out_user_considerable, int32_t* out_user_matched,
+                                            int32_t* out_key_kind, int32_t* out_key_code, double* out_key_total,
+                                            cook_phase_stats* out_stats) {
+  if (!pool) return COOK_E_BADARG;
+  const MMArrays out{out_counts, out_amounts, out_row_int, out_row_amount, out_first_job_id, out_first_cycles,
+                     out_user_considerable, out_user_matched, out_key_kind, out_key_code, out_key_total};
+  return match_metrics(pool, static_cast<PoolState*>(pool->state), n_users, n_dropped, dropped, unmatched_warn_cycles,
+                       key_cap, out, out_stats);
 }

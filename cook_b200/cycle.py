@@ -24,6 +24,8 @@ path end to end.  It computes nothing numeric: every placement decision is `engi
   usage_response        the body of GET /usage (get-user-usage, api.clj:2946-2969) from cook_state_user_usage answers
   instance_stats_response  the body of GET /stats/instances (task-stats/get-stats) from a cook_state_instance_stats
                         answer
+  match_cycle_metrics_response  the match-cycle logs (handle-match-cycle-metrics) and the unmatched-too-long warning
+                        from a cook_state_match_metrics answer
 """
 import numpy as np
 
@@ -642,4 +644,109 @@ def instance_stats_response(answer, *, user_name=None, reason_string=None):
             out["by-user-and-reason"].setdefault(name_of(u), {})[key(r)] = stats(d)
     out["leaders"] = {"cpu-seconds": {name_of(u): t for u, t in answer["leaders_cpu"]},
                       "mem-seconds": {name_of(u): t for u, t in answer["leaders_mem"]}}
+    return out
+
+
+JOB_STATS_ERROR = "Error collecting job stats"   # what jobs->stats returns when it throws (scheduler.clj:594-602)
+
+
+def _mm_key(kind, code, gpu_model_name, disk_type_name):
+    """A keyed total's resource key as jobs->resource-maps (scheduler.clj:511-545) writes it."""
+    if kind == abi.MM_GPUS:
+        return "gpus/" + (gpu_model_name(code) if code >= 0 else "unspecified-gpu-model")
+    t = disk_type_name(code) if code >= 0 else "unspecified-disk-type"
+    return f"disk/{t}/" + ("request" if kind == abi.MM_DISK_REQUEST else "limit")
+
+
+def _mm_resource_map(row, gpu_model_name, disk_type_name, uris):
+    """job->resource-map of a cook_state_match_metrics row, formatted for structured logging (numbers stay numbers,
+    the uris vector becomes its string)."""
+    m = {"cpus": row["cpus"], "mem": row["mem"]}
+    f = row["facts"]
+    if f & abi.JF_GPUS:
+        m[_mm_key(abi.MM_GPUS, row["gpu_model"], gpu_model_name, disk_type_name)] = row["gpus"]
+    if f & abi.JF_DISK_REQUEST:
+        m[_mm_key(abi.MM_DISK_REQUEST, row["disk_type"], gpu_model_name, disk_type_name)] = row["disk_request"]
+    if f & abi.JF_DISK_LIMIT:
+        m[_mm_key(abi.MM_DISK_LIMIT, row["disk_type"], gpu_model_name, disk_type_name)] = row["disk_limit"]
+    if f & abi.JF_URIS:
+        m["uris"] = str(uris(row["job_id"]))
+    return m
+
+
+def _mm_head_resources(row, gpu_model_name, disk_type_name, uris):
+    """tools/job-ent->resources of the head (tools.clj:247-273): cpus, mem, ports, gpus when present, the disk map (the
+    type only when the job names one) and the uris."""
+    f = row["facts"]
+    out = {"ports": row["ports"], "cpus": row["cpus"], "mem": row["mem"]}
+    if f & abi.JF_GPUS:
+        out["gpus"] = row["gpus"]
+    if f & abi.JF_DISK:
+        d = {"request": row["disk_request"] if f & abi.JF_DISK_REQUEST else None}
+        if f & abi.JF_DISK_LIMIT:
+            d["limit"] = row["disk_limit"]
+        if row["disk_type"] >= 0:
+            d["type"] = disk_type_name(row["disk_type"])
+        out["disk"] = d
+    if f & abi.JF_URIS:
+        out["uris"] = uris(row["job_id"])
+    return out
+
+
+def match_cycle_metrics_response(answer, considerable_job_id, *, pool, max_considerable, n_offers, n_offers_scheduled,
+                                 offers_stats=None,
+                                 user_name=None, job_name=None, gpu_model_name=None, disk_type_name=None, uris=None,
+                                 unmatched_cycles_warn_threshold=500, unmatched_fraction_warn_threshold=0.5):
+    """What handle-match-cycle-metrics (scheduler.clj:1210-1280) and the unmatched tracking (:1399-1486) log, from an
+    engine.state_match_metrics answer, the round's considerable job ids (the match's output) and the host's
+    dictionaries (each maps a code to its name; default: the code).
+    Returns {"users": ["user match cycle metric" maps, in ascending user code], "total": the "total match cycle metric"
+    map, "warn": the "Jobs are unmatched for too long" map or None, "front": (cpus, mem) of the front-of-queue gauges}.
+    match-percent is a fractions.Fraction, as Clojure's ratio.  :stats :offers (offers->stats) is the host's
+    `offers_stats`; :jobs-considerable is the error string when two or more considerable jobs carry uris.  uris(job id)
+    gives a job's uri vector (the one row jobs->resource-maps keeps, and the head's)."""
+    from fractions import Fraction
+    name_of = user_name or (lambda u: u)
+    job_of = job_name or (lambda j: j)
+    gname = gpu_model_name or (lambda c: str(c))
+    dname = disk_type_name or (lambda c: str(c))
+    uris = uris or (lambda j: [])
+    n, nm = answer["considerable"], answer["matched"]
+    out = {"users": [], "warn": None, "front": (0, 0)}
+    if n == 0:   # the slim form of the zero-considerable case
+        out["total"] = {"inputs": {"jobs-considerable": 0}, "pool": pool}
+        return out
+    for u, (c, m) in enumerate(zip(answer["user_considerable"], answer["user_matched"])):
+        if c:
+            out["users"].append({"user": name_of(u), "pool": pool, "user-considerable": int(c),
+                                 "user-matched": int(m), "user-unmatched": int(c - m)})
+    head, lc, lm = answer["rows"]
+    if answer["uris"] >= 2:
+        jobs_stats = JOB_STATS_ERROR
+    else:
+        totals = {"cpus": answer["total_cpus"], "mem": answer["total_mem"]}
+        for kind, code, total in answer["keys"]:
+            totals[_mm_key(kind, code, gname, dname)] = total
+        if answer["uris"] == 1:
+            totals["uris"] = str(uris(int(considerable_job_id[answer["uris_position"]])))
+        jobs_stats = {"largest-by": {"cpus": _mm_resource_map(lc, gname, dname, uris),
+                                     "mem": _mm_resource_map(lm, gname, dname, uris)},
+                      "percentiles": {r: dict(zip((50, 95, 100), answer["pct_" + r])) for r in ("cpus", "mem")},
+                      "totals": totals}
+    out["total"] = {
+        "inputs": {"jobs-considerable": n, "offers": n_offers, "max-considerable": max_considerable,
+                   "queue-was-full": max_considerable == n},
+        "matched": {"jobs-considerable": nm, "offers": n_offers_scheduled, "match-percent": Fraction(nm, n),
+                    "head-was-matched": bool(answer["head_matched"])},
+        "pool": pool,
+        "unmatched": {"jobs-considerable": n - nm, "offers": n_offers - n_offers_scheduled},
+        "stats": {"jobs-considerable": jobs_stats, "offers": offers_stats,
+                  "head-resources": _mm_head_resources(head, gname, dname, uris)}}
+    out["front"] = (head["cpus"], head["mem"])
+    # the warning's fraction test: Clojure's (/ a n) ratio compared as a double with the threshold
+    if float(Fraction(answer["too_long"], n)) > unmatched_fraction_warn_threshold:
+        out["warn"] = {"pool": pool, "first-ten-unmatched-too-long": [(job_of(j), c) for j, c in answer["first"]],
+                       "number-considerable": n, "number-unmatched-too-long": answer["too_long"],
+                       "unmatched-cycles-warn-threshold": unmatched_cycles_warn_threshold,
+                       "unmatched-fraction-warn-threshold": unmatched_fraction_warn_threshold}
     return out

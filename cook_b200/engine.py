@@ -243,6 +243,64 @@ class GpuEngine:
         if rc != 0:
             self._err(rc)
 
+    def state_job_facts(self, job_id, flags=None, gpu_model=None, disk_request=None, disk_limit=None, disk_type=None):
+        """cook_state_job_facts: the stats keys of live pending jobs (None: unchanged): abi.JF_* bits, the gpu model
+        and disk type codes (-1: unspecified) and the disk request and limit, each read under its bit."""
+        jid = np.ascontiguousarray(job_id, np.int64)
+        cols = [np.ascontiguousarray(c, dt) if c is not None else None
+                for c, dt in ((flags, np.uint8), (gpu_model, np.int32), (disk_request, np.float64),
+                              (disk_limit, np.float64), (disk_type, np.int32))]
+        if any(c is not None and len(c) != len(jid) for c in cols):
+            raise ValueError("state_job_facts: a column's length differs from job_id's")
+        pt = (abi.P_U8, abi.P_I32, abi.P_F64, abi.P_F64, abi.P_I32)
+        rc = self.lib.cook_state_job_facts(self.pool, len(jid), abi.ptr(jid, abi.P_I64),
+                                           *[abi.ptr(c, t) if c is not None else None for c, t in zip(cols, pt)])
+        if rc != 0:
+            self._err(rc)
+
+    def state_match_metrics(self, n_users, dropped=(), unmatched_warn_cycles=500, key_cap=64):
+        """cook_state_match_metrics over the last resident match round: `dropped` are the considerable positions the
+        launch-rate filter dropped.  Returns the counts by their abi.MMC_* names in lower case ('considerable',
+        'matched', 'head_job_id', ...), 'total_cpus', 'total_mem', 'pct_cpus' and 'pct_mem' [50, 95, 100], 'rows'
+        (head, largest by cpus, largest by mem: dicts of abi.MMR_INT and abi.MMR_AMOUNT), 'first' [(job id, cycles)]
+        in take order, 'user_considerable' and 'user_matched' [n_users], 'keys' [(kind, code, total)] in ascending
+        (kind, code), and 'stats' (abi.PhaseStats.as_dict()).  The call is made with key_cap keys first and, when
+        more are needed, once more with the count it reports."""
+        drop = np.ascontiguousarray(dropped, np.int32)
+        U = int(n_users)
+        ucons, umat = np.zeros(max(U, 1), np.int32), np.zeros(max(U, 1), np.int32)
+        counts, amounts = np.zeros(abi.MMC_N, np.int64), np.zeros(abi.MMA_N)
+        row_i, row_a = np.zeros((abi.MM_ROWS, len(abi.MMR_INT)), np.int64), np.zeros((abi.MM_ROWS, len(abi.MMR_AMOUNT)))
+        fj, fc = np.zeros(abi.MM_FIRST_N, np.int64), np.zeros(abi.MM_FIRST_N, np.int32)
+        st = abi.PhaseStats()
+        cap = max(int(key_cap), 0)
+        for _ in range(2):
+            kind, code, total = np.zeros(max(cap, 1), np.int32), np.zeros(max(cap, 1), np.int32), np.zeros(max(cap, 1))
+            rc = self.lib.cook_state_match_metrics(
+                self.pool, U, len(drop), abi.ptr(drop, abi.P_I32) if len(drop) else None, int(unmatched_warn_cycles),
+                cap, abi.ptr(counts, abi.P_I64), abi.ptr(amounts, abi.P_F64), abi.ptr(row_i, abi.P_I64),
+                abi.ptr(row_a, abi.P_F64), abi.ptr(fj, abi.P_I64), abi.ptr(fc, abi.P_I32), abi.ptr(ucons, abi.P_I32),
+                abi.ptr(umat, abi.P_I32), abi.ptr(kind, abi.P_I32), abi.ptr(code, abi.P_I32), abi.ptr(total, abi.P_F64),
+                C.byref(st))
+            if rc != abi.COOK_E_TOO_LARGE or counts[abi.MMC_KEYS] <= cap:
+                break
+            cap = int(counts[abi.MMC_KEYS])
+        if rc != 0:
+            self._err(rc)
+        names = ("considerable", "matched", "head_job_id", "head_matched", "uris", "uris_position", "keys_n",
+                 "too_long", "first_n")
+        res = {n: int(counts[i]) for i, n in enumerate(names)}
+        res["total_cpus"], res["total_mem"] = float(amounts[abi.MMA_TOTAL_CPUS]), float(amounts[abi.MMA_TOTAL_MEM])
+        res["pct_cpus"] = amounts[abi.MMA_PCT_CPUS:abi.MMA_PCT_CPUS + 3].tolist()
+        res["pct_mem"] = amounts[abi.MMA_PCT_MEM:abi.MMA_PCT_MEM + 3].tolist()
+        res["rows"] = [dict(zip(abi.MMR_INT, map(int, row_i[r])), **dict(zip(abi.MMR_AMOUNT, map(float, row_a[r]))))
+                       for r in range(abi.MM_ROWS)] if res["considerable"] else []
+        res["first"] = list(zip(fj[:res["first_n"]].tolist(), fc[:res["first_n"]].tolist()))
+        res["keys"] = [(int(kind[i]), int(code[i]), float(total[i])) for i in range(res["keys_n"])]
+        res["user_considerable"], res["user_matched"] = ucons[:U].copy(), umat[:U].copy()
+        res["stats"] = st.as_dict()
+        return res
+
     def state_finish(self, task_id, end_time_ms=None, success=None):
         """cook_state_finish: the tasks leave as a removal delta would take them; each successful one leaves a runtime
         record per group of its list (success None: none succeeded)."""

@@ -1231,6 +1231,94 @@ int32_t cook_state_history_stats(cook_pool* const* pools, int32_t n_pools, int32
                                  double* out_leader_total, int32_t* out_n_seg, int32_t* out_n_leader,
                                  cook_phase_stats* out_stats);
 
+/* ------------------------------------------------- match-cycle metrics of resident pools */
+/* What handle-match-cycle-metrics (scheduler.clj:1210-1280) and the unmatched tracking (:1399-1486) read after each
+ * match, before the launches, computed from the resident rows of the last match round.
+ *
+ * Job facts: the keys jobs->resource-maps (:511-545) reads, which are not the matcher's columns (P_GPU_MODEL and the
+ * disk constraint carry pool and config defaults).  On live pending rows, by job id, in place like
+ * cook_state_task_facts (live flag and generation kept); a NULL column is left unchanged.
+ *   flags[i]         COOK_JF_* bits: GPUS the job has a gpus resource (an amount of 0.0 counts: `(if gpus ...)`), DISK
+ *                    a disk resource, DISK_REQUEST / DISK_LIMIT its request / limit is present (needs DISK), URIS at
+ *                    least one uri
+ *   gpu_model[i]     the code of the job's COOK_GPU_MODEL environment value, -1: unspecified-gpu-model
+ *   disk_request[i], disk_limit[i]   the amounts, read under their bits
+ *   disk_type[i]     the code of :resource.disk/type, -1: unspecified-disk-type
+ * The gpus amount is the row's gpus column.  Every pending upsert of cook_state_apply writes flags 0 (no facts).  The
+ * facts are not part of cook_state_digest or cook_state_export: after a resync the caller sends them again.
+ * COOK_E_BADARG, before any change: n < 0; a NULL job_id while n > 0; a job id that is not live or appears twice; an
+ * unknown flag bit, or DISK_REQUEST / DISK_LIMIT without DISK; a gpu model or disk type code below -1; a NaN amount.
+ * Uploads exactly, when n > 0 and some column is given: n * (4 + [flags] 1 + [gpu_model] 4 + [disk_request] 8 +
+ * [disk_limit] 8 + [disk_type] 4) bytes.  Statistics: cook_last_stats(COOK_PHASE_STATE).                       */
+enum { COOK_JF_GPUS = 1, COOK_JF_DISK = 2, COOK_JF_DISK_REQUEST = 4, COOK_JF_DISK_LIMIT = 8, COOK_JF_URIS = 16 };
+int32_t cook_state_job_facts(cook_pool* pool, int32_t n, const int64_t* job_id, const uint8_t* flags,
+                             const int32_t* gpu_model, const double* disk_request, const double* disk_limit,
+                             const int32_t* disk_type);
+
+/* The metrics of the last cook_state_match, cook_state_match_derived or cook_state_match_offers on the handle: its
+ * considerable jobs in take order and their assignments.  dropped[n_dropped]: the considerable positions whose
+ * matches the launch-rate filter dropped (filter-matches-for-ratelimit :887-924); they count as unmatched.
+ *   Counts      out_counts[COOK_MMC_*]: considerable, matched (after the drops), the head's job id (-1: none), whether
+ *               the head is matched, the rows with a uri, that row's position when there is exactly one (else -1),
+ *               the keyed totals, the rows unmatched too long, the first ones listed (at most 10).
+ *   Per user    out_user_considerable[u], out_user_matched[u] for u < n_users (unmatched = the difference).
+ *   cpus, mem   out_amounts[COOK_MMA_*]: totals, left folds in take order (the exact grid or the serial chain,
+ *               DESIGN.md §2); percentiles 50, 95, 100: element ceil(p * n / 100) - 1 of the ascending values
+ *               (task_stats.clj's exact p/100); the largest rows: the LAST row of maximal value in take order (sort-by
+ *               is stable and `last` takes the last).
+ *   Keyed       one total per (kind, code) some considerable row carries, kind COOK_MM_GPUS (code: gpu model),
+ *               COOK_MM_DISK_REQUEST or COOK_MM_DISK_LIMIT (code: disk type), -1 being the unspecified value, in
+ *               ascending (kind, code): the left fold in take order of the rows that carry the key (merge-with +).
+ *               More keys than key_cap: only out_counts[COOK_MMC_KEYS] is written, COOK_E_TOO_LARGE, the round stays uncounted,
+ *               so the caller can retry with a larger cap.
+ *   Rows        the head, the largest by cpus and the largest by mem (COOK_MM_HEAD, _LARGEST_CPUS, _LARGEST_MEM): row r's
+ *               integers in out_row_int[COOK_MMR_NI * r + COOK_MMR_*] (job id, position, user, ports, COOK_JF_* facts,
+ *               gpu model, disk type; -1: unspecified) and its amounts in out_row_amount[COOK_MMR_NF * r + COOK_MMR_*]
+ *               (cpus, mem, gpus, disk request, disk limit; an absent disk amount is 0.0): :head-resources and
+ *               :largest-by without a job-entity read, except for the uri strings.
+ *   Uris        with two or more such rows, jobs->stats is "Error collecting job stats" (merge-with + adds two
+ *               vectors and throws); with one, its resource map keeps :uris.
+ *   Unmatched   every job has a cycle count, keyed by job id: after the call it is the previous count + 1 for a
+ *               considerable job that is unmatched (dropped ones included) and 0 for every other job, as the
+ *               reference's map rebuilt each cycle.  The counts live on the device as the last counted round's
+ *               unmatched (job id, count) pairs, so an upsert of a pending id, or its removal and return, keeps its
+ *               count.  COOK_MMC_TOO_LONG counts the rows with count > unmatched_warn_cycles (strictly);
+ *               out_first_job_id / out_first_cycles [10] list the first ten in TAKE ORDER (-1 and 0 past them), a fixed
+ *               choice: the reference takes them in hash-map order, which is
+ *               unspecified.  The fraction test of the warning stays with the caller.
+ * Call it after the match and before the launches, once per round.  A reset through cook_state_apply drops the round
+ * and the counts.
+ * Empty round (no considerable job): out_counts gets zeros (the head's job id and the uri position -1), the
+ * unmatched counts are zeroed, nothing else is written, no device work.
+ * COOK_E_BADARG, with nothing written and no count changed: no resident round on the handle (none yet, or another
+ * match ran on it since); the round was already counted; a considerable row upserted or removed since the match;
+ * a pending row's user code >= n_users, or n_users <= 0; a dropped position out of [0, n_considerable), repeated or
+ * holding no assignment; a NULL output (out_stats may be NULL), n_dropped < 0, a NULL dropped while n_dropped > 0,
+ * unmatched_warn_cycles < 0, key_cap < 0.  The first two of the dropped position rules and the ones before are
+ * checked before any device work, the others on the device before anything is written.
+ * Transfers exactly: up 4 * n_dropped; down 32 (the counts), plus 4 * n_considerable when a pending row was upserted
+ * or removed since the match (the rows' slots, for the check), plus 440 (the counts, amounts, rows and first ten as
+ * one block), then, unless COOK_E_TOO_LARGE, 8 * n_users + 16 * n_keys.  Nothing moves in an empty round.
+ * Statistics: out_stats (may be NULL) receives the call's own cook_phase_stats, as cook_state_user_stats; no
+ * cook_last_stats slot is written.  The match keeps its outputs, launches and transfers: it records the round with
+ * one device-to-device copy of its rows' slots.                                                               */
+enum { COOK_MM_GPUS = 0, COOK_MM_DISK_REQUEST = 1, COOK_MM_DISK_LIMIT = 2 };
+enum { COOK_MMC_CONSIDERABLE = 0, COOK_MMC_MATCHED = 1, COOK_MMC_HEAD_JOB_ID = 2, COOK_MMC_HEAD_MATCHED = 3,
+       COOK_MMC_URIS = 4, COOK_MMC_URIS_POSITION = 5, COOK_MMC_KEYS = 6, COOK_MMC_TOO_LONG = 7, COOK_MMC_FIRST = 8,
+       COOK_MMC_N = 9 };
+enum { COOK_MMA_TOTAL_CPUS = 0, COOK_MMA_TOTAL_MEM = 1, COOK_MMA_PCT_CPUS = 2, COOK_MMA_PCT_MEM = 5, COOK_MMA_N = 8 };
+enum { COOK_MM_HEAD = 0, COOK_MM_LARGEST_CPUS = 1, COOK_MM_LARGEST_MEM = 2, COOK_MM_ROWS = 3, COOK_MM_FIRST_N = 10 };
+enum { COOK_MMR_JOB_ID = 0, COOK_MMR_POSITION = 1, COOK_MMR_USER = 2, COOK_MMR_PORTS = 3, COOK_MMR_FACTS = 4,
+       COOK_MMR_GPU_MODEL = 5, COOK_MMR_DISK_TYPE = 6, COOK_MMR_NI = 7 };
+enum { COOK_MMR_CPUS = 0, COOK_MMR_MEM = 1, COOK_MMR_GPUS = 2, COOK_MMR_DISK_REQUEST = 3, COOK_MMR_DISK_LIMIT = 4,
+       COOK_MMR_NF = 5 };
+int32_t cook_state_match_metrics(cook_pool* pool, int32_t n_users, int32_t n_dropped, const int32_t* dropped,
+                                 int32_t unmatched_warn_cycles, int32_t key_cap, int64_t* out_counts,
+                                 double* out_amounts, int64_t* out_row_int, double* out_row_amount,
+                                 int64_t* out_first_job_id, int32_t* out_first_cycles, int32_t* out_user_considerable,
+                                 int32_t* out_user_matched, int32_t* out_key_kind, int32_t* out_key_code,
+                                 double* out_key_total, cook_phase_stats* out_stats);
+
 /* ----------------------------------------------------------------- multi-GPU */
 /* §8e: after a pool's match round every rank contributes its pools' usage
  * deltas {count,cpus,mem,gpus} per user; one ncclAllGather over NVLink makes

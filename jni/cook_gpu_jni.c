@@ -289,6 +289,25 @@ JFN(jint, stateTaskFacts)(JNIEnv* env, jclass k, jlong pool, jint n, jobject tas
 JFN(jint, stateTaskReason)(JNIEnv* env, jclass k, jlong pool, jint n, jobject task_id, jobject reason_code) {
   return cook_state_task_reason((cook_pool*)(intptr_t)pool, n, one(env, task_id), one(env, reason_code));
 }
+/* the stats keys of live pending jobs: job_id n longs, flags n bytes (COOK_JF_*), gpu_model n ints, disk_request and
+ * disk_limit n doubles, disk_type n ints (each but job_id may be null: unchanged) */
+JFN(jint, stateJobFacts)(JNIEnv* env, jclass k, jlong pool, jint n, jobject job_id, jobject flags, jobject gpu_model,
+                         jobject disk_request, jobject disk_limit, jobject disk_type) {
+  return cook_state_job_facts((cook_pool*)(intptr_t)pool, n, one(env, job_id), one(env, flags), one(env, gpu_model),
+                              one(env, disk_request), one(env, disk_limit), one(env, disk_type));
+}
+/* the match-cycle metrics of the last resident match: dropped n_dropped ints (may be null when 0); outs = {counts
+ * COOK_MMC_N longs, amounts COOK_MMA_N doubles, row ints 3 * COOK_MMR_NI longs, row amounts 3 * COOK_MMR_NF doubles,
+ * first job ids 10 longs, first cycles 10 ints, user considerable n_users ints, user matched n_users ints, key kinds,
+ * key codes key_cap ints each, key totals key_cap doubles}; out_stats a cook_phase_stats or null */
+JFN(jint, stateMatchMetrics)(JNIEnv* env, jclass k, jlong pool, jint n_users, jint n_dropped, jobject dropped,
+                             jint unmatched_warn_cycles, jint key_cap, jobjectArray outs, jobject out_stats) {
+  return cook_state_match_metrics((cook_pool*)(intptr_t)pool, n_users, n_dropped, one(env, dropped),
+                                  unmatched_warn_cycles, key_cap, buf(env, outs, 0), buf(env, outs, 1), buf(env, outs, 2),
+                                  buf(env, outs, 3), buf(env, outs, 4), buf(env, outs, 5), buf(env, outs, 6),
+                                  buf(env, outs, 7), buf(env, outs, 8), buf(env, outs, 9), buf(env, outs, 10),
+                                  (cook_phase_stats*)one(env, out_stats));
+}
 /* finished tasks: task_id and end_time_ms n longs, success n bytes (null: none succeeded) */
 JFN(jint, stateFinish)(JNIEnv* env, jclass k, jlong pool, jint n, jobject task_id, jobject end_time_ms,
                        jobject success) {

@@ -47,6 +47,12 @@ finishes through cook_state_finish_history against cook_state_finish, one advanc
 memory of the table and of the call's scratch:
   python tools/prof_state.py --history-stats --history-rows 1000000 --reps 5
   python tools/prof_state.py --history-stats --history-rows 10000000 --c3-group 4 --reps 3
+--match-metrics loads C2 (or config-#5 pool --c5-pool with --pool c5) into a resident handle with every pending job
+considerable, gives a tenth of the jobs a gpus fact and a tenth disk facts, and times cook_state_match_metrics after
+each match (a tenth of the matches dropped) against the numpy and Python restatement over a host mirror (sorts, folds,
+the dict of counters), with the answers compared bit for bit:
+  python tools/prof_state.py --match-metrics --pool c2 --reps 10
+  python tools/prof_state.py --match-metrics --pool c5 --c5-pool 5 --reps 10
 --unscheduled loads C2 (or config-#5 pool --c5-pool with --pool c5) into a resident handle, on the grid and off it,
 and times cook_state_unscheduled for one job, 1000 jobs and every waiting job of the user with the most, against numpy
 over a host mirror, with the answers compared bit for bit:
@@ -1307,6 +1313,97 @@ def history_stats_prof(a):
         x.close()
 
 
+def host_match_metrics(ids, matched, prev, thr, cpus, mem, gpus, user, facts, gmodel, dtype, dreq, dlim, U):
+    """The numpy and Python restatement over the host mirror's columns of the round's rows (take order): the per-user
+    counts, the left folds (np.add.accumulate is sequential), the stable sorts, the keyed folds and the dict of
+    counters the reference rebuilds each cycle."""
+    out = {"ucons": np.bincount(user, minlength=U), "umat": np.bincount(user[matched], minlength=U)}
+    out["tot"] = (np.add.accumulate(cpus)[-1], np.add.accumulate(mem)[-1])
+    N = len(ids)
+    pr = [(p * N + 99) // 100 - 1 for p in (50, 95, 100)]
+    oc, om = np.argsort(cpus, kind="stable"), np.argsort(mem, kind="stable")
+    out["pct"] = [cpus[oc[p]] for p in pr] + [mem[om[p]] for p in pr]
+    out["largest"] = (int(oc[-1]), int(om[-1]))
+    keys = []
+    for kind, bit, code, val in ((abi.MM_GPUS, abi.JF_GPUS, gmodel, gpus), (abi.MM_DISK_REQUEST, abi.JF_DISK_REQUEST,
+                                  dtype, dreq), (abi.MM_DISK_LIMIT, abi.JF_DISK_LIMIT, dtype, dlim)):
+        has = (facts & bit) != 0
+        for c in np.unique(code[has]):
+            keys.append((kind, int(c), float(np.add.accumulate(val[has & (code == c)])[-1])))
+    out["keys"] = keys
+    ms = np.zeros(N, bool)
+    ms[matched] = True
+    cyc = {j: prev.get(j, 0) + 1 for j, m in zip(ids.tolist(), ms.tolist()) if not m}
+    out["cycles"] = cyc
+    over = [(j, cyc[j]) for j in ids.tolist() if cyc.get(j, 0) > thr]
+    out["too_long"], out["first"] = len(over), over[:10]
+    return out
+
+
+def match_metrics_prof(a):
+    """cook_state_match_metrics after each match of a resident pool (C2, or config-#5 pool --c5-pool) with every
+    pending job considerable and a fifth of them carrying gpus or disk facts, against the numpy and Python
+    restatement over a host mirror; each answer is compared bit for bit."""
+    t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
+    jobs, pc, rc, users = t["jobs"], t["cols"]["pending"], t["cols"]["running"], t["users"]
+    J, U = jobs.n, users.n_users
+    store = Jobs(jobs, pc["priority"], pc["job_id"])
+    e = GpuEngine(pool_name="match-metrics")
+    e.state_apply(abi.make_delta(reset=True, running=abi.make_tasks(**{k: np.asarray(v) for k, v in rc.items()}),
+                                 pending=store.soa(np.arange(J)), pending_priority=store.prio,
+                                 pending_job_id=store.jid))
+    rng = np.random.default_rng(a.seed)
+    facts = np.where(rng.random(J) < 0.1, abi.JF_GPUS, 0) | np.where(
+        rng.random(J) < 0.1, abi.JF_DISK | abi.JF_DISK_REQUEST | abi.JF_DISK_LIMIT, 0)
+    facts = facts.astype(np.uint8)
+    gmodel = rng.integers(-1, 4, J).astype(np.int32)
+    dtype = rng.integers(-1, 2, J).astype(np.int32)
+    dreq, dlim = rng.choice([1024.0, 2048.0, 0.1], J), rng.choice([4096.0, 0.3], J)
+    e.state_job_facts(store.jid, facts, gpu_model=gmodel, disk_request=dreq, disk_limit=dlim, disk_type=dtype)
+    e.state_rank(users)
+    pos = {int(j): i for i, j in enumerate(store.jid)}
+    cols = {n: np.asarray(store.c[n] if n in store.c else np.zeros(J), np.float64) for n in ("cpus", "mem", "gpus")}
+    user = np.asarray(store.c["user"], np.int64)
+    prm = traces.match_params(J)
+    print(json.dumps({"card": card(), "pool": a.pool if a.pool == "c2" else f"c5/{a.c5_pool}", "jobs": J,
+                      "offers": t["offers"].n, "users": U}), flush=True)
+    prev, dev, wall, host, same = {}, [], [], [], True
+    for rep in range(a.reps + 3):
+        m = e.state_match(t["offers"], users, prm)
+        ids = m["considerable"]
+        matched = np.flatnonzero(m["assign"] >= 0)
+        dropped = matched[::10]
+        kept = np.setdiff1d(matched, dropped)
+        w0 = time.perf_counter()
+        got = e.state_match_metrics(U, dropped, unmatched_warn_cycles=2, key_cap=64)
+        w = time.perf_counter() - w0
+        r = np.array([pos[int(j)] for j in ids])
+        w0 = time.perf_counter()
+        h = host_match_metrics(ids, kept, prev, 2, cols["cpus"][r], cols["mem"][r], cols["gpus"][r], user[r], facts[r],
+                               gmodel[r], dtype[r], dreq[r], dlim[r], U)
+        hw = time.perf_counter() - w0
+        prev = h["cycles"]
+        f = lambda x: np.asarray(x, np.float64).view(np.int64).tolist()
+        same = same and got["user_considerable"].tolist() == h["ucons"].tolist() and \
+            got["user_matched"].tolist() == h["umat"].tolist() and \
+            f([got["total_cpus"], got["total_mem"]]) == f(h["tot"]) and f(got["pct_cpus"] + got["pct_mem"]) == f(h["pct"]) \
+            and (got["rows"][1]["position"], got["rows"][2]["position"]) == h["largest"] and \
+            [(k, c, f([v])) for k, c, v in got["keys"]] == [(k, c, f([v])) for k, c, v in h["keys"]] and \
+            got["too_long"] == h["too_long"] and got["first"] == h["first"]
+        if rep >= 3:   # the first calls carve and load the kernels
+            st = got["stats"]
+            dev.append(st["ms_h2d"] + st["ms_device"] + st["ms_d2h"])
+            wall.append(w)
+            host.append(hw)
+    print(json.dumps({"considerable": int(got["considerable"]), "matched": int(got["matched"]), "keys": len(got["keys"]),
+                      "too_long": got["too_long"], "device_ms": round(float(np.median(dev)), 4),
+                      "wall_ms": round(1e3 * float(np.median(wall)), 4), "h2d_bytes": st["h2d_bytes"],
+                      "d2h_bytes": st["d2h_bytes"], "n_launches": st["n_launches"],
+                      "host_restatement_ms": round(1e3 * float(np.median(host)), 4), "identical": bool(same)}),
+          flush=True)
+    e.close()
+
+
 def rank_quota_prof(a):
     t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
     pc, rc0, users = t["cols"]["pending"], t["cols"]["running"], t["users"]
@@ -1377,7 +1474,11 @@ def main():
     ap.add_argument("--history-stats", action="store_true",
                     help="cook_state_history_stats against numpy over a host mirror (--c3-group N: N config-#3 pools)")
     ap.add_argument("--history-rows", type=int, default=1_000_000, help="--history-stats: the finished rows in all")
+    ap.add_argument("--match-metrics", action="store_true",
+                    help="cook_state_match_metrics after each match against numpy over a host mirror (C2 or --pool c5)")
     a = ap.parse_args()
+    if a.match_metrics:
+        return match_metrics_prof(a)
     if a.history_stats:
         return history_stats_prof(a)
     if a.instance_stats:
