@@ -18,6 +18,8 @@
 ;;                                              task-reason! [cook_state_instance_stats, cook_state_task_reason], and
 ;;                                              for success / failed by history-seed!, finish-history! and
 ;;                                              history-advance! [cook_state_history_*]
+;;   :217-313 write-status-to-datomic       -> (status! ...), fed by retry-config! and retry-facts!
+;;                                             [cook_state_status, cook_state_retry_config, cook_state_retry_facts]
 ;;   :1210-1280 handle-match-cycle-metrics and the unmatched tracking :1399-1486
 ;;                                           -> (match-metrics! ...) + cycle.py's match_cycle_metrics_response, fed by
 ;;                                              job-facts! [cook_state_match_metrics, cook_state_job_facts]
@@ -392,6 +394,50 @@
                                             (longs-buf (map :end-ms done)) (bytes-buf (map :success? done))
                                             (when (some :reason-code done) (ints-buf (map #(or (:reason-code %) -1) done))))
           "cook_state_finish_history"))
+
+;; cook_state_status' outcomes, by COOK_JOB_* code
+(def ^:private job-outcomes [:completed :running :waiting :waiting-unretained :no-facts])
+
+(defn retry-config!
+  "At start-up: the :reason entities [{:code :mea-culpa? :failure-limit}] (:failure-limit nil: the global one) and
+   :scheduler.config/mea-culpa-failure-limit (5 when unset; -1 unlimited), as :job/reasons->attempts-consumed reads
+   them (schema.clj:1154-1172)."
+  [handle mea-culpa-limit reasons]
+  (check! handle (Native/stateRetryConfig handle (int mea-culpa-limit) (count reasons) (ints-buf (map :code reasons))
+                                          (bytes-buf (map :mea-culpa? reasons))
+                                          (ints-buf (map #(or (:failure-limit %) -2) reasons)))
+          "cook_state_retry_config"))
+
+(defn retry-facts!
+  "At start-up and on a leadership change after the load, and for each submitted job: [{:job-id :max-retries
+   :disable-mea-culpa? :completed? :done-reasons}], :done-reasons the :reason/code of each done (success or failed)
+   instance, nil for none (cycle.py's retry_facts).  A launch of such a job parks its pending row for status!."
+  [handle facts]
+  (let [lens (map (comp count :done-reasons) facts)]
+    (check! handle (Native/stateRetryFacts handle (count facts) (longs-buf (map :job-id facts))
+                                           (ints-buf (map :max-retries facts))
+                                           (bytes-buf (map #(bit-or (if (:disable-mea-culpa? %) 1 0)
+                                                                    (if (:completed? %) 2 0)) facts))
+                                           (ints-buf (reductions + 0 lens))
+                                           (ints-buf (map #(or % -1) (mapcat :done-reasons facts))))
+            "cook_state_retry_facts")))
+
+(defn status!
+  "finish-history!, and each row's job decided as :instance/update-state decides it (schema.clj:1242-1300), one
+   status at a time in order: [{:task-id :end-ms :success? :reason-code :preempted?}] from the tap's terminal status
+   datoms.  A waiting job whose row is parked is requeued on the device; returns one {:outcome :attempts} per row,
+   :outcome one of :completed :running :waiting :waiting-unretained (upsert the row, as before) :no-facts."
+  [handle done]
+  (let [n (count done)
+        out (direct (* 4 (max n 1)))
+        att (direct (* 4 (max n 1)))]
+    (check! handle (Native/stateStatus handle n (longs-buf (map :task-id done)) (bytes-buf (map :success? done))
+                                       (longs-buf (map :end-ms done))
+                                       (when (some :reason-code done) (ints-buf (map #(or (:reason-code %) -1) done)))
+                                       (bytes-buf (map :preempted? done)) out att)
+            "cook_state_status")
+    (let [ob (.asIntBuffer out) ab (.asIntBuffer att)]
+      (mapv (fn [i] {:outcome (job-outcomes (.get ob (int i))) :attempts (.get ab (int i))}) (range n)))))
 
 (defn history-seed!
   "At start-up and on a leadership change, after the reset and the load and before the tap resumes: the finished

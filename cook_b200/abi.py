@@ -167,6 +167,10 @@ JF_GPUS, JF_DISK, JF_DISK_REQUEST, JF_DISK_LIMIT, JF_URIS = 1, 2, 4, 8, 16
 MM_GPUS, MM_DISK_REQUEST, MM_DISK_LIMIT = 0, 1, 2
 MM_FIRST_N = 10
 
+# cook_state_retry_facts' bits and cook_state_status' outcomes
+RF_DISABLE_MEA_CULPA, RF_COMPLETED = 1, 2
+JOB_COMPLETED, JOB_RUNNING, JOB_WAITING, JOB_WAITING_UNRETAINED, JOB_NO_FACTS = 0, 1, 2, 3, 4
+
 MMC_CONSIDERABLE, MMC_MATCHED, MMC_HEAD_JOB_ID, MMC_HEAD_MATCHED, MMC_URIS, MMC_URIS_POSITION, MMC_KEYS = 0, 1, 2, 3, 4, 5, 6
 MMC_TOO_LONG, MMC_FIRST, MMC_N = 7, 8, 9
 MMA_TOTAL_CPUS, MMA_TOTAL_MEM, MMA_PCT_CPUS, MMA_PCT_MEM, MMA_N = 0, 1, 2, 5, 8
@@ -356,6 +360,9 @@ ARGTYPES = {
                                  P_I32, P_I32, P_I32, P_F64, _P(PhaseStats)],
     "cook_state_finish": [_H, _I32, P_I64, P_I64, P_U8],
     "cook_state_finish_history": [_H, _I32, P_I64, P_I64, P_U8, P_I32],
+    "cook_state_retry_config": [_H, _I32, _I32, P_I32, P_U8, P_I32],
+    "cook_state_retry_facts": [_H, _I32, P_I64, P_I32, P_U8, P_I32, P_I32],
+    "cook_state_status": [_H, _I32, P_I64, P_U8, P_I64, P_I32, P_U8, P_I32, P_I32],
     "cook_state_history_seed": [_H, C.c_int64, _I32, P_I64, P_I32, P_I64, P_I64, P_F64, P_F64, P_U8, P_I32],
     "cook_state_history_advance": [_H, C.c_int64],
     "cook_state_group_runtimes": [_H, _I32, P_I32, P_I32, _I32, P_I32],

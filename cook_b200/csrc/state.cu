@@ -162,6 +162,32 @@ __global__ void list_compact_kernel(OrderScan<int, 1> os, const uint8_t* live, i
   if (lane == 0) off[w] = start;
 }
 
+// a pending slot's list entries survive a compaction while it is live or parked
+__global__ void park_keep_kernel(const uint8_t* live, const uint8_t* park, int n, uint8_t* keep) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) keep[i] = live[i] | park[i];
+}
+
+// warp per requeued row whose novel-host list gains the entry code[w]: pending slot slot[w]'s list moves to the
+// arena's tail + the exclusive scan of the rows' new lengths, the entry after it, where an upsert's CSR would put it
+struct NovelLen {
+  const int32_t* slot; const int32_t* len;
+  __device__ void operator()(int p, int (&x)[1]) const { x[0] = len[slot[p]] + 1; }
+};
+__global__ void requeue_novel_kernel(OrderScan<int, 1> os, const int32_t* slot, const int32_t* code, int n,
+                                     int32_t* off, int32_t* len, int32_t* v, int32_t tail) {
+  const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (w >= n) return;
+  const int s = slot[w], l = len[s], start = tail + os.at(0, w) - (l + 1), o = off[s];
+  for (int i = lane; i < l; i += 32) v[start + i] = v[o + i];
+  __syncwarp();
+  if (lane == 0) {
+    v[start + l] = code[w];
+    off[s] = start;
+    len[s] = l + 1;
+  }
+}
+
 // warp per launched row: pending slot pslot[w]'s group list moves to the running arena at rtail + the exclusive scan
 // of the launched rows' lengths, where the equivalent delta's CSR puts it, and becomes running slot rslot[w]'s list
 __global__ void launch_lists_kernel(OrderScan<int, 1> os, const int32_t* pslot, const int32_t* rslot, int n,
@@ -579,7 +605,17 @@ struct PendingInfo {
   uint8_t jf = 0;            // the COOK_JF_* bits of the row's job facts
   int64_t touched = 0;       // PoolState::pend_epoch when the slot was last upserted or removed
   std::vector<int32_t> groups, attr_cols;
+  std::vector<int32_t> novel;   // the novel-host list: a requeue appends to it only what it does not hold
 };
+
+// A job's retry facts (cook_state_retry_facts): its max-retries, COOK_RF_* bits and its done instances' reason codes
+// counted per code (-1: none), as reasons->attempts-consumed reads them (frequencies).
+struct RetryFacts {
+  int32_t max_retries = 0;
+  uint8_t flags = 0;
+  std::map<int32_t, int32_t> done;
+};
+struct RetryReason { bool mea_culpa = false; int32_t limit = -2; };   // limit -2: the global one
 
 struct Table {
   int ncol = 0;
@@ -810,6 +846,7 @@ struct PoolState {
   std::vector<int64_t> rstart;                 // by running slot: its start time (cook_state_finish's checks)
   std::vector<uint8_t> rfacts;                 // by running slot: its RF_* bits
   std::vector<int64_t> rjid, rtid;             // by running slot: its job id and task id
+  std::vector<int32_t> rreason;                // by running slot: its reason fact (cook_state_task_reason)
   std::unordered_map<int64_t, std::vector<int32_t>> jobs_r;   // job id -> its live running slots (cook_state_unscheduled)
   int64_t grp_rows = 0;                        // live running rows with a group list
   Records rec;                                 // the successful runtimes per group
@@ -826,6 +863,14 @@ struct PoolState {
   int64_t pend_epoch = 0;             // counts the calls that upserted or removed a pending row
   MetricsRound mm;
   std::unordered_set<int32_t> reserved;   // the live pending slots whose reserved_host is not -1
+  // ---- retries (cook_state_retry_config / _facts, cook_state_status).  A launched job with facts keeps its pending
+  // slot parked: not live, not on the free list, its columns and lists kept for a requeue.
+  int32_t mc_limit = 5;                              // the global mea-culpa failure limit
+  std::unordered_map<int32_t, RetryReason> reasons;  // reason code -> mea-culpa and failure limit
+  std::unordered_map<int64_t, RetryFacts> retry;     // job id -> its facts
+  std::unordered_map<int64_t, int32_t> parked;       // job id -> its parked pending slot
+  int64_t park_len[3] = {};                          // list entries the parked slots hold (kept by the compaction)
+  uint8_t* park = nullptr; int32_t park_cap = 0;     // per pending slot: 1 while parked; allocated at the first park
   Arena stage;                        // one batch's uploads
   Arena scratch;                      // one call's device buffers
   Arena derive;                       // a derived match's or rebalance's running-side scratch (scratch is live then)
@@ -856,6 +901,7 @@ struct PoolState {
     for (auto& l : olists) l.release();
     stage.release(); scratch.release(); derive.release(); queue.release(); omerge.release();
     mm.release();
+    if (park) cudaFree(park);
     if (counters) cudaFree(counters);
     if (gf0) cudaFree(gf0);
   }
@@ -896,6 +942,42 @@ struct PoolState {
     if ((size_t)slot < ruser.size()) return;
     const size_t n = std::max<size_t>(slot + 1, 2 * ruser.size());
     ruser.resize(n); rhost.resize(n); rgroups.resize(n); rstart.resize(n); rfacts.resize(n); rjid.resize(n); rtid.resize(n);
+    rreason.resize(n);
+  }
+  // the park flags cover every pending slot: new ones zeroed, the old ones copied (device to device)
+  cudaError_t park_room(cudaStream_t st) {
+    if (park_cap >= pend.cap) return cudaSuccess;
+    uint8_t* p = nullptr;
+    cudaError_t e = cudaMalloc(&p, (size_t)pend.cap);
+    if (e == cudaSuccess) e = cudaMemsetAsync(p, 0, (size_t)pend.cap, st);
+    if (e == cudaSuccess && park_cap) e = cudaMemcpyAsync(p, park, (size_t)park_cap, cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { if (p) cudaFree(p); return e; }
+    if (park) cudaFree(park);
+    park = p;
+    park_cap = pend.cap;
+    return cudaSuccess;
+  }
+  // job jid's parked copy, if any, is freed: its slot back on the free list (appended to *freed), its entries dead
+  void unpark(int64_t jid, std::vector<int32_t>* freed) {
+    auto it = parked.find(jid);
+    if (it == parked.end()) return;
+    const int32_t s = it->second;
+    parked.erase(it);
+    for (int l = 0; l < 3; l++) park_len[l] -= pinfo[s].len[l];
+    pend.free.push_back(s);
+    freed->push_back(s);
+  }
+  // reasons->attempts-consumed (schema.clj:1154-1172) over a job's done instances
+  int32_t attempts(const RetryFacts& f) const {
+    int64_t a = 0;
+    for (const auto& kv : f.done) {
+      auto r = reasons.find(kv.first);
+      if (kv.first < 0 || r == reasons.end() || !r->second.mea_culpa) { a += kv.second; continue; }
+      const int32_t lim = (f.flags & COOK_RF_DISABLE_MEA_CULPA) ? 0 : r->second.limit != -2 ? r->second.limit : mc_limit;
+      if (lim != -1) a += std::max(0, kv.second - lim);
+    }
+    return (int32_t)std::min<int64_t>(a, INT32_MAX);
   }
   // a live pending slot's flag f after a patch of its column
   void set_flag(int32_t slot, int f, bool on) {
@@ -971,18 +1053,28 @@ void gather_lists(const PoolState* S, const JobDev& o, const int32_t* m_slot, in
 int32_t compact_lists(cook_pool* pool, PoolState* S, cudaStream_t st, int* nl) {
   for (int l = 0; l < L_N + OL_N; l++) {
     ListArena& A = l < L_N ? S->lists[l] : S->olists[l - L_N];
-    if (A.tail - A.live <= A.live) continue;
+    const bool parked = l < 3 && !S->parked.empty();   // parked slots' entries are kept, not dead
+    const int64_t kept = A.live + (l < 3 ? S->park_len[l] : 0);
+    if (A.tail - kept <= kept) continue;
     const Table& t = l == L_RGROUP ? S->run : l >= L_N ? S->offer : S->pend;
     const int n = t.hw, oc = t.lcol[l == L_RGROUP ? 0 : l >= L_N ? l - L_N : l];
-    if (A.live > 0 && n > 0) {
+    if (kept > 0 && n > 0) {
       for (int i = 0; i < A.k; i++)
         if (!A.alt[i]) CK(pool, cudaMalloc(&A.alt[i], (i ? A.esz1 : sizeof(int32_t)) * std::max<int64_t>(A.cap, 1)));
+      if (parked) CK(pool, S->park_room(st));
       OrderScan<int, 1> os;
+      uint8_t* keep = nullptr;
       CK(pool, carve(S->scratch, st, nullptr, nullptr, [&](Carve& c) {
         os.part[0] = c.take<int32_t>(n);
         os.tile[0] = c.take<int32_t>((n + OS_TILE - 1) / OS_TILE + 1);
+        if (parked) keep = c.take<uint8_t>(n);
       }));
       const uint8_t* live = static_cast<const uint8_t*>(t.col[t.live_col]);
+      if (parked) {
+        park_keep_kernel<<<(n + 255) / 256, 256, 0, st>>>(live, S->park, n, keep);
+        (*nl)++;
+        live = keep;
+      }
       int32_t* off = static_cast<int32_t*>(t.col[oc]);
       const int32_t* len = static_cast<const int32_t*>(t.col[oc + 1]);
       order_scan(os, SlotLen{live, len}, n, S->gf0, st, nl);
@@ -997,7 +1089,7 @@ int32_t compact_lists(cook_pool* pool, PoolState* S, cudaStream_t st, int* nl) {
       CK(pool, cudaGetLastError());
       for (int i = 0; i < A.k; i++) std::swap(A.v[i], A.alt[i]);
     }
-    A.tail = A.live;
+    A.tail = kept;
   }
   return COOK_OK;
 }
@@ -1095,8 +1187,21 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
     S->jf_keyed = 0;
     S->mm.on = false;
     S->mm.u_n = 0;
+    if (!S->parked.empty()) CK(pool, cudaMemsetAsync(S->park, 0, (size_t)S->park_cap, st));
+    S->parked.clear();
+    S->retry.clear();
+    for (auto& l : S->park_len) l = 0;
   }
   if (rs || np || npr) S->pend_epoch++;
+  // a pending upsert or removal drops the job's retry facts; an upsert frees its parked copy (the caller's row wins)
+  std::vector<int32_t> unparked;
+  if (!S->retry.empty()) {
+    for (int i = 0; i < npr; i++) S->retry.erase(d->pending_rm_job_id[i]);
+    for (int i = 0; i < np; i++) {
+      S->retry.erase(d->pending_job_id[i]);
+      S->unpark(d->pending_job_id[i], &unparked);
+    }
+  }
   std::vector<int32_t> prm_slot(npr), pup_slot(np), rrm_slot(nrr), rup_slot(nr);
   for (int i = 0; i < npr; i++) {
     auto it = S->pend.slot_of.find(d->pending_rm_job_id[i]);
@@ -1128,6 +1233,7 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
     pi.len[L_GROUP] = P.group_off ? P.group_off[i + 1] - P.group_off[i] : 0;
     pi.attr_cols.assign(P.attr_off ? P.attr_col + P.attr_off[i] : nullptr, P.attr_off ? P.attr_col + P.attr_off[i + 1] : nullptr);
     pi.groups.assign(P.group_off ? P.group_idx + P.group_off[i] : nullptr, P.group_off ? P.group_idx + P.group_off[i + 1] : nullptr);
+    pi.novel.assign(P.novel_off ? P.novel_host + P.novel_off[i] : nullptr, P.novel_off ? P.novel_host + P.novel_off[i + 1] : nullptr);
     const bool f[F_N] = {P.gpus && P.gpus[i] != 0.0, P.ports && P.ports[i] != 0, P.allowed && !P.allowed[i],
                          P.plugin_accept && !P.plugin_accept[i], P.gpu_model && P.gpu_model[i] != -1,
                          P.disk_request && P.disk_request[i] >= 0.0, P.est_end_ms && P.est_end_ms[i] != -1,
@@ -1156,6 +1262,7 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
     S->rgroups[s].assign(rgo ? d->running_group_idx + rgo[i] : nullptr, rgo ? d->running_group_idx + rgo[i + 1] : nullptr);
     S->rstart[s] = T.start_time[i];
     S->rfacts[s] = 0;
+    S->rreason[s] = -1;
     S->rjid[s] = T.job_id[i]; S->rtid[s] = T.task_id[i];
     S->add_running(s, +1);
     rup_slot[i] = s;
@@ -1178,10 +1285,17 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
   const int64_t radd = rgo ? rgo[nr] : 0;
   CK(pool, RG.grow(RG.tail + radd, st));
   RG.tail += radd;
-  ScatterArgs pu, pr, ru, rr;
+  ScatterArgs pu, pr, ru, rr, uk;
   memset(&pu, 0, sizeof(pu)); memset(&pr, 0, sizeof(pr)); memset(&ru, 0, sizeof(ru)); memset(&rr, 0, sizeof(rr));
+  memset(&uk, 0, sizeof(uk));
+  const int nuk = (int)unparked.size();
   int64_t h2d = 0;
   const cudaError_t carved = carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
+    if (nuk) {
+      uk.c[0] = ScatterCol{reinterpret_cast<char*>(S->park), nullptr, 0, 1};
+      uk.nc = 1;
+      uk.slot = c.up(unparked.data(), nuk);
+    }
     if (np) {
       const void* src[P_NDATA] = {P.user, d->pending_priority, d->pending_job_id, P.cpus, P.mem, P.gpus, P.ports,
                                   P.allowed, P.plugin_accept, P.gpu_model, P.disk_request, P.disk_type, P.est_end_ms,
@@ -1231,6 +1345,7 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
   scatter(rr, S->run, nrr, 0, R_LIVE, &rtail0, st, &nl);
   scatter(pu, S->pend, np, 1, P_LIVE, tail0, st, &nl);
   scatter(ru, S->run, nr, 1, R_LIVE, &rtail0, st, &nl);
+  scatter(uk, S->pend, nuk, 0, -1, nullptr, st, &nl);
   CK(pool, cudaGetLastError());
   int32_t rc = compact_lists(pool, S, st, &nl);
   if (rc != COOK_OK) return rc;
@@ -1274,15 +1389,26 @@ int32_t launch(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, cons
   }
   CK(pool, cudaSetDevice(pool->device));
   cudaStream_t st = pool->stream;
-  // ---- host side, in cook_state_apply's order: the removals free their slots, then the tasks take theirs
+  // ---- host side, in cook_state_apply's order: the removals free their slots, then the tasks take theirs.  A job
+  // with retry facts parks its slot instead of freeing it.
   if (n) S->pend_epoch++;
+  std::vector<int32_t> kslot, fslot;   // parked and freed slots, when some job parks
   for (int i = 0; i < n; i++) {
     const int32_t s = pslot[i];
     S->pend.slot_of.erase(job_id[i]);
     S->add_pending(s, S->pinfo[s], -1);
     S->pinfo[s].touched = S->pend_epoch;
-    S->pend.free.push_back(s);
+    if (!S->retry.empty() && S->retry.count(job_id[i])) {
+      S->parked.emplace(job_id[i], s);
+      for (int l = 0; l < 3; l++) S->park_len[l] += S->pinfo[s].len[l];
+      kslot.push_back(s);
+    } else {
+      S->pend.free.push_back(s);
+      fslot.push_back(s);
+    }
   }
+  const int nk = (int)kslot.size();
+  if (!nk) fslot.clear();   // the removal takes every row
   int64_t ng = 0;   // group list entries that move with the jobs
   for (int i = 0; i < n; i++) {
     const int32_t r = S->run.take_slot();
@@ -1293,6 +1419,7 @@ int32_t launch(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, cons
     S->rgroups[r] = S->pinfo[pslot[i]].groups;
     S->rstart[r] = start_time[i];
     S->rfacts[r] = 0;
+    S->rreason[r] = -1;
     S->rjid[r] = job_id[i]; S->rtid[r] = task_id[i];
     S->add_running(r, +1);
     ng += (int64_t)S->rgroups[r].size();
@@ -1301,11 +1428,12 @@ int32_t launch(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, cons
   // ---- device: capacity, the upload, the move (rows, then group lists), the pending slots' removal, then the
   // arena rule
   CK(pool, S->run.grow(S->run.hw, st));
+  if (nk) CK(pool, S->park_room(st));
   ListArena& RG = S->lists[L_RGROUP];
   const int32_t rtail0 = (int32_t)RG.tail;
   CK(pool, RG.grow(RG.tail + ng, st));
   RG.tail += ng;
-  const int32_t *d_pslot = nullptr, *d_rslot = nullptr, *d_host = nullptr;
+  const int32_t *d_pslot = nullptr, *d_rslot = nullptr, *d_host = nullptr, *d_kslot = nullptr, *d_fslot = nullptr;
   const int64_t *d_tid = nullptr, *d_start = nullptr;
   OrderScan<int, 1> os;
   int64_t h2d = 0;
@@ -1314,6 +1442,7 @@ int32_t launch(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, cons
     d_pslot = c.up(pslot.data(), n); d_rslot = c.up(rslot.data(), n);
     d_tid = c.up(task_id, n); d_start = c.up(start_time, n);
     d_host = c.up(hostname_id, n);
+    if (nk) { d_kslot = c.up(kslot.data(), nk); d_fslot = c.up(fslot.data(), fslot.size()); }
     if (ng) {   // device-only buffers: nothing uploaded
       os.part[0] = c.take<int32_t>(n);
       os.tile[0] = c.take<int32_t>((n + OS_TILE - 1) / OS_TILE + 1);
@@ -1335,10 +1464,18 @@ int32_t launch(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, cons
     }
     ScatterArgs rm;
     memset(&rm, 0, sizeof(rm));
-    rm.slot = d_pslot;
+    rm.slot = nk ? d_fslot : d_pslot;
     int32_t tail[3];
     for (int l = 0; l < 3; l++) tail[l] = (int32_t)S->lists[l].tail;
-    scatter(rm, S->pend, n, 0, P_LIVE, tail, st, &nl);
+    scatter(rm, S->pend, n - nk, 0, P_LIVE, tail, st, &nl);
+    if (nk) {   // parking: the live flag cleared and the generation bumped as a removal's, the lists kept
+      ScatterArgs pk;
+      memset(&pk, 0, sizeof(pk));
+      pk.c[0] = ScatterCol{reinterpret_cast<char*>(S->park), nullptr, 1, 1};
+      pk.nc = 1;
+      pk.slot = d_kslot;
+      scatter(pk, S->pend, nk, 0, P_LIVE, nullptr, st, &nl);
+    }
   }
   CK(pool, cudaGetLastError());
   int32_t rc = compact_lists(pool, S, st, &nl);
@@ -3170,6 +3307,7 @@ int32_t task_reason(cook_pool* pool, PoolState* S, int n, const int64_t* task_id
   if (const char* why = running_slots(S, n, task_id, &slot)) return set_err(pool, COOK_E_BADARG, "%s: %s", who, why);
   CK(pool, cudaSetDevice(pool->device));
   cudaStream_t st = pool->stream;
+  for (int i = 0; i < n; i++) S->rreason[slot[i]] = reason_code[i];   // cook_state_status decides from it
   ScatterArgs pa;
   memset(&pa, 0, sizeof(pa));
   int64_t h2d = 0;
@@ -3191,13 +3329,16 @@ int32_t task_reason(cook_pool* pool, PoolState* S, int n, const int64_t* task_id
 
 // What cook_state_finish_history adds to cook_state_finish: the rows' reason codes (NULL: each row's reason fact).
 struct FinishHistory { const int32_t* reason_code; };
+// What cook_state_status adds to cook_state_finish_history: the rows' preempted flags (NULL: none) and the outputs.
+struct FinishStatus { const uint8_t* preempted; int32_t* outcome; int32_t* attempts; };
 
 // running_rm_task_id = task_id, plus one record per group of each successful row; with `fh`, the rows that start at
 // or after the horizon of an enabled history are also appended to it
 int32_t finish(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, const int64_t* end_time_ms,
-               const uint8_t* success, const FinishHistory* fh = nullptr) {
-  const char* who = fh ? "cook_state_finish_history" : "cook_state_finish";
+               const uint8_t* success, const FinishHistory* fh = nullptr, const FinishStatus* fs = nullptr) {
+  const char* who = fs ? "cook_state_status" : fh ? "cook_state_finish_history" : "cook_state_finish";
   if (n < 0) return set_err(pool, COOK_E_BADARG, "%s: n < 0", who);
+  if (fs && n && (!fs->outcome || !fs->attempts)) return set_err(pool, COOK_E_BADARG, "%s: null out_outcome or out_attempts", who);
   if (n && !task_id) return set_err(pool, COOK_E_BADARG, "%s: null task_id", who);
   if (n && success && !end_time_ms) return set_err(pool, COOK_E_BADARG, "%s: success without end_time_ms", who);
   if (fh && n && (!end_time_ms || !success)) return set_err(pool, COOK_E_BADARG, "%s: null end_time_ms or success", who);
@@ -3224,7 +3365,9 @@ int32_t finish(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, con
   if (S->rec.tail + nrec > INT32_MAX) return set_err(pool, COOK_E_TOO_LARGE, "%s: more than 2^31 - 1 records", who);
   CK(pool, cudaSetDevice(pool->device));
   cudaStream_t st = pool->stream;
-  // ---- host side: cook_state_apply's removals, then the records' counts
+  // ---- host side: cook_state_apply's removals, then the records' counts.  With retry facts, in batch order: the
+  // status's job decision (cook_state_status) or, for a job's last live instance, its parked copy freed.
+  std::vector<int32_t> unparked, rq_slot, ap_slot, ap_code;
   for (int i = 0; i < n; i++) {
     const int32_t s = slot[i];
     S->run.slot_of.erase(task_id[i]);
@@ -3232,7 +3375,61 @@ int32_t finish(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, con
     S->run.free.push_back(s);
     if (success && success[i])
       for (int32_t g : S->rgroups[s]) count_add(S->rec_groups, g, +1);
+    const int64_t j = S->rjid[s];
+    auto f = S->retry.find(j);
+    if (fs && f == S->retry.end()) {
+      fs->outcome[i] = COOK_JOB_NO_FACTS;
+      fs->attempts[i] = -1;
+    }
+    if (f == S->retry.end()) continue;
+    const bool other = S->jobs_r.count(j) != 0;   // another live running or unknown instance
+    if (!fs) {
+      if (!other) {
+        S->unpark(j, &unparked);
+        if (!S->pend.slot_of.count(j)) S->retry.erase(f);
+      }
+      continue;
+    }
+    // :instance/update-state's job-state cond (schema.clj:1242-1300) for this one status
+    RetryFacts& F = f->second;
+    F.done[fh->reason_code ? fh->reason_code[i] : S->rreason[s]]++;
+    const int32_t att = S->attempts(F);
+    fs->attempts[i] = att;
+    int32_t oc;
+    if (F.flags & COOK_RF_COMPLETED) oc = COOK_JOB_COMPLETED;
+    else if (success[i] || (!other && att >= F.max_retries)) oc = COOK_JOB_COMPLETED;
+    else if (other) oc = COOK_JOB_RUNNING;
+    else oc = S->parked.count(j) ? COOK_JOB_WAITING : COOK_JOB_WAITING_UNRETAINED;
+    fs->outcome[i] = oc;
+    if (oc == COOK_JOB_COMPLETED) {
+      F.flags |= COOK_RF_COMPLETED;
+      S->unpark(j, &unparked);
+      if (!other && !S->pend.slot_of.count(j)) S->retry.erase(f);
+    } else if (oc == COOK_JOB_WAITING) {   // the requeue: the parked copy becomes the live row an upsert would write
+      auto it = S->parked.find(j);
+      const int32_t p = it->second;
+      S->parked.erase(it);
+      PendingInfo& pi = S->pinfo[p];
+      for (int l = 0; l < 3; l++) S->park_len[l] -= pi.len[l];
+      const int32_t h = S->rhost[s];
+      if (h != -1 && !(fs->preempted && fs->preempted[i]) && std::find(pi.novel.begin(), pi.novel.end(), h) == pi.novel.end()) {
+        pi.novel.push_back(h);
+        pi.len[L_NOVEL]++;
+        ap_slot.push_back(p);
+        ap_code.push_back(h);
+      }
+      if (rq_slot.empty()) S->pend_epoch++;
+      if ((pi.flags >> F_RESERVED) & 1) pi.flags ^= (uint16_t)(1u << F_RESERVED);   // reserved_host -1
+      pi.jf = 0;                                                                     // no job facts
+      pi.touched = S->pend_epoch;
+      S->pend.slot_of.emplace(j, p);
+      S->add_pending(p, pi, +1);
+      rq_slot.push_back(p);
+    }
   }
+  const int nrq = (int)rq_slot.size(), nap = (int)ap_slot.size(), nuk = (int)unparked.size();
+  int64_t nadd = 0;   // the novel-host entries the requeue's moved lists take
+  for (int32_t p : ap_slot) nadd += S->pinfo[p].len[L_NOVEL];
   // ---- device: the records (read before the removal empties the rows' lists), the removal, the arena rules
   Records& RC = S->rec;
   const int32_t rtail = (int32_t)RC.tail;
@@ -3243,15 +3440,42 @@ int32_t finish(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, con
   if (nhist) CK(pool, H.grow(H.tail + nhist, st));
   H.tail += nhist;
   const int32_t rgtail = (int32_t)S->lists[L_RGROUP].tail;
+  ListArena& NV = S->lists[L_NOVEL];
+  const int32_t ntail = (int32_t)NV.tail;
+  if (nadd) {
+    CK(pool, NV.grow(NV.tail + nadd, st));
+    NV.tail += nadd;
+  }
   const int32_t* d_slot = nullptr;
   const uint8_t* d_ok = nullptr;
   const int64_t* d_end = nullptr;
   const int32_t* d_reason = nullptr;
+  const int32_t *d_ap_slot = nullptr, *d_ap_code = nullptr;
   int32_t* hblk = nullptr;
-  OrderScan<int, 1> os;
+  OrderScan<int, 1> os, aos;
+  ScatterArgs rq, uk;
+  memset(&rq, 0, sizeof(rq)); memset(&uk, 0, sizeof(uk));
   int64_t h2d = 0;
   CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
     if (!n) return;
+    if (nrq) {   // live again with a new generation, reserved_host -1, no job facts, no longer parked
+      rq.c[0] = ScatterCol{static_cast<char*>(S->pend.col[P_RESERVED]), nullptr, -1, P_SZ[P_RESERVED]};
+      rq.c[1] = ScatterCol{static_cast<char*>(S->pend.col[P_JF]), nullptr, 0, P_SZ[P_JF]};
+      rq.c[2] = ScatterCol{reinterpret_cast<char*>(S->park), nullptr, 0, 1};
+      rq.nc = 3;
+      rq.slot = c.up(rq_slot.data(), nrq);
+    }
+    if (nap) {
+      d_ap_slot = c.up(ap_slot.data(), nap);
+      d_ap_code = c.up(ap_code.data(), nap);
+      aos.part[0] = c.take<int32_t>(nap);
+      aos.tile[0] = c.take<int32_t>((nap + OS_TILE - 1) / OS_TILE + 1);
+    }
+    if (nuk) {
+      uk.c[0] = ScatterCol{reinterpret_cast<char*>(S->park), nullptr, 0, 1};
+      uk.nc = 1;
+      uk.slot = c.up(unparked.data(), nuk);
+    }
     d_slot = c.up(slot.data(), n);
     if (success) { d_ok = c.up(success, n); d_end = c.up(end_time_ms, n); }
     if (nrec) {   // device-only buffers: nothing uploaded
@@ -3280,10 +3504,97 @@ int32_t finish(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, con
     rr.slot = d_slot;
     scatter(rr, S->run, n, 0, R_LIVE, &rgtail, st, &nl);
   }
+  if (nap) {   // the requeued rows' novel-host lists, each with its one new entry, to the arena's tail
+    order_scan(aos, NovelLen{d_ap_slot, S->pend.at<int32_t>(P_NLEN)}, nap, S->gf0, st, &nl);
+    requeue_novel_kernel<<<(nap + 7) / 8, 256, 0, st>>>(aos, d_ap_slot, d_ap_code, nap,
+                                                        static_cast<int32_t*>(S->pend.col[P_NOFF]),
+                                                        static_cast<int32_t*>(S->pend.col[P_NLEN]), NV.v[0], ntail);
+    nl++;
+  }
+  scatter(rq, S->pend, nrq, 1, P_LIVE, nullptr, st, &nl);
+  scatter(uk, S->pend, nuk, 0, -1, nullptr, st, &nl);
   CK(pool, cudaGetLastError());
   int32_t rc = compact_lists(pool, S, st, &nl);
   if (rc == COOK_OK) rc = compact_records(pool, S, st, &nl);
   if (rc != COOK_OK) return rc;
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  CK(pool, cudaStreamSynchronize(st));
+  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
+  return COOK_OK;
+}
+
+// the reason dictionary and the global mea-culpa limit; host only
+int32_t retry_config(cook_pool* pool, PoolState* S, int32_t mea_culpa_limit, int n, const int32_t* reason_code,
+                     const uint8_t* mea_culpa, const int32_t* failure_limit) {
+  const char* who = "cook_state_retry_config";
+  if (n < 0) return set_err(pool, COOK_E_BADARG, "%s: n_reasons < 0", who);
+  if (n && (!reason_code || !mea_culpa || !failure_limit)) return set_err(pool, COOK_E_BADARG, "%s: null array", who);
+  if (mea_culpa_limit < -1) return set_err(pool, COOK_E_BADARG, "%s: a mea_culpa_limit below -1", who);
+  std::unordered_map<int32_t, RetryReason> m;
+  m.reserve((size_t)n);
+  for (int i = 0; i < n; i++) {
+    if (reason_code[i] < 0) return set_err(pool, COOK_E_BADARG, "%s: a negative reason code", who);
+    if (failure_limit[i] < -2) return set_err(pool, COOK_E_BADARG, "%s: a failure limit below -2", who);
+    if (!m.emplace(reason_code[i], RetryReason{mea_culpa[i] != 0, failure_limit[i]}).second)
+      return set_err(pool, COOK_E_BADARG, "%s: reason code twice", who);
+  }
+  S->mc_limit = mea_culpa_limit;
+  S->reasons.swap(m);
+  return COOK_OK;
+}
+
+// the retry facts of jobs the handle holds (a live pending row, a parked copy or a live running instance)
+int32_t retry_facts(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, const int32_t* max_retries,
+                    const uint8_t* flags, const int32_t* done_off, const int32_t* done_reason) {
+  const char* who = "cook_state_retry_facts";
+  if (n < 0) return set_err(pool, COOK_E_BADARG, "%s: n < 0", who);
+  if (n && (!job_id || !max_retries || !flags)) return set_err(pool, COOK_E_BADARG, "%s: null job_id, max_retries or flags", who);
+  if (!csr_ok(done_off, n, done_reason, nullptr, false)) return set_err(pool, COOK_E_BADARG, "%s: malformed CSR offsets", who);
+  if (done_off && !idx_in_range(done_reason, done_off[n], -1, INT32_MAX))
+    return set_err(pool, COOK_E_BADARG, "%s: a reason code below -1", who);
+  {
+    std::unordered_set<int64_t> seen;
+    seen.reserve((size_t)n);
+    for (int i = 0; i < n; i++) {
+      if (max_retries[i] < 0) return set_err(pool, COOK_E_BADARG, "%s: a negative max_retries", who);
+      if (flags[i] & ~(COOK_RF_DISABLE_MEA_CULPA | COOK_RF_COMPLETED)) return set_err(pool, COOK_E_BADARG, "%s: unknown flag bits", who);
+      if (!seen.insert(job_id[i]).second) return set_err(pool, COOK_E_BADARG, "%s: job id twice", who);
+      if (!S->pend.slot_of.count(job_id[i]) && !S->parked.count(job_id[i]) && !S->jobs_r.count(job_id[i]))
+        return set_err(pool, COOK_E_BADARG, "%s: unknown job id", who);
+    }
+  }
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  // ---- host side: the facts replaced; a completed job without a live instance loses its parked copy and its facts
+  std::vector<int32_t> unparked;
+  for (int i = 0; i < n; i++) {
+    const int64_t j = job_id[i];
+    if ((flags[i] & COOK_RF_COMPLETED) && !S->jobs_r.count(j) && S->parked.count(j)) {
+      S->unpark(j, &unparked);
+      S->retry.erase(j);
+      continue;
+    }
+    RetryFacts& F = S->retry[j];
+    F.max_retries = max_retries[i];
+    F.flags = flags[i];
+    F.done.clear();
+    for (int k = done_off ? done_off[i] : 0; done_off && k < done_off[i + 1]; k++) F.done[done_reason[k]]++;
+  }
+  // ---- device: the freed copies' park flags
+  const int nuk = (int)unparked.size();
+  ScatterArgs uk;
+  memset(&uk, 0, sizeof(uk));
+  int64_t h2d = 0;
+  CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
+    if (!nuk) return;
+    uk.c[0] = ScatterCol{reinterpret_cast<char*>(S->park), nullptr, 0, 1};
+    uk.nc = 1;
+    uk.slot = c.up(unparked.data(), nuk);
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  int nl = 0;
+  scatter(uk, S->pend, nuk, 0, -1, nullptr, st, &nl);
+  CK(pool, cudaGetLastError());
   CK(pool, cudaEventRecord(pool->ev[22], st));
   CK(pool, cudaStreamSynchronize(st));
   record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
@@ -3761,6 +4072,37 @@ extern "C" int32_t cook_state_finish_history(cook_pool* pool, int32_t n, const i
   if (!S) return set_err(pool, COOK_E_OOM, "cook_state_finish_history: out of device memory");
   const FinishHistory fh{reason_code};
   return finish(pool, S, n, task_id, end_time_ms, success, &fh);
+}
+
+extern "C" int32_t cook_state_retry_config(cook_pool* pool, int32_t mea_culpa_limit, int32_t n_reasons,
+                                           const int32_t* reason_code, const uint8_t* mea_culpa,
+                                           const int32_t* failure_limit) {
+  if (!pool) return COOK_E_BADARG;
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_retry_config: out of device memory");
+  return retry_config(pool, S, mea_culpa_limit, n_reasons, reason_code, mea_culpa, failure_limit);
+}
+
+extern "C" int32_t cook_state_retry_facts(cook_pool* pool, int32_t n, const int64_t* job_id, const int32_t* max_retries,
+                                          const uint8_t* flags, const int32_t* done_off, const int32_t* done_reason) {
+  if (!pool) return COOK_E_BADARG;
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_retry_facts: out of device memory");
+  return retry_facts(pool, S, n, job_id, max_retries, flags, done_off, done_reason);
+}
+
+extern "C" int32_t cook_state_status(cook_pool* pool, int32_t n, const int64_t* task_id, const uint8_t* success,
+                                     const int64_t* end_time_ms, const int32_t* reason_code, const uint8_t* preempted,
+                                     int32_t* out_outcome, int32_t* out_attempts) {
+  if (!pool) return COOK_E_BADARG;
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_status: out of device memory");
+  const FinishHistory fh{reason_code};
+  const FinishStatus fs{preempted, out_outcome, out_attempts};
+  return finish(pool, S, n, task_id, end_time_ms, success, &fh, &fs);
 }
 
 extern "C" int32_t cook_state_history_seed(cook_pool* pool, int64_t since_ms, int32_t n, const int64_t* task_id,

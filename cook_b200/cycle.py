@@ -750,3 +750,11 @@ def match_cycle_metrics_response(answer, considerable_job_id, *, pool, max_consi
                        "unmatched-cycles-warn-threshold": unmatched_cycles_warn_threshold,
                        "unmatched-fraction-warn-threshold": unmatched_fraction_warn_threshold}
     return out
+
+
+def retry_facts(instances, reason_table):
+    """A job's done-instance reasons for cook_state_retry_facts, from its instances as (status, reason name or None):
+    the reason codes of the success and failed ones in order (-1: no reason; :job/attempts-consumed reads both), and
+    whether one succeeded (then the job is completed: pass abi.RF_COMPLETED).  reason_table: name -> :reason/code."""
+    done = [reason_table[r] if r is not None else -1 for st, r in instances if st in ("success", "failed")]
+    return done, any(st == "success" for st, _ in instances)

@@ -153,6 +153,16 @@ class GpuEngine:
         rc = self.lib.cook_state_apply(self.pool, C.byref(delta))
         if rc != 0:
             self._err(rc)
+        # a pending upsert or removal drops a job's retry facts and parked copy, a reset all of them
+        if hasattr(self, "_state_retry"):
+            if delta.reset:
+                for m in (self._state_retry, self._state_parked_glen, self._state_task_job):
+                    m.clear()
+            for c in ("pending_rm_job_id", "pending_job_id"):
+                ids = delta.col(c)
+                for j in (ids.tolist() if ids is not None else []):
+                    self._state_retry.discard(j)
+                    self._state_parked_glen.pop(j, None)
         # the live pending ids, O(delta): they size state_rank's output
         live = getattr(self, "_state_pending_ids", set())
         if delta.reset:
@@ -208,7 +218,12 @@ class GpuEngine:
         run.update(tid.tolist())
         self._state_running_ids = run
         png, rng_ = self._group_lengths()
-        rng_.update((t, png.pop(j, 0)) for j, t in zip(jid.tolist(), tid.tolist()))
+        retry = getattr(self, "_state_retry", ())
+        for j, t in zip(jid.tolist(), tid.tolist()):
+            rng_[t] = png.pop(j, 0)
+            if j in retry:   # the job parks: state_status may requeue it
+                self._state_parked_glen[j] = rng_[t]
+                self._state_task_job[t] = j
 
     def _group_lengths(self):
         """{job id: group list length} of the live pending rows and {task id: length} of the live running rows."""
@@ -318,6 +333,7 @@ class GpuEngine:
         rng_ = self._group_lengths()[1]
         for t in tid.tolist():
             rng_.pop(t, None)
+        self._forget_tasks(tid.tolist())
 
     def state_finish_history(self, task_id, end_time_ms, success, reason_code=None):
         """cook_state_finish_history: state_finish, and while the history is on, the rows that start at or after its
@@ -337,6 +353,96 @@ class GpuEngine:
         rng_ = self._group_lengths()[1]
         for t in tid.tolist():
             rng_.pop(t, None)
+        self._forget_tasks(tid.tolist())
+
+    def state_retry_config(self, mea_culpa_limit=5, reasons=()):
+        """cook_state_retry_config: the global mea-culpa limit (-1: unlimited) and the reason dictionary, an iterable of
+        (reason code, mea culpa, failure limit; -2: the global one, -1: unlimited)."""
+        r = list(reasons)
+        code = np.ascontiguousarray([x[0] for x in r], np.int32)
+        mc = np.ascontiguousarray([bool(x[1]) for x in r], np.uint8)
+        lim = np.ascontiguousarray([x[2] for x in r], np.int32)
+        rc = self.lib.cook_state_retry_config(self.pool, int(mea_culpa_limit), len(r), abi.ptr(code, abi.P_I32),
+                                              abi.ptr(mc, abi.P_U8), abi.ptr(lim, abi.P_I32))
+        if rc != 0:
+            self._err(rc)
+
+    def state_retry_facts(self, job_id, max_retries, flags, done_reasons=None):
+        """cook_state_retry_facts: the retry facts of jobs the handle holds: max-retries, abi.RF_* bits and, per job,
+        the reason codes of its earlier done instances (-1: none; None: no done instance for any job)."""
+        jid = np.ascontiguousarray(job_id, np.int64)
+        mr = np.ascontiguousarray(max_retries, np.int32)
+        fl = np.ascontiguousarray(flags, np.uint8)
+        if not len(jid) == len(mr) == len(fl) or (done_reasons is not None and len(done_reasons) != len(jid)):
+            raise ValueError("state_retry_facts: the columns differ in length")
+        off = val = None
+        if done_reasons is not None:
+            off = np.zeros(len(jid) + 1, np.int32)
+            off[1:] = np.cumsum([len(d) for d in done_reasons])
+            val = np.ascontiguousarray([c for d in done_reasons for c in d] or [0], np.int32)
+        rc = self.lib.cook_state_retry_facts(self.pool, len(jid), abi.ptr(jid, abi.P_I64), abi.ptr(mr, abi.P_I32),
+                                             abi.ptr(fl, abi.P_U8), abi.ptr(off, abi.P_I32) if off is not None else None,
+                                             abi.ptr(val, abi.P_I32) if val is not None else None)
+        if rc != 0:
+            self._err(rc)
+        self._retry_jobs().update(jid.tolist())
+
+    def _retry_jobs(self):
+        """The job ids given retry facts (a superset of those the handle holds facts for), the parked jobs' group list
+        lengths and the job of each task launched from one: what state_status needs to track a requeue."""
+        if not hasattr(self, "_state_retry"):
+            self._state_retry = set()
+            self._state_parked_glen = {}
+            self._state_task_job = {}
+        return self._state_retry
+
+    def _forget_tasks(self, tids):
+        """Tasks that ended without state_status: the job loses its parked copy, and its facts unless it is a live
+        pending row again (the library's rule, restated for the bookkeeping).  A job has at most one task launched
+        from a parked row: a requeue needs every instance gone."""
+        if not hasattr(self, "_state_retry"):
+            return
+        for t in tids:
+            j = self._state_task_job.pop(t, None)
+            if j is not None:
+                self._state_parked_glen.pop(j, None)
+                if j not in getattr(self, "_state_pending_ids", ()):
+                    self._state_retry.discard(j)
+
+    def state_status(self, task_id, success, end_time_ms, reason_code=None, preempted=None):
+        """cook_state_status: state_finish_history plus each row's job decided in batch order; returns (outcome
+        abi.JOB_* per row, attempts consumed per row).  A requeued job is a live pending row again."""
+        tid = np.ascontiguousarray(task_id, np.int64)
+        ok = np.ascontiguousarray(success, np.uint8)
+        end = np.ascontiguousarray(end_time_ms, np.int64)
+        rs = np.ascontiguousarray(reason_code, np.int32) if reason_code is not None else None
+        pre = np.ascontiguousarray(preempted, np.uint8) if preempted is not None else None
+        if any(c is not None and len(c) != len(tid) for c in (end, ok, rs, pre)):
+            raise ValueError("state_status: a column differs in length from task_id")
+        out = np.zeros(max(len(tid), 1), np.int32)
+        att = np.zeros(max(len(tid), 1), np.int32)
+        rc = self.lib.cook_state_status(self.pool, len(tid), abi.ptr(tid, abi.P_I64), abi.ptr(ok, abi.P_U8),
+                                        abi.ptr(end, abi.P_I64), abi.ptr(rs, abi.P_I32) if rs is not None else None,
+                                        abi.ptr(pre, abi.P_U8) if pre is not None else None, abi.ptr(out, abi.P_I32),
+                                        abi.ptr(att, abi.P_I32))
+        if rc != 0:
+            self._err(rc)
+        getattr(self, "_state_running_ids", set()).difference_update(tid.tolist())
+        png, rng_ = self._group_lengths()
+        self._retry_jobs()
+        live = self._state_pending_ids = getattr(self, "_state_pending_ids", set())
+        for t, o in zip(tid.tolist(), out[:len(tid)].tolist()):
+            rng_.pop(t, None)
+            j = self._state_task_job.pop(t, None)
+            if j is None:
+                continue
+            if o == abi.JOB_WAITING:
+                live.add(j)
+                png[j] = self._state_parked_glen.pop(j, 0)
+            elif o == abi.JOB_COMPLETED:
+                self._state_parked_glen.pop(j, None)
+                self._state_retry.discard(j)
+        return out[:len(tid)].copy(), att[:len(tid)].copy()
 
     def state_history_seed(self, since_ms, task_id=(), user=(), start_ms=(), end_ms=(), cpus=(), mem=(), success=(),
                            reason_code=()):

@@ -475,11 +475,15 @@ int32_t cook_state_apply(cook_pool* pool, const cook_state_delta* delta);
  * from those rows with running_hostname_id = hostname_id and, as running_group_off / running_group_idx, the
  * pending rows' group lists: the job leaves the last rank's queue, its counts and reservation leave with the
  * row, its group list moves to the task (copied on the device, in launch order) while its other list
- * entries leave, and the list arenas compact by the same rule.
+ * entries leave, and the list arenas compact by the same rule.  A job with retry facts (cook_state_retry_facts)
+ * parks its pending slot instead: the same state for every reader, but the slot keeps its columns and lists for
+ * cook_state_status and stays off the free list; the compaction keeps its entries (one more launch while some slot
+ * is parked).
  * COOK_E_BADARG, before any change: n < 0; a NULL job_id, task_id or start_time while n > 0; a job id that
  * is not live or appears twice; a task id that appears twice or is already live; a hostname code below -1.
  * Uploads exactly n * (4 + 4 + 8 + 8) bytes (pending slot, running slot, task id, start time), plus 4 * n
- * when hostname_id is not NULL.  Statistics: cook_last_stats(COOK_PHASE_STATE).                        */
+ * when hostname_id is not NULL, plus 4 * n when some job of the batch parks (the parked and the freed slots).
+ * Statistics: cook_last_stats(COOK_PHASE_STATE).                                                        */
 int32_t cook_state_launch(cook_pool* pool, int32_t n, const int64_t* job_id, const int64_t* task_id,
                           const int64_t* start_time, const int32_t* hostname_id);
 
@@ -1039,6 +1043,81 @@ int32_t cook_state_finish_history(cook_pool* pool, int32_t n, const int64_t* tas
  * Uploads nothing; downloads 4 bytes (the rows kept) when the table holds a row and since_ms is above the horizon,
  * else nothing.  Statistics: cook_last_stats(COOK_PHASE_STATE).                                                 */
 int32_t cook_state_history_advance(cook_pool* pool, int64_t since_ms);
+
+/* ------------------------------------------------------------- retries */
+/* A failed task whose job has retries left returns the job to the queue without a row re-sent: the decision of
+ * :instance/update-state (scheduler/src/cook/schema.clj:1242-1300) taken per status on the host from per-job retry
+ * facts, and the requeue done on the device from the job's parked pending slot.
+ * Fixed choices:
+ *   Parking   cook_state_launch of a job with retry facts parks its pending slot instead of freeing it: the live flag is
+ *             cleared and the generation bumped as by a removal (the job leaves the queue and every reader, all of
+ *             which test the live flag), the columns and the three lists are kept, and the slot stays off the free
+ *             list, so parked slots count against the pending table's capacity.  The host's counts drop the row as a
+ *             launch does; the list compaction keeps the parked slots' entries and counts them as kept.  A job without
+ *             retry facts launches exactly as before, and while no job of a handle has retry facts no call changes its
+ *             behaviour, launches, transfers or cost.  Parked copies and facts are outside cook_state_digest and
+ *             cook_state_export: a resync does not repair them (the caller sends the facts again; a job whose copy is
+ *             gone answers COOK_JOB_WAITING_UNRETAINED and is upserted).
+ *   Decision  one status at a time, in batch order (Cook writes each status in its own transaction).  The attempts
+ *             consumed are reasons->attempts-consumed (:1154-1172) over the job's done instances, this one included:
+ *             a reason counts once per instance, -1 (nil) or a code outside the dictionary as a plain failure, a
+ *             success's reason too; a mea-culpa reason is free up to its limit (its failure limit, the global limit
+ *             when -2, 0 under COOK_RF_DISABLE_MEA_CULPA; -1 unlimited).  Then, in order: the job is COOK_RF_COMPLETED
+ *             -> COOK_JOB_COMPLETED (no change); a success, or no other live instance and attempts >= max_retries ->
+ *             COOK_JOB_COMPLETED; another live running or unknown instance of the job -> COOK_JOB_RUNNING; else
+ *             COOK_JOB_WAITING with a parked copy, COOK_JOB_WAITING_UNRETAINED without one (a job whose tasks came in
+ *             through running upserts: the caller upserts the row as before).
+ *   Requeue   the parked slot becomes live with a new generation, so it enters the queue at the next cook_state_rank as
+ *             an upsert would; reserved_host becomes -1 (the reservation was consumed at launch), the job facts of
+ *             cook_state_job_facts are cleared as by an upsert, allowed and plugin_accept stay.  The failed instance's
+ *             hostname code is appended to the novel-host list (novel-host-constraint, constraints.clj:68-94) unless
+ *             it is -1, the instance was preempted, or the list holds it.  A list that gains an entry moves to the
+ *             arena's tail on the device (an order-wide scan of the new lengths, then a warp per row); the others stay
+ *             in place.  The state then equals, for every reader, cook_state_finish_history followed by a
+ *             cook_state_apply upsert of that row with the appended list and reserved_host = -1.
+ *   Freeing   a parked copy is freed (its entries dead, its slot back on the free list) by a COOK_JOB_COMPLETED
+ *             decision; by cook_state_retry_facts with COOK_RF_COMPLETED while the job has no live instance; by a
+ *             pending upsert of its job id (the caller's row wins); by cook_state_finish or cook_state_finish_history
+ *             of the job's last live instance; by a reset.  A pending upsert or removal of a job id drops its facts;
+ *             so do a COOK_JOB_COMPLETED decision and a finish of the last live instance when the job has no live
+ *             pending row.
+ *
+ * cook_state_retry_config: the reason dictionary (reason_code[i], whether it is mea culpa, its failure limit: -2 none,
+ * use mea_culpa_limit; -1 unlimited) and the global mea-culpa limit (-1 unlimited), replacing the previous ones.  A
+ * fresh handle has limit 5 and an empty dictionary.  Host only: no transfer, no device work, no statistics.
+ * COOK_E_BADARG, with nothing changed: n_reasons < 0; a NULL array while n_reasons > 0; a negative or repeated code; a
+ * failure limit below -2; mea_culpa_limit below -1.                                                              */
+enum { COOK_RF_DISABLE_MEA_CULPA = 1, COOK_RF_COMPLETED = 2 };
+enum { COOK_JOB_COMPLETED = 0, COOK_JOB_RUNNING = 1, COOK_JOB_WAITING = 2, COOK_JOB_WAITING_UNRETAINED = 3,
+       COOK_JOB_NO_FACTS = 4 };
+int32_t cook_state_retry_config(cook_pool* pool, int32_t mea_culpa_limit, int32_t n_reasons, const int32_t* reason_code,
+                                const uint8_t* mea_culpa, const int32_t* failure_limit);
+
+/* The retry facts of jobs the handle holds (a live pending row, a parked copy or a live running instance), replacing
+ * earlier ones: max_retries[i] (:job/max-retries), flags[i] (COOK_RF_*: :job/disable-mea-culpa-retries, the job is
+ * completed) and the reason codes done_reason[done_off[i], done_off[i + 1]) of its earlier done (success or failed)
+ * instances, -1 for none; done_off NULL: no done instance.  The facts survive launch and requeue.  A job given
+ * COOK_RF_COMPLETED while it has no live instance loses its parked copy and its facts.
+ * COOK_E_BADARG, before any change: n < 0; a NULL job_id, max_retries or flags while n > 0; malformed CSR offsets; a
+ * reason code below -1; a negative max_retries; unknown flag bits; a job id the handle does not hold or listed twice.
+ * Uploads exactly 4 bytes per parked copy freed, else nothing.  Statistics: cook_last_stats(COOK_PHASE_STATE).   */
+int32_t cook_state_retry_facts(cook_pool* pool, int32_t n, const int64_t* job_id, const int32_t* max_retries,
+                               const uint8_t* flags, const int32_t* done_off, const int32_t* done_reason);
+
+/* Terminal statuses by task id: exactly cook_state_finish_history(pool, n, task_id, end_time_ms, success, reason_code)
+ * (the removal, the straggler records, the history append, the same checks), and in addition each row's job decided
+ * as above, in batch order: out_outcome[i] (COOK_JOB_*) and out_attempts[i] (the attempts consumed after this instance;
+ * -1 with COOK_JOB_NO_FACTS, the job having no facts, when nothing else happens).  The reason is reason_code[i] or,
+ * with reason_code NULL, the row's cook_state_task_reason fact; preempted[i] != 0 (:instance/preempted?) keeps the host
+ * off the novel-host list; NULL: none preempted.  Requeues and frees as above, on the device.
+ * COOK_E_BADARG, before any change: everything cook_state_finish_history rejects; a NULL out_outcome or out_attempts
+ * while n > 0.  COOK_E_TOO_LARGE: as cook_state_finish_history.
+ * Uploads exactly cook_state_finish_history's, plus 4 per requeued row (its slot), 8 per requeued row whose list gains
+ * a host (its slot and the code) and 4 per parked copy freed.  Downloads nothing.
+ * Statistics: cook_last_stats(COOK_PHASE_STATE).                                                                  */
+int32_t cook_state_status(cook_pool* pool, int32_t n, const int64_t* task_id, const uint8_t* success,
+                          const int64_t* end_time_ms, const int32_t* reason_code, const uint8_t* preempted,
+                          int32_t* out_outcome, int32_t* out_attempts);
 
 /* The record table by hand: first every record of the groups forget_group[0, n_forget) leaves (groups the caller no
  * longer tracks), then n_add records (group[i], runtime_s[i]) are appended: the successes that finished before the

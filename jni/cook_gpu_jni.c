@@ -370,6 +370,26 @@ JFN(jint, stateFinishHistory)(JNIEnv* env, jclass k, jlong pool, jint n, jobject
   return cook_state_finish_history((cook_pool*)(intptr_t)pool, n, one(env, task_id), one(env, end_time_ms),
                                    one(env, success), one(env, reason_code));
 }
+/* the reason dictionary: reason_code n_reasons ints, mea_culpa n_reasons bytes, failure_limit n_reasons ints */
+JFN(jint, stateRetryConfig)(JNIEnv* env, jclass k, jlong pool, jint mea_culpa_limit, jint n_reasons, jobject reason_code,
+                            jobject mea_culpa, jobject failure_limit) {
+  return cook_state_retry_config((cook_pool*)(intptr_t)pool, mea_culpa_limit, n_reasons, one(env, reason_code),
+                                 one(env, mea_culpa), one(env, failure_limit));
+}
+/* jobs' retry facts: job_id n longs, max_retries n ints, flags n bytes (COOK_RF_*), done_off n + 1 ints and
+   done_reason ints (null: no done instance) */
+JFN(jint, stateRetryFacts)(JNIEnv* env, jclass k, jlong pool, jint n, jobject job_id, jobject max_retries, jobject flags,
+                           jobject done_off, jobject done_reason) {
+  return cook_state_retry_facts((cook_pool*)(intptr_t)pool, n, one(env, job_id), one(env, max_retries), one(env, flags),
+                                one(env, done_off), one(env, done_reason));
+}
+/* terminal statuses: as stateFinishHistory, plus preempted n bytes (null: none) and the outputs out_outcome and
+   out_attempts, n ints each */
+JFN(jint, stateStatus)(JNIEnv* env, jclass k, jlong pool, jint n, jobject task_id, jobject success, jobject end_time_ms,
+                       jobject reason_code, jobject preempted, jobject out_outcome, jobject out_attempts) {
+  return cook_state_status((cook_pool*)(intptr_t)pool, n, one(env, task_id), one(env, success), one(env, end_time_ms),
+                           one(env, reason_code), one(env, preempted), one(env, out_outcome), one(env, out_attempts));
+}
 /* the history's seed: cols the direct buffers of task_id, user, start_ms, end_ms, cpus, mem, success, reason_code */
 JFN(jint, stateHistorySeed)(JNIEnv* env, jclass k, jlong pool, jlong since_ms, jint n, jobjectArray cols) {
   return cook_state_history_seed((cook_pool*)(intptr_t)pool, since_ms, n, buf(env, cols, 0), buf(env, cols, 1),

@@ -57,6 +57,13 @@ the dict of counters), with the answers compared bit for bit:
 and times cook_state_unscheduled for one job, 1000 jobs and every waiting job of the user with the most, against numpy
 over a host mirror, with the answers compared bit for bit:
   python tools/prof_state.py --unscheduled --pool c2 --reps 20
+--status loads C2 (or config-#5 pool --c5-pool with --pool c5) into two resident handles, gives every job of one retry
+facts, and per rep launches --status-batch jobs on both (timing cook_state_launch with and without facts), then fails
+them: cook_state_status (every job parked, so every one is requeued on the device) against the host path it replaces,
+the requeued rows rebuilt from a host mirror, cook_state_finish_history and a cook_state_apply upsert, alternated,
+with the two handles' digests compared after every rep:
+  python tools/prof_state.py --status --pool c2 --reps 10
+  python tools/prof_state.py --status --pool c5 --c5-pool 5 --reps 10
 
 --launch runs the same cycles on two resident handles instead of the host arm.  Each cycle's launches go to one
 handle through cook_state_launch (job ids, task ids, start times, the hosts the match chose) and to its twin through
@@ -1404,6 +1411,84 @@ def match_metrics_prof(a):
     e.close()
 
 
+def requeued_soa(store, rows, host):
+    """The host path cook_state_status replaces: the pending rows of failed jobs rebuilt from the host mirror with
+    reserved_host -1 and the failed host appended to the novel-host list (unless -1 or already listed)."""
+    soa = store.soa(rows)
+    off, val = soa.col("novel_off"), soa.col("novel_host")
+    lists = [val[off[i]:off[i + 1]].tolist() if off is not None else [] for i in range(len(rows))]
+    for lst, h in zip(lists, host.tolist()):
+        if h != -1 and h not in lst:
+            lst.append(h)
+    noff = np.zeros(len(rows) + 1, np.int32)
+    noff[1:] = np.cumsum([len(x) for x in lists])
+    nval = np.asarray([h for x in lists for h in x] or [0], np.int32)
+    return _with(soa, reserved_host=np.full(len(rows), -1, np.int32), novel_off=noff, novel_host=nval)
+
+
+def status_prof(a):
+    """cook_state_status against the host path it replaces (requeued rows rebuilt from a host mirror, then
+    cook_state_finish_history and a cook_state_apply upsert), alternated in one run on two handles holding the same
+    rows (C2, or config-#5 pool --c5-pool with --pool c5): per rep, a launch of --status-batch jobs on both (with and
+    without retry facts), then their failures with retries left.  Every requeued job is parked, and the two handles'
+    digests must stay equal."""
+    t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
+    jobs, pc = t["jobs"], t["cols"]["pending"]
+    J, B = jobs.n, a.status_batch
+    store = Jobs(jobs, pc["priority"], pc["job_id"])
+    print(json.dumps({"card": card(), "pool": a.pool, "jobs": J, "batch": B}), flush=True)
+    res, twin = GpuEngine(pool_name="status"), GpuEngine(pool_name="twin")
+    for e in (res, twin):
+        e.state_apply(abi.make_delta(reset=True, pending=store.soa(np.arange(J)), pending_priority=store.prio,
+                                     pending_job_id=store.jid))
+    res.state_retry_config(5, [])
+    res.state_retry_facts(store.jid, np.full(J, 1000, np.int32), np.zeros(J, np.uint8))
+    rng = np.random.default_rng(a.seed)
+    n_hosts = max(t["offers"].n, 1)
+    tid = 1 << 40
+    out = {"launch_facts": [], "launch_plain": [], "status": [], "host_path": []}
+    order = rng.permutation(J)   # each job fails once: the host mirror's lists stay the trace's
+    for rep in range(a.reps + 1):
+        rows = np.sort(order[rep * B:(rep + 1) * B])
+        jid, host = store.jid[rows], rng.integers(0, n_hosts, B).astype(np.int32)
+        tids = np.arange(tid, tid + B, dtype=np.int64)
+        tid += B
+        start = np.full(B, 1_700_000_000_000, np.int64)
+        end, ok, reason = start + 1000, np.zeros(B, np.uint8), np.full(B, -1, np.int32)
+        for e, kind in ((res, "launch_facts"), (twin, "launch_plain"))[::1 if rep % 2 else -1]:
+            t0 = time.perf_counter()
+            e.state_launch(jid, tids, start, host)
+            wall = time.perf_counter() - t0
+            if rep:
+                st = e.last_stats(abi.PHASE_STATE)
+                out[kind].append((wall * 1e3, st["ms_device"], st["h2d_bytes"], st["n_launches"]))
+
+        def host_path():
+            soa = requeued_soa(store, rows, host)
+            twin.state_finish_history(tids, end, ok, reason)
+            twin.state_apply(abi.make_delta(pending=soa, pending_priority=store.prio[rows], pending_job_id=jid))
+
+        for kind in (("status", "host_path") if rep % 2 else ("host_path", "status")):
+            t0 = time.perf_counter()
+            if kind == "status":
+                oc, _ = res.state_status(tids, ok, end, reason)
+                assert (oc == abi.JOB_WAITING).all()
+            else:
+                host_path()
+            if rep:
+                out[kind].append((time.perf_counter() - t0) * 1e3)
+        da, db = res.state_digest(), twin.state_digest()
+        assert da["pending"] == db["pending"] and da["running"] == db["running"], "the two handles differ"
+    med = lambda xs, k=None: float(np.median([x[k] if k is not None else x for x in xs]))   # noqa: E731
+    print(json.dumps({
+        "status_wall_ms": med(out["status"]), "host_path_wall_ms": med(out["host_path"]),
+        "launch_with_facts": {"wall_ms": med(out["launch_facts"], 0), "device_ms": med(out["launch_facts"], 1),
+                              "h2d": out["launch_facts"][-1][2], "launches": out["launch_facts"][-1][3]},
+        "launch_without_facts": {"wall_ms": med(out["launch_plain"], 0), "device_ms": med(out["launch_plain"], 1),
+                                 "h2d": out["launch_plain"][-1][2], "launches": out["launch_plain"][-1][3]},
+        "reps": a.reps, "identical": True}), flush=True)
+
+
 def rank_quota_prof(a):
     t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
     pc, rc0, users = t["cols"]["pending"], t["cols"]["running"], t["users"]
@@ -1474,9 +1559,14 @@ def main():
     ap.add_argument("--history-stats", action="store_true",
                     help="cook_state_history_stats against numpy over a host mirror (--c3-group N: N config-#3 pools)")
     ap.add_argument("--history-rows", type=int, default=1_000_000, help="--history-stats: the finished rows in all")
+    ap.add_argument("--status", action="store_true",
+                    help="cook_state_status against rebuilding and re-sending the rows (C2 or --pool c5)")
+    ap.add_argument("--status-batch", type=int, default=1000, help="--status: the launches and failures per rep")
     ap.add_argument("--match-metrics", action="store_true",
                     help="cook_state_match_metrics after each match against numpy over a host mirror (C2 or --pool c5)")
     a = ap.parse_args()
+    if a.status:
+        return status_prof(a)
     if a.match_metrics:
         return match_metrics_prof(a)
     if a.history_stats:
