@@ -18,6 +18,9 @@
 ;;                                              task-reason! [cook_state_instance_stats, cook_state_task_reason], and
 ;;                                              for success / failed by history-seed!, finish-history! and
 ;;                                              history-advance! [cook_state_history_*]
+;;   api.clj:3038-3085 list-resource, :1684-1776 list-job-ents (waiting, running)
+;;                                           -> (list-jobs ...) + cycle.py's list_jobs_response, fed by list-facts!
+;;                                              [cook_state_list_jobs, cook_state_list_facts]
 ;;   :217-313 write-status-to-datomic       -> (status! ...), fed by retry-config! and retry-facts!
 ;;                                             [cook_state_status, cook_state_retry_config, cook_state_retry_facts]
 ;;   :1210-1280 handle-match-cycle-metrics and the unmatched tracking :1399-1486
@@ -585,6 +588,49 @@
                                              (vec (for [j (range 5)] (f64 (segs 5) (+ (* 15 d) (* 5 m) j))))))}))
        :leaders-cpu (lead 0)
        :leaders-mem (lead 1)})))
+
+;; ---------------------------------------------------------------------------------------------
+;; /list and /jobs over resident pools: the device half of get-active-jobs-by-user-and-state (tools.clj:445-466) for
+;; the waiting and running states; completed, success and failed, a name filter and a non-zero missing count keep the
+;; Datomic path
+(defn list-facts!
+  "The attributes the listing filters on, from the tx-report tap with each job upsert (which clears them), pending or
+   running: [{:job-id :submit-ms :submit-pool (code, nil: none) :custom-executor (true, false or nil)}].  They never
+   change over a job's life, so a launch and a requeue keep them."
+  [handle jobs]
+  (check! handle (Native/stateListFacts handle (count jobs) (longs-buf (map :job-id jobs))
+                                        (longs-buf (map :submit-ms jobs)) (ints-buf (map #(or (:submit-pool %) -1) jobs))
+                                        (ints-buf (map #(case (:custom-executor %) true 1 false 0 -1) jobs)))
+          "cook_state_list_facts"))
+
+(defn list-jobs
+  "`user`'s jobs in `states` (#{:waiting :running}) over `handles` (one device) submitted in [start-ms, end-ms), with
+   entity ids in [job-id-lo, job-id-hi) (d/entid-at of start - 1 h and end + 1 h), in pool `pool-code` (-1: any;
+   `handle-pools` each handle's pool code), only false custom executors unless `include-custom-executor?`, each state
+   cut to `limit`.  The call is made with `cap` entries and, when it needs more, once more with the count it reports.
+   Returns {:waiting [job-id] :running [job-id] :submit-ms {job-id ms} :missing n}, each state in entity-id order, for
+   fetch-job-map; a non-zero :missing keeps the Datomic path.  The handler merges and orders the states as
+   cook_b200/cycle.py's list_jobs_response does."
+  [handles user states start-ms end-ms job-id-lo job-id-hi pool-code handle-pools include-custom-executor? limit cap]
+  (loop [cap (max cap 1) tries 2]
+    (let [outs [(direct (* 4 cap)) (direct (* 8 cap)) (direct (* 8 cap)) (direct (* 4 cap))]
+          out-n (int-array 2)
+          rc (Native/stateListJobs (long-array handles) (long-array [start-ms end-ms job-id-lo job-id-hi])
+                                   (int-array [user (+ (if (states :waiting) 1 0) (if (states :running) 2 0)) pool-code
+                                               (if include-custom-executor? 1 0) limit cap])
+                                   (when (not= pool-code -1) (ints-buf handle-pools)) (object-array outs) out-n nil)]
+      (if (and (= rc -7) (> tries 1))
+        (recur (aget out-n 0) (dec tries))
+        (do (check! (first handles) rc "cook_state_list_jobs")
+            (let [n (aget out-n 0)
+                  at (fn [i] {:state (.getInt ^ByteBuffer (outs 0) (int (* 4 i)))
+                              :job-id (.getLong ^ByteBuffer (outs 1) (int (* 8 i)))
+                              :submit-ms (.getLong ^ByteBuffer (outs 2) (int (* 8 i)))})
+                  es (mapv at (range n))]
+              {:waiting (vec (for [e es :when (= 1 (:state e))] (:job-id e)))
+               :running (vec (for [e es :when (= 2 (:state e))] (:job-id e)))
+               :submit-ms (into {} (map (juxt :job-id :submit-ms)) es)
+               :missing (aget out-n 1)}))))))
 
 ;; ---------------------------------------------------------------------------------------------
 ;; the match-cycle metrics of a resident pool (handle-match-cycle-metrics scheduler.clj:1210-1280, the unmatched

@@ -167,6 +167,9 @@ JF_GPUS, JF_DISK, JF_DISK_REQUEST, JF_DISK_LIMIT, JF_URIS = 1, 2, 4, 8, 16
 MM_GPUS, MM_DISK_REQUEST, MM_DISK_LIMIT = 0, 1, 2
 MM_FIRST_N = 10
 
+# cook_state_list_jobs' states
+LJ_WAITING, LJ_RUNNING = 1, 2
+
 # cook_state_retry_facts' bits and cook_state_status' outcomes
 RF_DISABLE_MEA_CULPA, RF_COMPLETED = 1, 2
 JOB_COMPLETED, JOB_RUNNING, JOB_WAITING, JOB_WAITING_UNRETAINED, JOB_NO_FACTS = 0, 1, 2, 3, 4
@@ -356,6 +359,9 @@ ARGTYPES = {
     "cook_state_task_facts": [_H, _I32, P_I64, P_I64, P_U8, P_U8],
     "cook_state_task_reason": [_H, _I32, P_I64, P_I32],
     "cook_state_job_facts": [_H, _I32, P_I64, P_U8, P_I32, P_F64, P_F64, P_I32],
+    "cook_state_list_facts": [_H, _I32, P_I64, P_I64, P_I32, P_I32],
+    "cook_state_list_jobs": [_P(_H), _I32, _I32, _I32, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _I32, P_I32, _I32,
+                             _I32, _I32, P_I32, P_I64, P_I64, P_I32, P_I32, P_I32, _P(PhaseStats)],
     "cook_state_match_metrics": [_H, _I32, _I32, P_I32, _I32, _I32, P_I64, P_F64, P_I64, P_F64, P_I64, P_I32, P_I32,
                                  P_I32, P_I32, P_I32, P_F64, _P(PhaseStats)],
     "cook_state_finish": [_H, _I32, P_I64, P_I64, P_U8],

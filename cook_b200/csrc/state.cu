@@ -39,18 +39,21 @@ enum PCol {
   P_USER, P_PRIO, P_JID, P_CPUS, P_MEM, P_GPUS, P_PORTS, P_ALLOWED, P_PLUGIN, P_GPU_MODEL, P_DISK_REQ, P_DISK_TYPE,
   P_EST, P_CKPT, P_RESERVED, P_NDATA,   // the columns a delta row carries
   P_LIVE = P_NDATA, P_GEN, P_NOFF, P_NLEN, P_AOFF, P_ALEN, P_GOFF, P_GLEN,
-  P_JF, P_JF_GPU, P_JF_DREQ, P_JF_DLIM, P_JF_DTYPE, P_NCOL
+  P_JF, P_JF_GPU, P_JF_DREQ, P_JF_DLIM, P_JF_DTYPE, P_LF_SUBMIT, P_LF_POOL, P_LF_EXEC, P_NCOL
 };
-constexpr int P_SZ[P_NCOL] = {4, 4, 8, 8, 8, 8, 4, 1, 1, 4, 8, 4, 8, 4, 4, 1, 4, 4, 4, 4, 4, 4, 4, 1, 4, 8, 8, 4};
+constexpr int P_SZ[P_NCOL] = {4, 4, 8, 8, 8, 8, 4, 1, 1, 4, 8, 4, 8, 4, 4, 1, 4, 4, 4, 4, 4, 4, 4, 1, 4, 8, 8, 4, 8, 4, 1};
 // P_JF .. P_JF_DTYPE are the job facts cook_state_job_facts writes (the stats keys of jobs->resource-maps): the
 // COOK_JF_* bits, then the gpu model, disk request, disk limit and disk type, each read only under its bit.  Every
 // pending upsert writes P_JF = 0, so the others need no reset.
+// P_LF_* / R_LF_* are the list facts cook_state_list_facts writes (what /list and /jobs filter on): the submit time
+// in ms, the submit pool's code (-1: none) and LF_EXEC, 0 for no facts, else 2 + :job/custom-executor (-1 nil, 0
+// false, 1 true).  Every upsert writes LF_EXEC 0, so the others are read only once written; a launch copies them.
 // R_MAXRT and R_FACTS are the facts cook_state_task_facts writes: the job's max-runtime (-1: none) and the
 // RF_* bits; R_REASON the fact cook_state_task_reason writes: the instance's reason code (-1: none).  Every upsert
 // and launch writes their absent values.
 enum RCol { R_USER, R_PRIO, R_START, R_TID, R_JID, R_CPUS, R_MEM, R_GPUS, R_HOST, R_NDATA, R_LIVE = R_NDATA, R_GEN,
-            R_GOFF, R_GLEN, R_MAXRT, R_FACTS, R_REASON, R_NCOL };
-constexpr int R_SZ[R_NCOL] = {4, 4, 8, 8, 8, 8, 8, 8, 4, 1, 4, 4, 4, 8, 1, 4};
+            R_GOFF, R_GLEN, R_MAXRT, R_FACTS, R_REASON, R_LF_SUBMIT, R_LF_POOL, R_LF_EXEC, R_NCOL };
+constexpr int R_SZ[R_NCOL] = {4, 4, 8, 8, 8, 8, 8, 8, 4, 1, 4, 4, 4, 8, 1, 4, 8, 4, 1};
 enum { RF_CANCELLED = 1, RF_UNKNOWN = 2 };
 
 // The live offers (leases): one row per offer as it arrived, before any merge.  Data columns first, then the live
@@ -72,9 +75,10 @@ enum { OL_PORT = 0, OL_GPU = 1, OL_DISK = 2, OL_ATTR = 3, OL_N };
 // generation, which is what retires a queue entry.  A patch (live null) writes its columns only: the
 // slot keeps its live flag and generation, so its queue entry stays.
 constexpr int MAXC = 16;
+constexpr int SCATTER_MAXC = MAXC + 1;   // a pending upsert: its data columns, then the job and list facts' resets
 struct ScatterCol { char* dst; const char* src; long long dflt; int sz; };
 struct ScatterArgs {
-  ScatterCol c[MAXC];
+  ScatterCol c[SCATTER_MAXC];
   int nc, n, upsert;
   const int32_t* slot;
   uint8_t* live;           // null: a patch
@@ -90,7 +94,7 @@ __global__ void scatter_kernel(ScatterArgs a) {
   if (i >= a.n) return;
   const int s = a.slot[i];
 #pragma unroll
-  for (int k = 0; k < MAXC; k++) {
+  for (int k = 0; k < SCATTER_MAXC; k++) {
     if (k >= a.nc) break;
     const ScatterCol& c = a.c[k];
     if (c.sz == 1) reinterpret_cast<uint8_t*>(c.dst)[s] = c.src ? reinterpret_cast<const uint8_t*>(c.src)[i] : (uint8_t)c.dflt;
@@ -135,6 +139,9 @@ __global__ void launch_kernel(const int32_t* pslot, const int32_t* rslot, const 
   static_cast<int64_t*>(rc[R_MAXRT])[r] = -1;
   static_cast<uint8_t*>(rc[R_FACTS])[r] = 0;
   static_cast<int32_t*>(rc[R_REASON])[r] = -1;
+  static_cast<int64_t*>(rc[R_LF_SUBMIT])[r] = static_cast<const int64_t*>(pc[P_LF_SUBMIT])[s];
+  static_cast<int32_t*>(rc[R_LF_POOL])[r] = static_cast<const int32_t*>(pc[P_LF_POOL])[s];
+  static_cast<uint8_t*>(rc[R_LF_EXEC])[r] = static_cast<const uint8_t*>(pc[P_LF_EXEC])[s];
 }
 
 // ---- list lengths for the order-wide scan (integer sums: any association is exact)
@@ -1309,7 +1316,8 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
         pu.c[k] = ScatterCol{static_cast<char*>(S->pend.col[k]), up, dflt[k], P_SZ[k]};
       }
       pu.c[P_NDATA] = ScatterCol{static_cast<char*>(S->pend.col[P_JF]), nullptr, 0, P_SZ[P_JF]};   // no job facts
-      pu.nc = P_NDATA + 1;
+      pu.c[P_NDATA + 1] = ScatterCol{static_cast<char*>(S->pend.col[P_LF_EXEC]), nullptr, 0, 1};     // no list facts
+      pu.nc = P_NDATA + 2;
       pu.slot = c.up(pup_slot.data(), np);
       for (int l = 0; l < 3; l++) {
         pu.doff[l] = c.up(lists_off[l], np + 1);
@@ -1331,7 +1339,8 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
       ru.c[R_NDATA] = ScatterCol{static_cast<char*>(S->run.col[R_MAXRT]), nullptr, -1, R_SZ[R_MAXRT]};
       ru.c[R_NDATA + 1] = ScatterCol{static_cast<char*>(S->run.col[R_FACTS]), nullptr, 0, R_SZ[R_FACTS]};
       ru.c[R_NDATA + 2] = ScatterCol{static_cast<char*>(S->run.col[R_REASON]), nullptr, -1, R_SZ[R_REASON]};
-      ru.nc = R_NDATA + 3;
+      ru.c[R_NDATA + 3] = ScatterCol{static_cast<char*>(S->run.col[R_LF_EXEC]), nullptr, 0, 1};   // no list facts
+      ru.nc = R_NDATA + 4;
       ru.slot = c.up(rup_slot.data(), nr);
       ru.doff[0] = c.up(rgo, nr + 1);
       if (c.base && radd) c.copy(RG.v[0] + rtail0, d->running_group_idx, radd);
@@ -6359,4 +6368,293 @@ extern "C" int32_t cook_state_match_metrics(cook_pool* pool, int32_t n_users, in
                      out_user_considerable, out_user_matched, out_key_kind, out_key_code, out_key_total};
   return match_metrics(pool, static_cast<PoolState*>(pool->state), n_users, n_dropped, dropped, unmatched_warn_cycles,
                        key_cap, out, out_stats);
+}
+
+// ---- job listing (/list, /jobs for the waiting and running states; get-active-jobs-by-user-and-state,
+// tools.clj:445-466).  Per state: one flag pass per handle marks the user's live rows and counts those in the id window
+// without list facts; a compaction gathers them (job id, task id, pool index, submit time and whether the entry passes
+// the filters) after the handles before; one sort by (job id, pool index, task id descending) orders them across the
+// handles and puts each running job's representative first; a second compaction keeps the first row of each
+// (job id, pool index) that passes, up to `limit`, straight into the download buffers.
+namespace {
+
+struct LJCols {   // one table's columns the listing reads; tid null for the pending table
+  const uint8_t* live; const int32_t* user; const int64_t* jid; const int64_t* tid; const int64_t* submit;
+  const int32_t* spool; const uint8_t* exec;
+};
+struct LJSel { int64_t start, end, lo, hi; int32_t pool; int32_t all_exec; };
+
+__global__ void lj_flag_kernel(LJCols c, int n, int32_t user, int64_t lo, int64_t hi, uint8_t* flag, int32_t* missing) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  bool miss = false;
+  if (i < n) {
+    const bool mine = c.live[i] && c.user[i] == user;
+    flag[i] = mine;
+    miss = mine && c.exec[i] == 0 && c.jid[i] >= lo && c.jid[i] < hi;
+  }
+  const int m = __reduce_add_sync(FULL_MASK, miss ? 1 : 0);
+  if ((threadIdx.x & 31) == 0 && m) atomicAdd(missing, m);
+}
+
+// the flagged rows of one handle, dense after the handles before it (base); pool_ok: the handle is the requested pool
+struct LJRows {
+  LJCols c; const uint8_t* flag; int base; int32_t pidx; bool pool_ok; LJSel q;
+  int64_t* jid; int64_t* tid; int32_t* pi; int64_t* submit; uint8_t* ok;
+  __device__ bool keep(int i) const { return flag[i]; }
+  __device__ void emit(int i, int d) const {
+    d += base;
+    const int64_t j = c.jid[i], s = c.submit[i];
+    const uint8_t e = c.exec[i];
+    jid[d] = j;
+    if (tid) tid[d] = c.tid[i];
+    pi[d] = pidx;
+    submit[d] = s;
+    ok[d] = e != 0 && s >= q.start && s < q.end && j >= q.lo && j < q.hi && (pool_ok || c.spool[i] == q.pool) &&
+            (q.all_exec || e == 2);
+  }
+};
+
+// (job id, pool index, task id descending, dense index): a job's rows in one handle together, the representative first
+struct LessJobPoolTask {
+  const int64_t* jid; const int32_t* pi; const int64_t* tid;
+  __device__ bool operator()(int32_t a, int32_t b) const {
+    if (jid[a] != jid[b]) return jid[a] < jid[b];
+    if (pi[a] != pi[b]) return pi[a] < pi[b];
+    if (tid && tid[a] != tid[b]) return tid[a] > tid[b];
+    return a < b;
+  }
+};
+
+struct LJPick {
+  const int32_t* ord; const int64_t* jid; const int32_t* pi; const int64_t* submit; const uint8_t* ok;
+  int64_t* o_jid; int64_t* o_submit; int32_t* o_pi;
+  __device__ bool keep(int p) const {
+    const int i = ord[p];
+    if (p > 0) {
+      const int k = ord[p - 1];
+      if (jid[k] == jid[i] && pi[k] == pi[i]) return false;
+    }
+    return ok[i];
+  }
+  __device__ void emit(int p, int d) const {
+    const int i = ord[p];
+    o_jid[d] = jid[i]; o_submit[d] = submit[i]; o_pi[d] = pi[i];
+  }
+};
+
+LJCols lj_cols(const PoolState* s, bool running) {
+  if (running) {
+    const Table& t = s->run;
+    return {t.at<uint8_t>(R_LIVE), t.at<int32_t>(R_USER), t.at<int64_t>(R_JID), t.at<int64_t>(R_TID),
+            t.at<int64_t>(R_LF_SUBMIT), t.at<int32_t>(R_LF_POOL), t.at<uint8_t>(R_LF_EXEC)};
+  }
+  const Table& t = s->pend;
+  return {t.at<uint8_t>(P_LIVE), t.at<int32_t>(P_USER), t.at<int64_t>(P_JID), nullptr, t.at<int64_t>(P_LF_SUBMIT),
+          t.at<int32_t>(P_LF_POOL), t.at<uint8_t>(P_LF_EXEC)};
+}
+
+int32_t list_facts(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, const int64_t* submit_ms,
+                   const int32_t* submit_pool, const int32_t* custom_executor) {
+  const char* who = "cook_state_list_facts";
+  if (n < 0) return set_err(pool, COOK_E_BADARG, "%s: n < 0", who);
+  if (n && !job_id) return set_err(pool, COOK_E_BADARG, "%s: null job_id", who);
+  for (int i = 0; custom_executor && i < n; i++)
+    if (custom_executor[i] < -1 || custom_executor[i] > 1)
+      return set_err(pool, COOK_E_BADARG, "%s: a custom_executor outside {-1, 0, 1}", who);
+  if (!idx_in_range(submit_pool, n, -1, INT32_MAX)) return set_err(pool, COOK_E_BADARG, "%s: a submit pool code below -1", who);
+  // the rows written: the job's live pending row, then each of its live running rows; k: the batch row it takes from
+  std::vector<int32_t> pslot, pk, rslot, rk;
+  {
+    std::unordered_set<int64_t> seen;
+    seen.reserve((size_t)n);
+    for (int i = 0; i < n; i++) {
+      if (!seen.insert(job_id[i]).second) return set_err(pool, COOK_E_BADARG, "%s: job id twice", who);
+      auto p = S->pend.slot_of.find(job_id[i]);
+      auto r = S->jobs_r.find(job_id[i]);
+      if (p == S->pend.slot_of.end() && r == S->jobs_r.end())
+        return set_err(pool, COOK_E_BADARG, "%s: a job id neither live-pending nor live-running", who);
+      if (p != S->pend.slot_of.end()) { pslot.push_back(p->second); pk.push_back(i); }
+      if (r != S->jobs_r.end())
+        for (int32_t s : r->second) { rslot.push_back(s); rk.push_back(i); }
+    }
+  }
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  // ---- the values per row written (LF_EXEC stores 2 + custom_executor), then one patch scatter per table
+  const int np = (int)pslot.size(), nr = (int)rslot.size(), m = np + nr;
+  std::vector<int64_t> sub(submit_ms ? m : 0);
+  std::vector<int32_t> sp(submit_pool ? m : 0);
+  std::vector<uint8_t> ex(custom_executor ? m : 0);
+  for (int w = 0; w < m; w++) {
+    const int i = w < np ? pk[w] : rk[w - np];
+    if (submit_ms) sub[w] = submit_ms[i];
+    if (submit_pool) sp[w] = submit_pool[i];
+    if (custom_executor) ex[w] = (uint8_t)(custom_executor[i] + 2);
+  }
+  const bool cols = submit_ms || submit_pool || custom_executor;
+  ScatterArgs pa, ra;
+  memset(&pa, 0, sizeof(pa)); memset(&ra, 0, sizeof(ra));
+  int64_t h2d = 0;
+  CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
+    if (!cols) return;
+    const auto fill = [&](ScatterArgs& a, const Table& t, const int32_t* slot, int k, int off, int c_sub, int c_pool,
+                          int c_exec) {
+      if (!k) return;
+      a.slot = c.up(slot, k);
+      if (submit_ms) a.c[a.nc++] = ScatterCol{static_cast<char*>(t.col[c_sub]), reinterpret_cast<const char*>(c.up(sub.data() + off, k)), 0, 8};
+      if (submit_pool) a.c[a.nc++] = ScatterCol{static_cast<char*>(t.col[c_pool]), reinterpret_cast<const char*>(c.up(sp.data() + off, k)), 0, 4};
+      if (custom_executor) a.c[a.nc++] = ScatterCol{static_cast<char*>(t.col[c_exec]), reinterpret_cast<const char*>(c.up(ex.data() + off, k)), 0, 1};
+    };
+    fill(pa, S->pend, pslot.data(), np, 0, P_LF_SUBMIT, P_LF_POOL, P_LF_EXEC);
+    fill(ra, S->run, rslot.data(), nr, np, R_LF_SUBMIT, R_LF_POOL, R_LF_EXEC);
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  int nl = 0;
+  scatter(pa, S->pend, cols ? np : 0, 0, -1, nullptr, st, &nl);
+  scatter(ra, S->run, cols ? nr : 0, 0, -1, nullptr, st, &nl);
+  CK(pool, cudaGetLastError());
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  CK(pool, cudaStreamSynchronize(st));
+  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
+  return COOK_OK;
+}
+
+int32_t list_jobs(cook_pool* const* pools, int n, int32_t user, int32_t states, const LJSel& q, const int32_t* handle_pool,
+                  int32_t limit, int32_t cap, int32_t* o_state, int64_t* o_jid, int64_t* o_submit, int32_t* o_pool,
+                  int32_t* o_n, int32_t* o_missing, cook_phase_stats* out_stats) {
+  const char* who = "cook_state_list_jobs";
+  // ---- every check before any device work or output
+  if (!pools || n <= 0 || !pools[0]) return COOK_E_BADARG;
+  cook_pool* pool = pools[0];
+  if (int32_t rc = is_handles(pools, n, who)) return rc;
+  if (states <= 0 || (states & ~(COOK_LJ_WAITING | COOK_LJ_RUNNING)))
+    return set_err(pool, COOK_E_BADARG, "%s: states 0 or with unknown bits", who);
+  if (user < 0) return set_err(pool, COOK_E_BADARG, "%s: a negative user", who);
+  if (q.pool < -1 || (q.pool != -1 && !handle_pool))
+    return set_err(pool, COOK_E_BADARG, "%s: pool_code below -1, or no handle_pool", who);
+  if (q.all_exec != 0 && q.all_exec != 1) return set_err(pool, COOK_E_BADARG, "%s: include_custom_executor outside {0, 1}", who);
+  if (limit < 0 || cap < 0) return set_err(pool, COOK_E_BADARG, "%s: limit < 0 or cap < 0", who);
+  if (!o_state || !o_jid || !o_submit || !o_pool || !o_n || !o_missing) return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
+  // per state (0 waiting, 1 running): the handles holding a row of the user, and the rows (the host-side counts)
+  struct Src { const PoolState* s; int32_t k; int rows; };
+  std::vector<Src> hs[2];
+  int64_t C[2] = {0, 0};
+  int hw = 0;
+  for (int t = 0; t < 2; t++) {
+    if (!(states & (t ? COOK_LJ_RUNNING : COOK_LJ_WAITING))) continue;
+    for (int k = 0; k < n; k++) {
+      const PoolState* s = static_cast<const PoolState*>(pools[k]->state);
+      if (!s) continue;
+      const auto& users = t ? s->users_r : s->users_p;
+      auto it = users.find(user);
+      if (it == users.end()) continue;
+      hs[t].push_back({s, k, (int)it->second});
+      C[t] += it->second;
+      hw = std::max(hw, t ? s->run.hw : s->pend.hw);
+    }
+  }
+  if (C[0] > INT32_MAX || C[1] > INT32_MAX) return set_err(pool, COOK_E_TOO_LARGE, "%s: more than 2^31 - 1 rows in a state", who);
+  if (C[0] + C[1] == 0) {   // no row to read: empty results without device work
+    *o_n = 0;
+    *o_missing = 0;
+    if (out_stats) *out_stats = cook_phase_stats{};
+    return COOK_OK;
+  }
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S0 = state_of(pool, true);   // pools[0]'s scratch, even when it holds no row
+  if (!S0) return set_err(pool, COOK_E_OOM, "%s: out of device memory", who);
+  cudaStream_t st = pool->stream;
+  // ---- one carve: the flags, each state's rows, order and entries, the counts
+  struct Dense { int64_t *jid, *tid, *submit, *o_jid, *o_submit; int32_t *pi, *ord, *o_pi; uint8_t* ok; };
+  Dense D[2] = {};
+  int32_t *cnt = nullptr, *blk = nullptr, *tmp = nullptr;
+  uint8_t* flag = nullptr;
+  int64_t h2d = 0, d2h = 0;
+  const int Cmax = (int)std::max(C[0], C[1]);
+  CK(pool, carve(S0->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+    cnt = c.take<int32_t>(4);   // [0] [1] the states' entries, [2] rows without facts, [3] the row compactions' own
+    blk = c.take<int32_t>((size_t)std::max(hw, Cmax) / CP_BLOCK + 2);
+    flag = c.take<uint8_t>(hw);
+    tmp = c.take<int32_t>(Cmax);
+    for (int t = 0; t < 2; t++) {
+      if (!C[t]) continue;
+      const int Ct = (int)C[t], Ot = std::min(Ct, limit);
+      Dense& d = D[t];
+      d.jid = c.take<int64_t>(Ct); d.submit = c.take<int64_t>(Ct); d.pi = c.take<int32_t>(Ct);
+      d.ok = c.take<uint8_t>(Ct); d.ord = c.take<int32_t>(Ct);
+      if (t) d.tid = c.take<int64_t>(Ct);
+      d.o_jid = c.take<int64_t>(Ot); d.o_submit = c.take<int64_t>(Ot); d.o_pi = c.take<int32_t>(Ot);
+    }
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  CK(pool, cudaMemsetAsync(cnt, 0, sizeof(int32_t) * 4, st));
+  int nl = 0;
+  for (int t = 0; t < 2; t++) {
+    if (!C[t]) continue;
+    Dense& d = D[t];
+    int base = 0;
+    for (const Src& h : hs[t]) {
+      const LJCols cols = lj_cols(h.s, t == 1);
+      const int T = t ? h.s->run.hw : h.s->pend.hw;
+      lj_flag_kernel<<<(T + 255) / 256, 256, 0, st>>>(cols, T, user, q.lo, q.hi, flag, cnt + 2);
+      nl++;
+      const bool pool_ok = q.pool == -1 || handle_pool[h.k] == q.pool;
+      compact(LJRows{cols, flag, base, h.k, pool_ok, q, d.jid, d.tid, d.pi, d.submit, d.ok}, T, nullptr, blk, cnt + 3,
+              h.rows, st, &nl);
+      base += h.rows;
+    }
+    const int Ct = (int)C[t];
+    CK(pool, csort::sort_indices(d.ord, tmp, Ct, LessJobPoolTask{d.jid, d.pi, d.tid}, st, &nl));
+    compact(LJPick{d.ord, d.jid, d.pi, d.submit, d.ok, d.o_jid, d.o_submit, d.o_pi}, Ct, nullptr, blk, cnt + t, limit, st,
+            &nl);
+  }
+  CK(pool, cudaGetLastError());
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  int32_t got[3];
+  CK(pool, download(got, cnt, 3, st, &d2h));
+  CK(pool, cudaStreamSynchronize(st));
+  const int64_t need = (int64_t)got[0] + got[1];
+  if (need > cap) {
+    *o_n = (int32_t)need;
+    return set_err(pool, COOK_E_TOO_LARGE, "%s: more entries than cap: %lld", who, (long long)need);
+  }
+  int at = 0;
+  for (int t = 0; t < 2; t++) {
+    if (!got[t]) continue;
+    CK(pool, download(o_jid + at, D[t].o_jid, got[t], st, &d2h));
+    CK(pool, download(o_submit + at, D[t].o_submit, got[t], st, &d2h));
+    CK(pool, download(o_pool + at, D[t].o_pi, got[t], st, &d2h));
+    std::fill(o_state + at, o_state + at + got[t], t ? COOK_LJ_RUNNING : COOK_LJ_WAITING);
+    at += got[t];
+  }
+  CK(pool, cudaEventRecord(pool->ev[23], st));
+  CK(pool, cudaStreamSynchronize(st));
+  *o_n = at;
+  *o_missing = got[2];
+  if (out_stats)
+    *out_stats = {ev_ms(pool->ev[20], pool->ev[21]), ev_ms(pool->ev[21], pool->ev[22]), ev_ms(pool->ev[22], pool->ev[23]),
+                  h2d, d2h, nl, 0};
+  return COOK_OK;
+}
+
+}  // namespace
+
+extern "C" int32_t cook_state_list_facts(cook_pool* pool, int32_t n, const int64_t* job_id, const int64_t* submit_ms,
+                                         const int32_t* submit_pool, const int32_t* custom_executor) {
+  if (!pool) return COOK_E_BADARG;
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_list_facts: out of device memory");
+  return list_facts(pool, S, n, job_id, submit_ms, submit_pool, custom_executor);
+}
+
+extern "C" int32_t cook_state_list_jobs(cook_pool* const* pools, int32_t n_pools, int32_t user, int32_t states,
+                                        int64_t start_ms, int64_t end_ms, int64_t job_id_lo, int64_t job_id_hi,
+                                        int32_t pool_code, const int32_t* handle_pool, int32_t include_custom_executor,
+                                        int32_t limit, int32_t cap, int32_t* out_state, int64_t* out_job_id,
+                                        int64_t* out_submit_ms, int32_t* out_pool, int32_t* out_n,
+                                        int32_t* out_n_missing, cook_phase_stats* out_stats) {
+  const LJSel q{start_ms, end_ms, job_id_lo, job_id_hi, pool_code, include_custom_executor};
+  return list_jobs(pools, n_pools, user, states, q, handle_pool, limit, cap, out_state, out_job_id, out_submit_ms,
+                   out_pool, out_n, out_n_missing, out_stats);
 }

@@ -26,6 +26,8 @@ path end to end.  It computes nothing numeric: every placement decision is `engi
                         answer
   match_cycle_metrics_response  the match-cycle logs (handle-match-cycle-metrics) and the unmatched-too-long warning
                         from a cook_state_match_metrics answer
+  list_jobs_response    the jobs GET /list and GET /jobs list (get-jobs-by-user-and-states, list-job-ents) from a
+                        cook_state_list_jobs answer and the states the Datomic path answers
 """
 import numpy as np
 
@@ -758,3 +760,29 @@ def retry_facts(instances, reason_table):
     whether one succeeded (then the job is completed: pass abi.RF_COMPLETED).  reason_table: name -> :reason/code."""
     done = [reason_table[r] if r is not None else -1 for st, r in instances if st in ("success", "failed")]
     return done, any(st == "success" for st, _ in instances)
+
+
+LIST_STATE_NAMES = {abi.LJ_WAITING: "waiting", abi.LJ_RUNNING: "running"}
+
+
+def list_jobs_response(answer, *, states, limit, completed=(), uncommitted=()):
+    """The job ids GET /list or GET /jobs lists, newest first, from engine.state_list_jobs' answer (made with this
+    limit) and the host's part:
+      uncommitted  [(job id, submit ms)]: the uncommitted waiting jobs that pass the request's filters.  Only /list
+                   (include-custom-executor false) keeps them (get-active-jobs-by-user-and-state removes them only
+                   with include-custom-executor); they merge into the waiting list by job id, cut to limit again.
+      completed    {state: [(job id, submit ms)]} for "completed", "success" and "failed", each the Datomic path's
+                   answer, in entity-id order and cut to limit.
+    The per-state lists are concatenated in the order of `states` (mapcat), stably sorted by submit time and cut to
+    limit (get-jobs-by-user-and-states), then reversed (list-job-ents): entries of equal submit time come out in the
+    reverse of their concatenation order."""
+    per = {"waiting": [], "running": []}
+    for s, j, t in zip(answer["state"], answer["job_id"], answer["submit_ms"]):
+        per[LIST_STATE_NAMES[int(s)]].append((int(j), int(t)))
+    if uncommitted:
+        merged = per["waiting"] + [(int(j), int(t)) for j, t in uncommitted]
+        per["waiting"] = sorted(merged, key=lambda e: e[0])[:limit]
+    done = dict(completed)
+    cat = [e for s in states for e in (per[s] if s in per else done.get(s, []))]
+    oldest = sorted(cat, key=lambda e: e[1])[:limit]
+    return [j for j, _ in reversed(oldest)][:limit]

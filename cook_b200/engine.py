@@ -273,6 +273,20 @@ class GpuEngine:
         if rc != 0:
             self._err(rc)
 
+    def state_list_facts(self, job_id, submit_ms=None, submit_pool=None, custom_executor=None):
+        """cook_state_list_facts: the submit time (ms), submit pool code (-1: none) and custom executor (-1 nil, 0
+        false, 1 true) of jobs with a live pending or running row (None: unchanged), written on every such row."""
+        jid = np.ascontiguousarray(job_id, np.int64)
+        cols = [np.ascontiguousarray(c, dt) if c is not None else None
+                for c, dt in ((submit_ms, np.int64), (submit_pool, np.int32), (custom_executor, np.int32))]
+        if any(c is not None and len(c) != len(jid) for c in cols):
+            raise ValueError("state_list_facts: a column's length differs from job_id's")
+        pt = (abi.P_I64, abi.P_I32, abi.P_I32)
+        rc = self.lib.cook_state_list_facts(self.pool, len(jid), abi.ptr(jid, abi.P_I64),
+                                            *[abi.ptr(c, t) if c is not None else None for c, t in zip(cols, pt)])
+        if rc != 0:
+            self._err(rc)
+
     def state_match_metrics(self, n_users, dropped=(), unmatched_warn_cycles=500, key_cap=64):
         """cook_state_match_metrics over the last resident match round: `dropped` are the considerable positions the
         launch-rate filter dropped.  Returns the counts by their abi.MMC_* names in lower case ('considerable',
@@ -920,6 +934,43 @@ def state_user_usage(engines, users=None, per_pool=False, by_group=False):
     out["lists"] = [None if not by_group or out["group"][d] == abi.UU_TOTAL else
                     jid[off[d]:off[d] + jobs[d]].tolist() for d in range(n)]
     return out
+
+
+def state_list_jobs(engines, user, states, start_ms, end_ms, job_id_lo=-(1 << 63), job_id_hi=(1 << 63) - 1,
+                    pool_code=-1, handle_pool=None, include_custom_executor=True, limit=(1 << 31) - 1, cap=1024):
+    """cook_state_list_jobs over the live rows of `engines` (one device, the work on engines[0]'s stream): user code
+    `user`'s jobs in `states` (abi.LJ_WAITING | abi.LJ_RUNNING) submitted in [start_ms, end_ms), with job ids in
+    [job_id_lo, job_id_hi), in the pool `pool_code` (-1: any; handle_pool: each engine's pool code), each state cut to
+    `limit`.  Returns 'state', 'job_id', 'submit_ms' and 'pool' (the engine index) as numpy columns, waiting entries
+    first, each state in ascending (job id, pool); 'missing', the rows in the window without list facts; and 'stats',
+    the call's own phase statistics.  The call is made with `cap` entries first and, when more are needed, once more
+    with the count it reports."""
+    if not engines:
+        raise ValueError("state_list_jobs: at least one handle")
+    hp = np.ascontiguousarray(handle_pool if handle_pool is not None else (), np.int32)
+    if handle_pool is not None and len(hp) != len(engines):
+        raise ValueError("state_list_jobs: handle_pool differs in length from engines")
+    handles = (C.c_void_p * len(engines))(*[e.pool for e in engines])
+    n, missing = C.c_int32(0), C.c_int32(0)
+    st = abi.PhaseStats()
+    cap = max(int(cap), 0)
+    for _ in range(2):
+        m = max(cap, 1)
+        state, pool = np.zeros(m, np.int32), np.zeros(m, np.int32)
+        jid, sub = np.zeros(m, np.int64), np.zeros(m, np.int64)
+        rc = engines[0].lib.cook_state_list_jobs(
+            handles, len(engines), int(user), int(states), int(start_ms), int(end_ms), int(job_id_lo), int(job_id_hi),
+            int(pool_code), abi.ptr(hp, abi.P_I32) if handle_pool is not None else None, int(bool(include_custom_executor)),
+            int(limit), cap, abi.ptr(state, abi.P_I32), abi.ptr(jid, abi.P_I64), abi.ptr(sub, abi.P_I64),
+            abi.ptr(pool, abi.P_I32), C.byref(n), C.byref(missing), C.byref(st))
+        if rc != abi.COOK_E_TOO_LARGE or n.value <= cap:
+            break
+        cap = n.value
+    if rc != 0:
+        engines[0]._err(rc)
+    k = n.value
+    return {"state": state[:k], "job_id": jid[:k], "submit_ms": sub[:k], "pool": pool[:k], "missing": missing.value,
+            "stats": st.as_dict()}
 
 
 def _is_answer(engines, call, cap):

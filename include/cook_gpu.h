@@ -470,7 +470,8 @@ int32_t cook_state_apply(cook_pool* pool, const cook_state_delta* delta);
 
 /* Launches by job id: live pending job job_id[i] becomes running task task_id[i], started at start_time[i] on
  * hostname_id[i] (a code of the global hostname dictionary; a NULL column stores -1, "host unknown").  User,
- * priority, job id, cpus, mem and gpus are copied on the device from the pending row.  Leaves exactly the
+ * priority, job id, cpus, mem, gpus and the list facts (cook_state_list_facts) are copied on the device from the
+ * pending row.  Leaves exactly the
  * state cook_state_apply leaves after the batch pending_rm_job_id = job_id plus the running upserts built
  * from those rows with running_hostname_id = hostname_id and, as running_group_off / running_group_idx, the
  * pending rows' group lists: the job leaves the last rank's queue, its counts and reservation leave with the
@@ -1397,6 +1398,68 @@ int32_t cook_state_match_metrics(cook_pool* pool, int32_t n_users, int32_t n_dro
                                  int64_t* out_first_job_id, int32_t* out_first_cycles, int32_t* out_user_considerable,
                                  int32_t* out_user_matched, int32_t* out_key_kind, int32_t* out_key_code,
                                  double* out_key_total, cook_phase_stats* out_stats);
+
+/* ------------------------------------------------- job listing over resident pools */
+/* The device half of GET /list and the list form of GET /jobs for the waiting and running states
+ * (get-active-jobs-by-user-and-state, tools.clj:445-466): one user's jobs in a submit window, read from the resident
+ * rows instead of a walk of every job in the state.
+ *
+ * List facts: the three job attributes the listing filters on, which never change over a job's life.  By job id, on
+ * the job's live pending row and on each of its live running rows, in place like cook_state_job_facts (live flag and
+ * generation kept); a NULL column is left unchanged.
+ *   submit_ms[i]        :job/submit-time in ms since the epoch
+ *   submit_pool[i]      the code of :job/submit-pool-name (the caller's pool dictionary), -1: none
+ *   custom_executor[i]  :job/custom-executor, -1 nil, 0 false, 1 true (the filters tell the three apart)
+ * A row has facts once custom_executor has been written to it; the other two are read only then, so the caller sends
+ * the three together.  Every pending and every running upsert of cook_state_apply writes "no facts" (inside the
+ * scatter it already runs: apply's launches and transfers are unchanged).  cook_state_launch copies the pending row's
+ * facts to the new running row on the device (no upload).  A parked copy (cook_state_retry_facts) and the in-place
+ * requeue of cook_state_status keep them: unlike the job facts, which a requeue clears, these attributes are fixed
+ * when the job is submitted.  Not part of cook_state_digest or cook_state_export: after a resync the caller sends
+ * them again.  The columns add 13 B per pending row and 13 B per running row (submit 8, pool 4, executor and the
+ * facts-present state 1), about 130 MB at 10 M jobs.
+ * COOK_E_BADARG, before any change: n < 0; a NULL job_id while n > 0; a job id that is neither live-pending nor
+ * live-running, or that appears twice; a custom_executor outside {-1, 0, 1}; a submit pool code below -1.
+ * Uploads exactly, when n > 0 and some column is given: (P + R) * (4 + [submit_ms] 8 + [submit_pool] 4 +
+ * [custom_executor] 1) bytes, P the listed jobs with a live pending row and R their live running rows (a slot and
+ * each non-NULL column per row written; the executor goes up as its one-byte stored code).  Statistics: cook_last_stats(COOK_PHASE_STATE).                        */
+int32_t cook_state_list_facts(cook_pool* pool, int32_t n, const int64_t* job_id, const int64_t* submit_ms,
+                              const int32_t* submit_pool, const int32_t* custom_executor);
+
+/* The listing over the union of the live rows of pools[0, n_pools); the handles follow cook_state_user_stats' rules
+ * (one device, idle, the work on pools[0]'s stream and scratch).  states: COOK_LJ_WAITING and/or COOK_LJ_RUNNING.
+ *   Rows       waiting: the live pending rows (committed jobs only, so `(remove uncommitted?)` holds by
+ *              construction); running: the distinct (handle, job id) over the live running rows, running and unknown
+ *              alike, represented by the row with the greatest task id (cook_state_unscheduled's rule).
+ *   Selection  an entry is selected when its user is `user`, its (representative's) facts are present, start_ms <=
+ *              submit < end_ms (job-submitted-in-range?), job_id_lo <= job id < job_id_hi (the caller's d/entid-at of
+ *              start - 1 h and end + 1 h: the bound is part of the reference's semantics), the pool check passes
+ *              (check-pool-for-listing, pool.clj:22-42: pool_code == -1, or handle_pool[k] == pool_code, or the submit
+ *              pool == pool_code; a job without :job/pool lives in the default pool's handle) and the executor check
+ *              passes (include_custom_executor 0 keeps custom_executor == 0 only, the reference's `false?`, so nil is
+ *              dropped; 1 keeps every entry).
+ *   Order      within each state ascending (job id, pool index), the reference's entity-id traversal; each state keeps
+ *              its first `limit` entries, as its `(take limit)` before the merge.  Waiting entries first, then running.
+ *   Outputs    entry e < *out_n: out_state[e] (COOK_LJ_*), out_job_id, out_submit_ms, out_pool (the index in pools).
+ *              *out_n_missing: the rows of `user` in a requested state inside the id window without facts; when it is
+ *              not 0 the caller keeps the Datomic path.
+ * Changes nothing resident.
+ * COOK_E_BADARG, before any device work and with nothing written: cook_state_user_stats' handle cases; states 0 or
+ * with unknown bits; a negative user; pool_code below -1, or handle_pool NULL while pool_code != -1;
+ * include_custom_executor outside {0, 1}; limit < 0 or cap < 0; a NULL output (out_stats may be NULL).
+ * COOK_E_TOO_LARGE: more than 2^31 - 1 rows of `user` in a state over the handles, with nothing written; more than
+ * cap entries, with only *out_n (the entries needed) written, so that the caller can retry with that capacity.
+ * No row of `user` in a requested state: empty results without device work (statistics zero).
+ * Transfers exactly: up nothing; down 12 (the two states' entry counts and the missing count), plus, unless
+ * COOK_E_TOO_LARGE, 20 * *out_n (job id, submit time, pool index; the states are known on the host).  Nothing that
+ * scales with the tables crosses the bus.
+ * Statistics: out_stats (may be NULL), as cook_state_user_stats; no cook_last_stats slot is written.             */
+enum { COOK_LJ_WAITING = 1, COOK_LJ_RUNNING = 2 };
+int32_t cook_state_list_jobs(cook_pool* const* pools, int32_t n_pools, int32_t user, int32_t states, int64_t start_ms,
+                             int64_t end_ms, int64_t job_id_lo, int64_t job_id_hi, int32_t pool_code,
+                             const int32_t* handle_pool, int32_t include_custom_executor, int32_t limit, int32_t cap,
+                             int32_t* out_state, int64_t* out_job_id, int64_t* out_submit_ms, int32_t* out_pool,
+                             int32_t* out_n, int32_t* out_n_missing, cook_phase_stats* out_stats);
 
 /* ----------------------------------------------------------------- multi-GPU */
 /* §8e: after a pool's match round every rank contributes its pools' usage

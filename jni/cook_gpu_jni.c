@@ -390,6 +390,33 @@ JFN(jint, stateStatus)(JNIEnv* env, jclass k, jlong pool, jint n, jobject task_i
   return cook_state_status((cook_pool*)(intptr_t)pool, n, one(env, task_id), one(env, success), one(env, end_time_ms),
                            one(env, reason_code), one(env, preempted), one(env, out_outcome), one(env, out_attempts));
 }
+/* jobs' list facts: job_id n longs, submit_ms n longs, submit_pool n ints, custom_executor n ints (each null: kept) */
+JFN(jint, stateListFacts)(JNIEnv* env, jclass k, jlong pool, jint n, jobject job_id, jobject submit_ms,
+                          jobject submit_pool, jobject custom_executor) {
+  return cook_state_list_facts((cook_pool*)(intptr_t)pool, n, one(env, job_id), one(env, submit_ms),
+                               one(env, submit_pool), one(env, custom_executor));
+}
+/* the job listing: times [start_ms, end_ms, job_id_lo, job_id_hi]; args [user, states, pool_code,
+ * include_custom_executor, limit, cap]; handle_pool n_pools ints (null with pool_code -1); outs the direct buffers of
+ * state, job_id, submit_ms, pool (cap ints / longs); out_n gets [n, n_missing]; out_stats may be null */
+JFN(jint, stateListJobs)(JNIEnv* env, jclass k, jlongArray pools, jlongArray times, jintArray args, jobject handle_pool,
+                         jobjectArray outs, jintArray out_n, jobject out_stats) {
+  jsize n = (*env)->GetArrayLength(env, pools);
+  if (n > 64) return COOK_E_BADARG;
+  jlong* h = (*env)->GetLongArrayElements(env, pools, NULL);
+  cook_pool* p[64];
+  for (jsize i = 0; i < n; i++) p[i] = (cook_pool*)(intptr_t)h[i];
+  (*env)->ReleaseLongArrayElements(env, pools, h, JNI_ABORT);
+  jlong t[4]; (*env)->GetLongArrayRegion(env, times, 0, 4, t);
+  jint a[6]; (*env)->GetIntArrayRegion(env, args, 0, 6, a);
+  int32_t got[2] = {0, 0};
+  jint rc = cook_state_list_jobs(p, (int32_t)n, a[0], a[1], t[0], t[1], t[2], t[3], a[2], one(env, handle_pool), a[3],
+                                 a[4], a[5], buf(env, outs, 0), buf(env, outs, 1), buf(env, outs, 2), buf(env, outs, 3),
+                                 &got[0], &got[1], one(env, out_stats));
+  jint g[2] = {got[0], got[1]};
+  (*env)->SetIntArrayRegion(env, out_n, 0, 2, g);
+  return rc;
+}
 /* the history's seed: cols the direct buffers of task_id, user, start_ms, end_ms, cpus, mem, success, reason_code */
 JFN(jint, stateHistorySeed)(JNIEnv* env, jclass k, jlong pool, jlong since_ms, jint n, jobjectArray cols) {
   return cook_state_history_seed((cook_pool*)(intptr_t)pool, since_ms, n, buf(env, cols, 0), buf(env, cols, 1),

@@ -65,6 +65,13 @@ with the two handles' digests compared after every rep:
   python tools/prof_state.py --status --pool c2 --reps 10
   python tools/prof_state.py --status --pool c5 --c5-pool 5 --reps 10
 
+--list loads C2 (or config-#5 pool --c5-pool with --pool c5) into a resident handle, gives every job list facts (a
+submit time in one day, no submit pool, no custom executor), and times cook_state_list_jobs for the user with the
+most rows and one with the fewest, both states, a 24 h window covering every row, limits Integer/MAX_VALUE and 150,
+against numpy over a host mirror, with the answers compared exactly:
+  python tools/prof_state.py --list --pool c2 --reps 20
+  python tools/prof_state.py --list --pool c5 --c5-pool 5 --reps 20
+
 --launch runs the same cycles on two resident handles instead of the host arm.  Each cycle's launches go to one
 handle through cook_state_launch (job ids, task ids, start times, the hosts the match chose) and to its twin through
 the equivalent cook_state_apply batch (the jobs' removal plus their task rows); the rest of the batch goes to both
@@ -1411,6 +1418,81 @@ def match_metrics_prof(a):
     e.close()
 
 
+def host_list_jobs(mirror, user, start, end, limit):
+    """get-active-jobs-by-user-and-state for waiting and running over the host mirror (one handle, no pool filter,
+    every custom executor kept): [(state, job id, submit ms)], each state by job id and cut to limit."""
+    out = []
+    for state, m in ((abi.LJ_WAITING, mirror["pending"]), (abi.LJ_RUNNING, mirror["running"])):
+        sel = m["user"] == user
+        jid, sub = m["jid"][sel], m["submit"][sel]
+        if state == abi.LJ_RUNNING:   # one entry per job: its greatest task id
+            o = np.lexsort((-m["tid"][sel], jid))
+            jid, sub = jid[o], sub[o]
+            first = np.ones(len(jid), bool)
+            first[1:] = jid[1:] != jid[:-1]
+            jid, sub = jid[first], sub[first]
+        ok = (sub >= start) & (sub < end)
+        jid, sub = jid[ok], sub[ok]
+        o = np.argsort(jid, kind="stable")[:limit]
+        out += [(state, int(j), int(t)) for j, t in zip(jid[o], sub[o])]
+    return out
+
+
+def list_prof(a):
+    """cook_state_list_jobs on a resident pool (C2, or config-#5 pool --c5-pool) with list facts on every job, for the
+    user with the most rows and one with the fewest, both states, a 24 h window covering every row, limits
+    Integer/MAX_VALUE and 150, against numpy over a host mirror; each answer is compared exactly."""
+    t = traces.gen_c2() if a.pool == "c2" else traces.gen_config_pool("c5", a.c5_pool)
+    jobs, pc, rc = t["jobs"], t["cols"]["pending"], t["cols"]["running"]
+    J = jobs.n
+    store = Jobs(jobs, pc["priority"], pc["job_id"])
+    e = GpuEngine(pool_name="list")
+    run = {k: np.asarray(v) for k, v in rc.items()}
+    e.state_apply(abi.make_delta(reset=True, running=abi.make_tasks(**run), pending=store.soa(np.arange(J)),
+                                 pending_priority=store.prio, pending_job_id=store.jid))
+    rng = np.random.default_rng(a.seed)
+    day = 24 * 3600 * 1000
+    t0 = 1_700_000_000_000
+    ids = np.unique(np.concatenate([store.jid, run["job_id"]]))
+    submit = t0 + rng.integers(0, day, len(ids))
+    e.state_list_facts(ids, submit, np.full(len(ids), -1, np.int32), np.zeros(len(ids), np.int32))
+    sub_of = dict(zip(ids.tolist(), submit.tolist()))
+    mirror = {"pending": {"user": np.asarray(store.c["user"]), "jid": store.jid.copy(),
+                          "submit": np.array([sub_of[int(j)] for j in store.jid], np.int64)},
+              "running": {"user": run["user"], "jid": run["job_id"], "tid": run["task_id"],
+                          "submit": np.array([sub_of[int(j)] for j in run["job_id"]], np.int64)}}
+    counts = np.bincount(np.concatenate([mirror["pending"]["user"], mirror["running"]["user"]]))
+    heavy, light = int(np.argmax(counts)), int(np.flatnonzero(counts == counts[counts > 0].min())[0])
+    print(json.dumps({"card": card(), "pool": a.pool if a.pool == "c2" else f"c5/{a.c5_pool}", "pending": J,
+                      "running": len(run["task_id"]), "heavy_user_rows": int(counts[heavy]),
+                      "light_user_rows": int(counts[light])}), flush=True)
+    for who, user in (("heavy", heavy), ("light", light)):
+        for limit in ((1 << 31) - 1, 150):
+            dev, wall, host, same = [], [], [], True
+            for rep in range(a.reps + 3):
+                w0 = time.perf_counter()
+                got = engine.state_list_jobs([e], user, abi.LJ_WAITING | abi.LJ_RUNNING, t0, t0 + day, limit=limit,
+                                             cap=int(counts[user]) + 1)
+                w = time.perf_counter() - w0
+                w0 = time.perf_counter()
+                want = host_list_jobs(mirror, user, t0, t0 + day, limit)
+                hw = time.perf_counter() - w0
+                same = same and got["missing"] == 0 and \
+                    [(int(s), int(j), int(x)) for s, j, x in zip(got["state"], got["job_id"], got["submit_ms"])] == want
+                if rep >= 3:   # the first calls carve and load the kernels
+                    st = got["stats"]
+                    dev.append(st["ms_h2d"] + st["ms_device"] + st["ms_d2h"])
+                    wall.append(w)
+                    host.append(hw)
+            print(json.dumps({"user": who, "rows": int(counts[user]), "limit": limit, "entries": len(got["job_id"]),
+                              "device_ms": round(float(np.median(dev)), 4),
+                              "wall_ms": round(1e3 * float(np.median(wall)), 4), "h2d_bytes": st["h2d_bytes"],
+                              "d2h_bytes": st["d2h_bytes"], "n_launches": st["n_launches"],
+                              "host_restatement_ms": round(1e3 * float(np.median(host)), 4), "identical": bool(same)}),
+                  flush=True)
+    e.close()
+
+
 def requeued_soa(store, rows, host):
     """The host path cook_state_status replaces: the pending rows of failed jobs rebuilt from the host mirror with
     reserved_host -1 and the failed host appended to the novel-host list (unless -1 or already listed)."""
@@ -1562,9 +1644,13 @@ def main():
     ap.add_argument("--status", action="store_true",
                     help="cook_state_status against rebuilding and re-sending the rows (C2 or --pool c5)")
     ap.add_argument("--status-batch", type=int, default=1000, help="--status: the launches and failures per rep")
+    ap.add_argument("--list", action="store_true",
+                    help="cook_state_list_jobs against numpy over a host mirror (C2 or --pool c5)")
     ap.add_argument("--match-metrics", action="store_true",
                     help="cook_state_match_metrics after each match against numpy over a host mirror (C2 or --pool c5)")
     a = ap.parse_args()
+    if a.list:
+        return list_prof(a)
     if a.status:
         return status_prof(a)
     if a.match_metrics:
