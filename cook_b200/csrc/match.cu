@@ -731,9 +731,14 @@ constexpr int KC = 16;                // candidates per spec result
 #endif
 constexpr int LK = COOK_LK;           // entries a lane keeps while building a result
 #ifndef COOK_NCW
-#define COOK_NCW 4
+#define COOK_NCW 5
 #endif
-constexpr int NCW = COOK_NCW;         // commit warps
+// Commit warps.  Each owns every NCW-th turn and does its off-turn work (result, first look, folds) in
+// the NCW - 1 turns before it; with four, the owner was still folding an older entry when its turn came
+// in over half of C2's turns.  Constraint pools keep four: each of their commit warps holds the current
+// job's verdict bit for every offer in shared memory, and those rows bound the pool's offer count.
+constexpr int NCW_PLAIN = COOK_NCW, NCW_CONSTR = 4;
+constexpr int NCW_MAX = NCW_PLAIN > NCW_CONSTR ? NCW_PLAIN : NCW_CONSTR;
 
 enum { Q_JOB = 0, Q_END = 1, Q_EXIT = 2 };
 
@@ -748,8 +753,11 @@ struct Latest {
 // Per-turn timeline of the PROF instantiation (COOK_PROF=1 with COOK_PROF_TRACE=<file>): null unless the
 // host armed it.  turn_trace[g] = TURN_WORDS stamps of queue entry g (clock64 of the resolver SM, so every
 // role of CTA 0 is on one clock); blk_trace[b] = when the driver saw every row of block b scored.
-constexpr int TURN_WORDS = 10;
-enum { TT_FREE = 0, TT_LAND, TT_READY, TT_SEEN, TT_DONE, TT_FENCE, TT_INFO, TT_K, TT_EVAL, TT_DEC };
+// TT_HAND: 1 << 32 | the low word of the clock when the owner learned that turn g-1 had ended (0: not
+// stamped); TT_POLL: how often the owner waited for a turn to end before that (low word) | 1 << 32 when
+// it learned it right after folding an older entry.
+constexpr int TURN_WORDS = 12;
+enum { TT_FREE = 0, TT_LAND, TT_READY, TT_SEEN, TT_DONE, TT_FENCE, TT_INFO, TT_K, TT_EVAL, TT_DEC, TT_HAND, TT_POLL };
 enum { TP_EXACT = 0, TP_ZTAKE = 1, TP_FALLBACK = 2, TP_GROUP = 3 };
 __device__ unsigned long long* g_turn_trace;
 __device__ int g_turn_cap;
@@ -800,6 +808,8 @@ struct ResolverShared {
   SpecOut res[RING + 1];          // [RING] = the commit warps' fallback slot
   unsigned long long res_bar[RING];  // mbarrier per result slot: phase (g / RING) & 1 completes when the
                                      // result of entry g has landed (bulk copy) or the entry is END / EXIT
+  unsigned long long hand[NCW_MAX];  // mbarrier per commit warp: phase (g / NCW) & 1 of hand[g % NCW]
+                                     // completes when turn g has ended (its chain word is stored)
   volatile int q_seq[RING];       // g+1 once queue entry g is filled
   // chain word: (entries consumed by the commit warps) << 32 | (log entries written)
   volatile unsigned long long chain;
@@ -1357,9 +1367,26 @@ __device__ __forceinline__ double warp_argmax_fast(double f, int v, int& wv, int
   return __shfl_sync(0xffffffffu, f, wl);
 }
 
+// The hand-off of the commit turn (plain pools): the owner of turn t stores its chain word and then
+// arrives (release) on hand[t % NCW], completing phase t / NCW of that barrier; wait_turn(S, t) returns
+// (acquire) once it has, so every store of turn t is visible.  The owner of turn g waits only for a turn
+// t in [g - NCW + 1, g - 1] (its own turn g - NCW has ended), so the parity cannot alias: the barrier's
+// next phase completes at the end of turn t + NCW > g, owned by the same warp as turn t, which cannot
+// end before turn g does.  For the same reason a wait may be repeated.
+template <int NCW>
+__device__ __forceinline__ void wait_turn(ResolverShared& S, const int t) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n"
+      "WAIT_TURN:\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+      "@!p bra WAIT_TURN;\n\t}"
+      :: "r"(smem_u32(&S.hand[t % NCW])), "r"((unsigned)(t / NCW) & 1u) : "memory");
+}
+
 template <bool CONSTR, bool PROF>
 __device__ void commit_warp(const MatchArgs& a, ResolverShared& S, const Latest latest, const int cw,
                             unsigned* sbw) {  // sbw: this warp's copy of the current job's verdict bits
+  constexpr int NCW = CONSTR ? NCW_CONSTR : NCW_PLAIN;
   const int lane = threadIdx.x & 31;
   unsigned long long n_fast = 0, n_group = 0, n_matched = 0, n_fallback = 0, n_slow_turn = 0, n_ztake = 0, n_relook = 0;
   unsigned long long prof[6] = {0, 0, 0, 0, 0, 0};
@@ -1382,7 +1409,8 @@ __device__ void commit_warp(const MatchArgs& a, ResolverShared& S, const Latest 
     // lane 0: this turn's row of the timeline
     // (t_done is read right after the chain store: the row's other stamps may come back from local memory)
     auto trace_turn = [&](long long t_ready, long long t_seen, long long t_eval, long long t_dec, long long t_fence,
-                          long long t_done, unsigned long long info, int key) {
+                          long long t_done, unsigned long long info, int key, unsigned long long hand,
+                          unsigned long long poll) {
       if (PROF && lane == 0 && g < g_turn_cap) {
         unsigned long long* p = g_turn_trace + (size_t)g * TURN_WORDS;
         p[TT_FREE] = (unsigned long long)t0; p[TT_LAND] = (unsigned long long)t_land;
@@ -1390,6 +1418,7 @@ __device__ void commit_warp(const MatchArgs& a, ResolverShared& S, const Latest 
         p[TT_DONE] = (unsigned long long)t_done; p[TT_FENCE] = (unsigned long long)t_fence;
         p[TT_INFO] = info; p[TT_K] = (unsigned long long)(long long)key;
         p[TT_EVAL] = (unsigned long long)t_eval; p[TT_DEC] = (unsigned long long)t_dec;
+        p[TT_HAND] = hand; p[TT_POLL] = poll;
       }
     };
     if (type == Q_EXIT) {
@@ -1443,9 +1472,10 @@ __device__ void commit_warp(const MatchArgs& a, ResolverShared& S, const Latest 
         __threadfence();
         asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(a.published), "r"((unsigned)(b + 1)) : "memory");
         S.chain = chain_pack(g + 1, c);
+        const long long t_done = PROF ? clock64() : 0;   // the arrive belongs to the hand-off
+        if (!CONSTR) mbar_arrive(&S.hand[g % NCW]);
         if (PROF) {
-          const long long t_done = clock64();
-          trace_turn(t_land, t4, 0, 0, t_fence, t_done, 1ull | ((unsigned long long)b << 32), c - lo);
+          trace_turn(t_land, t4, 0, 0, t_fence, t_done, 1ull | ((unsigned long long)b << 32), c - lo, 0, 0);
         }
         if (PROF && S.bk_ring[b & 7] < a.n_cons / 4) a.stats[15] = (unsigned long long)(clock64() - t_start);  // timeline: end of the first quarter
       }
@@ -1498,6 +1528,12 @@ __device__ void commit_warp(const MatchArgs& a, ResolverShared& S, const Latest 
     long long t1 = PROF ? clock64() : 0;
     long long t_ready = 0, t_seen = 0;               // PROF: end of the (first) first look, turn observed
     unsigned n_fold = 0, n_rel = 0, slow = 0;        // PROF: entries folded one by one, relooks, slow turn
+    // PROF: t_hand = the low word of the clock when the owner learned that turn g-1 had ended;
+    // hp = HP_FOLDED (the last step was a fold) | HP_MID (it learned that right after a fold) | HP_HAND
+    // (t_hand taken) + HP_WAIT per wait for a turn to end; two registers, as the PROF instantiation spills
+    enum : unsigned { HP_FOLDED = 1u, HP_MID = 2u, HP_HAND = 4u, HP_WAIT = 8u };
+    unsigned t_hand = 0, hp = 0;
+    auto mark_hand = [&](bool mid) { t_hand = (unsigned)clock64(); hp |= HP_HAND | (mid ? HP_MID : 0u); };
     unsigned long long w;
     int c = 0;
   relook:
@@ -1507,6 +1543,8 @@ __device__ void commit_warp(const MatchArgs& a, ResolverShared& S, const Latest 
       const int gd = chain_gdone(w);
       const int c_now = chain_ncommit(w);
       const bool mine = gd == g;
+      // under a predicate computed from the chain word: the stamp waits for its load
+      if (PROF && mine && !(hp & HP_HAND)) mark_hand(have && ((hp & HP_FOLDED) || c_now > c_seen + 1));
       if (!have) {
         // (a) first look: one lane per log entry committed since s, TD argmax rounds
         double xf = 0.0;
@@ -1542,7 +1580,7 @@ __device__ void commit_warp(const MatchArgs& a, ResolverShared& S, const Latest 
       if (c_now > c_seen) {
         // (b) one more entry, not the last before the turn: every lane evaluates it (uniform)
         // and the list is updated without a warp collective
-        if (PROF) n_fold++;
+        if (PROF) { n_fold++; hp |= HP_FOLDED; }
         int nvm, kk;
         const VmState ne = load_log<CONSTR>(S, c_seen, nvm, kk);
         const double nf = eval_res<CONSTR>(a, r, nvm, ne, grp, CONSTR ? sb_shared(sbw, nvm) : true);
@@ -1578,21 +1616,34 @@ __device__ void commit_warp(const MatchArgs& a, ResolverShared& S, const Latest 
         }
         continue;
       }
-      if (gd < g - 1) __nanosleep(40);  // only the next in line polls hard
+      // every entry below c_now is folded: sleep until turn gd ends, then fold its entry, if any
+      if (PROF) hp = (hp & ~HP_FOLDED) + HP_WAIT;
+      if (CONSTR) {   // constraint pools poll for it: the barrier made config #3's step 0.6 % slower
+        if (gd < g - 1) __nanosleep(40);  // only the next in line polls hard
+        continue;
+      }
+      wait_turn<NCW>(S, gd);
+      if (gd < g - 1) continue;
+      // turn g-1 has ended and appended at most entry c_seen; the chain word's load is still in
+      // flight when the turn below issues the loads of that entry
+      if (PROF) mark_hand(false);
+      c = *reinterpret_cast<volatile int*>(&S.chain);   // the low word: log entries written
+      break;
     }
     long long t2 = PROF ? clock64() : 0;
     if (PROF) prof[1] += (unsigned long long)(t2 - t1);
     if (PROF && t_seen == 0) t_seen = t2;   // a relook after this point belongs to the turn
     // ---- the turn: c == c_seen (nothing new) or c == c_seen + 1 (one new entry)
-    VmState ne;
-    ne.ac = ne.am = ne.lc = ne.lm = ne.rc = ne.rm = ne.yc = ne.ym = 0.0; ne.an = ne.pu = 0;
-    ne.room = 0x7fffffff; ne.occ = 0; ne.ptot = 0;
-    int ne_vm = -1;
+    // log[c_seen] is loaded before c is tested, so its loads issue together with the chain word's:
+    // the entry's stores precede turn g-1's chain store (and, in plain pools, its arrive), so the entry
+    // is the committed one whenever the word covers it, and is not used otherwise
+    int ne_vm, kk;
+    VmState ne = load_log<CONSTR>(S, c_seen, ne_vm, kk);
     double nf = 0.0;
     if (c > c_seen) {  // uniform: every lane evaluates the newest entry
-      int kk;
-      ne = load_log<CONSTR>(S, c_seen, ne_vm, kk);
       nf = eval_res<CONSTR>(a, r, ne_vm, ne, grp, CONSTR ? sb_shared(sbw, ne_vm) : true);
+    } else {
+      ne_vm = -1;
     }
     // best old item that the newest entry did not supersede
     const bool first = !(d > 0 && tv[0] == ne_vm);
@@ -1675,12 +1726,15 @@ __device__ void commit_warp(const MatchArgs& a, ResolverShared& S, const Latest 
       }
       if (got) wv = 0;
     }
+    // lane 0 stored the chain word on every path above
+    const long long t_done = PROF ? clock64() : 0;   // the arrive belongs to the hand-off
+    if (!CONSTR && lane == 0) mbar_arrive(&S.hand[g % NCW]);
     if (PROF) {
-      const long long t_done = clock64();
       const unsigned path = wv_group ? TP_GROUP : take_z ? TP_ZTAKE : exact ? TP_EXACT : TP_FALLBACK;
       trace_turn(t_ready, t_seen, t_eval, t_dec, 0, t_done, (unsigned long long)(path << 4 | min(n_rel, 15u) << 8 | min(n_fold, 255u) << 12 |
                                                           slow << 20 | (wv >= 0 ? 1u : 0u) << 21) |
-                                         ((unsigned long long)qe.blk << 32), k);
+                                         ((unsigned long long)qe.blk << 32), k,
+                 (hp & HP_HAND) ? (1ull << 32 | t_hand) : 0ull, hp / HP_WAIT | (unsigned long long)((hp & HP_MID) ? 1u : 0u) << 32);
     }
     if (wv >= 0) n_matched++;
     __syncwarp();
@@ -1704,6 +1758,7 @@ __global__ void __launch_bounds__(RES_THREADS, 1) match_kernel(MatchArgs a) {
   const int ns = a.n_spec;
   if ((int)blockIdx.x <= ns) {
     // block 0: the resolver; blocks 1..ns: spec CTAs with a replica of the resolver's log
+    constexpr int NCW = CONSTR ? NCW_CONSTR : NCW_PLAIN;
     ResolverShared& S = *reinterpret_cast<ResolverShared*>(smem_raw);
     Latest latest;
     const size_t res_base = (sizeof(ResolverShared) + 15) & ~size_t(15);
@@ -1720,11 +1775,13 @@ __global__ void __launch_bounds__(RES_THREADS, 1) match_kernel(MatchArgs a) {
       S.bk_ring[0] = 0; S.bk_ring[1] = a.B; S.bk_ring[2] = 2 * a.B; S.bk_known = 2;  // = host-initialised bk0[0..2]
       S.out_done = 0; S.blk_c0 = 0; S.last_b = a.B;
       for (int i = 0; i < RING; i++) mbar_init(&S.res_bar[i], 1u);
+      for (int i = 0; i < NCW_MAX; i++) mbar_init(&S.hand[i], 1u);
       fence_proxy_async_smem();  // the barriers are visible to the async proxy (bulk copies complete on them)
     }
     __syncthreads();
     if (blockIdx.x == 0) {
-      // warps 0..3 sit on different schedulers (warp id mod 4): one commit warp each
+      // warps 0..3 sit on different schedulers (warp id mod 4): one commit warp each, a fifth shares
+      // warp 0's scheduler
       if (warp < NCW) commit_warp<CONSTR, PROF>(a, S, latest, warp, sbw_base + (size_t)warp * a.sb_words);
       else if (warp == NCW) driver_warp<CONSTR, false, PROF>(a, S);
       else if (warp == NCW + 1) publisher_warp<CONSTR>(a, S);
@@ -2751,7 +2808,7 @@ int32_t match_run(cook_pool* pool, int32_t* out_considerable, int64_t* out_job_i
       // resolver CTA: shared structures + the per-VM newest-log-entry table (global when too big)
       ma.sb_words = mp->constr ? (O + 31) / 32 : 0;
       const size_t res_base = ((sizeof(ResolverShared) + 15) & ~size_t(15)) +
-                              (((size_t)NCW * ma.sb_words * 4 + 15) & ~size_t(15));
+                              (((size_t)NCW_CONSTR * ma.sb_words * 4 + 15) & ~size_t(15));   // sb_words: constraint pools only
       size_t smem = res_base;
       ma.latest_global = nullptr;
       if (res_base + sizeof(int) * (size_t)O <= 200 * 1024) smem = std::max(smem, res_base + sizeof(int) * (size_t)O);

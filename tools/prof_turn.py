@@ -5,7 +5,12 @@ entry's turn with clock64 on the resolver SM, and splits each turn's wall time
 T_done(g) - T_done(g-1) into:
   (a) owner late      T_ready > T_done(g-1): the owner's top-3 was not built yet
                       (a_land: the result itself landed after T_done(g-1); a_look: it landed in time)
-  (b) hand-off        T_seen - max(T_done(g-1), T_ready): poll latency, STS -> other warp's LDS
+  (b) hand-off        T_seen - max(T_done(g-1), T_ready): from turn g-1's chain word and mbarrier arrive
+                      to the next owner's turn; split on the turns whose owner was ready in time into
+                        detect   T_hand - T_done(g-1): until the owner learned that turn g-1 had ended
+                        rest     T_seen - T_hand: from there to the start of the turn body
+                      with how often the owner waited for a turn to end before T_hand and whether it
+                      learned of the turn right after folding an older entry (mid-fold)
   (c) turn body       T_done - T_seen
   (d) END turns       the whole wall time of end-of-block entries
   (e) block boundary  the part of (a) before the driver saw every row of the turn's block scored
@@ -27,7 +32,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from cook_b200 import traces  # noqa: E402
 from cook_b200.engine import GpuEngine  # noqa: E402
 
-TT_FREE, TT_LAND, TT_READY, TT_SEEN, TT_DONE, TT_FENCE, TT_INFO, TT_K, TT_EVAL, TT_DEC = range(10)
+TT_FREE, TT_LAND, TT_READY, TT_SEEN, TT_DONE, TT_FENCE, TT_INFO, TT_K, TT_EVAL, TT_DEC, TT_HAND, TT_POLL = range(12)
 PATHS = ["exact", "take_z", "fallback", "group"]
 TERMS = ["a_land", "a_look", "b_handoff", "c_body", "d_end", "e_block"]
 
@@ -96,7 +101,15 @@ def split(hdr, T, blk):
         "end_publish": np.where(is_end, T[:, TT_FENCE] - seen, 0),
         "end_handoff": np.where(is_end, seen - np.maximum(prev, ready), 0),
     }
-    return dict(n=n, wall=wall, terms=t, extra=extra, job=job, is_end=is_end, q1=q1, info=info, fast=fast,
+    # (b) split: job turns whose owner was ready before turn g-1 ended and learned of its end afterwards
+    # TT_HAND holds the low word of the clock: its distance from T_done(g-1) is taken modulo 2^32
+    detect = (T[:, TT_HAND] - prev) & 0xFFFFFFFF
+    in_time = job & (ready <= prev) & (((T[:, TT_HAND] >> 32) & 1) == 1) & (detect < 1 << 31)
+    extra["hand_detect"] = np.where(in_time, detect, 0)
+    extra["hand_rest"] = np.where(in_time, seen - prev - detect, 0)
+    extra["hand_waits"] = np.where(in_time, T[:, TT_POLL] & 0xFFFFFFFF, 0)
+    extra["hand_midfold"] = np.where(in_time, (T[:, TT_POLL] >> 32) & 1, 0)
+    return dict(n=n, wall=wall, terms=t, extra=extra, job=job, is_end=is_end, q1=q1, info=info, fast=fast, in_time=in_time,
                 placed=job & (((info >> 21) & 1) == 1), land_late=land_late)
 
 
@@ -114,7 +127,8 @@ def summarise(name, hdr, S, mhz):
         sel[0] = False
         tot = S["wall"][sel].sum()
         npl = max(1, int((S["placed"] & sel).sum()))
-        r = {"placements": int((S["placed"] & sel).sum()), "cycles": int(tot), "cycles_per_placement": tot / npl, "terms": {}}
+        r = {"placements": int((S["placed"] & sel).sum()), "cycles": int(tot), "cycles_per_placement": tot / npl, "terms": {},
+             "in_time_turns": int((S["in_time"] & sel).sum())}
         for nm in TERMS:
             v = S["terms"][nm][sel]
             jv = S["terms"][nm][sel & (S["is_end"] if nm == "d_end" else S["job"])]
@@ -123,7 +137,8 @@ def summarise(name, hdr, S, mhz):
                               "p90": float(np.percentile(jv, 90)) if len(jv) else 0.0,
                               "p99": float(np.percentile(jv, 99)) if len(jv) else 0.0}
         for nm, v in S["extra"].items():
-            kind = S["is_end"] if nm.startswith("end") else S["fast"] if nm.startswith("body") else S["job"]
+            kind = (S["is_end"] if nm.startswith("end") else S["fast"] if nm.startswith("body") else
+                    S["in_time"] if nm.startswith("hand") else S["job"])
             sv = v[sel & kind]
             r.setdefault("diag", {})[nm] = {"mean": float(sv.mean()) if len(sv) else 0.0,
                                             "p50": float(np.percentile(sv, 50)) if len(sv) else 0.0}
@@ -160,7 +175,14 @@ def show(r, mhz):
             x = p["terms"][nm]
             print(f"      {nm:10s} {x['per_placement']:8.1f} cyc/placement {100 * x['share']:5.1f} %   "
                   f"per turn p50 {x['p50']:7.0f} p90 {x['p90']:7.0f} p99 {x['p99']:8.0f}")
-        print("      diag " + "  ".join(f"{k} mean {v['mean']:.0f} p50 {v['p50']:.0f}" for k, v in p["diag"].items()))
+        print("      diag " + "  ".join(f"{k} mean {v['mean']:.0f} p50 {v['p50']:.0f}" for k, v in p["diag"].items()
+                                   if not k.startswith("hand")))
+        h = p["diag"]
+        print(f"      (b) split over {p['in_time_turns']} turns with the owner ready in time: "
+              f"detect mean {h['hand_detect']['mean']:.0f} p50 {h['hand_detect']['p50']:.0f}, "
+              f"rest mean {h['hand_rest']['mean']:.0f} p50 {h['hand_rest']['p50']:.0f} cycles; "
+              f"waits mean {h['hand_waits']['mean']:.1f} p50 {h['hand_waits']['p50']:.0f}; "
+              f"mid-fold {100 * h['hand_midfold']['mean']:.1f} %")
 
 
 def main():
