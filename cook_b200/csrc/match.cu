@@ -477,8 +477,7 @@ struct EvalStatic {  // static VM table in shared memory (SoA), or null => globa
 
 // per-CTA exchange buffer: every warp's per-lane partial lists of one row.  The sizes of EvalShared, SparseLive
 // and ResolverShared set the offer counts where match_run moves the static VM table and latest[] to global
-// memory; tests/match_edge_cases.py builds cases on either side of those counts from the sizes it records
-// (SMEM_STATIC_O, LATEST_O): change them together.
+// memory; the static_assert after ResolverShared pins them for tests/match_edge_cases.py.
 struct EvalShared {
   double f[NW][TOPK][32];
   int32_t v[NW][TOPK][32];
@@ -820,6 +819,14 @@ struct ResolverShared {
   volatile int bk_known;          // blocks 0..bk_known have their first job recorded
   volatile int out_done, blk_c0, last_b;  // END bookkeeping shared by the commit warps
 };
+
+// These five numbers set the offer counts where match_run moves the static VM table and latest[] to global
+// memory.  tests/match_edge_cases.py reads them from this line and builds its size-edge cases on either side
+// of those counts: a layout change fails here until the numbers (and with them the cases) follow.
+static_assert(sizeof(EvalShared) == 49216 && sizeof(SparseLive) == 8324 && sizeof(ResolverShared) == 160272 &&
+                  NCW_PLAIN == 5 && NCW_CONSTR == 4,
+              "matcher shared-memory layout changed: update these numbers; tests/match_edge_cases.py derives its "
+              "size-edge cases from them");
 
 __device__ __forceinline__ int chain_gdone(unsigned long long w) { return (int)(w >> 32); }
 __device__ __forceinline__ int chain_ncommit(unsigned long long w) { return (int)(unsigned)w; }
@@ -2788,6 +2795,8 @@ int32_t match_run(cook_pool* pool, int32_t* out_considerable, int64_t* out_job_i
     ~TraceBuf() { if (p) cudaFree(p); }
   } trace;
   int trace_caps[2] = {0, 0};
+  int latest_smem = 0, static_smem = 0;   // COOK_PROF: where the launch put latest[] and the static VM table,
+  size_t smem_launch = 0;                 // and the dynamic shared memory it asked for
   CK(pool, cudaEventRecord(pool->ev[5], st));
   if (n_cons > 0) {
     if (O == 0) {
@@ -2813,12 +2822,15 @@ int32_t match_run(cook_pool* pool, int32_t* out_considerable, int64_t* out_job_i
       ma.latest_global = nullptr;
       if (res_base + sizeof(int) * (size_t)O <= 200 * 1024) smem = std::max(smem, res_base + sizeof(int) * (size_t)O);
       else ma.latest_global = mp->d_latest;
+      latest_smem = ma.latest_global ? 0 : 1;
       // evaluator CTAs: the static VM table (4 f64 per VM, SoA) when it fits
       const size_t ev_base = (sizeof(EvalShared) + 127) & ~size_t(127);
       ma.vs_in_smem = ev_base + (size_t)O * 32 + sizeof(SparseLive) <= 224 * 1024 ? 1 : 0;
       if (getenv("COOK_NO_SMEM_STATIC")) ma.vs_in_smem = 0;
       ma.sparse_ok = getenv("COOK_NO_SPARSE") ? 0 : 1;
       smem = std::max(smem, ev_base + (ma.vs_in_smem ? (size_t)O * 32 : 0) + sizeof(SparseLive));
+      static_smem = ma.vs_in_smem;
+      smem_launch = smem;
       void* kfn = mp->constr ? (prof_on ? (void*)match_kernel<true, true> : (void*)match_kernel<true, false>)
                              : (prof_on ? (void*)match_kernel<false, true> : (void*)match_kernel<false, false>);
       {
@@ -2908,13 +2920,18 @@ int32_t match_run(cook_pool* pool, int32_t* out_considerable, int64_t* out_job_i
                           "c_end_block", "c_fallback", "res_total", "res_q1_done", "eval_work", "eval_wait",
                           "eval_loop", "eval_sync", "eval_merge", "eval_work_q1", "eval_rowslots_q1", "blocks", "z_takes", "relooks", "rows_pretest_ei0"};
     for (int i = 0; i < 27; i++) fprintf(stderr, "[cook_prof] %-14s %llu\n", nm[i], hstats[i]);
+    fprintf(stderr, "[cook_prof] %-14s %d\n", "latest_smem", latest_smem);
+    fprintf(stderr, "[cook_prof] %-14s %d\n", "static_smem", static_smem);
+    fprintf(stderr, "[cook_prof] %-14s %zu\n", "smem", smem_launch);
   }
   if (trace.p) {
-    // header (8 x i64): magic, turn rows, block rows, words per turn row, resolver clocks, n_cons, matched, 0
+    // header (8 x i64): magic, turn rows, block rows, words per turn row, resolver clocks, n_cons, matched,
+    // commit warps (turn g belongs to warp g mod NCW)
     const size_t nw = (size_t)trace_caps[0] * TURN_WORDS + trace_caps[1];
     std::vector<unsigned long long> h(8 + nw);
     h[0] = 0x314e5254ull; h[1] = trace_caps[0]; h[2] = trace_caps[1]; h[3] = TURN_WORDS;
-    h[4] = hstats[14]; h[5] = (unsigned long long)n_cons; h[6] = hstats[3]; h[7] = 0;
+    h[4] = hstats[14]; h[5] = (unsigned long long)n_cons; h[6] = hstats[3];
+    h[7] = mp->constr ? NCW_CONSTR : NCW_PLAIN;
     CK(pool, cudaMemcpy(h.data() + 8, trace.p, nw * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
     if (FILE* f = fopen(trace_path, "wb")) {
       fwrite(h.data(), sizeof(unsigned long long), h.size(), f);

@@ -1,6 +1,7 @@
 """Matcher inputs that reach the rare decisions of match_kernel in cook_b200/csrc/match.cu: equal-fitness ties,
-fitnesses one ulp apart, exact fits, supply confined to one or two chunks, crowded commit turns, group conflicts
-and the pipeline's size edges.  Test infrastructure only: no GPU code is imported here.
+fitnesses one ulp apart, exact fits, supply confined to one or two chunks, crowded commit turns, group conflicts,
+the pipeline's size edges (catalogue()) and the commit hand-off at every turn residue (handoff_catalogue()).
+Test infrastructure only: no GPU code is imported here.
 
 Every builder returns a dict:
   args    cook_match's arguments before params: (ranked, jobs, offers, users); the ranked list is the job order
@@ -24,17 +25,45 @@ ORDERS = ("perm", "rev")
 TOPK = 8            # candidates per (job, chunk) in a row (match.cu)
 SL_MAX = 64         # live VMs per chunk in sparse mode (match.cu)
 
-# Where the kernel's tables leave shared memory.  Sizes from the structs of match.cu, compiled for sm_90a:
-# sizeof(EvalShared) = 49216, sizeof(SparseLive) = 8324, sizeof(ResolverShared) = 160224, NCW = 4 commit warps.
-#  static VM table (evaluators): ev_base + 32 O + sizeof(SparseLive) <= 224 KiB, ev_base = 49216 rounded up to
-#    128 = 49280: 32 O <= 229376 - 49280 - 8324 = 171772, so O <= 5367.
-#  latest[] (resolver): res_base + 4 O <= 200 KiB, res_base = 160224 (a multiple of 16) plus, in the constraint
-#    kernel, the four owners' verdict-bit rows NCW * ceil(O / 32) * 4 B (a multiple of 16).  Plain:
-#    4 O <= 204800 - 160224 = 44576, O <= 11144.  Constraint: 4 O + 16 ceil(O / 32) <= 44576, O <= 9904
-#    (9904: 39616 + 4960 = 44576; 9905: 39620 + 4960 = 44580).
-#  SBW_MAX = 1024 verdict-bit words per row in sparse mode (constraint kernel): O <= 32768.
-SMEM_STATIC_O = 5367
-LATEST_O = {False: 11144, True: 9904}
+RING = 32           # queue entries in flight, and the period of the result slots' mbarriers (match.cu)
+
+# Where the kernel's tables leave shared memory.  The layout of match.cu compiled for sm_90a, as the static_assert
+# after its ResolverShared pins it (test_threshold_constants checks that these are the numbers that line holds).
+# The commit warps: NCW_PLAIN in the plain kernel, NCW_CONSTR in the constraint kernel; turn g is warp g mod NCW's.
+LAYOUT = dict(EvalShared=49216, SparseLive=8324, ResolverShared=160272, NCW_PLAIN=5, NCW_CONSTR=4)
+NCW = {False: LAYOUT["NCW_PLAIN"], True: LAYOUT["NCW_CONSTR"]}
+
+
+def smem_plan(O, constr):
+    """match_run's choices for O offers: (latest[] in shared memory, static VM table in shared memory, dynamic
+    shared memory of the launch in bytes), without COOK_NO_SMEM_STATIC.
+      static VM table (evaluators): ev_base + 32 O + sizeof(SparseLive) <= 224 KiB, ev_base = sizeof(EvalShared)
+        rounded up to 128.
+      latest[] (resolver): res_base + 4 O <= 200 KiB, res_base = sizeof(ResolverShared) rounded up to 16 plus, in
+        the constraint kernel, the owners' verdict-bit rows NCW_CONSTR * ceil(O / 32) * 4 B rounded up to 16."""
+    r16 = lambda x: (x + 15) // 16 * 16
+    res_base = r16(LAYOUT["ResolverShared"]) + (r16(NCW[True] * -(-O // 32) * 4) if constr else 0)
+    latest = res_base + 4 * O <= 200 * 1024
+    ev_base = (LAYOUT["EvalShared"] + 127) // 128 * 128
+    static = ev_base + 32 * O + LAYOUT["SparseLive"] <= 224 * 1024
+    smem = max(res_base + (4 * O if latest else 0), ev_base + (32 * O if static else 0) + LAYOUT["SparseLive"])
+    return latest, static, smem
+
+
+def _last(fits, hi=1 << 20):
+    """The largest O >= 1 for which the monotone predicate `fits` holds."""
+    lo = 1
+    assert fits(lo) and not fits(hi)
+    while hi - lo > 1:
+        mid = (lo + hi) // 2
+        lo, hi = (mid, hi) if fits(mid) else (lo, mid)
+    return lo
+
+
+# the last offer counts with the table in shared memory (5367; plain 11132, constraint 9892)
+SMEM_STATIC_O = _last(lambda O: smem_plan(O, False)[1])
+LATEST_O = {ck: _last(lambda O, ck=ck: smem_plan(O, ck)[0]) for ck in (False, True)}
+# SBW_MAX = 1024 verdict-bit words per row in sparse mode (constraint kernel): O <= 32768.
 SBW_O = 32 * 1024
 
 
@@ -312,7 +341,7 @@ CROWD_KNOBS = [{}, {"COOK_KMIN": "1", "COOK_LOOKAHEAD": "2"}, {"COOK_KMIN": "2",
                {"COOK_KMIN": "2", "COOK_LOOKAHEAD": "8", "COOK_NO_SMEM_STATIC": "1"}]
 
 
-def crowded(per_vm, order, constr, O=600, J=500):
+def crowded(per_vm, order, constr, O=600, J=500, knobs=CROWD_KNOBS):
     """Every VM has a distinct fitness (distinct running mem) and room for per_vm identical jobs: the jobs fill
     the VMs best first, so each placement supersedes the best items every later owner holds (relooks, exact
     recomputations, the bound taken directly).  Job k goes to the (k // per_vm)-th best VM."""
@@ -324,7 +353,7 @@ def crowded(per_vm, order, constr, O=600, J=500):
     want = [int(best[k // per_vm]) if k < O * per_vm else -1 for k in range(J)]
     claims = dict(kind="crowded", want=want)
     return make(np.full(J, 2.0), np.full(J, 1024.0), np.full(O, lc), np.full(O, lm), np.full(O, 1.0), rm,
-                order, constr, claims, knobs=CROWD_KNOBS, rank=rank)
+                order, constr, claims, knobs=knobs, rank=rank)
 
 
 SWAP_KNOBS = [{"COOK_KMIN": "1", "COOK_LOOKAHEAD": str(la), "COOK_NSPEC": ns} for la in (3, 4, 6, 31)
@@ -435,6 +464,52 @@ def threshold(O, order, constr, J=64):
     return ties(O, order, constr, J=J, knobs=[{}])
 
 
+# ---- 8. commit hand-off -------------------------------------------------------------------------------------
+# The queue holds one entry per job that the driver found feasible, an END entry after each block's jobs and an
+# EXIT entry last; entry g is commit warp g mod NCW's turn.  In plain pools the owner of turn g arrives on
+# hand[g mod NCW] after its chain store (END turns too, the EXIT turn not), and the owner of turn g + 1 waits
+# on it with parity (g / NCW) & 1.
+HANDOFF_KNOBS = [{}, {"COOK_LOOKAHEAD": "2"}, {"COOK_KMIN": "1", "COOK_NSPEC": "1"}, {"max_ctas": 3}]
+SHORT_POOLS = {"fit": 256, "full": 3}
+
+
+def short_queue(J, pool, order, constr):
+    """J tied jobs (J <= 2 NCW + 2, one block): job turns 0..J-1, END at g = J, EXIT at g = J + 1, so across J the
+    END and the EXIT turn land on every owner, for J < NCW some owners get no job turn, and for J < NCW - 2 some
+    get no turn at all.  Pool
+    "fit": 256 VMs, every job placed; "full": 3 VMs, the pool fills mid-queue and the tail stays unplaced."""
+    return ties(SHORT_POOLS[pool], order, constr, J=J, knobs=HANDOFF_KNOBS)
+
+
+def thinned(order, constr, O=512, J=3000, every=3):
+    """Tied VMs with room for two jobs each, and a queue where only every third job fits any VM: the driver skips
+    the others, so a block places a third of its jobs and the resolver sizes the blocks up (about 96 plain, 192
+    constraint jobs), and the job keys of consecutive turns jump.  Every job that fits is placed, two per VM in
+    name order."""
+    lc, lm, rc, rm = 4.0, 4096.0, 2.0, 1024.0
+    fit = np.arange(J) % every == 0
+    rank = ranks(O, order)
+    br = by_rank(rank)
+    want, n = [], 0
+    for k in range(J):
+        want.append(int(br[n // 2]) if fit[k] and n < 2 * O else -1)
+        n += int(fit[k])
+    assert n <= 2 * O
+    claims = dict(kind="thinned", want=want)
+    return make(np.where(fit, lc / 2, 2 * lc), np.full(J, lm / 2), *_full(O, lc, lm, rc, rm), order, constr, claims,
+                knobs=HANDOFF_KNOBS, fails=[0, 1, J - 1], rank=rank)
+
+
+def long_queues():
+    """{name suffix: builder(order, constr)} of the queues with many adaptive blocks and more than 2 RING NCW
+    turns, so every hand[] barrier goes through dozens of phases: ties that fill the pool mid-queue, crowded
+    turns (every placement supersedes the best item of every later owner) that fill it too, and the thinned
+    queue."""
+    return {"ties": lambda od, ck: ties(1024, od, ck, per_vm=2, J=2400, knobs=HANDOFF_KNOBS),
+            "crowd": lambda od, ck: crowded(2, od, ck, O=640, J=1500, knobs=HANDOFF_KNOBS),
+            "thin": lambda od, ck: thinned(od, ck)}
+
+
 # ---- the catalogue ------------------------------------------------------------------------------------------
 def catalogue():
     """{name: builder(order)} of every case, both kernels where the case applies to both."""
@@ -473,6 +548,19 @@ def catalogue():
     for O in (SBW_O, SBW_O + 1):
         out[f"7-sbw-C-O{O}"] = lambda od, O=O: sbw_edge(O, od)
         out[f"7-gate-P-O{O}"] = lambda od, O=O: threshold(O, od, False)
+    return out
+
+
+def handoff_catalogue():
+    """{name: builder(order)} of family 8, the commit hand-off, for both kernels."""
+    out = {}
+    for ck in (False, True):
+        kn = "C" if ck else "P"
+        for pool in SHORT_POOLS:
+            for J in range(1, 2 * NCW[ck] + 3):
+                out[f"8-short-{kn}-{pool}-J{J}"] = lambda od, J=J, pool=pool, ck=ck: short_queue(J, pool, od, ck)
+        for nm, b in long_queues().items():
+            out[f"8-long-{kn}-{nm}"] = lambda od, b=b, ck=ck: b(od, ck)
     return out
 
 

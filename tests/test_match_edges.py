@@ -7,7 +7,7 @@ Without a GPU: every case's inputs are valid and the oracle's answer shows what 
 also equals a plain restatement of the greedy match (match_edge_cases.greedy) on every case without groups.
 With one: cook_match equals the oracle bit for bit under each of the case's knob settings, the failure counts
 agree, and the cases still reach their branches (public counters, and the COOK_PROF counters of the crowded
-turns).
+turns); the size-edge cases run with each table on the side of its edge they claim (COOK_PROF's report).
 """
 import contextlib
 import os
@@ -22,20 +22,25 @@ from cook_b200 import abi, traces
 CASES = E.catalogue()
 ALL = [(n, od) for n in CASES for od in E.ORDERS]
 ids = lambda cases: [f"{n}-{od}" for n, od in cases]
-KNOB_KEYS = ("COOK_KMIN", "COOK_LOOKAHEAD", "COOK_NSPEC", "COOK_NO_SPARSE", "COOK_NO_SMEM_STATIC", "COOK_PROF")
+KNOB_KEYS = ("COOK_KMIN", "COOK_LOOKAHEAD", "COOK_NSPEC", "COOK_NO_SPARSE", "COOK_NO_SMEM_STATIC", "COOK_PROF",
+             "COOK_PROF_TRACE")
 THRESHOLD = ("7-smem", "7-sbw", "7-gate")
+MATCH_CU = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "cook_b200", "csrc", "match.cu")
 
 
 @contextlib.contextmanager
-def knobs_env(kn, prof=False):
-    """The case's COOK_* settings for the duration of the block; the environment is restored after it."""
+def knobs_env(kn, prof=False, trace=None):
+    """The case's COOK_* settings for the duration of the block; the environment is restored after it.  prof:
+    the profiling instantiation (COOK_PROF=1); trace: also write its per-turn timeline to this file."""
     saved = {k: os.environ.get(k) for k in KNOB_KEYS}
     try:
         for k in KNOB_KEYS:
             os.environ.pop(k, None)
         os.environ.update({k: v for k, v in kn.items() if k.startswith("COOK_")})
-        if prof:
+        if prof or trace:
             os.environ["COOK_PROF"] = "1"
+        if trace:
+            os.environ["COOK_PROF_TRACE"] = str(trace)
         yield
     finally:
         for k, v in saved.items():
@@ -77,14 +82,38 @@ def test_catalogue():
     assert E.ranks(33, "perm").tolist() != E.ranks(33, "rev").tolist()
 
 
+def pinned_layout():
+    """The numbers the static_assert after ResolverShared in match.cu pins: the build fails unless they are the
+    struct sizes and commit-warp counts of the sm_90a build."""
+    with open(MATCH_CU) as f:
+        src = f.read()
+    m = re.search(r"static_assert\(sizeof\(EvalShared\) == (\d+) && sizeof\(SparseLive\) == (\d+) && "
+                  r"sizeof\(ResolverShared\) == (\d+) &&\s*NCW_PLAIN == (\d+) && NCW_CONSTR == (\d+),", src)
+    assert m, "match.cu no longer pins its shared-memory layout"
+    return dict(zip(("EvalShared", "SparseLive", "ResolverShared", "NCW_PLAIN", "NCW_CONSTR"), map(int, m.groups())))
+
+
 def test_threshold_constants():
-    """The shared-memory limits restated from the struct sizes (see match_edge_cases) and the catalogue's cases
-    on either side of them."""
-    ev_base = (49216 + 127) // 128 * 128
-    fits_static = lambda O: ev_base + 32 * O + 8324 <= 224 * 1024
-    res = lambda O, constr: 160224 + (16 * -(-O // 32) if constr else 0)
+    """The layout the cases are built from is the one match.cu pins, the catalogue's edges are where match_run
+    (restated here from the pinned numbers) moves each table out of shared memory, and the catalogue has cases on
+    either side of them."""
+    L = pinned_layout()
+    assert E.LAYOUT == L
+    assert E.NCW == {False: L["NCW_PLAIN"], True: L["NCW_CONSTR"]}
+    up = lambda x, a: -(-x // a) * a
+    ev_base = up(L["EvalShared"], 128)
+    fits_static = lambda O: ev_base + 32 * O + L["SparseLive"] <= 224 * 1024
+    # latest[] follows the resolver's struct and, in the constraint kernel, one verdict-bit row per commit warp
+    rows = lambda O: up(L["NCW_CONSTR"] * 4 * (up(O, 32) // 32), 16)
+    res = lambda O, constr: up(L["ResolverShared"], 16) + (rows(O) if constr else 0)
     fits_latest = lambda O, constr: res(O, constr) + 4 * O <= 200 * 1024
     assert fits_static(E.SMEM_STATIC_O) and not fits_static(E.SMEM_STATIC_O + 1)
+    edges = (E.SMEM_STATIC_O, E.LATEST_O[False], E.LATEST_O[True], E.SBW_O)
+    for O in (1,) + edges + tuple(O + 1 for O in edges):
+        for constr in (False, True):
+            latest, static, smem = E.smem_plan(O, constr)
+            assert (latest, static) == (fits_latest(O, constr), fits_static(O))
+            assert smem == max(res(O, constr) + 4 * O * latest, ev_base + 32 * O * static + L["SparseLive"])
     for constr in (False, True):
         O = E.LATEST_O[constr]
         assert fits_latest(O, constr) and not fits_latest(O + 1, constr)
@@ -98,7 +127,10 @@ def test_threshold_constants():
 @pytest.mark.parametrize("name,order", ALL, ids=ids(ALL))
 def test_oracle_reaches(oracle, name, order):
     """The oracle's answer equals the hand-computed one, and the plain greedy restatement (cases without groups)."""
-    c = CASES[name](order)
+    oracle_claims(oracle, CASES[name](order))
+
+
+def oracle_claims(oracle, c):
     o = oracle.match(*c["args"], traces.match_params(c["nc"]), **c["kw"])
     cl = c["claims"]
     assert o["considerable"].tolist() == list(range(c["nc"]))
@@ -112,6 +144,7 @@ def test_oracle_reaches(oracle, name, order):
             assert o["ports"].tolist() == [p + [-1] * (mp - len(p)) for p in ports]
     assert o["stats"]["n_matched"] == int((o["assign"] >= 0).sum())
     assert ((o["fail"] == abi.FAIL_NONE) == (o["assign"] >= 0)).all()
+    return o
 
 
 def _fit_all(c, j, assign_before=()):
@@ -360,3 +393,41 @@ def test_crowded_turns_reach_every_outcome(gpu, oracle, capfd, constr):
             for k in PROF_NAMES:
                 seen[k] += got[k]
     assert seen["fallbacks"] > 0 and seen["z_takes"] > 0 and seen["relooks"] > 0, seen
+
+
+SIDE_NAMES = ("latest_smem", "static_smem", "smem")
+SIDE_CASES = [n for n in CASES if n.startswith(("7-smem", "7-gate"))]
+
+
+def _side(err):
+    """match_run's COOK_PROF report of the launch: latest[] and the static VM table in shared memory (1) or
+    global memory (0), and the dynamic shared memory in bytes."""
+    out = {}
+    for k in SIDE_NAMES:
+        got = re.findall(rf"^\[cook_prof\] {k}\s+(\d+)$", err, re.M)
+        assert len(got) == 1, k
+        out[k] = int(got[0])
+    return out
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name", SIDE_CASES)
+def test_size_edges_run_on_their_side(gpu, oracle, capfd, name):
+    """The size-edge cases once more with COOK_PROF=1: equal to the oracle, and each table in shared memory at its
+    edge and in global memory one offer past it, in both kernels, with the dynamic shared memory match_run's
+    formula gives."""
+    c = CASES[name]("perm")
+    O, constr = c["args"][2].n, c["constr"]
+    o = run(oracle, c)
+    capfd.readouterr()
+    with knobs_env({}, prof=True):
+        g = run(gpu, c)
+    _same(g, o)
+    assert gpu.match_failures(c["fails"]) == oracle_failures(oracle, c)
+    side = _side(capfd.readouterr().err)
+    latest, static, smem = E.smem_plan(O, constr)
+    assert side == dict(latest_smem=int(latest), static_smem=int(static), smem=smem), (O, constr)
+    if O in (E.LATEST_O[constr], E.LATEST_O[constr] + 1):
+        assert side["latest_smem"] == (O == E.LATEST_O[constr])
+    if O in (E.SMEM_STATIC_O, E.SMEM_STATIC_O + 1):
+        assert side["static_smem"] == (O == E.SMEM_STATIC_O) and side["latest_smem"] == 1
