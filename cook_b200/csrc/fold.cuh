@@ -3,9 +3,12 @@
 // Every running sum is the reference's left fold (common.cuh, "Exact-grid fast path"): a parallel
 // scan when grid_exact says every partial sum is exact, else the lane-serial chain below, which keeps
 // the association.  Around them: segment bounds of a sorted order, the order-wide tile scan that
-// replaces per-segment folds on the grid, and stable stream compaction.  Beside the per-user task order
+// replaces per-segment folds on the grid, the fold of one segment that chooses between the two, and
+// stable stream compaction.  Beside the per-user task order
 // (LessUserTask): the order of dru/sorted-merge over those lists (LessMerge).
 #pragma once
+#include <algorithm>
+
 #include "common.cuh"
 
 namespace {   // one copy per translation unit, like the kernels that use it
@@ -291,6 +294,58 @@ inline void order_scan(const OrderScan<T, K>& os, const Load& load, int n, const
   order_scan_tiles<<<nb, OS_TB, 0, st>>>(os, load, n, gf);
   order_scan_totals<<<1, 32, 0, st>>>(os, nb, n, gf);
   if (launches) *launches += 2;
+}
+
+// ---- the left fold from +0.0 of positions [s, e) of a sorted order, on one warp (every lane gets it).
+// `whole`: grid_exact over the whole order, so os holds its order-wide scan and the two ends give the sum;
+// else warp_fold_sum, association-free when the segment alone is on the grid, else the serial chain.
+// load(p, x) fills the zeroed addends of position p, as order_scan takes it.  This is what keeps the
+// per-segment answers of the queries bit-identical to the reference's folds.
+template <int K, class Load>
+__device__ __forceinline__ void segment_fold(double (&acc)[K], int s, int e, bool whole, const OrderScan<double, K>& os,
+                                             const GridFlag* gf, const Load& load, double (*stage)[32]) {
+#pragma unroll
+  for (int k = 0; k < K; k++) acc[k] = 0.0;
+  if (whole) {
+    if (e > s)
+#pragma unroll
+      for (int k = 0; k < K; k++) acc[k] = os.segment_sum(k, e - 1, s);
+    return;
+  }
+  warp_fold_sum<K, 4>(acc, e - s, grid_exact(gf, e - s), [&](int i, double (&x)[K]) {
+    load(s + i, x);
+    return true;
+  }, stage);
+}
+
+// Warp per segment, grid-stride, over an order of n positions cut by a compaction of segment ends: segment g
+// is [end[g - 1], end[g]) (end[-1] = 0) for g < *n_seg, a count only the device knows.  `scan`: os holds the
+// order-wide scan of the order (read when the whole order is on the grid); off, every segment takes
+// warp_fold_sum.  Lane 0 calls out(g, s, e, acc).
+constexpr int SF_TB = 128;
+template <int K, class Load, class Out>
+__global__ void __launch_bounds__(SF_TB) segment_fold_kernel(const int32_t* end, const int32_t* n_seg, int n, bool scan,
+                                                             OrderScan<double, K> os, const GridFlag* gf, Load load,
+                                                             Out out) {
+  __shared__ double stage[SF_TB / 32][K][32];
+  const int ns = *n_seg, nw = gridDim.x * (blockDim.x >> 5);
+  const bool whole = scan && grid_exact(gf, n);
+  for (int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; g < ns; g += nw) {
+    const int s = g ? end[g - 1] : 0, e = end[g];
+    double acc[K];
+    segment_fold(acc, s, e, whole, os, gf, load, stage[threadIdx.x >> 5]);
+    if (threadIdx.x & 31) continue;
+    out(g, s, e, acc);
+  }
+}
+
+// at most n segments, one warp each up to 4096 blocks; *launches (if given) counts the launch
+template <int K, class Load, class Out>
+inline void fold_segments(const int32_t* end, const int32_t* n_seg, int n, bool scan, const OrderScan<double, K>& os,
+                          const GridFlag* gf, const Load& load, const Out& out, cudaStream_t st, int* launches = nullptr) {
+  const int warps = SF_TB / 32;
+  segment_fold_kernel<<<std::min((n + warps - 1) / warps, 4096), SF_TB, 0, st>>>(end, n_seg, n, scan, os, gf, load, out);
+  if (launches) (*launches)++;
 }
 
 // ---- stable stream compaction: the items i < n with f.keep(i) go, in order, to slots 0, 1, ... through

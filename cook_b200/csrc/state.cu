@@ -430,9 +430,8 @@ struct UsageArgs {
   double* pool_out;                                        // [4]
 };
 
-// Warp per segment (users, then hosts, then the pool): the left fold of cpus, mem and gpus in the segment's
-// order (ascending task id within it).  The whole order on the grid: the two ends of the order-wide scan;
-// else warp_fold_sum, association-free when the segment alone is on the grid, else the serial chain.
+// Warp per segment (users, then hosts, then the pool; a user or host without rows has an empty one): the left
+// fold of cpus, mem and gpus in the segment's order (ascending task id within it), by segment_fold.
 __global__ void __launch_bounds__(128) usage_fold_kernel(UsageArgs a) {
   __shared__ double stage[4][3][32];
   int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, kind = 0;
@@ -440,18 +439,13 @@ __global__ void __launch_bounds__(128) usage_fold_kernel(UsageArgs a) {
   if (kind == US_N) return;
   const UsageSegs& q = a.seg[kind];
   const int s = q.start ? q.start[g] : 0, e = q.start ? q.end[g] : a.R;
-  double acc[3] = {0.0, 0.0, 0.0};
-  if (q.scan && grid_exact(a.gf, a.R)) {
-    if (e > s)
-#pragma unroll
-      for (int k = 0; k < 3; k++) acc[k] = q.os.segment_sum(k, e - 1, s);
-  } else {
-    warp_fold_sum<3, 4>(acc, e - s, grid_exact(a.gf, e - s), [&](int k, double (&x)[3]) {
-      const int i = q.ord[s + k];
-      x[0] = a.amt[0][i]; x[1] = a.amt[1][i]; x[2] = a.amt[2][i];
-      return true;
-    }, stage[threadIdx.x >> 5]);
-  }
+  double acc[3];
+  // The load reads q.ord through the kernel parameter: a LoadSorted copy of the pointers compiled to a different load
+  // schedule and made the off-grid folds about 3 % slower on an H100.
+  segment_fold(acc, s, e, q.scan && grid_exact(a.gf, a.R), q.os, a.gf, [&](int p, double (&x)[3]) {
+    const int i = q.ord[p];
+    x[0] = a.amt[0][i]; x[1] = a.amt[1][i]; x[2] = a.amt[2][i];
+  }, stage[threadIdx.x >> 5]);
   if (threadIdx.x & 31) return;
   if (kind == US_USER) {
     a.user_out[g] = (double)(e - s);
@@ -1584,31 +1578,30 @@ struct UsageFold {
     blk = c.take<int32_t>((size_t)hw / CP_BLOCK + 2);
     tmp = c.take<int32_t>(R);
     gf = c.take<GridFlag>(1);
-    const auto segs = [&](UsageSegs& q, int n_seg, bool bounds) {
-      q.n = n_seg;
-      q.ord = c.take<int32_t>(R);
-      if (!bounds) return;
-      q.start = c.take<int32_t>(n_seg + 1); q.end = c.take<int32_t>(n_seg + 1);
-      q.scan = 1;
-      for (int k = 0; k < 3; k++) {
-        q.os.part[k] = c.take<double>(R);
-        q.os.tile[k] = c.take<double>(R / OS_TILE + 2);
-      }
-    };
-    if (U > 0) segs(a.seg[US_USER], U, true);
+    if (U > 0) take_segs(c, US_USER, U, true);
     if (H > 0) {
       rows.host = c.take<int32_t>(R);
-      segs(a.seg[US_HOST], H, true);
+      take_segs(c, US_HOST, H, true);
     }
-    if (pool) segs(a.seg[US_POOL], 1, false);
+    if (pool) take_segs(c, US_POOL, 1, false);
+  }
+  // kind k's order of the R rows; with bounds, its n_seg segments' bounds and the order-wide scan
+  void take_segs(Carve& c, int k, int n_seg, bool bounds) {
+    UsageSegs& q = a.seg[k];
+    q.n = n_seg;
+    q.ord = c.take<int32_t>(R);
+    if (!bounds) return;
+    q.start = c.take<int32_t>(n_seg + 1); q.end = c.take<int32_t>(n_seg + 1);
+    q.scan = 1;
+    for (int j = 0; j < 3; j++) {
+      q.os.part[j] = c.take<double>(R);
+      q.os.tile[j] = c.take<double>(R / OS_TILE + 2);
+    }
   }
 
-  // the live rows of handles S[0, n) (their counts in S[0]'s counters), the grid check, the orders with their
-  // segments and (on the grid) order-wide scans, the folds
+  // the live rows of handles S[0, n) (their counts in S[0]'s counters), then fold()
   cudaError_t run(const PoolState* const* S, int n, cudaStream_t st, int* nl) {
     rows.c = pending ? PEND_COLS : RUN_COLS; rows.H = H;
-    cudaError_t e = cudaMemsetAsync(gf, 0, sizeof(GridFlag), st);
-    if (e != cudaSuccess) return e;
     rows.base = 0;
     for (int k = 0; k < n; k++) {
       const Table& t = pending ? S[k]->pend : S[k]->run;
@@ -1618,6 +1611,14 @@ struct UsageFold {
       compact(rows, t.hw, nullptr, blk, S[0]->counters + (pending ? 1 : 0), live, st, nl);
       rows.base += live;
     }
+    return fold(st, nl);
+  }
+
+  // Over rows.user / id / amt (and host) [0, R): the grid check, each kind's order by (key, id) with its segments
+  // and (on the grid) order-wide scan, the folds.  Needs tmp, gf, a.user_out and the kinds take_segs carved.
+  cudaError_t fold(cudaStream_t st, int* nl) {
+    cudaError_t e = cudaMemsetAsync(gf, 0, sizeof(GridFlag), st);
+    if (e != cudaSuccess) return e;
     grid_check_kernel<<<(R + 255) / 256, 256, 0, st>>>(rows.amt[0], rows.amt[1], rows.amt[2], R, gf);
     (*nl)++;
     const int32_t* key[US_N] = {rows.user, rows.host, nullptr};
@@ -2958,22 +2959,37 @@ int32_t considerable(cook_pool* pool, PoolState* S, const cook_user_table* users
   return COOK_OK;
 }
 
-// cook_state_user_stats: the running and waiting folds per user over the union of the handles' live rows, classified
-int32_t user_stats(cook_pool* const* pools, int n, const cook_user_table* users, const uint8_t* rest_ok,
-                   int64_t* out_jobs, double* out_cpus, double* out_mem, uint8_t* out_member, int64_t* out_all_jobs,
-                   double* out_all_cpus, double* out_all_mem, int64_t* out_users, cook_phase_stats* out_stats) {
-  const char* who = "cook_state_user_stats";
-  // ---- every check before any device work or output
+// The handle set of a call over several pools: a NULL pools, n <= 0 or a NULL pools[0] is a bare COOK_E_BADARG (no
+// handle to hold the message); then every handle non-NULL, listed once and on pools[0]'s device.
+int32_t check_handle_set(cook_pool* const* pools, int n, const char* who) {
   if (!pools || n <= 0 || !pools[0]) return COOK_E_BADARG;
   cook_pool* pool = pools[0];
-  std::vector<const PoolState*> S;
-  int R = 0, J = 0, hw_r = 0, hw_p = 0;
   for (int k = 0; k < n; k++) {
     if (!pools[k]) return set_err(pool, COOK_E_BADARG, "%s: a NULL handle", who);
     if (std::find(pools, pools + k, pools[k]) != pools + k)
       return set_err(pool, COOK_E_BADARG, "%s: a handle listed twice", who);
     if (pools[k]->device != pool->device) return set_err(pool, COOK_E_BADARG, "%s: handles on different devices", who);
   }
+  return COOK_OK;
+}
+
+// A read-side call's own statistics, from its events ev[20 .. 23] (upload, device, download); no cook_last_stats
+// slot is written
+cook_phase_stats call_stats(const cook_pool* pool, int64_t h2d, int64_t d2h, int nl) {
+  return {ev_ms(pool->ev[20], pool->ev[21]), ev_ms(pool->ev[21], pool->ev[22]), ev_ms(pool->ev[22], pool->ev[23]), h2d,
+          d2h, nl, 0};
+}
+
+// cook_state_user_stats: the running and waiting folds per user over the union of the handles' live rows, classified
+int32_t user_stats(cook_pool* const* pools, int n, const cook_user_table* users, const uint8_t* rest_ok,
+                   int64_t* out_jobs, double* out_cpus, double* out_mem, uint8_t* out_member, int64_t* out_all_jobs,
+                   double* out_all_cpus, double* out_all_mem, int64_t* out_users, cook_phase_stats* out_stats) {
+  const char* who = "cook_state_user_stats";
+  // ---- every check before any device work or output
+  if (int32_t rc = check_handle_set(pools, n, who)) return rc;
+  cook_pool* pool = pools[0];
+  std::vector<const PoolState*> S;
+  int R = 0, J = 0, hw_r = 0, hw_p = 0;
   if (!users || !out_jobs || !out_cpus || !out_mem || !out_member || !out_all_jobs || !out_all_cpus || !out_all_mem ||
       !out_users)
     return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
@@ -3059,10 +3075,7 @@ int32_t user_stats(cook_pool* const* pools, int n, const cook_user_table* users,
   memcpy(out_all_cpus, t.cpus, sizeof t.cpus);
   memcpy(out_all_mem, t.mem, sizeof t.mem);
   memcpy(out_users, t.users, sizeof t.users);
-  // the call's own statistics: no cook_last_stats slot is written
-  if (out_stats)
-    *out_stats = {ev_ms(pool->ev[20], pool->ev[21]), ev_ms(pool->ev[21], pool->ev[22]), ev_ms(pool->ev[22], pool->ev[23]),
-                  h2d, d2h, nl, 0};
+  if (out_stats) *out_stats = call_stats(pool, h2d, d2h, nl);
   return COOK_OK;
 }
 
@@ -3857,14 +3870,8 @@ int32_t sweep(cook_pool* const* pools, int n, int64_t now, int64_t dflt, int64_t
               int32_t* s_grp, int64_t* s_tid, int32_t* s_pool, int32_t* s_n, cook_phase_stats* out_stats) {
   const char* who = "cook_state_sweep";
   // ---- every check before any device work or output
-  if (!pools || n <= 0 || !pools[0]) return COOK_E_BADARG;
+  if (int32_t rc = check_handle_set(pools, n, who)) return rc;
   cook_pool* pool = pools[0];
-  for (int k = 0; k < n; k++) {
-    if (!pools[k]) return set_err(pool, COOK_E_BADARG, "%s: a NULL handle", who);
-    if (std::find(pools, pools + k, pools[k]) != pools + k)
-      return set_err(pool, COOK_E_BADARG, "%s: a handle listed twice", who);
-    if (pools[k]->device != pool->device) return set_err(pool, COOK_E_BADARG, "%s: handles on different devices", who);
-  }
   const bool linger = l_tid != nullptr, cancel = c_tid != nullptr, strag = s_tid != nullptr;
   if ((linger && (!l_pool || !l_n)) || (cancel && (!c_pool || !c_n)) || (strag && (!s_grp || !s_pool || !s_n)))
     return set_err(pool, COOK_E_BADARG, "%s: a list without its pool column or count", who);
@@ -4036,9 +4043,7 @@ int32_t sweep(cook_pool* const* pools, int n, int64_t now, int64_t dflt, int64_t
   if (linger) *l_n = got[0];
   if (cancel) *c_n = got[1];
   if (strag) *s_n = got[2];
-  if (out_stats)
-    *out_stats = {ev_ms(pool->ev[20], pool->ev[21]), ev_ms(pool->ev[21], pool->ev[22]), ev_ms(pool->ev[22], pool->ev[23]),
-                  h2d, d2h, nl, 0};
+  if (out_stats) *out_stats = call_stats(pool, h2d, d2h, nl);
   return COOK_OK;
 }
 
@@ -4175,7 +4180,7 @@ __global__ void unsched_users_kernel(const int32_t* quser, int nU, int32_t* umap
 
 // The entries: the queried users' live running rows dense in [0, R), their live pending rows in [R, R + J), as rank's
 // task columns plus each entry's slot.  key: a pending entry's user index; the running entries' is written by
-// unsched_rep_kernel.  ru: a running entry's user index.
+// job_rep_kernel.  ru: a running entry's user index.
 struct UnschedCols {
   int32_t* key; int32_t* ru; int32_t* prio; int64_t* start; int64_t* tid; int64_t* jid; int32_t* slot;
   double* amt[3];   // [R]: the running entries' cpus, mem, gpus
@@ -4212,29 +4217,30 @@ struct UnschedPendRows {
     o.slot[d] = i;
   }
 };
-// (user, job id, task id, dense index): a (user, job)'s running rows together, its greatest task id last
-struct LessUserJobTask {
-  const int32_t* u; const int64_t* jid; const int64_t* tid;
+// (scope, job id, task id, dense index): a (scope, job)'s running rows together, its greatest task id last.  The scope
+// is a user (cook_state_unscheduled) or a handle (cook_state_user_usage).
+struct LessScopeJobTask {
+  const int32_t* scope; const int64_t* jid; const int64_t* tid;
   __device__ bool operator()(int32_t a, int32_t b) const {
-    if (u[a] != u[b]) return u[a] < u[b];
+    if (scope[a] != scope[b]) return scope[a] < scope[b];
     if (jid[a] != jid[b]) return jid[a] < jid[b];
     if (tid[a] != tid[b]) return tid[a] < tid[b];
     return a < b;
   }
 };
-// The representative of each (user, job) is its last running row in that order: it keeps its user index as key, the
-// other rows get nU, a segment after every user's that no output reads.
-__global__ void unsched_rep_kernel(const int32_t* ord, int R, const int32_t* ru, const int64_t* jid, int nU,
-                                   int32_t* key) {
+// The representative of each (scope, job) is its last running row in that order: out[i] = val[i] for it, dead for
+// the other rows.  out may be val: thread p reads no other row's val.
+__global__ void job_rep_kernel(const int32_t* ord, int R, const int32_t* scope, const int64_t* jid, const int32_t* val,
+                               int32_t dead, int32_t* out) {
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= R) return;
   const int i = ord[p];
   bool rep = p == R - 1;
   if (!rep) {
     const int n = ord[p + 1];
-    rep = ru[n] != ru[i] || jid[n] != jid[i];
+    rep = scope[n] != scope[i] || jid[n] != jid[i];
   }
-  key[i] = rep ? ru[i] : nU;
+  out[i] = rep ? val[i] : dead;
 }
 // slot -> position in the entries' order, for the running representatives (rpos) and the pending rows (ppos)
 __global__ void unsched_pos_kernel(const int32_t* ord, int E, int R, const int32_t* key, const int32_t* slot, int nU,
@@ -4347,9 +4353,8 @@ int32_t unscheduled(cook_pool* pool, int n, const int64_t* job_id, uint8_t* out_
   int32_t *umap = nullptr, *rank = nullptr, *blk = nullptr, *cnt = nullptr, *ord1 = nullptr, *ord3 = nullptr;
   int32_t *tmp = nullptr, *ostart = nullptr, *oend = nullptr, *rpos = nullptr, *ppos = nullptr;
   const int32_t *d_quser = nullptr, *d_qkey = nullptr;
-  GridFlag* gf = nullptr;
-  UsageArgs f = {};
-  UsageSegs& us = f.seg[US_USER];
+  UsageFold f;   // the users' fold over the running representatives: keyed by o.key, in ascending task id
+  f.R = R; f.U = nU;
   UnschedArgs a = {};
   const int hw = std::max(S->run.hw, S->pend.hw);
   int64_t h2d = 0, d2h = 0;
@@ -4361,18 +4366,13 @@ int32_t unscheduled(cook_pool* pool, int n, const int64_t* job_id, uint8_t* out_
     ord3 = c.take<int32_t>(E); tmp = c.take<int32_t>(E);
     ostart = c.take<int32_t>(nU + 2); oend = c.take<int32_t>(nU + 2);
     rpos = c.take<int32_t>(std::max(S->run.hw, 1)); ppos = c.take<int32_t>(std::max(S->pend.hw, 1));
-    f.user_out = c.take<double>(4 * (size_t)nU);
+    f.a.user_out = c.take<double>(4 * (size_t)nU);
     if (R) {
       o.ru = c.take<int32_t>(R);
       for (int k = 0; k < 3; k++) o.amt[k] = c.take<double>(R);
       ord1 = c.take<int32_t>(R);
-      gf = c.take<GridFlag>(1);
-      us.ord = c.take<int32_t>(R);
-      us.start = c.take<int32_t>(nU + 2); us.end = c.take<int32_t>(nU + 2);
-      for (int k = 0; k < 3; k++) {
-        us.os.part[k] = c.take<double>(R);
-        us.os.tile[k] = c.take<double>(R / OS_TILE + 2);
-      }
+      f.gf = c.take<GridFlag>(1);
+      f.take_segs(c, US_USER, nU, true);   // nU + 1 bounds: the non-representatives' segment nU
     }
     a.usage = c.take<double>(4 * (size_t)n); a.pos = c.take<int32_t>(n); a.n_ahead = c.take<int32_t>(n);
     a.ahead = c.take<int64_t>(COOK_UNSCHED_AHEAD * (size_t)n); a.plugin = c.take<uint8_t>(n);
@@ -4387,27 +4387,18 @@ int32_t unscheduled(cook_pool* pool, int n, const int64_t* job_id, uint8_t* out_
   // the entries
   if (R) compact(UnschedRunRows{S->run.d_col, umap, o}, S->run.hw, nullptr, blk, cnt, R, st, &nl);
   if (J) compact(UnschedPendRows{S->pend.d_col, umap, o, R}, S->pend.hw, nullptr, blk, cnt + 1, J, st, &nl);
-  // one running row per (user, job), then the users' folds over them in ascending task id (usage_fold_kernel)
+  // one running row per (user, job): it keeps its user index as key, the other rows get nU, a segment after every
+  // user's that no output reads; then the users' folds over the representatives in ascending task id
   if (R) {
-    CK(pool, csort::sort_indices(ord1, tmp, R, LessUserJobTask{o.ru, o.jid, o.tid}, st, &nl));
-    unsched_rep_kernel<<<(R + 255) / 256, 256, 0, st>>>(ord1, R, o.ru, o.jid, nU, o.key);
-    CK(pool, cudaMemsetAsync(gf, 0, sizeof(GridFlag), st));
-    grid_check_kernel<<<(R + 255) / 256, 256, 0, st>>>(o.amt[0], o.amt[1], o.amt[2], R, gf);
-    nl += 2;
-    CK(pool, csort::sort_indices(writable(us.ord), tmp, R, LessKeyTid{o.key, o.tid}, st, &nl));
-    CK(pool, cudaMemsetAsync(writable(us.start), 0, sizeof(int32_t) * (nU + 1), st));
-    CK(pool, cudaMemsetAsync(writable(us.end), 0, sizeof(int32_t) * (nU + 1), st));
-    seg_bounds_kernel<<<(R + 255) / 256, 256, 0, st>>>(SortedKey{us.ord, nullptr, o.key}, R, writable(us.start),
-                                                       writable(us.end), nullptr);
+    CK(pool, csort::sort_indices(ord1, tmp, R, LessScopeJobTask{o.ru, o.jid, o.tid}, st, &nl));
+    job_rep_kernel<<<(R + 255) / 256, 256, 0, st>>>(ord1, R, o.ru, o.jid, o.ru, nU, o.key);
     nl++;
-    order_scan(us.os, LoadSorted{us.ord, {o.amt[0], o.amt[1], o.amt[2]}}, R, gf, st, &nl);
-    us.scan = 1; us.n = nU;
-    for (int k = 0; k < 3; k++) f.amt[k] = o.amt[k];
-    f.gf = gf; f.R = R; f.U = nU;
-    usage_fold_kernel<<<(nU + 3) / 4, 128, 0, st>>>(f);
-    nl++;
+    f.rows.user = o.key; f.rows.id = o.tid;
+    for (int k = 0; k < 3; k++) f.rows.amt[k] = o.amt[k];
+    f.tmp = tmp;
+    CK(pool, f.fold(st, &nl));
   } else {
-    CK(pool, cudaMemsetAsync(f.user_out, 0, sizeof(double) * 4 * (size_t)nU, st));
+    CK(pool, cudaMemsetAsync(f.a.user_out, 0, sizeof(double) * 4 * (size_t)nU, st));
   }
   // the users' entries in rank's same-user order, each entry's position by slot, then the queries
   CK(pool, csort::sort_indices(ord3, tmp, E, LessUserTask{o.key, o.prio, o.start, o.tid, o.jid, rank}, st, &nl));
@@ -4416,7 +4407,7 @@ int32_t unscheduled(cook_pool* pool, int n, const int64_t* job_id, uint8_t* out_
   unsched_pos_kernel<<<(E + 255) / 256, 256, 0, st>>>(ord3, E, R, o.key, o.slot, nU, rpos, ppos);
   a.qkey = d_qkey; a.Q = n;
   a.ord = ord3; a.key = o.key; a.ostart = ostart; a.rpos = rpos; a.ppos = ppos; a.jid = o.jid;
-  a.user_out = f.user_out; a.nU = nU; a.pcol = S->pend.d_col;
+  a.user_out = f.a.user_out; a.nU = nU; a.pcol = S->pend.d_col;
   unsched_query_kernel<<<(n + 127) / 128, 128, 0, st>>>(a);
   nl += 3;
   CK(pool, cudaGetLastError());
@@ -4428,10 +4419,7 @@ int32_t unscheduled(cook_pool* pool, int n, const int64_t* job_id, uint8_t* out_
   CK(pool, download(out_plugin, a.plugin, n, st, &d2h));
   CK(pool, cudaEventRecord(pool->ev[23], st));
   CK(pool, cudaStreamSynchronize(st));
-  // the call's own statistics: no cook_last_stats slot is written
-  if (out_stats)
-    *out_stats = {ev_ms(pool->ev[20], pool->ev[21]), ev_ms(pool->ev[21], pool->ev[22]), ev_ms(pool->ev[22], pool->ev[23]),
-                  h2d, d2h, nl, 0};
+  if (out_stats) *out_stats = call_stats(pool, h2d, d2h, nl);
   return COOK_OK;
 }
 
@@ -4450,7 +4438,7 @@ extern "C" int32_t cook_state_unscheduled(cook_pool* pool, int32_t n, const int6
 // group segment's job ids.  The host sizes every buffer from its per-user counts; the device takes the queried users'
 // live running rows of every handle, keeps each (handle, job)'s row with the greatest task id, expands each
 // representative into one entry per level the call asks for, sorts the entries once by (segment, task id, dense
-// index) and folds each segment as usage_fold_kernel does.
+// index) and folds each segment with fold.cuh's segment fold.
 namespace {
 
 constexpr int32_t UU_DEAD = INT32_MAX;   // the user of an entry whose row is not its job's representative: sorts last
@@ -4480,41 +4468,19 @@ struct UURows {
     amt[2][d] = static_cast<const double*>(col[R_GPUS])[i];
   }
 };
-// (handle, job id, task id, dense index): a (handle, job)'s rows together, its greatest task id last
-struct LessPoolJobTask {
-  const int32_t* pidx; const int64_t* jid; const int64_t* tid;
-  __device__ bool operator()(int32_t a, int32_t b) const {
-    if (pidx[a] != pidx[b]) return pidx[a] < pidx[b];
-    if (jid[a] != jid[b]) return jid[a] < jid[b];
-    if (tid[a] != tid[b]) return tid[a] < tid[b];
-    return a < b;
-  }
-};
-__global__ void uu_rep_kernel(const int32_t* ord, int R, const int32_t* pidx, const int64_t* jid, uint8_t* rep) {
-  const int p = blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= R) return;
-  const int i = ord[p];
-  bool last = p == R - 1;
-  if (!last) {
-    const int n = ord[p + 1];
-    last = pidx[n] != pidx[i] || jid[n] != jid[i];
-  }
-  rep[i] = last;
-}
-
 // The entries: entry l * R + i is row i at level l.  Bit 0 of the level's code scopes the entry to its handle, bit 1
-// keys it by its group (per_pool: codes 0 .. L - 1; else 0 and, by_group, 2).  A row that is not a representative
-// gives entries of user UU_DEAD.
+// keys it by its group (per_pool: codes 0 .. L - 1; else 0 and, by_group, 2).  user: UU_DEAD for a row that is not
+// a representative.
 struct UUKey {
   int32_t* user; int32_t* scope; int32_t* grp;
   __device__ bool same(int a, int b) const { return user[a] == user[b] && scope[a] == scope[b] && grp[a] == grp[b]; }
 };
-__global__ void uu_expand_kernel(int R, int E, int per_pool, const uint8_t* rep, const int32_t* user,
-                                 const int32_t* pidx, const int32_t* grp, UUKey k, int32_t* row) {
+__global__ void uu_expand_kernel(int R, int E, int per_pool, const int32_t* user, const int32_t* pidx,
+                                 const int32_t* grp, UUKey k, int32_t* row) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x;
   if (x >= E) return;
   const int l = x / R, i = x - l * R, code = per_pool ? l : l << 1;
-  k.user[x] = rep[i] ? user[i] : UU_DEAD;
+  k.user[x] = user[i];
   k.scope[x] = code & 1 ? pidx[i] : -1;
   k.grp[x] = code & 2 ? grp[i] : COOK_UU_TOTAL;
   row[x] = i;
@@ -4555,48 +4521,28 @@ struct UUListed {
     if (p == 0 || !k.same(i, ord[p - 1])) head_off[p] = d;
   }
 };
-struct UULoad {   // the order-wide scan's addends: cpus, mem, gpus of the entry at position p
-  const int32_t* ord; const int32_t* row; const double* amt[3];
+// the addends of the entry at position p of a sorted order: three columns of its row (the order-wide scan's and
+// segment_fold's load, for /usage and the instance stats)
+struct LoadEntry {
+  const int32_t* ord; const int32_t* row; const double* col[3];
   __device__ void operator()(int p, double (&x)[3]) const {
     const int r = row[ord[p]];
-    x[0] = amt[0][r]; x[1] = amt[1][r]; x[2] = amt[2][r];
+    x[0] = col[0][r]; x[1] = col[1][r]; x[2] = col[2][r];
   }
 };
-struct UUFoldArgs {
-  const int32_t* ord; const int32_t* row; UUKey k; const double* amt[3];
-  const int32_t* end; const int32_t* n_seg; const int32_t* head_off;   // head_off null: no lists
-  OrderScan<double, 3> os; const GridFlag* gf; int E;
+// fold_segments' output: segment g's key, job count and cpus, mem and gpus folds in ascending (task id, dense index)
+struct UUFoldOut {
+  const int32_t* ord; UUKey k; const int32_t* head_off;   // head_off null: no lists
   int32_t *o_user, *o_scope, *o_grp, *o_off; int64_t* o_jobs; double* o_amt[3];
-};
-// Warp per segment, grid-stride: the left fold of cpus, mem and gpus in ascending (task id, dense index).  The whole
-// order on the grid: the two ends of the order-wide scan; else warp_fold_sum, association-free when the segment alone
-// is on the grid, else the serial chain.
-__global__ void __launch_bounds__(128) uu_fold_kernel(UUFoldArgs a) {
-  __shared__ double stage[4][3][32];
-  const int n = *a.n_seg, nw = gridDim.x * (blockDim.x >> 5);
-  const bool scan = grid_exact(a.gf, a.E);
-  for (int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; g < n; g += nw) {
-    const int s = g ? a.end[g - 1] : 0, e = a.end[g];
-    double acc[3] = {0.0, 0.0, 0.0};
-    if (scan) {
+  __device__ void operator()(int g, int s, int e, const double (&acc)[3]) const {
+    const int i = ord[s];
+    o_user[g] = k.user[i]; o_scope[g] = k.scope[i]; o_grp[g] = k.grp[i];
+    o_jobs[g] = e - s;
 #pragma unroll
-      for (int k = 0; k < 3; k++) acc[k] = a.os.segment_sum(k, e - 1, s);
-    } else {
-      warp_fold_sum<3, 4>(acc, e - s, grid_exact(a.gf, e - s), [&](int k, double (&x)[3]) {
-        const int r = a.row[a.ord[s + k]];
-        x[0] = a.amt[0][r]; x[1] = a.amt[1][r]; x[2] = a.amt[2][r];
-        return true;
-      }, stage[threadIdx.x >> 5]);
-    }
-    if (threadIdx.x & 31) continue;
-    const int i = a.ord[s];
-    a.o_user[g] = a.k.user[i]; a.o_scope[g] = a.k.scope[i]; a.o_grp[g] = a.k.grp[i];
-    a.o_jobs[g] = e - s;
-#pragma unroll
-    for (int k = 0; k < 3; k++) a.o_amt[k][g] = acc[k];
-    if (a.head_off) a.o_off[g] = a.k.grp[i] == COOK_UU_TOTAL ? -1 : a.head_off[s];
+    for (int j = 0; j < 3; j++) o_amt[j][g] = acc[j];
+    if (head_off) o_off[g] = k.grp[i] == COOK_UU_TOTAL ? -1 : head_off[s];
   }
-}
+};
 
 int32_t user_usage(cook_pool* const* pools, int n, const int32_t* user, int nU, int per_pool, int by_group,
                    int seg_cap, int32_t* o_user, int32_t* o_scope, int32_t* o_group, int64_t* o_jobs, double* o_cpus,
@@ -4604,14 +4550,8 @@ int32_t user_usage(cook_pool* const* pools, int n, const int32_t* user, int nU, 
                    int32_t* o_njob, cook_phase_stats* out_stats) {
   const char* who = "cook_state_user_usage";
   // ---- every check before any device work or output
-  if (!pools || n <= 0 || !pools[0]) return COOK_E_BADARG;
+  if (int32_t rc = check_handle_set(pools, n, who)) return rc;
   cook_pool* pool = pools[0];
-  for (int k = 0; k < n; k++) {
-    if (!pools[k]) return set_err(pool, COOK_E_BADARG, "%s: a NULL handle", who);
-    if (std::find(pools, pools + k, pools[k]) != pools + k)
-      return set_err(pool, COOK_E_BADARG, "%s: a handle listed twice", who);
-    if (pools[k]->device != pool->device) return set_err(pool, COOK_E_BADARG, "%s: handles on different devices", who);
-  }
   const bool pp = per_pool != 0, bg = by_group != 0;
   if (!o_user || !o_scope || !o_group || !o_jobs || !o_cpus || !o_mem || !o_gpus || !o_nseg || !o_njob ||
       (bg && (!o_off || !o_jid)))
@@ -4667,11 +4607,12 @@ int32_t user_usage(cook_pool* const* pools, int n, const int32_t* user, int nU, 
   int32_t *r_user = nullptr, *r_pidx = nullptr, *r_grp = nullptr, *row = nullptr, *head_off = nullptr;
   int64_t *r_jid = nullptr, *r_tid = nullptr, *d_jid = nullptr;
   double* amt[3] = {};
-  uint8_t *umap = nullptr, *rep = nullptr;
+  uint8_t* umap = nullptr;
   const int32_t* d_q = nullptr;
   GridFlag* gf = nullptr;
   UUKey key = {};
-  UUFoldArgs a = {};
+  OrderScan<double, 3> os = {};
+  UUFoldOut a = {};
   int64_t h2d = 0, d2h = 0;
   CK(pool, carve(S0->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
     cnt = c.take<int32_t>(3);   // segments, listed jobs, the row compactions' own
@@ -4680,13 +4621,13 @@ int32_t user_usage(cook_pool* const* pools, int n, const int32_t* user, int nU, 
     r_user = c.take<int32_t>(Rn); r_pidx = c.take<int32_t>(Rn); r_grp = c.take<int32_t>(Rn);
     r_jid = c.take<int64_t>(Rn); r_tid = c.take<int64_t>(Rn);
     for (int k = 0; k < 3; k++) amt[k] = c.take<double>(Rn);
-    rep = c.take<uint8_t>(Rn); ord1 = c.take<int32_t>(Rn);
+    ord1 = c.take<int32_t>(Rn);
     gf = c.take<GridFlag>(1);
     key.user = c.take<int32_t>(E); key.scope = c.take<int32_t>(E); key.grp = c.take<int32_t>(E);
     row = c.take<int32_t>(E); ord = c.take<int32_t>(E); tmp = c.take<int32_t>(E); end = c.take<int32_t>(E);
     for (int k = 0; k < 3; k++) {
-      a.os.part[k] = c.take<double>(E);
-      a.os.tile[k] = c.take<double>(E / OS_TILE + 2);
+      os.part[k] = c.take<double>(E);
+      os.tile[k] = c.take<double>(E / OS_TILE + 2);
     }
     a.o_user = c.take<int32_t>(E); a.o_scope = c.take<int32_t>(E); a.o_grp = c.take<int32_t>(E);
     a.o_jobs = c.take<int64_t>(E);
@@ -4715,20 +4656,19 @@ int32_t user_usage(cook_pool* const* pools, int n, const int32_t* user, int nU, 
   }
   grid_check_kernel<<<(Rn + 255) / 256, 256, 0, st>>>(amt[0], amt[1], amt[2], Rn, gf);
   nl++;
-  // one representative per (handle, job), then every level's entries in one (segment, task id) order
-  CK(pool, csort::sort_indices(ord1, tmp, Rn, LessPoolJobTask{r_pidx, r_jid, r_tid}, st, &nl));
-  uu_rep_kernel<<<(Rn + 255) / 256, 256, 0, st>>>(ord1, Rn, r_pidx, r_jid, rep);
-  uu_expand_kernel<<<(E + 255) / 256, 256, 0, st>>>(Rn, E, pp, rep, r_user, r_pidx, r_grp, key, row);
+  // one representative per (handle, job): the other rows' user becomes UU_DEAD in place; then every level's entries
+  // in one (segment, task id) order, and each segment's left folds
+  CK(pool, csort::sort_indices(ord1, tmp, Rn, LessScopeJobTask{r_pidx, r_jid, r_tid}, st, &nl));
+  job_rep_kernel<<<(Rn + 255) / 256, 256, 0, st>>>(ord1, Rn, r_pidx, r_jid, r_user, UU_DEAD, r_user);
+  uu_expand_kernel<<<(E + 255) / 256, 256, 0, st>>>(Rn, E, pp, r_user, r_pidx, r_grp, key, row);
   nl += 2;
   CK(pool, csort::sort_indices(ord, tmp, E, LessSegTid{key, row, r_tid}, st, &nl));
   compact(UUSegEnds{ord, key, E, end}, E, nullptr, blk, cnt + 0, E, st, &nl);
   if (bg) compact(UUListed{ord, key, row, r_jid, d_jid, head_off}, E, nullptr, blk, cnt + 1, J, st, &nl);
-  order_scan(a.os, UULoad{ord, row, {amt[0], amt[1], amt[2]}}, E, gf, st, &nl);
-  a.ord = ord; a.row = row; a.k = key;
-  for (int k = 0; k < 3; k++) a.amt[k] = amt[k];
-  a.end = end; a.n_seg = cnt; a.head_off = head_off; a.gf = gf; a.E = E;
-  uu_fold_kernel<<<std::min((E + 3) / 4, 4096), 128, 0, st>>>(a);
-  nl++;
+  const LoadEntry load{ord, row, {amt[0], amt[1], amt[2]}};
+  order_scan(os, load, E, gf, st, &nl);
+  a.ord = ord; a.k = key; a.head_off = head_off;
+  fold_segments(end, cnt, E, true, os, gf, load, a, st, &nl);
   CK(pool, cudaGetLastError());
   CK(pool, cudaEventRecord(pool->ev[22], st));
   int32_t got[2];
@@ -4750,10 +4690,7 @@ int32_t user_usage(cook_pool* const* pools, int n, const int32_t* user, int nU, 
   CK(pool, cudaStreamSynchronize(st));
   *o_nseg = ns;
   *o_njob = nj;
-  // the call's own statistics: no cook_last_stats slot is written
-  if (out_stats)
-    *out_stats = {ev_ms(pool->ev[20], pool->ev[21]), ev_ms(pool->ev[21], pool->ev[22]), ev_ms(pool->ev[22], pool->ev[23]),
-                  h2d, d2h, nl, 0};
+  if (out_stats) *out_stats = call_stats(pool, h2d, d2h, nl);
   return COOK_OK;
 }
 
@@ -4876,46 +4813,19 @@ struct ISSegEnds {   // end[d] = one past segment d's last position, segment d s
   __device__ bool keep(int p) const { return p == E - 1 || !k.same(ord[p], ord[p + 1]); }
   __device__ void emit(int p, int d) const { end[d] = p + 1; }
 };
-struct ISLoad {   // the order-wide scan's addends: the three metrics of the entry at position p
-  const int32_t* ord; const int32_t* row; const double* met[3];
-  __device__ void operator()(int p, double (&x)[3]) const {
-    const int r = row[ord[p]];
-    x[0] = met[0][r]; x[1] = met[1][r]; x[2] = met[2][r];
-  }
-};
-struct ISFoldArgs {
-  const int32_t* ord; const int32_t* row; ISKey k; const double* met[3];
-  const int32_t* end; const int32_t* n_seg;
-  OrderScan<double, 3> os; const GridFlag* gf; int E;
+// fold_segments' output: segment g's key, count and the left folds of the three metrics in ascending (task id, pool
+// index)
+struct ISFoldOut {
+  const int32_t* ord; ISKey k;
   int32_t *o_kind, *o_user, *o_reason; int64_t* o_count; double* o_total;   // o_total [3 * segment + metric]
-};
-// Warp per segment, grid-stride: the left fold of the three metrics in ascending (task id, pool index), as
-// uu_fold_kernel folds: the two ends of the order-wide scan when the whole order is on the grid, else warp_fold_sum.
-__global__ void __launch_bounds__(128) is_fold_kernel(ISFoldArgs a) {
-  __shared__ double stage[4][3][32];
-  const int n = *a.n_seg, nw = gridDim.x * (blockDim.x >> 5);
-  const bool scan = grid_exact(a.gf, a.E);
-  for (int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; g < n; g += nw) {
-    const int s = g ? a.end[g - 1] : 0, e = a.end[g];
-    double acc[3] = {0.0, 0.0, 0.0};
-    if (scan) {
+  __device__ void operator()(int g, int s, int e, const double (&acc)[3]) const {
+    const int i = ord[s];
+    o_kind[g] = k.kind[i]; o_user[g] = k.user[i]; o_reason[g] = k.reason[i];
+    o_count[g] = e - s;
 #pragma unroll
-      for (int k = 0; k < 3; k++) acc[k] = a.os.segment_sum(k, e - 1, s);
-    } else {
-      warp_fold_sum<3, 4>(acc, e - s, grid_exact(a.gf, e - s), [&](int k, double (&x)[3]) {
-        const int r = a.row[a.ord[s + k]];
-        x[0] = a.met[0][r]; x[1] = a.met[1][r]; x[2] = a.met[2][r];
-        return true;
-      }, stage[threadIdx.x >> 5]);
-    }
-    if (threadIdx.x & 31) continue;
-    const int i = a.ord[s];
-    a.o_kind[g] = a.k.kind[i]; a.o_user[g] = a.k.user[i]; a.o_reason[g] = a.k.reason[i];
-    a.o_count[g] = e - s;
-#pragma unroll
-    for (int k = 0; k < 3; k++) a.o_total[3 * g + k] = acc[k];
+    for (int j = 0; j < 3; j++) o_total[3 * g + j] = acc[j];
   }
-}
+};
 // thread per (returned segment, metric): element ceil(p * n / 100) - 1 of the segment's ascending values
 // (percentile, task_stats.clj: p/100 is a ratio, so exact integer arithmetic).  The user segments come last and are
 // skipped.
@@ -4998,17 +4908,6 @@ bool is_out_null(const ISOut& o) {
   return !o.kind || !o.user || !o.reason || !o.count || !o.total || !o.pct || !o.lead_user || !o.lead_total ||
          !o.n_seg || !o.n_lead;
 }
-// cook_state_user_stats' handle rules: non-NULL, distinct, one device
-int32_t is_handles(cook_pool* const* pools, int n, const char* who) {
-  cook_pool* pool = pools[0];
-  for (int k = 0; k < n; k++) {
-    if (!pools[k]) return set_err(pool, COOK_E_BADARG, "%s: a NULL handle", who);
-    if (std::find(pools, pools + k, pools[k]) != pools + k)
-      return set_err(pool, COOK_E_BADARG, "%s: a handle listed twice", who);
-    if (pools[k]->device != pool->device) return set_err(pool, COOK_E_BADARG, "%s: handles on different devices", who);
-  }
-  return COOK_OK;
-}
 
 // The selected rows with their metrics, and the pipeline's device buffers, carved by take() for at most Smax rows.
 // cnt: [0] selected, [1] the source's flag, [2] segments, [3] returned segments, [4] leaders, [5] the compactions' own.
@@ -5021,7 +4920,8 @@ struct ISPipe {
   ISKey key = {};
   int32_t *row = nullptr, *ord = nullptr, *tmp = nullptr, *end = nullptr, *vord[3] = {}, *l_user = nullptr;
   double *pct = nullptr, *l_total = nullptr;
-  ISFoldArgs a = {};
+  OrderScan<double, 3> os = {};
+  ISFoldOut a = {};
   // blk_n: the most items any compaction of the call runs over; pos: the selection carries table positions
   void take(Carve& c, int Smax, int blk_n, bool pos) {
     const int Emax = IS_LEVELS * Smax;
@@ -5037,8 +4937,8 @@ struct ISPipe {
     row = c.take<int32_t>(Emax); ord = c.take<int32_t>(Emax); tmp = c.take<int32_t>(Emax); end = c.take<int32_t>(Emax);
     for (int k = 0; k < 3; k++) vord[k] = c.take<int32_t>(Emax);
     for (int k = 0; k < 3; k++) {
-      a.os.part[k] = c.take<double>(Emax);
-      a.os.tile[k] = c.take<double>(Emax / OS_TILE + 2);
+      os.part[k] = c.take<double>(Emax);
+      os.tile[k] = c.take<double>(Emax / OS_TILE + 2);
     }
     a.o_kind = c.take<int32_t>(Emax); a.o_user = c.take<int32_t>(Emax); a.o_reason = c.take<int32_t>(Emax);
     a.o_count = c.take<int64_t>(Emax); a.o_total = c.take<double>(3 * (size_t)Emax);
@@ -5057,7 +4957,7 @@ int32_t is_answer(cook_pool* pool, cudaStream_t st, ISPipe& p, int S, int32_t se
                   int64_t* d2h) {
   const int E = IS_LEVELS * S, E3 = 3 * S;
   int32_t got[2] = {0, 0};
-  ISFoldArgs& a = p.a;
+  ISFoldOut& a = p.a;
   if (S > 0) {
     // ---- the entries, the fold order and its segments, the folds
     grid_check_kernel<<<(S + 255) / 256, 256, 0, st>>>(p.met[0], p.met[1], p.met[2], S, p.gf);
@@ -5065,12 +4965,10 @@ int32_t is_answer(cook_pool* pool, cudaStream_t st, ISPipe& p, int S, int32_t se
     *nl += 2;
     CK(pool, csort::sort_indices(p.ord, p.tmp, E, LessSegTidPool{p.key, p.row, p.s_tid, p.s_pidx, p.s_pos}, st, nl));
     compact(ISSegEnds{p.ord, p.key, E, p.end}, E, nullptr, p.blk, p.cnt + 2, E, st, nl);
-    order_scan(a.os, ISLoad{p.ord, p.row, {p.met[0], p.met[1], p.met[2]}}, E, p.gf, st, nl);
-    a.ord = p.ord; a.row = p.row; a.k = p.key;
-    for (int k = 0; k < 3; k++) a.met[k] = p.met[k];
-    a.end = p.end; a.n_seg = p.cnt + 2; a.gf = p.gf; a.E = E;
-    is_fold_kernel<<<std::min((E + 3) / 4, 4096), 128, 0, st>>>(a);
-    (*nl)++;
+    const LoadEntry load{p.ord, p.row, {p.met[0], p.met[1], p.met[2]}};
+    order_scan(p.os, load, E, p.gf, st, nl);
+    a.ord = p.ord; a.k = p.key;
+    fold_segments(p.end, p.cnt + 2, E, true, p.os, p.gf, load, a, st, nl);
     // ---- the ranks: the three levels returned are entries [0, 3 S), whose segments lead the fold order's
     for (int k = 0; k < 3; k++)
       CK(pool, csort::sort_indices(p.vord[k], p.tmp, E3, LessSegValue{p.key, p.row, p.met[k]}, st, nl));
@@ -5118,9 +5016,8 @@ int32_t instance_stats(cook_pool* const* pools, int n, int64_t now, int32_t stat
                        int64_t tid_lo, int64_t tid_hi, int32_t seg_cap, const ISOut& o, cook_phase_stats* out_stats) {
   const char* who = "cook_state_instance_stats";
   // ---- every check before any device work or output
-  if (!pools || n <= 0 || !pools[0]) return COOK_E_BADARG;
+  if (int32_t rc = check_handle_set(pools, n, who)) return rc;
   cook_pool* pool = pools[0];
-  if (int32_t rc = is_handles(pools, n, who)) return rc;
   if (status != COOK_IS_RUNNING && status != COOK_IS_UNKNOWN) return set_err(pool, COOK_E_BADARG, "%s: an unknown status", who);
   if (end_ms <= start_ms) return set_err(pool, COOK_E_BADARG, "%s: end_ms <= start_ms", who);
   if (is_out_null(o)) return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
@@ -5181,10 +5078,7 @@ int32_t instance_stats(cook_pool* const* pools, int n, int64_t now, int32_t stat
   CK(pool, cudaStreamSynchronize(st));
   if (sel[1]) return set_err(pool, COOK_E_BADARG, "%s: a selected task starts after now_ms", who);
   if (int32_t rc = is_answer(pool, st, p, sel[0], seg_cap, o, &nl, &d2h)) return rc;
-  // the call's own statistics: no cook_last_stats slot is written
-  if (out_stats)
-    *out_stats = {ev_ms(pool->ev[20], pool->ev[21]), ev_ms(pool->ev[21], pool->ev[22]), ev_ms(pool->ev[22], pool->ev[23]),
-                  h2d, d2h, nl, 0};
+  if (out_stats) *out_stats = call_stats(pool, h2d, d2h, nl);
   return COOK_OK;
 }
 
@@ -5219,9 +5113,8 @@ int32_t history_stats(cook_pool* const* pools, int n, int32_t status, int64_t st
                       int64_t tid_hi, int32_t seg_cap, const ISOut& o, cook_phase_stats* out_stats) {
   const char* who = "cook_state_history_stats";
   // ---- every check before any device work or output
-  if (!pools || n <= 0 || !pools[0]) return COOK_E_BADARG;
+  if (int32_t rc = check_handle_set(pools, n, who)) return rc;
   cook_pool* pool = pools[0];
-  if (int32_t rc = is_handles(pools, n, who)) return rc;
   if (status != COOK_IS_SUCCESS && status != COOK_IS_FAILED) return set_err(pool, COOK_E_BADARG, "%s: an unknown status", who);
   if (end_ms <= start_ms) return set_err(pool, COOK_E_BADARG, "%s: end_ms <= start_ms", who);
   if (is_out_null(o)) return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
@@ -5281,9 +5174,7 @@ int32_t history_stats(cook_pool* const* pools, int n, int32_t status, int64_t st
   }
   CK(pool, cudaGetLastError());
   if (int32_t rc = is_answer(pool, st, p, (int)S, seg_cap, o, &nl, &d2h)) return rc;
-  if (out_stats)
-    *out_stats = {ev_ms(pool->ev[20], pool->ev[21]), ev_ms(pool->ev[21], pool->ev[22]), ev_ms(pool->ev[22], pool->ev[23]),
-                  h2d, d2h, nl, 0};
+  if (out_stats) *out_stats = call_stats(pool, h2d, d2h, nl);
   return COOK_OK;
 }
 
@@ -5994,27 +5885,20 @@ struct MMSegEnds {   // end[d] = one past key d's last position in the sorted en
   __device__ bool keep(int p) const { return p == *n - 1 || !key.same(ent[ord[p]], ent[ord[p + 1]]); }
   __device__ void emit(int p, int d) const { end[d] = p + 1; }
 };
-// warp per key: the left fold of its entries' values in take order, on the grid or by the serial chain
-__global__ void __launch_bounds__(128) mm_key_fold_kernel(MMKey key, const double* gpus, const int32_t* ent,
-                                                          const int32_t* ord, const int32_t* end, const int32_t* n_keys,
-                                                          const GridFlag* gf, int32_t* o_kind, int32_t* o_code,
-                                                          double* o_total) {
-  __shared__ double stage[4][1][32];
-  const int n = *n_keys, nw = gridDim.x * (blockDim.x >> 5);
-  for (int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; g < n; g += nw) {
-    const int s = g ? end[g - 1] : 0, e = end[g];
-    double acc[1] = {0.0};
-    warp_fold_sum<1, 4>(acc, e - s, grid_exact(gf, e - s), [&](int i, double (&x)[1]) {
-      x[0] = key.value(ent[ord[s + i]], gpus);
-      return true;
-    }, stage[threadIdx.x >> 5]);
-    if (threadIdx.x & 31) continue;
+// a key's left fold in take order (fold_segments without the order-wide scan: on the grid or by the serial chain)
+struct MMKeyLoad {
+  MMKey key; const double* gpus; const int32_t* ent; const int32_t* ord;
+  __device__ void operator()(int p, double (&x)[1]) const { x[0] = key.value(ent[ord[p]], gpus); }
+};
+struct MMKeyOut {
+  MMKey key; const int32_t* ent; const int32_t* ord; int32_t* o_kind; int32_t* o_code; double* o_total;
+  __device__ void operator()(int g, int s, int, const double (&acc)[1]) const {
     const int e0 = ent[ord[s]];
     o_kind[g] = key.kind(e0);
     o_code[g] = key.code(e0);
     o_total[g] = acc[0];
   }
-}
+};
 
 struct LessValuePos {   // (value, position): no amount is NaN, and -0.0 and 0.0 compare equal as in Clojure's compare
   const double* v;
@@ -6304,9 +6188,8 @@ int32_t match_metrics(cook_pool* pool, PoolState* S, int32_t U, int32_t D, const
   if (ne) {
     CK(pool, csort::sort_indices(ord_e, tmp, ne, LessKindCodePos{key, ent}, st, &nl));
     compact(MMSegEnds{key, ent, ord_e, cnt + MMC_ENTRIES, end}, ne, nullptr, blk, cnt + MMC_KEYS, ne, st, &nl);
-    mm_key_fold_kernel<<<std::min((ne + 3) / 4, 4096), 128, 0, st>>>(key, r.gpus, ent, ord_e, end, cnt + MMC_KEYS, gf + 1,
-                                                                     o_kind, o_code, o_total);
-    nl++;
+    fold_segments(end, cnt + MMC_KEYS, ne, false, OrderScan<double, 1>{}, gf + 1, MMKeyLoad{key, r.gpus, ent, ord_e},
+                  MMKeyOut{key, ent, ord_e, o_kind, o_code, o_total}, st, &nl);
   }
   const int nxt = 1 - R.cur;
   if (nu) {
@@ -6338,9 +6221,7 @@ int32_t match_metrics(cook_pool* pool, PoolState* S, int32_t U, int32_t D, const
   R.cur = nxt;
   R.u_n = nu;
   R.counted = true;
-  if (out_stats)
-    *out_stats = {ev_ms(pool->ev[20], pool->ev[21]), ev_ms(pool->ev[21], pool->ev[22]), ev_ms(pool->ev[22], pool->ev[23]),
-                  h2d, d2h, nl, 0};
+  if (out_stats) *out_stats = call_stats(pool, h2d, d2h, nl);
   return COOK_OK;
 }
 
@@ -6524,9 +6405,8 @@ int32_t list_jobs(cook_pool* const* pools, int n, int32_t user, int32_t states, 
                   int32_t* o_n, int32_t* o_missing, cook_phase_stats* out_stats) {
   const char* who = "cook_state_list_jobs";
   // ---- every check before any device work or output
-  if (!pools || n <= 0 || !pools[0]) return COOK_E_BADARG;
+  if (int32_t rc = check_handle_set(pools, n, who)) return rc;
   cook_pool* pool = pools[0];
-  if (int32_t rc = is_handles(pools, n, who)) return rc;
   if (states <= 0 || (states & ~(COOK_LJ_WAITING | COOK_LJ_RUNNING)))
     return set_err(pool, COOK_E_BADARG, "%s: states 0 or with unknown bits", who);
   if (user < 0) return set_err(pool, COOK_E_BADARG, "%s: a negative user", who);
@@ -6631,9 +6511,7 @@ int32_t list_jobs(cook_pool* const* pools, int n, int32_t user, int32_t states, 
   CK(pool, cudaStreamSynchronize(st));
   *o_n = at;
   *o_missing = got[2];
-  if (out_stats)
-    *out_stats = {ev_ms(pool->ev[20], pool->ev[21]), ev_ms(pool->ev[21], pool->ev[22]), ev_ms(pool->ev[22], pool->ev[23]),
-                  h2d, d2h, nl, 0};
+  if (out_stats) *out_stats = call_stats(pool, h2d, d2h, nl);
   return COOK_OK;
 }
 

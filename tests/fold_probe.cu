@@ -150,6 +150,46 @@ cudaError_t run_order_scan(const T* x, int n, int bad, unsigned long long max_bi
   return b.finish();
 }
 
+// ---- fold_segments<K>: lane 0 of segment g's warp records its fold and bounds
+template <int K>
+struct FoldOut {
+  double* acc; int* se;
+  __device__ void operator()(int g, int s, int e, const double (&a)[K]) const {
+#pragma unroll
+    for (int k = 0; k < K; k++) acc[(size_t)g * K + k] = a[k];
+    se[2 * g] = s;
+    se[2 * g + 1] = e;
+  }
+};
+
+// the order is positions 0 .. n-1 with addends x[k][p]; with `scan`, order_scan runs first, under the flag
+template <int K>
+cudaError_t run_segment_fold(const double* x, int n, int bad, unsigned long long max_bits, int scan, const int* end,
+                             int end_len, int n_seg, double* acc, int* se) {
+  Bufs b;
+  const int nb = (n + OS_TILE - 1) / OS_TILE;
+  const double* d_x = b.upload(x, (size_t)K * n);
+  const int* d_end = b.upload(end, end_len);
+  const int* d_nseg = b.upload(&n_seg, 1);
+  const GridFlag hf{bad, max_bits};
+  const GridFlag* d_gf = b.upload(&hf, 1);
+  double* d_acc = b.upload(acc, (size_t)K * end_len);
+  int* d_se = b.upload(se, 2 * (size_t)end_len);
+  OrderScan<double, K> os = {};
+  if (scan)
+    for (int k = 0; k < K; k++) {
+      os.part[k] = b.alloc<double>(n);
+      os.tile[k] = b.alloc<double>(nb);
+    }
+  if (b.err != cudaSuccess) return b.err;
+  const LoadCols<double, K> load{d_x, n};
+  if (scan) order_scan(os, load, n, d_gf, 0);
+  fold_segments(d_end, d_nseg, n, scan != 0, os, d_gf, load, FoldOut<K>{d_acc, d_se}, 0);
+  b.download(acc, d_acc, (size_t)K * end_len);
+  b.download(se, d_se, 2 * (size_t)end_len);
+  return b.finish();
+}
+
 __global__ void grid_query_kernel(const GridFlag* f, const long long* qn, const double* qstart, int nq, uint8_t* ok) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < nq) ok[i] = grid_exact(f, qn[i], qstart[i]) ? 1 : 0;
@@ -259,6 +299,19 @@ int fp_order_scan_i32(const int* x, int n, int bad, unsigned long long max_bits,
                       int read, int* part, int* tile, int* at, int* seg) {
   if (n < 1) return (int)cudaErrorInvalidValue;
   return run_order_scan<int, 1>(x, n, bad, max_bits, qp, qs, nq, read, part, tile, at, seg);
+}
+
+// fold_segments<K> over x: [K][n]; end: [end_len], of which the first n_seg (a device count) cut the order; acc:
+// [end_len][K] and se: [end_len][2] come in pre-filled with a sentinel, and segment g < n_seg writes its fold and
+// (start, end) there
+int fp_segment_fold(int K, const double* x, int n, int bad, unsigned long long max_bits, int scan, const int* end,
+                    int end_len, int n_seg, double* acc, int* se) {
+  if (n < 1 || n_seg < 0 || n_seg > end_len) return (int)cudaErrorInvalidValue;
+  switch (K) {
+    case 1: return run_segment_fold<1>(x, n, bad, max_bits, scan, end, end_len, n_seg, acc, se);
+    case 3: return run_segment_fold<3>(x, n, bad, max_bits, scan, end, end_len, n_seg, acc, se);
+  }
+  return (int)cudaErrorInvalidValue;
 }
 
 int fp_order_scan_tile() { return OS_TILE; }

@@ -23,7 +23,7 @@ def probe():
     lib = C.CDLL(PROBE)
     for name in ("fp_warp_fold_prefix", "fp_warp_fold_sum", "fp_order_scan_f64", "fp_order_scan_i32",
                  "fp_grid_check", "fp_grid_value_ok", "fp_seg_bounds", "fp_compact", "fp_order_scan_tile",
-                 "fp_compact_block"):
+                 "fp_compact_block", "fp_segment_fold"):
         getattr(lib, name).restype = C.c_int
     assert lib.fp_order_scan_tile() == R.OS_TILE and lib.fp_compact_block() == R.CP_BLOCK
     return lib
@@ -201,6 +201,73 @@ def test_order_scan_i32(probe, n):
     c = np.cumsum(x.astype(np.int64))
     assert np.array_equal(at, c)
     assert np.array_equal(seg, [c[p] - (c[s - 1] if s > 0 else 0) for p, s in zip(qp, qs)])
+
+
+T = R.OS_TILE
+# empty segments (at the start, between, at the end), one-element ones, 31/32/33-lane chunks, and segments that
+# straddle tile edges: [2000, 2100) crosses T, [2229, 4126) crosses 2 T, the 4100-long one 3 T and 4 T
+FOLD_LENS = [0, 1, 31, 0, 32, 33, 1903, 100, 0, 129, 2 * T - 2199, 4100, 0, 64, 1, 0]
+
+
+def _segment_fold(probe, K, x, flag, scan, end, n_seg):
+    n = x.shape[1]
+    end = np.ascontiguousarray(end, np.int32)
+    acc = np.full((len(end), K), -9.0)
+    se = np.full((len(end), 2), -9, np.int32)
+    _ok(probe.fp_segment_fold(K, x.ctypes.data_as(C.c_void_p), n, flag[0], C.c_ulonglong(flag[1]), scan,
+                              end.ctypes.data_as(C.c_void_p), len(end), n_seg, acc.ctypes.data_as(C.c_void_p),
+                              se.ctypes.data_as(C.c_void_p)))
+    return acc, se
+
+
+def _fold_values(rng, regime, lens):
+    n = int(sum(lens))
+    if regime == "big":   # on the grid, with 2^32 addends: the order (n > 2047) is off it, segments below 2047 on it
+        v = GRIDV[rng.integers(0, len(GRIDV), n)]
+        v[rng.random(n) < 0.05] = R.MIXED_BIG
+        return v
+    return _values(rng, regime, n)
+
+
+@pytest.mark.parametrize("K", [1, 3])
+@pytest.mark.parametrize("regime,scan", [("grid", 1), ("grid", 0), ("off", 1), ("wild", 1), ("big", 1), ("wild", 0)])
+def test_segment_fold(probe, K, regime, scan):
+    """fold_segments / segment_fold: every segment's fold has the Python left fold's bits, from +0.0, whether it
+    takes the order-wide scan's ends (the whole order on the grid, scan on), the butterfly (the segment alone on
+    the grid) or the serial chain; empty segments give +0.0; segments past the device count are not written."""
+    rng = np.random.default_rng(K * 31 + len(regime) * 7 + scan)
+    lens = FOLD_LENS
+    x = np.ascontiguousarray(np.stack([_fold_values(rng, regime, lens) for _ in range(K)]))
+    n = x.shape[1]
+    flag = R.grid_flag(*x)
+    whole = R.grid_exact(flag, n)
+    assert whole == (regime == "grid")
+    if regime == "big":
+        assert any(R.grid_exact(flag, m) for m in lens if m > 1) and not all(R.grid_exact(flag, m) for m in lens)
+    ends = np.cumsum(lens).astype(np.int32)
+    for n_seg in (len(lens), len(lens) - 3, 0):
+        acc, se = _segment_fold(probe, K, x, flag, scan, np.concatenate([ends, [n, n]]), n_seg)
+        for g in range(n_seg):
+            s, e = (int(ends[g - 1]) if g else 0), int(ends[g])
+            assert (se[g] == [s, e]).all(), g
+            for k in range(K):
+                f = R.left_fold(x[k, s:e])
+                assert R.same_bits([acc[g, k]], [f[-1] if f else 0.0]), (g, k)
+        assert (acc[n_seg:] == -9.0).all() and (se[n_seg:] == -9).all()
+
+
+def test_segment_fold_grid_stride(probe):
+    """More segments than the 4096 blocks of 4 warps hold: each warp folds several, in both paths."""
+    rng = np.random.default_rng(5)
+    lens = rng.integers(1, 4, 4096 * 4 + 777)
+    ends = np.cumsum(lens).astype(np.int32)
+    for regime in ("grid", "off"):
+        x = np.ascontiguousarray(_values(rng, regime, int(ends[-1]))[None, :])
+        acc, se = _segment_fold(probe, 1, x, R.grid_flag(x[0]), 1, ends, len(ends))
+        starts = np.concatenate([[0], ends[:-1]])
+        assert np.array_equal(se[:, 0], starts) and np.array_equal(se[:, 1], ends)
+        want = [R.left_total(x[0, s:e]) for s, e in zip(starts, ends)]
+        assert R.same_bits(acc[:, 0], want)
 
 
 def _flag_and_queries(probe, cols, queries):
