@@ -21,6 +21,9 @@
 ;;   api.clj:3038-3085 list-resource, :1684-1776 list-job-ents (waiting, running)
 ;;                                           -> (list-jobs ...) + cycle.py's list_jobs_response, fed by list-facts!
 ;;                                              [cook_state_list_jobs, cook_state_list_facts]
+;;   tools.clj:393-434 get-completed-jobs-by-user (completed, success, failed)
+;;                                           -> (list-completed ...), fed by completed-seed!, completed-record! and
+;;                                              completed-advance! [cook_state_list_completed, cook_state_completed_*]
 ;;   :217-313 write-status-to-datomic       -> (status! ...), fed by retry-config! and retry-facts!
 ;;                                             [cook_state_status, cook_state_retry_config, cook_state_retry_facts]
 ;;   :1210-1280 handle-match-cycle-metrics and the unmatched tracking :1399-1486
@@ -591,8 +594,8 @@
 
 ;; ---------------------------------------------------------------------------------------------
 ;; /list and /jobs over resident pools: the device half of get-active-jobs-by-user-and-state (tools.clj:445-466) for
-;; the waiting and running states; completed, success and failed, a name filter and a non-zero missing count keep the
-;; Datomic path
+;; the waiting and running states (completed, success and failed: list-completed below); a name filter and a non-zero
+;; missing count keep the Datomic path
 (defn list-facts!
   "The attributes the listing filters on, from the tx-report tap with each job upsert (which clears them), pending or
    running: [{:job-id :submit-ms :submit-pool (code, nil: none) :custom-executor (true, false or nil)}].  They never
@@ -631,6 +634,67 @@
                :running (vec (for [e es :when (= 2 (:state e))] (:job-id e)))
                :submit-ms (into {} (map (juxt :job-id :submit-ms)) es)
                :missing (aget out-n 1)}))))))
+
+;; The completed, success and failed states from each handle's completed-job log.  The tap sends completed-record!
+;; one record per job per transaction, its columns read from the db-after entity, its stamp the transaction's t:
+;;   :job/state becomes :job.state/completed      -> :success or :failed, by tools/job-ent->state
+;;   :job/state leaves :job.state/completed       -> :reopened (:job/ensure-not-completed, :job/update-retry-count)
+;;   a completed job gains a successful instance  -> :success
+;;   a listed attribute of a completed job changes (user, submit time, submit pool, custom executor) -> a new record
+;; The listing handler sends a completed-family state to list-completed when there is no name filter, the request's
+;; pools are on one device, every handle's log is on and start >= every horizon; otherwise the Datomic path.
+(def ^:private completed-kinds {:success 1 :failed 2 :reopened 3})
+(defn- completed-cols [rows]
+  (object-array [(longs-buf (map :job-id rows)) (longs-buf (map :stamp rows)) (ints-buf (map :user rows))
+                 (longs-buf (map :submit-ms rows)) (ints-buf (map #(or (:submit-pool %) -1) rows))
+                 (ints-buf (map #(case (:custom-executor %) true 1 false 0 -1) rows))
+                 (let [b (direct (count rows))]
+                   (doseq [[i r] (map-indexed vector rows)] (.put b (int i) (byte (completed-kinds (:kind r)))))
+                   b)]))
+
+(defn completed-seed!
+  "At start-up and on a leadership change, after the reset and the load and before the tap resumes: the pool's
+   completed jobs with submit >= since-ms, read once from one database value, [{:job-id :stamp (its basis t) :user
+   (code) :submit-ms :submit-pool (code, nil: none) :custom-executor (true, false or nil) :kind (:success or
+   :failed)}].  Turns the log on at horizon since-ms."
+  [handle since-ms rows]
+  (check! handle (Native/stateCompletedSeed handle (long since-ms) (count rows) (completed-cols rows))
+          "cook_state_completed_seed"))
+
+(defn completed-record!
+  "The tap's records of one transaction, as completed-seed!'s rows with :kind also :reopened; those submitted before
+   the horizon are skipped by the call."
+  [handle rows]
+  (check! handle (Native/stateCompletedRecord handle (count rows) (completed-cols rows)) "cook_state_completed_record"))
+
+(defn completed-advance!
+  "Periodically, with now - retention (the shim's setting, default 32 days): the horizon rises and the records of
+   jobs submitted before it leave."
+  [handle since-ms]
+  (check! handle (Native/stateCompletedAdvance handle (long since-ms)) "cook_state_completed_advance"))
+
+(defn list-completed
+  "`user`'s jobs whose latest record over `handles` (one device) is in `state` (:success, :failed or :completed),
+   submitted in [start-ms, end-ms), with entity ids in [job-id-lo, job-id-hi), in pool `pool-code` (-1: any;
+   `handle-pools` each handle's pool code), only false custom executors unless `include-custom-executor?`, cut to
+   `limit` in entity-id order.  The call is made with `cap` entries and, when it needs more, once more with the count
+   it reports.  Returns {:job-ids [job-id] :submit-ms {job-id ms}}, the handler's completed part of
+   list_jobs_response."
+  [handles user state start-ms end-ms job-id-lo job-id-hi pool-code handle-pools include-custom-executor? limit cap]
+  (loop [cap (max cap 1) tries 2]
+    (let [outs [(direct (* 8 cap)) (direct (* 8 cap)) (direct (* 4 cap))]
+          out-n (int-array 1)
+          rc (Native/stateListCompleted (long-array handles) (long-array [start-ms end-ms job-id-lo job-id-hi])
+                                        (int-array [user ({:success 1 :failed 2 :completed 3} state) pool-code
+                                                    (if include-custom-executor? 1 0) limit cap])
+                                        (when (not= pool-code -1) (ints-buf handle-pools)) (object-array outs) out-n nil)]
+      (if (and (= rc -7) (> tries 1))
+        (recur (aget out-n 0) (dec tries))
+        (do (check! (first handles) rc "cook_state_list_completed")
+            (let [n (aget out-n 0)
+                  ids (mapv #(.getLong ^ByteBuffer (outs 0) (int (* 8 %))) (range n))]
+              {:job-ids ids
+               :submit-ms (zipmap ids (map #(.getLong ^ByteBuffer (outs 1) (int (* 8 %))) (range n)))}))))))
 
 ;; ---------------------------------------------------------------------------------------------
 ;; the match-cycle metrics of a resident pool (handle-match-cycle-metrics scheduler.clj:1210-1280, the unmatched

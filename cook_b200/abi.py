@@ -169,6 +169,9 @@ MM_FIRST_N = 10
 
 # cook_state_list_jobs' states
 LJ_WAITING, LJ_RUNNING = 1, 2
+# cook_state_completed_*: a record's kind; cook_state_list_completed: the listed state
+CJ_SUCCESS, CJ_FAILED, CJ_REOPENED = 1, 2, 3
+LC_SUCCESS, LC_FAILED, LC_COMPLETED = 1, 2, 3
 
 # cook_state_retry_facts' bits and cook_state_status' outcomes
 RF_DISABLE_MEA_CULPA, RF_COMPLETED = 1, 2
@@ -362,6 +365,11 @@ ARGTYPES = {
     "cook_state_list_facts": [_H, _I32, P_I64, P_I64, P_I32, P_I32],
     "cook_state_list_jobs": [_P(_H), _I32, _I32, _I32, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _I32, P_I32, _I32,
                              _I32, _I32, P_I32, P_I64, P_I64, P_I32, P_I32, P_I32, _P(PhaseStats)],
+    "cook_state_completed_seed": [_H, C.c_int64, _I32, P_I64, P_I64, P_I32, P_I64, P_I32, P_I32, P_U8],
+    "cook_state_completed_record": [_H, _I32, P_I64, P_I64, P_I32, P_I64, P_I32, P_I32, P_U8],
+    "cook_state_completed_advance": [_H, C.c_int64],
+    "cook_state_list_completed": [_P(_H), _I32, _I32, _I32, C.c_int64, C.c_int64, C.c_int64, C.c_int64, _I32, P_I32,
+                                  _I32, _I32, _I32, P_I64, P_I64, P_I32, P_I32, _P(PhaseStats)],
     "cook_state_match_metrics": [_H, _I32, _I32, P_I32, _I32, _I32, P_I64, P_F64, P_I64, P_F64, P_I64, P_I32, P_I32,
                                  P_I32, P_I32, P_I32, P_F64, _P(PhaseStats)],
     "cook_state_finish": [_H, _I32, P_I64, P_I64, P_U8],

@@ -738,8 +738,32 @@ struct Records {
   void release() { free_all(); cap = tail = n_live = 0; }
 };
 
-// The finished instances (cook_state_history_*): 49 B per row in arrival order, dense in [0, tail); rows leave only by
-// a stable compaction (cook_state_history_advance).  Off until seeded; `since` is the horizon on start time.
+// A handle's append-only device table (the history, the completed-job log): rows in arrival order, dense in [0, tail);
+// capacity doubles with device-to-device copies, and rows leave only by a stable compaction into new columns.  Off
+// until seeded; `since` is the horizon.  Cols: alloc(n), free_all(), and copy(src, n, stream) of the first n rows.
+template <class Cols>
+struct Log {
+  Cols c;
+  int64_t cap = 0, tail = 0, since = 0;
+  bool on = false;
+  // capacity >= n: new columns holding the first `tail` rows (device to device)
+  cudaError_t grow(int64_t n, cudaStream_t st) {
+    if (n <= cap) return cudaSuccess;
+    const int64_t ncap = std::max<int64_t>(n, std::max<int64_t>(2 * cap, 4096));
+    Cols nc;
+    cudaError_t e = nc.alloc(ncap);
+    if (e == cudaSuccess && tail) e = nc.copy(c, tail, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { nc.free_all(); return e; }
+    c.free_all();
+    c = nc;
+    cap = ncap;
+    return cudaSuccess;
+  }
+  void release() { c.free_all(); cap = tail = since = 0; on = false; }
+};
+
+// The finished instances (cook_state_history_*): 49 B per row; the horizon is on start time.
 struct HistCols {
   int64_t* tid = nullptr; int64_t* start = nullptr; int64_t* end = nullptr; double* cpus = nullptr; double* mem = nullptr;
   int32_t* user = nullptr; int32_t* reason = nullptr; uint8_t* ok = nullptr;
@@ -757,38 +781,58 @@ struct HistCols {
       if (p) cudaFree(p);
     *this = HistCols{};
   }
-};
-struct History {
-  HistCols c;
-  int64_t cap = 0, tail = 0, since = 0;
-  bool on = false;
-  // capacity >= n: new columns holding the first `tail` rows (device to device)
-  cudaError_t grow(int64_t n, cudaStream_t st) {
-    if (n <= cap) return cudaSuccess;
-    const int64_t ncap = std::max<int64_t>(n, std::max<int64_t>(2 * cap, 4096));
-    HistCols nc;
-    cudaError_t e = nc.alloc(ncap);
-    if (e == cudaSuccess && tail) e = copy_rows(nc, c, tail, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) { nc.free_all(); return e; }
-    c.free_all();
-    c = nc;
-    cap = ncap;
-    return cudaSuccess;
-  }
-  static cudaError_t copy_rows(const HistCols& d, const HistCols& s, int64_t n, cudaStream_t st) {
+  cudaError_t copy(const HistCols& s, int64_t n, cudaStream_t st) const {
     const cudaMemcpyKind k = cudaMemcpyDeviceToDevice;
-    cudaError_t e = cudaMemcpyAsync(d.tid, s.tid, 8 * n, k, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d.start, s.start, 8 * n, k, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d.end, s.end, 8 * n, k, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d.cpus, s.cpus, 8 * n, k, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d.mem, s.mem, 8 * n, k, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d.user, s.user, 4 * n, k, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d.reason, s.reason, 4 * n, k, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d.ok, s.ok, n, k, st);
+    cudaError_t e = cudaMemcpyAsync(tid, s.tid, 8 * n, k, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(start, s.start, 8 * n, k, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(end, s.end, 8 * n, k, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(cpus, s.cpus, 8 * n, k, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(mem, s.mem, 8 * n, k, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(user, s.user, 4 * n, k, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(reason, s.reason, 4 * n, k, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(ok, s.ok, n, k, st);
     return e;
   }
-  void release() { c.free_all(); cap = tail = since = 0; on = false; }
+};
+using History = Log<HistCols>;
+
+// The completed-job log (cook_state_completed_*): 34 B per row, a job-state record each; the horizon is on submit time.
+struct CJCols {
+  int64_t* jid = nullptr; int64_t* stamp = nullptr; int64_t* submit = nullptr; int32_t* user = nullptr;
+  int32_t* spool = nullptr; int8_t* exec = nullptr; uint8_t* kind = nullptr;
+  cudaError_t alloc(int64_t n) {
+    cudaError_t e = cudaSuccess;
+    for (void** p : {(void**)&jid, (void**)&stamp, (void**)&submit}) if (e == cudaSuccess) e = cudaMalloc(p, 8 * n);
+    for (void** p : {(void**)&user, (void**)&spool}) if (e == cudaSuccess) e = cudaMalloc(p, 4 * n);
+    for (void** p : {(void**)&exec, (void**)&kind}) if (e == cudaSuccess) e = cudaMalloc(p, n);
+    if (e != cudaSuccess) free_all();
+    return e;
+  }
+  void free_all() {
+    for (void* p : {(void*)jid, (void*)stamp, (void*)submit, (void*)user, (void*)spool, (void*)exec, (void*)kind})
+      if (p) cudaFree(p);
+    *this = CJCols{};
+  }
+  cudaError_t copy(const CJCols& s, int64_t n, cudaStream_t st) const {
+    const cudaMemcpyKind k = cudaMemcpyDeviceToDevice;
+    cudaError_t e = cudaMemcpyAsync(jid, s.jid, 8 * n, k, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(stamp, s.stamp, 8 * n, k, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(submit, s.submit, 8 * n, k, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(user, s.user, 4 * n, k, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(spool, s.spool, 4 * n, k, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(exec, s.exec, n, k, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(kind, s.kind, n, k, st);
+    return e;
+  }
+};
+// The device log and, by row on the host, each row's user and submit time: the listing sizes its buffers by the
+// user's rows, and the advance knows whose rows it drops, without a transfer.
+struct Completed : Log<CJCols> {
+  std::vector<int32_t> h_user;
+  std::vector<int64_t> h_submit;
+  std::unordered_map<int32_t, int64_t> users;   // user -> rows
+  void clear_rows() { tail = 0; h_user.clear(); h_submit.clear(); users.clear(); }
+  void release() { Log<CJCols>::release(); clear_rows(); }
 };
 
 void count_add(std::map<int32_t, int64_t>& m, int32_t code, int64_t d) {
@@ -853,6 +897,7 @@ struct PoolState {
   Records rec;                                 // the successful runtimes per group
   std::map<int32_t, int64_t> rec_groups;       // group code -> live records
   History hist;                                // the finished instances
+  Completed cj;                                // the completed-job log
   ListArena lists[L_N];
   ListArena olists[OL_N];
   std::map<int32_t, int64_t> users_p, users_r, attr_cols, groups;   // code -> live uses
@@ -897,7 +942,7 @@ struct PoolState {
     olists[OL_GPU].esz1 = olists[OL_DISK].esz1 = 8;
   }
   void release() {
-    pend.release(); run.release(); offer.release(); rec.release(); hist.release();
+    pend.release(); run.release(); offer.release(); rec.release(); hist.release(); cj.release();
     for (auto& l : lists) l.release();
     for (auto& l : olists) l.release();
     stage.release(); scratch.release(); derive.release(); queue.release(); omerge.release();
@@ -1180,6 +1225,9 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
     S->rec_groups.clear();
     S->hist.tail = S->hist.since = 0;
     S->hist.on = false;
+    S->cj.clear_rows();
+    S->cj.since = 0;
+    S->cj.on = false;
     S->reserved.clear();
     for (auto& f : S->nflag) f = 0;
     for (auto& l : S->lists) l.tail = l.live = 0;
@@ -6306,14 +6354,16 @@ struct LessJobPoolTask {
   }
 };
 
-struct LJPick {
+// the first row of each job (BY_POOL: of each (job id, pool index)) in a sorted order, when it passes the filters
+template <bool BY_POOL>
+struct JobPick {
   const int32_t* ord; const int64_t* jid; const int32_t* pi; const int64_t* submit; const uint8_t* ok;
   int64_t* o_jid; int64_t* o_submit; int32_t* o_pi;
   __device__ bool keep(int p) const {
     const int i = ord[p];
     if (p > 0) {
       const int k = ord[p - 1];
-      if (jid[k] == jid[i] && pi[k] == pi[i]) return false;
+      if (jid[k] == jid[i] && (!BY_POOL || pi[k] == pi[i])) return false;
     }
     return ok[i];
   }
@@ -6322,6 +6372,7 @@ struct LJPick {
     o_jid[d] = jid[i]; o_submit[d] = submit[i]; o_pi[d] = pi[i];
   }
 };
+using LJPick = JobPick<true>;
 
 LJCols lj_cols(const PoolState* s, bool running) {
   if (running) {
@@ -6400,6 +6451,26 @@ int32_t list_facts(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, 
   return COOK_OK;
 }
 
+// the listing arguments cook_state_list_jobs and cook_state_list_completed share
+int32_t check_list_args(cook_pool* pool, const char* who, int32_t user, const LJSel& q, const int32_t* handle_pool,
+                        int32_t limit, int32_t cap) {
+  if (user < 0) return set_err(pool, COOK_E_BADARG, "%s: a negative user", who);
+  if (q.pool < -1 || (q.pool != -1 && !handle_pool))
+    return set_err(pool, COOK_E_BADARG, "%s: pool_code below -1, or no handle_pool", who);
+  if (q.all_exec != 0 && q.all_exec != 1) return set_err(pool, COOK_E_BADARG, "%s: include_custom_executor outside {0, 1}", who);
+  if (limit < 0 || cap < 0) return set_err(pool, COOK_E_BADARG, "%s: limit < 0 or cap < 0", who);
+  return COOK_OK;
+}
+
+// n listed entries down: job id, submit time, pool index (20 B each)
+cudaError_t download_entries(int64_t* o_jid, int64_t* o_submit, int32_t* o_pool, const int64_t* jid, const int64_t* submit,
+                             const int32_t* pi, int n, cudaStream_t st, int64_t* d2h) {
+  cudaError_t e = download(o_jid, jid, n, st, d2h);
+  if (e == cudaSuccess) e = download(o_submit, submit, n, st, d2h);
+  if (e == cudaSuccess) e = download(o_pool, pi, n, st, d2h);
+  return e;
+}
+
 int32_t list_jobs(cook_pool* const* pools, int n, int32_t user, int32_t states, const LJSel& q, const int32_t* handle_pool,
                   int32_t limit, int32_t cap, int32_t* o_state, int64_t* o_jid, int64_t* o_submit, int32_t* o_pool,
                   int32_t* o_n, int32_t* o_missing, cook_phase_stats* out_stats) {
@@ -6409,11 +6480,7 @@ int32_t list_jobs(cook_pool* const* pools, int n, int32_t user, int32_t states, 
   cook_pool* pool = pools[0];
   if (states <= 0 || (states & ~(COOK_LJ_WAITING | COOK_LJ_RUNNING)))
     return set_err(pool, COOK_E_BADARG, "%s: states 0 or with unknown bits", who);
-  if (user < 0) return set_err(pool, COOK_E_BADARG, "%s: a negative user", who);
-  if (q.pool < -1 || (q.pool != -1 && !handle_pool))
-    return set_err(pool, COOK_E_BADARG, "%s: pool_code below -1, or no handle_pool", who);
-  if (q.all_exec != 0 && q.all_exec != 1) return set_err(pool, COOK_E_BADARG, "%s: include_custom_executor outside {0, 1}", who);
-  if (limit < 0 || cap < 0) return set_err(pool, COOK_E_BADARG, "%s: limit < 0 or cap < 0", who);
+  if (int32_t rc = check_list_args(pool, who, user, q, handle_pool, limit, cap)) return rc;
   if (!o_state || !o_jid || !o_submit || !o_pool || !o_n || !o_missing) return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
   // per state (0 waiting, 1 running): the handles holding a row of the user, and the rows (the host-side counts)
   struct Src { const PoolState* s; int32_t k; int rows; };
@@ -6501,9 +6568,8 @@ int32_t list_jobs(cook_pool* const* pools, int n, int32_t user, int32_t states, 
   int at = 0;
   for (int t = 0; t < 2; t++) {
     if (!got[t]) continue;
-    CK(pool, download(o_jid + at, D[t].o_jid, got[t], st, &d2h));
-    CK(pool, download(o_submit + at, D[t].o_submit, got[t], st, &d2h));
-    CK(pool, download(o_pool + at, D[t].o_pi, got[t], st, &d2h));
+    CK(pool, download_entries(o_jid + at, o_submit + at, o_pool + at, D[t].o_jid, D[t].o_submit, D[t].o_pi, got[t], st,
+                              &d2h));
     std::fill(o_state + at, o_state + at + got[t], t ? COOK_LJ_RUNNING : COOK_LJ_WAITING);
     at += got[t];
   }
@@ -6511,6 +6577,270 @@ int32_t list_jobs(cook_pool* const* pools, int n, int32_t user, int32_t states, 
   CK(pool, cudaStreamSynchronize(st));
   *o_n = at;
   *o_missing = got[2];
+  if (out_stats) *out_stats = call_stats(pool, h2d, d2h, nl);
+  return COOK_OK;
+}
+
+// ---- the completed-job log (cook_state_completed_*) and its listing (cook_state_list_completed, the completed, success
+// and failed states; get-completed-jobs-by-user, tools.clj:393-434).  The listing: a compaction per handle gathers the
+// user's records (job id, stamp, submit time, pool index, and whether the record passes the filters) after the handles
+// before; one sort by (job id, stamp descending, dense index descending) puts each job's latest record first (the dense
+// index grows with (handle, row)); a second compaction keeps each job's first record when it passes, up to `limit`.
+static_assert((int)COOK_CJ_SUCCESS == (int)COOK_LC_SUCCESS && (int)COOK_CJ_FAILED == (int)COOK_LC_FAILED,
+              "a listed state names the record kind it keeps");
+struct CJRows {
+  CJCols c; int32_t user; int base; int32_t pidx; bool pool_ok; LJSel q; int32_t state;
+  int64_t* jid; int64_t* stamp; int64_t* submit; int32_t* pi; uint8_t* ok;
+  __device__ bool keep(int i) const { return c.user[i] == user; }
+  __device__ void emit(int i, int d) const {
+    d += base;
+    const int64_t j = c.jid[i], s = c.submit[i];
+    const uint8_t k = c.kind[i];
+    jid[d] = j;
+    stamp[d] = c.stamp[i];
+    submit[d] = s;
+    pi[d] = pidx;
+    ok[d] = k != COOK_CJ_REOPENED && (state == COOK_LC_COMPLETED || k == state) && s >= q.start && s < q.end &&
+            j >= q.lo && j < q.hi && (pool_ok || c.spool[i] == q.pool) && (q.all_exec || c.exec[i] == 0);
+  }
+};
+
+// (job id, stamp descending, dense index descending): each job's latest record first
+struct LessJobStamp {
+  const int64_t* jid; const int64_t* stamp;
+  __device__ bool operator()(int32_t a, int32_t b) const {
+    if (jid[a] != jid[b]) return jid[a] < jid[b];
+    if (stamp[a] != stamp[b]) return stamp[a] > stamp[b];
+    return a > b;
+  }
+};
+
+struct CJKeep {   // the advance's compaction: the rows submitted at or after the new horizon, in order
+  CJCols s, d; int64_t since;
+  __device__ bool keep(int i) const { return s.submit[i] >= since; }
+  __device__ void emit(int i, int k) const {
+    d.jid[k] = s.jid[i]; d.stamp[k] = s.stamp[i]; d.submit[k] = s.submit[i]; d.user[k] = s.user[i];
+    d.spool[k] = s.spool[i]; d.exec[k] = s.exec[i]; d.kind[k] = s.kind[i];
+  }
+};
+
+// The host columns of a seed or record batch, checked row by row: the rows kept (submit >= since), the executor as the
+// stored byte.
+struct CJBatch {
+  std::vector<int64_t> jid, stamp, submit;
+  std::vector<int32_t> user, spool;
+  std::vector<int8_t> exec;
+  std::vector<uint8_t> kind;
+};
+
+int32_t cj_batch(cook_pool* pool, const char* who, int n, int64_t since, bool skip, const int64_t* job_id,
+                 const int64_t* stamp, const int32_t* user, const int64_t* submit_ms, const int32_t* submit_pool,
+                 const int32_t* custom_executor, const uint8_t* kind, CJBatch* b) {
+  if (n < 0) return set_err(pool, COOK_E_BADARG, "%s: n < 0", who);
+  if (n && (!job_id || !stamp || !user || !submit_ms || !submit_pool || !custom_executor || !kind))
+    return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
+  std::unordered_set<int64_t> seen;
+  seen.reserve((size_t)n);
+  for (int i = 0; i < n; i++) {
+    if (submit_ms[i] < since && !skip) return set_err(pool, COOK_E_BADARG, "%s: a row submitted before since_ms", who);
+    if (user[i] < 0 || stamp[i] < 0) return set_err(pool, COOK_E_BADARG, "%s: a negative user or stamp", who);
+    if (kind[i] < COOK_CJ_SUCCESS || kind[i] > COOK_CJ_REOPENED) return set_err(pool, COOK_E_BADARG, "%s: an unknown kind", who);
+    if (custom_executor[i] < -1 || custom_executor[i] > 1)
+      return set_err(pool, COOK_E_BADARG, "%s: a custom_executor outside {-1, 0, 1}", who);
+    if (submit_pool[i] < -1) return set_err(pool, COOK_E_BADARG, "%s: a submit pool code below -1", who);
+    if (!seen.insert(job_id[i]).second) return set_err(pool, COOK_E_BADARG, "%s: job id twice", who);
+  }
+  for (int i = 0; i < n; i++) {
+    if (submit_ms[i] < since) continue;
+    b->jid.push_back(job_id[i]); b->stamp.push_back(stamp[i]); b->submit.push_back(submit_ms[i]);
+    b->user.push_back(user[i]); b->spool.push_back(submit_pool[i]); b->exec.push_back((int8_t)custom_executor[i]);
+    b->kind.push_back(kind[i]);
+  }
+  return COOK_OK;
+}
+
+// the batch's rows appended at the log's tail, straight into its columns
+int32_t cj_append(cook_pool* pool, PoolState* S, const CJBatch& b, const char* who) {
+  Completed& L = S->cj;
+  const int64_t k = (int64_t)b.jid.size();
+  if (L.tail + k > INT32_MAX) return set_err(pool, COOK_E_TOO_LARGE, "%s: more than 2^31 - 1 log rows", who);
+  cudaStream_t st = pool->stream;
+  CK(pool, L.grow(L.tail + k, st));
+  CK(pool, cudaEventRecord(pool->ev[20], st));
+  Carve c;   // only its copy(): the bytes counted, the first error kept
+  c.st = st;
+  const int64_t t = L.tail;
+  if (k) {
+    c.copy(L.c.jid + t, b.jid.data(), k); c.copy(L.c.stamp + t, b.stamp.data(), k);
+    c.copy(L.c.submit + t, b.submit.data(), k); c.copy(L.c.user + t, b.user.data(), k);
+    c.copy(L.c.spool + t, b.spool.data(), k); c.copy(L.c.exec + t, b.exec.data(), k);
+    c.copy(L.c.kind + t, b.kind.data(), k);
+  }
+  CK(pool, c.err);
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  CK(pool, cudaStreamSynchronize(st));
+  L.tail += k;
+  L.h_user.insert(L.h_user.end(), b.user.begin(), b.user.end());
+  L.h_submit.insert(L.h_submit.end(), b.submit.begin(), b.submit.end());
+  for (int32_t u : b.user) L.users[u]++;
+  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], c.h2d, 0, 0);
+  return COOK_OK;
+}
+
+int32_t completed_seed(cook_pool* pool, PoolState* S, int64_t since_ms, int n, const int64_t* job_id, const int64_t* stamp,
+                       const int32_t* user, const int64_t* submit_ms, const int32_t* submit_pool,
+                       const int32_t* custom_executor, const uint8_t* kind) {
+  const char* who = "cook_state_completed_seed";
+  CJBatch b;
+  if (int32_t rc = cj_batch(pool, who, n, since_ms, false, job_id, stamp, user, submit_ms, submit_pool, custom_executor,
+                            kind, &b))
+    return rc;
+  Completed& L = S->cj;
+  L.clear_rows();
+  L.since = since_ms;
+  L.on = true;
+  return cj_append(pool, S, b, who);
+}
+
+int32_t completed_record(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, const int64_t* stamp,
+                         const int32_t* user, const int64_t* submit_ms, const int32_t* submit_pool,
+                         const int32_t* custom_executor, const uint8_t* kind) {
+  const char* who = "cook_state_completed_record";
+  if (!S->cj.on) return set_err(pool, COOK_E_BADARG, "%s: the log is off", who);
+  CJBatch b;
+  if (int32_t rc = cj_batch(pool, who, n, S->cj.since, true, job_id, stamp, user, submit_ms, submit_pool,
+                            custom_executor, kind, &b))
+    return rc;
+  return cj_append(pool, S, b, who);
+}
+
+// the horizon raised to since_ms: the rows submitted before it leave in one compaction into new columns, and from the
+// host's rows
+int32_t completed_advance(cook_pool* pool, PoolState* S, int64_t since_ms) {
+  const char* who = "cook_state_completed_advance";
+  Completed& L = S->cj;
+  if (!L.on) return set_err(pool, COOK_E_BADARG, "%s: the log is off", who);
+  if (since_ms < L.since) return set_err(pool, COOK_E_BADARG, "%s: since_ms below the horizon", who);
+  CK(pool, cudaSetDevice(pool->device));
+  cudaStream_t st = pool->stream;
+  int32_t* blk = nullptr;
+  const int T = (int)L.tail;
+  const bool move = T && since_ms > L.since;
+  CK(pool, carve(S->scratch, st, pool->ev[20], nullptr, [&](Carve& c) {
+    if (move) blk = c.take<int32_t>((size_t)T / CP_BLOCK + 2);
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  int nl = 0;
+  int64_t d2h = 0;
+  if (move) {
+    CJCols nc;
+    CK(pool, nc.alloc(L.cap));
+    compact(CJKeep{L.c, nc, since_ms}, T, nullptr, blk, S->counters + 7, T, st, &nl);
+    int32_t kept = 0;
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = download(&kept, S->counters + 7, 1, st, &d2h);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { nc.free_all(); CK(pool, e); }
+    L.c.free_all();
+    L.c = nc;
+    L.tail = kept;
+  }
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  CK(pool, cudaStreamSynchronize(st));
+  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], 0, d2h, nl);
+  if (move) {   // the host's rows, by the same rule and in the same order
+    int64_t w = 0;
+    for (int64_t i = 0; i < T; i++) {
+      if (L.h_submit[i] >= since_ms) {
+        L.h_user[w] = L.h_user[i];
+        L.h_submit[w++] = L.h_submit[i];
+      } else if (--L.users[L.h_user[i]] == 0) {
+        L.users.erase(L.h_user[i]);
+      }
+    }
+    L.h_user.resize(w);
+    L.h_submit.resize(w);
+    if (L.tail != w) return set_err(pool, COOK_E_CUDA, "%s: the device kept %lld rows, the host %lld", who,
+                                    (long long)L.tail, (long long)w);
+  }
+  L.since = since_ms;
+  return COOK_OK;
+}
+
+int32_t list_completed(cook_pool* const* pools, int n, int32_t user, int32_t state, const LJSel& q,
+                       const int32_t* handle_pool, int32_t limit, int32_t cap, int64_t* o_jid, int64_t* o_submit,
+                       int32_t* o_pool, int32_t* o_n, cook_phase_stats* out_stats) {
+  const char* who = "cook_state_list_completed";
+  // ---- every check before any device work or output
+  if (int32_t rc = check_handle_set(pools, n, who)) return rc;
+  cook_pool* pool = pools[0];
+  if (state != COOK_LC_SUCCESS && state != COOK_LC_FAILED && state != COOK_LC_COMPLETED)
+    return set_err(pool, COOK_E_BADARG, "%s: an unknown state", who);
+  if (int32_t rc = check_list_args(pool, who, user, q, handle_pool, limit, cap)) return rc;
+  if (!o_jid || !o_submit || !o_pool || !o_n) return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
+  // the handles holding a record of the user, and the records (the host-side counts)
+  struct Src { const Completed* l; int32_t k; int rows; };
+  std::vector<Src> hs;
+  int64_t C = 0;
+  int tmax = 0;
+  for (int k = 0; k < n; k++) {
+    const PoolState* s = static_cast<const PoolState*>(pools[k]->state);
+    if (!s || !s->cj.on) return set_err(pool, COOK_E_BADARG, "%s: a handle whose log is off", who);
+    if (s->cj.since > q.start) return set_err(pool, COOK_E_BADARG, "%s: start_ms before a handle's horizon", who);
+    auto it = s->cj.users.find(user);
+    if (it == s->cj.users.end()) continue;
+    hs.push_back({&s->cj, k, (int)it->second});
+    C += it->second;
+    tmax = std::max(tmax, (int)s->cj.tail);
+  }
+  if (C > INT32_MAX) return set_err(pool, COOK_E_TOO_LARGE, "%s: more than 2^31 - 1 records of the user", who);
+  if (C == 0) {   // no record to read: empty results without device work
+    *o_n = 0;
+    if (out_stats) *out_stats = cook_phase_stats{};
+    return COOK_OK;
+  }
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S0 = state_of(pool, true);   // pools[0]'s scratch, even when it holds no record
+  if (!S0) return set_err(pool, COOK_E_OOM, "%s: out of device memory", who);
+  cudaStream_t st = pool->stream;
+  // ---- one carve: the records, their order, the entries, the counts
+  const int Cn = (int)C, On = std::min(Cn, limit);
+  int64_t *jid = nullptr, *stamp = nullptr, *submit = nullptr, *e_jid = nullptr, *e_submit = nullptr;
+  int32_t *pi = nullptr, *ord = nullptr, *tmp = nullptr, *e_pi = nullptr, *cnt = nullptr, *blk = nullptr;
+  uint8_t* ok = nullptr;
+  int64_t h2d = 0, d2h = 0;
+  CK(pool, carve(S0->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+    cnt = c.take<int32_t>(2);   // [0] the entries, [1] the record compactions' own
+    blk = c.take<int32_t>((size_t)std::max(tmax, Cn) / CP_BLOCK + 2);
+    jid = c.take<int64_t>(Cn); stamp = c.take<int64_t>(Cn); submit = c.take<int64_t>(Cn);
+    pi = c.take<int32_t>(Cn); ok = c.take<uint8_t>(Cn); ord = c.take<int32_t>(Cn); tmp = c.take<int32_t>(Cn);
+    e_jid = c.take<int64_t>(On); e_submit = c.take<int64_t>(On); e_pi = c.take<int32_t>(On);
+  }));
+  CK(pool, cudaEventRecord(pool->ev[21], st));
+  int nl = 0;
+  int base = 0;
+  for (const Src& h : hs) {
+    const bool pool_ok = q.pool == -1 || handle_pool[h.k] == q.pool;
+    compact(CJRows{h.l->c, user, base, h.k, pool_ok, q, state, jid, stamp, submit, pi, ok}, (int)h.l->tail, nullptr, blk,
+            cnt + 1, h.rows, st, &nl);
+    base += h.rows;
+  }
+  CK(pool, csort::sort_indices(ord, tmp, Cn, LessJobStamp{jid, stamp}, st, &nl));
+  compact(JobPick<false>{ord, jid, pi, submit, ok, e_jid, e_submit, e_pi}, Cn, nullptr, blk, cnt, limit, st, &nl);
+  CK(pool, cudaGetLastError());
+  CK(pool, cudaEventRecord(pool->ev[22], st));
+  int32_t got = 0;
+  CK(pool, download(&got, cnt, 1, st, &d2h));
+  CK(pool, cudaStreamSynchronize(st));
+  if (got > cap) {
+    *o_n = got;
+    return set_err(pool, COOK_E_TOO_LARGE, "%s: more entries than cap: %d", who, got);
+  }
+  if (got) CK(pool, download_entries(o_jid, o_submit, o_pool, e_jid, e_submit, e_pi, got, st, &d2h));
+  CK(pool, cudaEventRecord(pool->ev[23], st));
+  CK(pool, cudaStreamSynchronize(st));
+  *o_n = got;
   if (out_stats) *out_stats = call_stats(pool, h2d, d2h, nl);
   return COOK_OK;
 }
@@ -6535,4 +6865,44 @@ extern "C" int32_t cook_state_list_jobs(cook_pool* const* pools, int32_t n_pools
   const LJSel q{start_ms, end_ms, job_id_lo, job_id_hi, pool_code, include_custom_executor};
   return list_jobs(pools, n_pools, user, states, q, handle_pool, limit, cap, out_state, out_job_id, out_submit_ms,
                    out_pool, out_n, out_n_missing, out_stats);
+}
+
+extern "C" int32_t cook_state_completed_seed(cook_pool* pool, int64_t since_ms, int32_t n, const int64_t* job_id,
+                                             const int64_t* stamp, const int32_t* user, const int64_t* submit_ms,
+                                             const int32_t* submit_pool, const int32_t* custom_executor,
+                                             const uint8_t* kind) {
+  if (!pool) return COOK_E_BADARG;
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_completed_seed: out of device memory");
+  return completed_seed(pool, S, since_ms, n, job_id, stamp, user, submit_ms, submit_pool, custom_executor, kind);
+}
+
+extern "C" int32_t cook_state_completed_record(cook_pool* pool, int32_t n, const int64_t* job_id, const int64_t* stamp,
+                                               const int32_t* user, const int64_t* submit_ms, const int32_t* submit_pool,
+                                               const int32_t* custom_executor, const uint8_t* kind) {
+  if (!pool) return COOK_E_BADARG;
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_completed_record: out of device memory");
+  return completed_record(pool, S, n, job_id, stamp, user, submit_ms, submit_pool, custom_executor, kind);
+}
+
+extern "C" int32_t cook_state_completed_advance(cook_pool* pool, int64_t since_ms) {
+  if (!pool) return COOK_E_BADARG;
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_completed_advance: out of device memory");
+  return completed_advance(pool, S, since_ms);
+}
+
+extern "C" int32_t cook_state_list_completed(cook_pool* const* pools, int32_t n_pools, int32_t user, int32_t state,
+                                             int64_t start_ms, int64_t end_ms, int64_t job_id_lo, int64_t job_id_hi,
+                                             int32_t pool_code, const int32_t* handle_pool,
+                                             int32_t include_custom_executor, int32_t limit, int32_t cap,
+                                             int64_t* out_job_id, int64_t* out_submit_ms, int32_t* out_pool,
+                                             int32_t* out_n, cook_phase_stats* out_stats) {
+  const LJSel q{start_ms, end_ms, job_id_lo, job_id_hi, pool_code, include_custom_executor};
+  return list_completed(pools, n_pools, user, state, q, handle_pool, limit, cap, out_job_id, out_submit_ms, out_pool,
+                        out_n, out_stats);
 }

@@ -482,6 +482,43 @@ class GpuEngine:
         if rc != 0:
             self._err(rc)
 
+    def _completed_cols(self, who, job_id, stamp, user, submit_ms, submit_pool, custom_executor, kind):
+        cols = (np.ascontiguousarray(job_id, np.int64), np.ascontiguousarray(stamp, np.int64),
+                np.ascontiguousarray(user, np.int32), np.ascontiguousarray(submit_ms, np.int64),
+                np.ascontiguousarray(submit_pool, np.int32), np.ascontiguousarray(custom_executor, np.int32),
+                np.ascontiguousarray(kind, np.uint8))
+        if any(len(c) != len(cols[0]) for c in cols):
+            raise ValueError(f"{who}: a column differs in length from job_id")
+        ptrs = [abi.ptr(c, t) for c, t in zip(cols, (abi.P_I64, abi.P_I64, abi.P_I32, abi.P_I64, abi.P_I32, abi.P_I32,
+                                                     abi.P_U8))]
+        return len(cols[0]), ptrs
+
+    def state_completed_seed(self, since_ms, job_id=(), stamp=(), user=(), submit_ms=(), submit_pool=(),
+                             custom_executor=(), kind=()):
+        """cook_state_completed_seed: the completed-job log replaced by these records (kind abi.CJ_*, custom executor
+        -1 nil, 0 false, 1 true) at horizon since_ms on submit time, and on."""
+        n, p = self._completed_cols("state_completed_seed", job_id, stamp, user, submit_ms, submit_pool,
+                                    custom_executor, kind)
+        rc = self.lib.cook_state_completed_seed(self.pool, int(since_ms), n, *p)
+        if rc != 0:
+            self._err(rc)
+
+    def state_completed_record(self, job_id=(), stamp=(), user=(), submit_ms=(), submit_pool=(), custom_executor=(),
+                               kind=()):
+        """cook_state_completed_record: these records appended in order; those submitted before the horizon are
+        skipped."""
+        n, p = self._completed_cols("state_completed_record", job_id, stamp, user, submit_ms, submit_pool,
+                                    custom_executor, kind)
+        rc = self.lib.cook_state_completed_record(self.pool, n, *p)
+        if rc != 0:
+            self._err(rc)
+
+    def state_completed_advance(self, since_ms):
+        """cook_state_completed_advance: the horizon raised to since_ms; the records submitted before it leave."""
+        rc = self.lib.cook_state_completed_advance(self.pool, int(since_ms))
+        if rc != 0:
+            self._err(rc)
+
     def state_group_runtimes(self, group=(), runtime_s=(), forget=()):
         """cook_state_group_runtimes: the records of the groups in `forget` leave, then (group[i], runtime_s[i]) are
         appended."""
@@ -971,6 +1008,42 @@ def state_list_jobs(engines, user, states, start_ms, end_ms, job_id_lo=-(1 << 63
     k = n.value
     return {"state": state[:k], "job_id": jid[:k], "submit_ms": sub[:k], "pool": pool[:k], "missing": missing.value,
             "stats": st.as_dict()}
+
+
+def state_list_completed(engines, user, state, start_ms, end_ms, job_id_lo=-(1 << 63), job_id_hi=(1 << 63) - 1,
+                         pool_code=-1, handle_pool=None, include_custom_executor=True, limit=(1 << 31) - 1, cap=1024):
+    """cook_state_list_completed over the completed-job logs of `engines` (one device, the work on engines[0]'s
+    stream): user code `user`'s jobs whose latest record is of `state` (abi.LC_SUCCESS, abi.LC_FAILED or
+    abi.LC_COMPLETED), submitted in [start_ms, end_ms), with job ids in [job_id_lo, job_id_hi), in the pool `pool_code`
+    (-1: any; handle_pool: each engine's pool code), cut to `limit`.  Returns 'job_id', 'submit_ms' and 'pool' (the
+    engine index of the latest record) as numpy columns in ascending job id, and 'stats', the call's own phase
+    statistics.  The call is made with `cap` entries first and, when more are needed, once more with the count it
+    reports."""
+    if not engines:
+        raise ValueError("state_list_completed: at least one handle")
+    hp = np.ascontiguousarray(handle_pool if handle_pool is not None else (), np.int32)
+    if handle_pool is not None and len(hp) != len(engines):
+        raise ValueError("state_list_completed: handle_pool differs in length from engines")
+    handles = (C.c_void_p * len(engines))(*[e.pool for e in engines])
+    n = C.c_int32(0)
+    st = abi.PhaseStats()
+    cap = max(int(cap), 0)
+    for _ in range(2):
+        m = max(cap, 1)
+        pool = np.zeros(m, np.int32)
+        jid, sub = np.zeros(m, np.int64), np.zeros(m, np.int64)
+        rc = engines[0].lib.cook_state_list_completed(
+            handles, len(engines), int(user), int(state), int(start_ms), int(end_ms), int(job_id_lo), int(job_id_hi),
+            int(pool_code), abi.ptr(hp, abi.P_I32) if handle_pool is not None else None, int(bool(include_custom_executor)),
+            int(limit), cap, abi.ptr(jid, abi.P_I64), abi.ptr(sub, abi.P_I64), abi.ptr(pool, abi.P_I32), C.byref(n),
+            C.byref(st))
+        if rc != abi.COOK_E_TOO_LARGE or n.value <= cap:
+            break
+        cap = n.value
+    if rc != 0:
+        engines[0]._err(rc)
+    k = n.value
+    return {"job_id": jid[:k], "submit_ms": sub[:k], "pool": pool[:k], "stats": st.as_dict()}
 
 
 def _is_answer(engines, call, cap):

@@ -1461,6 +1461,86 @@ int32_t cook_state_list_jobs(cook_pool* const* pools, int32_t n_pools, int32_t u
                              int32_t* out_state, int64_t* out_job_id, int64_t* out_submit_ms, int32_t* out_pool,
                              int32_t* out_n, int32_t* out_n_missing, cook_phase_stats* out_stats);
 
+/* ------------------------------------------------- completed-job log and its listing */
+/* The device half of GET /list and the list form of GET /jobs for the completed, success and failed states
+ * (get-completed-jobs-by-user, tools.clj:393-434), read from a per-handle log of job-state records instead of a walk
+ * of every job the user submitted in the window.
+ *
+ * A handle's log: a device table of job-state records, 34 B per row (job id i64, stamp i64, submit ms i64, user i32,
+ * submit pool code i32 with -1 for none, custom executor i8 with -1 nil / 0 false / 1 true, kind u8), in arrival
+ * order.  Capacity doubles with device-to-device copies; rows leave only by a stable compaction.  The host keeps each
+ * row's user and submit time too (12 B per row), so that the listing is sized without a transfer.  The log is off
+ * until seeded; while it is off, no other call changes its behaviour or cost.  Not part of cook_state_digest or
+ * cook_state_export (after a resync the caller seeds it again); a reset through cook_state_apply empties it and turns
+ * it off.  No other call writes it: cook_state_apply, _launch, _status and _finish_history keep their columns,
+ * launches and transfers.
+ * Fixed choices:
+ *   Kinds    COOK_CJ_SUCCESS and COOK_CJ_FAILED: the job is completed, its state success when an instance succeeded
+ *            (job-ent->state); COOK_CJ_REOPENED: the job left the completed state (:job/ensure-not-completed,
+ *            :job/update-retry-count, reached from /retry).
+ *   Latest   a job's state is its record with the greatest stamp over the handles asked; equal stamps go to the greater
+ *            handle index, then the later row.  The stamp is the Datomic t of the transaction that made the change, so
+ *            a record sent twice changes nothing, and a job that moved pools between a reopen and a second completion
+ *            is answered once.  A job whose latest record is REOPENED is not completed.
+ *   Horizon  on submit time: every completed job of the pool submitted at or after since_ms is in the log, and a
+ *            record submitted before it is not kept.  A listing that starts before a handle's horizon is refused,
+ *            never answered partially.
+ *
+ * cook_state_completed_seed: replaces the log with rows [0, n), sets the horizon to since_ms and turns the log on (the
+ * start-up and leadership-change path: the pool's completed jobs submitted at or after now - retention, read once
+ * from one database value, its basis t as their stamp; the order is reset, load, seed, then resume the tap).
+ * COOK_E_BADARG, before any change: n < 0; a NULL array while n > 0; a row submitted before since_ms; a negative user
+ * or stamp; a kind outside COOK_CJ_*; a custom_executor outside {-1, 0, 1}; a submit pool code below -1; a job id
+ * listed twice.
+ * Uploads exactly 34 * n bytes, copied straight into the table (the executor as its byte).
+ * Statistics: cook_last_stats(COOK_PHASE_STATE).                                                                  */
+enum { COOK_CJ_SUCCESS = 1, COOK_CJ_FAILED = 2, COOK_CJ_REOPENED = 3 };
+int32_t cook_state_completed_seed(cook_pool* pool, int64_t since_ms, int32_t n, const int64_t* job_id,
+                                  const int64_t* stamp, const int32_t* user, const int64_t* submit_ms,
+                                  const int32_t* submit_pool, const int32_t* custom_executor, const uint8_t* kind);
+
+/* Appends the batch's records in order, skipping (on the host) those submitted before the horizon.  The append costs
+ * O(n), not O(log).  COOK_E_BADARG, before any change: the log is off; every row check of cook_state_completed_seed
+ * except the horizon; a job id twice in the batch.  COOK_E_TOO_LARGE: more than 2^31 - 1 rows.
+ * Uploads exactly 34 * (the rows kept) bytes.  Statistics: cook_last_stats(COOK_PHASE_STATE).                      */
+int32_t cook_state_completed_record(cook_pool* pool, int32_t n, const int64_t* job_id, const int64_t* stamp,
+                                    const int32_t* user, const int64_t* submit_ms, const int32_t* submit_pool,
+                                    const int32_t* custom_executor, const uint8_t* kind);
+
+/* Raises the horizon to since_ms and drops the rows submitted before it in one stable device compaction (into new
+ * columns of the same capacity, the old ones then freed).  The caller calls it periodically with now - retention.
+ * COOK_E_BADARG: the log is off; since_ms below the current horizon.
+ * Uploads nothing; downloads 4 bytes (the rows kept) when the log holds a row and since_ms is above the horizon, else
+ * nothing.  Statistics: cook_last_stats(COOK_PHASE_STATE).                                                       */
+int32_t cook_state_completed_advance(cook_pool* pool, int64_t since_ms);
+
+/* The listing over the union of the logs of pools[0, n_pools); the handles follow cook_state_user_stats' rules.
+ * state: COOK_LC_SUCCESS, COOK_LC_FAILED or COOK_LC_COMPLETED (both).
+ *   Records    those of `user` with job_id_lo <= job id < job_id_hi (the caller's d/entid-at of start - 1 h and
+ *              end + 1 h; user and job id never change over a job's life).  Each job is its latest record; a REOPENED
+ *              one drops it.
+ *   Selection  the kind matches `state`, and on the latest record: start_ms <= submit < end_ms
+ *              (job-submitted-in-range?), the pool check and the executor check of cook_state_list_jobs.
+ *   Order      ascending job id, the reference's entity-id traversal, cut to `limit` after the filters (its
+ *              `(take limit)`).
+ *   Outputs    entry e < *out_n: out_job_id, out_submit_ms, out_pool (the index in pools of the latest record).
+ * Changes nothing resident.
+ * COOK_E_BADARG, before any device work and with nothing written: cook_state_list_jobs' handle and argument cases
+ * (except `states`); state outside COOK_LC_*; a handle whose log is off; a handle whose horizon is > start_ms (the
+ * caller then keeps the Datomic path); a NULL output (out_stats may be NULL).
+ * COOK_E_TOO_LARGE: more than 2^31 - 1 records of `user` over the handles, with nothing written; more than cap
+ * entries, with only *out_n (the entries needed) written, so that the caller can retry with that capacity.
+ * No record of `user`: empty results without device work (statistics zero).
+ * Transfers exactly: up nothing; down 4 (the entry count), plus, unless COOK_E_TOO_LARGE, 20 * *out_n (job id,
+ * submit time, pool index).
+ * Statistics: out_stats (may be NULL), as cook_state_user_stats; no cook_last_stats slot is written.             */
+enum { COOK_LC_SUCCESS = 1, COOK_LC_FAILED = 2, COOK_LC_COMPLETED = 3 };
+int32_t cook_state_list_completed(cook_pool* const* pools, int32_t n_pools, int32_t user, int32_t state,
+                                  int64_t start_ms, int64_t end_ms, int64_t job_id_lo, int64_t job_id_hi,
+                                  int32_t pool_code, const int32_t* handle_pool, int32_t include_custom_executor,
+                                  int32_t limit, int32_t cap, int64_t* out_job_id, int64_t* out_submit_ms,
+                                  int32_t* out_pool, int32_t* out_n, cook_phase_stats* out_stats);
+
 /* ----------------------------------------------------------------- multi-GPU */
 /* §8e: after a pool's match round every rank contributes its pools' usage
  * deltas {count,cpus,mem,gpus} per user; one ncclAllGather over NVLink makes

@@ -417,6 +417,42 @@ JFN(jint, stateListJobs)(JNIEnv* env, jclass k, jlongArray pools, jlongArray tim
   (*env)->SetIntArrayRegion(env, out_n, 0, 2, g);
   return rc;
 }
+/* the completed-job log: cols the direct buffers of job_id, stamp, user, submit_ms, submit_pool, custom_executor
+ * (n ints: -1 nil, 0 false, 1 true), kind (n bytes) */
+JFN(jint, stateCompletedSeed)(JNIEnv* env, jclass k, jlong pool, jlong since_ms, jint n, jobjectArray cols) {
+  return cook_state_completed_seed((cook_pool*)(intptr_t)pool, since_ms, n, buf(env, cols, 0), buf(env, cols, 1),
+                                   buf(env, cols, 2), buf(env, cols, 3), buf(env, cols, 4), buf(env, cols, 5),
+                                   buf(env, cols, 6));
+}
+JFN(jint, stateCompletedRecord)(JNIEnv* env, jclass k, jlong pool, jint n, jobjectArray cols) {
+  return cook_state_completed_record((cook_pool*)(intptr_t)pool, n, buf(env, cols, 0), buf(env, cols, 1),
+                                     buf(env, cols, 2), buf(env, cols, 3), buf(env, cols, 4), buf(env, cols, 5),
+                                     buf(env, cols, 6));
+}
+JFN(jint, stateCompletedAdvance)(JNIEnv* env, jclass k, jlong pool, jlong since_ms) {
+  return cook_state_completed_advance((cook_pool*)(intptr_t)pool, since_ms);
+}
+/* the completed listing: times [start_ms, end_ms, job_id_lo, job_id_hi]; args [user, state, pool_code,
+ * include_custom_executor, limit, cap]; handle_pool n_pools ints (null with pool_code -1); outs the direct buffers of
+ * job_id, submit_ms, pool (cap longs / ints); out_n gets [n]; out_stats may be null */
+JFN(jint, stateListCompleted)(JNIEnv* env, jclass k, jlongArray pools, jlongArray times, jintArray args,
+                              jobject handle_pool, jobjectArray outs, jintArray out_n, jobject out_stats) {
+  jsize n = (*env)->GetArrayLength(env, pools);
+  if (n > 64) return COOK_E_BADARG;
+  jlong* h = (*env)->GetLongArrayElements(env, pools, NULL);
+  cook_pool* p[64];
+  for (jsize i = 0; i < n; i++) p[i] = (cook_pool*)(intptr_t)h[i];
+  (*env)->ReleaseLongArrayElements(env, pools, h, JNI_ABORT);
+  jlong t[4]; (*env)->GetLongArrayRegion(env, times, 0, 4, t);
+  jint a[6]; (*env)->GetIntArrayRegion(env, args, 0, 6, a);
+  int32_t got = 0;
+  jint rc = cook_state_list_completed(p, (int32_t)n, a[0], a[1], t[0], t[1], t[2], t[3], a[2], one(env, handle_pool),
+                                      a[3], a[4], a[5], buf(env, outs, 0), buf(env, outs, 1), buf(env, outs, 2), &got,
+                                      one(env, out_stats));
+  jint g = got;
+  (*env)->SetIntArrayRegion(env, out_n, 0, 1, &g);
+  return rc;
+}
 /* the history's seed: cols the direct buffers of task_id, user, start_ms, end_ms, cpus, mem, success, reason_code */
 JFN(jint, stateHistorySeed)(JNIEnv* env, jclass k, jlong pool, jlong since_ms, jint n, jobjectArray cols) {
   return cook_state_history_seed((cook_pool*)(intptr_t)pool, since_ms, n, buf(env, cols, 0), buf(env, cols, 1),

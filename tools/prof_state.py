@@ -72,6 +72,13 @@ against numpy over a host mirror, with the answers compared exactly:
   python tools/prof_state.py --list --pool c2 --reps 20
   python tools/prof_state.py --list --pool c5 --c5-pool 5 --reps 20
 
+--list-completed builds one handle's completed-job log of --completed-rows records over 32 days (Zipf users as in
+traces.py, reopens, second completions and records sent twice) and times cook_state_list_completed for the heaviest
+user and a light one, 24 h and 7 d windows, limits Integer/MAX_VALUE and 150, states completed and success, against
+numpy over a host mirror with the answers compared exactly; then one cook_state_completed_record of 1000 rows and one
+cook_state_completed_advance that drops a day:
+  python tools/prof_state.py --list-completed --reps 10
+
 --launch runs the same cycles on two resident handles instead of the host arm.  Each cycle's launches go to one
 handle through cook_state_launch (job ids, task ids, start times, the hosts the match chose) and to its twin through
 the equivalent cook_state_apply batch (the jobs' removal plus their task rows); the rest of the batch goes to both
@@ -1493,6 +1500,119 @@ def list_prof(a):
     e.close()
 
 
+def host_list_completed(m, user, state, start, end, lo, hi, limit):
+    """get-completed-jobs-by-user over the host mirror of one log: each job's latest record (stamp, then row), REOPENED
+    dropped, the state, window and id window on it, ascending job id cut to limit: [(job id, submit ms)]."""
+    sel = np.flatnonzero((m["user"] == user) & (m["jid"] >= lo) & (m["jid"] < hi))
+    o = sel[np.lexsort((-sel, -m["stamp"][sel], m["jid"][sel]))]
+    first = np.ones(len(o), bool)
+    first[1:] = m["jid"][o[1:]] != m["jid"][o[:-1]]
+    o = o[first]
+    k, s = m["kind"][o], m["submit"][o]
+    ok = (k != abi.CJ_REOPENED) & (s >= start) & (s < end)
+    if state != abi.LC_COMPLETED:
+        ok &= k == state
+    o = o[ok][:limit]
+    return list(zip(m["jid"][o].tolist(), m["submit"][o].tolist()))
+
+
+def list_completed_prof(a):
+    """cook_state_list_completed over a synthetic log of --completed-rows records over 32 days (Zipf users as in
+    traces.py; 5 % of the jobs reopened, most of those completed again; 2 % of the records sent twice), for the
+    heaviest user and a light one, 24 h and 7 d windows ending at the log's end, limits Integer/MAX_VALUE and 150,
+    states completed and success, against numpy over a host mirror; then one cook_state_completed_record of 1000 rows
+    and one cook_state_completed_advance that drops a day."""
+    rng = np.random.default_rng(a.seed)
+    t_end = 1_700_000_000_000
+    since = t_end - 32 * DAY_MS
+    J = int(a.completed_rows / 1.1)
+    submit = np.sort(rng.integers(since, t_end, J))
+    jid = np.arange(1, J + 1, dtype=np.int64)          # entity ids grow with submit time
+    user = traces._zipf_owner(rng, J, 1000)
+    spool = np.full(J, -1, np.int32)
+    cex = rng.choice(np.array([-1, 0, 1], np.int32), J, p=[0.1, 0.85, 0.05])
+    done = submit + rng.integers(1000, 2 * 3_600_000, J)
+    recs = [(np.arange(J), done, rng.choice(np.array([abi.CJ_SUCCESS, abi.CJ_FAILED], np.uint8), J, p=[0.7, 0.3]))]
+    ro = np.flatnonzero(rng.random(J) < 0.05)           # reopened
+    recs.append((ro, done[ro] + rng.integers(1, DAY_MS, len(ro)), np.full(len(ro), abi.CJ_REOPENED, np.uint8)))
+    rc = ro[rng.random(len(ro)) < 0.6]                 # completed again
+    recs.append((rc, done[rc] + DAY_MS + rng.integers(1, DAY_MS, len(rc)),
+                 rng.choice(np.array([abi.CJ_SUCCESS, abi.CJ_FAILED], np.uint8), len(rc))))
+    du = np.flatnonzero(rng.random(J) < 0.02)           # the first record sent twice
+    recs.append((du, done[du], recs[0][2][du]))
+    e = GpuEngine(pool_name="list-completed")
+    e.state_completed_seed(since)
+    m = {k: [] for k in ("jid", "stamp", "user", "submit", "kind", "cex")}
+    for idx, stamp, kind in recs:   # one batch per occurrence (a job at most once per batch), in stamp order
+        o = np.argsort(stamp, kind="stable")
+        idx, stamp, kind = idx[o], stamp[o], kind[o]
+        for c0 in range(0, len(idx), 1 << 21):
+            s = slice(c0, c0 + (1 << 21))
+            i = idx[s]
+            e.state_completed_record(jid[i], stamp[s], user[i], submit[i], spool[i], cex[i], kind[s])
+            for k, v in (("jid", jid[i]), ("stamp", stamp[s]), ("user", user[i]), ("submit", submit[i]),
+                         ("kind", kind[s]), ("cex", cex[i])):
+                m[k].append(v)
+    m = {k: np.concatenate(v) for k, v in m.items()}
+    counts = np.bincount(m["user"])
+    heavy = int(np.argmax(counts))
+    light = int(np.flatnonzero(counts == np.sort(counts[counts > 0])[len(counts[counts > 0]) // 10])[0])
+    print(json.dumps({"card": card(), "records": len(m["jid"]), "jobs": J, "days": 32, "heavy_user_records":
+                      int(counts[heavy]), "light_user_records": int(counts[light])}), flush=True)
+    hour = 3_600_000
+    for who, u in (("heavy", heavy), ("light", light)):
+        for wname, w in (("24h", DAY_MS), ("7d", 7 * DAY_MS)):
+            start, end = t_end - w, t_end
+            lo, hi = int(jid[np.searchsorted(submit, start - hour)]), J + 1
+            for state, sname in ((abi.LC_COMPLETED, "completed"), (abi.LC_SUCCESS, "success")):
+                for limit in ((1 << 31) - 1, 150):
+                    dev, wall, host, same = [], [], [], True
+                    for rep in range(a.reps + 2):
+                        w0 = time.perf_counter()
+                        got = engine.state_list_completed([e], u, state, start, end, lo, hi, limit=limit,
+                                                          cap=int(counts[u]) + 1)
+                        wl = time.perf_counter() - w0
+                        if rep < 2:   # the first calls carve and load the kernels
+                            continue
+                        st = got["stats"]
+                        dev.append(st["ms_h2d"] + st["ms_device"] + st["ms_d2h"])
+                        wall.append(wl)
+                        if rep < 5:
+                            w0 = time.perf_counter()
+                            want = host_list_completed(m, u, state, start, end, lo, hi, limit)
+                            host.append(time.perf_counter() - w0)
+                            same = same and list(zip(got["job_id"].tolist(), got["submit_ms"].tolist())) == want
+                    print(json.dumps({"user": who, "window": wname, "state": sname, "limit": limit,
+                                      "entries": len(got["job_id"]), "device_ms": round(float(np.median(dev)), 4),
+                                      "wall_ms": round(1e3 * float(np.median(wall)), 4), "h2d_bytes": st["h2d_bytes"],
+                                      "d2h_bytes": st["d2h_bytes"], "n_launches": st["n_launches"],
+                                      "numpy_ms": round(1e3 * float(np.median(host)), 4), "identical": bool(same)}),
+                          flush=True)
+    # one record of 1000 new completions, and one advance that drops a day
+    res = []
+    for rep in range(a.reps + 1):
+        n0 = J + 1 + 1000 * rep
+        nj = np.arange(n0, n0 + 1000, dtype=np.int64)
+        w0 = time.perf_counter()
+        e.state_completed_record(nj, np.full(1000, t_end + rep, np.int64), user[:1000], np.full(1000, t_end, np.int64),
+                                 spool[:1000], cex[:1000], np.full(1000, abi.CJ_SUCCESS, np.uint8))
+        wl = time.perf_counter() - w0
+        st = e.last_stats(abi.PHASE_STATE)
+        if rep:
+            res.append((st["ms_h2d"] + st["ms_device"], 1e3 * wl, st["h2d_bytes"]))
+    print(json.dumps({"call": "record", "batch": 1000, "log_rows": len(m["jid"]) + 1000 * a.reps,
+                      "device_ms": round(float(np.median([x[0] for x in res])), 4),
+                      "wall_ms": round(float(np.median([x[1] for x in res])), 4), "h2d_bytes": res[-1][2]}), flush=True)
+    w0 = time.perf_counter()
+    e.state_completed_advance(since + DAY_MS)
+    wl = time.perf_counter() - w0
+    st = e.last_stats(abi.PHASE_STATE)
+    print(json.dumps({"call": "advance", "dropped_day": True, "device_ms": round(st["ms_device"], 4),
+                      "wall_ms": round(1e3 * wl, 4), "d2h_bytes": st["d2h_bytes"], "n_launches": st["n_launches"]}),
+          flush=True)
+    e.close()
+
+
 def requeued_soa(store, rows, host):
     """The host path cook_state_status replaces: the pending rows of failed jobs rebuilt from the host mirror with
     reserved_host -1 and the failed host appended to the novel-host list (unless -1 or already listed)."""
@@ -1646,9 +1766,14 @@ def main():
     ap.add_argument("--status-batch", type=int, default=1000, help="--status: the launches and failures per rep")
     ap.add_argument("--list", action="store_true",
                     help="cook_state_list_jobs against numpy over a host mirror (C2 or --pool c5)")
+    ap.add_argument("--list-completed", action="store_true",
+                    help="cook_state_list_completed over a synthetic log against numpy over a host mirror")
+    ap.add_argument("--completed-rows", type=int, default=10_000_000, help="--list-completed: the log's records")
     ap.add_argument("--match-metrics", action="store_true",
                     help="cook_state_match_metrics after each match against numpy over a host mirror (C2 or --pool c5)")
     a = ap.parse_args()
+    if a.list_completed:
+        return list_completed_prof(a)
     if a.list:
         return list_prof(a)
     if a.status:
