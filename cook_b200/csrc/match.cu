@@ -33,6 +33,7 @@
 #include <numeric>
 
 #include "constraints.cuh"
+#include "fitness.cuh"
 #include "fold.cuh"
 #include "sort.cuh"
 
@@ -49,8 +50,9 @@ struct __align__(32) VmStatic { double lc, lm, rc, rm; };
 // Dynamic record: cpus/mem assigned this cycle + the (static) correctly rounded
 // reciprocals of the fitness denominators, yc = RN(1/(lc+rc)), ym = RN(1/(lm+rm)):
 // x/den is then q0 = x*y, q = fma(fma(-den, q0, x), y, q0) == RN(x/den) (Markstein's
-// correction; checked against IEEE division in tests/test_fastdiv.py); y == 0 marks
-// denominators outside the safe range (true division is used for those).
+// correction, fitness.cuh; checked against exact division in tests/test_fitness_division.py);
+// y == 0 marks denominators outside the safe range and cycles the dividend guard flags
+// (true division is used for those).
 struct __align__(32) VmDyn { double ac, am, yc, ym; };
 struct __align__(8) VmCnt { int an, pu; };  // tasks assigned this cycle, ports used (constraint kernel)
 
@@ -335,39 +337,6 @@ __device__ __forceinline__ int first_failing_group(const MatchArgs& a, int j, in
 // against the live group state: every member placed so far
 __device__ bool group_pass(const MatchArgs& a, const JobRegs& r, int v) {
   return first_failing_group(a, r.j, v, [&](int g) { return __ldcg(a.gr.gp_n + g); }) < 0;
-}
-
-// x / den with y = RN(1 / den) (or 0 => plain division): three dependent f64 ops
-// instead of the ~10 of div.rn.f64, same correctly rounded result.
-__device__ __forceinline__ double div_y(double x, double den, double y) {
-  if (y == 0.0) return x / den;
-  const double q0 = x * y;
-  return fma(fma(-den, q0, x), y, q0);
-}
-// (y = 0 selects the IEEE division in div_y.)  The Markstein correction is proven for a faithful q0 and a
-// denominator whose significand is not all ones; such denominators take the plain division as well.
-__device__ __forceinline__ double safe_rcp(double den) {
-  const unsigned long long frac = (unsigned long long)__double_as_longlong(den) & 0x000fffffffffffffULL;
-  return (den > 1e-100 && den < 1e100 && frac != 0x000fffffffffffffULL) ? 1.0 / den : 0.0;
-}
-
-// FENZO 3a + 4 (see oracle): resource fit then cpuMemBinPacker fitness.
-// The usual case (both reciprocals usable) takes no branch between the two divisions, so their
-// dependent chains interleave: on the commit chain that is one 7-op f64 path instead of two 5-op ones
-// each fenced by a branch to the IEEE division.  Same operations, same results.
-__device__ __forceinline__ double fit_fitness(double jc, double jm, const VmState& st) {
-  const bool no = (st.ac + jc > st.lc) | (st.am + jm > st.lm);
-  double cpu_fit, mem_fit;
-  if (st.yc != 0.0 && st.ym != 0.0) {
-    const double xc = (jc + st.ac) + st.rc, xm = (jm + st.am) + st.rm;
-    const double qc = xc * st.yc, qm = xm * st.ym;
-    cpu_fit = fma(fma(-(st.lc + st.rc), qc, xc), st.yc, qc);
-    mem_fit = fma(fma(-(st.lm + st.rm), qm, xm), st.ym, qm);
-  } else {
-    cpu_fit = div_y((jc + st.ac) + st.rc, st.lc + st.rc, st.yc);
-    mem_fit = div_y((jm + st.am) + st.rm, st.lm + st.rm, st.ym);
-  }
-  return no ? 0.0 : (cpu_fit + mem_fit) * 0.5;
 }
 
 // Full evaluation of (job, VM v) against an explicit VM state.
@@ -1358,7 +1327,9 @@ __device__ __forceinline__ double warp_argmax_fast(double f, int v, int& wv, int
   const unsigned hi = (unsigned)__double2hiint(f);
   const unsigned mh = __reduce_max_sync(0xffffffffu, hi);
   unsigned cand = __ballot_sync(0xffffffffu, hi == mh);
-  if (mh == 0u) { wv = 0x7fffffff; wl = 0; return 0.0; }  // f in (0, 1] has a non-zero high word
+  if (mh == 0u) {   // every f is 0 or below 2^-1054 (a subnormal fitness): the low words decide
+    if (__reduce_max_sync(0xffffffffu, (unsigned)__double2loint(f)) == 0u) { wv = 0x7fffffff; wl = 0; return 0.0; }
+  }
   if (__popc(cand) > 1) {
     const unsigned lo = hi == mh ? (unsigned)__double2loint(f) : 0u;
     const unsigned ml = __reduce_max_sync(0xffffffffu, lo);
@@ -2041,10 +2012,13 @@ __global__ void __launch_bounds__(128) cons_user_kernel(ConsArgs a, const int32_
 // The considerable set and its per-k hot columns, slot by slot.
 struct ConsOut {
   int32_t* cons; double *kc, *km, *kg; int32_t* kports; uint8_t* kflags;
+  int* fit_guard_bits;   // the cycle's dividend guard (fitness.cuh), requests' share
   __device__ void put(const JobDev& jb, int j, int slot) const {
     cons[slot] = j;
-    kc[slot] = jb.cpus[j];
-    km[slot] = jb.mem[j];
+    const double c = jb.cpus[j], m = jb.mem[j];
+    kc[slot] = c;
+    km[slot] = m;
+    if (const int g = fit_guard(c, m)) atomicOr(fit_guard_bits, g);
     kg[slot] = jb.gpus ? jb.gpus[j] : 0.0;
     kports[slot] = jb.ports ? jb.ports[j] : 0;
     uint8_t fl = 0;
@@ -2139,8 +2113,9 @@ cudaError_t cons_pass(const ConsArgs& ca, int J, int32_t* pos, int32_t* tmp, int
 }
 
 // ------------------------------------------------------------------ setup
+// the offers' hot columns in rank space, and their share of the cycle's dividend guard (fitness.cuh)
 __global__ void gather_offers_kernel(const int32_t* perm, int O, const double* c, const double* m,
-                                     const double* rc, const double* rm, VmStatic* vs) {
+                                     const double* rc, const double* rm, VmStatic* vs, int* guard) {
   int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= O) return;
   int o = perm[v];
@@ -2148,6 +2123,7 @@ __global__ void gather_offers_kernel(const int32_t* perm, int O, const double* c
   x.lc = c[o]; x.lm = m[o];
   x.rc = rc ? rc[o] : 0.0; x.rm = rm ? rm[o] : 0.0;
   vs[v] = x;
+  if (const int g = fit_guard(x.lc, x.lm) | fit_guard(x.rc, x.rm)) atomicOr(guard, g);
 }
 
 // suffix minima of the considerable jobs' requests: block-local reverse scans, then every
@@ -2209,15 +2185,17 @@ __global__ void gather_cons_kernel(OfferDev of, VmCons* vc, int32_t* attr_v) {
 }
 
 // per-cycle reset of the dynamic state (both buffers) + the reciprocals of the fitness
-// denominators (static for the cycle)
-__global__ void init_dyn_kernel(const VmStatic* vs, int O, VmDyn* d0, VmDyn* d1, VmCnt* n0, VmCnt* n1) {
+// denominators (static for the cycle; 0 for a resource the cycle's dividend guard flags)
+__global__ void init_dyn_kernel(const VmStatic* vs, int O, const int* guard, VmDyn* d0, VmDyn* d1, VmCnt* n0,
+                                VmCnt* n1) {
   int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= O) return;
   const VmStatic x = vs[v];
+  const int g = *guard;
   VmDyn d;
   d.ac = 0.0; d.am = 0.0;
-  d.yc = safe_rcp(x.lc + x.rc);
-  d.ym = safe_rcp(x.lm + x.rm);
+  d.yc = (g & FIT_IEEE_CPU) ? 0.0 : safe_rcp(x.lc + x.rc);
+  d.ym = (g & FIT_IEEE_MEM) ? 0.0 : safe_rcp(x.lm + x.rm);
   d0[v] = d; d1[v] = d;
   VmCnt c;
   c.an = 0; c.pu = 0;
@@ -2754,11 +2732,10 @@ int32_t match_run(cook_pool* pool, int32_t* out_considerable, int64_t* out_job_i
 
   // ---- M0 considerable
   const int TB = 256;
+  int* fit_guard_bits = mp->d_counters + 11;   // zeroed above; the offers and the considerable requests set it
   if (O > 0) {
     gather_offers_kernel<<<(O + TB - 1) / TB, TB, 0, st>>>(mp->d_perm, O, mp->d_oc, mp->d_om, mp->d_orc,
-                                                           mp->d_orm, mp->d_vs);
-    launches++;
-    init_dyn_kernel<<<(O + TB - 1) / TB, TB, 0, st>>>(mp->d_vs, O, ma.dyn.d[0], ma.dyn.d[1], ma.dyn.n[0], ma.dyn.n[1]);
+                                                           mp->d_orm, mp->d_vs, fit_guard_bits);
     launches++;
     if (mp->d_ports_total) {
       ports_total_kernel<<<(O + TB - 1) / TB, TB, 0, st>>>(ma.of.port_off, ma.of.port_begin,
@@ -2770,9 +2747,14 @@ int32_t match_run(cook_pool* pool, int32_t* out_considerable, int64_t* out_job_i
       launches++;
     }
   }
-  const ConsOut cons_out{mp->d_cons, mp->d_kc, mp->d_km, mp->d_kg, mp->d_kports, mp->d_kflags};
+  const ConsOut cons_out{mp->d_cons, mp->d_kc, mp->d_km, mp->d_kg, mp->d_kports, mp->d_kflags, fit_guard_bits};
   CK(pool, cons_pass(ca, mp->J, mp->d_pos, mp->d_tmp, mp->d_seg_s, mp->d_seg_e, mp->d_keep, mp->d_gf, cons_out,
                      mp->d_counters, st, &launches));
+  if (O > 0) {   // after both shares of the dividend guard
+    init_dyn_kernel<<<(O + TB - 1) / TB, TB, 0, st>>>(mp->d_vs, O, fit_guard_bits, ma.dyn.d[0], ma.dyn.d[1],
+                                                      ma.dyn.n[0], ma.dyn.n[1]);
+    launches++;
+  }
   int32_t n_cons = 0;
   int64_t d2h = 0;
   CK(pool, download(&n_cons, mp->d_counters, 1, st, &d2h));

@@ -1008,7 +1008,9 @@ extern "C" int32_t oracle_rebalance_trace(int32_t dru_mode, const cook_running_s
 // (cook_b200/csrc/match.cu div_y).  This counts the inputs for which that differs
 // from the IEEE quotient x/den the reference computes (clojure `/` on doubles,
 // via Fenzo's cpuMemBinPacker) over three families: Cook's value grids, random
-// doubles, and denominators with (nearly) all-ones significands.
+// doubles, and denominators with (nearly) all-ones significands.  oracle_check_fastdiv_guard
+// covers the dividend guard (fitness.cuh fit_guard): dividends at the edges of what a guarded cycle
+// can divide, [2^-600, 2^602), against every denominator safe_rcp accepts, and below the guard.
 #include <cmath>
 static inline double fastdiv_q(double x, double den, double y) {
   const double q0 = x * y;
@@ -1047,6 +1049,51 @@ extern "C" int64_t oracle_check_fastdiv(int64_t n_random, uint64_t seed) {
     memcpy(&b, &bits, 8);
     const double x = rd(-5, 25);
     if (fastdiv_q(x, b, 1.0 / b) != x / b) bad++;
+  }
+  return bad;
+}
+
+// family 0: dividends guarded amounts can give -- 0, the least binades from 2^-600 up, the largest below
+//   2^602 -- by denominators across (1e-100, 1e100), with the bottom and top binades of each drawn often, so
+//   that the quotients reach down to 2^-933 and up to 2^934: every one must equal IEEE division.
+// family 1: dividends below the guard (subnormal, and normal up to 2^-960), by denominators across the range:
+//   the mismatches this counts are why the guard exists.
+extern "C" int64_t oracle_check_fastdiv_guard(int64_t n, uint64_t seed, int family) {
+  int64_t bad = 0;
+  uint64_t s = seed ? seed : 88172645463325252ull;
+  auto rnd = [&]() { s ^= s << 13; s ^= s >> 7; s ^= s << 17; return s; };
+  auto rd = [&](int emin, int emax) {   // normal double, exponent uniform in [emin, emax]
+    const uint64_t m = rnd() & ((1ull << 52) - 1);
+    const int e = emin + (int)(rnd() % (uint64_t)(emax - emin + 1));
+    const uint64_t bits = ((uint64_t)(e + 1023) << 52) | m;
+    double d;
+    memcpy(&d, &bits, 8);
+    return d;
+  };
+  auto safe = [](double den) {          // fitness.cuh safe_rcp
+    uint64_t bits;
+    memcpy(&bits, &den, 8);
+    const uint64_t frac = bits & 0x000fffffffffffffULL;
+    return (den > 1e-100 && den < 1e100 && frac != 0x000fffffffffffffULL) ? 1.0 / den : 0.0;
+  };
+  for (int64_t i = 0; i < n; i++) {
+    double x;
+    const uint64_t pick = rnd() % 8;
+    if (family == 0) {
+      x = pick == 0 ? 0.0 : pick < 4 ? rd(-600, -590) : pick < 7 ? rd(590, 601) : rd(-600, 601);
+    } else {
+      if (pick < 4) {
+        const uint64_t bits = 1 + rnd() % ((1ull << 52) - 1);   // subnormal
+        memcpy(&x, &bits, 8);
+      } else {
+        x = rd(-1022, -960);
+      }
+    }
+    const uint64_t dp = rnd() % 4;
+    const double den = dp == 0 ? rd(-333, -320) : dp == 1 ? rd(320, 332) : rd(-333, 332);
+    const double y = safe(den);
+    if (y == 0.0) continue;
+    if (fastdiv_q(x, den, y) != x / den) bad++;
   }
   return bad;
 }

@@ -1,11 +1,13 @@
 // fold_probe.cu — test-only harness: drives each primitive of cook_b200/csrc/fold.cuh, the comparator
-// sort of sort.cuh and the merge comparator LessMerge with host inputs.
+// sort of sort.cuh, the merge comparator LessMerge and the matcher's fitness arithmetic (fitness.cuh) with
+// host inputs.
 //
 // Built by __graft_entry__.build() into tests/libfoldprobe.so with the product's nvcc flags and loaded by
-// tests/test_fold_primitives.py and tests/test_merge_primitives.py.  Every entry point copies its host
+// tests/test_fold_primitives.py, tests/test_merge_primitives.py and tests/test_fitness_division.py.  Every entry point copies its host
 // inputs to the device, runs the primitive exactly as the product kernels do, copies the outputs back and
 // returns a cudaError_t (0 = success).  Device buffers are sized from the host arguments, so no call
 // reads or writes past them.
+#include "../cook_b200/csrc/fitness.cuh"
 #include "../cook_b200/csrc/fold.cuh"
 #include "../cook_b200/csrc/sort.cuh"
 
@@ -231,6 +233,31 @@ __global__ void less_matrix_kernel(LessMerge less, int n, uint8_t* out) {
   if (k < (long long)n * n) out[k] = less((int)(k / n), (int)(k % n)) ? 1 : 0;
 }
 
+// ---- the fitness division and the fitness, one element per thread
+__global__ void div_kernel(const double* x, const double* den, int n, double* out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = div_y(x[i], den[i], safe_rcp(den[i]));
+}
+
+// element i is one (job, VM) pair: a cycle of its own, whose assigned amounts count as requests, with the
+// reciprocals set as init_dyn_kernel sets them
+__global__ void fitness_kernel(const double* const* col, int n, double* out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  FitState st;
+  st.ac = col[2][i]; st.am = col[3][i]; st.lc = col[4][i]; st.lm = col[5][i]; st.rc = col[6][i]; st.rm = col[7][i];
+  const double jc = col[0][i], jm = col[1][i];
+  const int g = fit_guard(jc, jm) | fit_guard(st.ac, st.am) | fit_guard(st.lc, st.lm) | fit_guard(st.rc, st.rm);
+  st.yc = (g & FIT_IEEE_CPU) ? 0.0 : safe_rcp(st.lc + st.rc);
+  st.ym = (g & FIT_IEEE_MEM) ? 0.0 : safe_rcp(st.lm + st.rm);
+  out[i] = fit_fitness(jc, jm, st);
+}
+
+__global__ void guard_kernel(const double* c, const double* m, int n, int* out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = fit_guard(c[i], m[i]);
+}
+
 }  // namespace
 
 extern "C" {
@@ -432,6 +459,48 @@ int fp_less_merge(const double* dru, const int* user_at, const int* seg_start, c
     b.err = csort::sort_indices(d_idx, d_tmp, n, lm, 0, &launches);
     b.download(order, d_idx, n);
   }
+  return b.finish();
+}
+
+// div_y(x, den, safe_rcp(den)) over n pairs
+int fp_div(const double* x, const double* den, int n, double* out) {
+  if (n < 1) return (int)cudaErrorInvalidValue;
+  Bufs b;
+  const double* d_x = b.upload(x, n);
+  const double* d_den = b.upload(den, n);
+  double* d_out = b.alloc<double>(n);
+  if (b.err != cudaSuccess) return b.err;
+  div_kernel<<<(n + 255) / 256, 256>>>(d_x, d_den, n, d_out);
+  b.download(out, d_out, n);
+  return b.finish();
+}
+
+// fit_guard(c[i], m[i]): bit 0 (1) when the cpu (mem) amount sends its resource to IEEE division
+int fp_fit_guard(const double* c, const double* m, int n, int* out) {
+  if (n < 1) return (int)cudaErrorInvalidValue;
+  Bufs b;
+  const double* d_c = b.upload(c, n);
+  const double* d_m = b.upload(m, n);
+  int* d_out = b.alloc<int>(n);
+  if (b.err != cudaSuccess) return b.err;
+  guard_kernel<<<(n + 255) / 256, 256>>>(d_c, d_m, n, d_out);
+  b.download(out, d_out, n);
+  return b.finish();
+}
+
+// fit_fitness of request (jc, jm) on a VM with assigned (ac, am), lease (lc, lm) and running (rc, rm), n pairs
+int fp_fitness(const double* jc, const double* jm, const double* ac, const double* am, const double* lc,
+               const double* lm, const double* rc, const double* rm, int n, double* out) {
+  if (n < 1) return (int)cudaErrorInvalidValue;
+  Bufs b;
+  const double* h[8] = {jc, jm, ac, am, lc, lm, rc, rm};
+  const double* d[8];
+  for (int k = 0; k < 8; k++) d[k] = b.upload(h[k], n);
+  const double* const* d_col = b.upload(d, 8);
+  double* d_out = b.alloc<double>(n);
+  if (b.err != cudaSuccess) return b.err;
+  fitness_kernel<<<(n + 255) / 256, 256>>>(d_col, n, d_out);
+  b.download(out, d_out, n);
   return b.finish();
 }
 

@@ -1,6 +1,7 @@
 """Matcher inputs that reach the rare decisions of match_kernel in cook_b200/csrc/match.cu: equal-fitness ties,
 fitnesses one ulp apart, exact fits, supply confined to one or two chunks, crowded commit turns, group conflicts,
-the pipeline's size edges (catalogue()) and the commit hand-off at every turn residue (handoff_catalogue()).
+the pipeline's size edges, the fitness division's IEEE branch (catalogue()) and the commit hand-off at every turn
+residue (handoff_catalogue()).
 Test infrastructure only: no GPU code is imported here.
 
 Every builder returns a dict:
@@ -19,7 +20,8 @@ without changing any answer.
 """
 import numpy as np
 
-from cook_b200 import abi
+import fitness_ref as R
+from cook_b200 import abi, traces
 
 ORDERS = ("perm", "rev")
 TOPK = 8            # candidates per (job, chunk) in a row (match.cu)
@@ -510,6 +512,109 @@ def long_queues():
             "thin": lambda od, ck: thinned(od, ck)}
 
 
+# ---- 9. the fitness division --------------------------------------------------------------------------------
+# fit_fitness divides through reciprocals set once per VM and cycle (cook_b200/csrc/fitness.cuh); a VM whose
+# denominator safe_rcp rejects, and every VM of a cycle with an amount off the guarded range, divides with IEEE
+# division instead.
+def tiny_partner():
+    """(request, lease A, lease B): a job asking for `request` cpus and mem (subnormal) on VMs with cpu lease A or B,
+    mem lease 1 and nothing running fits B better under IEEE division, while the reciprocal shortcut rounds A's
+    cpu fit up to B's or past it."""
+    for K in range(3, 40):
+        j = K * R.TINY
+        seen = {}
+        for i in range(1, 256):
+            lc = 1.0 + i / 256
+            key = (R.fitness(j, j, 0, 0, lc, 1.0, 0, 0), R.shortcut_fitness(j, j, 0, 0, lc, 1.0, 0, 0))
+            seen.setdefault(key, lc)
+        for (fa, sa), la in seen.items():
+            for (fb, sb), lb in seen.items():
+                if 0 < fa < fb and sa >= sb:
+                    return j, la, lb
+    raise AssertionError("no pair of leases the shortcut orders differently")
+
+
+def tiny_flip(order, constr, P=3, J=3):
+    """P VMs A and P VMs B (tiny_partner), every A named below every B, and J jobs with the subnormal request.
+    IEEE division puts every job on the best-named B (a touched B only gets better); the shortcut would tie the
+    two kinds or prefer A, and the lowest name would then take them all to an A."""
+    O = 2 * P
+    j, la, lb = tiny_partner()
+    rank = ranks(O, order)
+    isb = rank >= P
+    br = by_rank(rank)
+    claims = dict(kind="tiny_flip", want=[int(br[P])] * J, shortcut_want=int(br[0]), request=j, leases=(la, lb),
+                  b_vms=[int(v) for v in np.flatnonzero(isb)])
+    return make(np.full(J, j), np.full(J, j), np.where(isb, lb, la), np.ones(O), np.zeros(O), np.zeros(O), order,
+                constr, claims, fails=[0, J - 1], rank=rank)
+
+
+# The IEEE-branch VM X of each reason safe_rcp returns 0 (its denominator lc + rc) and the job: (lc, lm, rc, rm),
+# (cpus, mem).  The fast-path VM F has cpu lease F_LC, nothing running in cpus, and mem lease F_LM with its running
+# mem tuned (rm_tuned) so that F fits the job one ulp above or below X.
+RCP_REASONS = {
+    "lo": ((1e-100, 4096.0, 0.0, 1024.0), (2.5e-101, 1024.0), 4e-100),      # den <= 1e-100
+    "hi": ((1e100, 4096.0, 0.0, 1024.0), (1.0, 1024.0), 64.0),              # den >= 1e100
+    "ones": ((float.fromhex("0x1.fffffffffffffp1"), 4096.0, 0.0, 1024.0), (1.0, 1024.0), 64.0),   # all-ones significand
+}
+F_LM = 4096.0
+
+
+def rm_tuned(job, lc, target):
+    """The running mem of a VM (lc, F_LM, 0, rm) on which `job` fits with fitness `target` bit for bit: the
+    fitness is monotone in rm, so a bisection over the bits of rm finds the first rm that reaches it."""
+    f = lambda rm: R.fitness(job[0], job[1], 0.0, 0.0, lc, F_LM, 0.0, rm)
+    lo, hi = int(np.float64(1.0).view(np.int64)), int(np.float64(2.0 ** 20).view(np.int64))
+    assert f(1.0) < target < f(2.0 ** 20)
+    while hi - lo > 1:
+        mid = (lo + hi) // 2
+        lo, hi = (mid, hi) if f(float(np.int64(mid).view(np.float64))) < target else (lo, mid)
+    rm = float(np.int64(hi).view(np.float64))
+    assert f(rm) == target, "the fitness steps over the target"
+    return rm
+
+
+def ieee_branch(reason, outcome, order, constr, P=2, J=10):
+    """P VMs X whose denominator safe_rcp rejects (`reason`) and P VMs F on the fast path that fit the job one ulp
+    worse (`outcome` "win": X wins) or one ulp better ("lose"); the better kind is named above the other.  Each VM
+    takes four jobs (mem), so the jobs fill the better kind in name order and then the other, and the evaluators
+    and the resolver both score VMs of each kind."""
+    O = 2 * P
+    x_vm, job, f_lc = RCP_REASONS[reason]
+    fx = R.fitness(job[0], job[1], 0.0, 0.0, *x_vm[:2], *x_vm[2:])
+    ft = float(np.nextafter(fx, -np.inf if outcome == "win" else np.inf))
+    rm_f = rm_tuned(job, f_lc, ft)
+    rank = ranks(O, order)
+    top = rank >= P                       # the better kind
+    isx = ~top if outcome == "lose" else top
+    lc = np.where(isx, x_vm[0], f_lc)
+    lm = np.where(isx, x_vm[1], F_LM)
+    rc = np.where(isx, x_vm[2], 0.0)
+    rm = np.where(isx, x_vm[3], rm_f)
+    br = by_rank(rank)
+    claims = dict(kind="ieee_branch", reason=reason, outcome=outcome, fx=fx, ff=ft, first=int(br[P]),
+                  x_vms=[int(v) for v in np.flatnonzero(isx)])
+    return make(np.full(J, job[0]), np.full(J, job[1]), lc, lm, rc, rm, order, constr, claims, fails=[0, J - 1],
+                rank=rank)
+
+
+GUARD_MIN = 2.0 ** -600   # the least nonzero amount of a cycle that keeps the reciprocal shortcut (fitness.cuh)
+
+
+def ieee_cycle(order, constr, J=2000, O=400):
+    """A C2-shaped pool (traces.gen_c2: cpu and mem requests and leases of Cook's sizes, running usage on the
+    offers) whose job J / 2 asks for a subnormal number of cpus: one amount below GUARD_MIN switches every VM of
+    the cycle to IEEE division, through many blocks of either kernel."""
+    t = traces.gen_c2(seed=17, n_jobs=J, n_offers=O, n_users=20, n_running=2 * O)
+    jobs, offers = t["jobs"], t["offers"]
+    c = jobs.col("cpus").astype(np.float64).copy()
+    c[J // 2] = 3 * R.TINY
+    claims = dict(kind="ieee_cycle", tiny=J // 2)
+    return make(c, jobs.col("mem"), *(offers.col(k) for k in ("cpus", "mem", "run_cpus", "run_mem")), order, constr,
+                claims, fails=[0, J // 2, J - 1])
+
+
+
 # ---- the catalogue ------------------------------------------------------------------------------------------
 def catalogue():
     """{name: builder(order)} of every case, both kernels where the case applies to both."""
@@ -544,6 +649,12 @@ def catalogue():
             out[f"7-sparse-{kn}-{live}"] = lambda od, live=live, ck=ck: sparse_edge(live, od, ck)
         for O in (SMEM_STATIC_O, SMEM_STATIC_O + 1, LATEST_O[ck], LATEST_O[ck] + 1):
             out[f"7-smem-{kn}-O{O}"] = lambda od, O=O, ck=ck: threshold(O, od, ck)
+        out[f"9-tiny-{kn}"] = lambda od, ck=ck: tiny_flip(od, ck)
+        for reason in RCP_REASONS:
+            for outcome in ("win", "lose"):
+                out[f"9-rcp-{reason}-{outcome}-{kn}"] = \
+                    lambda od, reason=reason, outcome=outcome, ck=ck: ieee_branch(reason, outcome, od, ck)
+        out[f"9-cycle-{kn}"] = lambda od, ck=ck: ieee_cycle(od, ck)
     out["6-groups"] = lambda od: group_conflicts(od)
     for O in (SBW_O, SBW_O + 1):
         out[f"7-sbw-C-O{O}"] = lambda od, O=O: sbw_edge(O, od)

@@ -1,7 +1,7 @@
 """The matcher's rare decisions against the oracle: equal-fitness ties at chunk and tile edges, fitnesses one
 ulp apart, exact fits on and off the grid (cpus, mem, ports), supply confined to one or two chunks, crowded
-commit turns under the pipeline's knobs, group conflicts, and the block, sparse-mode and shared-memory size
-edges.  The cases are built in match_edge_cases.py.
+commit turns under the pipeline's knobs, group conflicts, the block, sparse-mode and shared-memory size edges,
+and the fitness division's IEEE branch.  The cases are built in match_edge_cases.py.
 
 Without a GPU: every case's inputs are valid and the oracle's answer shows what the case claims; the oracle
 also equals a plain restatement of the greedy match (match_edge_cases.greedy) on every case without groups.
@@ -16,6 +16,7 @@ import re
 import numpy as np
 import pytest
 
+import fitness_ref as R
 import match_edge_cases as E
 from cook_b200 import abi, traces
 
@@ -78,7 +79,7 @@ def test_catalogue():
             assert c["nc"] == J and all(k.startswith("COOK_") or k == "max_ctas" for kn in c["knobs"] for k in kn)
             fam.setdefault(name[0], set()).add(c["constr"])
     assert fam == {"1": {False, True}, "2": {False, True}, "3": {False, True}, "4": {False, True},
-                   "5": {False, True}, "6": {True}, "7": {False, True}}
+                   "5": {False, True}, "6": {True}, "7": {False, True}, "9": {False, True}}
     assert E.ranks(33, "perm").tolist() != E.ranks(33, "rev").tolist()
 
 
@@ -330,6 +331,64 @@ def test_winner_ties_with_the_bound(oracle, side, constr):
         assert f.max() == cl["f_t"] and t in tied and len(tied) >= 2
         assert a[i + 2] == tied[np.argmin(rank[tied])]
         assert (a[i + 2] == t) == (side == "low")
+
+
+@pytest.mark.parametrize("order", E.ORDERS)
+def test_tiny_request_decided_by_the_division(oracle, order):
+    """A subnormal request: IEEE division puts it on a B, and the reciprocal shortcut, were the cycle left on it,
+    would tie an A with the B or prefer the A, and the A's name is lower."""
+    c = E.tiny_flip(order, False)
+    cl = c["claims"]
+    j, (la, lb) = cl["request"], cl["leases"]
+    assert 0 < j < E.GUARD_MIN
+    assert 0 < R.fitness(j, j, 0, 0, la, 1.0, 0, 0) < R.fitness(j, j, 0, 0, lb, 1.0, 0, 0)
+    assert R.shortcut_fitness(j, j, 0, 0, la, 1.0, 0, 0) >= R.shortcut_fitness(j, j, 0, 0, lb, 1.0, 0, 0)
+    b = cl["b_vms"]
+    assert cl["shortcut_want"] not in b and c["rank"][cl["shortcut_want"]] < min(c["rank"][b])
+    o = oracle.match(*c["args"], traces.match_params(c["nc"]))
+    assert o["assign"].tolist() == cl["want"] and cl["want"][0] in b
+
+
+@pytest.mark.parametrize("constr", [False, True])
+@pytest.mark.parametrize("outcome", ["win", "lose"])
+@pytest.mark.parametrize("reason", list(E.RCP_REASONS))
+def test_ieee_branch_decides_on_an_ulp(oracle, reason, outcome, constr):
+    """safe_rcp rejects the X VMs' denominators for `reason` and takes the F VMs', every amount stays within the
+    guard (the F's keep the shortcut), X fits one ulp better (win) or worse (lose), and the first job goes to the
+    better kind's lowest name."""
+    c = E.ieee_branch(reason, outcome, "perm", constr)
+    cl = c["claims"]
+    _, jobs, offers, _ = c["args"]
+    lc, lm, rc, rm = (offers.col(k) for k in ("cpus", "mem", "run_cpus", "run_mem"))
+    x = np.zeros(len(lc), bool)
+    x[cl["x_vms"]] = True
+    rcp = np.array([R.safe_rcp(d) for d in (lc + rc).tolist()])
+    assert (rcp[x] == 0).all() and (rcp[~x] != 0).all()
+    assert all(R.safe_rcp(d) != 0 for d in (lm + rm).tolist())
+    for a in (lc, lm, rc, rm, jobs.col("cpus"), jobs.col("mem")):
+        assert (((a >= E.GUARD_MIN) & (a <= 2.0 ** 600)) | (a == 0)).all()
+    assert cl["ff"] == np.nextafter(cl["fx"], -np.inf if outcome == "win" else np.inf)
+    f = _fit_all(c, 0)
+    assert f[x].max() == cl["fx"] and f[~x].max() == cl["ff"]
+    o = oracle.match(*c["args"], traces.match_params(c["nc"]))
+    a = o["assign"]
+    assert a[0] == cl["first"] and (a[0] in cl["x_vms"]) == (outcome == "win")
+    assert set(a[a >= 0].tolist()) & set(cl["x_vms"]) and set(a[a >= 0].tolist()) - set(cl["x_vms"])
+
+
+def test_one_tiny_request_in_a_c2_pool(oracle):
+    """One request below the guard among Cook's amounts, and the queue spans many blocks of either kernel."""
+    c = E.ieee_cycle("perm", False)
+    _, jobs, offers, _ = c["args"]
+    cpus = jobs.col("cpus")
+    tiny = c["claims"]["tiny"]
+    assert 0 < cpus[tiny] < E.GUARD_MIN
+    rest = np.concatenate([np.delete(cpus, tiny), jobs.col("mem")] +
+                          [offers.col(k) for k in ("cpus", "mem", "run_cpus", "run_mem")])
+    assert (((rest >= E.GUARD_MIN) & (rest <= 2.0 ** 600)) | (rest == 0)).all()
+    assert c["nc"] > 10 * 128
+    o = oracle.match(*c["args"], traces.match_params(c["nc"]))
+    assert o["assign"][tiny] >= 0 and (o["assign"] >= 0).sum() > 128
 
 
 # ---- GPU: the kernel against the oracle -----------------------------------------------------------------------
