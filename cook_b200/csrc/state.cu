@@ -76,6 +76,18 @@ enum { OL_PORT = 0, OL_GPU = 1, OL_DISK = 2, OL_ATTR = 3, OL_N };
 // slot keeps its live flag and generation, so its queue entry stays.
 constexpr int MAXC = 16;
 constexpr int SCATTER_MAXC = MAXC + 1;   // a pending upsert: its data columns, then the job and list facts' resets
+// The columns an upsert resets after the delta's own, with the absent value each gets.  The scatters write exactly these
+// lists, so a further reset column is one more entry here, and the column count that bounds ScatterArgs::c follows.
+struct ResetCol { int col; long long dflt; };
+constexpr ResetCol PENDING_UPSERT_RESETS[] = {{P_JF, 0},        // no job facts
+                                              {P_LF_EXEC, 0}};  // no list facts
+constexpr ResetCol RUNNING_UPSERT_RESETS[] = {{R_MAXRT, -1}, {R_FACTS, 0}, {R_REASON, -1},   // the absent task facts
+                                              {R_LF_EXEC, 0}};                              // no list facts
+constexpr int N_PENDING_UPSERT_RESETS = sizeof(PENDING_UPSERT_RESETS) / sizeof(ResetCol);
+constexpr int N_RUNNING_UPSERT_RESETS = sizeof(RUNNING_UPSERT_RESETS) / sizeof(ResetCol);
+static_assert(P_NDATA + N_PENDING_UPSERT_RESETS <= SCATTER_MAXC, "a pending upsert's columns do not fit ScatterArgs");
+static_assert(R_NDATA + N_RUNNING_UPSERT_RESETS <= SCATTER_MAXC, "a running upsert's columns do not fit ScatterArgs");
+static_assert(O_NDATA <= SCATTER_MAXC, "an offer's columns do not fit ScatterArgs");
 struct ScatterCol { char* dst; const char* src; long long dflt; int sz; };
 struct ScatterArgs {
   ScatterCol c[SCATTER_MAXC];
@@ -1357,9 +1369,9 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
         else up = reinterpret_cast<const char*>(c.up(static_cast<const int64_t*>(src[k]), np));
         pu.c[k] = ScatterCol{static_cast<char*>(S->pend.col[k]), up, dflt[k], P_SZ[k]};
       }
-      pu.c[P_NDATA] = ScatterCol{static_cast<char*>(S->pend.col[P_JF]), nullptr, 0, P_SZ[P_JF]};   // no job facts
-      pu.c[P_NDATA + 1] = ScatterCol{static_cast<char*>(S->pend.col[P_LF_EXEC]), nullptr, 0, 1};     // no list facts
-      pu.nc = P_NDATA + 2;
+      pu.nc = P_NDATA;
+      for (const ResetCol& r : PENDING_UPSERT_RESETS)
+        pu.c[pu.nc++] = ScatterCol{static_cast<char*>(S->pend.col[r.col]), nullptr, r.dflt, P_SZ[r.col]};
       pu.slot = c.up(pup_slot.data(), np);
       for (int l = 0; l < 3; l++) {
         pu.doff[l] = c.up(lists_off[l], np + 1);
@@ -1378,11 +1390,9 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
                                       : reinterpret_cast<const char*>(c.up(static_cast<const int64_t*>(src[k]), nr));
         ru.c[k] = ScatterCol{static_cast<char*>(S->run.col[k]), up, dflt[k], R_SZ[k]};
       }
-      ru.c[R_NDATA] = ScatterCol{static_cast<char*>(S->run.col[R_MAXRT]), nullptr, -1, R_SZ[R_MAXRT]};
-      ru.c[R_NDATA + 1] = ScatterCol{static_cast<char*>(S->run.col[R_FACTS]), nullptr, 0, R_SZ[R_FACTS]};
-      ru.c[R_NDATA + 2] = ScatterCol{static_cast<char*>(S->run.col[R_REASON]), nullptr, -1, R_SZ[R_REASON]};
-      ru.c[R_NDATA + 3] = ScatterCol{static_cast<char*>(S->run.col[R_LF_EXEC]), nullptr, 0, 1};   // no list facts
-      ru.nc = R_NDATA + 4;
+      ru.nc = R_NDATA;
+      for (const ResetCol& r : RUNNING_UPSERT_RESETS)
+        ru.c[ru.nc++] = ScatterCol{static_cast<char*>(S->run.col[r.col]), nullptr, r.dflt, R_SZ[r.col]};
       ru.slot = c.up(rup_slot.data(), nr);
       ru.doff[0] = c.up(rgo, nr + 1);
       if (c.base && radd) c.copy(RG.v[0] + rtail0, d->running_group_idx, radd);
@@ -3529,10 +3539,10 @@ int32_t finish(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, con
   CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
     if (!n) return;
     if (nrq) {   // live again with a new generation, reserved_host -1, no job facts, no longer parked
-      rq.c[0] = ScatterCol{static_cast<char*>(S->pend.col[P_RESERVED]), nullptr, -1, P_SZ[P_RESERVED]};
-      rq.c[1] = ScatterCol{static_cast<char*>(S->pend.col[P_JF]), nullptr, 0, P_SZ[P_JF]};
-      rq.c[2] = ScatterCol{reinterpret_cast<char*>(S->park), nullptr, 0, 1};
-      rq.nc = 3;
+      rq.nc = 0;   // carve runs this body twice: once to size, once to upload
+      rq.c[rq.nc++] = ScatterCol{static_cast<char*>(S->pend.col[P_RESERVED]), nullptr, -1, P_SZ[P_RESERVED]};
+      rq.c[rq.nc++] = ScatterCol{static_cast<char*>(S->pend.col[P_JF]), nullptr, 0, P_SZ[P_JF]};
+      rq.c[rq.nc++] = ScatterCol{reinterpret_cast<char*>(S->park), nullptr, 0, 1};
       rq.slot = c.up(rq_slot.data(), nrq);
     }
     if (nap) {
