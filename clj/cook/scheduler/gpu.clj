@@ -237,8 +237,8 @@
 
 (defn monitor-resident!
   "set-stats-counters! (monitor.clj:177-207) for one pool or quota-group name from its resident handles (the pool's
-   own, or every pool the quota grouping maps to the name; one device): cook_state_user_stats, then the per-user and
-   \"all\" counters through `set-user-counter!` (fn [state user type amount]) and the user counts through
+   own, or every pool the quota grouping maps to the name, on one device or several): cook_state_user_stats, then the
+   per-user and \"all\" counters through `set-user-counter!` (fn [state user type amount]) and the user counts through
    `set-total-counter!` (fn [state n]), the monitor's own setters, which clear stale users and feed Prometheus.
    `args` are Native/stateUserStats' n_users, users and quota_rest_ok; `names` maps user codes to names; `quota-extra`
    (fn [code]) gives a waiting-under-quota user's other quota keys ({\"gpus\" x \"launch-rate-saved\" y ...}), which
@@ -553,16 +553,16 @@
 ;; ---------------------------------------------------------------------------------------------
 ;; /stats/instances over resident pools: the device half of task-stats/get-stats (task_stats.clj), for status running
 ;; or unknown (the running rows) and success or failed (the finished-instance histories) without a name filter; the
-;; handler keeps the Datomic path for a name filter, for pools on several devices (percentiles do not compose from
-;; per-device summaries) and for a window that starts before a history's horizon
+;; handler keeps the Datomic path for a name filter and for a window that starts before a history's horizon.  Pools on
+;; several devices are answered by one call: the other devices' rows are gathered to the first handle's device
 (def ^:private instance-stats-leaders 10)
 (defn instance-stats!
-  "Instance stats over `handles` (one device): `status` :running or :unknown (the live running rows, one `now-ms`) or
+  "Instance stats over `handles` (one device or several): `status` :running or :unknown (the live running rows, one `now-ms`) or
    :success or :failed (the handles' histories, history-seed!; now-ms unused), the window [start-ms, end-ms), the
    entity-id bounds [task-id-lo, task-id-hi) (d/entid-at of start - 1 h and end + 1 h).  `n-rows` sizes the segments:
    the live running rows over the handles (the shim's count); for a history, a capacity the call may refuse with the
    count it needs (cook_state_history_stats' COOK_E_TOO_LARGE), and the handler retries with that count.  A name
-   filter, pools on several devices, or a window before a history's horizon keep the Datomic path.  Returns {:segments [{:kind 0|1|2 (overall, reason, user and
+   filter or a window before a history's horizon keep the Datomic path.  Returns {:segments [{:kind 0|1|2 (overall, reason, user and
    reason) :user :reason (-1: none) :count :totals [run cpu mem] :percentiles [[p50 p75 p95 p99 p100] x3]}]
    :leaders-cpu [[user total]] :leaders-mem [[user total]]}; the handler builds the response (user names, reason
    strings, the nil reason's key) as cook_b200/cycle.py's instance_stats_response does."
@@ -641,8 +641,8 @@
 ;;   :job/state leaves :job.state/completed       -> :reopened (:job/ensure-not-completed, :job/update-retry-count)
 ;;   a completed job gains a successful instance  -> :success
 ;;   a listed attribute of a completed job changes (user, submit time, submit pool, custom executor) -> a new record
-;; The listing handler sends a completed-family state to list-completed when there is no name filter, the request's
-;; pools are on one device, every handle's log is on and start >= every horizon; otherwise the Datomic path.
+;; The listing handler sends a completed-family state to list-completed when there is no name filter, every handle's
+;; log is on and start >= every horizon, the request's pools on one device or several; otherwise the Datomic path.
 (def ^:private completed-kinds {:success 1 :failed 2 :reopened 3})
 (defn- completed-cols [rows]
   (object-array [(longs-buf (map :job-id rows)) (longs-buf (map :stamp rows)) (ints-buf (map :user rows))
@@ -674,7 +674,7 @@
   (check! handle (Native/stateCompletedAdvance handle (long since-ms)) "cook_state_completed_advance"))
 
 (defn list-completed
-  "`user`'s jobs whose latest record over `handles` (one device) is in `state` (:success, :failed or :completed),
+  "`user`'s jobs whose latest record over `handles` (one device or several) is in `state` (:success, :failed or :completed),
    submitted in [start-ms, end-ms), with entity ids in [job-id-lo, job-id-hi), in pool `pool-code` (-1: any;
    `handle-pools` each handle's pool code), only false custom executors unless `include-custom-executor?`, cut to
    `limit` in entity-id order.  The call is made with `cap` entries and, when it needs more, once more with the count

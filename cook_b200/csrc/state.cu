@@ -25,7 +25,9 @@
 // cook_match's considerable pass (match.cu) run on them; a consuming call retires the taken entries' generations.
 #include <algorithm>
 #include <cmath>
+#include <cstdlib>
 #include <map>
+#include <type_traits>
 #include <unordered_map>
 #include <unordered_set>
 
@@ -396,6 +398,7 @@ struct UsageRows {
   int32_t* user; int64_t* id; int32_t* host; double* amt[3];   // host null: no host list
   const int32_t* host_of; int32_t n_codes, H;
   __device__ bool keep(int i) const { return static_cast<const uint8_t*>(col[c.live])[i]; }
+  template <class V> void outs(V&& v) { v(user); v(id); v(amt[0]); v(amt[1]); v(amt[2]); v(host); }
   __device__ void emit(int i, int d) const {
     d += base;
     user[d] = static_cast<const int32_t*>(col[c.user])[i];
@@ -1617,6 +1620,96 @@ cudaError_t map_hosts(int32_t* host_of, int32_t n_codes, const int32_t* d_codes,
   return cudaGetLastError();
 }
 
+// ---- the gather step of the reads whose handles may span devices (DESIGN.md §9a): cook_state_user_stats,
+// cook_state_instance_stats, cook_state_history_stats and cook_state_list_completed compact each handle's rows into
+// one dense range carved from pools[0]'s scratch, a handle's rows at `base`, after those of the handles before it.
+// A handle on pools[0]'s device compacts straight into that range on pools[0]'s stream.  A handle on another device
+// runs the same functor on its own device and stream into staging columns, a count and blk carved from its own
+// scratch; pools[0]'s stream waits on an event recorded there and copies each packed column to `base` with
+// cudaMemcpyPeerAsync (peer access is not enabled; no device or context setting changes).  Only the rows the
+// compaction keeps cross, rows x the functor's bytes per row.  Handle order and base are those of one device, so the
+// leader's pipeline reads the same rows in the same places.  COOK_STAGE_HANDLES=1 in the environment (read per call)
+// sends every handle after pools[0] through the staging even on pools[0]'s device, so that one GPU runs the path.
+// A gathered functor lists its output columns with outs(visitor) (a null column is not carved) and reads only its own
+// handle's tables, so no call-wide array has to exist on the handle's device.
+bool stage_handles() {
+  const char* e = getenv("COOK_STAGE_HANDLES");
+  return e && strcmp(e, "1") == 0;
+}
+
+struct Gather {
+  static constexpr int MAXO = 8;   // the most output columns a gathered functor has
+  cook_pool* lead;
+  bool all = stage_handles();
+  std::vector<const cook_pool*> used;   // the handles whose staging this call has filled
+
+  explicit Gather(cook_pool* p) : lead(p) {}
+  bool staged(const cook_pool* h) const { return h != lead && (all || h->device != lead->device); }
+
+  // body() with handle h's device current; pools[0]'s device current again afterwards
+  template <class Body>
+  cudaError_t on(const cook_pool* h, const Body& body) const {
+    cudaError_t e = cudaSetDevice(h->device);
+    if (e == cudaSuccess) e = body();
+    const cudaError_t back = cudaSetDevice(lead->device);
+    return e != cudaSuccess ? e : back;
+  }
+
+  // Handle h's compaction f (its base and output columns those of pools[0]'s range) over n_max items, `rows` of them
+  // kept.  Not staged: on pools[0]'s stream with blk and cnt (the call's own).  Counts its launches in *nl.
+  template <class F>
+  cudaError_t rows(cook_pool* h, const F& f, int n_max, int rows, int32_t* blk, int32_t* cnt, int* nl) {
+    if (!staged(h)) {
+      compact(f, n_max, nullptr, blk, cnt, rows, lead->stream, nl);
+      return cudaGetLastError();
+    }
+    F g = f;
+    char *dst[MAXO], *src[MAXO];
+    size_t sz[MAXO];
+    int nc = 0;
+    g.outs([&](auto* p) {
+      if (p) { dst[nc] = reinterpret_cast<char*>(p); sz[nc++] = sizeof(*p); }
+    });
+    // staging a second time in one call: its columns are free once pools[0]'s copies of the first have run
+    const bool again = std::find(used.begin(), used.end(), h) != used.end();
+    if (again) {
+      cudaError_t e = cudaEventRecord(lead->ev[19], lead->stream);
+      if (e != cudaSuccess) return e;
+    } else {
+      used.push_back(h);
+    }
+    cudaError_t e = on(h, [&]() -> cudaError_t {
+      if (again) {
+        const cudaError_t w = cudaStreamWaitEvent(h->stream, lead->ev[19], 0);
+        if (w != cudaSuccess) return w;
+      }
+      PoolState* R = state_of(const_cast<cook_pool*>(h), false);   // h holds the rows
+      int32_t *s_blk = nullptr, *s_cnt = nullptr;
+      const cudaError_t c = carve(R->scratch, h->stream, nullptr, nullptr, [&](Carve& cv) {
+        s_cnt = cv.take<int32_t>(1);
+        s_blk = cv.take<int32_t>((size_t)n_max / CP_BLOCK + 2);
+        for (int k = 0; k < nc; k++) src[k] = cv.take<char>(sz[k] * (size_t)rows);
+      });
+      if (c != cudaSuccess) return c;
+      int k = 0;
+      g.outs([&](auto*& p) {
+        if (p) p = reinterpret_cast<std::remove_reference_t<decltype(p)>>(src[k++]);
+      });
+      g.base = 0;
+      compact(g, n_max, nullptr, s_blk, s_cnt, rows, h->stream, nl);
+      const cudaError_t l = cudaGetLastError();
+      return l != cudaSuccess ? l : cudaEventRecord(h->ev[20], h->stream);
+    });
+    if (e != cudaSuccess) return e;
+    if ((e = cudaStreamWaitEvent(lead->stream, h->ev[20], 0)) != cudaSuccess) return e;
+    for (int k = 0; k < nc; k++)
+      if ((e = cudaMemcpyPeerAsync(dst[k] + sz[k] * (size_t)f.base, lead->device, src[k], h->device,
+                                   sz[k] * (size_t)rows, lead->stream)) != cudaSuccess)
+        return e;
+    return cudaSuccess;
+  }
+};
+
 // The usage of R live rows of one or more handles, each sum a left fold in ascending id: per user (U > 0), per
 // listed host (H > 0, running rows only) and of the pool.  The running rows by task id, or (pending) the pending rows
 // by job id; an id several handles hold, in handle order.  The caller sets rows.host_of / rows.n_codes (H > 0) and
@@ -1657,8 +1750,10 @@ struct UsageFold {
     }
   }
 
-  // the live rows of handles S[0, n) (their counts in S[0]'s counters), then fold()
-  cudaError_t run(const PoolState* const* S, int n, cudaStream_t st, int* nl) {
+  // the live rows of handles S[0, n) (their counts in S[0]'s counters), then fold().  With a gather g, hp[k] is S[k]'s
+  // handle and g->lead S[0]'s (cook_state_user_stats: the handles may span devices; no host is listed then).
+  cudaError_t run(const PoolState* const* S, int n, cudaStream_t st, int* nl, Gather* g = nullptr,
+                  cook_pool* const* hp = nullptr) {
     rows.c = pending ? PEND_COLS : RUN_COLS; rows.H = H;
     rows.base = 0;
     for (int k = 0; k < n; k++) {
@@ -1666,7 +1761,13 @@ struct UsageFold {
       const int live = (int)t.slot_of.size();
       if (!live) continue;
       rows.col = t.d_col;
-      compact(rows, t.hw, nullptr, blk, S[0]->counters + (pending ? 1 : 0), live, st, nl);
+      int32_t* cnt = S[0]->counters + (pending ? 1 : 0);
+      if (g) {
+        const cudaError_t e = g->rows(hp[k], rows, t.hw, live, blk, cnt, nl);
+        if (e != cudaSuccess) return e;
+      } else {
+        compact(rows, t.hw, nullptr, blk, cnt, live, st, nl);
+      }
       rows.base += live;
     }
     return fold(st, nl);
@@ -3018,15 +3119,17 @@ int32_t considerable(cook_pool* pool, PoolState* S, const cook_user_table* users
 }
 
 // The handle set of a call over several pools: a NULL pools, n <= 0 or a NULL pools[0] is a bare COOK_E_BADARG (no
-// handle to hold the message); then every handle non-NULL, listed once and on pools[0]'s device.
-int32_t check_handle_set(cook_pool* const* pools, int n, const char* who) {
+// handle to hold the message); then every handle non-NULL, listed once and, unless any_device (the calls with a
+// gather step), on pools[0]'s device.
+int32_t check_handle_set(cook_pool* const* pools, int n, const char* who, bool any_device = false) {
   if (!pools || n <= 0 || !pools[0]) return COOK_E_BADARG;
   cook_pool* pool = pools[0];
   for (int k = 0; k < n; k++) {
     if (!pools[k]) return set_err(pool, COOK_E_BADARG, "%s: a NULL handle", who);
     if (std::find(pools, pools + k, pools[k]) != pools + k)
       return set_err(pool, COOK_E_BADARG, "%s: a handle listed twice", who);
-    if (pools[k]->device != pool->device) return set_err(pool, COOK_E_BADARG, "%s: handles on different devices", who);
+    if (!any_device && pools[k]->device != pool->device)
+      return set_err(pool, COOK_E_BADARG, "%s: handles on different devices", who);
   }
   return COOK_OK;
 }
@@ -3044,9 +3147,10 @@ int32_t user_stats(cook_pool* const* pools, int n, const cook_user_table* users,
                    double* out_all_cpus, double* out_all_mem, int64_t* out_users, cook_phase_stats* out_stats) {
   const char* who = "cook_state_user_stats";
   // ---- every check before any device work or output
-  if (int32_t rc = check_handle_set(pools, n, who)) return rc;
+  if (int32_t rc = check_handle_set(pools, n, who, true)) return rc;
   cook_pool* pool = pools[0];
   std::vector<const PoolState*> S;
+  std::vector<cook_pool*> P;   // S[k]'s handle
   int R = 0, J = 0, hw_r = 0, hw_p = 0;
   if (!users || !out_jobs || !out_cpus || !out_mem || !out_member || !out_all_jobs || !out_all_cpus || !out_all_mem ||
       !out_users)
@@ -3062,6 +3166,7 @@ int32_t user_stats(cook_pool* const* pools, int n, const cook_user_table* users,
     if (std::max(count_max(s->users_p), count_max(s->users_r)) >= U)
       return set_err(pool, COOK_E_BADARG, "%s: a live row's user code is >= n_users", who);
     S.push_back(s);
+    P.push_back(pools[k]);
     R += (int)s->run.slot_of.size(); J += (int)s->pend.slot_of.size();
     hw_r = std::max(hw_r, s->run.hw); hw_p = std::max(hw_p, s->pend.hw);
   }
@@ -3080,8 +3185,12 @@ int32_t user_stats(cook_pool* const* pools, int n, const cook_user_table* users,
   CK(pool, cudaSetDevice(pool->device));
   PoolState* S0 = state_of(pool, true);   // pools[0]'s scratch and counters, even when it holds no row
   if (!S0) return set_err(pool, COOK_E_OOM, "%s: out of device memory", who);
-  if (S.empty() || S[0] != S0) S.insert(S.begin(), S0);   // S[0] owns the counters the compactions write
+  if (S.empty() || S[0] != S0) {   // S[0] owns the counters the compactions write
+    S.insert(S.begin(), S0);
+    P.insert(P.begin(), pool);
+  }
   cudaStream_t st = pool->stream;
+  Gather g(pool);
   // ---- one carve: the two folds, the user columns (uploaded), the per-state columns and the totals
   UsageFold fr, fw;
   fr.R = R; fr.U = U;
@@ -3109,9 +3218,9 @@ int32_t user_stats(cook_pool* const* pools, int n, const cook_user_table* users,
   const PoolState* const* list = S.data();
   const int ns = (int)S.size();
   fr.a.user_out = run; fw.a.user_out = wait;
-  if (R) CK(pool, fr.run(list, ns, st, &nl));
+  if (R) CK(pool, fr.run(list, ns, st, &nl, &g, P.data()));
   else CK(pool, cudaMemsetAsync(run, 0, sizeof(double) * 4 * (size_t)U, st));
-  if (J) CK(pool, fw.run(list, ns, st, &nl));
+  if (J) CK(pool, fw.run(list, ns, st, &nl, &g, P.data()));
   else CK(pool, cudaMemsetAsync(wait, 0, sizeof(double) * 4 * (size_t)U, st));
   a.run = run; a.wait = wait;
   user_stats_kernel<<<(U + 255) / 256, 256, 0, st>>>(a);
@@ -4786,6 +4895,7 @@ struct ISRows {
   int32_t* user; int32_t* reason; int64_t* tid; int32_t* pidx; int64_t* start; double* cpus; double* mem;
   uint8_t* facts;
   __device__ bool keep(int i) const { return static_cast<const uint8_t*>(col[R_LIVE])[i]; }
+  template <class V> void outs(V&& v) { v(user); v(reason); v(tid); v(pidx); v(start); v(cpus); v(mem); v(facts); }
   __device__ void emit(int i, int d) const {
     d += base;
     user[d] = static_cast<const int32_t*>(col[R_USER])[i];
@@ -5074,7 +5184,7 @@ int32_t instance_stats(cook_pool* const* pools, int n, int64_t now, int32_t stat
                        int64_t tid_lo, int64_t tid_hi, int32_t seg_cap, const ISOut& o, cook_phase_stats* out_stats) {
   const char* who = "cook_state_instance_stats";
   // ---- every check before any device work or output
-  if (int32_t rc = check_handle_set(pools, n, who)) return rc;
+  if (int32_t rc = check_handle_set(pools, n, who, true)) return rc;
   cook_pool* pool = pools[0];
   if (status != COOK_IS_RUNNING && status != COOK_IS_UNKNOWN) return set_err(pool, COOK_E_BADARG, "%s: an unknown status", who);
   if (end_ms <= start_ms) return set_err(pool, COOK_E_BADARG, "%s: end_ms <= start_ms", who);
@@ -5118,12 +5228,14 @@ int32_t instance_stats(cook_pool* const* pools, int n, int64_t now, int32_t stat
   CK(pool, p.clear(st));
   int nl = 0;
   // ---- the selection and its metrics
+  Gather g(pool);
   int base = 0;
   for (const auto& h : hs) {
     const int live = (int)h.first->run.slot_of.size();
-    compact(ISRows{h.first->run.d_col, base, h.second, a_user, a_reason, a_tid, a_pidx, a_start, a_cpus, a_mem,
-                   a_facts},
-            h.first->run.hw, nullptr, p.blk, p.cnt + 5, live, st, &nl);
+    CK(pool, g.rows(pools[h.second],
+                    ISRows{h.first->run.d_col, base, h.second, a_user, a_reason, a_tid, a_pidx, a_start, a_cpus, a_mem,
+                           a_facts},
+                    h.first->run.hw, live, p.blk, p.cnt + 5, &nl));
     base += live;
   }
   compact(ISSel{a_user, a_reason, a_tid, a_pidx, a_start, a_cpus, a_mem, a_facts, now, start_ms, end_ms, tid_lo, tid_hi,
@@ -5151,6 +5263,9 @@ struct HSSel {
     return (h.ok[i] != 0) == (success != 0) && h.tid[i] >= tid_lo && h.tid[i] < tid_hi && h.start[i] >= start_ms &&
            h.start[i] < end_ms;
   }
+  template <class V> void outs(V&& v) {
+    v(s_user); v(s_reason); v(s_tid); v(s_pidx); v(s_pos); v(met[0]); v(met[1]); v(met[2]);
+  }
   __device__ void emit(int i, int d) const {
     d += base;
     s_user[d] = h.user[i]; s_reason[d] = h.reason[i]; s_tid[d] = h.tid[i]; s_pidx[d] = pool; s_pos[d] = i;
@@ -5171,7 +5286,7 @@ int32_t history_stats(cook_pool* const* pools, int n, int32_t status, int64_t st
                       int64_t tid_hi, int32_t seg_cap, const ISOut& o, cook_phase_stats* out_stats) {
   const char* who = "cook_state_history_stats";
   // ---- every check before any device work or output
-  if (int32_t rc = check_handle_set(pools, n, who)) return rc;
+  if (int32_t rc = check_handle_set(pools, n, who, true)) return rc;
   cook_pool* pool = pools[0];
   if (status != COOK_IS_SUCCESS && status != COOK_IS_FAILED) return set_err(pool, COOK_E_BADARG, "%s: an unknown status", who);
   if (end_ms <= start_ms) return set_err(pool, COOK_E_BADARG, "%s: end_ms <= start_ms", who);
@@ -5202,21 +5317,47 @@ int32_t history_stats(cook_pool* const* pools, int n, int32_t status, int64_t st
     return HSSel{hs[j].first->c, base, hs[j].second, ok, start_ms, end_ms, tid_lo, tid_hi,
                  p.s_user, p.s_reason, p.s_tid, p.s_pidx, p.s_pos, {p.met[0], p.met[1], p.met[2]}};
   };
-  // ---- the selection's size per handle, so that every buffer after it is sized by the selection
+  // ---- the selection's size per handle, so that every buffer after it is sized by the selection.  A staged handle
+  // (Gather) counts on its own device, into its own scratch.
+  Gather g(pool);
   int32_t* hcnt = nullptr;
   int64_t h2d = 0, d2h = 0;
   CK(pool, carve(S0->scratch, st, pool->ev[20], &h2d, [&](Carve& c) { hcnt = c.take<int32_t>(H); }));
   CK(pool, cudaEventRecord(pool->ev[21], st));
   CK(pool, cudaMemsetAsync(hcnt, 0, sizeof(int32_t) * H, st));
   int nl = 0;
+  std::vector<int32_t> cnt(H);
   for (int j = 0; j < H; j++) {
     const int T = (int)hs[j].first->tail;
-    hs_count_kernel<<<(T + 255) / 256, 256, 0, st>>>(sel(j, 0, ISPipe{}), T, hcnt + j);
-    nl++;
+    cook_pool* h = pools[hs[j].second];
+    if (!g.staged(h)) {
+      hs_count_kernel<<<(T + 255) / 256, 256, 0, st>>>(sel(j, 0, ISPipe{}), T, hcnt + j);
+      nl++;
+      continue;
+    }
+    CK(pool, g.on(h, [&]() -> cudaError_t {
+      int32_t* rc = nullptr;
+      cudaError_t e = carve(state_of(h, false)->scratch, h->stream, nullptr, nullptr,
+                            [&](Carve& c) { rc = c.take<int32_t>(1); });
+      if (e == cudaSuccess) e = cudaMemsetAsync(rc, 0, sizeof(int32_t), h->stream);
+      if (e != cudaSuccess) return e;
+      hs_count_kernel<<<(T + 255) / 256, 256, 0, h->stream>>>(sel(j, 0, ISPipe{}), T, rc);
+      nl++;
+      return (e = cudaGetLastError()) == cudaSuccess ? download(&cnt[j], rc, 1, h->stream, &d2h) : e;
+    }));
   }
   CK(pool, cudaGetLastError());
-  std::vector<int32_t> cnt(H);
-  CK(pool, download(cnt.data(), hcnt, H, st, &d2h));
+  int n_staged = 0;
+  for (int j = 0; j < H; j++) n_staged += g.staged(pools[hs[j].second]) ? 1 : 0;
+  if (!n_staged) {
+    CK(pool, download(cnt.data(), hcnt, H, st, &d2h));
+  } else {   // 4 bytes per handle either way
+    for (int j = 0; j < H; j++) {
+      cook_pool* h = pools[hs[j].second];
+      if (g.staged(h)) CK(pool, cudaStreamSynchronize(h->stream));
+      else CK(pool, download(&cnt[j], hcnt + j, 1, st, &d2h));
+    }
+  }
   CK(pool, cudaStreamSynchronize(st));
   int64_t S = 0;
   for (int32_t c : cnt) S += c;
@@ -5227,7 +5368,8 @@ int32_t history_stats(cook_pool* const* pools, int n, int32_t status, int64_t st
   CK(pool, p.clear(st));
   int base = 0;
   for (int j = 0; j < H && S; j++) {
-    if (cnt[j]) compact(sel(j, base, p), (int)hs[j].first->tail, nullptr, p.blk, p.cnt + 5, cnt[j], st, &nl);
+    if (cnt[j])
+      CK(pool, g.rows(pools[hs[j].second], sel(j, base, p), (int)hs[j].first->tail, cnt[j], p.blk, p.cnt + 5, &nl));
     base += cnt[j];
   }
   CK(pool, cudaGetLastError());
@@ -6602,6 +6744,7 @@ struct CJRows {
   CJCols c; int32_t user; int base; int32_t pidx; bool pool_ok; LJSel q; int32_t state;
   int64_t* jid; int64_t* stamp; int64_t* submit; int32_t* pi; uint8_t* ok;
   __device__ bool keep(int i) const { return c.user[i] == user; }
+  template <class V> void outs(V&& v) { v(jid); v(stamp); v(submit); v(pi); v(ok); }
   __device__ void emit(int i, int d) const {
     d += base;
     const int64_t j = c.jid[i], s = c.submit[i];
@@ -6783,7 +6926,7 @@ int32_t list_completed(cook_pool* const* pools, int n, int32_t user, int32_t sta
                        int32_t* o_pool, int32_t* o_n, cook_phase_stats* out_stats) {
   const char* who = "cook_state_list_completed";
   // ---- every check before any device work or output
-  if (int32_t rc = check_handle_set(pools, n, who)) return rc;
+  if (int32_t rc = check_handle_set(pools, n, who, true)) return rc;
   cook_pool* pool = pools[0];
   if (state != COOK_LC_SUCCESS && state != COOK_LC_FAILED && state != COOK_LC_COMPLETED)
     return set_err(pool, COOK_E_BADARG, "%s: an unknown state", who);
@@ -6830,10 +6973,11 @@ int32_t list_completed(cook_pool* const* pools, int n, int32_t user, int32_t sta
   CK(pool, cudaEventRecord(pool->ev[21], st));
   int nl = 0;
   int base = 0;
+  Gather g(pool);
   for (const Src& h : hs) {
-    const bool pool_ok = q.pool == -1 || handle_pool[h.k] == q.pool;
-    compact(CJRows{h.l->c, user, base, h.k, pool_ok, q, state, jid, stamp, submit, pi, ok}, (int)h.l->tail, nullptr, blk,
-            cnt + 1, h.rows, st, &nl);
+    const bool pool_ok = q.pool == -1 || handle_pool[h.k] == q.pool;   // on the host: no array crosses devices
+    CK(pool, g.rows(pools[h.k], CJRows{h.l->c, user, base, h.k, pool_ok, q, state, jid, stamp, submit, pi, ok},
+                    (int)h.l->tail, h.rows, blk, cnt + 1, &nl));
     base += h.rows;
   }
   CK(pool, csort::sort_indices(ord, tmp, Cn, LessJobStamp{jid, stamp}, st, &nl));

@@ -1012,8 +1012,8 @@ def state_list_jobs(engines, user, states, start_ms, end_ms, job_id_lo=-(1 << 63
 
 def state_list_completed(engines, user, state, start_ms, end_ms, job_id_lo=-(1 << 63), job_id_hi=(1 << 63) - 1,
                          pool_code=-1, handle_pool=None, include_custom_executor=True, limit=(1 << 31) - 1, cap=1024):
-    """cook_state_list_completed over the completed-job logs of `engines` (one device, the work on engines[0]'s
-    stream): user code `user`'s jobs whose latest record is of `state` (abi.LC_SUCCESS, abi.LC_FAILED or
+    """cook_state_list_completed over the completed-job logs of `engines` (on one device or several: the work runs on
+    engines[0]'s stream, each other device's records of the user gathered to it): user code `user`'s jobs whose latest record is of `state` (abi.LC_SUCCESS, abi.LC_FAILED or
     abi.LC_COMPLETED), submitted in [start_ms, end_ms), with job ids in [job_id_lo, job_id_hi), in the pool `pool_code`
     (-1: any; handle_pool: each engine's pool code), cut to `limit`.  Returns 'job_id', 'submit_ms' and 'pool' (the
     engine index of the latest record) as numpy columns in ascending job id, and 'stats', the call's own phase
@@ -1068,7 +1068,8 @@ def _is_answer(engines, call, cap):
 
 
 def state_instance_stats(engines, now_ms, status, start_ms, end_ms, task_id_lo=-(1 << 63), task_id_hi=(1 << 63) - 1):
-    """cook_state_instance_stats over the live running rows of `engines` (one device, the work on engines[0]'s stream):
+    """cook_state_instance_stats over the live running rows of `engines` (on one device or several: the work runs on
+    engines[0]'s stream, each other device's rows gathered to it):
     the rows of `status` (abi.IS_RUNNING or abi.IS_UNKNOWN) with task_id_lo <= task id < task_id_hi and start_ms <=
     start < end_ms.  Returns the segments as numpy columns 'kind', 'user', 'reason', 'count' (int64), 'total' [n, 3]
     and 'pct' [n, 3, 5] (metrics by abi.IS_RUN_TIME / IS_CPU / IS_MEM, percentiles 50 75 95 99 100), the leaders
@@ -1087,7 +1088,8 @@ def state_instance_stats(engines, now_ms, status, start_ms, end_ms, task_id_lo=-
 
 def state_history_stats(engines, status, start_ms, end_ms, task_id_lo=-(1 << 63), task_id_hi=(1 << 63) - 1,
                         seg_cap=16384):
-    """cook_state_history_stats over the finished rows of `engines`' histories (one device): the rows of `status`
+    """cook_state_history_stats over the finished rows of `engines`' histories (on one device or several: each other
+    device's selection gathered to engines[0]'s): the rows of `status`
     (abi.IS_SUCCESS or abi.IS_FAILED) with task_id_lo <= task id < task_id_hi and start_ms <= start < end_ms.  Returns
     state_instance_stats' answer shape, so cycle.instance_stats_response builds the response unchanged.  The call is
     made with seg_cap segments first and, when more are needed, once more with the count it reports."""
@@ -1108,8 +1110,8 @@ USER_COUNTS = ("total", "starved", "waiting-under-quota", "hungry", "satisfied")
 
 
 def state_user_stats(engines, users, quota_rest_ok=None):
-    """cook_state_user_stats over the live rows of `engines` (one pool, or the pools of a quota group; one device, the
-    work on engines[0]'s stream).  quota_rest_ok: per user code, whether the user's other quota keys are all > 0
+    """cook_state_user_stats over the live rows of `engines` (one pool, or the pools of a quota group, on one device or
+    several: the work runs on engines[0]'s stream, each other device's rows gathered to it).  quota_rest_ok: per user code, whether the user's other quota keys are all > 0
     (None: all).  Returns 'jobs' (int64), 'cpus' and 'mem' as [4, n_users] arrays by abi.STATS_*, 'member' [n_users]
     (bit s: the user is in state s), 'all' {state: (jobs, cpus, mem)} and 'users' {count name: n}, keyed by
     STATS_KEYS and USER_COUNTS, and 'stats', the call's own phase statistics (abi.PhaseStats.as_dict())."""

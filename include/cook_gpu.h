@@ -907,9 +907,9 @@ int32_t cook_last_stats(cook_pool* pool, int32_t phase, cook_phase_stats* out);
  * one pool or of a quota group, and the queue lengths (jobs->queue-lengths, queue_limit.clj:64-90) as the waiting
  * state of single-pool calls.
  *   Rows     the union of the live rows of pools[0, n_pools): one handle gives a pool's stats; the handles of the pools
- *            a quota-group name maps to give that name's (job-ent-in-pool :35-38).  The handles follow
- *            cook_exchange_usage_batch's rules: one device, idle, each call serialised with each of them by the
- *            caller; the work runs on pools[0]'s stream and scratch.
+ *            a quota-group name maps to give that name's (job-ent-in-pool :35-38).  The handles are idle, each call
+ *            serialised with each of them by the caller, on one device or several (the gather step, DESIGN.md §9a);
+ *            the work runs on pools[0]'s stream and scratch, and the answer is the bits of one device.
  *   Folds    get-job-stats (:40-57) per user, each sum a left fold in a fixed order (DESIGN.md §2): waiting over the
  *            live pending rows in ascending job id, running over the live running rows in ascending task id; an id
  *            several handles hold, in the order of pools.  jobs is the number of rows.
@@ -934,15 +934,15 @@ int32_t cook_last_stats(cook_pool* pool, int32_t phase, cook_phase_stats* out);
  *            satisfied = running - waiting.
  * Changes nothing resident: no row, queue, match plan or COOK_USAGE_LAST_MATCH usage.
  * COOK_E_BADARG, before any device work and with nothing written: a NULL pools, users or out_* array; n_pools <= 0;
- * a NULL handle, a handle listed twice or one on another device than pools[0]; n_users <= 0; a NULL div_cpus, div_mem,
- * quota_count, quota_cpus or quota_mem; a live row's user code >= n_users.  A quota group whose pools sit on
- * different GPUs is served by one call per device and the host's addition of the folds.
+ * a NULL handle or a handle listed twice; n_users <= 0; a NULL div_cpus, div_mem, quota_count, quota_cpus or quota_mem;
+ * a live row's user code >= n_users.  An OOM or CUDA error on another handle's device is returned on pools[0], with
+ * nothing written.
  * No live row in any handle: every output zero, no device work.
- * Transfers exactly: up 40 * n_users (the five user columns) + n_users (quota_rest_ok, when given); down 97 * n_users
- * (the three [4][n_users] arrays and out_member) + 136 (the totals).
+ * Transfers exactly: up 40 * n_users (the five user columns) + n_users (quota_rest_ok, when given), none per device;
+ * down 97 * n_users (the three [4][n_users] arrays and out_member) + 136 (the totals); 36 B a live row between devices.
  * Statistics: out_stats (may be NULL) receives the call's own cook_phase_stats: upload of the user columns, the
- * compactions, sorts and folds of both tables, the classification and totals, the download; all zero after a call
- * without device work.  No cook_last_stats slot is written, so every phase reports its own calls as before.
+ * compactions, sorts and folds of both tables (launches on every device), the classification and totals, the download,
+ * timed on pools[0]; all zero without device work.  No cook_last_stats slot is written: each phase reports its own.
  * Outputs are plain caller arrays, like cook_state_usage's, rather than one result struct: every struct of this
  * header has a field-for-field ctypes mirror (cook_b200/abi.py), and arrays need none.                          */
 enum { COOK_STATS_RUNNING = 0, COOK_STATS_WAITING = 1, COOK_STATS_STARVED = 2, COOK_STATS_WUQ = 3 };
@@ -1241,8 +1241,8 @@ int32_t cook_state_user_usage(cook_pool* const* pools, int32_t n_pools, const in
 /* ------------------------------------------------------- instance stats over resident pools */
 /* The device half of GET /stats/instances with status running or unknown and no name filter (task-stats/get-stats,
  * task_stats.clj) over the union of the live running rows of pools[0, n_pools); the handles follow
- * cook_state_user_stats' rules (one device, idle, the work on pools[0]'s stream and scratch).  Pools on several devices
- * keep the Datomic path: percentiles do not compose from per-device summaries.
+ * cook_state_user_stats' rules (on one device or several).  Percentiles do not compose from per-device summaries, so
+ * another device sends its live running rows themselves, 45 B a row, and the answer is the bits of one device.
  *   Selection  (get-tasks) a row is selected when its status is `status` (COOK_IS_RUNNING: without the unknown fact of
  *              cook_state_task_facts; COOK_IS_UNKNOWN: with it), task_id_lo <= task id < task_id_hi (the caller's
  *              d/entid-at of start - 1 h and end + 1 h; the bound is part of the reference's semantics) and
@@ -1295,14 +1295,14 @@ int32_t cook_state_instance_stats(cook_pool* const* pools, int32_t n_pools, int6
  *   Order      every total is a left fold from +0.0 in ascending (task id, pool index, table position): the position
  *              keeps the answer deterministic when one handle holds a task id twice (a caller's divergence, not
  *              checked after the seed).  Leaders of equal totals go by ascending user code.
- * Sizes follow the selection S, not the table: every buffer after a count pass is sized by S.
+ * Sizes follow the selection S: every buffer after a count pass is sized by S, and only S crosses devices (48 B a row).
  * COOK_E_BADARG, before any device work and with nothing written: cook_state_user_stats' handle cases; an unknown
  * status; end_ms <= start_ms; a NULL output (out_stats may be NULL); seg_cap < 0; a handle whose history is off or
  * whose horizon is > start_ms (the caller then keeps the Datomic path).  COOK_E_TOO_LARGE: 4 * S >= 2^31, with nothing
  * written; more than seg_cap segments, with only *out_n_seg (the segments needed) written, so that the caller can
  * retry with that capacity.  No handle holds a row: empty results without device work (statistics zero).
- * Transfers exactly: up nothing; down 4 * H (the selected rows of each of the H handles holding a row), plus, when a
- * row is selected, 8 (the counts), plus, when *out_n_seg <= seg_cap, 164 * *out_n_seg + 24 * *out_n_leader.
+ * Transfers exactly: up nothing; down 4 * H (one count per handle holding a row, whichever device counts it), plus,
+ * when a row is selected, 8 (the counts), plus, when *out_n_seg <= seg_cap, 164 * *out_n_seg + 24 * *out_n_leader.
  * Statistics: out_stats (may be NULL), as cook_state_instance_stats.  Changes nothing resident.                    */
 int32_t cook_state_history_stats(cook_pool* const* pools, int32_t n_pools, int32_t status, int64_t start_ms,
                                  int64_t end_ms, int64_t task_id_lo, int64_t task_id_hi, int32_t seg_cap,
@@ -1514,7 +1514,11 @@ int32_t cook_state_completed_record(cook_pool* pool, int32_t n, const int64_t* j
  * nothing.  Statistics: cook_last_stats(COOK_PHASE_STATE).                                                       */
 int32_t cook_state_completed_advance(cook_pool* pool, int64_t since_ms);
 
-/* The listing over the union of the logs of pools[0, n_pools); the handles follow cook_state_user_stats' rules.
+/* The listing over the union of the logs of pools[0, n_pools); the handles follow cook_state_user_stats' rules, on one
+ * device or several.  A job that moved pools has records on two handles, so the records themselves cross: a handle on
+ * another device sends all of `user`'s records it holds (the job-id bounds and filters are applied on pools[0]), 29
+ * bytes per record (job id, stamp, submit time, pool index, the filters' verdict), and the latest record per job and
+ * the `limit` cut are those of one device.
  * state: COOK_LC_SUCCESS, COOK_LC_FAILED or COOK_LC_COMPLETED (both).
  *   Records    those of `user` with job_id_lo <= job id < job_id_hi (the caller's d/entid-at of start - 1 h and
  *              end + 1 h; user and job id never change over a job's life).  Each job is its latest record; a REOPENED
@@ -1526,8 +1530,8 @@ int32_t cook_state_completed_advance(cook_pool* pool, int64_t since_ms);
  *   Outputs    entry e < *out_n: out_job_id, out_submit_ms, out_pool (the index in pools of the latest record).
  * Changes nothing resident.
  * COOK_E_BADARG, before any device work and with nothing written: cook_state_list_jobs' handle and argument cases
- * (except `states`); state outside COOK_LC_*; a handle whose log is off; a handle whose horizon is > start_ms (the
- * caller then keeps the Datomic path); a NULL output (out_stats may be NULL).
+ * (except `states` and handles on different devices); state outside COOK_LC_*; a handle whose log is off; a handle
+ * whose horizon is > start_ms (the caller then keeps the Datomic path); a NULL output (out_stats may be NULL).
  * COOK_E_TOO_LARGE: more than 2^31 - 1 records of `user` over the handles, with nothing written; more than cap
  * entries, with only *out_n (the entries needed) written, so that the caller can retry with that capacity.
  * No record of `user`: empty results without device work (statistics zero).
