@@ -1175,6 +1175,90 @@ void scatter(ScatterArgs& a, Table& t, int n, int upsert, int live_col, const in
   (*nl)++;
 }
 
+// One column of a patch scatter: table column `col` from the host source `src` (n values; null: the column is not
+// written), with its absent value.
+struct PatchCol { int col; const void* src; long long dflt; };
+// Fills a patch scatter of table t's n rows at `slot` inside a carve: the slots, then each given column uploaded at the
+// table's own width.  The columns start from none on each pass of the carve.
+void patch_args(Carve& c, ScatterArgs& a, const Table& t, const int32_t* slot, int n, std::initializer_list<PatchCol> cols) {
+  a.slot = c.up(slot, n);
+  a.nc = 0;
+  for (const PatchCol& p : cols) {
+    if (!p.src) continue;
+    const int sz = t.sz[p.col];
+    const char* up = sz == 1   ? reinterpret_cast<const char*>(c.up(static_cast<const uint8_t*>(p.src), n))
+                     : sz == 4 ? reinterpret_cast<const char*>(c.up(static_cast<const int32_t*>(p.src), n))
+                               : reinterpret_cast<const char*>(c.up(static_cast<const int64_t*>(p.src), n));
+    a.c[a.nc++] = ScatterCol{static_cast<char*>(t.col[p.col]), up, p.dflt, sz};
+  }
+}
+
+// the slots of n distinct ids live in table t (`kind`: "job" or "task"), or the call's refusal
+int32_t live_slots(cook_pool* pool, const char* who, const Table& t, const char* kind, int n, const int64_t* id,
+                   std::vector<int32_t>* slot) {
+  std::unordered_set<int64_t> seen;
+  seen.reserve((size_t)n);
+  slot->resize(n);
+  for (int i = 0; i < n; i++) {
+    if (!seen.insert(id[i]).second) return set_err(pool, COOK_E_BADARG, "%s: %s id twice", who, kind);
+    auto it = t.slot_of.find(id[i]);
+    if (it == t.slot_of.end()) return set_err(pool, COOK_E_BADARG, "%s: unknown %s id", who, kind);
+    (*slot)[i] = it->second;
+  }
+  return COOK_OK;
+}
+
+// A single-handle call's entry: a NULL handle is a bare COOK_E_BADARG (no handle to hold the message); then the
+// handle's device is made current and body(S) runs on its state, created at the first call.
+template <class Body>
+int32_t on_state(cook_pool* pool, const char* who, const Body& body) {
+  if (!pool) return COOK_E_BADARG;
+  CK(pool, cudaSetDevice(pool->device));
+  PoolState* S = state_of(pool, true);
+  if (!S) return set_err(pool, COOK_E_OOM, "%s: out of device memory", who);
+  return body(S);
+}
+
+// A state write on the handle's stream: up() carves its uploads (from `stage` unless another arena is given) between
+// ev[20] and ev[21]; the call counts its launches in nl; end() checks the launches, records ev[22], synchronizes and
+// records the COOK_PHASE_STATE statistics of the bytes and launches counted here.
+struct StateWrite {
+  cook_pool* pool;
+  PoolState* S;
+  cudaStream_t st;
+  int64_t h2d = 0, d2h = 0;
+  int nl = 0;
+  StateWrite(cook_pool* p, PoolState* s) : pool(p), S(s), st(p->stream) {}
+  template <class Body>
+  int32_t up(const Body& body) { return up(S->stage, body); }
+  template <class Body>
+  int32_t up(Arena& a, const Body& body) {
+    CK(pool, carve(a, st, pool->ev[20], &h2d, body));
+    CK(pool, cudaEventRecord(pool->ev[21], st));
+    return COOK_OK;
+  }
+  // copies straight into device columns, nothing staged: body(Carve&) runs once, with only Carve::copy, between ev[20]
+  // and ev[21]
+  template <class Body>
+  int32_t direct(const Body& body) {
+    CK(pool, cudaEventRecord(pool->ev[20], st));
+    Carve c;
+    c.st = st;
+    body(c);
+    CK(pool, c.err);
+    h2d += c.h2d;
+    CK(pool, cudaEventRecord(pool->ev[21], st));
+    return COOK_OK;
+  }
+  int32_t end() {
+    CK(pool, cudaGetLastError());
+    CK(pool, cudaEventRecord(pool->ev[22], st));
+    CK(pool, cudaStreamSynchronize(st));
+    record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, d2h, nl);
+    return COOK_OK;
+  }
+};
+
 void offers_drop(PoolState* S);
 
 int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
@@ -1221,7 +1305,6 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
       if (rs || !S->run.slot_of.count(id)) return set_err(pool, COOK_E_BADARG, "cook_state_apply: removal of an unknown task id");
     }
   }
-  CK(pool, cudaSetDevice(pool->device));
   cudaStream_t st = pool->stream;
   // ---- the batch is valid: the host side first (slots, counts), all O(delta)
   if (rs) {
@@ -1353,8 +1436,8 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
   memset(&pu, 0, sizeof(pu)); memset(&pr, 0, sizeof(pr)); memset(&ru, 0, sizeof(ru)); memset(&rr, 0, sizeof(rr));
   memset(&uk, 0, sizeof(uk));
   const int nuk = (int)unparked.size();
-  int64_t h2d = 0;
-  const cudaError_t carved = carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
+  StateWrite w(pool, S);
+  if (int32_t rc = w.up([&](Carve& c) {
     if (nuk) {
       uk.c[0] = ScatterCol{reinterpret_cast<char*>(S->park), nullptr, 0, 1};
       uk.nc = 1;
@@ -1401,57 +1484,35 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
       if (c.base && radd) c.copy(RG.v[0] + rtail0, d->running_group_idx, radd);
     }
     if (nrr) rr.slot = c.up(rrm_slot.data(), nrr);
-  });
-  CK(pool, carved);
-  CK(pool, cudaEventRecord(pool->ev[21], st));
-  int nl = 0;
-  scatter(pr, S->pend, npr, 0, P_LIVE, tail0, st, &nl);
-  scatter(rr, S->run, nrr, 0, R_LIVE, &rtail0, st, &nl);
-  scatter(pu, S->pend, np, 1, P_LIVE, tail0, st, &nl);
-  scatter(ru, S->run, nr, 1, R_LIVE, &rtail0, st, &nl);
-  scatter(uk, S->pend, nuk, 0, -1, nullptr, st, &nl);
-  CK(pool, cudaGetLastError());
-  int32_t rc = compact_lists(pool, S, st, &nl);
-  if (rc != COOK_OK) return rc;
-  CK(pool, cudaEventRecord(pool->ev[22], st));
-  CK(pool, cudaStreamSynchronize(st));
-  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
-  return COOK_OK;
-}
-
-// the slots of n distinct live pending job ids, or why not
-const char* pending_slots(const PoolState* S, int n, const int64_t* job_id, std::vector<int32_t>* slot) {
-  std::unordered_set<int64_t> seen;
-  seen.reserve((size_t)n);
-  slot->resize(n);
-  for (int i = 0; i < n; i++) {
-    if (!seen.insert(job_id[i]).second) return "job id twice";
-    auto it = S->pend.slot_of.find(job_id[i]);
-    if (it == S->pend.slot_of.end()) return "unknown job id";
-    (*slot)[i] = it->second;
-  }
-  return nullptr;
+  }))
+    return rc;
+  scatter(pr, S->pend, npr, 0, P_LIVE, tail0, st, &w.nl);
+  scatter(rr, S->run, nrr, 0, R_LIVE, &rtail0, st, &w.nl);
+  scatter(pu, S->pend, np, 1, P_LIVE, tail0, st, &w.nl);
+  scatter(ru, S->run, nr, 1, R_LIVE, &rtail0, st, &w.nl);
+  scatter(uk, S->pend, nuk, 0, -1, nullptr, st, &w.nl);
+  if (int32_t rc = compact_lists(pool, S, st, &w.nl)) return rc;
+  return w.end();
 }
 
 // pending_rm = job_id plus the running upserts built from the rows, without their columns crossing the bus
-int32_t launch(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, const int64_t* task_id,
+int32_t launch(cook_pool* pool, PoolState* S, const char* who, int n, const int64_t* job_id, const int64_t* task_id,
                const int64_t* start_time, const int32_t* hostname_id) {
-  if (n < 0) return set_err(pool, COOK_E_BADARG, "cook_state_launch: n < 0");
+  if (n < 0) return set_err(pool, COOK_E_BADARG, "%s: n < 0", who);
   if (n && (!job_id || !task_id || !start_time))
-    return set_err(pool, COOK_E_BADARG, "cook_state_launch: null job_id, task_id or start_time");
+    return set_err(pool, COOK_E_BADARG, "%s: null job_id, task_id or start_time", who);
   if (!idx_in_range(hostname_id, n, -1, INT32_MAX))
-    return set_err(pool, COOK_E_BADARG, "cook_state_launch: a hostname code below -1");
+    return set_err(pool, COOK_E_BADARG, "%s: a hostname code below -1", who);
   std::vector<int32_t> pslot, rslot(n);
-  if (const char* why = pending_slots(S, n, job_id, &pslot)) return set_err(pool, COOK_E_BADARG, "cook_state_launch: %s", why);
+  if (int32_t rc = live_slots(pool, who, S->pend, "job", n, job_id, &pslot)) return rc;
   {
     std::unordered_set<int64_t> seen;
     seen.reserve((size_t)n);
     for (int i = 0; i < n; i++) {
-      if (!seen.insert(task_id[i]).second) return set_err(pool, COOK_E_BADARG, "cook_state_launch: task id twice");
-      if (S->run.slot_of.count(task_id[i])) return set_err(pool, COOK_E_BADARG, "cook_state_launch: task id already running");
+      if (!seen.insert(task_id[i]).second) return set_err(pool, COOK_E_BADARG, "%s: task id twice", who);
+      if (S->run.slot_of.count(task_id[i])) return set_err(pool, COOK_E_BADARG, "%s: task id already running", who);
     }
   }
-  CK(pool, cudaSetDevice(pool->device));
   cudaStream_t st = pool->stream;
   // ---- host side, in cook_state_apply's order: the removals free their slots, then the tasks take theirs.  A job
   // with retry facts parks its slot instead of freeing it.
@@ -1500,8 +1561,8 @@ int32_t launch(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, cons
   const int32_t *d_pslot = nullptr, *d_rslot = nullptr, *d_host = nullptr, *d_kslot = nullptr, *d_fslot = nullptr;
   const int64_t *d_tid = nullptr, *d_start = nullptr;
   OrderScan<int, 1> os;
-  int64_t h2d = 0;
-  CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
+  StateWrite w(pool, S);
+  if (int32_t rc = w.up([&](Carve& c) {
     if (!n) return;
     d_pslot = c.up(pslot.data(), n); d_rslot = c.up(rslot.data(), n);
     d_tid = c.up(task_id, n); d_start = c.up(start_time, n);
@@ -1511,56 +1572,48 @@ int32_t launch(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, cons
       os.part[0] = c.take<int32_t>(n);
       os.tile[0] = c.take<int32_t>((n + OS_TILE - 1) / OS_TILE + 1);
     }
-  }));
-  CK(pool, cudaEventRecord(pool->ev[21], st));
-  int nl = 0;
+  }))
+    return rc;
   if (n) {
     launch_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_pslot, d_rslot, d_tid, d_start, d_host, S->pend.d_col,
                                                    S->run.d_col, n, rtail0);
-    nl++;
+    w.nl++;
     if (ng) {
       const int32_t* plen = S->pend.at<int32_t>(P_GLEN);
-      order_scan(os, RowLen{d_pslot, plen}, n, S->gf0, st, &nl);
+      order_scan(os, RowLen{d_pslot, plen}, n, S->gf0, st, &w.nl);
       launch_lists_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, d_pslot, d_rslot, n, S->pend.at<int32_t>(P_GOFF), plen,
                                                        S->lists[L_GROUP].v[0], static_cast<int32_t*>(S->run.col[R_GOFF]),
                                                        static_cast<int32_t*>(S->run.col[R_GLEN]), RG.v[0], rtail0);
-      nl++;
+      w.nl++;
     }
     ScatterArgs rm;
     memset(&rm, 0, sizeof(rm));
     rm.slot = nk ? d_fslot : d_pslot;
     int32_t tail[3];
     for (int l = 0; l < 3; l++) tail[l] = (int32_t)S->lists[l].tail;
-    scatter(rm, S->pend, n - nk, 0, P_LIVE, tail, st, &nl);
+    scatter(rm, S->pend, n - nk, 0, P_LIVE, tail, st, &w.nl);
     if (nk) {   // parking: the live flag cleared and the generation bumped as a removal's, the lists kept
       ScatterArgs pk;
       memset(&pk, 0, sizeof(pk));
       pk.c[0] = ScatterCol{reinterpret_cast<char*>(S->park), nullptr, 1, 1};
       pk.nc = 1;
       pk.slot = d_kslot;
-      scatter(pk, S->pend, nk, 0, P_LIVE, nullptr, st, &nl);
+      scatter(pk, S->pend, nk, 0, P_LIVE, nullptr, st, &w.nl);
     }
   }
-  CK(pool, cudaGetLastError());
-  int32_t rc = compact_lists(pool, S, st, &nl);
-  if (rc != COOK_OK) return rc;
-  CK(pool, cudaEventRecord(pool->ev[22], st));
-  CK(pool, cudaStreamSynchronize(st));
-  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
-  return COOK_OK;
+  if (int32_t rc = compact_lists(pool, S, st, &w.nl)) return rc;
+  return w.end();
 }
 
 // the given match-time columns of live pending rows, in place; clear: every reservation is dropped first
-int32_t patch(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, const uint8_t* allowed,
+int32_t patch(cook_pool* pool, PoolState* S, const char* who, int n, const int64_t* job_id, const uint8_t* allowed,
               const uint8_t* plugin_accept, const int32_t* reserved_host, bool clear) {
-  if (n < 0) return set_err(pool, COOK_E_BADARG, "cook_state_patch: n < 0");
-  if (n && !job_id) return set_err(pool, COOK_E_BADARG, "cook_state_patch: null job_id");
+  if (n < 0) return set_err(pool, COOK_E_BADARG, "%s: n < 0", who);
+  if (n && !job_id) return set_err(pool, COOK_E_BADARG, "%s: null job_id", who);
   if (!idx_in_range(reserved_host, n, -1, INT32_MAX))
-    return set_err(pool, COOK_E_BADARG, "cook_state_patch: a reserved_host below -1");
+    return set_err(pool, COOK_E_BADARG, "%s: a reserved_host below -1", who);
   std::vector<int32_t> slot;
-  if (const char* why = pending_slots(S, n, job_id, &slot)) return set_err(pool, COOK_E_BADARG, "cook_state_patch: %s", why);
-  CK(pool, cudaSetDevice(pool->device));
-  cudaStream_t st = pool->stream;
+  if (int32_t rc = live_slots(pool, who, S->pend, "job", n, job_id, &slot)) return rc;
   // ---- host side: the per-slot flags and their counts, O(n + reservations cleared)
   std::vector<int32_t> cleared;
   if (clear) {
@@ -1578,32 +1631,21 @@ int32_t patch(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, const
   const bool cols = n && (allowed || plugin_accept || reserved_host);
   ScatterArgs cl, pa;
   memset(&cl, 0, sizeof(cl)); memset(&pa, 0, sizeof(pa));
-  int64_t h2d = 0;
-  CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
+  StateWrite w(pool, S);
+  if (int32_t rc = w.up([&](Carve& c) {
     if (nc) {
       cl.c[0] = ScatterCol{static_cast<char*>(S->pend.col[P_RESERVED]), nullptr, -1, P_SZ[P_RESERVED]};
       cl.nc = 1;
       cl.slot = c.up(cleared.data(), nc);
     }
-    if (cols) {
-      pa.slot = c.up(slot.data(), n);
-      if (allowed) pa.c[pa.nc++] = ScatterCol{static_cast<char*>(S->pend.col[P_ALLOWED]),
-                                              reinterpret_cast<const char*>(c.up(allowed, n)), 1, 1};
-      if (plugin_accept) pa.c[pa.nc++] = ScatterCol{static_cast<char*>(S->pend.col[P_PLUGIN]),
-                                                    reinterpret_cast<const char*>(c.up(plugin_accept, n)), 1, 1};
-      if (reserved_host) pa.c[pa.nc++] = ScatterCol{static_cast<char*>(S->pend.col[P_RESERVED]),
-                                                    reinterpret_cast<const char*>(c.up(reserved_host, n)), -1, 4};
-    }
-  }));
-  CK(pool, cudaEventRecord(pool->ev[21], st));
-  int nl = 0;
-  scatter(cl, S->pend, nc, 0, -1, nullptr, st, &nl);
-  scatter(pa, S->pend, cols ? n : 0, 0, -1, nullptr, st, &nl);
-  CK(pool, cudaGetLastError());
-  CK(pool, cudaEventRecord(pool->ev[22], st));
-  CK(pool, cudaStreamSynchronize(st));
-  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
-  return COOK_OK;
+    if (cols)
+      patch_args(c, pa, S->pend, slot.data(), n,
+                 {{P_ALLOWED, allowed, 1}, {P_PLUGIN, plugin_accept, 1}, {P_RESERVED, reserved_host, -1}});
+  }))
+    return rc;
+  scatter(cl, S->pend, nc, 0, -1, nullptr, w.st, &w.nl);
+  scatter(pa, S->pend, cols ? n : 0, 0, -1, nullptr, w.st, &w.nl);
+  return w.end();
 }
 
 // ---- the two running-side pipelines.  Each lists its scratch on a carve (take), writes into device
@@ -1869,7 +1911,6 @@ int32_t usage(cook_pool* pool, PoolState* S, int U, double* out_user, double* ou
     pool->phase[COOK_PHASE_USAGE] = cook_phase_stats{};
     return COOK_OK;
   }
-  CK(pool, cudaSetDevice(pool->device));
   cudaStream_t st = pool->stream;
   UsageFold f;
   f.R = R; f.U = users ? U : 0; f.H = hosts ? H : 0; f.pool = out_pool != nullptr;
@@ -2228,9 +2269,8 @@ void offers_drop(PoolState* S) {
   for (auto& l : S->olists) l.tail = l.live = 0;
 }
 
-int32_t offers_add(cook_pool* pool, PoolState* S, const cook_offers_soa* o, const int64_t* id, const uint8_t* single,
-                   const double* gpus, const char* name, const int32_t* name_off, int64_t now_ms) {
-  const char* who = "cook_state_offers_add";
+int32_t offers_add(cook_pool* pool, PoolState* S, const char* who, const cook_offers_soa* o, const int64_t* id,
+                   const uint8_t* single, const double* gpus, const char* name, const int32_t* name_off, int64_t now_ms) {
   if (!o) return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
   const int n = o->n;
   if (n < 0 || o->n_attr_cols < 0) return set_err(pool, COOK_E_BADARG, "%s: bad sizes", who);
@@ -2274,7 +2314,6 @@ int32_t offers_add(cook_pool* pool, PoolState* S, const cook_offers_soa* o, cons
     if (!S->ohost.count(code) && !batch_name.count(code))
       return set_err(pool, COOK_E_BADARG, "%s: a new hostname code without a name", who);
   }
-  CK(pool, cudaSetDevice(pool->device));
   cudaStream_t st = pool->stream;
   // ---- the host side, O(batch)
   for (const auto& kv : batch_name) {
@@ -2324,8 +2363,8 @@ int32_t offers_add(cook_pool* pool, PoolState* S, const cook_offers_soa* o, cons
   }
   ScatterArgs a;
   memset(&a, 0, sizeof(a));
-  int64_t h2d = 0;
-  CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
+  StateWrite w(pool, S);
+  if (int32_t rc = w.up([&](Carve& c) {
     const void* src[O_NDATA] = {o->hostname_id, o->cpus, o->mem, gpus, o->is_k8s, o->location, o->max_tasks,
                                 o->num_tasks, o->host_start_time, seq.data()};
     const long long dflt[O_NDATA] = {0, 0, 0, 0, 0, -1, -1, 0, -1, 0};
@@ -2348,17 +2387,11 @@ int32_t offers_add(cook_pool* pool, PoolState* S, const cook_offers_soa* o, cons
       else if (A.k > 1)
         c.copy(A.v[1] + tail0[l], static_cast<const int32_t*>(lv1[l]), nv[l]);
     }
-  }));
-  CK(pool, cudaEventRecord(pool->ev[21], st));
-  int nl = 0;
-  scatter(a, S->offer, n, 1, O_LIVE, tail0, st, &nl);
-  CK(pool, cudaGetLastError());
-  int32_t rc = compact_lists(pool, S, st, &nl);
-  if (rc != COOK_OK) return rc;
-  CK(pool, cudaEventRecord(pool->ev[22], st));
-  CK(pool, cudaStreamSynchronize(st));
-  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
-  return COOK_OK;
+  }))
+    return rc;
+  scatter(a, S->offer, n, 1, O_LIVE, tail0, st, &w.nl);
+  if (int32_t rc = compact_lists(pool, S, st, &w.nl)) return rc;
+  return w.end();
 }
 
 // step (a) and the plan's offer shape: the offers received incubate_ms or more before now_ms leave, then the VMs are
@@ -2493,42 +2526,33 @@ int32_t offers_spare(cook_pool* pool, PoolState* S, const RebRows& rows, const i
 }  // namespace
 
 extern "C" int32_t cook_state_apply(cook_pool* pool, const cook_state_delta* delta) {
-  if (!pool) return COOK_E_BADARG;
-  if (!delta) return set_err(pool, COOK_E_BADARG, "cook_state_apply: null argument");
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S = state_of(pool, true);
-  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_apply: out of device memory");
-  return apply(pool, S, delta);
+  const char* who = "cook_state_apply";
+  if (pool && !delta) return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
+  return on_state(pool, who, [&](PoolState* S) { return apply(pool, S, delta); });
 }
 
 extern "C" int32_t cook_state_launch(cook_pool* pool, int32_t n, const int64_t* job_id, const int64_t* task_id,
                                      const int64_t* start_time, const int32_t* hostname_id) {
-  if (!pool) return COOK_E_BADARG;
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S = state_of(pool, true);
-  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_launch: out of device memory");
-  return launch(pool, S, n, job_id, task_id, start_time, hostname_id);
+  const char* who = "cook_state_launch";
+  return on_state(pool, who, [&](PoolState* S) { return launch(pool, S, who, n, job_id, task_id, start_time, hostname_id); });
 }
 
 extern "C" int32_t cook_state_patch(cook_pool* pool, int32_t n, const int64_t* job_id, const uint8_t* allowed,
                                     const uint8_t* plugin_accept, const int32_t* reserved_host,
                                     int32_t clear_reservations) {
-  if (!pool) return COOK_E_BADARG;
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S = state_of(pool, true);
-  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_patch: out of device memory");
-  return patch(pool, S, n, job_id, allowed, plugin_accept, reserved_host, clear_reservations != 0);
+  const char* who = "cook_state_patch";
+  return on_state(pool, who, [&](PoolState* S) {
+    return patch(pool, S, who, n, job_id, allowed, plugin_accept, reserved_host, clear_reservations != 0);
+  });
 }
 
 extern "C" int32_t cook_state_usage(cook_pool* pool, int32_t n_users, double* out_user_usage, double* out_pool_usage,
                                     int32_t n_hosts, const int32_t* hostname_id, double* out_run_cpus,
                                     double* out_run_mem, int32_t* out_run_count) {
-  if (!pool) return COOK_E_BADARG;
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S = state_of(pool, true);
-  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_usage: out of device memory");
-  return usage(pool, S, n_users, out_user_usage, out_pool_usage, n_hosts, hostname_id, out_run_cpus, out_run_mem,
-               out_run_count);
+  return on_state(pool, "cook_state_usage", [&](PoolState* S) {
+    return usage(pool, S, n_users, out_user_usage, out_pool_usage, n_hosts, hostname_id, out_run_cpus, out_run_mem,
+                 out_run_count);
+  });
 }
 
 extern "C" int32_t cook_state_cotasks(cook_pool* pool, int32_t n_groups, const int32_t* attr_col,
@@ -3141,6 +3165,42 @@ cook_phase_stats call_stats(const cook_pool* pool, int64_t h2d, int64_t d2h, int
           d2h, nl, 0};
 }
 
+// A read-side call on pools[0]'s stream: open() makes its device current and finds its state (created at the first
+// call: the scratch and counters, even when it holds no row); scratch() carves from that scratch between ev[20] and
+// ev[21]; the call counts its bytes and launches here and records ev[22] after its kernels, before its first
+// download; close() records ev[23], synchronizes and returns the call's own statistics.
+struct ReadCall {
+  cook_pool* pool;
+  PoolState* S = nullptr;
+  cudaStream_t st;
+  int64_t h2d = 0, d2h = 0;
+  int nl = 0;
+  explicit ReadCall(cook_pool* p) : pool(p), st(p->stream) {}
+  int32_t open(const char* who) {
+    CK(pool, cudaSetDevice(pool->device));
+    S = state_of(pool, true);
+    return S ? COOK_OK : set_err(pool, COOK_E_OOM, "%s: out of device memory", who);
+  }
+  template <class Body>
+  int32_t scratch(const Body& body) {
+    CK(pool, carve(S->scratch, st, pool->ev[20], &h2d, body));
+    CK(pool, cudaEventRecord(pool->ev[21], st));
+    return COOK_OK;
+  }
+  int32_t close(cook_phase_stats* out) {
+    CK(pool, cudaEventRecord(pool->ev[23], st));
+    CK(pool, cudaStreamSynchronize(st));
+    if (out) *out = call_stats(pool, h2d, d2h, nl);
+    return COOK_OK;
+  }
+};
+
+// a read-side call with no row to read, its empty outputs written: zeroed statistics, no device work
+int32_t no_rows(cook_phase_stats* out) {
+  if (out) *out = cook_phase_stats{};
+  return COOK_OK;
+}
+
 // cook_state_user_stats: the running and waiting folds per user over the union of the handles' live rows, classified
 int32_t user_stats(cook_pool* const* pools, int n, const cook_user_table* users, const uint8_t* rest_ok,
                    int64_t* out_jobs, double* out_cpus, double* out_mem, uint8_t* out_member, int64_t* out_all_jobs,
@@ -3179,17 +3239,15 @@ int32_t user_stats(cook_pool* const* pools, int n, const cook_user_table* users,
     memset(out_all_cpus, 0, sizeof(double) * 4);
     memset(out_all_mem, 0, sizeof(double) * 4);
     memset(out_users, 0, sizeof(int64_t) * COOK_USERS_N);
-    if (out_stats) *out_stats = cook_phase_stats{};
-    return COOK_OK;
+    return no_rows(out_stats);
   }
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S0 = state_of(pool, true);   // pools[0]'s scratch and counters, even when it holds no row
-  if (!S0) return set_err(pool, COOK_E_OOM, "%s: out of device memory", who);
-  if (S.empty() || S[0] != S0) {   // S[0] owns the counters the compactions write
-    S.insert(S.begin(), S0);
+  ReadCall r(pool);
+  if (int32_t rc = r.open(who)) return rc;
+  if (S.empty() || S[0] != r.S) {   // S[0] owns the counters the compactions write
+    S.insert(S.begin(), r.S);
     P.insert(P.begin(), pool);
   }
-  cudaStream_t st = pool->stream;
+  cudaStream_t st = r.st;
   Gather g(pool);
   // ---- one carve: the two folds, the user columns (uploaded), the per-state columns and the totals
   UsageFold fr, fw;
@@ -3200,8 +3258,7 @@ int32_t user_stats(cook_pool* const* pools, int n, const cook_user_table* users,
   GridFlag* gf = nullptr;
   StatsTotals* tot = nullptr;
   double *run = nullptr, *wait = nullptr;
-  int64_t h2d = 0, d2h = 0;
-  CK(pool, carve(S0->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+  if (int32_t rc = r.scratch([&](Carve& c) {
     if (R) fr.take(c, hw_r);
     if (J) fw.take(c, hw_p);
     run = c.take<double>(4 * (size_t)U); wait = c.take<double>(4 * (size_t)U);
@@ -3212,9 +3269,10 @@ int32_t user_stats(cook_pool* const* pools, int n, const cook_user_table* users,
     a.div_cpus = c.up(ucol[0], U); a.div_mem = c.up(ucol[1], U);
     a.q_count = c.up(ucol[2], U); a.q_cpus = c.up(ucol[3], U); a.q_mem = c.up(ucol[4], U);
     a.rest_ok = c.up(rest_ok, U);
-  }));
-  CK(pool, cudaEventRecord(pool->ev[21], st));
-  int nl = 0;
+  }))
+    return rc;
+  int& nl = r.nl;
+  int64_t& d2h = r.d2h;
   const PoolState* const* list = S.data();
   const int ns = (int)S.size();
   fr.a.user_out = run; fw.a.user_out = wait;
@@ -3236,13 +3294,11 @@ int32_t user_stats(cook_pool* const* pools, int n, const cook_user_table* users,
   CK(pool, download(out_mem, a.mem, 4 * (size_t)U, st, &d2h));
   CK(pool, download(out_member, a.member, U, st, &d2h));
   CK(pool, download(&t, tot, 1, st, &d2h));
-  CK(pool, cudaEventRecord(pool->ev[23], st));
-  CK(pool, cudaStreamSynchronize(st));
+  if (int32_t rc = r.close(out_stats)) return rc;
   memcpy(out_all_jobs, t.jobs, sizeof t.jobs);
   memcpy(out_all_cpus, t.cpus, sizeof t.cpus);
   memcpy(out_all_mem, t.mem, sizeof t.mem);
   memcpy(out_users, t.users, sizeof t.users);
-  if (out_stats) *out_stats = call_stats(pool, h2d, d2h, nl);
   return COOK_OK;
 }
 
@@ -3301,11 +3357,10 @@ extern "C" int32_t cook_state_match_derived(cook_pool* pool, const cook_offers_s
 extern "C" int32_t cook_state_offers_add(cook_pool* pool, const cook_offers_soa* offers, const int64_t* offer_id,
                                          const uint8_t* single_shot, const double* offer_gpus, const char* hostname,
                                          const int32_t* hostname_off, int64_t now_ms) {
-  if (!pool) return COOK_E_BADARG;
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S = state_of(pool, true);
-  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_offers_add: out of device memory");
-  return offers_add(pool, S, offers, offer_id, single_shot, offer_gpus, hostname, hostname_off, now_ms);
+  const char* who = "cook_state_offers_add";
+  return on_state(pool, who, [&](PoolState* S) {
+    return offers_add(pool, S, who, offers, offer_id, single_shot, offer_gpus, hostname, hostname_off, now_ms);
+  });
 }
 
 extern "C" int32_t cook_state_match_offers(cook_pool* pool, int64_t now_ms, int64_t incubate_ms,
@@ -3429,31 +3484,14 @@ int32_t compact_records(cook_pool* pool, PoolState* S, cudaStream_t st, int* nl)
   return COOK_OK;
 }
 
-// the slots of n distinct live running task ids, or why not
-const char* running_slots(const PoolState* S, int n, const int64_t* task_id, std::vector<int32_t>* slot) {
-  std::unordered_set<int64_t> seen;
-  seen.reserve((size_t)n);
-  slot->resize(n);
-  for (int i = 0; i < n; i++) {
-    if (!seen.insert(task_id[i]).second) return "task id twice";
-    auto it = S->run.slot_of.find(task_id[i]);
-    if (it == S->run.slot_of.end()) return "unknown task id";
-    (*slot)[i] = it->second;
-  }
-  return nullptr;
-}
-
-int32_t task_facts(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, const int64_t* max_runtime_ms,
-                   const uint8_t* cancelled, const uint8_t* unknown) {
-  const char* who = "cook_state_task_facts";
+int32_t task_facts(cook_pool* pool, PoolState* S, const char* who, int n, const int64_t* task_id,
+                   const int64_t* max_runtime_ms, const uint8_t* cancelled, const uint8_t* unknown) {
   if (n < 0) return set_err(pool, COOK_E_BADARG, "%s: n < 0", who);
   if (n && !task_id) return set_err(pool, COOK_E_BADARG, "%s: null task_id", who);
   for (int i = 0; max_runtime_ms && i < n; i++)
     if (max_runtime_ms[i] < -1) return set_err(pool, COOK_E_BADARG, "%s: a max_runtime_ms below -1", who);
   std::vector<int32_t> slot;
-  if (const char* why = running_slots(S, n, task_id, &slot)) return set_err(pool, COOK_E_BADARG, "%s: %s", who, why);
-  CK(pool, cudaSetDevice(pool->device));
-  cudaStream_t st = pool->stream;
+  if (int32_t rc = live_slots(pool, who, S->run, "task", n, task_id, &slot)) return rc;
   // ---- host side: each row's bits, the given ones replaced
   const bool bits = cancelled || unknown;
   std::vector<uint8_t> facts(bits ? n : 0);
@@ -3467,53 +3505,34 @@ int32_t task_facts(cook_pool* pool, PoolState* S, int n, const int64_t* task_id,
   const bool cols = n && (max_runtime_ms || bits);
   ScatterArgs pa;
   memset(&pa, 0, sizeof(pa));
-  int64_t h2d = 0;
-  CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
-    if (!cols) return;
-    pa.slot = c.up(slot.data(), n);
-    if (max_runtime_ms) pa.c[pa.nc++] = ScatterCol{static_cast<char*>(S->run.col[R_MAXRT]),
-                                                   reinterpret_cast<const char*>(c.up(max_runtime_ms, n)), -1, 8};
-    if (bits) pa.c[pa.nc++] = ScatterCol{static_cast<char*>(S->run.col[R_FACTS]),
-                                         reinterpret_cast<const char*>(c.up(facts.data(), n)), 0, 1};
-  }));
-  CK(pool, cudaEventRecord(pool->ev[21], st));
-  int nl = 0;
-  scatter(pa, S->run, cols ? n : 0, 0, -1, nullptr, st, &nl);
-  CK(pool, cudaGetLastError());
-  CK(pool, cudaEventRecord(pool->ev[22], st));
-  CK(pool, cudaStreamSynchronize(st));
-  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
-  return COOK_OK;
+  StateWrite w(pool, S);
+  if (int32_t rc = w.up([&](Carve& c) {
+    if (cols)
+      patch_args(c, pa, S->run, slot.data(), n, {{R_MAXRT, max_runtime_ms, -1}, {R_FACTS, bits ? facts.data() : nullptr, 0}});
+  }))
+    return rc;
+  scatter(pa, S->run, cols ? n : 0, 0, -1, nullptr, w.st, &w.nl);
+  return w.end();
 }
 
 // the reason code of each listed live running row, in place (live flag and generation kept)
-int32_t task_reason(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, const int32_t* reason_code) {
-  const char* who = "cook_state_task_reason";
+int32_t task_reason(cook_pool* pool, PoolState* S, const char* who, int n, const int64_t* task_id,
+                    const int32_t* reason_code) {
   if (n < 0) return set_err(pool, COOK_E_BADARG, "%s: n < 0", who);
   if (n && (!task_id || !reason_code)) return set_err(pool, COOK_E_BADARG, "%s: null task_id or reason_code", who);
   if (!idx_in_range(reason_code, n, -1, INT32_MAX)) return set_err(pool, COOK_E_BADARG, "%s: a reason code below -1", who);
   std::vector<int32_t> slot;
-  if (const char* why = running_slots(S, n, task_id, &slot)) return set_err(pool, COOK_E_BADARG, "%s: %s", who, why);
-  CK(pool, cudaSetDevice(pool->device));
-  cudaStream_t st = pool->stream;
+  if (int32_t rc = live_slots(pool, who, S->run, "task", n, task_id, &slot)) return rc;
   for (int i = 0; i < n; i++) S->rreason[slot[i]] = reason_code[i];   // cook_state_status decides from it
   ScatterArgs pa;
   memset(&pa, 0, sizeof(pa));
-  int64_t h2d = 0;
-  CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
-    if (!n) return;
-    pa.slot = c.up(slot.data(), n);
-    pa.c[pa.nc++] = ScatterCol{static_cast<char*>(S->run.col[R_REASON]),
-                               reinterpret_cast<const char*>(c.up(reason_code, n)), -1, 4};
-  }));
-  CK(pool, cudaEventRecord(pool->ev[21], st));
-  int nl = 0;
-  scatter(pa, S->run, n, 0, -1, nullptr, st, &nl);
-  CK(pool, cudaGetLastError());
-  CK(pool, cudaEventRecord(pool->ev[22], st));
-  CK(pool, cudaStreamSynchronize(st));
-  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
-  return COOK_OK;
+  StateWrite w(pool, S);
+  if (int32_t rc = w.up([&](Carve& c) {
+    if (n) patch_args(c, pa, S->run, slot.data(), n, {{R_REASON, reason_code, -1}});
+  }))
+    return rc;
+  scatter(pa, S->run, n, 0, -1, nullptr, w.st, &w.nl);
+  return w.end();
 }
 
 // What cook_state_finish_history adds to cook_state_finish: the rows' reason codes (NULL: each row's reason fact).
@@ -3523,9 +3542,8 @@ struct FinishStatus { const uint8_t* preempted; int32_t* outcome; int32_t* attem
 
 // running_rm_task_id = task_id, plus one record per group of each successful row; with `fh`, the rows that start at
 // or after the horizon of an enabled history are also appended to it
-int32_t finish(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, const int64_t* end_time_ms,
+int32_t finish(cook_pool* pool, PoolState* S, const char* who, int n, const int64_t* task_id, const int64_t* end_time_ms,
                const uint8_t* success, const FinishHistory* fh = nullptr, const FinishStatus* fs = nullptr) {
-  const char* who = fs ? "cook_state_status" : fh ? "cook_state_finish_history" : "cook_state_finish";
   if (n < 0) return set_err(pool, COOK_E_BADARG, "%s: n < 0", who);
   if (fs && n && (!fs->outcome || !fs->attempts)) return set_err(pool, COOK_E_BADARG, "%s: null out_outcome or out_attempts", who);
   if (n && !task_id) return set_err(pool, COOK_E_BADARG, "%s: null task_id", who);
@@ -3534,7 +3552,7 @@ int32_t finish(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, con
   if (fh && !idx_in_range(fh->reason_code, n, -1, INT32_MAX))
     return set_err(pool, COOK_E_BADARG, "%s: a reason code below -1", who);
   std::vector<int32_t> slot;
-  if (const char* why = running_slots(S, n, task_id, &slot)) return set_err(pool, COOK_E_BADARG, "%s: %s", who, why);
+  if (int32_t rc = live_slots(pool, who, S->run, "task", n, task_id, &slot)) return rc;
   History& H = S->hist;
   int64_t nhist = 0;   // the rows the history appends
   for (int i = 0; fh && i < n; i++) {
@@ -3552,7 +3570,6 @@ int32_t finish(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, con
     nrec += (int64_t)S->rgroups[s].size();
   }
   if (S->rec.tail + nrec > INT32_MAX) return set_err(pool, COOK_E_TOO_LARGE, "%s: more than 2^31 - 1 records", who);
-  CK(pool, cudaSetDevice(pool->device));
   cudaStream_t st = pool->stream;
   // ---- host side: cook_state_apply's removals, then the records' counts.  With retry facts, in batch order: the
   // status's job decision (cook_state_status) or, for a job's last live instance, its parked copy freed.
@@ -3644,8 +3661,8 @@ int32_t finish(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, con
   OrderScan<int, 1> os, aos;
   ScatterArgs rq, uk;
   memset(&rq, 0, sizeof(rq)); memset(&uk, 0, sizeof(uk));
-  int64_t h2d = 0;
-  CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
+  StateWrite w(pool, S);
+  if (int32_t rc = w.up([&](Carve& c) {
     if (!n) return;
     if (nrq) {   // live again with a new generation, reserved_host -1, no job facts, no longer parked
       rq.nc = 0;   // carve runs this body twice: once to size, once to upload
@@ -3675,9 +3692,9 @@ int32_t finish(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, con
       d_reason = c.up(fh->reason_code, n);
       hblk = c.take<int32_t>((size_t)n / CP_BLOCK + 2);
     }
-  }));
-  CK(pool, cudaEventRecord(pool->ev[21], st));
-  int nl = 0;
+  }))
+    return rc;
+  int& nl = w.nl;
   if (nrec) {
     order_scan(os, FinishLen{d_slot, d_ok, S->run.at<int32_t>(R_GLEN)}, n, S->gf0, st, &nl);
     finish_records_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, d_slot, d_ok, d_end, n, S->run.d_col,
@@ -3702,20 +3719,14 @@ int32_t finish(cook_pool* pool, PoolState* S, int n, const int64_t* task_id, con
   }
   scatter(rq, S->pend, nrq, 1, P_LIVE, nullptr, st, &nl);
   scatter(uk, S->pend, nuk, 0, -1, nullptr, st, &nl);
-  CK(pool, cudaGetLastError());
   int32_t rc = compact_lists(pool, S, st, &nl);
   if (rc == COOK_OK) rc = compact_records(pool, S, st, &nl);
-  if (rc != COOK_OK) return rc;
-  CK(pool, cudaEventRecord(pool->ev[22], st));
-  CK(pool, cudaStreamSynchronize(st));
-  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
-  return COOK_OK;
+  return rc != COOK_OK ? rc : w.end();
 }
 
 // the reason dictionary and the global mea-culpa limit; host only
-int32_t retry_config(cook_pool* pool, PoolState* S, int32_t mea_culpa_limit, int n, const int32_t* reason_code,
-                     const uint8_t* mea_culpa, const int32_t* failure_limit) {
-  const char* who = "cook_state_retry_config";
+int32_t retry_config(cook_pool* pool, PoolState* S, const char* who, int32_t mea_culpa_limit, int n,
+                     const int32_t* reason_code, const uint8_t* mea_culpa, const int32_t* failure_limit) {
   if (n < 0) return set_err(pool, COOK_E_BADARG, "%s: n_reasons < 0", who);
   if (n && (!reason_code || !mea_culpa || !failure_limit)) return set_err(pool, COOK_E_BADARG, "%s: null array", who);
   if (mea_culpa_limit < -1) return set_err(pool, COOK_E_BADARG, "%s: a mea_culpa_limit below -1", who);
@@ -3733,9 +3744,8 @@ int32_t retry_config(cook_pool* pool, PoolState* S, int32_t mea_culpa_limit, int
 }
 
 // the retry facts of jobs the handle holds (a live pending row, a parked copy or a live running instance)
-int32_t retry_facts(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, const int32_t* max_retries,
-                    const uint8_t* flags, const int32_t* done_off, const int32_t* done_reason) {
-  const char* who = "cook_state_retry_facts";
+int32_t retry_facts(cook_pool* pool, PoolState* S, const char* who, int n, const int64_t* job_id,
+                    const int32_t* max_retries, const uint8_t* flags, const int32_t* done_off, const int32_t* done_reason) {
   if (n < 0) return set_err(pool, COOK_E_BADARG, "%s: n < 0", who);
   if (n && (!job_id || !max_retries || !flags)) return set_err(pool, COOK_E_BADARG, "%s: null job_id, max_retries or flags", who);
   if (!csr_ok(done_off, n, done_reason, nullptr, false)) return set_err(pool, COOK_E_BADARG, "%s: malformed CSR offsets", who);
@@ -3752,8 +3762,6 @@ int32_t retry_facts(cook_pool* pool, PoolState* S, int n, const int64_t* job_id,
         return set_err(pool, COOK_E_BADARG, "%s: unknown job id", who);
     }
   }
-  CK(pool, cudaSetDevice(pool->device));
-  cudaStream_t st = pool->stream;
   // ---- host side: the facts replaced; a completed job without a live instance loses its parked copy and its facts
   std::vector<int32_t> unparked;
   for (int i = 0; i < n; i++) {
@@ -3773,30 +3781,24 @@ int32_t retry_facts(cook_pool* pool, PoolState* S, int n, const int64_t* job_id,
   const int nuk = (int)unparked.size();
   ScatterArgs uk;
   memset(&uk, 0, sizeof(uk));
-  int64_t h2d = 0;
-  CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
+  StateWrite w(pool, S);
+  if (int32_t rc = w.up([&](Carve& c) {
     if (!nuk) return;
     uk.c[0] = ScatterCol{reinterpret_cast<char*>(S->park), nullptr, 0, 1};
     uk.nc = 1;
     uk.slot = c.up(unparked.data(), nuk);
-  }));
-  CK(pool, cudaEventRecord(pool->ev[21], st));
-  int nl = 0;
-  scatter(uk, S->pend, nuk, 0, -1, nullptr, st, &nl);
-  CK(pool, cudaGetLastError());
-  CK(pool, cudaEventRecord(pool->ev[22], st));
-  CK(pool, cudaStreamSynchronize(st));
-  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
-  return COOK_OK;
+  }))
+    return rc;
+  scatter(uk, S->pend, nuk, 0, -1, nullptr, w.st, &w.nl);
+  return w.end();
 }
 
 bool bad_amount(double x) { return !std::isfinite(x) || x < 0 || std::signbit(x); }
 
 // the history replaced by n rows at horizon since_ms, and on; the rows are copied straight into the table's columns
-int32_t history_seed(cook_pool* pool, PoolState* S, int64_t since_ms, int n, const int64_t* task_id,
+int32_t history_seed(cook_pool* pool, PoolState* S, const char* who, int64_t since_ms, int n, const int64_t* task_id,
                      const int32_t* user, const int64_t* start_ms, const int64_t* end_ms, const double* cpus,
                      const double* mem, const uint8_t* success, const int32_t* reason_code) {
-  const char* who = "cook_state_history_seed";
   if (n < 0) return set_err(pool, COOK_E_BADARG, "%s: n < 0", who);
   if (n && (!task_id || !user || !start_ms || !end_ms || !cpus || !mem || !success || !reason_code))
     return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
@@ -3812,29 +3814,20 @@ int32_t history_seed(cook_pool* pool, PoolState* S, int64_t since_ms, int n, con
     if (!seen.insert(task_id[i]).second) return set_err(pool, COOK_E_BADARG, "%s: task id twice", who);
     if (S->run.slot_of.count(task_id[i])) return set_err(pool, COOK_E_BADARG, "%s: a live running task id", who);
   }
-  CK(pool, cudaSetDevice(pool->device));
-  cudaStream_t st = pool->stream;
   History& H = S->hist;
   H.tail = 0;
   H.since = since_ms;
   H.on = true;
-  CK(pool, H.grow(n, st));
+  CK(pool, H.grow(n, pool->stream));
   H.tail = n;
-  // straight into the table's columns: no staging buffer
-  CK(pool, cudaEventRecord(pool->ev[20], st));
-  Carve c;   // only its copy(): the bytes counted, the first error kept
-  c.st = st;
-  if (n) {
+  StateWrite w(pool, S);
+  if (int32_t rc = w.direct([&](Carve& c) {
+    if (!n) return;
     c.copy(H.c.tid, task_id, n); c.copy(H.c.user, user, n); c.copy(H.c.start, start_ms, n); c.copy(H.c.end, end_ms, n);
     c.copy(H.c.cpus, cpus, n); c.copy(H.c.mem, mem, n); c.copy(H.c.ok, success, n); c.copy(H.c.reason, reason_code, n);
-  }
-  CK(pool, c.err);
-  const int64_t h2d = c.h2d;
-  CK(pool, cudaEventRecord(pool->ev[21], st));
-  CK(pool, cudaEventRecord(pool->ev[22], st));
-  CK(pool, cudaStreamSynchronize(st));
-  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, 0);
-  return COOK_OK;
+  }))
+    return rc;
+  return w.end();
 }
 
 struct HistKeep {   // the advance's compaction: the rows that start at or after the new horizon, in order
@@ -3847,45 +3840,37 @@ struct HistKeep {   // the advance's compaction: the rows that start at or after
 };
 
 // the horizon raised to since_ms: the rows that start before it leave in one compaction into new columns
-int32_t history_advance(cook_pool* pool, PoolState* S, int64_t since_ms) {
-  const char* who = "cook_state_history_advance";
+int32_t history_advance(cook_pool* pool, PoolState* S, const char* who, int64_t since_ms) {
   History& H = S->hist;
   if (!H.on) return set_err(pool, COOK_E_BADARG, "%s: history is off", who);
   if (since_ms < H.since) return set_err(pool, COOK_E_BADARG, "%s: since_ms below the horizon", who);
-  CK(pool, cudaSetDevice(pool->device));
-  cudaStream_t st = pool->stream;
   int32_t* blk = nullptr;
   const int T = (int)H.tail;
-  CK(pool, carve(S->scratch, st, pool->ev[20], nullptr, [&](Carve& c) {
+  StateWrite w(pool, S);
+  if (int32_t rc = w.up(S->scratch, [&](Carve& c) {
     if (T && since_ms > H.since) blk = c.take<int32_t>((size_t)T / CP_BLOCK + 2);
-  }));
-  CK(pool, cudaEventRecord(pool->ev[21], st));
-  int nl = 0;
-  int64_t d2h = 0;
+  }))
+    return rc;
   if (T && since_ms > H.since) {
     HistCols nc;
     CK(pool, nc.alloc(H.cap));
-    compact(HistKeep{H.c, nc, since_ms}, T, nullptr, blk, S->counters + 7, T, st, &nl);
+    compact(HistKeep{H.c, nc, since_ms}, T, nullptr, blk, S->counters + 7, T, w.st, &w.nl);
     int32_t kept = 0;
     cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = download(&kept, S->counters + 7, 1, st, &d2h);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e == cudaSuccess) e = download(&kept, S->counters + 7, 1, w.st, &w.d2h);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(w.st);
     if (e != cudaSuccess) { nc.free_all(); CK(pool, e); }
     H.c.free_all();
     H.c = nc;
     H.tail = kept;
   }
   H.since = since_ms;
-  CK(pool, cudaEventRecord(pool->ev[22], st));
-  CK(pool, cudaStreamSynchronize(st));
-  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], 0, d2h, nl);
-  return COOK_OK;
+  return w.end();
 }
 
 // the records of the forgotten groups leave, then the seeds are appended
-int32_t group_runtimes(cook_pool* pool, PoolState* S, int n_add, const int32_t* group, const int32_t* runtime_s,
-                       int n_forget, const int32_t* forget_group) {
-  const char* who = "cook_state_group_runtimes";
+int32_t group_runtimes(cook_pool* pool, PoolState* S, const char* who, int n_add, const int32_t* group,
+                       const int32_t* runtime_s, int n_forget, const int32_t* forget_group) {
   if (n_add < 0 || n_forget < 0) return set_err(pool, COOK_E_BADARG, "%s: a negative size", who);
   if ((n_add && (!group || !runtime_s)) || (n_forget && !forget_group))
     return set_err(pool, COOK_E_BADARG, "%s: null argument", who);
@@ -3894,7 +3879,6 @@ int32_t group_runtimes(cook_pool* pool, PoolState* S, int n_add, const int32_t* 
   if (!idx_in_range(runtime_s, n_add, 0, INT32_MAX)) return set_err(pool, COOK_E_BADARG, "%s: a negative runtime", who);
   Records& RC = S->rec;
   if (RC.tail + n_add > INT32_MAX) return set_err(pool, COOK_E_TOO_LARGE, "%s: more than 2^31 - 1 records", who);
-  CK(pool, cudaSetDevice(pool->device));
   cudaStream_t st = pool->stream;
   // ---- host side
   std::vector<int32_t> forget(forget_group, forget_group + n_forget);
@@ -3912,30 +3896,24 @@ int32_t group_runtimes(cook_pool* pool, PoolState* S, int n_add, const int32_t* 
   CK(pool, RC.grow(RC.tail + n_add, st));
   const int nf = (int)forget.size();
   const int32_t* d_forget = nullptr;
-  int64_t h2d = 0;
-  CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
+  StateWrite w(pool, S);
+  if (int32_t rc = w.up([&](Carve& c) {
     if (nf) d_forget = c.up(forget.data(), nf);
     if (c.base && n_add) {
       c.copy(RC.grp + tail0, group, n_add);
       c.copy(RC.rt + tail0, runtime_s, n_add);
     }
-  }));
-  CK(pool, cudaEventRecord(pool->ev[21], st));
-  int nl = 0;
+  }))
+    return rc;
   if (nf && tail0) {
     forget_records_kernel<<<(tail0 + 255) / 256, 256, 0, st>>>(RC.grp, RC.live, tail0, d_forget, nf);
-    nl++;
+    w.nl++;
   }
   if (n_add) CK(pool, cudaMemsetAsync(RC.live + tail0, 1, (size_t)n_add, st));
   RC.tail += n_add;
   RC.n_live += n_add;
-  CK(pool, cudaGetLastError());
-  int32_t rc = compact_records(pool, S, st, &nl);
-  if (rc != COOK_OK) return rc;
-  CK(pool, cudaEventRecord(pool->ev[22], st));
-  CK(pool, cudaStreamSynchronize(st));
-  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
-  return COOK_OK;
+  if (int32_t rc = compact_records(pool, S, st, &w.nl)) return rc;
+  return w.end();
 }
 
 // ---- cook_state_sweep
@@ -4078,13 +4056,11 @@ int32_t sweep(cook_pool* const* pools, int n, int64_t now, int64_t dflt, int64_t
     if (linger) *l_n = 0;
     if (cancel) *c_n = 0;
     if (strag) *s_n = 0;
-    if (out_stats) *out_stats = cook_phase_stats{};
-    return COOK_OK;
+    return no_rows(out_stats);
   }
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S0 = state_of(pool, true);   // pools[0]'s scratch, even when it holds no row
-  if (!S0) return set_err(pool, COOK_E_OOM, "%s: out of device memory", who);
-  cudaStream_t st = pool->stream;
+  ReadCall r(pool);
+  if (int32_t rc = r.open(who)) return rc;
+  cudaStream_t st = r.st;
   hw = std::max({hw, (int)R, (int)N});
   // ---- one carve
   int32_t *cnt = nullptr, *blk = nullptr, *ord = nullptr, *tmp = nullptr, *pidx = nullptr;
@@ -4100,8 +4076,7 @@ int32_t sweep(cook_pool* const* pools, int n, int64_t now, int64_t dflt, int64_t
   OrderScan<int, 1> os;
   int32_t *e_grp = nullptr, *e_pool = nullptr, *e_ord = nullptr, *e_tmp = nullptr;
   int64_t *e_tid = nullptr, *e_rt = nullptr;
-  int64_t h2d = 0, d2h = 0;
-  CK(pool, carve(S0->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+  if (int32_t rc = r.scratch([&](Carve& c) {
     cnt = c.take<int32_t>(5);   // lingering, cancelled, stragglers, start after now, the compactions' own
     blk = c.take<int32_t>((size_t)hw / CP_BLOCK + 2);
     if (rows) {
@@ -4121,10 +4096,11 @@ int32_t sweep(cook_pool* const* pools, int n, int64_t now, int64_t dflt, int64_t
       e_ord = c.take<int32_t>(N); e_tmp = c.take<int32_t>(N);
       o_sgrp = c.take<int32_t>(N); o_stid = c.take<int64_t>(N); o_spool = c.take<int32_t>(N);
     }
-  }));
-  CK(pool, cudaEventRecord(pool->ev[21], st));
+  }))
+    return rc;
   CK(pool, cudaMemsetAsync(cnt, 0, sizeof(int32_t) * 5, st));
-  int nl = 0;
+  int& nl = r.nl;
+  int64_t& d2h = r.d2h;
   if (rows) {
     int base = 0;
     for (const auto& h : hs) {
@@ -4174,7 +4150,7 @@ int32_t sweep(cook_pool* const* pools, int n, int64_t now, int64_t dflt, int64_t
       if (!Kk) continue;
       const int32_t* glen = s->run.at<int32_t>(R_GLEN);
       compact(GroupedRows{s->run.at<uint8_t>(R_LIVE), glen, slot + kbase}, s->run.hw, nullptr, blk, cnt + 4, Kk, st, &nl);
-      order_scan(os, RowLen{slot + kbase, glen}, Kk, S0->gf0, st, &nl);
+      order_scan(os, RowLen{slot + kbase, glen}, Kk, r.S->gf0, st, &nl);
       ExpandArgs a = {os, slot + kbase, Kk, ebase, h.second, s->run.d_col, s->lists[L_RGROUP].v[0], d_kind, now,
                       e_grp, e_tid, e_pool, e_rt, cnt + 3};
       straggler_expand_kernel<<<(Kk + 255) / 256, 256, 0, st>>>(a);
@@ -4205,12 +4181,10 @@ int32_t sweep(cook_pool* const* pools, int n, int64_t now, int64_t dflt, int64_t
     CK(pool, download(s_tid, o_stid, got[2], st, &d2h));
     CK(pool, download(s_pool, o_spool, got[2], st, &d2h));
   }
-  CK(pool, cudaEventRecord(pool->ev[23], st));
-  CK(pool, cudaStreamSynchronize(st));
+  if (int32_t rc = r.close(out_stats)) return rc;
   if (linger) *l_n = got[0];
   if (cancel) *c_n = got[1];
   if (strag) *s_n = got[2];
-  if (out_stats) *out_stats = call_stats(pool, h2d, d2h, nl);
   return COOK_OK;
 }
 
@@ -4219,99 +4193,81 @@ int32_t sweep(cook_pool* const* pools, int n, int64_t now, int64_t dflt, int64_t
 extern "C" int32_t cook_state_task_facts(cook_pool* pool, int32_t n, const int64_t* task_id,
                                          const int64_t* max_runtime_ms, const uint8_t* cancelled,
                                          const uint8_t* unknown) {
-  if (!pool) return COOK_E_BADARG;
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S = state_of(pool, true);
-  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_task_facts: out of device memory");
-  return task_facts(pool, S, n, task_id, max_runtime_ms, cancelled, unknown);
+  const char* who = "cook_state_task_facts";
+  return on_state(pool, who, [&](PoolState* S) {
+    return task_facts(pool, S, who, n, task_id, max_runtime_ms, cancelled, unknown);
+  });
 }
 
 extern "C" int32_t cook_state_task_reason(cook_pool* pool, int32_t n, const int64_t* task_id,
                                           const int32_t* reason_code) {
-  if (!pool) return COOK_E_BADARG;
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S = state_of(pool, true);
-  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_task_reason: out of device memory");
-  return task_reason(pool, S, n, task_id, reason_code);
+  const char* who = "cook_state_task_reason";
+  return on_state(pool, who, [&](PoolState* S) { return task_reason(pool, S, who, n, task_id, reason_code); });
 }
 
 extern "C" int32_t cook_state_finish(cook_pool* pool, int32_t n, const int64_t* task_id, const int64_t* end_time_ms,
                                      const uint8_t* success) {
-  if (!pool) return COOK_E_BADARG;
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S = state_of(pool, true);
-  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_finish: out of device memory");
-  return finish(pool, S, n, task_id, end_time_ms, success);
+  const char* who = "cook_state_finish";
+  return on_state(pool, who, [&](PoolState* S) { return finish(pool, S, who, n, task_id, end_time_ms, success); });
 }
 
 extern "C" int32_t cook_state_finish_history(cook_pool* pool, int32_t n, const int64_t* task_id,
                                              const int64_t* end_time_ms, const uint8_t* success,
                                              const int32_t* reason_code) {
-  if (!pool) return COOK_E_BADARG;
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S = state_of(pool, true);
-  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_finish_history: out of device memory");
+  const char* who = "cook_state_finish_history";
   const FinishHistory fh{reason_code};
-  return finish(pool, S, n, task_id, end_time_ms, success, &fh);
+  return on_state(pool, who, [&](PoolState* S) { return finish(pool, S, who, n, task_id, end_time_ms, success, &fh); });
 }
 
 extern "C" int32_t cook_state_retry_config(cook_pool* pool, int32_t mea_culpa_limit, int32_t n_reasons,
                                            const int32_t* reason_code, const uint8_t* mea_culpa,
                                            const int32_t* failure_limit) {
-  if (!pool) return COOK_E_BADARG;
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S = state_of(pool, true);
-  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_retry_config: out of device memory");
-  return retry_config(pool, S, mea_culpa_limit, n_reasons, reason_code, mea_culpa, failure_limit);
+  const char* who = "cook_state_retry_config";
+  return on_state(pool, who, [&](PoolState* S) {
+    return retry_config(pool, S, who, mea_culpa_limit, n_reasons, reason_code, mea_culpa, failure_limit);
+  });
 }
 
 extern "C" int32_t cook_state_retry_facts(cook_pool* pool, int32_t n, const int64_t* job_id, const int32_t* max_retries,
                                           const uint8_t* flags, const int32_t* done_off, const int32_t* done_reason) {
-  if (!pool) return COOK_E_BADARG;
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S = state_of(pool, true);
-  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_retry_facts: out of device memory");
-  return retry_facts(pool, S, n, job_id, max_retries, flags, done_off, done_reason);
+  const char* who = "cook_state_retry_facts";
+  return on_state(pool, who, [&](PoolState* S) {
+    return retry_facts(pool, S, who, n, job_id, max_retries, flags, done_off, done_reason);
+  });
 }
 
 extern "C" int32_t cook_state_status(cook_pool* pool, int32_t n, const int64_t* task_id, const uint8_t* success,
                                      const int64_t* end_time_ms, const int32_t* reason_code, const uint8_t* preempted,
                                      int32_t* out_outcome, int32_t* out_attempts) {
-  if (!pool) return COOK_E_BADARG;
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S = state_of(pool, true);
-  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_status: out of device memory");
+  const char* who = "cook_state_status";
   const FinishHistory fh{reason_code};
   const FinishStatus fs{preempted, out_outcome, out_attempts};
-  return finish(pool, S, n, task_id, end_time_ms, success, &fh, &fs);
+  return on_state(pool, who, [&](PoolState* S) {
+    return finish(pool, S, who, n, task_id, end_time_ms, success, &fh, &fs);
+  });
 }
 
 extern "C" int32_t cook_state_history_seed(cook_pool* pool, int64_t since_ms, int32_t n, const int64_t* task_id,
                                            const int32_t* user, const int64_t* start_ms, const int64_t* end_ms,
                                            const double* cpus, const double* mem, const uint8_t* success,
                                            const int32_t* reason_code) {
-  if (!pool) return COOK_E_BADARG;
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S = state_of(pool, true);
-  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_history_seed: out of device memory");
-  return history_seed(pool, S, since_ms, n, task_id, user, start_ms, end_ms, cpus, mem, success, reason_code);
+  const char* who = "cook_state_history_seed";
+  return on_state(pool, who, [&](PoolState* S) {
+    return history_seed(pool, S, who, since_ms, n, task_id, user, start_ms, end_ms, cpus, mem, success, reason_code);
+  });
 }
 
 extern "C" int32_t cook_state_history_advance(cook_pool* pool, int64_t since_ms) {
-  if (!pool) return COOK_E_BADARG;
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S = state_of(pool, true);
-  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_history_advance: out of device memory");
-  return history_advance(pool, S, since_ms);
+  const char* who = "cook_state_history_advance";
+  return on_state(pool, who, [&](PoolState* S) { return history_advance(pool, S, who, since_ms); });
 }
 
 extern "C" int32_t cook_state_group_runtimes(cook_pool* pool, int32_t n_add, const int32_t* group,
                                              const int32_t* runtime_s, int32_t n_forget, const int32_t* forget_group) {
-  if (!pool) return COOK_E_BADARG;
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S = state_of(pool, true);
-  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_group_runtimes: out of device memory");
-  return group_runtimes(pool, S, n_add, group, runtime_s, n_forget, forget_group);
+  const char* who = "cook_state_group_runtimes";
+  return on_state(pool, who, [&](PoolState* S) {
+    return group_runtimes(pool, S, who, n_add, group, runtime_s, n_forget, forget_group);
+  });
 }
 
 extern "C" int32_t cook_state_sweep(cook_pool* const* pools, int32_t n_pools, int64_t now_ms,
@@ -4501,8 +4457,7 @@ int32_t unscheduled(cook_pool* pool, int n, const int64_t* job_id, uint8_t* out_
     memset(out_n_ahead, 0, sizeof(int32_t) * (size_t)n);
     memset(out_ahead, 0, sizeof(int64_t) * COOK_UNSCHED_AHEAD * (size_t)n);
     memset(out_plugin, 0, (size_t)n);
-    if (out_stats) *out_stats = cook_phase_stats{};
-    return COOK_OK;
+    return no_rows(out_stats);
   }
   int R = 0, J = 0;
   for (int32_t u : quser) {
@@ -4513,8 +4468,9 @@ int32_t unscheduled(cook_pool* pool, int n, const int64_t* job_id, uint8_t* out_
   }
   const int E = R + J;
   const int n_codes = std::max(count_max(S->users_p), count_max(S->users_r)) + 1;
-  CK(pool, cudaSetDevice(pool->device));
-  cudaStream_t st = pool->stream;
+  ReadCall rd(pool);
+  if (int32_t rc = rd.open(who)) return rc;   // S: the handle holds the queried rows
+  cudaStream_t st = rd.st;
   // ---- one carve: the maps, the entries, the three orders, the fold, the outputs; up the users and the query keys
   UnschedCols o = {};
   int32_t *umap = nullptr, *rank = nullptr, *blk = nullptr, *cnt = nullptr, *ord1 = nullptr, *ord3 = nullptr;
@@ -4524,8 +4480,7 @@ int32_t unscheduled(cook_pool* pool, int n, const int64_t* job_id, uint8_t* out_
   f.R = R; f.U = nU;
   UnschedArgs a = {};
   const int hw = std::max(S->run.hw, S->pend.hw);
-  int64_t h2d = 0, d2h = 0;
-  CK(pool, carve(S->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+  if (int32_t rc = rd.scratch([&](Carve& c) {
     umap = c.take<int32_t>(n_codes); rank = c.take<int32_t>(nU + 1);
     blk = c.take<int32_t>((size_t)hw / CP_BLOCK + 2); cnt = c.take<int32_t>(2);
     o.key = c.take<int32_t>(E); o.prio = c.take<int32_t>(E); o.start = c.take<int64_t>(E);
@@ -4545,9 +4500,10 @@ int32_t unscheduled(cook_pool* pool, int n, const int64_t* job_id, uint8_t* out_
     a.ahead = c.take<int64_t>(COOK_UNSCHED_AHEAD * (size_t)n); a.plugin = c.take<uint8_t>(n);
     d_quser = c.up(quser.data(), nU);
     d_qkey = c.up(qkey.data(), n);
-  }));
-  CK(pool, cudaEventRecord(pool->ev[21], st));
-  int nl = 0;
+  }))
+    return rc;
+  int& nl = rd.nl;
+  int64_t& d2h = rd.d2h;
   CK(pool, cudaMemsetAsync(umap, 0xff, sizeof(int32_t) * (size_t)n_codes, st));
   unsched_users_kernel<<<(nU + 256) / 256, 256, 0, st>>>(d_quser, nU, umap, rank);
   nl++;
@@ -4584,10 +4540,7 @@ int32_t unscheduled(cook_pool* pool, int n, const int64_t* job_id, uint8_t* out_
   CK(pool, download(out_n_ahead, a.n_ahead, n, st, &d2h));
   CK(pool, download(out_ahead, a.ahead, COOK_UNSCHED_AHEAD * (size_t)n, st, &d2h));
   CK(pool, download(out_plugin, a.plugin, n, st, &d2h));
-  CK(pool, cudaEventRecord(pool->ev[23], st));
-  CK(pool, cudaStreamSynchronize(st));
-  if (out_stats) *out_stats = call_stats(pool, h2d, d2h, nl);
-  return COOK_OK;
+  return rd.close(out_stats);
 }
 
 }  // namespace
@@ -4760,13 +4713,11 @@ int32_t user_usage(cook_pool* const* pools, int n, const int32_t* user, int nU, 
   if (R == 0) {   // no row to read: empty results without device work
     *o_nseg = 0;
     *o_njob = 0;
-    if (out_stats) *out_stats = cook_phase_stats{};
-    return COOK_OK;
+    return no_rows(out_stats);
   }
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S0 = state_of(pool, true);   // pools[0]'s scratch, even when it holds no row
-  if (!S0) return set_err(pool, COOK_E_OOM, "%s: out of device memory", who);
-  cudaStream_t st = pool->stream;
+  ReadCall r(pool);
+  if (int32_t rc = r.open(who)) return rc;
+  cudaStream_t st = r.st;
   const int Rn = (int)R, E = Rn * L, J = bg ? Rn * (1 + pp) : 0;
   hw = std::max(hw, E);
   // ---- one carve: the rows, the representatives, the entries and their order, the folds, the outputs
@@ -4780,8 +4731,7 @@ int32_t user_usage(cook_pool* const* pools, int n, const int32_t* user, int nU, 
   UUKey key = {};
   OrderScan<double, 3> os = {};
   UUFoldOut a = {};
-  int64_t h2d = 0, d2h = 0;
-  CK(pool, carve(S0->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+  if (int32_t rc = r.scratch([&](Carve& c) {
     cnt = c.take<int32_t>(3);   // segments, listed jobs, the row compactions' own
     blk = c.take<int32_t>((size_t)hw / CP_BLOCK + 2);
     if (user) umap = c.take<uint8_t>(n_codes);
@@ -4804,11 +4754,12 @@ int32_t user_usage(cook_pool* const* pools, int n, const int32_t* user, int nU, 
       d_jid = c.take<int64_t>(J);
     }
     if (user) d_q = c.up(q.data(), nU);
-  }));
-  CK(pool, cudaEventRecord(pool->ev[21], st));
+  }))
+    return rc;
   CK(pool, cudaMemsetAsync(cnt, 0, sizeof(int32_t) * 3, st));
   CK(pool, cudaMemsetAsync(gf, 0, sizeof(GridFlag), st));
-  int nl = 0;
+  int& nl = r.nl;
+  int64_t& d2h = r.d2h;
   if (user) {
     CK(pool, cudaMemsetAsync(umap, 0, (size_t)n_codes, st));
     uu_users_kernel<<<(nU + 255) / 256, 256, 0, st>>>(d_q, nU, n_codes, umap);
@@ -4853,11 +4804,9 @@ int32_t user_usage(cook_pool* const* pools, int n, const int32_t* user, int nU, 
     CK(pool, download(o_off, a.o_off, ns, st, &d2h));
     CK(pool, download(o_jid, d_jid, nj, st, &d2h));
   }
-  CK(pool, cudaEventRecord(pool->ev[23], st));
-  CK(pool, cudaStreamSynchronize(st));
+  if (int32_t rc = r.close(out_stats)) return rc;
   *o_nseg = ns;
   *o_njob = nj;
-  if (out_stats) *out_stats = call_stats(pool, h2d, d2h, nl);
   return COOK_OK;
 }
 
@@ -5120,9 +5069,12 @@ struct ISPipe {
 };
 
 // From S selected rows on: the entries, the fold order and its segments, the folds, the ranks and the leaders; then
-// ev[22], the downloads and ev[23].  More segments than seg_cap: only *o.n_seg is written, COOK_E_TOO_LARGE.
-int32_t is_answer(cook_pool* pool, cudaStream_t st, ISPipe& p, int S, int32_t seg_cap, const ISOut& o, int* nl,
-                  int64_t* d2h) {
+// ev[22], the downloads and the close.  More segments than seg_cap: only *o.n_seg is written, COOK_E_TOO_LARGE.
+int32_t is_answer(ReadCall& r, ISPipe& p, int S, int32_t seg_cap, const ISOut& o, cook_phase_stats* out_stats) {
+  cook_pool* pool = r.pool;
+  cudaStream_t st = r.st;
+  int* nl = &r.nl;
+  int64_t* d2h = &r.d2h;
   const int E = IS_LEVELS * S, E3 = 3 * S;
   int32_t got[2] = {0, 0};
   ISFoldOut& a = p.a;
@@ -5167,17 +5119,16 @@ int32_t is_answer(cook_pool* pool, cudaStream_t st, ISPipe& p, int S, int32_t se
     CK(pool, download(o.lead_user + k * COOK_IS_LEADERS, p.l_user + k * COOK_IS_LEADERS, nlead, st, d2h));
     CK(pool, download(o.lead_total + k * COOK_IS_LEADERS, p.l_total + k * COOK_IS_LEADERS, nlead, st, d2h));
   }
-  CK(pool, cudaEventRecord(pool->ev[23], st));
-  CK(pool, cudaStreamSynchronize(st));
+  if (int32_t rc = r.close(out_stats)) return rc;
   *o.n_seg = ns;
   *o.n_lead = nlead;
   return COOK_OK;
 }
 
-void is_empty(const ISOut& o, cook_phase_stats* out_stats) {
+int32_t is_empty(const ISOut& o, cook_phase_stats* out_stats) {
   *o.n_seg = 0;
   *o.n_lead = 0;
-  if (out_stats) *out_stats = cook_phase_stats{};
+  return no_rows(out_stats);
 }
 
 int32_t instance_stats(cook_pool* const* pools, int n, int64_t now, int32_t status, int64_t start_ms, int64_t end_ms,
@@ -5202,14 +5153,10 @@ int32_t instance_stats(cook_pool* const* pools, int n, int64_t now, int32_t stat
   }
   if (R * IS_LEVELS > INT32_MAX) return set_err(pool, COOK_E_TOO_LARGE, "%s: more than 2^31 - 1 entries", who);
   if (seg_cap < 1 + 2 * R) return set_err(pool, COOK_E_BADARG, "%s: seg_cap below 1 + 2 * the live running rows", who);
-  if (R == 0) {   // no row to read: empty results without device work
-    is_empty(o, out_stats);
-    return COOK_OK;
-  }
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S0 = state_of(pool, true);   // pools[0]'s scratch, even when it holds no row
-  if (!S0) return set_err(pool, COOK_E_OOM, "%s: out of device memory", who);
-  cudaStream_t st = pool->stream;
+  if (R == 0) return is_empty(o, out_stats);   // no row to read
+  ReadCall r(pool);
+  if (int32_t rc = r.open(who)) return rc;
+  cudaStream_t st = r.st;
   const int Rn = (int)R;
   // ---- one carve, sized by the live rows: the rows, then the selection and the pipeline's buffers
   int32_t *a_user = nullptr, *a_reason = nullptr, *a_pidx = nullptr;
@@ -5217,16 +5164,14 @@ int32_t instance_stats(cook_pool* const* pools, int n, int64_t now, int32_t stat
   double *a_cpus = nullptr, *a_mem = nullptr;
   uint8_t* a_facts = nullptr;
   ISPipe p;
-  int64_t h2d = 0, d2h = 0;
-  CK(pool, carve(S0->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+  if (int32_t rc = r.scratch([&](Carve& c) {
     a_user = c.take<int32_t>(Rn); a_reason = c.take<int32_t>(Rn); a_pidx = c.take<int32_t>(Rn);
     a_tid = c.take<int64_t>(Rn); a_start = c.take<int64_t>(Rn);
     a_cpus = c.take<double>(Rn); a_mem = c.take<double>(Rn); a_facts = c.take<uint8_t>(Rn);
     p.take(c, Rn, hw, false);
-  }));
-  CK(pool, cudaEventRecord(pool->ev[21], st));
+  }))
+    return rc;
   CK(pool, p.clear(st));
-  int nl = 0;
   // ---- the selection and its metrics
   Gather g(pool);
   int base = 0;
@@ -5235,21 +5180,19 @@ int32_t instance_stats(cook_pool* const* pools, int n, int64_t now, int32_t stat
     CK(pool, g.rows(pools[h.second],
                     ISRows{h.first->run.d_col, base, h.second, a_user, a_reason, a_tid, a_pidx, a_start, a_cpus, a_mem,
                            a_facts},
-                    h.first->run.hw, live, p.blk, p.cnt + 5, &nl));
+                    h.first->run.hw, live, p.blk, p.cnt + 5, &r.nl));
     base += live;
   }
   compact(ISSel{a_user, a_reason, a_tid, a_pidx, a_start, a_cpus, a_mem, a_facts, now, start_ms, end_ms, tid_lo, tid_hi,
                 status == COOK_IS_UNKNOWN, p.s_user, p.s_reason, p.s_tid, p.s_pidx, {p.met[0], p.met[1], p.met[2]},
                 p.cnt + 1},
-          Rn, nullptr, p.blk, p.cnt + 0, Rn, st, &nl);
+          Rn, nullptr, p.blk, p.cnt + 0, Rn, st, &r.nl);
   CK(pool, cudaGetLastError());
   int32_t sel[2];
-  CK(pool, download(sel, p.cnt, 2, st, &d2h));
+  CK(pool, download(sel, p.cnt, 2, st, &r.d2h));
   CK(pool, cudaStreamSynchronize(st));
   if (sel[1]) return set_err(pool, COOK_E_BADARG, "%s: a selected task starts after now_ms", who);
-  if (int32_t rc = is_answer(pool, st, p, sel[0], seg_cap, o, &nl, &d2h)) return rc;
-  if (out_stats) *out_stats = call_stats(pool, h2d, d2h, nl);
-  return COOK_OK;
+  return is_answer(r, p, sel[0], seg_cap, o, out_stats);
 }
 
 // one handle's finished rows of the status with task id in [tid_lo, tid_hi) and start in [start_ms, end_ms), dense
@@ -5303,14 +5246,10 @@ int32_t history_stats(cook_pool* const* pools, int n, int32_t status, int64_t st
     hs.push_back({&s->hist, k});
     Tmax = std::max(Tmax, (int)s->hist.tail);
   }
-  if (hs.empty()) {   // no row to read: empty results without device work
-    is_empty(o, out_stats);
-    return COOK_OK;
-  }
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S0 = state_of(pool, true);
-  if (!S0) return set_err(pool, COOK_E_OOM, "%s: out of device memory", who);
-  cudaStream_t st = pool->stream;
+  if (hs.empty()) return is_empty(o, out_stats);   // no row to read
+  ReadCall r(pool);
+  if (int32_t rc = r.open(who)) return rc;
+  cudaStream_t st = r.st;
   const int H = (int)hs.size();
   const bool ok = status == COOK_IS_SUCCESS;
   auto sel = [&](int j, int base, const ISPipe& p) {
@@ -5321,11 +5260,10 @@ int32_t history_stats(cook_pool* const* pools, int n, int32_t status, int64_t st
   // (Gather) counts on its own device, into its own scratch.
   Gather g(pool);
   int32_t* hcnt = nullptr;
-  int64_t h2d = 0, d2h = 0;
-  CK(pool, carve(S0->scratch, st, pool->ev[20], &h2d, [&](Carve& c) { hcnt = c.take<int32_t>(H); }));
-  CK(pool, cudaEventRecord(pool->ev[21], st));
+  if (int32_t rc = r.scratch([&](Carve& c) { hcnt = c.take<int32_t>(H); })) return rc;
   CK(pool, cudaMemsetAsync(hcnt, 0, sizeof(int32_t) * H, st));
-  int nl = 0;
+  int& nl = r.nl;
+  int64_t& d2h = r.d2h;
   std::vector<int32_t> cnt(H);
   for (int j = 0; j < H; j++) {
     const int T = (int)hs[j].first->tail;
@@ -5364,7 +5302,7 @@ int32_t history_stats(cook_pool* const* pools, int n, int32_t status, int64_t st
   if (S * IS_LEVELS > INT32_MAX) return set_err(pool, COOK_E_TOO_LARGE, "%s: more than 2^31 - 1 entries", who);
   // ---- the selection and its metrics, then the pipeline
   ISPipe p;
-  CK(pool, carve(S0->scratch, st, nullptr, &h2d, [&](Carve& c) { p.take(c, (int)S, Tmax, true); }));
+  CK(pool, carve(r.S->scratch, st, nullptr, &r.h2d, [&](Carve& c) { p.take(c, (int)S, Tmax, true); }));
   CK(pool, p.clear(st));
   int base = 0;
   for (int j = 0; j < H && S; j++) {
@@ -5373,9 +5311,7 @@ int32_t history_stats(cook_pool* const* pools, int n, int32_t status, int64_t st
     base += cnt[j];
   }
   CK(pool, cudaGetLastError());
-  if (int32_t rc = is_answer(pool, st, p, (int)S, seg_cap, o, &nl, &d2h)) return rc;
-  if (out_stats) *out_stats = call_stats(pool, h2d, d2h, nl);
-  return COOK_OK;
+  return is_answer(r, p, (int)S, seg_cap, o, out_stats);
 }
 
 }  // namespace
@@ -6199,10 +6135,9 @@ int32_t mm_counters_room(cook_pool* pool, MetricsRound& R, int64_t n, cudaStream
   return COOK_OK;
 }
 
-int32_t job_facts(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, const uint8_t* flags,
+int32_t job_facts(cook_pool* pool, PoolState* S, const char* who, int n, const int64_t* job_id, const uint8_t* flags,
                   const int32_t* gpu_model, const double* disk_request, const double* disk_limit,
                   const int32_t* disk_type) {
-  const char* who = "cook_state_job_facts";
   if (n < 0) return set_err(pool, COOK_E_BADARG, "%s: n < 0", who);
   if (n && !job_id) return set_err(pool, COOK_E_BADARG, "%s: null job_id", who);
   const int all = COOK_JF_GPUS | COOK_JF_DISK | COOK_JF_DISK_REQUEST | COOK_JF_DISK_LIMIT | COOK_JF_URIS;
@@ -6217,9 +6152,7 @@ int32_t job_facts(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, c
     for (int i = 0; v && i < n; i++)
       if (std::isnan(v[i])) return set_err(pool, COOK_E_BADARG, "%s: a NaN disk amount", who);
   std::vector<int32_t> slot;
-  if (const char* why = pending_slots(S, n, job_id, &slot)) return set_err(pool, COOK_E_BADARG, "%s: %s", who, why);
-  CK(pool, cudaSetDevice(pool->device));
-  cudaStream_t st = pool->stream;
+  if (int32_t rc = live_slots(pool, who, S->pend, "job", n, job_id, &slot)) return rc;
   // ---- host side: the rows' bits, for the count of rows with a keyed resource
   for (int i = 0; flags && i < n; i++) {
     PendingInfo& pi = S->pinfo[slot[i]];
@@ -6231,27 +6164,16 @@ int32_t job_facts(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, c
   const bool cols = n && (flags || gpu_model || disk_request || disk_limit || disk_type);
   ScatterArgs pa;
   memset(&pa, 0, sizeof(pa));
-  int64_t h2d = 0;
-  CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
-    if (!cols) return;
-    pa.slot = c.up(slot.data(), n);
-    const auto col = [&](int k, const char* src) {
-      pa.c[pa.nc++] = ScatterCol{static_cast<char*>(S->pend.col[k]), src, 0, P_SZ[k]};
-    };
-    if (flags) col(P_JF, reinterpret_cast<const char*>(c.up(flags, n)));
-    if (gpu_model) col(P_JF_GPU, reinterpret_cast<const char*>(c.up(gpu_model, n)));
-    if (disk_request) col(P_JF_DREQ, reinterpret_cast<const char*>(c.up(disk_request, n)));
-    if (disk_limit) col(P_JF_DLIM, reinterpret_cast<const char*>(c.up(disk_limit, n)));
-    if (disk_type) col(P_JF_DTYPE, reinterpret_cast<const char*>(c.up(disk_type, n)));
-  }));
-  CK(pool, cudaEventRecord(pool->ev[21], st));
-  int nl = 0;
-  scatter(pa, S->pend, cols ? n : 0, 0, -1, nullptr, st, &nl);
-  CK(pool, cudaGetLastError());
-  CK(pool, cudaEventRecord(pool->ev[22], st));
-  CK(pool, cudaStreamSynchronize(st));
-  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
-  return COOK_OK;
+  StateWrite w(pool, S);
+  if (int32_t rc = w.up([&](Carve& c) {
+    if (cols)
+      patch_args(c, pa, S->pend, slot.data(), n,
+                 {{P_JF, flags, 0}, {P_JF_GPU, gpu_model, 0}, {P_JF_DREQ, disk_request, 0}, {P_JF_DLIM, disk_limit, 0},
+                  {P_JF_DTYPE, disk_type, 0}});
+  }))
+    return rc;
+  scatter(pa, S->pend, cols ? n : 0, 0, -1, nullptr, w.st, &w.nl);
+  return w.end();
 }
 
 // The caller's arrays of cook_state_match_metrics
@@ -6310,8 +6232,9 @@ int32_t match_metrics(cook_pool* pool, PoolState* S, int32_t U, int32_t D, const
     R.counted = true;
     return COOK_OK;
   }
-  CK(pool, cudaSetDevice(pool->device));
-  cudaStream_t st = pool->stream;
+  ReadCall rd(pool);
+  if (int32_t rc = rd.open(who)) return rc;   // S: the handle holds the round
+  cudaStream_t st = rd.st;
   if (int32_t rc = mm_counters_room(pool, R, N, st)) return rc;
   const bool changed = S->pend_epoch != R.epoch;
   const bool keyed = S->jf_keyed > 0;
@@ -6326,8 +6249,7 @@ int32_t match_metrics(cook_pool* pool, PoolState* S, int32_t U, int32_t D, const
   double* o_total = nullptr;
   GridFlag* gf = nullptr;
   MMOut* d_out = nullptr;
-  int64_t h2d = 0, d2h = 0;
-  CK(pool, carve(S->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+  if (int32_t rc = rd.scratch([&](Carve& c) {
     r.slot = c.take<int32_t>(N); r.user = c.take<int32_t>(N); r.jid = c.take<int64_t>(N);
     r.cpus = c.take<double>(N); r.mem = c.take<double>(N); r.gpus = c.take<double>(N); r.ports = c.take<int32_t>(N);
     r.jf = c.take<uint8_t>(N); r.gmodel = c.take<int32_t>(N); r.dtype = c.take<int32_t>(N);
@@ -6345,13 +6267,14 @@ int32_t match_metrics(cook_pool* pool, PoolState* S, int32_t U, int32_t D, const
     gf = c.take<GridFlag>(2);
     d_out = c.take<MMOut>(1);
     d_drop = c.up(D ? dropped : nullptr, D);
-  }));
-  CK(pool, cudaEventRecord(pool->ev[21], st));
+  }))
+    return rc;
   CK(pool, cudaMemsetAsync(cnt, 0, sizeof(int32_t) * MMC_N, st));
   CK(pool, cudaMemsetAsync(ucons, 0, sizeof(int32_t) * U, st));
   CK(pool, cudaMemsetAsync(umat, 0, sizeof(int32_t) * U, st));
   CK(pool, cudaMemsetAsync(gf, 0, sizeof(GridFlag) * 2, st));
-  int nl = 0;
+  int& nl = rd.nl;
+  int64_t& d2h = rd.d2h;
   // ---- the rows, the drops, the counts and cycles, the entries; the first-ten and the new pairs in take order
   mm_gather_kernel<<<(N + 255) / 256, 256, 0, st>>>(S->pend.d_col, R.slot, cons, assign, N, r);
   nl++;
@@ -6415,13 +6338,11 @@ int32_t match_metrics(cook_pool* pool, PoolState* S, int32_t U, int32_t D, const
     CK(pool, download(out_code, o_code, res.n_keys, st, &d2h));
     CK(pool, download(out_total, o_total, res.n_keys, st, &d2h));
   }
-  CK(pool, cudaEventRecord(pool->ev[23], st));
-  CK(pool, cudaStreamSynchronize(st));
+  if (int32_t rc = rd.close(out_stats)) return rc;
   out.put(res);
   R.cur = nxt;
   R.u_n = nu;
   R.counted = true;
-  if (out_stats) *out_stats = call_stats(pool, h2d, d2h, nl);
   return COOK_OK;
 }
 
@@ -6430,11 +6351,10 @@ int32_t match_metrics(cook_pool* pool, PoolState* S, int32_t U, int32_t D, const
 extern "C" int32_t cook_state_job_facts(cook_pool* pool, int32_t n, const int64_t* job_id, const uint8_t* flags,
                                         const int32_t* gpu_model, const double* disk_request, const double* disk_limit,
                                         const int32_t* disk_type) {
-  if (!pool) return COOK_E_BADARG;
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S = state_of(pool, true);
-  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_job_facts: out of device memory");
-  return job_facts(pool, S, n, job_id, flags, gpu_model, disk_request, disk_limit, disk_type);
+  const char* who = "cook_state_job_facts";
+  return on_state(pool, who, [&](PoolState* S) {
+    return job_facts(pool, S, who, n, job_id, flags, gpu_model, disk_request, disk_limit, disk_type);
+  });
 }
 
 extern "C" int32_t cook_state_match_metrics(cook_pool* pool, int32_t n_users, int32_t n_dropped, const int32_t* dropped,
@@ -6537,9 +6457,8 @@ LJCols lj_cols(const PoolState* s, bool running) {
           t.at<int32_t>(P_LF_POOL), t.at<uint8_t>(P_LF_EXEC)};
 }
 
-int32_t list_facts(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, const int64_t* submit_ms,
+int32_t list_facts(cook_pool* pool, PoolState* S, const char* who, int n, const int64_t* job_id, const int64_t* submit_ms,
                    const int32_t* submit_pool, const int32_t* custom_executor) {
-  const char* who = "cook_state_list_facts";
   if (n < 0) return set_err(pool, COOK_E_BADARG, "%s: n < 0", who);
   if (n && !job_id) return set_err(pool, COOK_E_BADARG, "%s: null job_id", who);
   for (int i = 0; custom_executor && i < n; i++)
@@ -6562,8 +6481,6 @@ int32_t list_facts(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, 
         for (int32_t s : r->second) { rslot.push_back(s); rk.push_back(i); }
     }
   }
-  CK(pool, cudaSetDevice(pool->device));
-  cudaStream_t st = pool->stream;
   // ---- the values per row written (LF_EXEC stores 2 + custom_executor), then one patch scatter per table
   const int np = (int)pslot.size(), nr = (int)rslot.size(), m = np + nr;
   std::vector<int64_t> sub(submit_ms ? m : 0);
@@ -6578,29 +6495,24 @@ int32_t list_facts(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, 
   const bool cols = submit_ms || submit_pool || custom_executor;
   ScatterArgs pa, ra;
   memset(&pa, 0, sizeof(pa)); memset(&ra, 0, sizeof(ra));
-  int64_t h2d = 0;
-  CK(pool, carve(S->stage, st, pool->ev[20], &h2d, [&](Carve& c) {
+  StateWrite w(pool, S);
+  if (int32_t rc = w.up([&](Carve& c) {
     if (!cols) return;
-    const auto fill = [&](ScatterArgs& a, const Table& t, const int32_t* slot, int k, int off, int c_sub, int c_pool,
-                          int c_exec) {
-      if (!k) return;
-      a.slot = c.up(slot, k);
-      if (submit_ms) a.c[a.nc++] = ScatterCol{static_cast<char*>(t.col[c_sub]), reinterpret_cast<const char*>(c.up(sub.data() + off, k)), 0, 8};
-      if (submit_pool) a.c[a.nc++] = ScatterCol{static_cast<char*>(t.col[c_pool]), reinterpret_cast<const char*>(c.up(sp.data() + off, k)), 0, 4};
-      if (custom_executor) a.c[a.nc++] = ScatterCol{static_cast<char*>(t.col[c_exec]), reinterpret_cast<const char*>(c.up(ex.data() + off, k)), 0, 1};
-    };
-    fill(pa, S->pend, pslot.data(), np, 0, P_LF_SUBMIT, P_LF_POOL, P_LF_EXEC);
-    fill(ra, S->run, rslot.data(), nr, np, R_LF_SUBMIT, R_LF_POOL, R_LF_EXEC);
-  }));
-  CK(pool, cudaEventRecord(pool->ev[21], st));
-  int nl = 0;
-  scatter(pa, S->pend, cols ? np : 0, 0, -1, nullptr, st, &nl);
-  scatter(ra, S->run, cols ? nr : 0, 0, -1, nullptr, st, &nl);
-  CK(pool, cudaGetLastError());
-  CK(pool, cudaEventRecord(pool->ev[22], st));
-  CK(pool, cudaStreamSynchronize(st));
-  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], h2d, 0, nl);
-  return COOK_OK;
+    // the batch's values from row `off` on (null: the column is not written)
+    const auto at = [](const auto& v, bool given, int off) { return given ? v.data() + off : nullptr; };
+    if (np)
+      patch_args(c, pa, S->pend, pslot.data(), np,
+                 {{P_LF_SUBMIT, at(sub, submit_ms, 0), 0}, {P_LF_POOL, at(sp, submit_pool, 0), 0},
+                  {P_LF_EXEC, at(ex, custom_executor, 0), 0}});
+    if (nr)
+      patch_args(c, ra, S->run, rslot.data(), nr,
+                 {{R_LF_SUBMIT, at(sub, submit_ms, np), 0}, {R_LF_POOL, at(sp, submit_pool, np), 0},
+                  {R_LF_EXEC, at(ex, custom_executor, np), 0}});
+  }))
+    return rc;
+  scatter(pa, S->pend, cols ? np : 0, 0, -1, nullptr, w.st, &w.nl);
+  scatter(ra, S->run, cols ? nr : 0, 0, -1, nullptr, w.st, &w.nl);
+  return w.end();
 }
 
 // the listing arguments cook_state_list_jobs and cook_state_list_completed share
@@ -6656,21 +6568,18 @@ int32_t list_jobs(cook_pool* const* pools, int n, int32_t user, int32_t states, 
   if (C[0] + C[1] == 0) {   // no row to read: empty results without device work
     *o_n = 0;
     *o_missing = 0;
-    if (out_stats) *out_stats = cook_phase_stats{};
-    return COOK_OK;
+    return no_rows(out_stats);
   }
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S0 = state_of(pool, true);   // pools[0]'s scratch, even when it holds no row
-  if (!S0) return set_err(pool, COOK_E_OOM, "%s: out of device memory", who);
-  cudaStream_t st = pool->stream;
+  ReadCall r(pool);
+  if (int32_t rc = r.open(who)) return rc;
+  cudaStream_t st = r.st;
   // ---- one carve: the flags, each state's rows, order and entries, the counts
   struct Dense { int64_t *jid, *tid, *submit, *o_jid, *o_submit; int32_t *pi, *ord, *o_pi; uint8_t* ok; };
   Dense D[2] = {};
   int32_t *cnt = nullptr, *blk = nullptr, *tmp = nullptr;
   uint8_t* flag = nullptr;
-  int64_t h2d = 0, d2h = 0;
   const int Cmax = (int)std::max(C[0], C[1]);
-  CK(pool, carve(S0->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+  if (int32_t rc = r.scratch([&](Carve& c) {
     cnt = c.take<int32_t>(4);   // [0] [1] the states' entries, [2] rows without facts, [3] the row compactions' own
     blk = c.take<int32_t>((size_t)std::max(hw, Cmax) / CP_BLOCK + 2);
     flag = c.take<uint8_t>(hw);
@@ -6684,10 +6593,11 @@ int32_t list_jobs(cook_pool* const* pools, int n, int32_t user, int32_t states, 
       if (t) d.tid = c.take<int64_t>(Ct);
       d.o_jid = c.take<int64_t>(Ot); d.o_submit = c.take<int64_t>(Ot); d.o_pi = c.take<int32_t>(Ot);
     }
-  }));
-  CK(pool, cudaEventRecord(pool->ev[21], st));
+  }))
+    return rc;
   CK(pool, cudaMemsetAsync(cnt, 0, sizeof(int32_t) * 4, st));
-  int nl = 0;
+  int& nl = r.nl;
+  int64_t& d2h = r.d2h;
   for (int t = 0; t < 2; t++) {
     if (!C[t]) continue;
     Dense& d = D[t];
@@ -6725,11 +6635,9 @@ int32_t list_jobs(cook_pool* const* pools, int n, int32_t user, int32_t states, 
     std::fill(o_state + at, o_state + at + got[t], t ? COOK_LJ_RUNNING : COOK_LJ_WAITING);
     at += got[t];
   }
-  CK(pool, cudaEventRecord(pool->ev[23], st));
-  CK(pool, cudaStreamSynchronize(st));
+  if (int32_t rc = r.close(out_stats)) return rc;
   *o_n = at;
   *o_missing = got[2];
-  if (out_stats) *out_stats = call_stats(pool, h2d, d2h, nl);
   return COOK_OK;
 }
 
@@ -6817,34 +6725,28 @@ int32_t cj_append(cook_pool* pool, PoolState* S, const CJBatch& b, const char* w
   Completed& L = S->cj;
   const int64_t k = (int64_t)b.jid.size();
   if (L.tail + k > INT32_MAX) return set_err(pool, COOK_E_TOO_LARGE, "%s: more than 2^31 - 1 log rows", who);
-  cudaStream_t st = pool->stream;
-  CK(pool, L.grow(L.tail + k, st));
-  CK(pool, cudaEventRecord(pool->ev[20], st));
-  Carve c;   // only its copy(): the bytes counted, the first error kept
-  c.st = st;
+  CK(pool, L.grow(L.tail + k, pool->stream));
   const int64_t t = L.tail;
-  if (k) {
+  StateWrite w(pool, S);
+  if (int32_t rc = w.direct([&](Carve& c) {
+    if (!k) return;
     c.copy(L.c.jid + t, b.jid.data(), k); c.copy(L.c.stamp + t, b.stamp.data(), k);
     c.copy(L.c.submit + t, b.submit.data(), k); c.copy(L.c.user + t, b.user.data(), k);
     c.copy(L.c.spool + t, b.spool.data(), k); c.copy(L.c.exec + t, b.exec.data(), k);
     c.copy(L.c.kind + t, b.kind.data(), k);
-  }
-  CK(pool, c.err);
-  CK(pool, cudaEventRecord(pool->ev[21], st));
-  CK(pool, cudaEventRecord(pool->ev[22], st));
-  CK(pool, cudaStreamSynchronize(st));
+  }))
+    return rc;
+  if (int32_t rc = w.end()) return rc;
   L.tail += k;
   L.h_user.insert(L.h_user.end(), b.user.begin(), b.user.end());
   L.h_submit.insert(L.h_submit.end(), b.submit.begin(), b.submit.end());
   for (int32_t u : b.user) L.users[u]++;
-  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], c.h2d, 0, 0);
   return COOK_OK;
 }
 
-int32_t completed_seed(cook_pool* pool, PoolState* S, int64_t since_ms, int n, const int64_t* job_id, const int64_t* stamp,
-                       const int32_t* user, const int64_t* submit_ms, const int32_t* submit_pool,
+int32_t completed_seed(cook_pool* pool, PoolState* S, const char* who, int64_t since_ms, int n, const int64_t* job_id,
+                       const int64_t* stamp, const int32_t* user, const int64_t* submit_ms, const int32_t* submit_pool,
                        const int32_t* custom_executor, const uint8_t* kind) {
-  const char* who = "cook_state_completed_seed";
   CJBatch b;
   if (int32_t rc = cj_batch(pool, who, n, since_ms, false, job_id, stamp, user, submit_ms, submit_pool, custom_executor,
                             kind, &b))
@@ -6856,10 +6758,9 @@ int32_t completed_seed(cook_pool* pool, PoolState* S, int64_t since_ms, int n, c
   return cj_append(pool, S, b, who);
 }
 
-int32_t completed_record(cook_pool* pool, PoolState* S, int n, const int64_t* job_id, const int64_t* stamp,
-                         const int32_t* user, const int64_t* submit_ms, const int32_t* submit_pool,
+int32_t completed_record(cook_pool* pool, PoolState* S, const char* who, int n, const int64_t* job_id,
+                         const int64_t* stamp, const int32_t* user, const int64_t* submit_ms, const int32_t* submit_pool,
                          const int32_t* custom_executor, const uint8_t* kind) {
-  const char* who = "cook_state_completed_record";
   if (!S->cj.on) return set_err(pool, COOK_E_BADARG, "%s: the log is off", who);
   CJBatch b;
   if (int32_t rc = cj_batch(pool, who, n, S->cj.since, true, job_id, stamp, user, submit_ms, submit_pool,
@@ -6870,38 +6771,32 @@ int32_t completed_record(cook_pool* pool, PoolState* S, int n, const int64_t* jo
 
 // the horizon raised to since_ms: the rows submitted before it leave in one compaction into new columns, and from the
 // host's rows
-int32_t completed_advance(cook_pool* pool, PoolState* S, int64_t since_ms) {
-  const char* who = "cook_state_completed_advance";
+int32_t completed_advance(cook_pool* pool, PoolState* S, const char* who, int64_t since_ms) {
   Completed& L = S->cj;
   if (!L.on) return set_err(pool, COOK_E_BADARG, "%s: the log is off", who);
   if (since_ms < L.since) return set_err(pool, COOK_E_BADARG, "%s: since_ms below the horizon", who);
-  CK(pool, cudaSetDevice(pool->device));
-  cudaStream_t st = pool->stream;
   int32_t* blk = nullptr;
   const int T = (int)L.tail;
   const bool move = T && since_ms > L.since;
-  CK(pool, carve(S->scratch, st, pool->ev[20], nullptr, [&](Carve& c) {
+  StateWrite w(pool, S);
+  if (int32_t rc = w.up(S->scratch, [&](Carve& c) {
     if (move) blk = c.take<int32_t>((size_t)T / CP_BLOCK + 2);
-  }));
-  CK(pool, cudaEventRecord(pool->ev[21], st));
-  int nl = 0;
-  int64_t d2h = 0;
+  }))
+    return rc;
   if (move) {
     CJCols nc;
     CK(pool, nc.alloc(L.cap));
-    compact(CJKeep{L.c, nc, since_ms}, T, nullptr, blk, S->counters + 7, T, st, &nl);
+    compact(CJKeep{L.c, nc, since_ms}, T, nullptr, blk, S->counters + 7, T, w.st, &w.nl);
     int32_t kept = 0;
     cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = download(&kept, S->counters + 7, 1, st, &d2h);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e == cudaSuccess) e = download(&kept, S->counters + 7, 1, w.st, &w.d2h);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(w.st);
     if (e != cudaSuccess) { nc.free_all(); CK(pool, e); }
     L.c.free_all();
     L.c = nc;
     L.tail = kept;
   }
-  CK(pool, cudaEventRecord(pool->ev[22], st));
-  CK(pool, cudaStreamSynchronize(st));
-  record_phase(pool, COOK_PHASE_STATE, pool->ev[20], pool->ev[21], pool->ev[22], pool->ev[22], 0, d2h, nl);
+  if (int32_t rc = w.end()) return rc;
   if (move) {   // the host's rows, by the same rule and in the same order
     int64_t w = 0;
     for (int64_t i = 0; i < T; i++) {
@@ -6950,28 +6845,26 @@ int32_t list_completed(cook_pool* const* pools, int n, int32_t user, int32_t sta
   if (C > INT32_MAX) return set_err(pool, COOK_E_TOO_LARGE, "%s: more than 2^31 - 1 records of the user", who);
   if (C == 0) {   // no record to read: empty results without device work
     *o_n = 0;
-    if (out_stats) *out_stats = cook_phase_stats{};
-    return COOK_OK;
+    return no_rows(out_stats);
   }
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S0 = state_of(pool, true);   // pools[0]'s scratch, even when it holds no record
-  if (!S0) return set_err(pool, COOK_E_OOM, "%s: out of device memory", who);
-  cudaStream_t st = pool->stream;
+  ReadCall r(pool);
+  if (int32_t rc = r.open(who)) return rc;
+  cudaStream_t st = r.st;
   // ---- one carve: the records, their order, the entries, the counts
   const int Cn = (int)C, On = std::min(Cn, limit);
   int64_t *jid = nullptr, *stamp = nullptr, *submit = nullptr, *e_jid = nullptr, *e_submit = nullptr;
   int32_t *pi = nullptr, *ord = nullptr, *tmp = nullptr, *e_pi = nullptr, *cnt = nullptr, *blk = nullptr;
   uint8_t* ok = nullptr;
-  int64_t h2d = 0, d2h = 0;
-  CK(pool, carve(S0->scratch, st, pool->ev[20], &h2d, [&](Carve& c) {
+  if (int32_t rc = r.scratch([&](Carve& c) {
     cnt = c.take<int32_t>(2);   // [0] the entries, [1] the record compactions' own
     blk = c.take<int32_t>((size_t)std::max(tmax, Cn) / CP_BLOCK + 2);
     jid = c.take<int64_t>(Cn); stamp = c.take<int64_t>(Cn); submit = c.take<int64_t>(Cn);
     pi = c.take<int32_t>(Cn); ok = c.take<uint8_t>(Cn); ord = c.take<int32_t>(Cn); tmp = c.take<int32_t>(Cn);
     e_jid = c.take<int64_t>(On); e_submit = c.take<int64_t>(On); e_pi = c.take<int32_t>(On);
-  }));
-  CK(pool, cudaEventRecord(pool->ev[21], st));
-  int nl = 0;
+  }))
+    return rc;
+  int& nl = r.nl;
+  int64_t& d2h = r.d2h;
   int base = 0;
   Gather g(pool);
   for (const Src& h : hs) {
@@ -6992,10 +6885,8 @@ int32_t list_completed(cook_pool* const* pools, int n, int32_t user, int32_t sta
     return set_err(pool, COOK_E_TOO_LARGE, "%s: more entries than cap: %d", who, got);
   }
   if (got) CK(pool, download_entries(o_jid, o_submit, o_pool, e_jid, e_submit, e_pi, got, st, &d2h));
-  CK(pool, cudaEventRecord(pool->ev[23], st));
-  CK(pool, cudaStreamSynchronize(st));
+  if (int32_t rc = r.close(out_stats)) return rc;
   *o_n = got;
-  if (out_stats) *out_stats = call_stats(pool, h2d, d2h, nl);
   return COOK_OK;
 }
 
@@ -7003,11 +6894,10 @@ int32_t list_completed(cook_pool* const* pools, int n, int32_t user, int32_t sta
 
 extern "C" int32_t cook_state_list_facts(cook_pool* pool, int32_t n, const int64_t* job_id, const int64_t* submit_ms,
                                          const int32_t* submit_pool, const int32_t* custom_executor) {
-  if (!pool) return COOK_E_BADARG;
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S = state_of(pool, true);
-  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_list_facts: out of device memory");
-  return list_facts(pool, S, n, job_id, submit_ms, submit_pool, custom_executor);
+  const char* who = "cook_state_list_facts";
+  return on_state(pool, who, [&](PoolState* S) {
+    return list_facts(pool, S, who, n, job_id, submit_ms, submit_pool, custom_executor);
+  });
 }
 
 extern "C" int32_t cook_state_list_jobs(cook_pool* const* pools, int32_t n_pools, int32_t user, int32_t states,
@@ -7025,29 +6915,24 @@ extern "C" int32_t cook_state_completed_seed(cook_pool* pool, int64_t since_ms, 
                                              const int64_t* stamp, const int32_t* user, const int64_t* submit_ms,
                                              const int32_t* submit_pool, const int32_t* custom_executor,
                                              const uint8_t* kind) {
-  if (!pool) return COOK_E_BADARG;
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S = state_of(pool, true);
-  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_completed_seed: out of device memory");
-  return completed_seed(pool, S, since_ms, n, job_id, stamp, user, submit_ms, submit_pool, custom_executor, kind);
+  const char* who = "cook_state_completed_seed";
+  return on_state(pool, who, [&](PoolState* S) {
+    return completed_seed(pool, S, who, since_ms, n, job_id, stamp, user, submit_ms, submit_pool, custom_executor, kind);
+  });
 }
 
 extern "C" int32_t cook_state_completed_record(cook_pool* pool, int32_t n, const int64_t* job_id, const int64_t* stamp,
                                                const int32_t* user, const int64_t* submit_ms, const int32_t* submit_pool,
                                                const int32_t* custom_executor, const uint8_t* kind) {
-  if (!pool) return COOK_E_BADARG;
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S = state_of(pool, true);
-  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_completed_record: out of device memory");
-  return completed_record(pool, S, n, job_id, stamp, user, submit_ms, submit_pool, custom_executor, kind);
+  const char* who = "cook_state_completed_record";
+  return on_state(pool, who, [&](PoolState* S) {
+    return completed_record(pool, S, who, n, job_id, stamp, user, submit_ms, submit_pool, custom_executor, kind);
+  });
 }
 
 extern "C" int32_t cook_state_completed_advance(cook_pool* pool, int64_t since_ms) {
-  if (!pool) return COOK_E_BADARG;
-  CK(pool, cudaSetDevice(pool->device));
-  PoolState* S = state_of(pool, true);
-  if (!S) return set_err(pool, COOK_E_OOM, "cook_state_completed_advance: out of device memory");
-  return completed_advance(pool, S, since_ms);
+  const char* who = "cook_state_completed_advance";
+  return on_state(pool, who, [&](PoolState* S) { return completed_advance(pool, S, who, since_ms); });
 }
 
 extern "C" int32_t cook_state_list_completed(cook_pool* const* pools, int32_t n_pools, int32_t user, int32_t state,
