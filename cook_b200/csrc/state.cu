@@ -24,6 +24,7 @@
 // Considerable jobs without a match: the live queue entries with their queue positions, their M0 columns gathered,
 // cook_match's considerable pass (match.cu) run on them; a consuming call retires the taken entries' generations.
 #include <algorithm>
+#include <cassert>
 #include <cmath>
 #include <cstdlib>
 #include <map>
@@ -633,221 +634,196 @@ struct RetryFacts {
 };
 struct RetryReason { bool mea_culpa = false; int32_t limit = -2; };   // limit -2: the global one
 
+// Up to MAXC device columns of `cap` rows each, column k w[k] bytes per row (1, 4 or 8): the storage of every growing
+// store of a handle.  A store fixes its widths, its capacity floor and whether new rows are zeroed when it is built.
+struct Columns {
+  static constexpr int MAXC = std::max({(int)P_NCOL, (int)R_NCOL, (int)O_NCOL});   // the widest slot table
+  int n = 0, w[MAXC] = {};
+  int64_t floor = 0;
+  bool zero = false;
+  void* p[MAXC] = {};
+  int64_t cap = 0;
+
+  Columns() = default;
+  Columns(const int* widths, int nc, int64_t fl, bool z) : n(nc), floor(fl), zero(z) {
+    assert(nc >= 0 && nc <= MAXC);
+    std::copy(widths, widths + nc, w);
+    for (int k = 0; k < nc; k++) assert(w[k] == 1 || w[k] == 4 || w[k] == 8);
+  }
+  Columns(std::initializer_list<int> widths, int64_t fl, bool z) : Columns(widths.begin(), (int)widths.size(), fl, z) {}
+
+  Columns shape() const { return Columns(w, n, floor, zero); }   // no rows
+  void* operator[](int k) const { return p[k]; }
+  template <class T>
+  T* at(int k) const { return static_cast<T*>(p[k]); }
+  // *out: a set of this shape with capacity max(want, 2 cap, floor) holding this set's first keep rows (device to
+  // device), the stream synchronized when rows were copied or zeroed.  On failure nothing is left allocated and *out
+  // is untouched.
+  cudaError_t grown(int64_t want, int64_t keep, cudaStream_t st, Columns* out) const {
+    Columns nc = shape();
+    nc.cap = std::max({want, 2 * cap, floor});
+    cudaError_t e = cudaSuccess;
+    for (int k = 0; k < n && e == cudaSuccess; k++) {
+      char* q = nullptr;
+      e = cudaMalloc(&q, (size_t)nc.cap * w[k]);
+      if (e != cudaSuccess) break;
+      nc.p[k] = q;
+      if (keep) e = cudaMemcpyAsync(q, p[k], (size_t)keep * w[k], cudaMemcpyDeviceToDevice, st);
+      if (e == cudaSuccess && zero) e = cudaMemsetAsync(q + keep * w[k], 0, (size_t)(nc.cap - keep) * w[k], st);
+    }
+    if (e == cudaSuccess && (keep || zero)) e = cudaStreamSynchronize(st);   // the copies and fills done
+    if (e != cudaSuccess) {
+      nc.release();
+      return e;
+    }
+    *out = nc;
+    return cudaSuccess;
+  }
+  // capacity >= want, the first keep rows kept; all or nothing: on failure the set is as it was
+  cudaError_t grow(int64_t want, int64_t keep, cudaStream_t st) {
+    if (want <= cap) return cudaSuccess;
+    Columns nc;
+    if (cudaError_t e = grown(want, keep, st, &nc)) return e;
+    release();
+    *this = nc;
+    return cudaSuccess;
+  }
+  void release() {
+    for (int k = 0; k < n; k++) if (p[k]) cudaFree(p[k]);
+    std::fill(p, p + n, nullptr);
+    cap = 0;
+  }
+  // inside a carve: host rows srcs[k][0, m) to rows [row, row + m) of column k, for the first srcs.size() columns.  A
+  // source past the set's columns must be null (the second array of a one-array list arena).
+  void copy(Carve& c, int64_t row, int64_t m, std::initializer_list<const void*> srcs) const {
+    for (int k = 0; k < (int)srcs.size(); k++) {
+      const void* s = srcs.begin()[k];
+      if (k >= n) {
+        assert(!s);
+        continue;
+      }
+      c.copy(static_cast<char*>(p[k]) + row * w[k], static_cast<const char*>(s), (size_t)m * w[k]);
+    }
+  }
+};
+
 struct Table {
-  int ncol = 0;
-  const int* sz = nullptr;
-  void* col[P_NCOL] = {};
-  void** d_col = nullptr;        // the column pointers on the device (for the gather kernels)
-  int32_t cap = 0, hw = 0;       // slots allocated, slots ever used
+  Columns col;                   // zeroed on growth: the live flag and generation of unused slots are read
+  Columns ptrs;                  // MAXC rows: the column pointers on the device (for the gather kernels)
+  void** d_col = nullptr;        // ptrs' column
+  int32_t hw = 0;                // slots ever used
   int nlist = 0, lcol[4] = {};   // the per-slot (off, len) column pairs of the table's lists: off at lcol[l]
   int live_col = 0;
   std::unordered_map<int64_t, int32_t> slot_of;
   std::vector<int32_t> free;
 
+  Table(const int* sz, int ncol) : col(sz, ncol, 1024, true), ptrs({(int)sizeof(void*)}, 0, false) {}
   template <class T>
-  const T* at(int k) const { return static_cast<const T*>(col[k]); }
-  // capacity >= n: new columns, zeroed, the old contents copied (device to device)
+  const T* at(int k) const { return col.at<const T>(k); }
+  // capacity >= n: the columns grown, and a fresh pointer array naming them, so that col and d_col change together
   cudaError_t grow(int32_t n, cudaStream_t st) {
-    if (n <= cap) return cudaSuccess;
-    const int32_t ncap = std::max<int32_t>(n, std::max<int32_t>(2 * cap, 1024));
-    void* nc[P_NCOL] = {};
-    for (int k = 0; k < ncol; k++) {
-      cudaError_t e = cudaMalloc(&nc[k], (size_t)ncap * sz[k]);
-      if (e == cudaSuccess) e = cudaMemsetAsync(nc[k], 0, (size_t)ncap * sz[k], st);
-      if (e == cudaSuccess && col[k]) e = cudaMemcpyAsync(nc[k], col[k], (size_t)cap * sz[k], cudaMemcpyDeviceToDevice, st);
-      if (e != cudaSuccess) {
-        for (int j = 0; j <= k; j++) if (nc[j]) cudaFree(nc[j]);
-        return e;
-      }
-    }
-    if (!d_col) {
-      cudaError_t e = cudaMalloc(&d_col, sizeof(void*) * P_NCOL);
-      if (e != cudaSuccess) return e;
-    }
-    cudaError_t e = cudaMemcpyAsync(d_col, nc, sizeof(void*) * P_NCOL, cudaMemcpyHostToDevice, st);
+    if (n <= col.cap) return cudaSuccess;
+    Columns nc, np = ptrs.shape();
+    cudaError_t e = col.grown(n, col.cap, st, &nc);
+    if (e == cudaSuccess) e = np.grow(Columns::MAXC, 0, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(np[0], nc.p, sizeof(nc.p), cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return e;
-    for (int k = 0; k < ncol; k++) {
-      if (col[k]) cudaFree(col[k]);
-      col[k] = nc[k];
+    if (e != cudaSuccess) {
+      nc.release();
+      np.release();
+      return e;
     }
-    cap = ncap;
+    release();
+    col = nc;
+    ptrs = np;
+    d_col = ptrs.at<void*>(0);
     return cudaSuccess;
   }
   int32_t take_slot() {
     if (!free.empty()) { const int32_t s = free.back(); free.pop_back(); return s; }
     return hw++;
   }
-  void release() {
-    for (int k = 0; k < ncol; k++) if (col[k]) cudaFree(col[k]);
-    if (d_col) cudaFree(d_col);
-  }
+  void release() { col.release(); ptrs.release(); }
 };
 
+// A CSR arena: one value array, or two for (attribute column, value) pairs, whose second one holds doubles in an
+// offer's gpu or disk map; and its compaction target, freed when the arena grows and made again at the next compaction.
 struct ListArena {
-  int k = 1;                      // value arrays: 2 for (attribute column, value)
-  int esz1 = 4;                   // bytes per entry of v[1]: 8 when it holds doubles (an offer's gpu or disk map)
-  int32_t* v[2] = {};
-  int32_t* alt[2] = {};           // compaction target, same capacity
-  int64_t cap = 0, tail = 0, live = 0;
+  Columns v, alt;
+  int64_t tail = 0, live = 0;
+  explicit ListArena(std::initializer_list<int> widths = {4}) : v(widths, 4096, false), alt(v.shape()) {}
+  int32_t* at(int i) const { return v.at<int32_t>(i); }   // value array i, as int32
   cudaError_t grow(int64_t n, cudaStream_t st) {
-    if (n <= cap) return cudaSuccess;
-    const int64_t ncap = std::max<int64_t>(n, std::max<int64_t>(2 * cap, 4096));
-    for (int i = 0; i < k; i++) {
-      int32_t* p = nullptr;
-      const size_t es = i ? esz1 : sizeof(int32_t);
-      cudaError_t e = cudaMalloc(&p, es * ncap);
-      if (e == cudaSuccess && tail) e = cudaMemcpyAsync(p, v[i], es * tail, cudaMemcpyDeviceToDevice, st);
-      if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-      if (e != cudaSuccess) { if (p) cudaFree(p); return e; }
-      if (v[i]) cudaFree(v[i]);
-      v[i] = p;
-      if (alt[i]) cudaFree(alt[i]);
-      alt[i] = nullptr;
-    }
-    cap = ncap;
+    if (n <= v.cap) return cudaSuccess;
+    if (cudaError_t e = v.grow(n, tail, st)) return e;
+    alt.release();
     return cudaSuccess;
   }
-  void release() {
-    for (int i = 0; i < 2; i++) { if (v[i]) cudaFree(v[i]); if (alt[i]) cudaFree(alt[i]); }
-  }
+  void release() { v.release(); alt.release(); }
 };
 
-// The successful runtimes the straggler sweep measures against: an append-only SoA of (group code, whole seconds)
-// with a live flag, compacted (compact_records) once its dead records outnumber the live ones.
-struct Records {
-  int32_t* grp = nullptr; int32_t* rt = nullptr; uint8_t* live = nullptr;
-  int32_t* alt_grp = nullptr; int32_t* alt_rt = nullptr; uint8_t* alt_live = nullptr;   // compaction target
-  int64_t cap = 0, tail = 0, n_live = 0;
-  void free_all() {
-    for (void* p : {(void*)grp, (void*)rt, (void*)live, (void*)alt_grp, (void*)alt_rt, (void*)alt_live})
-      if (p) cudaFree(p);
-    grp = rt = alt_grp = alt_rt = nullptr;
-    live = alt_live = nullptr;
-  }
-  // capacity >= n: new columns holding the first `tail` records, both sets
-  cudaError_t grow(int64_t n, cudaStream_t st) {
-    if (n <= cap) return cudaSuccess;
-    const int64_t ncap = std::max<int64_t>(n, std::max<int64_t>(2 * cap, 4096));
-    int32_t *g = nullptr, *r = nullptr, *ag = nullptr, *ar = nullptr;
-    uint8_t *l = nullptr, *al = nullptr;
-    cudaError_t e = cudaMalloc(&g, 4 * ncap);
-    if (e == cudaSuccess) e = cudaMalloc(&r, 4 * ncap);
-    if (e == cudaSuccess) e = cudaMalloc(&l, ncap);
-    if (e == cudaSuccess) e = cudaMalloc(&ag, 4 * ncap);
-    if (e == cudaSuccess) e = cudaMalloc(&ar, 4 * ncap);
-    if (e == cudaSuccess) e = cudaMalloc(&al, ncap);
-    if (e == cudaSuccess && tail) e = cudaMemcpyAsync(g, grp, 4 * tail, cudaMemcpyDeviceToDevice, st);
-    if (e == cudaSuccess && tail) e = cudaMemcpyAsync(r, rt, 4 * tail, cudaMemcpyDeviceToDevice, st);
-    if (e == cudaSuccess && tail) e = cudaMemcpyAsync(l, live, tail, cudaMemcpyDeviceToDevice, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) {
-      for (void* p : {(void*)g, (void*)r, (void*)l, (void*)ag, (void*)ar, (void*)al}) if (p) cudaFree(p);
-      return e;
-    }
-    free_all();
-    grp = g; rt = r; live = l; alt_grp = ag; alt_rt = ar; alt_live = al;
-    cap = ncap;
-    return cudaSuccess;
-  }
-  void release() { free_all(); cap = tail = n_live = 0; }
-};
-
-// A handle's append-only device table (the history, the completed-job log): rows in arrival order, dense in [0, tail);
-// capacity doubles with device-to-device copies, and rows leave only by a stable compaction into new columns.  Off
-// until seeded; `since` is the horizon.  Cols: alloc(n), free_all(), and copy(src, n, stream) of the first n rows.
-template <class Cols>
+// A handle's append-only device table (the history, the completed-job log, the straggler records): rows in arrival
+// order, dense in [0, tail), in one column set; rows leave only by a stable compaction (LogKeep).  Off until seeded;
+// `since` is the horizon.
 struct Log {
-  Cols c;
-  int64_t cap = 0, tail = 0, since = 0;
+  Columns c;
+  int64_t tail = 0, since = 0;
   bool on = false;
-  // capacity >= n: new columns holding the first `tail` rows (device to device)
-  cudaError_t grow(int64_t n, cudaStream_t st) {
-    if (n <= cap) return cudaSuccess;
-    const int64_t ncap = std::max<int64_t>(n, std::max<int64_t>(2 * cap, 4096));
-    Cols nc;
-    cudaError_t e = nc.alloc(ncap);
-    if (e == cudaSuccess && tail) e = nc.copy(c, tail, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) { nc.free_all(); return e; }
-    c.free_all();
-    c = nc;
-    cap = ncap;
-    return cudaSuccess;
-  }
-  void release() { c.free_all(); cap = tail = since = 0; on = false; }
+  explicit Log(std::initializer_list<int> widths) : c(widths, 4096, false) {}
+  cudaError_t grow(int64_t n, cudaStream_t st) { return c.grow(n, tail, st); }
+  void release() { c.release(); tail = since = 0; on = false; }
 };
 
-// The finished instances (cook_state_history_*): 49 B per row; the horizon is on start time.
+// The successful runtimes the straggler sweep measures against: (group code, whole seconds) with a live flag,
+// compacted (compact_records) into its own target once its dead records outnumber the live ones.
+enum { RC_GRP, RC_RT, RC_LIVE };
+struct Records : Log {
+  Columns alt;   // compaction target: freed when the table grows, made again at the next compaction
+  int64_t n_live = 0;
+  Records() : Log({4, 4, 1}), alt(c.shape()) {}
+  cudaError_t grow(int64_t n, cudaStream_t st) {
+    if (n <= c.cap) return cudaSuccess;
+    if (cudaError_t e = Log::grow(n, st)) return e;
+    alt.release();
+    return cudaSuccess;
+  }
+  void release() { Log::release(); alt.release(); n_live = 0; }
+};
+
+// The finished instances (cook_state_history_*): 49 B per row; the horizon is on start time.  HistCols: the typed
+// columns, as the readers take them.
+enum { H_TID, H_START, H_END, H_CPUS, H_MEM, H_USER, H_REASON, H_OK };
 struct HistCols {
   int64_t* tid = nullptr; int64_t* start = nullptr; int64_t* end = nullptr; double* cpus = nullptr; double* mem = nullptr;
   int32_t* user = nullptr; int32_t* reason = nullptr; uint8_t* ok = nullptr;
-  cudaError_t alloc(int64_t n) {
-    cudaError_t e = cudaSuccess;
-    for (void** p : {(void**)&tid, (void**)&start, (void**)&end, (void**)&cpus, (void**)&mem})
-      if (e == cudaSuccess) e = cudaMalloc(p, 8 * n);
-    for (void** p : {(void**)&user, (void**)&reason}) if (e == cudaSuccess) e = cudaMalloc(p, 4 * n);
-    if (e == cudaSuccess) e = cudaMalloc(&ok, n);
-    if (e != cudaSuccess) free_all();
-    return e;
-  }
-  void free_all() {
-    for (void* p : {(void*)tid, (void*)start, (void*)end, (void*)cpus, (void*)mem, (void*)user, (void*)reason, (void*)ok})
-      if (p) cudaFree(p);
-    *this = HistCols{};
-  }
-  cudaError_t copy(const HistCols& s, int64_t n, cudaStream_t st) const {
-    const cudaMemcpyKind k = cudaMemcpyDeviceToDevice;
-    cudaError_t e = cudaMemcpyAsync(tid, s.tid, 8 * n, k, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(start, s.start, 8 * n, k, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(end, s.end, 8 * n, k, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(cpus, s.cpus, 8 * n, k, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(mem, s.mem, 8 * n, k, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(user, s.user, 4 * n, k, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(reason, s.reason, 4 * n, k, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(ok, s.ok, n, k, st);
-    return e;
+};
+struct History : Log {
+  History() : Log({8, 8, 8, 8, 8, 4, 4, 1}) {}
+  HistCols cols() const {
+    return {c.at<int64_t>(H_TID), c.at<int64_t>(H_START), c.at<int64_t>(H_END), c.at<double>(H_CPUS),
+            c.at<double>(H_MEM), c.at<int32_t>(H_USER), c.at<int32_t>(H_REASON), c.at<uint8_t>(H_OK)};
   }
 };
-using History = Log<HistCols>;
 
 // The completed-job log (cook_state_completed_*): 34 B per row, a job-state record each; the horizon is on submit time.
+// The device log and, by row on the host, each row's user and submit time: the listing sizes its buffers by the
+// user's rows, and the advance knows whose rows it drops, without a transfer.
+enum { CJ_JID, CJ_STAMP, CJ_SUBMIT, CJ_USER, CJ_SPOOL, CJ_EXEC, CJ_KIND };
 struct CJCols {
   int64_t* jid = nullptr; int64_t* stamp = nullptr; int64_t* submit = nullptr; int32_t* user = nullptr;
   int32_t* spool = nullptr; int8_t* exec = nullptr; uint8_t* kind = nullptr;
-  cudaError_t alloc(int64_t n) {
-    cudaError_t e = cudaSuccess;
-    for (void** p : {(void**)&jid, (void**)&stamp, (void**)&submit}) if (e == cudaSuccess) e = cudaMalloc(p, 8 * n);
-    for (void** p : {(void**)&user, (void**)&spool}) if (e == cudaSuccess) e = cudaMalloc(p, 4 * n);
-    for (void** p : {(void**)&exec, (void**)&kind}) if (e == cudaSuccess) e = cudaMalloc(p, n);
-    if (e != cudaSuccess) free_all();
-    return e;
-  }
-  void free_all() {
-    for (void* p : {(void*)jid, (void*)stamp, (void*)submit, (void*)user, (void*)spool, (void*)exec, (void*)kind})
-      if (p) cudaFree(p);
-    *this = CJCols{};
-  }
-  cudaError_t copy(const CJCols& s, int64_t n, cudaStream_t st) const {
-    const cudaMemcpyKind k = cudaMemcpyDeviceToDevice;
-    cudaError_t e = cudaMemcpyAsync(jid, s.jid, 8 * n, k, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(stamp, s.stamp, 8 * n, k, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(submit, s.submit, 8 * n, k, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(user, s.user, 4 * n, k, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(spool, s.spool, 4 * n, k, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(exec, s.exec, n, k, st);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(kind, s.kind, n, k, st);
-    return e;
-  }
 };
-// The device log and, by row on the host, each row's user and submit time: the listing sizes its buffers by the
-// user's rows, and the advance knows whose rows it drops, without a transfer.
-struct Completed : Log<CJCols> {
+struct Completed : Log {
   std::vector<int32_t> h_user;
   std::vector<int64_t> h_submit;
   std::unordered_map<int32_t, int64_t> users;   // user -> rows
+  Completed() : Log({8, 8, 8, 4, 4, 1, 1}) {}
+  CJCols cols() const {
+    return {c.at<int64_t>(CJ_JID), c.at<int64_t>(CJ_STAMP), c.at<int64_t>(CJ_SUBMIT), c.at<int32_t>(CJ_USER),
+            c.at<int32_t>(CJ_SPOOL), c.at<int8_t>(CJ_EXEC), c.at<uint8_t>(CJ_KIND)};
+  }
   void clear_rows() { tail = 0; h_user.clear(); h_submit.clear(); users.clear(); }
-  void release() { Log<CJCols>::release(); clear_rows(); }
+  void release() { Log::release(); clear_rows(); }
 };
 
 void count_add(std::map<int32_t, int64_t>& m, int32_t code, int64_t d) {
@@ -878,18 +854,19 @@ struct MetricsRound {
   int32_t n_rows = 0;
   int64_t epoch = 0;
   uint64_t run = 0;
-  int32_t* slot = nullptr; int64_t slot_cap = 0;
-  int64_t* u_jid[2] = {}; int32_t* u_cyc[2] = {}; int64_t u_cap = 0; int cur = 0; int32_t u_n = 0;
+  Columns slot{{4}, 0, false};
+  Columns u[2] = {Columns({8, 4}, 0, false), Columns({8, 4}, 0, false)};   // (job id, cycles) each
+  int cur = 0; int32_t u_n = 0;
   void release() {
-    for (void* p : {(void*)slot, (void*)u_jid[0], (void*)u_jid[1], (void*)u_cyc[0], (void*)u_cyc[1]}) if (p) cudaFree(p);
+    slot.release(); u[0].release(); u[1].release();
     *this = MetricsRound{};
   }
 };
 
 struct PoolState {
-  Table pend, run;
+  Table pend{P_SZ, P_NCOL}, run{R_SZ, R_NCOL};
   // ---- the live offers (cook_state_offers_add, cook_state_match_offers)
-  Table offer;
+  Table offer{O_SZ, O_NCOL};
   std::vector<OfferInfo> oinfo;                  // by offer slot
   std::unordered_map<int32_t, OfferHost> ohost;  // by hostname code, every code the handle has a name for
   std::map<std::string, int32_t> code_of_name;   // every name the handle knows (byte order)
@@ -931,7 +908,7 @@ struct PoolState {
   std::unordered_map<int64_t, RetryFacts> retry;     // job id -> its facts
   std::unordered_map<int64_t, int32_t> parked;       // job id -> its parked pending slot
   int64_t park_len[3] = {};                          // list entries the parked slots hold (kept by the compaction)
-  uint8_t* park = nullptr; int32_t park_cap = 0;     // per pending slot: 1 while parked; allocated at the first park
+  Columns park{{1}, 0, true};                        // per pending slot: 1 while parked; allocated at the first park
   Arena stage;                        // one batch's uploads
   Arena scratch;                      // one call's device buffers
   Arena derive;                       // a derived match's or rebalance's running-side scratch (scratch is live then)
@@ -944,17 +921,14 @@ struct PoolState {
   bool ranked = false;
 
   PoolState() {
-    pend.ncol = P_NCOL; pend.sz = P_SZ;
-    run.ncol = R_NCOL; run.sz = R_SZ;
     pend.nlist = 3; pend.lcol[L_NOVEL] = P_NOFF; pend.lcol[L_ATTR] = P_AOFF; pend.lcol[L_GROUP] = P_GOFF;
     run.nlist = 1; run.lcol[0] = R_GOFF;
     pend.live_col = P_LIVE; run.live_col = R_LIVE;
-    offer.ncol = O_NCOL; offer.sz = O_SZ; offer.live_col = O_LIVE;
+    offer.live_col = O_LIVE;
     offer.nlist = 4;
     for (int l = 0; l < 4; l++) offer.lcol[l] = O_POFF + 2 * l;
-    lists[L_ATTR].k = 2;
-    olists[OL_PORT].k = olists[OL_GPU].k = olists[OL_DISK].k = 2;
-    olists[OL_GPU].esz1 = olists[OL_DISK].esz1 = 8;
+    lists[L_ATTR] = olists[OL_PORT] = ListArena({4, 4});
+    olists[OL_GPU] = olists[OL_DISK] = ListArena({4, 8});
   }
   void release() {
     pend.release(); run.release(); offer.release(); rec.release(); hist.release(); cj.release();
@@ -962,7 +936,7 @@ struct PoolState {
     for (auto& l : olists) l.release();
     stage.release(); scratch.release(); derive.release(); queue.release(); omerge.release();
     mm.release();
-    if (park) cudaFree(park);
+    park.release();
     if (counters) cudaFree(counters);
     if (gf0) cudaFree(gf0);
   }
@@ -1005,20 +979,9 @@ struct PoolState {
     ruser.resize(n); rhost.resize(n); rgroups.resize(n); rstart.resize(n); rfacts.resize(n); rjid.resize(n); rtid.resize(n);
     rreason.resize(n);
   }
-  // the park flags cover every pending slot: new ones zeroed, the old ones copied (device to device)
-  cudaError_t park_room(cudaStream_t st) {
-    if (park_cap >= pend.cap) return cudaSuccess;
-    uint8_t* p = nullptr;
-    cudaError_t e = cudaMalloc(&p, (size_t)pend.cap);
-    if (e == cudaSuccess) e = cudaMemsetAsync(p, 0, (size_t)pend.cap, st);
-    if (e == cudaSuccess && park_cap) e = cudaMemcpyAsync(p, park, (size_t)park_cap, cudaMemcpyDeviceToDevice, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) { if (p) cudaFree(p); return e; }
-    if (park) cudaFree(park);
-    park = p;
-    park_cap = pend.cap;
-    return cudaSuccess;
-  }
+  // the park flags cover every pending slot, new ones zeroed: their capacity is exactly pend's, since each growth of
+  // pend at least doubles it and the flags' capacity is one pend had before
+  cudaError_t park_room(cudaStream_t st) { return park.grow(pend.col.cap, park.cap, st); }
   // job jid's parked copy, if any, is freed: its slot back on the free list (appended to *freed), its entries dead
   void unpark(int64_t jid, std::vector<int32_t>* freed) {
     auto it = parked.find(jid);
@@ -1103,8 +1066,8 @@ void gather_lists(const PoolState* S, const JobDev& o, const int32_t* m_slot, in
     if (!doff[l]) continue;
     const int32_t* len = S->pend.at<int32_t>(loff[l] + 1);
     order_scan(os, RowLen{m_slot, len}, n, S->gf0, st, nl);
-    csr_gather_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, m_slot, n, S->pend.at<int32_t>(loff[l]), len, S->lists[l].v[0],
-                                                   S->lists[l].v[1], writable(doff[l]), writable(dst[l][0]),
+    csr_gather_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, m_slot, n, S->pend.at<int32_t>(loff[l]), len, S->lists[l].at(0),
+                                                   S->lists[l].at(1), writable(doff[l]), writable(dst[l][0]),
                                                    writable(dst[l][1]));
     (*nl)++;
   }
@@ -1120,8 +1083,7 @@ int32_t compact_lists(cook_pool* pool, PoolState* S, cudaStream_t st, int* nl) {
     const Table& t = l == L_RGROUP ? S->run : l >= L_N ? S->offer : S->pend;
     const int n = t.hw, oc = t.lcol[l == L_RGROUP ? 0 : l >= L_N ? l - L_N : l];
     if (kept > 0 && n > 0) {
-      for (int i = 0; i < A.k; i++)
-        if (!A.alt[i]) CK(pool, cudaMalloc(&A.alt[i], (i ? A.esz1 : sizeof(int32_t)) * std::max<int64_t>(A.cap, 1)));
+      CK(pool, A.alt.grow(A.v.cap, 0, st));
       if (parked) CK(pool, S->park_room(st));
       OrderScan<int, 1> os;
       uint8_t* keep = nullptr;
@@ -1132,23 +1094,22 @@ int32_t compact_lists(cook_pool* pool, PoolState* S, cudaStream_t st, int* nl) {
       }));
       const uint8_t* live = static_cast<const uint8_t*>(t.col[t.live_col]);
       if (parked) {
-        park_keep_kernel<<<(n + 255) / 256, 256, 0, st>>>(live, S->park, n, keep);
+        park_keep_kernel<<<(n + 255) / 256, 256, 0, st>>>(live, S->park.at<uint8_t>(0), n, keep);
         (*nl)++;
         live = keep;
       }
       int32_t* off = static_cast<int32_t*>(t.col[oc]);
       const int32_t* len = static_cast<const int32_t*>(t.col[oc + 1]);
       order_scan(os, SlotLen{live, len}, n, S->gf0, st, nl);
-      if (A.esz1 == 8)
-        list_compact_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, live, off, len, n, A.v[0],
-                                                         reinterpret_cast<const double*>(A.v[1]), A.alt[0],
-                                                         reinterpret_cast<double*>(A.alt[1]));
+      if (A.v.w[1] == 8)
+        list_compact_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, live, off, len, n, A.at(0), A.v.at<double>(1),
+                                                         A.alt.at<int32_t>(0), A.alt.at<double>(1));
       else
-        list_compact_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, live, off, len, n, A.v[0], A.v[1], A.alt[0],
-                                                         A.k > 1 ? A.alt[1] : nullptr);
+        list_compact_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, live, off, len, n, A.at(0), A.at(1),
+                                                         A.alt.at<int32_t>(0), A.alt.at<int32_t>(1));
       (*nl)++;
       CK(pool, cudaGetLastError());
-      for (int i = 0; i < A.k; i++) std::swap(A.v[i], A.alt[i]);
+      std::swap(A.v, A.alt);
     }
     A.tail = kept;
   }
@@ -1185,7 +1146,7 @@ void patch_args(Carve& c, ScatterArgs& a, const Table& t, const int32_t* slot, i
   a.nc = 0;
   for (const PatchCol& p : cols) {
     if (!p.src) continue;
-    const int sz = t.sz[p.col];
+    const int sz = t.col.w[p.col];
     const char* up = sz == 1   ? reinterpret_cast<const char*>(c.up(static_cast<const uint8_t*>(p.src), n))
                      : sz == 4 ? reinterpret_cast<const char*>(c.up(static_cast<const int32_t*>(p.src), n))
                                : reinterpret_cast<const char*>(c.up(static_cast<const int64_t*>(p.src), n));
@@ -1334,7 +1295,7 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
     S->jf_keyed = 0;
     S->mm.on = false;
     S->mm.u_n = 0;
-    if (!S->parked.empty()) CK(pool, cudaMemsetAsync(S->park, 0, (size_t)S->park_cap, st));
+    if (!S->parked.empty()) CK(pool, cudaMemsetAsync(S->park[0], 0, (size_t)S->park.cap, st));
     S->parked.clear();
     S->retry.clear();
     for (auto& l : S->park_len) l = 0;
@@ -1439,7 +1400,7 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
   StateWrite w(pool, S);
   if (int32_t rc = w.up([&](Carve& c) {
     if (nuk) {
-      uk.c[0] = ScatterCol{reinterpret_cast<char*>(S->park), nullptr, 0, 1};
+      uk.c[0] = ScatterCol{S->park.at<char>(0), nullptr, 0, 1};
       uk.nc = 1;
       uk.slot = c.up(unparked.data(), nuk);
     }
@@ -1462,8 +1423,7 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
       for (int l = 0; l < 3; l++) {
         pu.doff[l] = c.up(lists_off[l], np + 1);
         const int64_t nv = lists_off[l] ? lists_off[l][np] : 0;
-        for (int i = 0; i < S->lists[l].k; i++)
-          if (c.base && nv) c.copy(S->lists[l].v[i] + tail0[l], lists_v[l][i], nv);
+        if (c.base && nv) S->lists[l].v.copy(c, tail0[l], nv, {lists_v[l][0], lists_v[l][1]});
       }
     }
     if (npr) pr.slot = c.up(prm_slot.data(), npr);
@@ -1481,7 +1441,7 @@ int32_t apply(cook_pool* pool, PoolState* S, const cook_state_delta* d) {
         ru.c[ru.nc++] = ScatterCol{static_cast<char*>(S->run.col[r.col]), nullptr, r.dflt, R_SZ[r.col]};
       ru.slot = c.up(rup_slot.data(), nr);
       ru.doff[0] = c.up(rgo, nr + 1);
-      if (c.base && radd) c.copy(RG.v[0] + rtail0, d->running_group_idx, radd);
+      if (c.base && radd) RG.v.copy(c, rtail0, radd, {d->running_group_idx});
     }
     if (nrr) rr.slot = c.up(rrm_slot.data(), nrr);
   }))
@@ -1582,8 +1542,8 @@ int32_t launch(cook_pool* pool, PoolState* S, const char* who, int n, const int6
       const int32_t* plen = S->pend.at<int32_t>(P_GLEN);
       order_scan(os, RowLen{d_pslot, plen}, n, S->gf0, st, &w.nl);
       launch_lists_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, d_pslot, d_rslot, n, S->pend.at<int32_t>(P_GOFF), plen,
-                                                       S->lists[L_GROUP].v[0], static_cast<int32_t*>(S->run.col[R_GOFF]),
-                                                       static_cast<int32_t*>(S->run.col[R_GLEN]), RG.v[0], rtail0);
+                                                       S->lists[L_GROUP].at(0), static_cast<int32_t*>(S->run.col[R_GOFF]),
+                                                       static_cast<int32_t*>(S->run.col[R_GLEN]), RG.at(0), rtail0);
       w.nl++;
     }
     ScatterArgs rm;
@@ -1595,7 +1555,7 @@ int32_t launch(cook_pool* pool, PoolState* S, const char* who, int n, const int6
     if (nk) {   // parking: the live flag cleared and the generation bumped as a removal's, the lists kept
       ScatterArgs pk;
       memset(&pk, 0, sizeof(pk));
-      pk.c[0] = ScatterCol{reinterpret_cast<char*>(S->park), nullptr, 1, 1};
+      pk.c[0] = ScatterCol{S->park.at<char>(0), nullptr, 1, 1};
       pk.nc = 1;
       pk.slot = d_kslot;
       scatter(pk, S->pend, nk, 0, P_LIVE, nullptr, st, &w.nl);
@@ -1873,7 +1833,7 @@ struct CotaskList {
   // the rows, their entries, the (group, task id) order, the outputs
   cudaError_t run(const PoolState* S, cudaStream_t st, int* nl) {
     a.K = K;
-    a.goff = S->run.at<int32_t>(R_GOFF); a.glen = S->run.at<int32_t>(R_GLEN); a.arena = S->lists[L_RGROUP].v[0];
+    a.goff = S->run.at<int32_t>(R_GOFF); a.glen = S->run.at<int32_t>(R_GLEN); a.arena = S->lists[L_RGROUP].at(0);
     a.host = S->run.at<int32_t>(R_HOST); a.tid = S->run.at<int64_t>(R_TID);
     compact(CotaskRows{S->run.at<uint8_t>(R_LIVE), a.host, a.glen, writable(a.slot)}, S->run.hw, nullptr, blk,
             S->counters + 3, K, st, nl);
@@ -2379,13 +2339,7 @@ int32_t offers_add(cook_pool* pool, PoolState* S, const char* who, const cook_of
     a.slot = c.up(slot.data(), n);
     for (int l = 0; l < OL_N; l++) {
       a.doff[l] = c.up(loff[l], n + 1);
-      if (!c.base || !nv[l]) continue;
-      ListArena& A = S->olists[l];
-      c.copy(A.v[0] + tail0[l], lv0[l], nv[l]);
-      if (A.k > 1 && A.esz1 == 8)
-        c.copy(reinterpret_cast<double*>(A.v[1]) + tail0[l], static_cast<const double*>(lv1[l]), nv[l]);
-      else if (A.k > 1)
-        c.copy(A.v[1] + tail0[l], static_cast<const int32_t*>(lv1[l]), nv[l]);
+      if (c.base && nv[l]) S->olists[l].v.copy(c, tail0[l], nv[l], {lv0[l], lv1[l]});
     }
   }))
     return rc;
@@ -2465,11 +2419,11 @@ int32_t offers_merge(cook_pool* pool, PoolState* S, OfferPass& op, const MatchRo
   if (oc.port_off) {
     const int32_t* plen = S->offer.at<int32_t>(O_PLEN);
     order_scan(osp, RowLen{ss, plen}, L, S->gf0, st, nl);
-    csr_gather_kernel<<<(L + 7) / 8, 256, 0, st>>>(osp, ss, L, S->offer.at<int32_t>(O_POFF), plen, A[OL_PORT].v[0],
-                                                   A[OL_PORT].v[1], ldoff, oc.port_begin, oc.port_end);
+    csr_gather_kernel<<<(L + 7) / 8, 256, 0, st>>>(osp, ss, L, S->offer.at<int32_t>(O_POFF), plen, A[OL_PORT].at(0),
+                                                   A[OL_PORT].at(1), ldoff, oc.port_begin, oc.port_end);
     (*nl)++;
   }
-  MergeArgs ma = {S->offer.d_col, ss, start, end, O, osp, A[OL_ATTR].v[0], oc, op.osh.n_attr_cols, newest};
+  MergeArgs ma = {S->offer.d_col, ss, start, end, O, osp, A[OL_ATTR].at(0), oc, op.osh.n_attr_cols, newest};
   offer_merge_kernel<<<(O + 127) / 128, 128, 0, st>>>(ma);
   (*nl)++;
   const int lists[2] = {OL_GPU, OL_DISK};
@@ -2479,8 +2433,8 @@ int32_t offers_merge(cook_pool* pool, PoolState* S, OfferPass& op, const MatchRo
     OrderScan<int, 1>& os = l == OL_GPU ? osg : osd;
     const int32_t* len = S->offer.at<int32_t>(O_POFF + 2 * l + 1);
     order_scan(os, RowLen{newest, len}, O, S->gf0, st, nl);
-    csr_gather_kernel<<<(O + 7) / 8, 256, 0, st>>>(os, newest, O, S->offer.at<int32_t>(O_POFF + 2 * l), len, A[l].v[0],
-                                                   reinterpret_cast<const double*>(A[l].v[1]), doff,
+    csr_gather_kernel<<<(O + 7) / 8, 256, 0, st>>>(os, newest, O, S->offer.at<int32_t>(O_POFF + 2 * l), len, A[l].at(0),
+                                                   A[l].v.at<double>(1), doff,
                                                    l == OL_GPU ? oc.gpu_model : oc.disk_type,
                                                    l == OL_GPU ? oc.gpu_count : oc.disk_space);
     (*nl)++;
@@ -2569,15 +2523,8 @@ namespace {
 // transfer between host and device), the pending epoch and the plan's run.
 int32_t mm_record(cook_pool* pool, PoolState* S, const int32_t* m_slot, int n) {
   MetricsRound& R = S->mm;
-  if (n > R.slot_cap) {
-    const int64_t cap = std::max<int64_t>(n, 2 * R.slot_cap);
-    if (R.slot) cudaFree(R.slot);
-    R.slot = nullptr;
-    R.slot_cap = 0;
-    CK(pool, cudaMalloc(&R.slot, sizeof(int32_t) * cap));
-    R.slot_cap = cap;
-  }
-  if (n) CK(pool, cudaMemcpyAsync(R.slot, m_slot, sizeof(int32_t) * n, cudaMemcpyDeviceToDevice, pool->stream));
+  CK(pool, R.slot.grow(n, 0, pool->stream));
+  if (n) CK(pool, cudaMemcpyAsync(R.slot[0], m_slot, sizeof(int32_t) * n, cudaMemcpyDeviceToDevice, pool->stream));
   R.n_rows = n;
   R.epoch = S->pend_epoch;
   R.run = match_runs(pool);
@@ -2774,14 +2721,14 @@ int32_t state_match(cook_pool* pool, const char* who, bool derived, const cook_o
   if (has(F_PORTS)) c.ports = P.at<int32_t>(P_PORTS);
   if (has(F_NOT_ALLOWED)) c.allowed = P.at<uint8_t>(P_ALLOWED);
   if (has(F_NOT_PLUGIN)) c.plugin = P.at<uint8_t>(P_PLUGIN);
-  if (L[L_NOVEL].live) { c.novel_off = P.at<int32_t>(P_NOFF); c.novel_host = L[L_NOVEL].v[0]; }
+  if (L[L_NOVEL].live) { c.novel_off = P.at<int32_t>(P_NOFF); c.novel_host = L[L_NOVEL].at(0); }
   if (has(F_GPU_MODEL)) c.gpu_model = P.at<int32_t>(P_GPU_MODEL);
   if (has(F_DISK)) { c.disk_request = P.at<double>(P_DISK_REQ); c.disk_type = P.at<int32_t>(P_DISK_TYPE); }
-  if (L[L_ATTR].live) { c.attr_off = P.at<int32_t>(P_AOFF); c.attr_col = L[L_ATTR].v[0]; c.attr_val = L[L_ATTR].v[1]; }
+  if (L[L_ATTR].live) { c.attr_off = P.at<int32_t>(P_AOFF); c.attr_col = L[L_ATTR].at(0); c.attr_val = L[L_ATTR].at(1); }
   if (has(F_EST)) c.est_end_ms = P.at<int64_t>(P_EST);
   if (has(F_CKPT)) c.ckpt_location = P.at<int32_t>(P_CKPT);
   if (has(F_RESERVED)) c.reserved_host = P.at<int32_t>(P_RESERVED);
-  if (L[L_GROUP].live) { c.group_off = P.at<int32_t>(P_GOFF); c.group_idx = L[L_GROUP].v[0]; }
+  if (L[L_GROUP].live) { c.group_off = P.at<int32_t>(P_GOFF); c.group_idx = L[L_GROUP].at(0); }
   sh.n_novel = L[L_NOVEL].live; sh.n_attr = L[L_ATTR].live; sh.n_group = L[L_GROUP].live;
   sh.gp_off.assign(G + 1, 0);
   for (const auto& kv : S->groups) if (kv.first < G) sh.gp_off[kv.first + 1] = (int32_t)kv.second;
@@ -3462,10 +3409,27 @@ __global__ void forget_records_kernel(const int32_t* grp, uint8_t* live, int n_r
   if (lo < n && forget[lo] == g) live[i] = 0;
 }
 
-struct RecordKeep {   // the record table's compaction
-  const int32_t* grp; const int32_t* rt; const uint8_t* live; int32_t* d_grp; int32_t* d_rt; uint8_t* d_live;
-  __device__ bool keep(int i) const { return live[i]; }
-  __device__ void emit(int i, int d) const { d_grp[d] = grp[i]; d_rt[d] = rt[i]; d_live[d] = 1; }
+// A log's compaction into a target of its shape: every column copied by its width, in order, for the rows whose live
+// byte is set (live non-null) or else whose int64 key is at or after the horizon
+struct LogKeep {
+  static constexpr int MAXC = 8;   // the widest log, the history
+  const char* s[MAXC]; char* d[MAXC]; int w[MAXC]; int n;
+  const uint8_t* live; const int64_t* key; int64_t since;
+  LogKeep(const Columns& from, const Columns& to, const uint8_t* lv, const int64_t* k, int64_t t)
+      : n(from.n), live(lv), key(k), since(t) {
+    assert(n <= MAXC);
+    for (int c = 0; c < n; c++) { s[c] = from.at<const char>(c); d[c] = to.at<char>(c); w[c] = from.w[c]; }
+  }
+  __device__ bool keep(int i) const { return live ? live[i] != 0 : key[i] >= since; }
+  __device__ void emit(int i, int k) const {
+#pragma unroll
+    for (int c = 0; c < MAXC; c++) {
+      if (c >= n) break;
+      if (w[c] == 8) reinterpret_cast<int64_t*>(d[c])[k] = reinterpret_cast<const int64_t*>(s[c])[i];
+      else if (w[c] == 4) reinterpret_cast<int32_t*>(d[c])[k] = reinterpret_cast<const int32_t*>(s[c])[i];
+      else d[c][k] = s[c][i];   // width 1 (Columns allows 1, 4 and 8)
+    }
+  }
 };
 
 // the arena rule on the record table: compacted once its dead records outnumber the live ones
@@ -3473,12 +3437,13 @@ int32_t compact_records(cook_pool* pool, PoolState* S, cudaStream_t st, int* nl)
   Records& R = S->rec;
   if (R.tail - R.n_live <= R.n_live) return COOK_OK;
   if (R.n_live > 0) {
+    CK(pool, R.alt.grow(R.c.cap, 0, st));
     int32_t* blk = nullptr;
     CK(pool, carve(S->scratch, st, nullptr, nullptr, [&](Carve& c) { blk = c.take<int32_t>((size_t)R.tail / CP_BLOCK + 2); }));
-    compact(RecordKeep{R.grp, R.rt, R.live, R.alt_grp, R.alt_rt, R.alt_live}, (int)R.tail, nullptr, blk, S->counters + 6,
+    compact(LogKeep(R.c, R.alt, R.c.at<uint8_t>(RC_LIVE), nullptr, 0), (int)R.tail, nullptr, blk, S->counters + 6,
             (int)R.n_live, st, nl);
     CK(pool, cudaGetLastError());
-    std::swap(R.grp, R.alt_grp); std::swap(R.rt, R.alt_rt); std::swap(R.live, R.alt_live);
+    std::swap(R.c, R.alt);
   }
   R.tail = R.n_live;
   return COOK_OK;
@@ -3668,7 +3633,7 @@ int32_t finish(cook_pool* pool, PoolState* S, const char* who, int n, const int6
       rq.nc = 0;   // carve runs this body twice: once to size, once to upload
       rq.c[rq.nc++] = ScatterCol{static_cast<char*>(S->pend.col[P_RESERVED]), nullptr, -1, P_SZ[P_RESERVED]};
       rq.c[rq.nc++] = ScatterCol{static_cast<char*>(S->pend.col[P_JF]), nullptr, 0, P_SZ[P_JF]};
-      rq.c[rq.nc++] = ScatterCol{reinterpret_cast<char*>(S->park), nullptr, 0, 1};
+      rq.c[rq.nc++] = ScatterCol{S->park.at<char>(0), nullptr, 0, 1};
       rq.slot = c.up(rq_slot.data(), nrq);
     }
     if (nap) {
@@ -3678,7 +3643,7 @@ int32_t finish(cook_pool* pool, PoolState* S, const char* who, int n, const int6
       aos.tile[0] = c.take<int32_t>((nap + OS_TILE - 1) / OS_TILE + 1);
     }
     if (nuk) {
-      uk.c[0] = ScatterCol{reinterpret_cast<char*>(S->park), nullptr, 0, 1};
+      uk.c[0] = ScatterCol{S->park.at<char>(0), nullptr, 0, 1};
       uk.nc = 1;
       uk.slot = c.up(unparked.data(), nuk);
     }
@@ -3698,11 +3663,12 @@ int32_t finish(cook_pool* pool, PoolState* S, const char* who, int n, const int6
   if (nrec) {
     order_scan(os, FinishLen{d_slot, d_ok, S->run.at<int32_t>(R_GLEN)}, n, S->gf0, st, &nl);
     finish_records_kernel<<<(n + 7) / 8, 256, 0, st>>>(os, d_slot, d_ok, d_end, n, S->run.d_col,
-                                                       S->lists[L_RGROUP].v[0], RC.grp, RC.rt, RC.live, rtail);
+                                                       S->lists[L_RGROUP].at(0), RC.c.at<int32_t>(RC_GRP),
+                                                       RC.c.at<int32_t>(RC_RT), RC.c.at<uint8_t>(RC_LIVE), rtail);
     nl++;
   }
   if (nhist)   // read from the running rows before the removal
-    compact(HistAppend{d_slot, d_end, d_ok, d_reason, S->run.d_col, H.since, H.c, htail}, n, nullptr, hblk,
+    compact(HistAppend{d_slot, d_end, d_ok, d_reason, S->run.d_col, H.since, H.cols(), htail}, n, nullptr, hblk,
             S->counters + 7, (int)nhist, st, &nl);
   if (n) {
     ScatterArgs rr;
@@ -3714,7 +3680,7 @@ int32_t finish(cook_pool* pool, PoolState* S, const char* who, int n, const int6
     order_scan(aos, NovelLen{d_ap_slot, S->pend.at<int32_t>(P_NLEN)}, nap, S->gf0, st, &nl);
     requeue_novel_kernel<<<(nap + 7) / 8, 256, 0, st>>>(aos, d_ap_slot, d_ap_code, nap,
                                                         static_cast<int32_t*>(S->pend.col[P_NOFF]),
-                                                        static_cast<int32_t*>(S->pend.col[P_NLEN]), NV.v[0], ntail);
+                                                        static_cast<int32_t*>(S->pend.col[P_NLEN]), NV.at(0), ntail);
     nl++;
   }
   scatter(rq, S->pend, nrq, 1, P_LIVE, nullptr, st, &nl);
@@ -3784,7 +3750,7 @@ int32_t retry_facts(cook_pool* pool, PoolState* S, const char* who, int n, const
   StateWrite w(pool, S);
   if (int32_t rc = w.up([&](Carve& c) {
     if (!nuk) return;
-    uk.c[0] = ScatterCol{reinterpret_cast<char*>(S->park), nullptr, 0, 1};
+    uk.c[0] = ScatterCol{S->park.at<char>(0), nullptr, 0, 1};
     uk.nc = 1;
     uk.slot = c.up(unparked.data(), nuk);
   }))
@@ -3823,21 +3789,30 @@ int32_t history_seed(cook_pool* pool, PoolState* S, const char* who, int64_t sin
   StateWrite w(pool, S);
   if (int32_t rc = w.direct([&](Carve& c) {
     if (!n) return;
-    c.copy(H.c.tid, task_id, n); c.copy(H.c.user, user, n); c.copy(H.c.start, start_ms, n); c.copy(H.c.end, end_ms, n);
-    c.copy(H.c.cpus, cpus, n); c.copy(H.c.mem, mem, n); c.copy(H.c.ok, success, n); c.copy(H.c.reason, reason_code, n);
+    H.c.copy(c, 0, n, {task_id, start_ms, end_ms, cpus, mem, user, reason_code, success});
   }))
     return rc;
   return w.end();
 }
 
-struct HistKeep {   // the advance's compaction: the rows that start at or after the new horizon, in order
-  HistCols s, d; int64_t since;
-  __device__ bool keep(int i) const { return s.start[i] >= since; }
-  __device__ void emit(int i, int k) const {
-    d.tid[k] = s.tid[i]; d.user[k] = s.user[i]; d.start[k] = s.start[i]; d.end[k] = s.end[i];
-    d.cpus[k] = s.cpus[i]; d.mem[k] = s.mem[i]; d.reason[k] = s.reason[i]; d.ok[k] = s.ok[i];
-  }
-};
+// A log's horizon raised to since_ms: its rows whose int64 column `key` is before it leave in one compaction into new
+// columns of its capacity (blk: the compaction's block counts), and the log takes them and the kept count, or is left
+// as it was.
+int32_t log_advance(cook_pool* pool, PoolState* S, StateWrite& w, Log& L, int key, int64_t since_ms, int32_t* blk) {
+  const int T = (int)L.tail;
+  Columns nc = L.c.shape();
+  CK(pool, nc.grow(L.c.cap, 0, w.st));
+  compact(LogKeep(L.c, nc, nullptr, L.c.at<int64_t>(key), since_ms), T, nullptr, blk, S->counters + 7, T, w.st, &w.nl);
+  int32_t kept = 0;
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) e = download(&kept, S->counters + 7, 1, w.st, &w.d2h);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(w.st);
+  if (e != cudaSuccess) { nc.release(); CK(pool, e); }
+  L.c.release();
+  L.c = nc;
+  L.tail = kept;
+  return COOK_OK;
+}
 
 // the horizon raised to since_ms: the rows that start before it leave in one compaction into new columns
 int32_t history_advance(cook_pool* pool, PoolState* S, const char* who, int64_t since_ms) {
@@ -3851,19 +3826,8 @@ int32_t history_advance(cook_pool* pool, PoolState* S, const char* who, int64_t 
     if (T && since_ms > H.since) blk = c.take<int32_t>((size_t)T / CP_BLOCK + 2);
   }))
     return rc;
-  if (T && since_ms > H.since) {
-    HistCols nc;
-    CK(pool, nc.alloc(H.cap));
-    compact(HistKeep{H.c, nc, since_ms}, T, nullptr, blk, S->counters + 7, T, w.st, &w.nl);
-    int32_t kept = 0;
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = download(&kept, S->counters + 7, 1, w.st, &w.d2h);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(w.st);
-    if (e != cudaSuccess) { nc.free_all(); CK(pool, e); }
-    H.c.free_all();
-    H.c = nc;
-    H.tail = kept;
-  }
+  if (T && since_ms > H.since)
+    if (int32_t rc = log_advance(pool, S, w, H, H_START, since_ms, blk)) return rc;
   H.since = since_ms;
   return w.end();
 }
@@ -3899,17 +3863,15 @@ int32_t group_runtimes(cook_pool* pool, PoolState* S, const char* who, int n_add
   StateWrite w(pool, S);
   if (int32_t rc = w.up([&](Carve& c) {
     if (nf) d_forget = c.up(forget.data(), nf);
-    if (c.base && n_add) {
-      c.copy(RC.grp + tail0, group, n_add);
-      c.copy(RC.rt + tail0, runtime_s, n_add);
-    }
+    if (c.base && n_add) RC.c.copy(c, tail0, n_add, {group, runtime_s});
   }))
     return rc;
   if (nf && tail0) {
-    forget_records_kernel<<<(tail0 + 255) / 256, 256, 0, st>>>(RC.grp, RC.live, tail0, d_forget, nf);
+    forget_records_kernel<<<(tail0 + 255) / 256, 256, 0, st>>>(RC.c.at<int32_t>(RC_GRP), RC.c.at<uint8_t>(RC_LIVE),
+                                                               tail0, d_forget, nf);
     w.nl++;
   }
-  if (n_add) CK(pool, cudaMemsetAsync(RC.live + tail0, 1, (size_t)n_add, st));
+  if (n_add) CK(pool, cudaMemsetAsync(RC.c.at<uint8_t>(RC_LIVE) + tail0, 1, (size_t)n_add, st));
   RC.tail += n_add;
   RC.n_live += n_add;
   if (int32_t rc = compact_records(pool, S, st, &w.nl)) return rc;
@@ -4131,7 +4093,8 @@ int32_t sweep(cook_pool* const* pools, int n, int64_t now, int64_t dflt, int64_t
         for (const auto& kv : h.first->rec_groups)
           if (kind[kv.first] == COOK_SWEEP_QUANTILE_DEVIATION) mk += kv.second;
         if (!mk) continue;
-        compact(SweepRecords{rc.grp, rc.rt, rc.live, d_kind, base, r_grp, r_rt}, (int)rc.tail, nullptr, blk, cnt + 4,
+        compact(SweepRecords{rc.c.at<int32_t>(RC_GRP), rc.c.at<int32_t>(RC_RT), rc.c.at<uint8_t>(RC_LIVE), d_kind, base,
+                             r_grp, r_rt}, (int)rc.tail, nullptr, blk, cnt + 4,
                 (int)mk, st, &nl);
         base += (int)mk;
       }
@@ -4151,7 +4114,7 @@ int32_t sweep(cook_pool* const* pools, int n, int64_t now, int64_t dflt, int64_t
       const int32_t* glen = s->run.at<int32_t>(R_GLEN);
       compact(GroupedRows{s->run.at<uint8_t>(R_LIVE), glen, slot + kbase}, s->run.hw, nullptr, blk, cnt + 4, Kk, st, &nl);
       order_scan(os, RowLen{slot + kbase, glen}, Kk, r.S->gf0, st, &nl);
-      ExpandArgs a = {os, slot + kbase, Kk, ebase, h.second, s->run.d_col, s->lists[L_RGROUP].v[0], d_kind, now,
+      ExpandArgs a = {os, slot + kbase, Kk, ebase, h.second, s->run.d_col, s->lists[L_RGROUP].at(0), d_kind, now,
                       e_grp, e_tid, e_pool, e_rt, cnt + 3};
       straggler_expand_kernel<<<(Kk + 255) / 256, 256, 0, st>>>(a);
       nl++;
@@ -4767,7 +4730,7 @@ int32_t user_usage(cook_pool* const* pools, int n, const int32_t* user, int nU, 
   }
   int base = 0;
   for (const Src& h : hs) {
-    compact(UURows{h.s->run.d_col, umap, base, h.k, h.s->lists[L_RGROUP].v[0], r_user, r_jid, r_tid, r_pidx, r_grp,
+    compact(UURows{h.s->run.d_col, umap, base, h.k, h.s->lists[L_RGROUP].at(0), r_user, r_jid, r_tid, r_pidx, r_grp,
                    {amt[0], amt[1], amt[2]}},
             h.s->run.hw, nullptr, blk, cnt + 2, h.live, st, &nl);
     base += h.live;
@@ -5253,7 +5216,7 @@ int32_t history_stats(cook_pool* const* pools, int n, int32_t status, int64_t st
   const int H = (int)hs.size();
   const bool ok = status == COOK_IS_SUCCESS;
   auto sel = [&](int j, int base, const ISPipe& p) {
-    return HSSel{hs[j].first->c, base, hs[j].second, ok, start_ms, end_ms, tid_lo, tid_hi,
+    return HSSel{hs[j].first->cols(), base, hs[j].second, ok, start_ms, end_ms, tid_lo, tid_hi,
                  p.s_user, p.s_reason, p.s_tid, p.s_pidx, p.s_pos, {p.met[0], p.met[1], p.met[2]}};
   };
   // ---- the selection's size per handle, so that every buffer after it is sized by the selection.  A staged handle
@@ -5604,13 +5567,13 @@ int32_t digest(cook_pool* pool, PoolState* S, int nb, cook_state_digest_out* out
   const size_t shm = sizeof(unsigned long long) * 3 * (size_t)a.sb;
   if (S->pend.hw) {
     a.col = S->pend.d_col; a.n = S->pend.hw; a.bucket = bkt;
-    for (int l = 0; l < 3; l++) { a.v0[l] = S->lists[l].v[0]; a.v1[l] = S->lists[l].v[1]; }
+    for (int l = 0; l < 3; l++) { a.v0[l] = S->lists[l].at(0); a.v1[l] = S->lists[l].at(1); }
     audit_table_kernel<true><<<(a.n + 255) / 256, 256, shm, st>>>(a);
     nl++;
   }
   if (S->run.hw) {
     a.col = S->run.d_col; a.n = S->run.hw; a.bucket = bkt ? bkt + nb : nullptr;
-    a.v0[0] = S->lists[L_RGROUP].v[0]; a.v1[0] = nullptr;
+    a.v0[0] = S->lists[L_RGROUP].at(0); a.v1[0] = nullptr;
     audit_table_kernel<false><<<(a.n + 255) / 256, 256, shm, st>>>(a);
     nl++;
   }
@@ -5754,7 +5717,7 @@ int32_t export_rows(cook_pool* pool, PoolState* S, int nb, const uint8_t* mask, 
     for (int l = 0; l < L_N; l++) {
       if (!loff[l]) continue;
       d_off[l] = c.take<int32_t>(N[table_of[l]] + 1);
-      for (int i = 0; i < S->lists[l].k; i++) d_v[l][i] = c.take<int32_t>(std::max<int64_t>(E[l], 1));
+      for (int i = 0; i < S->lists[l].v.n; i++) d_v[l][i] = c.take<int32_t>(std::max<int64_t>(E[l], 1));
     }
     if (mask) d_mask = c.up(mask, nb);
   }));
@@ -5789,8 +5752,8 @@ int32_t export_rows(cook_pool* pool, PoolState* S, int nb, const uint8_t* mask, 
     list_total_kernel<<<1, 1, 0, st>>>(os, n[t], d_cnt + 2 + l);
     nl++;
     if (!d_off[l]) continue;
-    csr_gather_kernel<<<(n[t] + 7) / 8, 256, 0, st>>>(os, rs, n[t], tbl[t]->at<int32_t>(off_col[l]), len, S->lists[l].v[0],
-                                                       S->lists[l].v[1], d_off[l], d_v[l][0], d_v[l][1]);
+    csr_gather_kernel<<<(n[t] + 7) / 8, 256, 0, st>>>(os, rs, n[t], tbl[t]->at<int32_t>(off_col[l]), len, S->lists[l].at(0),
+                                                       S->lists[l].at(1), d_off[l], d_v[l][0], d_v[l][1]);
     nl++;
   }
   CK(pool, cudaGetLastError());
@@ -5810,7 +5773,7 @@ int32_t export_rows(cook_pool* pool, PoolState* S, int nb, const uint8_t* mask, 
     for (int l = 0; l < L_N; l++) {
       if (!loff[l]) continue;
       CK(pool, download(loff[l], d_off[l], (size_t)rows[table_of[l]] + 1, st, &d2h));
-      for (int i = 0; i < S->lists[l].k; i++)
+      for (int i = 0; i < S->lists[l].v.n; i++)
         if (entries[l]) CK(pool, download(lv[l][i], d_v[l][i], (size_t)entries[l], st, &d2h));
     }
   }
@@ -6108,30 +6071,9 @@ __global__ void __launch_bounds__(32) mm_finish_kernel(MMCols r, int N, const Gr
 
 // capacity for n pairs in both halves of the counters, the current half's u_n pairs kept
 int32_t mm_counters_room(cook_pool* pool, MetricsRound& R, int64_t n, cudaStream_t st) {
-  if (n <= R.u_cap) return COOK_OK;
-  const int64_t cap = std::max<int64_t>(n, 2 * R.u_cap);
-  int64_t* j[2] = {};
-  int32_t* c[2] = {};
-  cudaError_t e = cudaSuccess;
-  for (int h = 0; h < 2 && e == cudaSuccess; h++) {
-    e = cudaMalloc(&j[h], sizeof(int64_t) * cap);
-    if (e == cudaSuccess) e = cudaMalloc(&c[h], sizeof(int32_t) * cap);
-  }
-  if (e == cudaSuccess && R.u_n) e = cudaMemcpyAsync(j[0], R.u_jid[R.cur], sizeof(int64_t) * R.u_n, cudaMemcpyDeviceToDevice, st);
-  if (e == cudaSuccess && R.u_n) e = cudaMemcpyAsync(c[0], R.u_cyc[R.cur], sizeof(int32_t) * R.u_n, cudaMemcpyDeviceToDevice, st);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  if (e != cudaSuccess) {
-    for (void* p : {(void*)j[0], (void*)j[1], (void*)c[0], (void*)c[1]}) if (p) cudaFree(p);
-    return set_err(pool, COOK_E_OOM, "cook_state_match_metrics: out of device memory");
-  }
-  for (int h = 0; h < 2; h++) {
-    if (R.u_jid[h]) cudaFree(R.u_jid[h]);
-    if (R.u_cyc[h]) cudaFree(R.u_cyc[h]);
-    R.u_jid[h] = j[h];
-    R.u_cyc[h] = c[h];
-  }
-  R.cur = 0;
-  R.u_cap = cap;
+  cudaError_t e = R.u[1 - R.cur].grow(n, 0, st);
+  if (e == cudaSuccess) e = R.u[R.cur].grow(n, R.u_n, st);
+  if (e != cudaSuccess) return set_err(pool, COOK_E_OOM, "cook_state_match_metrics: out of device memory");
   return COOK_OK;
 }
 
@@ -6276,13 +6218,14 @@ int32_t match_metrics(cook_pool* pool, PoolState* S, int32_t U, int32_t D, const
   int& nl = rd.nl;
   int64_t& d2h = rd.d2h;
   // ---- the rows, the drops, the counts and cycles, the entries; the first-ten and the new pairs in take order
-  mm_gather_kernel<<<(N + 255) / 256, 256, 0, st>>>(S->pend.d_col, R.slot, cons, assign, N, r);
+  mm_gather_kernel<<<(N + 255) / 256, 256, 0, st>>>(S->pend.d_col, R.slot.at<int32_t>(0), cons, assign, N, r);
   nl++;
   if (D) {
     mm_drop_kernel<<<(D + 255) / 256, 256, 0, st>>>(d_drop, D, assign, r.matched, cnt + MMC_BAD);
     nl++;
   }
-  mm_count_kernel<<<(N + 255) / 256, 256, 0, st>>>(r, N, U, R.u_jid[R.cur], R.u_cyc[R.cur], R.u_n, ucons, umat, cnt);
+  mm_count_kernel<<<(N + 255) / 256, 256, 0, st>>>(r, N, U, R.u[R.cur].at<int64_t>(0), R.u[R.cur].at<int32_t>(1), R.u_n,
+                                                    ucons, umat, cnt);
   grid_check_kernel<<<(N + 255) / 256, 256, 0, st>>>(r.cpus, r.mem, nullptr, N, gf);
   nl += 2;
   const MMKey key{r.jf, r.gmodel, r.dtype, r.dreq, r.dlim, N};
@@ -6317,7 +6260,8 @@ int32_t match_metrics(cook_pool* pool, PoolState* S, int32_t U, int32_t D, const
   const int nxt = 1 - R.cur;
   if (nu) {
     CK(pool, csort::sort_indices(ord_u, tmp, nu, LessJid{n_jid}, st, &nl));
-    mm_map_kernel<<<(nu + 255) / 256, 256, 0, st>>>(ord_u, nu, n_jid, n_cyc, R.u_jid[nxt], R.u_cyc[nxt]);
+    mm_map_kernel<<<(nu + 255) / 256, 256, 0, st>>>(ord_u, nu, n_jid, n_cyc, R.u[nxt].at<int64_t>(0),
+                                                    R.u[nxt].at<int32_t>(1));
     nl++;
   }
   mm_finish_kernel<<<1, 32, 0, st>>>(r, N, gf, ord_c, ord_m, cnt, f_jid, f_cyc, d_out);
@@ -6676,15 +6620,6 @@ struct LessJobStamp {
   }
 };
 
-struct CJKeep {   // the advance's compaction: the rows submitted at or after the new horizon, in order
-  CJCols s, d; int64_t since;
-  __device__ bool keep(int i) const { return s.submit[i] >= since; }
-  __device__ void emit(int i, int k) const {
-    d.jid[k] = s.jid[i]; d.stamp[k] = s.stamp[i]; d.submit[k] = s.submit[i]; d.user[k] = s.user[i];
-    d.spool[k] = s.spool[i]; d.exec[k] = s.exec[i]; d.kind[k] = s.kind[i];
-  }
-};
-
 // The host columns of a seed or record batch, checked row by row: the rows kept (submit >= since), the executor as the
 // stored byte.
 struct CJBatch {
@@ -6730,10 +6665,8 @@ int32_t cj_append(cook_pool* pool, PoolState* S, const CJBatch& b, const char* w
   StateWrite w(pool, S);
   if (int32_t rc = w.direct([&](Carve& c) {
     if (!k) return;
-    c.copy(L.c.jid + t, b.jid.data(), k); c.copy(L.c.stamp + t, b.stamp.data(), k);
-    c.copy(L.c.submit + t, b.submit.data(), k); c.copy(L.c.user + t, b.user.data(), k);
-    c.copy(L.c.spool + t, b.spool.data(), k); c.copy(L.c.exec + t, b.exec.data(), k);
-    c.copy(L.c.kind + t, b.kind.data(), k);
+    L.c.copy(c, t, k, {b.jid.data(), b.stamp.data(), b.submit.data(), b.user.data(), b.spool.data(), b.exec.data(),
+                       b.kind.data()});
   }))
     return rc;
   if (int32_t rc = w.end()) return rc;
@@ -6783,19 +6716,8 @@ int32_t completed_advance(cook_pool* pool, PoolState* S, const char* who, int64_
     if (move) blk = c.take<int32_t>((size_t)T / CP_BLOCK + 2);
   }))
     return rc;
-  if (move) {
-    CJCols nc;
-    CK(pool, nc.alloc(L.cap));
-    compact(CJKeep{L.c, nc, since_ms}, T, nullptr, blk, S->counters + 7, T, w.st, &w.nl);
-    int32_t kept = 0;
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = download(&kept, S->counters + 7, 1, w.st, &w.d2h);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(w.st);
-    if (e != cudaSuccess) { nc.free_all(); CK(pool, e); }
-    L.c.free_all();
-    L.c = nc;
-    L.tail = kept;
-  }
+  if (move)
+    if (int32_t rc = log_advance(pool, S, w, L, CJ_SUBMIT, since_ms, blk)) return rc;
   if (int32_t rc = w.end()) return rc;
   if (move) {   // the host's rows, by the same rule and in the same order
     int64_t w = 0;
@@ -6869,7 +6791,7 @@ int32_t list_completed(cook_pool* const* pools, int n, int32_t user, int32_t sta
   Gather g(pool);
   for (const Src& h : hs) {
     const bool pool_ok = q.pool == -1 || handle_pool[h.k] == q.pool;   // on the host: no array crosses devices
-    CK(pool, g.rows(pools[h.k], CJRows{h.l->c, user, base, h.k, pool_ok, q, state, jid, stamp, submit, pi, ok},
+    CK(pool, g.rows(pools[h.k], CJRows{h.l->cols(), user, base, h.k, pool_ok, q, state, jid, stamp, submit, pi, ok},
                     (int)h.l->tail, h.rows, blk, cnt + 1, &nl));
     base += h.rows;
   }

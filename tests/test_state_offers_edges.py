@@ -35,9 +35,10 @@ class Counters:
     the offer table's hw (slots ever used since the reset: the peak of the live leases, as freed slots are taken
     first), and per list arena (ports, attributes) its entries, capacity and the compactions into a fresh buffer.
 
-    The model restates state.cu's policy and must follow it: ListArena::grow (capacity max(n, 2 cap, 4096), the
-    compaction buffer `alt` freed), compact_lists (when dead entries outnumber live ones; a kernel into `alt`, then
-    allocated if null, only with live entries) after every cook_state_offers_add and at the end of every
+    The model restates state.cu's policy and must follow it: ListArena::grow (the value arrays' column set grown to
+    capacity max(n, 2 cap, 4096), the compaction target `alt` released), compact_lists (when dead entries outnumber
+    live ones; a kernel into `alt`, grown again if released, only with live entries) after every cook_state_offers_add
+    and at the end of every
     cook_state_match_offers, and Table::take_slot (free slots first)."""
 
     def __init__(self):

@@ -41,14 +41,16 @@ class Mirror:
     def __init__(self, name="sweeps"):
         self.e = engine.GpuEngine(pool_name=name)
         self.rows, self.records = {}, []
-        self.tail = self.grew = self.compacted = 0   # the record table's tail, by the arena rule
+        # the record table's tail, by the arena rule; grew: past 4096 records; compacted: a compaction that kept
+        # records after that growth (into a target made again, as the growth freed it)
+        self.tail = self.grew = self.compacted = 0
 
     def _appended(self, n):
         if self.tail + n > 4096 >= self.tail:
             self.grew = 1
         self.tail += n
         if self.tail - len(self.records) > len(self.records):
-            self.compacted |= len(self.records) > 0
+            self.compacted |= self.grew and len(self.records) > 0
             self.tail = len(self.records)
 
     def close(self):
